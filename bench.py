@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- RAO solves/s of the B200-native hot path (BASELINE.json metric), one JSON line on rank 0.
+"""bench.py -- RAO solves/s of the H100-native hot path (BASELINE.json metric), one JSON line on rank 0.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload cfg2|cfg3|cfg3q|sweep]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload cfg2|cfg3|cfg3q|sweep] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path (Model.solveDynamics for every (design, case) unit of the batch:
 excitation tables, drag-linearisation fixed-point loop, 6x6 complex impedance solve per frequency).
@@ -16,6 +16,9 @@ workload sweep (BASELINE.json configs[3] shard): 1250 VolturnUS-S geometry varia
 
 value = units of all ranks / max-over-ranks device time (CUDA events, inputs resident in HBM).
 e2e   = same metric through the host-buffer C-ABI call (pinned host inputs -> H2D -> kernels -> D2H).
+--dump-outputs DIR: after the timed steps, rank 0 writes the outputs of the last timed step as DIR/<name>.npy (float64;
+complex arrays as [..., 2] = (re, im); at N > 1 the gathered arrays of all ranks; at most 60 MiB with the file headers, a
+seeded sample of units when larger).  Every workload, incl. farm (Xi_sys, info) and flex (Xi, status).
 """
 import argparse
 import json
@@ -281,6 +284,27 @@ def parity_block(designs, cs, Xi, status, max_designs=8):
                 checker="oracle/raft_oracle.c (pinned to reference pickles and reference runs: tests/test_oracle_golden.py)")
 
 
+DUMP_LIMIT = 60 << 20            # bytes of all files together, .npy headers included (< 64 MB)
+
+
+def dump_outputs(path, out, lead=2, seed=0):
+    """Write output tensors (name -> tensor whose first ``lead`` axes index the units, e.g. [nD, nC, ...]) as float64 .npy
+    files under ``path``.  Complex arrays become [..., 2] = (re, im).  When they exceed DUMP_LIMIT bytes in all, a fixed
+    seeded sample of units is written, the same rows of every array, and units.npy holds their flat (C-order) indices."""
+    import torch
+    os.makedirs(path, exist_ok=True)
+    arrs = {k: (torch.view_as_real(v) if v.is_complex() else v).detach().to("cpu", torch.float64).numpy() for k, v in out.items()}
+    n_units = int(np.prod(next(iter(arrs.values())).shape[:lead]))
+    per_unit = sum(a.size // n_units * 8 for a in arrs.values())
+    keep = (DUMP_LIMIT - 8 * n_units - 256 * (len(arrs) + 1)) // per_unit
+    if keep < n_units:
+        pick = np.sort(np.random.default_rng(seed).choice(n_units, size=keep, replace=False))
+        arrs = {k: a.reshape((n_units,) + a.shape[lead:])[pick] for k, a in arrs.items()}
+        arrs["units"] = pick.astype(np.float64)
+    for k, a in arrs.items():
+        np.save(os.path.join(path, k + ".npy"), np.ascontiguousarray(a))
+
+
 def run_reference(args, rank, world):
     """--impl reference: the reference's CPU implementation of the path on the box's host cores.  Two numbers:
     the pinned C oracle port with all host threads (the STRONG CPU figure: value of the line) and, when
@@ -352,7 +376,11 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the sustained-load and sweep-shard extra keys")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (float64, <= 60 MiB in all)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs dumps what the GPU path computed: --impl ours")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -384,7 +412,7 @@ def main():
         # the north-star's multi-GPU configuration next to the default line: configs[3] shard (design sweep), same
         # exchange, fewer steps; carried as an extra key so the driver's per-N records hold it too
         a2 = argparse.Namespace(**vars(args))
-        a2.workload, a2.nw, a2.cases, a2.designs, a2.steps, a2.warmup = "sweep", 0, 0, args.designs or 0, max(2, min(args.steps, 3)), 3
+        a2.workload, a2.nw, a2.cases, a2.designs, a2.warmup, a2.dump_outputs = "sweep", 0, 0, args.designs or 0, 3, None
         d2, c2, g2 = build_workload(a2, rank, world)
         t_build = g2["table_build_s"]
         sw = measure(a2, d2, c2, g2, rank, world, dev, full=False)
@@ -431,7 +459,7 @@ def measure(args, designs, cs, cfg, rank, world, dev, full):
     nD, nC, nw = batch.n_designs, cases.n_cases, batch.nw
     units = nD * nC * nw
     Xi = sess.out["Xi"]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 50 MB L2
     if world > 1 and sh is None:
         gathered = torch.empty((world,) + tuple(Xi.shape), dtype=Xi.dtype, device=dev)
     last = {}
@@ -453,7 +481,7 @@ def measure(args, designs, cs, cfg, rank, world, dev, full):
     if not os.environ.get("RAFTK_BENCH_NO_SAMPLER"):          # diagnostic switch (tools/r02_n2c.sh): is the NVML thread visible in the step time?
         sampler.start()
     # N > 1: at least 10 untimed steps, so that both alternating gathered buffers of every peer have been written through
-    # their NVLink mappings several times before the clock starts (one N = 2 box needed more than 5: profiles/r02_scaling.md)
+    # their NVLink mappings several times before the clock starts
     n_warm = args.warmup if world == 1 else max(args.warmup, 10)
     for _ in range(n_warm):
         step()
@@ -478,6 +506,16 @@ def measure(args, designs, cs, cfg, rank, world, dev, full):
     torch.cuda.synchronize()
     t_wall = time.perf_counter() - t_wall0
     launches = solver.launch_count() - launches0
+    if args.dump_outputs:
+        if sh is not None:                                 # what a caller of the sharded step receives: every rank's block
+            g, s = last["g"], last["s"]
+            final = dict(Xi=g.reshape((-1,) + tuple(g.shape[2:])), status=s.reshape((-1,) + tuple(s.shape[2:])))
+        elif world > 1:
+            final = dict(Xi=gathered.reshape((-1,) + tuple(gathered.shape[2:])))
+        else:
+            final = sess.out
+        if rank == 0:
+            dump_outputs(args.dump_outputs, final)
     clocks = sampler.stop() if sampler.run or not sampler.ok else dict(sm_mhz=None, sm_max_mhz=sampler.max_mhz, reasons=["sampler disabled (diagnostic run)"], samples=0)
     ms = sum(a.elapsed_time(b) for a, b in ev)
     t_ms = torch.tensor([ms], dtype=torch.float64, device=dev)
@@ -535,17 +573,12 @@ def measure(args, designs, cs, cfg, rank, world, dev, full):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
     achieved = b_alg * units_per_launch / (k2_ms * 1e-3) / 1e9
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json"))).get(args.workload)
-    except Exception:
-        pass
-    roofline = dict(bound="hbm", achieved=achieved, peak=hbm_peak, unit="GB/s", frac=achieved / hbm_peak, traffic=traffic,
+    roofline = dict(bound="hbm", achieved=achieved, peak=hbm_peak, unit="GB/s", frac=achieved / hbm_peak,
                     kernel="k_rao_fused (excitation + drag linearisation + 6x6 solves, on-chip)" if kn[1] == 0 else "k_drag_solve",
                     kernel_ms=k2_ms, share_of_step=kms[2] / max(sum(kms), 1e-30),
-                    algorithmic_bytes_per_solve=b_alg, peak_source="MEASURED_PEAKS.json" if peaks else "fallback 6.65 TB/s",
+                    algorithmic_bytes_per_solve=b_alg, peak_source="MEASURED_PEAKS.json" if peaks else "fallback 3.35 TB/s (H100 SXM data sheet)",
                     other_kernels_ms=dict(depth_table=kms[0] / max(kn[0], 1), excitation=kms[1] / max(kn[1], 1)),
                     note="the contract's two bounds are hbm | tensor; this kernel is neither: ~80 kflop of dependent FP64 per 104 "
                          "algorithmic bytes, DRAM traffic below the algorithmic bytes (tables live on chip). Its binding resource is "

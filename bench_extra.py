@@ -60,7 +60,7 @@ def _oracle_farm(packs, C_arr, cs):
     return Xo, passes
 
 
-def _time_farm(N, cs, dev, steps, warmup, parity=False):
+def _time_farm(N, cs, dev, steps, warmup, parity=False, dump=None):
     """-> dict: device-timed step (solve of N FOWTs + system response), e2e through the host call, optional parity."""
     import torch
     from raft_b200 import solver
@@ -86,6 +86,9 @@ def _time_farm(N, cs, dev, steps, warmup, parity=False):
         b.record()
     torch.cuda.synchronize()
     launches = solver.launch_count() - l0
+    if dump:
+        import bench
+        bench.dump_outputs(dump, dict(Xi_sys=xi, info=info), lead=1)
     ms = sum(a.elapsed_time(b) for a, b in ev) / steps
     solver.profile_enable(True)
     flush.fill_(1)
@@ -143,7 +146,7 @@ def bench_special(args, rank, world, dev):
     batch_cs = dict(Hs=rng.uniform(1, 10, nC), Tp=rng.uniform(5, 18, nC), gamma=np.zeros(nC), beta_deg=rng.uniform(-180, 180, nC),
                     spec=np.zeros(nC, dtype=np.int32))
     one = _time_farm(N, file_case, dev, args.steps, args.warmup, parity=not args.no_parity)
-    many = _time_farm(N, batch_cs, dev, args.steps, args.warmup, parity=(not args.no_parity) and N <= 4)
+    many = _time_farm(N, batch_cs, dev, args.steps, args.warmup, parity=(not args.no_parity) and N <= 4, dump=args.dump_outputs)
     sizes = {}
     if not args.no_extras:
         for n_ in (2, 4, 8, 16):
@@ -156,7 +159,7 @@ def bench_special(args, rank, world, dev):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
+    hbm = float(peaks.get("hbm_gbs", 3350.0))
     # SURVEY.md 8(d): farm bytes per solve = 16 n (Xi out) + 8 (zeta) + per-FOWT loads read by the system kernel (3 x 96 N) + ...
     b_alg = 16 * n + 8 + 3 * 96 * N + 288 * N / 1024.0
     ach = b_alg * many["cases"] * many["nw"] / (many["system_kernel_ms"] * 1e-3) / 1e9
@@ -213,10 +216,13 @@ def bench_flex(args, rank, world, dev):
     for a, b in ev:
         flush.fill_(1)
         a.record()
-        sess.solve(n_iter=10)
+        xi, st_ = sess.solve(n_iter=10)
         b.record()
     torch.cuda.synchronize()
     launches = solver.launch_count() - l0
+    if args.dump_outputs:
+        import bench
+        bench.dump_outputs(args.dump_outputs, dict(Xi=xi, status=st_), lead=1)
     ms = sum(a.elapsed_time(b) for a, b in ev) / args.steps
     solver.profile_enable(True)
     sess.solve(n_iter=10)
@@ -237,7 +243,7 @@ def bench_flex(args, rank, world, dev):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
+    hbm = float(peaks.get("hbm_gbs", 3350.0))
     b_alg = 16.0 * n + 8 + 16.0 * n * n / nC            # Xi out + zeta + the constant matrices shared by the cases of a bin
     ach = b_alg * units / (lu_ms * 1e-3) / 1e9
     parity = None

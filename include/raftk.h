@@ -1,5 +1,5 @@
 /*
- * raftk.h -- C ABI of the B200-native RAO-solve hot path (libraftk.so, sm_100a).
+ * raftk.h -- C ABI of the H100-native RAO-solve hot path (libraftk.so, sm_90a).
  *
  * The reference (WISDEM/RAFT) has no FFI: its boundary for this path is Python-method level.
  * Every entry point below therefore cites the reference method(s) it replaces
@@ -281,7 +281,7 @@ int raftk_qtf_slender_host(const raftk_slender *s, int32_t n_cases, const double
  * node motion = Tn Xi, node load -> Tn^T [f ; rr x f].  M, B, C: the constant system matrices of raft_model.py:1045-1047.
  * Xi complex [n_cases,n_dof,nw]; status [n_cases,4] = passes, converged, flags, 0.  The n_dof x n_dof impedance of every (case,
  * frequency, pass) is solved by a blocked LU with partial pivoting (LAPACK's pivot rule and elimination order); validated on
- * B200 against the reference's 150-DOF VolturnUS-S-flexible run (tests/test_general_dofs.py, 1e-10).  n_dof <= 256.
+ * the GPU against the reference's 150-DOF VolturnUS-S-flexible run (tests/test_general_dofs.py, 1e-10).  n_dof <= 256.
  */
 typedef struct raftk_general {
     int32_t n_dof, nw, n_nodes, _pad0;

@@ -1,6 +1,6 @@
-"""raft_b200 -- B200-native RAO-solve hot path behind the RAFT API (see DESIGN.md).
+"""raft_b200 -- H100-native RAO-solve hot path behind the RAFT API (see DESIGN.md).
 
-Importing the package loads ``csrc/libraftk.so`` (sm_100a).  There is no CPU fallback: a missing
+Importing the package loads ``csrc/libraftk.so`` (sm_90a).  There is no CPU fallback: a missing
 library is an ImportError."""
 from . import _lib  # noqa: F401  (fails loudly when the CUDA library has not been built)
 from . import bem, grid, packer, solver, sweep  # noqa: F401

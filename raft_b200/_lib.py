@@ -140,7 +140,7 @@ def _require():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             "raft_b200: CUDA library %s is missing. Build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). There is no CPU fallback." % LIB_PATH)
+            "(nvcc, sm_90a). There is no CPU fallback." % LIB_PATH)
 
 
 def _load():

@@ -52,7 +52,7 @@ def _interp_stations(x, xp, fp):
 def _member_tables(mi, heading, geom, nD, dlsMax, rho, g, Rp, r0, nw_unused=0):
     """All designs' strips of one member copy.  -> dict of padded arrays [nD, S] (+ member-level [nD, ...]) and the mask."""
     if str(mi.get("type", "rigid")) != "rigid":
-        raise NotImplementedError("member %r: only rigid members are supported by the B200 path" % mi["name"])
+        raise NotImplementedError("member %r: only rigid members are supported by the GPU path" % mi["name"])
     rA0 = np.broadcast_to(np.asarray(geom.get("rA", mi["rA"]), dtype=float), (nD, 3)).copy()
     rB0 = np.broadcast_to(np.asarray(geom.get("rB", mi["rB"]), dtype=float), (nD, 3)).copy()
     if np.any(rA0[:, 2] == 0) or np.any(rB0[:, 2] == 0):
@@ -348,7 +348,7 @@ def build_family_native(family, w, k, depth, matrices, r6=None):
     for mi in plat["members"]:
         mi = dict(mi)
         if str(mi.get("type", "rigid")) != "rigid":
-            raise NotImplementedError("member %r: only rigid members are supported by the B200 path" % mi["name"])
+            raise NotImplementedError("member %r: only rigid members are supported by the GPU path" % mi["name"])
         if master == 1:
             mi["potMod"] = False
         elif master in (2, 3):

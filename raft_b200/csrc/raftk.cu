@@ -1,4 +1,4 @@
-// raftk.cu -- sm_100a kernels + C ABI for the RAO-solve hot path (see include/raftk.h, DESIGN.md).
+// raftk.cu -- sm_90a kernels + C ABI for the RAO-solve hot path (see include/raftk.h, DESIGN.md).
 //
 // Kernels
 //   k_depth_table   : depth-decay functions cosh/sinh ratios per (node, frequency)      helpers.py:207-222
@@ -270,7 +270,7 @@ static int pick_cluster(int units, int nw, int requested)
         while (cs > 1 && nw / cs < 32) cs >>= 1;
         return cs;
     }
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int cs = 1;
@@ -303,8 +303,7 @@ static bool fused_try(const raftk_designs *d, int cs, bool have_ws, FPlan &pl)
     pl.maxW = d->max_w_classes > 0 ? d->max_w_classes : d->max_nodes;
     pl.maxH = d->max_h_classes > 0 ? d->max_h_classes : d->max_nodes;
     pl.maxZ = d->max_z_classes > 0 ? std::min(d->max_z_classes, d->max_members) : d->max_members;
-    // 255 registers cap residency at 256 threads per SM (measured: 168 registers / 3 CTAs is slower, the LU
-    // spills); shared memory must allow 2 CTAs of 128 threads or 1 of 256.  The linear excitation F0 lives in
+    // 255 registers cap residency at 256 threads per SM (at 168 registers for 3 CTAs the LU spills); shared memory must allow 2 CTAs of 128 threads or 1 of 256.  The linear excitation F0 lives in
     // shared memory when it fits, else in the caller's workspace.
     const size_t limit = (pl.T == 128) ? (size_t)112 * 1024 : (size_t)226 * 1024;
     pl.f0_global = false;
@@ -324,7 +323,7 @@ static bool fused_plan(const raftk_designs *d, int units, int requested_cs, bool
         while (cs > 1 && d->nw / cs < 32) cs >>= 1;
         return fused_try(d, cs, have_ws, pl);
     }
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     FPlan best; bool have = false;
@@ -740,7 +739,7 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
         return set_err(RAFTK_EINVAL, "farm response needs B_drag, F_drag, F_iner of the per-FOWT solve and farm.Xi_sys");
     if (d->n_bem_head > 0 && !solved->F_BEM) return set_err(RAFTK_EINVAL, "farm response: the designs carry BEM excitation, F_BEM is required");
     const int n = 6 * f->n_fowt;
-    const bool warp = n <= 24;                          // one warp per (frequency, case), wpc systems per CTA; at 6N = 48 it measured 13.6 ms vs 10.6 ms blocked
+    const bool warp = n <= 24;                          // one warp per (frequency, case), wpc systems per CTA; blocked LU above
     const size_t sys_bytes = (size_t)n * (n + 1) * sizeof(double2);
     const int wpc = warp ? (int)std::max<size_t>(1, std::min<size_t>(FARM_WPC, (100 * 1024) / sys_bytes)) : 1;
     const size_t smem = (size_t)wpc * sys_bytes;
@@ -761,9 +760,9 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
     P.Xi = reinterpret_cast<double2 *>(f->Xi_sys); P.info = f->info;
     {
         ProfScope ps(st, 1);
-        // 6N = 12 (the shipped two-FOWT farm): rows in registers, one lane per row, two systems per warp (k_farm_rows: 0.188 ms
-        // against 0.398 ms for 65 536 systems); RAFTK_FARM_SMEM=1 keeps the shared-memory warp kernel (A/B).  At 6N = 18 / 24 the
-        // register rows need 188 / 238 registers and lose (6N = 24: 2.46 ms against 1.37 ms), so those stay on the warp kernel.
+        // 6N = 12 (the shipped two-FOWT farm): rows in registers, one lane per row, two systems per warp (k_farm_rows);
+        // RAFTK_FARM_SMEM=1 keeps the shared-memory warp kernel (A/B).  At 6N = 18 / 24 the register rows need 188 / 238
+        // registers, so those stay on the warp kernel.
         const bool rows = n == 12 && !getenv("RAFTK_FARM_SMEM");
         if (rows) k_farm_rows<12><<<dim3((d->nw + 7) / 8, c->n_cases), 128, 0, st>>>(D, C, P);
         else if (warp) k_farm_response<true><<<dim3((d->nw + wpc - 1) / wpc, c->n_cases), 32 * wpc, smem, st>>>(D, C, P);
@@ -1466,7 +1465,7 @@ extern "C" void raftk_host_free(void *p) { if (p) cudaFreeHost(p); }
 
 extern "C" double raftk_fp64_peak_gflops(int iters)
 {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int blocks = sms * 8, threads = 256;

@@ -57,7 +57,7 @@ __host__ __device__ inline size_t fused_smem_bytes(int Nm, int NsP, int nchunk, 
 }
 
 // projection of the wave velocity on direction d plus a body-velocity term: a = E (C h + i S d_z) + m.
-// (A 3-way specialisation on exactly horizontal / vertical directions was measured: ptxas if-converts it
+// (A 3-way specialisation on exactly horizontal / vertical directions does not pay: ptxas if-converts it
 // into predicated code that issues all variants, so the generic 6-flop form is kept.)
 __device__ __forceinline__ void proj_add(double er, double ei, double Cc, double Sc, double h, double dz,
                                          double mr, double mi, double &ar, double &ai)
@@ -617,7 +617,7 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
                 const double lr = S.xi[(2 * a) * nwl + t], li = S.xi[(2 * a + 1) * nwl + t];
                 if (isnan(br[a]) || isnan(bi[a])) nan_local |= RAFTK_FLAG_NAN;
                 const double dr = br[a] - lr, di = bi[a] - li;
-                // raft_model.py:1103: |d| / (|x| + tol) < tol  <=>  |d| < tol |x| + tol^2   (no division: 4 % faster;
+                // raft_model.py:1103: |d| / (|x| + tol) < tol  <=>  |d| < tol |x| + tol^2   (no division;
                 // same decision up to the last ulp)
                 if (!(sqrt(dr * dr + di * di) < fma(P.tol, sqrt(br[a] * br[a] + bi[a] * bi[a]), P.tol * P.tol))) conv_local = 0;
                 S.xi[(2 * a) * nwl + t] = 0.2 * lr + 0.8 * br[a];

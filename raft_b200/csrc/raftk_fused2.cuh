@@ -1,12 +1,12 @@
 // raftk_fused2.cuh -- k_fused_plan + k_rao_fused2: second generation of the fused on-chip solver (included by raftk.cu only).
 //
-// Same algorithm and recurrences as k_rao_fused (raftk_fused.cuh); what changed is the mapping, driven by the measured FP64
-// pipe (profiles/r02_fp64_micro.txt: DFMA latency 8.2 cycles, one warp instruction per 2 cycles per scheduler; with the two
-// resident warps per scheduler that 254 registers allow, the pipe saturates only at >= 2 independent chains per thread):
+// Same algorithm and recurrences as k_rao_fused (raftk_fused.cuh); what changed is the mapping, driven by the FP64 pipe's
+// latency and issue rate (tools/micro/fp64_micro.cu measures both; with the two resident warps per scheduler that 254
+// registers allow, one dependent chain per thread cannot keep the pipe busy):
 //   * TWO frequency bins per thread.  The node walks of both bins are interleaved instruction by instruction (two
 //     independent E/A recurrences -> ILP 2); the per-node RMS accumulators, the linearised coefficients and the step-class
 //     indices are shared by both bins, so the warp reductions, the coefficient loads and the address arithmetic per bin halve.
-//     A CTA of 128 threads owns 256 bins: cfg2 runs as ONE wave of 4-CTA clusters instead of 1.73 waves of 8-CTA clusters.
+//     A CTA of 128 threads owns 256 bins: cfg2 runs as ONE wave of 4-CTA clusters on 132 SMs instead of two of 8-CTA clusters.
 //   * the per-design tables (member frames and lever arms, node columns, system matrices, step classes with every node's
 //     factor-table offsets) are built ONCE per design by k_fused_plan into a 16-byte aligned blob and staged into shared
 //     memory by ONE TMA bulk copy (cp.async.bulk + mbarrier) instead of being rebuilt with scalar loads by every CTA.
@@ -686,8 +686,8 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
         if (CS > 1) {
             cluster.sync();
             for (int t = tid; t < nchunk * 32; t += T) {
-                // every rank's partial is requested before the first one is used (a remote shared-memory read takes ~200
-                // cycles); ranks beyond the cluster contribute an exact +0.0, so the sum keeps its order and value
+                // every rank's partial is requested before the first one is used (remote shared-memory reads are
+                // slow); ranks beyond the cluster contribute an exact +0.0, so the sum keeps its order and value
                 double s = 0.0;
 #pragma unroll 1
                 for (int r0 = 0; r0 < CS; r0 += 4) {
@@ -843,9 +843,9 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
 #pragma unroll
                 for (int a = 0; a < 6; a++) P.Fdrag_out[ogl + (size_t)a * nw + i] = make_double2(br[a], bi[a]);
             }
-            double2 f0v[6];
+            // the linear excitation is added before the assembly: holding it across the 72-double matrix build spills on sm_90a
 #pragma unroll
-            for (int a = 0; a < 6; a++) f0v[a] = P.F0g[ogl + (size_t)a * nw + i];          // in flight during the assembly
+            for (int a = 0; a < 6; a++) { const double2 f = P.F0g[ogl + (size_t)a * nw + i]; br[a] += f.x; bi[a] += f.y; }
             double ar[6][6], ai[6][6];
             const double w2 = w * w;
             if (Aw) {
@@ -867,8 +867,6 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
                         ai[a][b] = w * s_bmat[6 * a + b];
                     }
             }
-#pragma unroll
-            for (int a = 0; a < 6; a++) { br[a] += f0v[a].x; bi[a] += f0v[a].y; }
             const bool ok = solve6(ar, ai, br, bi);
             if (!ok) nan_local |= RAFTK_FLAG_SINGULAR;
 #pragma unroll

@@ -1,6 +1,6 @@
 // raftk_general.cuh -- Model.solveDynamics for FOWTs with generalised degrees of freedom (flexible members, nDOF up to 256;
 // raft_fowt.py:1854-1857, 1886-1888, 1913-1929 and raft_model.py:1052-1142)  (included by raftk.cu only).  Validated on
-// B200 against the reference's 150-DOF VolturnUS-S-flexible run (tests/test_general_dofs.py).
+// the GPU against the reference's 150-DOF VolturnUS-S-flexible run (tests/test_general_dofs.py).
 //
 // The checker (oracle/raft_oracle.c: ro_general_*) is pinned to the reference's VolturnUS-S-flexible pickles and a 150-DOF
 // solveDynamics run; these kernels restate the same bookkeeping: every strip node j carries the 6 x n block Tn_j of fowt.T

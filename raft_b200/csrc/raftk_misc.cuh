@@ -178,9 +178,7 @@ __global__ void __launch_bounds__(128) k_system_solve(int n, int nrhs, double2 *
 // Z_sys = blockdiag_i(-w^2 (M0_i + A_w,i) + i w (B0_i + B_drag_i + B_w,i) + C0_i) + (-w^2 M_arr + i w B_arr + C_arr),
 // F = F_BEM_i + F_iner_i + F_drag_i (+ F_2nd_i) stacked, Xi_sys = Z_sys^-1 F.  Everything is read from device-resident
 // outputs of the drag-linearisation solve: no host assembly of Z, no per-case transfer of nw n^2 complex numbers.
-// WARP = true : small systems (6N <= 24), one WARP per (frequency, case), up to FARM_WPC systems per CTA, no CTA-wide barriers
-//               (65 536 systems: 6N = 12 0.40 ms against 0.90 ms with a CTA per system, 6N = 24 1.38 against 2.20 ms; at 6N = 48 the
-//               warp variant is slower -- 13.6 against 10.6 ms -- with only 6 warps resident per SM);
+// WARP = true : small systems (6N <= 24), one WARP per (frequency, case), up to FARM_WPC systems per CTA, no CTA-wide barriers;
 // WARP = false: one CTA per (frequency, case), blocked LU.
 // ------------------------------------------------------------------------------------------------
 struct FarmParams {
@@ -241,8 +239,8 @@ __global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(De
 }
 
 // ------------------------------------------------------------------------------------------------
-// K3c: farm system response for the two-FOWT array (6N = 12; the template also builds for 18 / 24, where it measured slower than
-// the shared-memory warp kernel and is not launched): the augmented system lives in REGISTERS, one lane per row.
+// K3c: farm system response for the two-FOWT array (6N = 12; the template also builds for 18 / 24, where it needs 188 / 238
+// registers and is not launched): the augmented system lives in REGISTERS, one lane per row.
 // A group of LPS lanes (16 for 6N = 12: two systems per warp; 32 above) owns one (frequency, case) system; lane r holds row r
 // (N6 matrix entries + the right-hand side).  Elimination step k (fully unrolled, so every register index is static):
 // pivot = first maximum of |re| + |im| over rows >= k (butterfly over the group, LAPACK izamax tie-break), ONE shuffle per

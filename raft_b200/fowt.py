@@ -59,7 +59,7 @@ class FOWT:
         self.potFirstOrder = int(plat.get("potFirstOrder", 0))
         mats = dict(matrices or {})
         # second-order wave loads (raft_fowt.py:409-431): 0 none, 2 external QTF file <hydroPath>.12d (or an injected
-        # table matrices['qtf'], ['qtf_w'], ['qtf_heads']); 1 (slender-body QTF) is outside the B200 path
+        # table matrices['qtf'], ['qtf_w'], ['qtf_heads']); 1 (slender-body QTF) is outside the GPU path
         self.potSecOrder = int(plat.get("potSecOrder", 0) or 0)
         self.outFolderQTF = None
         if self.potSecOrder == 1:                                      # slender-body QTF on its own frequency grid (:411-426)
@@ -101,7 +101,7 @@ class FOWT:
             mem.setPosition(self.r6)
 
     def calcStatics(self):
-        raise NotImplementedError("statics are outside the B200 hot path: inject M_struc, C_struc, C_hydro (DESIGN.md section 9)")
+        raise NotImplementedError("statics are outside the GPU hot path: inject M_struc, C_struc, C_hydro (DESIGN.md section 9)")
 
     # raft_fowt.py:1589-1625 -------------------------------------------------------------------------------
     def calcHydroConstants(self):
@@ -176,7 +176,7 @@ class FOWT:
         """Difference-frequency force amplitudes from the QTF table on the GPU: ``beta`` [rad], ``S0`` [nw] wave
         spectrum -> (f_mean [6], f [6,nw] real).  Only the reference's default ``interpMode='qtf'``."""
         if interpMode != "qtf":
-            raise NotImplementedError("only interpMode='qtf' (the reference's default) is on the B200 path")
+            raise NotImplementedError("only interpMode='qtf' (the reference's default) is on the GPU path")
         S0 = np.asarray(S0, dtype=float)
         one = solver.CaseTable(dict(Hs=[0.0], Tp=[1.0], gamma=[0.0], beta_deg=[float(beta) * 57.29577951308232], spec=[0]),
                                zeta=np.sqrt(2.0 * S0 * self.dw)[None, :])

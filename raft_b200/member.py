@@ -59,7 +59,7 @@ class Member:
         self.name = str(mi["name"])
         self.type = str(mi.get("type", "rigid"))
         if self.type != "rigid":
-            raise NotImplementedError("member %r: only rigid members are supported by the B200 path" % self.name)
+            raise NotImplementedError("member %r: only rigid members are supported by the GPU path" % self.name)
         self.part_of = part_of
         rA0, rB0 = np.array(mi["rA"], dtype=float), np.array(mi["rB"], dtype=float)
         if rA0[2] == 0 or rB0[2] == 0:

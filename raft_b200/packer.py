@@ -23,7 +23,7 @@ SQRT_8_OVER_PI = np.sqrt(8.0 / np.pi)
 
 def _member_is_supported(mem):
     if getattr(mem, "type", "rigid") != "rigid":
-        raise NotImplementedError("member %r: only rigid members are supported by the B200 path" % mem.name)
+        raise NotImplementedError("member %r: only rigid members are supported by the GPU path" % mem.name)
 
 
 def _uses_mcf(mem):
@@ -364,7 +364,7 @@ def pack_turbine_channels(fowt):
             avg.append(means[ax])
         mem_tower = fowt.memberList[fowt.nplatmems + ir]
         if getattr(mem_tower, "type", "rigid") != "rigid":
-            raise NotImplementedError("turbine channels: flexible towers (finite-element internal loads, raft_fowt.py:2541) are outside the B200 path")
+            raise NotImplementedError("turbine channels: flexible towers (finite-element internal loads, raft_fowt.py:2541) are outside the GPU path")
         mRNA, IrRNA, zRNA = float(rotor.mRNA), float(rotor.IrRNA), float(rotor.r_rel[2])
         mtow = float(fowt.mtower[ir])
         m_turb = mtow + mRNA                                              # :2509

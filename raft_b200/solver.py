@@ -22,8 +22,7 @@ _I4 = np.int32
 
 class _Tables(dict):
     """The named host arrays of a DesignBatch / CaseTable.  Every mutation bumps ``version``, which keys the cached C struct
-    of the host-buffer calls (building the ~30-pointer ctypes struct costs ~25 us of Python per call otherwise -- 6 % of a
-    0.4 ms end-to-end solve).  In-place edits of an array keep its address, so they need no invalidation."""
+    of the host-buffer calls (building the ~30-pointer ctypes struct costs ~25 us of Python per call otherwise).  In-place edits of an array keep its address, so they need no invalidation."""
     version = 0
 
     def _bump(self):

@@ -1,4 +1,4 @@
-"""GPU parity tests proper: the sm_100a kernels, called through the C ABI, against
+"""GPU parity tests proper: the sm_90a kernels, called through the C ABI, against
 (a) the golden fixtures (reference pickles + reference runs) and (b) the C oracle on larger seeded inputs.
 
 Tolerance: BASELINE.json north_star states fp64 rtol 1e-10 on the RAOs; the metric is

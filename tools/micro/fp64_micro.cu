@@ -1,6 +1,6 @@
-// FP64 pipe characterisation on the box (B200): dependent-DFMA latency, and DFMA throughput per SM as a function of
+// FP64 pipe characterisation of the GPU: dependent-DFMA latency, and DFMA throughput per SM as a function of
 // resident warps per scheduler and independent chains per thread (ILP).  Drives the occupancy / ILP decisions of k_rao_fused.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/micro/fp64_micro.bin tools/micro/fp64_micro.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/micro/fp64_micro.bin tools/micro/fp64_micro.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -78,7 +78,7 @@ static void run(int warps_per_sched, int sms, double *out, long long *cyc)
 
 int main()
 {
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     double *out; long long *cyc;
     cudaMalloc(&out, 1 << 22); cudaMalloc(&cyc, 8);

@@ -4,7 +4,7 @@
 //   variant W: 8 lanes per system (4 systems per warp): lane c holds column c of the augmented 6 x 7 system (12 registers of matrix),
 //              pivot row and multipliers broadcast with __shfl_sync inside the 8-lane group, full occupancy
 // Both read Z = C - w^2 M + i w B and F from global tables and write Xi; same pivot rule (|re| + |im|, first maximum).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/micro/lu6_ab.bin tools/micro/lu6_ab.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/micro/lu6_ab.bin tools/micro/lu6_ab.cu
 #include <cstdio>
 #include <cmath>
 #include <type_traits>
