@@ -271,4 +271,51 @@ def bench_flex(args, rank, world, dev):
                 roofline_fp64=dict(bound="fp64", achieved=flops_lu * units / (lu_ms * 1e-3) / 1e12, peak=fp64_peak / 1e3, unit="TFLOP/s",
                                    frac=flops_lu * units / (lu_ms * 1e-3) / 1e9 / fp64_peak, flops_per_system=flops_lu),
                 parity=parity)
+    del sess
+    line["trains"] = _flex_trains(args, P, M, B, Cm, cs, ms, flush, dev)
     print(json.dumps(line))
+
+
+def _flex_trains(args, P, M, B, Cm, cs, ms_single, flush, dev):
+    """The same sea states, each with a second seeded wave train (cases.primary): train 0 drives the linearisation, the
+    second is solved from the primary's LU factors.  The primaries repeat the single-train step's work exactly, so the
+    secondaries' share of the step is (ms_trains - ms_single) / ms_trains."""
+    import torch
+    from raft_b200 import solver
+    nC, nw = len(cs["Hs"]), len(P["w"])
+    rng = np.random.default_rng(7)
+    Hs2, Tp2, b2 = rng.uniform(1, 10, nC), rng.uniform(5, 18, nC), rng.uniform(-180, 180, nC)
+    rows = lambda a, b: np.stack([a, b], axis=1).reshape(-1)             # noqa: E731  case c -> trains 2c, 2c + 1
+    tab = dict(Hs=rows(cs["Hs"], Hs2), Tp=rows(cs["Tp"], Tp2), gamma=np.zeros(2 * nC), beta_deg=rows(cs["beta_deg"], b2),
+               spec=np.zeros(2 * nC, dtype=np.int32), primary=np.repeat(np.arange(0, 2 * nC, 2), 2).astype(np.int32))
+    ct = solver.CaseTable(tab)
+    sess = solver.GeneralSession(P, M, B, Cm, ct, device=dev)
+    for _ in range(max(args.warmup, 1)):
+        sess.solve(n_iter=10)
+    torch.cuda.synchronize()
+    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
+    for a, b in ev:
+        flush.fill_(1)
+        a.record()
+        sess.solve(n_iter=10)
+        b.record()
+    torch.cuda.synchronize()
+    ms = sum(a.elapsed_time(b) for a, b in ev) / args.steps
+    out = dict(trains_per_case=2, ms_per_step=ms, value=2 * nC * nw / (ms * 1e-3), unit="train RAO solves/s",
+               secondary_share_of_step=(ms - ms_single) / ms, parity=None)
+    if not args.no_parity:
+        import sys
+        from oracle import oracle as orc
+        sys.path.insert(0, os.path.join(ROOT, "tests"))
+        import general_trains_checker as gtc
+        Xi_h, st_h = solver.general_solve_dynamics(P, M, B, Cm, ct, n_iter=10)
+        worst, mism = 0.0, 0
+        for c in range(min(nC, 2)):
+            tr = np.array([[tab["Hs"][2 * c + h], tab["Tp"][2 * c + h], tab["beta_deg"][2 * c + h]] for h in range(2)])
+            Xo, so, _ = gtc.solve_trains(orc, P, M, B, Cm, tr, nIter=10)
+            for h in range(2):
+                worst = max(worst, float(np.abs(Xi_h[2 * c + h] - Xo[h]).max() / np.abs(Xo[h]).max()))
+            mism += int(so[0] != st_h[2 * c, 0])
+        out["parity"] = dict(max_rel_err=worst, pass_mismatch_cases=mism, cases_checked=min(nC, 2), rtol=1e-9,
+                             metric="max |Xi - Xi_oracle| / max |Xi_oracle| per train, both trains of each checked case")
+    return out

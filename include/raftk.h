@@ -130,7 +130,8 @@ typedef struct raftk_cases {
                                 the case drives its own drag linearisation; primary[c] = p != c: secondary train --
                                 its response uses the impedance and per-node drag coefficients of case p
                                 (raft_model.py:1200-1236; p must be a primary).  NULL: all cases independent.
-                                Only raftk_solve_dynamics_*; needs raftk_solve_workspace_bytes() of workspace. */
+                                raftk_solve_dynamics_* (needs raftk_solve_workspace_bytes() of workspace) and
+                                raftk_general_solve_dynamics_*. */
     const double *F_2nd;     /* optional real [nD,nC,6,nw]: second-order force amplitudes (fowt.Fhydro_2nd, from
                                 raftk_second_order_force_*) added to the linear excitation F_BEM + F_iner of every
                                 unit (raft_model.py:1048, :1212).  NULL: none, or computed by the solve (see below). */
@@ -276,12 +277,17 @@ int raftk_qtf_slender_host(const raftk_slender *s, int32_t n_cases, const double
 
 /*
  * Model.solveDynamics for ONE FOWT with generalised degrees of freedom (flexible members, n_dof > 6; raft_fowt.py:1854-1857,
- * 1886-1888, 1913-1929; raft_model.py:1052-1142) and n_cases single-train cases.  Every submerged strip node carries the
+ * 1886-1888, 1913-1929; raft_model.py:1052-1142) and n_cases cases or wave trains.  Every submerged strip node carries the
  * 6 x n_dof block of fowt.T of its structural node (Tn) and its offset from that node (rr; zero on flexible members):
  * node motion = Tn Xi, node load -> Tn^T [f ; rr x f].  M, B, C: the constant system matrices of raft_model.py:1045-1047.
  * Xi complex [n_cases,n_dof,nw]; status [n_cases,4] = passes, converged, flags, 0.  The n_dof x n_dof impedance of every (case,
  * frequency, pass) is solved by a blocked LU with partial pivoting (LAPACK's pivot rule and elimination order); validated on
  * the GPU against the reference's 150-DOF VolturnUS-S-flexible run (tests/test_general_dofs.py, 1e-10).  n_dof <= 256.
+ * Wave trains (cases.primary, raft_model.py:1200-1236): a secondary train runs no pass of its own; its response is solved with
+ * the LU factors of its primary's last impedance and the drag excitation of its own wave kinematics with the primary's last
+ * node drag coefficients.  Primaries keep the loop's final Xi.  Status rows of secondaries: 0, 1, flags, primary + 1.
+ * cases.F_2nd and cases.Xi_init are rejected.  raftk_general_workspace_bytes() covers any primary map; the pivot rows kept for
+ * the trains take n_cases * nw * n_dof * 4 bytes of it (rounded up to 256) whether or not the call has trains.
  */
 typedef struct raftk_general {
     int32_t n_dof, nw, n_nodes, _pad0;
@@ -304,6 +310,20 @@ int raftk_general_solve_dynamics_dev(const raftk_general *g, const raftk_cases *
                                      int32_t *status, void *workspace, size_t workspace_bytes, void *stream);
 int raftk_general_solve_dynamics_host(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
                                       int32_t *status);
+
+/*
+ * Output channels of FOWT.saveTurbineOutputs for a FOWT with generalised degrees of freedom (raft_fowt.py:2299-2604): PRP
+ * motions, nacelle accelerations and flexible-tower base loads are real linear functionals of the reduced response,
+ *   Y_ch(w) = w^wpow[ch] sum_b R[ch,b] Xi[b,w]     (raft_b200.packer.pack_general_channels; rad2deg folded into R)
+ * -> std = sqrt(1/2 sum_w |Y|^2), PSD(w) = 1/2 |Y|^2 / dw, amp = Y, with the reduction of raftk_channel_stats_*.
+ * w [nw] rad/s; R [n_ch,n_dof]; wpow [n_ch] 0 or 2; Xi complex [n_units,n_dof,nw] -> std [n_units,n_ch],
+ * psd [n_units,n_ch,nw] or NULL, amp complex [n_units,n_ch,nw] or NULL.
+ */
+int raftk_general_channel_stats_dev(int32_t n_units, int32_t n_dof, int32_t n_ch, int32_t nw, double dw, const double *w,
+                                    const double *R, const int32_t *wpow, const double *Xi, double *std, double *psd, double *amp,
+                                    void *stream);
+int raftk_general_channel_stats_host(int32_t n_units, int32_t n_dof, int32_t n_ch, int32_t nw, double dw, const double *w,
+                                     const double *R, const int32_t *wpow, const double *Xi, double *std, double *psd, double *amp);
 
 /*
  * Multi-GPU exchange of the responses (SURVEY.md 8e; the reference's sweep driver parametersweep.py:49-95 collects

@@ -123,7 +123,8 @@ SYMBOLS = [
     "raftk_qtf_slender_workspace_bytes", "raftk_qtf_slender_dev", "raftk_qtf_slender_host",
     "raftk_general_workspace_bytes", "raftk_general_solve_dynamics_dev", "raftk_general_solve_dynamics_host",
     "raftk_system_solve_dev", "raftk_system_solve_host", "raftk_response_stats_dev", "raftk_response_stats_host",
-    "raftk_channel_stats_dev", "raftk_channel_stats_host", "raftk_host_alloc", "raftk_host_free",
+    "raftk_channel_stats_dev", "raftk_channel_stats_host", "raftk_general_channel_stats_dev", "raftk_general_channel_stats_host",
+    "raftk_host_alloc", "raftk_host_free",
     "raftk_fp64_peak_gflops",
     "raftk_peer_alloc", "raftk_peer_free", "raftk_peer_open", "raftk_peer_close",
     "raftk_solve_dynamics_gather_dev", "raftk_peer_barrier_dev",
@@ -183,6 +184,10 @@ def _load():
     lib.raftk_response_stats_host.argtypes = [C.c_int32, C.c_int32, C.c_double, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.raftk_channel_stats_dev.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double] + [C.c_void_p] * 6
     lib.raftk_channel_stats_host.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double] + [C.c_void_p] * 5
+    lib.raftk_general_channel_stats_dev.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double] + [C.c_void_p] * 8
+    lib.raftk_general_channel_stats_host.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double] + [C.c_void_p] * 7
+    lib.raftk_general_channel_stats_dev.restype = C.c_int
+    lib.raftk_general_channel_stats_host.restype = C.c_int
     lib.raftk_channel_stats_dev.restype = C.c_int
     lib.raftk_channel_stats_host.restype = C.c_int
     lib.raftk_response_stats_dev.restype = C.c_int

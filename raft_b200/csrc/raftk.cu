@@ -1169,7 +1169,7 @@ extern "C" int raftk_second_order_force_host(const raftk_designs *d, const raftk
 }
 
 // ---- generalised degrees of freedom (flexible members) ---------------------------------------------------------------
-struct GenLayout { size_t u, f6, Fi, Fd, XL, Bm, Bd, Z, fl, total; };
+struct GenLayout { size_t u, f6, Fi, Fd, XL, Bm, Bd, Z, pv, fl, total; };
 static GenLayout gen_layout(const raftk_general *g, size_t nC)
 {
     const size_t n = g->n_dof, nw = g->nw, Ns = std::max(g->n_nodes, 1);
@@ -1178,7 +1178,7 @@ static GenLayout gen_layout(const raftk_general *g, size_t nC)
     L.u = take(nC * Ns * 3 * nw * 16); L.f6 = take(nC * Ns * 6 * nw * 16);
     L.Fi = take(nC * n * nw * 16); L.Fd = take(nC * n * nw * 16); L.XL = take(nC * n * nw * 16);
     L.Bm = take(nC * Ns * 9 * 8); L.Bd = take(nC * n * n * 8);
-    L.Z = take(nC * nw * n * (n + 1) * 16); L.fl = take(nC * 16);
+    L.Z = take(nC * nw * n * (n + 1) * 16); L.pv = take(nC * nw * n * 4); L.fl = take(nC * 16);
     L.total = t;
     return L;
 }
@@ -1195,7 +1195,7 @@ extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const ra
     if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
     if (g->n_dof <= 0 || g->n_dof > 256 || g->nw <= 0 || g->n_nodes < 0 || c->n_cases <= 0 || c->n_cases > 65535)
         return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, 0 < n_cases <= 65535");
-    if (c->primary || c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: wave trains / F_2nd / Xi_init are not supported");
+    if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
     const size_t nC = c->n_cases;
     const GenLayout L = gen_layout(g, nC);
     if (!workspace || workspace_bytes < L.total) return set_err(RAFTK_ENOMEM, "general solve: workspace too small");
@@ -1210,6 +1210,8 @@ extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const ra
     W.F_iner = reinterpret_cast<double2 *>(b + L.Fi); W.F_drag = reinterpret_cast<double2 *>(b + L.Fd);
     W.XiLast = reinterpret_cast<double2 *>(b + L.XL); W.Bmat = reinterpret_cast<double *>(b + L.Bm);
     W.B_drag = reinterpret_cast<double *>(b + L.Bd); W.Z = reinterpret_cast<double2 *>(b + L.Z); W.flags = reinterpret_cast<int *>(b + L.fl);
+    W.piv = reinterpret_cast<int *>(b + L.pv);
+    const int *prim = c->primary;
     CasesDev C = to_dev(c);
     cudaStream_t st = (cudaStream_t)stream;
     double2 *X = reinterpret_cast<double2 *>(Xi);
@@ -1222,14 +1224,14 @@ extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const ra
         CUDA_TRY(opt.ensure(k_gen_solve_blocked, lu_smem));
     }
     prof_begin_call();
-    k_gen_init<<<(unsigned)nC, 256, 0, st>>>(D, W, o->xi_start);
+    k_gen_init<<<(unsigned)nC, 256, 0, st>>>(D, W, o->xi_start, prim);
     if (g->n_nodes > 0) k_gen_wave<<<dim3(fb, g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, C, W);
-    k_gen_project<<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_iner, 0);
+    k_gen_project<<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_iner, 0, nullptr);
     g_launches += 3;
     for (int pass = 0; pass < o->n_iter + 1; pass++) {
-        if (g->n_nodes > 0) k_gen_node_pass<<<dim3(g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, W);
+        if (g->n_nodes > 0) k_gen_node_pass<false><<<dim3(g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, W, nullptr);
         k_gen_bdrag<<<dim3(g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W);
-        k_gen_project<<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_drag, 1);
+        k_gen_project<<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_drag, 1, nullptr);
         if (blocked) {
             ProfScope ps(st, 2);
             k_gen_solve_blocked<<<dim3(g->nw, (unsigned)nC), GT, lu_smem, st>>>(D, W, X, o->tol);
@@ -1240,7 +1242,13 @@ extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const ra
         k_gen_relax<<<(unsigned)nC, 256, 0, st>>>(D, W, X);
         g_launches += 5;
     }
-    k_gen_status<<<(unsigned)((nC + 127) / 128), 128, 0, st>>>((int)nC, W.flags, status);
+    if (prim) {                                        // secondary trains: the primary's last Bmat and LU factors
+        if (g->n_nodes > 0) k_gen_node_pass<true><<<dim3(g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, W, prim);
+        k_gen_project<<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_drag, 0, prim);
+        k_gen_train_solve<<<dim3(g->nw, (unsigned)nC), 128, 0, st>>>(D, W, prim, X);
+        g_launches += 3;
+    }
+    k_gen_status<<<(unsigned)((nC + 127) / 128), 128, 0, st>>>((int)nC, W.flags, prim, status);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
     return RAFTK_OK;
@@ -1252,6 +1260,11 @@ extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const r
     if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
     if (g->n_dof <= 0 || g->nw <= 0 || c->n_cases <= 0) return set_err(RAFTK_EINVAL, "general solve: empty problem");
     const size_t n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases;
+    if (c->primary)
+        for (size_t i = 0; i < nC; i++) {
+            const int p = c->primary[i];
+            if (p < 0 || (size_t)p >= nC || c->primary[p] != p) return set_err(RAFTK_EINVAL, "general solve: cases.primary must map every case to a primary case");
+        }
     size_t total = 0;
     auto take = [&](size_t b) { size_t o_ = total; total += align_up(std::max<size_t>(b, 8), 256); return o_; };
     raftk_general gg = *g; raftk_cases cc = *c;
@@ -1266,6 +1279,7 @@ extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const r
     add(g->M, n * n * 8, (const void **)&gg.M); add(g->B, n * n * 8, (const void **)&gg.B); add(g->C, n * n * 8, (const void **)&gg.C);
     add(c->Hs, nC * 8, (const void **)&cc.Hs); add(c->Tp, nC * 8, (const void **)&cc.Tp); add(c->gamma, nC * 8, (const void **)&cc.gamma);
     add(c->beta_deg, nC * 8, (const void **)&cc.beta_deg); add(c->spec, nC * 4, (const void **)&cc.spec); add(c->zeta, nC * nw * 8, (const void **)&cc.zeta);
+    add(c->primary, nC * 4, (const void **)&cc.primary);
     const size_t o_xi = take(nC * n * nw * 16), o_st = take(nC * 16);
     const size_t wb = raftk_general_workspace_bytes(g, (int32_t)nC), o_ws = take(wb);
     ScratchCall sc;
@@ -1447,6 +1461,47 @@ extern "C" int raftk_channel_stats_host(int32_t n_designs, int32_t n_cases, int3
     double *dP = psd ? sc.take<double>(pb) : nullptr, *dA = amp ? sc.take<double>(ab) : nullptr;
     CUDA_TRY(cudaMemcpy(dC, coef, cb, cudaMemcpyHostToDevice)); CUDA_TRY(cudaMemcpy(dX, Xi, xb, cudaMemcpyHostToDevice));
     int rc = raftk_channel_stats_dev(n_designs, n_cases, n_ch, nw, dw, dC, dX, dS, dP, dA, nullptr);
+    if (!rc) {
+        CUDA_TRY(cudaMemcpy(sd, dS, sb, cudaMemcpyDeviceToHost));
+        if (psd) CUDA_TRY(cudaMemcpy(psd, dP, pb, cudaMemcpyDeviceToHost));
+        if (amp) CUDA_TRY(cudaMemcpy(amp, dA, ab, cudaMemcpyDeviceToHost));
+    }
+    return rc;
+}
+
+extern "C" int raftk_general_channel_stats_dev(int32_t n_units, int32_t n_dof, int32_t n_ch, int32_t nw, double dw, const double *w,
+                                               const double *R, const int32_t *wpow, const double *Xi, double *sd, double *psd, double *amp,
+                                               void *stream)
+{
+    if (n_units <= 0 || n_dof <= 0 || n_ch <= 0 || nw <= 0 || !w || !R || !wpow || !Xi || !sd || !(dw > 0.0))
+        return set_err(RAFTK_EINVAL, "bad general channel-stats arguments");
+    const size_t rows = (size_t)n_units * n_ch;
+    if (rows > 2147483647u) return set_err(RAFTK_EINVAL, "general channel-stats: too many (unit, channel) rows");
+    k_general_channel_stats<<<(unsigned)rows, 128, 0, (cudaStream_t)stream>>>(n_dof, n_ch, nw, dw, w, R, wpow, reinterpret_cast<const double2 *>(Xi),
+                                                                            sd, psd, reinterpret_cast<double2 *>(amp));
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_general_channel_stats_host(int32_t n_units, int32_t n_dof, int32_t n_ch, int32_t nw, double dw, const double *w,
+                                                const double *R, const int32_t *wpow, const double *Xi, double *sd, double *psd, double *amp)
+{
+    if (n_units <= 0 || n_dof <= 0 || n_ch <= 0 || nw <= 0 || !w || !R || !wpow || !Xi || !sd || !(dw > 0.0))
+        return set_err(RAFTK_EINVAL, "bad general channel-stats arguments");
+    const size_t rows = (size_t)n_units * n_ch;
+    const size_t wb = (size_t)nw * 8, rb = (size_t)n_ch * n_dof * 8, pwb = (size_t)n_ch * 4, xb = (size_t)n_units * n_dof * nw * 16;
+    const size_t sb = rows * 8, pb = rows * nw * 8, ab = rows * nw * 16;
+    ScratchCall sc;
+    if (!sc.reserve(align_up(wb, 256) + align_up(rb, 256) + align_up(pwb, 256) + align_up(xb, 256) + align_up(sb, 256) + align_up(pb, 256) + align_up(ab, 256)))
+        return set_err(RAFTK_ENOMEM, "general channel stats: device scratch allocation failed");
+    double *dw_ = sc.take<double>(wb), *dR = sc.take<double>(rb);
+    int32_t *dp = sc.take<int32_t>(pwb);
+    double *dX = sc.take<double>(xb), *dS = sc.take<double>(sb);
+    double *dP = psd ? sc.take<double>(pb) : nullptr, *dA = amp ? sc.take<double>(ab) : nullptr;
+    CUDA_TRY(cudaMemcpy(dw_, w, wb, cudaMemcpyHostToDevice)); CUDA_TRY(cudaMemcpy(dR, R, rb, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(dp, wpow, pwb, cudaMemcpyHostToDevice)); CUDA_TRY(cudaMemcpy(dX, Xi, xb, cudaMemcpyHostToDevice));
+    int rc = raftk_general_channel_stats_dev(n_units, n_dof, n_ch, nw, dw, dw_, dR, dp, dX, dS, dP, dA, nullptr);
     if (!rc) {
         CUDA_TRY(cudaMemcpy(sd, dS, sb, cudaMemcpyDeviceToHost));
         if (psd) CUDA_TRY(cudaMemcpy(psd, dP, pb, cudaMemcpyDeviceToHost));

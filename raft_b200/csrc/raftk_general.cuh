@@ -14,6 +14,11 @@
 //   k_gen_project                     F_drag
 //   k_gen_solve     (case, w)         Z = -w^2 M + i w (B + B_drag) + C, dense complex LU with partial pivoting, Xi
 //   k_gen_relax     (case)            convergence bookkeeping, XiLast = 0.2 XiLast + 0.8 Xi
+// Wave trains (cases.primary): a secondary train takes no part in the loop (done at init); after it
+//   k_gen_node_pass<true>   (case, node)   drag node load from the PRIMARY's last Bmat and the train's own u
+//   k_gen_project                          F_drag of the secondaries
+//   k_gen_train_solve (case, w)            Xi = Z_p^-1 (F_iner + F_drag) from the primary's LU factors left in W.Z and W.piv:
+//                                          row interchanges, unit-lower and upper triangular solves, O(n^2) per system
 #pragma once
 
 struct GenDev {
@@ -40,7 +45,8 @@ struct GenWork {                 // per-call workspace views
     double2 *XiLast;             // [nC][n][nw]
     double *Bmat;                // [nC][Ns][9]
     double *B_drag;              // [nC][n][n]
-    double2 *Z;                  // [nC][nw][n][n+1]  augmented systems
+    double2 *Z;                  // [nC][nw][n][n+1]  augmented systems; after a case's last pass its LU factors (LAPACK layout)
+    int *piv;                    // [nC][nw][n]       pivot row of every elimination step of that factorisation
     int *flags;                  // [nC][4]: done, pass_not_converged, passes, nan
 };
 
@@ -89,11 +95,12 @@ __global__ void __launch_bounds__(128) k_gen_wave(GenDev D, CasesDev Cs, GenWork
     W.f6[fb + (size_t)5 * nw] = make_double2(rr[0] * f[1].x - rr[1] * f[0].x, rr[0] * f[1].y - rr[1] * f[0].y);
 }
 
-// k_gen_project: F[c][dof][i] = sum_j sum_b Tn_j[b][dof] f6_j[b][i].  grid (ceil(nw/128), n, nC), block 128
-__global__ void __launch_bounds__(128) k_gen_project(GenDev D, GenWork W, double2 *F, int skip_done)
+// k_gen_project: F[c][dof][i] = sum_j sum_b Tn_j[b][dof] f6_j[b][i].  grid (ceil(nw/128), n, nC), block 128.
+// sec_only (the primary map) restricts it to the secondary trains.
+__global__ void __launch_bounds__(128) k_gen_project(GenDev D, GenWork W, double2 *F, int skip_done, const int *sec_only)
 {
     const int i = blockIdx.x * 128 + threadIdx.x, dof = blockIdx.y, c = blockIdx.z;
-    if (i >= D.nw || (skip_done && W.flags[4 * c])) return;
+    if (i >= D.nw || (skip_done && W.flags[4 * c]) || (sec_only && sec_only[c] == c)) return;
     const int nw = D.nw, n = D.n;
     double sr = 0.0, si = 0.0;
     for (int j = 0; j < D.Ns; j++) {
@@ -110,16 +117,24 @@ __global__ void __launch_bounds__(128) k_gen_project(GenDev D, GenWork W, double
 }
 
 // k_gen_node_pass: grid (Ns, nC), block 128: RMS of the relative velocity components over w (raft_member.py:2071-2090),
-// Bmat (:2092-2116), then the drag node load f6 = [Bmat u ; rr x (Bmat u)] (:2122-2124)
-__global__ void __launch_bounds__(128) k_gen_node_pass(GenDev D, GenWork W)
+// Bmat (:2092-2116), then the drag node load f6 = [Bmat u ; rr x (Bmat u)] (:2122-2124).
+// TRAIN: secondary trains only, Bmat taken from their primary's last pass (calcDragExcitation(ih), raft_fowt.py:1940-1957).
+template <bool TRAIN>
+__global__ void __launch_bounds__(128) k_gen_node_pass(GenDev D, GenWork W, const int *primary)
 {
     __shared__ double red[4][4];
     __shared__ double bm[9];
     const int j = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, nw = D.nw, n = D.n;
-    if (W.flags[4 * c]) return;
-    const double *q = D.node_frame + 9 * j, *p1 = q + 3, *p2 = q + 6, *rr = D.rr + 3 * j, *T = D.Tn + (size_t)j * 6 * n;
-    const double2 *X = W.XiLast + (size_t)c * n * nw;
+    const double *rr = D.rr + 3 * j;
     const double2 *u = W.u + (((size_t)c * D.Ns + j) * 3) * nw;
+    if constexpr (TRAIN) {
+        const int p = primary[c];
+        if (p == c) return;
+        if (tid < 9) bm[tid] = W.Bmat[((size_t)p * D.Ns + j) * 9 + tid];
+    } else {
+    if (W.flags[4 * c]) return;
+    const double *q = D.node_frame + 9 * j, *p1 = q + 3, *p2 = q + 6, *T = D.Tn + (size_t)j * 6 * n;
+    const double2 *X = W.XiLast + (size_t)c * n * nw;
     double sq = 0.0, sp = 0.0, sp1 = 0.0, sp2 = 0.0;
     for (int i = tid; i < nw; i += 128) {
         double2 xn[6];
@@ -167,6 +182,7 @@ __global__ void __launch_bounds__(128) k_gen_node_pass(GenDev D, GenWork W)
             bm[3 * a + b] = m;
             W.Bmat[((size_t)c * D.Ns + j) * 9 + 3 * a + b] = m;
         }
+    }
     }
     __syncthreads();
     double2 *f6 = W.f6 + (((size_t)c * D.Ns + j) * 6) * nw;
@@ -264,11 +280,13 @@ __global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 
             double b0 = pv[0]; int r0 = pi_[0];
             for (int t = 1; t < 8; t++) if (pv[t] > b0 || (pv[t] == b0 && pi_[t] < r0)) { b0 = pv[t]; r0 = pi_[t]; }
             prow = r0;
+            W.piv[((size_t)c * nw + i) * n + k] = r0;
             if (!(b0 > 0.0)) bad = 1;
         }
         __syncthreads();
         const int p = prow;
-        if (p != k) for (int b = k + tid; b < nc; b += 256) { const double2 t1 = A[(size_t)k * nc + b]; A[(size_t)k * nc + b] = A[(size_t)p * nc + b]; A[(size_t)p * nc + b] = t1; }
+        // whole rows, so that L ends in LAPACK's layout (k_gen_train_solve reuses these factors)
+        if (p != k) for (int b = tid; b < nc; b += 256) { const double2 t1 = A[(size_t)k * nc + b]; A[(size_t)k * nc + b] = A[(size_t)p * nc + b]; A[(size_t)p * nc + b] = t1; }
         __syncthreads();
         if (tid == 0) { const double2 a = A[(size_t)k * nc + k]; const double dd = a.x * a.x + a.y * a.y; piv = make_double2(a.x / dd, -a.y / dd); }
         __syncthreads();
@@ -371,7 +389,7 @@ __global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W
             const double2 a = P[p * GB + j];
             const double dd = a.x * a.x + a.y * a.y;
             const double2 ip = make_double2(a.x / dd, -a.y / dd);
-            if (tid == 0) { pivrow[j] = p; if (!(b0 > 0.0)) bad = 1; }
+            if (tid == 0) { pivrow[j] = p; W.piv[((size_t)c * nw + i) * n + kb + j] = kb + p; if (!(b0 > 0.0)) bad = 1; }
             __syncthreads();
             if (p != j && tid < nb) { const double2 t1 = P[j * GB + tid]; P[j * GB + tid] = P[p * GB + tid]; P[p * GB + tid] = t1; }
             __syncthreads();
@@ -479,14 +497,67 @@ __global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W
     if (nan || bad) atomicOr(&W.flags[4 * c + 3], 1);
 }
 
-// k_gen_init: grid (nC), block 256: XiLast = XiStart (raft_model.py:999), flags = 0
-__global__ void __launch_bounds__(256) k_gen_init(GenDev D, GenWork W, double xi_start)
+// k_gen_init: grid (nC), block 256: XiLast = XiStart (raft_model.py:999), flags = 0; secondary trains start done
+__global__ void __launch_bounds__(256) k_gen_init(GenDev D, GenWork W, double xi_start, const int *primary)
 {
     const int c = blockIdx.x, tid = threadIdx.x;
     const size_t tot = (size_t)D.n * D.nw;
     double2 *L = W.XiLast + (size_t)c * tot;
     for (size_t t = tid; t < tot; t += 256) L[t] = make_double2(xi_start, 0.0);
-    if (tid < 4) W.flags[4 * c + tid] = 0;
+    if (tid < 4) W.flags[4 * c + tid] = (tid == 0 && primary && primary[c] != c) ? 1 : 0;
+}
+
+// k_gen_train_solve: grid (nw, nC), block 128, secondary trains only: Xi = Z_p^-1 (F_iner + F_drag) with the LU factors of the
+// primary's last pass (L unit lower, U upper, row interchanges piv applied in elimination order; raft_model.py:1200-1236)
+__global__ void __launch_bounds__(128) k_gen_train_solve(GenDev D, GenWork W, const int *primary, double2 *Xi)
+{
+    __shared__ double2 b[256];
+    const int i = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, n = D.n, nw = D.nw, nc = n + 1;
+    const int p = primary[c];
+    if (p == c) return;
+    const double2 *A = W.Z + ((size_t)p * nw + i) * (size_t)n * nc;
+    const int *pv = W.piv + ((size_t)p * nw + i) * n;
+    for (int a = tid; a < n; a += 128) {
+        const double2 f1 = W.F_iner[((size_t)c * n + a) * nw + i], f2 = W.F_drag[((size_t)c * n + a) * nw + i];
+        b[a] = make_double2(f1.x + f2.x, f1.y + f2.y);
+    }
+    __syncthreads();
+    if (tid == 0)
+        for (int k = 0; k < n; k++) { const int q = pv[k]; if (q != k) { const double2 t = b[k]; b[k] = b[q]; b[q] = t; } }
+    __syncthreads();
+    for (int k = 0; k < n - 1; k++) {                           // L y = P b
+        const double2 x = b[k];
+        for (int r = k + 1 + tid; r < n; r += 128) {
+            const double2 l = A[(size_t)r * nc + k];
+            double2 v = b[r];
+            v.x -= l.x * x.x - l.y * x.y; v.y -= l.x * x.y + l.y * x.x;
+            b[r] = v;
+        }
+        __syncthreads();
+    }
+    for (int k = n - 1; k >= 0; k--) {                          // U x = y, as the back substitution of k_gen_solve*
+        if (tid == 0) {
+            const double2 a = A[(size_t)k * nc + k], v = b[k];
+            const double dd = a.x * a.x + a.y * a.y;
+            b[k] = make_double2((v.x * a.x + v.y * a.y) / dd, (v.y * a.x - v.x * a.y) / dd);
+        }
+        __syncthreads();
+        const double2 x = b[k];
+        for (int r = tid; r < k; r += 128) {
+            const double2 a = A[(size_t)r * nc + k];
+            double2 v = b[r];
+            v.x -= a.x * x.x - a.y * x.y; v.y -= a.x * x.y + a.y * x.x;
+            b[r] = v;
+        }
+        __syncthreads();
+    }
+    int nan = 0;
+    for (int a = tid; a < n; a += 128) {
+        const double2 x = b[a];
+        Xi[((size_t)c * n + a) * nw + i] = x;
+        if (isnan(x.x) || isnan(x.y)) nan = 1;
+    }
+    if (nan) atomicOr(&W.flags[4 * c + 3], 1);
 }
 
 // k_gen_relax: grid (nC), block 256: close the pass (raft_model.py:1098-1133)
@@ -512,13 +583,14 @@ __global__ void __launch_bounds__(256) k_gen_relax(GenDev D, GenWork W, const do
     }
 }
 
-// status rows for the caller: passes, converged, flags (RAFTK_FLAG_NAN), 0
-__global__ void __launch_bounds__(128) k_gen_status(int nC, const int *flags, int *status)
+// status rows for the caller: passes, converged, flags (RAFTK_FLAG_NAN), 0; a secondary train: 0, 1, flags, primary + 1
+__global__ void __launch_bounds__(128) k_gen_status(int nC, const int *flags, const int *primary, int *status)
 {
     const int c = blockIdx.x * 128 + threadIdx.x;
     if (c >= nC) return;
+    const int p = primary ? primary[c] : c;
     status[4 * c + 0] = flags[4 * c + 2];
     status[4 * c + 1] = flags[4 * c] == 1 ? 1 : 0;
     status[4 * c + 2] = (flags[4 * c] == 2 || flags[4 * c + 3]) ? RAFTK_FLAG_NAN : 0;
-    status[4 * c + 3] = 0;
+    status[4 * c + 3] = p != c ? p + 1 : 0;
 }

@@ -344,6 +344,16 @@ __global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, Fa
     if (live && r == 0 && P.info) P.info[(size_t)c * nw + iw] = bad;
 }
 
+// std = sqrt(1/2 sum_w |Y|^2) of one 128-thread CTA from each thread's partial sum s: warp shuffles, then the four warps
+// in a fixed order (the same reduction tree for every statistics kernel)
+__device__ __forceinline__ void block_rms_tail(double s, double (&part)[4], int tid, double *out)
+{
+    for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((tid & 31) == 0) part[tid >> 5] = s;
+    __syncthreads();
+    if (tid == 0) *out = sqrt(0.5 * (((part[0] + part[1]) + part[2]) + part[3]));
+}
+
 // ------------------------------------------------------------------------------------------------
 // K4: response statistics (std, PSD) -- one CTA per (unit, dof), fixed-order block reduction over frequency
 // ------------------------------------------------------------------------------------------------
@@ -360,10 +370,7 @@ __global__ void __launch_bounds__(128) k_response_stats(int nw, double dw, int r
         s += a2;
         if (psd) psd[(size_t)row * nw + i] = 0.5 * a2 / dw;
     }
-    for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if ((tid & 31) == 0) part[tid >> 5] = s;
-    __syncthreads();
-    if (tid == 0) sd[row] = sqrt(0.5 * (((part[0] + part[1]) + part[2]) + part[3]));
+    block_rms_tail(s, part, tid, sd + row);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -391,10 +398,37 @@ __global__ void __launch_bounds__(128) k_channel_stats(int nC, int nch, int nw, 
         if (psd) psd[(size_t)row * nw + i] = 0.5 * a2 / dw;
         if (amp) amp[(size_t)row * nw + i] = make_double2(yr, yi);
     }
-    for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if ((tid & 31) == 0) part[tid >> 5] = s;
-    __syncthreads();
-    if (tid == 0) sd[row] = sqrt(0.5 * (((part[0] + part[1]) + part[2]) + part[3]));
+    block_rms_tail(s, part, tid, sd + row);
+}
+
+// ------------------------------------------------------------------------------------------------
+// K5g: output channels of a FOWT with generalised DOFs (raftk_general_channel_stats_*): real functionals of the reduced
+// response, Y(w) = w^wpow[ch] sum_b R[ch][b] Xi[unit][b][w] (PRP motions, nacelle accelerations, tower-base internal
+// loads; raft_fowt.py:2299-2604).  One CTA per (unit, channel).
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128) k_general_channel_stats(int n, int nch, int nw, double dw, const double *w, const double *R,
+                                                               const int *wpow, const double2 *Xi, double *sd, double *psd, double2 *amp)
+{
+    __shared__ double part[4];
+    const int row = blockIdx.x, ch = row % nch, unit = row / nch, tid = threadIdx.x;
+    const double *r = R + (size_t)ch * n;
+    const double2 *x = Xi + (size_t)unit * n * nw;
+    const int p = wpow[ch];
+    double s = 0.0;
+    for (int i = tid; i < nw; i += 128) {
+        double yr = 0.0, yi = 0.0;
+        for (int b = 0; b < n; b++) {
+            const double c = r[b];
+            const double2 v = x[(size_t)b * nw + i];
+            yr = fma(c, v.x, yr); yi = fma(c, v.y, yi);
+        }
+        if (p == 2) { const double w2 = w[i] * w[i]; yr *= w2; yi *= w2; }
+        const double a2 = yr * yr + yi * yi;
+        s += a2;
+        if (psd) psd[(size_t)row * nw + i] = 0.5 * a2 / dw;
+        if (amp) amp[(size_t)row * nw + i] = make_double2(yr, yi);
+    }
+    block_rms_tail(s, part, tid, sd + row);
 }
 
 // ------------------------------------------------------------------------------------------------

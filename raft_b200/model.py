@@ -77,7 +77,7 @@ class Model:
         self.results["status"] = out["status"]
         # response statistics per case and FOWT (raft_fowt.py:2299-2353; zero mean offsets: statics are out of scope).
         # getRMS / getPSD sum the squares over a case's wave trains (helpers.py:678-700), so the per-train device
-        # reductions are combined here: std = sqrt(sum std_t^2), PSD = sum PSD_t.
+        # reductions are combined here: std = sqrt(sum std_t^2), PSD = sum PSD_t (solver.combine_trains).
         nC = len(cases)
         owner = out["owner"]
         Xi_units = out["Xi_all"].reshape(len(owner), self.nFOWT, 6, self.nw)                  # [nTrains, nFOWT, 6, nw]
@@ -88,8 +88,7 @@ class Model:
         self.results["case_metrics"] = {}
         for ic in range(nC):
             idx = np.nonzero(owner == ic)[0]
-            sd = np.sqrt((sd_t[idx] ** 2).sum(axis=0))
-            psd = psd_t[idx].sum(axis=0)
+            sd, psd = solver.combine_trains(sd_t, psd_t, idx)
             self.results["case_metrics"][ic] = {}
             for i in range(self.nFOWT):
                 m = {}
@@ -103,8 +102,7 @@ class Model:
                 if ch_stats[i] is not None:                                                   # raft_fowt.py:2401-2444, 2504-2538
                     ch = self.channels[i]
                     nrot = 1 + max(ir for _, ir in ch["names"])
-                    sd_c = np.sqrt((ch_stats[i][0][idx] ** 2).sum(axis=0))
-                    psd_c = ch_stats[i][1][idx].sum(axis=0)
+                    sd_c, psd_c = solver.combine_trains(ch_stats[i][0], ch_stats[i][1], idx)
                     for k_, (nm, ir) in enumerate(ch["names"]):
                         for suffix in ("_avg", "_std", "_max", "_min"):
                             m.setdefault(nm + suffix, np.zeros(nrot))

@@ -390,6 +390,61 @@ def pack_turbine_channels(fowt):
     return dict(names=names, coef=np.array(coef), avg=np.array(avg, dtype=float))
 
 
+def pack_general_channels(fowt):
+    """Output channels of ``FOWT.saveTurbineOutputs`` for a FOWT with generalised degrees of freedom, as real linear
+    functionals of the reduced response: Y_ch(w) = w^wpow[ch] sum_b R[ch,b] Xi[b,w]  (``solver.general_channel_stats``,
+    C ABI ``raftk_general_channel_stats_*``).  Duck-typed on a live FOWT:
+
+      surge, sway, heave, roll, pitch, yaw   PRP motions from the rigidBodyNode rows of fowt.T    raft_fowt.py:2299-2353
+                                             (x + SmallRotate(-r0, theta); rotations in degrees)
+      AxRNA, AyRNA, AzRNA  per rotor         hub acceleration w^2 (T_hub Xi)[0..2]                  :2401-2444
+      FbaseX .. MbaseZ     per flexible tower  internal loads at the tower base -Kf[base] T_tower Xi  :2541-2597
+
+    Like the reference (:2302), the rigidBodyNode rows are taken at ``rigidBodyNode.id``, not ``6 * id``.
+    Returns dict(names [(name, rotor index or None)], R [nch, nDOF], wpow [nch] int32, avg [nch]).  ``avg`` holds the
+    reference's mean values (Xi0_PRP from r6, the hub node's r, the tower nodes' Xi0); 0 where those inputs are absent.
+    A rigid tower's Mbase (:2508-2538) mixes w^0 and w^2 terms with the aero matrices and is not a channel of this form:
+    NotImplementedError."""
+    T = np.asarray(fowt.T, dtype=float)
+    g = float(fowt.g)
+    names, R, wpow, avg = [], [], [], []
+
+    def add(name, ir, row, p, mean):
+        names.append((name, ir)), R.append(np.asarray(row, dtype=float)), wpow.append(p), avg.append(float(mean))
+    rb = fowt.rigidBodyNode
+    Trb = T[rb.id:rb.id + 6, :]
+    r = -np.asarray(rb.r0, dtype=float)[:3]
+    S = np.array([[0.0, r[2], -r[1]], [-r[2], 0.0, r[0]], [r[1], -r[0], 0.0]])      # SmallRotate(r, th) = S th (helpers.py:396)
+    r6 = np.asarray(getattr(fowt, "r6", np.zeros(6)), dtype=float)
+    Xi0 = r6 - np.array([float(getattr(fowt, "x_ref", 0.0)), float(getattr(fowt, "y_ref", 0.0)), 0, 0, 0, 0])
+    for a, nm in enumerate(("surge", "sway", "heave")):
+        add(nm, None, Trb[a] + S[a] @ Trb[3:], 0, Xi0[a])
+    for a, nm in enumerate(("roll", "pitch", "yaw")):
+        add(nm, None, np.rad2deg(Trb[3 + a]), 0, np.rad2deg(Xi0[3 + a]))
+    rotors = list(getattr(fowt, "rotorList", []) or [])
+    for ir, rotor in enumerate(rotors):
+        node = rotor.nodeList[0]
+        Th = T[node.id * 6:(node.id + 1) * 6, :]
+        means = (abs(np.sin(node.r[4]) * g), abs(np.sin(node.r[3]) * g), abs(g))
+        for ax, nm in enumerate(("AxRNA", "AyRNA", "AzRNA")):
+            add(nm, ir, Th[ax], 2, means[ax])
+    for ir, rotor in enumerate(rotors):
+        tow = fowt.memberList[fowt.nplatmems + ir]
+        if getattr(tow, "type", "rigid") == "rigid":
+            raise NotImplementedError("generalised channels: the tower-base moment of a rigid tower (raft_fowt.py:2508-2538) mixes "
+                                      "frequency powers and aero terms; only flexible towers are supported")
+        i0, i1 = tow.nodeList[0].id, tow.nodeList[-1].id
+        Kf = np.asarray(tow.Kf, dtype=float)
+        base = slice(0, 6) if tow.nodeList[0].r0[2] <= tow.nodeList[-1].r0[2] else slice(Kf.shape[0] - 6, Kf.shape[0])   # :2555-2560
+        Rb = -Kf[base] @ T[i0 * 6:(i1 + 1) * 6, :]
+        X0 = np.concatenate([np.asarray(getattr(n, "Xi0", np.zeros(6)), dtype=float) for n in tow.nodeList])
+        F0 = (-Kf @ X0)[base]
+        for a, nm in enumerate(("FbaseX", "FbaseY", "FbaseZ", "MbaseX", "MbaseY", "MbaseZ")):
+            add(nm, ir, Rb[a], 0, F0[a])
+    return dict(names=names, R=np.array(R).reshape(len(names), T.shape[1]), wpow=np.array(wpow, dtype=np.int32),
+                avg=np.array(avg, dtype=float))
+
+
 SPECTRUM_IDS = {"JONSWAP": 0, "unit": 1, "constant": 2, "none": 3, "still": 3}
 
 

@@ -500,7 +500,9 @@ def _general_struct(P, M, B, Cm, ptr_of):
 
 class GeneralSession:
     """Generalised-DOF solve with tables, workspace and outputs resident in HBM (torch tensors), kernels on torch's current
-    stream: ``solve()`` enqueues raftk_general_solve_dynamics_dev -> (Xi [nC,nDOF,nw] complex, status [nC,4])."""
+    stream: ``solve()`` enqueues raftk_general_solve_dynamics_dev -> (Xi [nT,nDOF,nw] complex, status [nT,4]); ``cases`` may
+    carry wave trains (``packer.pack_case_trains``).  ``stats(R, wpow)`` reduces the device Xi to output-channel statistics
+    on the device (raftk_general_channel_stats_dev), so the responses never leave HBM."""
 
     def __init__(self, P, M, B, Cm, cases, device=None):
         import torch
@@ -521,6 +523,8 @@ class GeneralSession:
             self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=self.device)
             self.Xi = torch.zeros([nC, n, nw], dtype=torch.complex128, device=self.device)
             self.status = torch.zeros([nC, 4], dtype=torch.int32, device=self.device)
+        self.n, self.nw, self.n_cases, self.dw = n, nw, nC, float(P["dw"])
+        self._ch = None
 
     def solve(self, n_iter=10, tol=0.01, xi_start=0.0):
         o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
@@ -529,11 +533,33 @@ class GeneralSession:
                                                        self.workspace.data_ptr(), self.workspace_bytes, self.torch.cuda.current_stream(self.device).cuda_stream))
         return self.Xi, self.status
 
+    def stats(self, R, wpow, psd=True, amp=False):
+        """Output-channel statistics of the last ``solve()`` (``packer.pack_general_channels``: R [nch,nDOF], wpow [nch]) on
+        the device -> (std [nT,nch], PSD [nT,nch,nw] or None, amplitudes complex [nT,nch,nw] or None), torch tensors."""
+        torch = self.torch
+        R = np.ascontiguousarray(R, dtype=_F8)
+        wpow = np.ascontiguousarray(wpow, dtype=_I4)
+        if R.ndim != 2 or R.shape[1] != self.n or wpow.shape != (R.shape[0],):
+            raise ValueError("R must be [nch, %d] and wpow [nch]" % self.n)
+        nch = R.shape[0]
+        with torch.cuda.device(self.device):
+            if self._ch is None or not (np.array_equal(self._ch[0], R) and np.array_equal(self._ch[1], wpow)):
+                self._ch = (R, wpow, torch.from_numpy(R).to(self.device), torch.from_numpy(wpow).to(self.device))
+            dR, dp = self._ch[2], self._ch[3]
+            sd = torch.empty([self.n_cases, nch], dtype=torch.float64, device=self.device)
+            P = torch.empty([self.n_cases, nch, self.nw], dtype=torch.float64, device=self.device) if psd else None
+            A = torch.empty([self.n_cases, nch, self.nw], dtype=torch.complex128, device=self.device) if amp else None
+            check(lib.raftk_general_channel_stats_dev(self.n_cases, self.n, nch, self.nw, self.dw, self.keep["w"].data_ptr(), dR.data_ptr(),
+                                                      dp.data_ptr(), self.Xi.data_ptr(), sd.data_ptr(), P.data_ptr() if psd else None,
+                                                      A.data_ptr() if amp else None, torch.cuda.current_stream(self.device).cuda_stream))
+        return sd, P, A
+
 
 def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0):
     """Model.solveDynamics for one FOWT with generalised degrees of freedom (flexible members), host buffers:
     ``P`` from ``packer.pack_general_dofs`` (node tables + ``gen_Tn``, ``gen_rr``), constant system
-    matrices ``M, B, Cm`` [nDOF,nDOF], ``cases`` a CaseTable -> (Xi complex [nC,nDOF,nw], status [nC,4])."""
+    matrices ``M, B, Cm`` [nDOF,nDOF], ``cases`` a CaseTable, with wave trains when built from ``packer.pack_case_trains``
+    (train 0 of a case drives the linearisation, raft_model.py:1200-1236) -> (Xi complex [nT,nDOF,nw], status [nT,4])."""
     n, nw, Ns = int(P["gen_nDOF"]), len(P["w"]), len(P["node_ls"])
     keep = {}
     g = RaftkGeneral()
@@ -562,6 +588,80 @@ def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0
     o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
     check(lib.raftk_general_solve_dynamics_host(C.byref(g), C.byref(c), C.byref(o), Xi.ctypes.data, st.ctypes.data))
     return Xi, st
+
+
+def combine_trains(std, psd, idx):
+    """helpers.getRMS / getPSD of a case with several wave trains (helpers.py:678-700) from per-train reductions ``std``
+    [nT,...] and ``psd`` [nT,...,nw]: the squares sum over the trains ``idx`` -> (sqrt(sum std^2), sum PSD)."""
+    return np.sqrt((std[idx] ** 2).sum(axis=0)), psd[idx].sum(axis=0)
+
+
+def general_channel_stats(R, wpow, w, Xi, dw, psd=True, amp=False):
+    """Output channels of a FOWT with generalised DOFs, Y = w^wpow R Xi (``packer.pack_general_channels``), host buffers:
+    R [nch,nDOF], wpow [nch], w [nw], Xi complex [nU,nDOF,nw] -> (std [nU,nch], PSD [nU,nch,nw] or None,
+    amplitudes complex [nU,nch,nw] or None)."""
+    R = np.ascontiguousarray(R, dtype=_F8)
+    wpow = np.ascontiguousarray(wpow, dtype=_I4)
+    w = np.ascontiguousarray(w, dtype=_F8)
+    Xi = np.ascontiguousarray(Xi, dtype=np.complex128)
+    nU, n, nw = Xi.shape
+    nch = R.shape[0]
+    if R.shape != (nch, n) or wpow.shape != (nch,) or w.shape != (nw,):
+        raise ValueError("R must be [nch,nDOF], wpow [nch], w [nw] for Xi [nU,nDOF,nw]")
+    sd = np.zeros([nU, nch])
+    P = np.zeros([nU, nch, nw]) if psd else None
+    A = np.zeros([nU, nch, nw], dtype=np.complex128) if amp else None
+    check(lib.raftk_general_channel_stats_host(nU, n, nch, nw, float(dw), w.ctypes.data, R.ctypes.data, wpow.ctypes.data, Xi.ctypes.data,
+                                               sd.ctypes.data, P.ctypes.data if psd else None, A.ctypes.data if amp else None))
+    return sd, P, A
+
+
+def general_case_metrics(channels, std, psd, amp, idx):
+    """The entries FOWT.saveTurbineOutputs stores for one case (raft_fowt.py:2299-2604) from per-train channel statistics
+    (std [nT,nch], PSD [nT,nch,nw], amplitudes [nT,nch,nw]) of the case's trains ``idx``: ``*_avg/_std/_max/_min/_PSD`` of every
+    channel, ``*_RA`` of the six PRP motions (all trains plus the zero row of Model.Xi), per-rotor channels as arrays
+    [nrotors] / PSD [nw, nrotors], and the ``Mbase`` alias of a flexible tower's MbaseY (:2599-2604)."""
+    sd, ps = combine_trains(std, psd, idx)
+    names, avg = channels["names"], channels["avg"]
+    nw = psd.shape[-1]
+    nrot = 1 + max([ir for _, ir in names if ir is not None], default=-1)
+    m = {}
+    for k, (nm, ir) in enumerate(names):
+        if ir is None:
+            m[nm + "_avg"], m[nm + "_std"] = avg[k], sd[k]
+            m[nm + "_max"], m[nm + "_min"] = avg[k] + 3 * sd[k], avg[k] - 3 * sd[k]
+            m[nm + "_PSD"] = ps[k]
+            ra = np.zeros([len(idx) + 1, nw], dtype=complex)
+            ra[:-1] = amp[idx, k]
+            m[nm + "_RA"] = ra
+            continue
+        for suffix in ("_avg", "_std", "_max", "_min"):
+            m.setdefault(nm + suffix, np.zeros(nrot))
+        m.setdefault(nm + "_PSD", np.zeros([nw, nrot]))
+        m[nm + "_avg"][ir], m[nm + "_std"][ir] = avg[k], sd[k]
+        m[nm + "_max"][ir], m[nm + "_min"][ir] = avg[k] + 3 * sd[k], avg[k] - 3 * sd[k]
+        m[nm + "_PSD"][:, ir] = ps[k]
+    if "MbaseY_std" in m:
+        for suffix in ("_avg", "_std", "_max", "_min", "_PSD"):
+            m["Mbase" + suffix] = m["MbaseY" + suffix].copy()
+    return m
+
+
+def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0):
+    """Model.analyzeCases (dynamics and output statistics) for one FOWT with generalised degrees of freedom: ``cases`` a list
+    of case dicts, scalar or list-valued wave keys (several wave trains); ``channels`` from ``packer.pack_general_channels``.
+    -> dict(Xi_trains [per case: nTrains,nDOF,nw], status [nC,4] of train 0, case_metrics {case: saveTurbineOutputs entries},
+    empty without channels)."""
+    from .packer import pack_case_trains
+    table, owner, first = pack_case_trains(cases)
+    Xi, st = general_solve_dynamics(P, M, B, Cm, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start)
+    raise_on_flags(st[first])                                           # raft_model.py:1089, :1098-1099
+    metrics = {}
+    if channels is not None:
+        sd, ps, amp = general_channel_stats(channels["R"], channels["wpow"], P["w"], Xi, float(P["dw"]), psd=True, amp=True)
+        for ic in range(len(cases)):
+            metrics[ic] = general_case_metrics(channels, sd, ps, amp, np.nonzero(owner == ic)[0])
+    return dict(Xi_trains=[Xi[owner == ic] for ic in range(len(cases))], status=st[first], case_metrics=metrics)
 
 
 def second_order_force(batch, cases):
