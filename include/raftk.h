@@ -47,7 +47,8 @@ enum {
 enum { RAFTK_SPEC_JONSWAP = 0, RAFTK_SPEC_UNIT = 1, RAFTK_SPEC_CONSTANT = 2, RAFTK_SPEC_NONE = 3 };
 
 /* status word per (design, case): int32[4] = {passes, converged, flags, reserved} */
-enum { RAFTK_FLAG_NAN = 1, RAFTK_FLAG_SINGULAR = 2, RAFTK_FLAG_PLAN = 4 /* step-class tables overflowed the hint */ };
+enum { RAFTK_FLAG_NAN = 1, RAFTK_FLAG_SINGULAR = 2, RAFTK_FLAG_PLAN = 4 /* step-class tables overflowed the hint */,
+       RAFTK_FLAG_XCHG = 8 /* the fused solver's exchange between a unit's CTAs timed out: the unit's results are invalid */ };
 
 /*
  * A batch of nD FOWT designs that share one frequency grid (w, k), water depth and density.

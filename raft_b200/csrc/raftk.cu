@@ -410,7 +410,7 @@ static int run_fused(const raftk_designs *d, const raftk_cases *c, const raftk_s
 }
 
 // ---- fused2 (two bins per thread, TMA-staged plan blob) planner / launcher --------------------------------------------
-struct F2Plan { int CS, nwl, nchunk, maxW, maxH, maxZ; size_t smem, blob, o_lin, o_E, o_A, o_plan, ws_bytes; };
+struct F2Plan { int CS, nwl, nchunk, maxW, maxH, maxZ; size_t smem, blob, o_lin, o_E, o_A, o_plan, o_xrow, o_xcnt, ws_bytes; bool xslots; };
 
 static bool fused2_plan(const raftk_designs *d, int n_cases, int requested_cs, F2Plan &pl)
 {
@@ -436,8 +436,73 @@ static bool fused2_plan(const raftk_designs *d, int n_cases, int requested_cs, F
     pl.o_E = o; o += align_up(units * (size_t)d->max_members * d->nw * sizeof(double2), 256);
     pl.o_A = o; o += align_up(units * (size_t)pl.maxZ * d->nw * sizeof(double2), 256);
     pl.o_plan = o; o += align_up((size_t)d->n_designs * pl.blob * sizeof(double), 256);
+    // exchange rows and arrival counters of the grid variant (k_rao_fused2<true>).  It needs all units x CS CTAs resident
+    // at once, at most 2 per SM (255 registers x 128 threads), so with CS >= 2 only batches of at most one unit per SM
+    // qualify; the rows are sized for the largest cluster (8) so that the workspace does not depend on cluster_size.
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    pl.xslots = units <= (size_t)sms;
+    pl.o_xrow = pl.o_xcnt = 0;
+    if (pl.xslots) {
+        pl.o_xrow = o; o += align_up(units * 2 * 8 * ((size_t)pl.nchunk * 32 + 2) * sizeof(double), 256);
+        pl.o_xcnt = o; o += align_up(units * sizeof(unsigned), 256);
+    }
     pl.ws_bytes = o;
     return true;
+}
+
+// Grid or cluster exchange for k_rao_fused2 (RAFTK_FUSED2_XCHG=cluster|grid overrides, read per call, for A/B runs and
+// tests).  The grid variant runs when a unit spans several CTAs, every CTA of the launch can be resident at once, and the
+// hardware cannot place every unit's cluster at once (cudaOccupancyMaxActiveClusters < units): then the clusters that do not
+// fit would start only when the first units finish.  The occupancy queries are cached per device and launch shape.
+static SmemOptIn g_f2_opt_cluster, g_f2_opt_grid;
+struct F2Occ { int dev, units, CS; size_t smem; int clusters, resident; };
+static std::mutex g_f2_occ_mu;
+static std::vector<F2Occ> g_f2_occ;
+
+static int f2_occupancy(const F2Plan &pl, int units, int &clusters, int &resident)
+{
+    const int dev = cur_dev();
+    {
+        std::lock_guard<std::mutex> lk(g_f2_occ_mu);
+        for (const F2Occ &e : g_f2_occ)
+            if (e.dev == dev && e.units == units && e.CS == pl.CS && e.smem == pl.smem) { clusters = e.clusters; resident = e.resident; return RAFTK_OK; }
+    }
+    CUDA_TRY(g_f2_opt_cluster.ensure(k_rao_fused2<false>, pl.smem));
+    CUDA_TRY(g_f2_opt_grid.ensure(k_rao_fused2<true>, pl.smem));
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3((unsigned)((size_t)units * pl.CS), 1, 1);
+    cfg.blockDim = dim3(F2_T, 1, 1);
+    cfg.dynamicSmemBytes = pl.smem;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = pl.CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    int per_sm = 0, sms = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveClusters(&clusters, k_rao_fused2<false>, &cfg));
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_rao_fused2<true>, F2_T, pl.smem));
+    CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    resident = per_sm * sms;
+    std::lock_guard<std::mutex> lk(g_f2_occ_mu);
+    g_f2_occ.push_back(F2Occ{dev, units, pl.CS, pl.smem, clusters, resident});
+    return RAFTK_OK;
+}
+
+static int f2_pick_grid(const F2Plan &pl, int units, bool &grid)
+{
+    grid = false;
+    const char *x = getenv("RAFTK_FUSED2_XCHG");
+    const bool force_c = x && !strcmp(x, "cluster"), force_g = x && !strcmp(x, "grid");
+    if (x && *x && !force_c && !force_g) return set_err(RAFTK_EINVAL, "RAFTK_FUSED2_XCHG must be 'cluster' or 'grid', not '%s'", x);
+    if (pl.CS <= 1 || force_c) return RAFTK_OK;                 // one CTA per unit: nothing to exchange
+    int clusters = 0, resident = 0;
+    if (int rc = f2_occupancy(pl, units, clusters, resident)) return rc;
+    const bool fits = pl.xslots && (size_t)units * pl.CS <= (size_t)resident;
+    if (force_g && !fits) return set_err(RAFTK_EINVAL, "RAFTK_FUSED2_XCHG=grid: the launch's CTAs cannot all be resident at once");
+    grid = fits && (force_g || clusters < units);
+    return RAFTK_OK;
 }
 
 static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
@@ -478,9 +543,10 @@ static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_
         k_fused_plan<<<d->n_designs, 128, psm, st>>>(D, plan, pl.blob, pl.maxW, pl.maxH, pl.maxZ, pl.nwl);
         g_launches++;
     }
-    static SmemOptIn opt;
-    CUDA_TRY(opt.ensure(k_rao_fused2, pl.smem));
     const int units = d->n_designs * c->n_cases;
+    bool grid = false;
+    if (int rc = f2_pick_grid(pl, units, grid)) return rc;
+    CUDA_TRY(grid ? g_f2_opt_grid.ensure(k_rao_fused2<true>, pl.smem) : g_f2_opt_cluster.ensure(k_rao_fused2<false>, pl.smem));
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3((unsigned)((size_t)units * pl.CS), 1, 1);
@@ -488,8 +554,15 @@ static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_
     cfg.dynamicSmemBytes = pl.smem;
     cfg.stream = st;
     cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = pl.CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    if (grid) {                    // all CTAs resident at once, or the launch fails: the exchange waits cannot deadlock
+        at[0].id = cudaLaunchAttributeCooperative;
+        at[0].val.cooperative = 1;
+        P.xrow = reinterpret_cast<double *>(ws + pl.o_xrow);
+        P.xcnt = reinterpret_cast<unsigned *>(ws + pl.o_xcnt);
+    } else {
+        at[0].id = cudaLaunchAttributeClusterDimension;
+        at[0].val.clusterDim.x = pl.CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    }
     cfg.attrs = at; cfg.numAttrs = 1;
     const int nphase = c->primary ? 2 : 1;
     if (c->primary) P.lin_g = reinterpret_cast<double *>(ws + pl.o_lin);
@@ -497,13 +570,42 @@ static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_
         P.phase = c->primary ? phase : -1;
         {
             ProfScope ps(st, 2);
-            CUDA_TRY(cudaLaunchKernelEx(&cfg, k_rao_fused2, D, C, P));
+            if (grid) {
+                CUDA_TRY(cudaMemsetAsync(P.xcnt, 0, (size_t)units * sizeof(unsigned), st));      // counters count up from 0 per launch
+                CUDA_TRY(cudaLaunchKernelEx(&cfg, k_rao_fused2<true>, D, C, P));
+            } else {
+                CUDA_TRY(cudaLaunchKernelEx(&cfg, k_rao_fused2<false>, D, C, P));
+            }
         }
         g_launches++;
     }
     CUDA_TRY(cudaGetLastError());
     return RAFTK_OK;
 }
+
+#ifdef RAFTK_F2_WAVE_TRACE
+// diagnostic build only: see g_f2_trace (raftk_fused2.cuh) and tools/fused2_waves.py
+extern "C" int raftk_f2_trace_read(unsigned long long *host, int n_cta)
+{
+    if (n_cta < 0 || n_cta > F2_TRACE_MAX) return set_err(RAFTK_EINVAL, "n_cta must be in [0, F2_TRACE_MAX]");
+    CUDA_TRY(cudaMemcpyFromSymbol(host, g_f2_trace, (size_t)n_cta * 3 * sizeof(unsigned long long)));
+    return RAFTK_OK;
+}
+// out: max co-resident clusters of the plan's cluster size, co-resident CTAs of the grid variant, grid variant picked (0/1),
+// cluster size, dynamic shared memory bytes
+extern "C" int raftk_f2_occupancy(const raftk_designs *d, int n_cases, int cluster_size, int out[5])
+{
+    F2Plan pl;
+    if (!fused2_plan(d, n_cases, cluster_size, pl)) return set_err(RAFTK_EINVAL, "not a k_rao_fused2 shape");
+    const int units = d->n_designs * n_cases;
+    int clusters = 0, resident = 0;
+    bool grid = false;
+    if (int rc = f2_occupancy(pl, units, clusters, resident)) return rc;
+    if (int rc = f2_pick_grid(pl, units, grid)) return rc;
+    out[0] = clusters; out[1] = resident; out[2] = grid ? 1 : 0; out[3] = pl.CS; out[4] = (int)pl.smem;
+    return RAFTK_OK;
+}
+#endif
 
 static int run(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
                const double *Xi_in, int mode /*0 solve, 1 linearise, 2 excitation only*/, bool do_excitation,

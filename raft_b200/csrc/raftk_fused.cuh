@@ -32,6 +32,8 @@ struct FusedParams {
     // k_rao_fused2 only: per-design plan blobs (k_fused_plan), member base phases / depth pairs in the workspace
     const double *plan; size_t plan_stride;
     double2 *Eg, *Ag;
+    // k_rao_fused2<true> only: per-unit exchange rows [unit][parity][rank][nchunk*32 + 2] and arrival counters [unit]
+    double *xrow; unsigned *xcnt;
     int n_peers, peer_rank;
     double2 *peer_Xi[RAFTK_MAX_PEERS];    // [p]: this rank's block inside rank p's gathered array, same indexing as Xi_out
     int *peer_status[RAFTK_MAX_PEERS];    // [p]: likewise for status, or NULL

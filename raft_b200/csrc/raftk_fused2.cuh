@@ -6,7 +6,8 @@
 //   * TWO frequency bins per thread.  The node walks of both bins are interleaved instruction by instruction (two
 //     independent E/A recurrences -> ILP 2); the per-node RMS accumulators, the linearised coefficients and the step-class
 //     indices are shared by both bins, so the warp reductions, the coefficient loads and the address arithmetic per bin halve.
-//     A CTA of 128 threads owns 256 bins: cfg2 runs as ONE wave of 4-CTA clusters on 132 SMs instead of two of 8-CTA clusters.
+//     A CTA of 128 threads owns 256 bins: cfg2's 256 CTAs fit the 264 slots of 132 SMs at once (with the grid exchange,
+//     k_rao_fused2<true>: as 4-CTA clusters only 62 of its 64 units fit).
 //   * the per-design tables (member frames and lever arms, node columns, system matrices, step classes with every node's
 //     factor-table offsets) are built ONCE per design by k_fused_plan into a 16-byte aligned blob and staged into shared
 //     memory by ONE TMA bulk copy (cp.async.bulk + mbarrier) instead of being rebuilt with scalar loads by every CTA.
@@ -288,16 +289,77 @@ __device__ __forceinline__ bool conv_ok(double dr, double di, double xr, double 
     return a < rhs * rhs;
 }
 
+#ifdef RAFTK_F2_WAVE_TRACE
+// diagnostic build only (-DRAFTK_F2_WAVE_TRACE, tools/fused2_waves.py): per CTA of the last k_rao_fused2 launch, the SM it
+// ran on and the global timer (ns) at entry and at exit, read back by raftk_f2_trace_read
+#define F2_TRACE_MAX 4096
+__device__ unsigned long long g_f2_trace[3 * F2_TRACE_MAX];
+__device__ __forceinline__ unsigned long long f2_globaltimer()
+{
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+__device__ __forceinline__ void f2_trace(int slot)
+{
+    if (threadIdx.x != 0 || blockIdx.x >= F2_TRACE_MAX) return;
+    unsigned smid;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+    g_f2_trace[3 * blockIdx.x + slot] = f2_globaltimer();
+    if (slot == 1) g_f2_trace[3 * blockIdx.x] = smid;
+}
+#define F2_TRACE(slot) f2_trace(slot)
+#else
+#define F2_TRACE(slot)
+#endif
+
+// Grid variant: RAFTK_FLAG_XCHG once an exchange wait of this CTA timed out, else 0 (kept in shared memory, not in a
+// register: the pass loop has none to spare)
+__device__ __forceinline__ int &f2_xchg_timeout()
+{
+    __shared__ int s_timeout;
+    return s_timeout;
+}
+
+// Grid variant's arrival barrier of one unit's CS CTAs (every thread calls it): the CTA's stores to its exchange row are
+// ordered before one arrival on the unit's counter; thread 0 then polls until `target` arrivals (CS per exchange so far).
+// The launch is cooperative, so every CTA of the unit is resident and the wait ends.  It is still bounded (~2 s at
+// 1.98 GHz): a timeout sets f2_xchg_timeout() instead of hanging the GPU, the CTA publishes it with its next flag word, and
+// every CTA of the unit stops after that pass with RAFTK_FLAG_XCHG in its status.
+__device__ __forceinline__ void f2_xchg_arrive_wait(unsigned *cnt, unsigned target)
+{
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        atomicAdd(cnt, 1u);
+        const long long t0 = clock64();
+        for (;;) {
+            unsigned v;
+            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(cnt) : "memory");
+            if (v >= target) break;
+            if (clock64() - t0 > 4000000000LL) { f2_xchg_timeout() = RAFTK_FLAG_XCHG; break; }
+        }
+    }
+    __syncthreads();
+}
+
+// GRID = false: the CS CTAs of a unit form a thread-block cluster and exchange the per-node RMS partials and the
+// converged / NaN flag words through distributed shared memory.  GRID = true: a cooperative launch without clusters; the
+// same rows go through the L2-resident workspace (P.xrow, P.xcnt), summed in the same rank order, so the results are
+// bit-identical.  The grid variant lets the hardware place the CTAs freely: on an H100, 64 4-CTA clusters of this kernel
+// do not all fit at once (cudaOccupancyMaxActiveClusters = 62) while its 256 CTAs do.
+template <bool GRID>
 __global__ void __launch_bounds__(F2_T, 2)
 k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
 {
+    F2_TRACE(1);
     extern __shared__ __align__(16) double smem_raw[];
     __shared__ __align__(8) unsigned long long mbar;
     constexpr int T = F2_T, nwarps = F2_T / 32;
     __shared__ int s_flw[nwarps];
     cg::cluster_group cluster = cg::this_cluster();
     const int CS = P.CS;
-    const int rank = (CS > 1) ? (int)cluster.block_rank() : 0;
+    const int rank = (CS > 1) ? (GRID ? (int)(blockIdx.x & (CS - 1)) : (int)cluster.block_rank()) : 0;     // CS: 1, 2, 4 or 8
     const int unit = blockIdx.x / CS;
     const int d = unit / Cs.nC, c = unit % Cs.nC;
     const int nw = D.nw, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -337,6 +399,7 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
 
     // ---- stage the design's plan blob with one TMA bulk copy -----------------------------------------------------------
     if (tid == 0) mbar_init(&mbar, 1);
+    if (GRID && tid == 0) f2_xchg_timeout() = 0;
     __syncthreads();
     if (tid == 0) {
         const unsigned bytes = (unsigned)L.total * 8u;
@@ -532,6 +595,10 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
     const double *Aw = D.A_w ? D.A_w + (size_t)d * 36 * nw : nullptr;
     const double *Bw = D.B_w ? D.B_w + (size_t)d * 36 * nw : nullptr;
     int passes = 0, converged = 0, flags = plan_overflow ? RAFTK_FLAG_PLAN : 0, par = 0;
+    // grid variant: this unit's exchange rows [parity][rank][sums_stride] and arrival counter, recomputed where they are used
+    // (kept live across the pass loop they cost spill).  A primary exchanges twice per pass, a secondary train once.
+#define F2_XROW (P.xrow + (size_t)(blockIdx.x / CS) * 2 * CS * sums_stride)
+#define F2_XCNT (P.xcnt + blockIdx.x / CS)
     const int max_pass = plan_overflow ? 0 : (secondary ? 1 : P.n_iter + 1);
     const size_t lin_stride = (size_t)NCOEF * NsP + 36;
     if (secondary && !plan_overflow) {
@@ -682,8 +749,27 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
             double s = 0.0;
             for (int wv = 0; wv < nwarps; wv++) s += s_wpart[(ch * nwarps + wv) * 32 + l];
             s_sums[par * sums_stride + t] = s;
+            if (GRID && CS > 1) F2_XROW[((size_t)par * CS + rank) * sums_stride + t] = s;
         }
-        if (CS > 1) {
+        if (GRID && CS > 1) {
+            // a timeout finishes the pass on incomplete sums; the flag word then makes the whole unit stop (below)
+            f2_xchg_arrive_wait(F2_XCNT, (unsigned)(CS * (2 * it + 1)));
+            const double *xrow = F2_XROW;
+            for (int t = tid; t < nchunk * 32; t += T) {
+                // the rows are read from L2 (ld.global.cg: this SM's L1 may hold the row of two passes ago); same order and
+                // +0.0 padding as the cluster variant below
+                double s = 0.0;
+#pragma unroll 1
+                for (int r0 = 0; r0 < CS; r0 += 4) {
+                    double v[4];
+#pragma unroll
+                    for (int r = 0; r < 4; r++) v[r] = (r0 + r < CS) ? __ldcg(xrow + ((size_t)par * CS + r0 + r) * sums_stride + t) : 0.0;
+#pragma unroll
+                    for (int r = 0; r < 4; r++) s += v[r];
+                }
+                s_tot[t] = s;
+            }
+        } else if (CS > 1) {
             cluster.sync();
             for (int t = tid; t < nchunk * 32; t += T) {
                 // every rank's partial is requested before the first one is used (remote shared-memory reads are
@@ -893,7 +979,24 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
             conv_all = !(all & 1u);
             nan_all = (int)(all >> 1) & (RAFTK_FLAG_NAN | RAFTK_FLAG_SINGULAR);
         }
-        if (CS > 1) {
+        if (GRID && CS > 1) {
+            double *xrow = F2_XROW;
+            if (tid == 0) { double *mine = xrow + ((size_t)par * CS + rank) * sums_stride + nchunk * 32; mine[0] = (double)conv_all; mine[1] = (double)(nan_all | f2_xchg_timeout()); }
+            f2_xchg_arrive_wait(F2_XCNT, (unsigned)(CS * (secondary ? it + 1 : 2 * it + 2)));
+            int ca = 1, na = 0;
+#pragma unroll 1
+            for (int r0 = 0; r0 < CS; r0 += 4) {
+                double fc[4], fn[4];
+#pragma unroll
+                for (int r = 0; r < 4; r++) {
+                    const double *rem = xrow + ((size_t)par * CS + (r0 + r < CS ? r0 + r : 0)) * sums_stride + nchunk * 32;
+                    fc[r] = __ldcg(rem); fn[r] = __ldcg(rem + 1);
+                }
+#pragma unroll
+                for (int r = 0; r < 4; r++) { ca &= (int)fc[r]; na |= (int)fn[r]; }
+            }
+            conv_all = ca; nan_all = na;                // every row is read, this CTA's own included
+        } else if (CS > 1) {
             if (tid == 0) { s_sums[par * sums_stride + nchunk * 32] = (double)conv_all; s_sums[par * sums_stride + nchunk * 32 + 1] = (double)nan_all; }
             cluster.sync();
             int ca = 1, na = 0;
@@ -912,7 +1015,7 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
         }
         par ^= 1;
         flags |= nan_all;
-        if (nan_all & RAFTK_FLAG_NAN) break;
+        if (nan_all & (GRID ? RAFTK_FLAG_NAN | RAFTK_FLAG_XCHG : RAFTK_FLAG_NAN)) break;
         if (conv_all) { converged = 1; break; }
     }
     if (P.status && rank == 0 && tid == 0) {
@@ -941,5 +1044,8 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
                 }
         }
     }
-    if (CS > 1) cluster.sync();
+    if (!GRID && CS > 1) cluster.sync();          // no CTA may leave while a peer still reads its shared memory
+    F2_TRACE(2);
 }
+#undef F2_XROW
+#undef F2_XCNT

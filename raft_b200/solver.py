@@ -357,7 +357,7 @@ def solve_dynamics_farm(batch, cases, C_arr=None, M_arr=None, B_arr=None, n_iter
     return outs
 
 
-FLAG_NAN, FLAG_SINGULAR, FLAG_PLAN = 1, 2, 4        # include/raftk.h RAFTK_FLAG_*
+FLAG_NAN, FLAG_SINGULAR, FLAG_PLAN, FLAG_XCHG = 1, 2, 4, 8        # include/raftk.h RAFTK_FLAG_*
 
 
 def raise_on_flags(status):
@@ -367,6 +367,8 @@ def raise_on_flags(status):
     fl = np.asarray(status)[..., 2]
     if np.any(fl & FLAG_PLAN):
         raise _lib.RaftkError("fused solver: step-class tables overflowed the hint; outputs of those units are zero")
+    if np.any(fl & FLAG_XCHG):
+        raise _lib.RaftkError("fused solver: the exchange between a unit's CTAs timed out; outputs of those units are invalid")
     if np.any(fl & FLAG_SINGULAR) and not np.any(fl & FLAG_NAN):
         raise np.linalg.LinAlgError("Singular matrix")
     if np.any(fl & FLAG_NAN):
