@@ -33,7 +33,7 @@
 extern "C" {
 #endif
 
-#define RAFTK_VERSION 131 /* 0.1.3.1: + native node-table builder for design families (raftk_family_sizes / raftk_build_family_host) */
+#define RAFTK_VERSION 132 /* 0.1.3.2: + raftk_last_dispatch (which kernel variant the last call launched) */
 
 enum {
     RAFTK_OK = 0,
@@ -177,6 +177,49 @@ const char *raftk_last_error(void);
 
 /* Number of CUDA kernel launches issued by this library since load (bench.py "gpu_launches"). */
 long long raftk_launch_count(void);
+
+/*
+ * Which kernel variant the last call on the calling host thread launched.  The entry points pick among several kernels by
+ * shape, workspace size and RAFTK_* environment switches; the launch sites themselves fill this record, so it describes what
+ * ran, not a plan recomputed afterwards.  Every entry point of the solve, second-order force, generalised-DOF, farm and
+ * system-solve families clears it first; a call that fails before its launch leaves it cleared.  When one call launches
+ * several families (a solve that computes its second-order force first, a farm host call) the last launch is reported.
+ * Host bookkeeping only: no device work, no synchronisation.
+ */
+enum { RAFTK_FAMILY_NONE = 0, RAFTK_FAMILY_SOLVE = 1, RAFTK_FAMILY_QTF = 2, RAFTK_FAMILY_GENERAL = 3, RAFTK_FAMILY_FARM = 4,
+       RAFTK_FAMILY_SYSTEM = 5 };
+enum {
+    RAFTK_KERNEL_NONE = 0,
+    RAFTK_KERNEL_V1 = 1,              /* k_depth_table + k_excitation (+ k_drag_solve), tables in the workspace          */
+    RAFTK_KERNEL_FUSED128 = 2,        /* k_rao_fused<128>                                                                 */
+    RAFTK_KERNEL_FUSED256 = 3,        /* k_rao_fused<256>                                                                 */
+    RAFTK_KERNEL_FUSED2_CLUSTER = 4,  /* k_rao_fused2<false>: per-unit sums exchanged through distributed shared memory   */
+    RAFTK_KERNEL_FUSED2_GRID = 5,     /* k_rao_fused2<true>: per-unit sums exchanged through the workspace                */
+    RAFTK_KERNEL_QTF_TILES = 6,       /* k_qtf_tiles + k_qtf_finish                                                       */
+    RAFTK_KERNEL_QTF_DIAG = 7,        /* k_qtf_force<false> (one QTF heading)                                             */
+    RAFTK_KERNEL_QTF_DIAG_MIX = 8,    /* k_qtf_force<true> (heading interpolation)                                        */
+    RAFTK_KERNEL_GEN_BLOCKED = 9,     /* k_gen_solve_blocked                                                              */
+    RAFTK_KERNEL_GEN_UNBLOCKED = 10,  /* k_gen_solve                                                                      */
+    RAFTK_KERNEL_FARM_ROWS12 = 11,    /* k_farm_rows<12>                                                                  */
+    RAFTK_KERNEL_FARM_WARP = 12,      /* k_farm_response<true>                                                            */
+    RAFTK_KERNEL_FARM_BLOCK = 13,     /* k_farm_response<false>                                                           */
+    RAFTK_KERNEL_SYS_UNBLOCKED = 14,  /* k_system_solve, column-at-a-time LU (n <= 24)                                    */
+    RAFTK_KERNEL_SYS_BLOCKED = 15     /* k_system_solve, blocked LU (n > 24)                                              */
+};
+typedef struct raftk_dispatch {
+    int32_t family;           /* RAFTK_FAMILY_*                                                                          */
+    int32_t kernel;           /* RAFTK_KERNEL_*                                                                          */
+    int32_t cluster_size;     /* CTAs per unit (solve family), else 0                                                    */
+    int32_t bins_per_cta;     /* frequency bins per CTA (solve family), else 0                                           */
+    int32_t threads_per_cta;
+    int32_t f0_global;        /* k_rao_fused keeps the linear excitation F0 in the workspace instead of shared memory    */
+    int32_t direct_d2h;       /* host entry point: the solve kernel stored Xi (and status) straight into page-locked host memory */
+    int32_t trains;           /* cases.primary: the fused solver ran its two wave-train phases, or the generalised-DOF
+                                 solve its secondary-train step                                                          */
+    int32_t chunks;           /* v1 solver: launches over design chunks (1 = the whole batch at once)                    */
+    int32_t _pad0;
+} raftk_dispatch;
+int raftk_last_dispatch(raftk_dispatch *out);
 
 /* Per-kernel device timing for the roofline report.  When enabled, every *_dev / *_host call
  * brackets each kernel it launches with CUDA events on the launching stream.

@@ -88,6 +88,12 @@ class RaftkSlender(C.Structure):
                  ("depth", C.c_double), ("rho", C.c_double), ("g", C.c_double)] + [(n, C.c_void_p) for n in SLENDER_ARRAYS])
 
 
+class RaftkDispatch(C.Structure):
+    """include/raftk.h raftk_dispatch: the kernel variant the last call on this thread launched."""
+    _fields_ = [(n, C.c_int32) for n in ("family", "kernel", "cluster_size", "bins_per_cta", "threads_per_cta", "f0_global", "direct_d2h",
+                                         "trains", "chunks", "_pad0")]
+
+
 # every symbol include/raftk.h declares (tests/test_abi.py checks the header against this list)
 
 class RaftkFamilyMember(C.Structure):
@@ -115,7 +121,7 @@ class RaftkFamilyTables(C.Structure):
 
 
 SYMBOLS = [
-    "raftk_version", "raftk_last_error", "raftk_launch_count", "raftk_profile_enable", "raftk_profile_read",
+    "raftk_version", "raftk_last_error", "raftk_launch_count", "raftk_last_dispatch", "raftk_profile_enable", "raftk_profile_read",
     "raftk_workspace_bytes", "raftk_solve_workspace_bytes",
     "raftk_hydro_excitation_dev", "raftk_hydro_linearization_dev", "raftk_solve_dynamics_dev",
     "raftk_hydro_excitation_host", "raftk_hydro_linearization_host", "raftk_solve_dynamics_host",
@@ -151,6 +157,8 @@ def _load():
     lib.raftk_version.restype = C.c_int
     lib.raftk_last_error.restype = C.c_char_p
     lib.raftk_launch_count.restype = C.c_longlong
+    lib.raftk_last_dispatch.argtypes = [P(RaftkDispatch)]
+    lib.raftk_last_dispatch.restype = C.c_int
     lib.raftk_profile_enable.argtypes = [C.c_int]
     lib.raftk_profile_read.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_int)]
     lib.raftk_profile_read.restype = C.c_int

@@ -126,6 +126,23 @@ extern "C" int raftk_version(void) { return RAFTK_VERSION; }
 extern "C" const char *raftk_last_error(void) { return g_err; }
 extern "C" long long raftk_launch_count(void) { return g_launches; }
 
+// ---- record of the kernel variant the last call launched (raftk_last_dispatch) ------------------------------------------
+// Written at the launch sites, per host thread.  disp_reset() at every entry point; disp_launch() next to each launch.
+static thread_local raftk_dispatch g_disp = {};
+static void disp_reset() { memset(&g_disp, 0, sizeof(g_disp)); }
+static void disp_launch(int family, int kernel, int threads, int cluster_size = 0, int bins_per_cta = 0)
+{
+    disp_reset();
+    g_disp.family = family; g_disp.kernel = kernel; g_disp.threads_per_cta = threads;
+    g_disp.cluster_size = cluster_size; g_disp.bins_per_cta = bins_per_cta;
+}
+extern "C" int raftk_last_dispatch(raftk_dispatch *out)
+{
+    if (!out) return set_err(RAFTK_EINVAL, "raftk_last_dispatch: null output");
+    *out = g_disp;
+    return RAFTK_OK;
+}
+
 #include "raftk_common.cuh"
 #include "raftk_tables.cuh"
 #include "raftk_fused.cuh"
@@ -245,6 +262,7 @@ static int run_qtf(const raftk_designs *d, const raftk_cases *c, double *F2, dou
         dim3 gf(6, c->n_cases, P.shared == 1 ? 1 : d->n_designs);
         k_qtf_finish<<<gf, 256, 0, st>>>(C, P);
         g_launches += 2;
+        disp_launch(RAFTK_FAMILY_QTF, RAFTK_KERNEL_QTF_TILES, QT_THREADS);
         CUDA_TRY(cudaGetLastError());
         return RAFTK_OK;
     }
@@ -253,12 +271,14 @@ static int run_qtf(const raftk_designs *d, const raftk_cases *c, double *F2, dou
     if (P.nh > 1) k_qtf_force<true><<<grid, QTF_THREADS, smem, st>>>(C, P);
     else k_qtf_force<false><<<grid, QTF_THREADS, smem, st>>>(C, P);
     g_launches++;
+    disp_launch(RAFTK_FAMILY_QTF, P.nh > 1 ? RAFTK_KERNEL_QTF_DIAG_MIX : RAFTK_KERNEL_QTF_DIAG, QTF_THREADS);
     CUDA_TRY(cudaGetLastError());
     return RAFTK_OK;
 }
 
 extern "C" int raftk_second_order_force_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *out, void *stream)
 {
+    disp_reset();
     if (!out || !out->F_2nd) return set_err(RAFTK_EINVAL, "outputs.F_2nd is required");
     return run_qtf(d, c, out->F_2nd, out->F_2nd_mean, (cudaStream_t)stream);
 }
@@ -360,6 +380,9 @@ static int fused_launch(const DesignsDev &D, const CasesDev &C, const FusedParam
         CUDA_TRY(cudaLaunchKernelEx(&cfg, k_rao_fused<T>, D, C, P));
     }
     g_launches++;
+    disp_launch(RAFTK_FAMILY_SOLVE, T == 128 ? RAFTK_KERNEL_FUSED128 : RAFTK_KERNEL_FUSED256, T, pl.CS, pl.nwl);
+    g_disp.f0_global = P.F0g != nullptr;
+    g_disp.trains = P.phase >= 0;
     CUDA_TRY(cudaGetLastError());
     return RAFTK_OK;
 }
@@ -579,6 +602,8 @@ static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_
         }
         g_launches++;
     }
+    disp_launch(RAFTK_FAMILY_SOLVE, grid ? RAFTK_KERNEL_FUSED2_GRID : RAFTK_KERNEL_FUSED2_CLUSTER, F2_T, pl.CS, pl.nwl);
+    g_disp.trains = c->primary != nullptr;
     CUDA_TRY(cudaGetLastError());
     return RAFTK_OK;
 }
@@ -697,6 +722,11 @@ static int run(const raftk_designs *d, const raftk_cases *c, const raftk_solve_o
             }
             g_launches++;
         }
+        if (d0 == 0) {
+            if (mode != 2) disp_launch(RAFTK_FAMILY_SOLVE, RAFTK_KERNEL_V1, SOLVE_THREADS, pl.CS, pl.nwl);
+            else disp_launch(RAFTK_FAMILY_SOLVE, RAFTK_KERNEL_V1, 128);
+        }
+        g_disp.chunks++;
         CUDA_TRY(cudaGetLastError());
     }
     return RAFTK_OK;
@@ -717,6 +747,7 @@ extern "C" size_t raftk_solve_workspace_bytes(const raftk_designs *d, int32_t n_
 extern "C" int raftk_hydro_excitation_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *out,
                                           void *workspace, size_t workspace_bytes, void *stream)
 {
+    disp_reset();
     if (!out) return set_err(RAFTK_EINVAL, "null outputs");
     if (d && c && chunk_bytes(d->n_designs, c->n_cases, d->max_nodes, d->nw) > workspace_bytes)
         return set_err(RAFTK_ENOMEM, "excitation needs the whole batch's tables in the workspace");
@@ -726,6 +757,7 @@ extern "C" int raftk_hydro_excitation_dev(const raftk_designs *d, const raftk_ca
 extern "C" int raftk_hydro_linearization_dev(const raftk_designs *d, const raftk_cases *c, const double *Xi_in,
                                              const raftk_outputs *out, void *workspace, size_t workspace_bytes, void *stream)
 {
+    disp_reset();
     if (!out || !Xi_in) return set_err(RAFTK_EINVAL, "null outputs / Xi_in");
     return run(d, c, nullptr, out, Xi_in, 1, false, workspace, workspace_bytes, (cudaStream_t)stream);
 }
@@ -733,6 +765,7 @@ extern "C" int raftk_hydro_linearization_dev(const raftk_designs *d, const raftk
 extern "C" int raftk_solve_dynamics_dev(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o,
                                         const raftk_outputs *out, void *workspace, size_t workspace_bytes, void *stream)
 {
+    disp_reset();
     if (!out || !out->Xi || !out->status || !o) return set_err(RAFTK_EINVAL, "Xi, status and opts are required");
     if (d && c && d->n_qtf_w > 0 && !c->F_2nd) {          // potSecOrder 2: the solve computes the force itself (raft_model.py:1035-1038)
         if (!out->F_2nd) return set_err(RAFTK_EINVAL, "designs carry a QTF: pass outputs.F_2nd as the buffer, or cases.F_2nd precomputed");
@@ -793,6 +826,7 @@ extern "C" int raftk_solve_dynamics_gather_dev(const raftk_designs *d, const raf
                                                const raftk_outputs *out, const raftk_peers *peers, void *workspace,
                                                size_t workspace_bytes, void *stream)
 {
+    disp_reset();
     if (!out || !out->Xi || !out->status || !o) return set_err(RAFTK_EINVAL, "Xi, status and opts are required");
     int rc = validate_peers(peers);
     if (rc) return rc;
@@ -822,6 +856,7 @@ extern "C" int raftk_peer_barrier_dev(const raftk_peers *peers, int32_t *timeout
 // ---- farm system solve ----------------------------------------------------------------------------
 extern "C" int raftk_system_solve_dev(int32_t n, int32_t nw, int32_t nrhs, double *Z, double *F, int32_t *info, void *stream)
 {
+    disp_reset();
     if (n <= 0 || nw <= 0 || nrhs <= 0 || !Z || !F) return set_err(RAFTK_EINVAL, "bad system-solve arguments");
     const size_t smem = (size_t)n * (n + nrhs) * sizeof(double2);
     if (smem > 227 * 1024) return set_err(RAFTK_EINVAL, "system too large for the shared-memory solver (n*(n+nrhs)*16 B > 227 KB)");
@@ -829,6 +864,7 @@ extern "C" int raftk_system_solve_dev(int32_t n, int32_t nw, int32_t nrhs, doubl
     CUDA_TRY(opt.ensure(k_system_solve, smem));
     k_system_solve<<<nw, 128, smem, (cudaStream_t)stream>>>(n, nrhs, reinterpret_cast<double2 *>(Z), reinterpret_cast<double2 *>(F), info);
     g_launches++;
+    disp_launch(RAFTK_FAMILY_SYSTEM, n > 24 ? RAFTK_KERNEL_SYS_BLOCKED : RAFTK_KERNEL_SYS_UNBLOCKED, 128);   // k_system_solve's switch
     CUDA_TRY(cudaGetLastError());
     return RAFTK_OK;
 }
@@ -869,6 +905,9 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
         if (rows) k_farm_rows<12><<<dim3((d->nw + 7) / 8, c->n_cases), 128, 0, st>>>(D, C, P);
         else if (warp) k_farm_response<true><<<dim3((d->nw + wpc - 1) / wpc, c->n_cases), 32 * wpc, smem, st>>>(D, C, P);
         else k_farm_response<false><<<dim3(d->nw, c->n_cases), 256, smem, st>>>(D, C, P);
+        if (rows) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_ROWS12, 128);
+        else if (warp) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_WARP, 32 * wpc);
+        else disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_BLOCK, 256);
     }
     g_launches++;
     CUDA_TRY(cudaGetLastError());
@@ -878,6 +917,7 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
 extern "C" int raftk_farm_response_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f,
                                        void *stream)
 {
+    disp_reset();
     return farm_launch(d, c, solved, f, (cudaStream_t)stream);
 }
 
@@ -1059,6 +1099,7 @@ static size_t in_bytes(const raftk_designs *d, const raftk_cases *c)
 static int host_run(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
                     const double *Xi_in, int mode, const raftk_farm *farm = nullptr)
 {
+    disp_reset();
     int rc = validate(d, c);
     if (rc) return rc;
     if (!out) return set_err(RAFTK_EINVAL, "null outputs");
@@ -1201,6 +1242,7 @@ static int host_run(const raftk_designs *d, const raftk_cases *c, const raftk_so
     down(out->zeta, od.zeta, nC * nw * 8);
     down(out->F_2nd, od.F_2nd, resp / 2); down(out->F_2nd_mean, od.F_2nd_mean, nD * nC * 48); down(out->Xi_last, od.Xi_last, resp);
     if (farm) { down(farm->Xi_sys, fd.Xi_sys, resp); down(farm->info, fd.info, nC * nw * 4); }
+    g_disp.direct_d2h = direct_xi;
     cudaError_t se = cudaStreamSynchronize(st);
     if (e != cudaSuccess || se != cudaSuccess)
         return set_err(RAFTK_ECUDA, "kernel/D2H: %s", cudaGetErrorString(se != cudaSuccess ? se : e));
@@ -1233,6 +1275,7 @@ extern "C" int raftk_solve_dynamics_farm_host(const raftk_designs *d, const raft
 
 extern "C" int raftk_second_order_force_host(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *out)
 {
+    disp_reset();
     if (!out || !out->F_2nd) return set_err(RAFTK_EINVAL, "outputs.F_2nd is required");
     int rc = validate_qtf(d, c);
     if (rc) return rc;
@@ -1294,6 +1337,7 @@ extern "C" size_t raftk_general_workspace_bytes(const raftk_general *g, int32_t 
 extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
                                                 int32_t *status, void *workspace, size_t workspace_bytes, void *stream)
 {
+    disp_reset();
     if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
     if (g->n_dof <= 0 || g->n_dof > 256 || g->nw <= 0 || g->n_nodes < 0 || c->n_cases <= 0 || c->n_cases > 65535)
         return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, 0 < n_cases <= 65535");
@@ -1350,6 +1394,8 @@ extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const ra
         k_gen_train_solve<<<dim3(g->nw, (unsigned)nC), 128, 0, st>>>(D, W, prim, X);
         g_launches += 3;
     }
+    disp_launch(RAFTK_FAMILY_GENERAL, blocked ? RAFTK_KERNEL_GEN_BLOCKED : RAFTK_KERNEL_GEN_UNBLOCKED, blocked ? GT : 256);
+    g_disp.trains = prim != nullptr;
     k_gen_status<<<(unsigned)((nC + 127) / 128), 128, 0, st>>>((int)nC, W.flags, prim, status);
     g_launches++;
     CUDA_TRY(cudaGetLastError());
@@ -1359,6 +1405,7 @@ extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const ra
 extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
                                                  int32_t *status)
 {
+    disp_reset();
     if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
     if (g->n_dof <= 0 || g->nw <= 0 || c->n_cases <= 0) return set_err(RAFTK_EINVAL, "general solve: empty problem");
     const size_t n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases;
@@ -1492,6 +1539,7 @@ extern "C" int raftk_qtf_slender_host(const raftk_slender *s, int32_t n_cases, c
 
 extern "C" int raftk_system_solve_host(int32_t n, int32_t nw, int32_t nrhs, double *Z, double *F, int32_t *info)
 {
+    disp_reset();
     if (n <= 0 || nw <= 0 || nrhs <= 0 || !Z || !F) return set_err(RAFTK_EINVAL, "bad system-solve arguments");
     const size_t zb = (size_t)nw * n * n * 16, fb = (size_t)nw * n * nrhs * 16, ib = (size_t)nw * 4;
     ScratchCall sc;

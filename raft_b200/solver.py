@@ -897,6 +897,23 @@ def launch_count():
     return int(lib.raftk_launch_count())
 
 
+DISPATCH_FAMILIES = ("none", "solve", "qtf", "general", "farm", "system")          # include/raftk.h RAFTK_FAMILY_*
+DISPATCH_KERNELS = ("none", "v1", "fused128", "fused256", "fused2-cluster", "fused2-grid", "qtf-tiles", "qtf-diag", "qtf-diag-mix",
+                    "gen-blocked", "gen-unblocked", "farm-rows12", "farm-warp", "farm-block", "sys-unblocked", "sys-blocked")   # RAFTK_KERNEL_*
+
+
+def last_dispatch():
+    """The kernel variant the last library call on this thread launched (raftk_last_dispatch) -> dict(family, kernel,
+    cluster_size, bins_per_cta, threads_per_cta, f0_global, direct_d2h, trains, chunks); family / kernel as names."""
+    r = _lib.RaftkDispatch()
+    check(lib.raftk_last_dispatch(C.byref(r)))
+    d = {n: int(getattr(r, n)) for n, _ in r._fields_ if not n.startswith("_")}
+    d["family"], d["kernel"] = DISPATCH_FAMILIES[d["family"]], DISPATCH_KERNELS[d["kernel"]]
+    for n in ("f0_global", "direct_d2h", "trains"):
+        d[n] = bool(d[n])
+    return d
+
+
 def fp64_peak_gflops(iters=20000):
     return float(lib.raftk_fp64_peak_gflops(int(iters)))
 

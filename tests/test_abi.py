@@ -19,14 +19,16 @@ def header_functions():
     return sorted(set(re.findall(r"\b(raftk_[a-z0-9_]+)\s*\(", src)))
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_declared_symbols_and_version():
+    """Every function include/raftk.h declares is exported and listed in _lib.SYMBOLS, and the library reports the header's
+    RAFTK_VERSION (132 since raftk_last_dispatch was added)."""
     from raft_b200 import _lib
     declared = header_functions()
     assert len(declared) >= 15
     assert sorted(_lib.SYMBOLS) == declared
     for name in declared:
         assert hasattr(_lib.lib, name), name
-    assert _lib.lib.raftk_version() == 131
+    assert _lib.lib.raftk_version() == 132
 
 
 def test_struct_layout_matches_header(tmp_path):
@@ -37,15 +39,37 @@ def test_struct_layout_matches_header(tmp_path):
                     'sizeof(raftk_designs), offsetof(raftk_designs, X_BEM), sizeof(raftk_cases), offsetof(raftk_cases, zeta),'
                     'sizeof(raftk_solve_opts), sizeof(raftk_outputs), offsetof(raftk_designs, node_in_p1_w));'
                     'printf("%zu %zu %zu %zu %zu %zu\\n", sizeof(raftk_family_member), offsetof(raftk_family_member, Ca_End), sizeof(raftk_family),'
-                    'offsetof(raftk_family, members), sizeof(raftk_family_tables), offsetof(raftk_family_tables, max_nodes));return 0;}\n')
+                    'offsetof(raftk_family, members), sizeof(raftk_family_tables), offsetof(raftk_family_tables, max_nodes));'
+                    'printf("%zu %zu %zu %zu\\n", sizeof(raftk_dispatch), offsetof(raftk_dispatch, f0_global), offsetof(raftk_dispatch, chunks),'
+                    'offsetof(raftk_dispatch, trains));return 0;}\n')
     exe = tmp_path / "layout"
     subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(prog), "-o", str(exe)])
     got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
     want = [C.sizeof(_lib.RaftkDesigns), _lib.RaftkDesigns.X_BEM.offset, C.sizeof(_lib.RaftkCases), _lib.RaftkCases.zeta.offset,
             C.sizeof(_lib.RaftkSolveOpts), C.sizeof(_lib.RaftkOutputs), _lib.RaftkDesigns.node_in_p1_w.offset,
             C.sizeof(_lib.RaftkFamilyMember), _lib.RaftkFamilyMember.Ca_End.offset, C.sizeof(_lib.RaftkFamily), _lib.RaftkFamily.members.offset,
-            C.sizeof(_lib.RaftkFamilyTables), _lib.RaftkFamilyTables.max_nodes.offset]
+            C.sizeof(_lib.RaftkFamilyTables), _lib.RaftkFamilyTables.max_nodes.offset,
+            C.sizeof(_lib.RaftkDispatch), _lib.RaftkDispatch.f0_global.offset, _lib.RaftkDispatch.chunks.offset, _lib.RaftkDispatch.trains.offset]
     assert got == want
+
+
+def test_dispatch_record_names_match_header():
+    """solver.last_dispatch() names the RAFTK_FAMILY_* / RAFTK_KERNEL_* values of include/raftk.h in order; a call that fails
+    before launching anything leaves the record cleared."""
+    from raft_b200 import _lib, solver
+    src = open(HEADER).read()
+    fam = dict((m[0], int(m[1])) for m in re.findall(r"RAFTK_FAMILY_([A-Z0-9_]+)\s*=\s*(\d+)", src))
+    ker = dict((m[0], int(m[1])) for m in re.findall(r"RAFTK_KERNEL_([A-Z0-9_]+)\s*=\s*(\d+)", src))
+    assert sorted(fam.values()) == list(range(len(solver.DISPATCH_FAMILIES)))
+    assert sorted(ker.values()) == list(range(len(solver.DISPATCH_KERNELS)))
+    for name, v in fam.items():
+        assert solver.DISPATCH_FAMILIES[v] == name.lower().replace("_", "-"), name
+    for name, v in ker.items():
+        assert solver.DISPATCH_KERNELS[v] == name.lower().replace("_", "-"), name
+    assert _lib.lib.raftk_system_solve_host(0, 1, 1, None, None, None) == -1
+    rec = solver.last_dispatch()
+    assert rec["family"] == "none" and rec["kernel"] == "none" and rec["chunks"] == 0 and not rec["direct_d2h"]
+    assert _lib.lib.raftk_last_dispatch(None) == -1
 
 
 def test_argument_validation_returns_codes():
