@@ -203,9 +203,6 @@ extern "C" size_t raftk_workspace_bytes(const raftk_designs *d, int32_t n_cases)
     return full <= cap ? full : std::max(cap, one);
 }
 
-struct FPlan { int CS, nwl, T, nchunk, maxW, maxH, maxZ; size_t smem; bool f0_global; };
-static bool fused_plan(const raftk_designs *d, int units, int requested_cs, bool have_ws, FPlan &pl);
-
 static int validate(const raftk_designs *d, const raftk_cases *c)
 {
     if (!d || !c) return set_err(RAFTK_EINVAL, "null designs/cases");
@@ -283,98 +280,180 @@ extern "C" int raftk_second_order_force_dev(const raftk_designs *d, const raftk_
     return run_qtf(d, c, out->F_2nd, out->F_2nd_mean, (cudaStream_t)stream);
 }
 
-static int pick_cluster(int units, int nw, int requested)
+// ---- the rigid solve's plan --------------------------------------------------------------------------------------------
+// One decision for every entry point: which kernel solves (k_rao_fused2, k_rao_fused<T> or k_drag_solve on the v1 tables
+// path), at what cluster size, and how the workspace is laid out.  The size queries, the host entry points and the launches
+// all read the plan made here.
+
+static int sm_count()                 // 132 (an H100 SXM) when no device answers, so that the size queries work without one
 {
-    if (requested == 1 || requested == 2 || requested == 4 || requested == 8) {
-        int cs = requested;
-        while (cs > 1 && nw / cs < 32) cs >>= 1;
-        return cs;
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+        cudaGetLastError();
+        return 132;
     }
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int cs = 1;
-    // fill ~2 CTAs per SM, keep >= 128 frequencies per CTA, and keep 12*nwl doubles of state <= 48 KB
-    while (cs < 8 && (units * cs < 2 * sms || nw / cs > 512) && nw / (cs * 2) >= 128) cs <<= 1;
-    return cs;
+    return sms;
 }
 
-struct Plan { int CS, nwl, nchunk; size_t smem; };
-
-static int make_plan(const raftk_designs *d, int units_hint, int requested_cs, Plan &pl)
+// ctas CTAs of `threads` threads with smem bytes of dynamic shared memory on st, in thread-block clusters of cs CTAs; at is
+// the cluster attribute cfg points to
+static void cluster_config(cudaLaunchConfig_t &cfg, cudaLaunchAttribute &at, size_t ctas, int threads, size_t smem, int cs, cudaStream_t st)
 {
-    pl.CS = pick_cluster(units_hint, d->nw, requested_cs);
-    pl.nwl = (d->nw + pl.CS - 1) / pl.CS;
-    pl.nchunk = (d->max_nodes + CHUNK_NODES - 1) / CHUNK_NODES;
-    pl.smem = smem_doubles(d->max_members, d->max_nodes, pl.nchunk, SOLVE_THREADS / 32, pl.nwl) * sizeof(double)
-              + (size_t)d->max_members * 3 * sizeof(int) + 16;
-    if (pl.smem > 227 * 1024) return set_err(RAFTK_EINVAL, "shared-memory plan exceeds 227 KB (nw per CTA too large)");
-    return 0;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3((unsigned)ctas, 1, 1);
+    cfg.blockDim = dim3(threads, 1, 1);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    at.id = cudaLaunchAttributeClusterDimension;
+    at.val.clusterDim.x = cs; at.val.clusterDim.y = 1; at.val.clusterDim.z = 1;
+    cfg.attrs = &at; cfg.numAttrs = 1;
 }
 
-// ---- fused (v2) planner / launcher -----------------------------------------------------------------
+enum SolveKind { SOLVE_V1, SOLVE_FUSED, SOLVE_FUSED2 };
+struct SolvePlan {
+    SolveKind kind;
+    int CS, nwl, T, nchunk, maxW, maxH, maxZ;    // cluster size, bins and threads per CTA, node chunks, step-class maxima
+    size_t smem;
+    bool f0_global;                              // k_rao_fused<T>: F0 in the workspace instead of shared memory
+    // Workspace of the fused kernels: F0 [units][6][nw] at 0, the wave-train hand-over [units][NCOEF*max_nodes + 36] from
+    // o_lin to lin_end; k_rao_fused2 adds Eg, Ag, the plan blobs (blob doubles per design) and, with xslots, the grid
+    // variant's exchange rows and arrival counters.  bytes: what the plan needs (v1: the tables' whole budget).
+    size_t o_lin, lin_end, o_E, o_A, o_plan, blob, o_xrow, o_xcnt, bytes;
+    bool xslots;
+    int per;                                     // v1: designs per chunk of tables
+};
+static const size_t WS_UNBOUNDED = SIZE_MAX;     // plan to size a workspace: it will hold whatever the plan needs
 
-static bool fused_try(const raftk_designs *d, int cs, bool have_ws, FPlan &pl)
+// Plan a solve of d x n_cases against wbytes of workspace.  requested_cs: the caller's cluster size when it is 1, 2, 4 or 8,
+// else the planner picks one.  v1_only: the tables path (excitation, linearisation), as RAFTK_FORCE_V1 does for the solve.
+static SolvePlan plan_solve(const raftk_designs *d, int n_cases, int requested_cs, size_t wbytes, bool v1_only = false)
 {
-    pl.CS = cs;
-    pl.nwl = (d->nw + cs - 1) / cs;
-    pl.T = pl.nwl > 128 ? 256 : 128;
-    pl.nchunk = (d->max_nodes + CHUNK_NODES - 1) / CHUNK_NODES;
-    pl.maxW = d->max_w_classes > 0 ? d->max_w_classes : d->max_nodes;
-    pl.maxH = d->max_h_classes > 0 ? d->max_h_classes : d->max_nodes;
-    pl.maxZ = d->max_z_classes > 0 ? std::min(d->max_z_classes, d->max_members) : d->max_members;
-    // 255 registers cap residency at 256 threads per SM (at 168 registers for 3 CTAs the LU spills); shared memory must allow 2 CTAs of 128 threads or 1 of 256.  The linear excitation F0 lives in
-    // shared memory when it fits, else in the caller's workspace.
-    const size_t limit = (pl.T == 128) ? (size_t)112 * 1024 : (size_t)226 * 1024;
-    pl.f0_global = false;
-    pl.smem = fused_smem_bytes(d->max_members, d->max_nodes, pl.nchunk, pl.T / 32, pl.nwl, pl.maxW, pl.maxH, pl.maxZ, true);
-    if (pl.smem > limit && have_ws) {
-        pl.f0_global = true;
-        pl.smem = fused_smem_bytes(d->max_members, d->max_nodes, pl.nchunk, pl.T / 32, pl.nwl, pl.maxW, pl.maxH, pl.maxZ, false);
-    }
-    return pl.smem <= limit && pl.nwl <= 2 * pl.T;
-}
+    const int nw = d->nw;
+    const size_t units = (size_t)d->n_designs * n_cases;
+    const int sms = sm_count();
+    // k_rao_fused2 takes a requested cluster size as given; the one-bin kernels halve it while a CTA would get < 32 bins
+    const int req = (requested_cs == 1 || requested_cs == 2 || requested_cs == 4 || requested_cs == 8) ? requested_cs : 0;
+    int req_halved = req;
+    while (req_halved > 1 && nw / req_halved < 32) req_halved >>= 1;
 
-static bool fused_plan(const raftk_designs *d, int units, int requested_cs, bool have_ws, FPlan &pl)
-{
-    if (getenv("RAFTK_FORCE_V1")) return false;
-    if (requested_cs == 1 || requested_cs == 2 || requested_cs == 4 || requested_cs == 8) {
-        int cs = requested_cs;
-        while (cs > 1 && d->nw / cs < 32) cs >>= 1;
-        return fused_try(d, cs, have_ws, pl);
-    }
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    FPlan best; bool have = false;
-    if (units >= 4 * sms) {                       // plenty of units: smallest cluster whose slice fits on chip
-        for (int cs = 1; cs <= 8 && !have; cs <<= 1) { FPlan t; if (fused_try(d, cs, have_ws, t) && t.nwl <= t.T) { best = t; have = true; } }
-        for (int cs = 1; cs <= 8 && !have; cs <<= 1) { FPlan t; if (fused_try(d, cs, have_ws, t)) { best = t; have = true; } }
-    } else {                                      // few units: largest cluster that keeps >= 128 bins per CTA
-        for (int cs = 8; cs >= 1 && !have; cs >>= 1) {
-            if (cs > 1 && d->nw / cs < 128) continue;
-            FPlan t; if (fused_try(d, cs, have_ws, t)) { best = t; have = true; }
+    SolvePlan base;
+    memset(&base, 0, sizeof(base));
+    base.nchunk = (d->max_nodes + CHUNK_NODES - 1) / CHUNK_NODES;
+    base.maxW = d->max_w_classes > 0 ? d->max_w_classes : d->max_nodes;
+    base.maxH = d->max_h_classes > 0 ? d->max_h_classes : d->max_nodes;
+    base.maxZ = d->max_z_classes > 0 ? std::min(d->max_z_classes, d->max_members) : d->max_members;
+    const size_t f0 = units * 6 * nw * sizeof(double2);
+    base.o_lin = align_up(f0, 256);
+    base.lin_end = base.o_lin + units * ((size_t)NCOEF * d->max_nodes + 36) * sizeof(double);
+
+    if (!v1_only && !getenv("RAFTK_FORCE_V1") && d->max_nodes > 0 && d->max_members > 0) {
+        SolvePlan p = base;
+        p.kind = SOLVE_FUSED2; p.T = F2_T;
+        p.CS = req;
+        if (!p.CS) for (p.CS = 1; p.CS < 8 && (nw + p.CS - 1) / p.CS > 2 * F2_T; p.CS <<= 1) {}
+        p.nwl = (nw + p.CS - 1) / p.CS;
+        // two bins per thread pay when most threads own two: 192 < bins per CTA <= 256; otherwise the one-bin kernel runs
+        if (p.nwl <= 2 * F2_T && p.nwl > (3 * F2_T) / 2) {
+            p.smem = fused2_smem_bytes(d->max_members, d->max_nodes, p.nchunk, p.nwl, p.maxW, p.maxH, p.maxZ);
+            p.blob = (size_t)plan_layout(d->max_members, d->max_nodes, p.maxW, p.maxH, p.maxZ).total;
+            size_t o = align_up(p.lin_end, 256);
+            p.o_E = o; o += align_up(units * (size_t)d->max_members * nw * sizeof(double2), 256);
+            p.o_A = o; o += align_up(units * (size_t)p.maxZ * nw * sizeof(double2), 256);
+            p.o_plan = o; o += align_up((size_t)d->n_designs * p.blob * sizeof(double), 256);
+            // exchange rows and arrival counters of the grid variant (k_rao_fused2<true>).  It needs all units x CS CTAs
+            // resident at once, at most 2 per SM (255 registers x 128 threads), so with CS >= 2 only batches of at most one
+            // unit per SM qualify; the rows are sized for the largest cluster (8) so that the workspace does not depend on
+            // cluster_size.
+            p.xslots = units <= (size_t)sms;
+            if (p.xslots) {
+                p.o_xrow = o; o += align_up(units * 2 * 8 * ((size_t)p.nchunk * 32 + 2) * sizeof(double), 256);
+                p.o_xcnt = o; o += align_up(units * sizeof(unsigned), 256);
+            }
+            p.bytes = o;
+            if (p.smem <= (size_t)113 * 1024 && wbytes >= p.bytes) return p;           // two CTAs per SM
+        }
+        // k_rao_fused<T> at cluster size cs.  255 registers cap residency at 256 threads per SM (at 168 registers for 3 CTAs
+        // the LU spills); shared memory must allow 2 CTAs of 128 threads or 1 of 256.  F0 lives in shared memory when it
+        // fits, else in the caller's workspace.
+        auto fused = [&](int cs) {
+            p = base;
+            p.kind = SOLVE_FUSED;
+            p.CS = cs;
+            p.nwl = (nw + cs - 1) / cs;
+            p.T = p.nwl > 128 ? 256 : 128;
+            p.bytes = align_up(p.lin_end, 256);
+            const size_t limit = (p.T == 128) ? (size_t)112 * 1024 : (size_t)226 * 1024;
+            p.smem = fused_smem_bytes(d->max_members, d->max_nodes, p.nchunk, p.T / 32, p.nwl, p.maxW, p.maxH, p.maxZ, true);
+            if (p.smem > limit && wbytes >= f0) {
+                p.f0_global = true;
+                p.smem = fused_smem_bytes(d->max_members, d->max_nodes, p.nchunk, p.T / 32, p.nwl, p.maxW, p.maxH, p.maxZ, false);
+            }
+            return p.smem <= limit && p.nwl <= 2 * p.T;
+        };
+        if (req_halved) {
+            if (fused(req_halved)) return p;
+        } else if (units >= (size_t)4 * sms) {     // plenty of units: smallest cluster whose slice fits on chip
+            for (int cs = 1; cs <= 8; cs <<= 1) if (fused(cs) && p.nwl <= p.T) return p;
+            for (int cs = 1; cs <= 8; cs <<= 1) if (fused(cs)) return p;
+        } else {                                   // few units: largest cluster that keeps >= 128 bins per CTA
+            for (int cs = 8; cs >= 1; cs >>= 1) if ((cs == 1 || nw / cs >= 128) && fused(cs)) return p;
         }
     }
-    if (have) pl = best;
-    return have;
+
+    // v1: the tables take the whole workspace, in chunks of at most 65535 designs
+    SolvePlan p = base;
+    p.kind = SOLVE_V1;
+    p.T = SOLVE_THREADS;
+    p.bytes = wbytes == WS_UNBOUNDED ? raftk_workspace_bytes(d, n_cases) : wbytes;
+    p.per = d->n_designs;
+    while (p.per > 1 && (chunk_bytes(p.per, n_cases, d->max_nodes, nw) > p.bytes || p.per > 65535)) p.per = (p.per + 1) / 2;
+    p.CS = req_halved;
+    if (!p.CS)     // fill ~2 CTAs per SM, keep >= 128 frequencies per CTA, and keep 12*nwl doubles of state <= 48 KB
+        for (p.CS = 1; p.CS < 8 && ((size_t)p.per * n_cases * p.CS < (size_t)2 * sms || nw / p.CS > 512) && nw / (p.CS * 2) >= 128; p.CS <<= 1) {}
+    p.nwl = (nw + p.CS - 1) / p.CS;
+    p.smem = smem_doubles(d->max_members, d->max_nodes, p.nchunk, SOLVE_THREADS / 32, p.nwl) * sizeof(double)
+             + (size_t)d->max_members * 3 * sizeof(int) + 16;
+    return p;
+}
+
+// ---- fused launchers ---------------------------------------------------------------------------------------------------
+
+// Parameters both fused kernels take: zeroed, then the options, the outputs, Xi_init and, with peers, this rank's block in
+// every rank's gathered arrays (each finished unit's Xi and status are stored there too).
+static FusedParams fused_params(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
+                                const SolvePlan &pl, const raftk_peers *peers)
+{
+    FusedParams P;
+    memset(&P, 0, sizeof(P));
+    P.n_iter = o->n_iter; P.CS = pl.CS; P.nwl = pl.nwl; P.maxW = pl.maxW; P.maxH = pl.maxH; P.maxZ = pl.maxZ;
+    P.tol = o->tol; P.xi_start = o->xi_start;
+    P.Xi_out = reinterpret_cast<double2 *>(out->Xi);
+    P.Fdrag_out = reinterpret_cast<double2 *>(out->F_drag);
+    P.Finer_out = reinterpret_cast<double2 *>(out->F_iner);
+    P.Fbem_out = reinterpret_cast<double2 *>(out->F_BEM);
+    P.Bdrag_out = out->B_drag; P.zeta_out = out->zeta; P.status = out->status;
+    P.Xilast_out = reinterpret_cast<double2 *>(out->Xi_last);
+    P.Xi_init = reinterpret_cast<const double2 *>(c->Xi_init);
+    P.phase = -1;
+    if (peers && peers->n_ranks > 1) {
+        P.n_peers = peers->n_ranks; P.peer_rank = peers->rank;
+        const size_t units_per_rank = peers->block_elems / ((size_t)6 * d->nw);
+        for (int p = 0; p < peers->n_ranks; p++) {
+            P.peer_Xi[p] = reinterpret_cast<double2 *>(peers->gathered[p]) + (size_t)peers->rank * peers->block_elems;
+            P.peer_status[p] = peers->status[p] ? peers->status[p] + (size_t)peers->rank * units_per_rank * 4 : nullptr;
+        }
+    }
+    return P;
 }
 
 template <int T>
-static int fused_launch(const DesignsDev &D, const CasesDev &C, const FusedParams &P, const FPlan &pl, int units, cudaStream_t st)
+static int fused_launch(const DesignsDev &D, const CasesDev &C, const FusedParams &P, const SolvePlan &pl, int units, cudaStream_t st)
 {
     static SmemOptIn opt;
     CUDA_TRY(opt.ensure(k_rao_fused<T>, pl.smem));
     cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)((size_t)units * pl.CS), 1, 1);
-    cfg.blockDim = dim3(T, 1, 1);
-    cfg.dynamicSmemBytes = pl.smem;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = pl.CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
+    cudaLaunchAttribute at;
+    cluster_config(cfg, at, (size_t)units * pl.CS, T, pl.smem, pl.CS, st);
     {
         ProfScope ps(st, 2);
         CUDA_TRY(cudaLaunchKernelEx(&cfg, k_rao_fused<T>, D, C, P));
@@ -388,39 +467,17 @@ static int fused_launch(const DesignsDev &D, const CasesDev &C, const FusedParam
 }
 
 static int run_fused(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
-                     const FPlan &pl, void *workspace, size_t wbytes, cudaStream_t st, const raftk_peers *peers = nullptr)
+                     const SolvePlan &pl, void *workspace, size_t wbytes, cudaStream_t st, const raftk_peers *peers)
 {
     prof_begin_call();
     DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
     CasesDev C = to_dev(c);
-    FusedParams P;
-    P.n_iter = o->n_iter; P.CS = pl.CS; P.nwl = pl.nwl; P.maxW = pl.maxW; P.maxH = pl.maxH; P.maxZ = pl.maxZ;
-    P.tol = o->tol; P.xi_start = o->xi_start;
-    P.Xi_out = reinterpret_cast<double2 *>(out->Xi);
-    P.Fdrag_out = reinterpret_cast<double2 *>(out->F_drag);
-    P.Finer_out = reinterpret_cast<double2 *>(out->F_iner);
-    P.Fbem_out = reinterpret_cast<double2 *>(out->F_BEM);
-    P.Bdrag_out = out->B_drag; P.zeta_out = out->zeta; P.status = out->status;
-    P.Xilast_out = reinterpret_cast<double2 *>(out->Xi_last);
-    P.Xi_init = reinterpret_cast<const double2 *>(c->Xi_init);
+    FusedParams P = fused_params(d, c, o, out, pl, peers);
     P.F0g = pl.f0_global ? reinterpret_cast<double2 *>(workspace) : nullptr;
     const int units = d->n_designs * c->n_cases;
-    P.lin_g = nullptr; P.phase = -1;
-    P.n_peers = 0; P.peer_rank = 0;
-    for (int p = 0; p < RAFTK_MAX_PEERS; p++) { P.peer_Xi[p] = nullptr; P.peer_status[p] = nullptr; }
-    if (peers && peers->n_ranks > 1) {
-        P.n_peers = peers->n_ranks; P.peer_rank = peers->rank;
-        const size_t units_per_rank = peers->block_elems / ((size_t)6 * d->nw);
-        for (int p = 0; p < peers->n_ranks; p++) {
-            P.peer_Xi[p] = reinterpret_cast<double2 *>(peers->gathered[p]) + (size_t)peers->rank * peers->block_elems;
-            P.peer_status[p] = peers->status[p] ? peers->status[p] + (size_t)peers->rank * units_per_rank * 4 : nullptr;
-        }
-    }
     if (c->primary) {                                  // wave trains: primaries first, then the trains that follow them
-        const size_t f0b = align_up((size_t)units * 6 * d->nw * sizeof(double2), 256);
-        const size_t need = f0b + (size_t)units * ((size_t)NCOEF * d->max_nodes + 36) * sizeof(double);
-        if (!workspace || wbytes < need) return set_err(RAFTK_ENOMEM, "wave-train cases need raftk_solve_workspace_bytes() of workspace");
-        P.lin_g = reinterpret_cast<double *>(static_cast<char *>(workspace) + f0b);
+        if (!workspace || wbytes < pl.lin_end) return set_err(RAFTK_ENOMEM, "wave-train cases need raftk_solve_workspace_bytes() of workspace");
+        P.lin_g = reinterpret_cast<double *>(static_cast<char *>(workspace) + pl.o_lin);
         for (int phase = 0; phase < 2; phase++) {
             P.phase = phase;
             const int rc = (pl.T == 128) ? fused_launch<128>(D, C, P, pl, units, st) : fused_launch<256>(D, C, P, pl, units, st);
@@ -432,49 +489,6 @@ static int run_fused(const raftk_designs *d, const raftk_cases *c, const raftk_s
     return fused_launch<256>(D, C, P, pl, units, st);
 }
 
-// ---- fused2 (two bins per thread, TMA-staged plan blob) planner / launcher --------------------------------------------
-struct F2Plan { int CS, nwl, nchunk, maxW, maxH, maxZ; size_t smem, blob, o_lin, o_E, o_A, o_plan, o_xrow, o_xcnt, ws_bytes; bool xslots; };
-
-static bool fused2_plan(const raftk_designs *d, int n_cases, int requested_cs, F2Plan &pl)
-{
-    if (getenv("RAFTK_FORCE_V1") || getenv("RAFTK_FUSED_GEN1")) return false;      // A/B: first-generation fused kernel
-    if (d->max_nodes <= 0 || d->max_members <= 0) return false;
-    int cs;
-    if (requested_cs == 1 || requested_cs == 2 || requested_cs == 4 || requested_cs == 8) cs = requested_cs;
-    else { cs = 1; while (cs < 8 && (d->nw + cs - 1) / cs > 2 * F2_T) cs <<= 1; }
-    pl.CS = cs;
-    pl.nwl = (d->nw + cs - 1) / cs;
-    // two bins per thread pay when most threads own two: 192 < bins per CTA <= 256; otherwise the one-bin kernel runs
-    if (pl.nwl > 2 * F2_T || pl.nwl <= (3 * F2_T) / 2) return false;
-    pl.nchunk = (d->max_nodes + CHUNK_NODES - 1) / CHUNK_NODES;
-    pl.maxW = d->max_w_classes > 0 ? d->max_w_classes : d->max_nodes;
-    pl.maxH = d->max_h_classes > 0 ? d->max_h_classes : d->max_nodes;
-    pl.maxZ = d->max_z_classes > 0 ? std::min(d->max_z_classes, d->max_members) : d->max_members;
-    pl.smem = fused2_smem_bytes(d->max_members, d->max_nodes, pl.nchunk, pl.nwl, pl.maxW, pl.maxH, pl.maxZ);
-    if (pl.smem > (size_t)113 * 1024) return false;                               // two CTAs per SM
-    const size_t units = (size_t)d->n_designs * n_cases;
-    pl.blob = (size_t)plan_layout(d->max_members, d->max_nodes, pl.maxW, pl.maxH, pl.maxZ).total;
-    size_t o = align_up(units * 6 * d->nw * sizeof(double2), 256);                 // F0 (same place as the first-generation kernel)
-    pl.o_lin = o; o += align_up(units * ((size_t)NCOEF * d->max_nodes + 36) * sizeof(double), 256);
-    pl.o_E = o; o += align_up(units * (size_t)d->max_members * d->nw * sizeof(double2), 256);
-    pl.o_A = o; o += align_up(units * (size_t)pl.maxZ * d->nw * sizeof(double2), 256);
-    pl.o_plan = o; o += align_up((size_t)d->n_designs * pl.blob * sizeof(double), 256);
-    // exchange rows and arrival counters of the grid variant (k_rao_fused2<true>).  It needs all units x CS CTAs resident
-    // at once, at most 2 per SM (255 registers x 128 threads), so with CS >= 2 only batches of at most one unit per SM
-    // qualify; the rows are sized for the largest cluster (8) so that the workspace does not depend on cluster_size.
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    pl.xslots = units <= (size_t)sms;
-    pl.o_xrow = pl.o_xcnt = 0;
-    if (pl.xslots) {
-        pl.o_xrow = o; o += align_up(units * 2 * 8 * ((size_t)pl.nchunk * 32 + 2) * sizeof(double), 256);
-        pl.o_xcnt = o; o += align_up(units * sizeof(unsigned), 256);
-    }
-    pl.ws_bytes = o;
-    return true;
-}
-
 // Grid or cluster exchange for k_rao_fused2 (RAFTK_FUSED2_XCHG=cluster|grid overrides, read per call, for A/B runs and
 // tests).  The grid variant runs when a unit spans several CTAs, every CTA of the launch can be resident at once, and the
 // hardware cannot place every unit's cluster at once (cudaOccupancyMaxActiveClusters < units): then the clusters that do not
@@ -484,7 +498,7 @@ struct F2Occ { int dev, units, CS; size_t smem; int clusters, resident; };
 static std::mutex g_f2_occ_mu;
 static std::vector<F2Occ> g_f2_occ;
 
-static int f2_occupancy(const F2Plan &pl, int units, int &clusters, int &resident)
+static int f2_occupancy(const SolvePlan &pl, int units, int &clusters, int &resident)
 {
     const int dev = cur_dev();
     {
@@ -495,25 +509,18 @@ static int f2_occupancy(const F2Plan &pl, int units, int &clusters, int &residen
     CUDA_TRY(g_f2_opt_cluster.ensure(k_rao_fused2<false>, pl.smem));
     CUDA_TRY(g_f2_opt_grid.ensure(k_rao_fused2<true>, pl.smem));
     cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)((size_t)units * pl.CS), 1, 1);
-    cfg.blockDim = dim3(F2_T, 1, 1);
-    cfg.dynamicSmemBytes = pl.smem;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = pl.CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    int per_sm = 0, sms = 0;
+    cudaLaunchAttribute at;
+    cluster_config(cfg, at, (size_t)units * pl.CS, F2_T, pl.smem, pl.CS, 0);
+    int per_sm = 0;
     CUDA_TRY(cudaOccupancyMaxActiveClusters(&clusters, k_rao_fused2<false>, &cfg));
     CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_rao_fused2<true>, F2_T, pl.smem));
-    CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    resident = per_sm * sms;
+    resident = per_sm * sm_count();
     std::lock_guard<std::mutex> lk(g_f2_occ_mu);
     g_f2_occ.push_back(F2Occ{dev, units, pl.CS, pl.smem, clusters, resident});
     return RAFTK_OK;
 }
 
-static int f2_pick_grid(const F2Plan &pl, int units, bool &grid)
+static int f2_pick_grid(const SolvePlan &pl, int units, bool &grid)
 {
     grid = false;
     const char *x = getenv("RAFTK_FUSED2_XCHG");
@@ -529,37 +536,18 @@ static int f2_pick_grid(const F2Plan &pl, int units, bool &grid)
 }
 
 static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
-                      const F2Plan &pl, void *workspace, cudaStream_t st, const raftk_peers *peers)
+                      const SolvePlan &pl, void *workspace, cudaStream_t st, const raftk_peers *peers)
 {
     prof_begin_call();
     DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
     CasesDev C = to_dev(c);
     char *ws = static_cast<char *>(workspace);
-    FusedParams P;
-    memset(&P, 0, sizeof(P));
-    P.n_iter = o->n_iter; P.CS = pl.CS; P.nwl = pl.nwl; P.maxW = pl.maxW; P.maxH = pl.maxH; P.maxZ = pl.maxZ;
-    P.tol = o->tol; P.xi_start = o->xi_start;
-    P.Xi_out = reinterpret_cast<double2 *>(out->Xi);
-    P.Fdrag_out = reinterpret_cast<double2 *>(out->F_drag);
-    P.Finer_out = reinterpret_cast<double2 *>(out->F_iner);
-    P.Fbem_out = reinterpret_cast<double2 *>(out->F_BEM);
-    P.Bdrag_out = out->B_drag; P.zeta_out = out->zeta; P.status = out->status;
-    P.Xilast_out = reinterpret_cast<double2 *>(out->Xi_last);
-    P.Xi_init = reinterpret_cast<const double2 *>(c->Xi_init);
+    FusedParams P = fused_params(d, c, o, out, pl, peers);
     P.F0g = reinterpret_cast<double2 *>(ws);
-    P.lin_g = nullptr; P.phase = -1;
     P.Eg = reinterpret_cast<double2 *>(ws + pl.o_E);
     P.Ag = reinterpret_cast<double2 *>(ws + pl.o_A);
     double *plan = reinterpret_cast<double *>(ws + pl.o_plan);
     P.plan = plan; P.plan_stride = pl.blob;
-    if (peers && peers->n_ranks > 1) {
-        P.n_peers = peers->n_ranks; P.peer_rank = peers->rank;
-        const size_t units_per_rank = peers->block_elems / ((size_t)6 * d->nw);
-        for (int p = 0; p < peers->n_ranks; p++) {
-            P.peer_Xi[p] = reinterpret_cast<double2 *>(peers->gathered[p]) + (size_t)peers->rank * peers->block_elems;
-            P.peer_status[p] = peers->status[p] ? peers->status[p] + (size_t)peers->rank * units_per_rank * 4 : nullptr;
-        }
-    }
     if (!(o->flags & RAFTK_SOLVE_REUSE_PLAN)) {
         ProfScope ps(st, 0);
         const size_t psm = (3 * (size_t)d->max_nodes + d->max_members) * sizeof(double) + (2 * (size_t)d->max_nodes + 2 * d->max_members) * sizeof(int);
@@ -571,22 +559,14 @@ static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_
     if (int rc = f2_pick_grid(pl, units, grid)) return rc;
     CUDA_TRY(grid ? g_f2_opt_grid.ensure(k_rao_fused2<true>, pl.smem) : g_f2_opt_cluster.ensure(k_rao_fused2<false>, pl.smem));
     cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)((size_t)units * pl.CS), 1, 1);
-    cfg.blockDim = dim3(F2_T, 1, 1);
-    cfg.dynamicSmemBytes = pl.smem;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
+    cudaLaunchAttribute at;
+    cluster_config(cfg, at, (size_t)units * pl.CS, F2_T, pl.smem, pl.CS, st);
     if (grid) {                    // all CTAs resident at once, or the launch fails: the exchange waits cannot deadlock
-        at[0].id = cudaLaunchAttributeCooperative;
-        at[0].val.cooperative = 1;
+        at.id = cudaLaunchAttributeCooperative;
+        at.val.cooperative = 1;
         P.xrow = reinterpret_cast<double *>(ws + pl.o_xrow);
         P.xcnt = reinterpret_cast<unsigned *>(ws + pl.o_xcnt);
-    } else {
-        at[0].id = cudaLaunchAttributeClusterDimension;
-        at[0].val.clusterDim.x = pl.CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
     }
-    cfg.attrs = at; cfg.numAttrs = 1;
     const int nphase = c->primary ? 2 : 1;
     if (c->primary) P.lin_g = reinterpret_cast<double *>(ws + pl.o_lin);
     for (int phase = 0; phase < nphase; phase++) {
@@ -620,8 +600,8 @@ extern "C" int raftk_f2_trace_read(unsigned long long *host, int n_cta)
 // cluster size, dynamic shared memory bytes
 extern "C" int raftk_f2_occupancy(const raftk_designs *d, int n_cases, int cluster_size, int out[5])
 {
-    F2Plan pl;
-    if (!fused2_plan(d, n_cases, cluster_size, pl)) return set_err(RAFTK_EINVAL, "not a k_rao_fused2 shape");
+    const SolvePlan pl = plan_solve(d, n_cases, cluster_size, WS_UNBOUNDED);
+    if (pl.kind != SOLVE_FUSED2) return set_err(RAFTK_EINVAL, "not a k_rao_fused2 shape");
     const int units = d->n_designs * n_cases;
     int clusters = 0, resident = 0;
     bool grid = false;
@@ -632,39 +612,25 @@ extern "C" int raftk_f2_occupancy(const raftk_designs *d, int n_cases, int clust
 }
 #endif
 
-static int run(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
-               const double *Xi_in, int mode /*0 solve, 1 linearise, 2 excitation only*/, bool do_excitation,
-               void *workspace, size_t wbytes, cudaStream_t st, const raftk_peers *peers = nullptr)
+// ---- v1 tables path ----------------------------------------------------------------------------------------------------
+// Depth and phase tables and F0 in the workspace (k_depth_table, k_excitation), then k_drag_solve linearises (mode 1) or
+// solves (mode 0); mode 2 stops after the excitation.  Linearisation reads the tables a preceding excitation left.  The
+// designs run in chunks of pl.per.
+static int run_tables(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
+                      const double *Xi_in, int mode /*0 solve, 1 linearise, 2 excitation only*/, const SolvePlan &pl,
+                      void *workspace, size_t wbytes, cudaStream_t st)
 {
-    int rc = validate(d, c);
-    if (rc) return rc;
-    const int nD = d->n_designs, nC = c->n_cases, nw = d->nw;
-    if (mode == 0) {                                   // fused on-chip solver when the slice fits in shared memory
-        F2Plan f2;
-        if (fused2_plan(d, nC, o ? o->cluster_size : 0, f2) && workspace && wbytes >= f2.ws_bytes)
-            return run_fused2(d, c, o, out, f2, workspace, st, peers);
-        FPlan fp;
-        const bool have_ws = workspace && wbytes >= (size_t)nD * nC * 6 * nw * sizeof(double2);
-        if (fused_plan(d, nD * nC, o ? o->cluster_size : 0, have_ws, fp)) return run_fused(d, c, o, out, fp, workspace, wbytes, st, peers);
-        if (peers && peers->n_ranks > 1) return set_err(RAFTK_EINVAL, "the fused exchange needs the fused solver; the design's frequency slice does not fit on chip");
-        if (c->primary) return set_err(RAFTK_EINVAL, "wave-train cases (cases.primary) need the fused solver; the design's frequency slice does not fit on chip");
-        if (c->Xi_init || out->Xi_last) return set_err(RAFTK_EINVAL, "cases.Xi_init / outputs.Xi_last need the fused solver; the design's frequency slice does not fit on chip");
-    }
     if (c->primary && mode != 2) return set_err(RAFTK_EINVAL, "cases.primary is only supported by raftk_solve_dynamics_*");
-    if (do_excitation) prof_begin_call();
+    const int nD = d->n_designs, nC = c->n_cases, nw = d->nw, per = pl.per;
+    const bool excitation = mode != 1;
+    if (excitation) prof_begin_call();
     DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
     CasesDev C = to_dev(c);
-    const size_t one = chunk_bytes(1, nC, d->max_nodes, nw);
-    if (!workspace || wbytes < one) return set_err(RAFTK_ENOMEM, "workspace smaller than one design's tables");
-    int per = nD;
-    while (per > 1 && (chunk_bytes(per, nC, d->max_nodes, nw) > wbytes || per > 65535)) per = (per + 1) / 2;
-    if (mode == 1 && !do_excitation && per < nD)
+    if (!workspace || wbytes < chunk_bytes(1, nC, d->max_nodes, nw)) return set_err(RAFTK_ENOMEM, "workspace smaller than one design's tables");
+    if (mode == 1 && per < nD)
         return set_err(RAFTK_ENOMEM, "linearization needs the whole batch's tables resident in the workspace");
-
-    Plan pl;
     if (mode != 2) {
-        rc = make_plan(d, std::min(per, nD) * nC, o ? o->cluster_size : 0, pl);
-        if (rc) return rc;
+        if (pl.smem > 227 * 1024) return set_err(RAFTK_EINVAL, "shared-memory plan exceeds 227 KB (nw per CTA too large)");
         static SmemOptIn opt;
         CUDA_TRY(opt.ensure(k_drag_solve, pl.smem));
     }
@@ -679,7 +645,7 @@ static int run(const raftk_designs *d, const raftk_cases *c, const raftk_solve_o
         W.F0 = reinterpret_cast<double2 *>(p); p += align_up((size_t)nDc * nC * 6 * nw * sizeof(double2), 256);
         W.zeta = reinterpret_cast<double *>(p);
 
-        if (do_excitation) {
+        if (excitation) {
             dim3 g0((nw + 127) / 128, nDc, 1);
             {
                 ProfScope ps(st, 0);
@@ -707,15 +673,8 @@ static int run(const raftk_designs *d, const raftk_cases *c, const raftk_solve_o
             P.Bdrag_out = out->B_drag;
             P.status = out->status;
             cudaLaunchConfig_t cfg;
-            memset(&cfg, 0, sizeof(cfg));
-            cfg.gridDim = dim3((unsigned)(nDc * nC * pl.CS), 1, 1);
-            cfg.blockDim = dim3(SOLVE_THREADS, 1, 1);
-            cfg.dynamicSmemBytes = pl.smem;
-            cfg.stream = st;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeClusterDimension;
-            at[0].val.clusterDim.x = pl.CS; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-            cfg.attrs = at; cfg.numAttrs = 1;
+            cudaLaunchAttribute at;
+            cluster_config(cfg, at, (size_t)nDc * nC * pl.CS, SOLVE_THREADS, pl.smem, pl.CS, st);
             {
                 ProfScope ps(st, 2);
                 CUDA_TRY(cudaLaunchKernelEx(&cfg, k_drag_solve, D, C, W, P));
@@ -732,16 +691,39 @@ static int run(const raftk_designs *d, const raftk_cases *c, const raftk_solve_o
     return RAFTK_OK;
 }
 
+// excitation (mode 2) or linearisation (mode 1) over the caller's workspace
+static int tables(const raftk_designs *d, const raftk_cases *c, const double *Xi_in, const raftk_outputs *out, int mode,
+                  void *workspace, size_t wbytes, cudaStream_t st)
+{
+    if (int rc = validate(d, c)) return rc;
+    return run_tables(d, c, nullptr, out, Xi_in, mode, plan_solve(d, c->n_cases, 0, wbytes, true), workspace, wbytes, st);
+}
+
+// ---- the rigid solve: launch a plan --------------------------------------------------------------------------------------
+static int launch_solve(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
+                        const SolvePlan &pl, void *workspace, size_t wbytes, cudaStream_t st, const raftk_peers *peers)
+{
+    if (pl.kind == SOLVE_FUSED2) return run_fused2(d, c, o, out, pl, workspace, st, peers);
+    if (pl.kind == SOLVE_FUSED) return run_fused(d, c, o, out, pl, workspace, wbytes, st, peers);
+    if (peers && peers->n_ranks > 1) return set_err(RAFTK_EINVAL, "the fused exchange needs the fused solver; the design's frequency slice does not fit on chip");
+    if (c->primary) return set_err(RAFTK_EINVAL, "wave-train cases (cases.primary) need the fused solver; the design's frequency slice does not fit on chip");
+    if (c->Xi_init || out->Xi_last) return set_err(RAFTK_EINVAL, "cases.Xi_init / outputs.Xi_last need the fused solver; the design's frequency slice does not fit on chip");
+    return run_tables(d, c, o, out, nullptr, 0, pl, workspace, wbytes, st);
+}
+
+// the rigid solve over the caller's workspace: planned against it, then launched
+static int solve(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
+                 void *workspace, size_t wbytes, cudaStream_t st, const raftk_peers *peers = nullptr)
+{
+    if (int rc = validate(d, c)) return rc;
+    const SolvePlan pl = plan_solve(d, c->n_cases, o->cluster_size, workspace ? wbytes : 0);
+    return launch_solve(d, c, o, out, pl, workspace, wbytes, st, peers);
+}
+
 extern "C" size_t raftk_solve_workspace_bytes(const raftk_designs *d, int32_t n_cases)
 {
     if (!d || d->n_designs <= 0 || n_cases <= 0) return 0;
-    F2Plan f2;
-    if (fused2_plan(d, n_cases, 0, f2)) return f2.ws_bytes;
-    FPlan fp;
-    if (d->max_nodes > 0 && d->max_members > 0 && fused_plan(d, d->n_designs * n_cases, 0, true, fp))
-        return align_up((size_t)d->n_designs * n_cases * 6 * d->nw * sizeof(double2), 256)
-               + align_up((size_t)d->n_designs * n_cases * ((size_t)NCOEF * d->max_nodes + 36) * sizeof(double), 256);
-    return raftk_workspace_bytes(d, n_cases);
+    return plan_solve(d, n_cases, 0, WS_UNBOUNDED).bytes;
 }
 
 extern "C" int raftk_hydro_excitation_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *out,
@@ -751,7 +733,7 @@ extern "C" int raftk_hydro_excitation_dev(const raftk_designs *d, const raftk_ca
     if (!out) return set_err(RAFTK_EINVAL, "null outputs");
     if (d && c && chunk_bytes(d->n_designs, c->n_cases, d->max_nodes, d->nw) > workspace_bytes)
         return set_err(RAFTK_ENOMEM, "excitation needs the whole batch's tables in the workspace");
-    return run(d, c, nullptr, out, nullptr, 2, true, workspace, workspace_bytes, (cudaStream_t)stream);
+    return tables(d, c, nullptr, out, 2, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int raftk_hydro_linearization_dev(const raftk_designs *d, const raftk_cases *c, const double *Xi_in,
@@ -759,7 +741,7 @@ extern "C" int raftk_hydro_linearization_dev(const raftk_designs *d, const raftk
 {
     disp_reset();
     if (!out || !Xi_in) return set_err(RAFTK_EINVAL, "null outputs / Xi_in");
-    return run(d, c, nullptr, out, Xi_in, 1, false, workspace, workspace_bytes, (cudaStream_t)stream);
+    return tables(d, c, Xi_in, out, 1, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int raftk_solve_dynamics_dev(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o,
@@ -773,9 +755,9 @@ extern "C" int raftk_solve_dynamics_dev(const raftk_designs *d, const raftk_case
         if (rc) return rc;
         raftk_cases cc = *c;
         cc.F_2nd = out->F_2nd;
-        return run(d, &cc, o, out, nullptr, 0, true, workspace, workspace_bytes, (cudaStream_t)stream);
+        return solve(d, &cc, o, out, workspace, workspace_bytes, (cudaStream_t)stream);
     }
-    return run(d, c, o, out, nullptr, 0, true, workspace, workspace_bytes, (cudaStream_t)stream);
+    return solve(d, c, o, out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 // ---- multi-GPU exchange fused into the solve (peer stores over NVLink) ------------------------------------------
@@ -836,7 +818,7 @@ extern "C" int raftk_solve_dynamics_gather_dev(const raftk_designs *d, const raf
     if (out->Xi != peers->gathered[peers->rank] + 2 * (size_t)peers->rank * peers->block_elems)
         return set_err(RAFTK_EINVAL, "outputs.Xi must be this rank's block of its own gathered array");
     if (d->n_qtf_w > 0 && !c->F_2nd) return set_err(RAFTK_EINVAL, "gather solve: pass cases.F_2nd precomputed (raftk_second_order_force_dev)");
-    return run(d, c, o, out, nullptr, 0, true, workspace, workspace_bytes, (cudaStream_t)stream, peers);
+    return solve(d, c, o, out, workspace, workspace_bytes, (cudaStream_t)stream, peers);
 }
 
 extern "C" int raftk_peer_barrier_dev(const raftk_peers *peers, int32_t *timeout_flag, void *stream)
@@ -1117,13 +1099,10 @@ static int host_run(const raftk_designs *d, const raftk_cases *c, const raftk_so
         // the system response reads the per-FOWT loads on the device: those buffers exist even when the caller does not want them back
         obytes += 4 * align_up(resp, 256) + align_up(nD * nC * 288, 256) + align_up(nC * nw * 4, 256) + 3 * align_up(36 * nD * nD * 8, 256);
     }
-    size_t wb = raftk_workspace_bytes(d, (int32_t)nC);
-    if (mode != 0) wb = chunk_bytes((int)nD, (int)nC, d->max_nodes, (int)nw);   // single chunk required
-    else {
-        F2Plan f2; FPlan fp;
-        if (fused2_plan(d, (int)nC, o ? o->cluster_size : 0, f2)) wb = f2.ws_bytes;
-        else if (fused_plan(d, (int)(nD * nC), o ? o->cluster_size : 0, true, fp)) wb = raftk_solve_workspace_bytes(d, (int32_t)nC);
-    }
+    // the solve is planned once, at the caller's cluster size, and launched with the workspace that plan needs; excitation
+    // and linearisation need the whole batch's tables in one chunk
+    const SolvePlan pl = mode == 0 ? plan_solve(d, (int)nC, o->cluster_size, WS_UNBOUNDED) : SolvePlan{};
+    const size_t wb = mode == 0 ? pl.bytes : chunk_bytes((int)nD, (int)nC, d->max_nodes, (int)nw);
     const size_t total = SMALL_REGION + in_bytes(d, c) + obytes + align_up(wb, 256) + 4096;
     Arena &A = g_arena[cur_dev()];
     if (A.reserve(total)) return set_err(RAFTK_ENOMEM, "device arena allocation failed");
@@ -1203,9 +1182,7 @@ static int host_run(const raftk_designs *d, const raftk_cases *c, const raftk_so
     bool direct_xi = false;
     raftk_peers hostpeer;
     if (mode == 0 && out->Xi && !getenv("RAFTK_NO_DIRECT_D2H")) {
-        F2Plan f2; FPlan fp;
-        const bool fused = (fused2_plan(&dd, (int)nC, o ? o->cluster_size : 0, f2) && wb >= f2.ws_bytes) ||
-                           fused_plan(&dd, (int)(nD * nC), o ? o->cluster_size : 0, true, fp);
+        const bool fused = pl.kind != SOLVE_V1;
         cudaPointerAttributes pa;
         const bool pinned_xi = cudaPointerGetAttributes(&pa, out->Xi) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer != nullptr;
         if (!pinned_xi) cudaGetLastError();
@@ -1221,11 +1198,10 @@ static int host_run(const raftk_designs *d, const raftk_cases *c, const raftk_so
             direct_xi = true;
         }
     }
-    if (mode == 0) rc = run(&dd, &cc, o, &od, nullptr, 0, true, ws, wb, st, direct_xi ? &hostpeer : nullptr);
-    else if (mode == 2) rc = run(&dd, &cc, nullptr, &od, nullptr, 2, true, ws, wb, st);
+    if (mode == 0) rc = launch_solve(&dd, &cc, o, &od, pl, ws, wb, st, direct_xi ? &hostpeer : nullptr);
     else {
-        rc = run(&dd, &cc, nullptr, &od, nullptr, 2, true, ws, wb, st);
-        if (!rc) rc = run(&dd, &cc, nullptr, &od, Xi_in_d, 1, false, ws, wb, st);
+        rc = tables(&dd, &cc, nullptr, &od, 2, ws, wb, st);
+        if (!rc && mode == 1) rc = tables(&dd, &cc, Xi_in_d, &od, 1, ws, wb, st);
     }
     if (rc) return rc;
     if (farm) {
@@ -1670,10 +1646,7 @@ extern "C" void raftk_host_free(void *p) { if (p) cudaFreeHost(p); }
 
 extern "C" double raftk_fp64_peak_gflops(int iters)
 {
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int blocks = sms * 8, threads = 256;
+    const int blocks = sm_count() * 8, threads = 256;
     double *out = nullptr;
     if (cudaMalloc(&out, (size_t)blocks * threads * 8) != cudaSuccess) return -1.0;
     cudaEvent_t a, b;

@@ -1,4 +1,4 @@
-"""Every kernel variant the rigid solver's planner can pick (raftk.cu: run, fused2_plan, fused_plan), reached by the shapes
+"""Every kernel variant the rigid solver's planner can pick (raftk.cu: plan_solve), reached by the shapes
 that make the planner itself choose it, asserted through solver.last_dispatch(), and compared with the C oracle:
 Xi and status with oracle.solve_cases, B_drag with oracle.solve_dynamics(want_Z=True), F_iner / F_BEM / zeta with
 oracle.calc_hydro_excitation.  Frequency counts are ragged (nw % cluster_size != 0, bins per CTA not a multiple of 32).
