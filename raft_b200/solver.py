@@ -395,19 +395,33 @@ def qtf_slender(P, beta_rad, Xi_rao):
     if Xi.shape != (n, 6, nw2):
         raise ValueError("Xi_rao must be [n,6,nw2] on the second-order grid")
     keep = {}
-    s = RaftkSlender()
-    nm = len(P["qs_mem_mcf"])
-    s.n_nodes, s.n_members, s.n_seg, s.nw = len(P["qs_node_mem"]), nm, len(P["qs_seg_mem"]), nw2
-    s.depth, s.rho, s.g = float(P["qs_depth"]), float(P["qs_rho"]), float(P["qs_g"])
-    start = np.concatenate([[0], np.cumsum(np.bincount(np.asarray(P["qs_node_mem"], dtype=np.int64), minlength=nm))])
-    for name in _lib.SLENDER_ARRAYS:
-        a = start if name == "mem_node_start" else np.asarray(P["qs_" + name])
-        a = np.ascontiguousarray(a, dtype=_I4 if name in ("mem_mcf", "mem_wl", "mem_node_start", "seg_mem") else _F8)
+
+    def ptr_of(name, a):
         keep[name] = a
-        setattr(s, name, a.ctypes.data)
+        return a.ctypes.data
+    s = _slender_struct(P, ptr_of)
     out = np.zeros([n, nw2, nw2, 6], dtype=np.complex128)
     check(lib.raftk_qtf_slender_host(C.byref(s), n, beta.ctypes.data, Xi.ctypes.data, out.ctypes.data))
     return out
+
+
+def _slender_struct(P, ptr_of):
+    """raftk_slender for a design's ``qs_*`` tables; ``ptr_of(name, array)`` returns the address to store (host or device).
+    The kernels find a node's member by scanning ``mem_node_start``, so the nodes of one member must be contiguous and in
+    member order: an unsorted ``qs_node_mem`` would silently pair nodes with the wrong members."""
+    nm = len(P["qs_mem_mcf"])
+    node_mem = np.asarray(P["qs_node_mem"], dtype=np.int64)
+    if np.any(np.diff(node_mem) < 0) or (len(node_mem) and (node_mem[0] < 0 or node_mem[-1] >= nm)):
+        raise ValueError("qs_node_mem must be non-decreasing member indices in [0, %d)" % nm)
+    s = RaftkSlender()
+    s.n_nodes, s.n_members, s.n_seg, s.nw = len(node_mem), nm, len(P["qs_seg_mem"]), len(P["qs_w"])
+    s.depth, s.rho, s.g = float(P["qs_depth"]), float(P["qs_rho"]), float(P["qs_g"])
+    start = np.concatenate([[0], np.cumsum(np.bincount(node_mem, minlength=nm))])
+    for name in _lib.SLENDER_ARRAYS:
+        a = start if name == "mem_node_start" else np.asarray(P["qs_" + name])
+        a = np.ascontiguousarray(a, dtype=_I4 if name in ("mem_mcf", "mem_wl", "mem_node_start", "seg_mem") else _F8)
+        setattr(s, name, ptr_of(name, a))
+    return s
 
 
 def get_rao(Xi, zeta):

@@ -286,6 +286,62 @@ def fixture_slender(name, yaml_path, pickle_path, solve_cases):
                                                              os.path.getsize(path) / 1024))
 
 
+SYNTH_MEMBERS = [
+    # inclined, tapered MacCamy-Fuchs brace through the waterline, added mass varying by station: the Kim & Yue force
+    # direction gets a vertical component, and the waterline force takes Ca from the last submerged node
+    dict(name="synth_brace", type="rigid", rA=[-30.0, 22.0, -24.0], rB=[-18.0, 31.0, 9.0], shape="circ", stations=[0, 0.45, 1],
+         d=[9.0, 7.5, 6.0], t=0.05, Cd=0.8, Ca=[[0.55, 0.6], [0.9, 0.85], [1.2, 1.1]], CdEnd=0.6, CaEnd=[0.5, 0.7, 0.9], MCF=True),
+    # rectangular member whose end A is above water
+    dict(name="synth_rect", type="rigid", rA=[24.0, -35.0, 6.0], rB=[30.0, -28.0, -18.0], shape="rect", stations=[0, 1],
+         d=[[5.0, 3.5], [4.0, 3.0]], gamma=20.0, t=0.05, Cd=[1.2, 1.8], Ca=[[0.7, 0.95], [1.05, 0.8]], CdEnd=0.6, CaEnd=0.4),
+]
+
+
+def fixture_slender_synth(name, yaml_path, depths=(40.0, 1000.0), headings_deg=(30.0, -135.0), seed=11):
+    """potSecOrder 1 on geometry the reference's own designs never reach: VolturnUS-S plus SYNTH_MEMBERS, at a depth where
+    every k h of the second-order grid is below 10 and at one where it spans ~6 .. 190 (all three depth branches of the
+    wave kinematics).  Per depth ``d<depth>_``: the packed design with its ``qs_*`` tables (``P_*``), fowt.M_struc,
+    and the unmodified reference's ``fowt.qtf`` for a fixed body (``qtf_fixed``) and for seeded random motion RAOs
+    (``Xi0`` on the first-order grid, ``qtf``) at each heading of ``beta`` [rad]."""
+    import contextlib
+    import copy
+    import io
+    t0 = time.time()
+    base = rh.load_design(yaml_path, sec_order=True)
+    assert int(base["platform"]["potSecOrder"]) == 1
+    base["platform"]["members"] = list(base["platform"]["members"]) + copy.deepcopy(SYNTH_MEMBERS)
+    plat = {k: v for k, v in base["platform"].items() if k not in ("hydroPath",)}
+    DESIGNS[name] = _plain(dict(settings=base.get("settings", {}), site=base["site"], platform=plat))
+    rng = np.random.default_rng(seed)
+    out = {"depths": np.array(depths, dtype=float)}
+    for depth in depths:
+        design = copy.deepcopy(base)
+        design["site"]["water_depth"] = float(depth)
+        model = rh.build_model(design)
+        fowt = model.fowtList[0]
+        P = packer.pack_fowt(fowt)
+        pre = "d%d_" % int(depth)
+        out.update({pre + "P_" + k: np.asarray(v) for k, v in P.items()})
+        out[pre + "M_struc"] = np.array(fowt.M_struc)
+        beta, qfix, Xi0, qmov = [], [], [], []
+        for hd in headings_deg:
+            with contextlib.redirect_stdout(io.StringIO()):
+                fowt.calcHydroExcitation(rh.make_case(2.0, 10.0, hd), memberList=fowt.memberList)
+                fowt.calcQTF_slenderBody(0)
+                qfix.append(np.array(fowt.qtf[:, :, 0, :]))
+                X = (rng.normal(size=(6, fowt.nw)) + 1j * rng.normal(size=(6, fowt.nw))) * np.array([1.5, 1.5, 1.0, 0.05, 0.05, 0.05])[:, None]
+                fowt.calcQTF_slenderBody(0, Xi0=X)
+                qmov.append(np.array(fowt.qtf[:, :, 0, :]))
+            beta.append(float(fowt.beta[0])), Xi0.append(X)
+        out[pre + "beta"], out[pre + "qtf_fixed"], out[pre + "Xi0"], out[pre + "qtf"] = np.array(beta), np.array(qfix), np.array(Xi0), np.array(qmov)
+        kh = np.asarray(P["qs_k"]) * depth
+        print("%-28s depth %6.0f: nw2=%3d Ns=%3d members=%d k h %.2f .. %.1f" % (name, depth, len(P["qs_w"]), len(P["qs_node_mem"]),
+                                                                              len(P["qs_mem_mcf"]), kh.min(), kh.max()))
+    path = os.path.join(OUT, name + ".npz")
+    np.savez_compressed(path, **out)
+    print("%-28s %.1f s  %.0f KB" % (name, time.time() - t0, os.path.getsize(path) / 1024))
+
+
 def fixture_flexible(name, yaml_path, pickles):
     """Generalised degrees of freedom (flexible members, nDOF = 150): the reference's golden excitation / linearisation
     pickles of VolturnUS-S-flexible with the tables packed by packer.pack_general_dofs (oracle groundwork for the next row).
@@ -437,6 +493,8 @@ def main():
     if not args.only or args.only in "slender_VolturnUS-S":
         fixture_slender("slender_VolturnUS-S", os.path.join(td, "VolturnUS-S.yaml"), os.path.join(td, "VolturnUS-S_true_calcQTF_slenderBody.pkl"),
                         solve_cases=[(6.0, 12.0, 30.0), (2.0, 7.5, -75.0), (9.0, 15.0, 160.0)])
+    if not args.only or args.only in "slender_synth_VolturnUS-S":
+        fixture_slender_synth("slender_synth_VolturnUS-S", os.path.join(td, "VolturnUS-S.yaml"))
     if not args.only or args.only in "farm_VolturnUS-S_farm_nw48":
         fixture_farm("farm_VolturnUS-S_farm_nw48", os.path.join(REF, "designs", "VolturnUS-S_farm.yaml"), nw=48, max_freq=0.1024,
                      cases=[(6.0, 12.0, 0.0), (3.5, 9.0, 40.0), (8.0, 14.0, -120.0)])

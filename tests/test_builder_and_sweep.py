@@ -13,7 +13,7 @@ TABLE_KEYS = ["mem_q", "mem_p1", "mem_p2", "mem_rA", "node_r", "node_ls", "node_
               "node_in_q", "node_in_p1", "node_in_p2", "node_pa", "node_a_i", "node_Imat", "k", "w"]
 
 
-@pytest.mark.parametrize("name", sorted(n for n in DESIGNS if not n.startswith("farm_")))
+@pytest.mark.parametrize("name", sorted(n for n in DESIGNS if not n.startswith(("farm_", "slender_synth_"))))   # slender_synth_: per-depth tables, own test
 def test_builder_matches_reference_tables(name):
     """raft_b200.member/fowt rebuild, from the design dict alone, the tables packed from the reference's objects
     (strip discretisation, frames, node positions, drag/inertia coefficients, MacCamy-Fuchs, A_hydro_morison)."""
@@ -138,12 +138,27 @@ def test_turbine_channel_coefficients_vs_reference_saveTurbineOutputs():
 def test_slender_qtf_tables_from_own_builder_match_reference_tables():
     """potSecOrder 1: raft_b200.FOWT builds the second-order grid (w1_2nd, k1_2nd) and, through
     packer.pack_qtf_members, the strip / waterline / Kim & Yue tables exactly as packed from the live reference."""
+    _check_slender_tables_from_own_builder("slender_VolturnUS-S", "test_VolturnUS-S", "")
+
+
+@pytest.mark.parametrize("depth", [40, 1000])
+def test_slender_qtf_tables_from_own_builder_synthetic_geometry(depth):
+    """The same on the synthetic design (inclined tapered MacCamy-Fuchs brace with station-varying Ca, rectangular member
+    with end A above water) at both of its depths."""
+    _check_slender_tables_from_own_builder("slender_synth_VolturnUS-S", "slender_synth_VolturnUS-S", "d%d_" % depth)
+
+
+def _check_slender_tables_from_own_builder(name, design_key, pre):
+    """``pre``: depth prefix of the fixture's keys ('' for a fixture with one packed design)."""
     from raft_b200.model import Model
-    z = np.load(os.path.join(GOLDEN, "slender_VolturnUS-S.npz"))
-    P = {k[2:]: z[k] for k in z.files if k.startswith("P_")}
-    D = DESIGNS["test_VolturnUS-S"]
+    z = np.load(os.path.join(GOLDEN, name + ".npz"))
+    P = {k[len(pre) + 2:]: z[k] for k in z.files if k.startswith(pre + "P_")}
+    D = DESIGNS[design_key]
     design = dict(D, platform=dict(D["platform"], potSecOrder=1), site=dict(D["site"], water_depth=float(P["depth"])))
-    mats = dict(M_struc=P["M0"] - z["A_hydro_morison"], C_struc=P["C0"] - z["C_moor"], C_moor=z["C_moor"])
+    if pre:
+        mats = dict(M_struc=z[pre + "M_struc"])
+    else:
+        mats = dict(M_struc=P["M0"] - z["A_hydro_morison"], C_struc=P["C0"] - z["C_moor"], C_moor=z["C_moor"])
     f = Model(design, matrices=mats).fowtList[0]
     assert f.potSecOrder == 1 and len(f.w1_2nd) == 23
     Q = f.pack()
@@ -158,6 +173,28 @@ def test_slender_qtf_tables_from_own_builder_match_reference_tables():
     bad = dict(design, platform={k: v for k, v in design["platform"].items() if k != "min_freq2nd"})
     with pytest.raises(Exception, match="min_freq2nd"):
         Model(bad, matrices=mats)
+
+
+def test_slender_struct_rejects_unsorted_node_members():
+    """The slender-body kernels map a node to its member through mem_node_start (counts of qs_node_mem): nodes out of member
+    order would be paired with the wrong member's frame and waterline data, so solver._slender_struct refuses them."""
+    from raft_b200 import solver
+    z = np.load(os.path.join(GOLDEN, "slender_VolturnUS-S.npz"))
+    P = {k[2:]: z[k] for k in z.files if k.startswith("P_")}
+    s = solver._slender_struct(P, lambda name, a: a.ctypes.data)
+    nm = len(P["qs_mem_mcf"])
+    assert (s.n_nodes, s.n_members, s.nw) == (len(P["qs_node_mem"]), nm, len(P["qs_w"]))
+    swapped = P["qs_node_mem"].copy()
+    i = int(np.flatnonzero(np.diff(swapped))[0])                   # last node of member 0 <-> first node of member 1
+    swapped[i], swapped[i + 1] = swapped[i + 1], swapped[i]
+    with pytest.raises(ValueError, match="non-decreasing"):
+        solver._slender_struct(dict(P, qs_node_mem=swapped), lambda name, a: a.ctypes.data)
+    for bad in (np.where(P["qs_node_mem"] == 0, -1, P["qs_node_mem"]), np.where(P["qs_node_mem"] == nm - 1, nm, P["qs_node_mem"])):
+        with pytest.raises(ValueError, match="non-decreasing"):
+            solver._slender_struct(dict(P, qs_node_mem=bad), lambda name, a: a.ctypes.data)
+    # no strip nodes at all (only waterline / Kim & Yue terms) is a valid table
+    empty = dict(P, qs_node_mem=np.zeros(0, dtype=np.int32))
+    assert solver._slender_struct(empty, lambda name, a: a.ctypes.data).n_nodes == 0
 
 
 def test_get_rao_and_second_order_case_plumbing():

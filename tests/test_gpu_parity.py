@@ -716,21 +716,57 @@ def _slender_golden():
     return z, {k[2:]: z[k] for k in z.files if k.startswith("P_")}
 
 
+def _slender_reference_sets(name):
+    """-> [(P, fixed-body (beta_rad, qtf) pairs, moving-body (beta_rad, Xi0 on P['w'], qtf) triples)] of a slender-body fixture:
+    the reference's own golden pickle and the QTFs it computed inside solveDynamics, or, for the synthetic design, the
+    reference's calcQTF_slenderBody at each of its depths."""
+    import os
+    from conftest import GOLDEN
+    z = np.load(os.path.join(GOLDEN, name + ".npz"))
+    deg = 0.017453292519943295
+    if "depths" not in z.files:
+        P = {k[2:]: z[k] for k in z.files if k.startswith("P_")}
+        fixed = [(z["ref_pickle_case"][2] * deg, z["ref_pickle_qtf"][:, :, 0, :])]
+        moving = [(c[2] * deg, x, q) for c, x, q in zip(z["ref_run_solve_cases"], z["ref_run_solve_Xi0"], z["ref_run_solve_qtf"])]
+        return [(P, fixed, moving)]
+    sets = []
+    for depth in z["depths"]:
+        pre = "d%d_" % int(depth)
+        P = {k[len(pre) + 2:]: z[k] for k in z.files if k.startswith(pre + "P_")}
+        sets.append((P, list(zip(z[pre + "beta"], z[pre + "qtf_fixed"])), list(zip(z[pre + "beta"], z[pre + "Xi0"], z[pre + "qtf"]))))
+    return sets
+
+
 def test_slender_qtf_vs_reference_pickle_and_run(solver, oracle):
     """k_slender_tables / k_slender_pairs: fixed body vs the reference's own golden pickle; moving body vs the QTFs the
     reference computed inside solveDynamics; random motions and headings vs the oracle (all pairs in one call)."""
-    z, P = _slender_golden()
+    _check_slender_vs_reference(solver, oracle, "slender_VolturnUS-S")
+
+
+@pytest.mark.parametrize("name", ["pinq_VolturnUS-S-pointInertia", "slender_synth_VolturnUS-S"])
+def test_slender_qtf_vs_other_reference_fixtures(name, solver, oracle):
+    """The same on the reference's second slender-body golden (VolturnUS-S-pointInertia) and on the synthetic design
+    (reference calcQTF_slenderBody at 40 m and 1000 m with an inclined MacCamy-Fuchs brace and a member with end A above water)."""
+    _check_slender_vs_reference(solver, oracle, name)
+
+
+def _check_slender_vs_reference(solver, oracle, name):
+    for P, fixed, moving in _slender_reference_sets(name):
+        n2 = len(P["qs_w"])
+        q = solver.qtf_slender(P, [b for b, _ in fixed], np.zeros([len(fixed), 6, n2], dtype=complex))
+        for i, (_, ref) in enumerate(fixed):
+            for a in range(6):
+                assert relerr(q[i][..., a], ref[..., a]) < RTOL, (i, a)
+        Xi2 = np.array([[np.interp(P["qs_w"], P["w"], x[a], left=0, right=0) for a in range(6)] for _, x, _ in moving])
+        q = solver.qtf_slender(P, [b for b, _, _ in moving], Xi2)
+        for i, (_, _, ref) in enumerate(moving):
+            for a in range(6):
+                assert relerr(q[i][..., a], ref[..., a]) < RTOL, (i, a)
+        _slender_random_vs_oracle(solver, oracle, P)
+
+
+def _slender_random_vs_oracle(solver, oracle, P):
     n2 = len(P["qs_w"])
-    deg = 0.017453292519943295
-    q = solver.qtf_slender(P, [z["ref_pickle_case"][2] * deg], np.zeros([1, 6, n2], dtype=complex))
-    for a in range(6):
-        assert relerr(q[0][..., a], z["ref_pickle_qtf"][:, :, 0, a]) < RTOL, a
-    cases = z["ref_run_solve_cases"]
-    Xi2 = np.array([[np.interp(P["qs_w"], P["w"], z["ref_run_solve_Xi0"][i][a], left=0, right=0) for a in range(6)] for i in range(len(cases))])
-    q = solver.qtf_slender(P, cases[:, 2] * deg, Xi2)
-    for i in range(len(cases)):
-        for a in range(6):
-            assert relerr(q[i][..., a], z["ref_run_solve_qtf"][i][..., a]) < RTOL, (i, a)
     rng = np.random.default_rng(5)
     Xr = (rng.normal(size=(4, 6, n2)) + 1j * rng.normal(size=(4, 6, n2))) * np.array([1, 1, 1, 0.03, 0.03, 0.03])[None, :, None]
     betas = rng.uniform(-np.pi, np.pi, 4)

@@ -240,6 +240,28 @@ def test_slender_body_qtf_second_reference_pickle(oracle):
     assert st[0] == z["ref_run_solve_passes"][0] and response_err(Xi, z["ref_run_solve_Xi"][0]) < 1e-11
 
 
+@pytest.mark.parametrize("depth", [40, 1000])
+def test_slender_body_qtf_synthetic_geometry_vs_reference_run(depth, oracle):
+    """The oracle's calcQTF_slenderBody against the unmodified reference on VolturnUS-S plus an inclined, tapered
+    MacCamy-Fuchs brace and a rectangular member with end A above water, at 40 m (every k h < 10) and 1000 m (k h up to
+    ~190): fixed body and seeded random motions, two headings, per DOF over every frequency pair."""
+    import os
+    from conftest import GOLDEN
+    z = np.load(os.path.join(GOLDEN, "slender_synth_VolturnUS-S.npz"))
+    pre = "d%d_" % depth
+    P = {k[len(pre) + 2:]: z[k] for k in z.files if k.startswith(pre + "P_")}
+    od = oracle.OracleDesign(P)
+    n2 = len(P["qs_w"])
+    kh = P["qs_k"] * depth
+    assert (kh.max() < 10) if depth == 40 else (kh.min() < 10 and kh.max() > 89.4)
+    for c, beta in enumerate(z[pre + "beta"]):
+        Xi2 = np.array([np.interp(P["qs_w"], P["w"], z[pre + "Xi0"][c][a], left=0, right=0) for a in range(6)])
+        for Xi, ref in ((np.zeros([6, n2], dtype=complex), z[pre + "qtf_fixed"][c]), (Xi2, z[pre + "qtf"][c])):
+            q = oracle.qtf_slender(od, beta, Xi)
+            for a in range(6):
+                assert relerr(q[..., a], ref[..., a]) < 1e-13, (c, a)
+
+
 def test_generalised_dofs_vs_reference_flexible_pickles(oracle):
     """Groundwork for the next row (flexible members, nDOF = 150): the oracle's generalised calcHydroExcitation /
     calcHydroLinearization with fowt.T against the reference's VolturnUS-S-flexible golden pickles."""

@@ -12,8 +12,8 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from raft_b200 import _lib, grid  # noqa: E402
-from raft_b200._lib import RaftkSlender, check, lib  # noqa: E402
+from raft_b200 import grid, solver  # noqa: E402
+from raft_b200._lib import check, lib  # noqa: E402
 
 z = np.load(os.path.join(ROOT, "tests", "golden", "slender_VolturnUS-S.npz"))
 P = {k[2:]: z[k] for k in z.files if k.startswith("P_")}
@@ -21,17 +21,13 @@ dev = torch.device("cuda", 0)
 
 
 def run(P, n, label, reps=5):
-    nw2, nm = len(P["qs_w"]), len(P["qs_mem_mcf"])
+    nw2 = len(P["qs_w"])
     keep = {}
-    s = RaftkSlender()
-    s.n_nodes, s.n_members, s.n_seg, s.nw = len(P["qs_node_mem"]), nm, len(P["qs_seg_mem"]), nw2
-    s.depth, s.rho, s.g = float(P["qs_depth"]), float(P["qs_rho"]), float(P["qs_g"])
-    start = np.concatenate([[0], np.cumsum(np.bincount(np.asarray(P["qs_node_mem"], dtype=np.int64), minlength=nm))])
-    for name in _lib.SLENDER_ARRAYS:
-        a = start if name == "mem_node_start" else np.asarray(P["qs_" + name])
-        a = np.ascontiguousarray(a, dtype=np.int32 if name in ("mem_mcf", "mem_wl", "mem_node_start", "seg_mem") else np.float64)
+
+    def to_dev(name, a):
         keep[name] = torch.from_numpy(a).to(dev)
-        setattr(s, name, keep[name].data_ptr())
+        return keep[name].data_ptr()
+    s = solver._slender_struct(P, to_dev)
     rng = np.random.default_rng(7)
     beta = torch.from_numpy(rng.uniform(-np.pi, np.pi, n)).to(dev)
     Xi = (rng.normal(size=(n, 6, nw2)) + 1j * rng.normal(size=(n, 6, nw2))) * np.array([1, 1, 1, 0.03, 0.03, 0.03])[None, :, None]
