@@ -95,6 +95,7 @@ def _time_farm(N, cs, dev, steps, warmup, parity=False, dump=None):
     sess.solve(n_iter=10, tol=0.01, xi_start=0.0)
     m1, _ = solver.profile_read()
     sess.farm_response(C_arr=C_arr)
+    kernel = solver.last_dispatch()["kernel"]
     m2, _ = solver.profile_read()
     solver.profile_enable(False)
     torch.cuda.synchronize()
@@ -115,7 +116,7 @@ def _time_farm(N, cs, dev, steps, warmup, parity=False, dump=None):
     assert np.array_equal(out["Xi_sys"], xi.cpu().numpy()), "e2e and resident farm paths disagree"
     units = nC * nw
     res = dict(n_fowt=N, n_dof=n, cases=nC, nw=nw, ms_per_step=ms, value=units / (ms * 1e-3), e2e_ms_per_step=e2e_ms, e2e_value=units / (e2e_ms * 1e-3),
-               launches_per_step=launches / steps, solve_kernels_ms=float(sum(m1)), system_kernel_ms=float(m2[1]),
+               launches_per_step=launches / steps, solve_kernels_ms=float(sum(m1)), system_kernel_ms=float(m2[1]), kernel=kernel,
                h2d=int(batch.input_bytes() + cases.input_bytes() + C_arr.nbytes),
                d2h=int(out["Xi_sys"].nbytes + out["Xi"].nbytes + out["status"].nbytes + out["info"].nbytes + out["B_drag"].nbytes))
     if parity:
@@ -171,7 +172,9 @@ def bench_special(args, rank, world, dev):
                             n_fowt=N, n_dof=n, nw=many["nw"], cases=many["cases"], l2="flushed between timed steps (256 MiB write)"),
                 e2e=dict(value=many["e2e_value"], unit=UNIT, ms_per_step=many["e2e_ms_per_step"], h2d_bytes_per_step=many["h2d"], d2h_bytes_per_step=many["d2h"]),
                 gpu_launches=int(round(many["launches_per_step"] * args.steps)),
-                roofline=dict(bound="hbm", kernel="k_farm_response (block assembly + %dx%d complex LU per (case, bin), matrix in shared memory)" % (n, n),
+                roofline=dict(bound="hbm", kernel=("k_farm_response_global (block assembly + %dx%d complex LU per (case, bin), matrix in a global-memory "
+                                                   "workspace slab)" if many["kernel"] == "farm-global" else
+                                                   "k_farm_response (block assembly + %dx%d complex LU per (case, bin), matrix in shared memory)") % (n, n),
                               achieved=ach, peak=hbm, unit="GB/s", frac=ach / hbm, traffic=None, kernel_ms=many["system_kernel_ms"],
                               algorithmic_bytes_per_solve=b_alg, lu_gflops=fl * many["cases"] * many["nw"] / (many["system_kernel_ms"] * 1e-3) / 1e9,
                               share_of_step=many["system_kernel_ms"] / (many["system_kernel_ms"] + many["solve_kernels_ms"])),

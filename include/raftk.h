@@ -204,7 +204,9 @@ enum {
     RAFTK_KERNEL_FARM_WARP = 12,      /* k_farm_response<true>                                                            */
     RAFTK_KERNEL_FARM_BLOCK = 13,     /* k_farm_response<false>                                                           */
     RAFTK_KERNEL_SYS_UNBLOCKED = 14,  /* k_system_solve, column-at-a-time LU (n <= 24)                                    */
-    RAFTK_KERNEL_SYS_BLOCKED = 15     /* k_system_solve, blocked LU (n > 24)                                              */
+    RAFTK_KERNEL_SYS_BLOCKED = 15,    /* k_system_solve, blocked LU (n > 24)                                              */
+    RAFTK_KERNEL_FARM_GLOBAL = 16,    /* k_farm_response_global: system in a workspace slab, LU blocked in global memory   */
+    RAFTK_KERNEL_SYS_GLOBAL = 17      /* k_system_solve_global: Z factored in place, LU blocked in global memory           */
 };
 typedef struct raftk_dispatch {
     int32_t family;           /* RAFTK_FAMILY_*                                                                          */
@@ -418,6 +420,9 @@ int raftk_solve_dynamics_host(const raftk_designs *d, const raftk_cases *c, cons
  * System (farm) response, raft_model.py:1164-1216: for every frequency solve the dense
  * n x n complex system Z_sys(w) Xi = F for nrhs right-hand sides (n = 6N).
  * Z complex [nw,n,n] row-major (destroyed), F complex [nw,n,nrhs] (overwritten with Xi).
+ * info [nw]: 0, or k+1 of the first zero pivot.  Any n: a system whose [n][n+nrhs] augmented matrix fits in the device's
+ * opt-in shared memory next to the kernel's static shared memory is solved there (k_system_solve); larger ones are factored
+ * in place in Z (k_system_solve_global).  Both pivot on |re| + |im| (first maximum wins) with the same elimination order.
  */
 int raftk_system_solve_dev(int32_t n, int32_t nw, int32_t nrhs, double *Z, double *F, int32_t *info,
                            void *stream);
@@ -446,6 +451,21 @@ typedef struct raftk_farm {
 
 int raftk_farm_response_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f,
                             void *stream);
+/*
+ * Farms of any size.  While a [6N][6N+1] complex system fits in the device's opt-in shared memory next to the static shared
+ * memory of the one-CTA-per-system kernel (on an H100: N <= 20 with the sm_90a build), the shared-memory kernels solve the
+ * farm and no workspace is used.  Larger farms are solved by k_farm_response_global: persistent CTAs, each assembling and
+ * factoring one (case, frequency) system after another in its own [6N][6N+1] slab of the workspace.
+ * raftk_farm_workspace_bytes: 0 when the shared-memory kernels take the shape; else the bytes of a full persistent grid
+ * (resident CTAs x slab, at most nC * nw slabs).  Without a device it answers for an H100 (132 SMs, 227 KB opt-in).
+ * raftk_farm_response_ws_dev: raftk_farm_response_dev with a device workspace; accepts every N.  Fewer bytes than the query
+ * returned run fewer CTAs with bit-identical results; less than one slab is RAFTK_EINVAL before any launch.
+ * raftk_farm_response_dev is the same call without a workspace, so it refuses the farms that need one.
+ * raftk_solve_dynamics_farm_host reserves the workspace itself and accepts every N.
+ */
+size_t raftk_farm_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm *f);
+int raftk_farm_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f,
+                               void *workspace, size_t workspace_bytes, void *stream);
 int raftk_solve_dynamics_farm_host(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o,
                                    const raftk_outputs *out, const raftk_farm *f);
 

@@ -134,7 +134,7 @@ SYMBOLS = [
     "raftk_fp64_peak_gflops",
     "raftk_peer_alloc", "raftk_peer_free", "raftk_peer_open", "raftk_peer_close",
     "raftk_solve_dynamics_gather_dev", "raftk_peer_barrier_dev",
-    "raftk_farm_response_dev", "raftk_solve_dynamics_farm_host",
+    "raftk_farm_response_dev", "raftk_solve_dynamics_farm_host", "raftk_farm_workspace_bytes", "raftk_farm_response_ws_dev",
     "raftk_family_sizes", "raftk_build_family_host",
 ]
 
@@ -216,6 +216,10 @@ def _load():
     lib.raftk_solve_dynamics_farm_host.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkSolveOpts), P(RaftkOutputs), P(RaftkFarm)]
     lib.raftk_farm_response_dev.restype = C.c_int
     lib.raftk_solve_dynamics_farm_host.restype = C.c_int
+    lib.raftk_farm_workspace_bytes.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkFarm)]
+    lib.raftk_farm_workspace_bytes.restype = C.c_size_t
+    lib.raftk_farm_response_ws_dev.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkOutputs), P(RaftkFarm), C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.raftk_farm_response_ws_dev.restype = C.c_int
     lib.raftk_family_sizes.argtypes = [P(RaftkFamily), P(C.c_int32), P(C.c_int32)]
     lib.raftk_build_family_host.argtypes = [P(RaftkFamily), P(RaftkFamilyTables)]
     lib.raftk_family_sizes.restype = C.c_int

@@ -836,12 +836,65 @@ extern "C" int raftk_peer_barrier_dev(const raftk_peers *peers, int32_t *timeout
 }
 
 // ---- farm system solve ----------------------------------------------------------------------------
+// Which dense solver takes a system.  The shared-memory kernels (k_system_solve, k_farm_response) keep every system whose
+// augmented matrix fits in the device's opt-in shared memory next to the kernel's static shared memory; everything larger
+// goes to the global-memory LU (lu_global).  Without a device the rule uses an H100's limits and the static sizes of the
+// sm_90a build, so that the workspace query answers the same on a machine without a GPU.
+static size_t dev_attr(cudaDeviceAttr a, size_t fallback)
+{
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&v, a, dev) != cudaSuccess) { cudaGetLastError(); return fallback; }
+    return (size_t)v;
+}
+static size_t smem_optin() { return dev_attr(cudaDevAttrMaxSharedMemoryPerBlockOptin, 227 * 1024); }
+static size_t smem_per_sm() { return dev_attr(cudaDevAttrMaxSharedMemoryPerMultiprocessor, 228 * 1024); }
+template <class K> static size_t static_smem(K kernel, size_t fallback)
+{
+    cudaFuncAttributes fa;
+    if (cudaFuncGetAttributes(&fa, kernel) != cudaSuccess) { cudaGetLastError(); return fallback; }
+    return fa.sharedSizeBytes;
+}
+// static shared memory of the sm_90a build (cudaFuncGetAttributes), used when no device answers
+#define SMEM_STATIC_SYS 32
+#define SMEM_STATIC_FARM_BLOCK 32
+#define SMEM_STATIC_GLU 176
+static bool smem_fits(size_t bytes, size_t static_bytes) { return bytes + static_bytes <= smem_optin(); }
+
+// Panel width and CTAs per SM of the global-memory LU: the widest panel (16, 8, ..., 1 columns; n x pw double2 of shared
+// memory) with which two CTAs share an SM, else the widest with which one CTA fits.  pw = 0: no panel fits (n > ~14 000).
+struct GluPlan { int pw = 0, per_sm = 0; size_t smem = 0; };
+static GluPlan glu_plan(int n)
+{
+    GluPlan g;
+    const size_t st = static_smem(k_system_solve_global, SMEM_STATIC_GLU), per_sm = smem_per_sm(), optin = smem_optin();
+    for (int ctas = 2; ctas >= 1 && !g.pw; ctas--)
+        for (int pw = GLU_PWMAX; pw >= 1; pw >>= 1) {
+            const size_t b = (size_t)n * pw * sizeof(double2);
+            if (b + st <= optin && ctas * (b + st + 1024) <= per_sm) { g.pw = pw; g.per_sm = ctas; g.smem = b; break; }
+        }
+    return g;
+}
+
+static int launch_system_global(int n, int nw, int nrhs, double *Z, double *F, int32_t *info, cudaStream_t st)
+{
+    const GluPlan g = glu_plan(n);
+    if (!g.pw) return set_err(RAFTK_EINVAL, "system solve: n too large for one panel column in shared memory");
+    static SmemOptIn opt(0);                          // static + dynamic shared memory may pass 48 KB below 48 KB of panel
+    CUDA_TRY(opt.ensure(k_system_solve_global, g.smem));
+    const int grid = std::min(nw, g.per_sm * sm_count());
+    k_system_solve_global<<<grid, GLU_T, g.smem, st>>>(n, nw, nrhs, g.pw, reinterpret_cast<double2 *>(Z), reinterpret_cast<double2 *>(F), info);
+    g_launches++;
+    disp_launch(RAFTK_FAMILY_SYSTEM, RAFTK_KERNEL_SYS_GLOBAL, GLU_T);
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
 extern "C" int raftk_system_solve_dev(int32_t n, int32_t nw, int32_t nrhs, double *Z, double *F, int32_t *info, void *stream)
 {
     disp_reset();
     if (n <= 0 || nw <= 0 || nrhs <= 0 || !Z || !F) return set_err(RAFTK_EINVAL, "bad system-solve arguments");
     const size_t smem = (size_t)n * (n + nrhs) * sizeof(double2);
-    if (smem > 227 * 1024) return set_err(RAFTK_EINVAL, "system too large for the shared-memory solver (n*(n+nrhs)*16 B > 227 KB)");
+    if (!smem_fits(smem, static_smem(k_system_solve, SMEM_STATIC_SYS))) return launch_system_global(n, nw, nrhs, Z, F, info, (cudaStream_t)stream);
     static SmemOptIn opt(48 * 1024);
     CUDA_TRY(opt.ensure(k_system_solve, smem));
     k_system_solve<<<nw, 128, smem, (cudaStream_t)stream>>>(n, nrhs, reinterpret_cast<double2 *>(Z), reinterpret_cast<double2 *>(F), info);
@@ -851,7 +904,31 @@ extern "C" int raftk_system_solve_dev(int32_t n, int32_t nw, int32_t nrhs, doubl
     return RAFTK_OK;
 }
 
-static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f, cudaStream_t st)
+// true when the shared-memory farm kernels take a farm of N FOWTs (6N <= 24: warp per system; else one CTA per system with
+// the [6N][6N+1] system in shared memory); false sends it to k_farm_response_global
+static bool farm_on_chip(int N)
+{
+    const int n = 6 * N;
+    return n <= 24 || smem_fits((size_t)n * (n + 1) * sizeof(double2), static_smem(k_farm_response<false>, SMEM_STATIC_FARM_BLOCK));
+}
+
+// workspace of k_farm_response_global: one [6N][6N+1] slab per resident CTA, no more slabs than (case, frequency) systems
+static size_t farm_slab_bytes(int N) { return (size_t)6 * N * (6 * N + 1) * sizeof(double2); }
+static size_t farm_ws_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm *f)
+{
+    if (!d || !c || !f || f->n_fowt < 1 || d->nw < 1 || c->n_cases < 1 || farm_on_chip(f->n_fowt)) return 0;
+    const GluPlan g = glu_plan(6 * f->n_fowt);
+    const long long slabs = std::min<long long>((long long)c->n_cases * d->nw, (long long)std::max(g.per_sm, 1) * sm_count());
+    return (size_t)slabs * farm_slab_bytes(f->n_fowt);
+}
+
+extern "C" size_t raftk_farm_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm *f)
+{
+    return farm_ws_bytes(d, c, f);
+}
+
+static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f, void *ws,
+                       size_t ws_bytes, cudaStream_t st)
 {
     if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "farm response: null argument");
     if (f->n_fowt != d->n_designs || f->n_fowt < 1) return set_err(RAFTK_EINVAL, "farm response: farm.n_fowt must equal designs.n_designs");
@@ -859,11 +936,41 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
         return set_err(RAFTK_EINVAL, "farm response needs B_drag, F_drag, F_iner of the per-FOWT solve and farm.Xi_sys");
     if (d->n_bem_head > 0 && !solved->F_BEM) return set_err(RAFTK_EINVAL, "farm response: the designs carry BEM excitation, F_BEM is required");
     const int n = 6 * f->n_fowt;
+    if (!farm_on_chip(f->n_fowt)) {
+        // persistent CTAs over the (case, frequency) systems, each CTA on its own slab of the caller's workspace
+        const GluPlan g = glu_plan(n);
+        if (!g.pw) return set_err(RAFTK_EINVAL, "farm response: 6N too large for one panel column in shared memory");
+        const size_t slab = farm_slab_bytes(f->n_fowt);
+        if (!ws || ws_bytes < slab)
+            return set_err(RAFTK_EINVAL, "farm response: a farm this size needs a workspace of at least one [6N][6N+1] slab "
+                                         "(raftk_farm_workspace_bytes, raftk_farm_response_ws_dev)");
+        const long long nsys = (long long)c->n_cases * d->nw;
+        const int grid = (int)std::min<long long>(std::min<long long>(nsys, (long long)(ws_bytes / slab)), (long long)g.per_sm * sm_count());
+        static SmemOptIn opt_g(0);
+        CUDA_TRY(opt_g.ensure(k_farm_response_global, g.smem));
+        DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
+        CasesDev C = to_dev(c);
+        FarmParams P;
+        P.N = f->n_fowt; P.nC = c->n_cases; P.nw = d->nw;
+        P.B_drag = solved->B_drag;
+        P.F_drag = reinterpret_cast<const double2 *>(solved->F_drag);
+        P.F_iner = reinterpret_cast<const double2 *>(solved->F_iner);
+        P.F_BEM = d->n_bem_head > 0 ? reinterpret_cast<const double2 *>(solved->F_BEM) : nullptr;
+        P.M_arr = f->M_arr; P.B_arr = f->B_arr; P.C_arr = f->C_arr;
+        P.Xi = reinterpret_cast<double2 *>(f->Xi_sys); P.info = f->info;
+        {
+            ProfScope ps(st, 1);
+            k_farm_response_global<<<grid, GLU_T, g.smem, st>>>(D, C, P, static_cast<double2 *>(ws), g.pw);
+            disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_GLOBAL, GLU_T);
+        }
+        g_launches++;
+        CUDA_TRY(cudaGetLastError());
+        return RAFTK_OK;
+    }
     const bool warp = n <= 24;                          // one warp per (frequency, case), wpc systems per CTA; blocked LU above
     const size_t sys_bytes = (size_t)n * (n + 1) * sizeof(double2);
     const int wpc = warp ? (int)std::max<size_t>(1, std::min<size_t>(FARM_WPC, (100 * 1024) / sys_bytes)) : 1;
     const size_t smem = (size_t)wpc * sys_bytes;
-    if (smem > 227 * 1024) return set_err(RAFTK_EINVAL, "farm too large for the shared-memory solver (6N (6N+1) 16 B > 227 KB: N <= 19)");
     if (c->n_cases > 65535) return set_err(RAFTK_EINVAL, "farm response: more than 65535 cases per call");
     static SmemOptIn opt_w(48 * 1024), opt_b(48 * 1024);
     if (warp) CUDA_TRY(opt_w.ensure(k_farm_response<true>, smem));
@@ -900,7 +1007,14 @@ extern "C" int raftk_farm_response_dev(const raftk_designs *d, const raftk_cases
                                        void *stream)
 {
     disp_reset();
-    return farm_launch(d, c, solved, f, (cudaStream_t)stream);
+    return farm_launch(d, c, solved, f, nullptr, 0, (cudaStream_t)stream);
+}
+
+extern "C" int raftk_farm_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f,
+                                          void *workspace, size_t workspace_bytes, void *stream)
+{
+    disp_reset();
+    return farm_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 
@@ -1098,6 +1212,7 @@ static int host_run(const raftk_designs *d, const raftk_cases *c, const raftk_so
     if (farm) {
         // the system response reads the per-FOWT loads on the device: those buffers exist even when the caller does not want them back
         obytes += 4 * align_up(resp, 256) + align_up(nD * nC * 288, 256) + align_up(nC * nw * 4, 256) + 3 * align_up(36 * nD * nD * 8, 256);
+        obytes += align_up(farm_ws_bytes(d, c, farm), 256);            // slabs of the global-memory system kernel (0 on chip)
     }
     // the solve is planned once, at the caller's cluster size, and launched with the workspace that plan needs; excitation
     // and linearisation need the whole batch's tables in one chunk
@@ -1207,7 +1322,8 @@ static int host_run(const raftk_designs *d, const raftk_cases *c, const raftk_so
     if (farm) {
         fd.Xi_sys = static_cast<double *>(A.take(resp));
         fd.info = farm->info ? static_cast<int32_t *>(A.take(nC * nw * 4)) : nullptr;
-        rc = farm_launch(&dd, &cc, &od, &fd, st);
+        const size_t fwb = farm_ws_bytes(d, c, farm);
+        rc = farm_launch(&dd, &cc, &od, &fd, fwb ? A.take(fwb) : nullptr, fwb, st);
         if (rc) return rc;
     }
     auto down = [&](void *h, const void *dv, size_t n) { if (h && dv) { cudaError_t r = cudaMemcpyAsync(h, dv, n, cudaMemcpyDeviceToHost, st); if (r != cudaSuccess) e = r; } };

@@ -191,18 +191,12 @@ struct FarmParams {
 };
 #define FARM_WPC 4
 
-template <bool WARP>
-__global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(DesignsDev D, CasesDev Cs, FarmParams P)
+// Assembly of one (case c, frequency iw) system, shared by k_farm_response and k_farm_response_global: Z_sys into A [n][nc]
+// (nc = n + 1) and the right-hand side into its column n, spread over the gsize threads of a group.
+__device__ __forceinline__ void farm_assemble(const DesignsDev &D, const CasesDev &Cs, const FarmParams &P, int c, int iw, double2 *A,
+                                              int gtid, int gsize)
 {
-    extern __shared__ __align__(16) double smem_raw[];
-    __shared__ int piv_s[FARM_WPC], bad_s[FARM_WPC];
-    __shared__ double2 rinv_s[FARM_WPC];
     const int n = 6 * P.N, nc = n + 1, nw = P.nw;
-    const int g = WARP ? (int)(threadIdx.x >> 5) : 0, gtid = WARP ? (int)(threadIdx.x & 31) : (int)threadIdx.x;
-    const int gsize = WARP ? 32 : (int)blockDim.x;
-    const int iw = WARP ? (int)(blockIdx.x * (blockDim.x >> 5)) + g : (int)blockIdx.x, c = blockIdx.y;
-    if (iw >= nw) return;                                            // (warp-uniform; no CTA-wide barrier follows in the WARP variant)
-    double2 *A = reinterpret_cast<double2 *>(smem_raw) + (size_t)g * n * nc;
     const double w = D.w[iw], w2 = w * w;
     const int cp = Cs.primary ? Cs.primary[c] : c;                   // secondary wave trains use their primary's damping
     for (int t = gtid; t < n * n; t += gsize) {
@@ -230,12 +224,203 @@ __global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(De
         if (Cs.F_2nd) f.x += Cs.F_2nd[o];
         A[a * nc + n] = f;
     }
+}
+
+template <bool WARP>
+__global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(DesignsDev D, CasesDev Cs, FarmParams P)
+{
+    extern __shared__ __align__(16) double smem_raw[];
+    __shared__ int piv_s[FARM_WPC], bad_s[FARM_WPC];
+    __shared__ double2 rinv_s[FARM_WPC];
+    const int n = 6 * P.N, nc = n + 1, nw = P.nw;
+    const int g = WARP ? (int)(threadIdx.x >> 5) : 0, gtid = WARP ? (int)(threadIdx.x & 31) : (int)threadIdx.x;
+    const int gsize = WARP ? 32 : (int)blockDim.x;
+    const int iw = WARP ? (int)(blockIdx.x * (blockDim.x >> 5)) + g : (int)blockIdx.x, c = blockIdx.y;
+    if (iw >= nw) return;                                            // (warp-uniform; no CTA-wide barrier follows in the WARP variant)
+    double2 *A = reinterpret_cast<double2 *>(smem_raw) + (size_t)g * n * nc;
+    farm_assemble(D, Cs, P, c, iw, A, gtid, gsize);
     if (gtid == 0) bad_s[g] = 0;
     gsync<WARP>();
     if (WARP) lu_unblocked<true>(A, n, nc, 1, gtid, gsize, &piv_s[g], &rinv_s[g], &bad_s[g]);
     else lu_blocked(A, n, nc, 1, &piv_s[g], &rinv_s[g], &bad_s[g]);
     for (int a = gtid; a < n; a += gsize) P.Xi[((size_t)c * n + a) * nw + iw] = A[a * nc + n];
     if (gtid == 0 && P.info) P.info[(size_t)c * nw + iw] = bad_s[g];
+}
+
+// ------------------------------------------------------------------------------------------------
+// K3d: dense solves whose augmented system does not fit in one CTA's shared memory (farms of 20 and more FOWTs, any n for
+// raftk_system_solve).  The system stays in global memory (L2-resident while the CTA works on it); lu_global factors it with
+// the numerical contract of lu_blocked: partial pivoting on |re| + |im| with the first maximum winning (LAPACK izamax), row
+// swaps over every column the solve still reads, and each trailing element receiving its rank-1 contributions in elimination
+// order, so the rounding sequence is the column-at-a-time algorithm's.  Per panel of pw columns:
+//   1. the panel (rows kb..n-1) is copied to shared memory and factored there column by column;
+//   2. it goes back, and one thread per remaining column applies the panel's row swaps in order and the unit-lower solve
+//      of the row block;
+//   3. the trailing matrix takes the panel's pw rank-1 contributions from a 4 x 2 register tile per thread: every element is
+//      loaded and stored once per panel, so the panel width divides the traffic to the matrix.
+// Back substitution of the nrhs right-hand sides follows row by row.  Every thread of the CTA takes part; each kernel
+// loops over its systems with persistent CTAs, so a result depends on nothing but the system itself.
+// ------------------------------------------------------------------------------------------------
+#define GLU_T 256
+#define GLU_PWMAX 16
+struct GluShared {
+    double best[GLU_T / 32];
+    int idx[GLU_T / 32];
+    int piv[GLU_PWMAX];
+    int bad;
+};
+
+__device__ __forceinline__ void cmsub(double2 &v, const double2 l, const double2 u)
+{
+    v.x -= l.x * u.x - l.y * u.y; v.y -= l.x * u.y + l.y * u.x;
+}
+
+// The augmented system [A | B]: A [n][lda] (columns 0..n-1), B [n][ldb] (the nrhs right-hand sides, columns n..n+nrhs-1).
+// Ps: dynamic shared memory of n * pw double2.  On return B holds the solutions and S.bad the info word (k+1 of the first
+// zero pivot, else 0; read it after a __syncthreads()).  The factored A's columns left of each panel keep their pre-swap rows.
+__device__ __forceinline__ void lu_global(double2 *A, int lda, double2 *B, int ldb, int n, int nrhs, int pw, double2 *Ps, GluShared &S)
+{
+    const int tid = threadIdx.x, nc = n + nrhs;
+    auto el = [&](int r, int col) -> double2 * { return col < n ? A + (size_t)r * lda + col : B + (size_t)r * ldb + (col - n); };
+    if (tid == 0) S.bad = 0;
+    for (int kb = 0; kb < n; kb += pw) {
+        const int nb = min(pw, n - kb), m = n - kb, c0 = kb + nb;
+        // ---- 1. panel LU in shared memory -----------------------------------------------------------------------
+        for (int t = tid; t < m * nb; t += GLU_T) { const int r = t / nb, j = t - r * nb; Ps[r * pw + j] = A[(size_t)(kb + r) * lda + kb + j]; }
+        __syncthreads();
+        for (int j = 0; j < nb; j++) {
+            double best = -1.0; int p = j;
+            for (int r = j + tid; r < m; r += GLU_T) {
+                const double2 v = Ps[r * pw + j];
+                const double t = fabs(v.x) + fabs(v.y);
+                if (t > best) { best = t; p = r; }
+            }
+            for (int o = 16; o >= 1; o >>= 1) {
+                const double ob = __shfl_xor_sync(0xffffffffu, best, o);
+                const int op = __shfl_xor_sync(0xffffffffu, p, o);
+                if (ob > best || (ob == best && op < p)) { best = ob; p = op; }
+            }
+            if ((tid & 31) == 0) { S.best[tid >> 5] = best; S.idx[tid >> 5] = p; }
+            __syncthreads();
+            best = S.best[0]; p = S.idx[0];                            // every thread finishes the reduction: same winner everywhere
+#pragma unroll
+            for (int q = 1; q < GLU_T / 32; q++) if (S.best[q] > best || (S.best[q] == best && S.idx[q] < p)) { best = S.best[q]; p = S.idx[q]; }
+            const double2 pv = Ps[p * pw + j];
+            const double den = pv.x * pv.x + pv.y * pv.y;
+            const double2 ri = (den > 0.0) ? make_double2(pv.x / den, -pv.y / den) : make_double2(0.0, 0.0);
+            __syncthreads();                                           // pivot and reduction slots read by all before they change
+            if (tid == 0) { S.piv[j] = p; if (!(den > 0.0) && S.bad == 0) S.bad = kb + j + 1; }
+            if (p != j && tid < nb) { const double2 t1 = Ps[j * pw + tid]; Ps[j * pw + tid] = Ps[p * pw + tid]; Ps[p * pw + tid] = t1; }
+            __syncthreads();
+            for (int r = j + 1 + tid; r < m; r += GLU_T) {             // multiplier, then the panel's columns right of j
+                const double2 v = Ps[r * pw + j];
+                const double2 l = make_double2(v.x * ri.x - v.y * ri.y, v.x * ri.y + v.y * ri.x);
+                Ps[r * pw + j] = l;
+                for (int b = j + 1; b < nb; b++) { double2 x = Ps[r * pw + b]; cmsub(x, l, Ps[j * pw + b]); Ps[r * pw + b] = x; }
+            }
+            __syncthreads();
+        }
+        // ---- 2. panel back; row swaps and the row block's unit-lower solve, one thread per column ---------------------
+        for (int t = tid; t < m * nb; t += GLU_T) { const int r = t / nb, j = t - r * nb; A[(size_t)(kb + r) * lda + kb + j] = Ps[r * pw + j]; }
+        for (int col = c0 + tid; col < nc; col += GLU_T) {
+            for (int j = 0; j < nb; j++) {
+                const int p = S.piv[j];
+                if (p != j) { double2 *x = el(kb + j, col), *y = el(kb + p, col); const double2 t1 = *x; *x = *y; *y = t1; }
+            }
+            for (int j = 0; j < nb; j++) {
+                const double2 uj = *el(kb + j, col);
+                for (int r = j + 1; r < nb; r++) { double2 *q = el(kb + r, col); double2 v = *q; cmsub(v, Ps[r * pw + j], uj); *q = v; }
+            }
+        }
+        __syncthreads();
+        // ---- 3. trailing update, 4 x 2 register tile, contributions in elimination order --------------------------------
+        const int m2 = n - c0, ncol = nc - c0, tr = (m2 + 3) / 4, tc = (ncol + 1) / 2;
+        for (int t = tid; t < tr * tc; t += GLU_T) {
+            const int r0 = 4 * (t / tc), b0 = 2 * (t - (t / tc) * tc);
+            double2 *cp[2];
+            size_t ld[2];
+#pragma unroll
+            for (int y = 0; y < 2; y++) {
+                const int col = min(c0 + b0 + y, nc - 1);
+                cp[y] = col < n ? A + col : B + (col - n);
+                ld[y] = col < n ? (size_t)lda : (size_t)ldb;
+            }
+            double2 acc[4][2];
+#pragma unroll
+            for (int x = 0; x < 4; x++)
+#pragma unroll
+                for (int y = 0; y < 2; y++)
+                    acc[x][y] = (r0 + x < m2 && b0 + y < ncol) ? cp[y][(size_t)(c0 + r0 + x) * ld[y]] : make_double2(0.0, 0.0);
+            for (int j = 0; j < nb; j++) {
+                double2 l[4], u[2];
+#pragma unroll
+                for (int x = 0; x < 4; x++) l[x] = Ps[min(nb + r0 + x, m - 1) * pw + j];
+#pragma unroll
+                for (int y = 0; y < 2; y++) u[y] = cp[y][(size_t)(kb + j) * ld[y]];
+#pragma unroll
+                for (int x = 0; x < 4; x++)
+#pragma unroll
+                    for (int y = 0; y < 2; y++) cmsub(acc[x][y], l[x], u[y]);
+            }
+#pragma unroll
+            for (int x = 0; x < 4; x++)
+#pragma unroll
+                for (int y = 0; y < 2; y++)
+                    if (r0 + x < m2 && b0 + y < ncol) cp[y][(size_t)(c0 + r0 + x) * ld[y]] = acc[x][y];
+        }
+        __syncthreads();
+    }
+    // ---- back substitution, every right-hand side ------------------------------------------------------------------
+    for (int r = n - 1; r >= 0; r--) {
+        const double2 pv = A[(size_t)r * lda + r];
+        const double den = pv.x * pv.x + pv.y * pv.y;
+        for (int rh = tid; rh < nrhs; rh += GLU_T) {
+            const double2 s = B[(size_t)r * ldb + rh];
+            B[(size_t)r * ldb + rh] = make_double2((s.x * pv.x + s.y * pv.y) / den, (s.y * pv.x - s.x * pv.y) / den);
+        }
+        __syncthreads();
+        for (int t = tid; t < r * nrhs; t += GLU_T) {
+            const int rr = t / nrhs, rh = t - rr * nrhs;
+            double2 b = B[(size_t)rr * ldb + rh];
+            cmsub(b, A[(size_t)rr * lda + r], B[(size_t)r * ldb + rh]);
+            B[(size_t)rr * ldb + rh] = b;
+        }
+        __syncthreads();
+    }
+}
+
+// farm system response of k_farm_response (same assembly) for any N: persistent CTAs, CTA b owns slab b of the workspace
+// ([6N][6N+1] double2) and solves the (case, frequency) systems b, b + gridDim.x, ...
+__global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D, CasesDev Cs, FarmParams P, double2 *ws, int pw)
+{
+    extern __shared__ __align__(16) double smem_raw[];
+    __shared__ GluShared S;
+    double2 *Ps = reinterpret_cast<double2 *>(smem_raw);
+    const int n = 6 * P.N, nc = n + 1, nw = P.nw;
+    double2 *A = ws + (size_t)blockIdx.x * n * nc;
+    const long long nsys = (long long)P.nC * nw;
+    for (long long s = blockIdx.x; s < nsys; s += gridDim.x) {
+        const int c = (int)(s / nw), iw = (int)(s - (long long)c * nw);
+        farm_assemble(D, Cs, P, c, iw, A, threadIdx.x, GLU_T);
+        __syncthreads();
+        lu_global(A, nc, A + n, nc, n, 1, pw, Ps, S);
+        for (int a = threadIdx.x; a < n; a += GLU_T) P.Xi[((size_t)c * n + a) * nw + iw] = A[(size_t)a * nc + n];
+        if (threadIdx.x == 0 && P.info) P.info[(size_t)c * nw + iw] = S.bad;
+        __syncthreads();                                               // the slab is rewritten by the next system
+    }
+}
+
+// raftk_system_solve for any n: Z [nw][n][n] factored in place, F [nw][n][nrhs] overwritten with the solutions
+__global__ void __launch_bounds__(GLU_T, 2) k_system_solve_global(int n, int nw, int nrhs, int pw, double2 *Z, double2 *F, int *info)
+{
+    extern __shared__ __align__(16) double smem_raw[];
+    __shared__ GluShared S;
+    double2 *Ps = reinterpret_cast<double2 *>(smem_raw);
+    for (int iw = blockIdx.x; iw < nw; iw += gridDim.x) {
+        lu_global(Z + (size_t)iw * n * n, n, F + (size_t)iw * n * nrhs, nrhs, n, nrhs, pw, Ps, S);
+        if (threadIdx.x == 0 && info) info[iw] = S.bad;
+        __syncthreads();
+    }
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -712,6 +712,14 @@ def hydro_linearization(batch, cases, Xi, want=("B_drag", "F_drag")):
     return outs
 
 
+def farm_workspace_bytes(n_fowt, n_cases, nw):
+    """Device workspace the farm system response needs (raftk_farm_workspace_bytes): 0 while the [6N][6N+1] system fits in
+    shared memory, else one slab per resident CTA of the global-memory kernel.  Answers for an H100 without a device."""
+    d, c, f = RaftkDesigns(), RaftkCases(), RaftkFarm()
+    d.n_designs, d.nw, c.n_cases, f.n_fowt = int(n_fowt), int(nw), int(n_cases), int(n_fowt)
+    return int(lib.raftk_farm_workspace_bytes(C.byref(d), C.byref(c), C.byref(f)))
+
+
 def system_solve(Z, F):
     """Farm system response (raft_model.py:1164-1216): Z [nw,n,n], F [nw,n] or [nw,n,nrhs] -> Xi, info."""
     Z = np.array(Z, dtype=np.complex128, order="C")
@@ -864,7 +872,9 @@ class DeviceSession:
 
     def farm_response(self, C_arr=None, M_arr=None, B_arr=None):
         """Enqueue the coupled 6N-DOF system response of the LAST ``solve`` (the session's designs are the FOWTs of the
-        array; it must have been created with want including B_drag, F_drag, F_iner [+ F_BEM]).  -> (Xi_sys [nC,6N,nw], info)."""
+        array; it must have been created with want including B_drag, F_drag, F_iner [+ F_BEM]).  -> (Xi_sys [nC,6N,nw], info).
+        Any N: farms whose system does not fit in shared memory are solved in a device workspace sized once
+        (raftk_farm_workspace_bytes) and kept with the session."""
         torch = self.torch
         N, nC, nw = self.batch.n_designs, self.cases.n_cases, self.batch.nw
         n = 6 * N
@@ -879,10 +889,14 @@ class DeviceSession:
             for nm, t in mats.items():
                 setattr(f, nm, t.data_ptr() if t is not None else None)
             f.Xi_sys, f.info = xi.data_ptr(), info.data_ptr()
-            self._farm = (f, mats, xi, info)
-        f, _, xi, info = self._farm
+            wsb = int(lib.raftk_farm_workspace_bytes(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(f)))
+            with torch.cuda.device(self.device):
+                ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=self.device)
+            self._farm = (f, mats, xi, info, ws, wsb)
+        f, _, xi, info, ws, wsb = self._farm
         with torch.cuda.device(self.device):
-            check(lib.raftk_farm_response_dev(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f), self._stream()))
+            check(lib.raftk_farm_response_ws_dev(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f),
+                                                 ws.data_ptr(), wsb, self._stream()))
         return xi, info
 
     def second_order_force(self):
@@ -913,7 +927,8 @@ def launch_count():
 
 DISPATCH_FAMILIES = ("none", "solve", "qtf", "general", "farm", "system")          # include/raftk.h RAFTK_FAMILY_*
 DISPATCH_KERNELS = ("none", "v1", "fused128", "fused256", "fused2-cluster", "fused2-grid", "qtf-tiles", "qtf-diag", "qtf-diag-mix",
-                    "gen-blocked", "gen-unblocked", "farm-rows12", "farm-warp", "farm-block", "sys-unblocked", "sys-blocked")   # RAFTK_KERNEL_*
+                    "gen-blocked", "gen-unblocked", "farm-rows12", "farm-warp", "farm-block", "sys-unblocked", "sys-blocked",
+                    "farm-global", "sys-global")   # RAFTK_KERNEL_*
 
 
 def last_dispatch():
