@@ -358,6 +358,39 @@ int raftk_general_solve_dynamics_host(const raftk_general *g, const raftk_cases 
                                       int32_t *status);
 
 /*
+ * Frequency-dependent terms of the generalised-DOF solve (raft_model.py:1005-1010, 1045-1048): the added mass and damping
+ * of operating rotors (sum A_aero, B_aero; raft_fowt.py:1557-1562) and of potential-flow coefficients (A_BEM, B_BEM, lumped on
+ * reduced DOFs 0-5 by readHydro, raft_fowt.py:1479-1480), and the BEM wave excitation F_BEM = T^T F_BEM_fullDOF
+ * (raft_fowt.py:1796-1849, 1885-1887).  raft_b200.packer.pack_general_matrices builds it.
+ * The matrices are given on their support fd_idx only: every entry outside it is zero, so the restricted table gives the same
+ * impedance as the dense [n_dof,n_dof,nw] sum.  On the support, M = M + A_w, B = (B + B_w) + B_drag and
+ * Z = fma(-w^2, M, C) + i w B (the rigid solver's grouping); every other entry is computed exactly as without fd.
+ * The BEM force of every case (secondary trains included) is added to the inertial excitation before the drag excitation:
+ * (F_BEM + F_iner) + F_drag.
+ * Pointers are device pointers for *_dev and host pointers for *_host.  Rejected with RAFTK_EINVAL before any launch: n_fd
+ * outside [0, n_dof], fd_idx out of range, repeated or unsorted, n_bem_head < 0, a missing table for a nonzero count, headings
+ * that decrease or fall outside [0, 360) (equal neighbours are legal).  The *_dev entry reads fd_idx and bem_headings back
+ * to the host for these checks (a copy on the caller's stream and a wait for it).
+ */
+typedef struct raftk_general_fd {
+    int32_t n_fd, n_bem_head;
+    const int32_t *fd_idx;          /* [n_fd] reduced DOFs carrying frequency-dependent terms, strictly increasing        */
+    const double *A_w, *B_w;        /* [n_fd,n_fd,nw] (the reference's [n,n,nw] layout restricted to fd_idx); NULL if n_fd = 0 */
+    const double *bem_headings;     /* [n_bem_head] deg, non-decreasing in [0,360)                                         */
+    const double *X_BEM;            /* complex [n_bem_head,6,nw], heading-relative (packer.pack_bem_excitation's table)      */
+    const double *T0;               /* [6,n_dof]: rows 0..5 of fowt.T (maps the full-DOF BEM force to reduced DOFs)          */
+    double x_ref, y_ref, heading_adjust;
+} raftk_general_fd;
+
+/* fd = NULL: the constant-matrix solve of raftk_general_solve_dynamics_*, bit for bit (those entry points call these).
+ * F_BEM: optional output, complex [n_cases,n_dof,nw] in reduced DOFs (zero without BEM tables), or NULL. */
+size_t raftk_general_fd_workspace_bytes(const raftk_general *g, const raftk_general_fd *fd, int32_t n_cases);
+int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c, const raftk_solve_opts *o,
+                                        double *Xi, int32_t *status, double *F_BEM, void *workspace, size_t workspace_bytes, void *stream);
+int raftk_general_solve_dynamics_fd_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c, const raftk_solve_opts *o,
+                                         double *Xi, int32_t *status, double *F_BEM);
+
+/*
  * Output channels of FOWT.saveTurbineOutputs for a FOWT with generalised degrees of freedom (raft_fowt.py:2299-2604): PRP
  * motions, nacelle accelerations and flexible-tower base loads are real linear functionals of the reduced response,
  *   Y_ch(w) = w^wpow[ch] sum_b R[ch,b] Xi[b,w]     (raft_b200.packer.pack_general_channels; rad2deg folded into R)

@@ -83,6 +83,13 @@ class RaftkGeneral(C.Structure):
                  ("depth", C.c_double), ("rho", C.c_double), ("dw", C.c_double)] + [(n, C.c_void_p) for n in GENERAL_ARRAYS])
 
 
+class RaftkGeneralFd(C.Structure):
+    """Frequency-dependent terms of the generalised-DOF solve, include/raftk.h raftk_general_fd."""
+    _fields_ = [("n_fd", C.c_int32), ("n_bem_head", C.c_int32), ("fd_idx", C.c_void_p), ("A_w", C.c_void_p), ("B_w", C.c_void_p),
+                ("bem_headings", C.c_void_p), ("X_BEM", C.c_void_p), ("T0", C.c_void_p),
+                ("x_ref", C.c_double), ("y_ref", C.c_double), ("heading_adjust", C.c_double)]
+
+
 class RaftkSlender(C.Structure):
     _fields_ = ([("n_nodes", C.c_int32), ("n_members", C.c_int32), ("n_seg", C.c_int32), ("nw", C.c_int32),
                  ("depth", C.c_double), ("rho", C.c_double), ("g", C.c_double)] + [(n, C.c_void_p) for n in SLENDER_ARRAYS])
@@ -128,6 +135,7 @@ SYMBOLS = [
     "raftk_second_order_force_dev", "raftk_second_order_force_host",
     "raftk_qtf_slender_workspace_bytes", "raftk_qtf_slender_dev", "raftk_qtf_slender_host",
     "raftk_general_workspace_bytes", "raftk_general_solve_dynamics_dev", "raftk_general_solve_dynamics_host",
+    "raftk_general_fd_workspace_bytes", "raftk_general_solve_dynamics_fd_dev", "raftk_general_solve_dynamics_fd_host",
     "raftk_system_solve_dev", "raftk_system_solve_host", "raftk_response_stats_dev", "raftk_response_stats_host",
     "raftk_channel_stats_dev", "raftk_channel_stats_host", "raftk_general_channel_stats_dev", "raftk_general_channel_stats_host",
     "raftk_host_alloc", "raftk_host_free",
@@ -186,6 +194,14 @@ def _load():
     lib.raftk_general_solve_dynamics_host.argtypes = [P(RaftkGeneral), P(RaftkCases), P(RaftkSolveOpts), C.c_void_p, C.c_void_p]
     lib.raftk_general_solve_dynamics_dev.restype = C.c_int
     lib.raftk_general_solve_dynamics_host.restype = C.c_int
+    lib.raftk_general_fd_workspace_bytes.restype = C.c_size_t
+    lib.raftk_general_fd_workspace_bytes.argtypes = [P(RaftkGeneral), P(RaftkGeneralFd), C.c_int32]
+    lib.raftk_general_solve_dynamics_fd_dev.argtypes = [P(RaftkGeneral), P(RaftkGeneralFd), P(RaftkCases), P(RaftkSolveOpts), C.c_void_p, C.c_void_p,
+                                                        C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.raftk_general_solve_dynamics_fd_host.argtypes = [P(RaftkGeneral), P(RaftkGeneralFd), P(RaftkCases), P(RaftkSolveOpts), C.c_void_p, C.c_void_p,
+                                                         C.c_void_p]
+    lib.raftk_general_solve_dynamics_fd_dev.restype = C.c_int
+    lib.raftk_general_solve_dynamics_fd_host.restype = C.c_int
     lib.raftk_system_solve_dev.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.raftk_system_solve_host.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.raftk_response_stats_dev.argtypes = [C.c_int32, C.c_int32, C.c_double, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -1406,42 +1406,88 @@ extern "C" int raftk_second_order_force_host(const raftk_designs *d, const raftk
 }
 
 // ---- generalised degrees of freedom (flexible members) ---------------------------------------------------------------
-struct GenLayout { size_t u, f6, Fi, Fd, XL, Bm, Bd, Z, pv, fl, total; };
-static GenLayout gen_layout(const raftk_general *g, size_t nC)
+struct GenLayout { size_t u, f6, Fi, Fd, XL, Bm, Bd, Z, pv, fl, fb6, FB, total; };
+static GenLayout gen_layout(const raftk_general *g, const raftk_general_fd *fd, size_t nC)
 {
     const size_t n = g->n_dof, nw = g->nw, Ns = std::max(g->n_nodes, 1);
+    const size_t nbem = (fd && fd->n_bem_head > 0) ? 1 : 0;
     GenLayout L; size_t t = 0;
     auto take = [&](size_t b) { size_t o = t; t += align_up(b, 256); return o; };
     L.u = take(nC * Ns * 3 * nw * 16); L.f6 = take(nC * Ns * 6 * nw * 16);
     L.Fi = take(nC * n * nw * 16); L.Fd = take(nC * n * nw * 16); L.XL = take(nC * n * nw * 16);
     L.Bm = take(nC * Ns * 9 * 8); L.Bd = take(nC * n * n * 8);
     L.Z = take(nC * nw * n * (n + 1) * 16); L.pv = take(nC * nw * n * 4); L.fl = take(nC * 16);
+    L.fb6 = take(nbem * nC * 6 * nw * 16); L.FB = take(nbem * nC * n * nw * 16);     // BEM force (full DOFs 0-5, reduced DOFs)
     L.total = t;
     return L;
 }
 
-extern "C" size_t raftk_general_workspace_bytes(const raftk_general *g, int32_t n_cases)
+// raftk_general_fd checks on host copies of fd_idx and bem_headings (include/raftk.h)
+static int validate_gen_fd(const raftk_general *g, const raftk_general_fd *fd, const int32_t *idx, const double *hd)
 {
-    if (!g || n_cases <= 0 || g->n_dof <= 0 || g->nw <= 0) return 0;
-    return gen_layout(g, (size_t)n_cases).total;
+    if (fd->n_fd < 0 || fd->n_fd > g->n_dof) return set_err(RAFTK_EINVAL, "general solve: fd.n_fd must be in [0, n_dof]");
+    if (fd->n_bem_head < 0) return set_err(RAFTK_EINVAL, "general solve: fd.n_bem_head must be >= 0");
+    if (fd->n_fd > 0 && (!fd->fd_idx || !fd->A_w || !fd->B_w))
+        return set_err(RAFTK_EINVAL, "general solve: fd.n_fd > 0 needs fd_idx, A_w and B_w");
+    if (fd->n_bem_head > 0 && (!fd->bem_headings || !fd->X_BEM || !fd->T0))
+        return set_err(RAFTK_EINVAL, "general solve: fd.n_bem_head > 0 needs bem_headings, X_BEM and T0");
+    for (int t = 0; t < fd->n_fd; t++) {
+        if (idx[t] < 0 || idx[t] >= g->n_dof) return set_err(RAFTK_EINVAL, "general solve: fd.fd_idx entry out of range [0, n_dof)");
+        if (t > 0 && idx[t] <= idx[t - 1]) return set_err(RAFTK_EINVAL, "general solve: fd.fd_idx must be strictly increasing (no repeats)");
+    }
+    for (int t = 0; t < fd->n_bem_head; t++) {
+        if (!(hd[t] >= 0.0 && hd[t] < 360.0)) return set_err(RAFTK_EINVAL, "general solve: fd.bem_headings must lie in [0, 360) deg");
+        if (t > 0 && hd[t] < hd[t - 1]) return set_err(RAFTK_EINVAL, "general solve: fd.bem_headings must be non-decreasing");
+    }
+    return 0;
 }
 
-extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
-                                                int32_t *status, void *workspace, size_t workspace_bytes, void *stream)
+extern "C" size_t raftk_general_fd_workspace_bytes(const raftk_general *g, const raftk_general_fd *fd, int32_t n_cases)
+{
+    if (!g || n_cases <= 0 || g->n_dof <= 0 || g->nw <= 0) return 0;
+    return gen_layout(g, fd, (size_t)n_cases).total;
+}
+
+extern "C" size_t raftk_general_workspace_bytes(const raftk_general *g, int32_t n_cases)
+{
+    return raftk_general_fd_workspace_bytes(g, nullptr, n_cases);
+}
+
+extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
+                                                   const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM,
+                                                   void *workspace, size_t workspace_bytes, void *stream)
 {
     disp_reset();
     if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
     if (g->n_dof <= 0 || g->n_dof > 256 || g->nw <= 0 || g->n_nodes < 0 || c->n_cases <= 0 || c->n_cases > 65535)
         return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, 0 < n_cases <= 65535");
     if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (fd) {                                          // the index and heading tables are read back for the checks
+        if (fd->n_fd < 0 || fd->n_fd > g->n_dof || fd->n_bem_head < 0 || (fd->n_fd > 0 && !fd->fd_idx) || (fd->n_bem_head > 0 && !fd->bem_headings))
+            return validate_gen_fd(g, fd, nullptr, nullptr);
+        std::vector<int32_t> idx(fd->n_fd);
+        std::vector<double> hd(fd->n_bem_head);
+        if (fd->n_fd > 0) CUDA_TRY(cudaMemcpyAsync(idx.data(), fd->fd_idx, idx.size() * 4, cudaMemcpyDeviceToHost, st));
+        if (fd->n_bem_head > 0) CUDA_TRY(cudaMemcpyAsync(hd.data(), fd->bem_headings, hd.size() * 8, cudaMemcpyDeviceToHost, st));
+        if (fd->n_fd > 0 || fd->n_bem_head > 0) CUDA_TRY(cudaStreamSynchronize(st));
+        if (int rc = validate_gen_fd(g, fd, idx.data(), hd.data())) return rc;
+    }
     const size_t nC = c->n_cases;
-    const GenLayout L = gen_layout(g, nC);
+    const GenLayout L = gen_layout(g, fd, nC);
     if (!workspace || workspace_bytes < L.total) return set_err(RAFTK_ENOMEM, "general solve: workspace too small");
+    const bool bem = fd && fd->n_bem_head > 0;
     GenDev D;
     D.n = g->n_dof; D.nw = g->nw; D.Ns = g->n_nodes; D.depth = g->depth; D.dw = g->dw; D.rho = g->rho;
     D.w = g->w; D.k = g->k; D.node_r = g->node_r; D.node_frame = g->node_frame; D.node_circ = g->node_circ;
     D.node_Imat = g->node_Imat; D.node_Imat_w = reinterpret_cast<const double2 *>(g->node_Imat_w);
     D.node_a_i = g->node_a_i; D.node_cd = g->node_cd; D.Tn = g->Tn; D.rr = g->rr; D.M = g->M; D.B = g->B; D.C = g->C;
+    GenFdDev Fx;
+    Fx.n_fd = fd ? fd->n_fd : 0; Fx.n_bem_head = bem ? fd->n_bem_head : 0;
+    Fx.fd_idx = fd ? fd->fd_idx : nullptr; Fx.A_w = fd ? fd->A_w : nullptr; Fx.B_w = fd ? fd->B_w : nullptr;
+    Fx.bem_headings = bem ? fd->bem_headings : nullptr; Fx.X_BEM = bem ? reinterpret_cast<const double2 *>(fd->X_BEM) : nullptr;
+    Fx.T0 = bem ? fd->T0 : nullptr;
+    Fx.x_ref = fd ? fd->x_ref : 0.0; Fx.y_ref = fd ? fd->y_ref : 0.0; Fx.hadj = fd ? fd->heading_adjust : 0.0;
     char *b = static_cast<char *>(workspace);
     GenWork W;
     W.u = reinterpret_cast<double2 *>(b + L.u); W.f6 = reinterpret_cast<double2 *>(b + L.f6);
@@ -1449,40 +1495,52 @@ extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const ra
     W.XiLast = reinterpret_cast<double2 *>(b + L.XL); W.Bmat = reinterpret_cast<double *>(b + L.Bm);
     W.B_drag = reinterpret_cast<double *>(b + L.Bd); W.Z = reinterpret_cast<double2 *>(b + L.Z); W.flags = reinterpret_cast<int *>(b + L.fl);
     W.piv = reinterpret_cast<int *>(b + L.pv);
+    Fx.fb6 = bem ? reinterpret_cast<double2 *>(b + L.fb6) : nullptr;
+    double2 *Fbem = bem ? (F_BEM ? reinterpret_cast<double2 *>(F_BEM) : reinterpret_cast<double2 *>(b + L.FB)) : nullptr;
+    Fx.F_BEM = Fbem;
     const int *prim = c->primary;
     CasesDev C = to_dev(c);
-    cudaStream_t st = (cudaStream_t)stream;
     double2 *X = reinterpret_cast<double2 *>(Xi);
     const unsigned fb = (unsigned)((g->nw + 127) / 128);
     // blocked LU (panel + row block in shared memory); RAFTK_GEN_UNBLOCKED=1 keeps the first, column-at-a-time kernel for A/B runs
     const size_t lu_smem = ((size_t)g->n_dof * GB + (size_t)GB * (g->n_dof + 1)) * sizeof(double2);
     const bool blocked = !getenv("RAFTK_GEN_UNBLOCKED") && lu_smem <= 110 * 1024;
+    const bool fdz = Fx.n_fd > 0;                      // impedance with the frequency-dependent terms on their support
     if (blocked) {
-        static SmemOptIn opt(48 * 1024);
-        CUDA_TRY(opt.ensure(k_gen_solve_blocked, lu_smem));
+        static SmemOptIn opt(48 * 1024), opt_fd(48 * 1024);
+        CUDA_TRY(fdz ? opt_fd.ensure(k_gen_solve_blocked<true>, lu_smem) : opt.ensure(k_gen_solve_blocked<false>, lu_smem));
     }
+    if (F_BEM && !bem) CUDA_TRY(cudaMemsetAsync(F_BEM, 0, nC * g->n_dof * g->nw * 16, st));
     prof_begin_call();
     k_gen_init<<<(unsigned)nC, 256, 0, st>>>(D, W, o->xi_start, prim);
     if (g->n_nodes > 0) k_gen_wave<<<dim3(fb, g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, C, W);
-    k_gen_project<<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_iner, 0, nullptr);
+    if (bem) {                                         // F_BEM = T0^T f_BEM, then F_iner = F_BEM + sum_j Tn_j^T f6_j
+        k_gen_bem<<<dim3(fb, (unsigned)nC), 128, 0, st>>>(D, C, Fx);
+        k_gen_project<true, false><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, Fbem, 0, nullptr, Fx);
+        g_launches += 2;
+    }
+    if (bem) k_gen_project<false, true><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_iner, 0, nullptr, Fx);
+    else k_gen_project<false, false><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_iner, 0, nullptr, Fx);
     g_launches += 3;
     for (int pass = 0; pass < o->n_iter + 1; pass++) {
         if (g->n_nodes > 0) k_gen_node_pass<false><<<dim3(g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, W, nullptr);
         k_gen_bdrag<<<dim3(g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W);
-        k_gen_project<<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_drag, 1, nullptr);
+        k_gen_project<false, false><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_drag, 1, nullptr, Fx);
         if (blocked) {
             ProfScope ps(st, 2);
-            k_gen_solve_blocked<<<dim3(g->nw, (unsigned)nC), GT, lu_smem, st>>>(D, W, X, o->tol);
+            if (fdz) k_gen_solve_blocked<true><<<dim3(g->nw, (unsigned)nC), GT, lu_smem, st>>>(D, W, X, o->tol, Fx);
+            else k_gen_solve_blocked<false><<<dim3(g->nw, (unsigned)nC), GT, lu_smem, st>>>(D, W, X, o->tol, Fx);
         } else {
             ProfScope ps(st, 2);
-            k_gen_solve<<<dim3(g->nw, (unsigned)nC), 256, 0, st>>>(D, W, X, o->tol);
+            if (fdz) k_gen_solve<true><<<dim3(g->nw, (unsigned)nC), 256, 0, st>>>(D, W, X, o->tol, Fx);
+            else k_gen_solve<false><<<dim3(g->nw, (unsigned)nC), 256, 0, st>>>(D, W, X, o->tol, Fx);
         }
         k_gen_relax<<<(unsigned)nC, 256, 0, st>>>(D, W, X);
         g_launches += 5;
     }
     if (prim) {                                        // secondary trains: the primary's last Bmat and LU factors
         if (g->n_nodes > 0) k_gen_node_pass<true><<<dim3(g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, W, prim);
-        k_gen_project<<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_drag, 0, prim);
+        k_gen_project<false, false><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_drag, 0, prim, Fx);
         k_gen_train_solve<<<dim3(g->nw, (unsigned)nC), 128, 0, st>>>(D, W, prim, X);
         g_launches += 3;
     }
@@ -1494,8 +1552,14 @@ extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const ra
     return RAFTK_OK;
 }
 
-extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
-                                                 int32_t *status)
+extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
+                                                int32_t *status, void *workspace, size_t workspace_bytes, void *stream)
+{
+    return raftk_general_solve_dynamics_fd_dev(g, nullptr, c, o, Xi, status, nullptr, workspace, workspace_bytes, stream);
+}
+
+extern "C" int raftk_general_solve_dynamics_fd_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
+                                                    const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM)
 {
     disp_reset();
     if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
@@ -1506,9 +1570,12 @@ extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const r
             const int p = c->primary[i];
             if (p < 0 || (size_t)p >= nC || c->primary[p] != p) return set_err(RAFTK_EINVAL, "general solve: cases.primary must map every case to a primary case");
         }
+    if (fd)
+        if (int rc = validate_gen_fd(g, fd, fd->fd_idx, fd->bem_headings)) return rc;
     size_t total = 0;
     auto take = [&](size_t b) { size_t o_ = total; total += align_up(std::max<size_t>(b, 8), 256); return o_; };
     raftk_general gg = *g; raftk_cases cc = *c;
+    raftk_general_fd ff = fd ? *fd : raftk_general_fd{};
     struct Item { size_t off; const void *h; size_t nb; const void **slot; };
     std::vector<Item> items;
     auto add = [&](const void *h, size_t nb, const void **slot) { if (h) items.push_back({take(nb), h, nb, slot}); };
@@ -1521,18 +1588,37 @@ extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const r
     add(c->Hs, nC * 8, (const void **)&cc.Hs); add(c->Tp, nC * 8, (const void **)&cc.Tp); add(c->gamma, nC * 8, (const void **)&cc.gamma);
     add(c->beta_deg, nC * 8, (const void **)&cc.beta_deg); add(c->spec, nC * 4, (const void **)&cc.spec); add(c->zeta, nC * nw * 8, (const void **)&cc.zeta);
     add(c->primary, nC * 4, (const void **)&cc.primary);
-    const size_t o_xi = take(nC * n * nw * 16), o_st = take(nC * 16);
-    const size_t wb = raftk_general_workspace_bytes(g, (int32_t)nC), o_ws = take(wb);
+    if (fd) {
+        const size_t nf = std::max(fd->n_fd, 0), nh = std::max(fd->n_bem_head, 0);
+        if (nf) {
+            add(fd->fd_idx, nf * 4, (const void **)&ff.fd_idx);
+            add(fd->A_w, nf * nf * nw * 8, (const void **)&ff.A_w); add(fd->B_w, nf * nf * nw * 8, (const void **)&ff.B_w);
+        }
+        if (nh) {
+            add(fd->bem_headings, nh * 8, (const void **)&ff.bem_headings); add(fd->X_BEM, nh * 6 * nw * 16, (const void **)&ff.X_BEM);
+            add(fd->T0, 6 * n * 8, (const void **)&ff.T0);
+        }
+    }
+    const size_t o_xi = take(nC * n * nw * 16), o_st = take(nC * 16), o_fb = F_BEM ? take(nC * n * nw * 16) : 0;
+    const size_t wb = raftk_general_fd_workspace_bytes(g, fd, (int32_t)nC), o_ws = take(wb);
     ScratchCall sc;
     if (!sc.reserve(total)) return set_err(RAFTK_ENOMEM, "general solve: device scratch allocation failed");
     char *base = sc.take<char>(total);
     for (auto &it : items) { CUDA_TRY(cudaMemcpy(base + it.off, it.h, it.nb, cudaMemcpyHostToDevice)); *it.slot = base + it.off; }
-    int rc = raftk_general_solve_dynamics_dev(&gg, &cc, o, reinterpret_cast<double *>(base + o_xi), reinterpret_cast<int32_t *>(base + o_st),
-                                              base + o_ws, wb, nullptr);
+    int rc = raftk_general_solve_dynamics_fd_dev(&gg, fd ? &ff : nullptr, &cc, o, reinterpret_cast<double *>(base + o_xi),
+                                                 reinterpret_cast<int32_t *>(base + o_st), F_BEM ? reinterpret_cast<double *>(base + o_fb) : nullptr,
+                                                 base + o_ws, wb, nullptr);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpy(Xi, base + o_xi, nC * n * nw * 16, cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemcpy(status, base + o_st, nC * 16, cudaMemcpyDeviceToHost));
+    if (F_BEM) CUDA_TRY(cudaMemcpy(F_BEM, base + o_fb, nC * n * nw * 16, cudaMemcpyDeviceToHost));
     return RAFTK_OK;
+}
+
+extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
+                                                 int32_t *status)
+{
+    return raftk_general_solve_dynamics_fd_host(g, nullptr, c, o, Xi, status, nullptr);
 }
 
 // ---- slender-body QTF ----------------------------------------------------------------------------------

@@ -7,12 +7,14 @@
 // of its structural node and its offset rr_j from it; node motion = Tn_j Xi, node load -> Tn_j^T [f ; rr_j x f].
 // Launch sequence per call (no host synchronisation; cases that have converged skip their CTAs):
 //   k_gen_wave      (case, node, w)   wave kinematics u, inertial node load f6 = [f ; rr x f]
-//   k_gen_project   (case, dof, w)    F = sum_j Tn_j^T f6_j                       (used for F_iner and F_drag)
+//   k_gen_bem       (case, w)         BEM tables only: 6-component BEM force (full DOFs 0-5) of every case and train
+//   k_gen_project   (case, dof, w)    F = sum_j Tn_j^T f6_j   (F_BEM = T0^T f_BEM; F_iner = F_BEM + sum_j Tn_j^T f6_j; F_drag)
 //   per pass:
 //   k_gen_node_pass (case, node)      node velocity from Tn_j XiLast, RMS over w, linearised Bmat_j, drag load f6
 //   k_gen_bdrag     (case, row)       B_drag = sum_j Tn_j^T B6_j Tn_j
 //   k_gen_project                     F_drag
-//   k_gen_solve     (case, w)         Z = -w^2 M + i w (B + B_drag) + C, dense complex LU with partial pivoting, Xi
+//   k_gen_solve     (case, w)         Z = -w^2 M + i w (B + B_drag) + C, dense complex LU with partial pivoting, Xi;
+//                                     on the support of the frequency-dependent terms M + A_w(w) and B + B_w(w) (gen_impedance)
 //   k_gen_relax     (case)            convergence bookkeeping, XiLast = 0.2 XiLast + 0.8 Xi
 // Wave trains (cases.primary): a secondary train takes no part in the loop (done at init); after it
 //   k_gen_node_pass<true>   (case, node)   drag node load from the PRIMARY's last Bmat and the train's own u
@@ -36,6 +38,20 @@ struct GenDev {
     const double *rr;            // [Ns][3]
     const double *M, *B, *C;     // [n][n]
     double rho;
+};
+
+// frequency-dependent terms (raftk_general_fd), a parameter of their own so that every kernel of the constant-matrix solve
+// keeps its parameter layout; n_fd = 0 / n_bem_head = 0 without them
+struct GenFdDev {
+    int n_fd, n_bem_head;
+    const int *fd_idx;           // [n_fd] strictly increasing reduced DOFs
+    const double *A_w, *B_w;     // [n_fd][n_fd][nw]
+    const double *bem_headings;  // [n_bem_head] deg
+    const double2 *X_BEM;        // [n_bem_head][6][nw] heading-relative
+    const double *T0;            // [6][n] rows 0..5 of fowt.T
+    double x_ref, y_ref, hadj;
+    double2 *fb6;                // [nC][6][nw] workspace: BEM force in full DOFs 0-5
+    const double2 *F_BEM;        // [nC][n][nw] BEM force in reduced DOFs, added to F_iner
 };
 
 struct GenWork {                 // per-call workspace views
@@ -95,17 +111,20 @@ __global__ void __launch_bounds__(128) k_gen_wave(GenDev D, CasesDev Cs, GenWork
     W.f6[fb + (size_t)5 * nw] = make_double2(rr[0] * f[1].x - rr[1] * f[0].x, rr[0] * f[1].y - rr[1] * f[0].y);
 }
 
-// k_gen_project: F[c][dof][i] = sum_j sum_b Tn_j[b][dof] f6_j[b][i].  grid (ceil(nw/128), n, nC), block 128.
-// sec_only (the primary map) restricts it to the secondary trains.
-__global__ void __launch_bounds__(128) k_gen_project(GenDev D, GenWork W, double2 *F, int skip_done, const int *sec_only)
+// k_gen_project: F[c][dof][i] = sum_j sum_b T_j[b][dof] f6_j[b][i] over Ns loads f6 [nC][Ns][6][nw] with their 6 x n blocks
+// T [Ns][6][n]: the strip nodes' Tn and node loads (BEM = false), or T0 and the BEM force of k_gen_bem (BEM = true, Ns = 1);
+// plus X.F_BEM with ADD (F_iner = F_BEM + ...).  grid (ceil(nw/128), n, nC), block 128.  sec_only (the primary map)
+// restricts it to the secondary trains.
+template <bool BEM, bool ADD>
+__global__ void __launch_bounds__(128) k_gen_project(GenDev D, GenWork W, double2 *F, int skip_done, const int *sec_only, GenFdDev X)
 {
     const int i = blockIdx.x * 128 + threadIdx.x, dof = blockIdx.y, c = blockIdx.z;
     if (i >= D.nw || (skip_done && W.flags[4 * c]) || (sec_only && sec_only[c] == c)) return;
     const int nw = D.nw, n = D.n;
     double sr = 0.0, si = 0.0;
-    for (int j = 0; j < D.Ns; j++) {
-        const double *T = D.Tn + (size_t)j * 6 * n + dof;
-        const double2 *f = W.f6 + (((size_t)c * D.Ns + j) * 6) * nw + i;
+    for (int j = 0; j < (BEM ? 1 : D.Ns); j++) {
+        const double *T = (BEM ? X.T0 : D.Tn) + (size_t)j * 6 * n + dof;
+        const double2 *f = (BEM ? X.fb6 : W.f6) + (((size_t)c * (BEM ? 1 : D.Ns) + j) * 6) * nw + i;
 #pragma unroll
         for (int b = 0; b < 6; b++) {
             const double t = T[(size_t)b * n];
@@ -113,7 +132,53 @@ __global__ void __launch_bounds__(128) k_gen_project(GenDev D, GenWork W, double
             sr = fma(t, v.x, sr); si = fma(t, v.y, si);
         }
     }
+    if constexpr (ADD) { const double2 a = X.F_BEM[((size_t)c * n + dof) * nw + i]; sr = a.x + sr; si = a.y + si; }
     F[((size_t)c * n + dof) * nw + i] = make_double2(sr, si);
+}
+
+// k_gen_bem: grid (ceil(nw/128), nC), block 128: BEM excitation of every case (secondary trains with their own heading and
+// sea state, raft_model.py:1200-1236) in full DOFs 0-5, from the rigid solvers' bem_excitation_table
+__global__ void __launch_bounds__(128) k_gen_bem(GenDev D, CasesDev Cs, GenFdDev X)
+{
+    const int i = blockIdx.x * 128 + threadIdx.x, c = blockIdx.y;
+    if (i >= D.nw) return;
+    const int nw = D.nw;
+    const double beta = Cs.beta_deg[c] * (CUDART_PI / 180.0);
+    double sb, cb;
+    sincos(beta, &sb, &cb);
+    const double zeta = sea_state_zeta(Cs, c, i, nw, D.w[i], D.dw);
+    double Br[6], Bi[6];
+    bem_excitation_table(X.bem_headings, X.n_bem_head, X.X_BEM, nw, X.x_ref, X.y_ref, X.hadj, i, D.k[i], beta, sb, cb, zeta, Br, Bi);
+    double2 *f = X.fb6 + (size_t)c * 6 * nw + i;
+#pragma unroll
+    for (int a = 0; a < 6; a++) f[(size_t)a * nw] = make_double2(Br[a], Bi[a]);
+}
+
+// DOF -> position on the support of the frequency-dependent terms (-1 off it), built once per CTA in shared memory
+__device__ __forceinline__ void gen_fd_map(const GenDev &D, const GenFdDev &X, int *fdpos, int tid, int nthr)
+{
+    for (int t = tid; t < D.n; t += nthr) fdpos[t] = -1;
+    __syncthreads();
+    for (int t = tid; t < X.n_fd; t += nthr) fdpos[X.fd_idx[t]] = t;
+    __syncthreads();
+}
+
+// impedance entry t = a n + b at frequency i (raft_model.py:1086).  On the support: M + A_w and (B + B_w) + B_drag with the
+// rigid solver's grouping (raftk_fused.cuh); elsewhere the constant-matrix expression.  FD = false (n_fd = 0) is the
+// constant-matrix kernel as it was, instruction for instruction: no map, no branch
+template <bool FD>
+__device__ __forceinline__ double2 gen_impedance(const GenDev &D, const GenFdDev &X, const int *fdpos, const double *Bd, int t, int i, double w,
+                                                 double w2)
+{
+    if constexpr (FD) {
+        const int pa = fdpos[t / D.n], pb = fdpos[t % D.n];
+        if (pa >= 0 && pb >= 0) {
+            const size_t e = ((size_t)pa * X.n_fd + pb) * D.nw + i;
+            const double M = D.M[t] + X.A_w[e], B = (D.B[t] + X.B_w[e]) + Bd[t];
+            return make_double2(fma(-w2, M, D.C[t]), w * B);
+        }
+    }
+    return make_double2(fma(-w2, D.M[t], D.C[t]), w * (D.B[t] + Bd[t]));
 }
 
 // k_gen_node_pass: grid (Ns, nC), block 128: RMS of the relative velocity components over w (raft_member.py:2071-2090),
@@ -245,20 +310,23 @@ __global__ void __launch_bounds__(128) k_gen_bdrag(GenDev D, GenWork W)
 
 // k_gen_solve: grid (nw, nC), block 256.  Augmented system [Z | F] (n x (n+1)) in global memory (L2-resident), right-looking
 // LU with partial pivoting on |re| + |im| (LAPACK izamax), back substitution; writes Xi and the convergence verdict.
-__global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 *Xi, double tol)
+template <bool FD>
+__global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 *Xi, double tol, GenFdDev X)
 {
     __shared__ double pv[8];
     __shared__ int pi_[8];
     __shared__ double2 piv;
     __shared__ int prow, bad;
+    __shared__ int fdpos[FD ? 256 : 1];
     const int i = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, n = D.n, nw = D.nw, nc = n + 1;
     if (W.flags[4 * c]) return;
     double2 *A = W.Z + ((size_t)c * nw + i) * (size_t)n * nc;
     const double w = D.w[i], w2 = w * w;
     const double *Bd = W.B_drag + (size_t)c * n * n;
+    if constexpr (FD) gen_fd_map(D, X, fdpos, tid, 256);
     for (int t = tid; t < n * n; t += 256) {
         const int a = t / n, b = t % n;
-        A[(size_t)a * nc + b] = make_double2(fma(-w2, D.M[t], D.C[t]), w * (D.B[t] + Bd[t]));       // raft_model.py:1086
+        A[(size_t)a * nc + b] = gen_impedance<FD>(D, X, fdpos, Bd, t, i, w, w2);
     }
     for (int a = tid; a < n; a += 256) {
         const double2 f1 = W.F_iner[((size_t)c * n + a) * nw + i], f2 = W.F_drag[((size_t)c * n + a) * nw + i];
@@ -343,13 +411,15 @@ __global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 
 //   9 Mflop per 150 x 150 system then run from registers and shared memory.
 #define GB 8
 #define GT 128
-__global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W, double2 *Xi, double tol)
+template <bool FD>
+__global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W, double2 *Xi, double tol, GenFdDev X)
 {
     extern __shared__ __align__(16) double smem_raw[];
     __shared__ double pv[GT / 32];
     __shared__ int pi_[GT / 32];
     __shared__ int bad;
     __shared__ int pivrow[GB];
+    __shared__ int fdpos[FD ? 256 : 1];
     const int i = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, n = D.n, nw = D.nw, nc = n + 1;
     if (W.flags[4 * c]) return;
     double2 *P = reinterpret_cast<double2 *>(smem_raw);          // panel  [n][GB]   (rows kb.. stored from 0)
@@ -357,9 +427,10 @@ __global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W
     double2 *A = W.Z + ((size_t)c * nw + i) * (size_t)n * nc;
     const double w = D.w[i], w2 = w * w;
     const double *Bd = W.B_drag + (size_t)c * n * n;
+    if constexpr (FD) gen_fd_map(D, X, fdpos, tid, GT);
     for (int t = tid; t < n * n; t += GT) {
         const int a = t / n, b = t % n;
-        A[(size_t)a * nc + b] = make_double2(fma(-w2, D.M[t], D.C[t]), w * (D.B[t] + Bd[t]));       // raft_model.py:1086
+        A[(size_t)a * nc + b] = gen_impedance<FD>(D, X, fdpos, Bd, t, i, w, w2);
     }
     for (int a = tid; a < n; a += GT) {
         const double2 f1 = W.F_iner[((size_t)c * n + a) * nw + i], f2 = W.F_drag[((size_t)c * n + a) * nw + i];

@@ -66,15 +66,14 @@ __device__ __forceinline__ double sea_state_zeta(const CasesDev &Cs, int c, int 
     return sqrt(2.0 * sea_state_S(Cs, c, i, nw, w, dw) * dw);
 }
 
-// BEM excitation of design d at frequency i for heading beta: bracket the heading in the (heading-relative)
-// coefficient table with wrap-around, interpolate, rotate back to the global frame, scale by the wave amplitude
-// and the array phase offset (raft_fowt.py:1796-1849).  Br/Bi receive the 6 complex force components.
-__device__ __forceinline__ void bem_excitation(const DesignsDev &D, int d, int i, double k, double beta, double sb, double cb,
-                                               double zeta, double (&Br)[6], double (&Bi)[6])
+// BEM excitation at frequency i for heading beta from one heading-relative coefficient table X [nhs][6][nw] on headings hd:
+// bracket the heading with wrap-around, interpolate, rotate back to the global frame, scale by the wave amplitude and the
+// array phase offset of (xr, yr) (raft_fowt.py:1796-1849).  Br/Bi receive the 6 complex force components (full DOFs 0-5).
+// Shared by the rigid solvers (bem_excitation below) and the generalised-DOF solve (k_gen_bem).
+__device__ __forceinline__ void bem_excitation_table(const double *hd, int nhs, const double2 *X, int nw, double xr, double yr,
+                                                     double hadj, int i, double k, double beta, double sb, double cb, double zeta,
+                                                     double (&Br)[6], double (&Bi)[6])
 {
-    const int nhs = D.n_bem_head, nw = D.nw;
-    const double *hd = D.bem_headings;
-    const double xr = D.bem_xyh[3 * d], yr = D.bem_xyh[3 * d + 1], hadj = D.bem_xyh[3 * d + 2];
     double bdeg = fmod(beta * (180.0 / CUDART_PI) - hadj, 360.0);
     if (bdeg < 0) bdeg += 360.0;                                   // python's % is non-negative
     int i1 = 0, i2 = 0; double f2 = 0;
@@ -88,7 +87,6 @@ __device__ __forceinline__ void bem_excitation(const DesignsDev &D, int d, int i
         for (int t = 0; t < nhs - 1; t++) if (hd[t + 1] > bdeg) { i1 = t; i2 = t + 1; f2 = (bdeg - hd[t]) / (hd[t + 1] - hd[t]); break; }
     }
     const double f1 = 1.0 - f2;
-    const double2 *X = reinterpret_cast<const double2 *>(D.X_BEM) + (size_t)d * nhs * 6 * nw;
     double Xr[6], Xi_[6];
 #pragma unroll
     for (int a = 0; a < 6; a++) {
@@ -107,6 +105,15 @@ __device__ __forceinline__ void bem_excitation(const DesignsDev &D, int d, int i
     const double pr = zeta * cp, pi = zeta * sp;
 #pragma unroll
     for (int a = 0; a < 6; a++) { Br[a] = Rr[a] * pr - Ri[a] * pi; Bi[a] = Rr[a] * pi + Ri[a] * pr; }
+}
+
+// BEM excitation of design d of a rigid batch: its table, headings and (x_ref, y_ref, heading_adjust)
+__device__ __forceinline__ void bem_excitation(const DesignsDev &D, int d, int i, double k, double beta, double sb, double cb,
+                                               double zeta, double (&Br)[6], double (&Bi)[6])
+{
+    const int nhs = D.n_bem_head, nw = D.nw;
+    bem_excitation_table(D.bem_headings, nhs, reinterpret_cast<const double2 *>(D.X_BEM) + (size_t)d * nhs * 6 * nw, nw,
+                         D.bem_xyh[3 * d], D.bem_xyh[3 * d + 1], D.bem_xyh[3 * d + 2], i, k, beta, sb, cb, zeta, Br, Bi);
 }
 
 struct ExcOut { double2 *F_iner, *F_BEM; double *zeta; };

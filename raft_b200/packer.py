@@ -216,22 +216,66 @@ def pack_general_dofs(fowt):
     members, nDOF > 6; raft_fowt.py:1854-1857, 1913-1929).  GROUNDWORK for the next row: so far only the CPU checker
     of the tests consumes these tables -- the CUDA path is rigid 6-DOF and ``pack_fowt`` keeps rejecting flexible members.
     Adds ``gen_nDOF``, ``gen_Tn`` [Ns,6,nDOF] (T rows of each strip node's structural node) and ``gen_rr`` [Ns,3]
-    (offset from that node; zero on flexible members, whose strip nodes are their structural nodes)."""
+    (offset from that node; zero on flexible members, whose strip nodes are their structural nodes).
+    The nodes of potential-flow members (potMod) carry no strip-theory inertial excitation (raft_member.py:1980): their
+    ``node_a_i`` is zero, like their Imat, and their wave force comes from the BEM table (``pack_general_matrices``)."""
     out = pack_members(fowt, allow_flexible=True)
     T = np.asarray(fowt.T, dtype=float)
-    Tn, rr = [], []
+    Tn, rr, pot = [], [], []
     for mem in fowt.memberList:
         sub = np.where(mem.r[:, 2] < 0)[0]
         for il in sub:
             node = mem.nodeList[0] if getattr(mem, "type", "rigid") == "rigid" else mem.nodeList[il]
             Tn.append(T[node.id * 6:(node.id + 1) * 6, :])
             rr.append(np.asarray(mem.r[il], dtype=float) - np.asarray(node.r[:3], dtype=float))
+            pot.append(bool(getattr(mem, "potMod", False)))
     ns = len(out["node_ls"])
+    if any(pot):
+        out["node_a_i"] = np.where(np.array(pot), 0.0, out["node_a_i"])
     out.update(gen_nDOF=np.int32(T.shape[1]), gen_Tn=np.array(Tn, dtype=float).reshape(ns, 6, T.shape[1]),
                gen_rr=np.array(rr, dtype=float).reshape(ns, 3), w=np.array(fowt.w, dtype=float), k=np.array(fowt.k, dtype=float),
                depth=np.float64(fowt.depth), dw=np.float64(fowt.w[1] - fowt.w[0]),
                M0=np.zeros([6, 6]), B0=np.zeros([6, 6]), C0=np.zeros([6, 6]))
     return out
+
+
+def pack_general_matrices(fowt):
+    """System matrices of a FOWT with generalised degrees of freedom (raft_model.py:1045-1047), split into the constant part
+    and the frequency-dependent part the solver adds on its support (C ABI ``raftk_general_fd``).  Duck-typed on a live FOWT.
+
+    Returns dict(M, B, C [nDOF,nDOF], fd):
+      M = M_struc + A_hydro_morison;  B = B_struc + sum B_gyro;  C = C_struc + C_hydro + C_moor + C_elast
+      fd: ``fd_idx`` [n_fd] int32, the reduced DOFs whose rows or columns of sum A_aero + A_BEM or sum B_aero + B_BEM are
+      nonzero (the rotor nodes' DOFs and DOFs 0-5, where readHydro lumps the BEM coefficients; raft_fowt.py:1479-1480,
+      1557-1562); ``A_w``, ``B_w`` [n_fd,n_fd,nw] those sums restricted to it (every entry outside it is exactly zero);
+      ``pack_bem_excitation``'s table (``X_BEM`` [nhead,6,nw] in full DOFs 0-5, ``bem_headings``, ``heading_adjust``) or
+      none; ``T0`` [6,nDOF] = rows 0-5 of ``fowt.T`` (F_BEM = T^T F_BEM_fullDOF, raft_fowt.py:1885-1887); ``x_ref``, ``y_ref``.
+    A FOWT without operating rotors and without BEM coefficients gets n_fd = 0."""
+    n, nw = int(fowt.nDOF), len(fowt.w)
+    M = np.array(fowt.M_struc, dtype=float) + np.array(fowt.A_hydro_morison, dtype=float)
+    B = np.array(fowt.B_struc, dtype=float)
+    B_gyro = getattr(fowt, "B_gyro", None)
+    if B_gyro is not None and np.size(B_gyro):
+        B = B + np.sum(B_gyro, axis=2)
+    C = (np.array(fowt.C_struc, dtype=float) + np.array(fowt.C_hydro, dtype=float)
+         + np.array(fowt.C_moor, dtype=float) + np.array(fowt.C_elast, dtype=float))
+    A_w, B_w = np.zeros([n, n, nw]), np.zeros([n, n, nw])
+    if getattr(fowt, "nrotors", 0) > 0:
+        A_w = A_w + np.sum(fowt.A_aero, axis=3)
+        B_w = B_w + np.sum(fowt.B_aero, axis=3)
+    for name, acc in (("A_BEM", A_w), ("B_BEM", B_w)):
+        t = getattr(fowt, name, None)
+        if t is not None and np.size(t):
+            acc += np.asarray(t, dtype=float)
+    nz = np.any(A_w != 0, axis=2) | np.any(B_w != 0, axis=2)
+    idx = np.nonzero(nz.any(axis=0) | nz.any(axis=1))[0].astype(np.int32)
+    fd = dict(fd_idx=idx, A_w=np.ascontiguousarray(A_w[np.ix_(idx, idx)]), B_w=np.ascontiguousarray(B_w[np.ix_(idx, idx)]),
+              T0=np.ascontiguousarray(np.asarray(fowt.T, dtype=float)[:6]),
+              x_ref=np.float64(getattr(fowt, "x_ref", 0.0)), y_ref=np.float64(getattr(fowt, "y_ref", 0.0)))
+    bem = pack_bem_excitation(fowt)
+    if bem is not None:
+        fd.update(bem)
+    return dict(M=M, B=B, C=C, fd=fd)
 
 
 def pack_qtf(fowt):

@@ -14,7 +14,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import RaftkCases, RaftkDesigns, RaftkFarm, RaftkGeneral, RaftkOutputs, RaftkSlender, RaftkSolveOpts, check, lib
+from ._lib import RaftkCases, RaftkDesigns, RaftkFarm, RaftkGeneral, RaftkGeneralFd, RaftkOutputs, RaftkSlender, RaftkSolveOpts, check, lib
 
 _F8 = np.float64
 _I4 = np.int32
@@ -514,13 +514,41 @@ def _general_struct(P, M, B, Cm, ptr_of):
     return g
 
 
+def _general_fd_struct(fd, n, nw, ptr_of):
+    """raftk_general_fd for the ``fd`` dict of ``packer.pack_general_matrices`` (keys fd_idx, A_w, B_w [n_fd,n_fd,nw]; optional
+    X_BEM [nhead,6,nw], bem_headings, heading_adjust, T0 [6,nDOF]; x_ref, y_ref), or None for fd=None."""
+    if fd is None:
+        return None
+    f = RaftkGeneralFd()
+    idx = np.ascontiguousarray(fd.get("fd_idx", np.zeros(0)), dtype=_I4)
+    f.n_fd = nf = len(idx)
+    if nf:
+        A_w, B_w = (np.ascontiguousarray(fd[k], dtype=_F8) for k in ("A_w", "B_w"))
+        if A_w.shape != (nf, nf, nw) or B_w.shape != (nf, nf, nw):
+            raise ValueError("fd: A_w and B_w must be [n_fd, n_fd, nw] = [%d, %d, %d]" % (nf, nf, nw))
+        f.fd_idx, f.A_w, f.B_w = ptr_of("fd_idx", idx), ptr_of("fd_A_w", A_w), ptr_of("fd_B_w", B_w)
+    if fd.get("X_BEM") is not None:
+        hd = np.ascontiguousarray(fd["bem_headings"], dtype=_F8)
+        X = np.ascontiguousarray(fd["X_BEM"], dtype=np.complex128)
+        T0 = np.ascontiguousarray(fd["T0"], dtype=_F8)
+        if X.shape != (len(hd), 6, nw) or T0.shape != (6, n):
+            raise ValueError("fd: X_BEM must be [n_bem_head, 6, nw] and T0 [6, nDOF]")
+        f.n_bem_head = len(hd)
+        f.bem_headings, f.X_BEM, f.T0 = ptr_of("fd_bem_headings", hd), ptr_of("fd_X_BEM", X), ptr_of("fd_T0", T0)
+        f.heading_adjust = float(fd.get("heading_adjust", 0.0))
+    f.x_ref, f.y_ref = float(fd.get("x_ref", 0.0)), float(fd.get("y_ref", 0.0))
+    return f
+
+
 class GeneralSession:
     """Generalised-DOF solve with tables, workspace and outputs resident in HBM (torch tensors), kernels on torch's current
     stream: ``solve()`` enqueues raftk_general_solve_dynamics_dev -> (Xi [nT,nDOF,nw] complex, status [nT,4]); ``cases`` may
     carry wave trains (``packer.pack_case_trains``).  ``stats(R, wpow)`` reduces the device Xi to output-channel statistics
-    on the device (raftk_general_channel_stats_dev), so the responses never leave HBM."""
+    on the device (raftk_general_channel_stats_dev), so the responses never leave HBM.  ``fd``: frequency-dependent added
+    mass, damping and BEM excitation (``packer.pack_general_matrices``); with ``F_BEM=True`` ``solve()`` also returns the BEM
+    excitation in reduced DOFs, complex [nT,nDOF,nw]."""
 
-    def __init__(self, P, M, B, Cm, cases, device=None):
+    def __init__(self, P, M, B, Cm, cases, device=None, fd=None, F_BEM=False):
         import torch
         self.torch = torch
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
@@ -535,19 +563,24 @@ class GeneralSession:
             self.ct = {k: torch.from_numpy(v).to(self.device) for k, v in cases.arrays.items()}
             self.c_struct = cases.struct(lambda name: self.ct[name].data_ptr())
             n, nw, nC = int(P["gen_nDOF"]), len(P["w"]), cases.n_cases
-            self.workspace_bytes = int(lib.raftk_general_workspace_bytes(C.byref(self.g), nC))
+            self.fd = _general_fd_struct(fd, n, nw, to_dev)
+            fdp = C.byref(self.fd) if self.fd is not None else None
+            self.workspace_bytes = int(lib.raftk_general_fd_workspace_bytes(C.byref(self.g), fdp, nC))
             self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=self.device)
             self.Xi = torch.zeros([nC, n, nw], dtype=torch.complex128, device=self.device)
             self.status = torch.zeros([nC, 4], dtype=torch.int32, device=self.device)
+            self.F_BEM = torch.zeros([nC, n, nw], dtype=torch.complex128, device=self.device) if F_BEM else None
         self.n, self.nw, self.n_cases, self.dw = n, nw, nC, float(P["dw"])
         self._ch = None
 
     def solve(self, n_iter=10, tol=0.01, xi_start=0.0):
         o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
         with self.torch.cuda.device(self.device):
-            check(lib.raftk_general_solve_dynamics_dev(C.byref(self.g), C.byref(self.c_struct), C.byref(o), self.Xi.data_ptr(), self.status.data_ptr(),
-                                                       self.workspace.data_ptr(), self.workspace_bytes, self.torch.cuda.current_stream(self.device).cuda_stream))
-        return self.Xi, self.status
+            check(lib.raftk_general_solve_dynamics_fd_dev(C.byref(self.g), C.byref(self.fd) if self.fd is not None else None, C.byref(self.c_struct),
+                                                          C.byref(o), self.Xi.data_ptr(), self.status.data_ptr(),
+                                                          self.F_BEM.data_ptr() if self.F_BEM is not None else None, self.workspace.data_ptr(),
+                                                          self.workspace_bytes, self.torch.cuda.current_stream(self.device).cuda_stream))
+        return (self.Xi, self.status) if self.F_BEM is None else (self.Xi, self.status, self.F_BEM)
 
     def stats(self, R, wpow, psd=True, amp=False):
         """Output-channel statistics of the last ``solve()`` (``packer.pack_general_channels``: R [nch,nDOF], wpow [nch]) on
@@ -571,39 +604,31 @@ class GeneralSession:
         return sd, P, A
 
 
-def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0):
+def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0, fd=None, F_BEM=False):
     """Model.solveDynamics for one FOWT with generalised degrees of freedom (flexible members), host buffers:
     ``P`` from ``packer.pack_general_dofs`` (node tables + ``gen_Tn``, ``gen_rr``), constant system
     matrices ``M, B, Cm`` [nDOF,nDOF], ``cases`` a CaseTable, with wave trains when built from ``packer.pack_case_trains``
-    (train 0 of a case drives the linearisation, raft_model.py:1200-1236) -> (Xi complex [nT,nDOF,nw], status [nT,4])."""
-    n, nw, Ns = int(P["gen_nDOF"]), len(P["w"]), len(P["node_ls"])
+    (train 0 of a case drives the linearisation, raft_model.py:1200-1236) -> (Xi complex [nT,nDOF,nw], status [nT,4]).
+    ``fd``: frequency-dependent added mass and damping (operating rotors, BEM coefficients) and BEM excitation, the ``fd``
+    dict of ``packer.pack_general_matrices`` (whose M, B, C are then the constant matrices).  ``F_BEM=True`` appends the BEM
+    excitation of every case and train in reduced DOFs, complex [nT,nDOF,nw], to the result."""
+    n, nw = int(P["gen_nDOF"]), len(P["w"])
     keep = {}
-    g = RaftkGeneral()
-    g.n_dof, g.nw, g.n_nodes = n, nw, Ns
-    g.depth, g.rho, g.dw = float(P["depth"]), float(P["rho"]), float(P["dw"])
-    mem = np.asarray(P["node_mem"], dtype=np.int64)
-    frame = np.concatenate([np.asarray(P["mem_q"])[mem], np.asarray(P["mem_p1"])[mem], np.asarray(P["mem_p2"])[mem]], axis=1) if Ns else np.zeros([0, 9])
-    cd = np.stack([np.asarray(P["node_a_q"]) * np.asarray(P["node_Cd_q"]), np.asarray(P["node_a_p1"]) * np.asarray(P["node_Cd_p1"]),
-                   np.asarray(P["node_a_p2"]) * np.asarray(P["node_Cd_p2"]), np.asarray(P["node_a_End"]) * np.asarray(P["node_Cd_End"])], axis=1) if Ns else np.zeros([0, 4])
-    arrays = dict(w=P["w"], k=P["k"], node_r=P["node_r"], node_frame=frame, node_circ=np.asarray(P["mem_circ"], dtype=_I4)[mem] if Ns else np.zeros(0, dtype=_I4),
-                  node_Imat=P["node_Imat"], node_a_i=P["node_a_i"], node_cd=cd, Tn=P["gen_Tn"], rr=P["gen_rr"], M=M, B=B, C=Cm)
-    if P.get("node_Imat_w") is not None:
-        arrays["node_Imat_w"] = np.ascontiguousarray(P["node_Imat_w"], dtype=np.complex128)
-    for name in _lib.GENERAL_ARRAYS:
-        if name not in arrays:
-            setattr(g, name, None)
-            continue
-        a = arrays[name]
-        a = np.ascontiguousarray(a, dtype=_I4 if name == "node_circ" else (np.complex128 if name == "node_Imat_w" else _F8))
+
+    def ptr(name, a):
         keep[name] = a
-        setattr(g, name, a.ctypes.data)
+        return a.ctypes.data
+    g = _general_struct(P, M, B, Cm, ptr)
+    f = _general_fd_struct(fd, n, nw, ptr)
     nC = cases.n_cases
     Xi = np.zeros([nC, n, nw], dtype=np.complex128)
     st = np.zeros([nC, 4], dtype=_I4)
+    Fb = np.zeros([nC, n, nw], dtype=np.complex128) if F_BEM else None
     c = cases.struct(_host_ptr(cases.arrays))
     o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
-    check(lib.raftk_general_solve_dynamics_host(C.byref(g), C.byref(c), C.byref(o), Xi.ctypes.data, st.ctypes.data))
-    return Xi, st
+    check(lib.raftk_general_solve_dynamics_fd_host(C.byref(g), C.byref(f) if f is not None else None, C.byref(c), C.byref(o), Xi.ctypes.data,
+                                                   st.ctypes.data, Fb.ctypes.data if F_BEM else None))
+    return (Xi, st, Fb) if F_BEM else (Xi, st)
 
 
 def combine_trains(std, psd, idx):
@@ -663,14 +688,14 @@ def general_case_metrics(channels, std, psd, amp, idx):
     return m
 
 
-def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0):
+def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, fd=None):
     """Model.analyzeCases (dynamics and output statistics) for one FOWT with generalised degrees of freedom: ``cases`` a list
     of case dicts, scalar or list-valued wave keys (several wave trains); ``channels`` from ``packer.pack_general_channels``.
     -> dict(Xi_trains [per case: nTrains,nDOF,nw], status [nC,4] of train 0, case_metrics {case: saveTurbineOutputs entries},
-    empty without channels)."""
+    empty without channels).  ``fd``: frequency-dependent terms, as for ``general_solve_dynamics``."""
     from .packer import pack_case_trains
     table, owner, first = pack_case_trains(cases)
-    Xi, st = general_solve_dynamics(P, M, B, Cm, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start)
+    Xi, st = general_solve_dynamics(P, M, B, Cm, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start, fd=fd)
     raise_on_flags(st[first])                                           # raft_model.py:1089, :1098-1099
     metrics = {}
     if channels is not None:
