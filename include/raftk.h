@@ -16,7 +16,7 @@
  *     nothing: the caller owns a workspace sized by raftk_workspace_bytes().  They are
  *     asynchronous w.r.t. the host and re-entrant per stream.
  *   - *_host entry points take HOST pointers, stage through an internal device arena
- *     (grown on demand, cached per process), and are synchronous.
+ *     (one per device, grown on demand, shared by every *_host call), and are synchronous.
  *
  * Scope: rigid 6-DOF FOWTs, strip-theory members (+ optional BEM tables, + optional external QTF or slender-body QTF for
  * second-order difference-frequency forces), one wave train drives the drag linearisation (raft_fowt.py:1910); coupled

@@ -1099,261 +1099,204 @@ extern "C" int raftk_build_family_host(const raftk_family *f, raftk_family_table
 }
 
 // ---- host-pointer front ends -------------------------------------------------------------------------
-
-struct Arena {
-    char *base = nullptr; size_t cap = 0, used = 0;
-    int reserve(size_t bytes)
-    {
-        if (bytes <= cap) return 0;
-        if (base) cudaFree(base);
-        base = nullptr; cap = 0;
-        if (cudaMalloc(&base, bytes) != cudaSuccess) { cudaGetLastError(); return -1; }
-        cap = bytes;
-        return 0;
-    }
-    void *take(size_t bytes) { void *p = base + used; used += align_up(bytes, 256); return p; }
-};
+// A *_host call stages through one Staging: it declares its inputs, device-only buffers and outputs, commits once (which
+// sizes the device arena from that same list and uploads the inputs), runs its *_dev twin and finishes (downloads, one
+// synchronise).  The arena is grow-only, one per device: no cudaMalloc / cudaFree on the call path once its high-water mark
+// has been reached (SURVEY.md 8b: no hidden allocation per call).
+//
+// Small inputs (grid, member/node tables, case table: ~30 arrays of a few KB) are packed into one pinned block and sent with
+// a single copy to the head of the arena; only large arrays (frequency tables, big sweeps) are copied one by one.  This trims
+// ~100 us of per-copy launch overhead per call.
+static const size_t PIN_BYTES = (size_t)256 << 10, PIN_MAX = (size_t)64 << 10;   // a typical call packs ~30 KB
+struct Arena { char *base = nullptr; size_t cap = 0; };
 static Arena g_arena[RAFTK_MAX_DEV];       // one per device: the *_host paths run on whichever device is current
-static std::mutex g_arena_mu;
+static char *g_pin = nullptr;              // pinned, PIN_BYTES, one per process
+static std::mutex g_stage_mu;              // the arenas and the pinned block
 
-// Device scratch of the small *_host wrappers (statistics, system solve, second-order force, slender-body QTF, generalised
-// DOFs): one grow-only block per device, bump-allocated per call -- no cudaMalloc / cudaFree on the call path once the
-// high-water mark has been reached (SURVEY.md 8b: no hidden allocation per call).
-static Arena g_scratch[RAFTK_MAX_DEV];
-static std::mutex g_scratch_mu;
-struct ScratchCall {
-    std::unique_lock<std::mutex> lk;
-    Arena &A;
-    ScratchCall() : lk(g_scratch_mu), A(g_scratch[cur_dev()]) { A.used = 0; }
-    bool reserve(size_t total) { return A.reserve(total + 4096) == 0; }
-    template <class T> T *take(size_t bytes) { return static_cast<T *>(A.take(bytes)); }
-};
+class Staging {
+    struct Buf { const void *from; void *to; size_t bytes; const void **slot; size_t off; bool pinned; };
+    std::lock_guard<std::mutex> lk_;
+    const char *who_;
+    std::vector<Buf> bufs_;
+    char *base_ = nullptr;
+    bool pending_ = false;                 // copies enqueued that finish() has not waited for
+    cudaError_t e_ = cudaSuccess;
+    void note(cudaError_t r) { if (r != cudaSuccess && e_ == cudaSuccess) e_ = r; }
 
-// Small input arrays (grid, member/node tables, case table: ~30 arrays of a few KB) are gathered in one pinned
-// staging block and sent with a single copy into a reserved region at the head of the arena; only large arrays
-// (frequency tables, big sweeps) are copied one by one.  This trims ~100 us of per-copy launch overhead per call.
-static const size_t SMALL_REGION = (size_t)1 << 20, SMALL_MAX = (size_t)64 << 10;
-struct Stager {
-    char *host = nullptr;            // pinned, SMALL_REGION bytes
-    size_t used = 0;
-    bool ensure()
+public:
+    explicit Staging(const char *who) : lk_(g_stage_mu), who_(who) { bufs_.reserve(64); }
+    ~Staging() { if (pending_) cudaStreamSynchronize(0); }     // an early return: the next call reuses the pinned block
+    // n elements on the device, uploaded from `from` by commit() and downloaded to `to` by finish() when those are given;
+    // *slot receives the device address, NULL when n is 0
+    template <class T> void buf(T *&slot, size_t n, const std::remove_const_t<T> *from = nullptr, std::remove_const_t<T> *to = nullptr)
     {
-        if (host) return true;
-        if (cudaHostAlloc(&host, SMALL_REGION, cudaHostAllocPortable) != cudaSuccess) { cudaGetLastError(); host = nullptr; return false; }
-        return true;
+        bufs_.push_back({from, to, n * sizeof(T), (const void **)&slot, 0, false});
+    }
+    template <class T> void in(T *&slot, const std::remove_const_t<T> *h, size_t n) { buf(slot, h ? n : 0, h); }   // NULL h: NULL slot
+    template <class T> void out(T *&slot, size_t n, std::remove_const_t<T> *h) { buf(slot, n, nullptr, h); }      // NULL h: no download
+
+    int commit()
+    {
+        if (!g_pin && cudaHostAlloc(&g_pin, PIN_BYTES, cudaHostAllocPortable) != cudaSuccess) { cudaGetLastError(); g_pin = nullptr; }
+        size_t pin = 0;                    // the head of the arena mirrors the pinned block
+        for (Buf &b : bufs_)
+            if (b.from && b.bytes && b.bytes <= PIN_MAX && g_pin && pin + align_up(b.bytes, 256) <= PIN_BYTES) {
+                b.off = pin; b.pinned = true; pin += align_up(b.bytes, 256);
+            }
+        size_t total = pin;
+        for (Buf &b : bufs_)
+            if (!b.pinned) { b.off = total; total += align_up(b.bytes, 256); }
+        Arena &A = g_arena[cur_dev()];
+        if (total > A.cap) {
+            if (A.base) cudaFree(A.base);
+            A.base = nullptr; A.cap = 0;
+            if (cudaMalloc(&A.base, total) != cudaSuccess) { cudaGetLastError(); A.base = nullptr; return set_err(RAFTK_ENOMEM, "%s: device arena allocation failed", who_); }
+            A.cap = total;
+        }
+        base_ = A.base;
+        pending_ = true;
+        for (Buf &b : bufs_) {
+            *b.slot = b.bytes ? base_ + b.off : nullptr;
+            if (!b.from || !b.bytes) continue;
+            if (b.pinned) memcpy(g_pin + b.off, b.from, b.bytes);
+            else note(cudaMemcpyAsync(base_ + b.off, b.from, b.bytes, cudaMemcpyHostToDevice, 0));
+        }
+        if (pin) note(cudaMemcpyAsync(base_, g_pin, pin, cudaMemcpyHostToDevice, 0));
+        return e_ == cudaSuccess ? RAFTK_OK : set_err(RAFTK_ECUDA, "%s: H2D copy: %s", who_, cudaGetErrorString(e_));
+    }
+
+    int finish()
+    {
+        for (const Buf &b : bufs_)
+            if (b.to && b.bytes) note(cudaMemcpyAsync(b.to, base_ + b.off, b.bytes, cudaMemcpyDeviceToHost, 0));
+        const cudaError_t se = cudaStreamSynchronize(0);
+        pending_ = false;
+        if (se != cudaSuccess) e_ = se;
+        return e_ == cudaSuccess ? RAFTK_OK : set_err(RAFTK_ECUDA, "%s: %s", who_, cudaGetErrorString(e_));
     }
 };
-static Stager g_stage;
 
-template <class T>
-static const T *up(Arena &A, const T *h, size_t n, cudaStream_t st, cudaError_t &e)
-{
-    if (!h || n == 0) return nullptr;
-    const size_t bytes = n * sizeof(T);
-    if (bytes <= SMALL_MAX && g_stage.host && g_stage.used + align_up(bytes, 256) <= SMALL_REGION) {
-        memcpy(g_stage.host + g_stage.used, h, bytes);                 // device twin: A.base + same offset
-        const T *dptr = reinterpret_cast<const T *>(A.base + g_stage.used);
-        g_stage.used += align_up(bytes, 256);
-        return dptr;
-    }
-    T *dptr = static_cast<T *>(A.take(bytes));
-    cudaError_t r = cudaMemcpyAsync(dptr, h, bytes, cudaMemcpyHostToDevice, st);
-    if (r != cudaSuccess) e = r;
-    return dptr;
-}
-
-static cudaError_t flush_small(Arena &A, cudaStream_t st)
-{
-    if (!g_stage.host || g_stage.used == 0) return cudaSuccess;
-    return cudaMemcpyAsync(A.base, g_stage.host, g_stage.used, cudaMemcpyHostToDevice, st);
-}
-
-static size_t in_bytes(const raftk_designs *d, const raftk_cases *c)
-{
-    const size_t nD = d->n_designs, nw = d->nw, Nm = d->n_members_total, Ns = d->n_nodes_total, nC = c->n_cases;
-    size_t b = 0;
-    auto add = [&](size_t n) { b += align_up(n, 256); };
-    add(nw * 8); add(nw * 8); add((nD + 1) * 4); add(Nm * 72); add(Nm * 24); add(Nm * 24); add((Nm + 1) * 4); add(Nm * 4);
-    for (int t = 0; t < 8; t++) add(Ns * 8);
-    if (d->node_in_p1_w) { add(Ns * nw * 16); add(Ns * nw * 16); }
-    add(nD * 288); add(nD * 288); add(nD * 288);
-    if (d->A_w) add(nD * 36 * nw * 8);
-    if (d->B_w) add(nD * 36 * nw * 8);
-    if (d->n_bem_head > 0) { add((size_t)d->n_bem_head * 8); add(nD * d->n_bem_head * 6 * nw * 16); add(nD * 24); }
-    for (int t = 0; t < 4; t++) add(nC * 8);
-    add(nC * 4); add(nC * 4);
-    if (c->zeta) add(nC * nw * 8);
-    if (c->F_2nd) add(nD * nC * 6 * nw * 8);
-    if (c->Xi_init) add(nD * nC * 6 * nw * 16);
-    if (d->n_qtf_w > 0) {
-        add((size_t)d->n_qtf_w * 8); add((size_t)d->n_qtf_head * 8);
-        add((d->qtf_shared == 1 ? 1 : (d->qtf_shared == 2 ? nD * nC : nD)) * (size_t)d->n_qtf_w * d->n_qtf_w * d->n_qtf_head * 96);
-    }
-    return b;
-}
-
-static int host_run(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
+static int host_run(const char *who, const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
                     const double *Xi_in, int mode, const raftk_farm *farm = nullptr)
 {
     disp_reset();
     int rc = validate(d, c);
     if (rc) return rc;
     if (!out) return set_err(RAFTK_EINVAL, "null outputs");
-    std::lock_guard<std::mutex> lk(g_arena_mu);
+    Staging S(who);
     const size_t nD = d->n_designs, nw = d->nw, nC = c->n_cases, Nm = d->n_members_total, Ns = d->n_nodes_total;
-    const size_t resp = nD * nC * 6 * nw * 16;
-    size_t obytes = 0;
-    auto oadd = [&](const void *p, size_t n) { if (p) obytes += align_up(n, 256); };
-    oadd(out->Xi, resp); oadd(out->status, nD * nC * 16); oadd(out->B_drag, nD * nC * 288); oadd(out->F_drag, resp);
-    oadd(out->F_iner, resp); oadd(out->F_BEM, resp); oadd(out->zeta, nC * nw * 8); oadd(out->Xi_last, resp);
-    const bool qtf_solve = (mode == 0 && d->n_qtf_w > 0 && !c->F_2nd);   // potSecOrder 2: compute the force on the device first
-    if (qtf_solve) obytes += align_up(resp / 2, 256) + align_up(nD * nC * 48, 256);
-    if (Xi_in) obytes += align_up(resp, 256);
-    if (farm) {
-        // the system response reads the per-FOWT loads on the device: those buffers exist even when the caller does not want them back
-        obytes += 4 * align_up(resp, 256) + align_up(nD * nC * 288, 256) + align_up(nC * nw * 4, 256) + 3 * align_up(36 * nD * nD * 8, 256);
-        obytes += align_up(farm_ws_bytes(d, c, farm), 256);            // slabs of the global-memory system kernel (0 on chip)
+    const size_t nR = nD * nC * 6 * nw * 2;             // doubles of one complex [nD,nC,6,nw] array
+    raftk_designs dd = *d;
+    S.in(dd.w, d->w, nw); S.in(dd.k, d->k, nw);
+    S.in(dd.member_offset, d->member_offset, nD + 1);
+    S.in(dd.mem_frame, d->mem_frame, Nm * 9); S.in(dd.mem_rA, d->mem_rA, Nm * 3); S.in(dd.mem_arm, d->mem_arm, Nm * 3);
+    S.in(dd.mem_node_start, d->mem_node_start, Nm + 1); S.in(dd.mem_circ, d->mem_circ, Nm);
+    S.in(dd.node_ls, d->node_ls, Ns); S.in(dd.node_cd_q, d->node_cd_q, Ns);
+    S.in(dd.node_cd_p1, d->node_cd_p1, Ns); S.in(dd.node_cd_p2, d->node_cd_p2, Ns);
+    S.in(dd.node_in_q, d->node_in_q, Ns); S.in(dd.node_in_p1, d->node_in_p1, Ns);
+    S.in(dd.node_in_p2, d->node_in_p2, Ns); S.in(dd.node_pa, d->node_pa, Ns);
+    S.in(dd.node_in_p1_w, d->node_in_p1_w, Ns * nw * 2); S.in(dd.node_in_p2_w, d->node_in_p2_w, Ns * nw * 2);
+    S.in(dd.M0, d->M0, nD * 36); S.in(dd.B0, d->B0, nD * 36); S.in(dd.C0, d->C0, nD * 36);
+    S.in(dd.A_w, d->A_w, nD * 36 * nw); S.in(dd.B_w, d->B_w, nD * 36 * nw);
+    if (d->n_bem_head > 0) {
+        S.in(dd.bem_headings, d->bem_headings, (size_t)d->n_bem_head);
+        S.in(dd.X_BEM, d->X_BEM, nD * d->n_bem_head * 6 * nw * 2);
+        S.in(dd.bem_xyh, d->bem_xyh, nD * 3);
+    }
+    raftk_cases cc = *c;
+    S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
+    S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC);
+    S.in(cc.zeta, c->zeta, nC * nw);
+    S.in(cc.primary, c->primary, nC);
+    S.in(cc.F_2nd, c->F_2nd, nR / 2);
+    S.in(cc.Xi_init, c->Xi_init, nR);
+    if (d->n_qtf_w > 0) {
+        S.in(dd.qtf_w, d->qtf_w, (size_t)d->n_qtf_w);
+        S.in(dd.qtf_heads, d->qtf_heads, (size_t)d->n_qtf_head);
+        S.in(dd.qtf, d->qtf, (d->qtf_shared == 1 ? 1 : (d->qtf_shared == 2 ? nD * nC : nD)) * (size_t)d->n_qtf_w * d->n_qtf_w * d->n_qtf_head * 12);
+    }
+    const double *Xi_in_d = nullptr;
+    S.in(Xi_in_d, Xi_in, nR);
+    raftk_farm fd;
+    memset(&fd, 0, sizeof(fd));
+    if (farm) {                                           // array-level matrices: staged with the other small inputs
+        fd = *farm;
+        S.in(fd.M_arr, farm->M_arr, 36 * nD * nD); S.in(fd.B_arr, farm->B_arr, 36 * nD * nD); S.in(fd.C_arr, farm->C_arr, 36 * nD * nD);
     }
     // the solve is planned once, at the caller's cluster size, and launched with the workspace that plan needs; excitation
     // and linearisation need the whole batch's tables in one chunk
     const SolvePlan pl = mode == 0 ? plan_solve(d, (int)nC, o->cluster_size, WS_UNBOUNDED) : SolvePlan{};
     const size_t wb = mode == 0 ? pl.bytes : chunk_bytes((int)nD, (int)nC, d->max_nodes, (int)nw);
-    const size_t total = SMALL_REGION + in_bytes(d, c) + obytes + align_up(wb, 256) + 4096;
-    Arena &A = g_arena[cur_dev()];
-    if (A.reserve(total)) return set_err(RAFTK_ENOMEM, "device arena allocation failed");
-    A.used = SMALL_REGION;                   // [0, SMALL_REGION) mirrors the pinned staging block
-    g_stage.ensure();
-    g_stage.used = 0;
-    cudaStream_t st = 0;
-    cudaError_t e = cudaSuccess;
-    raftk_designs dd = *d;
-    dd.w = up(A, d->w, nw, st, e); dd.k = up(A, d->k, nw, st, e);
-    dd.member_offset = up(A, d->member_offset, nD + 1, st, e);
-    dd.mem_frame = up(A, d->mem_frame, Nm * 9, st, e); dd.mem_rA = up(A, d->mem_rA, Nm * 3, st, e);
-    dd.mem_arm = up(A, d->mem_arm, Nm * 3, st, e);
-    dd.mem_node_start = up(A, d->mem_node_start, Nm + 1, st, e); dd.mem_circ = up(A, d->mem_circ, Nm, st, e);
-    dd.node_ls = up(A, d->node_ls, Ns, st, e); dd.node_cd_q = up(A, d->node_cd_q, Ns, st, e);
-    dd.node_cd_p1 = up(A, d->node_cd_p1, Ns, st, e); dd.node_cd_p2 = up(A, d->node_cd_p2, Ns, st, e);
-    dd.node_in_q = up(A, d->node_in_q, Ns, st, e); dd.node_in_p1 = up(A, d->node_in_p1, Ns, st, e);
-    dd.node_in_p2 = up(A, d->node_in_p2, Ns, st, e); dd.node_pa = up(A, d->node_pa, Ns, st, e);
-    dd.node_in_p1_w = up(A, d->node_in_p1_w, d->node_in_p1_w ? Ns * nw * 2 : 0, st, e);
-    dd.node_in_p2_w = up(A, d->node_in_p2_w, d->node_in_p2_w ? Ns * nw * 2 : 0, st, e);
-    dd.M0 = up(A, d->M0, nD * 36, st, e); dd.B0 = up(A, d->B0, nD * 36, st, e); dd.C0 = up(A, d->C0, nD * 36, st, e);
-    dd.A_w = up(A, d->A_w, nD * 36 * nw, st, e); dd.B_w = up(A, d->B_w, nD * 36 * nw, st, e);
-    if (d->n_bem_head > 0) {
-        dd.bem_headings = up(A, d->bem_headings, (size_t)d->n_bem_head, st, e);
-        dd.X_BEM = up(A, d->X_BEM, nD * d->n_bem_head * 6 * nw * 2, st, e);
-        dd.bem_xyh = up(A, d->bem_xyh, nD * 3, st, e);
-    }
-    raftk_cases cc = *c;
-    cc.Hs = up(A, c->Hs, nC, st, e); cc.Tp = up(A, c->Tp, nC, st, e); cc.gamma = up(A, c->gamma, nC, st, e);
-    cc.beta_deg = up(A, c->beta_deg, nC, st, e); cc.spec = up(A, c->spec, nC, st, e);
-    cc.zeta = up(A, c->zeta, nC * nw, st, e);
-    cc.primary = up(A, c->primary, c->primary ? nC : 0, st, e);
-    cc.F_2nd = up(A, c->F_2nd, c->F_2nd ? nD * nC * 6 * nw : 0, st, e);
-    cc.Xi_init = up(A, c->Xi_init, c->Xi_init ? nD * nC * 6 * nw * 2 : 0, st, e);
-    if (d->n_qtf_w > 0) {
-        dd.qtf_w = up(A, d->qtf_w, (size_t)d->n_qtf_w, st, e);
-        dd.qtf_heads = up(A, d->qtf_heads, (size_t)d->n_qtf_head, st, e);
-        dd.qtf = up(A, d->qtf, (d->qtf_shared == 1 ? 1 : (d->qtf_shared == 2 ? nD * nC : nD)) * (size_t)d->n_qtf_w * d->n_qtf_w * d->n_qtf_head * 12, st, e);
-    }
-    const double *Xi_in_d = up(A, Xi_in, Xi_in ? nD * nC * 6 * nw * 2 : 0, st, e);
-    raftk_farm fd;
-    memset(&fd, 0, sizeof(fd));
-    if (farm) {                                           // array-level matrices: staged with the other small inputs
-        fd = *farm;
-        const size_t nn = 36 * nD * nD;
-        fd.M_arr = up(A, farm->M_arr, farm->M_arr ? nn : 0, st, e);
-        fd.B_arr = up(A, farm->B_arr, farm->B_arr ? nn : 0, st, e);
-        fd.C_arr = up(A, farm->C_arr, farm->C_arr ? nn : 0, st, e);
-    }
-    {
-        cudaError_t r = flush_small(A, st);
-        if (r != cudaSuccess) e = r;
-    }
-    if (e != cudaSuccess) return set_err(RAFTK_ECUDA, "H2D copy: %s", cudaGetErrorString(e));
-    raftk_outputs od;
-    memset(&od, 0, sizeof(od));
-    if (out->Xi) od.Xi = static_cast<double *>(A.take(resp));
-    if (out->status) od.status = static_cast<int32_t *>(A.take(nD * nC * 16));
-    if (out->B_drag || farm) od.B_drag = static_cast<double *>(A.take(nD * nC * 288));
-    if (out->F_drag || farm) od.F_drag = static_cast<double *>(A.take(resp));
-    if (out->F_iner || farm) od.F_iner = static_cast<double *>(A.take(resp));
-    if (out->F_BEM || (farm && d->n_bem_head > 0)) od.F_BEM = static_cast<double *>(A.take(resp));
-    if (out->zeta) od.zeta = static_cast<double *>(A.take(nC * nw * 8));
-    if (out->Xi_last) od.Xi_last = static_cast<double *>(A.take(resp));
-    if (qtf_solve) {
-        od.F_2nd = static_cast<double *>(A.take(resp / 2));
-        od.F_2nd_mean = static_cast<double *>(A.take(nD * nC * 48));
-        rc = run_qtf(&dd, &cc, od.F_2nd, od.F_2nd_mean, st);
-        if (rc) return rc;
-        cc.F_2nd = od.F_2nd;
-    }
-    void *ws = A.take(wb);
     // Page-locked output buffers (raftk_host_alloc / cudaHostAlloc / cudaHostRegister): the solve kernel stores every finished
     // unit's Xi and status word straight into host memory through the unified address space -- the same epilogue that feeds
     // peer GPUs, with the host as the "peer" -- so the device-to-host transfer overlaps the units still iterating instead of
     // following the kernel as a separate copy.  RAFTK_NO_DIRECT_D2H=1 keeps the copy (A/B).
-    bool direct_xi = false;
-    raftk_peers hostpeer;
+    double *xi_direct = nullptr;
+    int32_t *st_direct = nullptr;
     if (mode == 0 && out->Xi && !getenv("RAFTK_NO_DIRECT_D2H")) {
-        const bool fused = pl.kind != SOLVE_V1;
         cudaPointerAttributes pa;
         const bool pinned_xi = cudaPointerGetAttributes(&pa, out->Xi) == cudaSuccess && pa.type == cudaMemoryTypeHost && pa.devicePointer != nullptr;
         if (!pinned_xi) cudaGetLastError();
-        if (fused && pinned_xi) {
-            memset(&hostpeer, 0, sizeof(hostpeer));
-            hostpeer.n_ranks = 2; hostpeer.rank = 0; hostpeer.epoch = 1; hostpeer.block_elems = resp / 16;
-            hostpeer.gathered[0] = od.Xi;
-            hostpeer.gathered[1] = static_cast<double *>(pa.devicePointer) - 0;          // block of "rank 0" inside the host array = its start
+        if (pl.kind != SOLVE_V1 && pinned_xi) {
+            xi_direct = static_cast<double *>(pa.devicePointer);          // block of "rank 0" inside the host array = its start
             cudaPointerAttributes ps;
             if (out->status && cudaPointerGetAttributes(&ps, out->status) == cudaSuccess && ps.type == cudaMemoryTypeHost && ps.devicePointer)
-                hostpeer.status[1] = static_cast<int32_t *>(ps.devicePointer);
+                st_direct = static_cast<int32_t *>(ps.devicePointer);
             else cudaGetLastError();
-            direct_xi = true;
         }
     }
-    if (mode == 0) rc = launch_solve(&dd, &cc, o, &od, pl, ws, wb, st, direct_xi ? &hostpeer : nullptr);
+    raftk_outputs od;
+    memset(&od, 0, sizeof(od));
+    S.out(od.Xi, out->Xi ? nR : 0, xi_direct ? nullptr : out->Xi);
+    S.out(od.status, out->status ? nD * nC * 4 : 0, st_direct ? nullptr : out->status);
+    // the system response reads the per-FOWT loads on the device: those buffers exist even when the caller does not want them back
+    S.out(od.B_drag, out->B_drag || farm ? nD * nC * 36 : 0, out->B_drag);
+    S.out(od.F_drag, out->F_drag || farm ? nR : 0, out->F_drag);
+    S.out(od.F_iner, out->F_iner || farm ? nR : 0, out->F_iner);
+    S.out(od.F_BEM, out->F_BEM || (farm && d->n_bem_head > 0) ? nR : 0, out->F_BEM);
+    S.out(od.zeta, out->zeta ? nC * nw : 0, out->zeta);
+    const bool qtf_solve = (mode == 0 && d->n_qtf_w > 0 && !c->F_2nd);   // potSecOrder 2: compute the force on the device first
+    if (qtf_solve) { S.out(od.F_2nd, nR / 2, out->F_2nd); S.out(od.F_2nd_mean, nD * nC * 6, out->F_2nd_mean); }
+    S.out(od.Xi_last, out->Xi_last ? nR : 0, out->Xi_last);
+    char *ws, *fws = nullptr;
+    S.buf(ws, wb);
+    const size_t fwb = farm ? farm_ws_bytes(d, c, farm) : 0;                  // slabs of the global-memory system kernel (0 on chip)
+    if (farm) { S.out(fd.Xi_sys, nR, farm->Xi_sys); S.out(fd.info, farm->info ? nC * nw : 0, farm->info); S.buf(fws, fwb); }
+    if ((rc = S.commit())) return rc;
+    if (qtf_solve) {
+        if ((rc = run_qtf(&dd, &cc, od.F_2nd, od.F_2nd_mean, 0))) return rc;
+        cc.F_2nd = od.F_2nd;
+    }
+    raftk_peers hostpeer;
+    if (xi_direct) {
+        memset(&hostpeer, 0, sizeof(hostpeer));
+        hostpeer.n_ranks = 2; hostpeer.rank = 0; hostpeer.epoch = 1; hostpeer.block_elems = nR / 2;
+        hostpeer.gathered[0] = od.Xi; hostpeer.gathered[1] = xi_direct; hostpeer.status[1] = st_direct;
+    }
+    if (mode == 0) rc = launch_solve(&dd, &cc, o, &od, pl, ws, wb, 0, xi_direct ? &hostpeer : nullptr);
     else {
-        rc = tables(&dd, &cc, nullptr, &od, 2, ws, wb, st);
-        if (!rc && mode == 1) rc = tables(&dd, &cc, Xi_in_d, &od, 1, ws, wb, st);
+        rc = tables(&dd, &cc, nullptr, &od, 2, ws, wb, 0);
+        if (!rc && mode == 1) rc = tables(&dd, &cc, Xi_in_d, &od, 1, ws, wb, 0);
     }
     if (rc) return rc;
-    if (farm) {
-        fd.Xi_sys = static_cast<double *>(A.take(resp));
-        fd.info = farm->info ? static_cast<int32_t *>(A.take(nC * nw * 4)) : nullptr;
-        const size_t fwb = farm_ws_bytes(d, c, farm);
-        rc = farm_launch(&dd, &cc, &od, &fd, fwb ? A.take(fwb) : nullptr, fwb, st);
-        if (rc) return rc;
-    }
-    auto down = [&](void *h, const void *dv, size_t n) { if (h && dv) { cudaError_t r = cudaMemcpyAsync(h, dv, n, cudaMemcpyDeviceToHost, st); if (r != cudaSuccess) e = r; } };
-    if (!direct_xi) down(out->Xi, od.Xi, resp);
-    if (!(direct_xi && hostpeer.status[1])) down(out->status, od.status, nD * nC * 16);
-    down(out->B_drag, od.B_drag, nD * nC * 288);
-    down(out->F_drag, od.F_drag, resp); down(out->F_iner, od.F_iner, resp); down(out->F_BEM, od.F_BEM, resp);
-    down(out->zeta, od.zeta, nC * nw * 8);
-    down(out->F_2nd, od.F_2nd, resp / 2); down(out->F_2nd_mean, od.F_2nd_mean, nD * nC * 48); down(out->Xi_last, od.Xi_last, resp);
-    if (farm) { down(farm->Xi_sys, fd.Xi_sys, resp); down(farm->info, fd.info, nC * nw * 4); }
-    g_disp.direct_d2h = direct_xi;
-    cudaError_t se = cudaStreamSynchronize(st);
-    if (e != cudaSuccess || se != cudaSuccess)
-        return set_err(RAFTK_ECUDA, "kernel/D2H: %s", cudaGetErrorString(se != cudaSuccess ? se : e));
-    return RAFTK_OK;
+    if (farm && (rc = farm_launch(&dd, &cc, &od, &fd, fws, fwb, 0))) return rc;
+    g_disp.direct_d2h = xi_direct != nullptr;
+    return S.finish();
 }
 
 extern "C" int raftk_hydro_excitation_host(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *out)
 {
-    return host_run(d, c, nullptr, out, nullptr, 2);
+    return host_run("raftk_hydro_excitation_host", d, c, nullptr, out, nullptr, 2);
 }
 extern "C" int raftk_hydro_linearization_host(const raftk_designs *d, const raftk_cases *c, const double *Xi_in, const raftk_outputs *out)
 {
     if (!Xi_in) return set_err(RAFTK_EINVAL, "null Xi_in");
-    return host_run(d, c, nullptr, out, Xi_in, 1);
+    return host_run("raftk_hydro_linearization_host", d, c, nullptr, out, Xi_in, 1);
 }
 extern "C" int raftk_solve_dynamics_host(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out)
 {
     if (!out || !out->Xi || !out->status || !o) return set_err(RAFTK_EINVAL, "Xi, status and opts are required");
-    return host_run(d, c, o, out, nullptr, 0);
+    return host_run("raftk_solve_dynamics_host", d, c, o, out, nullptr, 0);
 }
 
 extern "C" int raftk_solve_dynamics_farm_host(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o,
@@ -1362,7 +1305,7 @@ extern "C" int raftk_solve_dynamics_farm_host(const raftk_designs *d, const raft
     if (!out || !out->Xi || !out->status || !o) return set_err(RAFTK_EINVAL, "Xi, status and opts are required");
     if (!f || !f->Xi_sys) return set_err(RAFTK_EINVAL, "farm.Xi_sys is required");
     if (d && f->n_fowt != d->n_designs) return set_err(RAFTK_EINVAL, "farm response: farm.n_fowt must equal designs.n_designs");
-    return host_run(d, c, o, out, nullptr, 0, f);
+    return host_run("raftk_solve_dynamics_farm_host", d, c, o, out, nullptr, 0, f);
 }
 
 extern "C" int raftk_second_order_force_host(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *out)
@@ -1371,38 +1314,19 @@ extern "C" int raftk_second_order_force_host(const raftk_designs *d, const raftk
     if (!out || !out->F_2nd) return set_err(RAFTK_EINVAL, "outputs.F_2nd is required");
     int rc = validate_qtf(d, c);
     if (rc) return rc;
-    const size_t nD = d->n_designs, nw = d->nw, nC = c->n_cases, n2 = d->n_qtf_w, nh = d->n_qtf_head;
-    const size_t qb = (d->qtf_shared == 1 ? 1 : (d->qtf_shared == 2 ? nD * nC : nD)) * n2 * n2 * nh * 96, fb = nD * nC * 6 * nw * 8, mb = nD * nC * 48;
-    // one temporary block: grid, table axes, table, case columns, (zeta), outputs
-    size_t total = 0;
-    auto take = [&](size_t n) { size_t o = total; total += align_up(n, 256); return o; };
-    const size_t o_w = take(nw * 8), o_qw = take(n2 * 8), o_qh = take(nh * 8), o_q = take(qb);
-    const size_t o_hs = take(nC * 8), o_tp = take(nC * 8), o_ga = take(nC * 8), o_be = take(nC * 8), o_sp = take(nC * 4);
-    const size_t o_ze = take(c->zeta ? nC * nw * 8 : 0), o_f = take(fb), o_m = take(mb);
-    ScratchCall sc;
-    if (!sc.reserve(total)) return set_err(RAFTK_ENOMEM, "second-order force: device scratch allocation failed");
-    char *base = sc.take<char>(total);
-    cudaError_t e = cudaSuccess;
-    auto h2d = [&](size_t off, const void *h, size_t n) { if (h && n) { cudaError_t r = cudaMemcpy(base + off, h, n, cudaMemcpyHostToDevice); if (r != cudaSuccess) e = r; } };
-    h2d(o_w, d->w, nw * 8); h2d(o_qw, d->qtf_w, n2 * 8); h2d(o_qh, d->qtf_heads, nh * 8); h2d(o_q, d->qtf, qb);
-    h2d(o_hs, c->Hs, nC * 8); h2d(o_tp, c->Tp, nC * 8); h2d(o_ga, c->gamma, nC * 8); h2d(o_be, c->beta_deg, nC * 8);
-    h2d(o_sp, c->spec, nC * 4); h2d(o_ze, c->zeta, c->zeta ? nC * nw * 8 : 0);
+    const size_t nD = d->n_designs, nw = d->nw, nC = c->n_cases, n2 = d->n_qtf_w, nh = d->n_qtf_head, nF = nD * nC * 6 * nw;
+    Staging S("raftk_second_order_force_host");
     raftk_designs dd = *d;
-    dd.w = reinterpret_cast<double *>(base + o_w); dd.qtf_w = reinterpret_cast<double *>(base + o_qw);
-    dd.qtf_heads = reinterpret_cast<double *>(base + o_qh); dd.qtf = reinterpret_cast<double *>(base + o_q);
+    S.in(dd.w, d->w, nw); S.in(dd.qtf_w, d->qtf_w, n2); S.in(dd.qtf_heads, d->qtf_heads, nh);
+    S.in(dd.qtf, d->qtf, (d->qtf_shared == 1 ? 1 : (d->qtf_shared == 2 ? nD * nC : nD)) * n2 * n2 * nh * 12);
     raftk_cases cc = *c;
-    cc.Hs = reinterpret_cast<double *>(base + o_hs); cc.Tp = reinterpret_cast<double *>(base + o_tp);
-    cc.gamma = reinterpret_cast<double *>(base + o_ga); cc.beta_deg = reinterpret_cast<double *>(base + o_be);
-    cc.spec = reinterpret_cast<int32_t *>(base + o_sp);
-    cc.zeta = c->zeta ? reinterpret_cast<double *>(base + o_ze) : nullptr;
+    S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC); S.in(cc.beta_deg, c->beta_deg, nC);
+    S.in(cc.spec, c->spec, nC); S.in(cc.zeta, c->zeta, nC * nw);
     cc.primary = nullptr; cc.F_2nd = nullptr;
-    if (e == cudaSuccess) rc = run_qtf(&dd, &cc, reinterpret_cast<double *>(base + o_f), reinterpret_cast<double *>(base + o_m), nullptr);
-    if (e == cudaSuccess && !rc) {
-        e = cudaMemcpy(out->F_2nd, base + o_f, fb, cudaMemcpyDeviceToHost);
-        if (e == cudaSuccess && out->F_2nd_mean) e = cudaMemcpy(out->F_2nd_mean, base + o_m, mb, cudaMemcpyDeviceToHost);
-    }
-    if (e != cudaSuccess) return set_err(RAFTK_ECUDA, "second-order force: %s", cudaGetErrorString(e));
-    return rc;
+    double *F2, *F2mean;
+    S.out(F2, nF, out->F_2nd); S.out(F2mean, nF / nw, out->F_2nd_mean);
+    if ((rc = S.commit()) || (rc = run_qtf(&dd, &cc, F2, F2mean, 0))) return rc;
+    return S.finish();
 }
 
 // ---- generalised degrees of freedom (flexible members) ---------------------------------------------------------------
@@ -1572,47 +1496,33 @@ extern "C" int raftk_general_solve_dynamics_fd_host(const raftk_general *g, cons
         }
     if (fd)
         if (int rc = validate_gen_fd(g, fd, fd->fd_idx, fd->bem_headings)) return rc;
-    size_t total = 0;
-    auto take = [&](size_t b) { size_t o_ = total; total += align_up(std::max<size_t>(b, 8), 256); return o_; };
-    raftk_general gg = *g; raftk_cases cc = *c;
+    Staging S("raftk_general_solve_dynamics_fd_host");
+    raftk_general gg = *g;
+    S.in(gg.w, g->w, nw); S.in(gg.k, g->k, nw);
+    S.in(gg.node_r, g->node_r, Ns * 3); S.in(gg.node_frame, g->node_frame, Ns * 9);
+    S.in(gg.node_circ, g->node_circ, Ns); S.in(gg.node_Imat, g->node_Imat, Ns * 9);
+    S.in(gg.node_Imat_w, g->node_Imat_w, Ns * 9 * nw * 2); S.in(gg.node_a_i, g->node_a_i, Ns);
+    S.in(gg.node_cd, g->node_cd, Ns * 4); S.in(gg.Tn, g->Tn, Ns * 6 * n); S.in(gg.rr, g->rr, Ns * 3);
+    S.in(gg.M, g->M, n * n); S.in(gg.B, g->B, n * n); S.in(gg.C, g->C, n * n);
+    raftk_cases cc = *c;
+    S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
+    S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC); S.in(cc.zeta, c->zeta, nC * nw);
+    S.in(cc.primary, c->primary, nC);
     raftk_general_fd ff = fd ? *fd : raftk_general_fd{};
-    struct Item { size_t off; const void *h; size_t nb; const void **slot; };
-    std::vector<Item> items;
-    auto add = [&](const void *h, size_t nb, const void **slot) { if (h) items.push_back({take(nb), h, nb, slot}); };
-    add(g->w, nw * 8, (const void **)&gg.w); add(g->k, nw * 8, (const void **)&gg.k);
-    add(g->node_r, Ns * 24, (const void **)&gg.node_r); add(g->node_frame, Ns * 72, (const void **)&gg.node_frame);
-    add(g->node_circ, Ns * 4, (const void **)&gg.node_circ); add(g->node_Imat, Ns * 72, (const void **)&gg.node_Imat);
-    add(g->node_Imat_w, Ns * 9 * nw * 16, (const void **)&gg.node_Imat_w); add(g->node_a_i, Ns * 8, (const void **)&gg.node_a_i);
-    add(g->node_cd, Ns * 32, (const void **)&gg.node_cd); add(g->Tn, Ns * 6 * n * 8, (const void **)&gg.Tn); add(g->rr, Ns * 24, (const void **)&gg.rr);
-    add(g->M, n * n * 8, (const void **)&gg.M); add(g->B, n * n * 8, (const void **)&gg.B); add(g->C, n * n * 8, (const void **)&gg.C);
-    add(c->Hs, nC * 8, (const void **)&cc.Hs); add(c->Tp, nC * 8, (const void **)&cc.Tp); add(c->gamma, nC * 8, (const void **)&cc.gamma);
-    add(c->beta_deg, nC * 8, (const void **)&cc.beta_deg); add(c->spec, nC * 4, (const void **)&cc.spec); add(c->zeta, nC * nw * 8, (const void **)&cc.zeta);
-    add(c->primary, nC * 4, (const void **)&cc.primary);
     if (fd) {
-        const size_t nf = std::max(fd->n_fd, 0), nh = std::max(fd->n_bem_head, 0);
-        if (nf) {
-            add(fd->fd_idx, nf * 4, (const void **)&ff.fd_idx);
-            add(fd->A_w, nf * nf * nw * 8, (const void **)&ff.A_w); add(fd->B_w, nf * nf * nw * 8, (const void **)&ff.B_w);
-        }
-        if (nh) {
-            add(fd->bem_headings, nh * 8, (const void **)&ff.bem_headings); add(fd->X_BEM, nh * 6 * nw * 16, (const void **)&ff.X_BEM);
-            add(fd->T0, 6 * n * 8, (const void **)&ff.T0);
-        }
+        const size_t nf = fd->n_fd, nh = fd->n_bem_head;             // validate_gen_fd: both >= 0
+        S.in(ff.fd_idx, fd->fd_idx, nf); S.in(ff.A_w, fd->A_w, nf * nf * nw); S.in(ff.B_w, fd->B_w, nf * nf * nw);
+        S.in(ff.bem_headings, fd->bem_headings, nh); S.in(ff.X_BEM, fd->X_BEM, nh * 6 * nw * 2); S.in(ff.T0, fd->T0, nh ? 6 * n : 0);
     }
-    const size_t o_xi = take(nC * n * nw * 16), o_st = take(nC * 16), o_fb = F_BEM ? take(nC * n * nw * 16) : 0;
-    const size_t wb = raftk_general_fd_workspace_bytes(g, fd, (int32_t)nC), o_ws = take(wb);
-    ScratchCall sc;
-    if (!sc.reserve(total)) return set_err(RAFTK_ENOMEM, "general solve: device scratch allocation failed");
-    char *base = sc.take<char>(total);
-    for (auto &it : items) { CUDA_TRY(cudaMemcpy(base + it.off, it.h, it.nb, cudaMemcpyHostToDevice)); *it.slot = base + it.off; }
-    int rc = raftk_general_solve_dynamics_fd_dev(&gg, fd ? &ff : nullptr, &cc, o, reinterpret_cast<double *>(base + o_xi),
-                                                 reinterpret_cast<int32_t *>(base + o_st), F_BEM ? reinterpret_cast<double *>(base + o_fb) : nullptr,
-                                                 base + o_ws, wb, nullptr);
-    if (rc) return rc;
-    CUDA_TRY(cudaMemcpy(Xi, base + o_xi, nC * n * nw * 16, cudaMemcpyDeviceToHost));
-    CUDA_TRY(cudaMemcpy(status, base + o_st, nC * 16, cudaMemcpyDeviceToHost));
-    if (F_BEM) CUDA_TRY(cudaMemcpy(F_BEM, base + o_fb, nC * n * nw * 16, cudaMemcpyDeviceToHost));
-    return RAFTK_OK;
+    double *dXi, *dF_BEM;
+    int32_t *dStatus;
+    char *ws;
+    const size_t wb = raftk_general_fd_workspace_bytes(g, fd, (int32_t)nC);
+    S.out(dXi, nC * n * nw * 2, Xi); S.out(dStatus, nC * 4, status); S.out(dF_BEM, F_BEM ? nC * n * nw * 2 : 0, F_BEM);
+    S.buf(ws, wb);
+    int rc = S.commit();
+    if (rc || (rc = raftk_general_solve_dynamics_fd_dev(&gg, fd ? &ff : nullptr, &cc, o, dXi, dStatus, dF_BEM, ws, wb, nullptr))) return rc;
+    return S.finish();
 }
 
 extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
@@ -1675,62 +1585,42 @@ extern "C" int raftk_qtf_slender_host(const raftk_slender *s, int32_t n_cases, c
     if (rc) return rc;
     if (!beta_rad || !Xi_rao || !qtf) return set_err(RAFTK_EINVAL, "slender-body QTF: null beta / Xi_rao / qtf");
     const size_t Nm = s->n_members, Ns = s->n_nodes, Ng = s->n_seg, nw = s->nw, nC = n_cases;
-    size_t total = 0;
-    auto take = [&](size_t n) { size_t o = total; total += align_up(std::max<size_t>(n, 8), 256); return o; };
-    struct Item { size_t off; const void *h; size_t n; const void **slot; };
+    Staging S("raftk_qtf_slender_host");
     raftk_slender dd = *s;
-    std::vector<Item> items;
-    auto add = [&](const void *h, size_t n, const void **slot) { items.push_back({take(n), h, n, slot}); };
-    add(s->w, nw * 8, (const void **)&dd.w); add(s->k, nw * 8, (const void **)&dd.k);
-    add(s->mem_q, Nm * 24, (const void **)&dd.mem_q); add(s->mem_p1, Nm * 24, (const void **)&dd.mem_p1); add(s->mem_p2, Nm * 24, (const void **)&dd.mem_p2);
-    add(s->mem_mcf, Nm * 4, (const void **)&dd.mem_mcf); add(s->mem_wl, Nm * 4, (const void **)&dd.mem_wl);
-    add(s->mem_r_int, Nm * 24, (const void **)&dd.mem_r_int); add(s->mem_a_wl, Nm * 8, (const void **)&dd.mem_a_wl);
-    add(s->mem_rwl, Nm * 24, (const void **)&dd.mem_rwl); add(s->mem_R_wl, Nm * 8, (const void **)&dd.mem_R_wl);
-    add(s->mem_node_start, (Nm + 1) * 4, (const void **)&dd.mem_node_start);
-    add(s->node_r, Ns * 24, (const void **)&dd.node_r); add(s->node_v_side, Ns * 8, (const void **)&dd.node_v_side);
-    add(s->node_Ca_p1, Ns * 8, (const void **)&dd.node_Ca_p1); add(s->node_Ca_p2, Ns * 8, (const void **)&dd.node_Ca_p2);
-    add(s->node_Ca_End, Ns * 8, (const void **)&dd.node_Ca_End); add(s->node_v_end, Ns * 8, (const void **)&dd.node_v_end);
-    add(s->node_a_i, Ns * 8, (const void **)&dd.node_a_i);
-    add(s->seg_mem, Ng * 4, (const void **)&dd.seg_mem); add(s->seg_z1, Ng * 8, (const void **)&dd.seg_z1); add(s->seg_z2, Ng * 8, (const void **)&dd.seg_z2);
-    add(s->seg_R, Ng * 8, (const void **)&dd.seg_R); add(s->seg_rmid, Ng * 24, (const void **)&dd.seg_rmid);
-    add(s->M_struc, 288, (const void **)&dd.M_struc);
-    const size_t o_beta = take(nC * 8), o_xi = take(nC * 6 * nw * 16), o_q = take(nC * nw * nw * 6 * 16);
-    const size_t wb = raftk_qtf_slender_workspace_bytes(s, n_cases), o_ws = take(wb);
-    ScratchCall sc;
-    if (!sc.reserve(total)) return set_err(RAFTK_ENOMEM, "slender-body QTF: device scratch allocation failed");
-    char *base = sc.take<char>(total);
-    cudaError_t e = cudaSuccess;
-    for (auto &it : items) {
-        if (it.h && it.n) { cudaError_t r = cudaMemcpy(base + it.off, it.h, it.n, cudaMemcpyHostToDevice); if (r != cudaSuccess) e = r; }
-        *it.slot = base + it.off;
-    }
-    if (e == cudaSuccess) e = cudaMemcpy(base + o_beta, beta_rad, nC * 8, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(base + o_xi, Xi_rao, nC * 6 * nw * 16, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-        rc = raftk_qtf_slender_dev(&dd, n_cases, reinterpret_cast<double *>(base + o_beta), reinterpret_cast<double *>(base + o_xi),
-                                   reinterpret_cast<double *>(base + o_q), base + o_ws, wb, nullptr);
-        if (!rc) e = cudaMemcpy(qtf, base + o_q, nC * nw * nw * 6 * 16, cudaMemcpyDeviceToHost);
-    }
-    if (e != cudaSuccess) return set_err(RAFTK_ECUDA, "slender-body QTF: %s", cudaGetErrorString(e));
-    return rc;
+    S.in(dd.w, s->w, nw); S.in(dd.k, s->k, nw);
+    S.in(dd.mem_q, s->mem_q, Nm * 3); S.in(dd.mem_p1, s->mem_p1, Nm * 3); S.in(dd.mem_p2, s->mem_p2, Nm * 3);
+    S.in(dd.mem_mcf, s->mem_mcf, Nm); S.in(dd.mem_wl, s->mem_wl, Nm);
+    S.in(dd.mem_r_int, s->mem_r_int, Nm * 3); S.in(dd.mem_a_wl, s->mem_a_wl, Nm);
+    S.in(dd.mem_rwl, s->mem_rwl, Nm * 3); S.in(dd.mem_R_wl, s->mem_R_wl, Nm);
+    S.in(dd.mem_node_start, s->mem_node_start, Nm + 1);
+    S.in(dd.node_r, s->node_r, Ns * 3); S.in(dd.node_v_side, s->node_v_side, Ns);
+    S.in(dd.node_Ca_p1, s->node_Ca_p1, Ns); S.in(dd.node_Ca_p2, s->node_Ca_p2, Ns);
+    S.in(dd.node_Ca_End, s->node_Ca_End, Ns); S.in(dd.node_v_end, s->node_v_end, Ns);
+    S.in(dd.node_a_i, s->node_a_i, Ns);
+    S.in(dd.seg_mem, s->seg_mem, Ng); S.in(dd.seg_z1, s->seg_z1, Ng); S.in(dd.seg_z2, s->seg_z2, Ng);
+    S.in(dd.seg_R, s->seg_R, Ng); S.in(dd.seg_rmid, s->seg_rmid, Ng * 3);
+    S.in(dd.M_struc, s->M_struc, 36);
+    const double *dBeta, *dXi;
+    double *dQ;
+    char *ws;
+    const size_t wb = raftk_qtf_slender_workspace_bytes(s, n_cases);
+    S.in(dBeta, beta_rad, nC); S.in(dXi, Xi_rao, nC * 6 * nw * 2); S.out(dQ, nC * nw * nw * 6 * 2, qtf);
+    S.buf(ws, wb);
+    if ((rc = S.commit()) || (rc = raftk_qtf_slender_dev(&dd, n_cases, dBeta, dXi, dQ, ws, wb, nullptr))) return rc;
+    return S.finish();
 }
 
 extern "C" int raftk_system_solve_host(int32_t n, int32_t nw, int32_t nrhs, double *Z, double *F, int32_t *info)
 {
     disp_reset();
     if (n <= 0 || nw <= 0 || nrhs <= 0 || !Z || !F) return set_err(RAFTK_EINVAL, "bad system-solve arguments");
-    const size_t zb = (size_t)nw * n * n * 16, fb = (size_t)nw * n * nrhs * 16, ib = (size_t)nw * 4;
-    ScratchCall sc;
-    if (!sc.reserve(align_up(zb, 256) + align_up(fb, 256) + align_up(ib, 256))) return set_err(RAFTK_ENOMEM, "system solve: device scratch allocation failed");
-    double *dZ = sc.take<double>(zb), *dF = sc.take<double>(fb);
-    int32_t *dI = sc.take<int32_t>(ib);
-    CUDA_TRY(cudaMemcpy(dZ, Z, zb, cudaMemcpyHostToDevice)); CUDA_TRY(cudaMemcpy(dF, F, fb, cudaMemcpyHostToDevice));
-    int rc = raftk_system_solve_dev(n, nw, nrhs, dZ, dF, dI, nullptr);
-    if (!rc) {
-        CUDA_TRY(cudaMemcpy(F, dF, fb, cudaMemcpyDeviceToHost));
-        if (info) CUDA_TRY(cudaMemcpy(info, dI, ib, cudaMemcpyDeviceToHost));
-    }
-    return rc;
+    Staging S("raftk_system_solve_host");
+    double *dZ, *dF;
+    int32_t *dInfo;
+    S.in(dZ, Z, (size_t)nw * n * n * 2); S.buf(dF, (size_t)nw * n * nrhs * 2, F, F); S.out(dInfo, nw, info);
+    int rc = S.commit();
+    if (rc || (rc = raftk_system_solve_dev(n, nw, nrhs, dZ, dF, dInfo, nullptr))) return rc;
+    return S.finish();
 }
 
 extern "C" int raftk_response_stats_dev(int32_t n_units, int32_t nw, double dw, int32_t rot_deg, const double *Xi,
@@ -1747,17 +1637,13 @@ extern "C" int raftk_response_stats_host(int32_t n_units, int32_t nw, double dw,
                                          double *sd, double *psd)
 {
     if (n_units <= 0 || nw <= 0 || !Xi || !sd || !(dw > 0.0)) return set_err(RAFTK_EINVAL, "bad response-stats arguments");
-    const size_t xb = (size_t)n_units * 6 * nw * 16, sb = (size_t)n_units * 6 * 8, pb = (size_t)n_units * 6 * nw * 8;
-    ScratchCall sc;
-    if (!sc.reserve(align_up(xb, 256) + align_up(sb, 256) + align_up(pb, 256))) return set_err(RAFTK_ENOMEM, "response stats: device scratch allocation failed");
-    double *dX = sc.take<double>(xb), *dS = sc.take<double>(sb), *dP = psd ? sc.take<double>(pb) : nullptr;
-    CUDA_TRY(cudaMemcpy(dX, Xi, xb, cudaMemcpyHostToDevice));
-    int rc = raftk_response_stats_dev(n_units, nw, dw, rot_deg, dX, dS, dP, nullptr);
-    if (!rc) {
-        CUDA_TRY(cudaMemcpy(sd, dS, sb, cudaMemcpyDeviceToHost));
-        if (psd) CUDA_TRY(cudaMemcpy(psd, dP, pb, cudaMemcpyDeviceToHost));
-    }
-    return rc;
+    Staging S("raftk_response_stats_host");
+    const double *dXi;
+    double *dSd, *dPsd;
+    S.in(dXi, Xi, (size_t)n_units * 6 * nw * 2); S.out(dSd, (size_t)n_units * 6, sd); S.out(dPsd, psd ? (size_t)n_units * 6 * nw : 0, psd);
+    int rc = S.commit();
+    if (rc || (rc = raftk_response_stats_dev(n_units, nw, dw, rot_deg, dXi, dSd, dPsd, nullptr))) return rc;
+    return S.finish();
 }
 
 extern "C" int raftk_channel_stats_dev(int32_t n_designs, int32_t n_cases, int32_t n_ch, int32_t nw, double dw, const double *coef,
@@ -1780,21 +1666,14 @@ extern "C" int raftk_channel_stats_host(int32_t n_designs, int32_t n_cases, int3
     if (n_designs <= 0 || n_cases <= 0 || n_ch <= 0 || nw <= 0 || !coef || !Xi || !sd || !(dw > 0.0))
         return set_err(RAFTK_EINVAL, "bad channel-stats arguments");
     const size_t rows = (size_t)n_designs * n_cases * n_ch;
-    const size_t cb = (size_t)n_designs * n_ch * 6 * nw * 16, xb = (size_t)n_designs * n_cases * 6 * nw * 16;
-    const size_t sb = rows * 8, pb = rows * nw * 8, ab = rows * nw * 16;
-    ScratchCall sc;
-    if (!sc.reserve(align_up(cb, 256) + align_up(xb, 256) + align_up(sb, 256) + align_up(pb, 256) + align_up(ab, 256)))
-        return set_err(RAFTK_ENOMEM, "channel stats: device scratch allocation failed");
-    double *dC = sc.take<double>(cb), *dX = sc.take<double>(xb), *dS = sc.take<double>(sb);
-    double *dP = psd ? sc.take<double>(pb) : nullptr, *dA = amp ? sc.take<double>(ab) : nullptr;
-    CUDA_TRY(cudaMemcpy(dC, coef, cb, cudaMemcpyHostToDevice)); CUDA_TRY(cudaMemcpy(dX, Xi, xb, cudaMemcpyHostToDevice));
-    int rc = raftk_channel_stats_dev(n_designs, n_cases, n_ch, nw, dw, dC, dX, dS, dP, dA, nullptr);
-    if (!rc) {
-        CUDA_TRY(cudaMemcpy(sd, dS, sb, cudaMemcpyDeviceToHost));
-        if (psd) CUDA_TRY(cudaMemcpy(psd, dP, pb, cudaMemcpyDeviceToHost));
-        if (amp) CUDA_TRY(cudaMemcpy(amp, dA, ab, cudaMemcpyDeviceToHost));
-    }
-    return rc;
+    Staging S("raftk_channel_stats_host");
+    const double *dCoef, *dXi;
+    double *dSd, *dPsd, *dAmp;
+    S.in(dCoef, coef, (size_t)n_designs * n_ch * 6 * nw * 2); S.in(dXi, Xi, (size_t)n_designs * n_cases * 6 * nw * 2);
+    S.out(dSd, rows, sd); S.out(dPsd, psd ? rows * nw : 0, psd); S.out(dAmp, amp ? rows * nw * 2 : 0, amp);
+    int rc = S.commit();
+    if (rc || (rc = raftk_channel_stats_dev(n_designs, n_cases, n_ch, nw, dw, dCoef, dXi, dSd, dPsd, dAmp, nullptr))) return rc;
+    return S.finish();
 }
 
 extern "C" int raftk_general_channel_stats_dev(int32_t n_units, int32_t n_dof, int32_t n_ch, int32_t nw, double dw, const double *w,
@@ -1818,24 +1697,15 @@ extern "C" int raftk_general_channel_stats_host(int32_t n_units, int32_t n_dof, 
     if (n_units <= 0 || n_dof <= 0 || n_ch <= 0 || nw <= 0 || !w || !R || !wpow || !Xi || !sd || !(dw > 0.0))
         return set_err(RAFTK_EINVAL, "bad general channel-stats arguments");
     const size_t rows = (size_t)n_units * n_ch;
-    const size_t wb = (size_t)nw * 8, rb = (size_t)n_ch * n_dof * 8, pwb = (size_t)n_ch * 4, xb = (size_t)n_units * n_dof * nw * 16;
-    const size_t sb = rows * 8, pb = rows * nw * 8, ab = rows * nw * 16;
-    ScratchCall sc;
-    if (!sc.reserve(align_up(wb, 256) + align_up(rb, 256) + align_up(pwb, 256) + align_up(xb, 256) + align_up(sb, 256) + align_up(pb, 256) + align_up(ab, 256)))
-        return set_err(RAFTK_ENOMEM, "general channel stats: device scratch allocation failed");
-    double *dw_ = sc.take<double>(wb), *dR = sc.take<double>(rb);
-    int32_t *dp = sc.take<int32_t>(pwb);
-    double *dX = sc.take<double>(xb), *dS = sc.take<double>(sb);
-    double *dP = psd ? sc.take<double>(pb) : nullptr, *dA = amp ? sc.take<double>(ab) : nullptr;
-    CUDA_TRY(cudaMemcpy(dw_, w, wb, cudaMemcpyHostToDevice)); CUDA_TRY(cudaMemcpy(dR, R, rb, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(dp, wpow, pwb, cudaMemcpyHostToDevice)); CUDA_TRY(cudaMemcpy(dX, Xi, xb, cudaMemcpyHostToDevice));
-    int rc = raftk_general_channel_stats_dev(n_units, n_dof, n_ch, nw, dw, dw_, dR, dp, dX, dS, dP, dA, nullptr);
-    if (!rc) {
-        CUDA_TRY(cudaMemcpy(sd, dS, sb, cudaMemcpyDeviceToHost));
-        if (psd) CUDA_TRY(cudaMemcpy(psd, dP, pb, cudaMemcpyDeviceToHost));
-        if (amp) CUDA_TRY(cudaMemcpy(amp, dA, ab, cudaMemcpyDeviceToHost));
-    }
-    return rc;
+    Staging S("raftk_general_channel_stats_host");
+    const double *dW, *dR, *dXi;
+    const int32_t *dWpow;
+    double *dSd, *dPsd, *dAmp;
+    S.in(dW, w, nw); S.in(dR, R, (size_t)n_ch * n_dof); S.in(dWpow, wpow, n_ch); S.in(dXi, Xi, (size_t)n_units * n_dof * nw * 2);
+    S.out(dSd, rows, sd); S.out(dPsd, psd ? rows * nw : 0, psd); S.out(dAmp, amp ? rows * nw * 2 : 0, amp);
+    int rc = S.commit();
+    if (rc || (rc = raftk_general_channel_stats_dev(n_units, n_dof, n_ch, nw, dw, dW, dR, dWpow, dXi, dSd, dPsd, dAmp, nullptr))) return rc;
+    return S.finish();
 }
 
 extern "C" void *raftk_host_alloc(size_t bytes)
