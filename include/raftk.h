@@ -332,7 +332,7 @@ int raftk_qtf_slender_host(const raftk_slender *s, int32_t n_cases, const double
  * Wave trains (cases.primary, raft_model.py:1200-1236): a secondary train runs no pass of its own; its response is solved with
  * the LU factors of its primary's last impedance and the drag excitation of its own wave kinematics with the primary's last
  * node drag coefficients.  Primaries keep the loop's final Xi.  Status rows of secondaries: 0, 1, flags, primary + 1.
- * cases.F_2nd and cases.Xi_init are rejected.  raftk_general_workspace_bytes() covers any primary map; the pivot rows kept for
+ * cases.F_2nd and cases.Xi_init are rejected (second-order loads: raftk_general_qtf below).  raftk_general_workspace_bytes() covers any primary map; the pivot rows kept for
  * the trains take n_cases * nw * n_dof * 4 bytes of it (rounded up to 256) whether or not the call has trains.
  */
 typedef struct raftk_general {
@@ -389,6 +389,41 @@ int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const raftk_gene
                                         double *Xi, int32_t *status, double *F_BEM, void *workspace, size_t workspace_bytes, void *stream);
 int raftk_general_solve_dynamics_fd_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c, const raftk_solve_opts *o,
                                          double *Xi, int32_t *status, double *F_BEM);
+
+/*
+ * Second-order wave loads of the generalised-DOF solve (potSecOrder 2; raft_model.py:1035-1048, 1210-1212): the external
+ * difference-frequency QTF of the FOWT, the state FOWT.readQTF leaves behind (raft_fowt.py:2081-2128) with the DOF axis cut
+ * to the 6 rows a .12d file fills -- the reference lumps the force on reduced DOFs 0-5 ("Lumping at the first 6dofs",
+ * raft_model.py:1034), rows 6 and up are zero.  raft_b200.packer.pack_general_qtf builds it.  Same layout as
+ * raftk_designs.qtf for one FOWT.
+ * Every row of the case table, secondary trains included, gets F_2nd / F_2nd_mean of its own spectrum and heading
+ * (raftk_second_order_force_*: FOWT.calcHydroForce_2ndOrd, interpMode 'qtf'), computed on the call's stream before the loop
+ * and added to the real part of reduced rows 0-5 of the inertial excitation after the BEM force:
+ * ((F_BEM + F_iner) + F_2nd) + F_drag in every pass, and for the secondary trains.  k_qtf_tiles combines partial sums with
+ * atomic adds, so the last bits of F_2nd, and therefore of Xi, vary from run to run (as on the rigid path);
+ * RAFTK_QTF_DIAG=1 selects the diagonal kernel, which is reproducible.
+ * Rejected with RAFTK_EINVAL before any launch: n_qtf_w < 2, n_qtf_head < 1, a missing table, n_dof < 6, nw above the force
+ * kernel's shared-memory limit (nw * 20 bytes <= 227 KB), frequencies that do not strictly increase or headings that do not
+ * strictly increase.  The *_dev entry reads qtf_w and qtf_heads back to the host for these checks (a copy on the caller's
+ * stream and a wait for it).
+ */
+typedef struct raftk_general_qtf {
+    int32_t n_qtf_w, n_qtf_head;
+    const double *qtf_w;            /* [n_qtf_w] rad/s, strictly increasing (w1_2nd == w2_2nd)                              */
+    const double *qtf_heads;        /* [n_qtf_head] rad, strictly increasing (heads_2nd)                                    */
+    const double *qtf;              /* complex [n_qtf_w, n_qtf_w, n_qtf_head, 6]: fowt.qtf[..., :6], dimensional, Hermitian-filled */
+} raftk_general_qtf;
+
+/* qtf = NULL: raftk_general_solve_dynamics_fd_*, bit for bit (those entry points call these).  F_2nd: optional output, real
+ * [n_cases,6,nw] (the one-bin-shifted amplitudes; last bin zero); F_2nd_mean: optional output [n_cases,6]; without a table both
+ * are left untouched.  When NULL, the workspace holds them. */
+size_t raftk_general_qtf_workspace_bytes(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, int32_t n_cases);
+int raftk_general_solve_dynamics_qtf_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, const raftk_cases *c,
+                                         const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM, double *F_2nd,
+                                         double *F_2nd_mean, void *workspace, size_t workspace_bytes, void *stream);
+int raftk_general_solve_dynamics_qtf_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, const raftk_cases *c,
+                                          const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM, double *F_2nd,
+                                          double *F_2nd_mean);
 
 /*
  * Output channels of FOWT.saveTurbineOutputs for a FOWT with generalised degrees of freedom (raft_fowt.py:2299-2604): PRP

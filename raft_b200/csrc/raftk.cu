@@ -225,52 +225,59 @@ static int validate_qtf(const raftk_designs *d, const raftk_cases *c)
     return 0;
 }
 
-static int run_qtf(const raftk_designs *d, const raftk_cases *c, double *F2, double *F2mean, cudaStream_t st)
+// The second-order force launches for the table, grid and output rows in P (P.F2 required) and the sea states of c: the
+// rigid path (designs' table, run_qtf) and the generalised-DOF path (one FOWT's table) both come here.
+static int launch_qtf(const QtfParams &P, const raftk_cases *c, cudaStream_t st)
 {
-    int rc = validate_qtf(d, c);
-    if (rc) return rc;
-    if (!F2) return set_err(RAFTK_EINVAL, "second-order force needs the F_2nd buffer");
     CasesDev C = to_dev(c);
-    QtfParams P;
-    P.nD = d->n_designs; P.shared = d->qtf_shared;
-    P.n2 = d->n_qtf_w; P.nh = d->n_qtf_head; P.nw = d->nw; P.dw = d->dw;
-    P.w = d->w; P.qw = d->qtf_w; P.qh = d->qtf_heads;
-    P.qtf = reinterpret_cast<const double2 *>(d->qtf);
-    P.F2 = F2; P.F2mean = F2mean;
-    const size_t smem = (size_t)d->nw * 20;
+    const size_t smem = (size_t)P.nw * 20;
     static SmemOptIn opt_plain(48 * 1024), opt_mix(48 * 1024), opt_tiles(48 * 1024);
     CUDA_TRY(opt_plain.ensure(k_qtf_force<false>, smem));
     CUDA_TRY(opt_mix.ensure(k_qtf_force<true>, smem));
-    if (P.shared != 1 && d->n_designs > 65535) return set_err(RAFTK_EINVAL, "second-order force: more than 65535 designs per call");
+    if (P.shared != 1 && P.nD > 65535) return set_err(RAFTK_EINVAL, "second-order force: more than 65535 designs per call");
     if (c->n_cases > 65535) return set_err(RAFTK_EINVAL, "second-order force: more than 65535 cases per call");
     // tile variant (registers hold the table-cell corners, systolic diagonal accumulators) when its shared-memory
     // tables fit and the frequency rows fit k_qtf_finish's register staging; RAFTK_QTF_DIAG=1 forces the diagonal kernel
-    const int ncell = d->n_qtf_w - 1;
-    const size_t tsmem = (size_t)d->nw * 68 + (size_t)ncell * 8 + 16;
-    const bool tiles = !getenv("RAFTK_QTF_DIAG") && tsmem <= 226 * 1024 && d->nw <= 4096;
+    const int ncell = P.n2 - 1;
+    const size_t tsmem = (size_t)P.nw * 68 + (size_t)ncell * 8 + 16;
+    const bool tiles = !getenv("RAFTK_QTF_DIAG") && tsmem <= 226 * 1024 && P.nw <= 4096;
     if (tiles) {
         CUDA_TRY(opt_tiles.ensure(k_qtf_tiles, tsmem));
         QtfTileParams TP;
         TP.q = P; TP.ncell = ncell;
-        const size_t rows = (size_t)((P.shared == 1) ? 1 : d->n_designs) * c->n_cases * 6 * d->nw;
-        CUDA_TRY(cudaMemsetAsync(F2, 0, rows * sizeof(double), st));
-        dim3 gt(QT_GROUPS, c->n_cases, P.shared == 1 ? 1 : d->n_designs);
+        const size_t rows = (size_t)((P.shared == 1) ? 1 : P.nD) * c->n_cases * 6 * P.nw;
+        CUDA_TRY(cudaMemsetAsync(P.F2, 0, rows * sizeof(double), st));
+        dim3 gt(QT_GROUPS, c->n_cases, P.shared == 1 ? 1 : P.nD);
         k_qtf_tiles<<<gt, QT_THREADS, tsmem, st>>>(C, TP);
-        dim3 gf(6, c->n_cases, P.shared == 1 ? 1 : d->n_designs);
+        dim3 gf(6, c->n_cases, P.shared == 1 ? 1 : P.nD);
         k_qtf_finish<<<gf, 256, 0, st>>>(C, P);
         g_launches += 2;
         disp_launch(RAFTK_FAMILY_QTF, RAFTK_KERNEL_QTF_TILES, QT_THREADS);
         CUDA_TRY(cudaGetLastError());
         return RAFTK_OK;
     }
-    const int ntasks = d->nw / 2 + 1, per_cta = (QTF_THREADS / 32) * QTF_TASKS_PER_WARP;
-    dim3 grid((ntasks + per_cta - 1) / per_cta, c->n_cases, P.shared == 1 ? 1 : d->n_designs);
+    const int ntasks = P.nw / 2 + 1, per_cta = (QTF_THREADS / 32) * QTF_TASKS_PER_WARP;
+    dim3 grid((ntasks + per_cta - 1) / per_cta, c->n_cases, P.shared == 1 ? 1 : P.nD);
     if (P.nh > 1) k_qtf_force<true><<<grid, QTF_THREADS, smem, st>>>(C, P);
     else k_qtf_force<false><<<grid, QTF_THREADS, smem, st>>>(C, P);
     g_launches++;
     disp_launch(RAFTK_FAMILY_QTF, P.nh > 1 ? RAFTK_KERNEL_QTF_DIAG_MIX : RAFTK_KERNEL_QTF_DIAG, QTF_THREADS);
     CUDA_TRY(cudaGetLastError());
     return RAFTK_OK;
+}
+
+static int run_qtf(const raftk_designs *d, const raftk_cases *c, double *F2, double *F2mean, cudaStream_t st)
+{
+    int rc = validate_qtf(d, c);
+    if (rc) return rc;
+    if (!F2) return set_err(RAFTK_EINVAL, "second-order force needs the F_2nd buffer");
+    QtfParams P;
+    P.nD = d->n_designs; P.shared = d->qtf_shared;
+    P.n2 = d->n_qtf_w; P.nh = d->n_qtf_head; P.nw = d->nw; P.dw = d->dw;
+    P.w = d->w; P.qw = d->qtf_w; P.qh = d->qtf_heads;
+    P.qtf = reinterpret_cast<const double2 *>(d->qtf);
+    P.F2 = F2; P.F2mean = F2mean;
+    return launch_qtf(P, c, st);
 }
 
 extern "C" int raftk_second_order_force_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *out, void *stream)
@@ -1330,11 +1337,11 @@ extern "C" int raftk_second_order_force_host(const raftk_designs *d, const raftk
 }
 
 // ---- generalised degrees of freedom (flexible members) ---------------------------------------------------------------
-struct GenLayout { size_t u, f6, Fi, Fd, XL, Bm, Bd, Z, pv, fl, fb6, FB, total; };
-static GenLayout gen_layout(const raftk_general *g, const raftk_general_fd *fd, size_t nC)
+struct GenLayout { size_t u, f6, Fi, Fd, XL, Bm, Bd, Z, pv, fl, fb6, FB, F2, F2m, total; };
+static GenLayout gen_layout(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *q, size_t nC)
 {
     const size_t n = g->n_dof, nw = g->nw, Ns = std::max(g->n_nodes, 1);
-    const size_t nbem = (fd && fd->n_bem_head > 0) ? 1 : 0;
+    const size_t nbem = (fd && fd->n_bem_head > 0) ? 1 : 0, nq = q ? 1 : 0;
     GenLayout L; size_t t = 0;
     auto take = [&](size_t b) { size_t o = t; t += align_up(b, 256); return o; };
     L.u = take(nC * Ns * 3 * nw * 16); L.f6 = take(nC * Ns * 6 * nw * 16);
@@ -1342,8 +1349,25 @@ static GenLayout gen_layout(const raftk_general *g, const raftk_general_fd *fd, 
     L.Bm = take(nC * Ns * 9 * 8); L.Bd = take(nC * n * n * 8);
     L.Z = take(nC * nw * n * (n + 1) * 16); L.pv = take(nC * nw * n * 4); L.fl = take(nC * 16);
     L.fb6 = take(nbem * nC * 6 * nw * 16); L.FB = take(nbem * nC * n * nw * 16);     // BEM force (full DOFs 0-5, reduced DOFs)
+    L.F2 = take(nq * nC * 6 * nw * 8); L.F2m = take(nq * nC * 6 * 8);                 // second-order force and mean drift
     L.total = t;
     return L;
+}
+
+// raftk_general_qtf checks (include/raftk.h); qw, qh: host copies of qtf_w and qtf_heads, read only once the counts and
+// pointers have passed
+static int validate_gen_qtf(const raftk_general *g, const raftk_general_qtf *q, const double *qw, const double *qh)
+{
+    if (q->n_qtf_w < 2 || q->n_qtf_head < 1 || !q->qtf || !q->qtf_w || !q->qtf_heads)
+        return set_err(RAFTK_EINVAL, "general solve: qtf needs n_qtf_w >= 2, n_qtf_head >= 1, qtf, qtf_w and qtf_heads");
+    if (g->n_dof < 6) return set_err(RAFTK_EINVAL, "general solve: a QTF table needs n_dof >= 6 (it loads reduced DOFs 0-5)");
+    if ((size_t)g->nw * 20 > 227 * 1024) return set_err(RAFTK_EINVAL, "general solve: nw too large for the second-order force kernel's shared-memory tables");
+    if (!qw || !qh) return 0;
+    for (int t = 1; t < q->n_qtf_w; t++)
+        if (!(qw[t] > qw[t - 1])) return set_err(RAFTK_EINVAL, "general solve: qtf.qtf_w must be strictly increasing");
+    for (int t = 1; t < q->n_qtf_head; t++)
+        if (!(qh[t] > qh[t - 1])) return set_err(RAFTK_EINVAL, "general solve: qtf.qtf_heads must be strictly increasing");
+    return 0;
 }
 
 // raftk_general_fd checks on host copies of fd_idx and bem_headings (include/raftk.h)
@@ -1366,10 +1390,16 @@ static int validate_gen_fd(const raftk_general *g, const raftk_general_fd *fd, c
     return 0;
 }
 
-extern "C" size_t raftk_general_fd_workspace_bytes(const raftk_general *g, const raftk_general_fd *fd, int32_t n_cases)
+extern "C" size_t raftk_general_qtf_workspace_bytes(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                                    int32_t n_cases)
 {
     if (!g || n_cases <= 0 || g->n_dof <= 0 || g->nw <= 0) return 0;
-    return gen_layout(g, fd, (size_t)n_cases).total;
+    return gen_layout(g, fd, qtf, (size_t)n_cases).total;
+}
+
+extern "C" size_t raftk_general_fd_workspace_bytes(const raftk_general *g, const raftk_general_fd *fd, int32_t n_cases)
+{
+    return raftk_general_qtf_workspace_bytes(g, fd, nullptr, n_cases);
 }
 
 extern "C" size_t raftk_general_workspace_bytes(const raftk_general *g, int32_t n_cases)
@@ -1377,9 +1407,10 @@ extern "C" size_t raftk_general_workspace_bytes(const raftk_general *g, int32_t 
     return raftk_general_fd_workspace_bytes(g, nullptr, n_cases);
 }
 
-extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
-                                                   const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM,
-                                                   void *workspace, size_t workspace_bytes, void *stream)
+extern "C" int raftk_general_solve_dynamics_qtf_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                                    const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
+                                                    double *F_BEM, double *F_2nd, double *F_2nd_mean, void *workspace,
+                                                    size_t workspace_bytes, void *stream)
 {
     disp_reset();
     if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
@@ -1387,6 +1418,14 @@ extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const
         return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, 0 < n_cases <= 65535");
     if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
     cudaStream_t st = (cudaStream_t)stream;
+    if (qtf) {                                         // the frequency and heading vectors are read back for the checks
+        if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
+        std::vector<double> qw(qtf->n_qtf_w), qh(qtf->n_qtf_head);
+        CUDA_TRY(cudaMemcpyAsync(qw.data(), qtf->qtf_w, qw.size() * 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(qh.data(), qtf->qtf_heads, qh.size() * 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (int rc = validate_gen_qtf(g, qtf, qw.data(), qh.data())) return rc;
+    }
     if (fd) {                                          // the index and heading tables are read back for the checks
         if (fd->n_fd < 0 || fd->n_fd > g->n_dof || fd->n_bem_head < 0 || (fd->n_fd > 0 && !fd->fd_idx) || (fd->n_bem_head > 0 && !fd->bem_headings))
             return validate_gen_fd(g, fd, nullptr, nullptr);
@@ -1398,7 +1437,7 @@ extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const
         if (int rc = validate_gen_fd(g, fd, idx.data(), hd.data())) return rc;
     }
     const size_t nC = c->n_cases;
-    const GenLayout L = gen_layout(g, fd, nC);
+    const GenLayout L = gen_layout(g, fd, qtf, nC);
     if (!workspace || workspace_bytes < L.total) return set_err(RAFTK_ENOMEM, "general solve: workspace too small");
     const bool bem = fd && fd->n_bem_head > 0;
     GenDev D;
@@ -1435,6 +1474,17 @@ extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const
         CUDA_TRY(fdz ? opt_fd.ensure(k_gen_solve_blocked<true>, lu_smem) : opt.ensure(k_gen_solve_blocked<false>, lu_smem));
     }
     if (F_BEM && !bem) CUDA_TRY(cudaMemsetAsync(F_BEM, 0, nC * g->n_dof * g->nw * 16, st));
+    double *F2 = nullptr;
+    if (qtf) {                                         // second-order force of every case and train (k_qtf_*), before the loop
+        QtfParams QP;
+        QP.nD = 1; QP.shared = 0;
+        QP.n2 = qtf->n_qtf_w; QP.nh = qtf->n_qtf_head; QP.nw = g->nw; QP.dw = g->dw;
+        QP.w = g->w; QP.qw = qtf->qtf_w; QP.qh = qtf->qtf_heads;
+        QP.qtf = reinterpret_cast<const double2 *>(qtf->qtf);
+        QP.F2 = F2 = F_2nd ? F_2nd : reinterpret_cast<double *>(b + L.F2);
+        QP.F2mean = F_2nd_mean ? F_2nd_mean : reinterpret_cast<double *>(b + L.F2m);
+        if (int rc = launch_qtf(QP, c, st)) return rc;
+    }
     prof_begin_call();
     k_gen_init<<<(unsigned)nC, 256, 0, st>>>(D, W, o->xi_start, prim);
     if (g->n_nodes > 0) k_gen_wave<<<dim3(fb, g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, C, W);
@@ -1446,6 +1496,10 @@ extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const
     if (bem) k_gen_project<false, true><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_iner, 0, nullptr, Fx);
     else k_gen_project<false, false><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_iner, 0, nullptr, Fx);
     g_launches += 3;
+    if (F2) {                                          // (F_BEM + F_iner) + F_2nd on reduced DOFs 0-5
+        k_gen_add_2nd<<<dim3(fb, 6, (unsigned)nC), 128, 0, st>>>(D, W, F2);
+        g_launches++;
+    }
     for (int pass = 0; pass < o->n_iter + 1; pass++) {
         if (g->n_nodes > 0) k_gen_node_pass<false><<<dim3(g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, W, nullptr);
         k_gen_bdrag<<<dim3(g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W);
@@ -1476,14 +1530,22 @@ extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const
     return RAFTK_OK;
 }
 
+extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
+                                                   const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM,
+                                                   void *workspace, size_t workspace_bytes, void *stream)
+{
+    return raftk_general_solve_dynamics_qtf_dev(g, fd, nullptr, c, o, Xi, status, F_BEM, nullptr, nullptr, workspace, workspace_bytes, stream);
+}
+
 extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
                                                 int32_t *status, void *workspace, size_t workspace_bytes, void *stream)
 {
     return raftk_general_solve_dynamics_fd_dev(g, nullptr, c, o, Xi, status, nullptr, workspace, workspace_bytes, stream);
 }
 
-extern "C" int raftk_general_solve_dynamics_fd_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
-                                                    const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM)
+extern "C" int raftk_general_solve_dynamics_qtf_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                                     const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
+                                                     double *F_BEM, double *F_2nd, double *F_2nd_mean)
 {
     disp_reset();
     if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
@@ -1496,7 +1558,11 @@ extern "C" int raftk_general_solve_dynamics_fd_host(const raftk_general *g, cons
         }
     if (fd)
         if (int rc = validate_gen_fd(g, fd, fd->fd_idx, fd->bem_headings)) return rc;
-    Staging S("raftk_general_solve_dynamics_fd_host");
+    if (qtf) {
+        if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
+        if (int rc = validate_gen_qtf(g, qtf, qtf->qtf_w, qtf->qtf_heads)) return rc;
+    }
+    Staging S(qtf ? "raftk_general_solve_dynamics_qtf_host" : "raftk_general_solve_dynamics_fd_host");
     raftk_general gg = *g;
     S.in(gg.w, g->w, nw); S.in(gg.k, g->k, nw);
     S.in(gg.node_r, g->node_r, Ns * 3); S.in(gg.node_frame, g->node_frame, Ns * 9);
@@ -1514,15 +1580,28 @@ extern "C" int raftk_general_solve_dynamics_fd_host(const raftk_general *g, cons
         S.in(ff.fd_idx, fd->fd_idx, nf); S.in(ff.A_w, fd->A_w, nf * nf * nw); S.in(ff.B_w, fd->B_w, nf * nf * nw);
         S.in(ff.bem_headings, fd->bem_headings, nh); S.in(ff.X_BEM, fd->X_BEM, nh * 6 * nw * 2); S.in(ff.T0, fd->T0, nh ? 6 * n : 0);
     }
-    double *dXi, *dF_BEM;
+    raftk_general_qtf qq = qtf ? *qtf : raftk_general_qtf{};
+    if (qtf) {                                                    // validate_gen_qtf: both counts >= 1
+        const size_t n2 = qtf->n_qtf_w, nh = qtf->n_qtf_head;
+        S.in(qq.qtf_w, qtf->qtf_w, n2); S.in(qq.qtf_heads, qtf->qtf_heads, nh); S.in(qq.qtf, qtf->qtf, n2 * n2 * nh * 12);
+    }
+    double *dXi, *dF_BEM, *dF2, *dF2m;
     int32_t *dStatus;
     char *ws;
-    const size_t wb = raftk_general_fd_workspace_bytes(g, fd, (int32_t)nC);
+    const size_t wb = raftk_general_qtf_workspace_bytes(g, fd, qtf, (int32_t)nC);
     S.out(dXi, nC * n * nw * 2, Xi); S.out(dStatus, nC * 4, status); S.out(dF_BEM, F_BEM ? nC * n * nw * 2 : 0, F_BEM);
+    S.out(dF2, qtf && F_2nd ? nC * 6 * nw : 0, F_2nd); S.out(dF2m, qtf && F_2nd_mean ? nC * 6 : 0, F_2nd_mean);
     S.buf(ws, wb);
     int rc = S.commit();
-    if (rc || (rc = raftk_general_solve_dynamics_fd_dev(&gg, fd ? &ff : nullptr, &cc, o, dXi, dStatus, dF_BEM, ws, wb, nullptr))) return rc;
+    if (rc || (rc = raftk_general_solve_dynamics_qtf_dev(&gg, fd ? &ff : nullptr, qtf ? &qq : nullptr, &cc, o, dXi, dStatus, dF_BEM, dF2, dF2m,
+                                                         ws, wb, nullptr))) return rc;
     return S.finish();
+}
+
+extern "C" int raftk_general_solve_dynamics_fd_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
+                                                    const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM)
+{
+    return raftk_general_solve_dynamics_qtf_host(g, fd, nullptr, c, o, Xi, status, F_BEM, nullptr, nullptr);
 }
 
 extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,

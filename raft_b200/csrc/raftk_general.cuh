@@ -9,6 +9,7 @@
 //   k_gen_wave      (case, node, w)   wave kinematics u, inertial node load f6 = [f ; rr x f]
 //   k_gen_bem       (case, w)         BEM tables only: 6-component BEM force (full DOFs 0-5) of every case and train
 //   k_gen_project   (case, dof, w)    F = sum_j Tn_j^T f6_j   (F_BEM = T0^T f_BEM; F_iner = F_BEM + sum_j Tn_j^T f6_j; F_drag)
+//   k_gen_add_2nd   (case, 0-5, w)    QTF only: F_iner += F_2nd on reduced DOFs 0-5 (F_2nd from the k_qtf_* kernels, before)
 //   per pass:
 //   k_gen_node_pass (case, node)      node velocity from Tn_j XiLast, RMS over w, linearised Bmat_j, drag load f6
 //   k_gen_bdrag     (case, row)       B_drag = sum_j Tn_j^T B6_j Tn_j
@@ -152,6 +153,17 @@ __global__ void __launch_bounds__(128) k_gen_bem(GenDev D, CasesDev Cs, GenFdDev
     double2 *f = X.fb6 + (size_t)c * 6 * nw + i;
 #pragma unroll
     for (int a = 0; a < 6; a++) f[(size_t)a * nw] = make_double2(Br[a], Bi[a]);
+}
+
+// k_gen_add_2nd: grid (ceil(nw/128), 6, nC), block 128: the second-order force of every case and train (real amplitudes
+// [nC][6][nw] of k_qtf_tiles / k_qtf_force) added to reduced rows 0-5 of F_iner, which already hold F_BEM + F_iner:
+// (F_BEM + F_iner) + F_2nd (raft_model.py:1048, 1212; lumped on the first 6 DOFs, :1034)
+__global__ void __launch_bounds__(128) k_gen_add_2nd(GenDev D, GenWork W, const double *F2)
+{
+    const int i = blockIdx.x * 128 + threadIdx.x, a = blockIdx.y, c = blockIdx.z;
+    if (i >= D.nw) return;
+    double2 &f = W.F_iner[((size_t)c * D.n + a) * D.nw + i];
+    f.x = f.x + F2[((size_t)c * 6 + a) * D.nw + i];
 }
 
 // DOF -> position on the support of the frequency-dependent terms (-1 off it), built once per CTA in shared memory

@@ -297,6 +297,30 @@ def pack_qtf(fowt):
                 qtf_heads=np.asarray(fowt.heads_2nd, dtype=float))
 
 
+def pack_general_qtf(fowt):
+    """External difference-frequency QTF of a FOWT with generalised degrees of freedom (nDOF > 6, potSecOrder 2) for the
+    generalised-DOF solve (C ABI ``raftk_general_qtf``): ``qtf`` complex [nw1, nw1, nheads, 6], the reference's
+    ``fowt.qtf`` [nw1, nw2, nheads, nDOF] cut to reduced DOFs 0-5 -- FOWT.readQTF fills only those from a .12d file and the
+    force is lumped there (raft_fowt.py:2112-2123, raft_model.py:1034) -- with ``qtf_w`` [nw1] rad/s and ``qtf_heads``
+    [nheads] rad.  Empty dict for potSecOrder 0.  ValueError if any DOF from 6 up carries a nonzero entry (the solve would drop
+    it); NotImplementedError for potSecOrder 1, where the reference uses null QTFs for such FOWTs (raft_fowt.py:2015-2017)."""
+    sec = int(getattr(fowt, "potSecOrder", 0) or 0)
+    if sec == 0:
+        return {}
+    if sec == 1:
+        raise NotImplementedError("slender-body QTF of a FOWT with generalised DOFs: the reference uses null QTFs there "
+                                  "(raft_fowt.py:2015-2017)")
+    w1, w2 = np.asarray(fowt.w1_2nd, dtype=float), np.asarray(fowt.w2_2nd, dtype=float)
+    if w1.shape != w2.shape or not (w1 == w2).all():
+        raise ValueError("Both frequency columns in the input QTF must contain the same values.")   # raft_fowt.py:2109
+    q = np.asarray(fowt.qtf, dtype=np.complex128)
+    if q.ndim != 4 or q.shape[3] < 6:
+        raise ValueError("fowt.qtf must be [nw1, nw2, nheads, nDOF] with nDOF >= 6")
+    if np.any(q[..., 6:] != 0):
+        raise ValueError("fowt.qtf has nonzero entries on reduced DOFs 6 and up; the generalised-DOF solve loads DOFs 0-5 only")
+    return dict(qtf=np.ascontiguousarray(q[..., :6]), qtf_w=w1, qtf_heads=np.asarray(fowt.heads_2nd, dtype=float))
+
+
 def pack_qtf_members(fowt):
     """Tables of the slender-body QTF (potSecOrder 1; C ABI ``raftk_slender``), duck-typed on the reference's FOWT / Member
     objects.  Hoists what Member.calcQTF_slenderBody / correction_KAY evaluate inside their frequency-pair loops

@@ -14,7 +14,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import RaftkCases, RaftkDesigns, RaftkFarm, RaftkGeneral, RaftkGeneralFd, RaftkOutputs, RaftkSlender, RaftkSolveOpts, check, lib
+from ._lib import RaftkCases, RaftkDesigns, RaftkFarm, RaftkGeneral, RaftkGeneralFd, RaftkGeneralQtf, RaftkOutputs, RaftkSlender, RaftkSolveOpts, check, lib
 
 _F8 = np.float64
 _I4 = np.int32
@@ -540,15 +540,33 @@ def _general_fd_struct(fd, n, nw, ptr_of):
     return f
 
 
+def _general_qtf_struct(qtf, ptr_of):
+    """raftk_general_qtf for the dict of ``packer.pack_general_qtf`` (qtf complex [nw2,nw2,nheads,6], qtf_w [nw2] rad/s,
+    qtf_heads [nheads] rad), or None for qtf=None or {} (potSecOrder 0)."""
+    if not qtf:
+        return None
+    qw = np.ascontiguousarray(qtf["qtf_w"], dtype=_F8)
+    qh = np.ascontiguousarray(qtf["qtf_heads"], dtype=_F8)
+    Q = np.ascontiguousarray(qtf["qtf"], dtype=np.complex128)
+    if Q.shape != (len(qw), len(qw), len(qh), 6):
+        raise ValueError("qtf must be [nw2, nw2, nheads, 6] with nw2 = len(qtf_w), nheads = len(qtf_heads)")
+    q = RaftkGeneralQtf()
+    q.n_qtf_w, q.n_qtf_head = len(qw), len(qh)
+    q.qtf_w, q.qtf_heads, q.qtf = ptr_of("qtf_w", qw), ptr_of("qtf_heads", qh), ptr_of("qtf", Q)
+    return q
+
+
 class GeneralSession:
     """Generalised-DOF solve with tables, workspace and outputs resident in HBM (torch tensors), kernels on torch's current
     stream: ``solve()`` enqueues raftk_general_solve_dynamics_dev -> (Xi [nT,nDOF,nw] complex, status [nT,4]); ``cases`` may
     carry wave trains (``packer.pack_case_trains``).  ``stats(R, wpow)`` reduces the device Xi to output-channel statistics
     on the device (raftk_general_channel_stats_dev), so the responses never leave HBM.  ``fd``: frequency-dependent added
     mass, damping and BEM excitation (``packer.pack_general_matrices``); with ``F_BEM=True`` ``solve()`` also returns the BEM
-    excitation in reduced DOFs, complex [nT,nDOF,nw]."""
+    excitation in reduced DOFs, complex [nT,nDOF,nw].  ``qtf``: second-order wave loads (``packer.pack_general_qtf``); every
+    ``solve()`` then leaves the force of every case and train in the device tensors ``F_2nd`` [nT,6,nw] and ``F_2nd_mean``
+    [nT,6] (reduced DOFs 0-5)."""
 
-    def __init__(self, P, M, B, Cm, cases, device=None, fd=None, F_BEM=False):
+    def __init__(self, P, M, B, Cm, cases, device=None, fd=None, F_BEM=False, qtf=None):
         import torch
         self.torch = torch
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
@@ -564,22 +582,28 @@ class GeneralSession:
             self.c_struct = cases.struct(lambda name: self.ct[name].data_ptr())
             n, nw, nC = int(P["gen_nDOF"]), len(P["w"]), cases.n_cases
             self.fd = _general_fd_struct(fd, n, nw, to_dev)
+            self.qtf = _general_qtf_struct(qtf, to_dev)
             fdp = C.byref(self.fd) if self.fd is not None else None
-            self.workspace_bytes = int(lib.raftk_general_fd_workspace_bytes(C.byref(self.g), fdp, nC))
+            qp = C.byref(self.qtf) if self.qtf is not None else None
+            self.workspace_bytes = int(lib.raftk_general_qtf_workspace_bytes(C.byref(self.g), fdp, qp, nC))
             self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=self.device)
             self.Xi = torch.zeros([nC, n, nw], dtype=torch.complex128, device=self.device)
             self.status = torch.zeros([nC, 4], dtype=torch.int32, device=self.device)
             self.F_BEM = torch.zeros([nC, n, nw], dtype=torch.complex128, device=self.device) if F_BEM else None
+            self.F_2nd = torch.zeros([nC, 6, nw], dtype=torch.float64, device=self.device) if self.qtf is not None else None
+            self.F_2nd_mean = torch.zeros([nC, 6], dtype=torch.float64, device=self.device) if self.qtf is not None else None
         self.n, self.nw, self.n_cases, self.dw = n, nw, nC, float(P["dw"])
         self._ch = None
 
     def solve(self, n_iter=10, tol=0.01, xi_start=0.0):
         o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
+        ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
         with self.torch.cuda.device(self.device):
-            check(lib.raftk_general_solve_dynamics_fd_dev(C.byref(self.g), C.byref(self.fd) if self.fd is not None else None, C.byref(self.c_struct),
-                                                          C.byref(o), self.Xi.data_ptr(), self.status.data_ptr(),
-                                                          self.F_BEM.data_ptr() if self.F_BEM is not None else None, self.workspace.data_ptr(),
-                                                          self.workspace_bytes, self.torch.cuda.current_stream(self.device).cuda_stream))
+            check(lib.raftk_general_solve_dynamics_qtf_dev(C.byref(self.g), C.byref(self.fd) if self.fd is not None else None,
+                                                           C.byref(self.qtf) if self.qtf is not None else None, C.byref(self.c_struct),
+                                                           C.byref(o), self.Xi.data_ptr(), self.status.data_ptr(), ptr(self.F_BEM),
+                                                           ptr(self.F_2nd), ptr(self.F_2nd_mean), self.workspace.data_ptr(),
+                                                           self.workspace_bytes, self.torch.cuda.current_stream(self.device).cuda_stream))
         return (self.Xi, self.status) if self.F_BEM is None else (self.Xi, self.status, self.F_BEM)
 
     def stats(self, R, wpow, psd=True, amp=False):
@@ -604,14 +628,16 @@ class GeneralSession:
         return sd, P, A
 
 
-def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0, fd=None, F_BEM=False):
+def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0, fd=None, F_BEM=False, qtf=None, F_2nd=False):
     """Model.solveDynamics for one FOWT with generalised degrees of freedom (flexible members), host buffers:
     ``P`` from ``packer.pack_general_dofs`` (node tables + ``gen_Tn``, ``gen_rr``), constant system
     matrices ``M, B, Cm`` [nDOF,nDOF], ``cases`` a CaseTable, with wave trains when built from ``packer.pack_case_trains``
     (train 0 of a case drives the linearisation, raft_model.py:1200-1236) -> (Xi complex [nT,nDOF,nw], status [nT,4]).
     ``fd``: frequency-dependent added mass and damping (operating rotors, BEM coefficients) and BEM excitation, the ``fd``
     dict of ``packer.pack_general_matrices`` (whose M, B, C are then the constant matrices).  ``F_BEM=True`` appends the BEM
-    excitation of every case and train in reduced DOFs, complex [nT,nDOF,nw], to the result."""
+    excitation of every case and train in reduced DOFs, complex [nT,nDOF,nw], to the result.  ``qtf``: second-order wave
+    loads (potSecOrder 2), the dict of ``packer.pack_general_qtf``; ``F_2nd=True`` (with ``qtf``) then appends the force of
+    every case and train on reduced DOFs 0-5, F_2nd [nT,6,nw] and F_2nd_mean [nT,6]."""
     n, nw = int(P["gen_nDOF"]), len(P["w"])
     keep = {}
 
@@ -620,15 +646,20 @@ def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0
         return a.ctypes.data
     g = _general_struct(P, M, B, Cm, ptr)
     f = _general_fd_struct(fd, n, nw, ptr)
+    q = _general_qtf_struct(qtf, ptr)
+    if F_2nd and q is None:
+        raise ValueError("F_2nd=True needs a QTF table (qtf=, packer.pack_general_qtf)")
     nC = cases.n_cases
     Xi = np.zeros([nC, n, nw], dtype=np.complex128)
     st = np.zeros([nC, 4], dtype=_I4)
     Fb = np.zeros([nC, n, nw], dtype=np.complex128) if F_BEM else None
+    F2, F2m = (np.zeros([nC, 6, nw]), np.zeros([nC, 6])) if F_2nd else (None, None)
     c = cases.struct(_host_ptr(cases.arrays))
     o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
-    check(lib.raftk_general_solve_dynamics_fd_host(C.byref(g), C.byref(f) if f is not None else None, C.byref(c), C.byref(o), Xi.ctypes.data,
-                                                   st.ctypes.data, Fb.ctypes.data if F_BEM else None))
-    return (Xi, st, Fb) if F_BEM else (Xi, st)
+    hp = lambda a: a.ctypes.data if a is not None else None   # noqa: E731
+    check(lib.raftk_general_solve_dynamics_qtf_host(C.byref(g), C.byref(f) if f is not None else None, C.byref(q) if q is not None else None,
+                                                    C.byref(c), C.byref(o), Xi.ctypes.data, st.ctypes.data, hp(Fb), hp(F2), hp(F2m)))
+    return (Xi, st) + ((Fb,) if F_BEM else ()) + ((F2, F2m) if F_2nd else ())
 
 
 def combine_trains(std, psd, idx):
@@ -688,21 +719,32 @@ def general_case_metrics(channels, std, psd, amp, idx):
     return m
 
 
-def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, fd=None):
+def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, fd=None, qtf=None):
     """Model.analyzeCases (dynamics and output statistics) for one FOWT with generalised degrees of freedom: ``cases`` a list
     of case dicts, scalar or list-valued wave keys (several wave trains); ``channels`` from ``packer.pack_general_channels``.
     -> dict(Xi_trains [per case: nTrains,nDOF,nw], status [nC,4] of train 0, case_metrics {case: saveTurbineOutputs entries},
-    empty without channels).  ``fd``: frequency-dependent terms, as for ``general_solve_dynamics``."""
+    empty without channels).  ``fd``: frequency-dependent terms, as for ``general_solve_dynamics``.  ``qtf``: second-order
+    wave loads (``packer.pack_general_qtf``); the result then also holds, per case, the reference FOWT's ``Fhydro_2nd``
+    (complex [nTrains,nDOF,nw]) and ``Fhydro_2nd_mean`` ([nTrains,nDOF]), zero from reduced DOF 6 up (raft_model.py:1034-1036)."""
     from .packer import pack_case_trains
     table, owner, first = pack_case_trains(cases)
-    Xi, st = general_solve_dynamics(P, M, B, Cm, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start, fd=fd)
+    q = bool(qtf)
+    res = general_solve_dynamics(P, M, B, Cm, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start, fd=fd, qtf=qtf, F_2nd=q)
+    Xi, st = res[0], res[1]
     raise_on_flags(st[first])                                           # raft_model.py:1089, :1098-1099
     metrics = {}
     if channels is not None:
         sd, ps, amp = general_channel_stats(channels["R"], channels["wpow"], P["w"], Xi, float(P["dw"]), psd=True, amp=True)
         for ic in range(len(cases)):
             metrics[ic] = general_case_metrics(channels, sd, ps, amp, np.nonzero(owner == ic)[0])
-    return dict(Xi_trains=[Xi[owner == ic] for ic in range(len(cases))], status=st[first], case_metrics=metrics)
+    out = dict(Xi_trains=[Xi[owner == ic] for ic in range(len(cases))], status=st[first], case_metrics=metrics)
+    if q:
+        n, nw = Xi.shape[1], Xi.shape[2]
+        F2, F2m = np.zeros([len(Xi), n, nw], dtype=np.complex128), np.zeros([len(Xi), n])
+        F2[:, :6], F2m[:, :6] = res[2], res[3]
+        out["Fhydro_2nd"] = [F2[owner == ic] for ic in range(len(cases))]
+        out["Fhydro_2nd_mean"] = [F2m[owner == ic] for ic in range(len(cases))]
+    return out
 
 
 def second_order_force(batch, cases):
