@@ -430,8 +430,9 @@ int raftk_general_solve_dynamics_qtf_host(const raftk_general *g, const raftk_ge
  * motions, nacelle accelerations and flexible-tower base loads are real linear functionals of the reduced response,
  *   Y_ch(w) = w^wpow[ch] sum_b R[ch,b] Xi[b,w]     (raft_b200.packer.pack_general_channels; rad2deg folded into R)
  * -> std = sqrt(1/2 sum_w |Y|^2), PSD(w) = 1/2 |Y|^2 / dw, amp = Y, with the reduction of raftk_channel_stats_*.
- * w [nw] rad/s; R [n_ch,n_dof]; wpow [n_ch] 0 or 2; Xi complex [n_units,n_dof,nw] -> std [n_units,n_ch],
- * psd [n_units,n_ch,nw] or NULL, amp complex [n_units,n_ch,nw] or NULL.
+ * w [nw] rad/s; R [n_ch,n_dof]; wpow [n_ch] 0, 1 or 2 (displacement, velocity, acceleration); Xi complex [n_units,n_dof,nw]
+ * -> std [n_units,n_ch], psd [n_units,n_ch,nw] or NULL, amp complex [n_units,n_ch,nw] or NULL.  Any other wpow is refused
+ * with RAFTK_EINVAL before any launch; the _dev entry reads wpow back on its stream for that check (one synchronisation).
  */
 int raftk_general_channel_stats_dev(int32_t n_units, int32_t n_dof, int32_t n_ch, int32_t nw, double dw, const double *w,
                                     const double *R, const int32_t *wpow, const double *Xi, double *std, double *psd, double *amp,

@@ -1755,19 +1755,38 @@ extern "C" int raftk_channel_stats_host(int32_t n_designs, int32_t n_cases, int3
     return S.finish();
 }
 
+// k_general_channel_stats applies w^0, w^1 or w^2; wpow: a host copy
+static int validate_wpow(int32_t n_ch, const int32_t *wpow)
+{
+    for (int32_t t = 0; t < n_ch; t++)
+        if (wpow[t] < 0 || wpow[t] > 2) return set_err(RAFTK_EINVAL, "general channel-stats: wpow must be 0, 1 or 2");
+    return 0;
+}
+
+static int launch_general_channel_stats(int32_t n_units, int32_t n_dof, int32_t n_ch, int32_t nw, double dw, const double *w, const double *R,
+                                        const int32_t *wpow, const double *Xi, double *sd, double *psd, double *amp, cudaStream_t stream)
+{
+    const size_t rows = (size_t)n_units * n_ch;
+    if (rows > 2147483647u) return set_err(RAFTK_EINVAL, "general channel-stats: too many (unit, channel) rows");
+    k_general_channel_stats<<<(unsigned)rows, 128, 0, stream>>>(n_dof, n_ch, nw, dw, w, R, wpow, reinterpret_cast<const double2 *>(Xi),
+                                                              sd, psd, reinterpret_cast<double2 *>(amp));
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
 extern "C" int raftk_general_channel_stats_dev(int32_t n_units, int32_t n_dof, int32_t n_ch, int32_t nw, double dw, const double *w,
                                                const double *R, const int32_t *wpow, const double *Xi, double *sd, double *psd, double *amp,
                                                void *stream)
 {
     if (n_units <= 0 || n_dof <= 0 || n_ch <= 0 || nw <= 0 || !w || !R || !wpow || !Xi || !sd || !(dw > 0.0))
         return set_err(RAFTK_EINVAL, "bad general channel-stats arguments");
-    const size_t rows = (size_t)n_units * n_ch;
-    if (rows > 2147483647u) return set_err(RAFTK_EINVAL, "general channel-stats: too many (unit, channel) rows");
-    k_general_channel_stats<<<(unsigned)rows, 128, 0, (cudaStream_t)stream>>>(n_dof, n_ch, nw, dw, w, R, wpow, reinterpret_cast<const double2 *>(Xi),
-                                                                            sd, psd, reinterpret_cast<double2 *>(amp));
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
-    return RAFTK_OK;
+    cudaStream_t st = (cudaStream_t)stream;            // the powers are read back for the check
+    std::vector<int32_t> p(n_ch);
+    CUDA_TRY(cudaMemcpyAsync(p.data(), wpow, p.size() * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (int rc = validate_wpow(n_ch, p.data())) return rc;
+    return launch_general_channel_stats(n_units, n_dof, n_ch, nw, dw, w, R, wpow, Xi, sd, psd, amp, st);
 }
 
 extern "C" int raftk_general_channel_stats_host(int32_t n_units, int32_t n_dof, int32_t n_ch, int32_t nw, double dw, const double *w,
@@ -1775,6 +1794,7 @@ extern "C" int raftk_general_channel_stats_host(int32_t n_units, int32_t n_dof, 
 {
     if (n_units <= 0 || n_dof <= 0 || n_ch <= 0 || nw <= 0 || !w || !R || !wpow || !Xi || !sd || !(dw > 0.0))
         return set_err(RAFTK_EINVAL, "bad general channel-stats arguments");
+    if (int rc = validate_wpow(n_ch, wpow)) return rc;
     const size_t rows = (size_t)n_units * n_ch;
     Staging S("raftk_general_channel_stats_host");
     const double *dW, *dR, *dXi;
@@ -1783,7 +1803,7 @@ extern "C" int raftk_general_channel_stats_host(int32_t n_units, int32_t n_dof, 
     S.in(dW, w, nw); S.in(dR, R, (size_t)n_ch * n_dof); S.in(dWpow, wpow, n_ch); S.in(dXi, Xi, (size_t)n_units * n_dof * nw * 2);
     S.out(dSd, rows, sd); S.out(dPsd, psd ? rows * nw : 0, psd); S.out(dAmp, amp ? rows * nw * 2 : 0, amp);
     int rc = S.commit();
-    if (rc || (rc = raftk_general_channel_stats_dev(n_units, n_dof, n_ch, nw, dw, dW, dR, dWpow, dXi, dSd, dPsd, dAmp, nullptr))) return rc;
+    if (rc || (rc = launch_general_channel_stats(n_units, n_dof, n_ch, nw, dw, dW, dR, dWpow, dXi, dSd, dPsd, dAmp, nullptr))) return rc;
     return S.finish();
 }
 

@@ -608,6 +608,7 @@ __global__ void __launch_bounds__(128) k_general_channel_stats(int n, int nch, i
             yr = fma(c, v.x, yr); yi = fma(c, v.y, yi);
         }
         if (p == 2) { const double w2 = w[i] * w[i]; yr *= w2; yi *= w2; }
+        else if (p == 1) { const double w1 = w[i]; yr *= w1; yi *= w1; }
         const double a2 = yr * yr + yi * yi;
         s += a2;
         if (psd) psd[(size_t)row * nw + i] = 0.5 * a2 / dw;

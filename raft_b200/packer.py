@@ -469,7 +469,8 @@ def pack_general_channels(fowt):
       FbaseX .. MbaseZ     per flexible tower  internal loads at the tower base -Kf[base] T_tower Xi  :2541-2597
 
     Like the reference (:2302), the rigidBodyNode rows are taken at ``rigidBodyNode.id``, not ``6 * id``.
-    Returns dict(names [(name, rotor index or None)], R [nch, nDOF], wpow [nch] int32, avg [nch]).  ``avg`` holds the
+    Returns dict(names [(name, rotor index or None)], R [nch, nDOF], wpow [nch] int32 (0, 1 or 2; the channels here use 0
+    and 2), avg [nch]).  ``avg`` holds the
     reference's mean values (Xi0_PRP from r6, the hub node's r, the tower nodes' Xi0); 0 where those inputs are absent.
     A rigid tower's Mbase (:2508-2538) mixes w^0 and w^2 terms with the aero matrices and is not a channel of this form:
     NotImplementedError."""

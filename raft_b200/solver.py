@@ -614,6 +614,7 @@ class GeneralSession:
         wpow = np.ascontiguousarray(wpow, dtype=_I4)
         if R.ndim != 2 or R.shape[1] != self.n or wpow.shape != (R.shape[0],):
             raise ValueError("R must be [nch, %d] and wpow [nch]" % self.n)
+        _check_wpow(wpow)
         nch = R.shape[0]
         with torch.cuda.device(self.device):
             if self._ch is None or not (np.array_equal(self._ch[0], R) and np.array_equal(self._ch[1], wpow)):
@@ -668,9 +669,14 @@ def combine_trains(std, psd, idx):
     return np.sqrt((std[idx] ** 2).sum(axis=0)), psd[idx].sum(axis=0)
 
 
+def _check_wpow(wpow):
+    if wpow.size and (wpow.min() < 0 or wpow.max() > 2):
+        raise ValueError("wpow must be 0, 1 or 2 (displacement, velocity, acceleration)")
+
+
 def general_channel_stats(R, wpow, w, Xi, dw, psd=True, amp=False):
     """Output channels of a FOWT with generalised DOFs, Y = w^wpow R Xi (``packer.pack_general_channels``), host buffers:
-    R [nch,nDOF], wpow [nch], w [nw], Xi complex [nU,nDOF,nw] -> (std [nU,nch], PSD [nU,nch,nw] or None,
+    R [nch,nDOF], wpow [nch] 0, 1 or 2, w [nw], Xi complex [nU,nDOF,nw] -> (std [nU,nch], PSD [nU,nch,nw] or None,
     amplitudes complex [nU,nch,nw] or None)."""
     R = np.ascontiguousarray(R, dtype=_F8)
     wpow = np.ascontiguousarray(wpow, dtype=_I4)
@@ -680,6 +686,7 @@ def general_channel_stats(R, wpow, w, Xi, dw, psd=True, amp=False):
     nch = R.shape[0]
     if R.shape != (nch, n) or wpow.shape != (nch,) or w.shape != (nw,):
         raise ValueError("R must be [nch,nDOF], wpow [nch], w [nw] for Xi [nU,nDOF,nw]")
+    _check_wpow(wpow)
     sd = np.zeros([nU, nch])
     P = np.zeros([nU, nch, nw]) if psd else None
     A = np.zeros([nU, nch, nw], dtype=np.complex128) if amp else None
