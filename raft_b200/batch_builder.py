@@ -206,38 +206,36 @@ def _added_mass(T, r_ref):
     return A
 
 
-def _count_classes(keys, valid, rel):
-    """Per design: number of distinct keys (greedy first-occurrence dedupe with relative tolerance, like the kernel's
-    step-class builder).  keys [nD,P,c], valid [nD,P]."""
+def _count_classes(keys, valid, tol):
+    """Per design: the number of step classes by the fused kernels' rule (raftk_fused.cuh step_classes_warp), greedy in key
+    order: a key joins the first class whose key is within ``tol`` of it in every component, else opens one.
+    keys [nD,P,c], valid [nD,P], tol [nD,P] (each key's own tolerance)."""
+    nD = keys.shape[0]
     if keys.shape[1] == 0:
-        return np.zeros(keys.shape[0], dtype=np.int64)
-    # run-length compression first: a strip whose key repeats its predecessor's (the interior of a uniformly divided
-    # section) cannot open a class, so only run starts enter the pairwise comparison (a few per member)
-    # (reductions over the tiny trailing component axis are written out per component: NumPy's axis reductions cost ~10x
-    # more than the arithmetic on a length-1 or length-2 axis)
+        return np.zeros(nD, dtype=np.int64)
     nc = keys.shape[2]
-    comp = lambda a: [a[..., i] for i in range(nc)]
-    mag = sum(np.abs(x) for x in comp(keys))
-    close = np.ones(valid[:, 1:].shape, bool)
-    tol1 = rel * mag[:, 1:]
-    for x in comp(keys):
-        close &= np.abs(x[:, 1:] - x[:, :-1]) <= tol1
+    # a key equal to the valid key before it has the same tolerance and the same first match, so it opens no class: only
+    # the others are walked (the interior of a uniformly divided section repeats its step)
     rep = np.zeros(valid.shape, bool)
-    rep[:, 1:] = valid[:, :-1] & close
+    rep[:, 1:] = valid[:, :-1] & np.all(keys[:, 1:] == keys[:, :-1], axis=2)
     valid = valid & ~rep
     pmax = int(valid.sum(axis=1).max())
-    if pmax == 0:
-        return np.zeros(keys.shape[0], dtype=np.int64)
     order = np.argsort(~valid, axis=1, kind="stable")[:, :pmax]
     keys = np.take_along_axis(keys, order[:, :, None], axis=1)
     valid = np.take_along_axis(valid, order, axis=1)
-    tol = rel * sum(np.abs(x) for x in comp(keys))
-    same = np.ones((keys.shape[0], pmax, pmax), bool)                                                        # [nD,P(j),P(x)]
-    for x in comp(keys):
-        same &= np.abs(x[:, :, None] - x[:, None, :]) <= tol[:, :, None]
-    earlier = np.tril(np.ones((pmax, pmax), bool), -1)[None]                                                 # x < j
-    dup = np.any(same & earlier & valid[:, None, :], axis=2)
-    return (valid & ~dup).sum(axis=1)
+    tol = np.take_along_axis(tol, order, axis=1)
+    cls = np.zeros((nD, pmax, nc))                                        # class keys so far
+    n = np.zeros(nD, dtype=np.int64)
+    rows = np.arange(nD)
+    for p in range(pmax):
+        r = int(n.max())
+        hit = np.arange(r)[None, :] < n[:, None]
+        for i in range(nc):
+            hit &= np.abs(cls[:, :r, i] - keys[:, p, None, i]) <= tol[:, p, None]
+        new = valid[:, p] & ~hit.any(axis=1)
+        cls[rows[new], n[new]] = keys[new, p]
+        n += new
+    return n
 
 
 def build_family(family, w, k, depth, matrices, r6=None):
@@ -308,18 +306,16 @@ def build_family(family, w, k, depth, matrices, r6=None):
     kx, ky, kz = qv[:, :, None, 0] * step, qv[:, :, None, 1] * step, qv[:, :, None, 2] * step
     P = Nm * (S - 1)
     wk = np.stack([kx, ky], axis=3).reshape(nD, P, 2)
-    wv = (pair & ((np.abs(kx) > 1e-14) | (np.abs(ky) > 1e-14))).reshape(nD, P)
-    hv = (pair & (np.abs(kz) > 1e-14)).reshape(nD, P)
+    wv = (pair & ((np.abs(kx) > solver.STEP_ZERO) | (np.abs(ky) > solver.STEP_ZERO))).reshape(nD, P)
+    hv = (pair & (np.abs(kz) > solver.STEP_ZERO)).reshape(nD, P)
     z0 = rA[:, :, 2] + lsP[:, :, 0] * qv[:, :, 2]                                          # first submerged node of each member
-    zk = z0[:, :, None]
-    ztol = 1e-12 * np.maximum(1.0, np.abs(z0))
-    zsame = np.abs(zk - z0[:, None, :]) <= ztol[:, :, None]
-    zdup = np.any(zsame & np.tril(np.ones([Nm, Nm], bool), -1)[None] & has[:, None, :], axis=2)
+    counts = (_count_classes(wk, wv, solver.STEP_RTOL * (np.abs(wk[..., 0]) + np.abs(wk[..., 1]))),
+              _count_classes(kz.reshape(nD, P, 1), hv, solver.STEP_RTOL * np.abs(kz.reshape(nD, P))),
+              _count_classes(z0[:, :, None], has, solver.Z0_RTOL * np.maximum(1.0, np.abs(z0))))
     batch = solver.DesignBatch.from_tables(
         arrays, n_designs=nD, depth=float(depth), rho=rho, g=g, dw=float(w[1] - w[0]),
         max_nodes=int(max(1, cnt.sum(axis=1).max())), max_members=int(max(1, has.sum(axis=1).max())),
-        classes=(int(max(1, _count_classes(wk, wv, 1e-11).max())), int(max(1, _count_classes(kz.reshape(nD, P, 1), hv, 1e-11).max())),
-                 int(max(1, (has & ~zdup).sum(axis=1).max()))))
+        classes=tuple(int(max(1, c.max())) for c in counts))
     batch.A_hydro_morison = A_mor
     return batch
 

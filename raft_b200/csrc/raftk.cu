@@ -557,7 +557,7 @@ static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_
     P.plan = plan; P.plan_stride = pl.blob;
     if (!(o->flags & RAFTK_SOLVE_REUSE_PLAN)) {
         ProfScope ps(st, 0);
-        const size_t psm = (3 * (size_t)d->max_nodes + d->max_members) * sizeof(double) + (2 * (size_t)d->max_nodes + 2 * d->max_members) * sizeof(int);
+        const size_t psm = (3 * (size_t)d->max_nodes + d->max_members) * sizeof(double) + 2 * (size_t)d->max_members * sizeof(int);
         k_fused_plan<<<d->n_designs, 128, psm, st>>>(D, plan, pl.blob, pl.maxW, pl.maxH, pl.maxZ, pl.nwl);
         g_launches++;
     }

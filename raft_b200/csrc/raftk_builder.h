@@ -189,7 +189,8 @@ static int build_member(const raftk_family_member &M, int d, double rho, double 
     return 0;
 }
 
-// greedy first-occurrence class counts of one design (solver.DesignBatch._step_classes)
+// step-class counts of one design by the fused kernels' rule (raftk_fused.cuh step_classes_warp): greedy in node order,
+// a key joins the first class within the tolerance of its own key, else opens one (solver.DesignBatch._step_classes)
 static void count_classes(const std::vector<MemberOut> &mem, int &nW, int &nH, int &nZ)
 {
     std::vector<double> wk, hk, zk;
@@ -197,20 +198,20 @@ static void count_classes(const std::vector<MemberOut> &mem, int &nW, int &nH, i
         if (M.nodes.empty()) continue;
         const double z0 = M.rA[2] + M.nodes[0].ls * M.q[2];
         bool seen = false;
-        for (double a : zk) if (std::fabs(a - z0) <= 1e-12 * std::fmax(1.0, std::fabs(z0))) { seen = true; break; }
+        for (double a : zk) if (std::fabs(a - z0) <= Z0_RTOL * std::fmax(1.0, std::fabs(z0))) { seen = true; break; }
         if (!seen) zk.push_back(z0);
         for (size_t j = 1; j < M.nodes.size(); j++) {
             const double step = M.nodes[j].ls - M.nodes[j - 1].ls;
             const double kx = M.q[0] * step, ky = M.q[1] * step, kz = M.q[2] * step;
-            if (std::fabs(kx) > 1e-14 || std::fabs(ky) > 1e-14) {
-                const double tol = 1e-11 * (std::fabs(kx) + std::fabs(ky));
+            if (std::fabs(kx) > STEP_ZERO || std::fabs(ky) > STEP_ZERO) {
+                const double tol = STEP_RTOL * (std::fabs(kx) + std::fabs(ky));
                 bool s2 = false;
                 for (size_t x = 0; x + 1 < wk.size(); x += 2) if (std::fabs(wk[x] - kx) <= tol && std::fabs(wk[x + 1] - ky) <= tol) { s2 = true; break; }
                 if (!s2) { wk.push_back(kx); wk.push_back(ky); }
             }
-            if (std::fabs(kz) > 1e-14) {
+            if (std::fabs(kz) > STEP_ZERO) {
                 bool s3 = false;
-                for (double a : hk) if (std::fabs(a - kz) <= 1e-11 * std::fabs(kz)) { s3 = true; break; }
+                for (double a : hk) if (std::fabs(a - kz) <= STEP_RTOL * std::fabs(kz)) { s3 = true; break; }
                 if (!s3) hk.push_back(kz);
             }
         }

@@ -7,6 +7,13 @@
 #define SOLVE_THREADS 128
 #define CHUNK_NODES 10          // nodes per register-accumulator chunk in the RMS pass (3*10 <= 32)
 #define MEM_STRIDE 24           // doubles per member in shared memory
+// step classes of the fused solvers (DESIGN.md section 5): node spacings whose keys agree to STEP_RTOL (relative to the
+// node's own key) share one set of factors; a key at or below STEP_ZERO in every component is no step (identity row).
+// First-node depths agree to Z0_RTOL * max(1, |z0|).  The host-side hints (solver.py, batch_builder.py,
+// raftk_builder.h) count with the same constants.
+#define STEP_RTOL 5e-14
+#define STEP_ZERO 1e-14
+#define Z0_RTOL 1e-12
 
 struct DesignsDev {
     int nD, nw, max_nodes, max_members, n_bem_head;

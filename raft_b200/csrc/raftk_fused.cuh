@@ -45,8 +45,56 @@ struct FusedParams {
 struct FSmem {
     double *mem, *node, *coef, *msum, *mat, *warp_part, *sums, *tot, *xi, *f0, *ckpt, *wkey, *hkey, *zkey, *scr, *trans;
     double2 *ebase, *abase, *wtab, *htab;
-    int *imem, *node_w, *node_h, *iscr, *cnt;
+    int *imem, *node_w, *node_h, *cnt;
 };
+
+// The class of one key (NC = 2: (kx, ky) at keys[2c]; NC = 1: x at keys[c]) among the n classes so far, called by all 32
+// lanes of one warp with the same arguments: the FIRST class c with |key_c - key| <= tol in every component, else a new
+// class keyed by this key (lane 0 stores it), else -- n == maxn -- class 0 and over = 1.  The lanes compare 32 classes at once.
+template <int NC>
+__device__ __forceinline__ int warp_step_class(double *keys, int &n, int maxn, double x, double y, double tol, int &over)
+{
+    const int lane = threadIdx.x & 31;
+    for (int b = 0; b < n; b += 32) {
+        const int c = b + lane;
+        const bool hit = c < n && fabs(keys[NC * c] - x) <= tol && (NC == 1 || fabs(keys[NC * c + NC - 1] - y) <= tol);
+        const unsigned m = __ballot_sync(0xffffffffu, hit);
+        if (m) return b + __ffs(m) - 1;
+    }
+    if (n == maxn) { over = 1; return 0; }
+    if (lane == 0) { keys[NC * n] = x; if (NC == 2) keys[NC * n + NC - 1] = y; }
+    __syncwarp();
+    return n++;
+}
+
+// Step classes of one design (DESIGN.md section 5), by ONE warp: greedy in node order, each node joins the first class
+// whose key is within STEP_RTOL of the node's own key or opens a new one (then members' first-node depths likewise).
+// Whether a node opens a class depends on every earlier node's, so nodes are taken one at a time; this is the rule the
+// host-side hints count (solver.DesignBatch._step_classes, batch_builder._count_classes, raftk_builder.h count_classes),
+// so a hint equal to that count never overflows.  Keys per node: kx[j], ky[j], kz[j] (0 at a member's first node);
+// z0[m * z0_stride].  Writes the class keys, node_w / node_h = class * nwl (maxW / maxH * nwl: identity row, no step),
+// imem[IMEM_STRIDE m + 4] = z class, cnt = {nW, nH, overflow, nZ}; overflow (a class past maxW / maxH / maxZ) means
+// RAFTK_FLAG_PLAN: the unit runs no pass.
+__device__ __forceinline__ void step_classes_warp(const double *kx, const double *ky, const double *kz, int Ns, const double *z0,
+                                               int z0_stride, int Nm, int maxW, int maxH, int maxZ, int nwl, double *wkey,
+                                               double *hkey, double *zkey, int *node_w, int *node_h, int *imem, int *cnt)
+{
+    const int lane = threadIdx.x & 31;
+    int nW = 0, nH = 0, nZ = 0, over = 0;
+    for (int j = 0; j < Ns; j++) {
+        const double x = kx[j], y = ky[j], z = kz[j];
+        int wi = maxW, hi = maxH;
+        if (fabs(x) > STEP_ZERO || fabs(y) > STEP_ZERO) wi = warp_step_class<2>(wkey, nW, maxW, x, y, STEP_RTOL * (fabs(x) + fabs(y)), over);
+        if (fabs(z) > STEP_ZERO) hi = warp_step_class<1>(hkey, nH, maxH, z, 0.0, STEP_RTOL * fabs(z), over);
+        if (lane == 0) { node_w[j] = wi * nwl; node_h[j] = hi * nwl; }
+    }
+    for (int m = 0; m < Nm; m++) {
+        const double z = z0[(size_t)m * z0_stride];
+        const int zi = warp_step_class<1>(zkey, nZ, maxZ, z, 0.0, Z0_RTOL * fmax(1.0, fabs(z)), over);
+        if (lane == 0) imem[IMEM_STRIDE * m + 4] = zi;
+    }
+    if (lane == 0) { cnt[0] = nW; cnt[1] = nH; cnt[2] = over; cnt[3] = nZ; }
+}
 
 __host__ __device__ inline size_t fused_smem_bytes(int Nm, int NsP, int nchunk, int nwarps, int nwl, int maxW, int maxH, int maxZ, bool f0_smem)
 {
@@ -128,8 +176,7 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
         S.imem = reinterpret_cast<int *>(p);
         S.node_w = S.imem + (size_t)NmP * IMEM_STRIDE;     // per node: offset (class * nwl) of its step factors,
         S.node_h = S.node_w + NsP + 12;                     // identity row for a member's first node / zero steps
-        S.iscr = S.node_h + NsP + 12;       // 2*NsP ints   (+12: the node loop prefetches up to 10 entries ahead)
-        S.cnt = S.iscr + 2 * NsP;
+        S.cnt = S.node_h + NsP + 12;        // (+12: the node loop prefetches up to 10 entries ahead)
     }
     const int sums_stride = nchunk * 32 + 2;
 
@@ -137,7 +184,6 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
     const double beta = Cs.beta_deg[c] * (CUDART_PI / 180.0);
     double sb, cb;
     sincos(beta, &sb, &cb);
-    if (tid < 4) S.cnt[tid] = 0;
     for (int m = tid; m < Nm; m += T) {
         const double *fr = D.mem_frame + 9 * (m0 + m);
         const double *arm = D.mem_arm + 3 * (m0 + m);
@@ -169,8 +215,7 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
         S.mat[72 + t] = D.C0[(size_t)d * 36 + t];
     }
     __syncthreads();
-    // ---- step classes, built in parallel (thread per node / member) -----------------------------------
-    // A: keys per node
+    // ---- step classes: keys per node in parallel, classes by one warp (step_classes_warp) --------------
     for (int j = tid; j < Ns; j += T) {
         int m = 0;
         while (j >= S.imem[IMEM_STRIDE * m + 1]) m++;
@@ -183,55 +228,10 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
         S.scr[j] = kx; S.scr[NsP + j] = ky; S.scr[2 * NsP + j] = kz;
     }
     __syncthreads();
-    // B: representative (first node with the same key)
-    for (int j = tid; j < Ns; j += T) {
-        const double kx = S.scr[j], ky = S.scr[NsP + j], kz = S.scr[2 * NsP + j];
-        int rw = -1, rh = -1;
-        if (fabs(kx) > 1e-14 || fabs(ky) > 1e-14) {
-            const double tol = 1e-11 * (fabs(kx) + fabs(ky));
-            rw = j;
-            for (int x = 0; x < j; x++)
-                if (fabs(S.scr[x] - kx) <= tol && fabs(S.scr[NsP + x] - ky) <= tol) { rw = x; break; }
-        }
-        if (fabs(kz) > 1e-14) {
-            const double tol = 1e-11 * fabs(kz);
-            rh = j;
-            for (int x = 0; x < j; x++)
-                if (fabs(S.scr[2 * NsP + x] - kz) <= tol) { rh = x; break; }
-        }
-        S.iscr[j] = rw; S.iscr[NsP + j] = rh;
-    }
-    __syncthreads();
-    // C: class id = rank of the representative among representatives
-    for (int j = tid; j < Ns; j += T) {
-        const int rw = S.iscr[j], rh = S.iscr[NsP + j];
-        int wi = -1, hi = -1;
-        if (rw >= 0) { wi = 0; for (int x = 0; x < rw; x++) wi += (S.iscr[x] == x); }
-        if (rh >= 0) { hi = 0; for (int x = 0; x < rh; x++) hi += (S.iscr[NsP + x] == x); }
-        if (wi >= P.maxW) { wi = 0; S.cnt[2] = 1; }
-        if (hi >= P.maxH) { hi = 0; S.cnt[2] = 1; }
-        if (rw == j && wi >= 0 && S.cnt[2] == 0) { S.wkey[2 * wi] = S.scr[j]; S.wkey[2 * wi + 1] = S.scr[NsP + j]; atomicMax(&S.cnt[0], wi + 1); }
-        if (rh == j && hi >= 0 && S.cnt[2] == 0) { S.hkey[hi] = S.scr[2 * NsP + j]; atomicMax(&S.cnt[1], hi + 1); }
-        S.node_w[j] = (wi >= 0 ? wi : P.maxW) * nwl;        // identity row when the phase / depth does not change
-        S.node_h[j] = (hi >= 0 ? hi : P.maxH) * nwl;
-    }
+    if (warp == 0)
+        step_classes_warp(S.scr, S.scr + NsP, S.scr + 2 * NsP, Ns, S.mem + 21, MEM_STRIDE, Nm, P.maxW, P.maxH, P.maxZ, nwl,
+                          S.wkey, S.hkey, S.zkey, S.node_w, S.node_h, S.imem, S.cnt);
     for (int j = Ns + tid; j < NsP + 12; j += T) { S.node_w[j] = P.maxW * nwl; S.node_h[j] = P.maxH * nwl; }   // prefetch padding
-    // z classes of the members' first nodes
-    for (int m = tid; m < Nm; m += T) {
-        const double z0 = S.mem[m * MEM_STRIDE + 21];
-        int rep = m;
-        for (int x = 0; x < m; x++) if (fabs(S.mem[x * MEM_STRIDE + 21] - z0) <= 1e-12 * fmax(1.0, fabs(z0))) { rep = x; break; }
-        int zi = 0;
-        for (int x = 0; x < rep; x++) {
-            const double zx = S.mem[x * MEM_STRIDE + 21];
-            bool first = true;
-            for (int y = 0; y < x; y++) if (fabs(S.mem[y * MEM_STRIDE + 21] - zx) <= 1e-12 * fmax(1.0, fabs(zx))) { first = false; break; }
-            zi += first;
-        }
-        if (zi >= P.maxZ) { zi = 0; S.cnt[2] = 1; }
-        if (rep == m && S.cnt[2] == 0) { S.zkey[zi] = z0; atomicMax(&S.cnt[3], zi + 1); }
-        S.imem[IMEM_STRIDE * m + 4] = zi;
-    }
     __syncthreads();
     const int nW = S.cnt[0], nH = S.cnt[1], nZ = S.cnt[3];
     const bool plan_overflow = S.cnt[2] != 0;
@@ -343,9 +343,11 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
             else { S.xi[(2 * a) * nwl + t] = P.xi_start; S.xi[(2 * a + 1) * nwl + t] = 0.0; }
         }
     }
-    if (plan_overflow) {          // no pass will run: never hand back whatever the output buffer held before
+    if (plan_overflow) {          // no pass will run: never hand back whatever the output buffers held before
         for (int t = tid; t < nloc; t += T)
             for (int a = 0; a < 6; a++) P.Xi_out[ogl + (size_t)a * nw + f_begin + t] = make_double2(0.0, 0.0);
+        if (P.Xilast_out)
+            for (int t = tid; t < 6 * nloc; t += T) P.Xilast_out[ogl + (size_t)(t / nloc) * nw + f_begin + t % nloc] = make_double2(0.0, 0.0);
     }
     __syncthreads();
 

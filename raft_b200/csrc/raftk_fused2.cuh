@@ -52,7 +52,8 @@ __host__ __device__ inline PlanLayout plan_layout(int NmP, int NsP, int maxW, in
 
 // ------------------------------------------------------------------------------------------------
 // k_fused_plan: one CTA per design.  Stages the design's tables and builds the step classes (distinct node spacings
-// (q_x,q_y)*step and q_z*step, distinct first-node depths) exactly as k_rao_fused does per CTA, once, into the blob.
+// (q_x,q_y)*step and q_z*step, distinct first-node depths) with step_classes_warp, as k_rao_fused does per CTA, once, into
+// the blob.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) k_fused_plan(DesignsDev D, double *plan, size_t stride, int maxW, int maxH, int maxZ, int nwl)
 {
@@ -70,10 +71,8 @@ __global__ void __launch_bounds__(128) k_fused_plan(DesignsDev D, double *plan, 
     int *imem = ib + L.i_imem, *node_w = ib + L.i_nodew, *node_h = ib + L.i_nodeh, *node_m = ib + L.i_nodem, *cnt_g = ib + L.i_cnt;
     double *scr = smem_raw;                                   // 3 * NsP key components
     double *z0s = scr + 3 * (size_t)NsP;                      // NmP first-node depths
-    int *iscr = reinterpret_cast<int *>(z0s + NmP);           // 2 * NsP representatives
-    int *mstart = iscr + 2 * NsP;                             // 2 * NmP member node ranges
+    int *mstart = reinterpret_cast<int *>(z0s + NmP);         // 2 * NmP member node ranges
     __shared__ int cnt[4];
-    if (tid < 4) cnt[tid] = 0;
     for (int t = tid; t < L.total; t += T) blob[t] = 0.0;
     __syncthreads();
     for (int m = tid; m < Nm; m += T) {
@@ -128,55 +127,9 @@ __global__ void __launch_bounds__(128) k_fused_plan(DesignsDev D, double *plan, 
         scr[j] = kx; scr[NsP + j] = ky; scr[2 * NsP + j] = kz;
     }
     __syncthreads();
-    // B: representative (first node with the same key)
-    for (int j = tid; j < Ns; j += T) {
-        const double kx = scr[j], ky = scr[NsP + j], kz = scr[2 * NsP + j];
-        int rw = -1, rh = -1;
-        if (fabs(kx) > 1e-14 || fabs(ky) > 1e-14) {
-            const double tol = 1e-11 * (fabs(kx) + fabs(ky));
-            rw = j;
-            for (int x = 0; x < j; x++)
-                if (fabs(scr[x] - kx) <= tol && fabs(scr[NsP + x] - ky) <= tol) { rw = x; break; }
-        }
-        if (fabs(kz) > 1e-14) {
-            const double tol = 1e-11 * fabs(kz);
-            rh = j;
-            for (int x = 0; x < j; x++)
-                if (fabs(scr[2 * NsP + x] - kz) <= tol) { rh = x; break; }
-        }
-        iscr[j] = rw; iscr[NsP + j] = rh;
-    }
-    __syncthreads();
-    // C: class id = rank of the representative among representatives; offsets into the factor tables (class * nwl)
-    for (int j = tid; j < Ns; j += T) {
-        const int rw = iscr[j], rh = iscr[NsP + j];
-        int wi = -1, hi = -1;
-        if (rw >= 0) { wi = 0; for (int x = 0; x < rw; x++) wi += (iscr[x] == x); }
-        if (rh >= 0) { hi = 0; for (int x = 0; x < rh; x++) hi += (iscr[NsP + x] == x); }
-        if (wi >= maxW) { wi = 0; cnt[2] = 1; }
-        if (hi >= maxH) { hi = 0; cnt[2] = 1; }
-        if (rw == j && wi >= 0) { wkey[2 * wi] = scr[j]; wkey[2 * wi + 1] = scr[NsP + j]; atomicMax(&cnt[0], wi + 1); }
-        if (rh == j && hi >= 0) { hkey[hi] = scr[2 * NsP + j]; atomicMax(&cnt[1], hi + 1); }
-        node_w[j] = (wi >= 0 ? wi : maxW) * nwl;             // identity row when the phase / depth does not change
-        node_h[j] = (hi >= 0 ? hi : maxH) * nwl;
-    }
+    if (tid < 32)
+        step_classes_warp(scr, scr + NsP, scr + 2 * NsP, Ns, z0s, 1, Nm, maxW, maxH, maxZ, nwl, wkey, hkey, zkey, node_w, node_h, imem, cnt);
     for (int j = Ns + tid; j < NsP + 12; j += T) { node_w[j] = maxW * nwl; node_h[j] = maxH * nwl; node_m[j] = Nm > 0 ? Nm - 1 : 0; }
-    // z classes of the members' first nodes
-    for (int m = tid; m < Nm; m += T) {
-        const double z0 = z0s[m];
-        int rep = m;
-        for (int x = 0; x < m; x++) if (fabs(z0s[x] - z0) <= 1e-12 * fmax(1.0, fabs(z0))) { rep = x; break; }
-        int zi = 0;
-        for (int x = 0; x < rep; x++) {
-            const double zx = z0s[x];
-            bool first = true;
-            for (int y = 0; y < x; y++) if (fabs(z0s[y] - zx) <= 1e-12 * fmax(1.0, fabs(zx))) { first = false; break; }
-            zi += first;
-        }
-        if (zi >= maxZ) { zi = 0; cnt[2] = 1; }
-        if (rep == m) { zkey[zi] = z0; atomicMax(&cnt[3], zi + 1); }
-        imem[IMEM_STRIDE * m + 4] = zi;
-    }
     // drag-direction masks per chunk of CHUNK_NODES nodes.  The reference's strips carry axial drag only where a member ends
     // or steps (Cd_End, raft_member.py:2098-2117) and transverse drag only where the strip has a length, so most nodes need
     // one or two of the three relative-velocity projections: a direction whose coefficient is exactly zero contributes an
@@ -586,9 +539,11 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
             for (int a = 0; a < 6; a++) P.F0g[ogl + (size_t)a * nw + i] = make_double2(Fr[a], Fi[a]);
         }
     }
-    if (plan_overflow) {
+    if (plan_overflow) {          // no pass will run: never hand back whatever the output buffers held before
         for (int t = tid; t < nloc; t += T)
             for (int a = 0; a < 6; a++) P.Xi_out[ogl + (size_t)a * nw + f_begin + t] = make_double2(0.0, 0.0);
+        if (P.Xilast_out)
+            for (int t = tid; t < 6 * nloc; t += T) P.Xilast_out[ogl + (size_t)(t / nloc) * nw + f_begin + t % nloc] = make_double2(0.0, 0.0);
     }
     __syncthreads();
 

@@ -9,6 +9,7 @@ Two routes, both straight through the C ABI (no CPU fallback anywhere):
   (``raftk_*_dev`` on torch's current stream).  ``bench.py`` times this as ``value``; the sweep
   driver (``raft_b200.sweep``) all-gathers its output tensor over NCCL.
 """
+import copy
 import ctypes as C
 
 import numpy as np
@@ -189,8 +190,10 @@ class DesignBatch:
 
     @staticmethod
     def _step_classes(packed):
-        """Upper bounds on the number of distinct node spacings per design, as the fused kernel
-        deduplicates them (phase classes keyed by (q_x,q_y)*step, depth classes by q_z*step), + slack."""
+        """Step-class hints of the fused solvers: the largest number of classes of any design, counted by the kernels' rule
+        (raftk_fused.cuh step_classes_warp, DESIGN.md section 5): greedy in node order, a key joins the first class whose key
+        is within the tolerance of its own, else opens one.  Phase classes are keyed by (q_x,q_y)*step, depth classes by
+        q_z*step, z classes by the members' first-node depths."""
         mw = mh = mz = 0
         for P in packed:
             wk, hk, zk = [], [], []
@@ -200,16 +203,16 @@ class DesignBatch:
                 ls = np.asarray(P["node_ls"][ms[m]:ms[m + 1]], dtype=float)
                 if len(ls):
                     z0 = float(P["mem_rA"][m][2]) + ls[0] * q[2]
-                    if not any(abs(a - z0) <= 1e-12 * max(1.0, abs(z0)) for a in zk):
+                    if not any(abs(a - z0) <= Z0_RTOL * max(1.0, abs(z0)) for a in zk):
                         zk.append(z0)
                 for step in np.diff(ls):
                     kx, ky, kz = q[0] * step, q[1] * step, q[2] * step
-                    if abs(kx) > 1e-14 or abs(ky) > 1e-14:
-                        tol = 1e-11 * (abs(kx) + abs(ky))
+                    if abs(kx) > STEP_ZERO or abs(ky) > STEP_ZERO:
+                        tol = STEP_RTOL * (abs(kx) + abs(ky))
                         if not any(abs(a - kx) <= tol and abs(b - ky) <= tol for a, b in wk):
                             wk.append((kx, ky))
-                    if abs(kz) > 1e-14:
-                        if not any(abs(a - kz) <= 1e-11 * abs(kz) for a in hk):
+                    if abs(kz) > STEP_ZERO:
+                        if not any(abs(a - kz) <= STEP_RTOL * abs(kz) for a in hk):
                             hk.append(kz)
             mw, mh, mz = max(mw, len(wk)), max(mh, len(hk)), max(mz, len(zk))
         return max(1, mw), max(1, mh), max(1, mz)
@@ -306,15 +309,31 @@ def solve_dynamics(batch, cases, n_iter=10, tol=0.01, xi_start=0.0, cluster_size
     o = RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), 0, 0)
     os_ = _out_struct(outs, lambda a: a.ctypes.data)
     check(lib.raftk_solve_dynamics_host(C.byref(d), C.byref(c), C.byref(o), C.byref(os_)))
-    if np.any(outs["status"][..., 2] & FLAG_PLAN):
-        # the device deduplicated more distinct node spacings than the host-side hint allowed for (near-tolerance
-        # chains): those units ran no pass and hold zeros.  Re-run with worst-case table sizes (hint 0).
-        d = batch.struct(_host_ptr(batch.arrays))                 # a private copy: the cached struct keeps the hints
-        d.max_w_classes = d.max_h_classes = d.max_z_classes = 0
-        check(lib.raftk_solve_dynamics_host(C.byref(d), C.byref(c), C.byref(o), C.byref(os_)))
-        if np.any(outs["status"][..., 2] & FLAG_PLAN):
-            raise _lib.RaftkError("step-class tables overflowed even with worst-case sizes")
+    if _plan_overflowed(outs):
+        check(lib.raftk_solve_dynamics_host(C.byref(_host_struct(worst_case_hints(batch))), C.byref(c), C.byref(o), C.byref(os_)))
+        _raise_on_plan(outs)
     return outs
+
+
+def _plan_overflowed(outs):
+    """Whether a unit came back with RAFTK_FLAG_PLAN: the batch's step-class hints were below the number of classes the
+    kernels count (DesignBatch computes them by the kernels' rule, so only hints set by the caller can be), and those
+    units ran no pass and hold zeros."""
+    return bool(np.any(np.asarray(outs["status"])[..., 2] & FLAG_PLAN))
+
+
+def worst_case_hints(batch):
+    """A shallow copy of ``batch`` with the step-class hints at 0: the fused solvers then size their class tables for one
+    class per node, which cannot overflow.  ``batch`` keeps its hints."""
+    b = copy.copy(batch)
+    b.max_w_classes = b.max_h_classes = b.max_z_classes = 0
+    b.__dict__.pop("_host_struct_cache", None)
+    return b
+
+
+def _raise_on_plan(outs):
+    if _plan_overflowed(outs):
+        raise _lib.RaftkError("step-class tables overflowed even with worst-case sizes")
 
 
 def solve_dynamics_farm(batch, cases, C_arr=None, M_arr=None, B_arr=None, n_iter=10, tol=0.01, xi_start=0.0, cluster_size=0,
@@ -354,10 +373,14 @@ def solve_dynamics_farm(batch, cases, C_arr=None, M_arr=None, B_arr=None, n_iter
     o = RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), 0, 0)
     os_ = _out_struct(outs, lambda a: a.ctypes.data)
     check(lib.raftk_solve_dynamics_farm_host(C.byref(d), C.byref(c), C.byref(o), C.byref(os_), C.byref(f)))
+    if _plan_overflowed(outs):                      # Xi_sys was assembled from those units' zero loads: solve it all again
+        check(lib.raftk_solve_dynamics_farm_host(C.byref(_host_struct(worst_case_hints(batch))), C.byref(c), C.byref(o), C.byref(os_), C.byref(f)))
+        _raise_on_plan(outs)
     return outs
 
 
 FLAG_NAN, FLAG_SINGULAR, FLAG_PLAN, FLAG_XCHG = 1, 2, 4, 8        # include/raftk.h RAFTK_FLAG_*
+STEP_RTOL, STEP_ZERO, Z0_RTOL = 5e-14, 1e-14, 1e-12                # step-class tolerances (csrc/raftk_common.cuh)
 
 
 def raise_on_flags(status):

@@ -136,8 +136,13 @@ def build_variants_batched(base_design, base_matrices, factors, nw, max_freq, de
 def solve_sweep(packed_designs, cases, n_iter=10, tol=0.01, xi_start=0.0, device=None, group=None, n_total=None):
     """Solve this rank's designs on its GPU and all-gather the RAOs: -> (Xi [n_total,nC,6,nw], status [n_total,nC,4])."""
     from . import solver
-    sess = solver.DeviceSession(solver.DesignBatch(packed_designs), solver.CaseTable(cases), device=device)
-    out = sess.solve(n_iter=n_iter, tol=tol, xi_start=xi_start)
+    batch, ct = solver.DesignBatch(packed_designs), solver.CaseTable(cases)
+    out = solver.DeviceSession(batch, ct, device=device).solve(n_iter=n_iter, tol=tol, xi_start=xi_start)
+    if bool(((out["status"][..., 2] & solver.FLAG_PLAN) != 0).any()):
+        # units whose step classes overflowed the hints ran no pass and hold zeros: solve again with worst-case tables
+        out = solver.DeviceSession(solver.worst_case_hints(batch), ct, device=device).solve(n_iter=n_iter, tol=tol, xi_start=xi_start)
+        if bool(((out["status"][..., 2] & solver.FLAG_PLAN) != 0).any()):
+            raise solver._lib.RaftkError("step-class tables overflowed even with worst-case sizes")
     n_total = len(packed_designs) if n_total is None else n_total
     return all_gather_blocks(out["Xi"], n_total, group), all_gather_blocks(out["status"], n_total, group)
 
