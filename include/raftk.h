@@ -322,6 +322,44 @@ int raftk_qtf_slender_dev(const raftk_slender *s, int32_t n_cases, const double 
 int raftk_qtf_slender_host(const raftk_slender *s, int32_t n_cases, const double *beta_rad, const double *Xi_rao, double *qtf);
 
 /*
+ * Model.solveDynamics with potSecOrder 1 (raft_model.py:1052-1142) for every (design, case), in one call on one stream:
+ * loop A (the plain solve) -> motion RAOs of the units whose loop A converged, interpolated onto the second-order grid
+ * (helpers.getRAO + np.interp, same bits) -> slender-body QTF per unit (the kernels of raftk_qtf_slender_*, same bits per
+ * design) -> second-order force (qtf_shared = 2, one heading) -> loop B from loop A's last iterate (cases.Xi_init) with the
+ * force added (cases.F_2nd) and n_iter - 1 -> merge.  Units whose loop A did not converge keep loop A's outputs and get zero
+ * F_2nd, F_2nd_mean and qtf; elsewhere passes add up and the flags are OR-ed.  No host synchronisation.
+ *
+ * raftk_slender_batch: the raftk_slender tables of nD designs on ONE second-order grid, concatenated in design order.  cols.n_nodes /
+ * n_members / n_seg are the totals; design d owns nodes node_offset[d] .. node_offset[d+1]-1 (likewise members, segments);
+ * cols.mem_node_start holds each design's own [n_members_d + 1] starts (n_members_total + n_designs entries); seg_mem indexes the
+ * design's own members; cols.M_struc is [nD,36].  max_*: the largest per-design counts (at least every design's).
+ * raftk_slender_outputs (may be NULL): qtf complex [nD,nC,nw2,nw2,6] and Xi_rao complex [nD,nC,6,nw2], both optional;
+ * qtf_chunk: units whose QTF tables are built at once in the workspace (0: all; at most 65535 per chunk).  Each unit's QTF
+ * takes 96 nw2^2 bytes and its tables 16 nw2 (22 max_nodes + 10 max_members) bytes, so large batches want a chunk.
+ * The designs must not carry an external QTF; cases.primary, F_2nd and Xi_init must be NULL; n_iter >= 1.  The second-order
+ * force's tile kernel sums with atomics: the last bits of F_2nd, and so of loop B, vary run to run (RAFTK_QTF_DIAG=1: fixed).
+ */
+typedef struct raftk_slender_batch {
+    int32_t n_designs, max_nodes, max_members, max_seg;
+    const int32_t *node_offset, *member_offset, *seg_offset;   /* [n_designs+1] */
+    raftk_slender cols;
+} raftk_slender_batch;
+
+typedef struct raftk_slender_outputs {
+    double *qtf;                    /* optional complex [nD,nC,nw2,nw2,6]                                     */
+    double *Xi_rao;                 /* optional complex [nD,nC,6,nw2]: the RAOs the QTFs were computed from    */
+    int32_t qtf_chunk;              /* units per QTF chunk, 0 = all                                            */
+    int32_t _pad0;
+} raftk_slender_outputs;
+
+size_t raftk_solve_dynamics_slender_workspace_bytes(const raftk_designs *d, const raftk_slender_batch *s, int32_t n_cases, int32_t qtf_chunk);
+int raftk_solve_dynamics_slender_dev(const raftk_designs *d, const raftk_slender_batch *s, const raftk_cases *c, const raftk_solve_opts *o,
+                                     const raftk_outputs *out, const raftk_slender_outputs *so, void *workspace, size_t workspace_bytes,
+                                     void *stream);
+int raftk_solve_dynamics_slender_host(const raftk_designs *d, const raftk_slender_batch *s, const raftk_cases *c, const raftk_solve_opts *o,
+                                      const raftk_outputs *out, const raftk_slender_outputs *so);
+
+/*
  * Model.solveDynamics for ONE FOWT with generalised degrees of freedom (flexible members, n_dof > 6; raft_fowt.py:1854-1857,
  * 1886-1888, 1913-1929; raft_model.py:1052-1142) and n_cases cases or wave trains.  Every submerged strip node carries the
  * 6 x n_dof block of fowt.T of its structural node (Tn) and its offset from that node (rr; zero on flexible members):

@@ -100,6 +100,16 @@ class RaftkSlender(C.Structure):
                  ("depth", C.c_double), ("rho", C.c_double), ("g", C.c_double)] + [(n, C.c_void_p) for n in SLENDER_ARRAYS])
 
 
+class RaftkSlenderBatch(C.Structure):
+    """include/raftk.h raftk_slender_batch: the slender-body tables of several designs, concatenated (CSR offsets)."""
+    _fields_ = [("n_designs", C.c_int32), ("max_nodes", C.c_int32), ("max_members", C.c_int32), ("max_seg", C.c_int32),
+                ("node_offset", C.c_void_p), ("member_offset", C.c_void_p), ("seg_offset", C.c_void_p), ("cols", RaftkSlender)]
+
+
+class RaftkSlenderOutputs(C.Structure):
+    _fields_ = [("qtf", C.c_void_p), ("Xi_rao", C.c_void_p), ("qtf_chunk", C.c_int32), ("_pad0", C.c_int32)]
+
+
 class RaftkDispatch(C.Structure):
     """include/raftk.h raftk_dispatch: the kernel variant the last call on this thread launched."""
     _fields_ = [(n, C.c_int32) for n in ("family", "kernel", "cluster_size", "bins_per_cta", "threads_per_cta", "f0_global", "direct_d2h",
@@ -139,6 +149,7 @@ SYMBOLS = [
     "raftk_hydro_excitation_host", "raftk_hydro_linearization_host", "raftk_solve_dynamics_host",
     "raftk_second_order_force_dev", "raftk_second_order_force_host",
     "raftk_qtf_slender_workspace_bytes", "raftk_qtf_slender_dev", "raftk_qtf_slender_host",
+    "raftk_solve_dynamics_slender_workspace_bytes", "raftk_solve_dynamics_slender_dev", "raftk_solve_dynamics_slender_host",
     "raftk_general_workspace_bytes", "raftk_general_solve_dynamics_dev", "raftk_general_solve_dynamics_host",
     "raftk_general_fd_workspace_bytes", "raftk_general_solve_dynamics_fd_dev", "raftk_general_solve_dynamics_fd_host",
     "raftk_general_qtf_workspace_bytes", "raftk_general_solve_dynamics_qtf_dev", "raftk_general_solve_dynamics_qtf_host",
@@ -194,6 +205,14 @@ def _load():
     lib.raftk_qtf_slender_host.argtypes = [P(RaftkSlender), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.raftk_qtf_slender_dev.restype = C.c_int
     lib.raftk_qtf_slender_host.restype = C.c_int
+    lib.raftk_solve_dynamics_slender_workspace_bytes.restype = C.c_size_t
+    lib.raftk_solve_dynamics_slender_workspace_bytes.argtypes = [P(RaftkDesigns), P(RaftkSlenderBatch), C.c_int32, C.c_int32]
+    lib.raftk_solve_dynamics_slender_dev.argtypes = [P(RaftkDesigns), P(RaftkSlenderBatch), P(RaftkCases), P(RaftkSolveOpts), P(RaftkOutputs),
+                                                     P(RaftkSlenderOutputs), C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.raftk_solve_dynamics_slender_host.argtypes = [P(RaftkDesigns), P(RaftkSlenderBatch), P(RaftkCases), P(RaftkSolveOpts), P(RaftkOutputs),
+                                                      P(RaftkSlenderOutputs)]
+    lib.raftk_solve_dynamics_slender_dev.restype = C.c_int
+    lib.raftk_solve_dynamics_slender_host.restype = C.c_int
     lib.raftk_general_workspace_bytes.restype = C.c_size_t
     lib.raftk_general_workspace_bytes.argtypes = [P(RaftkGeneral), C.c_int32]
     lib.raftk_general_solve_dynamics_dev.argtypes = [P(RaftkGeneral), P(RaftkCases), P(RaftkSolveOpts), C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]

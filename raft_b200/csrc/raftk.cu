@@ -1183,17 +1183,11 @@ public:
     }
 };
 
-static int host_run(const char *who, const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
-                    const double *Xi_in, int mode, const raftk_farm *farm = nullptr)
+// the design and case tables of a host call (dd, cc: copies of *d, *c whose pointers commit() turns into device addresses)
+static void stage_designs_cases(Staging &S, const raftk_designs *d, const raftk_cases *c, raftk_designs &dd, raftk_cases &cc)
 {
-    disp_reset();
-    int rc = validate(d, c);
-    if (rc) return rc;
-    if (!out) return set_err(RAFTK_EINVAL, "null outputs");
-    Staging S(who);
     const size_t nD = d->n_designs, nw = d->nw, nC = c->n_cases, Nm = d->n_members_total, Ns = d->n_nodes_total;
     const size_t nR = nD * nC * 6 * nw * 2;             // doubles of one complex [nD,nC,6,nw] array
-    raftk_designs dd = *d;
     S.in(dd.w, d->w, nw); S.in(dd.k, d->k, nw);
     S.in(dd.member_offset, d->member_offset, nD + 1);
     S.in(dd.mem_frame, d->mem_frame, Nm * 9); S.in(dd.mem_rA, d->mem_rA, Nm * 3); S.in(dd.mem_arm, d->mem_arm, Nm * 3);
@@ -1210,7 +1204,6 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
         S.in(dd.X_BEM, d->X_BEM, nD * d->n_bem_head * 6 * nw * 2);
         S.in(dd.bem_xyh, d->bem_xyh, nD * 3);
     }
-    raftk_cases cc = *c;
     S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
     S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC);
     S.in(cc.zeta, c->zeta, nC * nw);
@@ -1222,6 +1215,21 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
         S.in(dd.qtf_heads, d->qtf_heads, (size_t)d->n_qtf_head);
         S.in(dd.qtf, d->qtf, (d->qtf_shared == 1 ? 1 : (d->qtf_shared == 2 ? nD * nC : nD)) * (size_t)d->n_qtf_w * d->n_qtf_w * d->n_qtf_head * 12);
     }
+}
+
+static int host_run(const char *who, const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
+                    const double *Xi_in, int mode, const raftk_farm *farm = nullptr)
+{
+    disp_reset();
+    int rc = validate(d, c);
+    if (rc) return rc;
+    if (!out) return set_err(RAFTK_EINVAL, "null outputs");
+    Staging S(who);
+    const size_t nD = d->n_designs, nw = d->nw, nC = c->n_cases;
+    const size_t nR = nD * nC * 6 * nw * 2;             // doubles of one complex [nD,nC,6,nw] array
+    raftk_designs dd = *d;
+    raftk_cases cc = *c;
+    stage_designs_cases(S, d, c, dd, cc);
     const double *Xi_in_d = nullptr;
     S.in(Xi_in_d, Xi_in, nR);
     raftk_farm fd;
@@ -1619,6 +1627,33 @@ static int validate_slender(const raftk_slender *s, int32_t n_cases)
     return 0;
 }
 
+static SlenderDev slender_dev(const raftk_slender *s)
+{
+    SlenderDev D;
+    D.n_nodes = s->n_nodes; D.n_members = s->n_members; D.n_seg = s->n_seg; D.nw = s->nw;
+    D.depth = s->depth; D.rho = s->rho; D.g = s->g;
+    D.mem_q = s->mem_q; D.mem_p1 = s->mem_p1; D.mem_p2 = s->mem_p2; D.mem_mcf = s->mem_mcf; D.mem_wl = s->mem_wl;
+    D.mem_r_int = s->mem_r_int; D.mem_a_wl = s->mem_a_wl; D.mem_rwl = s->mem_rwl; D.mem_R_wl = s->mem_R_wl;
+    D.mem_node_start = s->mem_node_start; D.node_r = s->node_r; D.node_v_side = s->node_v_side;
+    D.node_Ca_p1 = s->node_Ca_p1; D.node_Ca_p2 = s->node_Ca_p2; D.node_Ca_End = s->node_Ca_End; D.node_v_end = s->node_v_end; D.node_a_i = s->node_a_i;
+    D.seg_mem = s->seg_mem; D.seg_z1 = s->seg_z1; D.seg_z2 = s->seg_z2; D.seg_R = s->seg_R; D.seg_rmid = s->seg_rmid;
+    D.M_struc = s->M_struc; D.w = s->w; D.k = s->k;
+    return D;
+}
+
+// QTFs of `units` units (L.u0 ..) into qtf [units][nw][nw][6]: tables, pairs, Hermitian fill
+static int slender_launch(const SlenderDev &D, const SlenderLaunch &L, int units, const double *beta_rad, const cx *X, cx *Tn, cx *Tm, cx *Th,
+                          cx *Q, cudaStream_t st)
+{
+    k_slender_tables<<<dim3(L.maxN + 2 * L.maxM + L.maxS, units), SL_THREADS, 0, st>>>(D, L, beta_rad, X, Tn, Tm, Th);
+    const unsigned npairs = (unsigned)((size_t)D.nw * (D.nw + 1) / 2);
+    k_slender_pairs<<<dim3(npairs, units), SL_THREADS, 0, st>>>(D, L, beta_rad, X, Tn, Tm, Th, Q);
+    k_slender_fill<<<dim3(D.nw, units), 64, 0, st>>>(D.nw, Q);
+    g_launches += 3;
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
 extern "C" size_t raftk_qtf_slender_workspace_bytes(const raftk_slender *s, int32_t n_cases)
 {
     if (!s || n_cases <= 0) return 0;
@@ -1634,28 +1669,15 @@ extern "C" int raftk_qtf_slender_dev(const raftk_slender *s, int32_t n_cases, co
     if (rc) return rc;
     if (!beta_rad || !Xi_rao || !qtf) return set_err(RAFTK_EINVAL, "slender-body QTF: null beta / Xi_rao / qtf");
     if (!workspace || workspace_bytes < raftk_qtf_slender_workspace_bytes(s, n_cases)) return set_err(RAFTK_ENOMEM, "slender-body QTF: workspace too small");
-    SlenderDev D;
-    D.n_nodes = s->n_nodes; D.n_members = s->n_members; D.n_seg = s->n_seg; D.nw = s->nw;
-    D.depth = s->depth; D.rho = s->rho; D.g = s->g;
-    D.mem_q = s->mem_q; D.mem_p1 = s->mem_p1; D.mem_p2 = s->mem_p2; D.mem_mcf = s->mem_mcf; D.mem_wl = s->mem_wl;
-    D.mem_r_int = s->mem_r_int; D.mem_a_wl = s->mem_a_wl; D.mem_rwl = s->mem_rwl; D.mem_R_wl = s->mem_R_wl;
-    D.mem_node_start = s->mem_node_start; D.node_r = s->node_r; D.node_v_side = s->node_v_side;
-    D.node_Ca_p1 = s->node_Ca_p1; D.node_Ca_p2 = s->node_Ca_p2; D.node_Ca_End = s->node_Ca_End; D.node_v_end = s->node_v_end; D.node_a_i = s->node_a_i;
-    D.seg_mem = s->seg_mem; D.seg_z1 = s->seg_z1; D.seg_z2 = s->seg_z2; D.seg_R = s->seg_R; D.seg_rmid = s->seg_rmid;
-    D.M_struc = s->M_struc; D.w = s->w; D.k = s->k;
-    cudaStream_t st = (cudaStream_t)stream;
-    cx *Tn = static_cast<cx *>(workspace);
-    cx *Tm = reinterpret_cast<cx *>(static_cast<char *>(workspace) + align_up((size_t)n_cases * std::max(s->n_nodes, 1) * s->nw * SL_NODE_C * sizeof(cx), 256));
+    SlenderLaunch L;
+    L.node_off = L.mem_off = L.seg_off = nullptr;
+    L.nC = n_cases; L.u0 = 0; L.d0 = 0; L.maxN = s->n_nodes; L.maxM = s->n_members; L.maxS = s->n_seg;
+    char *ws = static_cast<char *>(workspace);
+    cx *Tn = reinterpret_cast<cx *>(ws);
+    cx *Tm = reinterpret_cast<cx *>(ws + align_up((size_t)n_cases * std::max(s->n_nodes, 1) * s->nw * SL_NODE_C * sizeof(cx), 256));
     cx *Th = reinterpret_cast<cx *>(reinterpret_cast<char *>(Tm) + align_up((size_t)n_cases * s->n_members * s->nw * SL_MEM_C * sizeof(cx), 256));
-    const cx *X = reinterpret_cast<const cx *>(Xi_rao);
-    cx *Q = reinterpret_cast<cx *>(qtf);
-    k_slender_tables<<<dim3(s->n_nodes + 2 * s->n_members + s->n_seg, n_cases), SL_THREADS, 0, st>>>(D, beta_rad, X, Tn, Tm, Th);
-    const unsigned npairs = (unsigned)((size_t)s->nw * (s->nw + 1) / 2);
-    k_slender_pairs<<<dim3(npairs, n_cases), SL_THREADS, 0, st>>>(D, beta_rad, X, Tn, Tm, Th, Q);
-    k_slender_fill<<<dim3(s->nw, n_cases), 64, 0, st>>>(s->nw, Q);
-    g_launches += 3;
-    CUDA_TRY(cudaGetLastError());
-    return RAFTK_OK;
+    return slender_launch(slender_dev(s), L, n_cases, beta_rad, reinterpret_cast<const cx *>(Xi_rao), Tn, Tm, Th, reinterpret_cast<cx *>(qtf),
+                          (cudaStream_t)stream);
 }
 
 extern "C" int raftk_qtf_slender_host(const raftk_slender *s, int32_t n_cases, const double *beta_rad, const double *Xi_rao, double *qtf)
@@ -1686,6 +1708,202 @@ extern "C" int raftk_qtf_slender_host(const raftk_slender *s, int32_t n_cases, c
     S.in(dBeta, beta_rad, nC); S.in(dXi, Xi_rao, nC * 6 * nw * 2); S.out(dQ, nC * nw * nw * 6 * 2, qtf);
     S.buf(ws, wb);
     if ((rc = S.commit()) || (rc = raftk_qtf_slender_dev(&dd, n_cases, dBeta, dXi, dQ, ws, wb, nullptr))) return rc;
+    return S.finish();
+}
+
+// ---- potSecOrder 1: loop A -> RAOs -> slender-body QTF -> second-order force -> loop B, one call -------------------------
+// Workspace: the solve's plan at its head, then loop A's outputs (the merge falls back to them), the RAOs, the second-order
+// force, and one chunk of QTF tables: per unit Tn, Tm and the QTF, plus the Hankel rows of the designs a chunk spans.
+struct SlenderWs { size_t solve, Xi, st, Xl, Bd, Fd, Fi, Fb, zeta, F2, rao, beta, Tn, Tm, Th, Q, total; int chunk; };
+
+static SlenderWs slender_ws(const raftk_designs *d, const raftk_slender_batch *s, int nC, int qtf_chunk)
+{
+    SlenderWs L;
+    const size_t units = (size_t)d->n_designs * nC, nw = d->nw, nw2 = s->cols.nw, R = units * 6 * nw * sizeof(cx);
+    L.chunk = (qtf_chunk <= 0 || (size_t)qtf_chunk > units) ? (int)units : qtf_chunk;
+    const size_t K = L.chunk, span = std::min((size_t)d->n_designs, (K - 1) / nC + 2);
+    size_t o = 0;
+    auto take = [&](size_t bytes) { const size_t at = o; o += align_up(bytes, 256); return at; };
+    L.solve = take(plan_solve(d, nC, 0, WS_UNBOUNDED).bytes);
+    L.Xi = take(R); L.st = take(units * 4 * sizeof(int32_t)); L.Xl = take(R);
+    L.Bd = take(units * 36 * sizeof(double)); L.Fd = take(R); L.Fi = take(R); L.Fb = take(R);
+    L.zeta = take((size_t)nC * nw * sizeof(double));
+    L.F2 = take(units * 6 * nw * sizeof(double));
+    L.rao = take(units * 6 * nw2 * sizeof(cx));
+    L.beta = take((size_t)nC * sizeof(double));
+    L.Tn = take(K * std::max(s->max_nodes, 1) * nw2 * SL_NODE_C * sizeof(cx));
+    L.Tm = take(K * s->max_members * nw2 * SL_MEM_C * sizeof(cx));
+    L.Th = take(span * (s->max_members + s->max_seg) * nw2 * SL_HANK * sizeof(cx));
+    L.Q = take(K * nw2 * nw2 * 6 * sizeof(cx));
+    L.total = o;
+    return L;
+}
+
+static int validate_slender_flow(const raftk_designs *d, const raftk_slender_batch *s, const raftk_cases *c, int qtf_chunk)
+{
+    if (int rc = validate(d, c)) return rc;
+    if (!s || s->n_designs != d->n_designs) return set_err(RAFTK_EINVAL, "slender flow: the slender tables must have one design per design of the batch");
+    if (!s->node_offset || !s->member_offset || !s->seg_offset || s->cols.nw <= 0 || s->max_members <= 0 || s->max_nodes < 0 || s->max_seg < 0)
+        return set_err(RAFTK_EINVAL, "slender flow: offsets, nw > 0 and max_members > 0 are required");
+    if (c->primary) return set_err(RAFTK_EINVAL, "slender flow: potSecOrder 1 takes one wave train per case");
+    if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "slender flow: cases.F_2nd / Xi_init are the flow's own");
+    if (d->n_qtf_w > 0) return set_err(RAFTK_EINVAL, "slender flow: the designs must not carry an external QTF table");
+    if ((size_t)d->nw * 20 > 227 * 1024) return set_err(RAFTK_EINVAL, "nw too large for the second-order force kernel's shared-memory tables");
+    const size_t units = (size_t)d->n_designs * c->n_cases;
+    const size_t K = (qtf_chunk <= 0 || (size_t)qtf_chunk > units) ? units : (size_t)qtf_chunk;
+    if (units > INT32_MAX || K > 65535) return set_err(RAFTK_EINVAL, "slender flow: more than 65535 units per QTF chunk (set qtf_chunk)");
+    return 0;
+}
+
+extern "C" size_t raftk_solve_dynamics_slender_workspace_bytes(const raftk_designs *d, const raftk_slender_batch *s, int32_t n_cases, int32_t qtf_chunk)
+{
+    if (!d || !s || d->n_designs <= 0 || n_cases <= 0 || s->cols.nw <= 0) return 0;
+    return slender_ws(d, s, n_cases, qtf_chunk).total;
+}
+
+extern "C" int raftk_solve_dynamics_slender_dev(const raftk_designs *d, const raftk_slender_batch *s, const raftk_cases *c,
+                                                const raftk_solve_opts *o, const raftk_outputs *out, const raftk_slender_outputs *so,
+                                                void *workspace, size_t workspace_bytes, void *stream)
+{
+    disp_reset();
+    if (!out || !out->Xi || !out->status || !o) return set_err(RAFTK_EINVAL, "Xi, status and opts are required");
+    if (o->n_iter < 1) return set_err(RAFTK_EINVAL, "slender flow: potSecOrder 1 needs n_iter >= 1");
+    const int qtf_chunk = so ? so->qtf_chunk : 0;
+    if (int rc = validate_slender_flow(d, s, c, qtf_chunk)) return rc;
+    const int nD = d->n_designs, nC = c->n_cases, nw = d->nw, nw2 = s->cols.nw, units = nD * nC;
+    const SlenderWs L = slender_ws(d, s, nC, qtf_chunk);
+    if (!workspace || workspace_bytes < L.total) return set_err(RAFTK_ENOMEM, "slender flow: workspace smaller than raftk_solve_dynamics_slender_workspace_bytes()");
+    cudaStream_t st = (cudaStream_t)stream;
+    char *ws = static_cast<char *>(workspace);
+    const size_t solve_bytes = L.Xi - L.solve;
+    // loop A: the plain solve, outputs in the workspace
+    raftk_outputs oA;
+    memset(&oA, 0, sizeof(oA));
+    oA.Xi = reinterpret_cast<double *>(ws + L.Xi); oA.status = reinterpret_cast<int32_t *>(ws + L.st);
+    oA.Xi_last = reinterpret_cast<double *>(ws + L.Xl); oA.zeta = reinterpret_cast<double *>(ws + L.zeta);
+    if (out->B_drag) oA.B_drag = reinterpret_cast<double *>(ws + L.Bd);
+    if (out->F_drag) oA.F_drag = reinterpret_cast<double *>(ws + L.Fd);
+    if (out->F_iner) oA.F_iner = reinterpret_cast<double *>(ws + L.Fi);
+    if (out->F_BEM) oA.F_BEM = reinterpret_cast<double *>(ws + L.Fb);
+    if (int rc = solve(d, c, o, &oA, ws + L.solve, solve_bytes, st)) return rc;
+    // RAOs of the converged units on the second-order grid
+    cx *rao = reinterpret_cast<cx *>(so && so->Xi_rao ? so->Xi_rao : reinterpret_cast<double *>(ws + L.rao));
+    double *beta = reinterpret_cast<double *>(ws + L.beta);
+    k_slender_rao<<<units, 64, 0, st>>>(nC, nw, nw2, d->w, s->cols.w, reinterpret_cast<const cx *>(oA.Xi), oA.zeta, oA.status, c->beta_deg, beta, rao);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    // QTF and second-order force, one chunk of units at a time
+    double *F2 = out->F_2nd ? out->F_2nd : reinterpret_cast<double *>(ws + L.F2);
+    const SlenderDev D = slender_dev(&s->cols);
+    const size_t slab = (size_t)nw2 * nw2 * 6;
+    for (int u0 = 0; u0 < units; u0 += L.chunk) {
+        const int K = std::min(L.chunk, units - u0);
+        SlenderLaunch SL;
+        SL.node_off = s->node_offset; SL.mem_off = s->member_offset; SL.seg_off = s->seg_offset;
+        SL.nC = nC; SL.u0 = u0; SL.d0 = u0 / nC; SL.maxN = s->max_nodes; SL.maxM = s->max_members; SL.maxS = s->max_seg;
+        cx *Q = so && so->qtf ? reinterpret_cast<cx *>(so->qtf) + (size_t)u0 * slab : reinterpret_cast<cx *>(ws + L.Q);
+        if (int rc = slender_launch(D, SL, K, beta, rao + (size_t)u0 * 6 * nw2, reinterpret_cast<cx *>(ws + L.Tn), reinterpret_cast<cx *>(ws + L.Tm),
+                                    reinterpret_cast<cx *>(ws + L.Th), Q, st)) return rc;
+        // the force of the chunk's units, one table per (design, case): whole designs in one launch, a design's partial case
+        // range in one of its own
+        for (int u = u0; u < u0 + K;) {
+            const int c0 = u % nC;
+            const int nd = (c0 == 0 && u + nC <= u0 + K) ? (u0 + K - u) / nC : 1;
+            const int nc = std::min(nC - c0, u0 + K - u);
+            raftk_cases cp;
+            memset(&cp, 0, sizeof(cp));
+            cp.n_cases = nc; cp.Hs = c->Hs + c0; cp.Tp = c->Tp + c0; cp.gamma = c->gamma + c0; cp.beta_deg = c->beta_deg + c0; cp.spec = c->spec + c0;
+            cp.zeta = c->zeta ? c->zeta + (size_t)c0 * nw : nullptr;
+            QtfParams P;
+            P.nD = nd; P.shared = 2; P.n2 = nw2; P.nh = 1; P.nw = nw; P.dw = d->dw;
+            P.w = d->w; P.qw = s->cols.w; P.qh = s->cols.w;                 // one heading: never read
+            P.qtf = reinterpret_cast<const double2 *>(Q + (size_t)(u - u0) * slab);
+            P.F2 = F2 + (size_t)u * 6 * nw;
+            P.F2mean = out->F_2nd_mean ? out->F_2nd_mean + (size_t)u * 6 : nullptr;
+            if (int rc = launch_qtf(P, &cp, st)) return rc;
+            u += nd * nc;
+        }
+    }
+    // loop B: continues from loop A's last iterate with the force added, n_iter - 1 more passes, into the caller's outputs
+    raftk_cases cB = *c;
+    cB.F_2nd = F2; cB.Xi_init = oA.Xi_last;
+    raftk_solve_opts oB = *o;
+    oB.n_iter = o->n_iter - 1; oB.flags |= RAFTK_SOLVE_REUSE_PLAN;        // loop A left the plan in the same workspace
+    raftk_outputs ob = *out;
+    ob.zeta = nullptr; ob.F_2nd = nullptr; ob.F_2nd_mean = nullptr;
+    if (int rc = solve(d, &cB, &oB, &ob, ws + L.solve, solve_bytes, st)) return rc;
+    SlenderMerge M;
+    M.nC = nC; M.nw = nw; M.nw2 = nw2;
+    M.stA = oA.status;
+    M.XiA = reinterpret_cast<const cx *>(oA.Xi); M.XlA = reinterpret_cast<const cx *>(oA.Xi_last);
+    M.FdA = reinterpret_cast<const cx *>(oA.F_drag); M.FiA = reinterpret_cast<const cx *>(oA.F_iner); M.FbA = reinterpret_cast<const cx *>(oA.F_BEM);
+    M.BdA = oA.B_drag; M.zetaA = oA.zeta;
+    M.st = out->status;
+    M.Xi = reinterpret_cast<cx *>(out->Xi); M.Xl = reinterpret_cast<cx *>(out->Xi_last);
+    M.Fd = reinterpret_cast<cx *>(out->F_drag); M.Fi = reinterpret_cast<cx *>(out->F_iner); M.Fb = reinterpret_cast<cx *>(out->F_BEM);
+    M.qtf = so && so->qtf ? reinterpret_cast<cx *>(so->qtf) : nullptr;
+    M.Bd = out->B_drag; M.zeta = out->zeta; M.F2 = out->F_2nd; M.F2m = out->F_2nd_mean;
+    k_slender_merge<<<units, 256, 0, st>>>(M);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_solve_dynamics_slender_host(const raftk_designs *d, const raftk_slender_batch *s, const raftk_cases *c,
+                                                 const raftk_solve_opts *o, const raftk_outputs *out, const raftk_slender_outputs *so)
+{
+    disp_reset();
+    if (!out || !out->Xi || !out->status || !o) return set_err(RAFTK_EINVAL, "Xi, status and opts are required");
+    if (o->n_iter < 1) return set_err(RAFTK_EINVAL, "slender flow: potSecOrder 1 needs n_iter >= 1");
+    const int qtf_chunk = so ? so->qtf_chunk : 0;
+    if (int rc = validate_slender_flow(d, s, c, qtf_chunk)) return rc;
+    Staging S("raftk_solve_dynamics_slender_host");
+    raftk_designs dd = *d;
+    raftk_cases cc = *c;
+    stage_designs_cases(S, d, c, dd, cc);
+    const size_t nD = d->n_designs, nw = d->nw, nC = c->n_cases, nR = nD * nC * 6 * nw * 2, nw2 = s->cols.nw;
+    const size_t Nm = s->cols.n_members, Ns = s->cols.n_nodes, Ng = s->cols.n_seg;
+    raftk_slender_batch sb = *s;
+    raftk_slender &sc = sb.cols;
+    const raftk_slender &h = s->cols;
+    S.in(sb.node_offset, s->node_offset, nD + 1); S.in(sb.member_offset, s->member_offset, nD + 1); S.in(sb.seg_offset, s->seg_offset, nD + 1);
+    S.in(sc.w, h.w, nw2); S.in(sc.k, h.k, nw2);
+    S.in(sc.mem_q, h.mem_q, Nm * 3); S.in(sc.mem_p1, h.mem_p1, Nm * 3); S.in(sc.mem_p2, h.mem_p2, Nm * 3);
+    S.in(sc.mem_mcf, h.mem_mcf, Nm); S.in(sc.mem_wl, h.mem_wl, Nm);
+    S.in(sc.mem_r_int, h.mem_r_int, Nm * 3); S.in(sc.mem_a_wl, h.mem_a_wl, Nm);
+    S.in(sc.mem_rwl, h.mem_rwl, Nm * 3); S.in(sc.mem_R_wl, h.mem_R_wl, Nm);
+    S.in(sc.mem_node_start, h.mem_node_start, Nm + nD);
+    S.in(sc.node_r, h.node_r, Ns * 3); S.in(sc.node_v_side, h.node_v_side, Ns);
+    S.in(sc.node_Ca_p1, h.node_Ca_p1, Ns); S.in(sc.node_Ca_p2, h.node_Ca_p2, Ns);
+    S.in(sc.node_Ca_End, h.node_Ca_End, Ns); S.in(sc.node_v_end, h.node_v_end, Ns);
+    S.in(sc.node_a_i, h.node_a_i, Ns);
+    S.in(sc.seg_mem, h.seg_mem, Ng); S.in(sc.seg_z1, h.seg_z1, Ng); S.in(sc.seg_z2, h.seg_z2, Ng);
+    S.in(sc.seg_R, h.seg_R, Ng); S.in(sc.seg_rmid, h.seg_rmid, Ng * 3);
+    S.in(sc.M_struc, h.M_struc, nD * 36);
+    raftk_outputs od;
+    memset(&od, 0, sizeof(od));
+    S.out(od.Xi, nR, out->Xi);
+    S.out(od.status, nD * nC * 4, out->status);
+    S.out(od.B_drag, out->B_drag ? nD * nC * 36 : 0, out->B_drag);
+    S.out(od.F_drag, out->F_drag ? nR : 0, out->F_drag);
+    S.out(od.F_iner, out->F_iner ? nR : 0, out->F_iner);
+    S.out(od.F_BEM, out->F_BEM ? nR : 0, out->F_BEM);
+    S.out(od.zeta, out->zeta ? nC * nw : 0, out->zeta);
+    S.out(od.F_2nd, out->F_2nd ? nR / 2 : 0, out->F_2nd);
+    S.out(od.F_2nd_mean, out->F_2nd_mean ? nD * nC * 6 : 0, out->F_2nd_mean);
+    S.out(od.Xi_last, out->Xi_last ? nR : 0, out->Xi_last);
+    raftk_slender_outputs sd;
+    memset(&sd, 0, sizeof(sd));
+    sd.qtf_chunk = qtf_chunk;
+    if (so) {
+        S.out(sd.qtf, so->qtf ? nD * nC * nw2 * nw2 * 12 : 0, so->qtf);
+        S.out(sd.Xi_rao, so->Xi_rao ? nD * nC * 6 * nw2 * 2 : 0, so->Xi_rao);
+    }
+    char *ws;
+    const size_t wb = slender_ws(d, s, (int)nC, qtf_chunk).total;
+    S.buf(ws, wb);
+    int rc;
+    if ((rc = S.commit()) || (rc = raftk_solve_dynamics_slender_dev(&dd, &sb, &cc, o, &od, &sd, ws, wb, nullptr))) return rc;
     return S.finish();
 }
 

@@ -195,15 +195,52 @@ struct SlenderDev {
 // ------------------------------------------------------------------------------------------------
 // tables: grid (n_nodes + n_members, n_cases), block SL_THREADS; thread loops over frequencies
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(SL_THREADS) k_slender_tables(SlenderDev D, const double *beta_rad, const cx *Xi /*[nC][6][nw]*/,
-                                                               cx *Tn /*[nC][Ns][nw][22]*/, cx *Tm /*[nC][Nm][nw][10]*/,
-                                                               cx *Th /*[Nm + n_seg][nw][14]*/)
+// One launch over units y = 0 .. gridDim.y-1 of a batch of designs: unit y is (design, case) = divmod(u0 + y, nC).  The
+// design tables are concatenated (CSR: node / member / segment offsets [nD+1]; mem_node_start holds every design's own
+// [n_members+1] starts, so design d's begin at mem_off[d] + d; seg_mem indexes the design's own members).  node_off NULL:
+// one design, D as given.  Per unit the node and member tables are maxN / maxM rows apart; Th holds the Hankel rows of the
+// designs from d0 on, each design's members then its segments.  Every design sees exactly the pointers, counts and loops
+// of a single-design call, so a design's QTF has the same bits whichever batch, chunk or unit offset it is computed in.
+struct SlenderLaunch {
+    const int *node_off, *mem_off, *seg_off;
+    int nC, u0, d0, maxN, maxM, maxS;
+};
+
+__device__ __forceinline__ SlenderDev sl_design(const SlenderDev &D, const SlenderLaunch &L, int d)
 {
-    const int c = blockIdx.y, nw = D.nw;
-    if ((int)blockIdx.x >= D.n_nodes + D.n_members) {
-        // Hankel functions of the Kim & Yue correction: they depend on (radius, frequency) only, not on the pair or the case
-        if (c != 0) return;
-        const int x = blockIdx.x - D.n_nodes - D.n_members;
+    if (!L.node_off) return D;
+    SlenderDev V = D;
+    const int n0 = L.node_off[d], m0 = L.mem_off[d], s0 = L.seg_off[d];
+    V.n_nodes = L.node_off[d + 1] - n0; V.n_members = L.mem_off[d + 1] - m0; V.n_seg = L.seg_off[d + 1] - s0;
+    V.mem_q += 3 * m0; V.mem_p1 += 3 * m0; V.mem_p2 += 3 * m0; V.mem_mcf += m0; V.mem_wl += m0;
+    V.mem_r_int += 3 * m0; V.mem_a_wl += m0; V.mem_rwl += 3 * m0; V.mem_R_wl += m0;
+    V.mem_node_start += m0 + d;
+    V.node_r += 3 * n0; V.node_v_side += n0; V.node_Ca_p1 += n0; V.node_Ca_p2 += n0; V.node_Ca_End += n0; V.node_v_end += n0; V.node_a_i += n0;
+    V.seg_mem += s0; V.seg_z1 += s0; V.seg_z2 += s0; V.seg_R += s0; V.seg_rmid += 3 * s0;
+    V.M_struc += 36 * d;
+    return V;
+}
+
+// first Hankel row of design d in Th
+__device__ __forceinline__ size_t sl_th_row(const SlenderLaunch &L, int d)
+{
+    return L.node_off ? (size_t)(L.mem_off[d] - L.mem_off[L.d0]) + (L.seg_off[d] - L.seg_off[L.d0]) : 0;
+}
+
+__global__ void __launch_bounds__(SL_THREADS) k_slender_tables(SlenderDev D0, SlenderLaunch L, const double *beta_rad /*[nC]*/,
+                                                               const cx *Xi /*[units][6][nw]*/, cx *Tn /*[units][maxN][nw][22]*/,
+                                                               cx *Tm /*[units][maxM][nw][10]*/, cx *Th /*[rows][nw][14]*/)
+{
+    const int y = blockIdx.y, u = L.u0 + y, d = u / L.nC, c = u % L.nC, nw = D0.nw;
+    const SlenderDev D = sl_design(D0, L, d);
+    if ((int)blockIdx.x >= L.maxN + L.maxM) {
+        // Hankel functions of the Kim & Yue correction: they depend on (radius, frequency) only, not on the pair or the case;
+        // the design's first unit of the launch writes them
+        if (y != 0 && c != 0) return;
+        int x = blockIdx.x - L.maxN - L.maxM;
+        if (x < L.maxM) { if (x >= D.n_members) return; }
+        else { x -= L.maxM; if (x >= D.n_seg) return; x += D.n_members; }
+        Th += sl_th_row(L, d) * nw * SL_HANK;
         const bool live = x < D.n_members ? (D.mem_mcf[x] != 0) : (D.mem_mcf[D.seg_mem[x - D.n_members]] != 0);
         const double R = x < D.n_members ? D.mem_R_wl[x] : D.seg_R[x - D.n_members];
         for (int t = threadIdx.x; t < nw * SL_HANK; t += SL_THREADS) {
@@ -213,9 +250,10 @@ __global__ void __launch_bounds__(SL_THREADS) k_slender_tables(SlenderDev D, con
         return;
     }
     const double beta = beta_rad[c], h = D.depth;
-    const cx *X = Xi + (size_t)c * 6 * nw;
-    if ((int)blockIdx.x < D.n_nodes) {
+    const cx *X = Xi + (size_t)y * 6 * nw;
+    if ((int)blockIdx.x < L.maxN) {
         const int j = blockIdx.x;
+        if (j >= D.n_nodes) return;
         int m = 0;
         while (D.mem_node_start[m + 1] <= j) m++;
         const double *r = D.node_r + 3 * j, *q = D.mem_q + 3 * m;
@@ -229,18 +267,19 @@ __global__ void __launch_bounds__(SL_THREADS) k_slender_tables(SlenderDev D, con
             const cx vax = dotr(u - v, q);                      // nodeV_axial_rel, from the FULL node velocity (raft_member.py:1517)
             const c3 gp = sl_grad_pres1st(D.k[i], beta, h, r, D.rho, D.g);
             const c3 vt = v - projq(q, v);                      // transverse node velocity (side effect of getWaveKin_axdivAcc)
-            cx *o = Tn + (((size_t)c * D.n_nodes + j) * nw + i) * SL_NODE_C;
+            cx *o = Tn + (((size_t)y * L.maxN + j) * nw + i) * SL_NODE_C;
             for (int a = 0; a < 3; a++) { o[a] = dr.v[a]; o[3 + a] = vt.v[a]; o[6 + a] = u.v[a]; o[19 + a] = gp.v[a]; }
             for (int a = 0; a < 3; a++) for (int b = 0; b < 3; b++) o[9 + 3 * a + b] = G.a[a][b];
             o[18] = vax;
         }
     } else {
-        const int m = blockIdx.x - D.n_nodes;
+        const int m = blockIdx.x - L.maxN;
+        if (m >= D.n_members) return;
         const double *p1 = D.mem_p1 + 3 * m, *p2 = D.mem_p2 + 3 * m, *r_int = D.mem_r_int + 3 * m;
         for (int i = threadIdx.x; i < nw; i += SL_THREADS) {
             cx X6[6];
             for (int a = 0; a < 6; a++) X6[a] = X[(size_t)a * nw + i];
-            cx *o = Tm + (((size_t)c * D.n_members + m) * nw + i) * SL_MEM_C;
+            cx *o = Tm + (((size_t)y * L.maxM + m) * nw + i) * SL_MEM_C;
             for (int a = 0; a < SL_MEM_C; a++) o[a] = mk(0.0);
             if (D.mem_wl[m]) {                                     // raft_member.py:1524-1539
                 c3 dr, v, acc, u, ud; cx eta;
@@ -384,19 +423,23 @@ __host__ __device__ inline void sl_member_terms(const SlenderDev &D, int m, cons
 }
 
 // ------------------------------------------------------------------------------------------------
-// pairs: grid (nw (nw + 1) / 2, n_cases), block SL_THREADS.  qtf [nC][nw][nw][6], upper triangle i2 >= i1.
+// pairs: grid (nw (nw + 1) / 2, units), block SL_THREADS.  qtf [units][nw][nw][6], upper triangle i2 >= i1.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(SL_THREADS) k_slender_pairs(SlenderDev D, const double *beta_rad, const cx *Xi, const cx *Tn, const cx *Tm,
-                                                              const cx *Th, cx *qtf)
+__global__ void __launch_bounds__(SL_THREADS) k_slender_pairs(SlenderDev D0, SlenderLaunch L, const double *beta_rad, const cx *Xi, const cx *Tn,
+                                                              const cx *Tm, const cx *Th, cx *qtf)
 {
     __shared__ cx part[SL_THREADS][6];
-    const int c = blockIdx.y, nw = D.nw, tid = threadIdx.x;
+    const int y = blockIdx.y, u = L.u0 + y, d = u / L.nC, c = u % L.nC, nw = D0.nw, tid = threadIdx.x;
+    const SlenderDev D = sl_design(D0, L, d);
+    Tn += (size_t)y * L.maxN * nw * SL_NODE_C;
+    Tm += (size_t)y * L.maxM * nw * SL_MEM_C;
+    Th += sl_th_row(L, d) * nw * SL_HANK;
     // pair index -> (i1, i2 >= i1), rows of decreasing length
     int i1 = 0, rem = blockIdx.x;
     while (rem >= nw - i1) { rem -= nw - i1; i1++; }
     const int i2 = i1 + rem;
     const double w1 = D.w[i1], w2 = D.w[i2], k1 = D.k[i1], k2 = D.k[i2], beta = beta_rad[c];
-    const cx *X = Xi + (size_t)c * 6 * nw;
+    const cx *X = Xi + (size_t)y * 6 * nw;
     cx F[6];
     for (int a = 0; a < 6; a++) F[a] = mk(0.0);
     if (!(w2 < w1)) {
@@ -411,13 +454,13 @@ __global__ void __launch_bounds__(SL_THREADS) k_slender_pairs(SlenderDev D, cons
         for (int j = tid; j < D.n_nodes; j += SL_THREADS) {
             int m = 0;
             while (D.mem_node_start[m + 1] <= j) m++;
-            const cx *t1 = Tn + (((size_t)c * D.n_nodes + j) * nw + i1) * SL_NODE_C;
-            const cx *t2 = Tn + (((size_t)c * D.n_nodes + j) * nw + i2) * SL_NODE_C;
+            const cx *t1 = Tn + ((size_t)j * nw + i1) * SL_NODE_C;
+            const cx *t2 = Tn + ((size_t)j * nw + i2) * SL_NODE_C;
             sl_node_terms(D, m, j, t1, t2, O1, O2, w1, w2, k1, k2, beta, F);
         }
         for (int m = tid; m < D.n_members; m += SL_THREADS) {
-            const cx *tm1 = Tm + (((size_t)c * D.n_members + m) * nw + i1) * SL_MEM_C;
-            const cx *tm2 = Tm + (((size_t)c * D.n_members + m) * nw + i2) * SL_MEM_C;
+            const cx *tm1 = Tm + ((size_t)m * nw + i1) * SL_MEM_C;
+            const cx *tm2 = Tm + ((size_t)m * nw + i2) * SL_MEM_C;
             sl_member_terms(D, m, tm1, tm2, Th, i1, i2, w1, w2, k1, k2, beta, F);
         }
         if (tid == 0) {                                           // Pinkster IV: rotation of the first-order forces (raft_fowt.py:2044-2058)
@@ -446,16 +489,115 @@ __global__ void __launch_bounds__(SL_THREADS) k_slender_pairs(SlenderDev D, cons
     if (tid < 6) {                                                // fixed-order reduction over the CTA's threads
         cx s = mk(0.0);
         for (int t = 0; t < SL_THREADS; t++) s = s + part[t][tid];
-        qtf[(((size_t)c * nw + i1) * nw + i2) * 6 + tid] = s;
+        qtf[(((size_t)y * nw + i1) * nw + i2) * 6 + tid] = s;
     }
 }
 
-// Hermitian fill (raft_fowt.py:2068-2070): lower triangle = conj of the upper one.  grid (nw, n_cases), block 64
+// Hermitian fill (raft_fowt.py:2068-2070): lower triangle = conj of the upper one.  grid (nw, units), block 64
 __global__ void __launch_bounds__(64) k_slender_fill(int nw, cx *qtf)
 {
     const int c = blockIdx.y, i2 = blockIdx.x;
     for (int t = threadIdx.x; t < i2 * 6; t += 64) {
         const int i1 = t / 6, a = t % 6;
         qtf[(((size_t)c * nw + i2) * nw + i1) * 6 + a] = cj(qtf[(((size_t)c * nw + i1) * nw + i2) * 6 + a]);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// The potSecOrder 1 flow on the device (raft_model.py:1106-1131): the glue between loop A, the QTF and loop B.
+// ------------------------------------------------------------------------------------------------
+
+// np.interp's complex path (real and imaginary parts separately) of helpers.getRAO's ratio, written with explicitly
+// rounded operations so that no multiply-add is contracted: the bits are NumPy's.  getRAO divides a complex by a real
+// zeta promoted to complex, i.e. NumPy's Smith division with a zero imaginary part.
+__device__ __forceinline__ cx sl_rao(cx x, double z)
+{
+    if (!(fabs(z) > 1e-6)) return mk(0.0);
+    const double rat = __ddiv_rn(0.0, z);
+    const double scl = __ddiv_rn(1.0, __dadd_rn(z, __dmul_rn(0.0, rat)));
+    return mk(__dmul_rn(__dadd_rn(x.x, __dmul_rn(x.y, rat)), scl), __dmul_rn(__dsub_rn(x.y, __dmul_rn(x.x, rat)), scl));
+}
+
+__device__ __forceinline__ double sl_lerp(double x, double x0, double x1, double y0, double y1, double inv_dx)
+{
+    const double slope = __dmul_rn(__dsub_rn(y1, y0), inv_dx);
+    double r = __dadd_rn(__dmul_rn(slope, __dsub_rn(x, x0)), y0);
+    if (isnan(r)) {                                   // NumPy tries the other end, then the flat segment
+        r = __dadd_rn(__dmul_rn(slope, __dsub_rn(x, x1)), y1);
+        if (isnan(r) && y0 == y1) r = y0;
+    }
+    return r;
+}
+
+// Motion RAOs of loop A on the second-order grid (raft_fowt.py:2021-2023, left = right = 0), zero for units whose loop A did
+// not converge; units u < nC also write beta_rad[u] = beta_deg[u] * deg2rad.  grid (units), block 64.
+__global__ void __launch_bounds__(64) k_slender_rao(int nC, int nw, int nw2, const double *w, const double *w2, const cx *Xi /*[units][6][nw]*/,
+                                                    const double *zeta /*[nC][nw]*/, const int *status /*[units][4]*/,
+                                                    const double *beta_deg, double *beta_rad, cx *rao /*[units][6][nw2]*/)
+{
+    const int u = blockIdx.x, c = u % nC;
+    if (u < nC && threadIdx.x == 0) beta_rad[u] = __dmul_rn(beta_deg[u], 0.017453292519943295);
+    const bool ok = status[(size_t)u * 4 + 1] == 1;
+    const cx *X = Xi + (size_t)u * 6 * nw;
+    const double *z = zeta + (size_t)c * nw;
+    for (int t = threadIdx.x; t < 6 * nw2; t += 64) {
+        const int a = t / nw2, i = t % nw2;
+        const double x = w2[i];
+        cx v = mk(0.0);
+        if (ok && !(x > w[nw - 1]) && !(x < w[0])) {
+            int j = 0, hi = nw - 1;                       // largest j with w[j] <= x
+            if (x >= w[hi]) j = hi;
+            else while (hi - j > 1) { const int mid = (j + hi) >> 1; if (w[mid] <= x) j = mid; else hi = mid; }
+            const cx y0 = sl_rao(X[(size_t)a * nw + j], z[j]);
+            if (j == nw - 1 || w[j] == x) v = y0;
+            else {
+                const cx y1 = sl_rao(X[(size_t)a * nw + j + 1], z[j + 1]);
+                const double inv_dx = __ddiv_rn(1.0, __dsub_rn(w[j + 1], w[j]));
+                v = mk(sl_lerp(x, w[j], w[j + 1], y0.x, y1.x, inv_dx), sl_lerp(x, w[j], w[j + 1], y0.y, y1.y, inv_dx));
+            }
+        }
+        rao[((size_t)u * 6 + a) * nw2 + i] = v;
+    }
+}
+
+// Loop B wrote every unit's outputs; where loop A did not converge they take loop A's values (kept in the workspace) and
+// the second-order force and QTF are zero.  Where it did, passes add up and the flags are OR-ed.  Case rows of zeta are
+// loop A's.  grid (units), block 256.
+struct SlenderMerge {
+    int nC, nw, nw2;
+    const int *stA;
+    const cx *XiA, *XlA, *FdA, *FiA, *FbA;
+    const double *BdA, *zetaA;
+    int *st;
+    cx *Xi, *Xl, *Fd, *Fi, *Fb, *qtf;
+    double *Bd, *zeta, *F2, *F2m;
+};
+
+__global__ void __launch_bounds__(256) k_slender_merge(SlenderMerge M)
+{
+    const int u = blockIdx.x, tid = threadIdx.x;
+    const size_t n6 = (size_t)6 * M.nw, o6 = (size_t)u * n6;
+    if (u < M.nC && M.zeta)
+        for (int i = tid; i < M.nw; i += 256) M.zeta[(size_t)u * M.nw + i] = M.zetaA[(size_t)u * M.nw + i];
+    const int *a = M.stA + (size_t)u * 4;
+    int *s = M.st + (size_t)u * 4;
+    if (a[1] == 1) {
+        if (tid == 0) { s[0] = a[0] + s[0]; s[2] = a[2] | s[2]; }
+        return;
+    }
+    if (tid < 4) s[tid] = a[tid];
+    for (size_t t = tid; t < n6; t += 256) {
+        M.Xi[o6 + t] = M.XiA[o6 + t];
+        if (M.Xl) M.Xl[o6 + t] = M.XlA[o6 + t];
+        if (M.Fd) M.Fd[o6 + t] = M.FdA[o6 + t];
+        if (M.Fi) M.Fi[o6 + t] = M.FiA[o6 + t];
+        if (M.Fb) M.Fb[o6 + t] = M.FbA[o6 + t];
+        if (M.F2) M.F2[o6 + t] = 0.0;
+    }
+    if (M.Bd && tid < 36) M.Bd[(size_t)u * 36 + tid] = M.BdA[(size_t)u * 36 + tid];
+    if (M.F2m && tid < 6) M.F2m[(size_t)u * 6 + tid] = 0.0;
+    if (M.qtf) {
+        const size_t nq = (size_t)M.nw2 * M.nw2 * 6;
+        for (size_t t = tid; t < nq; t += 256) M.qtf[(size_t)u * nq + t] = mk(0.0);
     }
 }

@@ -15,7 +15,8 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import RaftkCases, RaftkDesigns, RaftkFarm, RaftkGeneral, RaftkGeneralFd, RaftkGeneralQtf, RaftkOutputs, RaftkSlender, RaftkSolveOpts, check, lib
+from ._lib import (RaftkCases, RaftkDesigns, RaftkFarm, RaftkGeneral, RaftkGeneralFd, RaftkGeneralQtf, RaftkOutputs, RaftkSlender, RaftkSlenderBatch,
+                   RaftkSlenderOutputs, RaftkSolveOpts, check, lib)
 
 _F8 = np.float64
 _I4 = np.int32
@@ -432,19 +433,177 @@ def _slender_struct(P, ptr_of):
     """raftk_slender for a design's ``qs_*`` tables; ``ptr_of(name, array)`` returns the address to store (host or device).
     The kernels find a node's member by scanning ``mem_node_start``, so the nodes of one member must be contiguous and in
     member order: an unsorted ``qs_node_mem`` would silently pair nodes with the wrong members."""
+    start = _slender_node_start(P)
+    s = RaftkSlender()
+    s.n_nodes, s.n_members, s.n_seg, s.nw = int(start[-1]), len(start) - 1, len(P["qs_seg_mem"]), len(P["qs_w"])
+    s.depth, s.rho, s.g = float(P["qs_depth"]), float(P["qs_rho"]), float(P["qs_g"])
+    for name in _lib.SLENDER_ARRAYS:
+        a = start if name == "mem_node_start" else np.asarray(P["qs_" + name])
+        a = np.ascontiguousarray(a, dtype=_I4 if name in _SLENDER_I4 else _F8)
+        setattr(s, name, ptr_of(name, a))
+    return s
+
+
+_SLENDER_I4 = ("mem_mcf", "mem_wl", "mem_node_start", "seg_mem")
+
+
+def _slender_node_start(P):
+    """Each member's first strip node in the design's ``qs_*`` tables ([n_members + 1])."""
     nm = len(P["qs_mem_mcf"])
     node_mem = np.asarray(P["qs_node_mem"], dtype=np.int64)
     if np.any(np.diff(node_mem) < 0) or (len(node_mem) and (node_mem[0] < 0 or node_mem[-1] >= nm)):
         raise ValueError("qs_node_mem must be non-decreasing member indices in [0, %d)" % nm)
-    s = RaftkSlender()
-    s.n_nodes, s.n_members, s.n_seg, s.nw = len(node_mem), nm, len(P["qs_seg_mem"]), len(P["qs_w"])
-    s.depth, s.rho, s.g = float(P["qs_depth"]), float(P["qs_rho"]), float(P["qs_g"])
-    start = np.concatenate([[0], np.cumsum(np.bincount(node_mem, minlength=nm))])
-    for name in _lib.SLENDER_ARRAYS:
-        a = start if name == "mem_node_start" else np.asarray(P["qs_" + name])
-        a = np.ascontiguousarray(a, dtype=_I4 if name in ("mem_mcf", "mem_wl", "mem_node_start", "seg_mem") else _F8)
-        setattr(s, name, ptr_of(name, a))
-    return s
+    return np.concatenate([[0], np.cumsum(np.bincount(node_mem, minlength=nm))])
+
+
+class SlenderBatch:
+    """raftk_slender_batch: the ``qs_*`` tables (``packer.pack_qtf_members``) of several designs on ONE second-order grid,
+    concatenated in design order with node / member / segment offsets; each design keeps its own member-local
+    ``mem_node_start`` and ``seg_mem``."""
+
+    def __init__(self, packed):
+        if isinstance(packed, dict):
+            packed = [packed]
+        P0 = packed[0]
+        qw = np.ascontiguousarray(P0["qs_w"], dtype=_F8)
+        site = tuple(float(P0["qs_" + k]) for k in ("depth", "rho", "g"))
+        cols = {n: [] for n in _lib.SLENDER_ARRAYS if n not in ("w", "k")}
+        offs = dict(node=[0], member=[0], seg=[0])
+        for P in packed:
+            if not np.array_equal(np.asarray(P["qs_w"], dtype=_F8), qw):
+                raise ValueError("all designs of a batch must share the second-order frequency grid")
+            if tuple(float(P["qs_" + k]) for k in ("depth", "rho", "g")) != site:
+                raise ValueError("all designs of a batch must share the water depth, density and g of their second-order tables")
+            start = _slender_node_start(P)
+            for name in cols:
+                a = start if name == "mem_node_start" else P["qs_" + name]
+                cols[name].append(np.asarray(a, dtype=_I4 if name in _SLENDER_I4 else _F8).reshape(-1))
+            offs["node"].append(offs["node"][-1] + int(start[-1]))
+            offs["member"].append(offs["member"][-1] + len(start) - 1)
+            offs["seg"].append(offs["seg"][-1] + len(P["qs_seg_mem"]))
+        self.arrays = {n: np.ascontiguousarray(np.concatenate(v)) for n, v in cols.items()}
+        self.arrays["w"], self.arrays["k"] = qw, np.ascontiguousarray(P0["qs_k"], dtype=_F8)
+        for n, v in offs.items():
+            self.arrays[n + "_offset"] = np.array(v, dtype=_I4)
+        self.n_designs, self.nw2 = len(packed), len(qw)
+        self.depth, self.rho, self.g = site
+        self.max_nodes, self.max_members, self.max_seg = (int(np.diff(offs[n]).max()) for n in ("node", "member", "seg"))
+
+    def struct(self, ptr):
+        """The C struct; ``ptr(name)`` returns the address (host or device) of array ``name``."""
+        s = RaftkSlenderBatch()
+        s.n_designs, s.max_nodes, s.max_members, s.max_seg = self.n_designs, self.max_nodes, self.max_members, self.max_seg
+        s.node_offset, s.member_offset, s.seg_offset = ptr("node_offset"), ptr("member_offset"), ptr("seg_offset")
+        c = s.cols
+        c.n_nodes, c.n_members, c.n_seg = (int(self.arrays[n + "_offset"][-1]) for n in ("node", "member", "seg"))
+        c.nw, c.depth, c.rho, c.g = self.nw2, self.depth, self.rho, self.g
+        for name in _lib.SLENDER_ARRAYS:
+            setattr(c, name, ptr(name))
+        return s
+
+
+def _slender_inputs(packed, cases):
+    """The checks of ``solve_dynamics_slender`` -> (design batch without the second-order tables, slender tables, case table
+    without F_2nd / Xi_init)."""
+    if isinstance(packed, dict):
+        packed = [packed]
+    if "primary" in cases.arrays:
+        raise NotImplementedError("potSecOrder 1 with several wave trains fails in the reference itself (raft_model.py:1229 rebinds Fhydro_2nd)")
+    sb = SlenderBatch(packed)
+    batch = DesignBatch([{k: v for k, v in P.items() if not k.startswith(("qtf", "qs_"))} for P in packed])
+    base = {k: v for k, v in cases.arrays.items() if k not in ("F_2nd", "Xi_init")}
+    return batch, sb, CaseTable(base, zeta=base.get("zeta"))
+
+
+def _slender_shapes(nD, nC, nw, nw2):
+    return dict(Xi=([nD, nC, 6, nw], "c"), status=([nD, nC, 4], "i"), B_drag=([nD, nC, 6, 6], "f"), F_drag=([nD, nC, 6, nw], "c"),
+                F_iner=([nD, nC, 6, nw], "c"), F_BEM=([nD, nC, 6, nw], "c"), zeta=([nC, nw], "f"), F_2nd=([nD, nC, 6, nw], "f"),
+                F_2nd_mean=([nD, nC, 6], "f"), Xi_last=([nD, nC, 6, nw], "c"), qtf=([nD, nC, nw2, nw2, 6], "c"), Xi_rao=([nD, nC, 6, nw2], "c"))
+
+
+def _slender_want(want, shapes):
+    want = tuple(dict.fromkeys(("Xi", "status") + tuple(want)))
+    bad = [k for k in want if k not in shapes]
+    if bad:
+        raise ValueError("unknown outputs %s (known: %s)" % (bad, ", ".join(shapes)))
+    return want
+
+
+def slender_flow_host(packed, cases, n_iter=10, tol=0.01, xi_start=0.0, cluster_size=0, want=("Xi", "status", "B_drag"), qtf_chunk=0):
+    """``solve_dynamics_slender`` in ONE library call (raftk_solve_dynamics_slender_host: the whole flow on the device, host
+    buffers in and out) -> dict of NumPy arrays named as in ``want`` (``SlenderSession``'s names)."""
+    batch, sb, ct = _slender_inputs(packed, cases)
+    if n_iter < 1:
+        raise ValueError("potSecOrder 1 needs nIter >= 1")
+    shapes = _slender_shapes(batch.n_designs, ct.n_cases, batch.nw, sb.nw2)
+    want = _slender_want(want, shapes)
+    dt = dict(c=np.complex128, i=_I4, f=_F8)
+    outs = {k: np.zeros(shapes[k][0], dtype=dt[shapes[k][1]]) for k in want}
+    so = RaftkSlenderOutputs(outs["qtf"].ctypes.data if "qtf" in outs else None, outs["Xi_rao"].ctypes.data if "Xi_rao" in outs else None,
+                             int(qtf_chunk), 0)
+    o = RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), 0, 0)
+    check(lib.raftk_solve_dynamics_slender_host(C.byref(_host_struct(batch)), C.byref(sb.struct(_host_ptr(sb.arrays))), C.byref(_host_struct(ct)),
+                                                C.byref(o), C.byref(_out_struct(outs, lambda a: a.ctypes.data)), C.byref(so)))
+    return outs
+
+
+class SlenderSession:
+    """``solve_dynamics_slender`` (Model.solveDynamics with potSecOrder 1, raft_model.py:1052-1142) with tables, workspace and
+    outputs resident in HBM (torch tensors): ``solve()`` enqueues raftk_solve_dynamics_slender_dev on torch's current stream --
+    loop A, RAOs, slender-body QTF, second-order force, loop B and the merge, with no host synchronisation.  ``want``: the
+    names of ``DeviceSession`` plus F_2nd, F_2nd_mean, Xi_last, qtf [nD,nC,nw2,nw2,6] and Xi_rao [nD,nC,6,nw2].
+    ``qtf_chunk``: units whose QTF tables are built at once in the workspace (0: all); each unit's QTF alone takes
+    96 nw2^2 bytes.  ``farm_response()`` couples the designs as the FOWTs of an array, second-order force included."""
+
+    def __init__(self, packed, cases, device=None, want=("Xi", "status", "B_drag"), qtf_chunk=0):
+        import torch
+        self.torch = torch
+        batch, sb, ct = _slender_inputs(packed, cases)
+        shapes = _slender_shapes(batch.n_designs, ct.n_cases, batch.nw, sb.nw2)
+        self.want = want = _slender_want(want, shapes)
+        self.dev = DeviceSession(batch, ct, device=device, workspace_bytes=0,
+                                 want=tuple(k for k in want if k not in ("Xi_last", "qtf", "Xi_rao")))
+        self.device, self.batch, self.slender = self.dev.device, batch, sb
+        self.d_struct, self.c_struct = self.dev.d_struct, self.dev.c_struct
+        dt = dict(c=torch.complex128, i=torch.int32, f=torch.float64)
+        with torch.cuda.device(self.device):
+            self.st = {k: torch.from_numpy(v).to(self.device) for k, v in sb.arrays.items()}
+            self.s_struct = sb.struct(lambda name: self.st[name].data_ptr())
+            self.out = dict(self.dev.out)
+            for k in ("Xi_last", "qtf", "Xi_rao"):
+                if k in want:
+                    self.out[k] = torch.zeros(shapes[k][0], dtype=dt[shapes[k][1]], device=self.device)
+            self.o_struct = _out_struct(self.out, lambda t: t.data_ptr())
+            ptr = lambda k: self.out[k].data_ptr() if k in self.out else None   # noqa: E731
+            self.so = RaftkSlenderOutputs(ptr("qtf"), ptr("Xi_rao"), int(qtf_chunk), 0)
+            self.workspace_bytes = int(lib.raftk_solve_dynamics_slender_workspace_bytes(C.byref(self.d_struct), C.byref(self.s_struct),
+                                                                                         ct.n_cases, int(qtf_chunk)))
+            self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=self.device)
+        self.qtf_chunk = int(qtf_chunk)
+
+    def solve(self, n_iter=10, tol=0.01, xi_start=0.0, cluster_size=0):
+        """Enqueue the potSecOrder 1 solve of every unit on the current stream; returns the output dict (async)."""
+        if n_iter < 1:
+            raise ValueError("potSecOrder 1 needs nIter >= 1")
+        o = RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), 0, 0)
+        with self.torch.cuda.device(self.device):
+            check(lib.raftk_solve_dynamics_slender_dev(C.byref(self.d_struct), C.byref(self.s_struct), C.byref(self.c_struct), C.byref(o),
+                                                       C.byref(self.o_struct), C.byref(self.so), self.workspace.data_ptr(),
+                                                       self.workspace_bytes, self.dev._stream()))
+        return self.out
+
+    def farm_response(self, C_arr=None, M_arr=None, B_arr=None):
+        """Enqueue the coupled 6N-DOF system response of the LAST ``solve`` (raft_model.py:1164-1216) with each FOWT's
+        second-order force in its excitation (:1212) -> (Xi_sys [nC,6N,nw], info).  Needs want with B_drag, F_drag, F_iner,
+        F_2nd (and F_BEM when the designs carry BEM excitation)."""
+        need = ("B_drag", "F_drag", "F_iner", "F_2nd") + (("F_BEM",) if self.batch.n_bem_head else ())
+        missing = [k for k in need if k not in self.out]
+        if missing:
+            raise ValueError("farm_response needs the outputs %s in want" % missing)
+        cf = RaftkCases.from_buffer_copy(self.c_struct)
+        cf.F_2nd = self.out["F_2nd"].data_ptr()
+        self.dev.c_struct, self.dev.o_struct = cf, self.o_struct
+        return self.dev.farm_response(C_arr=C_arr, M_arr=M_arr, B_arr=B_arr)
 
 
 def get_rao(Xi, zeta):

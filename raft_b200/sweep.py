@@ -147,6 +147,19 @@ def solve_sweep(packed_designs, cases, n_iter=10, tol=0.01, xi_start=0.0, device
     return all_gather_blocks(out["Xi"], n_total, group), all_gather_blocks(out["status"], n_total, group)
 
 
+def solve_sweep_slender(packed_designs, cases, n_iter=10, tol=0.01, xi_start=0.0, device=None, group=None, n_total=None, qtf_chunk=0):
+    """``solve_sweep`` for designs with potSecOrder 1 (``build_variants`` emits their ``qs_*`` tables): this rank's designs
+    through ``solver.SlenderSession`` on its GPU, then the all-gather -> (Xi [n_total,nC,6,nw], status [n_total,nC,4]).
+    ``qtf_chunk``: units whose QTF tables are built at once (0: all)."""
+    from . import solver
+    out = solver.SlenderSession(packed_designs, solver.CaseTable(cases), device=device, qtf_chunk=qtf_chunk).solve(n_iter=n_iter, tol=tol,
+                                                                                                                  xi_start=xi_start)
+    if bool(((out["status"][..., 2] & solver.FLAG_PLAN) != 0).any()):
+        raise solver._lib.RaftkError("step-class tables overflowed the hints of the design batch")
+    n_total = len(packed_designs) if n_total is None else n_total
+    return all_gather_blocks(out["Xi"], n_total, group), all_gather_blocks(out["status"], n_total, group)
+
+
 class _DevMem:
     """Raw device allocation exposed through __cuda_array_interface__ so torch can view it without owning it."""
 
