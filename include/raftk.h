@@ -464,6 +464,34 @@ int raftk_general_solve_dynamics_qtf_host(const raftk_general *g, const raftk_ge
                                           double *F_2nd_mean);
 
 /*
+ * The generalised-DOF solve of a case table of any size through a bounded workspace.  The table is cut into chunks of at most
+ * max_chunk_cases cases (0: all cases in one chunk), each made of whole train groups -- a primary and every secondary train that
+ * points at it (cases.primary) stay in one chunk, because the secondaries are solved from the primary's LU factors.  Groups are
+ * packed greedily in table order.  Every chunk runs the launch sequence of raftk_general_solve_dynamics_qtf_dev on views of the
+ * case columns and outputs advanced to its first case, one after the other on the caller's stream in one workspace sized for the
+ * largest chunk, with no host synchronisation between chunks.  Every output equals the single-table entry's bit for bit (up to
+ * the atomic sums of k_qtf_tiles, see raftk_general_qtf); status word 3 of a secondary train still holds its primary's index in
+ * the whole table + 1.  Arguments are those of raftk_general_solve_dynamics_qtf_* plus max_chunk_cases; n_cases may exceed
+ * 65535 when max_chunk_cases <= 65535.
+ * raftk_general_stream_workspace_bytes(.., n_cases, K) = raftk_general_qtf_workspace_bytes(.., min(K, n_cases)), plus the chunk's
+ * rebased primary map (K * 4 bytes rounded up to 256) when K < n_cases.
+ * Rejected with RAFTK_EINVAL before any launch, in addition to the checks of the qtf entry: max_chunk_cases < 0 or a chunk of
+ * more than 65535 cases; a primary map whose train groups interleave (a group not contiguous in the table;
+ * raft_b200.packer.pack_case_trains never builds one); a group with more than max_chunk_cases cases; a workspace smaller than
+ * the query.  The *_dev entry reads cases.primary back to the host once to plan the chunks (a copy on the caller's stream and a
+ * wait for it), as it reads fd and qtf tables for their checks.
+ */
+size_t raftk_general_stream_workspace_bytes(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, int32_t n_cases,
+                                            int32_t max_chunk_cases);
+int raftk_general_solve_dynamics_stream_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                            const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM,
+                                            double *F_2nd, double *F_2nd_mean, void *workspace, size_t workspace_bytes,
+                                            int32_t max_chunk_cases, void *stream);
+int raftk_general_solve_dynamics_stream_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                             const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM,
+                                             double *F_2nd, double *F_2nd_mean, int32_t max_chunk_cases);
+
+/*
  * Output channels of FOWT.saveTurbineOutputs for a FOWT with generalised degrees of freedom (raft_fowt.py:2299-2604): PRP
  * motions, nacelle accelerations and flexible-tower base loads are real linear functionals of the reduced response,
  *   Y_ch(w) = w^wpow[ch] sum_b R[ch,b] Xi[b,w]     (raft_b200.packer.pack_general_channels; rad2deg folded into R)
@@ -515,6 +543,14 @@ int raftk_solve_dynamics_gather_dev(const raftk_designs *d, const raftk_cases *c
 /* Enqueue: tell every peer "my stores of this epoch are done", then wait (bounded: ~4 s, then *timeout_flag = 1 if
  * given) until every peer said so.  After it, gathered[rank] holds all ranks' blocks of this epoch. */
 int raftk_peer_barrier_dev(const raftk_peers *peers, int32_t *timeout_flag, void *stream);
+/* Generalised-DOF shards (raft_b200.sweep.ShardedGeneralSolve): a copy's responses are complex [n_ranks * rows_per_rank, n_dof,
+ * nw] (block_elems = rows_per_rank * n_dof * nw) and its status int32 [n_ranks * rows_per_rank, 4].  Enqueue stores of n_rows
+ * finished rows -- Xi complex [n_rows, n_dof, nw] and status [n_rows, 4] (or NULL) on this device -- into rows [row0, row0 +
+ * n_rows) of EVERY rank's copy through the peer-mapped pointers; status word 3 of a secondary train (primary + 1) is shifted by
+ * primary_base, so a shard solved as a table of its own publishes indices into the whole table.  Follow with
+ * raftk_peer_barrier_dev.  Rows past n_ranks * block_elems, or status without every rank's status copy: RAFTK_EINVAL. */
+int raftk_general_publish_dev(const raftk_peers *peers, const double *Xi, const int32_t *status, int32_t row0, int32_t n_rows,
+                              int32_t n_dof, int32_t nw, int32_t primary_base, void *stream);
 
 /* Same three operations with HOST pointers everywhere (tables, cases, outputs). */
 int raftk_hydro_excitation_host(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *out);

@@ -153,12 +153,13 @@ SYMBOLS = [
     "raftk_general_workspace_bytes", "raftk_general_solve_dynamics_dev", "raftk_general_solve_dynamics_host",
     "raftk_general_fd_workspace_bytes", "raftk_general_solve_dynamics_fd_dev", "raftk_general_solve_dynamics_fd_host",
     "raftk_general_qtf_workspace_bytes", "raftk_general_solve_dynamics_qtf_dev", "raftk_general_solve_dynamics_qtf_host",
+    "raftk_general_stream_workspace_bytes", "raftk_general_solve_dynamics_stream_dev", "raftk_general_solve_dynamics_stream_host",
     "raftk_system_solve_dev", "raftk_system_solve_host", "raftk_response_stats_dev", "raftk_response_stats_host",
     "raftk_channel_stats_dev", "raftk_channel_stats_host", "raftk_general_channel_stats_dev", "raftk_general_channel_stats_host",
     "raftk_host_alloc", "raftk_host_free",
     "raftk_fp64_peak_gflops",
     "raftk_peer_alloc", "raftk_peer_free", "raftk_peer_open", "raftk_peer_close",
-    "raftk_solve_dynamics_gather_dev", "raftk_peer_barrier_dev",
+    "raftk_solve_dynamics_gather_dev", "raftk_peer_barrier_dev", "raftk_general_publish_dev",
     "raftk_farm_response_dev", "raftk_solve_dynamics_farm_host", "raftk_farm_workspace_bytes", "raftk_farm_response_ws_dev",
     "raftk_family_sizes", "raftk_build_family_host",
 ]
@@ -236,6 +237,16 @@ def _load():
                                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.raftk_general_solve_dynamics_qtf_dev.restype = C.c_int
     lib.raftk_general_solve_dynamics_qtf_host.restype = C.c_int
+    lib.raftk_general_stream_workspace_bytes.restype = C.c_size_t
+    lib.raftk_general_stream_workspace_bytes.argtypes = [P(RaftkGeneral), P(RaftkGeneralFd), P(RaftkGeneralQtf), C.c_int32, C.c_int32]
+    lib.raftk_general_solve_dynamics_stream_dev.argtypes = [P(RaftkGeneral), P(RaftkGeneralFd), P(RaftkGeneralQtf), P(RaftkCases),
+                                                            P(RaftkSolveOpts), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                            C.c_void_p, C.c_size_t, C.c_int32, C.c_void_p]
+    lib.raftk_general_solve_dynamics_stream_host.argtypes = [P(RaftkGeneral), P(RaftkGeneralFd), P(RaftkGeneralQtf), P(RaftkCases),
+                                                             P(RaftkSolveOpts), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                             C.c_int32]
+    lib.raftk_general_solve_dynamics_stream_dev.restype = C.c_int
+    lib.raftk_general_solve_dynamics_stream_host.restype = C.c_int
     lib.raftk_system_solve_dev.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.raftk_system_solve_host.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.raftk_response_stats_dev.argtypes = [C.c_int32, C.c_int32, C.c_double, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -262,6 +273,8 @@ def _load():
     lib.raftk_solve_dynamics_gather_dev.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkSolveOpts), P(RaftkOutputs), P(RaftkPeers),
                                                     C.c_void_p, C.c_size_t, C.c_void_p]
     lib.raftk_peer_barrier_dev.argtypes = [P(RaftkPeers), C.c_void_p, C.c_void_p]
+    lib.raftk_general_publish_dev.argtypes = [P(RaftkPeers), C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                              C.c_void_p]
     lib.raftk_farm_response_dev.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkOutputs), P(RaftkFarm), C.c_void_p]
     lib.raftk_solve_dynamics_farm_host.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkSolveOpts), P(RaftkOutputs), P(RaftkFarm)]
     lib.raftk_farm_response_dev.restype = C.c_int
@@ -275,7 +288,7 @@ def _load():
     lib.raftk_family_sizes.restype = C.c_int
     lib.raftk_build_family_host.restype = C.c_int
     for fn in ("raftk_peer_alloc", "raftk_peer_open", "raftk_peer_free", "raftk_peer_close", "raftk_solve_dynamics_gather_dev",
-               "raftk_peer_barrier_dev"):
+               "raftk_peer_barrier_dev", "raftk_general_publish_dev"):
         getattr(lib, fn).restype = C.c_int
     for fn in ("raftk_hydro_excitation_dev", "raftk_hydro_linearization_dev", "raftk_solve_dynamics_dev",
                "raftk_hydro_excitation_host", "raftk_hydro_linearization_host", "raftk_solve_dynamics_host",

@@ -1415,17 +1415,16 @@ extern "C" size_t raftk_general_workspace_bytes(const raftk_general *g, int32_t 
     return raftk_general_fd_workspace_bytes(g, nullptr, n_cases);
 }
 
-extern "C" int raftk_general_solve_dynamics_qtf_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
-                                                    const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
-                                                    double *F_BEM, double *F_2nd, double *F_2nd_mean, void *workspace,
-                                                    size_t workspace_bytes, void *stream)
+// checks of the generalised-DOF entry points, before any launch; max_cases: the most cases the call takes (65535 for one
+// launch grid, any count when the call streams the table in chunks)
+static int gen_validate(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, const raftk_cases *c,
+                        const raftk_solve_opts *o, const double *Xi, const int32_t *status, int64_t max_cases, cudaStream_t st)
 {
-    disp_reset();
     if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
-    if (g->n_dof <= 0 || g->n_dof > 256 || g->nw <= 0 || g->n_nodes < 0 || c->n_cases <= 0 || c->n_cases > 65535)
-        return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, 0 < n_cases <= 65535");
+    if (g->n_dof <= 0 || g->n_dof > 256 || g->nw <= 0 || g->n_nodes < 0 || c->n_cases <= 0 || c->n_cases > max_cases)
+        return set_err(RAFTK_EINVAL, max_cases == 65535 ? "general solve: 0 < n_dof <= 256, nw > 0, 0 < n_cases <= 65535"
+                                                        : "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
     if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
-    cudaStream_t st = (cudaStream_t)stream;
     if (qtf) {                                         // the frequency and heading vectors are read back for the checks
         if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
         std::vector<double> qw(qtf->n_qtf_w), qh(qtf->n_qtf_head);
@@ -1444,9 +1443,17 @@ extern "C" int raftk_general_solve_dynamics_qtf_dev(const raftk_general *g, cons
         if (fd->n_fd > 0 || fd->n_bem_head > 0) CUDA_TRY(cudaStreamSynchronize(st));
         if (int rc = validate_gen_fd(g, fd, idx.data(), hd.data())) return rc;
     }
+    return 0;
+}
+
+// the launch sequence of one case table (at most 65535 cases) in a workspace of gen_layout(g, fd, qtf, c->n_cases).total bytes;
+// prof_reset: start a new profile record (the streamed entry keeps one record over its chunks)
+static int gen_launch(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, const raftk_cases *c,
+                      const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM, double *F_2nd, double *F_2nd_mean,
+                      void *workspace, cudaStream_t st, bool prof_reset)
+{
     const size_t nC = c->n_cases;
     const GenLayout L = gen_layout(g, fd, qtf, nC);
-    if (!workspace || workspace_bytes < L.total) return set_err(RAFTK_ENOMEM, "general solve: workspace too small");
     const bool bem = fd && fd->n_bem_head > 0;
     GenDev D;
     D.n = g->n_dof; D.nw = g->nw; D.Ns = g->n_nodes; D.depth = g->depth; D.dw = g->dw; D.rho = g->rho;
@@ -1493,7 +1500,7 @@ extern "C" int raftk_general_solve_dynamics_qtf_dev(const raftk_general *g, cons
         QP.F2mean = F_2nd_mean ? F_2nd_mean : reinterpret_cast<double *>(b + L.F2m);
         if (int rc = launch_qtf(QP, c, st)) return rc;
     }
-    prof_begin_call();
+    if (prof_reset) prof_begin_call();
     k_gen_init<<<(unsigned)nC, 256, 0, st>>>(D, W, o->xi_start, prim);
     if (g->n_nodes > 0) k_gen_wave<<<dim3(fb, g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, C, W);
     if (bem) {                                         // F_BEM = T0^T f_BEM, then F_iner = F_BEM + sum_j Tn_j^T f6_j
@@ -1536,6 +1543,18 @@ extern "C" int raftk_general_solve_dynamics_qtf_dev(const raftk_general *g, cons
     g_launches++;
     CUDA_TRY(cudaGetLastError());
     return RAFTK_OK;
+}
+
+extern "C" int raftk_general_solve_dynamics_qtf_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                                    const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
+                                                    double *F_BEM, double *F_2nd, double *F_2nd_mean, void *workspace,
+                                                    size_t workspace_bytes, void *stream)
+{
+    disp_reset();
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = gen_validate(g, fd, qtf, c, o, Xi, status, 65535, st)) return rc;
+    if (!workspace || workspace_bytes < gen_layout(g, fd, qtf, c->n_cases).total) return set_err(RAFTK_ENOMEM, "general solve: workspace too small");
+    return gen_launch(g, fd, qtf, c, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, st, true);
 }
 
 extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
@@ -1616,6 +1635,217 @@ extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const r
                                                  int32_t *status)
 {
     return raftk_general_solve_dynamics_fd_host(g, nullptr, c, o, Xi, status, nullptr);
+}
+
+// ---- generalised DOFs, streamed: the case table in chunks of whole train groups through one bounded workspace ----------
+static size_t gen_chunk_cap(int32_t n_cases, int32_t max_chunk_cases)
+{
+    return (max_chunk_cases <= 0 || max_chunk_cases >= n_cases) ? (size_t)n_cases : (size_t)max_chunk_cases;
+}
+
+// chunk-local primary map [K] at the end of the workspace when the table runs in more than one chunk
+static size_t gen_stream_bytes(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, int32_t n_cases,
+                               int32_t max_chunk_cases, size_t *prim_off)
+{
+    const size_t K = gen_chunk_cap(n_cases, max_chunk_cases);
+    const size_t base = gen_layout(g, fd, qtf, K).total;
+    if (prim_off) *prim_off = base;
+    return K < (size_t)n_cases ? base + align_up(K * 4, 256) : base;
+}
+
+extern "C" size_t raftk_general_stream_workspace_bytes(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                                       int32_t n_cases, int32_t max_chunk_cases)
+{
+    if (!g || n_cases <= 0 || g->n_dof <= 0 || g->nw <= 0) return 0;
+    return gen_stream_bytes(g, fd, qtf, n_cases, max_chunk_cases, nullptr);
+}
+
+// Chunk starts (and the end) of a case table: whole train groups, greedily packed into chunks of at most K cases.  prim: host
+// copy of cases.primary or NULL (every case a group of its own).  A group is the set of cases sharing one primary; it must be
+// contiguous in the table (packer.pack_case_trains lays tables out so) and no larger than K.
+static int gen_plan_chunks(const int32_t *prim, size_t nC, size_t K, std::vector<size_t> &starts)
+{
+    starts.clear();
+    std::vector<size_t> gs;                            // group starts
+    if (prim) {
+        std::vector<size_t> first(nC, SIZE_MAX), last(nC, 0), count(nC, 0);
+        for (size_t i = 0; i < nC; i++) {
+            const int p = prim[i];
+            if (p < 0 || (size_t)p >= nC || prim[p] != p) return set_err(RAFTK_EINVAL, "general solve: cases.primary must map every case to a primary case");
+            first[p] = std::min(first[p], i); last[p] = i; count[p]++;
+        }
+        for (size_t p = 0; p < nC; p++)
+            if (count[p] && last[p] - first[p] + 1 != count[p])
+                return set_err(RAFTK_EINVAL, "general stream: the train groups of cases.primary interleave (a group must be contiguous in the table)");
+        for (size_t i = 0; i < nC; i++)
+            if (i == 0 || prim[i] != prim[i - 1]) gs.push_back(i);
+    } else {
+        for (size_t i = 0; i < nC; i++) gs.push_back(i);
+    }
+    gs.push_back(nC);
+    starts.push_back(0);
+    for (size_t t = 0; t + 1 < gs.size(); t++) {
+        if (gs[t + 1] - gs[t] > K) return set_err(RAFTK_EINVAL, "general stream: a train group has more cases than max_chunk_cases");
+        if (gs[t + 1] - starts.back() > K) starts.push_back(gs[t]);
+    }
+    starts.push_back(nC);
+    return 0;
+}
+
+// the chunk loop on device pointers; hprim: host copy of c->primary (NULL without trains)
+static int gen_stream_run(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, const raftk_cases *c,
+                          const int32_t *hprim, const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM, double *F_2nd,
+                          double *F_2nd_mean, void *workspace, size_t workspace_bytes, int32_t max_chunk_cases, cudaStream_t st)
+{
+    const size_t nC = c->n_cases, K = gen_chunk_cap(c->n_cases, max_chunk_cases);
+    if (K > 65535) return set_err(RAFTK_EINVAL, "general stream: a chunk takes at most 65535 cases (max_chunk_cases)");
+    std::vector<size_t> starts;
+    if (int rc = gen_plan_chunks(hprim, nC, K, starts)) return rc;
+    size_t prim_off = 0;
+    const size_t need = gen_stream_bytes(g, fd, qtf, c->n_cases, max_chunk_cases, &prim_off);
+    if (!workspace || workspace_bytes < need) return set_err(RAFTK_EINVAL, "general stream: workspace smaller than raftk_general_stream_workspace_bytes()");
+    int *local = reinterpret_cast<int *>(static_cast<char *>(workspace) + prim_off);
+    const size_t n = g->n_dof, nw = g->nw, nch = starts.size() - 1;
+    for (size_t k = 0; k < nch; k++) {
+        const size_t c0 = starts[k], m = starts[k + 1] - c0;
+        raftk_cases cc = *c;
+        cc.n_cases = (int32_t)m;
+        cc.Hs = c->Hs ? c->Hs + c0 : nullptr; cc.Tp = c->Tp ? c->Tp + c0 : nullptr;
+        cc.gamma = c->gamma ? c->gamma + c0 : nullptr; cc.beta_deg = c->beta_deg ? c->beta_deg + c0 : nullptr;
+        cc.spec = c->spec ? c->spec + c0 : nullptr; cc.zeta = c->zeta ? c->zeta + c0 * nw : nullptr;
+        if (c->primary && nch > 1) {                   // absolute primaries -> chunk-local ones
+            k_gen_chunk_primary<<<(unsigned)((m + 127) / 128), 128, 0, st>>>((int)m, (int)c0, c->primary, local);
+            g_launches++;
+            cc.primary = local;
+        }
+        if (int rc = gen_launch(g, fd, qtf, &cc, o, Xi + c0 * n * nw * 2, status + c0 * 4, F_BEM ? F_BEM + c0 * n * nw * 2 : nullptr,
+                                F_2nd ? F_2nd + c0 * 6 * nw : nullptr, F_2nd_mean ? F_2nd_mean + c0 * 6 : nullptr, workspace, st, k == 0))
+            return rc;
+        if (c->primary && c0 > 0) {                    // status word 3 of the secondaries: the table's primary + 1
+            k_gen_status_rebase<<<(unsigned)((m + 127) / 128), 128, 0, st>>>((int)m, (int)c0, status + c0 * 4);
+            g_launches++;
+        }
+    }
+    g_disp.chunks = (int32_t)nch;
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_general_solve_dynamics_stream_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                                       const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
+                                                       double *F_BEM, double *F_2nd, double *F_2nd_mean, void *workspace,
+                                                       size_t workspace_bytes, int32_t max_chunk_cases, void *stream)
+{
+    disp_reset();
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = gen_validate(g, fd, qtf, c, o, Xi, status, INT32_MAX, st)) return rc;
+    if (max_chunk_cases < 0) return set_err(RAFTK_EINVAL, "general stream: max_chunk_cases must be >= 0 (0: all cases)");
+    std::vector<int32_t> hp;
+    if (c->primary) {                                  // the primary map is read back once to plan the chunks
+        hp.resize(c->n_cases);
+        CUDA_TRY(cudaMemcpyAsync(hp.data(), c->primary, hp.size() * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+    }
+    return gen_stream_run(g, fd, qtf, c, c->primary ? hp.data() : nullptr, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace,
+                          workspace_bytes, max_chunk_cases, st);
+}
+
+extern "C" int raftk_general_solve_dynamics_stream_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                                        const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
+                                                        double *F_BEM, double *F_2nd, double *F_2nd_mean, int32_t max_chunk_cases)
+{
+    disp_reset();
+    if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
+    if (g->n_dof <= 0 || g->nw <= 0 || c->n_cases <= 0) return set_err(RAFTK_EINVAL, "general solve: empty problem");
+    if (max_chunk_cases < 0) return set_err(RAFTK_EINVAL, "general stream: max_chunk_cases must be >= 0 (0: all cases)");
+    if (g->n_dof > 256 || g->n_nodes < 0) return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
+    if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
+    const size_t n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases, K = gen_chunk_cap(c->n_cases, max_chunk_cases);
+    if (K > 65535) return set_err(RAFTK_EINVAL, "general stream: a chunk takes at most 65535 cases (max_chunk_cases)");
+    std::vector<size_t> starts;                        // the plan's checks, before anything is staged
+    if (int rc = gen_plan_chunks(c->primary, nC, K, starts)) return rc;
+    if (fd)
+        if (int rc = validate_gen_fd(g, fd, fd->fd_idx, fd->bem_headings)) return rc;
+    if (qtf) {
+        if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
+        if (int rc = validate_gen_qtf(g, qtf, qtf->qtf_w, qtf->qtf_heads)) return rc;
+    }
+    Staging S("raftk_general_solve_dynamics_stream_host");
+    raftk_general gg = *g;
+    S.in(gg.w, g->w, nw); S.in(gg.k, g->k, nw);
+    S.in(gg.node_r, g->node_r, Ns * 3); S.in(gg.node_frame, g->node_frame, Ns * 9);
+    S.in(gg.node_circ, g->node_circ, Ns); S.in(gg.node_Imat, g->node_Imat, Ns * 9);
+    S.in(gg.node_Imat_w, g->node_Imat_w, Ns * 9 * nw * 2); S.in(gg.node_a_i, g->node_a_i, Ns);
+    S.in(gg.node_cd, g->node_cd, Ns * 4); S.in(gg.Tn, g->Tn, Ns * 6 * n); S.in(gg.rr, g->rr, Ns * 3);
+    S.in(gg.M, g->M, n * n); S.in(gg.B, g->B, n * n); S.in(gg.C, g->C, n * n);
+    raftk_cases cc = *c;
+    S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
+    S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC); S.in(cc.zeta, c->zeta, nC * nw);
+    S.in(cc.primary, c->primary, nC);
+    raftk_general_fd ff = fd ? *fd : raftk_general_fd{};
+    if (fd) {
+        const size_t nf = fd->n_fd, nh = fd->n_bem_head;
+        S.in(ff.fd_idx, fd->fd_idx, nf); S.in(ff.A_w, fd->A_w, nf * nf * nw); S.in(ff.B_w, fd->B_w, nf * nf * nw);
+        S.in(ff.bem_headings, fd->bem_headings, nh); S.in(ff.X_BEM, fd->X_BEM, nh * 6 * nw * 2); S.in(ff.T0, fd->T0, nh ? 6 * n : 0);
+    }
+    raftk_general_qtf qq = qtf ? *qtf : raftk_general_qtf{};
+    if (qtf) {
+        const size_t n2 = qtf->n_qtf_w, nh = qtf->n_qtf_head;
+        S.in(qq.qtf_w, qtf->qtf_w, n2); S.in(qq.qtf_heads, qtf->qtf_heads, nh); S.in(qq.qtf, qtf->qtf, n2 * n2 * nh * 12);
+    }
+    double *dXi, *dF_BEM, *dF2, *dF2m;
+    int32_t *dStatus;
+    char *ws;
+    const size_t wb = raftk_general_stream_workspace_bytes(g, fd, qtf, c->n_cases, max_chunk_cases);
+    S.out(dXi, nC * n * nw * 2, Xi); S.out(dStatus, nC * 4, status); S.out(dF_BEM, F_BEM ? nC * n * nw * 2 : 0, F_BEM);
+    S.out(dF2, qtf && F_2nd ? nC * 6 * nw : 0, F_2nd); S.out(dF2m, qtf && F_2nd_mean ? nC * 6 : 0, F_2nd_mean);
+    S.buf(ws, wb);
+    int rc = S.commit();
+    if (rc || (rc = gen_stream_run(&gg, fd ? &ff : nullptr, qtf ? &qq : nullptr, &cc, c->primary, o, dXi, dStatus, dF_BEM, dF2, dF2m, ws, wb,
+                             max_chunk_cases, nullptr))) return rc;
+    return S.finish();
+}
+
+// Peer publication of a streamed shard (raftk_general_publish_dev): rows [row0, row0 + n_rows) of every rank's gathered array
+__global__ void __launch_bounds__(256) k_gen_publish(GenPublish P, const double2 *Xi, const int *status)
+{
+    const int p = blockIdx.y;
+    const size_t stride = (size_t)gridDim.x * 256, t0 = (size_t)blockIdx.x * 256 + threadIdx.x;
+    double2 *dst = P.X[p];
+    for (size_t t = t0; t < P.elems; t += stride) dst[t] = Xi[t];
+    if (int *sd = P.S[p])
+        for (size_t t = t0; t < (size_t)P.rows * 4; t += stride) {
+            const int v = status[t];
+            sd[t] = ((t & 3) == 3 && v != 0) ? v + P.primary_base : v;
+        }
+}
+
+extern "C" int raftk_general_publish_dev(const raftk_peers *peers, const double *Xi, const int32_t *status, int32_t row0, int32_t n_rows,
+                                         int32_t n_dof, int32_t nw, int32_t primary_base, void *stream)
+{
+    disp_reset();
+    if (int rc = validate_peers(peers)) return rc;
+    if (!Xi || row0 < 0 || n_rows < 0 || n_dof <= 0 || nw <= 0)
+        return set_err(RAFTK_EINVAL, "general publish: Xi is required, row0 >= 0, n_rows >= 0, n_dof > 0, nw > 0");
+    const size_t row = (size_t)n_dof * nw;
+    if (((size_t)row0 + n_rows) * row > (size_t)peers->n_ranks * peers->block_elems)
+        return set_err(RAFTK_EINVAL, "general publish: rows past the gathered array (n_ranks * block_elems complex elements)");
+    if (status)
+        for (int r = 0; r < peers->n_ranks; r++)
+            if (!peers->status[r]) return set_err(RAFTK_EINVAL, "general publish: status given but a rank's gathered status is missing");
+    if (n_rows == 0) return RAFTK_OK;
+    GenPublish P;
+    P.elems = (size_t)n_rows * row; P.rows = n_rows; P.primary_base = primary_base;
+    for (int r = 0; r < RAFTK_MAX_PEERS; r++) {
+        const bool on = r < peers->n_ranks;
+        P.X[r] = on ? reinterpret_cast<double2 *>(peers->gathered[r]) + (size_t)row0 * row : nullptr;
+        P.S[r] = on && status ? peers->status[r] + (size_t)row0 * 4 : nullptr;
+    }
+    const unsigned bx = (unsigned)std::min<size_t>((P.elems + 255) / 256, 1024);
+    k_gen_publish<<<dim3(bx, (unsigned)peers->n_ranks), 256, 0, (cudaStream_t)stream>>>(P, reinterpret_cast<const double2 *>(Xi), status);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
 }
 
 // ---- slender-body QTF ----------------------------------------------------------------------------------

@@ -666,6 +666,31 @@ __global__ void __launch_bounds__(256) k_gen_relax(GenDev D, GenWork W, const do
     }
 }
 
+// Streamed tables (raftk_general_solve_dynamics_stream_*): every chunk holds whole train groups and runs the sequence above
+// on views advanced to its first case c0.  Around it:
+//   k_gen_chunk_primary (case)   cases.primary of the chunk, rebased to c0, into the workspace
+//   k_gen_status_rebase (case)   status word 3 of the chunk's secondaries back to the table's primary + 1
+__global__ void __launch_bounds__(128) k_gen_chunk_primary(int nC, int c0, const int *primary, int *local)
+{
+    const int c = blockIdx.x * 128 + threadIdx.x;
+    if (c < nC) local[c] = primary[c0 + c] - c0;
+}
+
+__global__ void __launch_bounds__(128) k_gen_status_rebase(int nC, int c0, int *status)
+{
+    const int c = blockIdx.x * 128 + threadIdx.x;
+    if (c < nC && status[4 * c + 3] != 0) status[4 * c + 3] += c0;
+}
+
+// raftk_general_publish_dev: rank p's gathered rows for this call, X[p] complex [rows][n][nw] and S[p] int [rows][4] (NULL: no
+// status); status word 3 of a secondary train is shifted by primary_base (shard-local primary + 1 -> the whole table's)
+struct GenPublish {
+    size_t elems;
+    int rows, primary_base;
+    double2 *X[RAFTK_MAX_PEERS];
+    int *S[RAFTK_MAX_PEERS];
+};
+
 // status rows for the caller: passes, converged, flags (RAFTK_FLAG_NAN), 0; a secondary train: 0, 1, flags, primary + 1
 __global__ void __launch_bounds__(128) k_gen_status(int nC, const int *flags, const int *primary, int *status)
 {

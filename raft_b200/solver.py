@@ -746,9 +746,12 @@ class GeneralSession:
     mass, damping and BEM excitation (``packer.pack_general_matrices``); with ``F_BEM=True`` ``solve()`` also returns the BEM
     excitation in reduced DOFs, complex [nT,nDOF,nw].  ``qtf``: second-order wave loads (``packer.pack_general_qtf``); every
     ``solve()`` then leaves the force of every case and train in the device tensors ``F_2nd`` [nT,6,nw] and ``F_2nd_mean``
-    [nT,6] (reduced DOFs 0-5)."""
+    [nT,6] (reduced DOFs 0-5).  ``max_chunk_cases``: None runs the table in one launch sequence (at most 65535 cases, a
+    workspace for every case at once); an integer K streams it in chunks of whole train groups of at most K cases (0: one
+    chunk) through a workspace sized for one chunk (raftk_general_solve_dynamics_stream_dev, ``general_chunk_for_budget``),
+    with the same results."""
 
-    def __init__(self, P, M, B, Cm, cases, device=None, fd=None, F_BEM=False, qtf=None):
+    def __init__(self, P, M, B, Cm, cases, device=None, fd=None, F_BEM=False, qtf=None, max_chunk_cases=None):
         import torch
         self.torch = torch
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
@@ -767,7 +770,13 @@ class GeneralSession:
             self.qtf = _general_qtf_struct(qtf, to_dev)
             fdp = C.byref(self.fd) if self.fd is not None else None
             qp = C.byref(self.qtf) if self.qtf is not None else None
-            self.workspace_bytes = int(lib.raftk_general_qtf_workspace_bytes(C.byref(self.g), fdp, qp, nC))
+            self.max_chunk_cases = None if max_chunk_cases is None else int(max_chunk_cases)
+            if self.max_chunk_cases is None:
+                self.workspace_bytes = int(lib.raftk_general_qtf_workspace_bytes(C.byref(self.g), fdp, qp, nC))
+            else:
+                if self.max_chunk_cases < 0:
+                    raise ValueError("max_chunk_cases must be >= 0 (0: all cases in one chunk)")
+                self.workspace_bytes = int(lib.raftk_general_stream_workspace_bytes(C.byref(self.g), fdp, qp, nC, self.max_chunk_cases))
             self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=self.device)
             self.Xi = torch.zeros([nC, n, nw], dtype=torch.complex128, device=self.device)
             self.status = torch.zeros([nC, 4], dtype=torch.int32, device=self.device)
@@ -780,12 +789,18 @@ class GeneralSession:
     def solve(self, n_iter=10, tol=0.01, xi_start=0.0):
         o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
         ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
+        fdp = C.byref(self.fd) if self.fd is not None else None
+        qp = C.byref(self.qtf) if self.qtf is not None else None
         with self.torch.cuda.device(self.device):
-            check(lib.raftk_general_solve_dynamics_qtf_dev(C.byref(self.g), C.byref(self.fd) if self.fd is not None else None,
-                                                           C.byref(self.qtf) if self.qtf is not None else None, C.byref(self.c_struct),
-                                                           C.byref(o), self.Xi.data_ptr(), self.status.data_ptr(), ptr(self.F_BEM),
-                                                           ptr(self.F_2nd), ptr(self.F_2nd_mean), self.workspace.data_ptr(),
-                                                           self.workspace_bytes, self.torch.cuda.current_stream(self.device).cuda_stream))
+            stream = self.torch.cuda.current_stream(self.device).cuda_stream
+            if self.max_chunk_cases is None:
+                check(lib.raftk_general_solve_dynamics_qtf_dev(C.byref(self.g), fdp, qp, C.byref(self.c_struct), C.byref(o), self.Xi.data_ptr(),
+                                                               self.status.data_ptr(), ptr(self.F_BEM), ptr(self.F_2nd), ptr(self.F_2nd_mean),
+                                                               self.workspace.data_ptr(), self.workspace_bytes, stream))
+            else:
+                check(lib.raftk_general_solve_dynamics_stream_dev(C.byref(self.g), fdp, qp, C.byref(self.c_struct), C.byref(o), self.Xi.data_ptr(),
+                                                                  self.status.data_ptr(), ptr(self.F_BEM), ptr(self.F_2nd), ptr(self.F_2nd_mean),
+                                                                  self.workspace.data_ptr(), self.workspace_bytes, self.max_chunk_cases, stream))
         return (self.Xi, self.status) if self.F_BEM is None else (self.Xi, self.status, self.F_BEM)
 
     def stats(self, R, wpow, psd=True, amp=False):
@@ -811,7 +826,8 @@ class GeneralSession:
         return sd, P, A
 
 
-def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0, fd=None, F_BEM=False, qtf=None, F_2nd=False):
+def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0, fd=None, F_BEM=False, qtf=None, F_2nd=False,
+                           max_chunk_cases=None):
     """Model.solveDynamics for one FOWT with generalised degrees of freedom (flexible members), host buffers:
     ``P`` from ``packer.pack_general_dofs`` (node tables + ``gen_Tn``, ``gen_rr``), constant system
     matrices ``M, B, Cm`` [nDOF,nDOF], ``cases`` a CaseTable, with wave trains when built from ``packer.pack_case_trains``
@@ -820,7 +836,8 @@ def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0
     dict of ``packer.pack_general_matrices`` (whose M, B, C are then the constant matrices).  ``F_BEM=True`` appends the BEM
     excitation of every case and train in reduced DOFs, complex [nT,nDOF,nw], to the result.  ``qtf``: second-order wave
     loads (potSecOrder 2), the dict of ``packer.pack_general_qtf``; ``F_2nd=True`` (with ``qtf``) then appends the force of
-    every case and train on reduced DOFs 0-5, F_2nd [nT,6,nw] and F_2nd_mean [nT,6]."""
+    every case and train on reduced DOFs 0-5, F_2nd [nT,6,nw] and F_2nd_mean [nT,6].  ``max_chunk_cases``: None solves the
+    table in one launch sequence; an integer K streams it through a device workspace for K cases (``GeneralSession``)."""
     n, nw = int(P["gen_nDOF"]), len(P["w"])
     keep = {}
 
@@ -840,9 +857,62 @@ def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0
     c = cases.struct(_host_ptr(cases.arrays))
     o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
     hp = lambda a: a.ctypes.data if a is not None else None   # noqa: E731
-    check(lib.raftk_general_solve_dynamics_qtf_host(C.byref(g), C.byref(f) if f is not None else None, C.byref(q) if q is not None else None,
-                                                    C.byref(c), C.byref(o), Xi.ctypes.data, st.ctypes.data, hp(Fb), hp(F2), hp(F2m)))
+    fp, qp = (C.byref(f) if f is not None else None), (C.byref(q) if q is not None else None)
+    if max_chunk_cases is None:
+        check(lib.raftk_general_solve_dynamics_qtf_host(C.byref(g), fp, qp, C.byref(c), C.byref(o), Xi.ctypes.data, st.ctypes.data, hp(Fb),
+                                                        hp(F2), hp(F2m)))
+    else:
+        check(lib.raftk_general_solve_dynamics_stream_host(C.byref(g), fp, qp, C.byref(c), C.byref(o), Xi.ctypes.data, st.ctypes.data,
+                                                           hp(Fb), hp(F2), hp(F2m), int(max_chunk_cases)))
     return (Xi, st) + ((Fb,) if F_BEM else ()) + ((F2, F2m) if F_2nd else ())
+
+
+def general_stream_workspace_bytes(P, fd, qtf, n_cases, max_chunk_cases):
+    """raftk_general_stream_workspace_bytes: device workspace of the streamed generalised-DOF solve of ``n_cases`` cases in
+    chunks of at most ``max_chunk_cases`` (0: all).  Depends on the counts only (DOFs, bins, nodes, BEM and QTF tables present)."""
+    n, nw = int(P["gen_nDOF"]), len(P["w"])
+    g = RaftkGeneral()
+    g.n_dof, g.nw, g.n_nodes = n, nw, len(P["node_ls"])
+    none = lambda name, a: None       # noqa: E731
+    f, q = _general_fd_struct(fd, n, nw, none), _general_qtf_struct(qtf, none)
+    return int(lib.raftk_general_stream_workspace_bytes(C.byref(g), C.byref(f) if f is not None else None,
+                                                        C.byref(q) if q is not None else None, int(n_cases), int(max_chunk_cases)))
+
+
+def general_chunk_plan(primary, n_cases, max_chunk_cases):
+    """The chunks raftk_general_solve_dynamics_stream_* cut a case table into -> [c_0 = 0, c_1, ..., n_cases]: whole train
+    groups (``sweep.general_groups``) packed greedily in table order into chunks of at most ``max_chunk_cases`` (0: all).
+    ValueError where the library refuses the table: interleaved groups, a group larger than a chunk."""
+    from .sweep import general_groups
+    n = int(n_cases)
+    K = n if (max_chunk_cases <= 0 or max_chunk_cases >= n) else int(max_chunk_cases)
+    g = general_groups(primary, n)
+    cuts = [0]
+    for a, b in zip(g[:-1], g[1:]):
+        if b - a > K:
+            raise ValueError("a train group has %d cases, more than max_chunk_cases = %d" % (b - a, K))
+        if b - cuts[-1] > K:
+            cuts.append(int(a))
+    return cuts + [n]
+
+
+def general_chunk_for_budget(P, fd, qtf, n_cases, budget_bytes):
+    """The largest ``max_chunk_cases`` whose streamed workspace fits ``budget_bytes`` (``n_cases`` when the whole table fits).
+    The chunk must still hold the largest train group of the table; ValueError when not even one case fits."""
+    n_cases, budget = int(n_cases), int(budget_bytes)
+    ws = lambda k: general_stream_workspace_bytes(P, fd, qtf, n_cases, k)     # noqa: E731
+    if ws(n_cases) <= budget:
+        return n_cases
+    if ws(1) > budget:
+        raise ValueError("a workspace of %d bytes does not hold one case (%d bytes)" % (budget, ws(1)))
+    lo, hi = 1, n_cases - 1                                # ws grows with the chunk below n_cases: ws(lo) fits
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        if ws(mid) <= budget:
+            lo = mid
+        else:
+            hi = mid - 1
+    return lo
 
 
 def combine_trains(std, psd, idx):

@@ -174,13 +174,14 @@ def _align(n, a=256):
 class PeerExchange:
     """Peer-shared gathered arrays for the exchange fused into the solve kernel (include/raftk.h ``raftk_peers``).
 
-    Every rank owns ``n_buffers`` copies of ``Xi [world, units_per_rank, 6, nw]`` (+ arrival flags + status words),
+    Every rank owns ``n_buffers`` copies of ``Xi [world, units_per_rank, dof, nw]`` (+ arrival flags + status words; ``dof``
+    is 6 for rigid units, n_dof for the rows of a generalised-DOF shard, ``ShardedGeneralSolve``),
     allocated by the library (cudaMalloc + CUDA IPC handle).  Handles are exchanged once with ``all_gather_object``
     and opened, so rank r's kernel can store its finished units straight into every rank's copy over NVLink -- the
     step has no separate collective.  Two copies alternate between steps because a rank may start the next step
     (and overwrite its block in a peer's copy) while that peer still reads the previous one."""
 
-    def __init__(self, units_per_rank, nw, device, group=None, n_buffers=2):
+    def __init__(self, units_per_rank, nw, device, group=None, n_buffers=2, dof=6):
         import ctypes as C
         import torch
         import torch.distributed as dist
@@ -192,8 +193,8 @@ class PeerExchange:
         if self.world > MAX_PEERS:
             raise ValueError("PeerExchange supports at most %d ranks" % MAX_PEERS)
         self.device = torch.device(device)
-        self.units, self.nw = int(units_per_rank), int(nw)
-        self.block_elems = self.units * 6 * self.nw
+        self.units, self.nw, self.dof = int(units_per_rank), int(nw), int(dof)
+        self.block_elems = self.units * self.dof * self.nw
         self.xi_bytes = self.world * self.block_elems * 16
         self.off_flags = _align(self.xi_bytes)
         self.off_status = self.off_flags + 256
@@ -230,7 +231,7 @@ class PeerExchange:
                 self.peers.append(pr)
                 raw = torch.as_tensor(_DevMem(self.local[b], self.total), device=self.device)
                 self.gathered.append(torch.view_as_complex(raw[:self.xi_bytes].view(torch.float64).view(-1, 2))
-                                     .view(self.world, self.units, 6, self.nw))
+                                     .view(self.world, self.units, self.dof, self.nw))
                 self.status.append(raw[self.off_status:self.off_status + self.world * self.units * 16].view(torch.int32)
                                    .view(self.world, self.units, 4))
             self.timeout = torch.zeros(1, dtype=torch.int32, device=self.device)
@@ -336,6 +337,125 @@ class ShardedSolve:
 
     def close(self):
         self.px.close()
+
+
+def general_groups(primary, n_cases):
+    """Start of every train group (the cases that share a primary) of a case table, plus ``n_cases``: the units the
+    generalised-DOF path never splits.  ``primary`` None: every case is a group.  ValueError when a group is not contiguous
+    in the table (``packer.pack_case_trains`` never builds one)."""
+    n = int(n_cases)
+    if primary is None:
+        return np.arange(n + 1)
+    pr = np.asarray(primary, dtype=np.int64)
+    starts = np.flatnonzero(np.r_[True, pr[1:] != pr[:-1]])
+    if len(np.unique(pr[starts])) != len(starts):
+        raise ValueError("the train groups of cases.primary interleave: every group must be contiguous in the table")
+    return np.r_[starts, n]
+
+
+def general_shards(primary, n_cases, world):
+    """[lo, hi) of every rank: contiguous runs of whole train groups, balanced by case count (each cut at the group start
+    nearest to r * n_cases / world, the later one on a tie).  A rank may get no cases when groups are large."""
+    g = general_groups(primary, n_cases)
+    cuts = [0]
+    for r in range(1, int(world)):
+        t = r * int(n_cases) / int(world)
+        i = int(np.searchsorted(g, t))
+        best = min((c for c in (g[max(i - 1, 0)], g[min(i, len(g) - 1)])), key=lambda c: (abs(c - t), -c))
+        cuts.append(max(int(best), cuts[-1]))
+    cuts.append(int(n_cases))
+    return [(cuts[r], cuts[r + 1]) for r in range(int(world))]
+
+
+def shard_case_table(cases, lo, hi):
+    """Rows [lo, hi) of a ``solver.CaseTable`` as a table of their own (whole train groups: primaries rebased to lo)."""
+    from . import solver
+    a = cases.arrays
+    sub = {k: a[k][lo:hi] for k in ("Hs", "Tp", "gamma", "beta_deg", "spec")}
+    if "primary" in a:
+        sub["primary"] = a["primary"][lo:hi] - lo
+    return solver.CaseTable(sub, zeta=a["zeta"][lo:hi] if "zeta" in a else None)
+
+
+class ShardedGeneralSolve:
+    """A generalised-DOF case table (flexible FOWT, ``solver.GeneralSession``) sharded over GPUs: rank r takes a contiguous,
+    count-balanced run of whole train groups (``general_shards``) and streams it through ``max_chunk_cases`` as
+    ``GeneralSession`` does.  ``step()`` enqueues the solve, then the exchange, and returns (Xi complex [nC, n_dof, nw],
+    status [nC, 4]) of the WHOLE table in table order, valid in stream order on every rank.
+
+    ``exchange="peer"``: the shard's rows are stored into every rank's gathered copy through CUDA IPC peer pointers
+    (raftk_general_publish_dev, ``PeerExchange`` with dof = n_dof, rows padded to the largest shard), then
+    raftk_peer_barrier_dev.  ``exchange="nccl"``: one ``all_gather_into_tensor`` of the padded shards instead.  Status word 3
+    of a secondary train holds its primary's index in the whole table + 1 either way.  With one rank it is the plain solve."""
+
+    def __init__(self, P, M, B, Cm, cases, fd=None, qtf=None, max_chunk_cases=None, group=None, device=None, exchange="peer"):
+        import torch
+        import torch.distributed as dist
+        from . import solver
+        if exchange not in ("peer", "nccl"):
+            raise ValueError("exchange must be 'peer' or 'nccl'")
+        self.torch, self.dist, self.group, self.exchange = torch, dist, group, exchange
+        on = dist.is_available() and dist.is_initialized()
+        self.world = dist.get_world_size(group) if on else 1
+        self.rank = dist.get_rank(group) if on else 0
+        ct = cases if isinstance(cases, solver.CaseTable) else solver.CaseTable(cases)
+        self.n_cases, self.n, self.nw = ct.n_cases, int(P["gen_nDOF"]), len(P["w"])
+        self.bounds = general_shards(ct.arrays.get("primary"), ct.n_cases, self.world)
+        self.lo, self.hi = self.bounds[self.rank]
+        self.rows = max(1, max(h - l for l, h in self.bounds))
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.sess = None
+        if self.hi > self.lo:
+            self.sess = solver.GeneralSession(P, M, B, Cm, shard_case_table(ct, self.lo, self.hi), device=self.device, fd=fd, qtf=qtf,
+                                              max_chunk_cases=max_chunk_cases)
+        self.index = torch.cat([torch.arange(h - l) + r * self.rows for r, (l, h) in enumerate(self.bounds)]).to(self.device)
+        self.px = None
+        if exchange == "peer":
+            self.px = PeerExchange(self.rows, self.nw, self.device, group=group, dof=self.n)
+        else:
+            with torch.cuda.device(self.device):
+                self.x_pad = torch.zeros([self.rows, self.n, self.nw], dtype=torch.complex128, device=self.device)
+                self.s_pad = torch.zeros([self.rows, 4], dtype=torch.int32, device=self.device)
+                self.x_all = torch.empty([self.world * self.rows, self.n, self.nw], dtype=torch.complex128, device=self.device)
+                self.s_all = torch.empty([self.world * self.rows, 4], dtype=torch.int32, device=self.device)
+
+    def step(self, n_iter=10, tol=0.01, xi_start=0.0):
+        import ctypes as C
+        from ._lib import check, lib
+        torch = self.torch
+        m = self.hi - self.lo
+        with torch.cuda.device(self.device):
+            stream = torch.cuda.current_stream(self.device)
+            if self.sess is not None:
+                self.sess.solve(n_iter=n_iter, tol=tol, xi_start=xi_start)
+            if self.px is not None:
+                b, peers = self.px.next()
+                if m:
+                    check(lib.raftk_general_publish_dev(C.byref(peers), self.sess.Xi.data_ptr(), self.sess.status.data_ptr(), self.rank * self.rows,
+                                                        m, self.n, self.nw, self.lo, stream.cuda_stream))
+                check(lib.raftk_peer_barrier_dev(C.byref(peers), self.px.timeout.data_ptr(), stream.cuda_stream))
+                X = self.px.gathered[b].view(self.world * self.rows, self.n, self.nw)
+                S = self.px.status[b].view(self.world * self.rows, 4)
+            else:
+                if m:
+                    self.x_pad[:m].copy_(self.sess.Xi)
+                    st = self.sess.status
+                    self.s_pad[:m].copy_(st)
+                    self.s_pad[:m, 3] = torch.where(st[:, 3] != 0, st[:, 3] + self.lo, st[:, 3])
+                if self.world > 1:
+                    self.dist.all_gather_into_tensor(self.x_all, self.x_pad, group=self.group)
+                    self.dist.all_gather_into_tensor(self.s_all, self.s_pad, group=self.group)
+                    X, S = self.x_all, self.s_all
+                else:
+                    X, S = self.x_pad, self.s_pad
+            return X.index_select(0, self.index), S.index_select(0, self.index)
+
+    def timed_out(self):
+        return bool(self.px.timeout.item()) if self.px is not None else False
+
+    def close(self):
+        if self.px is not None:
+            self.px.close()
 
 
 class PipelinedSolve:
