@@ -492,6 +492,53 @@ int raftk_general_solve_dynamics_stream_host(const raftk_general *g, const raftk
                                              double *F_2nd, double *F_2nd_mean, int32_t max_chunk_cases);
 
 /*
+ * Design batches of FOWTs with generalised degrees of freedom: n_designs flexible designs that share n_dof (one FE topology),
+ * the frequency grid (w, k, nw, dw), depth and rho, solved over one case table in one call.  raft_b200.solver.GeneralBatch
+ * builds the tables.
+ *   raftk_general g:  n_nodes = the total node count; every node array (node_r .. rr, Tn) is the designs' arrays concatenated,
+ *                     design d owning nodes node_offset[d] .. node_offset[d+1]-1 (a design with no submerged node is legal);
+ *                     M, B, C are [n_designs,n_dof,n_dof].
+ *   raftk_general_fd: n_fd and n_bem_head are the same for every design; fd_idx [nD,n_fd], A_w / B_w [nD,n_fd,n_fd,nw],
+ *                     bem_headings [nD,n_bem_head], X_BEM complex [nD,n_bem_head,6,nw], T0 [nD,6,n_dof]; x_ref, y_ref,
+ *                     heading_adjust per design in raftk_general_batch (NULL: fd's scalars for every design).
+ *   raftk_general_qtf: one grid (qtf_w, qtf_heads); the table is per design [nD, n_qtf_w, n_qtf_w, n_qtf_head, 6], or one table
+ *                     for every design (qtf_shared = 1).
+ * Units are (design, case) pairs, design-major (unit d * n_cases + c): every design runs the whole case table, train groups
+ * included.  Xi complex [nD,n_cases,n_dof,nw], status [nD,n_cases,4]; optional F_BEM complex [nD,n_cases,n_dof,nw], F_2nd
+ * [nD,n_cases,6,nw], F_2nd_mean [nD,n_cases,6].  Xi[d] equals raftk_general_solve_dynamics_* on design d alone bit for bit (up
+ * to the atomic sums of k_qtf_tiles, see raftk_general_qtf); status word 3 of a secondary train holds its primary's case index
+ * + 1 within the design.  The units run in chunks of at most max_chunk_units (0: all units in one chunk), cut only at train-group
+ * boundaries and possibly across designs, one after the other on the caller's stream in one workspace sized for the largest
+ * chunk, with no host synchronisation between chunks (the launch sequence of raftk_general_solve_dynamics_stream_*, whose
+ * kernels map every unit to its design's nodes, matrices and tables).  n_designs * n_cases may exceed 65535 when chunks do not.
+ * raftk_general_batch_workspace_bytes(.., K) = raftk_general_qtf_workspace_bytes of min(K, units) units with max_nodes node
+ * rows each, plus the chunk's primary map (K * 4 bytes rounded up to 256) when K < units or n_designs > 1.
+ * Rejected with RAFTK_EINVAL before any launch: every check of the qtf entry, applied to every design's fd rows; n_designs <= 0;
+ * node_offset missing, not starting at 0, decreasing, not ending at n_nodes, or a design with more than max_nodes nodes;
+ * qtf_shared not 0 or 1; max_chunk_units < 0 or a chunk of more than 65535 units; interleaved train groups; a train group with
+ * more cases than max_chunk_units; a workspace smaller than the query.  The *_dev entry reads node_offset, cases.primary, the fd
+ * index and heading rows and the QTF grid back to the host with one wait per call.
+ */
+typedef struct raftk_general_batch {
+    int32_t n_designs;
+    int32_t max_nodes;              /* >= the largest node_offset[d+1] - node_offset[d] (node rows of the workspace)           */
+    int32_t qtf_shared;             /* 0: qtf per design [nD, ...]; 1: one table for every design                            */
+    int32_t _pad0;
+    const int32_t *node_offset;     /* [n_designs + 1] CSR offsets into g's node arrays                                       */
+    const double *x_ref, *y_ref, *heading_adjust;   /* [n_designs] BEM reference point and heading adjustment, or NULL       */
+} raftk_general_batch;
+
+size_t raftk_general_batch_workspace_bytes(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd,
+                                           const raftk_general_qtf *qtf, int32_t n_cases, int32_t max_chunk_units);
+int raftk_general_batch_solve_dynamics_dev(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd,
+                                           const raftk_general_qtf *qtf, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
+                                           int32_t *status, double *F_BEM, double *F_2nd, double *F_2nd_mean, void *workspace,
+                                           size_t workspace_bytes, int32_t max_chunk_units, void *stream);
+int raftk_general_batch_solve_dynamics_host(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd,
+                                            const raftk_general_qtf *qtf, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
+                                            int32_t *status, double *F_BEM, double *F_2nd, double *F_2nd_mean, int32_t max_chunk_units);
+
+/*
  * Output channels of FOWT.saveTurbineOutputs for a FOWT with generalised degrees of freedom (raft_fowt.py:2299-2604): PRP
  * motions, nacelle accelerations and flexible-tower base loads are real linear functionals of the reduced response,
  *   Y_ch(w) = w^wpow[ch] sum_b R[ch,b] Xi[b,w]     (raft_b200.packer.pack_general_channels; rad2deg folded into R)

@@ -95,6 +95,12 @@ class RaftkGeneralQtf(C.Structure):
     _fields_ = [("n_qtf_w", C.c_int32), ("n_qtf_head", C.c_int32), ("qtf_w", C.c_void_p), ("qtf_heads", C.c_void_p), ("qtf", C.c_void_p)]
 
 
+class RaftkGeneralBatch(C.Structure):
+    """A design batch of the generalised-DOF solve, include/raftk.h raftk_general_batch."""
+    _fields_ = [("n_designs", C.c_int32), ("max_nodes", C.c_int32), ("qtf_shared", C.c_int32), ("_pad0", C.c_int32),
+                ("node_offset", C.c_void_p), ("x_ref", C.c_void_p), ("y_ref", C.c_void_p), ("heading_adjust", C.c_void_p)]
+
+
 class RaftkSlender(C.Structure):
     _fields_ = ([("n_nodes", C.c_int32), ("n_members", C.c_int32), ("n_seg", C.c_int32), ("nw", C.c_int32),
                  ("depth", C.c_double), ("rho", C.c_double), ("g", C.c_double)] + [(n, C.c_void_p) for n in SLENDER_ARRAYS])
@@ -154,6 +160,7 @@ SYMBOLS = [
     "raftk_general_fd_workspace_bytes", "raftk_general_solve_dynamics_fd_dev", "raftk_general_solve_dynamics_fd_host",
     "raftk_general_qtf_workspace_bytes", "raftk_general_solve_dynamics_qtf_dev", "raftk_general_solve_dynamics_qtf_host",
     "raftk_general_stream_workspace_bytes", "raftk_general_solve_dynamics_stream_dev", "raftk_general_solve_dynamics_stream_host",
+    "raftk_general_batch_workspace_bytes", "raftk_general_batch_solve_dynamics_dev", "raftk_general_batch_solve_dynamics_host",
     "raftk_system_solve_dev", "raftk_system_solve_host", "raftk_response_stats_dev", "raftk_response_stats_host",
     "raftk_channel_stats_dev", "raftk_channel_stats_host", "raftk_general_channel_stats_dev", "raftk_general_channel_stats_host",
     "raftk_host_alloc", "raftk_host_free",
@@ -247,6 +254,17 @@ def _load():
                                                              C.c_int32]
     lib.raftk_general_solve_dynamics_stream_dev.restype = C.c_int
     lib.raftk_general_solve_dynamics_stream_host.restype = C.c_int
+    lib.raftk_general_batch_workspace_bytes.restype = C.c_size_t
+    lib.raftk_general_batch_workspace_bytes.argtypes = [P(RaftkGeneral), P(RaftkGeneralBatch), P(RaftkGeneralFd), P(RaftkGeneralQtf), C.c_int32,
+                                                        C.c_int32]
+    lib.raftk_general_batch_solve_dynamics_dev.argtypes = [P(RaftkGeneral), P(RaftkGeneralBatch), P(RaftkGeneralFd), P(RaftkGeneralQtf),
+                                                           P(RaftkCases), P(RaftkSolveOpts), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                           C.c_void_p, C.c_void_p, C.c_size_t, C.c_int32, C.c_void_p]
+    lib.raftk_general_batch_solve_dynamics_host.argtypes = [P(RaftkGeneral), P(RaftkGeneralBatch), P(RaftkGeneralFd), P(RaftkGeneralQtf),
+                                                            P(RaftkCases), P(RaftkSolveOpts), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                            C.c_void_p, C.c_int32]
+    lib.raftk_general_batch_solve_dynamics_dev.restype = C.c_int
+    lib.raftk_general_batch_solve_dynamics_host.restype = C.c_int
     lib.raftk_system_solve_dev.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.raftk_system_solve_host.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.raftk_response_stats_dev.argtypes = [C.c_int32, C.c_int32, C.c_double, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

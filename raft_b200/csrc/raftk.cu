@@ -1346,9 +1346,10 @@ extern "C" int raftk_second_order_force_host(const raftk_designs *d, const raftk
 
 // ---- generalised degrees of freedom (flexible members) ---------------------------------------------------------------
 struct GenLayout { size_t u, f6, Fi, Fd, XL, Bm, Bd, Z, pv, fl, fb6, FB, F2, F2m, total; };
-static GenLayout gen_layout(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *q, size_t nC)
+// nC units of Ns_rows node rows each (one design: its n_nodes; a design batch: its largest design's count)
+static GenLayout gen_layout(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *q, size_t nC, int Ns_rows)
 {
-    const size_t n = g->n_dof, nw = g->nw, Ns = std::max(g->n_nodes, 1);
+    const size_t n = g->n_dof, nw = g->nw, Ns = std::max(Ns_rows, 1);
     const size_t nbem = (fd && fd->n_bem_head > 0) ? 1 : 0, nq = q ? 1 : 0;
     GenLayout L; size_t t = 0;
     auto take = [&](size_t b) { size_t o = t; t += align_up(b, 256); return o; };
@@ -1402,7 +1403,7 @@ extern "C" size_t raftk_general_qtf_workspace_bytes(const raftk_general *g, cons
                                                     int32_t n_cases)
 {
     if (!g || n_cases <= 0 || g->n_dof <= 0 || g->nw <= 0) return 0;
-    return gen_layout(g, fd, qtf, (size_t)n_cases).total;
+    return gen_layout(g, fd, qtf, (size_t)n_cases, g->n_nodes).total;
 }
 
 extern "C" size_t raftk_general_fd_workspace_bytes(const raftk_general *g, const raftk_general_fd *fd, int32_t n_cases)
@@ -1446,17 +1447,52 @@ static int gen_validate(const raftk_general *g, const raftk_general_fd *fd, cons
     return 0;
 }
 
-// the launch sequence of one case table (at most 65535 cases) in a workspace of gen_layout(g, fd, qtf, c->n_cases).total bytes;
-// prof_reset: start a new profile record (the streamed entry keeps one record over its chunks)
-static int gen_launch(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, const raftk_cases *c,
-                      const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM, double *F_2nd, double *F_2nd_mean,
-                      void *workspace, cudaStream_t st, bool prof_reset)
+// A design batch as the launch sequence sees it.  nD = 1 with node_off = NULL is one design: the single-design entries run as
+// that batch.  Units are (design, case) pairs, design-major: unit d * n_cases + c.
+struct GenBatch {
+    int nD = 1, max_nodes = 0, qtf_shared = 0;
+    const int32_t *node_off = nullptr;                 // device [nD+1], or NULL (one design)
+    const int32_t *hnode_off = nullptr;                // host copy of node_off (the chunks' node grids), or NULL
+    const double *x_ref = nullptr, *y_ref = nullptr, *hadj = nullptr;      // device [nD], or NULL: fd's scalars
+};
+
+static GenBatch gen_single(const raftk_general *g)
 {
-    const size_t nC = c->n_cases;
-    const GenLayout L = gen_layout(g, fd, qtf, nC);
+    GenBatch B;
+    B.max_nodes = g->n_nodes;
+    return B;
+}
+
+// cases c0 .. c0+m-1 of a case table
+static raftk_cases gen_case_view(const raftk_cases *c, size_t c0, size_t m, size_t nw)
+{
+    raftk_cases cc = *c;
+    cc.n_cases = (int32_t)m;
+    cc.Hs = c->Hs ? c->Hs + c0 : nullptr; cc.Tp = c->Tp ? c->Tp + c0 : nullptr;
+    cc.gamma = c->gamma ? c->gamma + c0 : nullptr; cc.beta_deg = c->beta_deg ? c->beta_deg + c0 : nullptr;
+    cc.spec = c->spec ? c->spec + c0 : nullptr; cc.zeta = c->zeta ? c->zeta + c0 * nw : nullptr;
+    cc.primary = c->primary ? c->primary + c0 : nullptr;
+    return cc;
+}
+
+// the launch sequence of units u0 .. u0+m-1 (m <= 65535) of batch Bt over the case table c, in a workspace of
+// gen_layout(g, fd, qtf, m, Bt.max_nodes).total bytes.  prim: the chunk's primary map as chunk-local units, or NULL; Xi, status,
+// F_BEM, F_2nd, F_2nd_mean: advanced to unit u0.  prof_reset: start a new profile record (a chunked call keeps one record)
+static int gen_launch(const raftk_general *g, const GenBatch &Bt, const raftk_general_fd *fd, const raftk_general_qtf *qtf, const raftk_cases *c,
+                      size_t u0, size_t m, const int *prim, const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM,
+                      double *F_2nd, double *F_2nd_mean, void *workspace, cudaStream_t st, bool prof_reset)
+{
+    const size_t nC = m, nCt = c->n_cases;
+    const GenLayout L = gen_layout(g, fd, qtf, nC, Bt.max_nodes);
     const bool bem = fd && fd->n_bem_head > 0;
+    int Ns_grid = Bt.max_nodes;                        // node grids: the chunk's largest design
+    if (Bt.hnode_off) {
+        Ns_grid = 0;
+        for (size_t d = u0 / nCt; d <= (u0 + m - 1) / nCt; d++) Ns_grid = std::max(Ns_grid, Bt.hnode_off[d + 1] - Bt.hnode_off[d]);
+    }
     GenDev D;
-    D.n = g->n_dof; D.nw = g->nw; D.Ns = g->n_nodes; D.depth = g->depth; D.dw = g->dw; D.rho = g->rho;
+    D.n = g->n_dof; D.nw = g->nw; D.Ns = Bt.max_nodes; D.depth = g->depth; D.dw = g->dw; D.rho = g->rho;
+    D.u0 = (int)u0; D.nCt = (int)nCt; D.node_off = Bt.node_off;
     D.w = g->w; D.k = g->k; D.node_r = g->node_r; D.node_frame = g->node_frame; D.node_circ = g->node_circ;
     D.node_Imat = g->node_Imat; D.node_Imat_w = reinterpret_cast<const double2 *>(g->node_Imat_w);
     D.node_a_i = g->node_a_i; D.node_cd = g->node_cd; D.Tn = g->Tn; D.rr = g->rr; D.M = g->M; D.B = g->B; D.C = g->C;
@@ -1466,6 +1502,7 @@ static int gen_launch(const raftk_general *g, const raftk_general_fd *fd, const 
     Fx.bem_headings = bem ? fd->bem_headings : nullptr; Fx.X_BEM = bem ? reinterpret_cast<const double2 *>(fd->X_BEM) : nullptr;
     Fx.T0 = bem ? fd->T0 : nullptr;
     Fx.x_ref = fd ? fd->x_ref : 0.0; Fx.y_ref = fd ? fd->y_ref : 0.0; Fx.hadj = fd ? fd->heading_adjust : 0.0;
+    Fx.x_ref_d = Bt.x_ref; Fx.y_ref_d = Bt.y_ref; Fx.hadj_d = Bt.hadj;
     char *b = static_cast<char *>(workspace);
     GenWork W;
     W.u = reinterpret_cast<double2 *>(b + L.u); W.f6 = reinterpret_cast<double2 *>(b + L.f6);
@@ -1476,7 +1513,6 @@ static int gen_launch(const raftk_general *g, const raftk_general_fd *fd, const 
     Fx.fb6 = bem ? reinterpret_cast<double2 *>(b + L.fb6) : nullptr;
     double2 *Fbem = bem ? (F_BEM ? reinterpret_cast<double2 *>(F_BEM) : reinterpret_cast<double2 *>(b + L.FB)) : nullptr;
     Fx.F_BEM = Fbem;
-    const int *prim = c->primary;
     CasesDev C = to_dev(c);
     double2 *X = reinterpret_cast<double2 *>(Xi);
     const unsigned fb = (unsigned)((g->nw + 127) / 128);
@@ -1491,18 +1527,28 @@ static int gen_launch(const raftk_general *g, const raftk_general_fd *fd, const 
     if (F_BEM && !bem) CUDA_TRY(cudaMemsetAsync(F_BEM, 0, nC * g->n_dof * g->nw * 16, st));
     double *F2 = nullptr;
     if (qtf) {                                         // second-order force of every case and train (k_qtf_*), before the loop
-        QtfParams QP;
-        QP.nD = 1; QP.shared = 0;
-        QP.n2 = qtf->n_qtf_w; QP.nh = qtf->n_qtf_head; QP.nw = g->nw; QP.dw = g->dw;
-        QP.w = g->w; QP.qw = qtf->qtf_w; QP.qh = qtf->qtf_heads;
-        QP.qtf = reinterpret_cast<const double2 *>(qtf->qtf);
-        QP.F2 = F2 = F_2nd ? F_2nd : reinterpret_cast<double *>(b + L.F2);
-        QP.F2mean = F_2nd_mean ? F_2nd_mean : reinterpret_cast<double *>(b + L.F2m);
-        if (int rc = launch_qtf(QP, c, st)) return rc;
+        F2 = F_2nd ? F_2nd : reinterpret_cast<double *>(b + L.F2);
+        double *F2m = F_2nd_mean ? F_2nd_mean : reinterpret_cast<double *>(b + L.F2m);
+        const size_t nw = g->nw, tab = (size_t)qtf->n_qtf_w * qtf->n_qtf_w * qtf->n_qtf_head * 12;
+        // one launch per run of units with a rectangular (design, case) layout: a partial design, or whole designs
+        for (size_t a = u0; a < u0 + m;) {
+            const size_t d = a / nCt, ca = a % nCt, left = u0 + m - a;
+            const size_t nd = (ca == 0 && left >= nCt) ? left / nCt : 1, ce = (ca == 0 && left >= nCt) ? nCt : std::min(nCt, ca + left);
+            QtfParams QP;
+            QP.nD = (int)nd; QP.shared = Bt.qtf_shared;
+            QP.n2 = qtf->n_qtf_w; QP.nh = qtf->n_qtf_head; QP.nw = g->nw; QP.dw = g->dw;
+            QP.w = g->w; QP.qw = qtf->qtf_w; QP.qh = qtf->qtf_heads;
+            QP.qtf = reinterpret_cast<const double2 *>(qtf->qtf + (Bt.qtf_shared ? 0 : d * tab));
+            QP.F2 = F2 + (a - u0) * 6 * nw;
+            QP.F2mean = F2m + (a - u0) * 6;
+            const raftk_cases cs = gen_case_view(c, ca, ce - ca, nw);
+            if (int rc = launch_qtf(QP, &cs, st)) return rc;
+            a += nd * (ce - ca);
+        }
     }
     if (prof_reset) prof_begin_call();
     k_gen_init<<<(unsigned)nC, 256, 0, st>>>(D, W, o->xi_start, prim);
-    if (g->n_nodes > 0) k_gen_wave<<<dim3(fb, g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, C, W);
+    if (Ns_grid > 0) k_gen_wave<<<dim3(fb, Ns_grid, (unsigned)nC), 128, 0, st>>>(D, C, W);
     if (bem) {                                         // F_BEM = T0^T f_BEM, then F_iner = F_BEM + sum_j Tn_j^T f6_j
         k_gen_bem<<<dim3(fb, (unsigned)nC), 128, 0, st>>>(D, C, Fx);
         k_gen_project<true, false><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, Fbem, 0, nullptr, Fx);
@@ -1516,7 +1562,7 @@ static int gen_launch(const raftk_general *g, const raftk_general_fd *fd, const 
         g_launches++;
     }
     for (int pass = 0; pass < o->n_iter + 1; pass++) {
-        if (g->n_nodes > 0) k_gen_node_pass<false><<<dim3(g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, W, nullptr);
+        if (Ns_grid > 0) k_gen_node_pass<false><<<dim3(Ns_grid, (unsigned)nC), 128, 0, st>>>(D, W, nullptr);
         k_gen_bdrag<<<dim3(g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W);
         k_gen_project<false, false><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_drag, 1, nullptr, Fx);
         if (blocked) {
@@ -1532,7 +1578,7 @@ static int gen_launch(const raftk_general *g, const raftk_general_fd *fd, const 
         g_launches += 5;
     }
     if (prim) {                                        // secondary trains: the primary's last Bmat and LU factors
-        if (g->n_nodes > 0) k_gen_node_pass<true><<<dim3(g->n_nodes, (unsigned)nC), 128, 0, st>>>(D, W, prim);
+        if (Ns_grid > 0) k_gen_node_pass<true><<<dim3(Ns_grid, (unsigned)nC), 128, 0, st>>>(D, W, prim);
         k_gen_project<false, false><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_drag, 0, prim, Fx);
         k_gen_train_solve<<<dim3(g->nw, (unsigned)nC), 128, 0, st>>>(D, W, prim, X);
         g_launches += 3;
@@ -1553,8 +1599,8 @@ extern "C" int raftk_general_solve_dynamics_qtf_dev(const raftk_general *g, cons
     disp_reset();
     cudaStream_t st = (cudaStream_t)stream;
     if (int rc = gen_validate(g, fd, qtf, c, o, Xi, status, 65535, st)) return rc;
-    if (!workspace || workspace_bytes < gen_layout(g, fd, qtf, c->n_cases).total) return set_err(RAFTK_ENOMEM, "general solve: workspace too small");
-    return gen_launch(g, fd, qtf, c, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, st, true);
+    if (!workspace || workspace_bytes < gen_layout(g, fd, qtf, c->n_cases, g->n_nodes).total) return set_err(RAFTK_ENOMEM, "general solve: workspace too small");
+    return gen_launch(g, gen_single(g), fd, qtf, c, 0, c->n_cases, c->primary, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, st, true);
 }
 
 extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
@@ -1637,36 +1683,38 @@ extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const r
     return raftk_general_solve_dynamics_fd_host(g, nullptr, c, o, Xi, status, nullptr);
 }
 
-// ---- generalised DOFs, streamed: the case table in chunks of whole train groups through one bounded workspace ----------
-static size_t gen_chunk_cap(int32_t n_cases, int32_t max_chunk_cases)
+// ---- generalised DOFs, streamed: the units in chunks of whole train groups through one bounded workspace ---------------
+static size_t gen_chunk_cap(int64_t n_units, int32_t max_chunk)
 {
-    return (max_chunk_cases <= 0 || max_chunk_cases >= n_cases) ? (size_t)n_cases : (size_t)max_chunk_cases;
+    return (max_chunk <= 0 || max_chunk >= n_units) ? (size_t)n_units : (size_t)max_chunk;
 }
 
-// chunk-local primary map [K] at the end of the workspace when the table runs in more than one chunk
-static size_t gen_stream_bytes(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, int32_t n_cases,
-                               int32_t max_chunk_cases, size_t *prim_off)
+// gen_layout of the largest chunk, plus the chunk-local primary map [K] at the end when the units run in more than one chunk or
+// span more than one design
+static size_t gen_run_bytes(const raftk_general *g, const GenBatch &Bt, const raftk_general_fd *fd, const raftk_general_qtf *qtf, int64_t n_units,
+                            int32_t max_chunk, size_t *prim_off)
 {
-    const size_t K = gen_chunk_cap(n_cases, max_chunk_cases);
-    const size_t base = gen_layout(g, fd, qtf, K).total;
+    const size_t K = gen_chunk_cap(n_units, max_chunk);
+    const size_t base = gen_layout(g, fd, qtf, K, Bt.max_nodes).total;
     if (prim_off) *prim_off = base;
-    return K < (size_t)n_cases ? base + align_up(K * 4, 256) : base;
+    return (K < (size_t)n_units || Bt.nD > 1) ? base + align_up(K * 4, 256) : base;
 }
 
 extern "C" size_t raftk_general_stream_workspace_bytes(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
                                                        int32_t n_cases, int32_t max_chunk_cases)
 {
     if (!g || n_cases <= 0 || g->n_dof <= 0 || g->nw <= 0) return 0;
-    return gen_stream_bytes(g, fd, qtf, n_cases, max_chunk_cases, nullptr);
+    return gen_run_bytes(g, gen_single(g), fd, qtf, n_cases, max_chunk_cases, nullptr);
 }
 
-// Chunk starts (and the end) of a case table: whole train groups, greedily packed into chunks of at most K cases.  prim: host
-// copy of cases.primary or NULL (every case a group of its own).  A group is the set of cases sharing one primary; it must be
-// contiguous in the table (packer.pack_case_trains lays tables out so) and no larger than K.
-static int gen_plan_chunks(const int32_t *prim, size_t nC, size_t K, std::vector<size_t> &starts)
+// Chunk starts (and the end) of the units of nD designs over a case table: whole train groups, greedily packed into chunks of
+// at most K units; a chunk may cross design boundaries.  prim: host copy of cases.primary or NULL (every case a group of its
+// own).  A group is the set of cases sharing one primary; it must be contiguous in the table (packer.pack_case_trains lays
+// tables out so) and no larger than K.  batch: the batch entry's wording (max_chunk_units).
+static int gen_plan_chunks(const int32_t *prim, size_t nC, size_t nD, size_t K, bool batch, std::vector<size_t> &starts)
 {
     starts.clear();
-    std::vector<size_t> gs;                            // group starts
+    std::vector<size_t> gs;                            // group starts within the case table
     if (prim) {
         std::vector<size_t> first(nC, SIZE_MAX), last(nC, 0), count(nC, 0);
         for (size_t i = 0; i < nC; i++) {
@@ -1683,46 +1731,49 @@ static int gen_plan_chunks(const int32_t *prim, size_t nC, size_t K, std::vector
         for (size_t i = 0; i < nC; i++) gs.push_back(i);
     }
     gs.push_back(nC);
+    for (size_t t = 0; t + 1 < gs.size(); t++)
+        if (gs[t + 1] - gs[t] > K)
+            return set_err(RAFTK_EINVAL, batch ? "general batch: a train group has more cases than max_chunk_units"
+                                               : "general stream: a train group has more cases than max_chunk_cases");
     starts.push_back(0);
-    for (size_t t = 0; t + 1 < gs.size(); t++) {
-        if (gs[t + 1] - gs[t] > K) return set_err(RAFTK_EINVAL, "general stream: a train group has more cases than max_chunk_cases");
-        if (gs[t + 1] - starts.back() > K) starts.push_back(gs[t]);
-    }
-    starts.push_back(nC);
+    for (size_t d = 0; d < nD; d++)
+        for (size_t t = 0; t + 1 < gs.size(); t++)
+            if (d * nC + gs[t + 1] - starts.back() > K) starts.push_back(d * nC + gs[t]);
+    starts.push_back(nD * nC);
     return 0;
 }
 
 // the chunk loop on device pointers; hprim: host copy of c->primary (NULL without trains)
-static int gen_stream_run(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, const raftk_cases *c,
-                          const int32_t *hprim, const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM, double *F_2nd,
-                          double *F_2nd_mean, void *workspace, size_t workspace_bytes, int32_t max_chunk_cases, cudaStream_t st)
+static int gen_run(const raftk_general *g, const GenBatch &Bt, const raftk_general_fd *fd, const raftk_general_qtf *qtf, const raftk_cases *c,
+                   const int32_t *hprim, const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM, double *F_2nd,
+                   double *F_2nd_mean, void *workspace, size_t workspace_bytes, int32_t max_chunk, bool batch, cudaStream_t st)
 {
-    const size_t nC = c->n_cases, K = gen_chunk_cap(c->n_cases, max_chunk_cases);
-    if (K > 65535) return set_err(RAFTK_EINVAL, "general stream: a chunk takes at most 65535 cases (max_chunk_cases)");
+    const size_t nC = c->n_cases, nU = (size_t)Bt.nD * nC, K = gen_chunk_cap((int64_t)nU, max_chunk);
+    if (K > 65535)
+        return set_err(RAFTK_EINVAL, batch ? "general batch: a chunk takes at most 65535 units (max_chunk_units)"
+                                           : "general stream: a chunk takes at most 65535 cases (max_chunk_cases)");
     std::vector<size_t> starts;
-    if (int rc = gen_plan_chunks(hprim, nC, K, starts)) return rc;
+    if (int rc = gen_plan_chunks(hprim, nC, Bt.nD, K, batch, starts)) return rc;
     size_t prim_off = 0;
-    const size_t need = gen_stream_bytes(g, fd, qtf, c->n_cases, max_chunk_cases, &prim_off);
-    if (!workspace || workspace_bytes < need) return set_err(RAFTK_EINVAL, "general stream: workspace smaller than raftk_general_stream_workspace_bytes()");
+    const size_t need = gen_run_bytes(g, Bt, fd, qtf, (int64_t)nU, max_chunk, &prim_off);
+    if (!workspace || workspace_bytes < need)
+        return set_err(RAFTK_EINVAL, batch ? "general batch: workspace smaller than raftk_general_batch_workspace_bytes()"
+                                           : "general stream: workspace smaller than raftk_general_stream_workspace_bytes()");
     int *local = reinterpret_cast<int *>(static_cast<char *>(workspace) + prim_off);
     const size_t n = g->n_dof, nw = g->nw, nch = starts.size() - 1;
     for (size_t k = 0; k < nch; k++) {
-        const size_t c0 = starts[k], m = starts[k + 1] - c0;
-        raftk_cases cc = *c;
-        cc.n_cases = (int32_t)m;
-        cc.Hs = c->Hs ? c->Hs + c0 : nullptr; cc.Tp = c->Tp ? c->Tp + c0 : nullptr;
-        cc.gamma = c->gamma ? c->gamma + c0 : nullptr; cc.beta_deg = c->beta_deg ? c->beta_deg + c0 : nullptr;
-        cc.spec = c->spec ? c->spec + c0 : nullptr; cc.zeta = c->zeta ? c->zeta + c0 * nw : nullptr;
-        if (c->primary && nch > 1) {                   // absolute primaries -> chunk-local ones
-            k_gen_chunk_primary<<<(unsigned)((m + 127) / 128), 128, 0, st>>>((int)m, (int)c0, c->primary, local);
+        const size_t u0 = starts[k], m = starts[k + 1] - u0;
+        const int *prim = c->primary;
+        if (c->primary && (nch > 1 || Bt.nD > 1)) {    // table primaries -> chunk-local units
+            k_gen_chunk_primary<<<(unsigned)((m + 127) / 128), 128, 0, st>>>((int)m, (int)u0, (int)nC, c->primary, local);
             g_launches++;
-            cc.primary = local;
+            prim = local;
         }
-        if (int rc = gen_launch(g, fd, qtf, &cc, o, Xi + c0 * n * nw * 2, status + c0 * 4, F_BEM ? F_BEM + c0 * n * nw * 2 : nullptr,
-                                F_2nd ? F_2nd + c0 * 6 * nw : nullptr, F_2nd_mean ? F_2nd_mean + c0 * 6 : nullptr, workspace, st, k == 0))
+        if (int rc = gen_launch(g, Bt, fd, qtf, c, u0, m, prim, o, Xi + u0 * n * nw * 2, status + u0 * 4, F_BEM ? F_BEM + u0 * n * nw * 2 : nullptr,
+                                F_2nd ? F_2nd + u0 * 6 * nw : nullptr, F_2nd_mean ? F_2nd_mean + u0 * 6 : nullptr, workspace, st, k == 0))
             return rc;
-        if (c->primary && c0 > 0) {                    // status word 3 of the secondaries: the table's primary + 1
-            k_gen_status_rebase<<<(unsigned)((m + 127) / 128), 128, 0, st>>>((int)m, (int)c0, status + c0 * 4);
+        if (c->primary && (u0 % nC != 0 || u0 % nC + m > nC)) {      // status word 3 of the secondaries: the primary's case + 1
+            k_gen_status_rebase<<<(unsigned)((m + 127) / 128), 128, 0, st>>>((int)m, (int)u0, (int)nC, status + u0 * 4);
             g_launches++;
         }
     }
@@ -1746,8 +1797,8 @@ extern "C" int raftk_general_solve_dynamics_stream_dev(const raftk_general *g, c
         CUDA_TRY(cudaMemcpyAsync(hp.data(), c->primary, hp.size() * 4, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
     }
-    return gen_stream_run(g, fd, qtf, c, c->primary ? hp.data() : nullptr, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace,
-                          workspace_bytes, max_chunk_cases, st);
+    return gen_run(g, gen_single(g), fd, qtf, c, c->primary ? hp.data() : nullptr, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace,
+                   workspace_bytes, max_chunk_cases, false, st);
 }
 
 extern "C" int raftk_general_solve_dynamics_stream_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
@@ -1763,7 +1814,7 @@ extern "C" int raftk_general_solve_dynamics_stream_host(const raftk_general *g, 
     const size_t n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases, K = gen_chunk_cap(c->n_cases, max_chunk_cases);
     if (K > 65535) return set_err(RAFTK_EINVAL, "general stream: a chunk takes at most 65535 cases (max_chunk_cases)");
     std::vector<size_t> starts;                        // the plan's checks, before anything is staged
-    if (int rc = gen_plan_chunks(c->primary, nC, K, starts)) return rc;
+    if (int rc = gen_plan_chunks(c->primary, nC, 1, K, false, starts)) return rc;
     if (fd)
         if (int rc = validate_gen_fd(g, fd, fd->fd_idx, fd->bem_headings)) return rc;
     if (qtf) {
@@ -1801,8 +1852,149 @@ extern "C" int raftk_general_solve_dynamics_stream_host(const raftk_general *g, 
     S.out(dF2, qtf && F_2nd ? nC * 6 * nw : 0, F_2nd); S.out(dF2m, qtf && F_2nd_mean ? nC * 6 : 0, F_2nd_mean);
     S.buf(ws, wb);
     int rc = S.commit();
-    if (rc || (rc = gen_stream_run(&gg, fd ? &ff : nullptr, qtf ? &qq : nullptr, &cc, c->primary, o, dXi, dStatus, dF_BEM, dF2, dF2m, ws, wb,
-                             max_chunk_cases, nullptr))) return rc;
+    if (rc || (rc = gen_run(&gg, gen_single(&gg), fd ? &ff : nullptr, qtf ? &qq : nullptr, &cc, c->primary, o, dXi, dStatus, dF_BEM, dF2, dF2m, ws,
+                            wb, max_chunk_cases, false, nullptr))) return rc;
+    return S.finish();
+}
+
+// ---- generalised DOFs, design batches: designs sharing n_dof, the frequency grid, depth and rho ------------------------
+static GenBatch gen_batch_of(const raftk_general_batch *b)
+{
+    GenBatch B;
+    B.nD = b->n_designs; B.max_nodes = b->max_nodes; B.qtf_shared = b->qtf_shared;
+    B.node_off = b->node_offset; B.x_ref = b->x_ref; B.y_ref = b->y_ref; B.hadj = b->heading_adjust;
+    return B;
+}
+
+// checks on counts and pointers, before anything is read back or staged
+static int gen_batch_counts(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                            const raftk_cases *c, const raftk_solve_opts *o, const double *Xi, const int32_t *status, int32_t max_chunk_units)
+{
+    if (!g || !b || !c || !o || !Xi || !status || !b->node_offset) return set_err(RAFTK_EINVAL, "general batch: null argument");
+    if (b->n_designs <= 0 || b->max_nodes < 0) return set_err(RAFTK_EINVAL, "general batch: n_designs > 0 and max_nodes >= 0");
+    if (g->n_dof <= 0 || g->n_dof > 256 || g->nw <= 0 || g->n_nodes < 0 || c->n_cases <= 0)
+        return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
+    if ((int64_t)b->n_designs * c->n_cases > INT32_MAX) return set_err(RAFTK_EINVAL, "general batch: n_designs * n_cases must stay below 2^31");
+    if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
+    if (max_chunk_units < 0) return set_err(RAFTK_EINVAL, "general batch: max_chunk_units must be >= 0 (0: all units)");
+    if (gen_chunk_cap((int64_t)b->n_designs * c->n_cases, max_chunk_units) > 65535)
+        return set_err(RAFTK_EINVAL, "general batch: a chunk takes at most 65535 units (max_chunk_units)");
+    if (b->qtf_shared < 0 || b->qtf_shared > 1) return set_err(RAFTK_EINVAL, "general batch: qtf_shared must be 0 or 1");
+    if (qtf)
+        if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
+    if (fd && (fd->n_fd < 0 || fd->n_fd > g->n_dof || fd->n_bem_head < 0 || (fd->n_fd > 0 && (!fd->fd_idx || !fd->A_w || !fd->B_w)) ||
+               (fd->n_bem_head > 0 && (!fd->bem_headings || !fd->X_BEM || !fd->T0))))
+        return validate_gen_fd(g, fd, nullptr, nullptr);
+    return 0;
+}
+
+// checks on host copies of node_offset, every design's fd_idx and bem_headings rows, qtf_w and qtf_heads
+static int gen_batch_tables(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                            const int32_t *off, const int32_t *idx, const double *hd, const double *qw, const double *qh)
+{
+    const int nD = b->n_designs;
+    if (off[0] != 0) return set_err(RAFTK_EINVAL, "general batch: node_offset must start at 0");
+    for (int d = 0; d < nD; d++) {
+        if (off[d + 1] < off[d]) return set_err(RAFTK_EINVAL, "general batch: node_offset must be non-decreasing");
+        if (off[d + 1] - off[d] > b->max_nodes) return set_err(RAFTK_EINVAL, "general batch: a design has more nodes than max_nodes");
+    }
+    if (off[nD] != g->n_nodes) return set_err(RAFTK_EINVAL, "general batch: node_offset[n_designs] must equal n_nodes");
+    if (fd)
+        for (int d = 0; d < nD; d++)
+            if (int rc = validate_gen_fd(g, fd, idx + (size_t)d * fd->n_fd, hd + (size_t)d * fd->n_bem_head)) return rc;
+    if (qtf)
+        if (int rc = validate_gen_qtf(g, qtf, qw, qh)) return rc;
+    return 0;
+}
+
+extern "C" size_t raftk_general_batch_workspace_bytes(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd,
+                                                      const raftk_general_qtf *qtf, int32_t n_cases, int32_t max_chunk_units)
+{
+    if (!g || !b || n_cases <= 0 || b->n_designs <= 0 || b->max_nodes < 0 || g->n_dof <= 0 || g->nw <= 0) return 0;
+    const int64_t nU = (int64_t)b->n_designs * n_cases;
+    if (nU > INT32_MAX) return 0;
+    return gen_run_bytes(g, gen_batch_of(b), fd, qtf, nU, max_chunk_units, nullptr);
+}
+
+extern "C" int raftk_general_batch_solve_dynamics_dev(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd,
+                                                      const raftk_general_qtf *qtf, const raftk_cases *c, const raftk_solve_opts *o,
+                                                      double *Xi, int32_t *status, double *F_BEM, double *F_2nd, double *F_2nd_mean,
+                                                      void *workspace, size_t workspace_bytes, int32_t max_chunk_units, void *stream)
+{
+    disp_reset();
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = gen_batch_counts(g, b, fd, qtf, c, o, Xi, status, max_chunk_units)) return rc;
+    const size_t nD = b->n_designs, nf = fd ? fd->n_fd : 0, nh = fd ? fd->n_bem_head : 0;
+    // every table the checks and the chunk plan need, read back with one wait
+    std::vector<int32_t> off(nD + 1), hp(c->primary ? c->n_cases : 0), idx(nD * nf);
+    std::vector<double> hd(nD * nh), qw(qtf ? qtf->n_qtf_w : 0), qh(qtf ? qtf->n_qtf_head : 0);
+    auto back = [&](void *h, const void *d, size_t bytes) { return bytes ? cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, st) : cudaSuccess; };
+    CUDA_TRY(back(off.data(), b->node_offset, off.size() * 4));
+    CUDA_TRY(back(hp.data(), c->primary, hp.size() * 4));
+    CUDA_TRY(back(idx.data(), fd ? fd->fd_idx : nullptr, idx.size() * 4));
+    CUDA_TRY(back(hd.data(), fd ? fd->bem_headings : nullptr, hd.size() * 8));
+    CUDA_TRY(back(qw.data(), qtf ? qtf->qtf_w : nullptr, qw.size() * 8));
+    CUDA_TRY(back(qh.data(), qtf ? qtf->qtf_heads : nullptr, qh.size() * 8));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (int rc = gen_batch_tables(g, b, fd, qtf, off.data(), idx.data(), hd.data(), qw.data(), qh.data())) return rc;
+    GenBatch Bt = gen_batch_of(b);
+    Bt.hnode_off = off.data();
+    return gen_run(g, Bt, fd, qtf, c, c->primary ? hp.data() : nullptr, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, workspace_bytes,
+                   max_chunk_units, true, st);
+}
+
+extern "C" int raftk_general_batch_solve_dynamics_host(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd,
+                                                       const raftk_general_qtf *qtf, const raftk_cases *c, const raftk_solve_opts *o,
+                                                       double *Xi, int32_t *status, double *F_BEM, double *F_2nd, double *F_2nd_mean,
+                                                       int32_t max_chunk_units)
+{
+    disp_reset();
+    if (int rc = gen_batch_counts(g, b, fd, qtf, c, o, Xi, status, max_chunk_units)) return rc;
+    if (int rc = gen_batch_tables(g, b, fd, qtf, b->node_offset, fd ? fd->fd_idx : nullptr, fd ? fd->bem_headings : nullptr,
+                                  qtf ? qtf->qtf_w : nullptr, qtf ? qtf->qtf_heads : nullptr)) return rc;
+    const size_t nD = b->n_designs, n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases, nU = nD * nC;
+    std::vector<size_t> starts;                        // the plan's checks, before anything is staged
+    if (int rc = gen_plan_chunks(c->primary, nC, nD, gen_chunk_cap((int64_t)nU, max_chunk_units), true, starts)) return rc;
+    Staging S("raftk_general_batch_solve_dynamics_host");
+    raftk_general gg = *g;
+    S.in(gg.w, g->w, nw); S.in(gg.k, g->k, nw);
+    S.in(gg.node_r, g->node_r, Ns * 3); S.in(gg.node_frame, g->node_frame, Ns * 9);
+    S.in(gg.node_circ, g->node_circ, Ns); S.in(gg.node_Imat, g->node_Imat, Ns * 9);
+    S.in(gg.node_Imat_w, g->node_Imat_w, Ns * 9 * nw * 2); S.in(gg.node_a_i, g->node_a_i, Ns);
+    S.in(gg.node_cd, g->node_cd, Ns * 4); S.in(gg.Tn, g->Tn, Ns * 6 * n); S.in(gg.rr, g->rr, Ns * 3);
+    S.in(gg.M, g->M, nD * n * n); S.in(gg.B, g->B, nD * n * n); S.in(gg.C, g->C, nD * n * n);
+    raftk_general_batch bb = *b;
+    S.in(bb.node_offset, b->node_offset, nD + 1);
+    S.in(bb.x_ref, b->x_ref, nD); S.in(bb.y_ref, b->y_ref, nD); S.in(bb.heading_adjust, b->heading_adjust, nD);
+    raftk_cases cc = *c;
+    S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
+    S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC); S.in(cc.zeta, c->zeta, nC * nw);
+    S.in(cc.primary, c->primary, nC);
+    raftk_general_fd ff = fd ? *fd : raftk_general_fd{};
+    if (fd) {
+        const size_t nf = fd->n_fd, nh = fd->n_bem_head;
+        S.in(ff.fd_idx, fd->fd_idx, nD * nf); S.in(ff.A_w, fd->A_w, nD * nf * nf * nw); S.in(ff.B_w, fd->B_w, nD * nf * nf * nw);
+        S.in(ff.bem_headings, fd->bem_headings, nD * nh); S.in(ff.X_BEM, fd->X_BEM, nD * nh * 6 * nw * 2); S.in(ff.T0, fd->T0, nh ? nD * 6 * n : 0);
+    }
+    raftk_general_qtf qq = qtf ? *qtf : raftk_general_qtf{};
+    if (qtf) {
+        const size_t n2 = qtf->n_qtf_w, nh = qtf->n_qtf_head;
+        S.in(qq.qtf_w, qtf->qtf_w, n2); S.in(qq.qtf_heads, qtf->qtf_heads, nh);
+        S.in(qq.qtf, qtf->qtf, (b->qtf_shared ? 1 : nD) * n2 * n2 * nh * 12);
+    }
+    double *dXi, *dF_BEM, *dF2, *dF2m;
+    int32_t *dStatus;
+    char *ws;
+    const size_t wb = raftk_general_batch_workspace_bytes(g, b, fd, qtf, c->n_cases, max_chunk_units);
+    S.out(dXi, nU * n * nw * 2, Xi); S.out(dStatus, nU * 4, status); S.out(dF_BEM, F_BEM ? nU * n * nw * 2 : 0, F_BEM);
+    S.out(dF2, qtf && F_2nd ? nU * 6 * nw : 0, F_2nd); S.out(dF2m, qtf && F_2nd_mean ? nU * 6 : 0, F_2nd_mean);
+    S.buf(ws, wb);
+    int rc = S.commit();
+    if (rc) return rc;
+    GenBatch Bt = gen_batch_of(&bb);
+    Bt.hnode_off = b->node_offset;
+    if ((rc = gen_run(&gg, Bt, fd ? &ff : nullptr, qtf ? &qq : nullptr, &cc, c->primary, o, dXi, dStatus, dF_BEM, dF2, dF2m, ws, wb,
+                      max_chunk_units, true, nullptr))) return rc;
     return S.finish();
 }
 

@@ -25,7 +25,9 @@
 #pragma once
 
 struct GenDev {
-    int n, nw, Ns;
+    int n, nw, Ns;               // Ns: node rows per unit in the workspace (a design batch: its largest design's count)
+    int u0, nCt;                 // unit u of a launch is unit u0 + u of the call = design d * nCt + case c (gen_unit)
+    const int *node_off;         // [nD+1] CSR node offsets of a design batch, or NULL: one design of Ns nodes
     double depth, dw;
     const double *w, *k;
     const double *node_r;        // [Ns][3]
@@ -37,20 +39,34 @@ struct GenDev {
     const double *node_cd;       // [Ns][4]  a_q Cd_q, a_p1 Cd_p1, a_p2 Cd_p2, a_End Cd_End
     const double *Tn;            // [Ns][6][n]
     const double *rr;            // [Ns][3]
-    const double *M, *B, *C;     // [n][n]
+    const double *M, *B, *C;     // [nD][n][n]
     double rho;
 };
 
+// unit u of a launch -> its design d, case c (index into the whole case table), first node j0 and node count Ns.  Node-indexed
+// grids run over the largest count of the chunk; blocks past their design's count return.
+struct GenUnit { int d, c, j0, Ns; };
+__device__ __forceinline__ GenUnit gen_unit(const GenDev &D, int u)
+{
+    GenUnit U;
+    const int t = D.u0 + u;
+    U.d = t / D.nCt; U.c = t - U.d * D.nCt;
+    U.j0 = D.node_off ? D.node_off[U.d] : 0;
+    U.Ns = D.node_off ? D.node_off[U.d + 1] - U.j0 : D.Ns;
+    return U;
+}
+
 // frequency-dependent terms (raftk_general_fd), a parameter of their own so that every kernel of the constant-matrix solve
-// keeps its parameter layout; n_fd = 0 / n_bem_head = 0 without them
+// keeps its parameter layout; n_fd = 0 / n_bem_head = 0 without them.  Tables carry a leading design axis [nD].
 struct GenFdDev {
     int n_fd, n_bem_head;
-    const int *fd_idx;           // [n_fd] strictly increasing reduced DOFs
-    const double *A_w, *B_w;     // [n_fd][n_fd][nw]
-    const double *bem_headings;  // [n_bem_head] deg
-    const double2 *X_BEM;        // [n_bem_head][6][nw] heading-relative
-    const double *T0;            // [6][n] rows 0..5 of fowt.T
+    const int *fd_idx;           // [nD][n_fd] strictly increasing reduced DOFs
+    const double *A_w, *B_w;     // [nD][n_fd][n_fd][nw]
+    const double *bem_headings;  // [nD][n_bem_head] deg
+    const double2 *X_BEM;        // [nD][n_bem_head][6][nw] heading-relative
+    const double *T0;            // [nD][6][n] rows 0..5 of fowt.T
     double x_ref, y_ref, hadj;
+    const double *x_ref_d, *y_ref_d, *hadj_d;   // [nD] per design, or NULL: x_ref, y_ref, hadj for every design
     double2 *fb6;                // [nC][6][nw] workspace: BEM force in full DOFs 0-5
     const double2 *F_BEM;        // [nC][n][nw] BEM force in reduced DOFs, added to F_iner
 };
@@ -70,13 +86,15 @@ struct GenWork {                 // per-call workspace views
 // k_gen_wave: grid (ceil(nw/128), Ns, nC), block 128
 __global__ void __launch_bounds__(128) k_gen_wave(GenDev D, CasesDev Cs, GenWork W)
 {
-    const int i = blockIdx.x * 128 + threadIdx.x, j = blockIdx.y, c = blockIdx.z;
+    const int i = blockIdx.x * 128 + threadIdx.x, j = blockIdx.y, un = blockIdx.z;
     if (i >= D.nw) return;
-    const int nw = D.nw;
+    const GenUnit U = gen_unit(D, un);
+    if (j >= U.Ns) return;
+    const int nw = D.nw, c = U.c, jn = U.j0 + j;
     const double w = D.w[i], k = D.k[i], h = D.depth;
     const double beta = Cs.beta_deg[c] * (CUDART_PI / 180.0);
     const double zeta0 = sea_state_zeta(Cs, c, i, nw, w, D.dw);
-    const double *r = D.node_r + 3 * j, *q = D.node_frame + 9 * j, *rr = D.rr + 3 * j;
+    const double *r = D.node_r + 3 * jn, *q = D.node_frame + 9 * jn, *rr = D.rr + 3 * jn;
     double sb, cb, sp, cp;
     sincos(beta, &sb, &cb);
     sincos(-(k * (cb * r[0] + sb * r[1])), &sp, &cp);
@@ -95,16 +113,16 @@ __global__ void __launch_bounds__(128) k_gen_wave(GenDev D, CasesDev Cs, GenWork
         double fr = 0.0, fi = 0.0;
         for (int b = 0; b < 3; b++) {
             if (D.node_Imat_w) {
-                const double2 m = D.node_Imat_w[((size_t)j * 9 + 3 * a + b) * nw + i];
+                const double2 m = D.node_Imat_w[((size_t)jn * 9 + 3 * a + b) * nw + i];
                 fr += m.x * ud[b].x - m.y * ud[b].y; fi += m.x * ud[b].y + m.y * ud[b].x;
             } else {
-                const double m = D.node_Imat[9 * j + 3 * a + b];
+                const double m = D.node_Imat[9 * jn + 3 * a + b];
                 fr += m * ud[b].x; fi += m * ud[b].y;
             }
         }
-        f[a] = make_double2(fr + pr * D.node_a_i[j] * q[a], fi + pi * D.node_a_i[j] * q[a]);
+        f[a] = make_double2(fr + pr * D.node_a_i[jn] * q[a], fi + pi * D.node_a_i[jn] * q[a]);
     }
-    const size_t ub = (((size_t)c * D.Ns + j) * 3) * nw + i, fb = (((size_t)c * D.Ns + j) * 6) * nw + i;
+    const size_t ub = (((size_t)un * D.Ns + j) * 3) * nw + i, fb = (((size_t)un * D.Ns + j) * 6) * nw + i;
     for (int a = 0; a < 3; a++) { W.u[ub + (size_t)a * nw] = u[a]; W.f6[fb + (size_t)a * nw] = f[a]; }
     // moments rr x f (translateForce3to6DOF)
     W.f6[fb + (size_t)3 * nw] = make_double2(rr[1] * f[2].x - rr[2] * f[1].x, rr[1] * f[2].y - rr[2] * f[1].y);
@@ -114,7 +132,7 @@ __global__ void __launch_bounds__(128) k_gen_wave(GenDev D, CasesDev Cs, GenWork
 
 // k_gen_project: F[c][dof][i] = sum_j sum_b T_j[b][dof] f6_j[b][i] over Ns loads f6 [nC][Ns][6][nw] with their 6 x n blocks
 // T [Ns][6][n]: the strip nodes' Tn and node loads (BEM = false), or T0 and the BEM force of k_gen_bem (BEM = true, Ns = 1);
-// plus X.F_BEM with ADD (F_iner = F_BEM + ...).  grid (ceil(nw/128), n, nC), block 128.  sec_only (the primary map)
+// plus X.F_BEM with ADD (F_iner = F_BEM + ...).  grid (ceil(nw/128), n, units), block 128.  sec_only (the primary map)
 // restricts it to the secondary trains.
 template <bool BEM, bool ADD>
 __global__ void __launch_bounds__(128) k_gen_project(GenDev D, GenWork W, double2 *F, int skip_done, const int *sec_only, GenFdDev X)
@@ -122,9 +140,10 @@ __global__ void __launch_bounds__(128) k_gen_project(GenDev D, GenWork W, double
     const int i = blockIdx.x * 128 + threadIdx.x, dof = blockIdx.y, c = blockIdx.z;
     if (i >= D.nw || (skip_done && W.flags[4 * c]) || (sec_only && sec_only[c] == c)) return;
     const int nw = D.nw, n = D.n;
+    const GenUnit U = gen_unit(D, c);
     double sr = 0.0, si = 0.0;
-    for (int j = 0; j < (BEM ? 1 : D.Ns); j++) {
-        const double *T = (BEM ? X.T0 : D.Tn) + (size_t)j * 6 * n + dof;
+    for (int j = 0; j < (BEM ? 1 : U.Ns); j++) {
+        const double *T = (BEM ? X.T0 + (size_t)U.d * 6 * n : D.Tn + (size_t)(U.j0 + j) * 6 * n) + dof;
         const double2 *f = (BEM ? X.fb6 : W.f6) + (((size_t)c * (BEM ? 1 : D.Ns) + j) * 6) * nw + i;
 #pragma unroll
         for (int b = 0; b < 6; b++) {
@@ -137,25 +156,28 @@ __global__ void __launch_bounds__(128) k_gen_project(GenDev D, GenWork W, double
     F[((size_t)c * n + dof) * nw + i] = make_double2(sr, si);
 }
 
-// k_gen_bem: grid (ceil(nw/128), nC), block 128: BEM excitation of every case (secondary trains with their own heading and
+// k_gen_bem: grid (ceil(nw/128), units), block 128: BEM excitation of every case (secondary trains with their own heading and
 // sea state, raft_model.py:1200-1236) in full DOFs 0-5, from the rigid solvers' bem_excitation_table
 __global__ void __launch_bounds__(128) k_gen_bem(GenDev D, CasesDev Cs, GenFdDev X)
 {
-    const int i = blockIdx.x * 128 + threadIdx.x, c = blockIdx.y;
+    const int i = blockIdx.x * 128 + threadIdx.x, u = blockIdx.y;
     if (i >= D.nw) return;
     const int nw = D.nw;
+    const GenUnit U = gen_unit(D, u);
+    const int c = U.c, d = U.d, nh = X.n_bem_head;
     const double beta = Cs.beta_deg[c] * (CUDART_PI / 180.0);
     double sb, cb;
     sincos(beta, &sb, &cb);
     const double zeta = sea_state_zeta(Cs, c, i, nw, D.w[i], D.dw);
     double Br[6], Bi[6];
-    bem_excitation_table(X.bem_headings, X.n_bem_head, X.X_BEM, nw, X.x_ref, X.y_ref, X.hadj, i, D.k[i], beta, sb, cb, zeta, Br, Bi);
-    double2 *f = X.fb6 + (size_t)c * 6 * nw + i;
+    bem_excitation_table(X.bem_headings + (size_t)d * nh, nh, X.X_BEM + (size_t)d * nh * 6 * nw, nw, X.x_ref_d ? X.x_ref_d[d] : X.x_ref,
+                         X.y_ref_d ? X.y_ref_d[d] : X.y_ref, X.hadj_d ? X.hadj_d[d] : X.hadj, i, D.k[i], beta, sb, cb, zeta, Br, Bi);
+    double2 *f = X.fb6 + (size_t)u * 6 * nw + i;
 #pragma unroll
     for (int a = 0; a < 6; a++) f[(size_t)a * nw] = make_double2(Br[a], Bi[a]);
 }
 
-// k_gen_add_2nd: grid (ceil(nw/128), 6, nC), block 128: the second-order force of every case and train (real amplitudes
+// k_gen_add_2nd: grid (ceil(nw/128), 6, units), block 128: the second-order force of every case and train (real amplitudes
 // [nC][6][nw] of k_qtf_tiles / k_qtf_force) added to reduced rows 0-5 of F_iner, which already hold F_BEM + F_iner:
 // (F_BEM + F_iner) + F_2nd (raft_model.py:1048, 1212; lumped on the first 6 DOFs, :1034)
 __global__ void __launch_bounds__(128) k_gen_add_2nd(GenDev D, GenWork W, const double *F2)
@@ -166,34 +188,46 @@ __global__ void __launch_bounds__(128) k_gen_add_2nd(GenDev D, GenWork W, const 
     f.x = f.x + F2[((size_t)c * 6 + a) * D.nw + i];
 }
 
-// DOF -> position on the support of the frequency-dependent terms (-1 off it), built once per CTA in shared memory
-__device__ __forceinline__ void gen_fd_map(const GenDev &D, const GenFdDev &X, int *fdpos, int tid, int nthr)
+// DOF -> position on the support of design d's frequency-dependent terms (-1 off it), built once per CTA in shared memory
+__device__ __forceinline__ void gen_fd_map(const GenDev &D, const GenFdDev &X, int d, int *fdpos, int tid, int nthr)
 {
+    const int *idx = X.fd_idx + (size_t)d * X.n_fd;
     for (int t = tid; t < D.n; t += nthr) fdpos[t] = -1;
     __syncthreads();
-    for (int t = tid; t < X.n_fd; t += nthr) fdpos[X.fd_idx[t]] = t;
+    for (int t = tid; t < X.n_fd; t += nthr) fdpos[idx[t]] = t;
     __syncthreads();
+}
+
+// one design's constant matrices and frequency-dependent tables
+struct GenMats { const double *M, *B, *C, *A_w, *B_w; };
+__device__ __forceinline__ GenMats gen_mats(const GenDev &D, const GenFdDev &X, int d)
+{
+    const size_t nn = (size_t)D.n * D.n, ff = (size_t)X.n_fd * X.n_fd * D.nw;
+    GenMats G;
+    G.M = D.M + d * nn; G.B = D.B + d * nn; G.C = D.C + d * nn;
+    G.A_w = X.A_w ? X.A_w + d * ff : nullptr; G.B_w = X.B_w ? X.B_w + d * ff : nullptr;
+    return G;
 }
 
 // impedance entry t = a n + b at frequency i (raft_model.py:1086).  On the support: M + A_w and (B + B_w) + B_drag with the
 // rigid solver's grouping (raftk_fused.cuh); elsewhere the constant-matrix expression.  FD = false (n_fd = 0) is the
 // constant-matrix kernel as it was, instruction for instruction: no map, no branch
 template <bool FD>
-__device__ __forceinline__ double2 gen_impedance(const GenDev &D, const GenFdDev &X, const int *fdpos, const double *Bd, int t, int i, double w,
-                                                 double w2)
+__device__ __forceinline__ double2 gen_impedance(const GenDev &D, const GenFdDev &X, const GenMats &G, const int *fdpos, const double *Bd, int t,
+                                                 int i, double w, double w2)
 {
     if constexpr (FD) {
         const int pa = fdpos[t / D.n], pb = fdpos[t % D.n];
         if (pa >= 0 && pb >= 0) {
             const size_t e = ((size_t)pa * X.n_fd + pb) * D.nw + i;
-            const double M = D.M[t] + X.A_w[e], B = (D.B[t] + X.B_w[e]) + Bd[t];
-            return make_double2(fma(-w2, M, D.C[t]), w * B);
+            const double M = G.M[t] + G.A_w[e], B = (G.B[t] + G.B_w[e]) + Bd[t];
+            return make_double2(fma(-w2, M, G.C[t]), w * B);
         }
     }
-    return make_double2(fma(-w2, D.M[t], D.C[t]), w * (D.B[t] + Bd[t]));
+    return make_double2(fma(-w2, G.M[t], G.C[t]), w * (G.B[t] + Bd[t]));
 }
 
-// k_gen_node_pass: grid (Ns, nC), block 128: RMS of the relative velocity components over w (raft_member.py:2071-2090),
+// k_gen_node_pass: grid (Ns, units), block 128: RMS of the relative velocity components over w (raft_member.py:2071-2090),
 // Bmat (:2092-2116), then the drag node load f6 = [Bmat u ; rr x (Bmat u)] (:2122-2124).
 // TRAIN: secondary trains only, Bmat taken from their primary's last pass (calcDragExcitation(ih), raft_fowt.py:1940-1957).
 template <bool TRAIN>
@@ -202,7 +236,10 @@ __global__ void __launch_bounds__(128) k_gen_node_pass(GenDev D, GenWork W, cons
     __shared__ double red[4][4];
     __shared__ double bm[9];
     const int j = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, nw = D.nw, n = D.n;
-    const double *rr = D.rr + 3 * j;
+    const GenUnit U = gen_unit(D, c);
+    if (j >= U.Ns) return;
+    const int jn = U.j0 + j;
+    const double *rr = D.rr + 3 * jn;
     const double2 *u = W.u + (((size_t)c * D.Ns + j) * 3) * nw;
     if constexpr (TRAIN) {
         const int p = primary[c];
@@ -210,7 +247,7 @@ __global__ void __launch_bounds__(128) k_gen_node_pass(GenDev D, GenWork W, cons
         if (tid < 9) bm[tid] = W.Bmat[((size_t)p * D.Ns + j) * 9 + tid];
     } else {
     if (W.flags[4 * c]) return;
-    const double *q = D.node_frame + 9 * j, *p1 = q + 3, *p2 = q + 6, *T = D.Tn + (size_t)j * 6 * n;
+    const double *q = D.node_frame + 9 * jn, *p1 = q + 3, *p2 = q + 6, *T = D.Tn + (size_t)jn * 6 * n;
     const double2 *X = W.XiLast + (size_t)c * n * nw;
     double sq = 0.0, sp = 0.0, sp1 = 0.0, sp2 = 0.0;
     for (int i = tid; i < nw; i += 128) {
@@ -249,10 +286,10 @@ __global__ void __launch_bounds__(128) k_gen_node_pass(GenDev D, GenWork W, cons
         double s[4];
         for (int t = 0; t < 4; t++) s[t] = ((red[0][t] + red[1][t]) + red[2][t]) + red[3][t];
         const double vq = sqrt(0.5 * s[0]);
-        const double v1 = D.node_circ[j] ? sqrt(0.5 * s[1]) : sqrt(0.5 * s[2]);
-        const double v2 = D.node_circ[j] ? v1 : sqrt(0.5 * s[3]);
+        const double v1 = D.node_circ[jn] ? sqrt(0.5 * s[1]) : sqrt(0.5 * s[2]);
+        const double v2 = D.node_circ[jn] ? v1 : sqrt(0.5 * s[3]);
         const double cc = sqrt(8.0 / CUDART_PI) * 0.5 * D.rho;
-        const double *cd = D.node_cd + 4 * j;
+        const double *cd = D.node_cd + 4 * jn;
         const double Bq = cc * vq * cd[0], Bp1 = cc * v1 * cd[1], Bp2 = cc * v2 * cd[2], Be = cc * vq * cd[3];
         for (int a = 0; a < 3; a++) for (int b = 0; b < 3; b++) {
             const double m = (Bq * (q[a] * q[b]) + Bp1 * (p1[a] * p1[b]) + Bp2 * (p2[a] * p2[b])) + Be * (q[a] * q[b]);
@@ -294,18 +331,19 @@ __host__ __device__ __forceinline__ void gen_B6(const double *Bm, const double *
     }
 }
 
-// k_gen_bdrag: B_drag[c][r][cc] = sum_j sum_{a,l} Tn_j[a][r] B6_j[a][l] Tn_j[l][cc].  grid (n, nC), block 128
+// k_gen_bdrag: B_drag[c][r][cc] = sum_j sum_{a,l} Tn_j[a][r] B6_j[a][l] Tn_j[l][cc].  grid (n, units), block 128
 __global__ void __launch_bounds__(128) k_gen_bdrag(GenDev D, GenWork W)
 {
     __shared__ double tb[6];
     const int r = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, n = D.n;
     if (W.flags[4 * c]) return;
+    const GenUnit U = gen_unit(D, c);
     double acc[2] = { 0.0, 0.0 };                            // columns tid and tid + 128 (n <= 256)
-    for (int j = 0; j < D.Ns; j++) {
-        const double *T = D.Tn + (size_t)j * 6 * n;
+    for (int j = 0; j < U.Ns; j++) {
+        const double *T = D.Tn + (size_t)(U.j0 + j) * 6 * n;
         if (tid < 6) {                                       // tb[l] = sum_a Tn[a][r] B6[a][l]
             double B6[6][6];
-            gen_B6(W.Bmat + ((size_t)c * D.Ns + j) * 9, D.rr + 3 * j, B6);
+            gen_B6(W.Bmat + ((size_t)c * D.Ns + j) * 9, D.rr + 3 * (U.j0 + j), B6);
             double s = 0.0;
             for (int a = 0; a < 6; a++) s += T[(size_t)a * n + r] * B6[a][tid];
             tb[tid] = s;
@@ -320,7 +358,7 @@ __global__ void __launch_bounds__(128) k_gen_bdrag(GenDev D, GenWork W)
     for (int e = 0; e < 2; e++) { const int cc = tid + 128 * e; if (cc < n) W.B_drag[((size_t)c * n + r) * n + cc] = acc[e]; }
 }
 
-// k_gen_solve: grid (nw, nC), block 256.  Augmented system [Z | F] (n x (n+1)) in global memory (L2-resident), right-looking
+// k_gen_solve: grid (nw, units), block 256.  Augmented system [Z | F] (n x (n+1)) in global memory (L2-resident), right-looking
 // LU with partial pivoting on |re| + |im| (LAPACK izamax), back substitution; writes Xi and the convergence verdict.
 template <bool FD>
 __global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 *Xi, double tol, GenFdDev X)
@@ -332,13 +370,15 @@ __global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 
     __shared__ int fdpos[FD ? 256 : 1];
     const int i = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, n = D.n, nw = D.nw, nc = n + 1;
     if (W.flags[4 * c]) return;
+    const int d = gen_unit(D, c).d;
+    const GenMats G = gen_mats(D, X, d);
     double2 *A = W.Z + ((size_t)c * nw + i) * (size_t)n * nc;
     const double w = D.w[i], w2 = w * w;
     const double *Bd = W.B_drag + (size_t)c * n * n;
-    if constexpr (FD) gen_fd_map(D, X, fdpos, tid, 256);
+    if constexpr (FD) gen_fd_map(D, X, d, fdpos, tid, 256);
     for (int t = tid; t < n * n; t += 256) {
         const int a = t / n, b = t % n;
-        A[(size_t)a * nc + b] = gen_impedance<FD>(D, X, fdpos, Bd, t, i, w, w2);
+        A[(size_t)a * nc + b] = gen_impedance<FD>(D, X, G, fdpos, Bd, t, i, w, w2);
     }
     for (int a = tid; a < n; a += 256) {
         const double2 f1 = W.F_iner[((size_t)c * n + a) * nw + i], f2 = W.F_drag[((size_t)c * n + a) * nw + i];
@@ -413,7 +453,7 @@ __global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 
     if (nan || bad) atomicOr(&W.flags[4 * c + 3], 1);
 }
 
-// k_gen_solve_blocked: grid (nw, nC), block 256.  Same system, same pivot rule and the same elimination order as
+// k_gen_solve_blocked: grid (nw, units), block 256.  Same system, same pivot rule and the same elimination order as
 // k_gen_solve, organised as a blocked right-looking LU (LAPACK zgetrf's structure) so that the work is done on chip:
 //   per block of GB columns:  panel (rows kb.., GB columns) factored in SHARED memory with partial pivoting; its row swaps
 //   applied to the rest of the rows; the GB x (rest) row block solved against the unit-lower panel head in shared memory;
@@ -434,15 +474,17 @@ __global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W
     __shared__ int fdpos[FD ? 256 : 1];
     const int i = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, n = D.n, nw = D.nw, nc = n + 1;
     if (W.flags[4 * c]) return;
+    const int d = gen_unit(D, c).d;
+    const GenMats G = gen_mats(D, X, d);
     double2 *P = reinterpret_cast<double2 *>(smem_raw);          // panel  [n][GB]   (rows kb.. stored from 0)
     double2 *U = P + (size_t)n * GB;                             // row block [GB][nc]
     double2 *A = W.Z + ((size_t)c * nw + i) * (size_t)n * nc;
     const double w = D.w[i], w2 = w * w;
     const double *Bd = W.B_drag + (size_t)c * n * n;
-    if constexpr (FD) gen_fd_map(D, X, fdpos, tid, GT);
+    if constexpr (FD) gen_fd_map(D, X, d, fdpos, tid, GT);
     for (int t = tid; t < n * n; t += GT) {
         const int a = t / n, b = t % n;
-        A[(size_t)a * nc + b] = gen_impedance<FD>(D, X, fdpos, Bd, t, i, w, w2);
+        A[(size_t)a * nc + b] = gen_impedance<FD>(D, X, G, fdpos, Bd, t, i, w, w2);
     }
     for (int a = tid; a < n; a += GT) {
         const double2 f1 = W.F_iner[((size_t)c * n + a) * nw + i], f2 = W.F_drag[((size_t)c * n + a) * nw + i];
@@ -666,20 +708,23 @@ __global__ void __launch_bounds__(256) k_gen_relax(GenDev D, GenWork W, const do
     }
 }
 
-// Streamed tables (raftk_general_solve_dynamics_stream_*): every chunk holds whole train groups and runs the sequence above
-// on views advanced to its first case c0.  Around it:
-//   k_gen_chunk_primary (case)   cases.primary of the chunk, rebased to c0, into the workspace
-//   k_gen_status_rebase (case)   status word 3 of the chunk's secondaries back to the table's primary + 1
-__global__ void __launch_bounds__(128) k_gen_chunk_primary(int nC, int c0, const int *primary, int *local)
+// Streamed tables and design batches (raftk_general_solve_dynamics_stream_*, raftk_general_batch_solve_dynamics_*): the
+// units (design, case), design-major, run in chunks of whole train groups, each chunk the sequence above on units u0 .. u0+m-1
+// (GenDev.u0; outputs advanced to unit u0).  Around it:
+//   k_gen_chunk_primary (unit)   cases.primary of the chunk as chunk-local units (a primary lies in its train's design)
+//   k_gen_status_rebase (unit)   status word 3 of the chunk's secondaries back to the primary's case index + 1
+__global__ void __launch_bounds__(128) k_gen_chunk_primary(int m, int u0, int nCt, const int *primary, int *local)
 {
-    const int c = blockIdx.x * 128 + threadIdx.x;
-    if (c < nC) local[c] = primary[c0 + c] - c0;
+    const int t = blockIdx.x * 128 + threadIdx.x;
+    if (t >= m) return;
+    const int c = (u0 + t) % nCt;
+    local[t] = t - c + primary[c];
 }
 
-__global__ void __launch_bounds__(128) k_gen_status_rebase(int nC, int c0, int *status)
+__global__ void __launch_bounds__(128) k_gen_status_rebase(int m, int u0, int nCt, int *status)
 {
-    const int c = blockIdx.x * 128 + threadIdx.x;
-    if (c < nC && status[4 * c + 3] != 0) status[4 * c + 3] += c0;
+    const int t = blockIdx.x * 128 + threadIdx.x;
+    if (t < m && status[4 * t + 3] != 0) status[4 * t + 3] += (u0 + t) % nCt - t;
 }
 
 // raftk_general_publish_dev: rank p's gathered rows for this call, X[p] complex [rows][n][nw] and S[p] int [rows][4] (NULL: no

@@ -15,7 +15,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (RaftkCases, RaftkDesigns, RaftkFarm, RaftkGeneral, RaftkGeneralFd, RaftkGeneralQtf, RaftkOutputs, RaftkSlender, RaftkSlenderBatch,
+from ._lib import (RaftkCases, RaftkDesigns, RaftkFarm, RaftkGeneral, RaftkGeneralBatch, RaftkGeneralFd, RaftkGeneralQtf, RaftkOutputs, RaftkSlender, RaftkSlenderBatch,
                    RaftkSlenderOutputs, RaftkSolveOpts, check, lib)
 
 _F8 = np.float64
@@ -989,21 +989,329 @@ def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01
     table, owner, first = pack_case_trains(cases)
     q = bool(qtf)
     res = general_solve_dynamics(P, M, B, Cm, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start, fd=fd, qtf=qtf, F_2nd=q)
-    Xi, st = res[0], res[1]
+    return _general_case_results(P, res[0], res[1], owner, first, len(cases), channels, res[2:4] if q else None)
+
+
+def _general_case_results(P, Xi, st, owner, first, n_cases, channels, F2nd):
+    """general_analyze_cases' result for one design from its train table's Xi [nT,nDOF,nw], status [nT,4] and, with a QTF
+    table, (F_2nd [nT,6,nw], F_2nd_mean [nT,6])."""
     raise_on_flags(st[first])                                           # raft_model.py:1089, :1098-1099
     metrics = {}
     if channels is not None:
         sd, ps, amp = general_channel_stats(channels["R"], channels["wpow"], P["w"], Xi, float(P["dw"]), psd=True, amp=True)
-        for ic in range(len(cases)):
+        for ic in range(n_cases):
             metrics[ic] = general_case_metrics(channels, sd, ps, amp, np.nonzero(owner == ic)[0])
-    out = dict(Xi_trains=[Xi[owner == ic] for ic in range(len(cases))], status=st[first], case_metrics=metrics)
-    if q:
+    out = dict(Xi_trains=[Xi[owner == ic] for ic in range(n_cases)], status=st[first], case_metrics=metrics)
+    if F2nd is not None:
         n, nw = Xi.shape[1], Xi.shape[2]
         F2, F2m = np.zeros([len(Xi), n, nw], dtype=np.complex128), np.zeros([len(Xi), n])
-        F2[:, :6], F2m[:, :6] = res[2], res[3]
-        out["Fhydro_2nd"] = [F2[owner == ic] for ic in range(len(cases))]
-        out["Fhydro_2nd_mean"] = [F2m[owner == ic] for ic in range(len(cases))]
+        F2[:, :6], F2m[:, :6] = F2nd[0], F2nd[1]
+        out["Fhydro_2nd"] = [F2[owner == ic] for ic in range(n_cases)]
+        out["Fhydro_2nd_mean"] = [F2m[owner == ic] for ic in range(n_cases)]
     return out
+
+
+# ---- design batches of flexible FOWTs (raftk_general_batch_*) ------------------------------------------------------------
+def _capture():
+    got = {}
+
+    def ptr(name, a):
+        got[name] = a
+    return got, ptr
+
+
+class GeneralBatch:
+    """The tables of a design batch of FOWTs with generalised DOFs (include/raftk.h raftk_general_batch): ``designs`` a list of
+    per-design inputs, each a dict with keys P, M, B, Cm and optional fd, qtf, or a tuple (P, M, B, Cm[, fd[, qtf]]) in the
+    layouts of ``general_solve_dynamics`` (``packer.pack_general_dofs`` / ``pack_general_matrices`` / ``pack_general_qtf``).
+    The node tables are concatenated (CSR ``node_offset``), the matrices and frequency-dependent tables stacked on a leading
+    design axis.  ``qtf``: one second-order table shared by every design (then no design may carry its own).  The designs must
+    share n_dof, the frequency grid, depth and rho, the count of fd DOFs and BEM headings, and the QTF grid: a ValueError names
+    the first design that differs from design 0."""
+
+    def __init__(self, designs, qtf=None):
+        designs = [self._entry(e) for e in designs]
+        if not designs:
+            raise ValueError("a design batch needs at least one design")
+        if qtf and any(e.get("qtf") for e in designs):
+            raise ValueError("qtf=: a shared QTF table, but design %d carries its own" % next(d for d, e in enumerate(designs) if e.get("qtf")))
+        per = []
+        for e in designs:
+            ga, gp = _capture()
+            g = _general_struct(e["P"], e["M"], e["B"], e["Cm"], gp)
+            fa, fp = _capture()
+            f = _general_fd_struct(e.get("fd"), g.n_dof, g.nw, fp)
+            qa, qp = _capture()
+            q = _general_qtf_struct(qtf if qtf else e.get("qtf"), qp)
+            per.append((g, ga, f, fa, q, qa))
+        g0, ga0, f0, _, q0, qa0 = per[0]
+        for d, (g, ga, f, _, q, qa) in enumerate(per[1:], 1):
+            why = None
+            if g.n_dof != g0.n_dof:
+                why = "n_dof (%d against %d)" % (g.n_dof, g0.n_dof)
+            elif g.nw != g0.nw or g.dw != g0.dw or not (np.array_equal(ga["w"], ga0["w"]) and np.array_equal(ga["k"], ga0["k"])):
+                why = "the frequency grid"
+            elif g.depth != g0.depth:
+                why = "depth"
+            elif g.rho != g0.rho:
+                why = "rho"
+            elif (f is None) != (f0 is None):
+                why = "fd (frequency-dependent tables given for one design and not the other)"
+            elif f is not None and f.n_fd != f0.n_fd:
+                why = "n_fd (%d against %d)" % (f.n_fd, f0.n_fd)
+            elif f is not None and f.n_bem_head != f0.n_bem_head:
+                why = "n_bem_head (%d against %d)" % (f.n_bem_head, f0.n_bem_head)
+            elif (q is None) != (q0 is None):
+                why = "qtf (a QTF table given for one design and not the other)"
+            elif q is not None and not (np.array_equal(qa["qtf_w"], qa0["qtf_w"]) and np.array_equal(qa["qtf_heads"], qa0["qtf_heads"])):
+                why = "the QTF grid"
+            elif ("node_Imat_w" in ga) != ("node_Imat_w" in ga0):
+                why = "node_Imat_w (MacCamy-Fuchs tables given for one design and not the other)"
+            if why:
+                raise ValueError("design %d: %s differs from design 0" % (d, why))
+        self.n_designs, self.n, self.nw = len(per), int(g0.n_dof), int(g0.nw)
+        self.depth, self.rho, self.dw = g0.depth, g0.rho, g0.dw
+        self.node_counts = np.array([g.n_nodes for g, *_ in per], dtype=_I4)
+        self.node_offset = np.concatenate([[0], np.cumsum(self.node_counts)]).astype(_I4)
+        self.max_nodes = int(self.node_counts.max())
+        A = {}
+        for name in _lib.GENERAL_ARRAYS:
+            if name in ("w", "k"):
+                A[name] = ga0[name]
+            elif name in ("M", "B", "C"):
+                A[name] = np.ascontiguousarray(np.stack([p[1][name] for p in per]))
+            elif name in ga0:                          # node tables, flattened and concatenated in design order
+                A[name] = np.ascontiguousarray(np.concatenate([p[1][name].ravel() for p in per]))
+        self.arrays = A
+        self.fd = None
+        if f0 is not None:
+            F = dict(fd_idx=np.ascontiguousarray(np.stack([p[3].get("fd_idx", np.zeros(0, dtype=_I4)) for p in per]), dtype=_I4))
+            for name in ("fd_A_w", "fd_B_w", "fd_bem_headings", "fd_X_BEM", "fd_T0"):
+                if name in per[0][3]:
+                    F[name] = np.ascontiguousarray(np.stack([p[3][name] for p in per]))
+            F["x_ref"] = np.array([p[2].x_ref for p in per])
+            F["y_ref"] = np.array([p[2].y_ref for p in per])
+            F["heading_adjust"] = np.array([p[2].heading_adjust for p in per])
+            self.fd = F
+            self.n_fd, self.n_bem_head = int(f0.n_fd), int(f0.n_bem_head)
+        self.qtf, self.qtf_shared = None, 1 if qtf else 0
+        if q0 is not None:
+            self.qtf = dict(qtf_w=qa0["qtf_w"], qtf_heads=qa0["qtf_heads"],
+                            qtf=qa0["qtf"] if qtf else np.ascontiguousarray(np.stack([p[5]["qtf"] for p in per])))
+            self.n_qtf_w, self.n_qtf_head = int(q0.n_qtf_w), int(q0.n_qtf_head)
+
+    @staticmethod
+    def _entry(e):
+        if isinstance(e, dict):
+            return e
+        return dict(zip(("P", "M", "B", "Cm", "fd", "qtf"), e))
+
+    def structs(self, ptr_of):
+        """(raftk_general, raftk_general_batch, raftk_general_fd or None, raftk_general_qtf or None); ``ptr_of(name, array)``
+        returns the address to store (host or device, None for the size queries)."""
+        g = RaftkGeneral()
+        g.n_dof, g.nw, g.n_nodes = self.n, self.nw, int(self.node_offset[-1])
+        g.depth, g.rho, g.dw = self.depth, self.rho, self.dw
+        for name in _lib.GENERAL_ARRAYS:
+            setattr(g, name, ptr_of(name, self.arrays[name]) if name in self.arrays else None)
+        b = RaftkGeneralBatch()
+        b.n_designs, b.max_nodes, b.qtf_shared = self.n_designs, self.max_nodes, self.qtf_shared
+        b.node_offset = ptr_of("node_offset", self.node_offset)
+        f = None
+        if self.fd is not None:
+            F = self.fd
+            f = RaftkGeneralFd()
+            f.n_fd, f.n_bem_head = self.n_fd, self.n_bem_head
+            if self.n_fd:
+                f.fd_idx, f.A_w, f.B_w = ptr_of("fd_idx", F["fd_idx"]), ptr_of("fd_A_w", F["fd_A_w"]), ptr_of("fd_B_w", F["fd_B_w"])
+            if self.n_bem_head:
+                f.bem_headings, f.X_BEM, f.T0 = (ptr_of(k, F[k]) for k in ("fd_bem_headings", "fd_X_BEM", "fd_T0"))
+            b.x_ref, b.y_ref, b.heading_adjust = (ptr_of(k, F[k]) for k in ("x_ref", "y_ref", "heading_adjust"))
+        q = None
+        if self.qtf is not None:
+            q = RaftkGeneralQtf()
+            q.n_qtf_w, q.n_qtf_head = self.n_qtf_w, self.n_qtf_head
+            q.qtf_w, q.qtf_heads, q.qtf = (ptr_of(k, self.qtf[k]) for k in ("qtf_w", "qtf_heads", "qtf"))
+        return g, b, f, q
+
+
+def _as_batch(designs, qtf=None):
+    if isinstance(designs, GeneralBatch):
+        if qtf:
+            raise ValueError("qtf= applies when the batch is built here; give it to GeneralBatch")
+        return designs
+    return GeneralBatch(designs, qtf=qtf)
+
+
+def _refs(*structs):
+    return [C.byref(s) if s is not None else None for s in structs]
+
+
+def general_batch_workspace_bytes(batch, n_cases, max_chunk_units=0):
+    """raftk_general_batch_workspace_bytes: device workspace of a design batch (``GeneralBatch``) over ``n_cases`` cases in
+    chunks of at most ``max_chunk_units`` (design, case) units (0: all).  Depends on the counts only."""
+    g, b, f, q = batch.structs(lambda name, a: None)
+    return int(lib.raftk_general_batch_workspace_bytes(*_refs(g, b, f, q), int(n_cases), int(max_chunk_units)))
+
+
+def general_batch_chunk_plan(primary, n_cases, n_designs, max_chunk_units):
+    """The chunks raftk_general_batch_solve_dynamics_* cut the units (design, case), design-major, into -> [u_0 = 0, ...,
+    n_designs * n_cases]: every design's train groups in table order, packed greedily into chunks of at most
+    ``max_chunk_units`` (0: all); a chunk may cross design boundaries.  ValueError where the library refuses the plan."""
+    from .sweep import general_groups
+    n, nD = int(n_cases), int(n_designs)
+    nU = n * nD
+    K = nU if (max_chunk_units <= 0 or max_chunk_units >= nU) else int(max_chunk_units)
+    g = general_groups(primary, n)
+    for a, b in zip(g[:-1], g[1:]):
+        if b - a > K:
+            raise ValueError("a train group has %d cases, more than max_chunk_units = %d" % (b - a, K))
+    cuts = [0]
+    for d in range(nD):
+        for a, b in zip(g[:-1], g[1:]):
+            if d * n + b - cuts[-1] > K:
+                cuts.append(int(d * n + a))
+    return cuts + [nU]
+
+
+def general_batch_chunk_for_budget(batch, n_cases, budget_bytes, primary=None):
+    """The largest ``max_chunk_units`` whose workspace fits ``budget_bytes`` (all units when everything fits).  With the
+    table's ``primary`` map the chunk must also hold its largest train group; ValueError when it cannot."""
+    nU, budget = int(n_cases) * batch.n_designs, int(budget_bytes)
+    ws = lambda k: general_batch_workspace_bytes(batch, n_cases, k)       # noqa: E731
+    big = 1
+    if primary is not None:
+        from .sweep import general_groups
+        big = int(np.diff(general_groups(primary, int(n_cases))).max())
+    if ws(nU) <= budget:
+        return nU
+    if ws(big) > budget:
+        raise ValueError("a workspace of %d bytes does not hold %d units (%d bytes)" % (budget, big, ws(big)))
+    lo, hi = big, nU - 1
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        if ws(mid) <= budget:
+            lo = mid
+        else:
+            hi = mid - 1
+    return lo
+
+
+def general_solve_dynamics_batch(designs, cases, n_iter=10, tol=0.01, xi_start=0.0, F_BEM=False, F_2nd=False, max_chunk_units=0, qtf=None):
+    """``general_solve_dynamics`` for a design batch in one call, host buffers: ``designs`` a ``GeneralBatch`` or its list of
+    per-design inputs (``qtf``: a table shared by all), ``cases`` a CaseTable run by every design -> (Xi complex
+    [nD,nT,nDOF,nw], status [nD,nT,4]) + (F_BEM [nD,nT,nDOF,nw],) with ``F_BEM`` + (F_2nd [nD,nT,6,nw], F_2nd_mean [nD,nT,6])
+    with ``F_2nd``.  ``Xi[d]`` is what ``general_solve_dynamics`` returns for design d alone.  ``max_chunk_units``: the most
+    (design, case) units per chunk of the device workspace (0: all)."""
+    bt = _as_batch(designs, qtf)
+    keep = {}
+
+    def ptr(name, a):
+        keep[name] = a
+        return a.ctypes.data
+    g, b, f, q = bt.structs(ptr)
+    if F_2nd and q is None:
+        raise ValueError("F_2nd=True needs a QTF table")
+    nD, nC, n, nw = bt.n_designs, cases.n_cases, bt.n, bt.nw
+    Xi = np.zeros([nD, nC, n, nw], dtype=np.complex128)
+    st = np.zeros([nD, nC, 4], dtype=_I4)
+    Fb = np.zeros([nD, nC, n, nw], dtype=np.complex128) if F_BEM else None
+    F2, F2m = (np.zeros([nD, nC, 6, nw]), np.zeros([nD, nC, 6])) if F_2nd else (None, None)
+    c = cases.struct(_host_ptr(cases.arrays))
+    o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
+    hp = lambda a: a.ctypes.data if a is not None else None   # noqa: E731
+    check(lib.raftk_general_batch_solve_dynamics_host(*_refs(g, b, f, q), C.byref(c), C.byref(o), Xi.ctypes.data, st.ctypes.data, hp(Fb),
+                                                      hp(F2), hp(F2m), int(max_chunk_units)))
+    return (Xi, st) + ((Fb,) if F_BEM else ()) + ((F2, F2m) if F_2nd else ())
+
+
+class GeneralBatchSession:
+    """A design batch (``GeneralBatch`` or its list of per-design inputs) with tables, workspace and outputs resident in HBM,
+    kernels on torch's current stream, the contract of ``GeneralSession``: ``solve()`` enqueues
+    raftk_general_batch_solve_dynamics_dev -> (Xi [nD,nT,nDOF,nw] complex, status [nD,nT,4]) (+ F_BEM [nD,nT,nDOF,nw] with
+    ``F_BEM=True``); with a QTF table every ``solve()`` leaves ``F_2nd`` [nD,nT,6,nw] and ``F_2nd_mean`` [nD,nT,6] on the
+    device.  ``max_chunk_units``: the most (design, case) units per chunk of the workspace (0: all; ``general_batch_chunk_for_budget``).
+    ``stats(R, wpow)`` takes channel rows per design, R [nD,nch,nDOF] (``packer.pack_general_channels`` of each design)."""
+
+    def __init__(self, designs, cases, device=None, F_BEM=False, qtf=None, max_chunk_units=0):
+        import torch
+        self.torch = torch
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.batch = bt = _as_batch(designs, qtf)
+        if int(max_chunk_units) < 0:
+            raise ValueError("max_chunk_units must be >= 0 (0: all units in one chunk)")
+        self.max_chunk_units = int(max_chunk_units)
+        self.keep = {}
+
+        def to_dev(name, a):
+            t = torch.from_numpy(a.view(np.float64) if a.dtype == np.complex128 else a).to(self.device)
+            self.keep[name] = t
+            return t.data_ptr()
+        nD, nC, n, nw = bt.n_designs, cases.n_cases, bt.n, bt.nw
+        with torch.cuda.device(self.device):
+            self.g, self.b, self.fd, self.qtf = bt.structs(to_dev)
+            self.ct = {k: torch.from_numpy(v).to(self.device) for k, v in cases.arrays.items()}
+            self.c_struct = cases.struct(lambda name: self.ct[name].data_ptr())
+            self.workspace_bytes = general_batch_workspace_bytes(bt, nC, self.max_chunk_units)
+            self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=self.device)
+            self.Xi = torch.zeros([nD, nC, n, nw], dtype=torch.complex128, device=self.device)
+            self.status = torch.zeros([nD, nC, 4], dtype=torch.int32, device=self.device)
+            self.F_BEM = torch.zeros([nD, nC, n, nw], dtype=torch.complex128, device=self.device) if F_BEM else None
+            self.F_2nd = torch.zeros([nD, nC, 6, nw], dtype=torch.float64, device=self.device) if self.qtf is not None else None
+            self.F_2nd_mean = torch.zeros([nD, nC, 6], dtype=torch.float64, device=self.device) if self.qtf is not None else None
+        self.n_designs, self.n, self.nw, self.n_cases, self.dw = nD, n, nw, nC, bt.dw
+
+    def solve(self, n_iter=10, tol=0.01, xi_start=0.0):
+        o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
+        ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
+        with self.torch.cuda.device(self.device):
+            stream = self.torch.cuda.current_stream(self.device).cuda_stream
+            check(lib.raftk_general_batch_solve_dynamics_dev(*_refs(self.g, self.b, self.fd, self.qtf), C.byref(self.c_struct), C.byref(o),
+                                                             self.Xi.data_ptr(), self.status.data_ptr(), ptr(self.F_BEM), ptr(self.F_2nd),
+                                                             ptr(self.F_2nd_mean), self.workspace.data_ptr(), self.workspace_bytes,
+                                                             self.max_chunk_units, stream))
+        return (self.Xi, self.status) if self.F_BEM is None else (self.Xi, self.status, self.F_BEM)
+
+    def stats(self, R, wpow, psd=True, amp=False):
+        """Output-channel statistics of the last ``solve()`` on the device, design by design (raftk_general_channel_stats_dev
+        on each design's slice of Xi): R [nD,nch,nDOF], wpow [nch] -> (std [nD,nT,nch], PSD [nD,nT,nch,nw] or None, amplitudes
+        complex [nD,nT,nch,nw] or None), torch tensors."""
+        torch = self.torch
+        R = np.ascontiguousarray(R, dtype=_F8)
+        wpow = np.ascontiguousarray(wpow, dtype=_I4)
+        nD, nC, n, nw = self.n_designs, self.n_cases, self.n, self.nw
+        if R.ndim != 3 or R.shape[0] != nD or R.shape[2] != n or wpow.shape != (R.shape[1],):
+            raise ValueError("R must be [%d, nch, %d] and wpow [nch]" % (nD, n))
+        _check_wpow(wpow)
+        nch = R.shape[1]
+        with torch.cuda.device(self.device):
+            dR, dp = torch.from_numpy(R).to(self.device), torch.from_numpy(wpow).to(self.device)
+            sd = torch.empty([nD, nC, nch], dtype=torch.float64, device=self.device)
+            P = torch.empty([nD, nC, nch, nw], dtype=torch.float64, device=self.device) if psd else None
+            A = torch.empty([nD, nC, nch, nw], dtype=torch.complex128, device=self.device) if amp else None
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            for d in range(nD):
+                check(lib.raftk_general_channel_stats_dev(nC, n, nch, nw, self.dw, self.keep["w"].data_ptr(), dR[d].data_ptr(), dp.data_ptr(),
+                                                          self.Xi[d].data_ptr(), sd[d].data_ptr(), P[d].data_ptr() if psd else None,
+                                                          A[d].data_ptr() if amp else None, stream))
+        return sd, P, A
+
+
+def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, qtf=None):
+    """``general_analyze_cases`` for every design of a batch in one solve: ``designs`` a list of per-design inputs (or a
+    ``GeneralBatch`` built from them), ``cases`` a list of case dicts run by every design, ``channels`` None or one
+    ``packer.pack_general_channels`` dict per design -> a list with, for each design, what ``general_analyze_cases`` returns
+    for that design alone."""
+    from .packer import pack_case_trains
+    bt = _as_batch(designs, qtf)
+    if channels is not None and len(channels) != bt.n_designs:
+        raise ValueError("channels: one entry per design (%d), got %d" % (bt.n_designs, len(channels)))
+    table, owner, first = pack_case_trains(cases)
+    q = bt.qtf is not None
+    res = general_solve_dynamics_batch(bt, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start, F_2nd=q)
+    P = dict(w=bt.arrays["w"], dw=bt.dw)
+    return [_general_case_results(P, res[0][d], res[1][d], owner, first, len(cases), None if channels is None else channels[d],
+                                  (res[2][d], res[3][d]) if q else None) for d in range(bt.n_designs)]
 
 
 def second_order_force(batch, cases):
