@@ -660,6 +660,36 @@ int raftk_solve_dynamics_farm_host(const raftk_designs *d, const raftk_cases *c,
                                    const raftk_outputs *out, const raftk_farm *f);
 
 /*
+ * Batches of farms (array layout and shared-mooring studies): n_farms arrays of n_fowt FOWTs each over one case table in
+ * one call.  Design f * n_fowt + i of the batch is FOWT i of farm f; the farms share the turbine count, frequency grid,
+ * depth and rho, and differ in positions (hence wave phasing), platforms and array matrices.  Every system is assembled and
+ * solved exactly as raftk_farm's: a farm's Xi_sys and info do not depend on the batch it is in, and the raftk_farm entries
+ * are n_farms = 1 launches of the same kernels.
+ * M_arr / B_arr / C_arr: [6N,6N] used by every farm when arr_shared = 1, [n_farms,6N,6N] when 0; any may be NULL.
+ * Xi_sys complex [n_farms, nC, 6N, nw]; info [n_farms, nC, nw] or NULL: a zero pivot is flagged in its own farm's rows only.
+ * Limits: with the system in shared memory or registers (N <= 20 on an H100) the grid is (frequency groups, case, farm), so
+ * at most 65535 cases and 65535 farms per call; larger farms walk a list of n_farms * nC * nw systems and have no such limit.
+ * raftk_farm_batch_workspace_bytes: as raftk_farm_workspace_bytes with n_farms * nC * nw systems (0 for N <= 20).
+ * raftk_farm_batch_response_ws_dev: `solved` holds the device outputs of raftk_solve_dynamics_dev on the same (d, c).
+ * RAFTK_EINVAL before any launch: n_farms or n_fowt < 1, n_farms * n_fowt != designs.n_designs, arr_shared not 0 or 1, no
+ * Xi_sys, a missing per-FOWT output (B_drag, F_drag, F_iner; F_BEM with BEM excitation), a grid limit above, or less than
+ * one slab of workspace when the shape needs one.
+ */
+typedef struct raftk_farm_batch {
+    int32_t n_farms, n_fowt;        /* n_farms * n_fowt must equal designs.n_designs */
+    int32_t arr_shared, _pad0;      /* 1: one M_arr/B_arr/C_arr for every farm; 0: [n_farms,6N,6N] */
+    const double *M_arr, *B_arr, *C_arr;
+    double *Xi_sys;
+    int32_t *info;
+} raftk_farm_batch;
+
+size_t raftk_farm_batch_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm_batch *f);
+int raftk_farm_batch_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
+                                     const raftk_farm_batch *f, void *workspace, size_t workspace_bytes, void *stream);
+int raftk_solve_dynamics_farm_batch_host(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o,
+                                         const raftk_outputs *out, const raftk_farm_batch *f);
+
+/*
  * Response statistics of FOWT.saveTurbineOutputs (raft_fowt.py:2299-2353) as reductions over Xi:
  * for every unit (design, case) and DOF   std = sqrt(1/2 sum_w |Xi|^2)   (helpers.getRMS, helpers.py:678-684)
  * and, if psd != NULL,                    PSD(w) = 1/2 |Xi(w)|^2 / dw    (helpers.getPSD, helpers.py:687-700).

@@ -69,6 +69,12 @@ class RaftkFarm(C.Structure):
                 ("Xi_sys", C.c_void_p), ("info", C.c_void_p)]
 
 
+class RaftkFarmBatch(C.Structure):
+    """include/raftk.h raftk_farm_batch: n_farms arrays of n_fowt FOWTs each, solved over one case table in one call."""
+    _fields_ = [("n_farms", C.c_int32), ("n_fowt", C.c_int32), ("arr_shared", C.c_int32), ("_pad0", C.c_int32),
+                ("M_arr", C.c_void_p), ("B_arr", C.c_void_p), ("C_arr", C.c_void_p), ("Xi_sys", C.c_void_p), ("info", C.c_void_p)]
+
+
 SLENDER_ARRAYS = ("w", "k", "mem_q", "mem_p1", "mem_p2", "mem_mcf", "mem_wl", "mem_r_int", "mem_a_wl", "mem_rwl", "mem_R_wl", "mem_node_start",
                   "node_r", "node_v_side", "node_Ca_p1", "node_Ca_p2", "node_Ca_End", "node_v_end", "node_a_i",
                   "seg_mem", "seg_z1", "seg_z2", "seg_R", "seg_rmid", "M_struc")
@@ -168,6 +174,7 @@ SYMBOLS = [
     "raftk_peer_alloc", "raftk_peer_free", "raftk_peer_open", "raftk_peer_close",
     "raftk_solve_dynamics_gather_dev", "raftk_peer_barrier_dev", "raftk_general_publish_dev",
     "raftk_farm_response_dev", "raftk_solve_dynamics_farm_host", "raftk_farm_workspace_bytes", "raftk_farm_response_ws_dev",
+    "raftk_farm_batch_workspace_bytes", "raftk_farm_batch_response_ws_dev", "raftk_solve_dynamics_farm_batch_host",
     "raftk_family_sizes", "raftk_build_family_host",
 ]
 
@@ -301,6 +308,13 @@ def _load():
     lib.raftk_farm_workspace_bytes.restype = C.c_size_t
     lib.raftk_farm_response_ws_dev.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkOutputs), P(RaftkFarm), C.c_void_p, C.c_size_t, C.c_void_p]
     lib.raftk_farm_response_ws_dev.restype = C.c_int
+    lib.raftk_farm_batch_workspace_bytes.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkFarmBatch)]
+    lib.raftk_farm_batch_workspace_bytes.restype = C.c_size_t
+    lib.raftk_farm_batch_response_ws_dev.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkOutputs), P(RaftkFarmBatch), C.c_void_p, C.c_size_t,
+                                                     C.c_void_p]
+    lib.raftk_farm_batch_response_ws_dev.restype = C.c_int
+    lib.raftk_solve_dynamics_farm_batch_host.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkSolveOpts), P(RaftkOutputs), P(RaftkFarmBatch)]
+    lib.raftk_solve_dynamics_farm_batch_host.restype = C.c_int
     lib.raftk_family_sizes.argtypes = [P(RaftkFamily), P(C.c_int32), P(C.c_int32)]
     lib.raftk_build_family_host.argtypes = [P(RaftkFamily), P(RaftkFamilyTables)]
     lib.raftk_family_sizes.restype = C.c_int

@@ -919,52 +919,82 @@ static bool farm_on_chip(int N)
     return n <= 24 || smem_fits((size_t)n * (n + 1) * sizeof(double2), static_smem(k_farm_response<false>, SMEM_STATIC_FARM_BLOCK));
 }
 
-// workspace of k_farm_response_global: one [6N][6N+1] slab per resident CTA, no more slabs than (case, frequency) systems
+// workspace of k_farm_response_global: one [6N][6N+1] slab per resident CTA, no more slabs than (farm, case, frequency) systems
 static size_t farm_slab_bytes(int N) { return (size_t)6 * N * (6 * N + 1) * sizeof(double2); }
-static size_t farm_ws_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm *f)
+static size_t farm_ws_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm_batch *f)
 {
-    if (!d || !c || !f || f->n_fowt < 1 || d->nw < 1 || c->n_cases < 1 || farm_on_chip(f->n_fowt)) return 0;
+    if (!d || !c || !f || f->n_farms < 1 || f->n_fowt < 1 || d->nw < 1 || c->n_cases < 1 || farm_on_chip(f->n_fowt)) return 0;
     const GluPlan g = glu_plan(6 * f->n_fowt);
-    const long long slabs = std::min<long long>((long long)c->n_cases * d->nw, (long long)std::max(g.per_sm, 1) * sm_count());
+    const long long slabs = std::min<long long>((long long)f->n_farms * c->n_cases * d->nw, (long long)std::max(g.per_sm, 1) * sm_count());
     return (size_t)slabs * farm_slab_bytes(f->n_fowt);
+}
+
+// one farm is a batch of one: its matrices are the shared set
+static raftk_farm_batch farm_as_batch(const raftk_farm *f)
+{
+    raftk_farm_batch b;
+    memset(&b, 0, sizeof(b));
+    b.n_farms = 1; b.n_fowt = f->n_fowt; b.arr_shared = 1;
+    b.M_arr = f->M_arr; b.B_arr = f->B_arr; b.C_arr = f->C_arr;
+    b.Xi_sys = f->Xi_sys; b.info = f->info;
+    return b;
 }
 
 extern "C" size_t raftk_farm_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm *f)
 {
+    if (!f) return 0;
+    const raftk_farm_batch b = farm_as_batch(f);
+    return farm_ws_bytes(d, c, &b);
+}
+
+extern "C" size_t raftk_farm_batch_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm_batch *f)
+{
     return farm_ws_bytes(d, c, f);
 }
 
-static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f, void *ws,
+// the shape of a farm batch against its designs (everything the host entry can refuse before it stages anything)
+static int farm_batch_shape(const raftk_designs *d, const raftk_farm_batch *f)
+{
+    if (f->n_farms < 1 || f->n_fowt < 1) return set_err(RAFTK_EINVAL, "farm batch: n_farms and n_fowt must be >= 1");
+    if ((long long)f->n_farms * f->n_fowt != d->n_designs)
+        return set_err(RAFTK_EINVAL, "farm batch: n_farms * n_fowt must equal designs.n_designs");
+    if (f->arr_shared != 0 && f->arr_shared != 1) return set_err(RAFTK_EINVAL, "farm batch: arr_shared must be 0 or 1");
+    if (!f->Xi_sys) return set_err(RAFTK_EINVAL, "farm batch: Xi_sys is required");
+    return RAFTK_OK;
+}
+
+static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm_batch *f, void *ws,
                        size_t ws_bytes, cudaStream_t st)
 {
     if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "farm response: null argument");
-    if (f->n_fowt != d->n_designs || f->n_fowt < 1) return set_err(RAFTK_EINVAL, "farm response: farm.n_fowt must equal designs.n_designs");
-    if (!solved->B_drag || !solved->F_drag || !solved->F_iner || !f->Xi_sys)
-        return set_err(RAFTK_EINVAL, "farm response needs B_drag, F_drag, F_iner of the per-FOWT solve and farm.Xi_sys");
+    if (int rc = farm_batch_shape(d, f)) return rc;
+    if (!solved->B_drag || !solved->F_drag || !solved->F_iner)
+        return set_err(RAFTK_EINVAL, "farm response needs B_drag, F_drag, F_iner of the per-FOWT solve");
     if (d->n_bem_head > 0 && !solved->F_BEM) return set_err(RAFTK_EINVAL, "farm response: the designs carry BEM excitation, F_BEM is required");
     const int n = 6 * f->n_fowt;
+    FarmParams P;
+    P.N = f->n_fowt; P.nC = c->n_cases; P.nw = d->nw; P.nF = f->n_farms;
+    P.arr_stride = f->arr_shared ? 0 : (size_t)n * n;
+    P.B_drag = solved->B_drag;
+    P.F_drag = reinterpret_cast<const double2 *>(solved->F_drag);
+    P.F_iner = reinterpret_cast<const double2 *>(solved->F_iner);
+    P.F_BEM = d->n_bem_head > 0 ? reinterpret_cast<const double2 *>(solved->F_BEM) : nullptr;
+    P.M_arr = f->M_arr; P.B_arr = f->B_arr; P.C_arr = f->C_arr;
+    P.Xi = reinterpret_cast<double2 *>(f->Xi_sys); P.info = f->info;
     if (!farm_on_chip(f->n_fowt)) {
-        // persistent CTAs over the (case, frequency) systems, each CTA on its own slab of the caller's workspace
+        // persistent CTAs over the (farm, case, frequency) systems, each CTA on its own slab of the caller's workspace
         const GluPlan g = glu_plan(n);
         if (!g.pw) return set_err(RAFTK_EINVAL, "farm response: 6N too large for one panel column in shared memory");
         const size_t slab = farm_slab_bytes(f->n_fowt);
         if (!ws || ws_bytes < slab)
             return set_err(RAFTK_EINVAL, "farm response: a farm this size needs a workspace of at least one [6N][6N+1] slab "
                                          "(raftk_farm_workspace_bytes, raftk_farm_response_ws_dev)");
-        const long long nsys = (long long)c->n_cases * d->nw;
+        const long long nsys = (long long)f->n_farms * c->n_cases * d->nw;
         const int grid = (int)std::min<long long>(std::min<long long>(nsys, (long long)(ws_bytes / slab)), (long long)g.per_sm * sm_count());
         static SmemOptIn opt_g(0);
         CUDA_TRY(opt_g.ensure(k_farm_response_global, g.smem));
         DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
         CasesDev C = to_dev(c);
-        FarmParams P;
-        P.N = f->n_fowt; P.nC = c->n_cases; P.nw = d->nw;
-        P.B_drag = solved->B_drag;
-        P.F_drag = reinterpret_cast<const double2 *>(solved->F_drag);
-        P.F_iner = reinterpret_cast<const double2 *>(solved->F_iner);
-        P.F_BEM = d->n_bem_head > 0 ? reinterpret_cast<const double2 *>(solved->F_BEM) : nullptr;
-        P.M_arr = f->M_arr; P.B_arr = f->B_arr; P.C_arr = f->C_arr;
-        P.Xi = reinterpret_cast<double2 *>(f->Xi_sys); P.info = f->info;
         {
             ProfScope ps(st, 1);
             k_farm_response_global<<<grid, GLU_T, g.smem, st>>>(D, C, P, static_cast<double2 *>(ws), g.pw);
@@ -978,29 +1008,24 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
     const size_t sys_bytes = (size_t)n * (n + 1) * sizeof(double2);
     const int wpc = warp ? (int)std::max<size_t>(1, std::min<size_t>(FARM_WPC, (100 * 1024) / sys_bytes)) : 1;
     const size_t smem = (size_t)wpc * sys_bytes;
+    // grid = (frequency groups, case, farm): the y and z extents of a grid end at 65535
     if (c->n_cases > 65535) return set_err(RAFTK_EINVAL, "farm response: more than 65535 cases per call");
+    if (f->n_farms > 65535) return set_err(RAFTK_EINVAL, "farm response: more than 65535 farms per call with the system in shared memory (6N <= 120)");
     static SmemOptIn opt_w(48 * 1024), opt_b(48 * 1024);
     if (warp) CUDA_TRY(opt_w.ensure(k_farm_response<true>, smem));
     else CUDA_TRY(opt_b.ensure(k_farm_response<false>, smem));
     DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
     CasesDev C = to_dev(c);
-    FarmParams P;
-    P.N = f->n_fowt; P.nC = c->n_cases; P.nw = d->nw;
-    P.B_drag = solved->B_drag;
-    P.F_drag = reinterpret_cast<const double2 *>(solved->F_drag);
-    P.F_iner = reinterpret_cast<const double2 *>(solved->F_iner);
-    P.F_BEM = d->n_bem_head > 0 ? reinterpret_cast<const double2 *>(solved->F_BEM) : nullptr;
-    P.M_arr = f->M_arr; P.B_arr = f->B_arr; P.C_arr = f->C_arr;
-    P.Xi = reinterpret_cast<double2 *>(f->Xi_sys); P.info = f->info;
     {
         ProfScope ps(st, 1);
         // 6N = 12 (the shipped two-FOWT farm): rows in registers, one lane per row, two systems per warp (k_farm_rows);
         // RAFTK_FARM_SMEM=1 keeps the shared-memory warp kernel (A/B).  At 6N = 18 / 24 the register rows need 188 / 238
         // registers, so those stay on the warp kernel.
         const bool rows = n == 12 && !getenv("RAFTK_FARM_SMEM");
-        if (rows) k_farm_rows<12><<<dim3((d->nw + 7) / 8, c->n_cases), 128, 0, st>>>(D, C, P);
-        else if (warp) k_farm_response<true><<<dim3((d->nw + wpc - 1) / wpc, c->n_cases), 32 * wpc, smem, st>>>(D, C, P);
-        else k_farm_response<false><<<dim3(d->nw, c->n_cases), 256, smem, st>>>(D, C, P);
+        const unsigned gy = c->n_cases, gz = f->n_farms;
+        if (rows) k_farm_rows<12><<<dim3((d->nw + 7) / 8, gy, gz), 128, 0, st>>>(D, C, P);
+        else if (warp) k_farm_response<true><<<dim3((d->nw + wpc - 1) / wpc, gy, gz), 32 * wpc, smem, st>>>(D, C, P);
+        else k_farm_response<false><<<dim3(d->nw, gy, gz), 256, smem, st>>>(D, C, P);
         if (rows) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_ROWS12, 128);
         else if (warp) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_WARP, 32 * wpc);
         else disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_BLOCK, 256);
@@ -1010,15 +1035,33 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
     return RAFTK_OK;
 }
 
+// the single-farm entries: farm.n_fowt names the whole batch of designs
+static int farm_launch_one(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f, void *ws,
+                           size_t ws_bytes, cudaStream_t st)
+{
+    if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "farm response: null argument");
+    if (f->n_fowt != d->n_designs || f->n_fowt < 1) return set_err(RAFTK_EINVAL, "farm response: farm.n_fowt must equal designs.n_designs");
+    if (!f->Xi_sys) return set_err(RAFTK_EINVAL, "farm response needs farm.Xi_sys");
+    const raftk_farm_batch b = farm_as_batch(f);
+    return farm_launch(d, c, solved, &b, ws, ws_bytes, st);
+}
+
 extern "C" int raftk_farm_response_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f,
                                        void *stream)
 {
     disp_reset();
-    return farm_launch(d, c, solved, f, nullptr, 0, (cudaStream_t)stream);
+    return farm_launch_one(d, c, solved, f, nullptr, 0, (cudaStream_t)stream);
 }
 
 extern "C" int raftk_farm_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f,
                                           void *workspace, size_t workspace_bytes, void *stream)
+{
+    disp_reset();
+    return farm_launch_one(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int raftk_farm_batch_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
+                                                const raftk_farm_batch *f, void *workspace, size_t workspace_bytes, void *stream)
 {
     disp_reset();
     return farm_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
@@ -1218,7 +1261,7 @@ static void stage_designs_cases(Staging &S, const raftk_designs *d, const raftk_
 }
 
 static int host_run(const char *who, const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
-                    const double *Xi_in, int mode, const raftk_farm *farm = nullptr)
+                    const double *Xi_in, int mode, const raftk_farm_batch *farm = nullptr)
 {
     disp_reset();
     int rc = validate(d, c);
@@ -1232,11 +1275,12 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
     stage_designs_cases(S, d, c, dd, cc);
     const double *Xi_in_d = nullptr;
     S.in(Xi_in_d, Xi_in, nR);
-    raftk_farm fd;
+    raftk_farm_batch fd;
     memset(&fd, 0, sizeof(fd));
-    if (farm) {                                           // array-level matrices: staged with the other small inputs
+    if (farm) {                                           // array-level matrices (one set, or one per farm): staged with the other small inputs
         fd = *farm;
-        S.in(fd.M_arr, farm->M_arr, 36 * nD * nD); S.in(fd.B_arr, farm->B_arr, 36 * nD * nD); S.in(fd.C_arr, farm->C_arr, 36 * nD * nD);
+        const size_t nA = (farm->arr_shared ? 1 : (size_t)farm->n_farms) * 36 * farm->n_fowt * farm->n_fowt;
+        S.in(fd.M_arr, farm->M_arr, nA); S.in(fd.B_arr, farm->B_arr, nA); S.in(fd.C_arr, farm->C_arr, nA);
     }
     // the solve is planned once, at the caller's cluster size, and launched with the workspace that plan needs; excitation
     // and linearisation need the whole batch's tables in one chunk
@@ -1276,7 +1320,7 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
     char *ws, *fws = nullptr;
     S.buf(ws, wb);
     const size_t fwb = farm ? farm_ws_bytes(d, c, farm) : 0;                  // slabs of the global-memory system kernel (0 on chip)
-    if (farm) { S.out(fd.Xi_sys, nR, farm->Xi_sys); S.out(fd.info, farm->info ? nC * nw : 0, farm->info); S.buf(fws, fwb); }
+    if (farm) { S.out(fd.Xi_sys, nR, farm->Xi_sys); S.out(fd.info, farm->info ? farm->n_farms * nC * nw : 0, farm->info); S.buf(fws, fwb); }
     if ((rc = S.commit())) return rc;
     if (qtf_solve) {
         if ((rc = run_qtf(&dd, &cc, od.F_2nd, od.F_2nd_mean, 0))) return rc;
@@ -1319,8 +1363,18 @@ extern "C" int raftk_solve_dynamics_farm_host(const raftk_designs *d, const raft
 {
     if (!out || !out->Xi || !out->status || !o) return set_err(RAFTK_EINVAL, "Xi, status and opts are required");
     if (!f || !f->Xi_sys) return set_err(RAFTK_EINVAL, "farm.Xi_sys is required");
-    if (d && f->n_fowt != d->n_designs) return set_err(RAFTK_EINVAL, "farm response: farm.n_fowt must equal designs.n_designs");
-    return host_run("raftk_solve_dynamics_farm_host", d, c, o, out, nullptr, 0, f);
+    if (d && (f->n_fowt != d->n_designs || f->n_fowt < 1)) return set_err(RAFTK_EINVAL, "farm response: farm.n_fowt must equal designs.n_designs");
+    const raftk_farm_batch b = farm_as_batch(f);
+    return host_run("raftk_solve_dynamics_farm_host", d, c, o, out, nullptr, 0, &b);
+}
+
+extern "C" int raftk_solve_dynamics_farm_batch_host(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o,
+                                                    const raftk_outputs *out, const raftk_farm_batch *f)
+{
+    if (!out || !out->Xi || !out->status || !o) return set_err(RAFTK_EINVAL, "Xi, status and opts are required");
+    if (!d || !f) return set_err(RAFTK_EINVAL, "farm batch: null argument");
+    if (int rc = farm_batch_shape(d, f)) return rc;
+    return host_run("raftk_solve_dynamics_farm_batch_host", d, c, o, out, nullptr, 0, f);
 }
 
 extern "C" int raftk_second_order_force_host(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *out)

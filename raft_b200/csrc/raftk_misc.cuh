@@ -180,43 +180,49 @@ __global__ void __launch_bounds__(128) k_system_solve(int n, int nrhs, double2 *
 // outputs of the drag-linearisation solve: no host assembly of Z, no per-case transfer of nw n^2 complex numbers.
 // WARP = true : small systems (6N <= 24), one WARP per (frequency, case), up to FARM_WPC systems per CTA, no CTA-wide barriers;
 // WARP = false: one CTA per (frequency, case), blocked LU.
+// A call solves nF farms of N FOWTs each (one farm: nF = 1): design f * N + i is FOWT i of farm f.  The shared-memory and
+// register kernels take the farm from blockIdx.z, so the systems a CTA packs along the frequency axis belong to one farm and
+// a ragged last group ends at nw; k_farm_response_global walks (farm, case, frequency) systems.
 // ------------------------------------------------------------------------------------------------
 struct FarmParams {
-    int N, nC, nw;
-    const double *B_drag;                       // [N][nC][36]
-    const double2 *F_drag, *F_iner, *F_BEM;     // [N][nC][6][nw]; F_BEM may be NULL
-    const double *M_arr, *B_arr, *C_arr;        // [6N][6N] or NULL
-    double2 *Xi;                                // [nC][6N][nw]
-    int *info;                                  // [nC][nw] or NULL
+    int N, nC, nw, nF;
+    size_t arr_stride;                          // doubles between two farms' array matrices: (6N)^2, or 0 when every farm shares one set
+    const double *B_drag;                       // [nF * N][nC][36]
+    const double2 *F_drag, *F_iner, *F_BEM;     // [nF * N][nC][6][nw]; F_BEM may be NULL
+    const double *M_arr, *B_arr, *C_arr;        // [nF or 1][6N][6N] or NULL
+    double2 *Xi;                                // [nF][nC][6N][nw]
+    int *info;                                  // [nF][nC][nw] or NULL
 };
 #define FARM_WPC 4
 
-// Assembly of one (case c, frequency iw) system, shared by k_farm_response and k_farm_response_global: Z_sys into A [n][nc]
-// (nc = n + 1) and the right-hand side into its column n, spread over the gsize threads of a group.
-__device__ __forceinline__ void farm_assemble(const DesignsDev &D, const CasesDev &Cs, const FarmParams &P, int c, int iw, double2 *A,
+// Assembly of one (farm, case c, frequency iw) system, shared by k_farm_response and k_farm_response_global: Z_sys into
+// A [n][nc] (nc = n + 1) and the right-hand side into its column n, spread over the gsize threads of a group.
+__device__ __forceinline__ void farm_assemble(const DesignsDev &D, const CasesDev &Cs, const FarmParams &P, int farm, int c, int iw, double2 *A,
                                               int gtid, int gsize)
 {
     const int n = 6 * P.N, nc = n + 1, nw = P.nw;
     const double w = D.w[iw], w2 = w * w;
     const int cp = Cs.primary ? Cs.primary[c] : c;                   // secondary wave trains use their primary's damping
+    const size_t d0 = (size_t)farm * P.N, ao = (size_t)farm * P.arr_stride;
     for (int t = gtid; t < n * n; t += gsize) {
-        const int a = t / n, b = t % n, i = a / 6, j = b / 6;
+        const int a = t / n, b = t % n, j = b / 6;
+        const size_t i = d0 + a / 6;                                 // design of block row a
         double zr = 0.0, zi = 0.0;
-        if (i == j) {
-            const int e = 6 * (a - 6 * i) + (b - 6 * j);
+        if (a / 6 == j) {
+            const int e = 6 * (a % 6) + (b - 6 * j);
             double M = D.M0[(size_t)i * 36 + e], B = D.B0[(size_t)i * 36 + e] + P.B_drag[((size_t)i * P.nC + cp) * 36 + e];
             if (D.A_w) { M += D.A_w[((size_t)i * 36 + e) * nw + iw]; B += D.B_w[((size_t)i * 36 + e) * nw + iw]; }
             zr = fma(-w2, M, D.C0[(size_t)i * 36 + e]);
             zi = w * B;
         }
-        if (P.C_arr) zr += P.C_arr[t];
-        if (P.M_arr) zr -= w2 * P.M_arr[t];
-        if (P.B_arr) zi += w * P.B_arr[t];
+        if (P.C_arr) zr += P.C_arr[ao + t];
+        if (P.M_arr) zr -= w2 * P.M_arr[ao + t];
+        if (P.B_arr) zi += w * P.B_arr[ao + t];
         A[a * nc + b] = make_double2(zr, zi);
     }
     for (int a = gtid; a < n; a += gsize) {
-        const int i = a / 6, e = a - 6 * i;
-        const size_t o = (((size_t)i * P.nC + c) * 6 + e) * nw + iw;
+        const int e = a % 6;
+        const size_t o = (((d0 + a / 6) * P.nC + c) * 6 + e) * nw + iw;
         double2 f = P.F_drag[o];
         const double2 h = P.F_iner[o];
         f.x += h.x; f.y += h.y;
@@ -235,16 +241,17 @@ __global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(De
     const int n = 6 * P.N, nc = n + 1, nw = P.nw;
     const int g = WARP ? (int)(threadIdx.x >> 5) : 0, gtid = WARP ? (int)(threadIdx.x & 31) : (int)threadIdx.x;
     const int gsize = WARP ? 32 : (int)blockDim.x;
-    const int iw = WARP ? (int)(blockIdx.x * (blockDim.x >> 5)) + g : (int)blockIdx.x, c = blockIdx.y;
+    const int iw = WARP ? (int)(blockIdx.x * (blockDim.x >> 5)) + g : (int)blockIdx.x, c = blockIdx.y, f = blockIdx.z;
     if (iw >= nw) return;                                            // (warp-uniform; no CTA-wide barrier follows in the WARP variant)
     double2 *A = reinterpret_cast<double2 *>(smem_raw) + (size_t)g * n * nc;
-    farm_assemble(D, Cs, P, c, iw, A, gtid, gsize);
+    const size_t u = (size_t)f * P.nC + c;                           // row of Xi and info
+    farm_assemble(D, Cs, P, f, c, iw, A, gtid, gsize);
     if (gtid == 0) bad_s[g] = 0;
     gsync<WARP>();
     if (WARP) lu_unblocked<true>(A, n, nc, 1, gtid, gsize, &piv_s[g], &rinv_s[g], &bad_s[g]);
     else lu_blocked(A, n, nc, 1, &piv_s[g], &rinv_s[g], &bad_s[g]);
-    for (int a = gtid; a < n; a += gsize) P.Xi[((size_t)c * n + a) * nw + iw] = A[a * nc + n];
-    if (gtid == 0 && P.info) P.info[(size_t)c * nw + iw] = bad_s[g];
+    for (int a = gtid; a < n; a += gsize) P.Xi[(u * n + a) * nw + iw] = A[a * nc + n];
+    if (gtid == 0 && P.info) P.info[u * nw + iw] = bad_s[g];
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -390,7 +397,7 @@ __device__ __forceinline__ void lu_global(double2 *A, int lda, double2 *B, int l
 }
 
 // farm system response of k_farm_response (same assembly) for any N: persistent CTAs, CTA b owns slab b of the workspace
-// ([6N][6N+1] double2) and solves the (case, frequency) systems b, b + gridDim.x, ...
+// ([6N][6N+1] double2) and solves the (farm, case, frequency) systems b, b + gridDim.x, ... of the nF * nC * nw in all
 __global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D, CasesDev Cs, FarmParams P, double2 *ws, int pw)
 {
     extern __shared__ __align__(16) double smem_raw[];
@@ -398,14 +405,15 @@ __global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D,
     double2 *Ps = reinterpret_cast<double2 *>(smem_raw);
     const int n = 6 * P.N, nc = n + 1, nw = P.nw;
     double2 *A = ws + (size_t)blockIdx.x * n * nc;
-    const long long nsys = (long long)P.nC * nw;
+    const long long nsys = (long long)P.nF * P.nC * nw;
     for (long long s = blockIdx.x; s < nsys; s += gridDim.x) {
-        const int c = (int)(s / nw), iw = (int)(s - (long long)c * nw);
-        farm_assemble(D, Cs, P, c, iw, A, threadIdx.x, GLU_T);
+        const long long u = s / nw;                                    // f * nC + c: row of Xi and info
+        const int iw = (int)(s - u * nw), f = (int)(u / P.nC), c = (int)(u - (long long)f * P.nC);
+        farm_assemble(D, Cs, P, f, c, iw, A, threadIdx.x, GLU_T);
         __syncthreads();
         lu_global(A, nc, A + n, nc, n, 1, pw, Ps, S);
-        for (int a = threadIdx.x; a < n; a += GLU_T) P.Xi[((size_t)c * n + a) * nw + iw] = A[(size_t)a * nc + n];
-        if (threadIdx.x == 0 && P.info) P.info[(size_t)c * nw + iw] = S.bad;
+        for (int a = threadIdx.x; a < n; a += GLU_T) P.Xi[((size_t)u * n + a) * nw + iw] = A[(size_t)a * nc + n];
+        if (threadIdx.x == 0 && P.info) P.info[(size_t)u * nw + iw] = S.bad;
         __syncthreads();                                               // the slab is rewritten by the next system
     }
 }
@@ -438,26 +446,27 @@ __global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, Fa
     constexpr int LPS = N6 <= 16 ? 16 : 32, SPW = 32 / LPS, NC = N6 + 1;
     const int nw = P.nw, lane = threadIdx.x & 31, r = lane & (LPS - 1);
     const int sys = ((int)blockIdx.x * ((int)blockDim.x >> 5) + ((int)threadIdx.x >> 5)) * SPW + lane / LPS;
-    const int c = blockIdx.y;
+    const int c = blockIdx.y, f = blockIdx.z;
     const bool live = sys < nw;                        // a group beyond the grid keeps shuffling with its neighbours but never stores
     const int iw = live ? sys : nw - 1;
     const bool row_ok = r < N6;
     const int a = row_ok ? r : 0;
     const double w = D.w[iw], w2 = w * w;
     const int cp = Cs.primary ? Cs.primary[c] : c;
-    const int i = a / 6, ea = a - 6 * i;
+    const int ib = a / 6, ea = a - 6 * ib;             // block row of the system; its design is FOWT ib of farm f
+    const size_t i = (size_t)f * P.N + ib, ao = (size_t)f * P.arr_stride, u = (size_t)f * P.nC + c;
     double2 row[NC];
 #pragma unroll
     for (int b = 0; b < N6; b++) {
         double zr = 0.0, zi = 0.0;
-        if (b / 6 == i) {
+        if (b / 6 == ib) {
             const int e = 6 * ea + (b - 6 * (b / 6));
             double M = D.M0[(size_t)i * 36 + e], B = D.B0[(size_t)i * 36 + e] + P.B_drag[((size_t)i * P.nC + cp) * 36 + e];
             if (D.A_w) { M += D.A_w[((size_t)i * 36 + e) * nw + iw]; B += D.B_w[((size_t)i * 36 + e) * nw + iw]; }
             zr = fma(-w2, M, D.C0[(size_t)i * 36 + e]);
             zi = w * B;
         }
-        const int t = a * N6 + b;
+        const size_t t = ao + a * N6 + b;
         if (P.C_arr) zr += P.C_arr[t];
         if (P.M_arr) zr -= w2 * P.M_arr[t];
         if (P.B_arr) zi += w * P.B_arr[t];
@@ -525,8 +534,8 @@ __global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, Fa
             row[N6].y -= pv.x * xk.y + pv.y * xk.x;
         }
     });
-    if (live && row_ok) P.Xi[((size_t)c * N6 + r) * nw + iw] = x;
-    if (live && r == 0 && P.info) P.info[(size_t)c * nw + iw] = bad;
+    if (live && row_ok) P.Xi[(u * N6 + r) * nw + iw] = x;
+    if (live && r == 0 && P.info) P.info[u * nw + iw] = bad;
 }
 
 // std = sqrt(1/2 sum_w |Y|^2) of one 128-thread CTA from each thread's partial sum s: warp shuffles, then the four warps

@@ -15,7 +15,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (RaftkCases, RaftkDesigns, RaftkFarm, RaftkGeneral, RaftkGeneralBatch, RaftkGeneralFd, RaftkGeneralQtf, RaftkOutputs, RaftkSlender, RaftkSlenderBatch,
+from ._lib import (RaftkCases, RaftkDesigns, RaftkFarm, RaftkFarmBatch, RaftkGeneral, RaftkGeneralBatch, RaftkGeneralFd, RaftkGeneralQtf, RaftkOutputs, RaftkSlender, RaftkSlenderBatch,
                    RaftkSlenderOutputs, RaftkSolveOpts, check, lib)
 
 _F8 = np.float64
@@ -376,6 +376,52 @@ def solve_dynamics_farm(batch, cases, C_arr=None, M_arr=None, B_arr=None, n_iter
     check(lib.raftk_solve_dynamics_farm_host(C.byref(d), C.byref(c), C.byref(o), C.byref(os_), C.byref(f)))
     if _plan_overflowed(outs):                      # Xi_sys was assembled from those units' zero loads: solve it all again
         check(lib.raftk_solve_dynamics_farm_host(C.byref(_host_struct(worst_case_hints(batch))), C.byref(c), C.byref(o), C.byref(os_), C.byref(f)))
+        _raise_on_plan(outs)
+    return outs
+
+
+def _farm_batch_matrices(n_farms, n, M_arr, B_arr, C_arr):
+    """The array matrices of a farm batch as C-contiguous float64 -> (dict name -> array, arr_shared): every matrix given is
+    [6N,6N] (one set for every farm) or every one is [F,6N,6N]."""
+    mats = {nm: np.ascontiguousarray(v, dtype=_F8) for nm, v in (("M_arr", M_arr), ("B_arr", B_arr), ("C_arr", C_arr)) if v is not None}
+    shapes = {a.shape for a in mats.values()}
+    if len(shapes) > 1 or not shapes <= {(n, n), (n_farms, n, n)}:
+        raise ValueError("M_arr, B_arr and C_arr must all be [%d, %d] or all be [%d, %d, %d]" % (n, n, n_farms, n, n))
+    return mats, 0 if shapes == {(n_farms, n, n)} else 1
+
+
+def solve_dynamics_farm_batch(batch, cases, n_fowt, C_arr=None, M_arr=None, B_arr=None, n_iter=10, tol=0.01, xi_start=0.0, cluster_size=0,
+                              want=("Xi", "status", "B_drag"), out=None):
+    """``solve_dynamics_farm`` for F farms of ``n_fowt`` FOWTs each in ONE call (a layout or shared-mooring study): design
+    ``f * n_fowt + i`` of ``batch`` is FOWT i of farm f, all farms over the same case table.  Array matrices: [6N,6N] used by
+    every farm, or [F,6N,6N].  -> the per-FOWT output dict plus ``Xi_sys`` complex [F, nC, 6N, nw] and ``info`` [F, nC, nw];
+    farm f's rows are what ``solve_dynamics_farm`` returns for that farm alone, bit for bit."""
+    N, nC, nw = int(n_fowt), cases.n_cases, batch.nw
+    if N < 1 or batch.n_designs % N:
+        raise ValueError("n_fowt must divide the batch's %d designs" % batch.n_designs)
+    F, n = batch.n_designs // N, 6 * N
+    mats, shared = _farm_batch_matrices(F, n, M_arr, B_arr, C_arr)
+    want = tuple(dict.fromkeys(tuple(want) + ("Xi", "status")))
+    outs = dict(out) if out is not None else {}
+    for k_, v in _alloc_outputs(batch.n_designs, nC, nw, tuple(k for k in want if k not in outs)).items():
+        outs[k_] = v
+    outs.setdefault("Xi_sys", np.zeros([F, nC, n, nw], dtype=np.complex128))
+    outs.setdefault("info", np.zeros([F, nC, nw], dtype=_I4))
+    for k_, shape, dt in (("Xi_sys", (F, nC, n, nw), np.complex128), ("info", (F, nC, nw), _I4)):
+        if outs[k_].shape != shape or outs[k_].dtype != dt or not outs[k_].flags.c_contiguous:
+            raise ValueError("out[%r] must be a C-contiguous %s array %s" % (k_, np.dtype(dt).name, list(shape)))
+    f = RaftkFarmBatch()
+    f.n_farms, f.n_fowt, f.arr_shared = F, N, shared
+    for nm in ("M_arr", "B_arr", "C_arr"):
+        setattr(f, nm, mats[nm].ctypes.data if nm in mats else None)
+    f.Xi_sys, f.info = outs["Xi_sys"].ctypes.data, outs["info"].ctypes.data
+    c = _host_struct(cases)
+    o = RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), 0, 0)
+    os_ = _out_struct(outs, lambda a: a.ctypes.data)
+    check(lib.raftk_solve_dynamics_farm_batch_host(C.byref(_host_struct(batch)), C.byref(c), C.byref(o), C.byref(os_), C.byref(f)))
+    if _plan_overflowed(outs):                      # Xi_sys was assembled from those units' zero loads: solve it all again
+        check(lib.raftk_solve_dynamics_farm_batch_host(C.byref(_host_struct(worst_case_hints(batch))), C.byref(c), C.byref(o), C.byref(os_),
+                                                       C.byref(f)))
         _raise_on_plan(outs)
     return outs
 
@@ -1354,6 +1400,14 @@ def farm_workspace_bytes(n_fowt, n_cases, nw):
     return int(lib.raftk_farm_workspace_bytes(C.byref(d), C.byref(c), C.byref(f)))
 
 
+def farm_batch_workspace_bytes(n_farms, n_fowt, n_cases, nw):
+    """``farm_workspace_bytes`` for a batch of ``n_farms`` farms (raftk_farm_batch_workspace_bytes): the slabs are capped at the
+    n_farms * n_cases * nw systems of the call."""
+    d, c, f = RaftkDesigns(), RaftkCases(), RaftkFarmBatch()
+    d.n_designs, d.nw, c.n_cases, f.n_farms, f.n_fowt, f.arr_shared = int(n_farms) * int(n_fowt), int(nw), int(n_cases), int(n_farms), int(n_fowt), 1
+    return int(lib.raftk_farm_batch_workspace_bytes(C.byref(d), C.byref(c), C.byref(f)))
+
+
 def system_solve(Z, F):
     """Farm system response (raft_model.py:1164-1216): Z [nw,n,n], F [nw,n] or [nw,n,nrhs] -> Xi, info."""
     Z = np.array(Z, dtype=np.complex128, order="C")
@@ -1504,33 +1558,47 @@ class DeviceSession:
                                                       C.byref(peers), self.workspace.data_ptr(), self.workspace_bytes, self._stream()))
             check(lib.raftk_peer_barrier_dev(C.byref(peers), timeout_flag, self._stream()))
 
-    def farm_response(self, C_arr=None, M_arr=None, B_arr=None):
+    def farm_response(self, C_arr=None, M_arr=None, B_arr=None, n_fowt=None):
         """Enqueue the coupled 6N-DOF system response of the LAST ``solve`` (the session's designs are the FOWTs of the
         array; it must have been created with want including B_drag, F_drag, F_iner [+ F_BEM]).  -> (Xi_sys [nC,6N,nw], info).
         Any N: farms whose system does not fit in shared memory are solved in a device workspace sized once
-        (raftk_farm_workspace_bytes) and kept with the session."""
+        (raftk_farm_workspace_bytes) and kept with the session.
+        ``n_fowt``: the session's designs are n_designs / n_fowt farms of n_fowt FOWTs each (design f * n_fowt + i is FOWT i
+        of farm f), array matrices [6N,6N] for every farm or [F,6N,6N] -> (Xi_sys [F,nC,6N,nw], info [F,nC,nw]).  The
+        matrices, outputs and workspace of either form are set up on its first call and kept with the session."""
         torch = self.torch
-        N, nC, nw = self.batch.n_designs, self.cases.n_cases, self.batch.nw
-        n = 6 * N
-        if not hasattr(self, "_farm"):
+        nC, nw = self.cases.n_cases, self.batch.nw
+        N = self.batch.n_designs if n_fowt is None else int(n_fowt)
+        if N < 1 or self.batch.n_designs % N:
+            raise ValueError("n_fowt must divide the session's %d designs" % self.batch.n_designs)
+        F, n = self.batch.n_designs // N, 6 * N
+        key = "_farm" if n_fowt is None else "_farm_batch"
+        if not hasattr(self, key) or getattr(self, key)[0].n_fowt != N:
+            host, shared = _farm_batch_matrices(F, n, M_arr, B_arr, C_arr)
+            lead = [] if n_fowt is None else [F]
             with torch.cuda.device(self.device):
-                mats = {nm: (torch.from_numpy(np.ascontiguousarray(v, dtype=_F8)).to(self.device) if v is not None else None)
-                        for nm, v in (("M_arr", M_arr), ("B_arr", B_arr), ("C_arr", C_arr))}
-                xi = torch.zeros([nC, n, nw], dtype=torch.complex128, device=self.device)
-                info = torch.zeros([nC, nw], dtype=torch.int32, device=self.device)
-            f = RaftkFarm()
+                mats = {nm: (torch.from_numpy(host[nm]).to(self.device) if nm in host else None) for nm in ("M_arr", "B_arr", "C_arr")}
+                xi = torch.zeros(lead + [nC, n, nw], dtype=torch.complex128, device=self.device)
+                info = torch.zeros(lead + [nC, nw], dtype=torch.int32, device=self.device)
+            if n_fowt is None:
+                f = RaftkFarm()
+                query = lib.raftk_farm_workspace_bytes
+            else:
+                f = RaftkFarmBatch()
+                f.n_farms, f.arr_shared = F, shared
+                query = lib.raftk_farm_batch_workspace_bytes
             f.n_fowt = N
             for nm, t in mats.items():
                 setattr(f, nm, t.data_ptr() if t is not None else None)
             f.Xi_sys, f.info = xi.data_ptr(), info.data_ptr()
-            wsb = int(lib.raftk_farm_workspace_bytes(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(f)))
+            wsb = int(query(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(f)))
             with torch.cuda.device(self.device):
                 ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=self.device)
-            self._farm = (f, mats, xi, info, ws, wsb)
-        f, _, xi, info, ws, wsb = self._farm
+            setattr(self, key, (f, mats, xi, info, ws, wsb))
+        f, _, xi, info, ws, wsb = getattr(self, key)
+        launch = lib.raftk_farm_response_ws_dev if n_fowt is None else lib.raftk_farm_batch_response_ws_dev
         with torch.cuda.device(self.device):
-            check(lib.raftk_farm_response_ws_dev(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f),
-                                                 ws.data_ptr(), wsb, self._stream()))
+            check(launch(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f), ws.data_ptr(), wsb, self._stream()))
         return xi, info
 
     def second_order_force(self):
