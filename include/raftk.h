@@ -182,12 +182,12 @@ long long raftk_launch_count(void);
  * Which kernel variant the last call on the calling host thread launched.  The entry points pick among several kernels by
  * shape, workspace size and RAFTK_* environment switches; the launch sites themselves fill this record, so it describes what
  * ran, not a plan recomputed afterwards.  Every entry point of the solve, second-order force, generalised-DOF, farm and
- * system-solve families clears it first; a call that fails before its launch leaves it cleared.  When one call launches
+ * system-solve and eigen families clears it first; a call that fails before its launch leaves it cleared.  When one call launches
  * several families (a solve that computes its second-order force first, a farm host call) the last launch is reported.
  * Host bookkeeping only: no device work, no synchronisation.
  */
 enum { RAFTK_FAMILY_NONE = 0, RAFTK_FAMILY_SOLVE = 1, RAFTK_FAMILY_QTF = 2, RAFTK_FAMILY_GENERAL = 3, RAFTK_FAMILY_FARM = 4,
-       RAFTK_FAMILY_SYSTEM = 5 };
+       RAFTK_FAMILY_SYSTEM = 5, RAFTK_FAMILY_EIGEN = 6 };
 enum {
     RAFTK_KERNEL_NONE = 0,
     RAFTK_KERNEL_V1 = 1,              /* k_depth_table + k_excitation (+ k_drag_solve), tables in the workspace          */
@@ -206,7 +206,10 @@ enum {
     RAFTK_KERNEL_SYS_UNBLOCKED = 14,  /* k_system_solve, column-at-a-time LU (n <= 24)                                    */
     RAFTK_KERNEL_SYS_BLOCKED = 15,    /* k_system_solve, blocked LU (n > 24)                                              */
     RAFTK_KERNEL_FARM_GLOBAL = 16,    /* k_farm_response_global: system in a workspace slab, LU blocked in global memory   */
-    RAFTK_KERNEL_SYS_GLOBAL = 17      /* k_system_solve_global: Z factored in place, LU blocked in global memory           */
+    RAFTK_KERNEL_SYS_GLOBAL = 17,     /* k_system_solve_global: Z factored in place, LU blocked in global memory           */
+    RAFTK_KERNEL_EIG_SMALL = 18,      /* k_eig_small: one system per thread (n <= 12)                                      */
+    RAFTK_KERNEL_EIG_CTA_SMEM = 19,   /* k_eig_cta<true>: one system per CTA, H in shared memory                           */
+    RAFTK_KERNEL_EIG_CTA_SLAB = 20    /* k_eig_cta<false>: one system per CTA, H in the workspace slab                     */
 };
 typedef struct raftk_dispatch {
     int32_t family;           /* RAFTK_FAMILY_*                                                                          */
@@ -688,6 +691,42 @@ int raftk_farm_batch_response_ws_dev(const raftk_designs *d, const raftk_cases *
                                      const raftk_farm_batch *f, void *workspace, size_t workspace_bytes, void *stream);
 int raftk_solve_dynamics_farm_batch_host(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o,
                                          const raftk_outputs *out, const raftk_farm_batch *f);
+
+/*
+ * Natural frequencies and mode shapes (Model.solveEigen raft_model.py:436-547, FOWT.solveEigen raft_fowt.py:1646-1729): the
+ * eigenvalues and right eigenvectors of M^-1 C for n_systems systems of n DOFs, what np.linalg.eig(np.linalg.solve(M, C))
+ * returns, in the reference's output order.  Per system: LU of M with partial pivoting, A = M^-1 C, power-of-two balancing,
+ * Householder Hessenberg reduction, Francis double-shift QR (at most 30 n iterations), eigenvectors by back-substitution on
+ * the real Schur form, un-balanced and scaled to unit 2-norm; a complex vector is rotated so that its largest component is
+ * real.  FP64 throughout.
+ * sort RAFTK_EIG_SORT_DOF: rows n-1..0 of |V| each claim the column of their largest entry (first index on a tie; a claimed
+ * column is zeroed and the search repeated), the claims reversed (raft_model.py:490-516).  A row that claims nothing leaves
+ * NaN in the last slot(s) of lam and modes, where the reference returns fewer modes.
+ * sort RAFTK_EIG_SORT_ASCENDING: by real part, then imaginary part (np.argsort of complex values); ties keep LAPACK's order.
+ * Kernels: n <= 12 one system per thread (k_eig_small, no workspace); n > 12 one system per CTA (k_eig_cta), persistent CTAs
+ * with Q and the back-substitution in a per-CTA workspace slab, H in shared memory while it fits the opt-in limit (n up to
+ * about 165 on an H100) and in the slab beyond.  A system's outputs do not depend on the batch or the workspace size.
+ * info flags per system: RAFTK_EIG_SMALL_DIAG a diagonal of M or C below 1 (the reference's viability check, on the inputs);
+ * RAFTK_EIG_NONPOSITIVE an eigenvalue with real part <= 0; RAFTK_EIG_COMPLEX a complex eigenvalue (informational);
+ * RAFTK_EIG_SINGULAR an exactly zero pivot of M; RAFTK_EIG_NOCONV the QR iteration did not converge.  The last two leave
+ * NaN in the system's lam and modes.  fns = sqrt(lam) / 2 pi is left to the caller.
+ * raftk_eigen_workspace_bytes: 0 for n <= 12, else whole slabs: one per resident CTA, at most one per system (without a
+ * device it answers for an H100).  Fewer bytes run fewer CTAs with the same results.
+ * RAFTK_EINVAL before any launch: n < 1, n_systems < 1, an unknown sort, a NULL M, C, lam or info, n too large for the
+ * per-system vectors in shared memory, or less than one slab of workspace when one is needed.
+ */
+enum { RAFTK_EIG_SORT_DOF = 0, RAFTK_EIG_SORT_ASCENDING = 1 };
+enum { RAFTK_EIG_SMALL_DIAG = 1, RAFTK_EIG_NONPOSITIVE = 2, RAFTK_EIG_COMPLEX = 4, RAFTK_EIG_SINGULAR = 8, RAFTK_EIG_NOCONV = 16 };
+typedef struct raftk_eigen {
+    int32_t n_systems, n, sort, _pad0;
+    const double *M, *C;   /* [n_systems, n, n] row-major                                    */
+    double *lam;           /* complex [n_systems, n]: eigenvalues of M^-1 C in output order    */
+    double *modes;         /* complex [n_systems, n, n] (column j = mode j) or NULL            */
+    int32_t *info;         /* [n_systems] RAFTK_EIG_* flags                                    */
+} raftk_eigen;
+size_t raftk_eigen_workspace_bytes(const raftk_eigen *e);
+int raftk_eigen_dev(const raftk_eigen *e, void *workspace, size_t workspace_bytes, void *stream);
+int raftk_eigen_host(const raftk_eigen *e);
 
 /*
  * Response statistics of FOWT.saveTurbineOutputs (raft_fowt.py:2299-2353) as reductions over Xi:

@@ -107,6 +107,12 @@ class RaftkGeneralBatch(C.Structure):
                 ("node_offset", C.c_void_p), ("x_ref", C.c_void_p), ("y_ref", C.c_void_p), ("heading_adjust", C.c_void_p)]
 
 
+class RaftkEigen(C.Structure):
+    """include/raftk.h raftk_eigen: eigenvalues and right eigenvectors of M^-1 C for a batch of systems."""
+    _fields_ = [("n_systems", C.c_int32), ("n", C.c_int32), ("sort", C.c_int32), ("_pad0", C.c_int32),
+                ("M", C.c_void_p), ("C", C.c_void_p), ("lam", C.c_void_p), ("modes", C.c_void_p), ("info", C.c_void_p)]
+
+
 class RaftkSlender(C.Structure):
     _fields_ = ([("n_nodes", C.c_int32), ("n_members", C.c_int32), ("n_seg", C.c_int32), ("nw", C.c_int32),
                  ("depth", C.c_double), ("rho", C.c_double), ("g", C.c_double)] + [(n, C.c_void_p) for n in SLENDER_ARRAYS])
@@ -176,6 +182,7 @@ SYMBOLS = [
     "raftk_farm_response_dev", "raftk_solve_dynamics_farm_host", "raftk_farm_workspace_bytes", "raftk_farm_response_ws_dev",
     "raftk_farm_batch_workspace_bytes", "raftk_farm_batch_response_ws_dev", "raftk_solve_dynamics_farm_batch_host",
     "raftk_family_sizes", "raftk_build_family_host",
+    "raftk_eigen_workspace_bytes", "raftk_eigen_dev", "raftk_eigen_host",
 ]
 
 
@@ -315,6 +322,12 @@ def _load():
     lib.raftk_farm_batch_response_ws_dev.restype = C.c_int
     lib.raftk_solve_dynamics_farm_batch_host.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkSolveOpts), P(RaftkOutputs), P(RaftkFarmBatch)]
     lib.raftk_solve_dynamics_farm_batch_host.restype = C.c_int
+    lib.raftk_eigen_workspace_bytes.argtypes = [P(RaftkEigen)]
+    lib.raftk_eigen_workspace_bytes.restype = C.c_size_t
+    lib.raftk_eigen_dev.argtypes = [P(RaftkEigen), C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.raftk_eigen_dev.restype = C.c_int
+    lib.raftk_eigen_host.argtypes = [P(RaftkEigen)]
+    lib.raftk_eigen_host.restype = C.c_int
     lib.raftk_family_sizes.argtypes = [P(RaftkFamily), P(C.c_int32), P(C.c_int32)]
     lib.raftk_build_family_host.argtypes = [P(RaftkFamily), P(RaftkFamilyTables)]
     lib.raftk_family_sizes.restype = C.c_int

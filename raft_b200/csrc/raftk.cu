@@ -151,6 +151,7 @@ extern "C" int raftk_last_dispatch(raftk_dispatch *out)
 #include "raftk_slender.cuh"
 #include "raftk_general.cuh"
 #include "raftk_misc.cuh"
+#include "raftk_eigen.cuh"
 #include "raftk_builder.h"
 
 // ------------------------------------------------------------------------------------------------
@@ -2498,6 +2499,99 @@ extern "C" int raftk_general_channel_stats_host(int32_t n_units, int32_t n_dof, 
     S.out(dSd, rows, sd); S.out(dPsd, psd ? rows * nw : 0, psd); S.out(dAmp, amp ? rows * nw * 2 : 0, amp);
     int rc = S.commit();
     if (rc || (rc = launch_general_channel_stats(n_units, n_dof, n_ch, nw, dw, dW, dR, dWpow, dXi, dSd, dPsd, dAmp, nullptr))) return rc;
+    return S.finish();
+}
+
+// ---- natural frequencies and mode shapes (raftk_eigen_*) ------------------------------------------------------------------
+// Which kernel takes n, its dynamic shared memory, its workspace slab and how many of its CTAs an SM holds.  kernel 0: n too
+// large for the per-system vectors in shared memory.  Without a device the rule answers for an H100.
+struct EigPlan { int kernel = 0, per_sm = 0; size_t smem = 0, slab = 0; };
+static EigPlan eig_plan(int n)
+{
+    EigPlan p;
+    const size_t mat = (size_t)n * eig_ld(n) * sizeof(double);
+    if (n <= EIG_SMALL_NMAX) {
+        p.kernel = RAFTK_KERNEL_EIG_SMALL;
+        p.smem = EIG_SMALL_T * (3 * mat + eig_vec_doubles(n) * sizeof(double) + eig_vec_ints(n) * sizeof(int));
+        return p;
+    }
+    const size_t vec = ((size_t)eig_vec_doubles(n) + (eig_vec_ints(n) + 1) / 2) * sizeof(double), optin = smem_optin();
+    if (vec + mat <= optin) { p.kernel = RAFTK_KERNEL_EIG_CTA_SMEM; p.smem = vec + mat; p.slab = align_up(2 * mat, 256); }
+    else if (vec <= optin) { p.kernel = RAFTK_KERNEL_EIG_CTA_SLAB; p.smem = vec; p.slab = align_up(3 * mat, 256); }
+    else return p;
+    p.per_sm = (int)std::max<size_t>(1, std::min<size_t>(2048 / EIG_CTA_T, smem_per_sm() / (p.smem + 1024)));
+    return p;
+}
+static long long eig_ctas(const raftk_eigen *e, const EigPlan &p) { return std::min<long long>(e->n_systems, (long long)p.per_sm * sm_count()); }
+
+static int eig_check(const raftk_eigen *e)
+{
+    if (!e) return set_err(RAFTK_EINVAL, "eigen: null argument");
+    if (e->n < 1 || e->n_systems < 1) return set_err(RAFTK_EINVAL, "eigen: n and n_systems must be >= 1");
+    if (e->sort != RAFTK_EIG_SORT_DOF && e->sort != RAFTK_EIG_SORT_ASCENDING)
+        return set_err(RAFTK_EINVAL, "eigen: sort must be RAFTK_EIG_SORT_DOF or RAFTK_EIG_SORT_ASCENDING");
+    if (!e->M || !e->C || !e->lam || !e->info) return set_err(RAFTK_EINVAL, "eigen: M, C, lam and info are required");
+    if (!eig_plan(e->n).kernel) return set_err(RAFTK_EINVAL, "eigen: n too large for the per-system vectors in shared memory");
+    return RAFTK_OK;
+}
+
+extern "C" size_t raftk_eigen_workspace_bytes(const raftk_eigen *e)
+{
+    if (!e || e->n < 1 || e->n_systems < 1) return 0;
+    const EigPlan p = eig_plan(e->n);
+    if (p.kernel == 0 || p.kernel == RAFTK_KERNEL_EIG_SMALL) return 0;
+    return (size_t)eig_ctas(e, p) * p.slab;
+}
+
+extern "C" int raftk_eigen_dev(const raftk_eigen *e, void *workspace, size_t workspace_bytes, void *stream)
+{
+    disp_reset();
+    int rc = eig_check(e);
+    if (rc) return rc;
+    const EigPlan p = eig_plan(e->n);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (p.kernel == RAFTK_KERNEL_EIG_SMALL) {
+        static SmemOptIn opt(48 * 1024);
+        CUDA_TRY(opt.ensure(k_eig_small, p.smem));
+        k_eig_small<<<(e->n_systems + EIG_SMALL_T - 1) / EIG_SMALL_T, EIG_SMALL_T, p.smem, st>>>(*e);
+        g_launches++;
+        disp_launch(RAFTK_FAMILY_EIGEN, p.kernel, EIG_SMALL_T);
+        CUDA_TRY(cudaGetLastError());
+        return RAFTK_OK;
+    }
+    const long long slabs = workspace ? (long long)(workspace_bytes / p.slab) : 0;
+    if (slabs < 1) return set_err(RAFTK_EINVAL, "eigen: the workspace holds less than one slab (raftk_eigen_workspace_bytes)");
+    const int grid = (int)std::min<long long>(slabs, eig_ctas(e, p));
+    double *ws = static_cast<double *>(workspace);
+    const size_t slab_doubles = p.slab / sizeof(double);
+    if (p.kernel == RAFTK_KERNEL_EIG_CTA_SMEM) {
+        static SmemOptIn opt(48 * 1024);
+        CUDA_TRY(opt.ensure(k_eig_cta<true>, p.smem));
+        k_eig_cta<true><<<grid, EIG_CTA_T, p.smem, st>>>(*e, ws, slab_doubles);
+    } else {
+        static SmemOptIn opt(48 * 1024);
+        CUDA_TRY(opt.ensure(k_eig_cta<false>, p.smem));
+        k_eig_cta<false><<<grid, EIG_CTA_T, p.smem, st>>>(*e, ws, slab_doubles);
+    }
+    g_launches++;
+    disp_launch(RAFTK_FAMILY_EIGEN, p.kernel, EIG_CTA_T);
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_eigen_host(const raftk_eigen *e)
+{
+    disp_reset();
+    int rc = eig_check(e);
+    if (rc) return rc;
+    const size_t nS = e->n_systems, n = e->n, wb = raftk_eigen_workspace_bytes(e);
+    raftk_eigen d = *e;
+    char *ws;
+    Staging S("raftk_eigen_host");
+    S.in(d.M, e->M, nS * n * n); S.in(d.C, e->C, nS * n * n);
+    S.out(d.lam, nS * n * 2, e->lam); S.out(d.modes, e->modes ? nS * n * n * 2 : 0, e->modes); S.out(d.info, nS, e->info);
+    S.buf(ws, wb);
+    if ((rc = S.commit()) || (rc = raftk_eigen_dev(&d, ws, wb, nullptr))) return rc;
     return S.finish();
 }
 

@@ -39,6 +39,7 @@ class FOWT:
         self.nrotors = 0
         self.body, self.ms, self.moorMod = mpb, None, 0
         plat = design["platform"]
+        self.yawstiff = plat.get("yaw_stiffness", 0)                   # raft_fowt.py:377-380
         self.potModMaster = int(plat.get("potModMaster", 0))
         dlsMax = float(plat.get("dlsMax", 5.0))
         names = [m["name"] for m in plat["members"]]
@@ -120,6 +121,16 @@ class FOWT:
         if getattr(self, "_batch", None) is None:
             self._batch = solver.DesignBatch(self.pack())
         return self._batch
+
+    # raft_fowt.py:1646-1729 -------------------------------------------------------------------------------
+    def solveEigen(self, display=0, outPath=None):
+        """Natural frequencies [Hz] and mode shapes of the FOWT on the GPU -> (fns, modes), in the reference's order (the DOF
+        claim for 6 DOFs, ascending otherwise) and with its exceptions.  Writing ``outPath`` and the ``display`` table are not
+        provided."""
+        if outPath is not None:
+            raise NotImplementedError("solveEigen(outPath=...): writing the modes JSON is not provided")
+        E = packer.pack_eigen(self)
+        return solver.eigen_fns_modes(E["M"], E["C"], "dof" if self.nDOF == 6 else "ascending")
 
     # raft_fowt.py:1732-1888 -------------------------------------------------------------------------------
     def calcHydroExcitation(self, case, memberList=None):

@@ -113,6 +113,31 @@ class Model:
                 self.results["case_metrics"][ic][i] = m
         return self.results
 
+    # raft_model.py:436-547 -------------------------------------------------------------------------------------
+    def solveEigen(self, display=0, outPath=None):
+        """Natural frequencies [Hz] and mode shapes of the floating system on the GPU -> (fns, modes), stored in
+        results['eigen'].  The reference's assembly order: per FOWT M_struc + A_hydro_morison + A_BEM[:, :, 0] and
+        C_struc + C_hydro + C_moor + C_elast on its diagonal block, yawstiff on its DOF 5, then the array mooring stiffness
+        (``array_stiffness``, standing in for ms.getCoupledStiffnessA); its order of the modes (the DOF claim when every FOWT
+        has 6 DOFs) and its exceptions.  Writing ``outPath`` and the ``display`` table are not provided."""
+        if outPath is not None:
+            raise NotImplementedError("solveEigen(outPath=...): writing the modes JSON is not provided")
+        M_tot = np.zeros([self.nDOF, self.nDOF])
+        C_tot = np.zeros([self.nDOF, self.nDOF])
+        for i, fowt in enumerate(self.fowtList):
+            i1, i2 = i * fowt.nDOF, (i + 1) * fowt.nDOF
+            M_tot[i1:i2, i1:i2] += fowt.M_struc + fowt.A_hydro_morison + fowt.A_BEM[:, :, 0]
+            C_tot[i1:i2, i1:i2] += fowt.C_struc + fowt.C_hydro + fowt.C_moor + fowt.C_elast
+            C_tot[i1 + 5, i1 + 5] += fowt.yawstiff
+        rigid = all(f.nDOF == 6 for f in self.fowtList)
+        if self.C_array is not None:
+            if not rigid:
+                raise Exception('Currently, array-level mooring eigen analysis only supported for fully rigid FOWTs (6 DOFs).')
+            C_tot += self.C_array
+        fns, modes = solver.eigen_fns_modes(M_tot, C_tot, "dof" if rigid else "ascending")
+        self.results['eigen'] = {'frequencies': fns, 'modes': modes}
+        return fns, modes
+
     def _solve_batch(self, cases, tol):
         table, owner, first = packer.pack_case_trains(cases)
         ct = solver.CaseTable(table)

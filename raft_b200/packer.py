@@ -211,6 +211,28 @@ def pack_fowt(fowt, w=None, k=None):
     return out
 
 
+def pack_eigen(fowt):
+    """Mass and stiffness of FOWT.solveEigen (raft_fowt.py:1646-1660), duck-typed on a live FOWT, with the reference's own
+    summation order: M = M_struc + A_hydro_morison + A_BEM[:, :, 0] (the BEM added mass at the grid's first bin) and
+    C = fowt.getStiffness() when the object has it (which includes a MoorPy body's stiffness), else the same sum from the
+    attributes: C_moor, yawstiff on DOF 5, body.getStiffness() of an attached body, then C_struc + C_hydro + C_elast
+    (raft_fowt.py:1628-1644).  -> dict(M, C [nDOF,nDOF])."""
+    n = int(fowt.nDOF)
+    A_BEM = getattr(fowt, "A_BEM", None)
+    A0 = np.asarray(A_BEM)[:, :, 0] if A_BEM is not None and np.size(A_BEM) else np.zeros([n, n])
+    M = fowt.M_struc + fowt.A_hydro_morison + A0
+    if hasattr(fowt, "getStiffness"):
+        C = fowt.getStiffness()
+    else:
+        C = np.zeros([n, n])
+        C += fowt.C_moor
+        C[5, 5] += getattr(fowt, "yawstiff", 0.0)
+        if getattr(fowt, "body", None):
+            C += fowt.body.getStiffness()
+        C += fowt.C_struc + fowt.C_hydro + fowt.C_elast
+    return dict(M=np.array(M, dtype=float), C=np.array(C, dtype=float))
+
+
 def pack_general_dofs(fowt):
     """Node tables + the per-strip-node blocks of ``fowt.T`` for FOWTs with generalised degrees of freedom (flexible
     members, nDOF > 6; raft_fowt.py:1854-1857, 1913-1929).  GROUNDWORK for the next row: so far only the CPU checker

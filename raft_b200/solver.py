@@ -1318,6 +1318,18 @@ class GeneralBatchSession:
                                                              self.max_chunk_units, stream))
         return (self.Xi, self.status) if self.F_BEM is None else (self.Xi, self.status, self.F_BEM)
 
+    def eigen(self, A0=None, yawstiff=0.0, sort="ascending", modes=True):
+        """Natural frequencies and mode shapes of every design on the device, on torch's current stream (async):
+        raftk_eigen_dev on M + A0 and Cm + yawstiff e5 e5^T from the resident tables.  ``A0`` [6,6] or [nD,6,6]: the BEM added
+        mass at the grid's first bin (A_BEM[:6, :6, 0]; readHydro lumps it on the reduced DOFs 0-5), None for none;
+        ``yawstiff`` scalar or [nD].  -> dict(lam [nD,n], fns [nD,n] = sqrt(lam) / 2 pi, modes [nD,n,n] or None) complex,
+        info [nD] int32 (RAFTK_EIG_* flags), torch tensors; ``sort`` as ``solve_eigen``."""
+        nD, n = self.n_designs, self.n
+        with self.torch.cuda.device(self.device):
+            M, K = _eigen_inputs(self.keep["M"].view(nD, n, n), self.keep["C"].view(nD, n, n), A0, yawstiff, nD, n, self.device)
+            r = _eigen_dev(M, K, sort, modes, self.device, self.torch.cuda.current_stream(self.device).cuda_stream)
+        return dict(lam=r["lam"], fns=self.torch.sqrt(r["lam"]) / (2.0 * np.pi), modes=r["modes"], info=r["info"])
+
     def stats(self, R, wpow, psd=True, amp=False):
         """Output-channel statistics of the last ``solve()`` on the device, design by design (raftk_general_channel_stats_dev
         on each design's slice of Xi): R [nD,nch,nDOF], wpow [nch] -> (std [nD,nT,nch], PSD [nD,nT,nch,nw] or None, amplitudes
@@ -1421,6 +1433,125 @@ def system_solve(Z, F):
     info = np.zeros(nw, dtype=_I4)
     check(lib.raftk_system_solve_host(n, nw, nrhs, Z.ctypes.data, F.ctypes.data, info.ctypes.data))
     return (F[:, :, 0] if squeeze else F), info
+
+
+EIG_SMALL_DIAG, EIG_NONPOSITIVE, EIG_COMPLEX, EIG_SINGULAR, EIG_NOCONV = 1, 2, 4, 8, 16    # include/raftk.h RAFTK_EIG_*
+_EIG_SORT = {"dof": 0, "ascending": 1}
+
+
+def _eigen_struct(n_systems, n, sort, M=None, C_=None, lam=None, modes=None, info=None):
+    if sort not in _EIG_SORT:
+        raise ValueError("sort must be 'dof' or 'ascending', not %r" % (sort,))
+    e = _lib.RaftkEigen()
+    e.n_systems, e.n, e.sort = int(n_systems), int(n), _EIG_SORT[sort]
+    e.M, e.C, e.lam, e.modes, e.info = M, C_, lam, modes, info
+    return e
+
+
+def eigen_workspace_bytes(n_systems, n):
+    """Device workspace of the eigen analysis (raftk_eigen_workspace_bytes): 0 for n <= 12, else whole per-CTA slabs.
+    Answers for an H100 without a device."""
+    return int(lib.raftk_eigen_workspace_bytes(C.byref(_eigen_struct(n_systems, n, "dof"))))
+
+
+def eigen_outputs(lam, modes, info):
+    """numpy's conventions for the raw outputs: lam -> real dtype when every eigenvalue is real (NaN slots of systems without a
+    spectrum do not count), likewise modes; fns = sqrt(lam) / 2 pi as the reference writes it (NaN for a negative real)."""
+    real = bool(np.all((lam.imag == 0.0) | np.isnan(lam.imag)))
+    if real:
+        lam = np.ascontiguousarray(lam.real)
+        modes = None if modes is None else np.ascontiguousarray(modes.real)
+    with np.errstate(invalid="ignore"):
+        fns = np.sqrt(lam) / 2.0 / np.pi
+    return dict(lam=lam, fns=fns, modes=modes, info=info)
+
+
+def solve_eigen(M, C_, sort="dof", modes=True):
+    """Natural frequencies and mode shapes of systems M x'' + C x = 0 on the GPU (raftk_eigen_host): the eigenvalues and unit
+    2-norm right eigenvectors of M^-1 C, as np.linalg.eig(np.linalg.solve(M, C)) returns them, in the reference's order
+    (``sort='dof'``: raft_model.py:490-516; ``'ascending'``: np.argsort).  M, C [n,n] or [nS,n,n] ->
+    dict(lam [nS,n], fns [nS,n] Hz, modes [nS,n,n] (column j = mode j) or None, info [nS] RAFTK_EIG_* flags); real dtypes
+    when every eigenvalue is real.  ``eigen_raise`` turns the flags into the reference's exceptions."""
+    M = np.ascontiguousarray(M, dtype=_F8)
+    K = np.ascontiguousarray(C_, dtype=_F8)
+    squeeze = M.ndim == 2
+    if squeeze:
+        M, K = M[None], K[None]
+    if M.ndim != 3 or M.shape != K.shape or M.shape[1] != M.shape[2]:
+        raise ValueError("M and C must both be [n,n] or [n_systems,n,n]")
+    nS, n = M.shape[:2]
+    lam = np.zeros([nS, n], dtype=np.complex128)
+    V = np.zeros([nS, n, n], dtype=np.complex128) if modes else None
+    info = np.zeros(nS, dtype=_I4)
+    e = _eigen_struct(nS, n, sort, M.ctypes.data, K.ctypes.data, lam.ctypes.data, V.ctypes.data if modes else None, info.ctypes.data)
+    check(lib.raftk_eigen_host(C.byref(e)))
+    out = eigen_outputs(lam, V, info)
+    if squeeze:
+        out = {k: (None if v is None else v[0]) for k, v in out.items()}
+    return out
+
+
+def eigen_raise(M, C_, info, sort="dof"):
+    """The reference's exceptions for one system's flags, in its order (raft_model.py:478-500, raft_fowt.py:1667-1683):
+    RuntimeError naming the diagonals of M and C below 1; np.linalg.LinAlgError for a singular M (np.linalg.solve) or a QR
+    iteration that did not converge (np.linalg.eig); with ``sort='dof'`` RuntimeError on an eigenvalue <= 0."""
+    info = int(info)
+    if info & EIG_SMALL_DIAG:
+        msg = ""
+        for i in range(len(M)):
+            if M[i, i] < 1.0:
+                msg += f'Diagonal entry {i} of system mass matrix is less than 1 ({M[i, i]}). '
+            if C_[i, i] < 1.0:
+                msg += f'Diagonal entry {i} of system stiffness matrix is less than 1 ({C_[i, i]}). '
+        raise RuntimeError('System matrices computed by RAFT have one or more small or negative diagonals: ' + msg)
+    if info & EIG_SINGULAR:
+        raise np.linalg.LinAlgError("Singular matrix")
+    if info & EIG_NOCONV:
+        raise np.linalg.LinAlgError("Eigenvalues did not converge")
+    if sort == "dof" and info & EIG_NONPOSITIVE:
+        raise RuntimeError("Error: zero or negative system eigenvalues detected.")
+
+
+def eigen_fns_modes(M, C_, sort):
+    """One system as Model.solveEigen / FOWT.solveEigen return it: (fns, modes) or the reference's exception.  A DOF claim
+    that leaves rows unclaimed returns fewer modes, as the reference does."""
+    r = solve_eigen(M, C_, sort=sort)
+    eigen_raise(M, C_, r["info"], sort)
+    fns, modes = r["fns"], r["modes"]
+    keep = ~np.isnan(r["lam"].real)
+    return fns[keep], modes[:, keep]
+
+
+def _eigen_dev(M, K, sort, modes, device, stream):
+    """raftk_eigen_dev on device tensors M, K [nS,n,n] float64 -> dict(lam, modes, info) as torch tensors, raw (complex)."""
+    import torch
+    nS, n = int(M.shape[0]), int(M.shape[1])
+    M, K = M.contiguous(), K.contiguous()
+    lam = torch.empty([nS, n], dtype=torch.complex128, device=device)
+    V = torch.empty([nS, n, n], dtype=torch.complex128, device=device) if modes else None
+    info = torch.empty([nS], dtype=torch.int32, device=device)
+    wsb = eigen_workspace_bytes(nS, n)
+    ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=device)
+    e = _eigen_struct(nS, n, sort, M.data_ptr(), K.data_ptr(), lam.data_ptr(), V.data_ptr() if modes else None, info.data_ptr())
+    check(lib.raftk_eigen_dev(C.byref(e), ws.data_ptr(), wsb, stream))
+    return dict(lam=lam, modes=V, info=info)
+
+
+def _eigen_inputs(M, K, A0, yawstiff, nD, n, device):
+    """M + A0 on DOFs 0-5 (A0 [6,6] shared or [nD,6,6]) and K + yawstiff on DOF 5 (scalar or [nD]), as new tensors."""
+    import torch
+    M = M.clone()
+    K = K.clone()
+    if A0 is not None:
+        A = torch.as_tensor(np.asarray(A0, dtype=_F8), device=device)
+        if tuple(A.shape) not in ((6, 6), (nD, 6, 6)):
+            raise ValueError("A0 must be [6,6] or [%d,6,6]" % nD)
+        M[:, :6, :6] += A
+    y = torch.as_tensor(np.asarray(yawstiff, dtype=_F8), device=device)
+    if y.ndim not in (0, 1) or (y.ndim == 1 and y.shape[0] != nD):
+        raise ValueError("yawstiff must be a scalar or [%d]" % nD)
+    K[:, 5, 5] += y
+    return M, K
 
 
 _PINNED = []
@@ -1601,6 +1732,19 @@ class DeviceSession:
             check(launch(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f), ws.data_ptr(), wsb, self._stream()))
         return xi, info
 
+    def eigen(self, A0=None, yawstiff=0.0, sort="dof", modes=True):
+        """Natural frequencies and mode shapes of every design on the device, on torch's current stream (async):
+        raftk_eigen_dev on M0 + A0 and C0 + yawstiff e5 e5^T from the resident tables (FOWT.solveEigen, raft_fowt.py:1646-1729).
+        ``A0`` [6,6] or [nD,6,6]: the BEM added mass at the grid's first bin (A_BEM[:, :, 0]), None for none -- the resident
+        A_w cannot stand in for it, it also holds the aero added mass; ``yawstiff`` scalar or [nD].  -> dict(lam [nD,6],
+        fns [nD,6] = sqrt(lam) / 2 pi, modes [nD,6,6] or None) complex, info [nD] int32 (RAFTK_EIG_* flags), torch tensors;
+        ``sort`` as ``solve_eigen``."""
+        nD = self.batch.n_designs
+        with self.torch.cuda.device(self.device):
+            M, K = _eigen_inputs(self.dt["M0"].view(nD, 6, 6), self.dt["C0"].view(nD, 6, 6), A0, yawstiff, nD, 6, self.device)
+            r = _eigen_dev(M, K, sort, modes, self.device, self._stream())
+        return dict(lam=r["lam"], fns=self.torch.sqrt(r["lam"]) / (2.0 * np.pi), modes=r["modes"], info=r["info"])
+
     def second_order_force(self):
         """Enqueue FOWT.calcHydroForce_2ndOrd for all units -> out['F_2nd'], out['F_2nd_mean'] (async)."""
         with self.torch.cuda.device(self.device):
@@ -1627,10 +1771,10 @@ def launch_count():
     return int(lib.raftk_launch_count())
 
 
-DISPATCH_FAMILIES = ("none", "solve", "qtf", "general", "farm", "system")          # include/raftk.h RAFTK_FAMILY_*
+DISPATCH_FAMILIES = ("none", "solve", "qtf", "general", "farm", "system", "eigen")          # include/raftk.h RAFTK_FAMILY_*
 DISPATCH_KERNELS = ("none", "v1", "fused128", "fused256", "fused2-cluster", "fused2-grid", "qtf-tiles", "qtf-diag", "qtf-diag-mix",
                     "gen-blocked", "gen-unblocked", "farm-rows12", "farm-warp", "farm-block", "sys-unblocked", "sys-blocked",
-                    "farm-global", "sys-global")   # RAFTK_KERNEL_*
+                    "farm-global", "sys-global", "eig-small", "eig-cta-smem", "eig-cta-slab")   # RAFTK_KERNEL_*
 
 
 def last_dispatch():
