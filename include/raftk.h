@@ -693,6 +693,45 @@ int raftk_solve_dynamics_farm_batch_host(const raftk_designs *d, const raftk_cas
                                          const raftk_outputs *out, const raftk_farm_batch *f);
 
 /*
+ * Output channels of farm batches: mooring line tensions (the array level of Model.analyzeCases, raft_model.py:371-433, and
+ * a FOWT's own lines, raft_fowt.py:2355-2399, moorMod 0) and any other real linear functional of the coupled response,
+ *   Y[f,r,ch,w] = w^wpow[ch] sum_b R_f[ch,b] Xi_sys[f,r,b,w]
+ * -> std = sqrt(1/2 sum_w |Y|^2), PSD(w) = 1/2 |Y|^2 / dw, amp = Y, for n_farms farms x n_rows rows (cases or wave trains)
+ * x n_ch channels.  Tensions: R = dT/dx, the line-end tension Jacobian (MoorPy getCoupledStiffness(tensions=True)[1]).
+ * dw is a parameter because the reference's Tmoor_PSD divides by w[0], not by the bin width w[1] - w[0]; pass w[0] to match it.
+ * Every std, PSD and amplitude is bit-identical to raftk_general_channel_stats_* on the same R and Xi (same per-bin
+ * summation order, same reduction), and a farm's values do not depend on the batch it is in or on the tile width.
+ * Xi_sys complex [n_farms, n_rows, n_dof, nw] (raftk_farm_batch's output, n_dof = 6N); w [nw] (may be NULL when every wpow
+ * is 0).  std [n_farms, n_rows, n_ch]; psd [n_farms, n_rows, n_ch, nw] or NULL; amp complex [n_farms, n_rows, n_ch, nw] or NULL.
+ * Kernels: one CTA per (farm, row, bin tile) stages the tile of Xi_sys in shared memory and computes every channel from it
+ * (bins per tile from n_dof and the opt-in shared-memory limit; Xi_sys is read from L2 when not even one bin fits), then one
+ * CTA per (farm, row, channel) reduces over frequency.  |Y|^2 passes through psd, or through the workspace when psd is NULL:
+ * raftk_farm_channel_stats_workspace_bytes is 0 with psd, else n_farms * n_rows * n_ch * nw doubles.
+ * _dev: device R, Xi_sys, w and outputs, caller-owned workspace, enqueued on `stream` without synchronising.  _host: host
+ * pointers everywhere.  wpow is HOST memory in both, read during the call.
+ * RAFTK_EINVAL before any launch: a count below 1, more than RAFTK_FARM_CH_MAX channels, R_shared not 0 or 1, a wpow
+ * outside {0, 1, 2}, NULL R, Xi_sys or std, no w while a wpow is not 0, dw <= 0, or (_dev) a workspace that is too small.
+ */
+#define RAFTK_FARM_CH_MAX 4096
+#define RAFTK_FARM_TILE_L2 (-1)
+typedef struct raftk_farm_channels {
+    int32_t n_ch;
+    int32_t R_shared;        /* 1: R [n_ch, n_dof] for every farm; 0: R [n_farms, n_ch, n_dof]                     */
+    const double *R;
+    const int32_t *wpow;     /* HOST [n_ch] 0, 1 or 2 (displacement, velocity, acceleration), or NULL: all 0      */
+    double dw;               /* PSD divisor (> 0)                                                                  */
+    double *std, *psd, *amp;
+    int32_t tile_w;          /* 0: automatic; > 0: at most tile_w bins per CTA; RAFTK_FARM_TILE_L2: read Xi_sys from L2 */
+    int32_t _pad0;
+} raftk_farm_channels;
+
+size_t raftk_farm_channel_stats_workspace_bytes(int32_t n_farms, int32_t n_rows, int32_t nw, const raftk_farm_channels *ch);
+int raftk_farm_channel_stats_dev(int32_t n_farms, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi_sys,
+                                 const raftk_farm_channels *ch, void *workspace, size_t workspace_bytes, void *stream);
+int raftk_farm_channel_stats_host(int32_t n_farms, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi_sys,
+                                  const raftk_farm_channels *ch);
+
+/*
  * Natural frequencies and mode shapes (Model.solveEigen raft_model.py:436-547, FOWT.solveEigen raft_fowt.py:1646-1729): the
  * eigenvalues and right eigenvectors of M^-1 C for n_systems systems of n DOFs, what np.linalg.eig(np.linalg.solve(M, C))
  * returns, in the reference's output order.  Per system: LU of M with partial pivoting, A = M^-1 C, power-of-two balancing,

@@ -107,6 +107,12 @@ class RaftkGeneralBatch(C.Structure):
                 ("node_offset", C.c_void_p), ("x_ref", C.c_void_p), ("y_ref", C.c_void_p), ("heading_adjust", C.c_void_p)]
 
 
+class RaftkFarmChannels(C.Structure):
+    """include/raftk.h raftk_farm_channels: channels Y = w^wpow R_f Xi_sys of farm batches (mooring tensions) and their outputs."""
+    _fields_ = [("n_ch", C.c_int32), ("R_shared", C.c_int32), ("R", C.c_void_p), ("wpow", C.c_void_p), ("dw", C.c_double),
+                ("std", C.c_void_p), ("psd", C.c_void_p), ("amp", C.c_void_p), ("tile_w", C.c_int32), ("_pad0", C.c_int32)]
+
+
 class RaftkEigen(C.Structure):
     """include/raftk.h raftk_eigen: eigenvalues and right eigenvectors of M^-1 C for a batch of systems."""
     _fields_ = [("n_systems", C.c_int32), ("n", C.c_int32), ("sort", C.c_int32), ("_pad0", C.c_int32),
@@ -183,6 +189,7 @@ SYMBOLS = [
     "raftk_farm_batch_workspace_bytes", "raftk_farm_batch_response_ws_dev", "raftk_solve_dynamics_farm_batch_host",
     "raftk_family_sizes", "raftk_build_family_host",
     "raftk_eigen_workspace_bytes", "raftk_eigen_dev", "raftk_eigen_host",
+    "raftk_farm_channel_stats_workspace_bytes", "raftk_farm_channel_stats_dev", "raftk_farm_channel_stats_host",
 ]
 
 
@@ -328,6 +335,13 @@ def _load():
     lib.raftk_eigen_dev.restype = C.c_int
     lib.raftk_eigen_host.argtypes = [P(RaftkEigen)]
     lib.raftk_eigen_host.restype = C.c_int
+    lib.raftk_farm_channel_stats_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32, P(RaftkFarmChannels)]
+    lib.raftk_farm_channel_stats_workspace_bytes.restype = C.c_size_t
+    lib.raftk_farm_channel_stats_dev.argtypes = [C.c_int32] * 4 + [C.c_void_p, C.c_void_p, P(RaftkFarmChannels), C.c_void_p, C.c_size_t,
+                                                                   C.c_void_p]
+    lib.raftk_farm_channel_stats_dev.restype = C.c_int
+    lib.raftk_farm_channel_stats_host.argtypes = [C.c_int32] * 4 + [C.c_void_p, C.c_void_p, P(RaftkFarmChannels)]
+    lib.raftk_farm_channel_stats_host.restype = C.c_int
     lib.raftk_family_sizes.argtypes = [P(RaftkFamily), P(C.c_int32), P(C.c_int32)]
     lib.raftk_build_family_host.argtypes = [P(RaftkFamily), P(RaftkFamilyTables)]
     lib.raftk_family_sizes.restype = C.c_int

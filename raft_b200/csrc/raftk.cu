@@ -2502,6 +2502,108 @@ extern "C" int raftk_general_channel_stats_host(int32_t n_units, int32_t n_dof, 
     return S.finish();
 }
 
+// ---- channels of farm batches (raftk_farm_channel_stats_*) -----------------------------------------------------------------
+static size_t farm_ch_scratch(int32_t n_farms, int32_t n_rows, int32_t nw, const raftk_farm_channels *ch)
+{
+    return (size_t)n_farms * n_rows * ch->n_ch * nw * sizeof(double);
+}
+
+static int farm_ch_check(int32_t n_farms, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi_sys,
+                         const raftk_farm_channels *ch)
+{
+    if (!ch) return set_err(RAFTK_EINVAL, "farm channel-stats: null argument");
+    if (n_farms < 1 || n_rows < 1 || n_dof < 1 || nw < 1 || ch->n_ch < 1)
+        return set_err(RAFTK_EINVAL, "farm channel-stats: n_farms, n_rows, n_dof, nw and n_ch must be >= 1");
+    if (ch->n_ch > RAFTK_FARM_CH_MAX) return set_err_i(RAFTK_EINVAL, "farm channel-stats: at most %d channels per call", RAFTK_FARM_CH_MAX);
+    if (ch->R_shared != 0 && ch->R_shared != 1) return set_err(RAFTK_EINVAL, "farm channel-stats: R_shared must be 0 or 1");
+    if (!ch->R || !Xi_sys || !ch->std) return set_err(RAFTK_EINVAL, "farm channel-stats: R, Xi_sys and std are required");
+    if (!(ch->dw > 0.0)) return set_err(RAFTK_EINVAL, "farm channel-stats: dw must be > 0");
+    bool powers = false;
+    for (int32_t t = 0; ch->wpow && t < ch->n_ch; t++) {
+        if (ch->wpow[t] < 0 || ch->wpow[t] > 2) return set_err(RAFTK_EINVAL, "farm channel-stats: wpow must be 0, 1 or 2");
+        powers = powers || ch->wpow[t] != 0;
+    }
+    if (powers && !w) return set_err(RAFTK_EINVAL, "farm channel-stats: w is required when a channel has wpow 1 or 2");
+    const size_t units = (size_t)n_farms * n_rows;
+    if (units * nw > 2147483647u || units * ch->n_ch > 2147483647u)
+        return set_err(RAFTK_EINVAL, "farm channel-stats: too many (farm, row, bin) or (farm, row, channel) rows");
+    return RAFTK_OK;
+}
+
+// Bins per CTA: as many as the opt-in shared memory holds (n x 16 bytes each), fewer when the batch alone would leave SMs
+// idle; 0 when not even one bin fits (Xi_sys is then read from L2).  tile_w > 0 caps it; RAFTK_FARM_TILE_L2 forces L2.
+static int farm_ch_tile(int32_t n_units, int32_t n_dof, int32_t nw, int32_t tile_w)
+{
+    if (tile_w == RAFTK_FARM_TILE_L2) return 0;
+    const int tmax = (int)std::min<size_t>((size_t)nw, smem_optin() / ((size_t)n_dof * sizeof(double2)));
+    if (tmax < 1) return 0;
+    if (tile_w > 0) return std::min(tmax, (int)tile_w);
+    const long long want = (2LL * sm_count() + n_units - 1) / n_units;                      // tiles per (farm, row)
+    const int split = (int)std::max<long long>(32, (nw + want - 1) / want);
+    return std::min(tmax, split);
+}
+
+extern "C" size_t raftk_farm_channel_stats_workspace_bytes(int32_t n_farms, int32_t n_rows, int32_t nw, const raftk_farm_channels *ch)
+{
+    if (!ch || n_farms < 1 || n_rows < 1 || nw < 1 || ch->n_ch < 1 || ch->psd) return 0;
+    return farm_ch_scratch(n_farms, n_rows, nw, ch);
+}
+
+extern "C" int raftk_farm_channel_stats_dev(int32_t n_farms, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w,
+                                            const double *Xi_sys, const raftk_farm_channels *ch, void *workspace,
+                                            size_t workspace_bytes, void *stream)
+{
+    if (int rc = farm_ch_check(n_farms, n_rows, n_dof, nw, w, Xi_sys, ch)) return rc;
+    if (!ch->psd && (!workspace || workspace_bytes < farm_ch_scratch(n_farms, n_rows, nw, ch)))
+        return set_err(RAFTK_EINVAL, "farm channel-stats: without psd the workspace must hold |Y|^2 (raftk_farm_channel_stats_workspace_bytes)");
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int32_t units = n_farms * n_rows;
+    FarmChParams P = {};
+    P.n = n_dof; P.nch = ch->n_ch; P.nw = nw; P.n_rows = n_rows;
+    P.r_stride = ch->R_shared ? 0 : (size_t)ch->n_ch * n_dof;
+    P.w = w; P.R = ch->R; P.Xi = reinterpret_cast<const double2 *>(Xi_sys);
+    P.a2 = ch->psd ? ch->psd : static_cast<double *>(workspace);
+    P.amp = reinterpret_cast<double2 *>(ch->amp);
+    for (int32_t t = 0; ch->wpow && t < ch->n_ch; t++) P.wbits[t >> 4] |= (unsigned)ch->wpow[t] << ((t & 15) * 2);
+    const int tile = farm_ch_tile(units, n_dof, nw, ch->tile_w);
+    P.tile = tile ? tile : std::min<int32_t>(nw, 64);
+    P.n_tiles = (nw + P.tile - 1) / P.tile;
+    const long long grid = (long long)units * P.n_tiles;
+    if (grid > 2147483647LL) return set_err(RAFTK_EINVAL, "farm channel-stats: too many (farm, row, bin tile) blocks");
+    if (tile) {
+        const size_t smem = (size_t)n_dof * tile * sizeof(double2);
+        static SmemOptIn opt(48 * 1024);
+        CUDA_TRY(opt.ensure(k_farm_channels<true>, smem));
+        k_farm_channels<true><<<(unsigned)grid, FARM_CH_T, smem, st>>>(P);
+    } else {
+        k_farm_channels<false><<<(unsigned)grid, FARM_CH_T, 0, st>>>(P);
+    }
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    k_farm_channel_reduce<<<(unsigned)(units * ch->n_ch), 128, 0, st>>>(nw, ch->dw, P.a2, ch->std, ch->psd);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_farm_channel_stats_host(int32_t n_farms, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w,
+                                             const double *Xi_sys, const raftk_farm_channels *ch)
+{
+    if (int rc = farm_ch_check(n_farms, n_rows, n_dof, nw, w, Xi_sys, ch)) return rc;
+    const size_t units = (size_t)n_farms * n_rows, rows = units * ch->n_ch, nch = ch->n_ch;
+    const size_t wb = raftk_farm_channel_stats_workspace_bytes(n_farms, n_rows, nw, ch);
+    raftk_farm_channels d = *ch;
+    const double *dW, *dXi;
+    char *ws;
+    Staging S("raftk_farm_channel_stats_host");
+    S.in(dW, w, nw); S.in(d.R, ch->R, (ch->R_shared ? 1 : (size_t)n_farms) * nch * n_dof); S.in(dXi, Xi_sys, units * n_dof * nw * 2);
+    S.out(d.std, rows, ch->std); S.out(d.psd, ch->psd ? rows * nw : 0, ch->psd); S.out(d.amp, ch->amp ? rows * nw * 2 : 0, ch->amp);
+    S.buf(ws, wb);
+    int rc;
+    if ((rc = S.commit()) || (rc = raftk_farm_channel_stats_dev(n_farms, n_rows, n_dof, nw, dW, dXi, &d, ws, wb, nullptr))) return rc;
+    return S.finish();
+}
+
 // ---- natural frequencies and mode shapes (raftk_eigen_*) ------------------------------------------------------------------
 // Which kernel takes n, its dynamic shared memory, its workspace slab and how many of its CTAs an SM holds.  kernel 0: n too
 // large for the per-system vectors in shared memory.  Without a device the rule answers for an H100.

@@ -627,6 +627,95 @@ __global__ void __launch_bounds__(128) k_general_channel_stats(int n, int nch, i
 }
 
 // ------------------------------------------------------------------------------------------------
+// K5f: output channels of farm batches (raftk_farm_channel_stats_*): mooring tensions and any other real functional of the
+// coupled response, Y[f,r,ch,w] = w^wpow[ch] sum_b R_f[ch][b] Xi_sys[f][r][b][w] (raft_model.py:371-433 applies J_arr to
+// Xi_sys, raft_fowt.py:2355-2399 J_moor to a FOWT's PRP motions).  k_general_channel_stats re-reads a unit's whole Xi for
+// every channel; here one CTA per (farm, row, bin tile) stages the tile's n x tile bins of Xi_sys in shared memory once (or
+// reads them from L2 when not even one bin fits) and computes every channel from it.  Each Y is the fma chain over
+// b = 0..n-1 of k_general_channel_stats and |Y|^2 the same expression, so with k_farm_channel_reduce (that kernel's
+// thread-strided sum and block_rms_tail) every std, PSD and amplitude is bit-identical to k_general_channel_stats' on the
+// same R and Xi, whatever the tile width and the batch.
+// ------------------------------------------------------------------------------------------------
+#define FARM_CH_T 256
+#define FARM_CH_B 4             // channels per thread
+struct FarmChParams {
+    int n, nch, nw, n_rows, tile, n_tiles;
+    size_t r_stride;            // doubles between two farms' R; 0: one R for every farm
+    const double *w, *R;
+    const double2 *Xi;          // [F, n_rows, n, nw]
+    double *a2;                 // |Y|^2 [F, n_rows, nch, nw]: the psd output or the workspace
+    double2 *amp;               // [F, n_rows, nch, nw] or NULL
+    unsigned wbits[RAFTK_FARM_CH_MAX / 16];
+};
+
+template <bool SMEM>
+__global__ void __launch_bounds__(FARM_CH_T) k_farm_channels(const __grid_constant__ FarmChParams P)
+{
+    extern __shared__ double2 xs[];                     // [n][tw] when SMEM
+    const int tid = threadIdx.x;
+    const int t = (int)(blockIdx.x % (unsigned)P.n_tiles);
+    const size_t fr = blockIdx.x / (unsigned)P.n_tiles;    // farm * n_rows + row
+    const int f = (int)(fr / (size_t)P.n_rows);
+    const int i0 = t * P.tile, tw = min(P.tile, P.nw - i0);
+    const double2 *x = P.Xi + fr * (size_t)P.n * P.nw + i0;
+    if (SMEM) {
+        for (int k = tid; k < P.n * tw; k += FARM_CH_T) {
+            const int b = k / tw, i = k - b * tw;
+            xs[k] = x[(size_t)b * P.nw + i];
+        }
+        __syncthreads();
+    }
+    // a thread computes FARM_CH_B channels of one bin: each Xi value read feeds FARM_CH_B independent chains (every chain
+    // still runs over b = 0..n-1 in order); a warp's threads share their channels, so the R loads are broadcasts
+    const double *Rf = P.R + (size_t)f * P.r_stride;
+    const int nchb = (P.nch + FARM_CH_B - 1) / FARM_CH_B;
+    for (int k = tid; k < nchb * tw; k += FARM_CH_T) {
+        const int c0 = (k / tw) * FARM_CH_B, i = k - (k / tw) * tw;
+        const double *r[FARM_CH_B];
+        double yr[FARM_CH_B], yi[FARM_CH_B];
+#pragma unroll
+        for (int j = 0; j < FARM_CH_B; j++) { r[j] = Rf + (size_t)min(c0 + j, P.nch - 1) * P.n; yr[j] = 0.0; yi[j] = 0.0; }
+        for (int b = 0; b < P.n; b++) {
+            const double2 v = SMEM ? xs[b * tw + i] : x[(size_t)b * P.nw + i];
+#pragma unroll
+            for (int j = 0; j < FARM_CH_B; j++) {
+                const double c = r[j][b];
+                yr[j] = fma(c, v.x, yr[j]); yi[j] = fma(c, v.y, yi[j]);
+            }
+        }
+        const int iw = i0 + i;
+#pragma unroll
+        for (int j = 0; j < FARM_CH_B; j++) {
+            const int ch = c0 + j;
+            if (ch >= P.nch) break;
+            double re = yr[j], im = yi[j];
+            const int p = (P.wbits[ch >> 4] >> ((ch & 15) * 2)) & 3;
+            if (p == 2) { const double w2 = P.w[iw] * P.w[iw]; re *= w2; im *= w2; }
+            else if (p == 1) { const double w1 = P.w[iw]; re *= w1; im *= w1; }
+            const size_t o = (fr * P.nch + ch) * P.nw + iw;
+            P.a2[o] = re * re + im * im;
+            if (P.amp) P.amp[o] = make_double2(re, im);
+        }
+    }
+}
+
+// std = sqrt(1/2 sum_w |Y|^2) and PSD = 1/2 |Y|^2 / dw per (farm, row, channel): one 128-thread CTA per row, summing a2 in
+// k_general_channel_stats' thread-strided order.  psd may be a2 itself (each thread rewrites the bins it read).
+__global__ void __launch_bounds__(128) k_farm_channel_reduce(int nw, double dw, const double *a2, double *sd, double *psd)
+{
+    __shared__ double part[4];
+    const size_t row = blockIdx.x;
+    const int tid = threadIdx.x;
+    double s = 0.0;
+    for (int i = tid; i < nw; i += 128) {
+        const double v = a2[row * nw + i];
+        s += v;
+        if (psd) psd[row * nw + i] = 0.5 * v / dw;
+    }
+    block_rms_tail(s, part, tid, sd + row);
+}
+
+// ------------------------------------------------------------------------------------------------
 // FP64 FMA peak micro-kernel
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) k_fp64_peak(double *out, int iters)

@@ -13,9 +13,14 @@ from .fowt import FOWT
 
 
 class Model:
-    def __init__(self, design, matrices=None, array_stiffness=None, channels=None):
+    def __init__(self, design, matrices=None, array_stiffness=None, channels=None, tension_jacobian=None, mean_tensions=None,
+                 array_tension_jacobian=None, array_mean_tensions=None):
         """``channels``: optional turbine output channels per FOWT (``packer.pack_turbine_channels`` dicts: nacelle
-        accelerations, tower-base moment) -- the turbine itself is outside this path, its constants enter here."""
+        accelerations, tower-base moment) -- the turbine itself is outside this path, its constants enter here.
+        ``tension_jacobian`` [2L,6] / ``mean_tensions`` [2L] (one for every FOWT, or a list with None for a FOWT without its
+        own lines) and ``array_tension_jacobian`` [2L,6N] / ``array_mean_tensions`` [2L]: the mooring line-end tensions of
+        moorMod 0, standing in for fowt.ms / model.ms (MoorPy getCoupledStiffness(tensions=True)[1] and getTensions(), see
+        ``packer.pack_mooring_tensions``) as ``array_stiffness`` stands in for getCoupledStiffnessA."""
         s = design.setdefault("settings", {})
         min_freq, max_freq = float(s.get("min_freq", 0.01)), float(s.get("max_freq", 1.00))
         self.XiStart = float(s.get("XiStart", 0.1))
@@ -44,6 +49,16 @@ class Model:
         self.C_array = None if array_stiffness is None else np.array(array_stiffness, dtype=float)   # stands in for ms.getCoupledStiffnessA
         self.results = {}
         self.channels = list(channels) if isinstance(channels, (list, tuple)) else [channels] * self.nFOWT
+        per = lambda v: list(v) if isinstance(v, (list, tuple)) else [v] * self.nFOWT
+        self.tensions = [None if J is None else packer.pack_mooring_tensions(dict(J=J, T0=T0))
+                         for J, T0 in zip(per(tension_jacobian), per(mean_tensions))]
+        self.array_tensions = (None if array_tension_jacobian is None else
+                               packer.pack_mooring_tensions(dict(J=array_tension_jacobian, T0=array_mean_tensions)))
+        for t in self.tensions:
+            if t is not None and t["J"].shape[1] != 6:
+                raise ValueError("tension_jacobian must be [2L, 6]")
+        if self.array_tensions is not None and self.array_tensions["J"].shape[1] != self.nDOF:
+            raise ValueError("array_tension_jacobian must be [2L, %d]" % self.nDOF)
         for f in self.fowtList:
             f.calcHydroConstants()
 
@@ -66,7 +81,10 @@ class Model:
         """All load cases in ONE batched GPU call.  Positional arguments as the reference's
         ``analyzeCases(display=0, meshDir=..., RAO_plot=False)`` (raft_model.py:264; meshDir / RAO_plot concern the BEM mesh
         and plotting, outside this path and ignored); ``cases=``: list of case dicts (default: the design's table).
-        Fills results['freq_rad'], results['Xi'] [nCases, nDOF, nw], results['status'] [nCases, nFOWT, 4]."""
+        Fills results['freq_rad'], results['Xi'] [nCases, nDOF, nw], results['status'] [nCases, nFOWT, 4], and per case and
+        FOWT the saveTurbineOutputs statistics: PRP motions, turbine channels, wave_PSD and, with tension Jacobians, Tmoor_* of
+        the FOWT's lines and case_metrics[iCase]['array_mooring'] of the array's (raft_fowt.py:2355-2399, raft_model.py:371-433;
+        max / min = avg +- 3 std, Tmoor_PSD divided by w[0] as the reference does)."""
         if cases is None:
             keys = self.design["cases"]["keys"]
             cases = [dict(zip(keys, row)) for row in self.design["cases"]["data"]]
@@ -85,6 +103,13 @@ class Model:
         names = ("surge", "sway", "heave", "roll", "pitch", "yaw")
         ch_stats = [None if ch is None else solver.channel_stats(ch["coef"], Xi_units[:, i], self.w[1] - self.w[0])
                     for i, ch in enumerate(self.channels)]                                     # (std [nT,nch], PSD [nT,nch,nw], -)
+        # line-end tensions T = J Xi (moorMod 0): a FOWT's lines on its PRP motions through channel_stats (J constant over w),
+        # the array's lines on the coupled response through farm_channel_stats; PSDs divided by w[0] (raft_fowt.py:2370, 2399)
+        w0 = float(self.w[0])
+        ten = [None if t is None else solver.channel_stats(np.repeat(t["J"][:, :, None], self.nw, axis=2) + 0j, Xi_units[:, i], w0)
+               for i, t in enumerate(self.tensions)]
+        arr = None if self.array_tensions is None else solver.farm_channel_stats(self.array_tensions["J"], out["Xi_all"], w0)
+        dw = self.w[1] - self.w[0]
         self.results["case_metrics"] = {}
         for ic in range(nC):
             idx = np.nonzero(owner == ic)[0]
@@ -110,7 +135,13 @@ class Model:
                         m[nm + "_avg"][ir], m[nm + "_std"][ir] = ch["avg"][k_], sd_c[k_]
                         m[nm + "_max"][ir], m[nm + "_min"][ir] = ch["avg"][k_] + 3 * sd_c[k_], ch["avg"][k_] - 3 * sd_c[k_]
                         m[nm + "_PSD"][:, ir] = psd_c[k_]
+                if ten[i] is not None:
+                    m.update(solver.tension_metrics(self.tensions[i]["T0"], *solver.combine_trains(ten[i][0], ten[i][1], idx)))
+                m["wave_PSD"] = (0.5 * np.abs(out["zeta"][idx]) ** 2 / dw).sum(axis=0)          # getPSD(zeta, dw) (:2608)
                 self.results["case_metrics"][ic][i] = m
+            if arr is not None:
+                self.results["case_metrics"][ic]["array_mooring"] = solver.tension_metrics(self.array_tensions["T0"],
+                                                                                           *solver.combine_trains(arr[0], arr[1], idx))
         return self.results
 
     # raft_model.py:436-547 -------------------------------------------------------------------------------------
@@ -189,7 +220,7 @@ class Model:
             # (slender-body QTF path) coupled system: Z_sys = blockdiag(Z_i) + C_array; F = Z_i Xi_i  (raft_model.py:1164-1216)
             Xi_all = self._couple(o, nT)
         Xi_trains = [Xi_all[owner == ic] for ic in range(nC)]
-        return dict(Xi=Xi_all[first], Xi_trains=Xi_trains, status=np.moveaxis(st, 0, 1), Xi_all=Xi_all, owner=owner)
+        return dict(Xi=Xi_all[first], Xi_trains=Xi_trains, status=np.moveaxis(st, 0, 1), Xi_all=Xi_all, owner=owner, zeta=o["zeta"])
 
     def _couple(self, o, nC):
         n, nw, w = self.nDOF, self.nw, self.w

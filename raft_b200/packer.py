@@ -480,7 +480,7 @@ def pack_turbine_channels(fowt):
     return dict(names=names, coef=np.array(coef), avg=np.array(avg, dtype=float))
 
 
-def pack_general_channels(fowt):
+def pack_general_channels(fowt, tensions=None):
     """Output channels of ``FOWT.saveTurbineOutputs`` for a FOWT with generalised degrees of freedom, as real linear
     functionals of the reduced response: Y_ch(w) = w^wpow[ch] sum_b R[ch,b] Xi[b,w]  (``solver.general_channel_stats``,
     C ABI ``raftk_general_channel_stats_*``).  Duck-typed on a live FOWT:
@@ -495,7 +495,10 @@ def pack_general_channels(fowt):
     and 2), avg [nch]).  ``avg`` holds the
     reference's mean values (Xi0_PRP from r6, the hub node's r, the tower nodes' Xi0); 0 where those inputs are absent.
     A rigid tower's Mbase (:2508-2538) mixes w^0 and w^2 terms with the aero matrices and is not a channel of this form:
-    NotImplementedError."""
+    NotImplementedError.
+    ``tensions``: the FOWT's mooring (``pack_mooring_tensions`` result, a MoorPy system or {J, T0}, J [2L, 6] on the PRP
+    motions) adds rows ("Tmoor", line end k) = J[k] @ R_PRP with R_PRP in radians (:2355-2399), and
+    ``tension`` = dict(row0, T0, w0) so that ``solver.general_case_metrics`` reports them as the reference's Tmoor_* arrays."""
     T = np.asarray(fowt.T, dtype=float)
     g = float(fowt.g)
     names, R, wpow, avg = [], [], [], []
@@ -532,8 +535,46 @@ def pack_general_channels(fowt):
         F0 = (-Kf @ X0)[base]
         for a, nm in enumerate(("FbaseX", "FbaseY", "FbaseZ", "MbaseX", "MbaseY", "MbaseZ")):
             add(nm, ir, Rb[a], 0, F0[a])
-    return dict(names=names, R=np.array(R).reshape(len(names), T.shape[1]), wpow=np.array(wpow, dtype=np.int32),
-                avg=np.array(avg, dtype=float))
+    out = dict(names=names, R=np.array(R).reshape(len(names), T.shape[1]), wpow=np.array(wpow, dtype=np.int32),
+               avg=np.array(avg, dtype=float))
+    if tensions is not None:
+        # mooring line-end tensions J @ Xi_PRP (:2355-2399, moorMod 0): PRP motions in metres and RADIANS -- the roll / pitch /
+        # yaw rows above carry rad2deg and cannot be reused
+        ten = tensions if isinstance(tensions, dict) and "n_lines" in tensions else pack_mooring_tensions(tensions)
+        if ten["J"].shape[1] != 6:
+            raise ValueError("the tension Jacobian of a FOWT must be [2L, 6] (its PRP motions)")
+        R_prp = np.vstack([Trb[:3] + S @ Trb[3:], Trb[3:]])
+        row0 = len(names)
+        for k in range(len(ten["T0"])):
+            add("Tmoor", k, ten["J"][k] @ R_prp, 0, ten["T0"][k])
+        out.update(R=np.array(R).reshape(len(names), T.shape[1]), wpow=np.array(wpow, dtype=np.int32), avg=np.array(avg, dtype=float),
+                   tension=dict(row0=row0, T0=ten["T0"].copy(), w0=float(np.asarray(fowt.w, dtype=float)[0])))
+    return out
+
+
+def pack_mooring_tensions(ms, moorMod=0):
+    """Line-end tensions of a mooring system as linear functionals of the motions of its coupled bodies (moorMod 0,
+    raft_fowt.py:2362-2367, raft_model.py:379-386): T_amp = J @ Xi.  Duck-typed on a MoorPy system as the reference holds it
+    after lines2ss: J = ms.getCoupledStiffness(lines_only=True, tensions=True)[1] [2L, 6 * bodies], the mean tensions
+    T0 = ms.getTensions() [2L], L = len(ms.lineList) (line ends A then B).  A plain dict {J, T0} stands in for the system.
+    moorMod 1 / 2 take the tensions from MoorPy's dynamicSolve of every line (:2373-2386): NotImplementedError.
+    -> dict(J [2L, nDOF], T0 [2L], n_lines L)."""
+    if int(moorMod) != 0:
+        raise NotImplementedError("mooring tensions for moorMod %d (MoorPy dynamicSolve per line) are not provided; moorMod 0 only"
+                                  % int(moorMod))
+    if isinstance(ms, dict):
+        J, T0 = ms["J"], ms["T0"]
+        n_lines = None
+    else:
+        J = ms.getCoupledStiffness(lines_only=True, tensions=True)[1]
+        T0 = ms.getTensions()
+        n_lines = len(ms.lineList)
+    J, T0 = np.array(J, dtype=float), np.array(T0, dtype=float).reshape(-1)
+    if J.ndim != 2 or J.shape[0] % 2 or T0.shape != (J.shape[0],):
+        raise ValueError("the tension Jacobian must be [2L, nDOF] and the mean tensions [2L]")
+    if n_lines is not None and 2 * n_lines != J.shape[0]:
+        raise ValueError("the tension Jacobian has %d rows for %d lines" % (J.shape[0], n_lines))
+    return dict(J=J, T0=T0, n_lines=J.shape[0] // 2)
 
 
 SPECTRUM_IDS = {"JONSWAP": 0, "unit": 1, "constant": 2, "none": 3, "still": 3}

@@ -993,17 +993,89 @@ def general_channel_stats(R, wpow, w, Xi, dw, psd=True, amp=False):
     return sd, P, A
 
 
-def general_case_metrics(channels, std, psd, amp, idx):
+def _farm_channels_struct(R, wpow, n_farms, n, dw, tile_w):
+    """R [nch,n] (every farm) or [F,nch,n] and wpow -> (raftk_farm_channels without pointers to outputs, R, wpow) checked."""
+    R = np.ascontiguousarray(R, dtype=_F8)
+    if R.ndim == 2:
+        R_shared = 1
+    elif R.ndim == 3 and R.shape[0] == n_farms:
+        R_shared = 0
+    else:
+        raise ValueError("R must be [nch, %d] or [%d, nch, %d]" % (n, n_farms, n))
+    nch = R.shape[-2]
+    if R.shape[-1] != n:
+        raise ValueError("R must be [nch, %d] or [%d, nch, %d]" % (n, n_farms, n))
+    wpow = np.zeros(nch, dtype=_I4) if wpow is None else np.ascontiguousarray(wpow, dtype=_I4)
+    if wpow.shape != (nch,):
+        raise ValueError("wpow must be [nch]")
+    _check_wpow(wpow)
+    if not dw > 0:
+        raise ValueError("dw must be > 0")
+    ch = _lib.RaftkFarmChannels()
+    ch.n_ch, ch.R_shared, ch.wpow, ch.dw, ch.tile_w = nch, R_shared, wpow.ctypes.data, float(dw), int(tile_w)
+    return ch, R, wpow
+
+
+def farm_channel_stats(R, Xi_sys, dw, w=None, wpow=None, psd=True, amp=False, tile_w=0):
+    """Channels of farm batches on the device (raftk_farm_channel_stats_host), host buffers: Y[f,r,ch] = w^wpow R_f Xi_sys[f,r]
+    -- mooring tensions with R = the line-end tension Jacobian dT/dx (raft_model.py:371-433, raft_fowt.py:2355-2399).
+    ``R`` [nch,6N] for every farm or [F,nch,6N]; ``Xi_sys`` complex [F,nR,6N,nw] (``solve_dynamics_farm_batch``; [nR,6N,nw]
+    for one farm); ``dw`` the PSD divisor (the reference's Tmoor_PSD uses w[0]); ``w`` [nw], needed when a ``wpow`` is 1 or 2.
+    -> (std [F,nR,nch], PSD [F,nR,nch,nw] or None, amplitudes complex [F,nR,nch,nw] or None), without the farm axis when
+    ``Xi_sys`` had none.  Bit-identical to ``general_channel_stats`` on the same R and Xi.  Several wave trains of a case:
+    ``combine_trains``.  ``tile_w``: bins per CTA (0 automatic; -1 reads Xi_sys from L2), the results do not depend on it."""
+    Xi_sys = np.ascontiguousarray(Xi_sys, dtype=np.complex128)
+    squeeze = Xi_sys.ndim == 3
+    if squeeze:
+        Xi_sys = Xi_sys[None]
+    if Xi_sys.ndim != 4:
+        raise ValueError("Xi_sys must be [F, nR, n, nw] or [nR, n, nw]")
+    F, nR, n, nw = Xi_sys.shape
+    ch, R, wpow = _farm_channels_struct(R, wpow, F, n, dw, tile_w)
+    w = None if w is None else np.ascontiguousarray(w, dtype=_F8)
+    if w is not None and w.shape != (nw,):
+        raise ValueError("w must be [nw]")
+    nch = ch.n_ch
+    sd = np.zeros([F, nR, nch])
+    P = np.zeros([F, nR, nch, nw]) if psd else None
+    A = np.zeros([F, nR, nch, nw], dtype=np.complex128) if amp else None
+    ch.R, ch.std = R.ctypes.data, sd.ctypes.data
+    ch.psd, ch.amp = (P.ctypes.data if psd else None), (A.ctypes.data if amp else None)
+    check(lib.raftk_farm_channel_stats_host(F, nR, n, nw, None if w is None else w.ctypes.data, Xi_sys.ctypes.data, C.byref(ch)))
+    if squeeze:
+        sd, P, A = sd[0], (P[0] if psd else None), (A[0] if amp else None)
+    return sd, P, A
+
+
+def tension_metrics(T0, std, psd):
+    """Model.analyzeCases' Tmoor entries (raft_fowt.py:2389-2399, raft_model.py:406-418) from the mean tensions T0 [2L] and one
+    case's combined statistics std [2L], PSD [2L,nw]: avg, std, max / min = avg +- 3 std, PSD."""
+    T0 = np.asarray(T0, dtype=float)
+    return dict(Tmoor_avg=T0.copy(), Tmoor_std=np.array(std, dtype=float), Tmoor_max=T0 + 3 * std, Tmoor_min=T0 - 3 * std,
+                Tmoor_PSD=np.array(psd, dtype=float))
+
+
+def general_case_metrics(channels, std, psd, amp, idx, dw=None):
     """The entries FOWT.saveTurbineOutputs stores for one case (raft_fowt.py:2299-2604) from per-train channel statistics
     (std [nT,nch], PSD [nT,nch,nw], amplitudes [nT,nch,nw]) of the case's trains ``idx``: ``*_avg/_std/_max/_min/_PSD`` of every
     channel, ``*_RA`` of the six PRP motions (all trains plus the zero row of Model.Xi), per-rotor channels as arrays
-    [nrotors] / PSD [nw, nrotors], and the ``Mbase`` alias of a flexible tower's MbaseY (:2599-2604)."""
+    [nrotors] / PSD [nw, nrotors], and the ``Mbase`` alias of a flexible tower's MbaseY (:2599-2604).  Mooring tension rows
+    (``channels['tension']``) give Tmoor_avg/std/max/min [2L] and Tmoor_PSD [2L,nw], whose PSD divides by w[0] like the
+    reference's (:2370, :2399): ``dw``, the divisor of ``psd``, is then required."""
     sd, ps = combine_trains(std, psd, idx)
     names, avg = channels["names"], channels["avg"]
     nw = psd.shape[-1]
-    nrot = 1 + max([ir for _, ir in names if ir is not None], default=-1)
+    ten = channels.get("tension")
+    nrot = 1 + max([ir for nm, ir in names if ir is not None and nm != "Tmoor"], default=-1)
     m = {}
+    if ten is not None:
+        if dw is None:
+            raise ValueError("general_case_metrics: tension rows need dw, the PSD divisor of psd")
+        rows = slice(ten["row0"], ten["row0"] + len(ten["T0"]))
+        m.update(tension_metrics(ten["T0"], sd[rows], ps[rows] * (float(dw) / ten["w0"])))
     for k, (nm, ir) in enumerate(names):
+        if nm == "Tmoor":
+            continue
         if ir is None:
             m[nm + "_avg"], m[nm + "_std"] = avg[k], sd[k]
             m[nm + "_max"], m[nm + "_min"] = avg[k] + 3 * sd[k], avg[k] - 3 * sd[k]
@@ -1028,7 +1100,7 @@ def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01
     """Model.analyzeCases (dynamics and output statistics) for one FOWT with generalised degrees of freedom: ``cases`` a list
     of case dicts, scalar or list-valued wave keys (several wave trains); ``channels`` from ``packer.pack_general_channels``.
     -> dict(Xi_trains [per case: nTrains,nDOF,nw], status [nC,4] of train 0, case_metrics {case: saveTurbineOutputs entries},
-    empty without channels).  ``fd``: frequency-dependent terms, as for ``general_solve_dynamics``.  ``qtf``: second-order
+    empty without channels; with ``pack_general_channels(fowt, tensions=...)`` they include Tmoor_*).  ``fd``: frequency-dependent terms, as for ``general_solve_dynamics``.  ``qtf``: second-order
     wave loads (``packer.pack_general_qtf``); the result then also holds, per case, the reference FOWT's ``Fhydro_2nd``
     (complex [nTrains,nDOF,nw]) and ``Fhydro_2nd_mean`` ([nTrains,nDOF]), zero from reduced DOF 6 up (raft_model.py:1034-1036)."""
     from .packer import pack_case_trains
@@ -1046,7 +1118,7 @@ def _general_case_results(P, Xi, st, owner, first, n_cases, channels, F2nd):
     if channels is not None:
         sd, ps, amp = general_channel_stats(channels["R"], channels["wpow"], P["w"], Xi, float(P["dw"]), psd=True, amp=True)
         for ic in range(n_cases):
-            metrics[ic] = general_case_metrics(channels, sd, ps, amp, np.nonzero(owner == ic)[0])
+            metrics[ic] = general_case_metrics(channels, sd, ps, amp, np.nonzero(owner == ic)[0], dw=float(P["dw"]))
     out = dict(Xi_trains=[Xi[owner == ic] for ic in range(n_cases)], status=st[first], case_metrics=metrics)
     if F2nd is not None:
         n, nw = Xi.shape[1], Xi.shape[2]
@@ -1731,6 +1803,36 @@ class DeviceSession:
         with torch.cuda.device(self.device):
             check(launch(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f), ws.data_ptr(), wsb, self._stream()))
         return xi, info
+
+    def farm_channel_stats(self, R, dw, wpow=None, psd=True, amp=False, n_fowt=None, tile_w=0):
+        """Enqueue channel statistics of the LAST ``farm_response`` on the resident Xi_sys (raftk_farm_channel_stats_dev; no
+        host round trip): mooring tensions with R the tension Jacobian.  ``n_fowt`` names the form of ``farm_response`` that
+        ran (None: one farm).  ``R``, ``dw``, ``wpow``, ``tile_w`` as ``farm_channel_stats``.  -> torch tensors (std [F,nC,nch],
+        PSD [F,nC,nch,nw] or None, amplitudes complex [F,nC,nch,nw] or None), without the farm axis for ``n_fowt=None``."""
+        torch = self.torch
+        key = "_farm" if n_fowt is None else "_farm_batch"
+        if not hasattr(self, key):
+            raise RuntimeError("farm_channel_stats: call farm_response(n_fowt=%r) first" % (n_fowt,))
+        xi = getattr(self, key)[2]
+        lead = list(xi.shape[:-2]) if n_fowt is not None else [1, xi.shape[0]]
+        F, nR, n, nw = lead[0], lead[1], xi.shape[-2], xi.shape[-1]
+        ch, R, wpow = _farm_channels_struct(R, wpow, F, n, dw, tile_w)
+        nch = ch.n_ch
+        with torch.cuda.device(self.device):
+            dR = torch.from_numpy(R).to(self.device)
+            sd = torch.zeros([F, nR, nch], dtype=torch.float64, device=self.device)
+            P = torch.zeros([F, nR, nch, nw], dtype=torch.float64, device=self.device) if psd else None
+            A = torch.zeros([F, nR, nch, nw], dtype=torch.complex128, device=self.device) if amp else None
+            ch.R, ch.std = dR.data_ptr(), sd.data_ptr()
+            ch.psd, ch.amp = (P.data_ptr() if psd else None), (A.data_ptr() if amp else None)
+            wsb = int(lib.raftk_farm_channel_stats_workspace_bytes(F, nR, nw, C.byref(ch)))
+            ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=self.device)
+            check(lib.raftk_farm_channel_stats_dev(F, nR, n, nw, self.dt["w"].data_ptr(), xi.data_ptr(), C.byref(ch), ws.data_ptr(), wsb,
+                                                   self._stream()))
+            self._farm_ch_keep = (dR, ws)             # the launch reads them after this call returns
+        if n_fowt is None:
+            sd, P, A = sd[0], (P[0] if psd else None), (A[0] if amp else None)
+        return sd, P, A
 
     def eigen(self, A0=None, yawstiff=0.0, sort="dof", modes=True):
         """Natural frequencies and mode shapes of every design on the device, on torch's current stream (async):
