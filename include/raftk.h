@@ -732,6 +732,48 @@ int raftk_farm_channel_stats_host(int32_t n_farms, int32_t n_rows, int32_t n_dof
                                   const raftk_farm_channels *ch);
 
 /*
+ * Rotor speed, generator torque and blade pitch statistics (FOWT.saveTurbineOutputs raft_fowt.py:2610-2679) for
+ * n_units units (designs or farms) x n_cases cases x n_rot rotors.  Per (unit u, case c, rotor k) and row h of the case:
+ *   y_h(w) = sum_b R[k,b] Xi[u, h, col0[k] + b, w]           (the hub row XiHub[h, ir], a real functional of the response)
+ *   phi_h = C y_h for every row of the case, plus one wind row phi = -C V_w / (j w)   (:2643-2646)
+ *   omega = j w phi, torque = (j w kp_tau + ki_tau) phi, bPitch = (j w kp_beta + ki_beta) phi   (:2649-2651)
+ * std[u,c,k,:] = sqrt(1/2 sum_rows sum_w |.|^2) and psd[u,c,k,:,w] = 1/2 sum_rows |.|^2 / dw of (omega, torque, bPitch),
+ * omega in rpm (/ 0.1047, the reference's radps2rpm; PSD times its square), torque in N m, bPitch in degrees (x
+ * 57.29577951308232; PSD times its square).  A (case, rotor) with C = 0 and V_w = 0 gives exact zeros (the reference's
+ * outputs when aeroServoMod <= 1 or the inflow speed is 0).  Means and bounds (omega_avg = Omega_case, avg +- 2 std, ...)
+ * are the caller's.
+ * Xi complex [n_units, n_rows, n_dof, nw]; the rows of case c are case_row0[c] .. case_row0[c+1]-1 (its wave trains).
+ * w [nw], every bin > 0: the wind row divides by w, so a bin at w <= 0 has no finite value (the reference's grids start at
+ * min_freq > 0); _host refuses such a w, _dev cannot read it and leaves NaN in that (unit, case, rotor)'s outputs.
+ * One CTA per (unit, case, rotor); a result does not depend on which units, cases or rotors share the call.
+ * _dev: device w, Xi, R, C, V_w, gains and outputs, enqueued on `stream` without synchronising.  _host: host pointers
+ * everywhere.  col0 and case_row0 are HOST memory in both, read during the call.
+ * RAFTK_EINVAL before any launch: a count below 1, n_r > n_dof, a col0 < 0 or col0 + n_r > n_dof, a case_row0 that does not
+ * start at 0 or end at n_rows or has an empty or decreasing case, R_shared or tf_shared not 0 or 1, a NULL w, Xi, R, C, V_w,
+ * gains, std, col0 or case_row0, dw <= 0, or (_host) a w <= 0.
+ */
+typedef struct raftk_rotor_outputs {
+    int32_t n_cases, n_rot;
+    int32_t n_r;               /* hub-row length: 6 for rigid FOWTs and farm FOWTs, n_dof for generalised DOFs        */
+    int32_t R_shared;          /* 1: R [n_rot, n_r] for every unit; 0: R [n_units, n_rot, n_r]                      */
+    int32_t tf_shared;         /* 1: C, V_w, gains [n_cases, n_rot, ...] for every unit; 0: [n_units, n_cases, n_rot, ...] */
+    int32_t _pad0;
+    const int32_t *col0;       /* HOST [n_rot]: first response column of each rotor's hub row                       */
+    const int32_t *case_row0;  /* HOST [n_cases + 1]                                                                 */
+    const double *R;
+    const double *C, *V_w;     /* complex [..., nw]: control transfer function, turbulent-wind amplitudes          */
+    const double *gains;       /* [..., 4]: kp_tau, ki_tau, kp_beta, ki_beta                                        */
+    double dw;                 /* PSD divisor (> 0)                                                                 */
+    double *std;               /* [n_units, n_cases, n_rot, 3]                                                       */
+    double *psd;               /* [n_units, n_cases, n_rot, 3, nw] or NULL                                           */
+} raftk_rotor_outputs;
+
+int raftk_rotor_stats_dev(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                          const raftk_rotor_outputs *ro, void *stream);
+int raftk_rotor_stats_host(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                           const raftk_rotor_outputs *ro);
+
+/*
  * Natural frequencies and mode shapes (Model.solveEigen raft_model.py:436-547, FOWT.solveEigen raft_fowt.py:1646-1729): the
  * eigenvalues and right eigenvectors of M^-1 C for n_systems systems of n DOFs, what np.linalg.eig(np.linalg.solve(M, C))
  * returns, in the reference's output order.  Per system: LU of M with partial pivoting, A = M^-1 C, power-of-two balancing,

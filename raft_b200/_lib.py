@@ -113,6 +113,13 @@ class RaftkFarmChannels(C.Structure):
                 ("std", C.c_void_p), ("psd", C.c_void_p), ("amp", C.c_void_p), ("tile_w", C.c_int32), ("_pad0", C.c_int32)]
 
 
+class RaftkRotorOutputs(C.Structure):
+    """include/raftk.h raftk_rotor_outputs: hub rows, control transfer functions and gains of rotors, and their statistics."""
+    _fields_ = [("n_cases", C.c_int32), ("n_rot", C.c_int32), ("n_r", C.c_int32), ("R_shared", C.c_int32), ("tf_shared", C.c_int32),
+                ("_pad0", C.c_int32), ("col0", C.c_void_p), ("case_row0", C.c_void_p), ("R", C.c_void_p), ("C", C.c_void_p),
+                ("V_w", C.c_void_p), ("gains", C.c_void_p), ("dw", C.c_double), ("std", C.c_void_p), ("psd", C.c_void_p)]
+
+
 class RaftkEigen(C.Structure):
     """include/raftk.h raftk_eigen: eigenvalues and right eigenvectors of M^-1 C for a batch of systems."""
     _fields_ = [("n_systems", C.c_int32), ("n", C.c_int32), ("sort", C.c_int32), ("_pad0", C.c_int32),
@@ -190,6 +197,7 @@ SYMBOLS = [
     "raftk_family_sizes", "raftk_build_family_host",
     "raftk_eigen_workspace_bytes", "raftk_eigen_dev", "raftk_eigen_host",
     "raftk_farm_channel_stats_workspace_bytes", "raftk_farm_channel_stats_dev", "raftk_farm_channel_stats_host",
+    "raftk_rotor_stats_dev", "raftk_rotor_stats_host",
 ]
 
 
@@ -342,6 +350,10 @@ def _load():
     lib.raftk_farm_channel_stats_dev.restype = C.c_int
     lib.raftk_farm_channel_stats_host.argtypes = [C.c_int32] * 4 + [C.c_void_p, C.c_void_p, P(RaftkFarmChannels)]
     lib.raftk_farm_channel_stats_host.restype = C.c_int
+    lib.raftk_rotor_stats_dev.argtypes = [C.c_int32] * 4 + [C.c_void_p, C.c_void_p, P(RaftkRotorOutputs), C.c_void_p]
+    lib.raftk_rotor_stats_dev.restype = C.c_int
+    lib.raftk_rotor_stats_host.argtypes = [C.c_int32] * 4 + [C.c_void_p, C.c_void_p, P(RaftkRotorOutputs)]
+    lib.raftk_rotor_stats_host.restype = C.c_int
     lib.raftk_family_sizes.argtypes = [P(RaftkFamily), P(C.c_int32), P(C.c_int32)]
     lib.raftk_build_family_host.argtypes = [P(RaftkFamily), P(RaftkFamilyTables)]
     lib.raftk_family_sizes.restype = C.c_int

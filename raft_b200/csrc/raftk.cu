@@ -151,6 +151,7 @@ extern "C" int raftk_last_dispatch(raftk_dispatch *out)
 #include "raftk_slender.cuh"
 #include "raftk_general.cuh"
 #include "raftk_misc.cuh"
+#include "raftk_rotor.cuh"
 #include "raftk_eigen.cuh"
 #include "raftk_builder.h"
 
@@ -2601,6 +2602,82 @@ extern "C" int raftk_farm_channel_stats_host(int32_t n_farms, int32_t n_rows, in
     S.buf(ws, wb);
     int rc;
     if ((rc = S.commit()) || (rc = raftk_farm_channel_stats_dev(n_farms, n_rows, n_dof, nw, dW, dXi, &d, ws, wb, nullptr))) return rc;
+    return S.finish();
+}
+
+// ---- rotor speed, generator torque and blade pitch (raftk_rotor_stats_*) ---------------------------------------------------
+static int rotor_check(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                       const raftk_rotor_outputs *ro)
+{
+    if (!ro) return set_err(RAFTK_EINVAL, "rotor-stats: null argument");
+    if (n_units < 1 || n_rows < 1 || n_dof < 1 || nw < 1 || ro->n_cases < 1 || ro->n_rot < 1 || ro->n_r < 1)
+        return set_err(RAFTK_EINVAL, "rotor-stats: n_units, n_rows, n_dof, nw, n_cases, n_rot and n_r must be >= 1");
+    if (ro->R_shared != 0 && ro->R_shared != 1) return set_err(RAFTK_EINVAL, "rotor-stats: R_shared must be 0 or 1");
+    if (ro->tf_shared != 0 && ro->tf_shared != 1) return set_err(RAFTK_EINVAL, "rotor-stats: tf_shared must be 0 or 1");
+    if (!w || !Xi || !ro->R || !ro->C || !ro->V_w || !ro->gains || !ro->std || !ro->col0 || !ro->case_row0)
+        return set_err(RAFTK_EINVAL, "rotor-stats: w, Xi, R, C, V_w, gains, std, col0 and case_row0 are required");
+    if (!(ro->dw > 0.0)) return set_err(RAFTK_EINVAL, "rotor-stats: dw must be > 0");
+    if (ro->n_r > n_dof) return set_err(RAFTK_EINVAL, "rotor-stats: n_r must be <= n_dof");
+    for (int32_t k = 0; k < ro->n_rot; k++)
+        if (ro->col0[k] < 0 || ro->col0[k] > n_dof - ro->n_r)
+            return set_err(RAFTK_EINVAL, "rotor-stats: every col0 must satisfy 0 <= col0 and col0 + n_r <= n_dof");
+    if (ro->case_row0[0] != 0 || ro->case_row0[ro->n_cases] != n_rows)
+        return set_err(RAFTK_EINVAL, "rotor-stats: case_row0 must start at 0 and end at n_rows");
+    for (int32_t c = 0; c < ro->n_cases; c++)
+        if (ro->case_row0[c + 1] <= ro->case_row0[c]) return set_err(RAFTK_EINVAL, "rotor-stats: every case needs at least one row");
+    if ((size_t)n_units * ro->n_cases * ro->n_rot > 2147483647u)
+        return set_err(RAFTK_EINVAL, "rotor-stats: too many (unit, case, rotor) blocks");
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_rotor_stats_dev(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                                     const raftk_rotor_outputs *ro, void *stream)
+{
+    if (int rc = rotor_check(n_units, n_rows, n_dof, nw, w, Xi, ro)) return rc;
+    const cudaStream_t st = (cudaStream_t)stream;
+    RotorParams P = {};
+    P.n_rows = n_rows; P.n_dof = n_dof; P.nw = nw; P.n_r = ro->n_r;
+    P.n_cases = ro->n_cases; P.n_rot = ro->n_rot;
+    P.r_stride = ro->R_shared ? 0 : (size_t)ro->n_rot * ro->n_r;
+    P.tf_stride = ro->tf_shared ? 0 : (size_t)ro->n_cases * ro->n_rot;
+    P.dw = ro->dw;
+    P.w = w; P.R = ro->R; P.gains = ro->gains;
+    P.Xi = reinterpret_cast<const double2 *>(Xi);
+    P.C = reinterpret_cast<const double2 *>(ro->C);
+    P.Vw = reinterpret_cast<const double2 *>(ro->V_w);
+    P.sd = ro->std; P.psd = ro->psd;
+    // chunks of cases and rotors only bound the launch parameters: every CTA computes the same thing in any chunk
+    for (int32_t c0 = 0; c0 < ro->n_cases; c0 += ROTOR_CHUNK) {
+        P.c0 = c0; P.nc = std::min<int32_t>(ROTOR_CHUNK, ro->n_cases - c0);
+        for (int j = 0; j <= P.nc; j++) P.row0[j] = ro->case_row0[c0 + j];
+        for (int32_t k0 = 0; k0 < ro->n_rot; k0 += ROTOR_CHUNK) {
+            P.k0 = k0; P.nk = std::min<int32_t>(ROTOR_CHUNK, ro->n_rot - k0);
+            for (int j = 0; j < P.nk; j++) P.col0[j] = ro->col0[k0 + j];
+            k_rotor_stats<<<(unsigned)((size_t)n_units * P.nc * P.nk), ROTOR_T, 0, st>>>(P);
+            g_launches++;
+            CUDA_TRY(cudaGetLastError());
+        }
+    }
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_rotor_stats_host(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                                      const raftk_rotor_outputs *ro)
+{
+    if (int rc = rotor_check(n_units, n_rows, n_dof, nw, w, Xi, ro)) return rc;
+    for (int32_t i = 0; i < nw; i++)
+        if (!(w[i] > 0.0)) return set_err(RAFTK_EINVAL, "rotor-stats: every w must be > 0 (the wind row divides by w)");
+    const size_t tf = (ro->tf_shared ? 1 : (size_t)n_units) * ro->n_cases * ro->n_rot;
+    const size_t rows = (size_t)n_units * ro->n_cases * ro->n_rot * 3;
+    raftk_rotor_outputs d = *ro;
+    const double *dW, *dXi;
+    Staging S("raftk_rotor_stats_host");
+    S.in(dW, w, nw); S.in(dXi, Xi, (size_t)n_units * n_rows * n_dof * nw * 2);
+    S.in(d.R, ro->R, (ro->R_shared ? 1 : (size_t)n_units) * ro->n_rot * ro->n_r);
+    S.in(d.C, ro->C, tf * nw * 2); S.in(d.V_w, ro->V_w, tf * nw * 2); S.in(d.gains, ro->gains, tf * 4);
+    S.out(d.std, rows, ro->std); S.out(d.psd, ro->psd ? rows * nw : 0, ro->psd);
+    int rc;
+    if ((rc = S.commit()) || (rc = raftk_rotor_stats_dev(n_units, n_rows, n_dof, nw, dW, dXi, &d, nullptr))) return rc;
     return S.finish();
 }
 

@@ -14,13 +14,17 @@ from .fowt import FOWT
 
 class Model:
     def __init__(self, design, matrices=None, array_stiffness=None, channels=None, tension_jacobian=None, mean_tensions=None,
-                 array_tension_jacobian=None, array_mean_tensions=None):
+                 array_tension_jacobian=None, array_mean_tensions=None, rotors=None):
         """``channels``: optional turbine output channels per FOWT (``packer.pack_turbine_channels`` dicts: nacelle
         accelerations, tower-base moment) -- the turbine itself is outside this path, its constants enter here.
         ``tension_jacobian`` [2L,6] / ``mean_tensions`` [2L] (one for every FOWT, or a list with None for a FOWT without its
         own lines) and ``array_tension_jacobian`` [2L,6N] / ``array_mean_tensions`` [2L]: the mooring line-end tensions of
         moorMod 0, standing in for fowt.ms / model.ms (MoorPy getCoupledStiffness(tensions=True)[1] and getTensions(), see
-        ``packer.pack_mooring_tensions``) as ``array_stiffness`` stands in for getCoupledStiffnessA."""
+        ``packer.pack_mooring_tensions``) as ``array_stiffness`` stands in for getCoupledStiffnessA.
+        ``rotors``: ``packer.pack_rotor_outputs`` of each FOWT for the cases ``analyzeCases`` will run (one dict for a single
+        FOWT, a list with None for a FOWT without rotor outputs for an array): the rotors' control transfer functions, wind
+        amplitudes, gains and operating points, standing in for Rotor.calcAero (CCBlade), as ``matrices`` stand in for the
+        turbine's constants."""
         s = design.setdefault("settings", {})
         min_freq, max_freq = float(s.get("min_freq", 0.01)), float(s.get("max_freq", 1.00))
         self.XiStart = float(s.get("XiStart", 0.1))
@@ -54,6 +58,10 @@ class Model:
                          for J, T0 in zip(per(tension_jacobian), per(mean_tensions))]
         self.array_tensions = (None if array_tension_jacobian is None else
                                packer.pack_mooring_tensions(dict(J=array_tension_jacobian, T0=array_mean_tensions)))
+        self.rotors = per(rotors)
+        for r in self.rotors:
+            if r is not None and r["R"].shape[1] != 6:
+                raise ValueError("rotors: the hub rows of a rigid FOWT must be [nrot, 6]")
         for t in self.tensions:
             if t is not None and t["J"].shape[1] != 6:
                 raise ValueError("tension_jacobian must be [2L, 6]")
@@ -84,7 +92,8 @@ class Model:
         Fills results['freq_rad'], results['Xi'] [nCases, nDOF, nw], results['status'] [nCases, nFOWT, 4], and per case and
         FOWT the saveTurbineOutputs statistics: PRP motions, turbine channels, wave_PSD and, with tension Jacobians, Tmoor_* of
         the FOWT's lines and case_metrics[iCase]['array_mooring'] of the array's (raft_fowt.py:2355-2399, raft_model.py:371-433;
-        max / min = avg +- 3 std, Tmoor_PSD divided by w[0] as the reference does)."""
+        max / min = avg +- 3 std, Tmoor_PSD divided by w[0] as the reference does) and, with ``rotors``, the rotor entries
+        omega / torque / bPitch / power and wind_PSD (raft_fowt.py:2610-2679; ``solver.rotor_metrics``)."""
         if cases is None:
             keys = self.design["cases"]["keys"]
             cases = [dict(zip(keys, row)) for row in self.design["cases"]["data"]]
@@ -110,6 +119,7 @@ class Model:
                for i, t in enumerate(self.tensions)]
         arr = None if self.array_tensions is None else solver.farm_channel_stats(self.array_tensions["J"], out["Xi_all"], w0)
         dw = self.w[1] - self.w[0]
+        rot = self._rotor_stats(cases, out, dw)
         self.results["case_metrics"] = {}
         for ic in range(nC):
             idx = np.nonzero(owner == ic)[0]
@@ -138,11 +148,35 @@ class Model:
                 if ten[i] is not None:
                     m.update(solver.tension_metrics(self.tensions[i]["T0"], *solver.combine_trains(ten[i][0], ten[i][1], idx)))
                 m["wave_PSD"] = (0.5 * np.abs(out["zeta"][idx]) ** 2 / dw).sum(axis=0)          # getPSD(zeta, dw) (:2608)
+                if self.rotors[i] is not None:
+                    k = rot[1][i]
+                    m.update(solver.rotor_metrics(self.rotors[i], ic, rot[0][0][ic, k], rot[0][1][ic, k], dw))
                 self.results["case_metrics"][ic][i] = m
             if arr is not None:
                 self.results["case_metrics"][ic]["array_mooring"] = solver.tension_metrics(self.array_tensions["T0"],
                                                                                            *solver.combine_trains(arr[0], arr[1], idx))
         return self.results
+
+    def _rotor_stats(self, cases, out, dw):
+        """Rotor statistics of every FOWT's rotors in one device call on the (coupled) response Xi_all [nTrains, 6N, nw]:
+        FOWT i's hub rows read columns 6 i .. 6 i + 5.  -> ((std [nC, nrot, 3], PSD [nC, nrot, 3, nw]), per FOWT the slice of
+        its rotors), or None without rotor inputs."""
+        have = [i for i, r in enumerate(self.rotors) if r is not None]
+        if not have:
+            return None
+        for i in have:
+            if self.rotors[i]["C"].shape[0] != len(cases):
+                raise ValueError("rotors: FOWT %d's are packed for %d cases, %d given" % (i, self.rotors[i]["C"].shape[0], len(cases)))
+        cat = lambda k: np.concatenate([self.rotors[i][k] for i in have], axis=1 if k != "R" else 0)   # noqa: E731
+        col0 = np.concatenate([np.full(len(self.rotors[i]["R"]), 6 * i) for i in have])
+        first = np.nonzero(np.diff(np.append(-1, out["owner"])))[0]
+        stats = solver.rotor_stats(cat("R"), cat("C"), cat("V_w"), cat("gains"), self.w, out["Xi_all"], dw,
+                                   case_row0=np.append(first, len(out["owner"])), col0=col0)
+        sl, k0 = [None] * self.nFOWT, 0
+        for i in have:
+            sl[i] = slice(k0, k0 + len(self.rotors[i]["R"]))
+            k0 = sl[i].stop
+        return stats, sl
 
     # raft_model.py:436-547 -------------------------------------------------------------------------------------
     def solveEigen(self, display=0, outPath=None):

@@ -552,6 +552,72 @@ def pack_general_channels(fowt, tensions=None):
     return out
 
 
+ROTOR_KEYS = ("omega_avg", "omega_std", "omega_max", "omega_min", "omega_PSD", "torque_avg", "torque_std", "torque_PSD",
+              "power_avg", "bPitch_avg", "bPitch_std", "bPitch_PSD")
+
+
+def pack_rotor_outputs(fowt, rotor_states, cases):
+    """Inputs of the rotor channels of ``FOWT.saveTurbineOutputs`` (raft_fowt.py:2610-2679) for ``solver.rotor_stats`` /
+    ``raftk_rotor_stats_*``.  Duck-typed on a live FOWT (``rotorList``, ``T``, the hub nodes' ``id``); ``rotor_states[c][ir]``
+    is rotor ir after the reference's ``Rotor.calcAero`` for case c (CCBlade is out of scope), or a dict with the same
+    attribute names: C, V_w (complex [nw]), kp_tau, ki_tau, kp_beta, ki_beta, Omega_case, aero_torque, Ng, aero_power,
+    pitch_case, aeroServoMod, r3.  ``cases``: the case dicts, for the inflow speed.
+
+    Rotor ir's hub row is column ir of the reference's stacked hub array XiHub[ih, ir, :] (:2402, :2423, :2644), that is
+    DOF ir % 6 of rotor ir // 6's hub node: row 6 * rotorList[ir // 6].nodeList[0].id + ir % 6 of fowt.T.  With one rotor
+    that is the hub surge, with two rotors the second one reads the first hub's sway -- the reference's indexing, kept.
+    A (case, rotor) is active when aeroServoMod > 1 and the inflow speed (current_speed, default 1.0, below the waterline
+    r3[2] < 0; wind_speed, default 10.0, otherwise) is above 0 (:2633-2640); an inactive one gets C = V_w = 0 and zero
+    means, which is what the reference reports for it.  kp_tau / ki_tau are the rotor's raw attributes (-VS_KP, -VS_KI,
+    raft_rotor.py:800-801), as :2650 uses them, not the gated locals of calcAero (:909-910).
+    -> dict(R [nrot, nDOF], C, V_w complex [nC, nrot, nw], gains [nC, nrot, 4] (kp_tau, ki_tau, kp_beta, ki_beta),
+    omega_avg, torque_avg (aero_torque / Ng), power_avg, bPitch_avg [nC, nrot], active [nC, nrot] bool, wind [nC] (the V_w
+    of the case's last active rotor, the source of wind_PSD, or None)).  aeroServoMod 2 without C: NotImplementedError."""
+    rotors = list(getattr(fowt, "rotorList", []) or [])
+    T = np.asarray(fowt.T, dtype=float)
+    nrot, nC = len(rotors), len(cases)
+    if nrot == 0:
+        raise ValueError("pack_rotor_outputs: the FOWT has no rotors")
+    if len(rotor_states) != nC or any(len(s) != nrot for s in rotor_states):
+        raise ValueError("rotor_states: one entry per case (%d), each with one state per rotor (%d)" % (nC, nrot))
+    R = np.array([T[6 * rotors[ir // 6].nodeList[0].id + ir % 6] for ir in range(nrot)])
+    out = dict(R=R, active=np.zeros([nC, nrot], dtype=bool), gains=np.zeros([nC, nrot, 4]), wind=[None] * nC)
+    for k in ("omega_avg", "torque_avg", "power_avg", "bPitch_avg"):
+        out[k] = np.zeros([nC, nrot])
+    C_, V = [], []
+    for c, case in enumerate(cases):
+        Cc, Vc = [], []
+        for ir in range(nrot):
+            s = rotor_states[c][ir]
+            get = (lambda k, d=None: s.get(k, d)) if isinstance(s, dict) else (lambda k, d=None: getattr(s, k, d))
+            r3 = np.asarray(get("r3", getattr(rotors[ir], "r3", np.zeros(3))), dtype=float)
+            mod = int(get("aeroServoMod", getattr(rotors[ir], "aeroServoMod", 0)))
+            speed = float(case.get("current_speed", 1.0) if r3[2] < 0 else case.get("wind_speed", 10.0))
+            if mod > 1 and speed > 0.0:
+                if get("C") is None:
+                    raise NotImplementedError("rotor outputs need the control transfer function C of Rotor.calcAero "
+                                              "(aeroServoMod %d)" % mod)
+                Cc.append(np.asarray(get("C"), dtype=complex))
+                Vc.append(np.asarray(get("V_w"), dtype=complex))
+                out["active"][c, ir] = True
+                out["gains"][c, ir] = [float(get(k)) for k in ("kp_tau", "ki_tau", "kp_beta", "ki_beta")]
+                out["omega_avg"][c, ir] = float(get("Omega_case"))
+                out["torque_avg"][c, ir] = float(get("aero_torque")) / float(get("Ng"))
+                out["power_avg"][c, ir] = float(get("aero_power"))
+                out["bPitch_avg"][c, ir] = float(get("pitch_case"))
+                out["wind"][c] = Vc[-1]                                       # the last active rotor's (:2679)
+            else:
+                Cc.append(None), Vc.append(None)
+        C_.append(Cc), V.append(Vc)
+    shapes = {np.shape(a) for row in C_ + V for a in row if a is not None}
+    if len(shapes) > 1:
+        raise ValueError("pack_rotor_outputs: C and V_w must all be [nw]")
+    nw = shapes.pop()[0] if shapes else len(np.asarray(getattr(fowt, "w", [])))
+    out["C"] = np.array([[np.zeros(nw, dtype=complex) if a is None else a for a in row] for row in C_]).reshape(nC, nrot, nw)
+    out["V_w"] = np.array([[np.zeros(nw, dtype=complex) if a is None else a for a in row] for row in V]).reshape(nC, nrot, nw)
+    return out
+
+
 def pack_mooring_tensions(ms, moorMod=0):
     """Line-end tensions of a mooring system as linear functionals of the motions of its coupled bodies (moorMod 0,
     raft_fowt.py:2362-2367, raft_model.py:379-386): T_amp = J @ Xi.  Duck-typed on a MoorPy system as the reference holds it

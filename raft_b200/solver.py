@@ -871,6 +871,16 @@ class GeneralSession:
                                                       A.data_ptr() if amp else None, torch.cuda.current_stream(self.device).cuda_stream))
         return sd, P, A
 
+    def rotor_stats(self, R, C_, V_w, gains, case_row0=None, psd=True):
+        """Rotor speed, generator torque and blade pitch statistics of the last ``solve()`` on the device
+        (raftk_rotor_stats_dev, no host round trip): ``R`` [nrot, nDOF], ``C``, ``V_w``, ``gains`` and ``case_row0`` as
+        ``rotor_stats`` (``packer.pack_rotor_outputs``; the first train of every case, e.g. ``pack_case_trains``' ``first``
+        + [nT]).  -> (std [nC, nrot, 3], PSD [nC, nrot, 3, nw] or None), torch tensors."""
+        stream = self.torch.cuda.current_stream(self.device).cuda_stream
+        sd, P, self._rot_keep = _rotor_stats_dev(self.torch, self.device, stream, self.Xi[None], self.keep["w"], R, C_, V_w, gains,
+                                                 self.dw, case_row0, None, psd)
+        return sd[0], (P[0] if psd else None)
+
 
 def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0, fd=None, F_BEM=False, qtf=None, F_2nd=False,
                            max_chunk_cases=None):
@@ -1055,6 +1065,101 @@ def tension_metrics(T0, std, psd):
                 Tmoor_PSD=np.array(psd, dtype=float))
 
 
+def _rotor_struct(R, C_, V_w, gains, n_units, nw, dw, case_row0, col0):
+    """Shapes of rotor_stats' inputs (numpy arrays or torch tensors) checked -> (raftk_rotor_outputs without data pointers,
+    case_row0, col0 as int32 host arrays).  R [nrot, n_r] (every unit) or [n_units, nrot, n_r]; C, V_w [nC, nrot, nw] (every
+    unit) or [n_units, nC, nrot, nw]; gains [..., 4] over the same leading axes."""
+    if len(R.shape) not in (2, 3) or (len(R.shape) == 3 and R.shape[0] != n_units):
+        raise ValueError("R must be [nrot, n_r] or [%d, nrot, n_r]" % n_units)
+    nrot, n_r = R.shape[-2:]
+    if len(C_.shape) not in (3, 4) or (len(C_.shape) == 4 and C_.shape[0] != n_units) or tuple(C_.shape[-2:]) != (nrot, nw):
+        raise ValueError("C must be [nC, %d, %d] or [%d, nC, %d, %d]" % (nrot, nw, n_units, nrot, nw))
+    if tuple(V_w.shape) != tuple(C_.shape) or tuple(gains.shape) != tuple(C_.shape[:-1]) + (4,):
+        raise ValueError("V_w must have C's shape and gains C's leading axes + [4]")
+    nC = C_.shape[-3]
+    case_row0 = np.arange(nC + 1, dtype=_I4) if case_row0 is None else np.ascontiguousarray(case_row0, dtype=_I4)
+    col0 = np.zeros(nrot, dtype=_I4) if col0 is None else np.ascontiguousarray(col0, dtype=_I4)
+    if case_row0.shape != (nC + 1,) or col0.shape != (nrot,):
+        raise ValueError("case_row0 must be [nC + 1] and col0 [nrot]")
+    ro = _lib.RaftkRotorOutputs()
+    ro.n_cases, ro.n_rot, ro.n_r = nC, nrot, n_r
+    ro.R_shared, ro.tf_shared = int(len(R.shape) == 2), int(len(C_.shape) == 3)
+    ro.col0, ro.case_row0, ro.dw = col0.ctypes.data, case_row0.ctypes.data, float(dw)
+    return ro, case_row0, col0
+
+
+def rotor_stats(R, C_, V_w, gains, w, Xi, dw, case_row0=None, col0=None, psd=True):
+    """Rotor speed, generator torque and blade pitch statistics on the device (raftk_rotor_stats_host), host buffers
+    (FOWT.saveTurbineOutputs raft_fowt.py:2610-2679): per unit, case and rotor, the hub row y = R[rot] . Xi[col0[rot]:...],
+    phi = C y over the case's rows plus the wind row -C V_w / (j w), and omega = j w phi, torque = (j w kp_tau + ki_tau) phi,
+    bPitch = (j w kp_beta + ki_beta) phi.  ``Xi`` complex [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]; ``R``, ``C``,
+    ``V_w``, ``gains`` as ``packer.pack_rotor_outputs`` gives them for every unit, or with a leading unit axis;
+    ``case_row0`` [nC + 1] the first row of every case (None: one row per case); ``col0`` [nrot] the first column of every
+    rotor's hub row (None: 0).  -> (std [n_units, nC, nrot, 3] (omega rpm, torque N m, bPitch deg), PSD [n_units, nC, nrot,
+    3, nw] or None), without the unit axis when ``Xi`` had none."""
+    Xi = np.ascontiguousarray(Xi, dtype=np.complex128)
+    squeeze = Xi.ndim == 3
+    if squeeze:
+        Xi = Xi[None]
+    if Xi.ndim != 4:
+        raise ValueError("Xi must be [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]")
+    nU, nR, n, nw = Xi.shape
+    R, C_ = np.ascontiguousarray(R, dtype=_F8), np.ascontiguousarray(C_, dtype=np.complex128)
+    V_w, gains = np.ascontiguousarray(V_w, dtype=np.complex128), np.ascontiguousarray(gains, dtype=_F8)
+    w = np.ascontiguousarray(w, dtype=_F8)
+    if w.shape != (nw,):
+        raise ValueError("w must be [nw]")
+    ro, rows, cols = _rotor_struct(R, C_, V_w, gains, nU, nw, dw, case_row0, col0)
+    sd = np.zeros([nU, ro.n_cases, ro.n_rot, 3])
+    P = np.zeros([nU, ro.n_cases, ro.n_rot, 3, nw]) if psd else None
+    ro.R, ro.C, ro.V_w, ro.gains = R.ctypes.data, C_.ctypes.data, V_w.ctypes.data, gains.ctypes.data
+    ro.std, ro.psd = sd.ctypes.data, (P.ctypes.data if psd else None)
+    check(lib.raftk_rotor_stats_host(nU, nR, n, nw, w.ctypes.data, Xi.ctypes.data, C.byref(ro)))
+    if squeeze:
+        sd, P = sd[0], (P[0] if psd else None)
+    return sd, P
+
+
+def _rotor_stats_dev(torch, device, stream, Xi, w, R, C_, V_w, gains, dw, case_row0, col0, psd):
+    """rotor_stats on a resident Xi [n_units, n_rows, n_dof, nw] (torch, complex128) and w; R, C, V_w, gains numpy arrays or
+    torch tensors -> (std, PSD or None) torch tensors, enqueued on ``stream`` (raftk_rotor_stats_dev)."""
+    nU, nR, n, nw = Xi.shape
+
+    def dev(a, dt):
+        if isinstance(a, torch.Tensor):
+            return a.to(device=device, dtype=dt).contiguous()
+        a = np.ascontiguousarray(a, dtype=np.complex128 if dt == torch.complex128 else _F8)
+        return torch.from_numpy(a).to(device)
+    with torch.cuda.device(device):
+        R, C_, V_w, gains = dev(R, torch.float64), dev(C_, torch.complex128), dev(V_w, torch.complex128), dev(gains, torch.float64)
+        ro, rows, cols = _rotor_struct(R, C_, V_w, gains, nU, nw, dw, case_row0, col0)
+        sd = torch.empty([nU, ro.n_cases, ro.n_rot, 3], dtype=torch.float64, device=device)
+        P = torch.empty([nU, ro.n_cases, ro.n_rot, 3, nw], dtype=torch.float64, device=device) if psd else None
+        ro.R, ro.C, ro.V_w, ro.gains = R.data_ptr(), C_.data_ptr(), V_w.data_ptr(), gains.data_ptr()
+        ro.std, ro.psd = sd.data_ptr(), (P.data_ptr() if psd else None)
+        check(lib.raftk_rotor_stats_dev(nU, nR, n, nw, w.data_ptr(), Xi.data_ptr(), C.byref(ro), stream))
+    return sd, P, (R, C_, V_w, gains)
+
+
+def rotor_metrics(rotors, ic, std, psd, dw):
+    """The rotor entries FOWT.saveTurbineOutputs stores for case ``ic`` (raft_fowt.py:2617-2679) from ``rotors``
+    (``packer.pack_rotor_outputs``) and the case's statistics std [nrot, 3], PSD [nrot, 3, nw]: *_avg / *_std [nrot],
+    omega_max / min = avg +- 2 std, *_PSD [nw, nrot], power_avg, and wind_PSD = getPSD(V_w, dw) of the case's last active
+    rotor (absent when none is active).  Inactive rotors report zeros, as in the reference."""
+    std, psd = np.asarray(std, dtype=float), np.asarray(psd, dtype=float)
+    m = {}
+    for j, nm in enumerate(("omega", "torque", "bPitch")):
+        m[nm + "_avg"] = np.array(rotors[nm + "_avg"][ic], dtype=float)
+        m[nm + "_std"] = std[:, j].copy()
+        m[nm + "_PSD"] = np.ascontiguousarray(psd[:, j].T)
+    m["omega_max"] = m["omega_avg"] + 2 * m["omega_std"]
+    m["omega_min"] = m["omega_avg"] - 2 * m["omega_std"]
+    m["power_avg"] = np.array(rotors["power_avg"][ic], dtype=float)
+    if rotors["wind"][ic] is not None:
+        m["wind_PSD"] = 0.5 * np.abs(rotors["wind"][ic]) ** 2 / dw
+    return m
+
+
 def general_case_metrics(channels, std, psd, amp, idx, dw=None):
     """The entries FOWT.saveTurbineOutputs stores for one case (raft_fowt.py:2299-2604) from per-train channel statistics
     (std [nT,nch], PSD [nT,nch,nw], amplitudes [nT,nch,nw]) of the case's trains ``idx``: ``*_avg/_std/_max/_min/_PSD`` of every
@@ -1096,21 +1201,23 @@ def general_case_metrics(channels, std, psd, amp, idx, dw=None):
     return m
 
 
-def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, fd=None, qtf=None):
+def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, fd=None, qtf=None, rotors=None):
     """Model.analyzeCases (dynamics and output statistics) for one FOWT with generalised degrees of freedom: ``cases`` a list
     of case dicts, scalar or list-valued wave keys (several wave trains); ``channels`` from ``packer.pack_general_channels``.
     -> dict(Xi_trains [per case: nTrains,nDOF,nw], status [nC,4] of train 0, case_metrics {case: saveTurbineOutputs entries},
     empty without channels; with ``pack_general_channels(fowt, tensions=...)`` they include Tmoor_*).  ``fd``: frequency-dependent terms, as for ``general_solve_dynamics``.  ``qtf``: second-order
     wave loads (``packer.pack_general_qtf``); the result then also holds, per case, the reference FOWT's ``Fhydro_2nd``
-    (complex [nTrains,nDOF,nw]) and ``Fhydro_2nd_mean`` ([nTrains,nDOF]), zero from reduced DOF 6 up (raft_model.py:1034-1036)."""
+    (complex [nTrains,nDOF,nw]) and ``Fhydro_2nd_mean`` ([nTrains,nDOF]), zero from reduced DOF 6 up (raft_model.py:1034-1036).
+    ``rotors``: ``packer.pack_rotor_outputs`` of the FOWT for these cases; every case's metrics then hold the rotor entries
+    (omega / torque / bPitch / power, wind_PSD; ``rotor_metrics``)."""
     from .packer import pack_case_trains
     table, owner, first = pack_case_trains(cases)
     q = bool(qtf)
     res = general_solve_dynamics(P, M, B, Cm, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start, fd=fd, qtf=qtf, F_2nd=q)
-    return _general_case_results(P, res[0], res[1], owner, first, len(cases), channels, res[2:4] if q else None)
+    return _general_case_results(P, res[0], res[1], owner, first, len(cases), channels, res[2:4] if q else None, rotors)
 
 
-def _general_case_results(P, Xi, st, owner, first, n_cases, channels, F2nd):
+def _general_case_results(P, Xi, st, owner, first, n_cases, channels, F2nd, rotors=None):
     """general_analyze_cases' result for one design from its train table's Xi [nT,nDOF,nw], status [nT,4] and, with a QTF
     table, (F_2nd [nT,6,nw], F_2nd_mean [nT,6])."""
     raise_on_flags(st[first])                                           # raft_model.py:1089, :1098-1099
@@ -1119,6 +1226,13 @@ def _general_case_results(P, Xi, st, owner, first, n_cases, channels, F2nd):
         sd, ps, amp = general_channel_stats(channels["R"], channels["wpow"], P["w"], Xi, float(P["dw"]), psd=True, amp=True)
         for ic in range(n_cases):
             metrics[ic] = general_case_metrics(channels, sd, ps, amp, np.nonzero(owner == ic)[0], dw=float(P["dw"]))
+    if rotors is not None:
+        if rotors["C"].shape[0] != n_cases:
+            raise ValueError("rotors: packed for %d cases, %d given" % (rotors["C"].shape[0], n_cases))
+        rsd, rps = rotor_stats(rotors["R"], rotors["C"], rotors["V_w"], rotors["gains"], P["w"], Xi, float(P["dw"]),
+                               case_row0=np.append(first, len(owner)))
+        for ic in range(n_cases):
+            metrics.setdefault(ic, {}).update(rotor_metrics(rotors, ic, rsd[ic], rps[ic], float(P["dw"])))
     out = dict(Xi_trains=[Xi[owner == ic] for ic in range(n_cases)], status=st[first], case_metrics=metrics)
     if F2nd is not None:
         n, nw = Xi.shape[1], Xi.shape[2]
@@ -1426,22 +1540,35 @@ class GeneralBatchSession:
                                                           A[d].data_ptr() if amp else None, stream))
         return sd, P, A
 
+    def rotor_stats(self, R, C_, V_w, gains, case_row0=None, psd=True):
+        """Rotor statistics of the last ``solve()`` for every design in one launch sequence (raftk_rotor_stats_dev on the
+        resident Xi [nD, nT, nDOF, nw]): ``R`` [nD, nrot, nDOF] (each design's hub rows) or [nrot, nDOF]; ``C``, ``V_w``,
+        ``gains`` for every design ([nC, nrot, ...]) or per design ([nD, nC, nrot, ...]); ``case_row0`` as ``rotor_stats``.
+        -> (std [nD, nC, nrot, 3], PSD [nD, nC, nrot, 3, nw] or None), torch tensors."""
+        stream = self.torch.cuda.current_stream(self.device).cuda_stream
+        sd, P, self._rot_keep = _rotor_stats_dev(self.torch, self.device, stream, self.Xi, self.keep["w"], R, C_, V_w, gains,
+                                                 self.dw, case_row0, None, psd)
+        return sd, P
 
-def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, qtf=None):
+
+def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, qtf=None, rotors=None):
     """``general_analyze_cases`` for every design of a batch in one solve: ``designs`` a list of per-design inputs (or a
     ``GeneralBatch`` built from them), ``cases`` a list of case dicts run by every design, ``channels`` None or one
-    ``packer.pack_general_channels`` dict per design -> a list with, for each design, what ``general_analyze_cases`` returns
-    for that design alone."""
+    ``packer.pack_general_channels`` dict per design, ``rotors`` None or one ``packer.pack_rotor_outputs`` dict per design
+    -> a list with, for each design, what ``general_analyze_cases`` returns for that design alone."""
     from .packer import pack_case_trains
     bt = _as_batch(designs, qtf)
     if channels is not None and len(channels) != bt.n_designs:
         raise ValueError("channels: one entry per design (%d), got %d" % (bt.n_designs, len(channels)))
+    if rotors is not None and len(rotors) != bt.n_designs:
+        raise ValueError("rotors: one entry per design (%d), got %d" % (bt.n_designs, len(rotors)))
     table, owner, first = pack_case_trains(cases)
     q = bt.qtf is not None
     res = general_solve_dynamics_batch(bt, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start, F_2nd=q)
     P = dict(w=bt.arrays["w"], dw=bt.dw)
     return [_general_case_results(P, res[0][d], res[1][d], owner, first, len(cases), None if channels is None else channels[d],
-                                  (res[2][d], res[3][d]) if q else None) for d in range(bt.n_designs)]
+                                  (res[2][d], res[3][d]) if q else None, None if rotors is None else rotors[d])
+            for d in range(bt.n_designs)]
 
 
 def second_order_force(batch, cases):
@@ -1833,6 +1960,27 @@ class DeviceSession:
         if n_fowt is None:
             sd, P, A = sd[0], (P[0] if psd else None), (A[0] if amp else None)
         return sd, P, A
+
+    def rotor_stats(self, R, C_, V_w, gains, dw, case_row0=None, col0=None, psd=True, farm=False, n_fowt=None):
+        """Enqueue rotor speed, generator torque and blade pitch statistics on a resident response (raftk_rotor_stats_dev; no
+        host round trip).  ``farm=False``: the last ``solve``'s Xi [nD, nC, 6, nw], one unit per design; ``farm=True``: the
+        Xi_sys of the LAST ``farm_response`` of the form ``n_fowt`` names (as ``farm_channel_stats``), one unit per farm, FOWT
+        i's hub rows at ``col0`` = 6 i.  ``R``, ``C``, ``V_w``, ``gains``, ``case_row0``, ``col0`` as ``rotor_stats`` (numpy or
+        torch).  -> (std [nU, nCases, nrot, 3], PSD [nU, nCases, nrot, 3, nw] or None) torch tensors, without the unit axis
+        for one farm (``farm=True``, ``n_fowt=None``)."""
+        if farm:
+            key = "_farm" if n_fowt is None else "_farm_batch"
+            if not hasattr(self, key):
+                raise RuntimeError("rotor_stats: call farm_response(n_fowt=%r) first" % (n_fowt,))
+            xi = getattr(self, key)[2]
+            xi = xi[None] if n_fowt is None else xi
+        else:
+            xi = self.out["Xi"]
+        sd, P, self._rot_keep = _rotor_stats_dev(self.torch, self.device, self._stream(), xi, self.dt["w"], R, C_, V_w, gains, dw,
+                                                 case_row0, col0, psd)
+        if farm and n_fowt is None:
+            sd, P = sd[0], (P[0] if psd else None)
+        return sd, P
 
     def eigen(self, A0=None, yawstiff=0.0, sort="dof", modes=True):
         """Natural frequencies and mode shapes of every design on the device, on torch's current stream (async):
