@@ -786,7 +786,7 @@ int raftk_rotor_stats_host(int32_t n_units, int32_t n_rows, int32_t n_dof, int32
  * sort RAFTK_EIG_SORT_ASCENDING: by real part, then imaginary part (np.argsort of complex values); ties keep LAPACK's order.
  * Kernels: n <= 12 one system per thread (k_eig_small, no workspace); n > 12 one system per CTA (k_eig_cta), persistent CTAs
  * with Q and the back-substitution in a per-CTA workspace slab, H in shared memory while it fits the opt-in limit (n up to
- * about 165 on an H100) and in the slab beyond.  A system's outputs do not depend on the batch or the workspace size.
+ * 167 on an H100) and in the slab beyond.  A system's outputs do not depend on the batch or the workspace size.
  * info flags per system: RAFTK_EIG_SMALL_DIAG a diagonal of M or C below 1 (the reference's viability check, on the inputs);
  * RAFTK_EIG_NONPOSITIVE an eigenvalue with real part <= 0; RAFTK_EIG_COMPLEX a complex eigenvalue (informational);
  * RAFTK_EIG_SINGULAR an exactly zero pivot of M; RAFTK_EIG_NOCONV the QR iteration did not converge.  The last two leave

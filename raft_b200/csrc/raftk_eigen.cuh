@@ -7,8 +7,10 @@
 //   3. Householder reduction to upper Hessenberg form, Q accumulated;
 //   4. Francis double-shift implicit QR to real Schur form T = Q^T A Q (deflation on small subdiagonals, exceptional shifts
 //      every 10th iteration, 2x2 blocks standardised), at most 30 n iterations in total;
-//   5. eigenvectors of T by back-substitution (real eigenvalues and complex-conjugate pairs), back-transformed with Q,
-//      un-balanced, scaled to unit 2-norm; a complex vector is rotated so that its largest component is real;
+//   5. eigenvectors of T by back-substitution (real eigenvalues and complex-conjugate pairs; the partial vector rescaled by a
+//      power of two before a step could grow it past 2^400, as LAPACK's dtrevc rescales), back-transformed with Q,
+//      un-balanced, scaled to unit 2-norm (the norm recomputed with max-abs scaling when the sum of squares leaves
+//      [2^-900, 2^900]); a complex vector is rotated so that its largest component is real;
 //   6. the output order: ascending (real part, then imaginary part; stable) or the DOF claim of the reference.
 // The storage of one system is a set of accessors (EigSys) and the work is written as loops over `tid += nt` with sync()
 // between phases, so the same device functions run one system per thread (k_eig_small: nt = 1, sync a no-op, working set
@@ -54,6 +56,7 @@ struct EigSys {
 #define EIG_SFMAX1 (1.0 / EIG_SFMIN1)
 #define EIG_SFMIN2 (EIG_SFMIN1 * 2.0)
 #define EIG_SFMAX2 (1.0 / EIG_SFMIN2)
+#define EIG_GROW_LOG2 400                               // a back-substitution step keeps |quotient| * max(1, |column of T|) below 2^400 |pivot|
 
 // (i, j) over [r0, r1) x [c0, c1), shared by the threads of a system
 template <class S, class F> __device__ __forceinline__ void eig_par2(const S &s, int r0, int r1, int c0, int c1, F f)
@@ -498,7 +501,10 @@ __device__ inline void eig_solve2(double a00, double a01, double a10, double a11
     if (pc) { b0 = x1; b1 = x0; } else { b0 = x0; b1 = x1; }
 }
 
-// eigenvector of T for eigenvalue ki (real) or the pair (ki-1, ki) into X(:, ki) (real) or X(:, ki-1) + i X(:, ki), rows 0..ki
+// eigenvector of T for eigenvalue ki (real) or the pair (ki-1, ki) into X(:, ki) (real) or X(:, ki-1) + i X(:, ki), rows 0..ki.
+// w(j) holds the largest |T(k, j)|, k < j.  Dividing by a pivot near smin grows the partial vector by up to 1 / smin per step
+// (a Jordan block overflows after about 20 steps), so before a step whose quotient times max(1, w) could pass 2^400 |pivot| the
+// vector is scaled down by a power of two; the unit-norm scaling later makes the result independent of that scale.
 template <bool CPX, class S> __device__ void eig_trevc(const S &s, int ki)
 {
     const int n = s.n;
@@ -507,6 +513,12 @@ template <bool CPX, class S> __device__ void eig_trevc(const S &s, int ki)
     const double smin = fmax(EIG_ULP * (fabs(lam.r) + fabs(lam.i)), EIG_SAFMIN * ((double)n / EIG_ULP));
     auto get = [&](int k) -> EigC { return {s.X(k, kr), CPX ? s.X(k, ki) : 0.0}; };
     auto put = [&](int k, EigC v) { s.X(k, kr) = v.r; if (CPX) s.X(k, ki) = v.i; };
+    auto guard = [&](double xa, double g, double da) {     // rescale so that xa max(1, g) < 2^EIG_GROW_LOG2 da
+        g = fmax(1.0, g);
+        if (!(xa * g > scalbn(da, EIG_GROW_LOG2))) return;
+        const double f = scalbn(1.0, ilogb(da) + EIG_GROW_LOG2 - ilogb(xa) - ilogb(g) - 2);
+        for (int k = 0; k <= ki; k++) { s.X(k, kr) *= f; if (CPX) s.X(k, ki) *= f; }
+    };
     int top;
     if (CPX) {
         EigC a, b;
@@ -521,7 +533,8 @@ template <bool CPX, class S> __device__ void eig_trevc(const S &s, int ki)
         top = ki - 1;
     }
     for (int j = top; j >= 0;) {
-        if (j > 0 && s.H(j, j - 1) != 0.0) {                // 2x2 diagonal block (j-1, j)
+        if (j > 0 && s.H(j, j - 1) != 0.0) {                // 2x2 diagonal block (j-1, j): |x| <= 8 |b| / smin
+            guard(fmax(eig_cabs1(get(j - 1)), eig_cabs1(get(j))), fmax(s.w(j - 1), s.w(j)), 0.125 * smin);
             EigC b0 = get(j - 1), b1 = get(j);
             eig_solve2(s.H(j - 1, j - 1), s.H(j - 1, j), s.H(j, j - 1), s.H(j, j), lam, smin, b0, b1);
             put(j - 1, b0); put(j, b1);
@@ -533,6 +546,7 @@ template <bool CPX, class S> __device__ void eig_trevc(const S &s, int ki)
         } else {
             EigC d = {s.H(j, j) - lam.r, -lam.i};
             if (eig_cabs1(d) < smin) d = {smin, 0.0};
+            guard(eig_cabs1(get(j)), s.w(j), eig_cabs1(d));
             const EigC y = eig_cdiv(get(j), d);
             put(j, y);
             for (int k = 0; k < j; k++) {
@@ -549,6 +563,12 @@ template <bool CPX, class S> __device__ void eig_trevc(const S &s, int ki)
 template <class S> __device__ void eig_vectors(const S &s)
 {
     const int n = s.n;
+    for (int j = s.tid; j < n; j += s.nt) {                 // the growth bound of each back-substitution step
+        double g = 0.0;
+        for (int k = 0; k < j; k++) g = fmax(g, fabs(s.H(k, j)));
+        s.w(j) = g;
+    }
+    s.sync();
     for (int k = s.tid; k < n; k += s.nt) {                 // one eigenvector (or pair) per thread
         if (s.wi(k) == 0.0) eig_trevc<false>(s, k);
         else if (s.wi(k) < 0.0) eig_trevc<true>(s, k);
@@ -575,12 +595,31 @@ template <class S> __device__ void eig_vectors(const S &s)
         if (s.wi(c) == 0.0) {
             double nn = 0.0;
             for (int r = 0; r < n; r++) nn += s.Q(r, c) * s.Q(r, c);
-            const double f = 1.0 / sqrt(nn);
+            double f = 1.0 / sqrt(nn);
+            if (!(nn >= 0x1p-900 && nn <= 0x1p+900)) {      // the sum of squares over- or underflows: scale by the largest entry
+                double amax = 0.0;
+                for (int r = 0; r < n; r++) amax = fmax(amax, fabs(s.Q(r, c)));
+                const int e = ilogb(amax);
+                double t = 0.0;
+                for (int r = 0; r < n; r++) { const double v = scalbn(s.Q(r, c), -e); t += v * v; }
+                f = scalbn(1.0 / sqrt(t), -e);
+            }
             for (int r = 0; r < n; r++) s.Q(r, c) *= f;
         } else if (s.wi(c) > 0.0) {
             double n0 = 0.0, n1 = 0.0;
             for (int r = 0; r < n; r++) { n0 += s.Q(r, c) * s.Q(r, c); n1 += s.Q(r, c + 1) * s.Q(r, c + 1); }
-            const double f = 1.0 / hypot(sqrt(n0), sqrt(n1));
+            double f = 1.0 / hypot(sqrt(n0), sqrt(n1));
+            if (!(n0 + n1 >= 0x1p-900 && n0 + n1 <= 0x1p+900)) {     // as for a real vector
+                double amax = 0.0;
+                for (int r = 0; r < n; r++) amax = fmax(amax, fmax(fabs(s.Q(r, c)), fabs(s.Q(r, c + 1))));
+                const int e = ilogb(amax);
+                double t = 0.0;
+                for (int r = 0; r < n; r++) {
+                    const double u = scalbn(s.Q(r, c), -e), v = scalbn(s.Q(r, c + 1), -e);
+                    t += u * u + v * v;
+                }
+                f = scalbn(1.0 / sqrt(t), -e);
+            }
             int kmax = 0;
             double best = -1.0;
             for (int r = 0; r < n; r++) {
