@@ -139,6 +139,20 @@ typedef struct raftk_cases {
     const double *Xi_init;   /* optional complex [nD,nC,6,nw]: start the fixed-point loop from this iterate instead of the
                                 constant opts.xi_start (the loop that continues after the slender-body QTF has been
                                 added, raft_model.py:1106-1131).  Fused solver only. */
+    const int32_t *op;       /* optional [nC]: operating point of every case (calcTurbineConstants(case), raft_fowt.py:1514-1586);
+                                NULL: none.  A secondary train must name its primary's operating point.  Unit (d, c) solves with
+                                M0 + (A_w + op_A_w[op[c]]) and B0 + B_drag + (B_w + op_B_w[op[c]]) (the design's and the operating
+                                point's tables summed first; a design without A_w takes the operating point's alone), so a call
+                                equals one call per operating point with that point's tables summed into A_w / B_w, bit for bit.
+                                Honoured by raftk_solve_dynamics_*, the farm entries and raftk_solve_dynamics_slender_*; refused
+                                by raftk_general_*; ignored by the entries that assemble no impedance (excitation, linearisation,
+                                second-order force).  The *_host entries refuse an index outside [0, n_op) and a secondary train
+                                whose point differs from its primary's; the *_dev entries check n_op, op_shared and the tables but
+                                do not read op back (no host synchronisation): its values must be valid. */
+    int32_t n_op;            /* operating points, >= 1 when op is given                                                   */
+    int32_t op_shared;       /* 0: tables per design [nD, n_op, 36, nw]; 1: one set for every design [n_op, 36, nw]       */
+    const double *op_A_w;    /* sum_r A_aero                  -- added to M0 + A_w                                         */
+    const double *op_B_w;    /* sum_r B_aero + sum_r B_gyro   -- added to B0 + B_w                                         */
 } raftk_cases;
 
 /* Fixed-point loop controls (raft_model.py:966 tol, :977 nIter, :978 XiStart, :1133 relaxation) */

@@ -39,6 +39,7 @@ class RaftkCases(C.Structure):
         ("n_cases", C.c_int32), ("_pad0", C.c_int32),
         ("Hs", C.c_void_p), ("Tp", C.c_void_p), ("gamma", C.c_void_p), ("beta_deg", C.c_void_p),
         ("spec", C.c_void_p), ("zeta", C.c_void_p), ("primary", C.c_void_p), ("F_2nd", C.c_void_p), ("Xi_init", C.c_void_p),
+        ("op", C.c_void_p), ("n_op", C.c_int32), ("op_shared", C.c_int32), ("op_A_w", C.c_void_p), ("op_B_w", C.c_void_p),
     ]
 
 

@@ -180,8 +180,39 @@ static CasesDev to_dev(const raftk_cases *c)
     CasesDev C;
     C.nC = c->n_cases; C.Hs = c->Hs; C.Tp = c->Tp; C.gamma = c->gamma; C.beta_deg = c->beta_deg;
     C.zeta_in = c->zeta; C.spec = c->spec; C.primary = c->primary; C.F_2nd = c->F_2nd;
+    C.op = c->op; C.n_op = c->n_op; C.op_shared = c->op_shared; C.op_A_w = c->op_A_w; C.op_B_w = c->op_B_w;
     return C;
 }
+
+// cases.op (operating points): the counts and tables, then -- when host copies are given -- every case's index and the
+// wave trains' agreement with their primaries.  Nothing is checked without op.
+static int validate_op(const raftk_cases *c, const int32_t *op_h, const int32_t *prim_h)
+{
+    if (!c || !c->op) return 0;
+    if (c->n_op < 1) return set_err(RAFTK_EINVAL, "cases.op: n_op must be >= 1");
+    if (c->op_shared != 0 && c->op_shared != 1) return set_err(RAFTK_EINVAL, "cases.op_shared must be 0 or 1");
+    if (!c->op_A_w || !c->op_B_w) return set_err(RAFTK_EINVAL, "cases.op needs op_A_w and op_B_w");
+    if (!op_h) return 0;
+    char m[160];
+    for (int i = 0; i < c->n_cases; i++)
+        if (op_h[i] < 0 || op_h[i] >= c->n_op) {
+            snprintf(m, sizeof(m), "cases.op[%d] = %d is outside [0, n_op = %d)", i, op_h[i], c->n_op);
+            return set_err(RAFTK_EINVAL, "%s", m);
+        }
+    if (prim_h)
+        for (int i = 0; i < c->n_cases; i++) {
+            const int p = prim_h[i];
+            if (p >= 0 && p < c->n_cases && op_h[p] != op_h[i]) {
+                snprintf(m, sizeof(m), "cases.op: secondary train %d names operating point %d, its primary %d names %d", i, op_h[i], p, op_h[p]);
+                return set_err(RAFTK_EINVAL, "%s", m);
+            }
+        }
+    return 0;
+}
+
+// validate_op for a *_dev entry: op and primary are device memory, which these entries do not read back (they run without a
+// host synchronisation); their values are the caller's to check (solver.CaseTable does, and the host entries do)
+static int validate_op_dev(const raftk_cases *c) { return validate_op(c, nullptr, nullptr); }
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
@@ -502,7 +533,7 @@ static int run_fused(const raftk_designs *d, const raftk_cases *c, const raftk_s
 // tests).  The grid variant runs when a unit spans several CTAs, every CTA of the launch can be resident at once, and the
 // hardware cannot place every unit's cluster at once (cudaOccupancyMaxActiveClusters < units): then the clusters that do not
 // fit would start only when the first units finish.  The occupancy queries are cached per device and launch shape.
-static SmemOptIn g_f2_opt_cluster, g_f2_opt_grid;
+static SmemOptIn g_f2_opt_cluster, g_f2_opt_grid, g_f2_opt_cluster_op, g_f2_opt_grid_op;
 struct F2Occ { int dev, units, CS; size_t smem; int clusters, resident; };
 static std::mutex g_f2_occ_mu;
 static std::vector<F2Occ> g_f2_occ;
@@ -566,7 +597,9 @@ static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_
     const int units = d->n_designs * c->n_cases;
     bool grid = false;
     if (int rc = f2_pick_grid(pl, units, grid)) return rc;
-    CUDA_TRY(grid ? g_f2_opt_grid.ensure(k_rao_fused2<true>, pl.smem) : g_f2_opt_cluster.ensure(k_rao_fused2<false>, pl.smem));
+    const bool op = c->op != nullptr;        // the instantiation with operating points (same registers and occupancy)
+    if (op) CUDA_TRY(grid ? g_f2_opt_grid_op.ensure(k_rao_fused2<true, true>, pl.smem) : g_f2_opt_cluster_op.ensure(k_rao_fused2<false, true>, pl.smem));
+    else CUDA_TRY(grid ? g_f2_opt_grid.ensure(k_rao_fused2<true>, pl.smem) : g_f2_opt_cluster.ensure(k_rao_fused2<false>, pl.smem));
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute at;
     cluster_config(cfg, at, (size_t)units * pl.CS, F2_T, pl.smem, pl.CS, st);
@@ -584,9 +617,9 @@ static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_
             ProfScope ps(st, 2);
             if (grid) {
                 CUDA_TRY(cudaMemsetAsync(P.xcnt, 0, (size_t)units * sizeof(unsigned), st));      // counters count up from 0 per launch
-                CUDA_TRY(cudaLaunchKernelEx(&cfg, k_rao_fused2<true>, D, C, P));
+                CUDA_TRY(op ? cudaLaunchKernelEx(&cfg, k_rao_fused2<true, true>, D, C, P) : cudaLaunchKernelEx(&cfg, k_rao_fused2<true>, D, C, P));
             } else {
-                CUDA_TRY(cudaLaunchKernelEx(&cfg, k_rao_fused2<false>, D, C, P));
+                CUDA_TRY(op ? cudaLaunchKernelEx(&cfg, k_rao_fused2<false, true>, D, C, P) : cudaLaunchKernelEx(&cfg, k_rao_fused2<false>, D, C, P));
             }
         }
         g_launches++;
@@ -758,6 +791,7 @@ extern "C" int raftk_solve_dynamics_dev(const raftk_designs *d, const raftk_case
 {
     disp_reset();
     if (!out || !out->Xi || !out->status || !o) return set_err(RAFTK_EINVAL, "Xi, status and opts are required");
+    if (int rc = validate_op_dev(c)) return rc;
     if (d && c && d->n_qtf_w > 0 && !c->F_2nd) {          // potSecOrder 2: the solve computes the force itself (raft_model.py:1035-1038)
         if (!out->F_2nd) return set_err(RAFTK_EINVAL, "designs carry a QTF: pass outputs.F_2nd as the buffer, or cases.F_2nd precomputed");
         int rc = run_qtf(d, c, out->F_2nd, out->F_2nd_mean, (cudaStream_t)stream);
@@ -827,6 +861,7 @@ extern "C" int raftk_solve_dynamics_gather_dev(const raftk_designs *d, const raf
     if (out->Xi != peers->gathered[peers->rank] + 2 * (size_t)peers->rank * peers->block_elems)
         return set_err(RAFTK_EINVAL, "outputs.Xi must be this rank's block of its own gathered array");
     if (d->n_qtf_w > 0 && !c->F_2nd) return set_err(RAFTK_EINVAL, "gather solve: pass cases.F_2nd precomputed (raftk_second_order_force_dev)");
+    if ((rc = validate_op_dev(c))) return rc;
     return solve(d, c, o, out, workspace, workspace_bytes, (cudaStream_t)stream, peers);
 }
 
@@ -993,13 +1028,15 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
                                          "(raftk_farm_workspace_bytes, raftk_farm_response_ws_dev)");
         const long long nsys = (long long)f->n_farms * c->n_cases * d->nw;
         const int grid = (int)std::min<long long>(std::min<long long>(nsys, (long long)(ws_bytes / slab)), (long long)g.per_sm * sm_count());
-        static SmemOptIn opt_g(0);
-        CUDA_TRY(opt_g.ensure(k_farm_response_global, g.smem));
+        static SmemOptIn opt_g(0), opt_go(0);
+        const bool op = c->op != nullptr;                   // the instantiations with operating points
+        CUDA_TRY(op ? opt_go.ensure(k_farm_response_global<true>, g.smem) : opt_g.ensure(k_farm_response_global<false>, g.smem));
         DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
         CasesDev C = to_dev(c);
         {
             ProfScope ps(st, 1);
-            k_farm_response_global<<<grid, GLU_T, g.smem, st>>>(D, C, P, static_cast<double2 *>(ws), g.pw);
+            if (op) k_farm_response_global<true><<<grid, GLU_T, g.smem, st>>>(D, C, P, static_cast<double2 *>(ws), g.pw);
+            else k_farm_response_global<false><<<grid, GLU_T, g.smem, st>>>(D, C, P, static_cast<double2 *>(ws), g.pw);
             disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_GLOBAL, GLU_T);
         }
         g_launches++;
@@ -1013,9 +1050,10 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
     // grid = (frequency groups, case, farm): the y and z extents of a grid end at 65535
     if (c->n_cases > 65535) return set_err(RAFTK_EINVAL, "farm response: more than 65535 cases per call");
     if (f->n_farms > 65535) return set_err(RAFTK_EINVAL, "farm response: more than 65535 farms per call with the system in shared memory (6N <= 120)");
-    static SmemOptIn opt_w(48 * 1024), opt_b(48 * 1024);
-    if (warp) CUDA_TRY(opt_w.ensure(k_farm_response<true>, smem));
-    else CUDA_TRY(opt_b.ensure(k_farm_response<false>, smem));
+    static SmemOptIn opt_w(48 * 1024), opt_b(48 * 1024), opt_wo(48 * 1024), opt_bo(48 * 1024);
+    const bool op = c->op != nullptr;                       // the instantiations with operating points
+    if (warp) CUDA_TRY(op ? opt_wo.ensure(k_farm_response<true, true>, smem) : opt_w.ensure(k_farm_response<true>, smem));
+    else CUDA_TRY(op ? opt_bo.ensure(k_farm_response<false, true>, smem) : opt_b.ensure(k_farm_response<false>, smem));
     DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
     CasesDev C = to_dev(c);
     {
@@ -1025,9 +1063,10 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
         // registers, so those stay on the warp kernel.
         const bool rows = n == 12 && !getenv("RAFTK_FARM_SMEM");
         const unsigned gy = c->n_cases, gz = f->n_farms;
-        if (rows) k_farm_rows<12><<<dim3((d->nw + 7) / 8, gy, gz), 128, 0, st>>>(D, C, P);
-        else if (warp) k_farm_response<true><<<dim3((d->nw + wpc - 1) / wpc, gy, gz), 32 * wpc, smem, st>>>(D, C, P);
-        else k_farm_response<false><<<dim3(d->nw, gy, gz), 256, smem, st>>>(D, C, P);
+        const dim3 gr((d->nw + 7) / 8, gy, gz), gw((d->nw + wpc - 1) / wpc, gy, gz), gb(d->nw, gy, gz);
+        if (rows) { if (op) k_farm_rows<12, true><<<gr, 128, 0, st>>>(D, C, P); else k_farm_rows<12><<<gr, 128, 0, st>>>(D, C, P); }
+        else if (warp) { if (op) k_farm_response<true, true><<<gw, 32 * wpc, smem, st>>>(D, C, P); else k_farm_response<true><<<gw, 32 * wpc, smem, st>>>(D, C, P); }
+        else { if (op) k_farm_response<false, true><<<gb, 256, smem, st>>>(D, C, P); else k_farm_response<false><<<gb, 256, smem, st>>>(D, C, P); }
         if (rows) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_ROWS12, 128);
         else if (warp) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_WARP, 32 * wpc);
         else disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_BLOCK, 256);
@@ -1052,6 +1091,7 @@ extern "C" int raftk_farm_response_dev(const raftk_designs *d, const raftk_cases
                                        void *stream)
 {
     disp_reset();
+    if (int rc = validate_op_dev(c)) return rc;
     return farm_launch_one(d, c, solved, f, nullptr, 0, (cudaStream_t)stream);
 }
 
@@ -1059,6 +1099,7 @@ extern "C" int raftk_farm_response_ws_dev(const raftk_designs *d, const raftk_ca
                                           void *workspace, size_t workspace_bytes, void *stream)
 {
     disp_reset();
+    if (int rc = validate_op_dev(c)) return rc;
     return farm_launch_one(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
@@ -1066,6 +1107,7 @@ extern "C" int raftk_farm_batch_response_ws_dev(const raftk_designs *d, const ra
                                                 const raftk_farm_batch *f, void *workspace, size_t workspace_bytes, void *stream)
 {
     disp_reset();
+    if (int rc = validate_op_dev(c)) return rc;
     return farm_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
@@ -1255,6 +1297,11 @@ static void stage_designs_cases(Staging &S, const raftk_designs *d, const raftk_
     S.in(cc.primary, c->primary, nC);
     S.in(cc.F_2nd, c->F_2nd, nR / 2);
     S.in(cc.Xi_init, c->Xi_init, nR);
+    if (c->op) {
+        S.in(cc.op, c->op, nC);
+        const size_t nT = (c->op_shared ? 1 : nD) * (size_t)c->n_op * 36 * nw;
+        S.in(cc.op_A_w, c->op_A_w, nT); S.in(cc.op_B_w, c->op_B_w, nT);
+    }
     if (d->n_qtf_w > 0) {
         S.in(dd.qtf_w, d->qtf_w, (size_t)d->n_qtf_w);
         S.in(dd.qtf_heads, d->qtf_heads, (size_t)d->n_qtf_head);
@@ -1269,6 +1316,10 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
     int rc = validate(d, c);
     if (rc) return rc;
     if (!out) return set_err(RAFTK_EINVAL, "null outputs");
+    raftk_cases cin = *c;
+    if (mode != 0) cin.op = nullptr;                      // excitation and linearisation assemble no impedance
+    else if ((rc = validate_op(c, c->op, c->primary))) return rc;
+    c = &cin;
     Staging S(who);
     const size_t nD = d->n_designs, nw = d->nw, nC = c->n_cases;
     const size_t nR = nD * nC * 6 * nw * 2;             // doubles of one complex [nD,nC,6,nw] array
@@ -1393,7 +1444,7 @@ extern "C" int raftk_second_order_force_host(const raftk_designs *d, const raftk
     raftk_cases cc = *c;
     S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC); S.in(cc.beta_deg, c->beta_deg, nC);
     S.in(cc.spec, c->spec, nC); S.in(cc.zeta, c->zeta, nC * nw);
-    cc.primary = nullptr; cc.F_2nd = nullptr;
+    cc.primary = nullptr; cc.F_2nd = nullptr; cc.op = nullptr;
     double *F2, *F2mean;
     S.out(F2, nF, out->F_2nd); S.out(F2mean, nF / nw, out->F_2nd_mean);
     if ((rc = S.commit()) || (rc = run_qtf(&dd, &cc, F2, F2mean, 0))) return rc;
@@ -1482,6 +1533,7 @@ static int gen_validate(const raftk_general *g, const raftk_general_fd *fd, cons
         return set_err(RAFTK_EINVAL, max_cases == 65535 ? "general solve: 0 < n_dof <= 256, nw > 0, 0 < n_cases <= 65535"
                                                         : "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
     if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
+    if (c->op) return set_err(RAFTK_EINVAL, "general solve: cases.op (per-case operating points) is not supported for generalised-DOF FOWTs");
     if (qtf) {                                         // the frequency and heading vectors are read back for the checks
         if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
         std::vector<double> qw(qtf->n_qtf_w), qh(qtf->n_qtf_head);
@@ -1679,6 +1731,7 @@ extern "C" int raftk_general_solve_dynamics_qtf_host(const raftk_general *g, con
     disp_reset();
     if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
     if (g->n_dof <= 0 || g->nw <= 0 || c->n_cases <= 0) return set_err(RAFTK_EINVAL, "general solve: empty problem");
+    if (c->op) return set_err(RAFTK_EINVAL, "general solve: cases.op (per-case operating points) is not supported for generalised-DOF FOWTs");
     const size_t n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases;
     if (c->primary)
         for (size_t i = 0; i < nC; i++) {
@@ -1867,6 +1920,7 @@ extern "C" int raftk_general_solve_dynamics_stream_host(const raftk_general *g, 
     if (max_chunk_cases < 0) return set_err(RAFTK_EINVAL, "general stream: max_chunk_cases must be >= 0 (0: all cases)");
     if (g->n_dof > 256 || g->n_nodes < 0) return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
     if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
+    if (c->op) return set_err(RAFTK_EINVAL, "general solve: cases.op (per-case operating points) is not supported for generalised-DOF FOWTs");
     const size_t n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases, K = gen_chunk_cap(c->n_cases, max_chunk_cases);
     if (K > 65535) return set_err(RAFTK_EINVAL, "general stream: a chunk takes at most 65535 cases (max_chunk_cases)");
     std::vector<size_t> starts;                        // the plan's checks, before anything is staged
@@ -1932,6 +1986,7 @@ static int gen_batch_counts(const raftk_general *g, const raftk_general_batch *b
         return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
     if ((int64_t)b->n_designs * c->n_cases > INT32_MAX) return set_err(RAFTK_EINVAL, "general batch: n_designs * n_cases must stay below 2^31");
     if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
+    if (c->op) return set_err(RAFTK_EINVAL, "general solve: cases.op (per-case operating points) is not supported for generalised-DOF FOWTs");
     if (max_chunk_units < 0) return set_err(RAFTK_EINVAL, "general batch: max_chunk_units must be >= 0 (0: all units)");
     if (gen_chunk_cap((int64_t)b->n_designs * c->n_cases, max_chunk_units) > 65535)
         return set_err(RAFTK_EINVAL, "general batch: a chunk takes at most 65535 units (max_chunk_units)");
@@ -2248,6 +2303,7 @@ extern "C" int raftk_solve_dynamics_slender_dev(const raftk_designs *d, const ra
     if (o->n_iter < 1) return set_err(RAFTK_EINVAL, "slender flow: potSecOrder 1 needs n_iter >= 1");
     const int qtf_chunk = so ? so->qtf_chunk : 0;
     if (int rc = validate_slender_flow(d, s, c, qtf_chunk)) return rc;
+    if (int rc = validate_op_dev(c)) return rc;
     const int nD = d->n_designs, nC = c->n_cases, nw = d->nw, nw2 = s->cols.nw, units = nD * nC;
     const SlenderWs L = slender_ws(d, s, nC, qtf_chunk);
     if (!workspace || workspace_bytes < L.total) return set_err(RAFTK_ENOMEM, "slender flow: workspace smaller than raftk_solve_dynamics_slender_workspace_bytes()");
@@ -2335,6 +2391,7 @@ extern "C" int raftk_solve_dynamics_slender_host(const raftk_designs *d, const r
     if (o->n_iter < 1) return set_err(RAFTK_EINVAL, "slender flow: potSecOrder 1 needs n_iter >= 1");
     const int qtf_chunk = so ? so->qtf_chunk : 0;
     if (int rc = validate_slender_flow(d, s, c, qtf_chunk)) return rc;
+    if (int rc = validate_op(c, c->op, nullptr)) return rc;
     Staging S("raftk_solve_dynamics_slender_host");
     raftk_designs dd = *d;
     raftk_cases cc = *c;

@@ -34,7 +34,45 @@ struct CasesDev {
     const int *spec;
     const int *primary;     // [nC] or NULL: case whose drag linearisation this case reuses (secondary wave trains)
     const double *F_2nd;    // [nD][nC][6][nw] real second-order force amplitudes added to F_BEM + F_iner, or NULL
+    const int *op;          // [nC] operating point of every case, or NULL (raftk_cases.op)
+    int n_op, op_shared;
+    const double *op_A_w, *op_B_w;   // [nD or 1][n_op][36][nw]
 };
+
+// The operating-point table `tab` (op_A_w or op_B_w) of unit (design d, case c), or NULL without operating points.
+__device__ __forceinline__ const double *op_table(const CasesDev &Cs, const double *tab, size_t d, int c, int nw)
+{
+    return Cs.op ? tab + ((Cs.op_shared ? 0 : d * Cs.n_op) + (size_t)Cs.op[c]) * 36 * nw : nullptr;
+}
+
+// Frequency-dependent term at table offset e: the design's (dt) plus the operating point's (ot), summed before either meets
+// M0 / B0, so that a call with operating points equals one with the point's tables summed into A_w / B_w, bit for bit.
+// At least one of dt, ot is non-NULL.
+__device__ __forceinline__ double tab_term(const double *dt, const double *ot, size_t e)
+{
+    return ot ? (dt ? dt[e] + ot[e] : ot[e]) : dt[e];
+}
+
+// The fused solvers' impedance at bin i for a unit with an operating point (Ao, Bo; DESIGN: the design's Aw, Bw too), the
+// same arithmetic as their table branch with tab_term's sums: ar + i ai = C - w^2 (M + A) + i w (B + B_w).  Ms, Bs, Cm: the
+// unit's 6x6 mass, damping (drag included) and stiffness.  Kept apart from the table branch so that the solves without
+// operating points compile as before.
+template <bool DESIGN>
+__device__ __forceinline__ void op_impedance(double (&ar)[6][6], double (&ai)[6][6], const double *Ms, const double *Bs, const double *Cm,
+                                             const double *Aw, const double *Bw, const double *Ao, const double *Bo, int i, int nw,
+                                             double w, double w2)
+{
+#pragma unroll
+    for (int a = 0; a < 6; a++)
+#pragma unroll
+        for (int b = 0; b < 6; b++) {
+            const size_t e = (size_t)(6 * a + b) * nw + i;
+            const double M = Ms[6 * a + b] + (DESIGN ? Aw[e] + Ao[e] : Ao[e]);
+            const double B = Bs[6 * a + b] + (DESIGN ? Bw[e] + Bo[e] : Bo[e]);
+            ar[a][b] = fma(-w2, M, Cm[6 * a + b]);
+            ai[a][b] = w * B;
+        }
+}
 
 struct Work {          // workspace views for one chunk of designs [d0, d0+nDc)
     int d0, nDc;

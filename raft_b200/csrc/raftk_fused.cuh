@@ -595,7 +595,11 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
                 for (int a = 0; a < 6; a++) { br[a] += S.f0[(2 * a) * nwl + t]; bi[a] += S.f0[(2 * a + 1) * nwl + t]; }
             }
             const double w2 = w * w;
-            if (Aw) {                      // frequency-dependent added mass / damping tables (BEM, aero)
+            if (Cs.op) {                   // the case's operating point (per-case aero-servo terms) on top of the design's tables
+                const double *Ao = op_table(Cs, Cs.op_A_w, d, c, nw), *Bo = op_table(Cs, Cs.op_B_w, d, c, nw);
+                if (Aw) op_impedance<true>(ar, ai, S.mat, S.mat + 36, S.mat + 72, Aw, Bw, Ao, Bo, i, nw, w, w2);
+                else op_impedance<false>(ar, ai, S.mat, S.mat + 36, S.mat + 72, nullptr, nullptr, Ao, Bo, i, nw, w, w2);
+            } else if (Aw) {               // frequency-dependent added mass / damping tables (BEM, aero)
 #pragma unroll
                 for (int a = 0; a < 6; a++)
 #pragma unroll

@@ -301,7 +301,9 @@ __device__ __forceinline__ void f2_xchg_arrive_wait(unsigned *cnt, unsigned targ
 // same rows go through the L2-resident workspace (P.xrow, P.xcnt), summed in the same rank order, so the results are
 // bit-identical.  The grid variant lets the hardware place the CTAs freely: on an H100, 64 4-CTA clusters of this kernel
 // do not all fit at once (cudaOccupancyMaxActiveClusters = 62) while its 256 CTAs do.
-template <bool GRID>
+// OP: the case table carries operating points (cases.op); a separate instantiation, so that the solves without them compile
+// exactly as before (this kernel is at the register cap: any term in its per-bin assembly costs spill).
+template <bool GRID, bool OP = false>
 __global__ void __launch_bounds__(F2_T, 2)
 k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
 {
@@ -889,7 +891,12 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
             for (int a = 0; a < 6; a++) { const double2 f = P.F0g[ogl + (size_t)a * nw + i]; br[a] += f.x; bi[a] += f.y; }
             double ar[6][6], ai[6][6];
             const double w2 = w * w;
-            if (Aw) {
+            if (OP) {
+                // the unit's operating-point tables, formed here from the parameters (held across the pass loop they cost spill)
+                const double *Ao = op_table(Cs, Cs.op_A_w, d, c, nw), *Bo = op_table(Cs, Cs.op_B_w, d, c, nw);
+                if (Aw) op_impedance<true>(ar, ai, s_mat, s_bmat, s_mat + 72, Aw, Bw, Ao, Bo, i, nw, w, w2);
+                else op_impedance<false>(ar, ai, s_mat, s_bmat, s_mat + 72, nullptr, nullptr, Ao, Bo, i, nw, w, w2);
+            } else if (Aw) {
 #pragma unroll
                 for (int a = 0; a < 6; a++)
 #pragma unroll

@@ -195,8 +195,22 @@ struct FarmParams {
 };
 #define FARM_WPC 4
 
+// The frequency-dependent terms of design i's block entry e at bin iw for a case c with an operating point: the design's
+// A_w / B_w plus the operating point's (tab_term), added to M and B.  (A secondary train's operating point is its primary's:
+// raftk_cases.op.)
+__device__ __forceinline__ void farm_op_terms(const DesignsDev &D, const CasesDev &Cs, size_t i, int c, int e, int iw, double &M, double &B)
+{
+    const size_t nw = D.nw, o = (size_t)e * nw + iw;
+    const double *Aw = D.A_w ? D.A_w + i * 36 * nw : nullptr, *Bw = D.B_w ? D.B_w + i * 36 * nw : nullptr;
+    M += tab_term(Aw, op_table(Cs, Cs.op_A_w, i, c, (int)nw), o);
+    B += tab_term(Bw, op_table(Cs, Cs.op_B_w, i, c, (int)nw), o);
+}
+
 // Assembly of one (farm, case c, frequency iw) system, shared by k_farm_response and k_farm_response_global: Z_sys into
 // A [n][nc] (nc = n + 1) and the right-hand side into its column n, spread over the gsize threads of a group.
+// OP: the case table carries operating points (cases.op) -- the farm kernels take it in instantiations of their own, so that
+// the calls without them compile as before.
+template <bool OP>
 __device__ __forceinline__ void farm_assemble(const DesignsDev &D, const CasesDev &Cs, const FarmParams &P, int farm, int c, int iw, double2 *A,
                                               int gtid, int gsize)
 {
@@ -211,7 +225,8 @@ __device__ __forceinline__ void farm_assemble(const DesignsDev &D, const CasesDe
         if (a / 6 == j) {
             const int e = 6 * (a % 6) + (b - 6 * j);
             double M = D.M0[(size_t)i * 36 + e], B = D.B0[(size_t)i * 36 + e] + P.B_drag[((size_t)i * P.nC + cp) * 36 + e];
-            if (D.A_w) { M += D.A_w[((size_t)i * 36 + e) * nw + iw]; B += D.B_w[((size_t)i * 36 + e) * nw + iw]; }
+            if (OP) farm_op_terms(D, Cs, i, c, e, iw, M, B);
+            else if (D.A_w) { M += D.A_w[((size_t)i * 36 + e) * nw + iw]; B += D.B_w[((size_t)i * 36 + e) * nw + iw]; }
             zr = fma(-w2, M, D.C0[(size_t)i * 36 + e]);
             zi = w * B;
         }
@@ -232,7 +247,7 @@ __device__ __forceinline__ void farm_assemble(const DesignsDev &D, const CasesDe
     }
 }
 
-template <bool WARP>
+template <bool WARP, bool OP = false>
 __global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(DesignsDev D, CasesDev Cs, FarmParams P)
 {
     extern __shared__ __align__(16) double smem_raw[];
@@ -245,7 +260,7 @@ __global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(De
     if (iw >= nw) return;                                            // (warp-uniform; no CTA-wide barrier follows in the WARP variant)
     double2 *A = reinterpret_cast<double2 *>(smem_raw) + (size_t)g * n * nc;
     const size_t u = (size_t)f * P.nC + c;                           // row of Xi and info
-    farm_assemble(D, Cs, P, f, c, iw, A, gtid, gsize);
+    farm_assemble<OP>(D, Cs, P, f, c, iw, A, gtid, gsize);
     if (gtid == 0) bad_s[g] = 0;
     gsync<WARP>();
     if (WARP) lu_unblocked<true>(A, n, nc, 1, gtid, gsize, &piv_s[g], &rinv_s[g], &bad_s[g]);
@@ -398,6 +413,7 @@ __device__ __forceinline__ void lu_global(double2 *A, int lda, double2 *B, int l
 
 // farm system response of k_farm_response (same assembly) for any N: persistent CTAs, CTA b owns slab b of the workspace
 // ([6N][6N+1] double2) and solves the (farm, case, frequency) systems b, b + gridDim.x, ... of the nF * nC * nw in all
+template <bool OP = false>
 __global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D, CasesDev Cs, FarmParams P, double2 *ws, int pw)
 {
     extern __shared__ __align__(16) double smem_raw[];
@@ -409,7 +425,7 @@ __global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D,
     for (long long s = blockIdx.x; s < nsys; s += gridDim.x) {
         const long long u = s / nw;                                    // f * nC + c: row of Xi and info
         const int iw = (int)(s - u * nw), f = (int)(u / P.nC), c = (int)(u - (long long)f * P.nC);
-        farm_assemble(D, Cs, P, f, c, iw, A, threadIdx.x, GLU_T);
+        farm_assemble<OP>(D, Cs, P, f, c, iw, A, threadIdx.x, GLU_T);
         __syncthreads();
         lu_global(A, nc, A + n, nc, n, 1, pw, Ps, S);
         for (int a = threadIdx.x; a < n; a += GLU_T) P.Xi[((size_t)u * n + a) * nw + iw] = A[(size_t)a * nc + n];
@@ -440,7 +456,7 @@ __global__ void __launch_bounds__(GLU_T, 2) k_system_solve_global(int n, int nw,
 // entry moves the pivot row to everybody and old row k to the pivot's lane, every row below k eliminates itself.  No shared
 // memory, no barriers; back substitution broadcasts one unknown per step.  Same assembly arithmetic as k_farm_response.
 // ------------------------------------------------------------------------------------------------
-template <int N6>
+template <int N6, bool OP = false>
 __global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, FarmParams P)
 {
     constexpr int LPS = N6 <= 16 ? 16 : 32, SPW = 32 / LPS, NC = N6 + 1;
@@ -462,7 +478,8 @@ __global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, Fa
         if (b / 6 == ib) {
             const int e = 6 * ea + (b - 6 * (b / 6));
             double M = D.M0[(size_t)i * 36 + e], B = D.B0[(size_t)i * 36 + e] + P.B_drag[((size_t)i * P.nC + cp) * 36 + e];
-            if (D.A_w) { M += D.A_w[((size_t)i * 36 + e) * nw + iw]; B += D.B_w[((size_t)i * 36 + e) * nw + iw]; }
+            if (OP) farm_op_terms(D, Cs, i, c, e, iw, M, B);
+            else if (D.A_w) { M += D.A_w[((size_t)i * 36 + e) * nw + iw]; B += D.B_w[((size_t)i * 36 + e) * nw + iw]; }
             zr = fma(-w2, M, D.C0[(size_t)i * 36 + e]);
             zi = w * B;
         }

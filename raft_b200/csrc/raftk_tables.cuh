@@ -510,6 +510,18 @@ k_drag_solve(DesignsDev D, CasesDev Cs, Work W, SolveParams P)
                 br[a] += f0.x; bi[a] += f0.y;
             }
             const double w2 = w * w;
+            if (Cs.op) {                // the case's operating point, summed with the design's table first (tab_term)
+                const double *Ao = op_table(Cs, Cs.op_A_w, d, c, nw), *Bo = op_table(Cs, Cs.op_B_w, d, c, nw);
+#pragma unroll
+                for (int a = 0; a < 6; a++)
+#pragma unroll
+                    for (int b = 0; b < 6; b++) {
+                        const double M = S.mat[6 * a + b] + tab_term(Aw, Ao, (size_t)(6 * a + b) * nw + i);
+                        const double B = S.mat[36 + 6 * a + b] + tab_term(Bw, Bo, (size_t)(6 * a + b) * nw + i);
+                        ar[a][b] = S.mat[72 + 6 * a + b] - w2 * M;
+                        ai[a][b] = w * B;
+                    }
+            } else {
 #pragma unroll
             for (int a = 0; a < 6; a++)
 #pragma unroll
@@ -520,6 +532,7 @@ k_drag_solve(DesignsDev D, CasesDev Cs, Work W, SolveParams P)
                     ar[a][b] = S.mat[72 + 6 * a + b] - w2 * M;
                     ai[a][b] = w * B;
                 }
+            }
             const bool ok = solve6(ar, ai, br, bi);
             if (!ok) nan_local |= RAFTK_FLAG_SINGULAR;
             // convergence test (raft_model.py:1103-1104) and relaxation (:1133)

@@ -14,7 +14,7 @@ from .fowt import FOWT
 
 class Model:
     def __init__(self, design, matrices=None, array_stiffness=None, channels=None, tension_jacobian=None, mean_tensions=None,
-                 array_tension_jacobian=None, array_mean_tensions=None, rotors=None):
+                 array_tension_jacobian=None, array_mean_tensions=None, rotors=None, turbine_constants=None):
         """``channels``: optional turbine output channels per FOWT (``packer.pack_turbine_channels`` dicts: nacelle
         accelerations, tower-base moment) -- the turbine itself is outside this path, its constants enter here.
         ``tension_jacobian`` [2L,6] / ``mean_tensions`` [2L] (one for every FOWT, or a list with None for a FOWT without its
@@ -24,7 +24,13 @@ class Model:
         ``rotors``: ``packer.pack_rotor_outputs`` of each FOWT for the cases ``analyzeCases`` will run (one dict for a single
         FOWT, a list with None for a FOWT without rotor outputs for an array): the rotors' control transfer functions, wind
         amplitudes, gains and operating points, standing in for Rotor.calcAero (CCBlade), as ``matrices`` stand in for the
-        turbine's constants."""
+        turbine's constants.
+        ``turbine_constants``: per FOWT a list with one snapshot per case of the case table (a list of such lists for an
+        array), each what the reference's calcTurbineConstants(case) leaves on the FOWT (a live FOWT or a dict with A_aero,
+        B_aero, B_gyro; ``packer.pack_operating_points``).  Every case is then solved with its own aero-servo added mass and
+        damping (raft_model.py:1005-1010, 1045-1046), on top of the case-independent ``matrices``; ``channels`` may then be
+        a per-case list of ``pack_turbine_channels`` dicts per FOWT, taken after each case's calcTurbineConstants, so that
+        Mbase's aero reaction and mean follow the case too."""
         s = design.setdefault("settings", {})
         min_freq, max_freq = float(s.get("min_freq", 0.01)), float(s.get("max_freq", 1.00))
         self.XiStart = float(s.get("XiStart", 0.1))
@@ -52,7 +58,15 @@ class Model:
         self.nDOF = 6 * self.nFOWT
         self.C_array = None if array_stiffness is None else np.array(array_stiffness, dtype=float)   # stands in for ms.getCoupledStiffnessA
         self.results = {}
+        if self.nFOWT == 1 and isinstance(channels, (list, tuple)) and len(channels) > 1:
+            channels = [channels]                                        # one FOWT's per-case list
         self.channels = list(channels) if isinstance(channels, (list, tuple)) else [channels] * self.nFOWT
+        tc = turbine_constants
+        if tc is not None and self.nFOWT == 1 and len(tc) and not isinstance(tc[0], (list, tuple)):
+            tc = [tc]                                                    # one FOWT's per-case list
+        if tc is not None and len(tc) != self.nFOWT:
+            raise ValueError("turbine_constants: one per-case list per FOWT (%d), got %d" % (self.nFOWT, len(tc)))
+        self.turbine_constants = None if tc is None else [list(t) for t in tc]
         per = lambda v: list(v) if isinstance(v, (list, tuple)) else [v] * self.nFOWT
         self.tensions = [None if J is None else packer.pack_mooring_tensions(dict(J=J, T0=T0))
                          for J, T0 in zip(per(tension_jacobian), per(mean_tensions))]
@@ -72,8 +86,11 @@ class Model:
 
     # raft_model.py:966-1302 -------------------------------------------------------------------------------
     def solveDynamics(self, case, tol=0.01, conv_plot=0, RAO_plot=0, display=0):
-        """Response amplitudes for one load case -> self.Xi [nWaves+1, nDOF, nw] (last row zero, as :1195)."""
-        out = self._solve_batch([case], tol)
+        """Response amplitudes for one load case -> self.Xi [nWaves+1, nDOF, nw] (last row zero, as :1195).  With
+        ``turbine_constants`` the case's operating point is that of case ``case['iCase']`` of the table."""
+        if self.turbine_constants is not None and "iCase" not in case:
+            raise ValueError("solveDynamics: with turbine_constants the case must name its row of the case table (case['iCase'])")
+        out = self._solve_batch([case], tol, icases=[int(case["iCase"])] if self.turbine_constants is not None else None)
         trains = out["Xi_trains"][0]                                      # [nWaves, nDOF, nw]
         Xi = np.zeros([len(trains) + 1, self.nDOF, self.nw], dtype=complex)
         Xi[:-1] = trains
@@ -110,8 +127,7 @@ class Model:
         Xi_units = out["Xi_all"].reshape(len(owner), self.nFOWT, 6, self.nw)                  # [nTrains, nFOWT, 6, nw]
         sd_t, psd_t = solver.response_stats(Xi_units, self.w[1] - self.w[0])
         names = ("surge", "sway", "heave", "roll", "pitch", "yaw")
-        ch_stats = [None if ch is None else solver.channel_stats(ch["coef"], Xi_units[:, i], self.w[1] - self.w[0])
-                    for i, ch in enumerate(self.channels)]                                     # (std [nT,nch], PSD [nT,nch,nw], -)
+        ch_stats = [None if ch is None else self._channel_stats(ch, Xi_units[:, i], owner, nC) for i, ch in enumerate(self.channels)]
         # line-end tensions T = J Xi (moorMod 0): a FOWT's lines on its PRP motions through channel_stats (J constant over w),
         # the array's lines on the coupled response through farm_channel_stats; PSDs divided by w[0] (raft_fowt.py:2370, 2399)
         w0 = float(self.w[0])
@@ -135,7 +151,7 @@ class Model:
                     ra[:-1] = Xi_units[idx, i, k_] * (57.29577951308232 if k_ >= 3 else 1.0)
                     m[nm + "_RA"] = ra
                 if ch_stats[i] is not None:                                                   # raft_fowt.py:2401-2444, 2504-2538
-                    ch = self.channels[i]
+                    ch = self.channels[i][ic] if isinstance(self.channels[i], (list, tuple)) else self.channels[i]
                     nrot = 1 + max(ir for _, ir in ch["names"])
                     sd_c, psd_c = solver.combine_trains(ch_stats[i][0], ch_stats[i][1], idx)
                     for k_, (nm, ir) in enumerate(ch["names"]):
@@ -156,6 +172,31 @@ class Model:
                 self.results["case_metrics"][ic]["array_mooring"] = solver.tension_metrics(self.array_tensions["T0"],
                                                                                            *solver.combine_trains(arr[0], arr[1], idx))
         return self.results
+
+    def _channel_stats(self, ch, Xi, owner, nC):
+        """Turbine channel statistics of one FOWT on its trains Xi [nT, 6, nw]: ``ch`` one pack_turbine_channels dict, or one
+        per case (each train then takes its case's coefficients) -> (std [nT, nch], PSD [nT, nch, nw])."""
+        dw = self.w[1] - self.w[0]
+        if not isinstance(ch, (list, tuple)):
+            return solver.channel_stats(ch["coef"], Xi, dw)[:2]
+        if len(ch) != nC:
+            raise ValueError("channels: a per-case list must hold one entry per case (%d), got %d" % (nC, len(ch)))
+        sd, P, _ = solver.channel_stats(np.stack([ch[c]["coef"] for c in owner]), Xi[:, None], dw)
+        return sd[:, 0], P[:, 0]
+
+    def _ops(self, icases, owner, n_table=None):
+        """The operating points of the trains (case ``icases[owner[t]]`` of the turbine constants) -> CaseTable ops, or None.
+        ``n_table``: the case table's length, which every FOWT's list must have (analyzeCases)."""
+        if self.turbine_constants is None:
+            return None
+        for i, tc in enumerate(self.turbine_constants):
+            if n_table is not None and len(tc) != n_table:
+                raise ValueError("turbine_constants: FOWT %d holds %d cases, the case table %d" % (i, len(tc), n_table))
+            bad = [ic for ic in icases if not 0 <= ic < len(tc)]
+            if bad:
+                raise ValueError("turbine_constants: FOWT %d holds %d cases, case %d asked for" % (i, len(tc), bad[0]))
+        P = packer.pack_operating_points([[tc[ic] for ic in icases] for tc in self.turbine_constants])
+        return dict(op=P["op"][owner], A_w=P["A_w"], B_w=P["B_w"])
 
     def _rotor_stats(self, cases, out, dw):
         """Rotor statistics of every FOWT's rotors in one device call on the (coupled) response Xi_all [nTrains, 6N, nw]:
@@ -203,9 +244,10 @@ class Model:
         self.results['eigen'] = {'frequencies': fns, 'modes': modes}
         return fns, modes
 
-    def _solve_batch(self, cases, tol):
+    def _solve_batch(self, cases, tol, icases=None):
         table, owner, first = packer.pack_case_trains(cases)
-        ct = solver.CaseTable(table)
+        ops = self._ops(list(range(len(cases))) if icases is None else icases, owner, len(cases) if icases is None else None)
+        ct = solver.CaseTable(table, ops=ops)
         nC = len(cases)
         packs = [f.pack() for f in self.fowtList]
         batch = solver.DesignBatch([{k: v for k, v in P.items() if not k.startswith("qs_")} for P in packs])
@@ -243,20 +285,29 @@ class Model:
             if "F_2nd" in o:
                 f.Fhydro_2nd[:] = o["F_2nd"][i, last]
                 f.Fhydro_2nd_mean[:] = o["F_2nd_mean"][i, last]
-            M = P["M0"][:, :, None] + (P["A_w"] if "A_w" in P else 0.0)
-            B = (P["B0"] + f.B_hydro_drag)[:, :, None] + (P["B_w"] if "B_w" in P else 0.0)
-            f.Z = -w ** 2 * M + 1j * w * B + P["C0"][:, :, None]             # raft_model.py:1086, 1155 (last case)
+            M = P["M0"][:, :, None] + self._tab(P, "A_w", ops, i, first[-1])
+            B = (P["B0"] + f.B_hydro_drag)[:, :, None] + self._tab(P, "B_w", ops, i, first[-1])
+            f.Z = -w ** 2 * M + 1j * w * B + P["C0"][:, :, None]             # raft_model.py:1086, 1155 (last case, its own aero)
         nT = ct.n_cases
         Xi_all = np.moveaxis(o["Xi"], 0, 1).reshape(nT, self.nDOF, self.nw)  # [nTrains, 6N, nw]
         if "Xi_sys" in o:
             Xi_all = o["Xi_sys"]                                            # coupled system response, computed on the device
         elif self.nFOWT > 1 and self.C_array is not None:
             # (slender-body QTF path) coupled system: Z_sys = blockdiag(Z_i) + C_array; F = Z_i Xi_i  (raft_model.py:1164-1216)
-            Xi_all = self._couple(o, nT)
+            Xi_all = self._couple(o, nT, ops)
         Xi_trains = [Xi_all[owner == ic] for ic in range(nC)]
         return dict(Xi=Xi_all[first], Xi_trains=Xi_trains, status=np.moveaxis(st, 0, 1), Xi_all=Xi_all, owner=owner, zeta=o["zeta"])
 
-    def _couple(self, o, nC):
+    @staticmethod
+    def _tab(P, name, ops, i, t):
+        """FOWT i's frequency-dependent A_w / B_w for train t: the design's plus the train's operating point (as the kernels
+        sum them), 0.0 without either."""
+        if ops is None:
+            return P[name] if name in P else 0.0
+        o = ops[name][i, ops["op"][t]]
+        return P[name] + o if name in P else o
+
+    def _couple(self, o, nC, ops=None):
         n, nw, w = self.nDOF, self.nw, self.w
         Xi = np.zeros([nC, n, nw], dtype=complex)
         packs = [f.pack() for f in self.fowtList]
@@ -264,8 +315,8 @@ class Model:
             Z = np.zeros([nw, n, n], dtype=complex)
             F = np.zeros([nw, n], dtype=complex)
             for i, P in enumerate(packs):
-                M = P["M0"][:, :, None] + (P["A_w"] if "A_w" in P else 0.0)
-                B = (P["B0"] + o["B_drag"][i, c])[:, :, None] + (P["B_w"] if "B_w" in P else 0.0)
+                M = P["M0"][:, :, None] + Model._tab(P, "A_w", ops, i, c)
+                B = (P["B0"] + o["B_drag"][i, c])[:, :, None] + Model._tab(P, "B_w", ops, i, c)
                 Zi = np.moveaxis(-w ** 2 * M + 1j * w * B + P["C0"][:, :, None], 2, 0)     # [nw,6,6]
                 Z[:, 6 * i:6 * i + 6, 6 * i:6 * i + 6] = Zi
                 Fi = o["F_BEM"][i, c] + o["F_iner"][i, c] + o["F_drag"][i, c]

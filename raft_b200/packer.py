@@ -179,6 +179,49 @@ def pack_matrices(fowt, nw):
     return out
 
 
+def pack_operating_points(states):
+    """Per-case aero-servo added mass and damping of FOWTs (raftk_cases.op, ``solver.CaseTable(ops=)``).
+
+    ``states[d][c]``: FOWT d right after the reference's ``calcTurbineConstants(case c)`` (raft_fowt.py:1514-1586) -- the live
+    FOWT or a dict with A_aero [6,6,nw,nrot], B_aero [6,6,nw,nrot] and B_gyro [6,6,nrot].  Its operating point is
+    A(w) = sum_r A_aero[:,:,w,r] and B(w) = sum_r B_aero[:,:,w,r] + sum_r B_gyro[:,:,r]: what that case adds to the FOWT's
+    mass and damping (raft_model.py:1045-1047).  Cases whose tables are bit-identical over every design share one point.
+    -> dict(op [nC] int32, A_w, B_w [nD, n_op, 6, 6, nw], n_op).  The design's own matrices (``pack_matrices``) must then
+    not carry these terms."""
+    get = lambda s, k: s[k] if isinstance(s, dict) else getattr(s, k)       # noqa: E731
+    nD = len(states)
+    nC = len(states[0]) if nD else 0
+    if nD < 1 or nC < 1 or any(len(row) != nC for row in states):
+        raise ValueError("states must hold one snapshot per case (the same count) for every design")
+    nw = None
+    tabs = []                                                       # [nC][nD] (A, B)
+    for c in range(nC):
+        row = []
+        for d in range(nD):
+            s = states[d][c]
+            n = get(s, "nDOF") if not isinstance(s, dict) and hasattr(s, "nDOF") else np.shape(get(s, "A_aero"))[0]
+            if n != 6:
+                raise NotImplementedError("operating points: only rigid 6-DOF FOWTs (flexible FOWTs, raftk_general_*, are a follow-up)")
+            A, B, G = (np.asarray(get(s, k), dtype=float) for k in ("A_aero", "B_aero", "B_gyro"))
+            nw = A.shape[2] if nw is None and A.ndim == 4 else nw
+            if A.ndim != 4 or A.shape[:2] != (6, 6) or B.shape != A.shape or A.shape[2] != nw or G.shape != (6, 6, A.shape[3]):
+                raise ValueError("operating point of design %d, case %d: A_aero / B_aero must be [6,6,%s,nrot] and B_gyro [6,6,nrot]"
+                                 % (d, c, nw))
+            row.append((np.sum(A, axis=3), np.sum(B, axis=3) + np.sum(G, axis=2)[:, :, None]))
+        tabs.append(row)
+    op = np.zeros(nC, dtype=np.int32)
+    seen, first = {}, []
+    for c, row in enumerate(tabs):
+        key = b"".join(np.ascontiguousarray(t).tobytes() for pair in row for t in pair)
+        if key not in seen:
+            seen[key] = len(first)
+            first.append(c)
+        op[c] = seen[key]
+    A_w = np.ascontiguousarray([[tabs[c][d][0] for c in first] for d in range(nD)])
+    B_w = np.ascontiguousarray([[tabs[c][d][1] for c in first] for d in range(nD)])
+    return dict(op=op, A_w=A_w, B_w=B_w, n_op=len(first))
+
+
 def pack_bem_excitation(fowt):
     """BEM excitation coefficient table for heading interpolation (raft_fowt.py:1796-1849).
 

@@ -242,9 +242,13 @@ class DesignBatch:
 class CaseTable:
     """SoA case table (``packer.pack_cases`` dict, or keyword arrays)."""
 
-    def __init__(self, cases, zeta=None, F_2nd=None, Xi_init=None):
+    def __init__(self, cases, zeta=None, F_2nd=None, Xi_init=None, ops=None):
         """``F_2nd``: optional real [nD,nC,6,nw] second-order force amplitudes added to the linear excitation.
-        ``Xi_init``: optional complex [nD,nC,6,nw] starting iterate of the fixed-point loop (instead of xi_start)."""
+        ``Xi_init``: optional complex [nD,nC,6,nw] starting iterate of the fixed-point loop (instead of xi_start).
+        ``ops``: optional operating points (``packer.pack_operating_points``): dict(op [nC] int, A_w, B_w) with tables
+        [nD, n_op, 6, 6, nw] per design or [n_op, 6, 6, nw] for one set every design shares -- the aero-servo added mass and
+        damping (B_gyro folded into B_w) that the reference's calcTurbineConstants(case) adds to case c's system matrices:
+        unit (d, c) solves with M0 + (A_w + ops.A_w[op[c]]) and B0 + B_drag + (B_w + ops.B_w[op[c]]) (raftk_cases.op)."""
         self.arrays = a = _Tables()
         for kname in ("Hs", "Tp", "gamma", "beta_deg"):
             a[kname] = np.ascontiguousarray(cases[kname], dtype=_F8)
@@ -263,6 +267,29 @@ class CaseTable:
             a["F_2nd"] = np.ascontiguousarray(F_2nd, dtype=_F8)
         if Xi_init is not None:
             a["Xi_init"] = np.ascontiguousarray(Xi_init, dtype=np.complex128)
+        self.ops, self.n_op, self.op_shared = None, 0, 0
+        if ops is not None:
+            op = np.ascontiguousarray(ops["op"], dtype=_I4)
+            A, B = (np.ascontiguousarray(ops[k], dtype=_F8) for k in ("A_w", "B_w"))
+            if op.shape != (self.n_cases,):
+                raise ValueError("ops['op'] must name one operating point per case (%d)" % self.n_cases)
+            if A.shape != B.shape or A.ndim not in (4, 5) or A.shape[-3:-1] != (6, 6):
+                raise ValueError("ops A_w / B_w must both be [nD, n_op, 6, 6, nw] or [n_op, 6, 6, nw]")
+            self.n_op, self.op_shared = int(A.shape[-4]), int(A.ndim == 4)
+            if np.any(op < 0) or np.any(op >= self.n_op):
+                raise ValueError("ops['op'] must lie in [0, %d)" % self.n_op)
+            if "primary" in a and np.any(op[a["primary"]] != op):
+                raise ValueError("a secondary wave train must share its primary's operating point")
+            a["op"], a["op_A_w"], a["op_B_w"] = op, A, B
+            self.ops = dict(op=op, A_w=A, B_w=B)
+
+    def check_ops(self, batch):
+        """Refuse operating-point tables whose design count or frequency grid is not ``batch``'s."""
+        if self.ops is None:
+            return
+        A = self.ops["A_w"]
+        if A.shape[-1] != batch.nw or (not self.op_shared and A.shape[0] != batch.n_designs):
+            raise ValueError("operating-point tables %s do not match %d designs x %d bins" % (list(A.shape), batch.n_designs, batch.nw))
 
     def input_bytes(self):
         return int(sum(v.nbytes for v in self.arrays.values()))
@@ -270,8 +297,9 @@ class CaseTable:
     def struct(self, ptr):
         s = RaftkCases()
         s.n_cases = self.n_cases
-        for name in ("Hs", "Tp", "gamma", "beta_deg", "spec", "zeta", "primary", "F_2nd", "Xi_init"):
+        for name in ("Hs", "Tp", "gamma", "beta_deg", "spec", "zeta", "primary", "F_2nd", "Xi_init", "op", "op_A_w", "op_B_w"):
             setattr(s, name, ptr(name) if name in self.arrays else None)
+        s.n_op, s.op_shared = self.n_op, self.op_shared
         return s
 
 
@@ -305,6 +333,7 @@ def solve_dynamics(batch, cases, n_iter=10, tol=0.01, xi_start=0.0, cluster_size
     """
     want = tuple(dict.fromkeys(tuple(want) + ("Xi", "status")))
     outs = out if out is not None else _alloc_outputs(batch.n_designs, cases.n_cases, batch.nw, want)
+    cases.check_ops(batch)
     d = _host_struct(batch)
     c = _host_struct(cases)
     o = RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), 0, 0)
@@ -346,6 +375,7 @@ def solve_dynamics_farm(batch, cases, C_arr=None, M_arr=None, B_arr=None, n_iter
     ``out``: caller-owned result arrays (e.g. page-locked ones from ``pinned_empty``: device-to-host copies then run at
     the link rate instead of through the driver's staging of pageable memory); missing ones are allocated."""
     N, nC, nw = batch.n_designs, cases.n_cases, batch.nw
+    cases.check_ops(batch)
     n = 6 * N
     want = tuple(dict.fromkeys(tuple(want) + ("Xi", "status")))
     outs = dict(out) if out is not None else {}
@@ -397,6 +427,7 @@ def solve_dynamics_farm_batch(batch, cases, n_fowt, C_arr=None, M_arr=None, B_ar
     every farm, or [F,6N,6N].  -> the per-FOWT output dict plus ``Xi_sys`` complex [F, nC, 6N, nw] and ``info`` [F, nC, nw];
     farm f's rows are what ``solve_dynamics_farm`` returns for that farm alone, bit for bit."""
     N, nC, nw = int(n_fowt), cases.n_cases, batch.nw
+    cases.check_ops(batch)
     if N < 1 or batch.n_designs % N:
         raise ValueError("n_fowt must divide the batch's %d designs" % batch.n_designs)
     F, n = batch.n_designs // N, 6 * N
@@ -558,7 +589,7 @@ def _slender_inputs(packed, cases):
     sb = SlenderBatch(packed)
     batch = DesignBatch([{k: v for k, v in P.items() if not k.startswith(("qtf", "qs_"))} for P in packed])
     base = {k: v for k, v in cases.arrays.items() if k not in ("F_2nd", "Xi_init")}
-    return batch, sb, CaseTable(base, zeta=base.get("zeta"))
+    return batch, sb, CaseTable(base, zeta=base.get("zeta"), ops=cases.ops)
 
 
 def _slender_shapes(nD, nC, nw, nw2):
@@ -682,7 +713,7 @@ def solve_dynamics_slender(packed, cases, n_iter=10, tol=0.01, xi_start=0.0, clu
     nD, nC, nw = batch.n_designs, cases.n_cases, batch.nw
     base = {k: v for k, v in cases.arrays.items() if k not in ("F_2nd", "Xi_init")}
     wantA = tuple(dict.fromkeys(tuple(want) + ("Xi", "status", "zeta", "Xi_last")))
-    A = solve_dynamics(batch, CaseTable(base, zeta=base.get("zeta")), n_iter=n_iter, tol=tol, xi_start=xi_start, cluster_size=cluster_size, want=wantA)
+    A = solve_dynamics(batch, CaseTable(base, zeta=base.get("zeta"), ops=cases.ops), n_iter=n_iter, tol=tol, xi_start=xi_start, cluster_size=cluster_size, want=wantA)
     qw = np.ascontiguousarray(packed[0]["qs_w"], dtype=_F8)
     beta_rad = cases.arrays["beta_deg"] * 0.017453292519943295
     qtf = np.zeros([nD, nC, len(qw), len(qw), 6], dtype=np.complex128)
@@ -700,7 +731,7 @@ def solve_dynamics_slender(packed, cases, n_iter=10, tol=0.01, xi_start=0.0, clu
     qb.arrays["qtf"] = np.ascontiguousarray(qtf.reshape(nD, nC, len(qw), len(qw), 1, 6))
     qb.n_qtf_w, qb.n_qtf_head, qb.qtf_shared = len(qw), 1, 2
     F2 = second_order_force(qb, CaseTable(base, zeta=base.get("zeta")))
-    B = solve_dynamics(batch, CaseTable(base, zeta=base.get("zeta"), F_2nd=F2["F_2nd"], Xi_init=A["Xi_last"]), n_iter=n_iter - 1, tol=tol,
+    B = solve_dynamics(batch, CaseTable(base, zeta=base.get("zeta"), F_2nd=F2["F_2nd"], Xi_init=A["Xi_last"], ops=cases.ops), n_iter=n_iter - 1, tol=tol,
                        xi_start=xi_start, cluster_size=cluster_size, want=wantA)
     ok = A["status"][:, :, 1] == 1                                                   # units whose first loop converged
     out = {}
@@ -1201,7 +1232,8 @@ def general_case_metrics(channels, std, psd, amp, idx, dw=None):
     return m
 
 
-def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, fd=None, qtf=None, rotors=None):
+def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, fd=None, qtf=None, rotors=None,
+                          turbine_constants=None):
     """Model.analyzeCases (dynamics and output statistics) for one FOWT with generalised degrees of freedom: ``cases`` a list
     of case dicts, scalar or list-valued wave keys (several wave trains); ``channels`` from ``packer.pack_general_channels``.
     -> dict(Xi_trains [per case: nTrains,nDOF,nw], status [nC,4] of train 0, case_metrics {case: saveTurbineOutputs entries},
@@ -1209,8 +1241,10 @@ def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01
     wave loads (``packer.pack_general_qtf``); the result then also holds, per case, the reference FOWT's ``Fhydro_2nd``
     (complex [nTrains,nDOF,nw]) and ``Fhydro_2nd_mean`` ([nTrains,nDOF]), zero from reduced DOF 6 up (raft_model.py:1034-1036).
     ``rotors``: ``packer.pack_rotor_outputs`` of the FOWT for these cases; every case's metrics then hold the rotor entries
-    (omega / torque / bPitch / power, wind_PSD; ``rotor_metrics``)."""
+    (omega / torque / bPitch / power, wind_PSD; ``rotor_metrics``).  ``turbine_constants`` (per-case operating points, as
+    ``Model(turbine_constants=)``) are not supported for generalised-DOF FOWTs: NotImplementedError."""
     from .packer import pack_case_trains
+    _no_general_ops(turbine_constants)
     table, owner, first = pack_case_trains(cases)
     q = bool(qtf)
     res = general_solve_dynamics(P, M, B, Cm, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start, fd=fd, qtf=qtf, F_2nd=q)
@@ -1551,12 +1585,21 @@ class GeneralBatchSession:
         return sd, P
 
 
-def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, qtf=None, rotors=None):
+def _no_general_ops(turbine_constants):
+    if turbine_constants is not None:
+        raise NotImplementedError("per-case turbine constants (operating points) are not supported for generalised-DOF FOWTs yet: "
+                                  "the rigid-body solve takes them (Model(turbine_constants=))")
+
+
+def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, qtf=None, rotors=None,
+                                turbine_constants=None):
     """``general_analyze_cases`` for every design of a batch in one solve: ``designs`` a list of per-design inputs (or a
     ``GeneralBatch`` built from them), ``cases`` a list of case dicts run by every design, ``channels`` None or one
     ``packer.pack_general_channels`` dict per design, ``rotors`` None or one ``packer.pack_rotor_outputs`` dict per design
-    -> a list with, for each design, what ``general_analyze_cases`` returns for that design alone."""
+    -> a list with, for each design, what ``general_analyze_cases`` returns for that design alone.  ``turbine_constants``:
+    NotImplementedError, as for ``general_analyze_cases``."""
     from .packer import pack_case_trains
+    _no_general_ops(turbine_constants)
     bt = _as_batch(designs, qtf)
     if channels is not None and len(channels) != bt.n_designs:
         raise ValueError("channels: one entry per design (%d), got %d" % (bt.n_designs, len(channels)))
@@ -1819,6 +1862,7 @@ class DeviceSession:
         self.torch = torch
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self.batch, self.cases = batch, cases
+        cases.check_ops(batch)
         with torch.cuda.device(self.device):
             # every input table (design + case columns) lives in ONE device block, 256-byte aligned slots: a caller that
             # refreshes the tables from the host (sweep.ShardedSolve.step_host) sends them with a single copy

@@ -370,6 +370,8 @@ def general_shards(primary, n_cases, world):
 def shard_case_table(cases, lo, hi):
     """Rows [lo, hi) of a ``solver.CaseTable`` as a table of their own (whole train groups: primaries rebased to lo)."""
     from . import solver
+    if cases.ops is not None:
+        raise NotImplementedError("per-case operating points (CaseTable ops) are not supported for generalised-DOF FOWTs")
     a = cases.arrays
     sub = {k: a[k][lo:hi] for k in ("Hs", "Tp", "gamma", "beta_deg", "spec")}
     if "primary" in a:
@@ -399,6 +401,8 @@ class ShardedGeneralSolve:
         self.world = dist.get_world_size(group) if on else 1
         self.rank = dist.get_rank(group) if on else 0
         ct = cases if isinstance(cases, solver.CaseTable) else solver.CaseTable(cases)
+        if ct.ops is not None:
+            raise NotImplementedError("per-case operating points (CaseTable ops) are not supported for generalised-DOF FOWTs")
         self.n_cases, self.n, self.nw = ct.n_cases, int(P["gen_nDOF"]), len(P["w"])
         self.bounds = general_shards(ct.arrays.get("primary"), ct.n_cases, self.world)
         self.lo, self.hi = self.bounds[self.rank]
