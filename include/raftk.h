@@ -144,13 +144,16 @@ typedef struct raftk_cases {
                                 M0 + (A_w + op_A_w[op[c]]) and B0 + B_drag + (B_w + op_B_w[op[c]]) (the design's and the operating
                                 point's tables summed first; a design without A_w takes the operating point's alone), so a call
                                 equals one call per operating point with that point's tables summed into A_w / B_w, bit for bit.
-                                Honoured by raftk_solve_dynamics_*, the farm entries and raftk_solve_dynamics_slender_*; refused
-                                by raftk_general_*; ignored by the entries that assemble no impedance (excitation, linearisation,
-                                second-order force).  The *_host entries refuse an index outside [0, n_op) and a secondary train
-                                whose point differs from its primary's; the *_dev entries check n_op, op_shared and the tables but
-                                do not read op back (no host synchronisation): its values must be valid. */
+                                Honoured by raftk_solve_dynamics_*, the farm entries, raftk_solve_dynamics_slender_* and every
+                                raftk_general_* solve (there the tables are given on the support of raftk_general_fd: see below);
+                                ignored by the entries that assemble no impedance (excitation, linearisation, second-order force).
+                                The *_host entries refuse an index outside [0, n_op) and a secondary train whose point differs from
+                                its primary's; the rigid and farm *_dev entries check n_op, op_shared and the tables but do not read
+                                op back (no host synchronisation): its values must be valid.  The raftk_general_* *_dev entries
+                                read op back in the same wait as fd_idx and check it as the *_host entries do. */
     int32_t n_op;            /* operating points, >= 1 when op is given                                                   */
-    int32_t op_shared;       /* 0: tables per design [nD, n_op, 36, nw]; 1: one set for every design [n_op, 36, nw]       */
+    int32_t op_shared;       /* 0: tables per design [nD, n_op, 36, nw]; 1: one set for every design [n_op, 36, nw]
+                                (generalised DOFs: [nD, n_op, n_fd, n_fd, nw] / [n_op, n_fd, n_fd, nw])                   */
     const double *op_A_w;    /* sum_r A_aero                  -- added to M0 + A_w                                         */
     const double *op_B_w;    /* sum_r B_aero + sum_r B_gyro   -- added to B0 + B_w                                         */
 } raftk_cases;
@@ -426,6 +429,17 @@ int raftk_general_solve_dynamics_host(const raftk_general *g, const raftk_cases 
  * outside [0, n_dof], fd_idx out of range, repeated or unsorted, n_bem_head < 0, a missing table for a nonzero count, headings
  * that decrease or fall outside [0, 360) (equal neighbours are legal).  The *_dev entry reads fd_idx and bem_headings back
  * to the host for these checks (a copy on the caller's stream and a wait for it).
+ *
+ * Per-case operating points (raftk_cases.op; calcTurbineConstants(case), raft_fowt.py:1514-1586) on a generalised-DOF FOWT:
+ * every raftk_general_* solve (plain, _fd, _qtf, _stream, _batch; _host and _dev) takes them on the support of fd, in the
+ * same [n_fd,n_fd,nw] layout as A_w / B_w: op_A_w, op_B_w are [nD,n_op,n_fd,n_fd,nw], or [n_op,n_fd,n_fd,nw] with
+ * op_shared = 1 (single-design entries: nD = 1).  Unit (d, c) solves with M + (A_w + op_A_w[op[c]]) and
+ * (B + (B_w + op_B_w[op[c]])) + B_drag on the support and exactly as without them off it, so a call equals one call per
+ * operating point with that point's tables summed into fd.A_w / fd.B_w, bit for bit (except the k_qtf_tiles atomics: see
+ * RAFTK_QTF_DIAG).  A batch unit reads table op_shared ? 0 : d.  Rejected with RAFTK_EINVAL before any launch: op without fd
+ * or with n_fd = 0, n_op < 1, op_shared not 0 or 1, a missing table, an index outside [0, n_op), a secondary train whose
+ * point differs from its primary's.  The *_dev entries read op (and primary) back in the same wait as fd_idx.  Workspace
+ * sizes do not depend on them.
  */
 typedef struct raftk_general_fd {
     int32_t n_fd, n_bem_head;

@@ -1506,6 +1506,24 @@ static int validate_gen_fd(const raftk_general *g, const raftk_general_fd *fd, c
     return 0;
 }
 
+// cases.op on the generalised-DOF path: the tables live on the support of fd, so an fd with n_fd >= 1 is required; then
+// validate_op's counts and tables and, with host copies op_h / prim_h, every index and the trains' agreement with their primaries
+static int validate_gen_op(const raftk_general_fd *fd, const raftk_cases *c, const int32_t *op_h, const int32_t *prim_h)
+{
+    if (!c->op) return 0;
+    if (!fd || fd->n_fd < 1)
+        return set_err(RAFTK_EINVAL, "general solve: cases.op (per-case operating points) without fd.n_fd >= 1 is not supported for "
+                                     "generalised-DOF FOWTs: the tables are given on the support of fd_idx");
+    return validate_op(c, op_h, prim_h);
+}
+
+// the elements of one operating-point table of a call: [nD or 1][n_op][n_fd][n_fd][nw] doubles
+static size_t gen_op_elems(const raftk_general_fd *fd, const raftk_cases *c, size_t nD, size_t nw)
+{
+    const size_t nf = fd->n_fd;
+    return (c->op_shared ? 1 : nD) * (size_t)c->n_op * nf * nf * nw;
+}
+
 extern "C" size_t raftk_general_qtf_workspace_bytes(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
                                                     int32_t n_cases)
 {
@@ -1533,7 +1551,7 @@ static int gen_validate(const raftk_general *g, const raftk_general_fd *fd, cons
         return set_err(RAFTK_EINVAL, max_cases == 65535 ? "general solve: 0 < n_dof <= 256, nw > 0, 0 < n_cases <= 65535"
                                                         : "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
     if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
-    if (c->op) return set_err(RAFTK_EINVAL, "general solve: cases.op (per-case operating points) is not supported for generalised-DOF FOWTs");
+    if (int rc = validate_gen_op(fd, c, nullptr, nullptr)) return rc;
     if (qtf) {                                         // the frequency and heading vectors are read back for the checks
         if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
         std::vector<double> qw(qtf->n_qtf_w), qh(qtf->n_qtf_head);
@@ -1542,15 +1560,18 @@ static int gen_validate(const raftk_general *g, const raftk_general_fd *fd, cons
         CUDA_TRY(cudaStreamSynchronize(st));
         if (int rc = validate_gen_qtf(g, qtf, qw.data(), qh.data())) return rc;
     }
-    if (fd) {                                          // the index and heading tables are read back for the checks
+    if (fd) {                                          // the index and heading tables (and cases.op) are read back for the checks
         if (fd->n_fd < 0 || fd->n_fd > g->n_dof || fd->n_bem_head < 0 || (fd->n_fd > 0 && !fd->fd_idx) || (fd->n_bem_head > 0 && !fd->bem_headings))
             return validate_gen_fd(g, fd, nullptr, nullptr);
-        std::vector<int32_t> idx(fd->n_fd);
+        std::vector<int32_t> idx(fd->n_fd), hop(c->op ? c->n_cases : 0), hprim(c->op && c->primary ? c->n_cases : 0);
         std::vector<double> hd(fd->n_bem_head);
         if (fd->n_fd > 0) CUDA_TRY(cudaMemcpyAsync(idx.data(), fd->fd_idx, idx.size() * 4, cudaMemcpyDeviceToHost, st));
         if (fd->n_bem_head > 0) CUDA_TRY(cudaMemcpyAsync(hd.data(), fd->bem_headings, hd.size() * 8, cudaMemcpyDeviceToHost, st));
+        if (!hop.empty()) CUDA_TRY(cudaMemcpyAsync(hop.data(), c->op, hop.size() * 4, cudaMemcpyDeviceToHost, st));      // (op: n_fd >= 1)
+        if (!hprim.empty()) CUDA_TRY(cudaMemcpyAsync(hprim.data(), c->primary, hprim.size() * 4, cudaMemcpyDeviceToHost, st));
         if (fd->n_fd > 0 || fd->n_bem_head > 0) CUDA_TRY(cudaStreamSynchronize(st));
         if (int rc = validate_gen_fd(g, fd, idx.data(), hd.data())) return rc;
+        if (int rc = validate_gen_op(fd, c, hop.data(), hprim.empty() ? nullptr : hprim.data())) return rc;
     }
     return 0;
 }
@@ -1580,6 +1601,7 @@ static raftk_cases gen_case_view(const raftk_cases *c, size_t c0, size_t m, size
     cc.gamma = c->gamma ? c->gamma + c0 : nullptr; cc.beta_deg = c->beta_deg ? c->beta_deg + c0 : nullptr;
     cc.spec = c->spec ? c->spec + c0 : nullptr; cc.zeta = c->zeta ? c->zeta + c0 * nw : nullptr;
     cc.primary = c->primary ? c->primary + c0 : nullptr;
+    cc.op = c->op ? c->op + c0 : nullptr;
     return cc;
 }
 
@@ -1628,9 +1650,14 @@ static int gen_launch(const raftk_general *g, const GenBatch &Bt, const raftk_ge
     const size_t lu_smem = ((size_t)g->n_dof * GB + (size_t)GB * (g->n_dof + 1)) * sizeof(double2);
     const bool blocked = !getenv("RAFTK_GEN_UNBLOCKED") && lu_smem <= 110 * 1024;
     const bool fdz = Fx.n_fd > 0;                      // impedance with the frequency-dependent terms on their support
+    const bool op = c->op != nullptr;                  // plus every case's operating point there (validate_gen_op: n_fd >= 1)
+    GenFdOpDev Fo;
+    static_cast<GenFdDev &>(Fo) = Fx;
+    Fo.op = c->op; Fo.n_op = c->n_op; Fo.op_shared = c->op_shared; Fo.op_A_w = c->op_A_w; Fo.op_B_w = c->op_B_w;
     if (blocked) {
-        static SmemOptIn opt(48 * 1024), opt_fd(48 * 1024);
-        CUDA_TRY(fdz ? opt_fd.ensure(k_gen_solve_blocked<true>, lu_smem) : opt.ensure(k_gen_solve_blocked<false>, lu_smem));
+        static SmemOptIn opt(48 * 1024), opt_fd(48 * 1024), opt_op(48 * 1024);
+        CUDA_TRY(op ? opt_op.ensure(k_gen_solve_blocked<true, true>, lu_smem)
+                    : fdz ? opt_fd.ensure(k_gen_solve_blocked<true>, lu_smem) : opt.ensure(k_gen_solve_blocked<false>, lu_smem));
     }
     if (F_BEM && !bem) CUDA_TRY(cudaMemsetAsync(F_BEM, 0, nC * g->n_dof * g->nw * 16, st));
     double *F2 = nullptr;
@@ -1675,11 +1702,13 @@ static int gen_launch(const raftk_general *g, const GenBatch &Bt, const raftk_ge
         k_gen_project<false, false><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_drag, 1, nullptr, Fx);
         if (blocked) {
             ProfScope ps(st, 2);
-            if (fdz) k_gen_solve_blocked<true><<<dim3(g->nw, (unsigned)nC), GT, lu_smem, st>>>(D, W, X, o->tol, Fx);
+            if (op) k_gen_solve_blocked<true, true><<<dim3(g->nw, (unsigned)nC), GT, lu_smem, st>>>(D, W, X, o->tol, Fo);
+            else if (fdz) k_gen_solve_blocked<true><<<dim3(g->nw, (unsigned)nC), GT, lu_smem, st>>>(D, W, X, o->tol, Fx);
             else k_gen_solve_blocked<false><<<dim3(g->nw, (unsigned)nC), GT, lu_smem, st>>>(D, W, X, o->tol, Fx);
         } else {
             ProfScope ps(st, 2);
-            if (fdz) k_gen_solve<true><<<dim3(g->nw, (unsigned)nC), 256, 0, st>>>(D, W, X, o->tol, Fx);
+            if (op) k_gen_solve<true, true><<<dim3(g->nw, (unsigned)nC), 256, 0, st>>>(D, W, X, o->tol, Fo);
+            else if (fdz) k_gen_solve<true><<<dim3(g->nw, (unsigned)nC), 256, 0, st>>>(D, W, X, o->tol, Fx);
             else k_gen_solve<false><<<dim3(g->nw, (unsigned)nC), 256, 0, st>>>(D, W, X, o->tol, Fx);
         }
         k_gen_relax<<<(unsigned)nC, 256, 0, st>>>(D, W, X);
@@ -1731,7 +1760,6 @@ extern "C" int raftk_general_solve_dynamics_qtf_host(const raftk_general *g, con
     disp_reset();
     if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
     if (g->n_dof <= 0 || g->nw <= 0 || c->n_cases <= 0) return set_err(RAFTK_EINVAL, "general solve: empty problem");
-    if (c->op) return set_err(RAFTK_EINVAL, "general solve: cases.op (per-case operating points) is not supported for generalised-DOF FOWTs");
     const size_t n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases;
     if (c->primary)
         for (size_t i = 0; i < nC; i++) {
@@ -1740,6 +1768,7 @@ extern "C" int raftk_general_solve_dynamics_qtf_host(const raftk_general *g, con
         }
     if (fd)
         if (int rc = validate_gen_fd(g, fd, fd->fd_idx, fd->bem_headings)) return rc;
+    if (int rc = validate_gen_op(fd, c, c->op, c->primary)) return rc;
     if (qtf) {
         if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
         if (int rc = validate_gen_qtf(g, qtf, qtf->qtf_w, qtf->qtf_heads)) return rc;
@@ -1756,6 +1785,7 @@ extern "C" int raftk_general_solve_dynamics_qtf_host(const raftk_general *g, con
     S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
     S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC); S.in(cc.zeta, c->zeta, nC * nw);
     S.in(cc.primary, c->primary, nC);
+    if (c->op) { S.in(cc.op, c->op, nC); S.in(cc.op_A_w, c->op_A_w, gen_op_elems(fd, c, 1, nw)); S.in(cc.op_B_w, c->op_B_w, gen_op_elems(fd, c, 1, nw)); }
     raftk_general_fd ff = fd ? *fd : raftk_general_fd{};
     if (fd) {
         const size_t nf = fd->n_fd, nh = fd->n_bem_head;             // validate_gen_fd: both >= 0
@@ -1920,13 +1950,13 @@ extern "C" int raftk_general_solve_dynamics_stream_host(const raftk_general *g, 
     if (max_chunk_cases < 0) return set_err(RAFTK_EINVAL, "general stream: max_chunk_cases must be >= 0 (0: all cases)");
     if (g->n_dof > 256 || g->n_nodes < 0) return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
     if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
-    if (c->op) return set_err(RAFTK_EINVAL, "general solve: cases.op (per-case operating points) is not supported for generalised-DOF FOWTs");
     const size_t n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases, K = gen_chunk_cap(c->n_cases, max_chunk_cases);
     if (K > 65535) return set_err(RAFTK_EINVAL, "general stream: a chunk takes at most 65535 cases (max_chunk_cases)");
     std::vector<size_t> starts;                        // the plan's checks, before anything is staged
     if (int rc = gen_plan_chunks(c->primary, nC, 1, K, false, starts)) return rc;
     if (fd)
         if (int rc = validate_gen_fd(g, fd, fd->fd_idx, fd->bem_headings)) return rc;
+    if (int rc = validate_gen_op(fd, c, c->op, c->primary)) return rc;
     if (qtf) {
         if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
         if (int rc = validate_gen_qtf(g, qtf, qtf->qtf_w, qtf->qtf_heads)) return rc;
@@ -1943,6 +1973,7 @@ extern "C" int raftk_general_solve_dynamics_stream_host(const raftk_general *g, 
     S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
     S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC); S.in(cc.zeta, c->zeta, nC * nw);
     S.in(cc.primary, c->primary, nC);
+    if (c->op) { S.in(cc.op, c->op, nC); S.in(cc.op_A_w, c->op_A_w, gen_op_elems(fd, c, 1, nw)); S.in(cc.op_B_w, c->op_B_w, gen_op_elems(fd, c, 1, nw)); }
     raftk_general_fd ff = fd ? *fd : raftk_general_fd{};
     if (fd) {
         const size_t nf = fd->n_fd, nh = fd->n_bem_head;
@@ -1986,7 +2017,7 @@ static int gen_batch_counts(const raftk_general *g, const raftk_general_batch *b
         return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
     if ((int64_t)b->n_designs * c->n_cases > INT32_MAX) return set_err(RAFTK_EINVAL, "general batch: n_designs * n_cases must stay below 2^31");
     if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
-    if (c->op) return set_err(RAFTK_EINVAL, "general solve: cases.op (per-case operating points) is not supported for generalised-DOF FOWTs");
+    if (int rc = validate_gen_op(fd, c, nullptr, nullptr)) return rc;
     if (max_chunk_units < 0) return set_err(RAFTK_EINVAL, "general batch: max_chunk_units must be >= 0 (0: all units)");
     if (gen_chunk_cap((int64_t)b->n_designs * c->n_cases, max_chunk_units) > 65535)
         return set_err(RAFTK_EINVAL, "general batch: a chunk takes at most 65535 units (max_chunk_units)");
@@ -2037,7 +2068,7 @@ extern "C" int raftk_general_batch_solve_dynamics_dev(const raftk_general *g, co
     if (int rc = gen_batch_counts(g, b, fd, qtf, c, o, Xi, status, max_chunk_units)) return rc;
     const size_t nD = b->n_designs, nf = fd ? fd->n_fd : 0, nh = fd ? fd->n_bem_head : 0;
     // every table the checks and the chunk plan need, read back with one wait
-    std::vector<int32_t> off(nD + 1), hp(c->primary ? c->n_cases : 0), idx(nD * nf);
+    std::vector<int32_t> off(nD + 1), hp(c->primary ? c->n_cases : 0), idx(nD * nf), hop(c->op ? c->n_cases : 0);
     std::vector<double> hd(nD * nh), qw(qtf ? qtf->n_qtf_w : 0), qh(qtf ? qtf->n_qtf_head : 0);
     auto back = [&](void *h, const void *d, size_t bytes) { return bytes ? cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, st) : cudaSuccess; };
     CUDA_TRY(back(off.data(), b->node_offset, off.size() * 4));
@@ -2046,8 +2077,10 @@ extern "C" int raftk_general_batch_solve_dynamics_dev(const raftk_general *g, co
     CUDA_TRY(back(hd.data(), fd ? fd->bem_headings : nullptr, hd.size() * 8));
     CUDA_TRY(back(qw.data(), qtf ? qtf->qtf_w : nullptr, qw.size() * 8));
     CUDA_TRY(back(qh.data(), qtf ? qtf->qtf_heads : nullptr, qh.size() * 8));
+    CUDA_TRY(back(hop.data(), c->op, hop.size() * 4));
     CUDA_TRY(cudaStreamSynchronize(st));
     if (int rc = gen_batch_tables(g, b, fd, qtf, off.data(), idx.data(), hd.data(), qw.data(), qh.data())) return rc;
+    if (int rc = validate_gen_op(fd, c, hop.data(), c->primary ? hp.data() : nullptr)) return rc;
     GenBatch Bt = gen_batch_of(b);
     Bt.hnode_off = off.data();
     return gen_run(g, Bt, fd, qtf, c, c->primary ? hp.data() : nullptr, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, workspace_bytes,
@@ -2063,6 +2096,7 @@ extern "C" int raftk_general_batch_solve_dynamics_host(const raftk_general *g, c
     if (int rc = gen_batch_counts(g, b, fd, qtf, c, o, Xi, status, max_chunk_units)) return rc;
     if (int rc = gen_batch_tables(g, b, fd, qtf, b->node_offset, fd ? fd->fd_idx : nullptr, fd ? fd->bem_headings : nullptr,
                                   qtf ? qtf->qtf_w : nullptr, qtf ? qtf->qtf_heads : nullptr)) return rc;
+    if (int rc = validate_gen_op(fd, c, c->op, c->primary)) return rc;
     const size_t nD = b->n_designs, n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases, nU = nD * nC;
     std::vector<size_t> starts;                        // the plan's checks, before anything is staged
     if (int rc = gen_plan_chunks(c->primary, nC, nD, gen_chunk_cap((int64_t)nU, max_chunk_units), true, starts)) return rc;
@@ -2081,6 +2115,7 @@ extern "C" int raftk_general_batch_solve_dynamics_host(const raftk_general *g, c
     S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
     S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC); S.in(cc.zeta, c->zeta, nC * nw);
     S.in(cc.primary, c->primary, nC);
+    if (c->op) { S.in(cc.op, c->op, nC); S.in(cc.op_A_w, c->op_A_w, gen_op_elems(fd, c, nD, nw)); S.in(cc.op_B_w, c->op_B_w, gen_op_elems(fd, c, nD, nw)); }
     raftk_general_fd ff = fd ? *fd : raftk_general_fd{};
     if (fd) {
         const size_t nf = fd->n_fd, nh = fd->n_bem_head;

@@ -15,7 +15,8 @@
 //   k_gen_bdrag     (case, row)       B_drag = sum_j Tn_j^T B6_j Tn_j
 //   k_gen_project                     F_drag
 //   k_gen_solve     (case, w)         Z = -w^2 M + i w (B + B_drag) + C, dense complex LU with partial pivoting, Xi;
-//                                     on the support of the frequency-dependent terms M + A_w(w) and B + B_w(w) (gen_impedance)
+//                                     on the support of the frequency-dependent terms M + A_w(w) and B + B_w(w) (gen_impedance),
+//                                     plus the case's operating point there when the case table carries them (OP)
 //   k_gen_relax     (case)            convergence bookkeeping, XiLast = 0.2 XiLast + 0.8 Xi
 // Wave trains (cases.primary): a secondary train takes no part in the loop (done at init); after it
 //   k_gen_node_pass<true>   (case, node)   drag node load from the PRIMARY's last Bmat and the train's own u
@@ -70,6 +71,16 @@ struct GenFdDev {
     double2 *fb6;                // [nC][6][nw] workspace: BEM force in full DOFs 0-5
     const double2 *F_BEM;        // [nC][n][nw] BEM force in reduced DOFs, added to F_iner
 };
+
+// per-case operating points (raftk_cases.op) on the support of fd_idx: GenFdDev plus the case table's op column and the tables
+// [nD or 1][n_op][n_fd][n_fd][nw].  Only the OP instantiations of k_gen_solve* take it, so that every other kernel keeps its
+// parameter layout.
+struct GenFdOpDev : GenFdDev {
+    const int *op;               // [nC of the whole table] operating point of every case
+    int n_op, op_shared;         // op_shared: one set of tables for every design
+    const double *op_A_w, *op_B_w;
+};
+template <bool OP> using GenFdArg = typename std::conditional<OP, GenFdOpDev, GenFdDev>::type;
 
 struct GenWork {                 // per-call workspace views
     double2 *u;                  // [nC][Ns][3][nw]
@@ -209,18 +220,27 @@ __device__ __forceinline__ GenMats gen_mats(const GenDev &D, const GenFdDev &X, 
     return G;
 }
 
+// the operating-point tables of unit U (design d, case U.c of the whole table): op_A_w / op_B_w at [op_shared ? 0 : d][op[c]]
+__device__ __forceinline__ void gen_op_tables(const GenDev &D, const GenFdOpDev &X, const GenUnit &U, const double *&Ao, const double *&Bo)
+{
+    const size_t ff = (size_t)X.n_fd * X.n_fd * D.nw, o = ((X.op_shared ? 0 : (size_t)U.d * X.n_op) + (size_t)X.op[U.c]) * ff;
+    Ao = X.op_A_w + o; Bo = X.op_B_w + o;
+}
+
 // impedance entry t = a n + b at frequency i (raft_model.py:1086).  On the support: M + A_w and (B + B_w) + B_drag with the
 // rigid solver's grouping (raftk_fused.cuh); elsewhere the constant-matrix expression.  FD = false (n_fd = 0) is the
-// constant-matrix kernel as it was, instruction for instruction: no map, no branch
-template <bool FD>
+// constant-matrix kernel as it was, instruction for instruction: no map, no branch.  OP: the case's operating point (Ao, Bo
+// on the same support) summed with the design's table first, M + (A_w + Ao) and (B + (B_w + Bo)) + B_drag, so that a call
+// with operating points equals one with each point's tables summed into fd.A_w / fd.B_w, bit for bit.
+template <bool FD, bool OP = false>
 __device__ __forceinline__ double2 gen_impedance(const GenDev &D, const GenFdDev &X, const GenMats &G, const int *fdpos, const double *Bd, int t,
-                                                 int i, double w, double w2)
+                                                 int i, double w, double w2, const double *Ao = nullptr, const double *Bo = nullptr)
 {
     if constexpr (FD) {
         const int pa = fdpos[t / D.n], pb = fdpos[t % D.n];
         if (pa >= 0 && pb >= 0) {
             const size_t e = ((size_t)pa * X.n_fd + pb) * D.nw + i;
-            const double M = G.M[t] + G.A_w[e], B = (G.B[t] + G.B_w[e]) + Bd[t];
+            const double M = G.M[t] + (OP ? G.A_w[e] + Ao[e] : G.A_w[e]), B = (G.B[t] + (OP ? G.B_w[e] + Bo[e] : G.B_w[e])) + Bd[t];
             return make_double2(fma(-w2, M, G.C[t]), w * B);
         }
     }
@@ -360,9 +380,12 @@ __global__ void __launch_bounds__(128) k_gen_bdrag(GenDev D, GenWork W)
 
 // k_gen_solve: grid (nw, units), block 256.  Augmented system [Z | F] (n x (n+1)) in global memory (L2-resident), right-looking
 // LU with partial pivoting on |re| + |im| (LAPACK izamax), back substitution; writes Xi and the convergence verdict.
-template <bool FD>
-__global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 *Xi, double tol, GenFdDev X)
+// OP (with FD): the case table carries operating points (GenFdOpDev); an instantiation of its own, so that the solves without
+// them compile as before.
+template <bool FD, bool OP = false>
+__global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 *Xi, double tol, GenFdArg<OP> X)
 {
+    static_assert(FD || !OP, "operating points live on the support of the frequency-dependent terms");
     __shared__ double pv[8];
     __shared__ int pi_[8];
     __shared__ double2 piv;
@@ -370,15 +393,18 @@ __global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 
     __shared__ int fdpos[FD ? 256 : 1];
     const int i = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, n = D.n, nw = D.nw, nc = n + 1;
     if (W.flags[4 * c]) return;
-    const int d = gen_unit(D, c).d;
+    const GenUnit U = gen_unit(D, c);
+    const int d = U.d;
     const GenMats G = gen_mats(D, X, d);
+    const double *Ao = nullptr, *Bo = nullptr;
+    if constexpr (OP) gen_op_tables(D, X, U, Ao, Bo);
     double2 *A = W.Z + ((size_t)c * nw + i) * (size_t)n * nc;
     const double w = D.w[i], w2 = w * w;
     const double *Bd = W.B_drag + (size_t)c * n * n;
     if constexpr (FD) gen_fd_map(D, X, d, fdpos, tid, 256);
     for (int t = tid; t < n * n; t += 256) {
         const int a = t / n, b = t % n;
-        A[(size_t)a * nc + b] = gen_impedance<FD>(D, X, G, fdpos, Bd, t, i, w, w2);
+        A[(size_t)a * nc + b] = gen_impedance<FD, OP>(D, X, G, fdpos, Bd, t, i, w, w2, Ao, Bo);
     }
     for (int a = tid; a < n; a += 256) {
         const double2 f1 = W.F_iner[((size_t)c * n + a) * nw + i], f2 = W.F_drag[((size_t)c * n + a) * nw + i];
@@ -463,9 +489,10 @@ __global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 
 //   9 Mflop per 150 x 150 system then run from registers and shared memory.
 #define GB 8
 #define GT 128
-template <bool FD>
-__global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W, double2 *Xi, double tol, GenFdDev X)
+template <bool FD, bool OP = false>
+__global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W, double2 *Xi, double tol, GenFdArg<OP> X)
 {
+    static_assert(FD || !OP, "operating points live on the support of the frequency-dependent terms");
     extern __shared__ __align__(16) double smem_raw[];
     __shared__ double pv[GT / 32];
     __shared__ int pi_[GT / 32];
@@ -474,8 +501,11 @@ __global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W
     __shared__ int fdpos[FD ? 256 : 1];
     const int i = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, n = D.n, nw = D.nw, nc = n + 1;
     if (W.flags[4 * c]) return;
-    const int d = gen_unit(D, c).d;
+    const GenUnit Un = gen_unit(D, c);
+    const int d = Un.d;
     const GenMats G = gen_mats(D, X, d);
+    const double *Ao = nullptr, *Bo = nullptr;
+    if constexpr (OP) gen_op_tables(D, X, Un, Ao, Bo);
     double2 *P = reinterpret_cast<double2 *>(smem_raw);          // panel  [n][GB]   (rows kb.. stored from 0)
     double2 *U = P + (size_t)n * GB;                             // row block [GB][nc]
     double2 *A = W.Z + ((size_t)c * nw + i) * (size_t)n * nc;
@@ -484,7 +514,7 @@ __global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W
     if constexpr (FD) gen_fd_map(D, X, d, fdpos, tid, GT);
     for (int t = tid; t < n * n; t += GT) {
         const int a = t / n, b = t % n;
-        A[(size_t)a * nc + b] = gen_impedance<FD>(D, X, G, fdpos, Bd, t, i, w, w2);
+        A[(size_t)a * nc + b] = gen_impedance<FD, OP>(D, X, G, fdpos, Bd, t, i, w, w2, Ao, Bo);
     }
     for (int a = tid; a < n; a += GT) {
         const double2 f1 = W.F_iner[((size_t)c * n + a) * nw + i], f2 = W.F_drag[((size_t)c * n + a) * nw + i];

@@ -201,7 +201,8 @@ def pack_operating_points(states):
             s = states[d][c]
             n = get(s, "nDOF") if not isinstance(s, dict) and hasattr(s, "nDOF") else np.shape(get(s, "A_aero"))[0]
             if n != 6:
-                raise NotImplementedError("operating points: only rigid 6-DOF FOWTs (flexible FOWTs, raftk_general_*, are a follow-up)")
+                raise NotImplementedError("operating points: only rigid 6-DOF FOWTs here (the follow-up for flexible FOWTs, "
+                                          "raftk_general_*, is pack_general_operating_points)")
             A, B, G = (np.asarray(get(s, k), dtype=float) for k in ("A_aero", "B_aero", "B_gyro"))
             nw = A.shape[2] if nw is None and A.ndim == 4 else nw
             if A.ndim != 4 or A.shape[:2] != (6, 6) or B.shape != A.shape or A.shape[2] != nw or G.shape != (6, 6, A.shape[3]):
@@ -304,7 +305,7 @@ def pack_general_dofs(fowt):
     return out
 
 
-def pack_general_matrices(fowt):
+def pack_general_matrices(fowt, states=None):
     """System matrices of a FOWT with generalised degrees of freedom (raft_model.py:1045-1047), split into the constant part
     and the frequency-dependent part the solver adds on its support (C ABI ``raftk_general_fd``).  Duck-typed on a live FOWT.
 
@@ -315,17 +316,23 @@ def pack_general_matrices(fowt):
       1557-1562); ``A_w``, ``B_w`` [n_fd,n_fd,nw] those sums restricted to it (every entry outside it is exactly zero);
       ``pack_bem_excitation``'s table (``X_BEM`` [nhead,6,nw] in full DOFs 0-5, ``bem_headings``, ``heading_adjust``) or
       none; ``T0`` [6,nDOF] = rows 0-5 of ``fowt.T`` (F_BEM = T^T F_BEM_fullDOF, raft_fowt.py:1885-1887); ``x_ref``, ``y_ref``.
-    A FOWT without operating rotors and without BEM coefficients gets n_fd = 0."""
+    A FOWT without operating rotors and without BEM coefficients gets n_fd = 0.
+
+    ``states``: one turbine state per load case, as ``pack_general_operating_points`` takes them for one design (the live
+    FOWT right after ``calcTurbineConstants(case)``, or a dict).  The FOWT's own A_aero, B_aero and B_gyro are then ignored:
+    B = B_struc; ``fd_idx`` is the union of the BEM support and the support of every state; ``fd``'s A_w / B_w carry the BEM
+    terms alone (zero on the DOFs only the operating points touch); and the result gains ``ops``, the
+    ``pack_general_operating_points`` dict on that support, for ``solver.CaseTable(ops=)``."""
     n, nw = int(fowt.nDOF), len(fowt.w)
     M = np.array(fowt.M_struc, dtype=float) + np.array(fowt.A_hydro_morison, dtype=float)
     B = np.array(fowt.B_struc, dtype=float)
     B_gyro = getattr(fowt, "B_gyro", None)
-    if B_gyro is not None and np.size(B_gyro):
+    if states is None and B_gyro is not None and np.size(B_gyro):
         B = B + np.sum(B_gyro, axis=2)
     C = (np.array(fowt.C_struc, dtype=float) + np.array(fowt.C_hydro, dtype=float)
          + np.array(fowt.C_moor, dtype=float) + np.array(fowt.C_elast, dtype=float))
     A_w, B_w = np.zeros([n, n, nw]), np.zeros([n, n, nw])
-    if getattr(fowt, "nrotors", 0) > 0:
+    if states is None and getattr(fowt, "nrotors", 0) > 0:
         A_w = A_w + np.sum(fowt.A_aero, axis=3)
         B_w = B_w + np.sum(fowt.B_aero, axis=3)
     for name, acc in (("A_BEM", A_w), ("B_BEM", B_w)):
@@ -333,14 +340,88 @@ def pack_general_matrices(fowt):
         if t is not None and np.size(t):
             acc += np.asarray(t, dtype=float)
     nz = np.any(A_w != 0, axis=2) | np.any(B_w != 0, axis=2)
-    idx = np.nonzero(nz.any(axis=0) | nz.any(axis=1))[0].astype(np.int32)
+    sup = nz.any(axis=0) | nz.any(axis=1)
+    if states is not None:
+        for s in states:
+            sup |= _general_state_support(s)
+    idx = np.nonzero(sup)[0].astype(np.int32)
     fd = dict(fd_idx=idx, A_w=np.ascontiguousarray(A_w[np.ix_(idx, idx)]), B_w=np.ascontiguousarray(B_w[np.ix_(idx, idx)]),
               T0=np.ascontiguousarray(np.asarray(fowt.T, dtype=float)[:6]),
               x_ref=np.float64(getattr(fowt, "x_ref", 0.0)), y_ref=np.float64(getattr(fowt, "y_ref", 0.0)))
     bem = pack_bem_excitation(fowt)
     if bem is not None:
         fd.update(bem)
-    return dict(M=M, B=B, C=C, fd=fd)
+    out = dict(M=M, B=B, C=C, fd=fd)
+    if states is not None:
+        out["ops"] = pack_general_operating_points([states], idx)
+    return out
+
+
+def _general_state(s):
+    """(A_aero [n,n,nw,nrot], B_aero, B_gyro [n,n,nrot]) of one turbine state (live FOWT or dict), float arrays."""
+    get = (lambda k: s[k]) if isinstance(s, dict) else (lambda k: getattr(s, k))     # noqa: E731
+    return tuple(np.asarray(get(k), dtype=float) for k in ("A_aero", "B_aero", "B_gyro"))
+
+
+def _general_state_support(s):
+    """Reduced DOFs whose rows or columns of a turbine state's A_aero, B_aero or B_gyro hold a nonzero entry -> bool [n]."""
+    A, B, G = _general_state(s)
+    nz = np.any(A != 0, axis=(2, 3)) | np.any(B != 0, axis=(2, 3)) | np.any(G != 0, axis=2)
+    return nz.any(axis=0) | nz.any(axis=1)
+
+
+def pack_general_operating_points(states, fd_idx):
+    """Per-case aero-servo added mass and damping of FOWTs with generalised degrees of freedom (raftk_cases.op on the
+    raftk_general_* solves, ``solver.CaseTable(ops=)``), on the support ``fd_idx`` of their frequency-dependent terms.
+
+    ``states[d][c]``: design d right after the reference's ``calcTurbineConstants(case c)`` (raft_fowt.py:1514-1586) -- the
+    live FOWT or a dict with A_aero [n,n,nw,nrot], B_aero [n,n,nw,nrot] and B_gyro [n,n,nrot] in reduced DOFs (the reference's
+    own T^T a T of the rotor node).  Its operating point is A(w) = sum_r A_aero[:,:,w,r] and B(w) = sum_r B_aero[:,:,w,r] +
+    sum_r B_gyro[:,:,r] (the gyroscopic term in every bin), restricted to ``fd_idx`` ([n_fd] for every design, or [nD, n_fd]).
+    Cases whose tables are bit-identical over every design share one point.  -> dict(op [nC] int32, A_w, B_w
+    [nD, n_op, n_fd, n_fd, nw], n_op).  ValueError when a state is nonzero off ``fd_idx`` or its shapes disagree; the
+    design's own matrices (``pack_general_matrices(fowt, states=...)``) must then not carry these terms."""
+    nD = len(states)
+    nC = len(states[0]) if nD else 0
+    if nD < 1 or nC < 1 or any(len(row) != nC for row in states):
+        raise ValueError("states must hold one snapshot per case (the same count) for every design")
+    idx = np.asarray(fd_idx, dtype=np.int64)
+    idx = np.broadcast_to(idx, (nD,) + idx.shape[-1:]) if idx.ndim == 1 else idx
+    if idx.ndim != 2 or idx.shape[0] != nD or idx.shape[1] < 1:
+        raise ValueError("fd_idx must be [n_fd] or [nD, n_fd] with n_fd >= 1")
+    shape = None
+    tabs = []                                                       # [nC][nD] (A, B)
+    for c in range(nC):
+        row = []
+        for d in range(nD):
+            A, B, G = _general_state(states[d][c])
+            shape = A.shape[:3] if shape is None else shape
+            n = A.shape[0] if A.ndim == 4 else -1
+            if A.ndim != 4 or A.shape[:3] != shape or A.shape[1] != n or B.shape != A.shape or G.shape != (n, n, A.shape[3]):
+                raise ValueError("operating point of design %d, case %d: A_aero / B_aero must be [n,n,nw,nrot] (%s) and B_gyro "
+                                 "[n,n,nrot]" % (d, c, list(shape)))
+            if np.any(idx[d] < 0) or np.any(idx[d] >= n):
+                raise ValueError("fd_idx of design %d: entries outside [0, %d)" % (d, n))
+            off = np.ones(n, dtype=bool)
+            off[idx[d]] = False
+            Ad, Bd = np.sum(A, axis=3), np.sum(B, axis=3) + np.sum(G, axis=2)[:, :, None]
+            if np.any(Ad[off]) or np.any(Ad[:, off]) or np.any(Bd[off]) or np.any(Bd[:, off]) or np.any(G[off]) or np.any(G[:, off]):
+                raise ValueError("operating point of design %d, case %d is nonzero off fd_idx (pack_general_matrices(fowt, "
+                                 "states=...) takes the union of the supports)" % (d, c))
+            sub = np.ix_(idx[d], idx[d])
+            row.append((np.ascontiguousarray(Ad[sub]), np.ascontiguousarray(Bd[sub])))
+        tabs.append(row)
+    op = np.zeros(nC, dtype=np.int32)
+    seen, first = {}, []
+    for c, row in enumerate(tabs):
+        key = b"".join(t.tobytes() for pair in row for t in pair)
+        if key not in seen:
+            seen[key] = len(first)
+            first.append(c)
+        op[c] = seen[key]
+    A_w = np.ascontiguousarray([[tabs[c][d][0] for c in first] for d in range(nD)])
+    B_w = np.ascontiguousarray([[tabs[c][d][1] for c in first] for d in range(nD)])
+    return dict(op=op, A_w=A_w, B_w=B_w, n_op=len(first))
 
 
 def pack_qtf(fowt):

@@ -248,7 +248,10 @@ class CaseTable:
         ``ops``: optional operating points (``packer.pack_operating_points``): dict(op [nC] int, A_w, B_w) with tables
         [nD, n_op, 6, 6, nw] per design or [n_op, 6, 6, nw] for one set every design shares -- the aero-servo added mass and
         damping (B_gyro folded into B_w) that the reference's calcTurbineConstants(case) adds to case c's system matrices:
-        unit (d, c) solves with M0 + (A_w + ops.A_w[op[c]]) and B0 + B_drag + (B_w + ops.B_w[op[c]]) (raftk_cases.op)."""
+        unit (d, c) solves with M0 + (A_w + ops.A_w[op[c]]) and B0 + B_drag + (B_w + ops.B_w[op[c]]) (raftk_cases.op).
+        The generalised-DOF solves take square tables [.., n_fd, n_fd, nw] on the support of their ``fd``
+        (``packer.pack_general_operating_points``); each solve checks the table size against its designs (``check_ops``,
+        ``check_general_ops``)."""
         self.arrays = a = _Tables()
         for kname in ("Hs", "Tp", "gamma", "beta_deg"):
             a[kname] = np.ascontiguousarray(cases[kname], dtype=_F8)
@@ -273,8 +276,9 @@ class CaseTable:
             A, B = (np.ascontiguousarray(ops[k], dtype=_F8) for k in ("A_w", "B_w"))
             if op.shape != (self.n_cases,):
                 raise ValueError("ops['op'] must name one operating point per case (%d)" % self.n_cases)
-            if A.shape != B.shape or A.ndim not in (4, 5) or A.shape[-3:-1] != (6, 6):
-                raise ValueError("ops A_w / B_w must both be [nD, n_op, 6, 6, nw] or [n_op, 6, 6, nw]")
+            if A.shape != B.shape or A.ndim not in (4, 5) or A.shape[-3] != A.shape[-2] or A.shape[-3] < 1:
+                raise ValueError("ops A_w / B_w must both be [nD, n_op, m, m, nw] or [n_op, m, m, nw] (m = 6, or n_fd for "
+                                 "generalised DOFs)")
             self.n_op, self.op_shared = int(A.shape[-4]), int(A.ndim == 4)
             if np.any(op < 0) or np.any(op >= self.n_op):
                 raise ValueError("ops['op'] must lie in [0, %d)" % self.n_op)
@@ -288,8 +292,23 @@ class CaseTable:
         if self.ops is None:
             return
         A = self.ops["A_w"]
+        if A.shape[-3:-1] != (6, 6):
+            raise ValueError("operating-point tables %s: the rigid-body solves take 6 x 6 tables" % list(A.shape))
         if A.shape[-1] != batch.nw or (not self.op_shared and A.shape[0] != batch.n_designs):
             raise ValueError("operating-point tables %s do not match %d designs x %d bins" % (list(A.shape), batch.n_designs, batch.nw))
+
+    def check_general_ops(self, n_fd, n_designs, nw):
+        """Refuse operating points on a generalised-DOF solve whose ``fd`` has no support (n_fd = 0 or no fd), and tables that
+        are not [n_designs, n_op, n_fd, n_fd, nw] or [n_op, n_fd, n_fd, nw]."""
+        if self.ops is None:
+            return
+        if not n_fd:
+            raise ValueError("per-case operating points without frequency-dependent terms (fd with n_fd >= 1) are not supported "
+                             "for generalised-DOF FOWTs: pack them with packer.pack_general_matrices(fowt, states=...)")
+        A = self.ops["A_w"]
+        if A.shape[-3:-1] != (n_fd, n_fd) or A.shape[-1] != nw or (not self.op_shared and A.shape[0] != n_designs):
+            raise ValueError("operating-point tables %s do not match %d designs x [%d, %d] support x %d bins"
+                             % (list(A.shape), n_designs, n_fd, n_fd, nw))
 
     def input_bytes(self):
         return int(sum(v.nbytes for v in self.arrays.values()))
@@ -826,7 +845,7 @@ class GeneralSession:
     [nT,6] (reduced DOFs 0-5).  ``max_chunk_cases``: None runs the table in one launch sequence (at most 65535 cases, a
     workspace for every case at once); an integer K streams it in chunks of whole train groups of at most K cases (0: one
     chunk) through a workspace sized for one chunk (raftk_general_solve_dynamics_stream_dev, ``general_chunk_for_budget``),
-    with the same results."""
+    with the same results.  ``cases`` may carry per-case operating points, as for ``general_solve_dynamics``."""
 
     def __init__(self, P, M, B, Cm, cases, device=None, fd=None, F_BEM=False, qtf=None, max_chunk_cases=None):
         import torch
@@ -843,6 +862,7 @@ class GeneralSession:
             self.ct = {k: torch.from_numpy(v).to(self.device) for k, v in cases.arrays.items()}
             self.c_struct = cases.struct(lambda name: self.ct[name].data_ptr())
             n, nw, nC = int(P["gen_nDOF"]), len(P["w"]), cases.n_cases
+            cases.check_general_ops(int(len(fd.get("fd_idx", ()))) if fd is not None else 0, 1, nw)
             self.fd = _general_fd_struct(fd, n, nw, to_dev)
             self.qtf = _general_qtf_struct(qtf, to_dev)
             fdp = C.byref(self.fd) if self.fd is not None else None
@@ -924,7 +944,9 @@ def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0
     excitation of every case and train in reduced DOFs, complex [nT,nDOF,nw], to the result.  ``qtf``: second-order wave
     loads (potSecOrder 2), the dict of ``packer.pack_general_qtf``; ``F_2nd=True`` (with ``qtf``) then appends the force of
     every case and train on reduced DOFs 0-5, F_2nd [nT,6,nw] and F_2nd_mean [nT,6].  ``max_chunk_cases``: None solves the
-    table in one launch sequence; an integer K streams it through a device workspace for K cases (``GeneralSession``)."""
+    table in one launch sequence; an integer K streams it through a device workspace for K cases (``GeneralSession``).
+    ``cases`` may carry per-case operating points on the support of ``fd`` (``CaseTable(ops=)``, tables [1 or none, n_op,
+    n_fd, n_fd, nw]; ``packer.pack_general_matrices(fowt, states=...)``); without fd they are refused."""
     n, nw = int(P["gen_nDOF"]), len(P["w"])
     keep = {}
 
@@ -936,6 +958,7 @@ def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0
     q = _general_qtf_struct(qtf, ptr)
     if F_2nd and q is None:
         raise ValueError("F_2nd=True needs a QTF table (qtf=, packer.pack_general_qtf)")
+    cases.check_general_ops(f.n_fd if f is not None else 0, 1, nw)
     nC = cases.n_cases
     Xi = np.zeros([nC, n, nw], dtype=np.complex128)
     st = np.zeros([nC, 4], dtype=_I4)
@@ -1233,7 +1256,7 @@ def general_case_metrics(channels, std, psd, amp, idx, dw=None):
 
 
 def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, fd=None, qtf=None, rotors=None,
-                          turbine_constants=None):
+                          turbine_constants=None, ops=None):
     """Model.analyzeCases (dynamics and output statistics) for one FOWT with generalised degrees of freedom: ``cases`` a list
     of case dicts, scalar or list-valued wave keys (several wave trains); ``channels`` from ``packer.pack_general_channels``.
     -> dict(Xi_trains [per case: nTrains,nDOF,nw], status [nC,4] of train 0, case_metrics {case: saveTurbineOutputs entries},
@@ -1241,13 +1264,16 @@ def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01
     wave loads (``packer.pack_general_qtf``); the result then also holds, per case, the reference FOWT's ``Fhydro_2nd``
     (complex [nTrains,nDOF,nw]) and ``Fhydro_2nd_mean`` ([nTrains,nDOF]), zero from reduced DOF 6 up (raft_model.py:1034-1036).
     ``rotors``: ``packer.pack_rotor_outputs`` of the FOWT for these cases; every case's metrics then hold the rotor entries
-    (omega / torque / bPitch / power, wind_PSD; ``rotor_metrics``).  ``turbine_constants`` (per-case operating points, as
-    ``Model(turbine_constants=)``) are not supported for generalised-DOF FOWTs: NotImplementedError."""
+    (omega / torque / bPitch / power, wind_PSD; ``rotor_metrics``).  ``ops``: per-case operating points, one per case of
+    ``cases`` (op [nC]; ``packer.pack_general_matrices(fowt, states=...)['ops']``, whose M, B and fd then go with it): every
+    wave train of a case is solved at its case's point.  ``turbine_constants`` (raw per-case snapshots, as
+    ``Model(turbine_constants=)``): NotImplementedError, since M, B and fd come here already packed."""
     from .packer import pack_case_trains
     _no_general_ops(turbine_constants)
     table, owner, first = pack_case_trains(cases)
     q = bool(qtf)
-    res = general_solve_dynamics(P, M, B, Cm, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start, fd=fd, qtf=qtf, F_2nd=q)
+    res = general_solve_dynamics(P, M, B, Cm, CaseTable(table, ops=_train_ops(ops, owner, len(cases))), n_iter=n_iter, tol=tol,
+                                 xi_start=xi_start, fd=fd, qtf=qtf, F_2nd=q)
     return _general_case_results(P, res[0], res[1], owner, first, len(cases), channels, res[2:4] if q else None, rotors)
 
 
@@ -1478,6 +1504,7 @@ def general_solve_dynamics_batch(designs, cases, n_iter=10, tol=0.01, xi_start=0
     g, b, f, q = bt.structs(ptr)
     if F_2nd and q is None:
         raise ValueError("F_2nd=True needs a QTF table")
+    cases.check_general_ops(f.n_fd if f is not None else 0, bt.n_designs, bt.nw)
     nD, nC, n, nw = bt.n_designs, cases.n_cases, bt.n, bt.nw
     Xi = np.zeros([nD, nC, n, nw], dtype=np.complex128)
     st = np.zeros([nD, nC, 4], dtype=_I4)
@@ -1514,6 +1541,7 @@ class GeneralBatchSession:
             self.keep[name] = t
             return t.data_ptr()
         nD, nC, n, nw = bt.n_designs, cases.n_cases, bt.n, bt.nw
+        cases.check_general_ops(bt.n_fd if bt.fd is not None else 0, nD, nw)
         with torch.cuda.device(self.device):
             self.g, self.b, self.fd, self.qtf = bt.structs(to_dev)
             self.ct = {k: torch.from_numpy(v).to(self.device) for k, v in cases.arrays.items()}
@@ -1587,17 +1615,29 @@ class GeneralBatchSession:
 
 def _no_general_ops(turbine_constants):
     if turbine_constants is not None:
-        raise NotImplementedError("per-case turbine constants (operating points) are not supported for generalised-DOF FOWTs yet: "
-                                  "the rigid-body solve takes them (Model(turbine_constants=))")
+        raise NotImplementedError("turbine_constants= (raw per-case snapshots) is not taken by the generalised-DOF analysis, whose "
+                                  "M, B and fd come packed and would count the snapshots' terms twice: pack them with "
+                                  "packer.pack_general_matrices(fowt, states=...) and pass its M, B, fd and ops=")
+
+
+def _train_ops(ops, owner, n_cases):
+    """Per-case operating points (op [n_cases]) expanded to the rows of a train table (``pack_case_trains``' owner)."""
+    if ops is None:
+        return None
+    op = np.asarray(ops["op"])
+    if op.shape != (n_cases,):
+        raise ValueError("ops['op'] must name one operating point per case (%d), got shape %s" % (n_cases, list(op.shape)))
+    return dict(op=op[owner], A_w=ops["A_w"], B_w=ops["B_w"])
 
 
 def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, qtf=None, rotors=None,
-                                turbine_constants=None):
+                                turbine_constants=None, ops=None):
     """``general_analyze_cases`` for every design of a batch in one solve: ``designs`` a list of per-design inputs (or a
     ``GeneralBatch`` built from them), ``cases`` a list of case dicts run by every design, ``channels`` None or one
     ``packer.pack_general_channels`` dict per design, ``rotors`` None or one ``packer.pack_rotor_outputs`` dict per design
-    -> a list with, for each design, what ``general_analyze_cases`` returns for that design alone.  ``turbine_constants``:
-    NotImplementedError, as for ``general_analyze_cases``."""
+    -> a list with, for each design, what ``general_analyze_cases`` returns for that design alone.  ``ops``: one operating
+    point per case, tables per design [nD, n_op, n_fd, n_fd, nw] or shared [n_op, n_fd, n_fd, nw]
+    (``packer.pack_general_operating_points``).  ``turbine_constants``: NotImplementedError, as for ``general_analyze_cases``."""
     from .packer import pack_case_trains
     _no_general_ops(turbine_constants)
     bt = _as_batch(designs, qtf)
@@ -1607,7 +1647,8 @@ def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.
         raise ValueError("rotors: one entry per design (%d), got %d" % (bt.n_designs, len(rotors)))
     table, owner, first = pack_case_trains(cases)
     q = bt.qtf is not None
-    res = general_solve_dynamics_batch(bt, CaseTable(table), n_iter=n_iter, tol=tol, xi_start=xi_start, F_2nd=q)
+    res = general_solve_dynamics_batch(bt, CaseTable(table, ops=_train_ops(ops, owner, len(cases))), n_iter=n_iter, tol=tol,
+                                       xi_start=xi_start, F_2nd=q)
     P = dict(w=bt.arrays["w"], dw=bt.dw)
     return [_general_case_results(P, res[0][d], res[1][d], owner, first, len(cases), None if channels is None else channels[d],
                                   (res[2][d], res[3][d]) if q else None, None if rotors is None else rotors[d])

@@ -368,15 +368,15 @@ def general_shards(primary, n_cases, world):
 
 
 def shard_case_table(cases, lo, hi):
-    """Rows [lo, hi) of a ``solver.CaseTable`` as a table of their own (whole train groups: primaries rebased to lo)."""
+    """Rows [lo, hi) of a ``solver.CaseTable`` as a table of their own (whole train groups: primaries rebased to lo).  Per-case
+    operating points keep their rows of ``op`` and the whole tables."""
     from . import solver
-    if cases.ops is not None:
-        raise NotImplementedError("per-case operating points (CaseTable ops) are not supported for generalised-DOF FOWTs")
     a = cases.arrays
     sub = {k: a[k][lo:hi] for k in ("Hs", "Tp", "gamma", "beta_deg", "spec")}
     if "primary" in a:
         sub["primary"] = a["primary"][lo:hi] - lo
-    return solver.CaseTable(sub, zeta=a["zeta"][lo:hi] if "zeta" in a else None)
+    ops = None if cases.ops is None else dict(cases.ops, op=cases.ops["op"][lo:hi])
+    return solver.CaseTable(sub, zeta=a["zeta"][lo:hi] if "zeta" in a else None, ops=ops)
 
 
 class ShardedGeneralSolve:
@@ -401,8 +401,6 @@ class ShardedGeneralSolve:
         self.world = dist.get_world_size(group) if on else 1
         self.rank = dist.get_rank(group) if on else 0
         ct = cases if isinstance(cases, solver.CaseTable) else solver.CaseTable(cases)
-        if ct.ops is not None:
-            raise NotImplementedError("per-case operating points (CaseTable ops) are not supported for generalised-DOF FOWTs")
         self.n_cases, self.n, self.nw = ct.n_cases, int(P["gen_nDOF"]), len(P["w"])
         self.bounds = general_shards(ct.arrays.get("primary"), ct.n_cases, self.world)
         self.lo, self.hi = self.bounds[self.rank]
