@@ -802,6 +802,72 @@ int raftk_rotor_stats_host(int32_t n_units, int32_t n_rows, int32_t n_dof, int32
                            const raftk_rotor_outputs *ro);
 
 /*
+ * Fatigue damage-equivalent loads (DELs) by spectral methods, for n_units units (designs, farms or designs of a flexible
+ * batch) x n_cases cases x n_ch channels.  Per (unit u, case c, channel ch), over the rows h of the case (its wave trains):
+ *   real form:    Y_h(w) = w^wpow[ch] sum_b R[ch,b] Xi[u,h,b,w]          (as raftk_general_channel_stats / raftk_farm_channel_stats)
+ *   complex form: Y_h(w) = sum_b coef[ch,b,w] Xi[u,h,b,w]                 (as raftk_channel_stats, e.g. a rigid tower's Mbase)
+ *   moments lambda_k = sum_h sum_j w_j^k 1/2 |Y_h(w_j)|^2, k = 0, 1, 2, 4  (rad/s, one-sided; lambda_0 = std^2)
+ * Dirlik (RAFTK_FATIGUE_DIRLIK): xm = (l1/l0) sqrt(l2/l4), g = l2 / sqrt(l0 l4), E[P] = sqrt(l4/l2) / 2 pi,
+ *   D1 = 2 (xm - g^2) / (1 + g^2), R = (g - xm - D1^2) / (1 - g - D1 + D1^2), D2 = (1 - g - D1 + D1^2) / (1 - R),
+ *   D3 = 1 - D1 - D2, Q = 1.25 (g - D3 - D2 R) / D1,
+ *   E[S^m] = (2 sqrt(l0))^m [D1 Q^m Gamma(1+m) + 2^(m/2) Gamma(1+m/2) (D2 |R|^m + D3)],  d = E[P] E[S^m]  (S: stress range).
+ * Narrow band (RAFTK_FATIGUE_NARROWBAND, and Dirlik's fallback): d = sqrt(l2/l0) / 2 pi (2 sqrt(2 l0))^m Gamma(1+m/2).
+ * DEL[u,c,ch] = (d / f_eq)^(1/m[ch]); DEL_life[u,ch] = (sum_c p_c d_c / (f_eq sum_c p_c))^(1/m[ch]) with p = weights (NULL:
+ * every case weighs 1).  No mean-stress correction; one S-N slope per channel.
+ * info[u,c,ch]: RAFTK_FATIGUE_ZERO when l0 or l2 is 0 (DEL exactly 0: e.g. a rotor channel at wind 0, a zero Jacobian row);
+ * RAFTK_FATIGUE_NARROWBAND when the narrow-band form gave the value -- requested, or a Dirlik request with
+ * 1 - g < RAFTK_FATIGUE_NB_SWITCH, a D1, Q or R that is not finite and positive (the narrow-band limit g -> 1, D1 -> 0,
+ * R = 0/0; a single-bin spectrum) or D2 |R|^m + D3 <= 0.  Across the switch the DEL moves by less than 1e-6 relative.
+ * d is evaluated in the log domain (lgamma, m log(2 sqrt(l0))) and exponentiated after the 1/m root, so a DEL is finite
+ * whenever it is representable, also for large loads and exponents; DEL_life sums p_c d_c scaled by its largest term.
+ * Xi complex [n_units, n_rows, n_dof, nw]; w [nw] rad/s.  Exactly one of R (R_shared 1: [n_ch, n_dof]; 0: [n_units, n_ch,
+ * n_dof]) and coef (complex; coef_mode RAFTK_FATIGUE_COEF_SHARED [n_ch, n_dof, nw], _UNIT [n_units, n_ch, n_dof, nw], _ROW
+ * [n_units, n_rows, n_ch, n_dof, nw]) is given.  Outputs: moments [n_units, n_cases, n_ch, 4] (l0, l1, l2, l4) or NULL,
+ * DEL and info [n_units, n_cases, n_ch], DEL_life [n_units, n_ch] or NULL.
+ * Kernels: one CTA per (unit, row, bin tile) stages the tile of Xi in shared memory (read from L2 when not even 32 bins fit)
+ * and reduces each channel's moments per 32-bin chunk with a fixed warp tree into the workspace; one thread per (unit, case,
+ * channel) sums the chunks in order and applies the closed form; one thread per (unit, channel) sums the cases.  No
+ * atomics: a result does not depend on the batch, the other cases or channels, or the tile width.  FP64 throughout.
+ * raftk_fatigue_workspace_bytes: n_units * n_rows * ceil(nw / 32) * n_ch * 4 doubles, plus n_units * n_cases * n_ch doubles
+ * with DEL_life.
+ * _dev: device Xi, w, R / coef and outputs, caller-owned workspace (32-byte aligned), enqueued on `stream`; it allocates
+ * nothing and never synchronises.  _host: host pointers everywhere, staged through the device arena.  case_row0, wpow, m and weights are HOST
+ * memory in both, read during the call.
+ * RAFTK_EINVAL before any launch: a count below 1, more than RAFTK_FATIGUE_CH_MAX channels, not exactly one of R and coef,
+ * R_shared not 0 or 1, an unknown coef_mode or method, a wpow outside {0, 1, 2}, a NULL w, Xi, m, case_row0, DEL or info, a
+ * case_row0 that does not start at 0 or end at n_rows or has an empty or decreasing case, an m that is not finite and > 0,
+ * an f_eq that is not finite and > 0, a negative or non-finite weight or all-zero weights, or (_dev) a workspace that is too small
+ * or not 32-byte aligned.
+ */
+#define RAFTK_FATIGUE_CH_MAX 4096
+#define RAFTK_FATIGUE_NB_SWITCH 1e-6
+enum { RAFTK_FATIGUE_DIRLIK = 0, RAFTK_FATIGUE_NARROWBAND_METHOD = 1 };
+enum { RAFTK_FATIGUE_ZERO = 1, RAFTK_FATIGUE_NARROWBAND = 2 };
+enum { RAFTK_FATIGUE_COEF_SHARED = 0, RAFTK_FATIGUE_COEF_UNIT = 1, RAFTK_FATIGUE_COEF_ROW = 2 };
+typedef struct raftk_fatigue {
+    int32_t n_cases, n_ch;
+    int32_t method;            /* RAFTK_FATIGUE_DIRLIK or RAFTK_FATIGUE_NARROWBAND_METHOD                                */
+    int32_t tile_w;            /* 0: automatic; > 0: at most tile_w bins per CTA (whole 32-bin chunks); RAFTK_FARM_TILE_L2 */
+    const int32_t *case_row0;  /* HOST [n_cases + 1]                                                                    */
+    const double *R;           /* real form, or NULL                                                                    */
+    const int32_t *wpow;       /* HOST [n_ch] 0, 1 or 2, or NULL: all 0 (real form only)                                */
+    const double *coef;        /* complex form, or NULL                                                                 */
+    int32_t R_shared, coef_mode;
+    const double *m;           /* HOST [n_ch] Woehler exponents                                                          */
+    const double *weights;     /* HOST [n_cases] or NULL                                                                 */
+    double f_eq;               /* equivalent frequency (Hz), e.g. 1 for the 1 Hz DEL                                     */
+    double *moments, *DEL;
+    int32_t *info;
+    double *DEL_life;
+} raftk_fatigue;
+
+size_t raftk_fatigue_workspace_bytes(int32_t n_units, int32_t n_rows, int32_t nw, const raftk_fatigue *fa);
+int raftk_fatigue_dev(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                      const raftk_fatigue *fa, void *workspace, size_t workspace_bytes, void *stream);
+int raftk_fatigue_host(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                       const raftk_fatigue *fa);
+
+/*
  * Natural frequencies and mode shapes (Model.solveEigen raft_model.py:436-547, FOWT.solveEigen raft_fowt.py:1646-1729): the
  * eigenvalues and right eigenvectors of M^-1 C for n_systems systems of n DOFs, what np.linalg.eig(np.linalg.solve(M, C))
  * returns, in the reference's output order.  Per system: LU of M with partial pivoting, A = M^-1 C, power-of-two balancing,

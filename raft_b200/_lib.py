@@ -121,6 +121,14 @@ class RaftkRotorOutputs(C.Structure):
                 ("V_w", C.c_void_p), ("gains", C.c_void_p), ("dw", C.c_double), ("std", C.c_void_p), ("psd", C.c_void_p)]
 
 
+class RaftkFatigue(C.Structure):
+    """include/raftk.h raftk_fatigue: channels, S-N exponents and case weights of spectral fatigue DELs, and their outputs."""
+    _fields_ = [("n_cases", C.c_int32), ("n_ch", C.c_int32), ("method", C.c_int32), ("tile_w", C.c_int32), ("case_row0", C.c_void_p),
+                ("R", C.c_void_p), ("wpow", C.c_void_p), ("coef", C.c_void_p), ("R_shared", C.c_int32), ("coef_mode", C.c_int32),
+                ("m", C.c_void_p), ("weights", C.c_void_p), ("f_eq", C.c_double), ("moments", C.c_void_p), ("DEL", C.c_void_p),
+                ("info", C.c_void_p), ("DEL_life", C.c_void_p)]
+
+
 class RaftkEigen(C.Structure):
     """include/raftk.h raftk_eigen: eigenvalues and right eigenvectors of M^-1 C for a batch of systems."""
     _fields_ = [("n_systems", C.c_int32), ("n", C.c_int32), ("sort", C.c_int32), ("_pad0", C.c_int32),
@@ -199,6 +207,7 @@ SYMBOLS = [
     "raftk_eigen_workspace_bytes", "raftk_eigen_dev", "raftk_eigen_host",
     "raftk_farm_channel_stats_workspace_bytes", "raftk_farm_channel_stats_dev", "raftk_farm_channel_stats_host",
     "raftk_rotor_stats_dev", "raftk_rotor_stats_host",
+    "raftk_fatigue_workspace_bytes", "raftk_fatigue_dev", "raftk_fatigue_host",
 ]
 
 
@@ -355,6 +364,12 @@ def _load():
     lib.raftk_rotor_stats_dev.restype = C.c_int
     lib.raftk_rotor_stats_host.argtypes = [C.c_int32] * 4 + [C.c_void_p, C.c_void_p, P(RaftkRotorOutputs)]
     lib.raftk_rotor_stats_host.restype = C.c_int
+    lib.raftk_fatigue_workspace_bytes.argtypes = [C.c_int32] * 3 + [P(RaftkFatigue)]
+    lib.raftk_fatigue_workspace_bytes.restype = C.c_size_t
+    lib.raftk_fatigue_dev.argtypes = [C.c_int32] * 4 + [C.c_void_p, C.c_void_p, P(RaftkFatigue), C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.raftk_fatigue_dev.restype = C.c_int
+    lib.raftk_fatigue_host.argtypes = [C.c_int32] * 4 + [C.c_void_p, C.c_void_p, P(RaftkFatigue)]
+    lib.raftk_fatigue_host.restype = C.c_int
     lib.raftk_family_sizes.argtypes = [P(RaftkFamily), P(C.c_int32), P(C.c_int32)]
     lib.raftk_build_family_host.argtypes = [P(RaftkFamily), P(RaftkFamilyTables)]
     lib.raftk_family_sizes.restype = C.c_int

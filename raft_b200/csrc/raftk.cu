@@ -152,6 +152,7 @@ extern "C" int raftk_last_dispatch(raftk_dispatch *out)
 #include "raftk_general.cuh"
 #include "raftk_misc.cuh"
 #include "raftk_rotor.cuh"
+#include "raftk_fatigue.cuh"
 #include "raftk_eigen.cuh"
 #include "raftk_builder.h"
 
@@ -2770,6 +2771,175 @@ extern "C" int raftk_rotor_stats_host(int32_t n_units, int32_t n_rows, int32_t n
     S.out(d.std, rows, ro->std); S.out(d.psd, ro->psd ? rows * nw : 0, ro->psd);
     int rc;
     if ((rc = S.commit()) || (rc = raftk_rotor_stats_dev(n_units, n_rows, n_dof, nw, dW, dXi, &d, nullptr))) return rc;
+    return S.finish();
+}
+
+// ---- fatigue damage-equivalent loads (raftk_fatigue_*) --------------------------------------------------------------------
+static size_t fat_part_elems(int32_t n_units, int32_t n_rows, int32_t nw, int32_t n_ch)
+{
+    return (size_t)n_units * n_rows * ((nw + FAT_CHUNK - 1) / FAT_CHUNK) * n_ch * 4;
+}
+
+static int fat_check(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi, const raftk_fatigue *fa)
+{
+    if (!fa) return set_err(RAFTK_EINVAL, "fatigue: null argument");
+    if (n_units < 1 || n_rows < 1 || n_dof < 1 || nw < 1 || fa->n_cases < 1 || fa->n_ch < 1)
+        return set_err(RAFTK_EINVAL, "fatigue: n_units, n_rows, n_dof, nw, n_cases and n_ch must be >= 1");
+    if (fa->n_ch > RAFTK_FATIGUE_CH_MAX) return set_err_i(RAFTK_EINVAL, "fatigue: at most %d channels per call", RAFTK_FATIGUE_CH_MAX);
+    if (!fa->R == !fa->coef) return set_err(RAFTK_EINVAL, "fatigue: give exactly one of R (real rows) and coef (complex coefficients)");
+    if (fa->R && fa->R_shared != 0 && fa->R_shared != 1) return set_err(RAFTK_EINVAL, "fatigue: R_shared must be 0 or 1");
+    if (fa->coef && (fa->coef_mode < RAFTK_FATIGUE_COEF_SHARED || fa->coef_mode > RAFTK_FATIGUE_COEF_ROW))
+        return set_err(RAFTK_EINVAL, "fatigue: unknown coef_mode");
+    if (fa->method != RAFTK_FATIGUE_DIRLIK && fa->method != RAFTK_FATIGUE_NARROWBAND_METHOD)
+        return set_err(RAFTK_EINVAL, "fatigue: unknown method");
+    if (!w || !Xi || !fa->m || !fa->case_row0 || !fa->DEL || !fa->info)
+        return set_err(RAFTK_EINVAL, "fatigue: w, Xi, m, case_row0, DEL and info are required");
+    for (int32_t t = 0; fa->R && fa->wpow && t < fa->n_ch; t++)
+        if (fa->wpow[t] < 0 || fa->wpow[t] > 2) return set_err(RAFTK_EINVAL, "fatigue: wpow must be 0, 1 or 2");
+    if (fa->case_row0[0] != 0 || fa->case_row0[fa->n_cases] != n_rows)
+        return set_err(RAFTK_EINVAL, "fatigue: case_row0 must start at 0 and end at n_rows");
+    for (int32_t c = 0; c < fa->n_cases; c++)
+        if (fa->case_row0[c + 1] <= fa->case_row0[c]) return set_err(RAFTK_EINVAL, "fatigue: every case needs at least one row");
+    for (int32_t t = 0; t < fa->n_ch; t++)
+        if (!(std::isfinite(fa->m[t]) && fa->m[t] > 0.0)) return set_err(RAFTK_EINVAL, "fatigue: every m must be finite and > 0");
+    if (!(std::isfinite(fa->f_eq) && fa->f_eq > 0.0)) return set_err(RAFTK_EINVAL, "fatigue: f_eq must be finite and > 0");
+    if (fa->weights) {
+        double s = 0.0;
+        for (int32_t c = 0; c < fa->n_cases; c++) {
+            if (!(std::isfinite(fa->weights[c]) && fa->weights[c] >= 0.0)) return set_err(RAFTK_EINVAL, "fatigue: weights must be finite and >= 0");
+            s += fa->weights[c];
+        }
+        if (!(s > 0.0)) return set_err(RAFTK_EINVAL, "fatigue: the weights must not all be 0");
+    }
+    const size_t rows = (size_t)n_units * n_rows;
+    if (rows * ((nw + FAT_CHUNK - 1) / FAT_CHUNK) > 2147483647u || (size_t)n_units * fa->n_ch > 2147483647u)
+        return set_err(RAFTK_EINVAL, "fatigue: too many (unit, row, bin tile) blocks");
+    return RAFTK_OK;
+}
+
+static size_t fat_ws(int32_t n_units, int32_t n_rows, int32_t nw, const raftk_fatigue *fa)
+{
+    return (fat_part_elems(n_units, n_rows, nw, fa->n_ch) + (fa->DEL_life ? (size_t)n_units * fa->n_cases * fa->n_ch : 0)) * sizeof(double);
+}
+
+// Bins per CTA, whole FAT_CHUNK chunks: at most what the opt-in shared memory holds (n x 16 bytes per bin) and 256, fewer when
+// the batch alone would leave SMs idle; 0 when not even one chunk fits (Xi is then read from L2).  tile_w > 0 caps it.
+static int fat_tile(size_t n_rows_total, int32_t n_dof, int32_t nw, int32_t tile_w)
+{
+    if (tile_w == RAFTK_FARM_TILE_L2) return 0;
+    const int round_nw = (nw + FAT_CHUNK - 1) / FAT_CHUNK * FAT_CHUNK;
+    const int tmax = (int)std::min<size_t>((size_t)round_nw, smem_optin() / ((size_t)n_dof * sizeof(double2))) / FAT_CHUNK * FAT_CHUNK;
+    if (tmax < FAT_CHUNK) return 0;
+    if (tile_w > 0) return std::max(FAT_CHUNK, std::min(tmax, (int)tile_w / FAT_CHUNK * FAT_CHUNK));
+    const long long want = (2LL * sm_count() + (long long)n_rows_total - 1) / (long long)n_rows_total;   // tiles per (unit, row)
+    const int split = (int)((nw + want - 1) / want + FAT_CHUNK - 1) / FAT_CHUNK * FAT_CHUNK;
+    return std::min(std::min(tmax, 256), std::max(FAT_CHUNK, split));
+}
+
+extern "C" size_t raftk_fatigue_workspace_bytes(int32_t n_units, int32_t n_rows, int32_t nw, const raftk_fatigue *fa)
+{
+    if (!fa || n_units < 1 || n_rows < 1 || nw < 1 || fa->n_cases < 1 || fa->n_ch < 1) return 0;
+    return fat_ws(n_units, n_rows, nw, fa);
+}
+
+extern "C" int raftk_fatigue_dev(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                                 const raftk_fatigue *fa, void *workspace, size_t workspace_bytes, void *stream)
+{
+    if (int rc = fat_check(n_units, n_rows, n_dof, nw, w, Xi, fa)) return rc;
+    if (!workspace || workspace_bytes < fat_ws(n_units, n_rows, nw, fa))
+        return set_err(RAFTK_EINVAL, "fatigue: the workspace is too small (raftk_fatigue_workspace_bytes)");
+    if ((uintptr_t)workspace % 32) return set_err(RAFTK_EINVAL, "fatigue: the workspace must be 32-byte aligned");
+    const cudaStream_t st = (cudaStream_t)stream;
+    const size_t rows = (size_t)n_units * n_rows;
+    double *part = static_cast<double *>(workspace);
+    double *wd = fa->DEL_life ? part + fat_part_elems(n_units, n_rows, nw, fa->n_ch) : nullptr;
+    FatMomParams P = {};
+    P.n = n_dof; P.nch = fa->n_ch; P.nw = nw; P.n_rows = n_rows;
+    P.n_chunks = (nw + FAT_CHUNK - 1) / FAT_CHUNK;
+    P.w = w; P.R = fa->R; P.Xi = reinterpret_cast<const double2 *>(Xi); P.part = part;
+    P.coef = reinterpret_cast<const double2 *>(fa->coef);
+    const size_t cf = (size_t)fa->n_ch * n_dof * nw;
+    P.r_stride = fa->R_shared ? 0 : (size_t)fa->n_ch * n_dof;
+    P.cf_ustride = fa->coef_mode == RAFTK_FATIGUE_COEF_UNIT ? cf : (fa->coef_mode == RAFTK_FATIGUE_COEF_ROW ? cf * n_rows : 0);
+    P.cf_rstride = fa->coef_mode == RAFTK_FATIGUE_COEF_ROW ? cf : 0;
+    for (int32_t t = 0; fa->R && fa->wpow && t < fa->n_ch; t++) P.wbits[t >> 4] |= (unsigned)fa->wpow[t] << ((t & 15) * 2);
+    const int tile = fat_tile(rows, n_dof, nw, fa->tile_w);
+    P.tile = tile ? tile : std::min<int32_t>((nw + FAT_CHUNK - 1) / FAT_CHUNK * FAT_CHUNK, 256);
+    P.n_tiles = (nw + P.tile - 1) / P.tile;
+    const size_t grid = rows * P.n_tiles;
+    const bool coef = fa->coef != nullptr;
+    if (tile) {
+        const size_t smem = (size_t)n_dof * tile * sizeof(double2);
+        static SmemOptIn opt_r(48 * 1024), opt_c(48 * 1024);
+        if (coef) {
+            CUDA_TRY(opt_c.ensure(k_fatigue_moments<true, true>, smem));
+            k_fatigue_moments<true, true><<<(unsigned)grid, FAT_T, smem, st>>>(P);
+        } else {
+            CUDA_TRY(opt_r.ensure(k_fatigue_moments<true, false>, smem));
+            k_fatigue_moments<true, false><<<(unsigned)grid, FAT_T, smem, st>>>(P);
+        }
+    } else if (coef) {
+        k_fatigue_moments<false, true><<<(unsigned)grid, FAT_T, 0, st>>>(P);
+    } else {
+        k_fatigue_moments<false, false><<<(unsigned)grid, FAT_T, 0, st>>>(P);
+    }
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    // chunks of cases and channels only bound the launch parameters: every thread computes the same thing in any chunk
+    FatFinParams F = {};
+    F.n_rows = n_rows; F.n_cases = fa->n_cases; F.nch = fa->n_ch; F.n_chunks = P.n_chunks; F.method = fa->method;
+    F.f_eq = fa->f_eq; F.part = part; F.moments = fa->moments; F.DEL = fa->DEL; F.wd = wd; F.info = fa->info;
+    for (int32_t c0 = 0; c0 < fa->n_cases; c0 += FAT_LAUNCH_CHUNK) {
+        F.c0 = c0; F.nc = std::min<int32_t>(FAT_LAUNCH_CHUNK, fa->n_cases - c0);
+        for (int j = 0; j <= F.nc; j++) F.row0[j] = fa->case_row0[c0 + j];
+        for (int j = 0; j < F.nc; j++) F.p[j] = fa->weights ? fa->weights[c0 + j] : 1.0;
+        for (int32_t k0 = 0; k0 < fa->n_ch; k0 += FAT_LAUNCH_CHUNK) {
+            F.k0 = k0; F.nk = std::min<int32_t>(FAT_LAUNCH_CHUNK, fa->n_ch - k0);
+            for (int j = 0; j < F.nk; j++) F.m[j] = fa->m[k0 + j];
+            const size_t nt = (size_t)n_units * F.nc * F.nk;
+            k_fatigue_finish<<<(unsigned)((nt + FAT_FIN_T - 1) / FAT_FIN_T), FAT_FIN_T, 0, st>>>(F, nt);
+            g_launches++;
+            CUDA_TRY(cudaGetLastError());
+        }
+    }
+    if (fa->DEL_life) {
+        FatLifeParams L = {};
+        double W = 0.0;
+        for (int32_t c = 0; c < fa->n_cases; c++) W += fa->weights ? fa->weights[c] : 1.0;
+        L.n_cases = fa->n_cases; L.nch = fa->n_ch; L.log_fw = std::log(fa->f_eq * W); L.wd = wd; L.DEL_life = fa->DEL_life;
+        for (int32_t k0 = 0; k0 < fa->n_ch; k0 += FAT_LAUNCH_CHUNK) {
+            L.k0 = k0; L.nk = std::min<int32_t>(FAT_LAUNCH_CHUNK, fa->n_ch - k0);
+            for (int j = 0; j < L.nk; j++) L.m[j] = fa->m[k0 + j];
+            const size_t nt = (size_t)n_units * L.nk;
+            k_fatigue_life<<<(unsigned)((nt + FAT_FIN_T - 1) / FAT_FIN_T), FAT_FIN_T, 0, st>>>(L, nt);
+            g_launches++;
+            CUDA_TRY(cudaGetLastError());
+        }
+    }
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_fatigue_host(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                                  const raftk_fatigue *fa)
+{
+    if (int rc = fat_check(n_units, n_rows, n_dof, nw, w, Xi, fa)) return rc;
+    const size_t out = (size_t)n_units * fa->n_cases * fa->n_ch, nch = fa->n_ch;
+    const size_t wb = fat_ws(n_units, n_rows, nw, fa);
+    size_t n_coef = 0;
+    if (fa->coef)
+        n_coef = (fa->coef_mode == RAFTK_FATIGUE_COEF_SHARED ? 1 : (size_t)n_units) * (fa->coef_mode == RAFTK_FATIGUE_COEF_ROW ? n_rows : 1)
+                 * nch * n_dof * nw * 2;
+    raftk_fatigue d = *fa;
+    const double *dW, *dXi;
+    char *ws;
+    Staging S("raftk_fatigue_host");
+    S.in(dW, w, nw); S.in(dXi, Xi, (size_t)n_units * n_rows * n_dof * nw * 2);
+    S.in(d.R, fa->R, (fa->R_shared ? 1 : (size_t)n_units) * nch * n_dof); S.in(d.coef, fa->coef, n_coef);
+    S.out(d.moments, fa->moments ? out * 4 : 0, fa->moments); S.out(d.DEL, out, fa->DEL); S.out(d.info, out, fa->info);
+    S.out(d.DEL_life, fa->DEL_life ? (size_t)n_units * nch : 0, fa->DEL_life);
+    S.buf(ws, wb);
+    int rc;
+    if ((rc = S.commit()) || (rc = raftk_fatigue_dev(n_units, n_rows, n_dof, nw, dW, dXi, &d, ws, wb, nullptr))) return rc;
     return S.finish();
 }
 

@@ -14,7 +14,7 @@ from .fowt import FOWT
 
 class Model:
     def __init__(self, design, matrices=None, array_stiffness=None, channels=None, tension_jacobian=None, mean_tensions=None,
-                 array_tension_jacobian=None, array_mean_tensions=None, rotors=None, turbine_constants=None):
+                 array_tension_jacobian=None, array_mean_tensions=None, rotors=None, turbine_constants=None, fatigue=None):
         """``channels``: optional turbine output channels per FOWT (``packer.pack_turbine_channels`` dicts: nacelle
         accelerations, tower-base moment) -- the turbine itself is outside this path, its constants enter here.
         ``tension_jacobian`` [2L,6] / ``mean_tensions`` [2L] (one for every FOWT, or a list with None for a FOWT without its
@@ -30,7 +30,12 @@ class Model:
         B_aero, B_gyro; ``packer.pack_operating_points``).  Every case is then solved with its own aero-servo added mass and
         damping (raft_model.py:1005-1010, 1045-1046), on top of the case-independent ``matrices``; ``channels`` may then be
         a per-case list of ``pack_turbine_channels`` dicts per FOWT, taken after each case's calcTurbineConstants, so that
-        Mbase's aero reaction and mean follow the case too."""
+        Mbase's aero reaction and mean follow the case too.
+        ``fatigue``: dict(m={channel name: Woehler exponent}, f_eq=1.0, method="dirlik", weights=None)
+        (``solver.fatigue_options``), e.g. m={"Mbase": 4.0, "Tmoor": 3.0}: analyzeCases then adds, per case and FOWT,
+        ``<name>_DEL`` of the named turbine channels ([nrot]) and ``Tmoor_DEL`` [2L] of the FOWT's lines,
+        case_metrics[iCase]['array_mooring']['Tmoor_DEL'] of the array's, and with weights the lifetime DELs in
+        results['fatigue'] (the same keys per FOWT, and 'array_mooring').  Without it the results are unchanged."""
         s = design.setdefault("settings", {})
         min_freq, max_freq = float(s.get("min_freq", 0.01)), float(s.get("max_freq", 1.00))
         self.XiStart = float(s.get("XiStart", 0.1))
@@ -81,6 +86,13 @@ class Model:
                 raise ValueError("tension_jacobian must be [2L, 6]")
         if self.array_tensions is not None and self.array_tensions["J"].shape[1] != self.nDOF:
             raise ValueError("array_tension_jacobian must be [2L, %d]" % self.nDOF)
+        self.fatigue = None if fatigue is None else solver.fatigue_options(fatigue)
+        if self.fatigue is not None:
+            known = {"Tmoor"} | {nm for ch in self.channels if ch is not None
+                                 for nm, _ in (ch[0] if isinstance(ch, (list, tuple)) else ch)["names"]}
+            missing = sorted(set(self.fatigue["m"]) - known)
+            if missing:
+                raise ValueError("fatigue=: no channel named %s" % missing)
         for f in self.fowtList:
             f.calcHydroConstants()
 
@@ -136,6 +148,7 @@ class Model:
         arr = None if self.array_tensions is None else solver.farm_channel_stats(self.array_tensions["J"], out["Xi_all"], w0)
         dw = self.w[1] - self.w[0]
         rot = self._rotor_stats(cases, out, dw)
+        fat = None if self.fatigue is None else self._fatigue(cases, out, Xi_units)
         self.results["case_metrics"] = {}
         for ic in range(nC):
             idx = np.nonzero(owner == ic)[0]
@@ -167,11 +180,59 @@ class Model:
                 if self.rotors[i] is not None:
                     k = rot[1][i]
                     m.update(solver.rotor_metrics(self.rotors[i], ic, rot[0][0][ic, k], rot[0][1][ic, k], dw))
+                if fat is not None:
+                    m.update(fat["case"][ic][i])
                 self.results["case_metrics"][ic][i] = m
             if arr is not None:
                 self.results["case_metrics"][ic]["array_mooring"] = solver.tension_metrics(self.array_tensions["T0"],
                                                                                            *solver.combine_trains(arr[0], arr[1], idx))
+                if fat is not None and "array_mooring" in fat["case"][ic]:
+                    self.results["case_metrics"][ic]["array_mooring"].update(fat["case"][ic]["array_mooring"])
+        if fat is not None and fat["life"] is not None:
+            self.results["fatigue"] = fat["life"]
         return self.results
+
+    def _fatigue(self, cases, out, Xi_units):
+        """Fatigue DELs of every case (``fatigue=``) on the device: each FOWT's named turbine channels (their coefficients,
+        per case when ``channels`` is a per-case list) and lines on its trains Xi_units [nT, nFOWT, 6, nw], the array's lines
+        on the coupled response.  -> dict(case=[{FOWT i: entries, 'array_mooring': entries}], life={...} or None)."""
+        o = self.fatigue
+        nC, owner = len(cases), out["owner"]
+        row0 = np.append(np.nonzero(np.diff(np.append(-1, owner)))[0], len(owner))
+        kw = dict(case_row0=row0, f_eq=o["f_eq"], method=o["method"], weights=o["weights"], moments=False)
+        case = [dict() for _ in range(nC)]
+        life = {} if o["weights"] is not None else None
+
+        def put(key, sel, r):
+            for ic in range(nC):
+                case[ic].setdefault(key, {}).update(solver.fatigue_entries(sel, r["DEL"][ic]))
+            if life is not None:
+                life.setdefault(key, {}).update(solver.fatigue_entries(sel, r["DEL_life"]))
+        for i in range(self.nFOWT):
+            ch = self.channels[i]
+            if ch is not None:
+                per_case = isinstance(ch, (list, tuple))
+                sel = solver.fatigue_selection((ch[0] if per_case else ch)["names"], o["m"])
+                if sel:
+                    ks = [s_[1] for s_ in sel]
+                    ms = [s_[3] for s_ in sel]
+                    if per_case:
+                        coef = np.stack([np.asarray(ch[c]["coef"])[ks] for c in owner])[None]      # [1, nT, nsel, 6, nw]
+                        r = {k: v[0] for k, v in solver.fatigue(Xi_units[None, :, i], self.w, ms, coef=coef, **kw).items()}
+                    else:
+                        r = solver.fatigue(Xi_units[:, i], self.w, ms, coef=np.asarray(ch["coef"])[ks], **kw)
+                    put(i, sel, r)
+            if self.tensions[i] is not None and "Tmoor" in o["m"]:
+                J = self.tensions[i]["J"]
+                sel = [("Tmoor", k, k, float(o["m"]["Tmoor"])) for k in range(len(J))]
+                put(i, sel, solver.fatigue(Xi_units[:, i], self.w, o["m"]["Tmoor"], R=J, **kw))
+            for ic in range(nC):
+                case[ic].setdefault(i, {})
+        if self.array_tensions is not None and "Tmoor" in o["m"]:
+            J = self.array_tensions["J"]
+            sel = [("Tmoor", k, k, float(o["m"]["Tmoor"])) for k in range(len(J))]
+            put("array_mooring", sel, solver.fatigue(out["Xi_all"], self.w, o["m"]["Tmoor"], R=J, **kw))
+        return dict(case=case, life=life)
 
     def _channel_stats(self, ch, Xi, owner, nC):
         """Turbine channel statistics of one FOWT on its trains Xi [nT, 6, nw]: ``ch`` one pack_turbine_channels dict, or one

@@ -932,6 +932,16 @@ class GeneralSession:
                                                  self.dw, case_row0, None, psd)
         return sd[0], (P[0] if psd else None)
 
+    def fatigue(self, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, method="dirlik", weights=None, life=None,
+                moments=True, tile_w=0):
+        """Fatigue DELs of the last ``solve()`` on the device (raftk_fatigue_dev, no host round trip): ``R`` [nch, nDOF] with
+        ``wpow`` (``packer.pack_general_channels``' rows) or ``coef``, and the other arguments as ``fatigue``; ``case_row0``
+        groups the trains into cases.  -> dict of torch tensors as ``fatigue`` without the unit axis."""
+        stream = self.torch.cuda.current_stream(self.device).cuda_stream
+        out, self._fat_keep = _fatigue_dev(self.torch, self.device, stream, self.Xi[None], self.keep["w"], m, R, wpow, coef, case_row0,
+                                           f_eq, method, weights, life, moments, tile_w)
+        return {k: v[0] for k, v in out.items()}
+
 
 def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0, fd=None, F_BEM=False, qtf=None, F_2nd=False,
                            max_chunk_cases=None):
@@ -1214,6 +1224,195 @@ def rotor_metrics(rotors, ic, std, psd, dw):
     return m
 
 
+FATIGUE_METHODS = {"dirlik": 0, "narrowband": 1}
+FATIGUE_ZERO, FATIGUE_NARROWBAND = 1, 2          # info bits (include/raftk.h RAFTK_FATIGUE_ZERO / _NARROWBAND)
+
+
+def _fatigue_struct(n_units, n_rows, n, nw, m, R, wpow, coef, case_row0, f_eq, method, weights, tile_w):
+    """Shapes and options of fatigue's inputs (R / coef numpy arrays or torch tensors) checked -> (raftk_fatigue without data
+    pointers, the host arrays it points to).  R [nch, n] (every unit) or [n_units, nch, n]; coef [nch, n, nw] (every unit),
+    [n_units, nch, n, nw] or [n_units, n_rows, nch, n, nw] (one set per row, e.g. per-case operating points)."""
+    if (R is None) == (coef is None):
+        raise ValueError("fatigue: give exactly one of R (real rows) and coef (complex coefficients)")
+    fa = _lib.RaftkFatigue()
+    if R is not None:
+        if len(R.shape) not in (2, 3) or (len(R.shape) == 3 and R.shape[0] != n_units) or R.shape[-1] != n:
+            raise ValueError("R must be [nch, %d] or [%d, nch, %d]" % (n, n_units, n))
+        nch = R.shape[-2]
+        fa.R_shared = int(len(R.shape) == 2)
+        wpow = np.zeros(nch, dtype=_I4) if wpow is None else np.ascontiguousarray(wpow, dtype=_I4)
+        if wpow.shape != (nch,):
+            raise ValueError("wpow must be [nch]")
+        _check_wpow(wpow)
+    else:
+        lead = {3: (), 4: (n_units,), 5: (n_units, n_rows)}.get(len(coef.shape))
+        if lead is None or tuple(coef.shape[:len(lead)]) != lead or tuple(coef.shape[-2:]) != (n, nw):
+            raise ValueError("coef must be [nch, %d, %d], [%d, nch, %d, %d] or [%d, %d, nch, %d, %d]" % (n, nw, n_units, n, nw, n_units, n_rows, n, nw))
+        nch = coef.shape[-3]
+        fa.coef_mode = len(coef.shape) - 3
+        if wpow is not None:
+            raise ValueError("wpow applies to real rows R only")
+    m = np.ascontiguousarray(np.broadcast_to(np.asarray(m, dtype=_F8), (nch,)))
+    if not (np.all(np.isfinite(m)) and np.all(m > 0)):
+        raise ValueError("every m must be finite and > 0")
+    if not (np.isfinite(f_eq) and f_eq > 0):
+        raise ValueError("f_eq must be finite and > 0")
+    if method not in FATIGUE_METHODS:
+        raise ValueError("method must be one of %s" % sorted(FATIGUE_METHODS))
+    nC = n_rows if case_row0 is None else len(case_row0) - 1
+    case_row0 = np.arange(nC + 1, dtype=_I4) if case_row0 is None else np.ascontiguousarray(case_row0, dtype=_I4)
+    if nC < 1 or case_row0[0] != 0 or case_row0[-1] != n_rows or np.any(np.diff(case_row0) < 1):
+        raise ValueError("case_row0 must start at 0, end at %d and give every case at least one row" % n_rows)
+    if weights is not None:
+        weights = np.ascontiguousarray(weights, dtype=_F8)
+        if weights.shape != (nC,) or not np.all(np.isfinite(weights)) or np.any(weights < 0) or not weights.sum() > 0:
+            raise ValueError("weights must be [nC], finite, >= 0 and not all 0")
+    fa.n_cases, fa.n_ch, fa.method, fa.tile_w = nC, nch, FATIGUE_METHODS[method], int(tile_w)
+    fa.case_row0, fa.m, fa.f_eq = case_row0.ctypes.data, m.ctypes.data, float(f_eq)
+    fa.wpow = wpow.ctypes.data if R is not None else None
+    fa.weights = weights.ctypes.data if weights is not None else None
+    return fa, (case_row0, m, wpow, weights)
+
+
+def fatigue(Xi, w, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, method="dirlik", weights=None, life=None,
+            moments=True, tile_w=0):
+    """Spectral fatigue damage-equivalent loads on the device (raftk_fatigue_host), host buffers.  Per unit, case and channel
+    the moments lambda_k = sum over the case's rows and bins of w^k |Y|^2 / 2 (k = 0, 1, 2, 4) of the channel Y = w^wpow R Xi
+    (real rows) or Y = sum_b coef[b] Xi[b] (complex per-bin coefficients), then Dirlik's closed form (``method="dirlik"``,
+    narrow band where the spectrum is too narrow for it) or the narrow-band form (``"narrowband"``) of the damage rate d,
+    and DEL = (d / f_eq)^(1/m).  ``Xi`` complex [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]; ``w`` [nw] rad/s; ``m``
+    the Woehler exponent, scalar or [nch]; ``R`` / ``coef`` as ``_fatigue_struct``; ``case_row0`` [nC + 1] the first row of
+    every case (None: one row per case); ``weights`` [nC] case probabilities; ``life`` (default: weights given) adds DEL_life
+    = (sum_c p_c d_c / (f_eq sum_c p_c))^(1/m).  -> dict(DEL [n_units, nC, nch], info int32 (FATIGUE_ZERO, FATIGUE_NARROWBAND
+    bits), moments [n_units, nC, nch, 4] (l0, l1, l2, l4) or absent, DEL_life [n_units, nch] or absent), without the unit
+    axis when ``Xi`` had none.  ``tile_w``: bins per CTA (0 automatic, -1 reads Xi from L2); the results do not depend on it."""
+    Xi = np.ascontiguousarray(Xi, dtype=np.complex128)
+    squeeze = Xi.ndim == 3
+    if squeeze:
+        Xi = Xi[None]
+    if Xi.ndim != 4:
+        raise ValueError("Xi must be [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]")
+    nU, nR, n, nw = Xi.shape
+    w = np.ascontiguousarray(w, dtype=_F8)
+    if w.shape != (nw,):
+        raise ValueError("w must be [nw]")
+    R = None if R is None else np.ascontiguousarray(R, dtype=_F8)
+    coef = None if coef is None else np.ascontiguousarray(coef, dtype=np.complex128)
+    fa, keep = _fatigue_struct(nU, nR, n, nw, m, R, wpow, coef, case_row0, f_eq, method, weights, tile_w)
+    life = weights is not None if life is None else bool(life)
+    nC, nch = fa.n_cases, fa.n_ch
+    out = dict(DEL=np.zeros([nU, nC, nch]), info=np.zeros([nU, nC, nch], dtype=_I4))
+    if moments:
+        out["moments"] = np.zeros([nU, nC, nch, 4])
+    if life:
+        out["DEL_life"] = np.zeros([nU, nch])
+    fa.R = R.ctypes.data if R is not None else None
+    fa.coef = coef.ctypes.data if coef is not None else None
+    fa.DEL, fa.info = out["DEL"].ctypes.data, out["info"].ctypes.data
+    fa.moments = out["moments"].ctypes.data if moments else None
+    fa.DEL_life = out["DEL_life"].ctypes.data if life else None
+    check(lib.raftk_fatigue_host(nU, nR, n, nw, w.ctypes.data, Xi.ctypes.data, C.byref(fa)))
+    return {k: v[0] for k, v in out.items()} if squeeze else out
+
+
+def _fatigue_dev(torch, device, stream, Xi, w, m, R, wpow, coef, case_row0, f_eq, method, weights, life, moments, tile_w):
+    """fatigue on a resident Xi [n_units, n_rows, n_dof, nw] (torch, complex128) and w; R / coef numpy arrays or torch tensors
+    -> (dict of torch tensors as ``fatigue``, tensors the enqueued launches still read), enqueued on ``stream``
+    (raftk_fatigue_dev)."""
+    nU, nR, n, nw = Xi.shape
+    with torch.cuda.device(device):
+        if R is not None:
+            R = R.to(device=device, dtype=torch.float64).contiguous() if isinstance(R, torch.Tensor) else \
+                torch.from_numpy(np.ascontiguousarray(R, dtype=_F8)).to(device)
+        if coef is not None:
+            coef = coef.to(device=device, dtype=torch.complex128).contiguous() if isinstance(coef, torch.Tensor) else \
+                torch.from_numpy(np.ascontiguousarray(coef, dtype=np.complex128)).to(device)
+        fa, _ = _fatigue_struct(nU, nR, n, nw, m, R, wpow, coef, case_row0, f_eq, method, weights, tile_w)
+        life = weights is not None if life is None else bool(life)
+        nC, nch = fa.n_cases, fa.n_ch
+        out = dict(DEL=torch.empty([nU, nC, nch], dtype=torch.float64, device=device),
+                   info=torch.empty([nU, nC, nch], dtype=torch.int32, device=device))
+        if moments:
+            out["moments"] = torch.empty([nU, nC, nch, 4], dtype=torch.float64, device=device)
+        if life:
+            out["DEL_life"] = torch.empty([nU, nch], dtype=torch.float64, device=device)
+        fa.R = R.data_ptr() if R is not None else None
+        fa.coef = coef.data_ptr() if coef is not None else None
+        fa.DEL, fa.info = out["DEL"].data_ptr(), out["info"].data_ptr()
+        fa.moments = out["moments"].data_ptr() if moments else None
+        fa.DEL_life = out["DEL_life"].data_ptr() if life else None
+        wsb = int(lib.raftk_fatigue_workspace_bytes(nU, nR, nw, C.byref(fa)))
+        ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=device)
+        check(lib.raftk_fatigue_dev(nU, nR, n, nw, w.data_ptr(), Xi.data_ptr(), C.byref(fa), ws.data_ptr(), wsb, stream))
+    return out, (R, coef, ws)
+
+
+def fatigue_options(fatigue):
+    """The ``fatigue=`` option of ``Model``, ``general_analyze_cases`` and ``general_analyze_cases_batch``:
+    dict(m={channel name: Woehler exponent}, f_eq=1.0, method="dirlik", weights=None) -> the same dict, checked and completed.
+    Channel names are those of the channels (``Mbase``, ``AxRNA``, ``FbaseX`` .. ``MbaseZ``, ``surge`` ...) and ``Tmoor`` for
+    mooring line-end tensions; ``weights`` [nCases] adds the lifetime DELs (``results['fatigue']``)."""
+    if not isinstance(fatigue, dict) or not isinstance(fatigue.get("m"), dict) or not fatigue["m"]:
+        raise ValueError("fatigue= must be a dict with m = {channel name: Woehler exponent}, e.g. dict(m={'Mbase': 4.0})")
+    bad = sorted(set(fatigue) - {"m", "f_eq", "method", "weights"})
+    if bad:
+        raise ValueError("fatigue=: unknown option(s) %s" % bad)
+    for nm, e in fatigue["m"].items():
+        if not (np.isfinite(e) and e > 0):
+            raise ValueError("fatigue=: the exponent of %r must be finite and > 0" % nm)
+    return dict(m=dict(fatigue["m"]), f_eq=float(fatigue.get("f_eq", 1.0)), method=fatigue.get("method", "dirlik"),
+                weights=fatigue.get("weights"))
+
+
+def fatigue_selection(names, m):
+    """The DEL outputs of channels ``names`` [(name, index or None)] under exponents ``m`` -> [(output name, row, index,
+    exponent)].  A flexible tower's ``Mbase`` is the alias of its ``MbaseY`` (raft_fowt.py:2599-2604), so m['Mbase'] also
+    selects the MbaseY rows when no channel is called Mbase."""
+    plain = {nm for nm, _ in names}
+    sel = []
+    for k, (nm, ir) in enumerate(names):
+        if nm in m:
+            sel.append((nm, k, ir, float(m[nm])))
+        if nm == "MbaseY" and "Mbase" in m and "Mbase" not in plain:
+            sel.append(("Mbase", k, ir, float(m["Mbase"])))
+    return sel
+
+
+def fatigue_entries(sel, DEL):
+    """``<name>_DEL`` entries of one case (or of the lifetime) from the DELs [len(sel)] of ``fatigue_selection``'s outputs:
+    a scalar for a channel without index, else an array over the index (rotors [nrot], line ends [2L])."""
+    size = {}
+    for nm, _, ir, _ in sel:
+        if ir is not None:
+            size[nm] = max(size.get(nm, 0), ir + 1)
+    out = {}
+    for j, (nm, _, ir, _) in enumerate(sel):
+        if ir is None:
+            out[nm + "_DEL"] = float(DEL[j])
+        else:
+            out.setdefault(nm + "_DEL", np.zeros(size[nm]))[ir] = DEL[j]
+    return out
+
+
+def _general_fatigue(opts, channels, P, Xi, owner, first, n_cases, metrics, out):
+    """general_analyze_cases' fatigue= on one design: the DELs of the named channels into every case's metrics, the lifetime
+    DELs into out['fatigue'] when weights are given."""
+    if channels is None:
+        raise ValueError("fatigue= needs channels (packer.pack_general_channels)")
+    sel = fatigue_selection(channels["names"], opts["m"])
+    missing = sorted(set(opts["m"]) - {s[0] for s in sel})
+    if missing:
+        raise ValueError("fatigue=: no channel named %s" % missing)
+    rows = [s[1] for s in sel]
+    r = fatigue(Xi, P["w"], [s[3] for s in sel], R=np.asarray(channels["R"])[rows], wpow=np.asarray(channels["wpow"])[rows],
+                case_row0=np.append(first, len(owner)), f_eq=opts["f_eq"], method=opts["method"], weights=opts["weights"],
+                moments=False)
+    for ic in range(n_cases):
+        metrics.setdefault(ic, {}).update(fatigue_entries(sel, r["DEL"][ic]))
+    if "DEL_life" in r:
+        out["fatigue"] = fatigue_entries(sel, r["DEL_life"])
+
+
 def general_case_metrics(channels, std, psd, amp, idx, dw=None):
     """The entries FOWT.saveTurbineOutputs stores for one case (raft_fowt.py:2299-2604) from per-train channel statistics
     (std [nT,nch], PSD [nT,nch,nw], amplitudes [nT,nch,nw]) of the case's trains ``idx``: ``*_avg/_std/_max/_min/_PSD`` of every
@@ -1256,7 +1455,7 @@ def general_case_metrics(channels, std, psd, amp, idx, dw=None):
 
 
 def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, fd=None, qtf=None, rotors=None,
-                          turbine_constants=None, ops=None):
+                          turbine_constants=None, ops=None, fatigue=None):
     """Model.analyzeCases (dynamics and output statistics) for one FOWT with generalised degrees of freedom: ``cases`` a list
     of case dicts, scalar or list-valued wave keys (several wave trains); ``channels`` from ``packer.pack_general_channels``.
     -> dict(Xi_trains [per case: nTrains,nDOF,nw], status [nC,4] of train 0, case_metrics {case: saveTurbineOutputs entries},
@@ -1267,17 +1466,21 @@ def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01
     (omega / torque / bPitch / power, wind_PSD; ``rotor_metrics``).  ``ops``: per-case operating points, one per case of
     ``cases`` (op [nC]; ``packer.pack_general_matrices(fowt, states=...)['ops']``, whose M, B and fd then go with it): every
     wave train of a case is solved at its case's point.  ``turbine_constants`` (raw per-case snapshots, as
-    ``Model(turbine_constants=)``): NotImplementedError, since M, B and fd come here already packed."""
+    ``Model(turbine_constants=)``): NotImplementedError, since M, B and fd come here already packed.
+    ``fatigue``: dict(m={channel name: Woehler exponent}, f_eq=1.0, method="dirlik", weights=None) (``fatigue_options``)
+    adds every case's ``<name>_DEL`` of the named channels (per-rotor channels [nrot], ``Tmoor_DEL`` [2L], ``Mbase_DEL`` the
+    alias of ``MbaseY_DEL``) and, with weights, the lifetime DELs in the result's ``fatigue``.  Without it nothing changes."""
     from .packer import pack_case_trains
     _no_general_ops(turbine_constants)
+    opts = None if fatigue is None else fatigue_options(fatigue)
     table, owner, first = pack_case_trains(cases)
     q = bool(qtf)
     res = general_solve_dynamics(P, M, B, Cm, CaseTable(table, ops=_train_ops(ops, owner, len(cases))), n_iter=n_iter, tol=tol,
                                  xi_start=xi_start, fd=fd, qtf=qtf, F_2nd=q)
-    return _general_case_results(P, res[0], res[1], owner, first, len(cases), channels, res[2:4] if q else None, rotors)
+    return _general_case_results(P, res[0], res[1], owner, first, len(cases), channels, res[2:4] if q else None, rotors, opts)
 
 
-def _general_case_results(P, Xi, st, owner, first, n_cases, channels, F2nd, rotors=None):
+def _general_case_results(P, Xi, st, owner, first, n_cases, channels, F2nd, rotors=None, fatigue=None):
     """general_analyze_cases' result for one design from its train table's Xi [nT,nDOF,nw], status [nT,4] and, with a QTF
     table, (F_2nd [nT,6,nw], F_2nd_mean [nT,6])."""
     raise_on_flags(st[first])                                           # raft_model.py:1089, :1098-1099
@@ -1300,6 +1503,8 @@ def _general_case_results(P, Xi, st, owner, first, n_cases, channels, F2nd, roto
         F2[:, :6], F2m[:, :6] = F2nd[0], F2nd[1]
         out["Fhydro_2nd"] = [F2[owner == ic] for ic in range(n_cases)]
         out["Fhydro_2nd_mean"] = [F2m[owner == ic] for ic in range(n_cases)]
+    if fatigue is not None:
+        _general_fatigue(fatigue, channels, P, Xi, owner, first, n_cases, metrics, out)
     return out
 
 
@@ -1612,6 +1817,16 @@ class GeneralBatchSession:
                                                  self.dw, case_row0, None, psd)
         return sd, P
 
+    def fatigue(self, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, method="dirlik", weights=None, life=None,
+                moments=True, tile_w=0):
+        """Fatigue DELs of the last ``solve()`` for every design in one launch sequence (raftk_fatigue_dev on the resident Xi
+        [nD, nT, nDOF, nw]): ``R`` [nD, nch, nDOF] (each design's rows) or [nch, nDOF], or ``coef``; the other arguments as
+        ``fatigue``.  -> dict of torch tensors as ``fatigue`` (DEL [nD, nC, nch], ...)."""
+        stream = self.torch.cuda.current_stream(self.device).cuda_stream
+        out, self._fat_keep = _fatigue_dev(self.torch, self.device, stream, self.Xi, self.keep["w"], m, R, wpow, coef, case_row0,
+                                           f_eq, method, weights, life, moments, tile_w)
+        return out
+
 
 def _no_general_ops(turbine_constants):
     if turbine_constants is not None:
@@ -1631,15 +1846,17 @@ def _train_ops(ops, owner, n_cases):
 
 
 def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, qtf=None, rotors=None,
-                                turbine_constants=None, ops=None):
+                                turbine_constants=None, ops=None, fatigue=None):
     """``general_analyze_cases`` for every design of a batch in one solve: ``designs`` a list of per-design inputs (or a
     ``GeneralBatch`` built from them), ``cases`` a list of case dicts run by every design, ``channels`` None or one
     ``packer.pack_general_channels`` dict per design, ``rotors`` None or one ``packer.pack_rotor_outputs`` dict per design
     -> a list with, for each design, what ``general_analyze_cases`` returns for that design alone.  ``ops``: one operating
     point per case, tables per design [nD, n_op, n_fd, n_fd, nw] or shared [n_op, n_fd, n_fd, nw]
-    (``packer.pack_general_operating_points``).  ``turbine_constants``: NotImplementedError, as for ``general_analyze_cases``."""
+    (``packer.pack_general_operating_points``).  ``turbine_constants``: NotImplementedError, as for ``general_analyze_cases``.
+    ``fatigue``: as for ``general_analyze_cases``, every design with the same exponents."""
     from .packer import pack_case_trains
     _no_general_ops(turbine_constants)
+    opts = None if fatigue is None else fatigue_options(fatigue)
     bt = _as_batch(designs, qtf)
     if channels is not None and len(channels) != bt.n_designs:
         raise ValueError("channels: one entry per design (%d), got %d" % (bt.n_designs, len(channels)))
@@ -1651,7 +1868,7 @@ def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.
                                        xi_start=xi_start, F_2nd=q)
     P = dict(w=bt.arrays["w"], dw=bt.dw)
     return [_general_case_results(P, res[0][d], res[1][d], owner, first, len(cases), None if channels is None else channels[d],
-                                  (res[2][d], res[3][d]) if q else None, None if rotors is None else rotors[d])
+                                  (res[2][d], res[3][d]) if q else None, None if rotors is None else rotors[d], opts)
             for d in range(bt.n_designs)]
 
 
@@ -2066,6 +2283,27 @@ class DeviceSession:
         if farm and n_fowt is None:
             sd, P = sd[0], (P[0] if psd else None)
         return sd, P
+
+    def fatigue(self, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, method="dirlik", weights=None, life=None,
+                moments=True, tile_w=0, farm=False, n_fowt=None):
+        """Enqueue fatigue DELs on a resident response (raftk_fatigue_dev; no host round trip).  ``farm=False``: the last
+        ``solve``'s Xi [nD, nC, 6, nw], one unit per design (e.g. ``coef`` [nch, 6, nw] of ``packer.pack_turbine_channels``
+        for Mbase); ``farm=True``: the Xi_sys of the LAST ``farm_response`` of the form ``n_fowt`` names (as
+        ``farm_channel_stats``), one unit per farm (e.g. the tension Jacobian as ``R``).  The other arguments as ``fatigue``.
+        -> dict of torch tensors as ``fatigue``, without the unit axis for one farm (``farm=True``, ``n_fowt=None``)."""
+        if farm:
+            key = "_farm" if n_fowt is None else "_farm_batch"
+            if not hasattr(self, key):
+                raise RuntimeError("fatigue: call farm_response(n_fowt=%r) first" % (n_fowt,))
+            xi = getattr(self, key)[2]
+            xi = xi[None] if n_fowt is None else xi
+        else:
+            xi = self.out["Xi"]
+        out, self._fat_keep = _fatigue_dev(self.torch, self.device, self._stream(), xi, self.dt["w"], m, R, wpow, coef, case_row0,
+                                           f_eq, method, weights, life, moments, tile_w)
+        if farm and n_fowt is None:
+            out = {k: v[0] for k, v in out.items()}
+        return out
 
     def eigen(self, A0=None, yawstiff=0.0, sort="dof", modes=True):
         """Natural frequencies and mode shapes of every design on the device, on torch's current stream (async):
