@@ -168,12 +168,7 @@ class Model:
                     nrot = 1 + max(ir for _, ir in ch["names"])
                     sd_c, psd_c = solver.combine_trains(ch_stats[i][0], ch_stats[i][1], idx)
                     for k_, (nm, ir) in enumerate(ch["names"]):
-                        for suffix in ("_avg", "_std", "_max", "_min"):
-                            m.setdefault(nm + suffix, np.zeros(nrot))
-                        m.setdefault(nm + "_PSD", np.zeros([self.nw, nrot]))
-                        m[nm + "_avg"][ir], m[nm + "_std"][ir] = ch["avg"][k_], sd_c[k_]
-                        m[nm + "_max"][ir], m[nm + "_min"][ir] = ch["avg"][k_] + 3 * sd_c[k_], ch["avg"][k_] - 3 * sd_c[k_]
-                        m[nm + "_PSD"][:, ir] = psd_c[k_]
+                        solver.rotor_channel_entries(m, nm, ir, nrot, ch["avg"][k_], sd_c[k_], psd_c[k_])
                 if ten[i] is not None:
                     m.update(solver.tension_metrics(self.tensions[i]["T0"], *solver.combine_trains(ten[i][0], ten[i][1], idx)))
                 m["wave_PSD"] = (0.5 * np.abs(out["zeta"][idx]) ** 2 / dw).sum(axis=0)          # getPSD(zeta, dw) (:2608)

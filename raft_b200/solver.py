@@ -19,6 +19,7 @@ from ._lib import (RaftkCases, RaftkDesigns, RaftkFarm, RaftkFarmBatch, RaftkGen
                    RaftkSlenderOutputs, RaftkSolveOpts, check, lib)
 
 _F8 = np.float64
+_C16 = np.complex128
 _I4 = np.int32
 
 
@@ -881,7 +882,6 @@ class GeneralSession:
             self.F_2nd = torch.zeros([nC, 6, nw], dtype=torch.float64, device=self.device) if self.qtf is not None else None
             self.F_2nd_mean = torch.zeros([nC, 6], dtype=torch.float64, device=self.device) if self.qtf is not None else None
         self.n, self.nw, self.n_cases, self.dw = n, nw, nC, float(P["dw"])
-        self._ch = None
 
     def solve(self, n_iter=10, tol=0.01, xi_start=0.0):
         o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
@@ -903,44 +903,22 @@ class GeneralSession:
     def stats(self, R, wpow, psd=True, amp=False):
         """Output-channel statistics of the last ``solve()`` (``packer.pack_general_channels``: R [nch,nDOF], wpow [nch]) on
         the device -> (std [nT,nch], PSD [nT,nch,nw] or None, amplitudes complex [nT,nch,nw] or None), torch tensors."""
-        torch = self.torch
-        R = np.ascontiguousarray(R, dtype=_F8)
-        wpow = np.ascontiguousarray(wpow, dtype=_I4)
-        if R.ndim != 2 or R.shape[1] != self.n or wpow.shape != (R.shape[0],):
-            raise ValueError("R must be [nch, %d] and wpow [nch]" % self.n)
-        _check_wpow(wpow)
-        nch = R.shape[0]
-        with torch.cuda.device(self.device):
-            if self._ch is None or not (np.array_equal(self._ch[0], R) and np.array_equal(self._ch[1], wpow)):
-                self._ch = (R, wpow, torch.from_numpy(R).to(self.device), torch.from_numpy(wpow).to(self.device))
-            dR, dp = self._ch[2], self._ch[3]
-            sd = torch.empty([self.n_cases, nch], dtype=torch.float64, device=self.device)
-            P = torch.empty([self.n_cases, nch, self.nw], dtype=torch.float64, device=self.device) if psd else None
-            A = torch.empty([self.n_cases, nch, self.nw], dtype=torch.complex128, device=self.device) if amp else None
-            check(lib.raftk_general_channel_stats_dev(self.n_cases, self.n, nch, self.nw, self.dw, self.keep["w"].data_ptr(), dR.data_ptr(),
-                                                      dp.data_ptr(), self.Xi.data_ptr(), sd.data_ptr(), P.data_ptr() if psd else None,
-                                                      A.data_ptr() if amp else None, torch.cuda.current_stream(self.device).cuda_stream))
-        return sd, P, A
+        return _general_channel_stats(_session_buffers(self), R, wpow, self.keep["w"], self.Xi, self.dw, psd, amp)
 
     def rotor_stats(self, R, C_, V_w, gains, case_row0=None, psd=True):
         """Rotor speed, generator torque and blade pitch statistics of the last ``solve()`` on the device
         (raftk_rotor_stats_dev, no host round trip): ``R`` [nrot, nDOF], ``C``, ``V_w``, ``gains`` and ``case_row0`` as
         ``rotor_stats`` (``packer.pack_rotor_outputs``; the first train of every case, e.g. ``pack_case_trains``' ``first``
         + [nT]).  -> (std [nC, nrot, 3], PSD [nC, nrot, 3, nw] or None), torch tensors."""
-        stream = self.torch.cuda.current_stream(self.device).cuda_stream
-        sd, P, self._rot_keep = _rotor_stats_dev(self.torch, self.device, stream, self.Xi[None], self.keep["w"], R, C_, V_w, gains,
-                                                 self.dw, case_row0, None, psd)
-        return sd[0], (P[0] if psd else None)
+        return _rotor_stats(_session_buffers(self), R, C_, V_w, gains, self.keep["w"], self.Xi, self.dw, case_row0, None, psd)
 
     def fatigue(self, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, method="dirlik", weights=None, life=None,
                 moments=True, tile_w=0):
         """Fatigue DELs of the last ``solve()`` on the device (raftk_fatigue_dev, no host round trip): ``R`` [nch, nDOF] with
         ``wpow`` (``packer.pack_general_channels``' rows) or ``coef``, and the other arguments as ``fatigue``; ``case_row0``
         groups the trains into cases.  -> dict of torch tensors as ``fatigue`` without the unit axis."""
-        stream = self.torch.cuda.current_stream(self.device).cuda_stream
-        out, self._fat_keep = _fatigue_dev(self.torch, self.device, stream, self.Xi[None], self.keep["w"], m, R, wpow, coef, case_row0,
-                                           f_eq, method, weights, life, moments, tile_w)
-        return {k: v[0] for k, v in out.items()}
+        return _fatigue(_session_buffers(self), self.Xi, self.keep["w"], m, R, wpow, coef, case_row0, f_eq, method, weights, life,
+                        moments, tile_w)
 
 
 def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0, fd=None, F_BEM=False, qtf=None, F_2nd=False,
@@ -1035,6 +1013,74 @@ def general_chunk_for_budget(P, fd, qtf, n_cases, budget_bytes):
     return lo
 
 
+# ---- post-solve reductions (rotor, fatigue, channel statistics, eigen), written once for host and device buffers ------------
+class _Host:
+    """Host buffers (numpy) for a reduction: ``raftk_<name>_host`` stages them through the library's device arena and
+    returns with the results in them."""
+
+    @staticmethod
+    def array(a, dtype):
+        return np.ascontiguousarray(a, dtype=dtype)
+
+    @staticmethod
+    def empty(shape, dtype=_F8):
+        return np.zeros(shape, dtype=dtype)
+
+    @staticmethod
+    def ptr(a):
+        return None if a is None else a.ctypes.data
+
+    @staticmethod
+    def call(name, *args, ws=None):
+        check(getattr(lib, "raftk_%s_host" % name)(*args))
+
+
+_HOST = _Host()
+
+
+class _Device:
+    """Torch tensors on ``device`` for a reduction: ``raftk_<name>_dev`` is enqueued on torch's current stream, after a
+    workspace sized by ``raftk_<name>_workspace_bytes(*ws)`` when the entry takes one.  ``reads`` holds the inputs this
+    object converted and the workspace: the enqueued launches read them after ``call`` returns, so whoever enqueues keeps
+    the object until they are done."""
+
+    def __init__(self, device):
+        import torch
+        self.torch, self.device, self.reads = torch, torch.device(device), []
+        self._dtype = {_F8: torch.float64, _C16: torch.complex128, _I4: torch.int32}
+
+    def array(self, a, dtype):
+        if isinstance(a, self.torch.Tensor):
+            a = a.to(device=self.device, dtype=self._dtype[dtype]).contiguous()
+        else:
+            a = self.torch.from_numpy(np.ascontiguousarray(a, dtype=dtype)).to(self.device)
+        self.reads.append(a)
+        return a
+
+    def empty(self, shape, dtype=_F8):
+        return self.torch.empty(shape, dtype=self._dtype[dtype], device=self.device)
+
+    @staticmethod
+    def ptr(a):
+        return None if a is None else a.data_ptr()
+
+    def call(self, name, *args, ws=None):
+        torch = self.torch
+        with torch.cuda.device(self.device):
+            if ws is not None:
+                wsb = int(getattr(lib, "raftk_%s_workspace_bytes" % name)(*ws))
+                buf = torch.empty(max(wsb, 1), dtype=torch.uint8, device=self.device)
+                self.reads.append(buf)
+                args += (buf.data_ptr(), wsb)
+            check(getattr(lib, "raftk_%s_dev" % name)(*args, torch.cuda.current_stream(self.device).cuda_stream))
+
+
+def _session_buffers(session):
+    """Device buffers for one reduction of ``session``, held as its ``_reads`` until its next reduction."""
+    session._reads = _Device(session.device)
+    return session._reads
+
+
 def combine_trains(std, psd, idx):
     """helpers.getRMS / getPSD of a case with several wave trains (helpers.py:678-700) from per-train reductions ``std``
     [nT,...] and ``psd`` [nT,...,nw]: the squares sum over the trains ``idx`` -> (sqrt(sum std^2), sum PSD)."""
@@ -1050,20 +1096,31 @@ def general_channel_stats(R, wpow, w, Xi, dw, psd=True, amp=False):
     """Output channels of a FOWT with generalised DOFs, Y = w^wpow R Xi (``packer.pack_general_channels``), host buffers:
     R [nch,nDOF], wpow [nch] 0, 1 or 2, w [nw], Xi complex [nU,nDOF,nw] -> (std [nU,nch], PSD [nU,nch,nw] or None,
     amplitudes complex [nU,nch,nw] or None)."""
-    R = np.ascontiguousarray(R, dtype=_F8)
-    wpow = np.ascontiguousarray(wpow, dtype=_I4)
-    w = np.ascontiguousarray(w, dtype=_F8)
-    Xi = np.ascontiguousarray(Xi, dtype=np.complex128)
-    nU, n, nw = Xi.shape
-    nch = R.shape[0]
-    if R.shape != (nch, n) or wpow.shape != (nch,) or w.shape != (nw,):
+    return _general_channel_stats(_HOST, R, wpow, w, Xi, dw, psd, amp)
+
+
+def _general_channel_stats(be, R, wpow, w, Xi, dw, psd, amp):
+    """``general_channel_stats`` on ``be``'s buffers; also design by design, R [nD,nch,nDOF] on Xi [nD,nU,nDOF,nw] -> outputs
+    [nD,nU,...] (one entry call per design).  wpow stays [nch]."""
+    R, wpow, w, Xi = be.array(R, _F8), np.ascontiguousarray(wpow, dtype=_I4), be.array(w, _F8), be.array(Xi, _C16)
+    squeeze = Xi.ndim == 3
+    if squeeze:
+        R, Xi = R[None], Xi[None]
+    if (Xi.ndim != 4 or R.ndim != 3 or R.shape[0] != Xi.shape[0] or R.shape[2] != Xi.shape[2] or wpow.shape != (R.shape[1],)
+            or tuple(w.shape) != (Xi.shape[3],)):
         raise ValueError("R must be [nch,nDOF], wpow [nch], w [nw] for Xi [nU,nDOF,nw]")
+    nD, nU, n, nw = Xi.shape
+    nch = R.shape[1]
     _check_wpow(wpow)
-    sd = np.zeros([nU, nch])
-    P = np.zeros([nU, nch, nw]) if psd else None
-    A = np.zeros([nU, nch, nw], dtype=np.complex128) if amp else None
-    check(lib.raftk_general_channel_stats_host(nU, n, nch, nw, float(dw), w.ctypes.data, R.ctypes.data, wpow.ctypes.data, Xi.ctypes.data,
-                                               sd.ctypes.data, P.ctypes.data if psd else None, A.ctypes.data if amp else None))
+    wp = be.array(wpow, _I4)
+    sd = be.empty([nD, nU, nch])
+    P = be.empty([nD, nU, nch, nw]) if psd else None
+    A = be.empty([nD, nU, nch, nw], _C16) if amp else None
+    for d in range(nD):
+        be.call("general_channel_stats", nU, n, nch, nw, float(dw), be.ptr(w), be.ptr(R[d]), be.ptr(wp), be.ptr(Xi[d]), be.ptr(sd[d]),
+                be.ptr(P[d]) if psd else None, be.ptr(A[d]) if amp else None)
+    if squeeze:
+        sd, P, A = sd[0], (P[0] if psd else None), (A[0] if amp else None)
     return sd, P, A
 
 
@@ -1098,7 +1155,12 @@ def farm_channel_stats(R, Xi_sys, dw, w=None, wpow=None, psd=True, amp=False, ti
     -> (std [F,nR,nch], PSD [F,nR,nch,nw] or None, amplitudes complex [F,nR,nch,nw] or None), without the farm axis when
     ``Xi_sys`` had none.  Bit-identical to ``general_channel_stats`` on the same R and Xi.  Several wave trains of a case:
     ``combine_trains``.  ``tile_w``: bins per CTA (0 automatic; -1 reads Xi_sys from L2), the results do not depend on it."""
-    Xi_sys = np.ascontiguousarray(Xi_sys, dtype=np.complex128)
+    return _farm_channel_stats(_HOST, R, Xi_sys, dw, w, wpow, psd, amp, tile_w)
+
+
+def _farm_channel_stats(be, R, Xi_sys, dw, w, wpow, psd, amp, tile_w):
+    """``farm_channel_stats`` on ``be``'s buffers (R and wpow: numpy)."""
+    Xi_sys = be.array(Xi_sys, _C16)
     squeeze = Xi_sys.ndim == 3
     if squeeze:
         Xi_sys = Xi_sys[None]
@@ -1106,16 +1168,16 @@ def farm_channel_stats(R, Xi_sys, dw, w=None, wpow=None, psd=True, amp=False, ti
         raise ValueError("Xi_sys must be [F, nR, n, nw] or [nR, n, nw]")
     F, nR, n, nw = Xi_sys.shape
     ch, R, wpow = _farm_channels_struct(R, wpow, F, n, dw, tile_w)
-    w = None if w is None else np.ascontiguousarray(w, dtype=_F8)
-    if w is not None and w.shape != (nw,):
+    w = None if w is None else be.array(w, _F8)
+    if w is not None and tuple(w.shape) != (nw,):
         raise ValueError("w must be [nw]")
     nch = ch.n_ch
-    sd = np.zeros([F, nR, nch])
-    P = np.zeros([F, nR, nch, nw]) if psd else None
-    A = np.zeros([F, nR, nch, nw], dtype=np.complex128) if amp else None
-    ch.R, ch.std = R.ctypes.data, sd.ctypes.data
-    ch.psd, ch.amp = (P.ctypes.data if psd else None), (A.ctypes.data if amp else None)
-    check(lib.raftk_farm_channel_stats_host(F, nR, n, nw, None if w is None else w.ctypes.data, Xi_sys.ctypes.data, C.byref(ch)))
+    R = be.array(R, _F8)
+    sd = be.empty([F, nR, nch])
+    P = be.empty([F, nR, nch, nw]) if psd else None
+    A = be.empty([F, nR, nch, nw], _C16) if amp else None
+    ch.R, ch.std, ch.psd, ch.amp = be.ptr(R), be.ptr(sd), be.ptr(P), be.ptr(A)
+    be.call("farm_channel_stats", F, nR, n, nw, be.ptr(w), be.ptr(Xi_sys), C.byref(ch), ws=(F, nR, nw, C.byref(ch)))
     if squeeze:
         sd, P, A = sd[0], (P[0] if psd else None), (A[0] if amp else None)
     return sd, P, A
@@ -1161,48 +1223,31 @@ def rotor_stats(R, C_, V_w, gains, w, Xi, dw, case_row0=None, col0=None, psd=Tru
     ``case_row0`` [nC + 1] the first row of every case (None: one row per case); ``col0`` [nrot] the first column of every
     rotor's hub row (None: 0).  -> (std [n_units, nC, nrot, 3] (omega rpm, torque N m, bPitch deg), PSD [n_units, nC, nrot,
     3, nw] or None), without the unit axis when ``Xi`` had none."""
-    Xi = np.ascontiguousarray(Xi, dtype=np.complex128)
+    return _rotor_stats(_HOST, R, C_, V_w, gains, w, Xi, dw, case_row0, col0, psd)
+
+
+def _rotor_stats(be, R, C_, V_w, gains, w, Xi, dw, case_row0, col0, psd):
+    """``rotor_stats`` on ``be``'s buffers (case_row0 and col0: numpy)."""
+    Xi = be.array(Xi, _C16)
     squeeze = Xi.ndim == 3
     if squeeze:
         Xi = Xi[None]
     if Xi.ndim != 4:
         raise ValueError("Xi must be [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]")
     nU, nR, n, nw = Xi.shape
-    R, C_ = np.ascontiguousarray(R, dtype=_F8), np.ascontiguousarray(C_, dtype=np.complex128)
-    V_w, gains = np.ascontiguousarray(V_w, dtype=np.complex128), np.ascontiguousarray(gains, dtype=_F8)
-    w = np.ascontiguousarray(w, dtype=_F8)
-    if w.shape != (nw,):
+    R, C_, V_w, gains = be.array(R, _F8), be.array(C_, _C16), be.array(V_w, _C16), be.array(gains, _F8)
+    w = be.array(w, _F8)
+    if tuple(w.shape) != (nw,):
         raise ValueError("w must be [nw]")
     ro, rows, cols = _rotor_struct(R, C_, V_w, gains, nU, nw, dw, case_row0, col0)
-    sd = np.zeros([nU, ro.n_cases, ro.n_rot, 3])
-    P = np.zeros([nU, ro.n_cases, ro.n_rot, 3, nw]) if psd else None
-    ro.R, ro.C, ro.V_w, ro.gains = R.ctypes.data, C_.ctypes.data, V_w.ctypes.data, gains.ctypes.data
-    ro.std, ro.psd = sd.ctypes.data, (P.ctypes.data if psd else None)
-    check(lib.raftk_rotor_stats_host(nU, nR, n, nw, w.ctypes.data, Xi.ctypes.data, C.byref(ro)))
+    sd = be.empty([nU, ro.n_cases, ro.n_rot, 3])
+    P = be.empty([nU, ro.n_cases, ro.n_rot, 3, nw]) if psd else None
+    ro.R, ro.C, ro.V_w, ro.gains = be.ptr(R), be.ptr(C_), be.ptr(V_w), be.ptr(gains)
+    ro.std, ro.psd = be.ptr(sd), be.ptr(P)
+    be.call("rotor_stats", nU, nR, n, nw, be.ptr(w), be.ptr(Xi), C.byref(ro))
     if squeeze:
         sd, P = sd[0], (P[0] if psd else None)
     return sd, P
-
-
-def _rotor_stats_dev(torch, device, stream, Xi, w, R, C_, V_w, gains, dw, case_row0, col0, psd):
-    """rotor_stats on a resident Xi [n_units, n_rows, n_dof, nw] (torch, complex128) and w; R, C, V_w, gains numpy arrays or
-    torch tensors -> (std, PSD or None) torch tensors, enqueued on ``stream`` (raftk_rotor_stats_dev)."""
-    nU, nR, n, nw = Xi.shape
-
-    def dev(a, dt):
-        if isinstance(a, torch.Tensor):
-            return a.to(device=device, dtype=dt).contiguous()
-        a = np.ascontiguousarray(a, dtype=np.complex128 if dt == torch.complex128 else _F8)
-        return torch.from_numpy(a).to(device)
-    with torch.cuda.device(device):
-        R, C_, V_w, gains = dev(R, torch.float64), dev(C_, torch.complex128), dev(V_w, torch.complex128), dev(gains, torch.float64)
-        ro, rows, cols = _rotor_struct(R, C_, V_w, gains, nU, nw, dw, case_row0, col0)
-        sd = torch.empty([nU, ro.n_cases, ro.n_rot, 3], dtype=torch.float64, device=device)
-        P = torch.empty([nU, ro.n_cases, ro.n_rot, 3, nw], dtype=torch.float64, device=device) if psd else None
-        ro.R, ro.C, ro.V_w, ro.gains = R.data_ptr(), C_.data_ptr(), V_w.data_ptr(), gains.data_ptr()
-        ro.std, ro.psd = sd.data_ptr(), (P.data_ptr() if psd else None)
-        check(lib.raftk_rotor_stats_dev(nU, nR, n, nw, w.data_ptr(), Xi.data_ptr(), C.byref(ro), stream))
-    return sd, P, (R, C_, V_w, gains)
 
 
 def rotor_metrics(rotors, ic, std, psd, dw):
@@ -1286,65 +1331,35 @@ def fatigue(Xi, w, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, me
     = (sum_c p_c d_c / (f_eq sum_c p_c))^(1/m).  -> dict(DEL [n_units, nC, nch], info int32 (FATIGUE_ZERO, FATIGUE_NARROWBAND
     bits), moments [n_units, nC, nch, 4] (l0, l1, l2, l4) or absent, DEL_life [n_units, nch] or absent), without the unit
     axis when ``Xi`` had none.  ``tile_w``: bins per CTA (0 automatic, -1 reads Xi from L2); the results do not depend on it."""
-    Xi = np.ascontiguousarray(Xi, dtype=np.complex128)
+    return _fatigue(_HOST, Xi, w, m, R, wpow, coef, case_row0, f_eq, method, weights, life, moments, tile_w)
+
+
+def _fatigue(be, Xi, w, m, R, wpow, coef, case_row0, f_eq, method, weights, life, moments, tile_w):
+    """``fatigue`` on ``be``'s buffers (m, wpow, case_row0 and weights: numpy)."""
+    Xi = be.array(Xi, _C16)
     squeeze = Xi.ndim == 3
     if squeeze:
         Xi = Xi[None]
     if Xi.ndim != 4:
         raise ValueError("Xi must be [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]")
     nU, nR, n, nw = Xi.shape
-    w = np.ascontiguousarray(w, dtype=_F8)
-    if w.shape != (nw,):
+    w = be.array(w, _F8)
+    if tuple(w.shape) != (nw,):
         raise ValueError("w must be [nw]")
-    R = None if R is None else np.ascontiguousarray(R, dtype=_F8)
-    coef = None if coef is None else np.ascontiguousarray(coef, dtype=np.complex128)
+    R = None if R is None else be.array(R, _F8)
+    coef = None if coef is None else be.array(coef, _C16)
     fa, keep = _fatigue_struct(nU, nR, n, nw, m, R, wpow, coef, case_row0, f_eq, method, weights, tile_w)
     life = weights is not None if life is None else bool(life)
     nC, nch = fa.n_cases, fa.n_ch
-    out = dict(DEL=np.zeros([nU, nC, nch]), info=np.zeros([nU, nC, nch], dtype=_I4))
+    out = dict(DEL=be.empty([nU, nC, nch]), info=be.empty([nU, nC, nch], _I4))
     if moments:
-        out["moments"] = np.zeros([nU, nC, nch, 4])
+        out["moments"] = be.empty([nU, nC, nch, 4])
     if life:
-        out["DEL_life"] = np.zeros([nU, nch])
-    fa.R = R.ctypes.data if R is not None else None
-    fa.coef = coef.ctypes.data if coef is not None else None
-    fa.DEL, fa.info = out["DEL"].ctypes.data, out["info"].ctypes.data
-    fa.moments = out["moments"].ctypes.data if moments else None
-    fa.DEL_life = out["DEL_life"].ctypes.data if life else None
-    check(lib.raftk_fatigue_host(nU, nR, n, nw, w.ctypes.data, Xi.ctypes.data, C.byref(fa)))
+        out["DEL_life"] = be.empty([nU, nch])
+    fa.R, fa.coef, fa.DEL, fa.info = be.ptr(R), be.ptr(coef), be.ptr(out["DEL"]), be.ptr(out["info"])
+    fa.moments, fa.DEL_life = be.ptr(out.get("moments")), be.ptr(out.get("DEL_life"))
+    be.call("fatigue", nU, nR, n, nw, be.ptr(w), be.ptr(Xi), C.byref(fa), ws=(nU, nR, nw, C.byref(fa)))
     return {k: v[0] for k, v in out.items()} if squeeze else out
-
-
-def _fatigue_dev(torch, device, stream, Xi, w, m, R, wpow, coef, case_row0, f_eq, method, weights, life, moments, tile_w):
-    """fatigue on a resident Xi [n_units, n_rows, n_dof, nw] (torch, complex128) and w; R / coef numpy arrays or torch tensors
-    -> (dict of torch tensors as ``fatigue``, tensors the enqueued launches still read), enqueued on ``stream``
-    (raftk_fatigue_dev)."""
-    nU, nR, n, nw = Xi.shape
-    with torch.cuda.device(device):
-        if R is not None:
-            R = R.to(device=device, dtype=torch.float64).contiguous() if isinstance(R, torch.Tensor) else \
-                torch.from_numpy(np.ascontiguousarray(R, dtype=_F8)).to(device)
-        if coef is not None:
-            coef = coef.to(device=device, dtype=torch.complex128).contiguous() if isinstance(coef, torch.Tensor) else \
-                torch.from_numpy(np.ascontiguousarray(coef, dtype=np.complex128)).to(device)
-        fa, _ = _fatigue_struct(nU, nR, n, nw, m, R, wpow, coef, case_row0, f_eq, method, weights, tile_w)
-        life = weights is not None if life is None else bool(life)
-        nC, nch = fa.n_cases, fa.n_ch
-        out = dict(DEL=torch.empty([nU, nC, nch], dtype=torch.float64, device=device),
-                   info=torch.empty([nU, nC, nch], dtype=torch.int32, device=device))
-        if moments:
-            out["moments"] = torch.empty([nU, nC, nch, 4], dtype=torch.float64, device=device)
-        if life:
-            out["DEL_life"] = torch.empty([nU, nch], dtype=torch.float64, device=device)
-        fa.R = R.data_ptr() if R is not None else None
-        fa.coef = coef.data_ptr() if coef is not None else None
-        fa.DEL, fa.info = out["DEL"].data_ptr(), out["info"].data_ptr()
-        fa.moments = out["moments"].data_ptr() if moments else None
-        fa.DEL_life = out["DEL_life"].data_ptr() if life else None
-        wsb = int(lib.raftk_fatigue_workspace_bytes(nU, nR, nw, C.byref(fa)))
-        ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=device)
-        check(lib.raftk_fatigue_dev(nU, nR, n, nw, w.data_ptr(), Xi.data_ptr(), C.byref(fa), ws.data_ptr(), wsb, stream))
-    return out, (R, coef, ws)
 
 
 def fatigue_options(fatigue):
@@ -1442,16 +1457,22 @@ def general_case_metrics(channels, std, psd, amp, idx, dw=None):
             ra[:-1] = amp[idx, k]
             m[nm + "_RA"] = ra
             continue
-        for suffix in ("_avg", "_std", "_max", "_min"):
-            m.setdefault(nm + suffix, np.zeros(nrot))
-        m.setdefault(nm + "_PSD", np.zeros([nw, nrot]))
-        m[nm + "_avg"][ir], m[nm + "_std"][ir] = avg[k], sd[k]
-        m[nm + "_max"][ir], m[nm + "_min"][ir] = avg[k] + 3 * sd[k], avg[k] - 3 * sd[k]
-        m[nm + "_PSD"][:, ir] = ps[k]
+        rotor_channel_entries(m, nm, ir, nrot, avg[k], sd[k], ps[k])
     if "MbaseY_std" in m:
         for suffix in ("_avg", "_std", "_max", "_min", "_PSD"):
             m["Mbase" + suffix] = m["MbaseY" + suffix].copy()
     return m
+
+
+def rotor_channel_entries(m, nm, ir, nrot, avg, std, psd):
+    """Rotor ``ir``'s value of the per-rotor channel ``nm`` into one case's entries ``m`` (raft_fowt.py:2401-2444, 2504-2538):
+    ``nm``_avg / _std / _max / _min [nrot] with max / min = avg +- 3 std, and ``nm``_PSD [nw, nrot] from the PSD [nw]."""
+    for suffix in ("_avg", "_std", "_max", "_min"):
+        m.setdefault(nm + suffix, np.zeros(nrot))
+    m.setdefault(nm + "_PSD", np.zeros([len(psd), nrot]))
+    m[nm + "_avg"][ir], m[nm + "_std"][ir] = avg, std
+    m[nm + "_max"][ir], m[nm + "_min"][ir] = avg + 3 * std, avg - 3 * std
+    m[nm + "_PSD"][:, ir] = psd
 
 
 def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, fd=None, qtf=None, rotors=None,
@@ -1778,54 +1799,28 @@ class GeneralBatchSession:
         ``yawstiff`` scalar or [nD].  -> dict(lam [nD,n], fns [nD,n] = sqrt(lam) / 2 pi, modes [nD,n,n] or None) complex,
         info [nD] int32 (RAFTK_EIG_* flags), torch tensors; ``sort`` as ``solve_eigen``."""
         nD, n = self.n_designs, self.n
-        with self.torch.cuda.device(self.device):
-            M, K = _eigen_inputs(self.keep["M"].view(nD, n, n), self.keep["C"].view(nD, n, n), A0, yawstiff, nD, n, self.device)
-            r = _eigen_dev(M, K, sort, modes, self.device, self.torch.cuda.current_stream(self.device).cuda_stream)
-        return dict(lam=r["lam"], fns=self.torch.sqrt(r["lam"]) / (2.0 * np.pi), modes=r["modes"], info=r["info"])
+        return _session_eigen(self, self.keep["M"].view(nD, n, n), self.keep["C"].view(nD, n, n), A0, yawstiff, sort, modes)
 
     def stats(self, R, wpow, psd=True, amp=False):
         """Output-channel statistics of the last ``solve()`` on the device, design by design (raftk_general_channel_stats_dev
         on each design's slice of Xi): R [nD,nch,nDOF], wpow [nch] -> (std [nD,nT,nch], PSD [nD,nT,nch,nw] or None, amplitudes
         complex [nD,nT,nch,nw] or None), torch tensors."""
-        torch = self.torch
-        R = np.ascontiguousarray(R, dtype=_F8)
-        wpow = np.ascontiguousarray(wpow, dtype=_I4)
-        nD, nC, n, nw = self.n_designs, self.n_cases, self.n, self.nw
-        if R.ndim != 3 or R.shape[0] != nD or R.shape[2] != n or wpow.shape != (R.shape[1],):
-            raise ValueError("R must be [%d, nch, %d] and wpow [nch]" % (nD, n))
-        _check_wpow(wpow)
-        nch = R.shape[1]
-        with torch.cuda.device(self.device):
-            dR, dp = torch.from_numpy(R).to(self.device), torch.from_numpy(wpow).to(self.device)
-            sd = torch.empty([nD, nC, nch], dtype=torch.float64, device=self.device)
-            P = torch.empty([nD, nC, nch, nw], dtype=torch.float64, device=self.device) if psd else None
-            A = torch.empty([nD, nC, nch, nw], dtype=torch.complex128, device=self.device) if amp else None
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-            for d in range(nD):
-                check(lib.raftk_general_channel_stats_dev(nC, n, nch, nw, self.dw, self.keep["w"].data_ptr(), dR[d].data_ptr(), dp.data_ptr(),
-                                                          self.Xi[d].data_ptr(), sd[d].data_ptr(), P[d].data_ptr() if psd else None,
-                                                          A[d].data_ptr() if amp else None, stream))
-        return sd, P, A
+        return _general_channel_stats(_session_buffers(self), R, wpow, self.keep["w"], self.Xi, self.dw, psd, amp)
 
     def rotor_stats(self, R, C_, V_w, gains, case_row0=None, psd=True):
         """Rotor statistics of the last ``solve()`` for every design in one launch sequence (raftk_rotor_stats_dev on the
         resident Xi [nD, nT, nDOF, nw]): ``R`` [nD, nrot, nDOF] (each design's hub rows) or [nrot, nDOF]; ``C``, ``V_w``,
         ``gains`` for every design ([nC, nrot, ...]) or per design ([nD, nC, nrot, ...]); ``case_row0`` as ``rotor_stats``.
         -> (std [nD, nC, nrot, 3], PSD [nD, nC, nrot, 3, nw] or None), torch tensors."""
-        stream = self.torch.cuda.current_stream(self.device).cuda_stream
-        sd, P, self._rot_keep = _rotor_stats_dev(self.torch, self.device, stream, self.Xi, self.keep["w"], R, C_, V_w, gains,
-                                                 self.dw, case_row0, None, psd)
-        return sd, P
+        return _rotor_stats(_session_buffers(self), R, C_, V_w, gains, self.keep["w"], self.Xi, self.dw, case_row0, None, psd)
 
     def fatigue(self, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, method="dirlik", weights=None, life=None,
                 moments=True, tile_w=0):
         """Fatigue DELs of the last ``solve()`` for every design in one launch sequence (raftk_fatigue_dev on the resident Xi
         [nD, nT, nDOF, nw]): ``R`` [nD, nch, nDOF] (each design's rows) or [nch, nDOF], or ``coef``; the other arguments as
         ``fatigue``.  -> dict of torch tensors as ``fatigue`` (DEL [nD, nC, nch], ...)."""
-        stream = self.torch.cuda.current_stream(self.device).cuda_stream
-        out, self._fat_keep = _fatigue_dev(self.torch, self.device, stream, self.Xi, self.keep["w"], m, R, wpow, coef, case_row0,
-                                           f_eq, method, weights, life, moments, tile_w)
-        return out
+        return _fatigue(_session_buffers(self), self.Xi, self.keep["w"], m, R, wpow, coef, case_row0, f_eq, method, weights, life,
+                        moments, tile_w)
 
 
 def _no_general_ops(turbine_constants):
@@ -1977,18 +1972,25 @@ def solve_eigen(M, C_, sort="dof", modes=True):
     squeeze = M.ndim == 2
     if squeeze:
         M, K = M[None], K[None]
-    if M.ndim != 3 or M.shape != K.shape or M.shape[1] != M.shape[2]:
-        raise ValueError("M and C must both be [n,n] or [n_systems,n,n]")
-    nS, n = M.shape[:2]
-    lam = np.zeros([nS, n], dtype=np.complex128)
-    V = np.zeros([nS, n, n], dtype=np.complex128) if modes else None
-    info = np.zeros(nS, dtype=_I4)
-    e = _eigen_struct(nS, n, sort, M.ctypes.data, K.ctypes.data, lam.ctypes.data, V.ctypes.data if modes else None, info.ctypes.data)
-    check(lib.raftk_eigen_host(C.byref(e)))
-    out = eigen_outputs(lam, V, info)
+    r = _eigen(_HOST, M, K, sort, modes)
+    out = eigen_outputs(r["lam"], r["modes"], r["info"])
     if squeeze:
         out = {k: (None if v is None else v[0]) for k, v in out.items()}
     return out
+
+
+def _eigen(be, M, K, sort, modes):
+    """The eigen analysis of M, K [nS,n,n] on ``be``'s buffers -> dict(lam, modes, info), raw (complex)."""
+    M, K = be.array(M, _F8), be.array(K, _F8)
+    if M.ndim != 3 or M.shape != K.shape or M.shape[1] != M.shape[2]:
+        raise ValueError("M and C must both be [n,n] or [n_systems,n,n]")
+    nS, n = M.shape[:2]
+    lam = be.empty([nS, n], _C16)
+    V = be.empty([nS, n, n], _C16) if modes else None
+    info = be.empty([nS], _I4)
+    e = _eigen_struct(nS, n, sort, be.ptr(M), be.ptr(K), be.ptr(lam), be.ptr(V), be.ptr(info))
+    be.call("eigen", C.byref(e), ws=(C.byref(e),))
+    return dict(lam=lam, modes=V, info=info)
 
 
 def eigen_raise(M, C_, info, sort="dof"):
@@ -2022,19 +2024,12 @@ def eigen_fns_modes(M, C_, sort):
     return fns[keep], modes[:, keep]
 
 
-def _eigen_dev(M, K, sort, modes, device, stream):
-    """raftk_eigen_dev on device tensors M, K [nS,n,n] float64 -> dict(lam, modes, info) as torch tensors, raw (complex)."""
-    import torch
-    nS, n = int(M.shape[0]), int(M.shape[1])
-    M, K = M.contiguous(), K.contiguous()
-    lam = torch.empty([nS, n], dtype=torch.complex128, device=device)
-    V = torch.empty([nS, n, n], dtype=torch.complex128, device=device) if modes else None
-    info = torch.empty([nS], dtype=torch.int32, device=device)
-    wsb = eigen_workspace_bytes(nS, n)
-    ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=device)
-    e = _eigen_struct(nS, n, sort, M.data_ptr(), K.data_ptr(), lam.data_ptr(), V.data_ptr() if modes else None, info.data_ptr())
-    check(lib.raftk_eigen_dev(C.byref(e), ws.data_ptr(), wsb, stream))
-    return dict(lam=lam, modes=V, info=info)
+def _session_eigen(session, M, K, A0, yawstiff, sort, modes):
+    """A session's eigen(): the eigen analysis of ``_eigen_inputs`` on its resident M, K [nD,n,n], plus fns = sqrt(lam) / 2 pi."""
+    nD, n = M.shape[:2]
+    be = _session_buffers(session)
+    r = _eigen(be, *_eigen_inputs(M, K, A0, yawstiff, nD, n, session.device), sort, modes)
+    return dict(lam=r["lam"], fns=be.torch.sqrt(r["lam"]) / (2.0 * np.pi), modes=r["modes"], info=r["info"])
 
 
 def _eigen_inputs(M, K, A0, yawstiff, nD, n, device):
@@ -2233,35 +2228,24 @@ class DeviceSession:
             check(launch(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f), ws.data_ptr(), wsb, self._stream()))
         return xi, info
 
+    def _response(self, what, farm, n_fowt):
+        """The resident response reduction ``what`` runs on: the last ``solve``'s Xi [nD,nC,6,nw], or with ``farm`` the Xi_sys of
+        the last ``farm_response`` of the form ``n_fowt`` names ([nC,6N,nw] for one farm, which the reductions return without
+        the unit axis, [F,nC,6N,nw] for a batch)."""
+        if not farm:
+            return self.out["Xi"]
+        key = "_farm" if n_fowt is None else "_farm_batch"
+        if not hasattr(self, key):
+            raise RuntimeError("%s: call farm_response(n_fowt=%r) first" % (what, n_fowt))
+        return getattr(self, key)[2]
+
     def farm_channel_stats(self, R, dw, wpow=None, psd=True, amp=False, n_fowt=None, tile_w=0):
         """Enqueue channel statistics of the LAST ``farm_response`` on the resident Xi_sys (raftk_farm_channel_stats_dev; no
         host round trip): mooring tensions with R the tension Jacobian.  ``n_fowt`` names the form of ``farm_response`` that
         ran (None: one farm).  ``R``, ``dw``, ``wpow``, ``tile_w`` as ``farm_channel_stats``.  -> torch tensors (std [F,nC,nch],
         PSD [F,nC,nch,nw] or None, amplitudes complex [F,nC,nch,nw] or None), without the farm axis for ``n_fowt=None``."""
-        torch = self.torch
-        key = "_farm" if n_fowt is None else "_farm_batch"
-        if not hasattr(self, key):
-            raise RuntimeError("farm_channel_stats: call farm_response(n_fowt=%r) first" % (n_fowt,))
-        xi = getattr(self, key)[2]
-        lead = list(xi.shape[:-2]) if n_fowt is not None else [1, xi.shape[0]]
-        F, nR, n, nw = lead[0], lead[1], xi.shape[-2], xi.shape[-1]
-        ch, R, wpow = _farm_channels_struct(R, wpow, F, n, dw, tile_w)
-        nch = ch.n_ch
-        with torch.cuda.device(self.device):
-            dR = torch.from_numpy(R).to(self.device)
-            sd = torch.zeros([F, nR, nch], dtype=torch.float64, device=self.device)
-            P = torch.zeros([F, nR, nch, nw], dtype=torch.float64, device=self.device) if psd else None
-            A = torch.zeros([F, nR, nch, nw], dtype=torch.complex128, device=self.device) if amp else None
-            ch.R, ch.std = dR.data_ptr(), sd.data_ptr()
-            ch.psd, ch.amp = (P.data_ptr() if psd else None), (A.data_ptr() if amp else None)
-            wsb = int(lib.raftk_farm_channel_stats_workspace_bytes(F, nR, nw, C.byref(ch)))
-            ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=self.device)
-            check(lib.raftk_farm_channel_stats_dev(F, nR, n, nw, self.dt["w"].data_ptr(), xi.data_ptr(), C.byref(ch), ws.data_ptr(), wsb,
-                                                   self._stream()))
-            self._farm_ch_keep = (dR, ws)             # the launch reads them after this call returns
-        if n_fowt is None:
-            sd, P, A = sd[0], (P[0] if psd else None), (A[0] if amp else None)
-        return sd, P, A
+        xi = self._response("farm_channel_stats", True, n_fowt)
+        return _farm_channel_stats(_session_buffers(self), R, xi, dw, self.dt["w"], wpow, psd, amp, tile_w)
 
     def rotor_stats(self, R, C_, V_w, gains, dw, case_row0=None, col0=None, psd=True, farm=False, n_fowt=None):
         """Enqueue rotor speed, generator torque and blade pitch statistics on a resident response (raftk_rotor_stats_dev; no
@@ -2270,19 +2254,8 @@ class DeviceSession:
         i's hub rows at ``col0`` = 6 i.  ``R``, ``C``, ``V_w``, ``gains``, ``case_row0``, ``col0`` as ``rotor_stats`` (numpy or
         torch).  -> (std [nU, nCases, nrot, 3], PSD [nU, nCases, nrot, 3, nw] or None) torch tensors, without the unit axis
         for one farm (``farm=True``, ``n_fowt=None``)."""
-        if farm:
-            key = "_farm" if n_fowt is None else "_farm_batch"
-            if not hasattr(self, key):
-                raise RuntimeError("rotor_stats: call farm_response(n_fowt=%r) first" % (n_fowt,))
-            xi = getattr(self, key)[2]
-            xi = xi[None] if n_fowt is None else xi
-        else:
-            xi = self.out["Xi"]
-        sd, P, self._rot_keep = _rotor_stats_dev(self.torch, self.device, self._stream(), xi, self.dt["w"], R, C_, V_w, gains, dw,
-                                                 case_row0, col0, psd)
-        if farm and n_fowt is None:
-            sd, P = sd[0], (P[0] if psd else None)
-        return sd, P
+        xi = self._response("rotor_stats", farm, n_fowt)
+        return _rotor_stats(_session_buffers(self), R, C_, V_w, gains, self.dt["w"], xi, dw, case_row0, col0, psd)
 
     def fatigue(self, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, method="dirlik", weights=None, life=None,
                 moments=True, tile_w=0, farm=False, n_fowt=None):
@@ -2291,19 +2264,9 @@ class DeviceSession:
         for Mbase); ``farm=True``: the Xi_sys of the LAST ``farm_response`` of the form ``n_fowt`` names (as
         ``farm_channel_stats``), one unit per farm (e.g. the tension Jacobian as ``R``).  The other arguments as ``fatigue``.
         -> dict of torch tensors as ``fatigue``, without the unit axis for one farm (``farm=True``, ``n_fowt=None``)."""
-        if farm:
-            key = "_farm" if n_fowt is None else "_farm_batch"
-            if not hasattr(self, key):
-                raise RuntimeError("fatigue: call farm_response(n_fowt=%r) first" % (n_fowt,))
-            xi = getattr(self, key)[2]
-            xi = xi[None] if n_fowt is None else xi
-        else:
-            xi = self.out["Xi"]
-        out, self._fat_keep = _fatigue_dev(self.torch, self.device, self._stream(), xi, self.dt["w"], m, R, wpow, coef, case_row0,
-                                           f_eq, method, weights, life, moments, tile_w)
-        if farm and n_fowt is None:
-            out = {k: v[0] for k, v in out.items()}
-        return out
+        xi = self._response("fatigue", farm, n_fowt)
+        return _fatigue(_session_buffers(self), xi, self.dt["w"], m, R, wpow, coef, case_row0, f_eq, method, weights, life, moments,
+                        tile_w)
 
     def eigen(self, A0=None, yawstiff=0.0, sort="dof", modes=True):
         """Natural frequencies and mode shapes of every design on the device, on torch's current stream (async):
@@ -2313,10 +2276,7 @@ class DeviceSession:
         fns [nD,6] = sqrt(lam) / 2 pi, modes [nD,6,6] or None) complex, info [nD] int32 (RAFTK_EIG_* flags), torch tensors;
         ``sort`` as ``solve_eigen``."""
         nD = self.batch.n_designs
-        with self.torch.cuda.device(self.device):
-            M, K = _eigen_inputs(self.dt["M0"].view(nD, 6, 6), self.dt["C0"].view(nD, 6, 6), A0, yawstiff, nD, 6, self.device)
-            r = _eigen_dev(M, K, sort, modes, self.device, self._stream())
-        return dict(lam=r["lam"], fns=self.torch.sqrt(r["lam"]) / (2.0 * np.pi), modes=r["modes"], info=r["info"])
+        return _session_eigen(self, self.dt["M0"].view(nD, 6, 6), self.dt["C0"].view(nD, 6, 6), A0, yawstiff, sort, modes)
 
     def second_order_force(self):
         """Enqueue FOWT.calcHydroForce_2ndOrd for all units -> out['F_2nd'], out['F_2nd_mean'] (async)."""

@@ -436,8 +436,8 @@ def test_host_equals_dev_and_farm_columns_equal_rigid_slices():
     dw = w[1] - w[0]
     sd, P = solver.rotor_stats(R, C_, V_w, g, w, Xi, dw, case_row0=row0, col0=col0)
     dev = torch.device("cuda", 0)
-    sdd, Pd, _ = solver._rotor_stats_dev(torch, dev, torch.cuda.current_stream(dev).cuda_stream, torch.from_numpy(Xi).to(dev),
-                                         torch.from_numpy(w).to(dev), R, C_, V_w, g, dw, row0, col0, True)
+    sdd, Pd = solver._rotor_stats(solver._Device(dev), R, C_, V_w, g, torch.from_numpy(w).to(dev), torch.from_numpy(Xi).to(dev), dw,
+                                  row0, col0, True)
     torch.cuda.synchronize()
     assert np.array_equal(sdd.cpu().numpy(), sd) and np.array_equal(Pd.cpu().numpy(), P)
     for i in range(N):

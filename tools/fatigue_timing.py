@@ -62,13 +62,12 @@ def run(name, U, nR, n, nw, nch, form, row0, numpy_units):
         ch = dict(R=rng.normal(size=(U, nch, n)), wpow=np.zeros(nch, dtype=np.int32))
         ch_bytes = U * nch * n * 8
     dch = {k: (torch.from_numpy(v).to(dev) if k != "wpow" else v) for k, v in ch.items()}
-    stream = torch.cuda.current_stream(dev).cuda_stream
     keep = []
 
     def call():
-        out, k = solver._fatigue_dev(torch, dev, stream, Xi, w, 4.0, dch.get("R"), dch.get("wpow"), dch.get("coef"), row0, 1.0,
-                                     "dirlik", None, True, True, 0)
-        keep[:] = [out, k]
+        be = solver._Device(dev)
+        out = solver._fatigue(be, Xi, w, 4.0, dch.get("R"), dch.get("wpow"), dch.get("coef"), row0, 1.0, "dirlik", None, True, True, 0)
+        keep[:] = [out, be]
         return out
     t_med, t_min, t_max = device_time(call)
     out = call()
