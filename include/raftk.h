@@ -868,6 +868,75 @@ int raftk_fatigue_host(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t n
                        const raftk_fatigue *fa);
 
 /*
+ * Tower-base axial stress around the circumference (the reference's helpers.getSigmaXPSD, helpers.py:1164), for n_units units
+ * x n_cases cases x n_rings rings (tower bases) x n_angles angles.  Per (unit u, case c, ring), over the rows h of the case, the
+ * fore-aft moment a_h and the side-side moment b_h in the channel forms of raftk_fatigue (ring k's channels read the n_r columns
+ * col0[k] .. col0[k] + n_r - 1 of Xi, e.g. 6 i for FOWT i of a farm's Xi_sys):
+ *   real form:    a_h(w) = w^wpow[k,0] sum_j R[k,0,j] Xi[u,h,col0[k]+j,w], b_h the same with row 1
+ *   complex form: a_h(w) = sum_j coef[k,0,j,w] Xi[u,h,col0[k]+j,w], b_h the same with row 1
+ * n_ch = 1 gives the fore-aft moment only (b = 0: a rigid tower's Mbase, which has no side-side moment).  Thin-wall section:
+ *   Izz = pi/8 t d^3, c = (d/2) / Izz / 1e6, sigma_h(theta, w) = c (a_h cos theta - b_h sin theta)  (MPa for N m and m)
+ *   S_xy,k = sum_h sum_j w_j^k 1/2 Re(x_h conj(y_h)) for xy = aa, bb, ab and k = 0, 1, 2, 4
+ *   lambda_k(theta) = c^2 (cos^2 S_aa,k - 2 sin cos S_ab,k + sin^2 S_bb,k)
+ *   std = sqrt(lambda_0), avg = c (cos theta mean_a - sin theta mean_b), max / min = avg +- 3 std
+ *   DEL (m > 0): raftk_fatigue's closed form on lambda_k(theta) (Dirlik, narrow band as the fallback or on request, f_eq),
+ *     info as raftk_fatigue's; DEL_life (weights or not) as raftk_fatigue's DEL_life, per angle.
+ *   hot [.., 6] = {angle of the largest std on the grid, that std, angle of the largest DEL, that DEL (0, 0 without m), the
+ *     largest std over the whole circle c sqrt(mu) with mu the larger eigenvalue of [[S_aa,0, S_ab,0], [S_ab,0, S_bb,0]], its
+ *     angle in [0, pi)}; ties go to the first angle.  hot_life [.., 2] = {angle of the largest DEL_life, that DEL_life}.
+ *   psd (optional, output-bound): per bin sum_h 1/2 |sigma_h(theta, w)|^2 / dw.
+ * Xi complex [n_units, n_rows, n_dof, nw]; w [nw] rad/s.  Exactly one of R (R_shared 1: [n_rings, n_ch, n_r]; 0: [n_units,
+ * n_rings, n_ch, n_r]) and coef (complex; coef_mode RAFTK_FATIGUE_COEF_SHARED [n_rings, n_ch, n_r, nw], _UNIT [n_units, ...],
+ * _ROW [n_units, n_rows, ...]).  mean [n_units, n_cases, n_rings, n_ch] (device) or NULL (0).  Outputs [n_units, n_cases,
+ * n_rings, n_angles]: std, avg, max, min (required), DEL and info (required with m > 0); hot [n_units, n_cases, n_rings, 6] or
+ * NULL; DEL_life [n_units, n_rings, n_angles] and hot_life [n_units, n_rings, 2] or NULL; psd [n_units, n_cases, n_rings,
+ * n_angles, nw] or NULL.  Kernels: one CTA per (unit, row, bin tile) forms the twelve sums per 32-bin chunk into the
+ * workspace; one thread per (unit, case, ring, angle) sums them in (row, chunk) order and finishes; one thread per (unit, case,
+ * ring) finds the hot spot.  No atomics: a result does not depend on the batch, the other cases, rings or angles, or the tile
+ * width.  FP64 throughout.
+ * raftk_stress_ring_workspace_bytes: n_units * n_rows * ceil(nw / 32) * n_rings * 12 doubles, plus n_units * n_cases *
+ * n_rings * n_angles doubles with DEL_life.
+ * _dev: device Xi, w, R / coef, mean and outputs, caller-owned workspace (32-byte aligned), enqueued on `stream`; it
+ * allocates nothing and never synchronises.  _host: host pointers everywhere, staged through the device arena.  case_row0,
+ * col0, wpow, angles and weights are HOST memory in both, read during the call.
+ * RAFTK_EINVAL before any launch: a count below 1, n_ch not 1 or 2, more than RAFTK_STRESS_RING_MAX rings or
+ * RAFTK_STRESS_ANGLE_MAX angles, n_r above n_dof, a col0 outside [0, n_dof - n_r], not exactly one of R and coef, R_shared not 0
+ * or 1, an unknown coef_mode or method, a wpow outside {0, 1, 2}, a NULL w, Xi, angles, case_row0, std, avg, max or min, an
+ * angle that is not finite, a d or t that is not finite and > 0, an m that is not 0 or finite and > 0, m > 0 without DEL and
+ * info, DEL_life without m, hot_life without DEL_life, psd without a finite dw > 0, an f_eq that is not finite and > 0, a
+ * case_row0 as raftk_fatigue refuses it, weights as raftk_fatigue refuses them, or (_dev) a workspace that is too small or
+ * not 32-byte aligned.
+ */
+#define RAFTK_STRESS_RING_MAX 64
+#define RAFTK_STRESS_ANGLE_MAX 256
+typedef struct raftk_stress_ring {
+    int32_t n_cases, n_rings, n_ch, n_r, n_angles;
+    int32_t method;            /* RAFTK_FATIGUE_DIRLIK or RAFTK_FATIGUE_NARROWBAND_METHOD                                */
+    int32_t tile_w;            /* 0: automatic; > 0: at most tile_w bins per CTA (whole 32-bin chunks); RAFTK_FARM_TILE_L2 */
+    int32_t R_shared, coef_mode, _pad0;
+    const int32_t *case_row0;  /* HOST [n_cases + 1]                                                                    */
+    const int32_t *col0;       /* HOST [n_rings] or NULL: all 0                                                          */
+    const int32_t *wpow;       /* HOST [n_rings, n_ch] 0, 1 or 2, or NULL: all 0 (real form only)                        */
+    const double *R, *coef;
+    const double *angles;      /* HOST [n_angles] rad                                                                    */
+    double d, t;               /* tower-base diameter and wall thickness (m)                                            */
+    double m;                  /* Woehler exponent, or 0: no DEL                                                         */
+    double f_eq;               /* equivalent frequency (Hz) of the DEL                                                   */
+    double dw;                 /* PSD divisor (with psd)                                                                 */
+    const double *weights;     /* HOST [n_cases] or NULL                                                                 */
+    const double *mean;
+    double *std, *avg, *max, *min, *DEL;
+    int32_t *info;
+    double *hot, *DEL_life, *hot_life, *psd;
+} raftk_stress_ring;
+
+size_t raftk_stress_ring_workspace_bytes(int32_t n_units, int32_t n_rows, int32_t nw, const raftk_stress_ring *sr);
+int raftk_stress_ring_dev(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                          const raftk_stress_ring *sr, void *workspace, size_t workspace_bytes, void *stream);
+int raftk_stress_ring_host(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                           const raftk_stress_ring *sr);
+
+/*
  * Natural frequencies and mode shapes (Model.solveEigen raft_model.py:436-547, FOWT.solveEigen raft_fowt.py:1646-1729): the
  * eigenvalues and right eigenvectors of M^-1 C for n_systems systems of n DOFs, what np.linalg.eig(np.linalg.solve(M, C))
  * returns, in the reference's output order.  Per system: LU of M with partial pivoting, A = M^-1 C, power-of-two balancing,

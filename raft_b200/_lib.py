@@ -129,6 +129,18 @@ class RaftkFatigue(C.Structure):
                 ("info", C.c_void_p), ("DEL_life", C.c_void_p)]
 
 
+class RaftkStressRing(C.Structure):
+    """include/raftk.h raftk_stress_ring: tower-base moments, section, angles and S-N options of the circumferential axial
+    stress, and its outputs."""
+    _fields_ = [("n_cases", C.c_int32), ("n_rings", C.c_int32), ("n_ch", C.c_int32), ("n_r", C.c_int32), ("n_angles", C.c_int32),
+                ("method", C.c_int32), ("tile_w", C.c_int32), ("R_shared", C.c_int32), ("coef_mode", C.c_int32), ("_pad0", C.c_int32),
+                ("case_row0", C.c_void_p), ("col0", C.c_void_p), ("wpow", C.c_void_p), ("R", C.c_void_p), ("coef", C.c_void_p),
+                ("angles", C.c_void_p), ("d", C.c_double), ("t", C.c_double), ("m", C.c_double), ("f_eq", C.c_double), ("dw", C.c_double),
+                ("weights", C.c_void_p), ("mean", C.c_void_p), ("std", C.c_void_p), ("avg", C.c_void_p), ("max", C.c_void_p),
+                ("min", C.c_void_p), ("DEL", C.c_void_p), ("info", C.c_void_p), ("hot", C.c_void_p), ("DEL_life", C.c_void_p),
+                ("hot_life", C.c_void_p), ("psd", C.c_void_p)]
+
+
 class RaftkEigen(C.Structure):
     """include/raftk.h raftk_eigen: eigenvalues and right eigenvectors of M^-1 C for a batch of systems."""
     _fields_ = [("n_systems", C.c_int32), ("n", C.c_int32), ("sort", C.c_int32), ("_pad0", C.c_int32),
@@ -208,6 +220,7 @@ SYMBOLS = [
     "raftk_farm_channel_stats_workspace_bytes", "raftk_farm_channel_stats_dev", "raftk_farm_channel_stats_host",
     "raftk_rotor_stats_dev", "raftk_rotor_stats_host",
     "raftk_fatigue_workspace_bytes", "raftk_fatigue_dev", "raftk_fatigue_host",
+    "raftk_stress_ring_workspace_bytes", "raftk_stress_ring_dev", "raftk_stress_ring_host",
 ]
 
 
@@ -370,6 +383,12 @@ def _load():
     lib.raftk_fatigue_dev.restype = C.c_int
     lib.raftk_fatigue_host.argtypes = [C.c_int32] * 4 + [C.c_void_p, C.c_void_p, P(RaftkFatigue)]
     lib.raftk_fatigue_host.restype = C.c_int
+    lib.raftk_stress_ring_workspace_bytes.argtypes = [C.c_int32] * 3 + [P(RaftkStressRing)]
+    lib.raftk_stress_ring_workspace_bytes.restype = C.c_size_t
+    lib.raftk_stress_ring_dev.argtypes = [C.c_int32] * 4 + [C.c_void_p, C.c_void_p, P(RaftkStressRing), C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.raftk_stress_ring_dev.restype = C.c_int
+    lib.raftk_stress_ring_host.argtypes = [C.c_int32] * 4 + [C.c_void_p, C.c_void_p, P(RaftkStressRing)]
+    lib.raftk_stress_ring_host.restype = C.c_int
     lib.raftk_family_sizes.argtypes = [P(RaftkFamily), P(C.c_int32), P(C.c_int32)]
     lib.raftk_build_family_host.argtypes = [P(RaftkFamily), P(RaftkFamilyTables)]
     lib.raftk_family_sizes.restype = C.c_int

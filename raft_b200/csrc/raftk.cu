@@ -153,6 +153,7 @@ extern "C" int raftk_last_dispatch(raftk_dispatch *out)
 #include "raftk_misc.cuh"
 #include "raftk_rotor.cuh"
 #include "raftk_fatigue.cuh"
+#include "raftk_stress.cuh"
 #include "raftk_eigen.cuh"
 #include "raftk_builder.h"
 
@@ -2940,6 +2941,209 @@ extern "C" int raftk_fatigue_host(int32_t n_units, int32_t n_rows, int32_t n_dof
     S.buf(ws, wb);
     int rc;
     if ((rc = S.commit()) || (rc = raftk_fatigue_dev(n_units, n_rows, n_dof, nw, dW, dXi, &d, ws, wb, nullptr))) return rc;
+    return S.finish();
+}
+
+// ---- tower-base axial stress around the circumference (raftk_stress_ring_*) -------------------------------------------------
+static size_t str_part_elems(int32_t n_units, int32_t n_rows, int32_t nw, int32_t n_rings)
+{
+    return (size_t)n_units * n_rows * ((nw + STR_CHUNK_BINS - 1) / STR_CHUNK_BINS) * n_rings * STR_NS;
+}
+
+static size_t str_ws(int32_t n_units, int32_t n_rows, int32_t nw, const raftk_stress_ring *sr)
+{
+    return (str_part_elems(n_units, n_rows, nw, sr->n_rings)
+            + (sr->DEL_life ? (size_t)n_units * sr->n_cases * sr->n_rings * sr->n_angles : 0)) * sizeof(double);
+}
+
+static int str_check(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi, const raftk_stress_ring *sr)
+{
+    if (!sr) return set_err(RAFTK_EINVAL, "stress ring: null argument");
+    if (n_units < 1 || n_rows < 1 || n_dof < 1 || nw < 1 || sr->n_cases < 1 || sr->n_rings < 1 || sr->n_r < 1 || sr->n_angles < 1)
+        return set_err(RAFTK_EINVAL, "stress ring: n_units, n_rows, n_dof, nw, n_cases, n_rings, n_r and n_angles must be >= 1");
+    if (sr->n_ch != 1 && sr->n_ch != 2) return set_err(RAFTK_EINVAL, "stress ring: n_ch must be 1 (fore-aft) or 2 (fore-aft, side-side)");
+    if (sr->n_rings > RAFTK_STRESS_RING_MAX) return set_err_i(RAFTK_EINVAL, "stress ring: at most %d rings per call", RAFTK_STRESS_RING_MAX);
+    if (sr->n_angles > RAFTK_STRESS_ANGLE_MAX) return set_err_i(RAFTK_EINVAL, "stress ring: at most %d angles per call", RAFTK_STRESS_ANGLE_MAX);
+    if (sr->n_r > n_dof) return set_err(RAFTK_EINVAL, "stress ring: n_r must not exceed n_dof");
+    for (int32_t k = 0; sr->col0 && k < sr->n_rings; k++)
+        if (sr->col0[k] < 0 || sr->col0[k] > n_dof - sr->n_r) return set_err_i(RAFTK_EINVAL, "stress ring: col0 of ring %d outside [0, n_dof - n_r]", k);
+    if (!sr->R == !sr->coef) return set_err(RAFTK_EINVAL, "stress ring: give exactly one of R (real rows) and coef (complex coefficients)");
+    if (sr->R && sr->R_shared != 0 && sr->R_shared != 1) return set_err(RAFTK_EINVAL, "stress ring: R_shared must be 0 or 1");
+    if (sr->coef && (sr->coef_mode < RAFTK_FATIGUE_COEF_SHARED || sr->coef_mode > RAFTK_FATIGUE_COEF_ROW))
+        return set_err(RAFTK_EINVAL, "stress ring: unknown coef_mode");
+    if (sr->method != RAFTK_FATIGUE_DIRLIK && sr->method != RAFTK_FATIGUE_NARROWBAND_METHOD)
+        return set_err(RAFTK_EINVAL, "stress ring: unknown method");
+    if (!w || !Xi || !sr->angles || !sr->case_row0 || !sr->std || !sr->avg || !sr->max || !sr->min)
+        return set_err(RAFTK_EINVAL, "stress ring: w, Xi, angles, case_row0, std, avg, max and min are required");
+    for (int32_t t = 0; sr->R && sr->wpow && t < sr->n_rings * sr->n_ch; t++)
+        if (sr->wpow[t] < 0 || sr->wpow[t] > 2) return set_err(RAFTK_EINVAL, "stress ring: wpow must be 0, 1 or 2");
+    for (int32_t a = 0; a < sr->n_angles; a++)
+        if (!std::isfinite(sr->angles[a])) return set_err(RAFTK_EINVAL, "stress ring: every angle must be finite");
+    if (!(std::isfinite(sr->d) && sr->d > 0.0) || !(std::isfinite(sr->t) && sr->t > 0.0))
+        return set_err(RAFTK_EINVAL, "stress ring: d and t must be finite and > 0");
+    if (!(sr->m == 0.0 || (std::isfinite(sr->m) && sr->m > 0.0))) return set_err(RAFTK_EINVAL, "stress ring: m must be 0 (no DEL) or finite and > 0");
+    if (sr->m > 0.0 && (!sr->DEL || !sr->info)) return set_err(RAFTK_EINVAL, "stress ring: DEL and info are required with m > 0");
+    if (sr->DEL_life && !(sr->m > 0.0)) return set_err(RAFTK_EINVAL, "stress ring: DEL_life needs m > 0");
+    if (sr->hot_life && !sr->DEL_life) return set_err(RAFTK_EINVAL, "stress ring: hot_life needs DEL_life");
+    if (sr->psd && !(std::isfinite(sr->dw) && sr->dw > 0.0)) return set_err(RAFTK_EINVAL, "stress ring: psd needs a finite dw > 0");
+    if (!(std::isfinite(sr->f_eq) && sr->f_eq > 0.0)) return set_err(RAFTK_EINVAL, "stress ring: f_eq must be finite and > 0");
+    if (sr->case_row0[0] != 0 || sr->case_row0[sr->n_cases] != n_rows)
+        return set_err(RAFTK_EINVAL, "stress ring: case_row0 must start at 0 and end at n_rows");
+    for (int32_t c = 0; c < sr->n_cases; c++)
+        if (sr->case_row0[c + 1] <= sr->case_row0[c]) return set_err(RAFTK_EINVAL, "stress ring: every case needs at least one row");
+    if (sr->weights) {
+        double s = 0.0;
+        for (int32_t c = 0; c < sr->n_cases; c++) {
+            if (!(std::isfinite(sr->weights[c]) && sr->weights[c] >= 0.0)) return set_err(RAFTK_EINVAL, "stress ring: weights must be finite and >= 0");
+            s += sr->weights[c];
+        }
+        if (!(s > 0.0)) return set_err(RAFTK_EINVAL, "stress ring: the weights must not all be 0");
+    }
+    const size_t rows = (size_t)n_units * n_rows;
+    if (rows * ((nw + STR_CHUNK_BINS - 1) / STR_CHUNK_BINS) > 2147483647u || (size_t)n_units * sr->n_rings * sr->n_angles > 2147483647u)
+        return set_err(RAFTK_EINVAL, "stress ring: too many (unit, row, bin tile) blocks");
+    return RAFTK_OK;
+}
+
+extern "C" size_t raftk_stress_ring_workspace_bytes(int32_t n_units, int32_t n_rows, int32_t nw, const raftk_stress_ring *sr)
+{
+    if (!sr || n_units < 1 || n_rows < 1 || nw < 1 || sr->n_cases < 1 || sr->n_rings < 1 || sr->n_angles < 1) return 0;
+    return str_ws(n_units, n_rows, nw, sr);
+}
+
+extern "C" int raftk_stress_ring_dev(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                                     const raftk_stress_ring *sr, void *workspace, size_t workspace_bytes, void *stream)
+{
+    if (int rc = str_check(n_units, n_rows, n_dof, nw, w, Xi, sr)) return rc;
+    if (!workspace || workspace_bytes < str_ws(n_units, n_rows, nw, sr))
+        return set_err(RAFTK_EINVAL, "stress ring: the workspace is too small (raftk_stress_ring_workspace_bytes)");
+    if ((uintptr_t)workspace % 32) return set_err(RAFTK_EINVAL, "stress ring: the workspace must be 32-byte aligned");
+    const cudaStream_t st = (cudaStream_t)stream;
+    const size_t rows = (size_t)n_units * n_rows;
+    double *part = static_cast<double *>(workspace);
+    double *wd = sr->DEL_life ? part + str_part_elems(n_units, n_rows, nw, sr->n_rings) : nullptr;
+    StrParams P = {};
+    P.n = n_dof; P.n_r = sr->n_r; P.nw = nw; P.n_rows = n_rows; P.n_rings = sr->n_rings; P.n_ch = sr->n_ch;
+    P.n_chunks = (nw + STR_CHUNK_BINS - 1) / STR_CHUNK_BINS;
+    P.w = w; P.R = sr->R; P.Xi = reinterpret_cast<const double2 *>(Xi); P.part = part;
+    P.coef = reinterpret_cast<const double2 *>(sr->coef);
+    const size_t cf = (size_t)sr->n_rings * sr->n_ch * sr->n_r * nw;
+    P.r_stride = sr->R_shared ? 0 : (size_t)sr->n_rings * sr->n_ch * sr->n_r;
+    P.cf_ustride = sr->coef_mode == RAFTK_FATIGUE_COEF_UNIT ? cf : (sr->coef_mode == RAFTK_FATIGUE_COEF_ROW ? cf * n_rows : 0);
+    P.cf_rstride = sr->coef_mode == RAFTK_FATIGUE_COEF_ROW ? cf : 0;
+    for (int32_t k = 0; k < sr->n_rings; k++) P.col0[k] = sr->col0 ? sr->col0[k] : 0;
+    for (int32_t t = 0; sr->R && sr->wpow && t < sr->n_rings * sr->n_ch; t++) {
+        const int k = t / sr->n_ch, j = t - k * sr->n_ch;
+        P.wbits[k >> 3] |= (unsigned)sr->wpow[t] << ((k & 7) * 4 + 2 * j);
+    }
+    const double Izz = 3.141592653589793 / 8.0 * sr->t * sr->d * sr->d * sr->d;
+    P.c = 0.5 * sr->d / Izz / 1e6; P.c2 = P.c * P.c;
+    P.n_cases = sr->n_cases; P.n_angles = sr->n_angles; P.method = sr->method;
+    P.f_eq = sr->f_eq; P.m = sr->m; P.dw = sr->dw; P.mean = sr->mean;
+    P.std = sr->std; P.avg = sr->avg; P.mx = sr->max; P.mn = sr->min; P.DEL = sr->DEL; P.info = sr->info; P.wd = wd;
+    P.psd = sr->psd;
+    for (int32_t a = 0; a < sr->n_angles; a++) P.angle[a] = sr->angles[a];
+    const int tile = fat_tile(rows, n_dof, nw, sr->tile_w);
+    P.tile = tile ? tile : std::min<int32_t>((nw + STR_CHUNK_BINS - 1) / STR_CHUNK_BINS * STR_CHUNK_BINS, 256);
+    P.n_tiles = (nw + P.tile - 1) / P.tile;
+    const size_t grid = rows * P.n_tiles;
+    const bool coef = sr->coef != nullptr;
+    if (tile) {
+        const size_t smem = (size_t)n_dof * tile * sizeof(double2);
+        static SmemOptIn opt_r(48 * 1024), opt_c(48 * 1024);
+        if (coef) {
+            CUDA_TRY(opt_c.ensure(k_stress_moments<true, true>, smem));
+            k_stress_moments<true, true><<<(unsigned)grid, STR_T, smem, st>>>(P);
+        } else {
+            CUDA_TRY(opt_r.ensure(k_stress_moments<true, false>, smem));
+            k_stress_moments<true, false><<<(unsigned)grid, STR_T, smem, st>>>(P);
+        }
+    } else if (coef) {
+        k_stress_moments<false, true><<<(unsigned)grid, STR_T, 0, st>>>(P);
+    } else {
+        k_stress_moments<false, false><<<(unsigned)grid, STR_T, 0, st>>>(P);
+    }
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    // chunks of cases only bound the launch parameters: every thread computes the same thing in any chunk
+    for (int32_t c0 = 0; c0 < sr->n_cases; c0 += STR_LAUNCH_CASES) {
+        P.c0 = c0; P.nc = std::min<int32_t>(STR_LAUNCH_CASES, sr->n_cases - c0);
+        for (int j = 0; j <= P.nc; j++) P.row0[j] = sr->case_row0[c0 + j];
+        for (int j = 0; j < P.nc; j++) P.p[j] = sr->weights ? sr->weights[c0 + j] : 1.0;
+        const size_t nt = (size_t)n_units * P.nc * sr->n_rings * sr->n_angles;
+        k_stress_finish<<<(unsigned)((nt + STR_FIN_T - 1) / STR_FIN_T), STR_FIN_T, 0, st>>>(P, nt);
+        g_launches++;
+        CUDA_TRY(cudaGetLastError());
+        if (sr->hot) {
+            P.hot = sr->hot;
+            const size_t nh = (size_t)n_units * P.nc * sr->n_rings;
+            k_stress_hot<<<(unsigned)((nh + STR_FIN_T - 1) / STR_FIN_T), STR_FIN_T, 0, st>>>(P, nh);
+            g_launches++;
+            CUDA_TRY(cudaGetLastError());
+        }
+        if (sr->psd) {
+            const size_t np_ = (size_t)n_units * P.nc * sr->n_rings * nw;
+            const unsigned gp = (unsigned)((np_ + STR_FIN_T - 1) / STR_FIN_T);
+            if (coef) k_stress_psd<true><<<gp, STR_FIN_T, 0, st>>>(P, np_);
+            else k_stress_psd<false><<<gp, STR_FIN_T, 0, st>>>(P, np_);
+            g_launches++;
+            CUDA_TRY(cudaGetLastError());
+        }
+    }
+    if (sr->DEL_life) {
+        // per (ring, angle) the lifetime sum of k_fatigue_life, the (ring, angle) pairs taking the place of its channels
+        FatLifeParams L = {};
+        double W = 0.0;
+        for (int32_t c = 0; c < sr->n_cases; c++) W += sr->weights ? sr->weights[c] : 1.0;
+        const int32_t nk = sr->n_rings * sr->n_angles;
+        L.n_cases = sr->n_cases; L.nch = nk; L.log_fw = std::log(sr->f_eq * W); L.wd = wd; L.DEL_life = sr->DEL_life;
+        for (int j = 0; j < FAT_LAUNCH_CHUNK; j++) L.m[j] = sr->m;
+        for (int32_t k0 = 0; k0 < nk; k0 += FAT_LAUNCH_CHUNK) {
+            L.k0 = k0; L.nk = std::min<int32_t>(FAT_LAUNCH_CHUNK, nk - k0);
+            const size_t nt = (size_t)n_units * L.nk;
+            k_fatigue_life<<<(unsigned)((nt + FAT_FIN_T - 1) / FAT_FIN_T), FAT_FIN_T, 0, st>>>(L, nt);
+            g_launches++;
+            CUDA_TRY(cudaGetLastError());
+        }
+        if (sr->hot_life) {
+            P.hot = sr->hot_life;
+            const size_t nh = (size_t)n_units * sr->n_rings;
+            k_stress_hot_life<<<(unsigned)((nh + STR_FIN_T - 1) / STR_FIN_T), STR_FIN_T, 0, st>>>(P, sr->DEL_life, nh);
+            g_launches++;
+            CUDA_TRY(cudaGetLastError());
+        }
+    }
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_stress_ring_host(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
+                                      const raftk_stress_ring *sr)
+{
+    if (int rc = str_check(n_units, n_rows, n_dof, nw, w, Xi, sr)) return rc;
+    const size_t ring = (size_t)sr->n_rings, na = sr->n_angles;
+    const size_t out = (size_t)n_units * sr->n_cases * ring * na, ucr = (size_t)n_units * sr->n_cases * ring;
+    const size_t per = ring * sr->n_ch * sr->n_r;
+    const size_t wb = str_ws(n_units, n_rows, nw, sr);
+    size_t n_coef = 0;
+    if (sr->coef)
+        n_coef = (sr->coef_mode == RAFTK_FATIGUE_COEF_SHARED ? 1 : (size_t)n_units) * (sr->coef_mode == RAFTK_FATIGUE_COEF_ROW ? n_rows : 1)
+                 * per * nw * 2;
+    raftk_stress_ring d = *sr;
+    const double *dW, *dXi;
+    char *ws;
+    Staging S("raftk_stress_ring_host");
+    S.in(dW, w, nw); S.in(dXi, Xi, (size_t)n_units * n_rows * n_dof * nw * 2);
+    S.in(d.R, sr->R, (sr->R_shared ? 1 : (size_t)n_units) * per); S.in(d.coef, sr->coef, n_coef);
+    S.in(d.mean, sr->mean, ucr * sr->n_ch);
+    S.out(d.std, out, sr->std); S.out(d.avg, out, sr->avg); S.out(d.max, out, sr->max); S.out(d.min, out, sr->min);
+    S.out(d.DEL, sr->DEL ? out : 0, sr->DEL); S.out(d.info, sr->info ? out : 0, sr->info);
+    S.out(d.hot, sr->hot ? ucr * 6 : 0, sr->hot);
+    S.out(d.DEL_life, sr->DEL_life ? (size_t)n_units * ring * na : 0, sr->DEL_life);
+    S.out(d.hot_life, sr->hot_life ? (size_t)n_units * ring * 2 : 0, sr->hot_life);
+    S.out(d.psd, sr->psd ? out * nw : 0, sr->psd);
+    S.buf(ws, wb);
+    int rc;
+    if ((rc = S.commit()) || (rc = raftk_stress_ring_dev(n_units, n_rows, n_dof, nw, dW, dXi, &d, ws, wb, nullptr))) return rc;
     return S.finish();
 }
 

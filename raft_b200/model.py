@@ -14,7 +14,7 @@ from .fowt import FOWT
 
 class Model:
     def __init__(self, design, matrices=None, array_stiffness=None, channels=None, tension_jacobian=None, mean_tensions=None,
-                 array_tension_jacobian=None, array_mean_tensions=None, rotors=None, turbine_constants=None, fatigue=None):
+                 array_tension_jacobian=None, array_mean_tensions=None, rotors=None, turbine_constants=None, fatigue=None, stress=None):
         """``channels``: optional turbine output channels per FOWT (``packer.pack_turbine_channels`` dicts: nacelle
         accelerations, tower-base moment) -- the turbine itself is outside this path, its constants enter here.
         ``tension_jacobian`` [2L,6] / ``mean_tensions`` [2L] (one for every FOWT, or a list with None for a FOWT without its
@@ -35,7 +35,13 @@ class Model:
         (``solver.fatigue_options``), e.g. m={"Mbase": 4.0, "Tmoor": 3.0}: analyzeCases then adds, per case and FOWT,
         ``<name>_DEL`` of the named turbine channels ([nrot]) and ``Tmoor_DEL`` [2L] of the FOWT's lines,
         case_metrics[iCase]['array_mooring']['Tmoor_DEL'] of the array's, and with weights the lifetime DELs in
-        results['fatigue'] (the same keys per FOWT, and 'array_mooring').  Without it the results are unchanged."""
+        results['fatigue'] (the same keys per FOWT, and 'array_mooring').  Without it the results are unchanged.
+        ``stress``: dict(d=10.0, t=0.083, angles=None, m=None, f_eq=1.0, method="dirlik", weights=None, psd=False)
+        (``solver.stress_options``): analyzeCases then adds, per case and FOWT with turbine channels, the tower-base axial
+        stress around the circumference from each tower's Mbase (``solver.stress_ring``, helpers.getSigmaXPSD; a rigid tower
+        has no side-side moment): ``sigmaX_avg/_std/_max/_min`` [nrot, nA], ``sigmaX_PSD`` [nrot, nA, nw] with psd,
+        ``sigmaX_DEL`` [nrot, nA] with m, ``sigmaX_hot`` (``solver.stress_hot``), and with weights (and m)
+        results['fatigue'][i]['sigmaX_DEL'] and ['sigmaX_hot'] of the lifetime.  Without it the results are unchanged."""
         s = design.setdefault("settings", {})
         min_freq, max_freq = float(s.get("min_freq", 0.01)), float(s.get("max_freq", 1.00))
         self.XiStart = float(s.get("XiStart", 0.1))
@@ -93,6 +99,13 @@ class Model:
             missing = sorted(set(self.fatigue["m"]) - known)
             if missing:
                 raise ValueError("fatigue=: no channel named %s" % missing)
+        self.stress = None if stress is None else solver.stress_options(stress)
+        if self.stress is not None:
+            have = [ch for ch in self.channels if ch is not None]
+            if not have:
+                raise ValueError("stress=: the channels have no tower-base moment (Mbase, or MbaseY and MbaseX)")
+            for ch in have:
+                solver.stress_rows((ch[0] if isinstance(ch, (list, tuple)) else ch)["names"])
         for f in self.fowtList:
             f.calcHydroConstants()
 
@@ -149,6 +162,7 @@ class Model:
         dw = self.w[1] - self.w[0]
         rot = self._rotor_stats(cases, out, dw)
         fat = None if self.fatigue is None else self._fatigue(cases, out, Xi_units)
+        sig = None if self.stress is None else self._stress(cases, out, Xi_units)
         self.results["case_metrics"] = {}
         for ic in range(nC):
             idx = np.nonzero(owner == ic)[0]
@@ -177,6 +191,8 @@ class Model:
                     m.update(solver.rotor_metrics(self.rotors[i], ic, rot[0][0][ic, k], rot[0][1][ic, k], dw))
                 if fat is not None:
                     m.update(fat["case"][ic][i])
+                if sig is not None and sig[i] is not None:
+                    m.update(solver.stress_entries(sig[i], ic))
                 self.results["case_metrics"][ic][i] = m
             if arr is not None:
                 self.results["case_metrics"][ic]["array_mooring"] = solver.tension_metrics(self.array_tensions["T0"],
@@ -185,7 +201,37 @@ class Model:
                     self.results["case_metrics"][ic]["array_mooring"].update(fat["case"][ic]["array_mooring"])
         if fat is not None and fat["life"] is not None:
             self.results["fatigue"] = fat["life"]
+        for i, r in enumerate(sig or []):
+            if r is not None and "DEL_life" in r:
+                self.results.setdefault("fatigue", {}).setdefault(i, {}).update(sigmaX_DEL=np.array(r["DEL_life"]),
+                                                                                sigmaX_hot=solver.stress_hot(r))
         return self.results
+
+    def _stress(self, cases, out, Xi_units):
+        """The tower-base stress ring of every FOWT with turbine channels (``stress=``) on its trains Xi_units [nT, nFOWT, 6,
+        nw]: each tower's Mbase coefficients (per case when ``channels`` is a per-case list) as the fore-aft moment.  -> per
+        FOWT a solver.stress_ring result without the unit axis, or None."""
+        o = self.stress
+        owner = out["owner"]
+        row0 = np.append(np.nonzero(np.diff(np.append(-1, owner)))[0], len(owner))
+        first = row0[:-1]
+        res = []
+        for i, ch in enumerate(self.channels):
+            if ch is None:
+                res.append(None)
+                continue
+            per_case = isinstance(ch, (list, tuple))
+            rows, _ = solver.stress_rows((ch[0] if per_case else ch)["names"])
+            if per_case:
+                fa = np.stack([np.asarray(ch[c]["coef"])[rows] for c in owner])[None]            # [1, nT, nrot, 6, nw]
+                mean = np.stack([np.asarray(ch[owner[t]]["avg"])[rows] for t in first])[None, :, :, None]
+                xi = Xi_units[None, :, i]
+            else:
+                fa, mean, xi = np.asarray(ch["coef"])[rows], np.asarray(ch["avg"])[rows][:, None], Xi_units[:, i]
+            r = solver.stress_ring(xi, self.w, fa, None, o["angles"], o["d"], o["t"], m=o["m"], f_eq=o["f_eq"], method=o["method"],
+                                   weights=o["weights"], case_row0=row0, psd=o["psd"], mean=mean, dw=self.w[1] - self.w[0])
+            res.append({k: v[0] for k, v in r.items()} if per_case else r)
+        return res
 
     def _fatigue(self, cases, out, Xi_units):
         """Fatigue DELs of every case (``fatigue=``) on the device: each FOWT's named turbine channels (their coefficients,

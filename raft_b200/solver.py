@@ -920,6 +920,14 @@ class GeneralSession:
         return _fatigue(_session_buffers(self), self.Xi, self.keep["w"], m, R, wpow, coef, case_row0, f_eq, method, weights, life,
                         moments, tile_w)
 
+    def stress_ring(self, fa, ss, angles=None, d=10.0, t=0.083, m=None, f_eq=1.0, method="dirlik", weights=None, case_row0=None,
+                    col0=None, psd=False, mean=None, wpow=None, tile_w=0):
+        """Tower-base axial stress around the circumference of the last ``solve()`` (raftk_stress_ring_dev on the resident Xi [nT, nDOF, nw]):
+        ``fa`` / ``ss`` the fore-aft / side-side rows (MbaseY / MbaseX of ``packer.pack_general_channels``); the other
+        arguments as ``stress_ring``.  -> dict of torch tensors as ``stress_ring`` (std [nC, n_rings, nA], ...)."""
+        return _stress_ring(_session_buffers(self), self.Xi, self.keep["w"], fa, ss, angles, d, t, m, f_eq, method, weights, case_row0,
+                            col0, psd, mean, wpow, self.dw, tile_w)
+
 
 def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0, fd=None, F_BEM=False, qtf=None, F_2nd=False,
                            max_chunk_cases=None):
@@ -1362,6 +1370,206 @@ def _fatigue(be, Xi, w, m, R, wpow, coef, case_row0, f_eq, method, weights, life
     return {k: v[0] for k, v in out.items()} if squeeze else out
 
 
+STRESS_ANGLES = np.linspace(0, 2 * np.pi, 50)       # helpers.getSigmaXPSD's default angles (helpers.py:1164)
+STRESS_HOT = ("angle", "std", "angle_DEL", "DEL", "std_exact", "angle_exact")   # include/raftk.h raftk_stress_ring hot
+
+
+def _stress_channels(be, fa, ss, n_units, n_rows, n, nw, wpow):
+    """Fore-aft / side-side channels of stress_ring -> (stacked R or coef on ``be``, n_rings, n_r, n_ch, R_shared or coef_mode,
+    wpow [n_rings, n_ch] int32 or None).  Real rows: fa [n_r], [n_rings, n_r] or [n_units, n_rings, n_r]; complex per-bin
+    coefficients: fa [n_r, nw], [n_rings, n_r, nw], [n_units, n_rings, n_r, nw] or [n_units, n_rows, n_rings, n_r, nw];
+    ss None (fore-aft only) or the same form and shape."""
+    def cplx(a):
+        return a.is_complex() if hasattr(a, "is_complex") else np.iscomplexobj(a)
+    coef = cplx(fa)
+    if ss is not None and (cplx(ss) != coef or tuple(ss.shape) != tuple(fa.shape)):
+        raise ValueError("stress_ring: ss must have fa's form and shape")
+    dt = _C16 if coef else _F8
+    chans = [be.array(fa, dt)] + ([] if ss is None else [be.array(ss, dt)])
+    nd = len(chans[0].shape)
+    tail = 2 if coef else 1                               # (n_r, nw) or (n_r,)
+    if coef:
+        lead = {2: (), 3: (), 4: (n_units,), 5: (n_units, n_rows)}.get(nd)
+        mode = {2: 0, 3: 0, 4: 1, 5: 2}.get(nd)
+    else:
+        lead = {1: (), 2: (), 3: (n_units,)}.get(nd)
+        mode = {1: 1, 2: 1, 3: 0}.get(nd)
+    if lead is None or tuple(chans[0].shape[:len(lead)]) != lead or (coef and chans[0].shape[-1] != nw):
+        raise ValueError("stress_ring: fa must be real [n_r], [n_rings, n_r] or [%d, n_rings, n_r], or complex [n_r, %d], "
+                         "[n_rings, n_r, %d], [%d, n_rings, n_r, %d] or [%d, %d, n_rings, n_r, %d]"
+                         % (n_units, nw, nw, n_units, nw, n_units, n_rows, nw))
+    if nd == len(lead) + tail:                            # one ring
+        chans = [c.reshape(tuple(lead) + (1,) + tuple(c.shape[len(lead):])) for c in chans]
+    n_rings, n_r = chans[0].shape[len(lead)], chans[0].shape[len(lead) + 1]
+    if n_r > n:
+        raise ValueError("stress_ring: the channels read %d columns of a response with %d" % (n_r, n))
+    stk = np if isinstance(chans[0], np.ndarray) else be.torch
+    X = stk.stack(chans, len(lead) + 1) if len(chans) == 2 else chans[0].reshape(tuple(lead) + (n_rings, 1) + tuple(chans[0].shape[len(lead) + 1:]))
+    X = be.array(X, dt)
+    if coef:
+        if wpow is not None:
+            raise ValueError("wpow applies to real rows only")
+        return X, n_rings, n_r, len(chans), mode, None
+    wp = np.ascontiguousarray(np.broadcast_to(np.zeros(1, dtype=_I4) if wpow is None else np.asarray(wpow, dtype=_I4), (n_rings, len(chans))))
+    _check_wpow(wp)
+    return X, n_rings, n_r, len(chans), mode, wp
+
+
+def stress_ring(Xi, w, fa, ss, angles=None, d=10.0, t=0.083, m=None, f_eq=1.0, method="dirlik", weights=None, case_row0=None,
+                col0=None, psd=False, mean=None, wpow=None, dw=None, tile_w=0):
+    """Tower-base axial stress around the circumference on the device (raftk_stress_ring_host), host buffers: the reference's
+    helpers.getSigmaXPSD (helpers.py:1164) for every unit, case, ring (tower base) and angle, and its statistics.  Thin-wall
+    section, Izz = pi/8 t d^3, sigma(theta) = (a cos theta - b sin theta) (d/2) / Izz / 1e6 (MPa) of the fore-aft moment a
+    (``fa``) and the side-side moment b (``ss``; None: fore-aft only, as a rigid tower's Mbase) over the case's rows.  The
+    response is walked once for the cross-spectral moments of a and b; every angle follows in closed form.
+    ``Xi`` complex [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]; ``fa`` / ``ss`` real rows (``packer.pack_general_
+    channels``' MbaseY / MbaseX rows, ``wpow`` [n_rings, 2]) or complex per-bin coefficients (``pack_turbine_channels``'
+    Mbase), as ``_stress_channels``; ``angles`` rad (None: 50 over [0, 2 pi]); ``d``, ``t`` diameter and wall thickness (m);
+    ``col0`` [n_rings] the first response column of every ring's channels (FOWT i of a farm: 6 i); ``mean`` the channels'
+    mean values, broadcast to [n_units, nC, n_rings, n_ch] (None: 0); ``m``: the Woehler exponent of the per-angle DELs
+    (``fatigue``'s closed form, ``f_eq``, ``method``); ``weights`` [nC] with m: the per-angle lifetime DEL_life, as
+    ``fatigue``'s, and its hot spot; ``psd``: per-bin stress PSD, divided by ``dw`` (default w[1] - w[0]).
+    -> dict(std, avg, max, min [n_units, nC, n_rings, nA] (max / min = avg +- 3 std), hot [n_units, nC, n_rings, 6] (
+    ``STRESS_HOT``: sampled argmax angle and std, argmax angle and DEL, exact largest std and its angle in [0, pi)), DEL and
+    info (with m), DEL_life [n_units, n_rings, nA] and hot_life [n_units, n_rings, 2] (angle, DEL) with weights and m, psd [n_units,
+    nC, n_rings, nA, nw] with psd), without the unit axis when ``Xi`` had none.  ``tile_w`` as ``fatigue``."""
+    return _stress_ring(_HOST, Xi, w, fa, ss, angles, d, t, m, f_eq, method, weights, case_row0, col0, psd, mean, wpow, dw, tile_w)
+
+
+def _stress_ring(be, Xi, w, fa, ss, angles, d, t, m, f_eq, method, weights, case_row0, col0, psd, mean, wpow, dw, tile_w):
+    """``stress_ring`` on ``be``'s buffers (angles, case_row0, col0, wpow and weights: numpy)."""
+    Xi = be.array(Xi, _C16)
+    squeeze = Xi.ndim == 3
+    if squeeze:
+        Xi = Xi[None]
+    if Xi.ndim != 4:
+        raise ValueError("Xi must be [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]")
+    nU, nR, n, nw = Xi.shape
+    w = be.array(w, _F8)
+    if tuple(w.shape) != (nw,):
+        raise ValueError("w must be [nw]")
+    X, n_rings, n_r, n_ch, mode, wp = _stress_channels(be, fa, ss, nU, nR, n, nw, wpow)
+    angles = np.ascontiguousarray(STRESS_ANGLES if angles is None else np.atleast_1d(np.asarray(angles, dtype=_F8)))
+    if angles.ndim != 1 or not 1 <= len(angles) <= 256 or not np.all(np.isfinite(angles)):
+        raise ValueError("angles must be 1 to 256 finite values (rad)")
+    if not (np.isfinite(d) and d > 0 and np.isfinite(t) and t > 0):
+        raise ValueError("d and t must be finite and > 0")
+    if m is not None and not (np.isfinite(m) and m > 0):
+        raise ValueError("m must be finite and > 0")
+    if not (np.isfinite(f_eq) and f_eq > 0):
+        raise ValueError("f_eq must be finite and > 0")
+    if method not in FATIGUE_METHODS:
+        raise ValueError("method must be one of %s" % sorted(FATIGUE_METHODS))
+    nC = nR if case_row0 is None else len(case_row0) - 1
+    case_row0 = np.arange(nC + 1, dtype=_I4) if case_row0 is None else np.ascontiguousarray(case_row0, dtype=_I4)
+    if nC < 1 or case_row0[0] != 0 or case_row0[-1] != nR or np.any(np.diff(case_row0) < 1):
+        raise ValueError("case_row0 must start at 0, end at %d and give every case at least one row" % nR)
+    if n_rings > 64:
+        raise ValueError("at most 64 rings per call")
+    col0 = np.zeros(n_rings, dtype=_I4) if col0 is None else np.ascontiguousarray(np.broadcast_to(np.asarray(col0, dtype=_I4), (n_rings,)))
+    if np.any(col0 < 0) or np.any(col0 > n - n_r):
+        raise ValueError("col0 must lie in [0, %d]" % (n - n_r))
+    if weights is not None:
+        weights = np.ascontiguousarray(weights, dtype=_F8)
+        if weights.shape != (nC,) or not np.all(np.isfinite(weights)) or np.any(weights < 0) or not weights.sum() > 0:
+            raise ValueError("weights must be [nC], finite, >= 0 and not all 0")
+    life = weights is not None and m is not None
+    dw = (float(w[1] - w[0]) if nw > 1 else 1.0) if dw is None else float(dw)
+    if psd and not (np.isfinite(dw) and dw > 0):
+        raise ValueError("dw must be finite and > 0")
+    mu = None if mean is None else be.array(np.broadcast_to(np.asarray(mean, dtype=_F8), (nU, nC, n_rings, n_ch)), _F8)
+    sr = _lib.RaftkStressRing()
+    sr.n_cases, sr.n_rings, sr.n_ch, sr.n_r, sr.n_angles = nC, n_rings, n_ch, n_r, len(angles)
+    sr.method, sr.tile_w = FATIGUE_METHODS[method], int(tile_w)
+    if wp is None:
+        sr.coef_mode = mode
+    else:
+        sr.R_shared = mode
+    sr.case_row0, sr.col0, sr.wpow, sr.angles = case_row0.ctypes.data, col0.ctypes.data, None if wp is None else wp.ctypes.data, angles.ctypes.data
+    sr.d, sr.t, sr.m, sr.f_eq, sr.dw = float(d), float(t), 0.0 if m is None else float(m), float(f_eq), dw
+    sr.weights = None if weights is None else weights.ctypes.data
+    shp = [nU, nC, n_rings, len(angles)]
+    out = {k: be.empty(shp) for k in ("std", "avg", "max", "min")}
+    out["hot"] = be.empty([nU, nC, n_rings, 6])
+    if m is not None:
+        out["DEL"], out["info"] = be.empty(shp), be.empty(shp, _I4)
+    if life:
+        out["DEL_life"], out["hot_life"] = be.empty([nU, n_rings, len(angles)]), be.empty([nU, n_rings, 2])
+    if psd:
+        out["psd"] = be.empty(shp + [nw])
+    if wp is None:
+        sr.coef = be.ptr(X)
+    else:
+        sr.R = be.ptr(X)
+    sr.mean = be.ptr(mu)
+    for k in ("std", "avg", "max", "min", "hot", "DEL", "info", "DEL_life", "hot_life", "psd"):
+        setattr(sr, k, be.ptr(out.get(k)))
+    be.call("stress_ring", nU, nR, n, nw, be.ptr(w), be.ptr(Xi), C.byref(sr), ws=(nU, nR, nw, C.byref(sr)))
+    return {k: v[0] for k, v in out.items()} if squeeze else out
+
+
+def stress_hot(r, ic=None):
+    """``sigmaX_hot`` entries from a stress_ring result without the unit axis: case ``ic`` -> per ring dict(angle, std,
+    angle_DEL, DEL (with m), std_exact, angle_exact) as arrays [n_rings]; ``ic`` None: the lifetime's dict(angle, DEL)."""
+    if ic is None:
+        h = np.asarray(r["hot_life"])
+        return dict(angle=h[:, 0].copy(), DEL=h[:, 1].copy())
+    h = np.asarray(r["hot"][ic])
+    out = {k: h[:, j].copy() for j, k in enumerate(STRESS_HOT)}
+    if "DEL" not in r:
+        del out["angle_DEL"], out["DEL"]
+    return out
+
+
+def stress_entries(r, ic):
+    """The ``sigmaX_*`` entries of case ``ic`` from a stress_ring result without the unit axis: _avg / _std / _max / _min
+    [n_rings, nA], _PSD [n_rings, nA, nw] (with psd), _DEL [n_rings, nA] (with m) and _hot (``stress_hot``)."""
+    m = {"sigmaX" + s: np.array(r[k][ic]) for s, k in (("_avg", "avg"), ("_std", "std"), ("_max", "max"), ("_min", "min"))}
+    if "psd" in r:
+        m["sigmaX_PSD"] = np.array(r["psd"][ic])
+    if "DEL" in r:
+        m["sigmaX_DEL"] = np.array(r["DEL"][ic])
+    m["sigmaX_hot"] = stress_hot(r, ic)
+    return m
+
+
+def stress_options(stress):
+    """The ``stress=`` option of ``Model``, ``general_analyze_cases`` and ``general_analyze_cases_batch``: dict(d=10.0,
+    t=0.083, angles=None (50 over [0, 2 pi]), m=None, f_eq=1.0, method="dirlik", weights=None, psd=False) -> the same dict,
+    checked and completed."""
+    if not isinstance(stress, dict):
+        raise ValueError("stress= must be a dict, e.g. dict(d=10.0, t=0.083, m=4.0)")
+    bad = sorted(set(stress) - {"d", "t", "angles", "m", "f_eq", "method", "weights", "psd"})
+    if bad:
+        raise ValueError("stress=: unknown option(s) %s" % bad)
+    o = dict(d=float(stress.get("d", 10.0)), t=float(stress.get("t", 0.083)),
+             angles=np.array(STRESS_ANGLES if stress.get("angles") is None else stress["angles"], dtype=float),
+             m=None if stress.get("m") is None else float(stress["m"]), f_eq=float(stress.get("f_eq", 1.0)),
+             method=stress.get("method", "dirlik"), weights=stress.get("weights"), psd=bool(stress.get("psd", False)))
+    if not (np.isfinite(o["d"]) and o["d"] > 0 and np.isfinite(o["t"]) and o["t"] > 0):
+        raise ValueError("stress=: d and t must be finite and > 0")
+    if o["m"] is not None and not (np.isfinite(o["m"]) and o["m"] > 0):
+        raise ValueError("stress=: m must be finite and > 0")
+    if o["method"] not in FATIGUE_METHODS:
+        raise ValueError("stress=: method must be one of %s" % sorted(FATIGUE_METHODS))
+    if o["angles"].ndim != 1 or not 1 <= len(o["angles"]) <= 256 or not np.all(np.isfinite(o["angles"])):
+        raise ValueError("stress=: angles must be 1 to 256 finite values (rad)")
+    return o
+
+
+def stress_rows(names):
+    """Rows of the tower-base moments in channels ``names`` [(name, rotor index)]: -> (fore-aft rows, side-side rows or
+    None, per rotor), a flexible tower's MbaseY / MbaseX, else a rigid tower's Mbase (fore-aft only).  ValueError when
+    there is neither."""
+    idx = {(nm, ir): k for k, (nm, ir) in enumerate(names)}
+    rot = sorted({ir for nm, ir in names if nm in ("Mbase", "MbaseY") and ir is not None})
+    if rot and all(("MbaseY", ir) in idx and ("MbaseX", ir) in idx for ir in rot):
+        return [idx["MbaseY", ir] for ir in rot], [idx["MbaseX", ir] for ir in rot]
+    if rot and all(("Mbase", ir) in idx for ir in rot):
+        return [idx["Mbase", ir] for ir in rot], None
+    raise ValueError("stress=: the channels have no tower-base moment (Mbase, or MbaseY and MbaseX)")
+
+
 def fatigue_options(fatigue):
     """The ``fatigue=`` option of ``Model``, ``general_analyze_cases`` and ``general_analyze_cases_batch``:
     dict(m={channel name: Woehler exponent}, f_eq=1.0, method="dirlik", weights=None) -> the same dict, checked and completed.
@@ -1476,7 +1684,7 @@ def rotor_channel_entries(m, nm, ir, nrot, avg, std, psd):
 
 
 def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, fd=None, qtf=None, rotors=None,
-                          turbine_constants=None, ops=None, fatigue=None):
+                          turbine_constants=None, ops=None, fatigue=None, stress=None):
     """Model.analyzeCases (dynamics and output statistics) for one FOWT with generalised degrees of freedom: ``cases`` a list
     of case dicts, scalar or list-valued wave keys (several wave trains); ``channels`` from ``packer.pack_general_channels``.
     -> dict(Xi_trains [per case: nTrains,nDOF,nw], status [nC,4] of train 0, case_metrics {case: saveTurbineOutputs entries},
@@ -1490,18 +1698,51 @@ def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01
     ``Model(turbine_constants=)``): NotImplementedError, since M, B and fd come here already packed.
     ``fatigue``: dict(m={channel name: Woehler exponent}, f_eq=1.0, method="dirlik", weights=None) (``fatigue_options``)
     adds every case's ``<name>_DEL`` of the named channels (per-rotor channels [nrot], ``Tmoor_DEL`` [2L], ``Mbase_DEL`` the
-    alias of ``MbaseY_DEL``) and, with weights, the lifetime DELs in the result's ``fatigue``.  Without it nothing changes."""
+    alias of ``MbaseY_DEL``) and, with weights, the lifetime DELs in the result's ``fatigue``.  Without it nothing changes.
+    ``stress``: dict(d=10.0, t=0.083, angles=None, m=None, f_eq=1.0, method="dirlik", weights=None, psd=False)
+    (``stress_options``) adds every case's tower-base axial stress around the circumference from MbaseY (fore-aft) and MbaseX
+    (side-side) (``stress_ring``, helpers.getSigmaXPSD): ``sigmaX_avg/_std/_max/_min`` [nrot, nA], ``sigmaX_PSD``
+    [nrot, nA, nw] with psd, ``sigmaX_DEL`` [nrot, nA] with m, and ``sigmaX_hot`` (``stress_hot``); with weights (and m) the
+    lifetime ``sigmaX_DEL`` and ``sigmaX_hot`` in the result's ``fatigue``.  Without it nothing changes."""
     from .packer import pack_case_trains
     _no_general_ops(turbine_constants)
     opts = None if fatigue is None else fatigue_options(fatigue)
+    sopts = _general_stress_options(stress, [channels])
     table, owner, first = pack_case_trains(cases)
     q = bool(qtf)
     res = general_solve_dynamics(P, M, B, Cm, CaseTable(table, ops=_train_ops(ops, owner, len(cases))), n_iter=n_iter, tol=tol,
                                  xi_start=xi_start, fd=fd, qtf=qtf, F_2nd=q)
-    return _general_case_results(P, res[0], res[1], owner, first, len(cases), channels, res[2:4] if q else None, rotors, opts)
+    return _general_case_results(P, res[0], res[1], owner, first, len(cases), channels, res[2:4] if q else None, rotors, opts, sopts)
 
 
-def _general_case_results(P, Xi, st, owner, first, n_cases, channels, F2nd, rotors=None, fatigue=None):
+def _general_stress_options(stress, channels):
+    """``stress=`` of the generalised-DOF analyses checked against every design's channels before anything is solved."""
+    if stress is None:
+        return None
+    o = stress_options(stress)
+    for ch in channels:
+        if ch is None:
+            raise ValueError("stress= needs channels (packer.pack_general_channels)")
+        stress_rows(ch["names"])
+    return o
+
+
+def _general_stress(opts, channels, P, Xi, owner, first, n_cases, metrics, out):
+    """general_analyze_cases' stress= on one design: the tower-base stress ring of every rotor's tower into every case's
+    metrics, the lifetime DELs and their hot spot into out['fatigue'] when weights and m are given."""
+    fa, ss = stress_rows(channels["names"])
+    R, wp, avg = np.asarray(channels["R"]), np.asarray(channels["wpow"]), np.asarray(channels["avg"])
+    rows = fa if ss is None else np.stack([fa, ss], axis=1)
+    r = stress_ring(Xi, P["w"], R[fa], None if ss is None else R[ss], opts["angles"], opts["d"], opts["t"], m=opts["m"],
+                    f_eq=opts["f_eq"], method=opts["method"], weights=opts["weights"], case_row0=np.append(first, len(owner)),
+                    psd=opts["psd"], mean=avg[rows].reshape(len(fa), -1), wpow=wp[rows].reshape(len(fa), -1), dw=float(P["dw"]))
+    for ic in range(n_cases):
+        metrics.setdefault(ic, {}).update(stress_entries(r, ic))
+    if "DEL_life" in r:
+        out.setdefault("fatigue", {}).update(sigmaX_DEL=np.array(r["DEL_life"]), sigmaX_hot=stress_hot(r))
+
+
+def _general_case_results(P, Xi, st, owner, first, n_cases, channels, F2nd, rotors=None, fatigue=None, stress=None):
     """general_analyze_cases' result for one design from its train table's Xi [nT,nDOF,nw], status [nT,4] and, with a QTF
     table, (F_2nd [nT,6,nw], F_2nd_mean [nT,6])."""
     raise_on_flags(st[first])                                           # raft_model.py:1089, :1098-1099
@@ -1526,6 +1767,8 @@ def _general_case_results(P, Xi, st, owner, first, n_cases, channels, F2nd, roto
         out["Fhydro_2nd_mean"] = [F2m[owner == ic] for ic in range(n_cases)]
     if fatigue is not None:
         _general_fatigue(fatigue, channels, P, Xi, owner, first, n_cases, metrics, out)
+    if stress is not None:
+        _general_stress(stress, channels, P, Xi, owner, first, n_cases, metrics, out)
     return out
 
 
@@ -1822,6 +2065,14 @@ class GeneralBatchSession:
         return _fatigue(_session_buffers(self), self.Xi, self.keep["w"], m, R, wpow, coef, case_row0, f_eq, method, weights, life,
                         moments, tile_w)
 
+    def stress_ring(self, fa, ss, angles=None, d=10.0, t=0.083, m=None, f_eq=1.0, method="dirlik", weights=None, case_row0=None,
+                    col0=None, psd=False, mean=None, wpow=None, tile_w=0):
+        """Tower-base axial stress around the circumference of the last ``solve()`` (raftk_stress_ring_dev on the resident Xi [nD, nT, nDOF, nw], one unit per design):
+        ``fa`` / ``ss`` the fore-aft / side-side rows (MbaseY / MbaseX of ``packer.pack_general_channels``), [n_rings, nDOF] for every design or [nD, n_rings, nDOF]; the other
+        arguments as ``stress_ring``.  -> dict of torch tensors as ``stress_ring`` (std [nD, nC, n_rings, nA], ...)."""
+        return _stress_ring(_session_buffers(self), self.Xi, self.keep["w"], fa, ss, angles, d, t, m, f_eq, method, weights, case_row0,
+                            col0, psd, mean, wpow, self.dw, tile_w)
+
 
 def _no_general_ops(turbine_constants):
     if turbine_constants is not None:
@@ -1841,14 +2092,14 @@ def _train_ops(ops, owner, n_cases):
 
 
 def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.01, xi_start=0.0, qtf=None, rotors=None,
-                                turbine_constants=None, ops=None, fatigue=None):
+                                turbine_constants=None, ops=None, fatigue=None, stress=None):
     """``general_analyze_cases`` for every design of a batch in one solve: ``designs`` a list of per-design inputs (or a
     ``GeneralBatch`` built from them), ``cases`` a list of case dicts run by every design, ``channels`` None or one
     ``packer.pack_general_channels`` dict per design, ``rotors`` None or one ``packer.pack_rotor_outputs`` dict per design
     -> a list with, for each design, what ``general_analyze_cases`` returns for that design alone.  ``ops``: one operating
     point per case, tables per design [nD, n_op, n_fd, n_fd, nw] or shared [n_op, n_fd, n_fd, nw]
     (``packer.pack_general_operating_points``).  ``turbine_constants``: NotImplementedError, as for ``general_analyze_cases``.
-    ``fatigue``: as for ``general_analyze_cases``, every design with the same exponents."""
+    ``fatigue``, ``stress``: as for ``general_analyze_cases``, every design with the same options."""
     from .packer import pack_case_trains
     _no_general_ops(turbine_constants)
     opts = None if fatigue is None else fatigue_options(fatigue)
@@ -1857,13 +2108,14 @@ def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.
         raise ValueError("channels: one entry per design (%d), got %d" % (bt.n_designs, len(channels)))
     if rotors is not None and len(rotors) != bt.n_designs:
         raise ValueError("rotors: one entry per design (%d), got %d" % (bt.n_designs, len(rotors)))
+    sopts = None if stress is None else _general_stress_options(stress, [None] * bt.n_designs if channels is None else channels)
     table, owner, first = pack_case_trains(cases)
     q = bt.qtf is not None
     res = general_solve_dynamics_batch(bt, CaseTable(table, ops=_train_ops(ops, owner, len(cases))), n_iter=n_iter, tol=tol,
                                        xi_start=xi_start, F_2nd=q)
     P = dict(w=bt.arrays["w"], dw=bt.dw)
     return [_general_case_results(P, res[0][d], res[1][d], owner, first, len(cases), None if channels is None else channels[d],
-                                  (res[2][d], res[3][d]) if q else None, None if rotors is None else rotors[d], opts)
+                                  (res[2][d], res[3][d]) if q else None, None if rotors is None else rotors[d], opts, sopts)
             for d in range(bt.n_designs)]
 
 
@@ -2267,6 +2519,17 @@ class DeviceSession:
         xi = self._response("fatigue", farm, n_fowt)
         return _fatigue(_session_buffers(self), xi, self.dt["w"], m, R, wpow, coef, case_row0, f_eq, method, weights, life, moments,
                         tile_w)
+
+    def stress_ring(self, fa, ss, angles=None, d=10.0, t=0.083, m=None, f_eq=1.0, method="dirlik", weights=None, case_row0=None,
+                    col0=None, psd=False, mean=None, wpow=None, tile_w=0, farm=False, n_fowt=None):
+        """Enqueue the tower-base axial stress around the circumference on a resident response (raftk_stress_ring_dev; no host
+        round trip).  ``farm=False``: the last ``solve``'s Xi [nD, nC, 6, nw], one unit per design (e.g. ``fa`` the Mbase
+        coefficients of ``packer.pack_turbine_channels``, ``ss`` None); ``farm=True``: the Xi_sys of the LAST ``farm_response``
+        of the form ``n_fowt`` names, one unit per farm, FOWT i's tower at ``col0`` = 6 i.  The other arguments as
+        ``stress_ring``.  -> dict of torch tensors as ``stress_ring``, without the unit axis for one farm."""
+        xi = self._response("stress_ring", farm, n_fowt)
+        return _stress_ring(_session_buffers(self), xi, self.dt["w"], fa, ss, angles, d, t, m, f_eq, method, weights, case_row0, col0,
+                            psd, mean, wpow, self.batch.dw, tile_w)
 
     def eigen(self, A0=None, yawstiff=0.0, sort="dof", modes=True):
         """Natural frequencies and mode shapes of every design on the device, on torch's current stream (async):
