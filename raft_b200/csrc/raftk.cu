@@ -2545,12 +2545,46 @@ extern "C" int raftk_channel_stats_host(int32_t n_designs, int32_t n_cases, int3
     return S.finish();
 }
 
-// k_general_channel_stats applies w^0, w^1 or w^2; wpow: a host copy
-static int validate_wpow(int32_t n_ch, const int32_t *wpow)
+// ---- argument checks shared by the post-solve reductions -------------------------------------------------------------------
+// `who` is the entry's prefix of its refusals ("fatigue", "stress ring", "rotor-stats", ...).
+
+// The channel kernels apply w^0, w^1 or w^2; wpow: a host copy of n powers, or NULL (every power 0)
+static int check_wpow(const char *who, const int32_t *wpow, int32_t n)
 {
-    for (int32_t t = 0; t < n_ch; t++)
-        if (wpow[t] < 0 || wpow[t] > 2) return set_err(RAFTK_EINVAL, "general channel-stats: wpow must be 0, 1 or 2");
-    return 0;
+    for (int32_t t = 0; wpow && t < n; t++)
+        if (wpow[t] < 0 || wpow[t] > 2) return set_err(RAFTK_EINVAL, "%s: wpow must be 0, 1 or 2", who);
+    return RAFTK_OK;
+}
+
+// case c reads rows case_row0[c] .. case_row0[c + 1] - 1 of every unit
+static int check_case_rows(const char *who, const int32_t *case_row0, int32_t n_cases, int32_t n_rows)
+{
+    if (case_row0[0] != 0 || case_row0[n_cases] != n_rows)
+        return set_err(RAFTK_EINVAL, "%s: case_row0 must start at 0 and end at n_rows", who);
+    for (int32_t c = 0; c < n_cases; c++)
+        if (case_row0[c + 1] <= case_row0[c]) return set_err(RAFTK_EINVAL, "%s: every case needs at least one row", who);
+    return RAFTK_OK;
+}
+
+// the case probabilities of a lifetime sum, or NULL (every case 1)
+static int check_weights(const char *who, const double *weights, int32_t n_cases)
+{
+    if (!weights) return RAFTK_OK;
+    double s = 0.0;
+    for (int32_t c = 0; c < n_cases; c++) {
+        if (!(std::isfinite(weights[c]) && weights[c] >= 0.0)) return set_err(RAFTK_EINVAL, "%s: weights must be finite and >= 0", who);
+        s += weights[c];
+    }
+    if (!(s > 0.0)) return set_err(RAFTK_EINVAL, "%s: the weights must not all be 0", who);
+    return RAFTK_OK;
+}
+
+// a _dev entry's workspace: at least `need` bytes (what `sizer` returns), 32-byte aligned for the kernels' double4 reads
+static int check_workspace(const char *who, const char *sizer, const void *ws, size_t bytes, size_t need)
+{
+    if (!ws || bytes < need) return set_err(RAFTK_EINVAL, "%s: the workspace is too small (%s)", who, sizer);
+    if ((uintptr_t)ws % 32) return set_err(RAFTK_EINVAL, "%s: the workspace must be 32-byte aligned", who);
+    return RAFTK_OK;
 }
 
 static int launch_general_channel_stats(int32_t n_units, int32_t n_dof, int32_t n_ch, int32_t nw, double dw, const double *w, const double *R,
@@ -2575,7 +2609,7 @@ extern "C" int raftk_general_channel_stats_dev(int32_t n_units, int32_t n_dof, i
     std::vector<int32_t> p(n_ch);
     CUDA_TRY(cudaMemcpyAsync(p.data(), wpow, p.size() * 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
-    if (int rc = validate_wpow(n_ch, p.data())) return rc;
+    if (int rc = check_wpow("general channel-stats", p.data(), n_ch)) return rc;
     return launch_general_channel_stats(n_units, n_dof, n_ch, nw, dw, w, R, wpow, Xi, sd, psd, amp, st);
 }
 
@@ -2584,7 +2618,7 @@ extern "C" int raftk_general_channel_stats_host(int32_t n_units, int32_t n_dof, 
 {
     if (n_units <= 0 || n_dof <= 0 || n_ch <= 0 || nw <= 0 || !w || !R || !wpow || !Xi || !sd || !(dw > 0.0))
         return set_err(RAFTK_EINVAL, "bad general channel-stats arguments");
-    if (int rc = validate_wpow(n_ch, wpow)) return rc;
+    if (int rc = check_wpow("general channel-stats", wpow, n_ch)) return rc;
     const size_t rows = (size_t)n_units * n_ch;
     Staging S("raftk_general_channel_stats_host");
     const double *dW, *dR, *dXi;
@@ -2613,11 +2647,8 @@ static int farm_ch_check(int32_t n_farms, int32_t n_rows, int32_t n_dof, int32_t
     if (ch->R_shared != 0 && ch->R_shared != 1) return set_err(RAFTK_EINVAL, "farm channel-stats: R_shared must be 0 or 1");
     if (!ch->R || !Xi_sys || !ch->std) return set_err(RAFTK_EINVAL, "farm channel-stats: R, Xi_sys and std are required");
     if (!(ch->dw > 0.0)) return set_err(RAFTK_EINVAL, "farm channel-stats: dw must be > 0");
-    bool powers = false;
-    for (int32_t t = 0; ch->wpow && t < ch->n_ch; t++) {
-        if (ch->wpow[t] < 0 || ch->wpow[t] > 2) return set_err(RAFTK_EINVAL, "farm channel-stats: wpow must be 0, 1 or 2");
-        powers = powers || ch->wpow[t] != 0;
-    }
+    if (int rc = check_wpow("farm channel-stats", ch->wpow, ch->n_ch)) return rc;
+    const bool powers = ch->wpow && std::any_of(ch->wpow, ch->wpow + ch->n_ch, [](int32_t p) { return p != 0; });
     if (powers && !w) return set_err(RAFTK_EINVAL, "farm channel-stats: w is required when a channel has wpow 1 or 2");
     const size_t units = (size_t)n_farms * n_rows;
     if (units * nw > 2147483647u || units * ch->n_ch > 2147483647u)
@@ -2715,10 +2746,7 @@ static int rotor_check(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t n
     for (int32_t k = 0; k < ro->n_rot; k++)
         if (ro->col0[k] < 0 || ro->col0[k] > n_dof - ro->n_r)
             return set_err(RAFTK_EINVAL, "rotor-stats: every col0 must satisfy 0 <= col0 and col0 + n_r <= n_dof");
-    if (ro->case_row0[0] != 0 || ro->case_row0[ro->n_cases] != n_rows)
-        return set_err(RAFTK_EINVAL, "rotor-stats: case_row0 must start at 0 and end at n_rows");
-    for (int32_t c = 0; c < ro->n_cases; c++)
-        if (ro->case_row0[c + 1] <= ro->case_row0[c]) return set_err(RAFTK_EINVAL, "rotor-stats: every case needs at least one row");
+    if (int rc = check_case_rows("rotor-stats", ro->case_row0, ro->n_cases, n_rows)) return rc;
     if ((size_t)n_units * ro->n_cases * ro->n_rot > 2147483647u)
         return set_err(RAFTK_EINVAL, "rotor-stats: too many (unit, case, rotor) blocks");
     return RAFTK_OK;
@@ -2775,10 +2803,103 @@ extern "C" int raftk_rotor_stats_host(int32_t n_units, int32_t n_rows, int32_t n
     return S.finish();
 }
 
+// ---- spectral moments shared by fatigue and the stress ring: channel form, bin tiles, launches ------------------------------
+// The channels of k_fatigue_moments and k_stress_moments: real rows R, one set for every unit (R_shared 1) or one per unit,
+// or complex per-bin coefficients coef, one set (RAFTK_FATIGUE_COEF_SHARED), one per unit (_UNIT) or one per (unit, row)
+// (_ROW); method: the DEL closed form
+static int check_channel_form(const char *who, const void *R, int32_t R_shared, const void *coef, int32_t coef_mode, int32_t method)
+{
+    if (!R == !coef) return set_err(RAFTK_EINVAL, "%s: give exactly one of R (real rows) and coef (complex coefficients)", who);
+    if (R && R_shared != 0 && R_shared != 1) return set_err(RAFTK_EINVAL, "%s: R_shared must be 0 or 1", who);
+    if (coef && (coef_mode < RAFTK_FATIGUE_COEF_SHARED || coef_mode > RAFTK_FATIGUE_COEF_ROW))
+        return set_err(RAFTK_EINVAL, "%s: unknown coef_mode", who);
+    if (method != RAFTK_FATIGUE_DIRLIK && method != RAFTK_FATIGUE_NARROWBAND_METHOD) return set_err(RAFTK_EINVAL, "%s: unknown method", who);
+    return RAFTK_OK;
+}
+
+// The strides of a checked channel form, `per` doubles of R (or coefficients per bin) for one unit: between two units' R, two
+// units' and two rows' coefficients (0: shared); and the doubles of R and coef that raftk_*_host stages
+struct ChannelForm { size_t r_stride, cf_ustride, cf_rstride, n_R, n_coef; };
+static ChannelForm channel_form(int32_t R_shared, const void *coef, int32_t coef_mode, size_t per, int32_t n_units, int32_t n_rows,
+                                int32_t nw)
+{
+    const size_t cf = per * nw;
+    ChannelForm f;
+    f.r_stride = R_shared ? 0 : per;
+    f.cf_ustride = coef_mode == RAFTK_FATIGUE_COEF_UNIT ? cf : (coef_mode == RAFTK_FATIGUE_COEF_ROW ? cf * n_rows : 0);
+    f.cf_rstride = coef_mode == RAFTK_FATIGUE_COEF_ROW ? cf : 0;
+    f.n_R = (R_shared ? 1 : (size_t)n_units) * per;
+    f.n_coef = coef ? (coef_mode == RAFTK_FATIGUE_COEF_SHARED ? 1 : (size_t)n_units) * (coef_mode == RAFTK_FATIGUE_COEF_ROW ? n_rows : 1) * cf * 2
+                    : 0;
+    return f;
+}
+
+static int moment_chunks(int32_t nw) { return (nw + FAT_CHUNK - 1) / FAT_CHUNK; }
+
+// Bins per CTA of the moment kernels, whole FAT_CHUNK chunks: at most what the opt-in shared memory holds (n x 16 bytes per bin)
+// and 256, fewer when the batch alone would leave SMs idle; 0 when not even one chunk fits (Xi is then read from L2).  tile_w > 0
+// caps it.
+static int moment_tile(size_t n_rows_total, int32_t n_dof, int32_t nw, int32_t tile_w)
+{
+    if (tile_w == RAFTK_FARM_TILE_L2) return 0;
+    const int round_nw = moment_chunks(nw) * FAT_CHUNK;
+    const int tmax = (int)std::min<size_t>((size_t)round_nw, smem_optin() / ((size_t)n_dof * sizeof(double2))) / FAT_CHUNK * FAT_CHUNK;
+    if (tmax < FAT_CHUNK) return 0;
+    if (tile_w > 0) return std::max(FAT_CHUNK, std::min(tmax, (int)tile_w / FAT_CHUNK * FAT_CHUNK));
+    const long long want = (2LL * sm_count() + (long long)n_rows_total - 1) / (long long)n_rows_total;   // tiles per (unit, row)
+    const int split = (int)((nw + want - 1) / want + FAT_CHUNK - 1) / FAT_CHUNK * FAT_CHUNK;
+    return std::min(std::min(tmax, 256), std::max(FAT_CHUNK, split));
+}
+
+// Sets P's bin tiling (n_chunks, tile, n_tiles) for `rows` (unit, row) pairs and launches the moment kernel k[SMEM][COEF]: the
+// Xi tile in shared memory when moment_tile gives one, else from L2.  The opt-in is per function, so each instantiation of this
+// template (one per moment kernel) keeps one SmemOptIn per shared-memory kernel.
+template <class Prm>
+static int launch_moments(void (*const (&k)[2][2])(Prm), int threads, Prm &P, size_t rows, int32_t n_dof, int32_t nw, int32_t tile_w,
+                          bool coef, cudaStream_t st)
+{
+    static SmemOptIn opt[2] = {SmemOptIn(48 * 1024), SmemOptIn(48 * 1024)};
+    const int tile = moment_tile(rows, n_dof, nw, tile_w);
+    P.n_chunks = moment_chunks(nw);
+    P.tile = tile ? tile : std::min<int32_t>(P.n_chunks * FAT_CHUNK, 256);
+    P.n_tiles = (nw + P.tile - 1) / P.tile;
+    const unsigned grid = (unsigned)(rows * P.n_tiles);
+    if (tile) {
+        const size_t smem = (size_t)n_dof * tile * sizeof(double2);
+        CUDA_TRY(opt[coef].ensure(k[1][coef], smem));
+        k[1][coef]<<<grid, threads, smem, st>>>(P);
+    } else {
+        k[0][coef]<<<grid, threads, 0, st>>>(P);
+    }
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
+// DEL_life [U, nk] from the log(p_c d_c) table wd [U, n_cases, nk] (nk channels, or (ring, angle) pairs) through
+// k_fatigue_life; column k's exponent is m[k * m_stride]
+static int launch_life(int32_t n_units, int32_t n_cases, int32_t nk, const double *weights, double f_eq, const double *m, int m_stride,
+                       const double *wd, double *DEL_life, cudaStream_t st)
+{
+    FatLifeParams L = {};
+    double W = 0.0;
+    for (int32_t c = 0; c < n_cases; c++) W += weights ? weights[c] : 1.0;
+    L.n_cases = n_cases; L.nch = nk; L.log_fw = std::log(f_eq * W); L.wd = wd; L.DEL_life = DEL_life;
+    for (int32_t k0 = 0; k0 < nk; k0 += FAT_LAUNCH_CHUNK) {
+        L.k0 = k0; L.nk = std::min<int32_t>(FAT_LAUNCH_CHUNK, nk - k0);
+        for (int j = 0; j < L.nk; j++) L.m[j] = m[(size_t)(k0 + j) * m_stride];
+        const size_t nt = (size_t)n_units * L.nk;
+        k_fatigue_life<<<(unsigned)((nt + FAT_FIN_T - 1) / FAT_FIN_T), FAT_FIN_T, 0, st>>>(L, nt);
+        g_launches++;
+        CUDA_TRY(cudaGetLastError());
+    }
+    return RAFTK_OK;
+}
+
 // ---- fatigue damage-equivalent loads (raftk_fatigue_*) --------------------------------------------------------------------
 static size_t fat_part_elems(int32_t n_units, int32_t n_rows, int32_t nw, int32_t n_ch)
 {
-    return (size_t)n_units * n_rows * ((nw + FAT_CHUNK - 1) / FAT_CHUNK) * n_ch * 4;
+    return (size_t)n_units * n_rows * moment_chunks(nw) * n_ch * 4;
 }
 
 static int fat_check(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi, const raftk_fatigue *fa)
@@ -2787,33 +2908,16 @@ static int fat_check(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw,
     if (n_units < 1 || n_rows < 1 || n_dof < 1 || nw < 1 || fa->n_cases < 1 || fa->n_ch < 1)
         return set_err(RAFTK_EINVAL, "fatigue: n_units, n_rows, n_dof, nw, n_cases and n_ch must be >= 1");
     if (fa->n_ch > RAFTK_FATIGUE_CH_MAX) return set_err_i(RAFTK_EINVAL, "fatigue: at most %d channels per call", RAFTK_FATIGUE_CH_MAX);
-    if (!fa->R == !fa->coef) return set_err(RAFTK_EINVAL, "fatigue: give exactly one of R (real rows) and coef (complex coefficients)");
-    if (fa->R && fa->R_shared != 0 && fa->R_shared != 1) return set_err(RAFTK_EINVAL, "fatigue: R_shared must be 0 or 1");
-    if (fa->coef && (fa->coef_mode < RAFTK_FATIGUE_COEF_SHARED || fa->coef_mode > RAFTK_FATIGUE_COEF_ROW))
-        return set_err(RAFTK_EINVAL, "fatigue: unknown coef_mode");
-    if (fa->method != RAFTK_FATIGUE_DIRLIK && fa->method != RAFTK_FATIGUE_NARROWBAND_METHOD)
-        return set_err(RAFTK_EINVAL, "fatigue: unknown method");
+    if (int rc = check_channel_form("fatigue", fa->R, fa->R_shared, fa->coef, fa->coef_mode, fa->method)) return rc;
     if (!w || !Xi || !fa->m || !fa->case_row0 || !fa->DEL || !fa->info)
         return set_err(RAFTK_EINVAL, "fatigue: w, Xi, m, case_row0, DEL and info are required");
-    for (int32_t t = 0; fa->R && fa->wpow && t < fa->n_ch; t++)
-        if (fa->wpow[t] < 0 || fa->wpow[t] > 2) return set_err(RAFTK_EINVAL, "fatigue: wpow must be 0, 1 or 2");
-    if (fa->case_row0[0] != 0 || fa->case_row0[fa->n_cases] != n_rows)
-        return set_err(RAFTK_EINVAL, "fatigue: case_row0 must start at 0 and end at n_rows");
-    for (int32_t c = 0; c < fa->n_cases; c++)
-        if (fa->case_row0[c + 1] <= fa->case_row0[c]) return set_err(RAFTK_EINVAL, "fatigue: every case needs at least one row");
+    if (int rc = check_wpow("fatigue", fa->R ? fa->wpow : nullptr, fa->n_ch)) return rc;
+    if (int rc = check_case_rows("fatigue", fa->case_row0, fa->n_cases, n_rows)) return rc;
     for (int32_t t = 0; t < fa->n_ch; t++)
         if (!(std::isfinite(fa->m[t]) && fa->m[t] > 0.0)) return set_err(RAFTK_EINVAL, "fatigue: every m must be finite and > 0");
     if (!(std::isfinite(fa->f_eq) && fa->f_eq > 0.0)) return set_err(RAFTK_EINVAL, "fatigue: f_eq must be finite and > 0");
-    if (fa->weights) {
-        double s = 0.0;
-        for (int32_t c = 0; c < fa->n_cases; c++) {
-            if (!(std::isfinite(fa->weights[c]) && fa->weights[c] >= 0.0)) return set_err(RAFTK_EINVAL, "fatigue: weights must be finite and >= 0");
-            s += fa->weights[c];
-        }
-        if (!(s > 0.0)) return set_err(RAFTK_EINVAL, "fatigue: the weights must not all be 0");
-    }
-    const size_t rows = (size_t)n_units * n_rows;
-    if (rows * ((nw + FAT_CHUNK - 1) / FAT_CHUNK) > 2147483647u || (size_t)n_units * fa->n_ch > 2147483647u)
+    if (int rc = check_weights("fatigue", fa->weights, fa->n_cases)) return rc;
+    if ((size_t)n_units * n_rows * moment_chunks(nw) > 2147483647u || (size_t)n_units * fa->n_ch > 2147483647u)
         return set_err(RAFTK_EINVAL, "fatigue: too many (unit, row, bin tile) blocks");
     return RAFTK_OK;
 }
@@ -2821,20 +2925,6 @@ static int fat_check(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw,
 static size_t fat_ws(int32_t n_units, int32_t n_rows, int32_t nw, const raftk_fatigue *fa)
 {
     return (fat_part_elems(n_units, n_rows, nw, fa->n_ch) + (fa->DEL_life ? (size_t)n_units * fa->n_cases * fa->n_ch : 0)) * sizeof(double);
-}
-
-// Bins per CTA, whole FAT_CHUNK chunks: at most what the opt-in shared memory holds (n x 16 bytes per bin) and 256, fewer when
-// the batch alone would leave SMs idle; 0 when not even one chunk fits (Xi is then read from L2).  tile_w > 0 caps it.
-static int fat_tile(size_t n_rows_total, int32_t n_dof, int32_t nw, int32_t tile_w)
-{
-    if (tile_w == RAFTK_FARM_TILE_L2) return 0;
-    const int round_nw = (nw + FAT_CHUNK - 1) / FAT_CHUNK * FAT_CHUNK;
-    const int tmax = (int)std::min<size_t>((size_t)round_nw, smem_optin() / ((size_t)n_dof * sizeof(double2))) / FAT_CHUNK * FAT_CHUNK;
-    if (tmax < FAT_CHUNK) return 0;
-    if (tile_w > 0) return std::max(FAT_CHUNK, std::min(tmax, (int)tile_w / FAT_CHUNK * FAT_CHUNK));
-    const long long want = (2LL * sm_count() + (long long)n_rows_total - 1) / (long long)n_rows_total;   // tiles per (unit, row)
-    const int split = (int)((nw + want - 1) / want + FAT_CHUNK - 1) / FAT_CHUNK * FAT_CHUNK;
-    return std::min(std::min(tmax, 256), std::max(FAT_CHUNK, split));
 }
 
 extern "C" size_t raftk_fatigue_workspace_bytes(int32_t n_units, int32_t n_rows, int32_t nw, const raftk_fatigue *fa)
@@ -2847,45 +2937,21 @@ extern "C" int raftk_fatigue_dev(int32_t n_units, int32_t n_rows, int32_t n_dof,
                                  const raftk_fatigue *fa, void *workspace, size_t workspace_bytes, void *stream)
 {
     if (int rc = fat_check(n_units, n_rows, n_dof, nw, w, Xi, fa)) return rc;
-    if (!workspace || workspace_bytes < fat_ws(n_units, n_rows, nw, fa))
-        return set_err(RAFTK_EINVAL, "fatigue: the workspace is too small (raftk_fatigue_workspace_bytes)");
-    if ((uintptr_t)workspace % 32) return set_err(RAFTK_EINVAL, "fatigue: the workspace must be 32-byte aligned");
+    if (int rc = check_workspace("fatigue", "raftk_fatigue_workspace_bytes", workspace, workspace_bytes, fat_ws(n_units, n_rows, nw, fa)))
+        return rc;
     const cudaStream_t st = (cudaStream_t)stream;
-    const size_t rows = (size_t)n_units * n_rows;
     double *part = static_cast<double *>(workspace);
     double *wd = fa->DEL_life ? part + fat_part_elems(n_units, n_rows, nw, fa->n_ch) : nullptr;
+    const ChannelForm cf = channel_form(fa->R_shared, fa->coef, fa->coef_mode, (size_t)fa->n_ch * n_dof, n_units, n_rows, nw);
     FatMomParams P = {};
     P.n = n_dof; P.nch = fa->n_ch; P.nw = nw; P.n_rows = n_rows;
-    P.n_chunks = (nw + FAT_CHUNK - 1) / FAT_CHUNK;
     P.w = w; P.R = fa->R; P.Xi = reinterpret_cast<const double2 *>(Xi); P.part = part;
     P.coef = reinterpret_cast<const double2 *>(fa->coef);
-    const size_t cf = (size_t)fa->n_ch * n_dof * nw;
-    P.r_stride = fa->R_shared ? 0 : (size_t)fa->n_ch * n_dof;
-    P.cf_ustride = fa->coef_mode == RAFTK_FATIGUE_COEF_UNIT ? cf : (fa->coef_mode == RAFTK_FATIGUE_COEF_ROW ? cf * n_rows : 0);
-    P.cf_rstride = fa->coef_mode == RAFTK_FATIGUE_COEF_ROW ? cf : 0;
+    P.r_stride = cf.r_stride; P.cf_ustride = cf.cf_ustride; P.cf_rstride = cf.cf_rstride;
     for (int32_t t = 0; fa->R && fa->wpow && t < fa->n_ch; t++) P.wbits[t >> 4] |= (unsigned)fa->wpow[t] << ((t & 15) * 2);
-    const int tile = fat_tile(rows, n_dof, nw, fa->tile_w);
-    P.tile = tile ? tile : std::min<int32_t>((nw + FAT_CHUNK - 1) / FAT_CHUNK * FAT_CHUNK, 256);
-    P.n_tiles = (nw + P.tile - 1) / P.tile;
-    const size_t grid = rows * P.n_tiles;
-    const bool coef = fa->coef != nullptr;
-    if (tile) {
-        const size_t smem = (size_t)n_dof * tile * sizeof(double2);
-        static SmemOptIn opt_r(48 * 1024), opt_c(48 * 1024);
-        if (coef) {
-            CUDA_TRY(opt_c.ensure(k_fatigue_moments<true, true>, smem));
-            k_fatigue_moments<true, true><<<(unsigned)grid, FAT_T, smem, st>>>(P);
-        } else {
-            CUDA_TRY(opt_r.ensure(k_fatigue_moments<true, false>, smem));
-            k_fatigue_moments<true, false><<<(unsigned)grid, FAT_T, smem, st>>>(P);
-        }
-    } else if (coef) {
-        k_fatigue_moments<false, true><<<(unsigned)grid, FAT_T, 0, st>>>(P);
-    } else {
-        k_fatigue_moments<false, false><<<(unsigned)grid, FAT_T, 0, st>>>(P);
-    }
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
+    static void (*const mom[2][2])(FatMomParams) = {{k_fatigue_moments<false, false>, k_fatigue_moments<false, true>},
+                                                    {k_fatigue_moments<true, false>, k_fatigue_moments<true, true>}};
+    if (int rc = launch_moments(mom, FAT_T, P, (size_t)n_units * n_rows, n_dof, nw, fa->tile_w, fa->coef != nullptr, st)) return rc;
     // chunks of cases and channels only bound the launch parameters: every thread computes the same thing in any chunk
     FatFinParams F = {};
     F.n_rows = n_rows; F.n_cases = fa->n_cases; F.nch = fa->n_ch; F.n_chunks = P.n_chunks; F.method = fa->method;
@@ -2903,21 +2969,7 @@ extern "C" int raftk_fatigue_dev(int32_t n_units, int32_t n_rows, int32_t n_dof,
             CUDA_TRY(cudaGetLastError());
         }
     }
-    if (fa->DEL_life) {
-        FatLifeParams L = {};
-        double W = 0.0;
-        for (int32_t c = 0; c < fa->n_cases; c++) W += fa->weights ? fa->weights[c] : 1.0;
-        L.n_cases = fa->n_cases; L.nch = fa->n_ch; L.log_fw = std::log(fa->f_eq * W); L.wd = wd; L.DEL_life = fa->DEL_life;
-        for (int32_t k0 = 0; k0 < fa->n_ch; k0 += FAT_LAUNCH_CHUNK) {
-            L.k0 = k0; L.nk = std::min<int32_t>(FAT_LAUNCH_CHUNK, fa->n_ch - k0);
-            for (int j = 0; j < L.nk; j++) L.m[j] = fa->m[k0 + j];
-            const size_t nt = (size_t)n_units * L.nk;
-            k_fatigue_life<<<(unsigned)((nt + FAT_FIN_T - 1) / FAT_FIN_T), FAT_FIN_T, 0, st>>>(L, nt);
-            g_launches++;
-            CUDA_TRY(cudaGetLastError());
-        }
-    }
-    return RAFTK_OK;
+    return fa->DEL_life ? launch_life(n_units, fa->n_cases, fa->n_ch, fa->weights, fa->f_eq, fa->m, 1, wd, fa->DEL_life, st) : RAFTK_OK;
 }
 
 extern "C" int raftk_fatigue_host(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi,
@@ -2926,16 +2978,13 @@ extern "C" int raftk_fatigue_host(int32_t n_units, int32_t n_rows, int32_t n_dof
     if (int rc = fat_check(n_units, n_rows, n_dof, nw, w, Xi, fa)) return rc;
     const size_t out = (size_t)n_units * fa->n_cases * fa->n_ch, nch = fa->n_ch;
     const size_t wb = fat_ws(n_units, n_rows, nw, fa);
-    size_t n_coef = 0;
-    if (fa->coef)
-        n_coef = (fa->coef_mode == RAFTK_FATIGUE_COEF_SHARED ? 1 : (size_t)n_units) * (fa->coef_mode == RAFTK_FATIGUE_COEF_ROW ? n_rows : 1)
-                 * nch * n_dof * nw * 2;
+    const ChannelForm cf = channel_form(fa->R_shared, fa->coef, fa->coef_mode, nch * n_dof, n_units, n_rows, nw);
     raftk_fatigue d = *fa;
     const double *dW, *dXi;
     char *ws;
     Staging S("raftk_fatigue_host");
     S.in(dW, w, nw); S.in(dXi, Xi, (size_t)n_units * n_rows * n_dof * nw * 2);
-    S.in(d.R, fa->R, (fa->R_shared ? 1 : (size_t)n_units) * nch * n_dof); S.in(d.coef, fa->coef, n_coef);
+    S.in(d.R, fa->R, cf.n_R); S.in(d.coef, fa->coef, cf.n_coef);
     S.out(d.moments, fa->moments ? out * 4 : 0, fa->moments); S.out(d.DEL, out, fa->DEL); S.out(d.info, out, fa->info);
     S.out(d.DEL_life, fa->DEL_life ? (size_t)n_units * nch : 0, fa->DEL_life);
     S.buf(ws, wb);
@@ -2947,7 +2996,7 @@ extern "C" int raftk_fatigue_host(int32_t n_units, int32_t n_rows, int32_t n_dof
 // ---- tower-base axial stress around the circumference (raftk_stress_ring_*) -------------------------------------------------
 static size_t str_part_elems(int32_t n_units, int32_t n_rows, int32_t nw, int32_t n_rings)
 {
-    return (size_t)n_units * n_rows * ((nw + STR_CHUNK_BINS - 1) / STR_CHUNK_BINS) * n_rings * STR_NS;
+    return (size_t)n_units * n_rows * moment_chunks(nw) * n_rings * STR_NS;
 }
 
 static size_t str_ws(int32_t n_units, int32_t n_rows, int32_t nw, const raftk_stress_ring *sr)
@@ -2967,16 +3016,10 @@ static int str_check(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw,
     if (sr->n_r > n_dof) return set_err(RAFTK_EINVAL, "stress ring: n_r must not exceed n_dof");
     for (int32_t k = 0; sr->col0 && k < sr->n_rings; k++)
         if (sr->col0[k] < 0 || sr->col0[k] > n_dof - sr->n_r) return set_err_i(RAFTK_EINVAL, "stress ring: col0 of ring %d outside [0, n_dof - n_r]", k);
-    if (!sr->R == !sr->coef) return set_err(RAFTK_EINVAL, "stress ring: give exactly one of R (real rows) and coef (complex coefficients)");
-    if (sr->R && sr->R_shared != 0 && sr->R_shared != 1) return set_err(RAFTK_EINVAL, "stress ring: R_shared must be 0 or 1");
-    if (sr->coef && (sr->coef_mode < RAFTK_FATIGUE_COEF_SHARED || sr->coef_mode > RAFTK_FATIGUE_COEF_ROW))
-        return set_err(RAFTK_EINVAL, "stress ring: unknown coef_mode");
-    if (sr->method != RAFTK_FATIGUE_DIRLIK && sr->method != RAFTK_FATIGUE_NARROWBAND_METHOD)
-        return set_err(RAFTK_EINVAL, "stress ring: unknown method");
+    if (int rc = check_channel_form("stress ring", sr->R, sr->R_shared, sr->coef, sr->coef_mode, sr->method)) return rc;
     if (!w || !Xi || !sr->angles || !sr->case_row0 || !sr->std || !sr->avg || !sr->max || !sr->min)
         return set_err(RAFTK_EINVAL, "stress ring: w, Xi, angles, case_row0, std, avg, max and min are required");
-    for (int32_t t = 0; sr->R && sr->wpow && t < sr->n_rings * sr->n_ch; t++)
-        if (sr->wpow[t] < 0 || sr->wpow[t] > 2) return set_err(RAFTK_EINVAL, "stress ring: wpow must be 0, 1 or 2");
+    if (int rc = check_wpow("stress ring", sr->R ? sr->wpow : nullptr, sr->n_rings * sr->n_ch)) return rc;
     for (int32_t a = 0; a < sr->n_angles; a++)
         if (!std::isfinite(sr->angles[a])) return set_err(RAFTK_EINVAL, "stress ring: every angle must be finite");
     if (!(std::isfinite(sr->d) && sr->d > 0.0) || !(std::isfinite(sr->t) && sr->t > 0.0))
@@ -2987,20 +3030,9 @@ static int str_check(int32_t n_units, int32_t n_rows, int32_t n_dof, int32_t nw,
     if (sr->hot_life && !sr->DEL_life) return set_err(RAFTK_EINVAL, "stress ring: hot_life needs DEL_life");
     if (sr->psd && !(std::isfinite(sr->dw) && sr->dw > 0.0)) return set_err(RAFTK_EINVAL, "stress ring: psd needs a finite dw > 0");
     if (!(std::isfinite(sr->f_eq) && sr->f_eq > 0.0)) return set_err(RAFTK_EINVAL, "stress ring: f_eq must be finite and > 0");
-    if (sr->case_row0[0] != 0 || sr->case_row0[sr->n_cases] != n_rows)
-        return set_err(RAFTK_EINVAL, "stress ring: case_row0 must start at 0 and end at n_rows");
-    for (int32_t c = 0; c < sr->n_cases; c++)
-        if (sr->case_row0[c + 1] <= sr->case_row0[c]) return set_err(RAFTK_EINVAL, "stress ring: every case needs at least one row");
-    if (sr->weights) {
-        double s = 0.0;
-        for (int32_t c = 0; c < sr->n_cases; c++) {
-            if (!(std::isfinite(sr->weights[c]) && sr->weights[c] >= 0.0)) return set_err(RAFTK_EINVAL, "stress ring: weights must be finite and >= 0");
-            s += sr->weights[c];
-        }
-        if (!(s > 0.0)) return set_err(RAFTK_EINVAL, "stress ring: the weights must not all be 0");
-    }
-    const size_t rows = (size_t)n_units * n_rows;
-    if (rows * ((nw + STR_CHUNK_BINS - 1) / STR_CHUNK_BINS) > 2147483647u || (size_t)n_units * sr->n_rings * sr->n_angles > 2147483647u)
+    if (int rc = check_case_rows("stress ring", sr->case_row0, sr->n_cases, n_rows)) return rc;
+    if (int rc = check_weights("stress ring", sr->weights, sr->n_cases)) return rc;
+    if ((size_t)n_units * n_rows * moment_chunks(nw) > 2147483647u || (size_t)n_units * sr->n_rings * sr->n_angles > 2147483647u)
         return set_err(RAFTK_EINVAL, "stress ring: too many (unit, row, bin tile) blocks");
     return RAFTK_OK;
 }
@@ -3015,22 +3047,17 @@ extern "C" int raftk_stress_ring_dev(int32_t n_units, int32_t n_rows, int32_t n_
                                      const raftk_stress_ring *sr, void *workspace, size_t workspace_bytes, void *stream)
 {
     if (int rc = str_check(n_units, n_rows, n_dof, nw, w, Xi, sr)) return rc;
-    if (!workspace || workspace_bytes < str_ws(n_units, n_rows, nw, sr))
-        return set_err(RAFTK_EINVAL, "stress ring: the workspace is too small (raftk_stress_ring_workspace_bytes)");
-    if ((uintptr_t)workspace % 32) return set_err(RAFTK_EINVAL, "stress ring: the workspace must be 32-byte aligned");
+    if (int rc = check_workspace("stress ring", "raftk_stress_ring_workspace_bytes", workspace, workspace_bytes, str_ws(n_units, n_rows, nw, sr)))
+        return rc;
     const cudaStream_t st = (cudaStream_t)stream;
-    const size_t rows = (size_t)n_units * n_rows;
     double *part = static_cast<double *>(workspace);
     double *wd = sr->DEL_life ? part + str_part_elems(n_units, n_rows, nw, sr->n_rings) : nullptr;
+    const ChannelForm cf = channel_form(sr->R_shared, sr->coef, sr->coef_mode, (size_t)sr->n_rings * sr->n_ch * sr->n_r, n_units, n_rows, nw);
     StrParams P = {};
     P.n = n_dof; P.n_r = sr->n_r; P.nw = nw; P.n_rows = n_rows; P.n_rings = sr->n_rings; P.n_ch = sr->n_ch;
-    P.n_chunks = (nw + STR_CHUNK_BINS - 1) / STR_CHUNK_BINS;
     P.w = w; P.R = sr->R; P.Xi = reinterpret_cast<const double2 *>(Xi); P.part = part;
     P.coef = reinterpret_cast<const double2 *>(sr->coef);
-    const size_t cf = (size_t)sr->n_rings * sr->n_ch * sr->n_r * nw;
-    P.r_stride = sr->R_shared ? 0 : (size_t)sr->n_rings * sr->n_ch * sr->n_r;
-    P.cf_ustride = sr->coef_mode == RAFTK_FATIGUE_COEF_UNIT ? cf : (sr->coef_mode == RAFTK_FATIGUE_COEF_ROW ? cf * n_rows : 0);
-    P.cf_rstride = sr->coef_mode == RAFTK_FATIGUE_COEF_ROW ? cf : 0;
+    P.r_stride = cf.r_stride; P.cf_ustride = cf.cf_ustride; P.cf_rstride = cf.cf_rstride;
     for (int32_t k = 0; k < sr->n_rings; k++) P.col0[k] = sr->col0 ? sr->col0[k] : 0;
     for (int32_t t = 0; sr->R && sr->wpow && t < sr->n_rings * sr->n_ch; t++) {
         const int k = t / sr->n_ch, j = t - k * sr->n_ch;
@@ -3043,28 +3070,10 @@ extern "C" int raftk_stress_ring_dev(int32_t n_units, int32_t n_rows, int32_t n_
     P.std = sr->std; P.avg = sr->avg; P.mx = sr->max; P.mn = sr->min; P.DEL = sr->DEL; P.info = sr->info; P.wd = wd;
     P.psd = sr->psd;
     for (int32_t a = 0; a < sr->n_angles; a++) P.angle[a] = sr->angles[a];
-    const int tile = fat_tile(rows, n_dof, nw, sr->tile_w);
-    P.tile = tile ? tile : std::min<int32_t>((nw + STR_CHUNK_BINS - 1) / STR_CHUNK_BINS * STR_CHUNK_BINS, 256);
-    P.n_tiles = (nw + P.tile - 1) / P.tile;
-    const size_t grid = rows * P.n_tiles;
     const bool coef = sr->coef != nullptr;
-    if (tile) {
-        const size_t smem = (size_t)n_dof * tile * sizeof(double2);
-        static SmemOptIn opt_r(48 * 1024), opt_c(48 * 1024);
-        if (coef) {
-            CUDA_TRY(opt_c.ensure(k_stress_moments<true, true>, smem));
-            k_stress_moments<true, true><<<(unsigned)grid, STR_T, smem, st>>>(P);
-        } else {
-            CUDA_TRY(opt_r.ensure(k_stress_moments<true, false>, smem));
-            k_stress_moments<true, false><<<(unsigned)grid, STR_T, smem, st>>>(P);
-        }
-    } else if (coef) {
-        k_stress_moments<false, true><<<(unsigned)grid, STR_T, 0, st>>>(P);
-    } else {
-        k_stress_moments<false, false><<<(unsigned)grid, STR_T, 0, st>>>(P);
-    }
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
+    static void (*const mom[2][2])(StrParams) = {{k_stress_moments<false, false>, k_stress_moments<false, true>},
+                                                 {k_stress_moments<true, false>, k_stress_moments<true, true>}};
+    if (int rc = launch_moments(mom, STR_T, P, (size_t)n_units * n_rows, n_dof, nw, sr->tile_w, coef, st)) return rc;
     // chunks of cases only bound the launch parameters: every thread computes the same thing in any chunk
     for (int32_t c0 = 0; c0 < sr->n_cases; c0 += STR_LAUNCH_CASES) {
         P.c0 = c0; P.nc = std::min<int32_t>(STR_LAUNCH_CASES, sr->n_cases - c0);
@@ -3092,19 +3101,8 @@ extern "C" int raftk_stress_ring_dev(int32_t n_units, int32_t n_rows, int32_t n_
     }
     if (sr->DEL_life) {
         // per (ring, angle) the lifetime sum of k_fatigue_life, the (ring, angle) pairs taking the place of its channels
-        FatLifeParams L = {};
-        double W = 0.0;
-        for (int32_t c = 0; c < sr->n_cases; c++) W += sr->weights ? sr->weights[c] : 1.0;
-        const int32_t nk = sr->n_rings * sr->n_angles;
-        L.n_cases = sr->n_cases; L.nch = nk; L.log_fw = std::log(sr->f_eq * W); L.wd = wd; L.DEL_life = sr->DEL_life;
-        for (int j = 0; j < FAT_LAUNCH_CHUNK; j++) L.m[j] = sr->m;
-        for (int32_t k0 = 0; k0 < nk; k0 += FAT_LAUNCH_CHUNK) {
-            L.k0 = k0; L.nk = std::min<int32_t>(FAT_LAUNCH_CHUNK, nk - k0);
-            const size_t nt = (size_t)n_units * L.nk;
-            k_fatigue_life<<<(unsigned)((nt + FAT_FIN_T - 1) / FAT_FIN_T), FAT_FIN_T, 0, st>>>(L, nt);
-            g_launches++;
-            CUDA_TRY(cudaGetLastError());
-        }
+        if (int rc = launch_life(n_units, sr->n_cases, sr->n_rings * sr->n_angles, sr->weights, sr->f_eq, &sr->m, 0, wd, sr->DEL_life, st))
+            return rc;
         if (sr->hot_life) {
             P.hot = sr->hot_life;
             const size_t nh = (size_t)n_units * sr->n_rings;
@@ -3122,18 +3120,14 @@ extern "C" int raftk_stress_ring_host(int32_t n_units, int32_t n_rows, int32_t n
     if (int rc = str_check(n_units, n_rows, n_dof, nw, w, Xi, sr)) return rc;
     const size_t ring = (size_t)sr->n_rings, na = sr->n_angles;
     const size_t out = (size_t)n_units * sr->n_cases * ring * na, ucr = (size_t)n_units * sr->n_cases * ring;
-    const size_t per = ring * sr->n_ch * sr->n_r;
     const size_t wb = str_ws(n_units, n_rows, nw, sr);
-    size_t n_coef = 0;
-    if (sr->coef)
-        n_coef = (sr->coef_mode == RAFTK_FATIGUE_COEF_SHARED ? 1 : (size_t)n_units) * (sr->coef_mode == RAFTK_FATIGUE_COEF_ROW ? n_rows : 1)
-                 * per * nw * 2;
+    const ChannelForm cf = channel_form(sr->R_shared, sr->coef, sr->coef_mode, ring * sr->n_ch * sr->n_r, n_units, n_rows, nw);
     raftk_stress_ring d = *sr;
     const double *dW, *dXi;
     char *ws;
     Staging S("raftk_stress_ring_host");
     S.in(dW, w, nw); S.in(dXi, Xi, (size_t)n_units * n_rows * n_dof * nw * 2);
-    S.in(d.R, sr->R, (sr->R_shared ? 1 : (size_t)n_units) * per); S.in(d.coef, sr->coef, n_coef);
+    S.in(d.R, sr->R, cf.n_R); S.in(d.coef, sr->coef, cf.n_coef);
     S.in(d.mean, sr->mean, ucr * sr->n_ch);
     S.out(d.std, out, sr->std); S.out(d.avg, out, sr->avg); S.out(d.max, out, sr->max); S.out(d.min, out, sr->min);
     S.out(d.DEL, sr->DEL ? out : 0, sr->DEL); S.out(d.info, sr->info ? out : 0, sr->info);

@@ -42,13 +42,7 @@ __global__ void __launch_bounds__(FAT_T) k_fatigue_moments(const __grid_constant
     const size_t u = ur / (size_t)P.n_rows, r = ur - u * P.n_rows;
     const int i0 = t * P.tile, tw = min(P.tile, P.nw - i0);
     const double2 *x = P.Xi + ur * (size_t)P.n * P.nw + i0;
-    if (SMEM) {
-        for (int k = tid; k < P.n * tw; k += FAT_T) {
-            const int b = k / tw, i = k - b * tw;
-            xs[k] = x[(size_t)b * P.nw + i];
-        }
-        __syncthreads();
-    }
+    stage_xi_tile<SMEM, FAT_T>(P, xs, x, tw, tid);
     const int nchb = (P.nch + FAT_CH_B - 1) / FAT_CH_B;
     const int n_ck = (tw + FAT_CHUNK - 1) / FAT_CHUNK;
     for (int k = warp; k < nchb * n_ck; k += FAT_T / 32) {
@@ -155,6 +149,27 @@ __device__ __forceinline__ double fatigue_log_rate(double l0, double l1, double 
     return 0.5 * log(l2 / l0) - log_2pi + m * (ln2 + 0.5 * log(2.0 * l0)) + lgamma(1.0 + 0.5 * m);
 }
 
+// DEL = (d / P.f_eq)^(1/m) of moments l0, l1, l2, l4 into P.DEL[o] and P.info[o] (RAFTK_FATIGUE_ZERO when l0 or l2 is 0), and
+// log(p_c d_c) of the weight p_c = P.p[cl] of local case cl into P.wd[o] for the lifetime sum when P.wd is given; shared by
+// k_fatigue_finish and k_stress_finish.  The exponent *mp is read only where it is used, which keeps both kernels' code as it
+// was before they shared this.
+template <class Prm>
+__device__ __forceinline__ void fatigue_del(const Prm &P, double l0, double l1, double l2, double l4, const double *mp, int cl, size_t o)
+{
+    int info = 0;
+    double ld = -CUDART_INF, del = 0.0;
+    if (!(l0 > 0.0) || !(l2 > 0.0)) {
+        info = RAFTK_FATIGUE_ZERO;
+    } else {
+        const double m = *mp;
+        ld = fatigue_log_rate(l0, l1, l2, l4, m, P.method, &info);
+        del = exp((ld - log(P.f_eq)) / m);
+    }
+    P.DEL[o] = del;
+    P.info[o] = info;
+    if (P.wd) P.wd[o] = P.p[cl] > 0.0 ? log(P.p[cl]) + ld : -CUDART_INF;
+}
+
 __global__ void __launch_bounds__(FAT_FIN_T) k_fatigue_finish(const __grid_constant__ FatFinParams P, size_t n_threads)
 {
     const size_t g = (size_t)blockIdx.x * FAT_FIN_T + threadIdx.x;
@@ -176,18 +191,7 @@ __global__ void __launch_bounds__(FAT_FIN_T) k_fatigue_finish(const __grid_const
         double *q = P.moments + o * 4;
         q[0] = l0; q[1] = l1; q[2] = l2; q[3] = l4;
     }
-    int info = 0;
-    double ld = -CUDART_INF, del = 0.0;
-    if (!(l0 > 0.0) || !(l2 > 0.0)) {
-        info = RAFTK_FATIGUE_ZERO;
-    } else {
-        const double m = P.m[kl];
-        ld = fatigue_log_rate(l0, l1, l2, l4, m, P.method, &info);
-        del = exp((ld - log(P.f_eq)) / m);
-    }
-    P.DEL[o] = del;
-    P.info[o] = info;
-    if (P.wd) P.wd[o] = P.p[cl] > 0.0 ? log(P.p[cl]) + ld : -CUDART_INF;      // log(p_c d_c)
+    fatigue_del(P, l0, l1, l2, l4, &P.m[kl], cl, o);
 }
 
 struct FatLifeParams {

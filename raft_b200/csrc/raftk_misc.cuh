@@ -653,6 +653,20 @@ __global__ void __launch_bounds__(128) k_general_channel_stats(int n, int nch, i
 // thread-strided sum and block_rms_tail) every std, PSD and amplitude is bit-identical to k_general_channel_stats' on the
 // same R and Xi, whatever the tile width and the batch.
 // ------------------------------------------------------------------------------------------------
+// Xi tile staging shared by the tiled reductions (k_farm_channels, k_fatigue_moments, k_stress_moments): with SMEM the CTA's
+// T threads copy the tile's P.n x tw bins, x the tile's bin 0 of column 0 (stride P.nw between columns), to xs [P.n][tw]
+template <bool SMEM, int T, class Prm>
+__device__ __forceinline__ void stage_xi_tile(const Prm &P, double2 *xs, const double2 *x, int tw, int tid)
+{
+    if (SMEM) {
+        for (int k = tid; k < P.n * tw; k += T) {
+            const int b = k / tw, i = k - b * tw;
+            xs[k] = x[(size_t)b * P.nw + i];
+        }
+        __syncthreads();
+    }
+}
+
 #define FARM_CH_T 256
 #define FARM_CH_B 4             // channels per thread
 struct FarmChParams {
@@ -675,13 +689,7 @@ __global__ void __launch_bounds__(FARM_CH_T) k_farm_channels(const __grid_consta
     const int f = (int)(fr / (size_t)P.n_rows);
     const int i0 = t * P.tile, tw = min(P.tile, P.nw - i0);
     const double2 *x = P.Xi + fr * (size_t)P.n * P.nw + i0;
-    if (SMEM) {
-        for (int k = tid; k < P.n * tw; k += FARM_CH_T) {
-            const int b = k / tw, i = k - b * tw;
-            xs[k] = x[(size_t)b * P.nw + i];
-        }
-        __syncthreads();
-    }
+    stage_xi_tile<SMEM, FARM_CH_T>(P, xs, x, tw, tid);
     // a thread computes FARM_CH_B channels of one bin: each Xi value read feeds FARM_CH_B independent chains (every chain
     // still runs over b = 0..n-1 in order); a warp's threads share their channels, so the R loads are broadcasts
     const double *Rf = P.R + (size_t)f * P.r_stride;

@@ -9,10 +9,11 @@
 // So the response is walked once for the 3 x 4 sums, whatever the number of angles.
 //
 // k_stress_moments: one CTA per (unit, row, bin tile), built like k_fatigue_moments: the tile of Xi staged in shared memory
-// (read from L2 when not even one chunk fits), a warp per (ring, 32-bin chunk), one bin per lane, the chunk's twelve sums
-// reduced with a fixed shuffle tree.  Tiles are whole chunks, so a chunk's partial sums do not depend on the tile width.
+// (read from L2 when not even one chunk fits), a warp per (ring, FAT_CHUNK-bin chunk), one bin per lane, the chunk's twelve
+// sums reduced with a fixed shuffle tree.  Tiles are whole chunks of the tile rule the two share (moment_tile), so a chunk's
+// partial sums do not depend on the tile width.
 // k_stress_finish: one thread per (unit, case, ring, angle) sums the chunk partials of the case's rows in (row, chunk) order,
-// forms lambda_k(theta) and gives std, avg, max, min and the DEL through fatigue_log_rate, the closed form k_fatigue_finish
+// forms lambda_k(theta) and gives std, avg, max, min and the DEL through fatigue_del, the closed form k_fatigue_finish
 // applies.  k_stress_hot: one thread per (unit, case, ring): the argmax angles of std and DEL over the grid, and the largest
 // std over the circle, c sqrt(mu), mu the larger eigenvalue of [[S_aa,0, S_ab,0], [S_ab,0, S_bb,0]].  k_stress_psd: one thread
 // per (unit, case, ring, bin), the per-bin PSD sum_h 1/2 |sigma_h|^2 / dw of every angle.
@@ -21,7 +22,6 @@
 
 #define STR_T 256
 #define STR_FIN_T 128
-#define STR_CHUNK_BINS 32       // bins per partial sum: one warp, one bin per lane
 #define STR_NS 12               // sums per (ring, chunk): {aa, bb, ab} x {w^0, w^1, w^2, w^4}
 #define STR_LAUNCH_CASES 64     // cases per finish / hot / PSD launch: their row table travels in the launch parameters
 
@@ -94,17 +94,11 @@ __global__ void __launch_bounds__(STR_T) k_stress_moments(const __grid_constant_
     const size_t u = ur / (size_t)P.n_rows, r = ur - u * P.n_rows;
     const int i0 = t * P.tile, tw = min(P.tile, P.nw - i0);
     const double2 *x = P.Xi + ur * (size_t)P.n * P.nw + i0;
-    if (SMEM) {
-        for (int k = tid; k < P.n * tw; k += STR_T) {
-            const int b = k / tw, i = k - b * tw;
-            xs[k] = x[(size_t)b * P.nw + i];
-        }
-        __syncthreads();
-    }
-    const int n_ck = (tw + STR_CHUNK_BINS - 1) / STR_CHUNK_BINS;
+    stage_xi_tile<SMEM, STR_T>(P, xs, x, tw, tid);
+    const int n_ck = (tw + FAT_CHUNK - 1) / FAT_CHUNK;
     for (int k = warp; k < P.n_rings * n_ck; k += STR_T / 32) {
         const int ring = k / n_ck, ck = k - ring * n_ck;
-        const int i = ck * STR_CHUNK_BINS + lane, iw = i0 + i;
+        const int i = ck * FAT_CHUNK + lane, iw = i0 + i;
         const bool live = i < tw;
         double2 a = make_double2(0.0, 0.0), b = a;
         if (live) {
@@ -124,7 +118,7 @@ __global__ void __launch_bounds__(STR_T) k_stress_moments(const __grid_constant_
             double v = s[0];
 #pragma unroll
             for (int j = 1; j < STR_NS; j++) if (lane == j) v = s[j];
-            P.part[((ur * P.n_chunks + (size_t)(i0 / STR_CHUNK_BINS + ck)) * P.n_rings + ring) * STR_NS + lane] = v;
+            P.part[((ur * P.n_chunks + (size_t)(i0 / FAT_CHUNK + ck)) * P.n_rings + ring) * STR_NS + lane] = v;
         }
     }
 }
@@ -171,19 +165,7 @@ __global__ void __launch_bounds__(STR_FIN_T) k_stress_finish(const __grid_consta
         avg = P.c * (cs * mu[0] - (P.n_ch == 2 ? sn * mu[1] : 0.0));
     }
     P.std[o] = sd; P.avg[o] = avg; P.mx[o] = avg + 3.0 * sd; P.mn[o] = avg - 3.0 * sd;
-    if (P.m > 0.0) {
-        int info = 0;
-        double ld = -CUDART_INF, del = 0.0;
-        if (!(l[0] > 0.0) || !(l[2] > 0.0)) {
-            info = RAFTK_FATIGUE_ZERO;
-        } else {
-            ld = fatigue_log_rate(l[0], l[1], l[2], l[3], P.m, P.method, &info);
-            del = exp((ld - log(P.f_eq)) / P.m);
-        }
-        P.DEL[o] = del;
-        P.info[o] = info;
-        if (P.wd) P.wd[o] = P.p[cl] > 0.0 ? log(P.p[cl]) + ld : -CUDART_INF;      // log(p_c d_c), as k_fatigue_finish
-    }
+    if (P.m > 0.0) fatigue_del(P, l[0], l[1], l[2], l[3], &P.m, cl, o);
 }
 
 // argmax over the grid of std (and DEL) and the largest std over the circle, for (unit, case, ring):

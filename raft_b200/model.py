@@ -99,13 +99,10 @@ class Model:
             missing = sorted(set(self.fatigue["m"]) - known)
             if missing:
                 raise ValueError("fatigue=: no channel named %s" % missing)
-        self.stress = None if stress is None else solver.stress_options(stress)
-        if self.stress is not None:
-            have = [ch for ch in self.channels if ch is not None]
-            if not have:
-                raise ValueError("stress=: the channels have no tower-base moment (Mbase, or MbaseY and MbaseX)")
-            for ch in have:
-                solver.stress_rows((ch[0] if isinstance(ch, (list, tuple)) else ch)["names"])
+        # FOWTs without turbine channels have no stress ring; when none has channels, stress= is refused like channels
+        # without a tower-base moment
+        have = [ch[0] if isinstance(ch, (list, tuple)) else ch for ch in self.channels if ch is not None]
+        self.stress = solver.stress_options_for(stress, have or [dict(names=[])])
         for f in self.fowtList:
             f.calcHydroConstants()
 

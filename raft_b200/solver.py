@@ -1100,6 +1100,39 @@ def _check_wpow(wpow):
         raise ValueError("wpow must be 0, 1 or 2 (displacement, velocity, acceleration)")
 
 
+def _unit_response(be, Xi, w):
+    """The response of a per-unit reduction on ``be``'s buffers: Xi complex [n_units, n_rows, n_dof, nw] or [n_rows, n_dof,
+    nw], w [nw] -> (Xi [n_units, n_rows, n_dof, nw], w, whether Xi had no unit axis)."""
+    Xi = be.array(Xi, _C16)
+    squeeze = Xi.ndim == 3
+    if squeeze:
+        Xi = Xi[None]
+    if Xi.ndim != 4:
+        raise ValueError("Xi must be [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]")
+    w = be.array(w, _F8)
+    if tuple(w.shape) != (Xi.shape[3],):
+        raise ValueError("w must be [nw]")
+    return Xi, w, squeeze
+
+
+def _case_rows(case_row0, n_rows):
+    """``case_row0`` [nC + 1], the first row of every case (None: one row per case), checked -> int32 host array."""
+    case_row0 = np.arange(n_rows + 1, dtype=_I4) if case_row0 is None else np.ascontiguousarray(case_row0, dtype=_I4)
+    if len(case_row0) < 2 or case_row0[0] != 0 or case_row0[-1] != n_rows or np.any(np.diff(case_row0) < 1):
+        raise ValueError("case_row0 must start at 0, end at %d and give every case at least one row" % n_rows)
+    return case_row0
+
+
+def _case_weights(weights, n_cases):
+    """Case probabilities ``weights`` [n_cases] of a lifetime sum, or None, checked -> float64 host array or None."""
+    if weights is None:
+        return None
+    weights = np.ascontiguousarray(weights, dtype=_F8)
+    if weights.shape != (n_cases,) or not np.all(np.isfinite(weights)) or np.any(weights < 0) or not weights.sum() > 0:
+        raise ValueError("weights must be [nC], finite, >= 0 and not all 0")
+    return weights
+
+
 def general_channel_stats(R, wpow, w, Xi, dw, psd=True, amp=False):
     """Output channels of a FOWT with generalised DOFs, Y = w^wpow R Xi (``packer.pack_general_channels``), host buffers:
     R [nch,nDOF], wpow [nch] 0, 1 or 2, w [nw], Xi complex [nU,nDOF,nw] -> (std [nU,nch], PSD [nU,nch,nw] or None,
@@ -1236,17 +1269,9 @@ def rotor_stats(R, C_, V_w, gains, w, Xi, dw, case_row0=None, col0=None, psd=Tru
 
 def _rotor_stats(be, R, C_, V_w, gains, w, Xi, dw, case_row0, col0, psd):
     """``rotor_stats`` on ``be``'s buffers (case_row0 and col0: numpy)."""
-    Xi = be.array(Xi, _C16)
-    squeeze = Xi.ndim == 3
-    if squeeze:
-        Xi = Xi[None]
-    if Xi.ndim != 4:
-        raise ValueError("Xi must be [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]")
+    Xi, w, squeeze = _unit_response(be, Xi, w)
     nU, nR, n, nw = Xi.shape
     R, C_, V_w, gains = be.array(R, _F8), be.array(C_, _C16), be.array(V_w, _C16), be.array(gains, _F8)
-    w = be.array(w, _F8)
-    if tuple(w.shape) != (nw,):
-        raise ValueError("w must be [nw]")
     ro, rows, cols = _rotor_struct(R, C_, V_w, gains, nU, nw, dw, case_row0, col0)
     sd = be.empty([nU, ro.n_cases, ro.n_rot, 3])
     P = be.empty([nU, ro.n_cases, ro.n_rot, 3, nw]) if psd else None
@@ -1281,6 +1306,17 @@ FATIGUE_METHODS = {"dirlik": 0, "narrowband": 1}
 FATIGUE_ZERO, FATIGUE_NARROWBAND = 1, 2          # info bits (include/raftk.h RAFTK_FATIGUE_ZERO / _NARROWBAND)
 
 
+def _fatigue_law(m, f_eq, method, prefix=""):
+    """The DEL closed form's Woehler exponent ``m`` (scalar, per channel, or None: no DEL), ``f_eq`` and ``method`` checked;
+    ``prefix`` starts every refusal."""
+    if m is not None and not (np.all(np.isfinite(m)) and np.all(np.asarray(m) > 0)):
+        raise ValueError(prefix + ("every m" if np.ndim(m) else "m") + " must be finite and > 0")
+    if not (np.isfinite(f_eq) and f_eq > 0):
+        raise ValueError(prefix + "f_eq must be finite and > 0")
+    if method not in FATIGUE_METHODS:
+        raise ValueError(prefix + "method must be one of %s" % sorted(FATIGUE_METHODS))
+
+
 def _fatigue_struct(n_units, n_rows, n, nw, m, R, wpow, coef, case_row0, f_eq, method, weights, tile_w):
     """Shapes and options of fatigue's inputs (R / coef numpy arrays or torch tensors) checked -> (raftk_fatigue without data
     pointers, the host arrays it points to).  R [nch, n] (every unit) or [n_units, nch, n]; coef [nch, n, nw] (every unit),
@@ -1306,20 +1342,10 @@ def _fatigue_struct(n_units, n_rows, n, nw, m, R, wpow, coef, case_row0, f_eq, m
         if wpow is not None:
             raise ValueError("wpow applies to real rows R only")
     m = np.ascontiguousarray(np.broadcast_to(np.asarray(m, dtype=_F8), (nch,)))
-    if not (np.all(np.isfinite(m)) and np.all(m > 0)):
-        raise ValueError("every m must be finite and > 0")
-    if not (np.isfinite(f_eq) and f_eq > 0):
-        raise ValueError("f_eq must be finite and > 0")
-    if method not in FATIGUE_METHODS:
-        raise ValueError("method must be one of %s" % sorted(FATIGUE_METHODS))
-    nC = n_rows if case_row0 is None else len(case_row0) - 1
-    case_row0 = np.arange(nC + 1, dtype=_I4) if case_row0 is None else np.ascontiguousarray(case_row0, dtype=_I4)
-    if nC < 1 or case_row0[0] != 0 or case_row0[-1] != n_rows or np.any(np.diff(case_row0) < 1):
-        raise ValueError("case_row0 must start at 0, end at %d and give every case at least one row" % n_rows)
-    if weights is not None:
-        weights = np.ascontiguousarray(weights, dtype=_F8)
-        if weights.shape != (nC,) or not np.all(np.isfinite(weights)) or np.any(weights < 0) or not weights.sum() > 0:
-            raise ValueError("weights must be [nC], finite, >= 0 and not all 0")
+    _fatigue_law(m, f_eq, method)
+    case_row0 = _case_rows(case_row0, n_rows)
+    nC = len(case_row0) - 1
+    weights = _case_weights(weights, nC)
     fa.n_cases, fa.n_ch, fa.method, fa.tile_w = nC, nch, FATIGUE_METHODS[method], int(tile_w)
     fa.case_row0, fa.m, fa.f_eq = case_row0.ctypes.data, m.ctypes.data, float(f_eq)
     fa.wpow = wpow.ctypes.data if R is not None else None
@@ -1344,16 +1370,8 @@ def fatigue(Xi, w, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, me
 
 def _fatigue(be, Xi, w, m, R, wpow, coef, case_row0, f_eq, method, weights, life, moments, tile_w):
     """``fatigue`` on ``be``'s buffers (m, wpow, case_row0 and weights: numpy)."""
-    Xi = be.array(Xi, _C16)
-    squeeze = Xi.ndim == 3
-    if squeeze:
-        Xi = Xi[None]
-    if Xi.ndim != 4:
-        raise ValueError("Xi must be [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]")
+    Xi, w, squeeze = _unit_response(be, Xi, w)
     nU, nR, n, nw = Xi.shape
-    w = be.array(w, _F8)
-    if tuple(w.shape) != (nw,):
-        raise ValueError("w must be [nw]")
     R = None if R is None else be.array(R, _F8)
     coef = None if coef is None else be.array(coef, _C16)
     fa, keep = _fatigue_struct(nU, nR, n, nw, m, R, wpow, coef, case_row0, f_eq, method, weights, tile_w)
@@ -1438,41 +1456,23 @@ def stress_ring(Xi, w, fa, ss, angles=None, d=10.0, t=0.083, m=None, f_eq=1.0, m
 
 def _stress_ring(be, Xi, w, fa, ss, angles, d, t, m, f_eq, method, weights, case_row0, col0, psd, mean, wpow, dw, tile_w):
     """``stress_ring`` on ``be``'s buffers (angles, case_row0, col0, wpow and weights: numpy)."""
-    Xi = be.array(Xi, _C16)
-    squeeze = Xi.ndim == 3
-    if squeeze:
-        Xi = Xi[None]
-    if Xi.ndim != 4:
-        raise ValueError("Xi must be [n_units, n_rows, n_dof, nw] or [n_rows, n_dof, nw]")
+    Xi, w, squeeze = _unit_response(be, Xi, w)
     nU, nR, n, nw = Xi.shape
-    w = be.array(w, _F8)
-    if tuple(w.shape) != (nw,):
-        raise ValueError("w must be [nw]")
     X, n_rings, n_r, n_ch, mode, wp = _stress_channels(be, fa, ss, nU, nR, n, nw, wpow)
     angles = np.ascontiguousarray(STRESS_ANGLES if angles is None else np.atleast_1d(np.asarray(angles, dtype=_F8)))
     if angles.ndim != 1 or not 1 <= len(angles) <= 256 or not np.all(np.isfinite(angles)):
         raise ValueError("angles must be 1 to 256 finite values (rad)")
     if not (np.isfinite(d) and d > 0 and np.isfinite(t) and t > 0):
         raise ValueError("d and t must be finite and > 0")
-    if m is not None and not (np.isfinite(m) and m > 0):
-        raise ValueError("m must be finite and > 0")
-    if not (np.isfinite(f_eq) and f_eq > 0):
-        raise ValueError("f_eq must be finite and > 0")
-    if method not in FATIGUE_METHODS:
-        raise ValueError("method must be one of %s" % sorted(FATIGUE_METHODS))
-    nC = nR if case_row0 is None else len(case_row0) - 1
-    case_row0 = np.arange(nC + 1, dtype=_I4) if case_row0 is None else np.ascontiguousarray(case_row0, dtype=_I4)
-    if nC < 1 or case_row0[0] != 0 or case_row0[-1] != nR or np.any(np.diff(case_row0) < 1):
-        raise ValueError("case_row0 must start at 0, end at %d and give every case at least one row" % nR)
+    _fatigue_law(m, f_eq, method)
+    case_row0 = _case_rows(case_row0, nR)
+    nC = len(case_row0) - 1
     if n_rings > 64:
         raise ValueError("at most 64 rings per call")
     col0 = np.zeros(n_rings, dtype=_I4) if col0 is None else np.ascontiguousarray(np.broadcast_to(np.asarray(col0, dtype=_I4), (n_rings,)))
     if np.any(col0 < 0) or np.any(col0 > n - n_r):
         raise ValueError("col0 must lie in [0, %d]" % (n - n_r))
-    if weights is not None:
-        weights = np.ascontiguousarray(weights, dtype=_F8)
-        if weights.shape != (nC,) or not np.all(np.isfinite(weights)) or np.any(weights < 0) or not weights.sum() > 0:
-            raise ValueError("weights must be [nC], finite, >= 0 and not all 0")
+    weights = _case_weights(weights, nC)
     life = weights is not None and m is not None
     dw = (float(w[1] - w[0]) if nw > 1 else 1.0) if dw is None else float(dw)
     if psd and not (np.isfinite(dw) and dw > 0):
@@ -1548,10 +1548,7 @@ def stress_options(stress):
              method=stress.get("method", "dirlik"), weights=stress.get("weights"), psd=bool(stress.get("psd", False)))
     if not (np.isfinite(o["d"]) and o["d"] > 0 and np.isfinite(o["t"]) and o["t"] > 0):
         raise ValueError("stress=: d and t must be finite and > 0")
-    if o["m"] is not None and not (np.isfinite(o["m"]) and o["m"] > 0):
-        raise ValueError("stress=: m must be finite and > 0")
-    if o["method"] not in FATIGUE_METHODS:
-        raise ValueError("stress=: method must be one of %s" % sorted(FATIGUE_METHODS))
+    _fatigue_law(o["m"], o["f_eq"], o["method"], "stress=: ")
     if o["angles"].ndim != 1 or not 1 <= len(o["angles"]) <= 256 or not np.all(np.isfinite(o["angles"])):
         raise ValueError("stress=: angles must be 1 to 256 finite values (rad)")
     return o
@@ -1707,7 +1704,7 @@ def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01
     from .packer import pack_case_trains
     _no_general_ops(turbine_constants)
     opts = None if fatigue is None else fatigue_options(fatigue)
-    sopts = _general_stress_options(stress, [channels])
+    sopts = stress_options_for(stress, [channels])
     table, owner, first = pack_case_trains(cases)
     q = bool(qtf)
     res = general_solve_dynamics(P, M, B, Cm, CaseTable(table, ops=_train_ops(ops, owner, len(cases))), n_iter=n_iter, tol=tol,
@@ -1715,8 +1712,9 @@ def general_analyze_cases(P, M, B, Cm, cases, channels=None, n_iter=10, tol=0.01
     return _general_case_results(P, res[0], res[1], owner, first, len(cases), channels, res[2:4] if q else None, rotors, opts, sopts)
 
 
-def _general_stress_options(stress, channels):
-    """``stress=`` of the generalised-DOF analyses checked against every design's channels before anything is solved."""
+def stress_options_for(stress, channels):
+    """``stress=`` (``stress_options``) checked against the channels of every FOWT or design it applies to, before anything
+    is solved: each must have a tower-base moment (``stress_rows``); None (no channels) is refused.  None when ``stress`` is."""
     if stress is None:
         return None
     o = stress_options(stress)
@@ -2108,7 +2106,7 @@ def general_analyze_cases_batch(designs, cases, channels=None, n_iter=10, tol=0.
         raise ValueError("channels: one entry per design (%d), got %d" % (bt.n_designs, len(channels)))
     if rotors is not None and len(rotors) != bt.n_designs:
         raise ValueError("rotors: one entry per design (%d), got %d" % (bt.n_designs, len(rotors)))
-    sopts = None if stress is None else _general_stress_options(stress, [None] * bt.n_designs if channels is None else channels)
+    sopts = None if stress is None else stress_options_for(stress, [None] * bt.n_designs if channels is None else channels)
     table, owner, first = pack_case_trains(cases)
     q = bt.qtf is not None
     res = general_solve_dynamics_batch(bt, CaseTable(table, ops=_train_ops(ops, owner, len(cases))), n_iter=n_iter, tol=tol,

@@ -293,7 +293,7 @@ def _base(nU=2, nR=3, n=6, nw=40, nch=2):
 
 
 def _refusals():
-    """(name, mutation of (fa, keep, dims) -> dims) for every refusal the header lists."""
+    """(name, mutation of (fa, keep, dims) -> dims, the refusal's reason) for every refusal the header lists."""
     def setf(**kv):
         def f(fa, keep, dims):
             for k, v in kv.items():
@@ -314,29 +314,39 @@ def _refusals():
             d[i] = v
             return tuple(d)
         return f
+    ge1, req, rows = ">= 1", "are required", "case_row0 must start at 0 and end at n_rows"
     return [
-        ("n_units", dims(0, 0)), ("n_rows", dims(1, 0)), ("n_dof", dims(2, 0)), ("nw", dims(3, 0)),
-        ("n_cases", setf(n_cases=0)), ("n_ch", setf(n_ch=0)), ("too_many_ch", setf(n_ch=4097)),
-        ("no_R_no_coef", setf(R=None)), ("both_R_and_coef", lambda fa, k, d: (setattr(fa, "coef", k["coef"].ctypes.data), d)[1]),
-        ("R_shared", setf(R_shared=2)), ("coef_mode", lambda fa, k, d: (setattr(fa, "R", None), setattr(fa, "coef", k["coef"].ctypes.data),
-                                                                          setattr(fa, "coef_mode", 3), d)[3]),
-        ("method", setf(method=2)), ("wpow", arr("wpow", [0, 3], "wpow", np.int32)), ("wpow_neg", arr("wpow", [-1, 0], "wpow", np.int32)),
-        ("m_null", setf(m=None)), ("case_row0_null", setf(case_row0=None)), ("DEL_null", setf(DEL=None)), ("info_null", setf(info=None)),
-        ("row0_start", arr("row0", [1, 2, 3], "case_row0", np.int32)), ("row0_end", arr("row0", [0, 1, 2], "case_row0", np.int32)),
-        ("row0_empty", arr("row0", [0, 0, 3], "case_row0", np.int32)), ("row0_decreasing", arr("row0", [0, 2, 1], "case_row0", np.int32)),
-        ("m_zero", arr("m", [4.0, 0.0], "m")), ("m_neg", arr("m", [-3.0, 4.0], "m")), ("m_nan", arr("m", [np.nan, 4.0], "m")),
-        ("m_inf", arr("m", [np.inf, 4.0], "m")), ("f_eq_zero", setf(f_eq=0.0)), ("f_eq_neg", setf(f_eq=-1.0)), ("f_eq_nan", setf(f_eq=float("nan"))),
-        ("weights_neg", arr("weights", [1.0, -1.0], "weights")), ("weights_zero", arr("weights", [0.0, 0.0], "weights")),
-        ("weights_nan", arr("weights", [np.nan, 1.0], "weights")),
+        ("n_units", dims(0, 0), ge1), ("n_rows", dims(1, 0), ge1), ("n_dof", dims(2, 0), ge1), ("nw", dims(3, 0), ge1),
+        ("n_cases", setf(n_cases=0), ge1), ("n_ch", setf(n_ch=0), ge1), ("too_many_ch", setf(n_ch=4097), "at most 4096 channels per call"),
+        ("no_R_no_coef", setf(R=None), "give exactly one of R"),
+        ("both_R_and_coef", lambda fa, k, d: (setattr(fa, "coef", k["coef"].ctypes.data), d)[1], "give exactly one of R"),
+        ("R_shared", setf(R_shared=2), "R_shared must be 0 or 1"),
+        ("coef_mode", lambda fa, k, d: (setattr(fa, "R", None), setattr(fa, "coef", k["coef"].ctypes.data), setattr(fa, "coef_mode", 3), d)[3],
+         "unknown coef_mode"),
+        ("method", setf(method=2), "unknown method"), ("wpow", arr("wpow", [0, 3], "wpow", np.int32), "wpow must be 0, 1 or 2"),
+        ("wpow_neg", arr("wpow", [-1, 0], "wpow", np.int32), "wpow must be 0, 1 or 2"),
+        ("m_null", setf(m=None), req), ("case_row0_null", setf(case_row0=None), req), ("DEL_null", setf(DEL=None), req),
+        ("info_null", setf(info=None), req),
+        ("row0_start", arr("row0", [1, 2, 3], "case_row0", np.int32), rows), ("row0_end", arr("row0", [0, 1, 2], "case_row0", np.int32), rows),
+        ("row0_empty", arr("row0", [0, 0, 3], "case_row0", np.int32), "every case needs at least one row"),
+        ("row0_decreasing", arr("row0", [0, 2, 1], "case_row0", np.int32), rows),
+        ("m_zero", arr("m", [4.0, 0.0], "m"), "every m must be finite and > 0"), ("m_neg", arr("m", [-3.0, 4.0], "m"), "every m must be finite and > 0"),
+        ("m_nan", arr("m", [np.nan, 4.0], "m"), "every m must be finite and > 0"), ("m_inf", arr("m", [np.inf, 4.0], "m"), "every m must be finite and > 0"),
+        ("f_eq_zero", setf(f_eq=0.0), "f_eq must be finite and > 0"), ("f_eq_neg", setf(f_eq=-1.0), "f_eq must be finite and > 0"),
+        ("f_eq_nan", setf(f_eq=float("nan")), "f_eq must be finite and > 0"),
+        ("weights_neg", arr("weights", [1.0, -1.0], "weights"), "weights must be finite and >= 0"),
+        ("weights_zero", arr("weights", [0.0, 0.0], "weights"), "the weights must not all be 0"),
+        ("weights_nan", arr("weights", [np.nan, 1.0], "weights"), "weights must be finite and >= 0"),
     ]
 
 
 @pytest.mark.parametrize("name", [r[0] for r in _refusals()])
 def test_every_refusal_before_any_launch(name):
-    """RAFTK_EINVAL (-1) from both entries, before any launch (raftk_launch_count unchanged), for each refusal of the header."""
+    """RAFTK_EINVAL (-1) from both entries with the refusal's reason after the "fatigue: " prefix, before any launch
+    (raftk_launch_count unchanged), for each refusal of the header."""
     from raft_b200 import _lib
     lib = _lib.lib
-    mut = dict(_refusals())[name]
+    mut, msg = {r[0]: r[1:] for r in _refusals()}[name]
     for entry in ("host", "dev"):
         fa, keep, dims = _base()
         dims = mut(fa, keep, dims)
@@ -347,7 +357,8 @@ def test_every_refusal_before_any_launch(name):
             rc = lib.raftk_fatigue_dev(*dims, keep["w"].ctypes.data, keep["Xi"].ctypes.data, C.byref(fa), keep["Xi"].ctypes.data, 1 << 30, None)
         assert rc == -1, (name, entry, rc)
         assert lib.raftk_launch_count() == n0
-        assert lib.raftk_last_error()
+        err = lib.raftk_last_error().decode()
+        assert err.startswith("fatigue: ") and msg in err, (name, entry, err)
 
 
 def test_refusals_without_inputs_and_small_workspace():

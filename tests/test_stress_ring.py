@@ -148,33 +148,47 @@ def _refusals():
     def both(sr, keep, d):
         sr.coef, sr.coef_mode = keep["coef"].ctypes.data, 0
         return d
-    return [("n_units", dims(0, 0)), ("n_rows", dims(1, 0)), ("n_dof", dims(2, 0)), ("nw", dims(3, 0)),
-            ("n_cases", setf(n_cases=0)), ("n_rings", setf(n_rings=0)), ("n_r", setf(n_r=0)), ("n_angles", setf(n_angles=0)),
-            ("n_ch 0", setf(n_ch=0)), ("n_ch 3", setf(n_ch=3)), ("rings", setf(n_rings=65)), ("angles max", setf(n_angles=257)),
-            ("n_r above n_dof", setf(n_r=13)), ("col0 high", arr("col0", [7], "col0", np.int32)),
-            ("col0 negative", arr("col0", [-1], "col0", np.int32)), ("no channels", setf(R=None)), ("both forms", both),
-            ("R_shared", setf(R_shared=2)), ("method", setf(method=2)), ("wpow", arr("wpow", [0, 3], "wpow", np.int32)),
-            ("w", lambda sr, k, d: (k.__setitem__("nullw", True), d)[1]), ("Xi", lambda sr, k, d: (k.__setitem__("nullxi", True), d)[1]),
-            ("angles null", setf(angles=None)), ("case_row0 null", setf(case_row0=None)), ("std null", setf(std=None)),
-            ("avg null", setf(avg=None)), ("max null", setf(max=None)), ("min null", setf(min=None)),
-            ("angle nan", arr("angles", [0, np.nan, 1, 2, 3], "angles")), ("d", setf(d=0.0)), ("t", setf(t=-1.0)),
-            ("d inf", setf(d=np.inf)), ("m negative", setf(m=-1.0)), ("m nan", setf(m=np.nan)), ("DEL null", setf(DEL=None)),
-            ("info null", setf(info=None)), ("life without m", lambda sr, k, d: (setattr(sr, "DEL_life", k["DEL_life"].ctypes.data),
-                                                                                setattr(sr, "m", 0.0), d)[2]),
-            ("hot_life without life", lambda sr, k, d: (setattr(sr, "hot_life", k["DEL_life"].ctypes.data), d)[1]),
-            ("psd without dw", lambda sr, k, d: (setattr(sr, "psd", k["psd"].ctypes.data), setattr(sr, "dw", 0.0), d)[2]),
-            ("f_eq", setf(f_eq=0.0)), ("row0 start", arr("row0", [1, 1, 3], "case_row0", np.int32)),
-            ("row0 end", arr("row0", [0, 1, 2], "case_row0", np.int32)), ("row0 empty", arr("row0", [0, 0, 3], "case_row0", np.int32)),
-            ("weights negative", arr("weights", [1.0, -1.0], "weights")), ("weights zero", arr("weights", [0.0, 0.0], "weights")),
-            ("weights nan", arr("weights", [np.nan, 1.0], "weights"))]
+    def coef_mode(sr, keep, d):
+        sr.R, sr.coef, sr.coef_mode = None, keep["coef"].ctypes.data, 3
+        return d
+    ge1, req, rows = ">= 1", "are required", "case_row0 must start at 0 and end at n_rows"
+    col0, dt, m, de = "col0 of ring 0 outside [0, n_dof - n_r]", "d and t must be finite and > 0", "m must be 0 (no DEL) or finite and > 0", \
+        "DEL and info are required with m > 0"
+    return [("n_units", dims(0, 0), ge1), ("n_rows", dims(1, 0), ge1), ("n_dof", dims(2, 0), ge1), ("nw", dims(3, 0), ge1),
+            ("n_cases", setf(n_cases=0), ge1), ("n_rings", setf(n_rings=0), ge1), ("n_r", setf(n_r=0), ge1), ("n_angles", setf(n_angles=0), ge1),
+            ("n_ch 0", setf(n_ch=0), "n_ch must be 1"), ("n_ch 3", setf(n_ch=3), "n_ch must be 1"),
+            ("rings", setf(n_rings=65), "at most 64 rings per call"), ("angles max", setf(n_angles=257), "at most 256 angles per call"),
+            ("n_r above n_dof", setf(n_r=13), "n_r must not exceed n_dof"), ("col0 high", arr("col0", [7], "col0", np.int32), col0),
+            ("col0 negative", arr("col0", [-1], "col0", np.int32), col0), ("no channels", setf(R=None), "give exactly one of R"),
+            ("both forms", both, "give exactly one of R"), ("R_shared", setf(R_shared=2), "R_shared must be 0 or 1"),
+            ("coef_mode", coef_mode, "unknown coef_mode"), ("method", setf(method=2), "unknown method"),
+            ("wpow", arr("wpow", [0, 3], "wpow", np.int32), "wpow must be 0, 1 or 2"),
+            ("w", lambda sr, k, d: (k.__setitem__("nullw", True), d)[1], req), ("Xi", lambda sr, k, d: (k.__setitem__("nullxi", True), d)[1], req),
+            ("angles null", setf(angles=None), req), ("case_row0 null", setf(case_row0=None), req), ("std null", setf(std=None), req),
+            ("avg null", setf(avg=None), req), ("max null", setf(max=None), req), ("min null", setf(min=None), req),
+            ("angle nan", arr("angles", [0, np.nan, 1, 2, 3], "angles"), "every angle must be finite"), ("d", setf(d=0.0), dt),
+            ("t", setf(t=-1.0), dt), ("d inf", setf(d=np.inf), dt), ("m negative", setf(m=-1.0), m), ("m nan", setf(m=np.nan), m),
+            ("DEL null", setf(DEL=None), de), ("info null", setf(info=None), de),
+            ("life without m", lambda sr, k, d: (setattr(sr, "DEL_life", k["DEL_life"].ctypes.data), setattr(sr, "m", 0.0), d)[2],
+             "DEL_life needs m > 0"),
+            ("hot_life without life", lambda sr, k, d: (setattr(sr, "hot_life", k["DEL_life"].ctypes.data), d)[1], "hot_life needs DEL_life"),
+            ("psd without dw", lambda sr, k, d: (setattr(sr, "psd", k["psd"].ctypes.data), setattr(sr, "dw", 0.0), d)[2],
+             "psd needs a finite dw > 0"),
+            ("f_eq", setf(f_eq=0.0), "f_eq must be finite and > 0"), ("row0 start", arr("row0", [1, 1, 3], "case_row0", np.int32), rows),
+            ("row0 end", arr("row0", [0, 1, 2], "case_row0", np.int32), rows),
+            ("row0 empty", arr("row0", [0, 0, 3], "case_row0", np.int32), "every case needs at least one row"),
+            ("weights negative", arr("weights", [1.0, -1.0], "weights"), "weights must be finite and >= 0"),
+            ("weights zero", arr("weights", [0.0, 0.0], "weights"), "the weights must not all be 0"),
+            ("weights nan", arr("weights", [np.nan, 1.0], "weights"), "weights must be finite and >= 0")]
 
 
-@pytest.mark.parametrize("name", [n for n, _ in _refusals()])
+@pytest.mark.parametrize("name", [r[0] for r in _refusals()])
 def test_invalid_arguments_are_refused_before_any_launch(name):
-    """Every refusal the header lists returns RAFTK_EINVAL from _host and _dev, before any launch."""
+    """Every refusal the header lists returns RAFTK_EINVAL from _host and _dev with its reason after the "stress ring: "
+    prefix, before any launch."""
     from raft_b200 import _lib
     lib = _lib.lib
-    mut = dict(_refusals())[name]
+    mut, msg = {r[0]: r[1:] for r in _refusals()}[name]
     for entry in ("host", "dev"):
         sr, keep, dims = _base()
         dims = mut(sr, keep, dims)
@@ -188,6 +202,8 @@ def test_invalid_arguments_are_refused_before_any_launch(name):
             rc = lib.raftk_stress_ring_dev(*dims, w, xi, C.byref(sr), (buf.ctypes.data + 31) // 32 * 32, 1 << 18, None)
         assert rc == -1, (name, entry, rc)
         assert lib.raftk_launch_count() == n0
+        err = lib.raftk_last_error().decode()
+        assert err.startswith("stress ring: ") and msg in err, (name, entry, err)
 
 
 def test_workspace_too_small_or_misaligned_is_refused():
