@@ -67,7 +67,9 @@ typedef struct raftk_designs {
     int32_t max_w_classes;      /* hints for the fused solver's on-chip tables: max number of distinct     */
     int32_t max_h_classes;      /* (q_x,q_y)*step resp. q_z*step node spacings of any design; 0 = worst case */
     int32_t max_z_classes;      /* max distinct first-node depths z0 of any design's members; 0 = worst case   */
-    int32_t _pad1;
+    int32_t walk_exact;         /* 1: the fused solvers' node walk is exact for every member on this grid: no deep-water
+                                   bin with k |z0| > 700 and no finite-depth bin with k (z0 - z_min) > 10 (DESIGN.md
+                                   section 4; raft_b200.solver.fused_walk_exact); 0 = not, or not known: the v1 solver runs */
     double depth, rho, g, dw;   /* site (raft_fowt.py:167-173); dw = w[1]-w[0]                  */
     const double *w;            /* [nw] rad/s           raft_model.py:57                       */
     const double *k;            /* [nw] wave numbers    raft_fowt.py:170 (helpers.py:377)      */
@@ -239,7 +241,7 @@ typedef struct raftk_dispatch {
     int32_t trains;           /* cases.primary: the fused solver ran its two wave-train phases, or the generalised-DOF
                                  solve its secondary-train step                                                          */
     int32_t chunks;           /* v1 solver: launches over design chunks (1 = the whole batch at once)                    */
-    int32_t _pad0;
+    int32_t inexact_walk;     /* the v1 solver ran because designs.walk_exact is 0                                       */
 } raftk_dispatch;
 int raftk_last_dispatch(raftk_dispatch *out);
 

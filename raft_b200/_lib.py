@@ -18,7 +18,7 @@ c_int32_p = C.POINTER(C.c_int32)
 class RaftkDesigns(C.Structure):
     _fields_ = [
         ("n_designs", C.c_int32), ("nw", C.c_int32), ("n_members_total", C.c_int32), ("n_nodes_total", C.c_int32),
-        ("max_nodes", C.c_int32), ("max_members", C.c_int32), ("max_w_classes", C.c_int32), ("max_h_classes", C.c_int32), ("max_z_classes", C.c_int32), ("_pad1", C.c_int32),
+        ("max_nodes", C.c_int32), ("max_members", C.c_int32), ("max_w_classes", C.c_int32), ("max_h_classes", C.c_int32), ("max_z_classes", C.c_int32), ("walk_exact", C.c_int32),
         ("depth", C.c_double), ("rho", C.c_double), ("g", C.c_double), ("dw", C.c_double),
         ("w", C.c_void_p), ("k", C.c_void_p), ("member_offset", C.c_void_p),
         ("mem_frame", C.c_void_p), ("mem_rA", C.c_void_p), ("mem_arm", C.c_void_p),
@@ -165,7 +165,7 @@ class RaftkSlenderOutputs(C.Structure):
 class RaftkDispatch(C.Structure):
     """include/raftk.h raftk_dispatch: the kernel variant the last call on this thread launched."""
     _fields_ = [(n, C.c_int32) for n in ("family", "kernel", "cluster_size", "bins_per_cta", "threads_per_cta", "f0_global", "direct_d2h",
-                                         "trains", "chunks", "_pad0")]
+                                         "trains", "chunks", "inexact_walk")]
 
 
 # every symbol include/raftk.h declares (tests/test_abi.py checks the header against this list)

@@ -368,6 +368,7 @@ static const size_t WS_UNBOUNDED = SIZE_MAX;     // plan to size a workspace: it
 
 // Plan a solve of d x n_cases against wbytes of workspace.  requested_cs: the caller's cluster size when it is 1, 2, 4 or 8,
 // else the planner picks one.  v1_only: the tables path (excitation, linearisation), as RAFTK_FORCE_V1 does for the solve.
+// Designs whose node walk the fused kernels cannot carry exactly (d->walk_exact == 0, DESIGN.md section 4) go to v1.
 static SolvePlan plan_solve(const raftk_designs *d, int n_cases, int requested_cs, size_t wbytes, bool v1_only = false)
 {
     const int nw = d->nw;
@@ -388,7 +389,7 @@ static SolvePlan plan_solve(const raftk_designs *d, int n_cases, int requested_c
     base.o_lin = align_up(f0, 256);
     base.lin_end = base.o_lin + units * ((size_t)NCOEF * d->max_nodes + 36) * sizeof(double);
 
-    if (!v1_only && !getenv("RAFTK_FORCE_V1") && d->max_nodes > 0 && d->max_members > 0) {
+    if (!v1_only && !getenv("RAFTK_FORCE_V1") && d->walk_exact && d->max_nodes > 0 && d->max_members > 0) {
         SolvePlan p = base;
         p.kind = SOLVE_FUSED2; p.T = F2_T;
         p.CS = req;
@@ -749,10 +750,14 @@ static int launch_solve(const raftk_designs *d, const raftk_cases *c, const raft
 {
     if (pl.kind == SOLVE_FUSED2) return run_fused2(d, c, o, out, pl, workspace, st, peers);
     if (pl.kind == SOLVE_FUSED) return run_fused(d, c, o, out, pl, workspace, wbytes, st, peers);
-    if (peers && peers->n_ranks > 1) return set_err(RAFTK_EINVAL, "the fused exchange needs the fused solver; the design's frequency slice does not fit on chip");
-    if (c->primary) return set_err(RAFTK_EINVAL, "wave-train cases (cases.primary) need the fused solver; the design's frequency slice does not fit on chip");
-    if (c->Xi_init || out->Xi_last) return set_err(RAFTK_EINVAL, "cases.Xi_init / outputs.Xi_last need the fused solver; the design's frequency slice does not fit on chip");
-    return run_tables(d, c, o, out, nullptr, 0, pl, workspace, wbytes, st);
+    const char *why = d->walk_exact ? "the design's frequency slice does not fit on chip"
+                                     : "its node walk is inexact on this design and grid (designs.walk_exact = 0)";
+    if (peers && peers->n_ranks > 1) return set_err(RAFTK_EINVAL, "the fused exchange needs the fused solver; %s", why);
+    if (c->primary) return set_err(RAFTK_EINVAL, "wave-train cases (cases.primary) need the fused solver; %s", why);
+    if (c->Xi_init || out->Xi_last) return set_err(RAFTK_EINVAL, "cases.Xi_init / outputs.Xi_last need the fused solver; %s", why);
+    const int rc = run_tables(d, c, o, out, nullptr, 0, pl, workspace, wbytes, st);
+    g_disp.inexact_walk = !d->walk_exact;
+    return rc;
 }
 
 // the rigid solve over the caller's workspace: planned against it, then launched

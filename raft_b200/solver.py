@@ -172,6 +172,7 @@ class DesignBatch:
         self.max_nodes = max(1, max_nodes)
         self.max_members = max(1, max_members)
         self.max_w_classes, self.max_h_classes, self.max_z_classes = self._step_classes(packed)
+        self.walk_exact = fused_walk_exact(a, self.k, self.depth)
 
     @classmethod
     def from_tables(cls, arrays, n_designs, depth, rho, g, dw, max_nodes, max_members, classes):
@@ -188,6 +189,7 @@ class DesignBatch:
         self.n_nodes_total = int(a["mem_node_start"][-1])
         self.max_nodes, self.max_members = int(max_nodes), int(max_members)
         self.max_w_classes, self.max_h_classes, self.max_z_classes = (int(c) for c in classes)
+        self.walk_exact = fused_walk_exact(a, self.k, self.depth)
         return self
 
     @staticmethod
@@ -229,6 +231,7 @@ class DesignBatch:
         s.n_members_total, s.n_nodes_total = self.n_members_total, self.n_nodes_total
         s.max_nodes, s.max_members = self.max_nodes, self.max_members
         s.max_w_classes, s.max_h_classes, s.max_z_classes = self.max_w_classes, self.max_h_classes, self.max_z_classes
+        s.walk_exact = int(self.walk_exact)
         s.depth, s.rho, s.g, s.dw = self.depth, self.rho, self.g, self.dw
         for name in ("w", "k", "member_offset", "mem_frame", "mem_rA", "mem_arm", "mem_node_start", "mem_circ",
                      "node_ls", "node_cd_q", "node_cd_p1", "node_cd_p2", "node_in_q", "node_in_p1", "node_in_p2",
@@ -479,6 +482,34 @@ def solve_dynamics_farm_batch(batch, cases, n_fowt, C_arr=None, M_arr=None, B_ar
 
 FLAG_NAN, FLAG_SINGULAR, FLAG_PLAN, FLAG_XCHG = 1, 2, 4, 8        # include/raftk.h RAFTK_FLAG_*
 STEP_RTOL, STEP_ZERO, Z0_RTOL = 5e-14, 1e-14, 1e-12                # step-class tolerances (csrc/raftk_common.cuh)
+DEEP_KH = 89.4                 # depth_funcs' deep-water branch (helpers.py:211)
+WALK_SEED_EXP = 700.0          # deep-water seed exp(k z0) stays a normal double: e^-700 > DBL_MIN = e^-708.4
+WALK_DOWN_EXP = 10.0           # a downward walk grows its seed's rounding by e^(k drop): e^10 * 2^-53 = 2.4e-12
+
+
+def fused_walk_exact(a, k, depth):
+    """Whether the fused solvers' node walk (DESIGN.md section 4) is exact for every member of the CSR tables ``a`` on the
+    wave numbers ``k`` at water depth ``depth``.  The walk seeds a member's depth factors at its first submerged node z0,
+    (C+S)/2 and (C-S)/2, and multiplies them by exp(+-k dz) per step.  It is inexact where
+      - a deep-water bin (k h > 89.4) has k |z0| > WALK_SEED_EXP: the seed exp(k z0) is subnormal or zero, and so is every
+        node of the member, the surface ones included;
+      - a finite-depth bin has k (z0 - z_min) > WALK_DOWN_EXP on a member that walks down from z0: (C-S)/2 is the
+        difference of two nearly equal numbers there, and its rounding grows by exp(k dz) at every step down.
+    The planner sends inexact designs to the v1 solver, which evaluates depth_funcs at every node."""
+    k = np.asarray(k, dtype=_F8)
+    start = np.asarray(a["mem_node_start"], dtype=np.int64)
+    cnt = np.diff(start)
+    if not len(cnt) or not cnt.sum() or not np.any(k > 0):
+        return True
+    frame, rA, ls = (np.asarray(a[n], dtype=_F8) for n in ("mem_frame", "mem_rA", "node_ls"))
+    mem = np.repeat(np.arange(len(cnt)), cnt)
+    z = rA[mem, 2] + ls * frame[mem, 2]
+    full = cnt > 0
+    z0 = z[start[:-1][full]]
+    drop = z0 - np.minimum.reduceat(z, start[:-1][full])
+    deep = k * depth > DEEP_KH
+    k_deep, k_fin = (float(k[m].max()) if np.any(m) else 0.0 for m in (deep, ~deep))
+    return bool(k_deep * max(0.0, -float(z0.min())) <= WALK_SEED_EXP and k_fin * float(drop.max()) <= WALK_DOWN_EXP)
 
 
 def raise_on_flags(status):
