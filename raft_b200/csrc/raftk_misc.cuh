@@ -10,6 +10,37 @@
 // A "group" of gsize threads (a warp when WARP, else the whole CTA) works on one system; gtid is the thread's index in it.
 template <bool WARP> __device__ __forceinline__ void gsync() { if (WARP) __syncwarp(); else __syncthreads(); }
 
+// Pivot reciprocals and back-substitution quotients are formed at the pivot's own scale: p is multiplied by sc = 2^-e, e the
+// binary exponent of max(|re|, |im|), before |p|^2 is taken, and the result by sc again.  |p|^2 alone overflows above
+// |p| ~ 1.3e154 (a zero reciprocal: nothing eliminated) and underflows below 1.5e-154 (a false zero pivot).  Power-of-two
+// scaling is exact, so wherever the unscaled formula stayed in the normal range the bits are the same.  sc is built from the
+// exponent field, clamped to [1, 2045] so that it stays a normal double (a subnormal or zero pivot takes 2^1022, one at or
+// above 2^1022 takes 2^-1022); a zero pivot still gives |q|^2 = 0, and inf / NaN go through as before.
+__device__ __forceinline__ double piv_scale(const double2 p)
+{
+    const int eb = min(max((__double2hiint(fmax(fabs(p.x), fabs(p.y))) >> 20) & 0x7ff, 1), 2045);
+    return __hiloint2double((2046 - eb) << 20, 0);
+}
+
+// 1 / p, and 0 for a zero pivot (zero set)
+__device__ __forceinline__ double2 piv_recip(const double2 p, bool &zero)
+{
+    const double sc = piv_scale(p);
+    const double2 q = make_double2(p.x * sc, p.y * sc);
+    const double den = q.x * q.x + q.y * q.y;
+    zero = !(den > 0.0);
+    return zero ? make_double2(0.0, 0.0) : make_double2(q.x / den * sc, -q.y / den * sc);
+}
+
+// s / p
+__device__ __forceinline__ double2 piv_div(const double2 s, const double2 p)
+{
+    const double sc = piv_scale(p);
+    const double2 q = make_double2(p.x * sc, p.y * sc);
+    const double den = q.x * q.x + q.y * q.y;
+    return make_double2((s.x * q.x + s.y * q.y) / den * sc, (s.y * q.x - s.x * q.y) / den * sc);
+}
+
 // one elimination step on column col: pivot search over rows col..n-1, swap of the full rows, multipliers.  Returns via *bad.
 template <bool WARP>
 __device__ __forceinline__ void lu_pivot_step(double2 *A, int n, int nc, int col, int gtid, int gsize, int *piv_s, double2 *rinv_s, int *bad_s)
@@ -27,10 +58,9 @@ __device__ __forceinline__ void lu_pivot_step(double2 *A, int n, int nc, int col
         }
         if (gtid == 0) {
             *piv_s = p;
-            const double2 pv = A[p * nc + col];
-            const double den = pv.x * pv.x + pv.y * pv.y;
-            *rinv_s = (den > 0.0) ? make_double2(pv.x / den, -pv.y / den) : make_double2(0.0, 0.0);
-            if (!(den > 0.0) && *bad_s == 0) *bad_s = col + 1;
+            bool zero;
+            *rinv_s = piv_recip(A[p * nc + col], zero);
+            if (zero && *bad_s == 0) *bad_s = col + 1;
         }
     }
     gsync<WARP>();
@@ -51,11 +81,7 @@ __device__ __forceinline__ void lu_back_subst(double2 *A, int n, int nc, int nrh
 {
     for (int r = n - 1; r >= 0; r--) {
         const double2 pv = A[r * nc + r];
-        const double den = pv.x * pv.x + pv.y * pv.y;
-        for (int rh = gtid; rh < nrhs; rh += gsize) {
-            const double2 s = A[r * nc + n + rh];
-            A[r * nc + n + rh] = make_double2((s.x * pv.x + s.y * pv.y) / den, (s.y * pv.x - s.x * pv.y) / den);
-        }
+        for (int rh = gtid; rh < nrhs; rh += gsize) A[r * nc + n + rh] = piv_div(A[r * nc + n + rh], pv);
         gsync<WARP>();
         for (int t = gtid; t < r * nrhs; t += gsize) {
             const int rr = t / nrhs, rh = t - rr * nrhs;
@@ -327,11 +353,10 @@ __device__ __forceinline__ void lu_global(double2 *A, int lda, double2 *B, int l
             best = S.best[0]; p = S.idx[0];                            // every thread finishes the reduction: same winner everywhere
 #pragma unroll
             for (int q = 1; q < GLU_T / 32; q++) if (S.best[q] > best || (S.best[q] == best && S.idx[q] < p)) { best = S.best[q]; p = S.idx[q]; }
-            const double2 pv = Ps[p * pw + j];
-            const double den = pv.x * pv.x + pv.y * pv.y;
-            const double2 ri = (den > 0.0) ? make_double2(pv.x / den, -pv.y / den) : make_double2(0.0, 0.0);
+            bool zero;
+            const double2 ri = piv_recip(Ps[p * pw + j], zero);
             __syncthreads();                                           // pivot and reduction slots read by all before they change
-            if (tid == 0) { S.piv[j] = p; if (!(den > 0.0) && S.bad == 0) S.bad = kb + j + 1; }
+            if (tid == 0) { S.piv[j] = p; if (zero && S.bad == 0) S.bad = kb + j + 1; }
             if (p != j && tid < nb) { const double2 t1 = Ps[j * pw + tid]; Ps[j * pw + tid] = Ps[p * pw + tid]; Ps[p * pw + tid] = t1; }
             __syncthreads();
             for (int r = j + 1 + tid; r < m; r += GLU_T) {             // multiplier, then the panel's columns right of j
@@ -395,11 +420,7 @@ __device__ __forceinline__ void lu_global(double2 *A, int lda, double2 *B, int l
     // ---- back substitution, every right-hand side ------------------------------------------------------------------
     for (int r = n - 1; r >= 0; r--) {
         const double2 pv = A[(size_t)r * lda + r];
-        const double den = pv.x * pv.x + pv.y * pv.y;
-        for (int rh = tid; rh < nrhs; rh += GLU_T) {
-            const double2 s = B[(size_t)r * ldb + rh];
-            B[(size_t)r * ldb + rh] = make_double2((s.x * pv.x + s.y * pv.y) / den, (s.y * pv.x - s.x * pv.y) / den);
-        }
+        for (int rh = tid; rh < nrhs; rh += GLU_T) B[(size_t)r * ldb + rh] = piv_div(B[(size_t)r * ldb + rh], pv);
         __syncthreads();
         for (int t = tid; t < r * nrhs; t += GLU_T) {
             const int rr = t / nrhs, rh = t - rr * nrhs;
@@ -521,9 +542,12 @@ __global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, Fa
             if (r == p) { piv[j] = row[j]; row[j] = t; }
             else { piv[j] = t; if (r == k) row[j] = t; }
         });
-        const double den = piv[k].x * piv[k].x + piv[k].y * piv[k].y;
+        // 1 / p at the pivot's scale (piv_recip), one division per step: q = p sc, 1 / |q|^2 times sc, times q
+        const double sc = piv_scale(piv[k]);
+        const double2 q = make_double2(piv[k].x * sc, piv[k].y * sc);
+        const double den = q.x * q.x + q.y * q.y;
         double2 ri = make_double2(0.0, 0.0);
-        if (den > 0.0) { const double inv = 1.0 / den; ri = make_double2(piv[k].x * inv, -piv[k].y * inv); }      // one division per step
+        if (den > 0.0) { const double inv = 1.0 / den * sc; ri = make_double2(q.x * inv, -q.y * inv); }
         else if (bad == 0) bad = k + 1;
         if (r == k) myinv = ri;                          // 1 / U_kk stays with row k for the back substitution
         if (row_ok && r > k) {
