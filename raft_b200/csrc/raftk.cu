@@ -1493,7 +1493,8 @@ static int validate_gen_qtf(const raftk_general *g, const raftk_general_qtf *q, 
     return 0;
 }
 
-// raftk_general_fd checks on host copies of fd_idx and bem_headings (include/raftk.h)
+// raftk_general_fd checks (include/raftk.h); idx, hd: host copies of fd_idx and bem_headings, read only once the counts and
+// pointers have passed (both NULL: those checks alone)
 static int validate_gen_fd(const raftk_general *g, const raftk_general_fd *fd, const int32_t *idx, const double *hd)
 {
     if (fd->n_fd < 0 || fd->n_fd > g->n_dof) return set_err(RAFTK_EINVAL, "general solve: fd.n_fd must be in [0, n_dof]");
@@ -1502,6 +1503,7 @@ static int validate_gen_fd(const raftk_general *g, const raftk_general_fd *fd, c
         return set_err(RAFTK_EINVAL, "general solve: fd.n_fd > 0 needs fd_idx, A_w and B_w");
     if (fd->n_bem_head > 0 && (!fd->bem_headings || !fd->X_BEM || !fd->T0))
         return set_err(RAFTK_EINVAL, "general solve: fd.n_bem_head > 0 needs bem_headings, X_BEM and T0");
+    if (!idx && !hd) return 0;
     for (int t = 0; t < fd->n_fd; t++) {
         if (idx[t] < 0 || idx[t] >= g->n_dof) return set_err(RAFTK_EINVAL, "general solve: fd.fd_idx entry out of range [0, n_dof)");
         if (t > 0 && idx[t] <= idx[t - 1]) return set_err(RAFTK_EINVAL, "general solve: fd.fd_idx must be strictly increasing (no repeats)");
@@ -1546,41 +1548,6 @@ extern "C" size_t raftk_general_fd_workspace_bytes(const raftk_general *g, const
 extern "C" size_t raftk_general_workspace_bytes(const raftk_general *g, int32_t n_cases)
 {
     return raftk_general_fd_workspace_bytes(g, nullptr, n_cases);
-}
-
-// checks of the generalised-DOF entry points, before any launch; max_cases: the most cases the call takes (65535 for one
-// launch grid, any count when the call streams the table in chunks)
-static int gen_validate(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf, const raftk_cases *c,
-                        const raftk_solve_opts *o, const double *Xi, const int32_t *status, int64_t max_cases, cudaStream_t st)
-{
-    if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
-    if (g->n_dof <= 0 || g->n_dof > 256 || g->nw <= 0 || g->n_nodes < 0 || c->n_cases <= 0 || c->n_cases > max_cases)
-        return set_err(RAFTK_EINVAL, max_cases == 65535 ? "general solve: 0 < n_dof <= 256, nw > 0, 0 < n_cases <= 65535"
-                                                        : "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
-    if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
-    if (int rc = validate_gen_op(fd, c, nullptr, nullptr)) return rc;
-    if (qtf) {                                         // the frequency and heading vectors are read back for the checks
-        if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
-        std::vector<double> qw(qtf->n_qtf_w), qh(qtf->n_qtf_head);
-        CUDA_TRY(cudaMemcpyAsync(qw.data(), qtf->qtf_w, qw.size() * 8, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaMemcpyAsync(qh.data(), qtf->qtf_heads, qh.size() * 8, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        if (int rc = validate_gen_qtf(g, qtf, qw.data(), qh.data())) return rc;
-    }
-    if (fd) {                                          // the index and heading tables (and cases.op) are read back for the checks
-        if (fd->n_fd < 0 || fd->n_fd > g->n_dof || fd->n_bem_head < 0 || (fd->n_fd > 0 && !fd->fd_idx) || (fd->n_bem_head > 0 && !fd->bem_headings))
-            return validate_gen_fd(g, fd, nullptr, nullptr);
-        std::vector<int32_t> idx(fd->n_fd), hop(c->op ? c->n_cases : 0), hprim(c->op && c->primary ? c->n_cases : 0);
-        std::vector<double> hd(fd->n_bem_head);
-        if (fd->n_fd > 0) CUDA_TRY(cudaMemcpyAsync(idx.data(), fd->fd_idx, idx.size() * 4, cudaMemcpyDeviceToHost, st));
-        if (fd->n_bem_head > 0) CUDA_TRY(cudaMemcpyAsync(hd.data(), fd->bem_headings, hd.size() * 8, cudaMemcpyDeviceToHost, st));
-        if (!hop.empty()) CUDA_TRY(cudaMemcpyAsync(hop.data(), c->op, hop.size() * 4, cudaMemcpyDeviceToHost, st));      // (op: n_fd >= 1)
-        if (!hprim.empty()) CUDA_TRY(cudaMemcpyAsync(hprim.data(), c->primary, hprim.size() * 4, cudaMemcpyDeviceToHost, st));
-        if (fd->n_fd > 0 || fd->n_bem_head > 0) CUDA_TRY(cudaStreamSynchronize(st));
-        if (int rc = validate_gen_fd(g, fd, idx.data(), hd.data())) return rc;
-        if (int rc = validate_gen_op(fd, c, hop.data(), hprim.empty() ? nullptr : hprim.data())) return rc;
-    }
-    return 0;
 }
 
 // A design batch as the launch sequence sees it.  nD = 1 with node_off = NULL is one design: the single-design entries run as
@@ -1735,100 +1702,6 @@ static int gen_launch(const raftk_general *g, const GenBatch &Bt, const raftk_ge
     return RAFTK_OK;
 }
 
-extern "C" int raftk_general_solve_dynamics_qtf_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
-                                                    const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
-                                                    double *F_BEM, double *F_2nd, double *F_2nd_mean, void *workspace,
-                                                    size_t workspace_bytes, void *stream)
-{
-    disp_reset();
-    cudaStream_t st = (cudaStream_t)stream;
-    if (int rc = gen_validate(g, fd, qtf, c, o, Xi, status, 65535, st)) return rc;
-    if (!workspace || workspace_bytes < gen_layout(g, fd, qtf, c->n_cases, g->n_nodes).total) return set_err(RAFTK_ENOMEM, "general solve: workspace too small");
-    return gen_launch(g, gen_single(g), fd, qtf, c, 0, c->n_cases, c->primary, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, st, true);
-}
-
-extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
-                                                   const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM,
-                                                   void *workspace, size_t workspace_bytes, void *stream)
-{
-    return raftk_general_solve_dynamics_qtf_dev(g, fd, nullptr, c, o, Xi, status, F_BEM, nullptr, nullptr, workspace, workspace_bytes, stream);
-}
-
-extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
-                                                int32_t *status, void *workspace, size_t workspace_bytes, void *stream)
-{
-    return raftk_general_solve_dynamics_fd_dev(g, nullptr, c, o, Xi, status, nullptr, workspace, workspace_bytes, stream);
-}
-
-extern "C" int raftk_general_solve_dynamics_qtf_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
-                                                     const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
-                                                     double *F_BEM, double *F_2nd, double *F_2nd_mean)
-{
-    disp_reset();
-    if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
-    if (g->n_dof <= 0 || g->nw <= 0 || c->n_cases <= 0) return set_err(RAFTK_EINVAL, "general solve: empty problem");
-    const size_t n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases;
-    if (c->primary)
-        for (size_t i = 0; i < nC; i++) {
-            const int p = c->primary[i];
-            if (p < 0 || (size_t)p >= nC || c->primary[p] != p) return set_err(RAFTK_EINVAL, "general solve: cases.primary must map every case to a primary case");
-        }
-    if (fd)
-        if (int rc = validate_gen_fd(g, fd, fd->fd_idx, fd->bem_headings)) return rc;
-    if (int rc = validate_gen_op(fd, c, c->op, c->primary)) return rc;
-    if (qtf) {
-        if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
-        if (int rc = validate_gen_qtf(g, qtf, qtf->qtf_w, qtf->qtf_heads)) return rc;
-    }
-    Staging S(qtf ? "raftk_general_solve_dynamics_qtf_host" : "raftk_general_solve_dynamics_fd_host");
-    raftk_general gg = *g;
-    S.in(gg.w, g->w, nw); S.in(gg.k, g->k, nw);
-    S.in(gg.node_r, g->node_r, Ns * 3); S.in(gg.node_frame, g->node_frame, Ns * 9);
-    S.in(gg.node_circ, g->node_circ, Ns); S.in(gg.node_Imat, g->node_Imat, Ns * 9);
-    S.in(gg.node_Imat_w, g->node_Imat_w, Ns * 9 * nw * 2); S.in(gg.node_a_i, g->node_a_i, Ns);
-    S.in(gg.node_cd, g->node_cd, Ns * 4); S.in(gg.Tn, g->Tn, Ns * 6 * n); S.in(gg.rr, g->rr, Ns * 3);
-    S.in(gg.M, g->M, n * n); S.in(gg.B, g->B, n * n); S.in(gg.C, g->C, n * n);
-    raftk_cases cc = *c;
-    S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
-    S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC); S.in(cc.zeta, c->zeta, nC * nw);
-    S.in(cc.primary, c->primary, nC);
-    if (c->op) { S.in(cc.op, c->op, nC); S.in(cc.op_A_w, c->op_A_w, gen_op_elems(fd, c, 1, nw)); S.in(cc.op_B_w, c->op_B_w, gen_op_elems(fd, c, 1, nw)); }
-    raftk_general_fd ff = fd ? *fd : raftk_general_fd{};
-    if (fd) {
-        const size_t nf = fd->n_fd, nh = fd->n_bem_head;             // validate_gen_fd: both >= 0
-        S.in(ff.fd_idx, fd->fd_idx, nf); S.in(ff.A_w, fd->A_w, nf * nf * nw); S.in(ff.B_w, fd->B_w, nf * nf * nw);
-        S.in(ff.bem_headings, fd->bem_headings, nh); S.in(ff.X_BEM, fd->X_BEM, nh * 6 * nw * 2); S.in(ff.T0, fd->T0, nh ? 6 * n : 0);
-    }
-    raftk_general_qtf qq = qtf ? *qtf : raftk_general_qtf{};
-    if (qtf) {                                                    // validate_gen_qtf: both counts >= 1
-        const size_t n2 = qtf->n_qtf_w, nh = qtf->n_qtf_head;
-        S.in(qq.qtf_w, qtf->qtf_w, n2); S.in(qq.qtf_heads, qtf->qtf_heads, nh); S.in(qq.qtf, qtf->qtf, n2 * n2 * nh * 12);
-    }
-    double *dXi, *dF_BEM, *dF2, *dF2m;
-    int32_t *dStatus;
-    char *ws;
-    const size_t wb = raftk_general_qtf_workspace_bytes(g, fd, qtf, (int32_t)nC);
-    S.out(dXi, nC * n * nw * 2, Xi); S.out(dStatus, nC * 4, status); S.out(dF_BEM, F_BEM ? nC * n * nw * 2 : 0, F_BEM);
-    S.out(dF2, qtf && F_2nd ? nC * 6 * nw : 0, F_2nd); S.out(dF2m, qtf && F_2nd_mean ? nC * 6 : 0, F_2nd_mean);
-    S.buf(ws, wb);
-    int rc = S.commit();
-    if (rc || (rc = raftk_general_solve_dynamics_qtf_dev(&gg, fd ? &ff : nullptr, qtf ? &qq : nullptr, &cc, o, dXi, dStatus, dF_BEM, dF2, dF2m,
-                                                         ws, wb, nullptr))) return rc;
-    return S.finish();
-}
-
-extern "C" int raftk_general_solve_dynamics_fd_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
-                                                    const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM)
-{
-    return raftk_general_solve_dynamics_qtf_host(g, fd, nullptr, c, o, Xi, status, F_BEM, nullptr, nullptr);
-}
-
-extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
-                                                 int32_t *status)
-{
-    return raftk_general_solve_dynamics_fd_host(g, nullptr, c, o, Xi, status, nullptr);
-}
-
 // ---- generalised DOFs, streamed: the units in chunks of whole train groups through one bounded workspace ---------------
 static size_t gen_chunk_cap(int64_t n_units, int32_t max_chunk)
 {
@@ -1928,83 +1801,6 @@ static int gen_run(const raftk_general *g, const GenBatch &Bt, const raftk_gener
     return RAFTK_OK;
 }
 
-extern "C" int raftk_general_solve_dynamics_stream_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
-                                                       const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
-                                                       double *F_BEM, double *F_2nd, double *F_2nd_mean, void *workspace,
-                                                       size_t workspace_bytes, int32_t max_chunk_cases, void *stream)
-{
-    disp_reset();
-    cudaStream_t st = (cudaStream_t)stream;
-    if (int rc = gen_validate(g, fd, qtf, c, o, Xi, status, INT32_MAX, st)) return rc;
-    if (max_chunk_cases < 0) return set_err(RAFTK_EINVAL, "general stream: max_chunk_cases must be >= 0 (0: all cases)");
-    std::vector<int32_t> hp;
-    if (c->primary) {                                  // the primary map is read back once to plan the chunks
-        hp.resize(c->n_cases);
-        CUDA_TRY(cudaMemcpyAsync(hp.data(), c->primary, hp.size() * 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-    }
-    return gen_run(g, gen_single(g), fd, qtf, c, c->primary ? hp.data() : nullptr, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace,
-                   workspace_bytes, max_chunk_cases, false, st);
-}
-
-extern "C" int raftk_general_solve_dynamics_stream_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
-                                                        const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
-                                                        double *F_BEM, double *F_2nd, double *F_2nd_mean, int32_t max_chunk_cases)
-{
-    disp_reset();
-    if (!g || !c || !o || !Xi || !status) return set_err(RAFTK_EINVAL, "general solve: null argument");
-    if (g->n_dof <= 0 || g->nw <= 0 || c->n_cases <= 0) return set_err(RAFTK_EINVAL, "general solve: empty problem");
-    if (max_chunk_cases < 0) return set_err(RAFTK_EINVAL, "general stream: max_chunk_cases must be >= 0 (0: all cases)");
-    if (g->n_dof > 256 || g->n_nodes < 0) return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
-    if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
-    const size_t n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases, K = gen_chunk_cap(c->n_cases, max_chunk_cases);
-    if (K > 65535) return set_err(RAFTK_EINVAL, "general stream: a chunk takes at most 65535 cases (max_chunk_cases)");
-    std::vector<size_t> starts;                        // the plan's checks, before anything is staged
-    if (int rc = gen_plan_chunks(c->primary, nC, 1, K, false, starts)) return rc;
-    if (fd)
-        if (int rc = validate_gen_fd(g, fd, fd->fd_idx, fd->bem_headings)) return rc;
-    if (int rc = validate_gen_op(fd, c, c->op, c->primary)) return rc;
-    if (qtf) {
-        if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
-        if (int rc = validate_gen_qtf(g, qtf, qtf->qtf_w, qtf->qtf_heads)) return rc;
-    }
-    Staging S("raftk_general_solve_dynamics_stream_host");
-    raftk_general gg = *g;
-    S.in(gg.w, g->w, nw); S.in(gg.k, g->k, nw);
-    S.in(gg.node_r, g->node_r, Ns * 3); S.in(gg.node_frame, g->node_frame, Ns * 9);
-    S.in(gg.node_circ, g->node_circ, Ns); S.in(gg.node_Imat, g->node_Imat, Ns * 9);
-    S.in(gg.node_Imat_w, g->node_Imat_w, Ns * 9 * nw * 2); S.in(gg.node_a_i, g->node_a_i, Ns);
-    S.in(gg.node_cd, g->node_cd, Ns * 4); S.in(gg.Tn, g->Tn, Ns * 6 * n); S.in(gg.rr, g->rr, Ns * 3);
-    S.in(gg.M, g->M, n * n); S.in(gg.B, g->B, n * n); S.in(gg.C, g->C, n * n);
-    raftk_cases cc = *c;
-    S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
-    S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC); S.in(cc.zeta, c->zeta, nC * nw);
-    S.in(cc.primary, c->primary, nC);
-    if (c->op) { S.in(cc.op, c->op, nC); S.in(cc.op_A_w, c->op_A_w, gen_op_elems(fd, c, 1, nw)); S.in(cc.op_B_w, c->op_B_w, gen_op_elems(fd, c, 1, nw)); }
-    raftk_general_fd ff = fd ? *fd : raftk_general_fd{};
-    if (fd) {
-        const size_t nf = fd->n_fd, nh = fd->n_bem_head;
-        S.in(ff.fd_idx, fd->fd_idx, nf); S.in(ff.A_w, fd->A_w, nf * nf * nw); S.in(ff.B_w, fd->B_w, nf * nf * nw);
-        S.in(ff.bem_headings, fd->bem_headings, nh); S.in(ff.X_BEM, fd->X_BEM, nh * 6 * nw * 2); S.in(ff.T0, fd->T0, nh ? 6 * n : 0);
-    }
-    raftk_general_qtf qq = qtf ? *qtf : raftk_general_qtf{};
-    if (qtf) {
-        const size_t n2 = qtf->n_qtf_w, nh = qtf->n_qtf_head;
-        S.in(qq.qtf_w, qtf->qtf_w, n2); S.in(qq.qtf_heads, qtf->qtf_heads, nh); S.in(qq.qtf, qtf->qtf, n2 * n2 * nh * 12);
-    }
-    double *dXi, *dF_BEM, *dF2, *dF2m;
-    int32_t *dStatus;
-    char *ws;
-    const size_t wb = raftk_general_stream_workspace_bytes(g, fd, qtf, c->n_cases, max_chunk_cases);
-    S.out(dXi, nC * n * nw * 2, Xi); S.out(dStatus, nC * 4, status); S.out(dF_BEM, F_BEM ? nC * n * nw * 2 : 0, F_BEM);
-    S.out(dF2, qtf && F_2nd ? nC * 6 * nw : 0, F_2nd); S.out(dF2m, qtf && F_2nd_mean ? nC * 6 : 0, F_2nd_mean);
-    S.buf(ws, wb);
-    int rc = S.commit();
-    if (rc || (rc = gen_run(&gg, gen_single(&gg), fd ? &ff : nullptr, qtf ? &qq : nullptr, &cc, c->primary, o, dXi, dStatus, dF_BEM, dF2, dF2m, ws,
-                            wb, max_chunk_cases, false, nullptr))) return rc;
-    return S.finish();
-}
-
 // ---- generalised DOFs, design batches: designs sharing n_dof, the frequency grid, depth and rho ------------------------
 static GenBatch gen_batch_of(const raftk_general_batch *b)
 {
@@ -2012,48 +1808,6 @@ static GenBatch gen_batch_of(const raftk_general_batch *b)
     B.nD = b->n_designs; B.max_nodes = b->max_nodes; B.qtf_shared = b->qtf_shared;
     B.node_off = b->node_offset; B.x_ref = b->x_ref; B.y_ref = b->y_ref; B.hadj = b->heading_adjust;
     return B;
-}
-
-// checks on counts and pointers, before anything is read back or staged
-static int gen_batch_counts(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
-                            const raftk_cases *c, const raftk_solve_opts *o, const double *Xi, const int32_t *status, int32_t max_chunk_units)
-{
-    if (!g || !b || !c || !o || !Xi || !status || !b->node_offset) return set_err(RAFTK_EINVAL, "general batch: null argument");
-    if (b->n_designs <= 0 || b->max_nodes < 0) return set_err(RAFTK_EINVAL, "general batch: n_designs > 0 and max_nodes >= 0");
-    if (g->n_dof <= 0 || g->n_dof > 256 || g->nw <= 0 || g->n_nodes < 0 || c->n_cases <= 0)
-        return set_err(RAFTK_EINVAL, "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
-    if ((int64_t)b->n_designs * c->n_cases > INT32_MAX) return set_err(RAFTK_EINVAL, "general batch: n_designs * n_cases must stay below 2^31");
-    if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
-    if (int rc = validate_gen_op(fd, c, nullptr, nullptr)) return rc;
-    if (max_chunk_units < 0) return set_err(RAFTK_EINVAL, "general batch: max_chunk_units must be >= 0 (0: all units)");
-    if (gen_chunk_cap((int64_t)b->n_designs * c->n_cases, max_chunk_units) > 65535)
-        return set_err(RAFTK_EINVAL, "general batch: a chunk takes at most 65535 units (max_chunk_units)");
-    if (b->qtf_shared < 0 || b->qtf_shared > 1) return set_err(RAFTK_EINVAL, "general batch: qtf_shared must be 0 or 1");
-    if (qtf)
-        if (int rc = validate_gen_qtf(g, qtf, nullptr, nullptr)) return rc;
-    if (fd && (fd->n_fd < 0 || fd->n_fd > g->n_dof || fd->n_bem_head < 0 || (fd->n_fd > 0 && (!fd->fd_idx || !fd->A_w || !fd->B_w)) ||
-               (fd->n_bem_head > 0 && (!fd->bem_headings || !fd->X_BEM || !fd->T0))))
-        return validate_gen_fd(g, fd, nullptr, nullptr);
-    return 0;
-}
-
-// checks on host copies of node_offset, every design's fd_idx and bem_headings rows, qtf_w and qtf_heads
-static int gen_batch_tables(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
-                            const int32_t *off, const int32_t *idx, const double *hd, const double *qw, const double *qh)
-{
-    const int nD = b->n_designs;
-    if (off[0] != 0) return set_err(RAFTK_EINVAL, "general batch: node_offset must start at 0");
-    for (int d = 0; d < nD; d++) {
-        if (off[d + 1] < off[d]) return set_err(RAFTK_EINVAL, "general batch: node_offset must be non-decreasing");
-        if (off[d + 1] - off[d] > b->max_nodes) return set_err(RAFTK_EINVAL, "general batch: a design has more nodes than max_nodes");
-    }
-    if (off[nD] != g->n_nodes) return set_err(RAFTK_EINVAL, "general batch: node_offset[n_designs] must equal n_nodes");
-    if (fd)
-        for (int d = 0; d < nD; d++)
-            if (int rc = validate_gen_fd(g, fd, idx + (size_t)d * fd->n_fd, hd + (size_t)d * fd->n_bem_head)) return rc;
-    if (qtf)
-        if (int rc = validate_gen_qtf(g, qtf, qw, qh)) return rc;
-    return 0;
 }
 
 extern "C" size_t raftk_general_batch_workspace_bytes(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd,
@@ -2065,33 +1819,290 @@ extern "C" size_t raftk_general_batch_workspace_bytes(const raftk_general *g, co
     return gen_run_bytes(g, gen_batch_of(b), fd, qtf, nU, max_chunk_units, nullptr);
 }
 
+// ---- generalised DOFs, the entry points: one-shot, streamed and design batches through one set of checks, one staging
+// list and one launch path -------------------------------------------------------------------------------------------
+enum GenMode { GEN_ONE_SHOT, GEN_STREAM, GEN_BATCH };
+
+// One call as its entry received it.  b is NULL on the single-design entries, which run as gen_single()'s batch; nD and
+// qtf_shared size the per-design tables (1 and 0 there).
+struct GenCall {
+    const raftk_general *g; const raftk_general_batch *b; const raftk_general_fd *fd; const raftk_general_qtf *qtf; const raftk_cases *c;
+    int nD, qtf_shared;
+};
+
+static GenCall gen_call(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                        const raftk_cases *c)
+{
+    return {g, b, fd, qtf, c, b ? b->n_designs : 1, b ? b->qtf_shared : 0};
+}
+
+// Host copies of the tables the checks and the chunk plan read; NULL: not in the call, or not read back
+struct GenTables { const int32_t *off, *idx; const double *hd, *qw, *qh; const int32_t *op, *prim; };
+
+// The checks that need no table contents, before anything is read back or staged.  The wording follows the entry family:
+// the one-shot entries take at most one launch grid of cases, the stream and batch entries a chunk cap max_chunk.
+static int gen_check_counts(const GenCall &k, GenMode mode, const raftk_solve_opts *o, const double *Xi, const int32_t *status,
+                            int32_t max_chunk)
+{
+    const raftk_general *g = k.g;
+    const raftk_cases *c = k.c;
+    const bool one = mode == GEN_ONE_SHOT, batch = mode == GEN_BATCH;
+    if (!g || !c || !o || !Xi || !status || (batch && (!k.b || !k.b->node_offset)))
+        return set_err(RAFTK_EINVAL, batch ? "general batch: null argument" : "general solve: null argument");
+    if (batch && (k.nD <= 0 || k.b->max_nodes < 0)) return set_err(RAFTK_EINVAL, "general batch: n_designs > 0 and max_nodes >= 0");
+    if (g->n_dof <= 0 || g->n_dof > 256 || g->nw <= 0 || g->n_nodes < 0 || c->n_cases <= 0 || (one && c->n_cases > 65535))
+        return set_err(RAFTK_EINVAL, one ? "general solve: 0 < n_dof <= 256, nw > 0, 0 < n_cases <= 65535"
+                                         : "general solve: 0 < n_dof <= 256, nw > 0, n_cases > 0");
+    const int64_t nU = (int64_t)k.nD * c->n_cases;
+    if (nU > INT32_MAX) return set_err(RAFTK_EINVAL, "general batch: n_designs * n_cases must stay below 2^31");
+    if (c->F_2nd || c->Xi_init) return set_err(RAFTK_EINVAL, "general solve: F_2nd / Xi_init are not supported");
+    if (int rc = validate_gen_op(k.fd, c, nullptr, nullptr)) return rc;
+    if (!one && max_chunk < 0)
+        return set_err(RAFTK_EINVAL, batch ? "general batch: max_chunk_units must be >= 0 (0: all units)"
+                                           : "general stream: max_chunk_cases must be >= 0 (0: all cases)");
+    if (!one && gen_chunk_cap(nU, max_chunk) > 65535)
+        return set_err(RAFTK_EINVAL, batch ? "general batch: a chunk takes at most 65535 units (max_chunk_units)"
+                                           : "general stream: a chunk takes at most 65535 cases (max_chunk_cases)");
+    if (k.qtf_shared < 0 || k.qtf_shared > 1) return set_err(RAFTK_EINVAL, "general batch: qtf_shared must be 0 or 1");
+    if (k.qtf)
+        if (int rc = validate_gen_qtf(g, k.qtf, nullptr, nullptr)) return rc;
+    return k.fd ? validate_gen_fd(g, k.fd, nullptr, nullptr) : 0;
+}
+
+// The checks on table contents, on host copies t of a call that passed gen_check_counts: node_offset, every design's fd_idx
+// and bem_headings rows, the QTF grid, cases.op and, when t holds it, that every case maps to a case that is its own primary.
+// The chunk plan's own rule (each train group contiguous in the table) stays with gen_plan_chunks.
+static int gen_check_tables(const GenCall &k, const GenTables &t)
+{
+    const raftk_general *g = k.g;
+    const int nD = k.nD, nC = k.c->n_cases;
+    if (const int32_t *off = t.off) {                  // (a design batch)
+        if (off[0] != 0) return set_err(RAFTK_EINVAL, "general batch: node_offset must start at 0");
+        for (int d = 0; d < nD; d++) {
+            if (off[d + 1] < off[d]) return set_err(RAFTK_EINVAL, "general batch: node_offset must be non-decreasing");
+            if (off[d + 1] - off[d] > k.b->max_nodes) return set_err(RAFTK_EINVAL, "general batch: a design has more nodes than max_nodes");
+        }
+        if (off[nD] != g->n_nodes) return set_err(RAFTK_EINVAL, "general batch: node_offset[n_designs] must equal n_nodes");
+    }
+    if (k.fd)
+        for (int d = 0; d < nD; d++)
+            if (int rc = validate_gen_fd(g, k.fd, t.idx + (size_t)d * k.fd->n_fd, t.hd + (size_t)d * k.fd->n_bem_head)) return rc;
+    if (k.qtf)
+        if (int rc = validate_gen_qtf(g, k.qtf, t.qw, t.qh)) return rc;
+    if (int rc = validate_gen_op(k.fd, k.c, t.op, t.prim)) return rc;
+    if (t.prim)
+        for (int i = 0; i < nC; i++) {
+            const int p = t.prim[i];
+            if (p < 0 || p >= nC || t.prim[p] != p) return set_err(RAFTK_EINVAL, "general solve: cases.primary must map every case to a primary case");
+        }
+    return 0;
+}
+
+// The tables a *_dev call's checks read, copied back with one wait (none when there is nothing to read).  cases.primary is read
+// when the chunk plan needs it (primary) or cases.op is checked against it.
+struct GenReadback { std::vector<int32_t> off, idx, op, prim; std::vector<double> hd, qw, qh; GenTables t{}; };
+
+static int gen_read_back(const GenCall &k, bool primary, cudaStream_t st, GenReadback &r)
+{
+    const raftk_general_fd *fd = k.fd;
+    const raftk_general_qtf *q = k.qtf;
+    const raftk_cases *c = k.c;
+    const size_t nD = k.nD, nC = c->n_cases;
+    cudaError_t e = cudaSuccess;
+    auto back = [&](auto &v, const auto *d, size_t n) -> decltype(d) {
+        if (!d || !n) return nullptr;
+        v.resize(n);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(v.data(), d, n * sizeof(v[0]), cudaMemcpyDeviceToHost, st);
+        return v.data();
+    };
+    r.t.off = back(r.off, k.b ? k.b->node_offset : nullptr, nD + 1);
+    r.t.idx = back(r.idx, fd ? fd->fd_idx : nullptr, fd ? nD * fd->n_fd : 0);
+    r.t.hd = back(r.hd, fd ? fd->bem_headings : nullptr, fd ? nD * fd->n_bem_head : 0);
+    r.t.qw = back(r.qw, q ? q->qtf_w : nullptr, q ? q->n_qtf_w : 0);
+    r.t.qh = back(r.qh, q ? q->qtf_heads : nullptr, q ? q->n_qtf_head : 0);
+    r.t.op = back(r.op, c->op, nC);
+    r.t.prim = back(r.prim, primary || c->op ? c->primary : nullptr, nC);
+    if (e == cudaSuccess && (r.t.off || r.t.idx || r.t.hd || r.t.qw || r.t.op || r.t.prim)) e = cudaStreamSynchronize(st);
+    return e == cudaSuccess ? 0 : set_err(RAFTK_ECUDA, "general solve: reading the tables back: %s", cudaGetErrorString(e));
+}
+
+// workspace bytes of a checked call
+static size_t gen_ws_bytes(GenMode mode, const GenCall &k, int32_t max_chunk)
+{
+    if (mode == GEN_ONE_SHOT) return gen_layout(k.g, k.fd, k.qtf, k.c->n_cases, k.g->n_nodes).total;
+    return gen_run_bytes(k.g, k.b ? gen_batch_of(k.b) : gen_single(k.g), k.fd, k.qtf, (int64_t)k.nD * k.c->n_cases, max_chunk, nullptr);
+}
+
+// A checked call on device pointers: the one-shot launch sequence, or the chunk loop.  t: host copies of node_offset and
+// cases.primary for the chunks' node grids and plan.
+static int gen_go(GenMode mode, const GenCall &k, const GenTables &t, const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM,
+                  double *F_2nd, double *F_2nd_mean, void *workspace, size_t workspace_bytes, int32_t max_chunk, cudaStream_t st)
+{
+    if (mode == GEN_ONE_SHOT) {
+        if (!workspace || workspace_bytes < gen_ws_bytes(mode, k, 0)) return set_err(RAFTK_ENOMEM, "general solve: workspace too small");
+        return gen_launch(k.g, gen_single(k.g), k.fd, k.qtf, k.c, 0, k.c->n_cases, k.c->primary, o, Xi, status, F_BEM, F_2nd, F_2nd_mean,
+                          workspace, st, true);
+    }
+    GenBatch Bt = k.b ? gen_batch_of(k.b) : gen_single(k.g);
+    Bt.hnode_off = t.off;
+    return gen_run(k.g, Bt, k.fd, k.qtf, k.c, t.prim, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, workspace_bytes, max_chunk,
+                   mode == GEN_BATCH, st);
+}
+
+static int gen_dev(GenMode mode, const GenCall &k, const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM, double *F_2nd,
+                   double *F_2nd_mean, void *workspace, size_t workspace_bytes, int32_t max_chunk, void *stream)
+{
+    disp_reset();
+    cudaStream_t st = (cudaStream_t)stream;
+    GenReadback r;
+    if (int rc = gen_check_counts(k, mode, o, Xi, status, max_chunk)) return rc;
+    if (int rc = gen_read_back(k, mode != GEN_ONE_SHOT, st, r)) return rc;
+    if (int rc = gen_check_tables(k, r.t)) return rc;
+    return gen_go(mode, k, r.t, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, workspace_bytes, max_chunk, st);
+}
+
+// The device side of a *_host call: copies of its structs, whose pointers Staging::commit() turns into device addresses, the
+// five outputs and the workspace
+struct GenStaged {
+    raftk_general g; raftk_general_batch b; raftk_general_fd fd; raftk_general_qtf qtf; raftk_cases c; GenCall k;
+    double *Xi, *F_BEM, *F_2nd, *F_2nd_mean; int32_t *status; char *ws;
+};
+
+// every input of call k (the per-design tables nD deep, the QTF table qtf_shared-deep), the outputs the caller asked for and
+// wb bytes of workspace
+static void gen_stage(Staging &S, const GenCall &k, double *Xi, int32_t *status, double *F_BEM, double *F_2nd, double *F_2nd_mean,
+                      size_t wb, GenStaged &D)
+{
+    const raftk_general *g = k.g;
+    const raftk_general_fd *fd = k.fd;
+    const raftk_general_qtf *q = k.qtf;
+    const raftk_cases *c = k.c;
+    const size_t nD = k.nD, n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases, nU = nD * nC;
+    D.g = *g;
+    S.in(D.g.w, g->w, nw); S.in(D.g.k, g->k, nw);
+    S.in(D.g.node_r, g->node_r, Ns * 3); S.in(D.g.node_frame, g->node_frame, Ns * 9);
+    S.in(D.g.node_circ, g->node_circ, Ns); S.in(D.g.node_Imat, g->node_Imat, Ns * 9);
+    S.in(D.g.node_Imat_w, g->node_Imat_w, Ns * 9 * nw * 2); S.in(D.g.node_a_i, g->node_a_i, Ns);
+    S.in(D.g.node_cd, g->node_cd, Ns * 4); S.in(D.g.Tn, g->Tn, Ns * 6 * n); S.in(D.g.rr, g->rr, Ns * 3);
+    S.in(D.g.M, g->M, nD * n * n); S.in(D.g.B, g->B, nD * n * n); S.in(D.g.C, g->C, nD * n * n);
+    if (k.b) {
+        D.b = *k.b;
+        S.in(D.b.node_offset, k.b->node_offset, nD + 1);
+        S.in(D.b.x_ref, k.b->x_ref, nD); S.in(D.b.y_ref, k.b->y_ref, nD); S.in(D.b.heading_adjust, k.b->heading_adjust, nD);
+    }
+    D.c = *c;
+    S.in(D.c.Hs, c->Hs, nC); S.in(D.c.Tp, c->Tp, nC); S.in(D.c.gamma, c->gamma, nC);
+    S.in(D.c.beta_deg, c->beta_deg, nC); S.in(D.c.spec, c->spec, nC); S.in(D.c.zeta, c->zeta, nC * nw);
+    S.in(D.c.primary, c->primary, nC);
+    if (c->op) { S.in(D.c.op, c->op, nC); S.in(D.c.op_A_w, c->op_A_w, gen_op_elems(fd, c, nD, nw)); S.in(D.c.op_B_w, c->op_B_w, gen_op_elems(fd, c, nD, nw)); }
+    if (fd) {                                          // validate_gen_fd: both counts >= 0
+        const size_t nf = fd->n_fd, nh = fd->n_bem_head;
+        D.fd = *fd;
+        S.in(D.fd.fd_idx, fd->fd_idx, nD * nf); S.in(D.fd.A_w, fd->A_w, nD * nf * nf * nw); S.in(D.fd.B_w, fd->B_w, nD * nf * nf * nw);
+        S.in(D.fd.bem_headings, fd->bem_headings, nD * nh); S.in(D.fd.X_BEM, fd->X_BEM, nD * nh * 6 * nw * 2);
+        S.in(D.fd.T0, fd->T0, nh ? nD * 6 * n : 0);
+    }
+    if (q) {                                           // validate_gen_qtf: both counts >= 1
+        const size_t n2 = q->n_qtf_w, nh = q->n_qtf_head;
+        D.qtf = *q;
+        S.in(D.qtf.qtf_w, q->qtf_w, n2); S.in(D.qtf.qtf_heads, q->qtf_heads, nh);
+        S.in(D.qtf.qtf, q->qtf, (k.qtf_shared ? 1 : nD) * n2 * n2 * nh * 12);
+    }
+    S.out(D.Xi, nU * n * nw * 2, Xi); S.out(D.status, nU * 4, status); S.out(D.F_BEM, F_BEM ? nU * n * nw * 2 : 0, F_BEM);
+    S.out(D.F_2nd, q && F_2nd ? nU * 6 * nw : 0, F_2nd); S.out(D.F_2nd_mean, q && F_2nd_mean ? nU * 6 : 0, F_2nd_mean);
+    S.buf(D.ws, wb);
+    D.k = {&D.g, k.b ? &D.b : nullptr, fd ? &D.fd : nullptr, q ? &D.qtf : nullptr, &D.c, k.nD, k.qtf_shared};
+}
+
+// Every check on the caller's arrays (the stream and batch entries' chunk plan included) before any CUDA call, then one
+// staging, the launch path and one download
+static int gen_host(const char *who, GenMode mode, const GenCall &k, const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM,
+                    double *F_2nd, double *F_2nd_mean, int32_t max_chunk)
+{
+    disp_reset();
+    if (int rc = gen_check_counts(k, mode, o, Xi, status, max_chunk)) return rc;
+    const GenTables t = {k.b ? k.b->node_offset : nullptr, k.fd ? k.fd->fd_idx : nullptr, k.fd ? k.fd->bem_headings : nullptr,
+                         k.qtf ? k.qtf->qtf_w : nullptr, k.qtf ? k.qtf->qtf_heads : nullptr, k.c->op, k.c->primary};
+    if (int rc = gen_check_tables(k, t)) return rc;
+    std::vector<size_t> starts;                        // the chunk plan's checks, before anything is staged
+    const size_t nC = k.c->n_cases;
+    if (mode != GEN_ONE_SHOT)
+        if (int rc = gen_plan_chunks(t.prim, nC, k.nD, gen_chunk_cap((int64_t)k.nD * nC, max_chunk), mode == GEN_BATCH, starts)) return rc;
+    Staging S(who);
+    GenStaged D;
+    const size_t wb = gen_ws_bytes(mode, k, max_chunk);
+    gen_stage(S, k, Xi, status, F_BEM, F_2nd, F_2nd_mean, wb, D);
+    int rc = S.commit();
+    if (rc || (rc = gen_go(mode, D.k, t, o, D.Xi, D.status, D.F_BEM, D.F_2nd, D.F_2nd_mean, D.ws, wb, max_chunk, nullptr))) return rc;
+    return S.finish();
+}
+
+extern "C" int raftk_general_solve_dynamics_qtf_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                                    const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
+                                                    double *F_BEM, double *F_2nd, double *F_2nd_mean, void *workspace,
+                                                    size_t workspace_bytes, void *stream)
+{
+    return gen_dev(GEN_ONE_SHOT, gen_call(g, nullptr, fd, qtf, c), o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, workspace_bytes, 0,
+                   stream);
+}
+
+extern "C" int raftk_general_solve_dynamics_fd_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
+                                                   const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM,
+                                                   void *workspace, size_t workspace_bytes, void *stream)
+{
+    return raftk_general_solve_dynamics_qtf_dev(g, fd, nullptr, c, o, Xi, status, F_BEM, nullptr, nullptr, workspace, workspace_bytes, stream);
+}
+
+extern "C" int raftk_general_solve_dynamics_dev(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
+                                                int32_t *status, void *workspace, size_t workspace_bytes, void *stream)
+{
+    return raftk_general_solve_dynamics_fd_dev(g, nullptr, c, o, Xi, status, nullptr, workspace, workspace_bytes, stream);
+}
+
+extern "C" int raftk_general_solve_dynamics_qtf_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                                     const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
+                                                     double *F_BEM, double *F_2nd, double *F_2nd_mean)
+{
+    return gen_host(qtf ? "raftk_general_solve_dynamics_qtf_host" : "raftk_general_solve_dynamics_fd_host", GEN_ONE_SHOT,
+                    gen_call(g, nullptr, fd, qtf, c), o, Xi, status, F_BEM, F_2nd, F_2nd_mean, 0);
+}
+
+extern "C" int raftk_general_solve_dynamics_fd_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_cases *c,
+                                                    const raftk_solve_opts *o, double *Xi, int32_t *status, double *F_BEM)
+{
+    return raftk_general_solve_dynamics_qtf_host(g, fd, nullptr, c, o, Xi, status, F_BEM, nullptr, nullptr);
+}
+
+extern "C" int raftk_general_solve_dynamics_host(const raftk_general *g, const raftk_cases *c, const raftk_solve_opts *o, double *Xi,
+                                                 int32_t *status)
+{
+    return raftk_general_solve_dynamics_fd_host(g, nullptr, c, o, Xi, status, nullptr);
+}
+
+extern "C" int raftk_general_solve_dynamics_stream_dev(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                                       const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
+                                                       double *F_BEM, double *F_2nd, double *F_2nd_mean, void *workspace,
+                                                       size_t workspace_bytes, int32_t max_chunk_cases, void *stream)
+{
+    return gen_dev(GEN_STREAM, gen_call(g, nullptr, fd, qtf, c), o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, workspace_bytes,
+                   max_chunk_cases, stream);
+}
+
+extern "C" int raftk_general_solve_dynamics_stream_host(const raftk_general *g, const raftk_general_fd *fd, const raftk_general_qtf *qtf,
+                                                        const raftk_cases *c, const raftk_solve_opts *o, double *Xi, int32_t *status,
+                                                        double *F_BEM, double *F_2nd, double *F_2nd_mean, int32_t max_chunk_cases)
+{
+    return gen_host("raftk_general_solve_dynamics_stream_host", GEN_STREAM, gen_call(g, nullptr, fd, qtf, c), o, Xi, status, F_BEM, F_2nd,
+                    F_2nd_mean, max_chunk_cases);
+}
+
 extern "C" int raftk_general_batch_solve_dynamics_dev(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd,
                                                       const raftk_general_qtf *qtf, const raftk_cases *c, const raftk_solve_opts *o,
                                                       double *Xi, int32_t *status, double *F_BEM, double *F_2nd, double *F_2nd_mean,
                                                       void *workspace, size_t workspace_bytes, int32_t max_chunk_units, void *stream)
 {
-    disp_reset();
-    cudaStream_t st = (cudaStream_t)stream;
-    if (int rc = gen_batch_counts(g, b, fd, qtf, c, o, Xi, status, max_chunk_units)) return rc;
-    const size_t nD = b->n_designs, nf = fd ? fd->n_fd : 0, nh = fd ? fd->n_bem_head : 0;
-    // every table the checks and the chunk plan need, read back with one wait
-    std::vector<int32_t> off(nD + 1), hp(c->primary ? c->n_cases : 0), idx(nD * nf), hop(c->op ? c->n_cases : 0);
-    std::vector<double> hd(nD * nh), qw(qtf ? qtf->n_qtf_w : 0), qh(qtf ? qtf->n_qtf_head : 0);
-    auto back = [&](void *h, const void *d, size_t bytes) { return bytes ? cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, st) : cudaSuccess; };
-    CUDA_TRY(back(off.data(), b->node_offset, off.size() * 4));
-    CUDA_TRY(back(hp.data(), c->primary, hp.size() * 4));
-    CUDA_TRY(back(idx.data(), fd ? fd->fd_idx : nullptr, idx.size() * 4));
-    CUDA_TRY(back(hd.data(), fd ? fd->bem_headings : nullptr, hd.size() * 8));
-    CUDA_TRY(back(qw.data(), qtf ? qtf->qtf_w : nullptr, qw.size() * 8));
-    CUDA_TRY(back(qh.data(), qtf ? qtf->qtf_heads : nullptr, qh.size() * 8));
-    CUDA_TRY(back(hop.data(), c->op, hop.size() * 4));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (int rc = gen_batch_tables(g, b, fd, qtf, off.data(), idx.data(), hd.data(), qw.data(), qh.data())) return rc;
-    if (int rc = validate_gen_op(fd, c, hop.data(), c->primary ? hp.data() : nullptr)) return rc;
-    GenBatch Bt = gen_batch_of(b);
-    Bt.hnode_off = off.data();
-    return gen_run(g, Bt, fd, qtf, c, c->primary ? hp.data() : nullptr, o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, workspace_bytes,
-                   max_chunk_units, true, st);
+    return gen_dev(GEN_BATCH, gen_call(g, b, fd, qtf, c), o, Xi, status, F_BEM, F_2nd, F_2nd_mean, workspace, workspace_bytes,
+                   max_chunk_units, stream);
 }
 
 extern "C" int raftk_general_batch_solve_dynamics_host(const raftk_general *g, const raftk_general_batch *b, const raftk_general_fd *fd,
@@ -2099,56 +2110,8 @@ extern "C" int raftk_general_batch_solve_dynamics_host(const raftk_general *g, c
                                                        double *Xi, int32_t *status, double *F_BEM, double *F_2nd, double *F_2nd_mean,
                                                        int32_t max_chunk_units)
 {
-    disp_reset();
-    if (int rc = gen_batch_counts(g, b, fd, qtf, c, o, Xi, status, max_chunk_units)) return rc;
-    if (int rc = gen_batch_tables(g, b, fd, qtf, b->node_offset, fd ? fd->fd_idx : nullptr, fd ? fd->bem_headings : nullptr,
-                                  qtf ? qtf->qtf_w : nullptr, qtf ? qtf->qtf_heads : nullptr)) return rc;
-    if (int rc = validate_gen_op(fd, c, c->op, c->primary)) return rc;
-    const size_t nD = b->n_designs, n = g->n_dof, nw = g->nw, Ns = g->n_nodes, nC = c->n_cases, nU = nD * nC;
-    std::vector<size_t> starts;                        // the plan's checks, before anything is staged
-    if (int rc = gen_plan_chunks(c->primary, nC, nD, gen_chunk_cap((int64_t)nU, max_chunk_units), true, starts)) return rc;
-    Staging S("raftk_general_batch_solve_dynamics_host");
-    raftk_general gg = *g;
-    S.in(gg.w, g->w, nw); S.in(gg.k, g->k, nw);
-    S.in(gg.node_r, g->node_r, Ns * 3); S.in(gg.node_frame, g->node_frame, Ns * 9);
-    S.in(gg.node_circ, g->node_circ, Ns); S.in(gg.node_Imat, g->node_Imat, Ns * 9);
-    S.in(gg.node_Imat_w, g->node_Imat_w, Ns * 9 * nw * 2); S.in(gg.node_a_i, g->node_a_i, Ns);
-    S.in(gg.node_cd, g->node_cd, Ns * 4); S.in(gg.Tn, g->Tn, Ns * 6 * n); S.in(gg.rr, g->rr, Ns * 3);
-    S.in(gg.M, g->M, nD * n * n); S.in(gg.B, g->B, nD * n * n); S.in(gg.C, g->C, nD * n * n);
-    raftk_general_batch bb = *b;
-    S.in(bb.node_offset, b->node_offset, nD + 1);
-    S.in(bb.x_ref, b->x_ref, nD); S.in(bb.y_ref, b->y_ref, nD); S.in(bb.heading_adjust, b->heading_adjust, nD);
-    raftk_cases cc = *c;
-    S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
-    S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC); S.in(cc.zeta, c->zeta, nC * nw);
-    S.in(cc.primary, c->primary, nC);
-    if (c->op) { S.in(cc.op, c->op, nC); S.in(cc.op_A_w, c->op_A_w, gen_op_elems(fd, c, nD, nw)); S.in(cc.op_B_w, c->op_B_w, gen_op_elems(fd, c, nD, nw)); }
-    raftk_general_fd ff = fd ? *fd : raftk_general_fd{};
-    if (fd) {
-        const size_t nf = fd->n_fd, nh = fd->n_bem_head;
-        S.in(ff.fd_idx, fd->fd_idx, nD * nf); S.in(ff.A_w, fd->A_w, nD * nf * nf * nw); S.in(ff.B_w, fd->B_w, nD * nf * nf * nw);
-        S.in(ff.bem_headings, fd->bem_headings, nD * nh); S.in(ff.X_BEM, fd->X_BEM, nD * nh * 6 * nw * 2); S.in(ff.T0, fd->T0, nh ? nD * 6 * n : 0);
-    }
-    raftk_general_qtf qq = qtf ? *qtf : raftk_general_qtf{};
-    if (qtf) {
-        const size_t n2 = qtf->n_qtf_w, nh = qtf->n_qtf_head;
-        S.in(qq.qtf_w, qtf->qtf_w, n2); S.in(qq.qtf_heads, qtf->qtf_heads, nh);
-        S.in(qq.qtf, qtf->qtf, (b->qtf_shared ? 1 : nD) * n2 * n2 * nh * 12);
-    }
-    double *dXi, *dF_BEM, *dF2, *dF2m;
-    int32_t *dStatus;
-    char *ws;
-    const size_t wb = raftk_general_batch_workspace_bytes(g, b, fd, qtf, c->n_cases, max_chunk_units);
-    S.out(dXi, nU * n * nw * 2, Xi); S.out(dStatus, nU * 4, status); S.out(dF_BEM, F_BEM ? nU * n * nw * 2 : 0, F_BEM);
-    S.out(dF2, qtf && F_2nd ? nU * 6 * nw : 0, F_2nd); S.out(dF2m, qtf && F_2nd_mean ? nU * 6 : 0, F_2nd_mean);
-    S.buf(ws, wb);
-    int rc = S.commit();
-    if (rc) return rc;
-    GenBatch Bt = gen_batch_of(&bb);
-    Bt.hnode_off = b->node_offset;
-    if ((rc = gen_run(&gg, Bt, fd ? &ff : nullptr, qtf ? &qq : nullptr, &cc, c->primary, o, dXi, dStatus, dF_BEM, dF2, dF2m, ws, wb,
-                      max_chunk_units, true, nullptr))) return rc;
-    return S.finish();
+    return gen_host("raftk_general_batch_solve_dynamics_host", GEN_BATCH, gen_call(g, b, fd, qtf, c), o, Xi, status, F_BEM, F_2nd,
+                    F_2nd_mean, max_chunk_units);
 }
 
 // Peer publication of a streamed shard (raftk_general_publish_dev): rows [row0, row0 + n_rows) of every rank's gathered array

@@ -866,7 +866,81 @@ def _general_qtf_struct(qtf, ptr_of):
     return q
 
 
-class GeneralSession:
+class _GeneralResident:
+    """What ``GeneralSession`` and ``GeneralBatchSession`` share: their tables uploaded into torch tensors on ``device``
+    (``keep``), the workspace and output tensors over the leading unit axes (``[nT]`` or ``[nD, nT]``), the solve's
+    enqueueing and the reductions of the last ``solve()`` on the resident Xi [..., nT, nDOF, nw]."""
+
+    def _open(self, device):
+        import torch
+        self.torch = torch
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.keep = {}
+
+    def _to_dev(self, name, a):
+        t = self.torch.from_numpy(a.view(np.float64) if a.dtype == np.complex128 else a).to(self.device)
+        self.keep[name] = t
+        return t.data_ptr()
+
+    def _upload_cases(self, cases):
+        self.ct = {k: self.torch.from_numpy(v).to(self.device) for k, v in cases.arrays.items()}
+        self.c_struct = cases.struct(lambda name: self.ct[name].data_ptr())
+
+    def _outputs(self, lead, n, nw, F_BEM):
+        """The workspace of ``workspace_bytes`` and the outputs: Xi, status, F_BEM with ``F_BEM``, F_2nd and F_2nd_mean with
+        a QTF table."""
+        torch, dev, qtf = self.torch, self.device, self.qtf is not None
+        self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=dev)
+        self.Xi = torch.zeros(lead + [n, nw], dtype=torch.complex128, device=dev)
+        self.status = torch.zeros(lead + [4], dtype=torch.int32, device=dev)
+        self.F_BEM = torch.zeros(lead + [n, nw], dtype=torch.complex128, device=dev) if F_BEM else None
+        self.F_2nd = torch.zeros(lead + [6, nw], dtype=torch.float64, device=dev) if qtf else None
+        self.F_2nd_mean = torch.zeros(lead + [6], dtype=torch.float64, device=dev) if qtf else None
+
+    def _enqueue(self, entry, structs, n_iter, tol, xi_start, *max_chunk):
+        """``entry`` (a raftk_general_*_dev solve) on the resident tables and outputs, on torch's current stream."""
+        o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
+        ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
+        with self.torch.cuda.device(self.device):
+            stream = self.torch.cuda.current_stream(self.device).cuda_stream
+            check(entry(*_refs(*structs), C.byref(self.c_struct), C.byref(o), self.Xi.data_ptr(), self.status.data_ptr(), ptr(self.F_BEM),
+                        ptr(self.F_2nd), ptr(self.F_2nd_mean), self.workspace.data_ptr(), self.workspace_bytes, *max_chunk, stream))
+        return (self.Xi, self.status) if self.F_BEM is None else (self.Xi, self.status, self.F_BEM)
+
+    def stats(self, R, wpow, psd=True, amp=False):
+        """Output-channel statistics of the last ``solve()`` on the device (raftk_general_channel_stats_dev, on each design's
+        slice of Xi): R [nch,nDOF] (``packer.pack_general_channels``), or [nD,nch,nDOF] in a design batch, wpow [nch] ->
+        (std [..., nT,nch], PSD [..., nT,nch,nw] or None, amplitudes complex [..., nT,nch,nw] or None), torch tensors."""
+        return _general_channel_stats(_session_buffers(self), R, wpow, self.keep["w"], self.Xi, self.dw, psd, amp)
+
+    def rotor_stats(self, R, C_, V_w, gains, case_row0=None, psd=True):
+        """Rotor speed, generator torque and blade pitch statistics of the last ``solve()`` on the device
+        (raftk_rotor_stats_dev, no host round trip, every design in one launch sequence): ``R`` [nrot, nDOF] or, in a design
+        batch, [nD, nrot, nDOF] (each design's hub rows); ``C``, ``V_w``, ``gains`` ([nC, nrot, ...], or per design [nD, nC,
+        nrot, ...]) and ``case_row0`` as ``rotor_stats`` (``packer.pack_rotor_outputs``; the first train of every case, e.g.
+        ``pack_case_trains``' ``first`` + [nT]).  -> (std [..., nC, nrot, 3], PSD [..., nC, nrot, 3, nw] or None), torch tensors."""
+        return _rotor_stats(_session_buffers(self), R, C_, V_w, gains, self.keep["w"], self.Xi, self.dw, case_row0, None, psd)
+
+    def fatigue(self, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, method="dirlik", weights=None, life=None,
+                moments=True, tile_w=0):
+        """Fatigue DELs of the last ``solve()`` on the device (raftk_fatigue_dev, no host round trip, every design in one
+        launch sequence): ``R`` [nch, nDOF] or, in a design batch, [nD, nch, nDOF] with ``wpow`` (``packer.pack_general_channels``'
+        rows) or ``coef``, and the other arguments as ``fatigue``; ``case_row0`` groups the trains into cases.  -> dict of
+        torch tensors as ``fatigue`` (DEL [..., nC, nch], ...)."""
+        return _fatigue(_session_buffers(self), self.Xi, self.keep["w"], m, R, wpow, coef, case_row0, f_eq, method, weights, life,
+                        moments, tile_w)
+
+    def stress_ring(self, fa, ss, angles=None, d=10.0, t=0.083, m=None, f_eq=1.0, method="dirlik", weights=None, case_row0=None,
+                    col0=None, psd=False, mean=None, wpow=None, tile_w=0):
+        """Tower-base axial stress around the circumference of the last ``solve()`` (raftk_stress_ring_dev on the resident Xi,
+        one unit per design): ``fa`` / ``ss`` the fore-aft / side-side rows (MbaseY / MbaseX of ``packer.pack_general_channels``),
+        [n_rings, nDOF] or, in a design batch, [nD, n_rings, nDOF]; the other arguments as ``stress_ring``.  -> dict of torch
+        tensors as ``stress_ring`` (std [..., nC, n_rings, nA], ...)."""
+        return _stress_ring(_session_buffers(self), self.Xi, self.keep["w"], fa, ss, angles, d, t, m, f_eq, method, weights, case_row0,
+                            col0, psd, mean, wpow, self.dw, tile_w)
+
+
+class GeneralSession(_GeneralResident):
     """Generalised-DOF solve with tables, workspace and outputs resident in HBM (torch tensors), kernels on torch's current
     stream: ``solve()`` enqueues raftk_general_solve_dynamics_dev -> (Xi [nT,nDOF,nw] complex, status [nT,4]); ``cases`` may
     carry wave trains (``packer.pack_case_trains``).  ``stats(R, wpow)`` reduces the device Xi to output-channel statistics
@@ -880,84 +954,30 @@ class GeneralSession:
     with the same results.  ``cases`` may carry per-case operating points, as for ``general_solve_dynamics``."""
 
     def __init__(self, P, M, B, Cm, cases, device=None, fd=None, F_BEM=False, qtf=None, max_chunk_cases=None):
-        import torch
-        self.torch = torch
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self.keep = {}
-
-        def to_dev(name, a):
-            t = torch.from_numpy(a.view(np.float64) if a.dtype == np.complex128 else a).to(self.device)
-            self.keep[name] = t
-            return t.data_ptr()
-        with torch.cuda.device(self.device):
-            self.g = _general_struct(P, M, B, Cm, to_dev)
-            self.ct = {k: torch.from_numpy(v).to(self.device) for k, v in cases.arrays.items()}
-            self.c_struct = cases.struct(lambda name: self.ct[name].data_ptr())
+        self._open(device)
+        with self.torch.cuda.device(self.device):
+            self.g = _general_struct(P, M, B, Cm, self._to_dev)
+            self._upload_cases(cases)
             n, nw, nC = int(P["gen_nDOF"]), len(P["w"]), cases.n_cases
             cases.check_general_ops(int(len(fd.get("fd_idx", ()))) if fd is not None else 0, 1, nw)
-            self.fd = _general_fd_struct(fd, n, nw, to_dev)
-            self.qtf = _general_qtf_struct(qtf, to_dev)
-            fdp = C.byref(self.fd) if self.fd is not None else None
-            qp = C.byref(self.qtf) if self.qtf is not None else None
+            self.fd = _general_fd_struct(fd, n, nw, self._to_dev)
+            self.qtf = _general_qtf_struct(qtf, self._to_dev)
+            g, fdp, qp = _refs(self.g, self.fd, self.qtf)
             self.max_chunk_cases = None if max_chunk_cases is None else int(max_chunk_cases)
             if self.max_chunk_cases is None:
-                self.workspace_bytes = int(lib.raftk_general_qtf_workspace_bytes(C.byref(self.g), fdp, qp, nC))
+                self.workspace_bytes = int(lib.raftk_general_qtf_workspace_bytes(g, fdp, qp, nC))
             else:
                 if self.max_chunk_cases < 0:
                     raise ValueError("max_chunk_cases must be >= 0 (0: all cases in one chunk)")
-                self.workspace_bytes = int(lib.raftk_general_stream_workspace_bytes(C.byref(self.g), fdp, qp, nC, self.max_chunk_cases))
-            self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=self.device)
-            self.Xi = torch.zeros([nC, n, nw], dtype=torch.complex128, device=self.device)
-            self.status = torch.zeros([nC, 4], dtype=torch.int32, device=self.device)
-            self.F_BEM = torch.zeros([nC, n, nw], dtype=torch.complex128, device=self.device) if F_BEM else None
-            self.F_2nd = torch.zeros([nC, 6, nw], dtype=torch.float64, device=self.device) if self.qtf is not None else None
-            self.F_2nd_mean = torch.zeros([nC, 6], dtype=torch.float64, device=self.device) if self.qtf is not None else None
+                self.workspace_bytes = int(lib.raftk_general_stream_workspace_bytes(g, fdp, qp, nC, self.max_chunk_cases))
+            self._outputs([nC], n, nw, F_BEM)
         self.n, self.nw, self.n_cases, self.dw = n, nw, nC, float(P["dw"])
 
     def solve(self, n_iter=10, tol=0.01, xi_start=0.0):
-        o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
-        ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
-        fdp = C.byref(self.fd) if self.fd is not None else None
-        qp = C.byref(self.qtf) if self.qtf is not None else None
-        with self.torch.cuda.device(self.device):
-            stream = self.torch.cuda.current_stream(self.device).cuda_stream
-            if self.max_chunk_cases is None:
-                check(lib.raftk_general_solve_dynamics_qtf_dev(C.byref(self.g), fdp, qp, C.byref(self.c_struct), C.byref(o), self.Xi.data_ptr(),
-                                                               self.status.data_ptr(), ptr(self.F_BEM), ptr(self.F_2nd), ptr(self.F_2nd_mean),
-                                                               self.workspace.data_ptr(), self.workspace_bytes, stream))
-            else:
-                check(lib.raftk_general_solve_dynamics_stream_dev(C.byref(self.g), fdp, qp, C.byref(self.c_struct), C.byref(o), self.Xi.data_ptr(),
-                                                                  self.status.data_ptr(), ptr(self.F_BEM), ptr(self.F_2nd), ptr(self.F_2nd_mean),
-                                                                  self.workspace.data_ptr(), self.workspace_bytes, self.max_chunk_cases, stream))
-        return (self.Xi, self.status) if self.F_BEM is None else (self.Xi, self.status, self.F_BEM)
-
-    def stats(self, R, wpow, psd=True, amp=False):
-        """Output-channel statistics of the last ``solve()`` (``packer.pack_general_channels``: R [nch,nDOF], wpow [nch]) on
-        the device -> (std [nT,nch], PSD [nT,nch,nw] or None, amplitudes complex [nT,nch,nw] or None), torch tensors."""
-        return _general_channel_stats(_session_buffers(self), R, wpow, self.keep["w"], self.Xi, self.dw, psd, amp)
-
-    def rotor_stats(self, R, C_, V_w, gains, case_row0=None, psd=True):
-        """Rotor speed, generator torque and blade pitch statistics of the last ``solve()`` on the device
-        (raftk_rotor_stats_dev, no host round trip): ``R`` [nrot, nDOF], ``C``, ``V_w``, ``gains`` and ``case_row0`` as
-        ``rotor_stats`` (``packer.pack_rotor_outputs``; the first train of every case, e.g. ``pack_case_trains``' ``first``
-        + [nT]).  -> (std [nC, nrot, 3], PSD [nC, nrot, 3, nw] or None), torch tensors."""
-        return _rotor_stats(_session_buffers(self), R, C_, V_w, gains, self.keep["w"], self.Xi, self.dw, case_row0, None, psd)
-
-    def fatigue(self, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, method="dirlik", weights=None, life=None,
-                moments=True, tile_w=0):
-        """Fatigue DELs of the last ``solve()`` on the device (raftk_fatigue_dev, no host round trip): ``R`` [nch, nDOF] with
-        ``wpow`` (``packer.pack_general_channels``' rows) or ``coef``, and the other arguments as ``fatigue``; ``case_row0``
-        groups the trains into cases.  -> dict of torch tensors as ``fatigue`` without the unit axis."""
-        return _fatigue(_session_buffers(self), self.Xi, self.keep["w"], m, R, wpow, coef, case_row0, f_eq, method, weights, life,
-                        moments, tile_w)
-
-    def stress_ring(self, fa, ss, angles=None, d=10.0, t=0.083, m=None, f_eq=1.0, method="dirlik", weights=None, case_row0=None,
-                    col0=None, psd=False, mean=None, wpow=None, tile_w=0):
-        """Tower-base axial stress around the circumference of the last ``solve()`` (raftk_stress_ring_dev on the resident Xi [nT, nDOF, nw]):
-        ``fa`` / ``ss`` the fore-aft / side-side rows (MbaseY / MbaseX of ``packer.pack_general_channels``); the other
-        arguments as ``stress_ring``.  -> dict of torch tensors as ``stress_ring`` (std [nC, n_rings, nA], ...)."""
-        return _stress_ring(_session_buffers(self), self.Xi, self.keep["w"], fa, ss, angles, d, t, m, f_eq, method, weights, case_row0,
-                            col0, psd, mean, wpow, self.dw, tile_w)
+        structs = (self.g, self.fd, self.qtf)
+        if self.max_chunk_cases is None:
+            return self._enqueue(lib.raftk_general_solve_dynamics_qtf_dev, structs, n_iter, tol, xi_start)
+        return self._enqueue(lib.raftk_general_solve_dynamics_stream_dev, structs, n_iter, tol, xi_start, self.max_chunk_cases)
 
 
 def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0, fd=None, F_BEM=False, qtf=None, F_2nd=False,
@@ -1020,17 +1040,27 @@ def general_chunk_plan(primary, n_cases, max_chunk_cases):
     """The chunks raftk_general_solve_dynamics_stream_* cut a case table into -> [c_0 = 0, c_1, ..., n_cases]: whole train
     groups (``sweep.general_groups``) packed greedily in table order into chunks of at most ``max_chunk_cases`` (0: all).
     ValueError where the library refuses the table: interleaved groups, a group larger than a chunk."""
+    return _chunk_plan(primary, n_cases, 1, max_chunk_cases, "max_chunk_cases")
+
+
+def _chunk_plan(primary, n_cases, n_designs, max_chunk, cap_name):
+    """The chunk starts of ``n_designs`` designs' units over a case table, design-major, and n_designs * n_cases: every
+    design's train groups in table order, packed greedily into chunks of at most ``max_chunk`` units (0: all); a chunk may
+    cross design boundaries.  ``cap_name``: the chunk cap's argument name in the messages."""
     from .sweep import general_groups
-    n = int(n_cases)
-    K = n if (max_chunk_cases <= 0 or max_chunk_cases >= n) else int(max_chunk_cases)
+    n, nD = int(n_cases), int(n_designs)
+    nU = n * nD
+    K = nU if (max_chunk <= 0 or max_chunk >= nU) else int(max_chunk)
     g = general_groups(primary, n)
-    cuts = [0]
     for a, b in zip(g[:-1], g[1:]):
         if b - a > K:
-            raise ValueError("a train group has %d cases, more than max_chunk_cases = %d" % (b - a, K))
-        if b - cuts[-1] > K:
-            cuts.append(int(a))
-    return cuts + [n]
+            raise ValueError("a train group has %d cases, more than %s = %d" % (b - a, cap_name, K))
+    cuts = [0]
+    for d in range(nD):
+        for a, b in zip(g[:-1], g[1:]):
+            if d * n + b - cuts[-1] > K:
+                cuts.append(int(d * n + a))
+    return cuts + [nU]
 
 
 def general_chunk_for_budget(P, fd, qtf, n_cases, budget_bytes):
@@ -1042,7 +1072,13 @@ def general_chunk_for_budget(P, fd, qtf, n_cases, budget_bytes):
         return n_cases
     if ws(1) > budget:
         raise ValueError("a workspace of %d bytes does not hold one case (%d bytes)" % (budget, ws(1)))
-    lo, hi = 1, n_cases - 1                                # ws grows with the chunk below n_cases: ws(lo) fits
+    return _largest_chunk(ws, 1, n_cases, budget)
+
+
+def _largest_chunk(ws, lo, n_units, budget):
+    """The largest chunk in [lo, n_units) whose workspace ``ws(chunk)`` fits ``budget``, given that ws(lo) fits and the
+    whole, ws(n_units), does not: ws grows with the chunk below n_units."""
+    hi = n_units - 1
     while lo < hi:
         mid = (lo + hi + 1) // 2
         if ws(mid) <= budget:
@@ -1948,20 +1984,7 @@ def general_batch_chunk_plan(primary, n_cases, n_designs, max_chunk_units):
     """The chunks raftk_general_batch_solve_dynamics_* cut the units (design, case), design-major, into -> [u_0 = 0, ...,
     n_designs * n_cases]: every design's train groups in table order, packed greedily into chunks of at most
     ``max_chunk_units`` (0: all); a chunk may cross design boundaries.  ValueError where the library refuses the plan."""
-    from .sweep import general_groups
-    n, nD = int(n_cases), int(n_designs)
-    nU = n * nD
-    K = nU if (max_chunk_units <= 0 or max_chunk_units >= nU) else int(max_chunk_units)
-    g = general_groups(primary, n)
-    for a, b in zip(g[:-1], g[1:]):
-        if b - a > K:
-            raise ValueError("a train group has %d cases, more than max_chunk_units = %d" % (b - a, K))
-    cuts = [0]
-    for d in range(nD):
-        for a, b in zip(g[:-1], g[1:]):
-            if d * n + b - cuts[-1] > K:
-                cuts.append(int(d * n + a))
-    return cuts + [nU]
+    return _chunk_plan(primary, n_cases, n_designs, max_chunk_units, "max_chunk_units")
 
 
 def general_batch_chunk_for_budget(batch, n_cases, budget_bytes, primary=None):
@@ -1977,14 +2000,7 @@ def general_batch_chunk_for_budget(batch, n_cases, budget_bytes, primary=None):
         return nU
     if ws(big) > budget:
         raise ValueError("a workspace of %d bytes does not hold %d units (%d bytes)" % (budget, big, ws(big)))
-    lo, hi = big, nU - 1
-    while lo < hi:
-        mid = (lo + hi + 1) // 2
-        if ws(mid) <= budget:
-            lo = mid
-        else:
-            hi = mid - 1
-    return lo
+    return _largest_chunk(ws, big, nU, budget)
 
 
 def general_solve_dynamics_batch(designs, cases, n_iter=10, tol=0.01, xi_start=0.0, F_BEM=False, F_2nd=False, max_chunk_units=0, qtf=None):
@@ -2016,7 +2032,7 @@ def general_solve_dynamics_batch(designs, cases, n_iter=10, tol=0.01, xi_start=0
     return (Xi, st) + ((Fb,) if F_BEM else ()) + ((F2, F2m) if F_2nd else ())
 
 
-class GeneralBatchSession:
+class GeneralBatchSession(_GeneralResident):
     """A design batch (``GeneralBatch`` or its list of per-design inputs) with tables, workspace and outputs resident in HBM,
     kernels on torch's current stream, the contract of ``GeneralSession``: ``solve()`` enqueues
     raftk_general_batch_solve_dynamics_dev -> (Xi [nD,nT,nDOF,nw] complex, status [nD,nT,4]) (+ F_BEM [nD,nT,nDOF,nw] with
@@ -2025,44 +2041,23 @@ class GeneralBatchSession:
     ``stats(R, wpow)`` takes channel rows per design, R [nD,nch,nDOF] (``packer.pack_general_channels`` of each design)."""
 
     def __init__(self, designs, cases, device=None, F_BEM=False, qtf=None, max_chunk_units=0):
-        import torch
-        self.torch = torch
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self._open(device)
         self.batch = bt = _as_batch(designs, qtf)
         if int(max_chunk_units) < 0:
             raise ValueError("max_chunk_units must be >= 0 (0: all units in one chunk)")
         self.max_chunk_units = int(max_chunk_units)
-        self.keep = {}
-
-        def to_dev(name, a):
-            t = torch.from_numpy(a.view(np.float64) if a.dtype == np.complex128 else a).to(self.device)
-            self.keep[name] = t
-            return t.data_ptr()
         nD, nC, n, nw = bt.n_designs, cases.n_cases, bt.n, bt.nw
         cases.check_general_ops(bt.n_fd if bt.fd is not None else 0, nD, nw)
-        with torch.cuda.device(self.device):
-            self.g, self.b, self.fd, self.qtf = bt.structs(to_dev)
-            self.ct = {k: torch.from_numpy(v).to(self.device) for k, v in cases.arrays.items()}
-            self.c_struct = cases.struct(lambda name: self.ct[name].data_ptr())
+        with self.torch.cuda.device(self.device):
+            self.g, self.b, self.fd, self.qtf = bt.structs(self._to_dev)
+            self._upload_cases(cases)
             self.workspace_bytes = general_batch_workspace_bytes(bt, nC, self.max_chunk_units)
-            self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=self.device)
-            self.Xi = torch.zeros([nD, nC, n, nw], dtype=torch.complex128, device=self.device)
-            self.status = torch.zeros([nD, nC, 4], dtype=torch.int32, device=self.device)
-            self.F_BEM = torch.zeros([nD, nC, n, nw], dtype=torch.complex128, device=self.device) if F_BEM else None
-            self.F_2nd = torch.zeros([nD, nC, 6, nw], dtype=torch.float64, device=self.device) if self.qtf is not None else None
-            self.F_2nd_mean = torch.zeros([nD, nC, 6], dtype=torch.float64, device=self.device) if self.qtf is not None else None
+            self._outputs([nD, nC], n, nw, F_BEM)
         self.n_designs, self.n, self.nw, self.n_cases, self.dw = nD, n, nw, nC, bt.dw
 
     def solve(self, n_iter=10, tol=0.01, xi_start=0.0):
-        o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
-        ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
-        with self.torch.cuda.device(self.device):
-            stream = self.torch.cuda.current_stream(self.device).cuda_stream
-            check(lib.raftk_general_batch_solve_dynamics_dev(*_refs(self.g, self.b, self.fd, self.qtf), C.byref(self.c_struct), C.byref(o),
-                                                             self.Xi.data_ptr(), self.status.data_ptr(), ptr(self.F_BEM), ptr(self.F_2nd),
-                                                             ptr(self.F_2nd_mean), self.workspace.data_ptr(), self.workspace_bytes,
-                                                             self.max_chunk_units, stream))
-        return (self.Xi, self.status) if self.F_BEM is None else (self.Xi, self.status, self.F_BEM)
+        return self._enqueue(lib.raftk_general_batch_solve_dynamics_dev, (self.g, self.b, self.fd, self.qtf), n_iter, tol, xi_start,
+                             self.max_chunk_units)
 
     def eigen(self, A0=None, yawstiff=0.0, sort="ascending", modes=True):
         """Natural frequencies and mode shapes of every design on the device, on torch's current stream (async):
@@ -2072,35 +2067,6 @@ class GeneralBatchSession:
         info [nD] int32 (RAFTK_EIG_* flags), torch tensors; ``sort`` as ``solve_eigen``."""
         nD, n = self.n_designs, self.n
         return _session_eigen(self, self.keep["M"].view(nD, n, n), self.keep["C"].view(nD, n, n), A0, yawstiff, sort, modes)
-
-    def stats(self, R, wpow, psd=True, amp=False):
-        """Output-channel statistics of the last ``solve()`` on the device, design by design (raftk_general_channel_stats_dev
-        on each design's slice of Xi): R [nD,nch,nDOF], wpow [nch] -> (std [nD,nT,nch], PSD [nD,nT,nch,nw] or None, amplitudes
-        complex [nD,nT,nch,nw] or None), torch tensors."""
-        return _general_channel_stats(_session_buffers(self), R, wpow, self.keep["w"], self.Xi, self.dw, psd, amp)
-
-    def rotor_stats(self, R, C_, V_w, gains, case_row0=None, psd=True):
-        """Rotor statistics of the last ``solve()`` for every design in one launch sequence (raftk_rotor_stats_dev on the
-        resident Xi [nD, nT, nDOF, nw]): ``R`` [nD, nrot, nDOF] (each design's hub rows) or [nrot, nDOF]; ``C``, ``V_w``,
-        ``gains`` for every design ([nC, nrot, ...]) or per design ([nD, nC, nrot, ...]); ``case_row0`` as ``rotor_stats``.
-        -> (std [nD, nC, nrot, 3], PSD [nD, nC, nrot, 3, nw] or None), torch tensors."""
-        return _rotor_stats(_session_buffers(self), R, C_, V_w, gains, self.keep["w"], self.Xi, self.dw, case_row0, None, psd)
-
-    def fatigue(self, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, method="dirlik", weights=None, life=None,
-                moments=True, tile_w=0):
-        """Fatigue DELs of the last ``solve()`` for every design in one launch sequence (raftk_fatigue_dev on the resident Xi
-        [nD, nT, nDOF, nw]): ``R`` [nD, nch, nDOF] (each design's rows) or [nch, nDOF], or ``coef``; the other arguments as
-        ``fatigue``.  -> dict of torch tensors as ``fatigue`` (DEL [nD, nC, nch], ...)."""
-        return _fatigue(_session_buffers(self), self.Xi, self.keep["w"], m, R, wpow, coef, case_row0, f_eq, method, weights, life,
-                        moments, tile_w)
-
-    def stress_ring(self, fa, ss, angles=None, d=10.0, t=0.083, m=None, f_eq=1.0, method="dirlik", weights=None, case_row0=None,
-                    col0=None, psd=False, mean=None, wpow=None, tile_w=0):
-        """Tower-base axial stress around the circumference of the last ``solve()`` (raftk_stress_ring_dev on the resident Xi [nD, nT, nDOF, nw], one unit per design):
-        ``fa`` / ``ss`` the fore-aft / side-side rows (MbaseY / MbaseX of ``packer.pack_general_channels``), [n_rings, nDOF] for every design or [nD, n_rings, nDOF]; the other
-        arguments as ``stress_ring``.  -> dict of torch tensors as ``stress_ring`` (std [nD, nC, n_rings, nA], ...)."""
-        return _stress_ring(_session_buffers(self), self.Xi, self.keep["w"], fa, ss, angles, d, t, m, f_eq, method, weights, case_row0,
-                            col0, psd, mean, wpow, self.dw, tile_w)
 
 
 def _no_general_ops(turbine_constants):
