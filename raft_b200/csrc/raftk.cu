@@ -2218,27 +2218,35 @@ extern "C" int raftk_qtf_slender_dev(const raftk_slender *s, int32_t n_cases, co
                           (cudaStream_t)stream);
 }
 
+// the slender-body columns of nD designs: one design's tables, or a batch's concatenated ones, where every design has its own
+// member-local mem_node_start row (its n_members + 1 entries) and its own M_struc
+static void stage_slender(Staging &S, const raftk_slender &from, raftk_slender &to, size_t nD)
+{
+    const size_t Nm = from.n_members, Ns = from.n_nodes, Ng = from.n_seg, nw = from.nw;
+    S.in(to.w, from.w, nw); S.in(to.k, from.k, nw);
+    S.in(to.mem_q, from.mem_q, Nm * 3); S.in(to.mem_p1, from.mem_p1, Nm * 3); S.in(to.mem_p2, from.mem_p2, Nm * 3);
+    S.in(to.mem_mcf, from.mem_mcf, Nm); S.in(to.mem_wl, from.mem_wl, Nm);
+    S.in(to.mem_r_int, from.mem_r_int, Nm * 3); S.in(to.mem_a_wl, from.mem_a_wl, Nm);
+    S.in(to.mem_rwl, from.mem_rwl, Nm * 3); S.in(to.mem_R_wl, from.mem_R_wl, Nm);
+    S.in(to.mem_node_start, from.mem_node_start, Nm + nD);
+    S.in(to.node_r, from.node_r, Ns * 3); S.in(to.node_v_side, from.node_v_side, Ns);
+    S.in(to.node_Ca_p1, from.node_Ca_p1, Ns); S.in(to.node_Ca_p2, from.node_Ca_p2, Ns);
+    S.in(to.node_Ca_End, from.node_Ca_End, Ns); S.in(to.node_v_end, from.node_v_end, Ns);
+    S.in(to.node_a_i, from.node_a_i, Ns);
+    S.in(to.seg_mem, from.seg_mem, Ng); S.in(to.seg_z1, from.seg_z1, Ng); S.in(to.seg_z2, from.seg_z2, Ng);
+    S.in(to.seg_R, from.seg_R, Ng); S.in(to.seg_rmid, from.seg_rmid, Ng * 3);
+    S.in(to.M_struc, from.M_struc, nD * 36);
+}
+
 extern "C" int raftk_qtf_slender_host(const raftk_slender *s, int32_t n_cases, const double *beta_rad, const double *Xi_rao, double *qtf)
 {
     int rc = validate_slender(s, n_cases);
     if (rc) return rc;
     if (!beta_rad || !Xi_rao || !qtf) return set_err(RAFTK_EINVAL, "slender-body QTF: null beta / Xi_rao / qtf");
-    const size_t Nm = s->n_members, Ns = s->n_nodes, Ng = s->n_seg, nw = s->nw, nC = n_cases;
+    const size_t nw = s->nw, nC = n_cases;
     Staging S("raftk_qtf_slender_host");
     raftk_slender dd = *s;
-    S.in(dd.w, s->w, nw); S.in(dd.k, s->k, nw);
-    S.in(dd.mem_q, s->mem_q, Nm * 3); S.in(dd.mem_p1, s->mem_p1, Nm * 3); S.in(dd.mem_p2, s->mem_p2, Nm * 3);
-    S.in(dd.mem_mcf, s->mem_mcf, Nm); S.in(dd.mem_wl, s->mem_wl, Nm);
-    S.in(dd.mem_r_int, s->mem_r_int, Nm * 3); S.in(dd.mem_a_wl, s->mem_a_wl, Nm);
-    S.in(dd.mem_rwl, s->mem_rwl, Nm * 3); S.in(dd.mem_R_wl, s->mem_R_wl, Nm);
-    S.in(dd.mem_node_start, s->mem_node_start, Nm + 1);
-    S.in(dd.node_r, s->node_r, Ns * 3); S.in(dd.node_v_side, s->node_v_side, Ns);
-    S.in(dd.node_Ca_p1, s->node_Ca_p1, Ns); S.in(dd.node_Ca_p2, s->node_Ca_p2, Ns);
-    S.in(dd.node_Ca_End, s->node_Ca_End, Ns); S.in(dd.node_v_end, s->node_v_end, Ns);
-    S.in(dd.node_a_i, s->node_a_i, Ns);
-    S.in(dd.seg_mem, s->seg_mem, Ng); S.in(dd.seg_z1, s->seg_z1, Ng); S.in(dd.seg_z2, s->seg_z2, Ng);
-    S.in(dd.seg_R, s->seg_R, Ng); S.in(dd.seg_rmid, s->seg_rmid, Ng * 3);
-    S.in(dd.M_struc, s->M_struc, 36);
+    stage_slender(S, *s, dd, 1);
     const double *dBeta, *dXi;
     double *dQ;
     char *ws;
@@ -2402,24 +2410,9 @@ extern "C" int raftk_solve_dynamics_slender_host(const raftk_designs *d, const r
     raftk_cases cc = *c;
     stage_designs_cases(S, d, c, dd, cc);
     const size_t nD = d->n_designs, nw = d->nw, nC = c->n_cases, nR = nD * nC * 6 * nw * 2, nw2 = s->cols.nw;
-    const size_t Nm = s->cols.n_members, Ns = s->cols.n_nodes, Ng = s->cols.n_seg;
     raftk_slender_batch sb = *s;
-    raftk_slender &sc = sb.cols;
-    const raftk_slender &h = s->cols;
     S.in(sb.node_offset, s->node_offset, nD + 1); S.in(sb.member_offset, s->member_offset, nD + 1); S.in(sb.seg_offset, s->seg_offset, nD + 1);
-    S.in(sc.w, h.w, nw2); S.in(sc.k, h.k, nw2);
-    S.in(sc.mem_q, h.mem_q, Nm * 3); S.in(sc.mem_p1, h.mem_p1, Nm * 3); S.in(sc.mem_p2, h.mem_p2, Nm * 3);
-    S.in(sc.mem_mcf, h.mem_mcf, Nm); S.in(sc.mem_wl, h.mem_wl, Nm);
-    S.in(sc.mem_r_int, h.mem_r_int, Nm * 3); S.in(sc.mem_a_wl, h.mem_a_wl, Nm);
-    S.in(sc.mem_rwl, h.mem_rwl, Nm * 3); S.in(sc.mem_R_wl, h.mem_R_wl, Nm);
-    S.in(sc.mem_node_start, h.mem_node_start, Nm + nD);
-    S.in(sc.node_r, h.node_r, Ns * 3); S.in(sc.node_v_side, h.node_v_side, Ns);
-    S.in(sc.node_Ca_p1, h.node_Ca_p1, Ns); S.in(sc.node_Ca_p2, h.node_Ca_p2, Ns);
-    S.in(sc.node_Ca_End, h.node_Ca_End, Ns); S.in(sc.node_v_end, h.node_v_end, Ns);
-    S.in(sc.node_a_i, h.node_a_i, Ns);
-    S.in(sc.seg_mem, h.seg_mem, Ng); S.in(sc.seg_z1, h.seg_z1, Ng); S.in(sc.seg_z2, h.seg_z2, Ng);
-    S.in(sc.seg_R, h.seg_R, Ng); S.in(sc.seg_rmid, h.seg_rmid, Ng * 3);
-    S.in(sc.M_struc, h.M_struc, nD * 36);
+    stage_slender(S, s->cols, sb.cols, nD);
     raftk_outputs od;
     memset(&od, 0, sizeof(od));
     S.out(od.Xi, nR, out->Xi);

@@ -330,12 +330,45 @@ def _host_ptr(arrays):
     return lambda name: arrays[name].ctypes.data
 
 
-def _alloc_outputs(nD, nC, nw, want, alloc=np.zeros):
-    shapes = dict(Xi=([nD, nC, 6, nw], np.complex128), status=([nD, nC, 4], _I4), B_drag=([nD, nC, 6, 6], _F8),
-                  F_drag=([nD, nC, 6, nw], np.complex128), F_iner=([nD, nC, 6, nw], np.complex128),
-                  F_BEM=([nD, nC, 6, nw], np.complex128), zeta=([nC, nw], _F8),
-                  F_2nd=([nD, nC, 6, nw], _F8), F_2nd_mean=([nD, nC, 6], _F8), Xi_last=([nD, nC, 6, nw], np.complex128))
-    return {k: alloc(shapes[k][0], dtype=shapes[k][1]) for k in want}
+def _output_table(nD, nC, nw, nw2=0):
+    """name -> (shape, numpy dtype) of every output of the rigid-FOWT solves; qtf and Xi_rao are on the second-order grid."""
+    u = [nD, nC]
+    return dict(Xi=(u + [6, nw], _C16), status=(u + [4], _I4), B_drag=(u + [6, 6], _F8), F_drag=(u + [6, nw], _C16),
+                F_iner=(u + [6, nw], _C16), F_BEM=(u + [6, nw], _C16), zeta=([nC, nw], _F8), F_2nd=(u + [6, nw], _F8),
+                F_2nd_mean=(u + [6], _F8), Xi_last=(u + [6, nw], _C16), qtf=(u + [nw2, nw2, 6], _C16), Xi_rao=(u + [6, nw2], _C16))
+
+
+_HOST_OUTPUTS = ("Xi", "status", "B_drag", "F_drag", "F_iner", "F_BEM", "zeta", "F_2nd", "F_2nd_mean", "Xi_last")
+_SESSION_OUTPUTS = _HOST_OUTPUTS[:-1]
+_SLENDER_OUTPUTS = _HOST_OUTPUTS + ("qtf", "Xi_rao")
+
+
+def _check_outputs(want, known):
+    bad = [k for k in want if k not in known]
+    if bad:
+        raise ValueError("unknown outputs %s (known: %s)" % (bad, ", ".join(known)))
+
+
+def _alloc_outputs(nD, nC, nw, want, known=_HOST_OUTPUTS, nw2=0, zeros=np.zeros):
+    """The outputs named in ``want``, each one of ``known``, as ``zeros(shape, dtype)`` of the output table."""
+    _check_outputs(want, known)
+    table = _output_table(nD, nC, nw, nw2)
+    return {k: zeros(*table[k]) for k in want}
+
+
+def _torch_dtype(dtype):
+    import torch
+    return torch.from_numpy(np.empty(0, dtype)).dtype
+
+
+def _torch_zeros(device):
+    """``np.zeros`` for torch tensors on ``device``."""
+    import torch
+    return lambda shape, dtype: torch.zeros(shape, dtype=_torch_dtype(dtype), device=device)
+
+
+def _opts(n_iter, tol, xi_start, cluster_size=0, flags=0):
+    return RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), flags, 0)
 
 
 def _out_struct(outs, ptr):
@@ -357,22 +390,32 @@ def solve_dynamics(batch, cases, n_iter=10, tol=0.01, xi_start=0.0, cluster_size
     want = tuple(dict.fromkeys(tuple(want) + ("Xi", "status")))
     outs = out if out is not None else _alloc_outputs(batch.n_designs, cases.n_cases, batch.nw, want)
     cases.check_ops(batch)
-    d = _host_struct(batch)
     c = _host_struct(cases)
-    o = RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), 0, 0)
+    o = _opts(n_iter, tol, xi_start, cluster_size)
     os_ = _out_struct(outs, lambda a: a.ctypes.data)
-    check(lib.raftk_solve_dynamics_host(C.byref(d), C.byref(c), C.byref(o), C.byref(os_)))
-    if _plan_overflowed(outs):
-        check(lib.raftk_solve_dynamics_host(C.byref(_host_struct(worst_case_hints(batch))), C.byref(c), C.byref(o), C.byref(os_)))
-        _raise_on_plan(outs)
+
+    def run(b):
+        check(lib.raftk_solve_dynamics_host(C.byref(_host_struct(b)), C.byref(c), C.byref(o), C.byref(os_)))
+        return outs
+    return _retry_on_plan(batch, run)
+
+
+def _plan_overflowed(status):
+    """Whether a unit came back with RAFTK_FLAG_PLAN in ``status`` (numpy or torch): the batch's step-class hints were below
+    the number of classes the kernels count (DesignBatch computes them by the kernels' rule, so only hints set by the
+    caller can be), and those units ran no pass and hold zeros."""
+    return bool((status[..., 2] & FLAG_PLAN).any())
+
+
+def _retry_on_plan(batch, run):
+    """``run(batch) -> outs``, run once more on ``worst_case_hints(batch)`` when a unit came back with RAFTK_FLAG_PLAN (a farm's
+    Xi_sys was then assembled from those units' zero loads, so everything is solved again)."""
+    outs = run(batch)
+    if _plan_overflowed(outs["status"]):
+        outs = run(worst_case_hints(batch))
+        if _plan_overflowed(outs["status"]):
+            raise _lib.RaftkError("step-class tables overflowed even with worst-case sizes")
     return outs
-
-
-def _plan_overflowed(outs):
-    """Whether a unit came back with RAFTK_FLAG_PLAN: the batch's step-class hints were below the number of classes the
-    kernels count (DesignBatch computes them by the kernels' rule, so only hints set by the caller can be), and those
-    units ran no pass and hold zeros."""
-    return bool(np.any(np.asarray(outs["status"])[..., 2] & FLAG_PLAN))
 
 
 def worst_case_hints(batch):
@@ -384,53 +427,17 @@ def worst_case_hints(batch):
     return b
 
 
-def _raise_on_plan(outs):
-    if _plan_overflowed(outs):
-        raise _lib.RaftkError("step-class tables overflowed even with worst-case sizes")
-
-
 def solve_dynamics_farm(batch, cases, C_arr=None, M_arr=None, B_arr=None, n_iter=10, tol=0.01, xi_start=0.0, cluster_size=0,
                         want=("Xi", "status", "B_drag"), out=None):
     """Coupled farm response (raft_model.py:1164-1236), host buffers in/out, ONE call: the designs of ``batch`` are the N
     FOWTs of the array; every FOWT's drag linearisation runs as in ``solve_dynamics``, then the 6N x 6N system
     blockdiag(Z_i) + (-w^2 M_arr + i w B_arr + C_arr) is assembled and solved per (case, frequency) on the device.
+    Array matrices: [6N,6N], or [1,6N,6N] as for a batch of one farm.
     -> the per-FOWT output dict plus ``Xi_sys`` complex [nC, 6N, nw] and ``info`` [nC, nw] (k+1 of a zero pivot).
     ``out``: caller-owned result arrays (e.g. page-locked ones from ``pinned_empty``: device-to-host copies then run at
     the link rate instead of through the driver's staging of pageable memory); missing ones are allocated."""
-    N, nC, nw = batch.n_designs, cases.n_cases, batch.nw
     cases.check_ops(batch)
-    n = 6 * N
-    want = tuple(dict.fromkeys(tuple(want) + ("Xi", "status")))
-    outs = dict(out) if out is not None else {}
-    for k_, v in _alloc_outputs(N, nC, nw, tuple(k for k in want if k not in outs)).items():
-        outs[k_] = v
-    mats = {}
-    for nm, v in (("M_arr", M_arr), ("B_arr", B_arr), ("C_arr", C_arr)):
-        if v is not None:
-            a = np.ascontiguousarray(v, dtype=_F8)
-            if a.shape != (n, n):
-                raise ValueError("%s must be [%d, %d]" % (nm, n, n))
-            mats[nm] = a
-    if "Xi_sys" not in outs:
-        outs["Xi_sys"] = np.zeros([nC, n, nw], dtype=np.complex128)
-    if "info" not in outs:
-        outs["info"] = np.zeros([nC, nw], dtype=_I4)
-    if outs["Xi_sys"].shape != (nC, n, nw) or outs["Xi_sys"].dtype != np.complex128 or not outs["Xi_sys"].flags.c_contiguous:
-        raise ValueError("out['Xi_sys'] must be a C-contiguous complex128 array [%d, %d, %d]" % (nC, n, nw))
-    f = RaftkFarm()
-    f.n_fowt = N
-    for nm in ("M_arr", "B_arr", "C_arr"):
-        setattr(f, nm, mats[nm].ctypes.data if nm in mats else None)
-    f.Xi_sys, f.info = outs["Xi_sys"].ctypes.data, outs["info"].ctypes.data
-    d = _host_struct(batch)
-    c = _host_struct(cases)
-    o = RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), 0, 0)
-    os_ = _out_struct(outs, lambda a: a.ctypes.data)
-    check(lib.raftk_solve_dynamics_farm_host(C.byref(d), C.byref(c), C.byref(o), C.byref(os_), C.byref(f)))
-    if _plan_overflowed(outs):                      # Xi_sys was assembled from those units' zero loads: solve it all again
-        check(lib.raftk_solve_dynamics_farm_host(C.byref(_host_struct(worst_case_hints(batch))), C.byref(c), C.byref(o), C.byref(os_), C.byref(f)))
-        _raise_on_plan(outs)
-    return outs
+    return _solve_farms(batch, cases, batch.n_designs, None, M_arr, B_arr, C_arr, _opts(n_iter, tol, xi_start, cluster_size), want, out)
 
 
 def _farm_batch_matrices(n_farms, n, M_arr, B_arr, C_arr):
@@ -443,41 +450,62 @@ def _farm_batch_matrices(n_farms, n, M_arr, B_arr, C_arr):
     return mats, 0 if shapes == {(n_farms, n, n)} else 1
 
 
+def _farm_setup(N, F, nC, nw, M_arr, B_arr, C_arr, out=None, device=None):
+    """``F`` farms of ``N`` FOWTs as the farm-batch entries take them; ``F`` None is one farm, a batch of one whose outputs
+    have no farm axis.  -> (RaftkFarmBatch, matrices, Xi_sys [F,nC,6N,nw], info [F,nC,nw]).  Host arrays, or with ``device``
+    torch tensors there; ``out``: host Xi_sys / info the caller owns, checked and used in place."""
+    n = 6 * N
+    mats, shared = _farm_batch_matrices(F or 1, n, M_arr, B_arr, C_arr)
+    lead = [] if F is None else [F]
+    res = dict(Xi_sys=(lead + [nC, n, nw], _C16), info=(lead + [nC, nw], _I4))
+    if device is None:
+        ptr = lambda a: a.ctypes.data   # noqa: E731
+        for k, (shape, dt) in res.items():
+            a = (out or {}).get(k)
+            if a is not None and (a.shape != tuple(shape) or a.dtype != dt or not a.flags.c_contiguous):
+                raise ValueError("out[%r] must be a C-contiguous %s array %s" % (k, np.dtype(dt).name, shape))
+            res[k] = np.zeros(shape, dt) if a is None else a
+    else:
+        import torch
+        ptr = lambda t: t.data_ptr()    # noqa: E731
+        mats = {nm: torch.from_numpy(a).to(device) for nm, a in mats.items()}
+        res = {k: _torch_zeros(device)(*v) for k, v in res.items()}
+    f = RaftkFarmBatch()
+    f.n_farms, f.n_fowt, f.arr_shared = F or 1, N, shared
+    for nm in ("M_arr", "B_arr", "C_arr"):
+        setattr(f, nm, ptr(mats[nm]) if nm in mats else None)
+    f.Xi_sys, f.info = ptr(res["Xi_sys"]), ptr(res["info"])
+    return f, mats, res["Xi_sys"], res["info"]
+
+
+def _solve_farms(batch, cases, N, F, M_arr, B_arr, C_arr, o, want, out):
+    """``solve_dynamics_farm`` (``F`` None) and ``solve_dynamics_farm_batch`` through raftk_solve_dynamics_farm_batch_host."""
+    f, mats, xi, info = _farm_setup(N, F, cases.n_cases, batch.nw, M_arr, B_arr, C_arr, out)
+    want = tuple(dict.fromkeys(tuple(want) + ("Xi", "status")))
+    outs = dict(out) if out is not None else {}
+    outs.update(_alloc_outputs(batch.n_designs, cases.n_cases, batch.nw, tuple(k for k in want if k not in outs)))
+    outs["Xi_sys"], outs["info"] = xi, info
+    c = _host_struct(cases)
+    os_ = _out_struct(outs, lambda a: a.ctypes.data)
+
+    def run(b):
+        check(lib.raftk_solve_dynamics_farm_batch_host(C.byref(_host_struct(b)), C.byref(c), C.byref(o), C.byref(os_), C.byref(f)))
+        return outs
+    return _retry_on_plan(batch, run)
+
+
 def solve_dynamics_farm_batch(batch, cases, n_fowt, C_arr=None, M_arr=None, B_arr=None, n_iter=10, tol=0.01, xi_start=0.0, cluster_size=0,
                               want=("Xi", "status", "B_drag"), out=None):
     """``solve_dynamics_farm`` for F farms of ``n_fowt`` FOWTs each in ONE call (a layout or shared-mooring study): design
     ``f * n_fowt + i`` of ``batch`` is FOWT i of farm f, all farms over the same case table.  Array matrices: [6N,6N] used by
     every farm, or [F,6N,6N].  -> the per-FOWT output dict plus ``Xi_sys`` complex [F, nC, 6N, nw] and ``info`` [F, nC, nw];
     farm f's rows are what ``solve_dynamics_farm`` returns for that farm alone, bit for bit."""
-    N, nC, nw = int(n_fowt), cases.n_cases, batch.nw
+    N = int(n_fowt)
     cases.check_ops(batch)
     if N < 1 or batch.n_designs % N:
         raise ValueError("n_fowt must divide the batch's %d designs" % batch.n_designs)
-    F, n = batch.n_designs // N, 6 * N
-    mats, shared = _farm_batch_matrices(F, n, M_arr, B_arr, C_arr)
-    want = tuple(dict.fromkeys(tuple(want) + ("Xi", "status")))
-    outs = dict(out) if out is not None else {}
-    for k_, v in _alloc_outputs(batch.n_designs, nC, nw, tuple(k for k in want if k not in outs)).items():
-        outs[k_] = v
-    outs.setdefault("Xi_sys", np.zeros([F, nC, n, nw], dtype=np.complex128))
-    outs.setdefault("info", np.zeros([F, nC, nw], dtype=_I4))
-    for k_, shape, dt in (("Xi_sys", (F, nC, n, nw), np.complex128), ("info", (F, nC, nw), _I4)):
-        if outs[k_].shape != shape or outs[k_].dtype != dt or not outs[k_].flags.c_contiguous:
-            raise ValueError("out[%r] must be a C-contiguous %s array %s" % (k_, np.dtype(dt).name, list(shape)))
-    f = RaftkFarmBatch()
-    f.n_farms, f.n_fowt, f.arr_shared = F, N, shared
-    for nm in ("M_arr", "B_arr", "C_arr"):
-        setattr(f, nm, mats[nm].ctypes.data if nm in mats else None)
-    f.Xi_sys, f.info = outs["Xi_sys"].ctypes.data, outs["info"].ctypes.data
-    c = _host_struct(cases)
-    o = RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), 0, 0)
-    os_ = _out_struct(outs, lambda a: a.ctypes.data)
-    check(lib.raftk_solve_dynamics_farm_batch_host(C.byref(_host_struct(batch)), C.byref(c), C.byref(o), C.byref(os_), C.byref(f)))
-    if _plan_overflowed(outs):                      # Xi_sys was assembled from those units' zero loads: solve it all again
-        check(lib.raftk_solve_dynamics_farm_batch_host(C.byref(_host_struct(worst_case_hints(batch))), C.byref(c), C.byref(o), C.byref(os_),
-                                                       C.byref(f)))
-        _raise_on_plan(outs)
-    return outs
+    return _solve_farms(batch, cases, N, batch.n_designs // N, M_arr, B_arr, C_arr, _opts(n_iter, tol, xi_start, cluster_size), want,
+                        out)
 
 
 FLAG_NAN, FLAG_SINGULAR, FLAG_PLAN, FLAG_XCHG = 1, 2, 4, 8        # include/raftk.h RAFTK_FLAG_*
@@ -530,10 +558,8 @@ def raise_on_flags(status):
 def hydro_excitation(batch, cases, want=("F_iner", "F_BEM", "zeta")):
     """FOWT.calcHydroExcitation for every (design, case) (raft_fowt.py:1732-1888), host buffers."""
     outs = _alloc_outputs(batch.n_designs, cases.n_cases, batch.nw, want)
-    d = batch.struct(_host_ptr(batch.arrays))
-    c = cases.struct(_host_ptr(cases.arrays))
     os_ = _out_struct(outs, lambda a: a.ctypes.data)
-    check(lib.raftk_hydro_excitation_host(C.byref(d), C.byref(c), C.byref(os_)))
+    check(lib.raftk_hydro_excitation_host(C.byref(_host_struct(batch)), C.byref(_host_struct(cases)), C.byref(os_)))
     return outs
 
 
@@ -643,33 +669,21 @@ def _slender_inputs(packed, cases):
     return batch, sb, CaseTable(base, zeta=base.get("zeta"), ops=cases.ops)
 
 
-def _slender_shapes(nD, nC, nw, nw2):
-    return dict(Xi=([nD, nC, 6, nw], "c"), status=([nD, nC, 4], "i"), B_drag=([nD, nC, 6, 6], "f"), F_drag=([nD, nC, 6, nw], "c"),
-                F_iner=([nD, nC, 6, nw], "c"), F_BEM=([nD, nC, 6, nw], "c"), zeta=([nC, nw], "f"), F_2nd=([nD, nC, 6, nw], "f"),
-                F_2nd_mean=([nD, nC, 6], "f"), Xi_last=([nD, nC, 6, nw], "c"), qtf=([nD, nC, nw2, nw2, 6], "c"), Xi_rao=([nD, nC, 6, nw2], "c"))
-
-
-def _slender_want(want, shapes):
-    want = tuple(dict.fromkeys(("Xi", "status") + tuple(want)))
-    bad = [k for k in want if k not in shapes]
-    if bad:
-        raise ValueError("unknown outputs %s (known: %s)" % (bad, ", ".join(shapes)))
-    return want
+def _check_slender_iters(n_iter):
+    if n_iter < 1:
+        raise ValueError("potSecOrder 1 needs nIter >= 1")
 
 
 def slender_flow_host(packed, cases, n_iter=10, tol=0.01, xi_start=0.0, cluster_size=0, want=("Xi", "status", "B_drag"), qtf_chunk=0):
     """``solve_dynamics_slender`` in ONE library call (raftk_solve_dynamics_slender_host: the whole flow on the device, host
     buffers in and out) -> dict of NumPy arrays named as in ``want`` (``SlenderSession``'s names)."""
     batch, sb, ct = _slender_inputs(packed, cases)
-    if n_iter < 1:
-        raise ValueError("potSecOrder 1 needs nIter >= 1")
-    shapes = _slender_shapes(batch.n_designs, ct.n_cases, batch.nw, sb.nw2)
-    want = _slender_want(want, shapes)
-    dt = dict(c=np.complex128, i=_I4, f=_F8)
-    outs = {k: np.zeros(shapes[k][0], dtype=dt[shapes[k][1]]) for k in want}
+    _check_slender_iters(n_iter)
+    want = tuple(dict.fromkeys(("Xi", "status") + tuple(want)))
+    outs = _alloc_outputs(batch.n_designs, ct.n_cases, batch.nw, want, _SLENDER_OUTPUTS, sb.nw2)
     so = RaftkSlenderOutputs(outs["qtf"].ctypes.data if "qtf" in outs else None, outs["Xi_rao"].ctypes.data if "Xi_rao" in outs else None,
                              int(qtf_chunk), 0)
-    o = RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), 0, 0)
+    o = _opts(n_iter, tol, xi_start, cluster_size)
     check(lib.raftk_solve_dynamics_slender_host(C.byref(_host_struct(batch)), C.byref(sb.struct(_host_ptr(sb.arrays))), C.byref(_host_struct(ct)),
                                                 C.byref(o), C.byref(_out_struct(outs, lambda a: a.ctypes.data)), C.byref(so)))
     return outs
@@ -687,20 +701,17 @@ class SlenderSession:
         import torch
         self.torch = torch
         batch, sb, ct = _slender_inputs(packed, cases)
-        shapes = _slender_shapes(batch.n_designs, ct.n_cases, batch.nw, sb.nw2)
-        self.want = want = _slender_want(want, shapes)
-        self.dev = DeviceSession(batch, ct, device=device, workspace_bytes=0,
-                                 want=tuple(k for k in want if k not in ("Xi_last", "qtf", "Xi_rao")))
+        self.want = want = tuple(dict.fromkeys(("Xi", "status") + tuple(want)))
+        _check_outputs(want, _SLENDER_OUTPUTS)
+        own = tuple(k for k in want if k in ("Xi_last", "qtf", "Xi_rao"))
+        self.dev = DeviceSession(batch, ct, device=device, workspace_bytes=0, want=tuple(k for k in want if k not in own))
         self.device, self.batch, self.slender = self.dev.device, batch, sb
         self.d_struct, self.c_struct = self.dev.d_struct, self.dev.c_struct
-        dt = dict(c=torch.complex128, i=torch.int32, f=torch.float64)
         with torch.cuda.device(self.device):
             self.st = {k: torch.from_numpy(v).to(self.device) for k, v in sb.arrays.items()}
             self.s_struct = sb.struct(lambda name: self.st[name].data_ptr())
             self.out = dict(self.dev.out)
-            for k in ("Xi_last", "qtf", "Xi_rao"):
-                if k in want:
-                    self.out[k] = torch.zeros(shapes[k][0], dtype=dt[shapes[k][1]], device=self.device)
+            self.out.update(_alloc_outputs(batch.n_designs, ct.n_cases, batch.nw, own, _SLENDER_OUTPUTS, sb.nw2, _torch_zeros(self.device)))
             self.o_struct = _out_struct(self.out, lambda t: t.data_ptr())
             ptr = lambda k: self.out[k].data_ptr() if k in self.out else None   # noqa: E731
             self.so = RaftkSlenderOutputs(ptr("qtf"), ptr("Xi_rao"), int(qtf_chunk), 0)
@@ -711,9 +722,8 @@ class SlenderSession:
 
     def solve(self, n_iter=10, tol=0.01, xi_start=0.0, cluster_size=0):
         """Enqueue the potSecOrder 1 solve of every unit on the current stream; returns the output dict (async)."""
-        if n_iter < 1:
-            raise ValueError("potSecOrder 1 needs nIter >= 1")
-        o = RaftkSolveOpts(int(n_iter), int(cluster_size), float(tol), float(xi_start), 0, 0)
+        _check_slender_iters(n_iter)
+        o = _opts(n_iter, tol, xi_start, cluster_size)
         with self.torch.cuda.device(self.device):
             check(lib.raftk_solve_dynamics_slender_dev(C.byref(self.d_struct), C.byref(self.s_struct), C.byref(self.c_struct), C.byref(o),
                                                        C.byref(self.o_struct), C.byref(self.so), self.workspace.data_ptr(),
@@ -755,31 +765,25 @@ def solve_dynamics_slender(packed, cases, n_iter=10, tol=0.01, xi_start=0.0, clu
     wave train per case).  Extra outputs: F_2nd, F_2nd_mean, qtf [nD,nC,nw2,nw2,6]."""
     if isinstance(packed, dict):
         packed = [packed]
-    if "primary" in cases.arrays:
-        raise NotImplementedError("potSecOrder 1 with several wave trains fails in the reference itself (raft_model.py:1229 rebinds Fhydro_2nd)")
-    if n_iter < 1:
-        raise ValueError("potSecOrder 1 needs nIter >= 1")
-    plain = [{k: v for k, v in P.items() if not k.startswith(("qtf", "qs_"))} for P in packed]
-    batch = DesignBatch(plain)
+    batch, sb, ct = _slender_inputs(packed, cases)
+    _check_slender_iters(n_iter)
     nD, nC, nw = batch.n_designs, cases.n_cases, batch.nw
-    base = {k: v for k, v in cases.arrays.items() if k not in ("F_2nd", "Xi_init")}
+    base = ct.arrays
     wantA = tuple(dict.fromkeys(tuple(want) + ("Xi", "status", "zeta", "Xi_last")))
-    A = solve_dynamics(batch, CaseTable(base, zeta=base.get("zeta"), ops=cases.ops), n_iter=n_iter, tol=tol, xi_start=xi_start, cluster_size=cluster_size, want=wantA)
-    qw = np.ascontiguousarray(packed[0]["qs_w"], dtype=_F8)
+    A = solve_dynamics(batch, ct, n_iter=n_iter, tol=tol, xi_start=xi_start, cluster_size=cluster_size, want=wantA)
+    qw = sb.arrays["w"]
     beta_rad = cases.arrays["beta_deg"] * 0.017453292519943295
     qtf = np.zeros([nD, nC, len(qw), len(qw), 6], dtype=np.complex128)
     for d, P in enumerate(packed):
-        if not np.array_equal(P["qs_w"], qw):
-            raise ValueError("all designs of a batch must share the second-order frequency grid")
         Xi2 = np.zeros([nC, 6, len(qw)], dtype=np.complex128)
         for c in range(nC):
             r = get_rao(A["Xi"][d, c], A["zeta"][c])
             for a in range(6):
                 Xi2[c, a] = np.interp(qw, batch.w, r[a], left=0, right=0)          # raft_fowt.py:2021-2023
         qtf[d] = qtf_slender(P, beta_rad, Xi2)
-    qb = DesignBatch(plain)
-    qb.arrays["qtf_w"], qb.arrays["qtf_heads"] = qw, np.zeros(1)
-    qb.arrays["qtf"] = np.ascontiguousarray(qtf.reshape(nD, nC, len(qw), len(qw), 1, 6))
+    qb = copy.copy(batch)                                                           # the designs with these QTFs as their table
+    qb.__dict__.pop("_host_struct_cache", None)
+    qb.arrays = _Tables(batch.arrays, qtf_w=qw, qtf_heads=np.zeros(1), qtf=np.ascontiguousarray(qtf.reshape(nD, nC, len(qw), len(qw), 1, 6)))
     qb.n_qtf_w, qb.n_qtf_head, qb.qtf_shared = len(qw), 1, 2
     F2 = second_order_force(qb, CaseTable(base, zeta=base.get("zeta")))
     B = solve_dynamics(batch, CaseTable(base, zeta=base.get("zeta"), F_2nd=F2["F_2nd"], Xi_init=A["Xi_last"], ops=cases.ops), n_iter=n_iter - 1, tol=tol,
@@ -899,7 +903,7 @@ class _GeneralResident:
 
     def _enqueue(self, entry, structs, n_iter, tol, xi_start, *max_chunk):
         """``entry`` (a raftk_general_*_dev solve) on the resident tables and outputs, on torch's current stream."""
-        o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
+        o = _opts(n_iter, tol, xi_start)
         ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
         with self.torch.cuda.device(self.device):
             stream = self.torch.cuda.current_stream(self.device).cuda_stream
@@ -1012,7 +1016,7 @@ def general_solve_dynamics(P, M, B, Cm, cases, n_iter=10, tol=0.01, xi_start=0.0
     Fb = np.zeros([nC, n, nw], dtype=np.complex128) if F_BEM else None
     F2, F2m = (np.zeros([nC, 6, nw]), np.zeros([nC, 6])) if F_2nd else (None, None)
     c = cases.struct(_host_ptr(cases.arrays))
-    o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
+    o = _opts(n_iter, tol, xi_start)
     hp = lambda a: a.ctypes.data if a is not None else None   # noqa: E731
     fp, qp = (C.byref(f) if f is not None else None), (C.byref(q) if q is not None else None)
     if max_chunk_cases is None:
@@ -2025,7 +2029,7 @@ def general_solve_dynamics_batch(designs, cases, n_iter=10, tol=0.01, xi_start=0
     Fb = np.zeros([nD, nC, n, nw], dtype=np.complex128) if F_BEM else None
     F2, F2m = (np.zeros([nD, nC, 6, nw]), np.zeros([nD, nC, 6])) if F_2nd else (None, None)
     c = cases.struct(_host_ptr(cases.arrays))
-    o = RaftkSolveOpts(int(n_iter), 0, float(tol), float(xi_start), 0, 0)
+    o = _opts(n_iter, tol, xi_start)
     hp = lambda a: a.ctypes.data if a is not None else None   # noqa: E731
     check(lib.raftk_general_batch_solve_dynamics_host(*_refs(g, b, f, q), C.byref(c), C.byref(o), Xi.ctypes.data, st.ctypes.data, hp(Fb),
                                                       hp(F2), hp(F2m), int(max_chunk_units)))
@@ -2120,10 +2124,8 @@ def second_order_force(batch, cases):
     if batch.n_qtf_w == 0:
         raise ValueError("the designs carry no QTF table (potSecOrder 2 / packer.pack_qtf)")
     outs = _alloc_outputs(batch.n_designs, cases.n_cases, batch.nw, ("F_2nd", "F_2nd_mean"))
-    d = batch.struct(_host_ptr(batch.arrays))
-    c = cases.struct(_host_ptr(cases.arrays))
     os_ = _out_struct(outs, lambda a: a.ctypes.data)
-    check(lib.raftk_second_order_force_host(C.byref(d), C.byref(c), C.byref(os_)))
+    check(lib.raftk_second_order_force_host(C.byref(_host_struct(batch)), C.byref(_host_struct(cases)), C.byref(os_)))
     return outs
 
 
@@ -2139,19 +2141,15 @@ def hydro_linearization(batch, cases, Xi, want=("B_drag", "F_drag")):
     if Xi.shape != (nD, nC, 6, nw):
         raise ValueError("Xi must have shape [nD,nC,6,nw] or [6,nw]")
     outs = _alloc_outputs(nD, nC, nw, want)
-    d = batch.struct(_host_ptr(batch.arrays))
-    c = cases.struct(_host_ptr(cases.arrays))
     os_ = _out_struct(outs, lambda a: a.ctypes.data)
-    check(lib.raftk_hydro_linearization_host(C.byref(d), C.byref(c), Xi.ctypes.data, C.byref(os_)))
+    check(lib.raftk_hydro_linearization_host(C.byref(_host_struct(batch)), C.byref(_host_struct(cases)), Xi.ctypes.data, C.byref(os_)))
     return outs
 
 
 def farm_workspace_bytes(n_fowt, n_cases, nw):
-    """Device workspace the farm system response needs (raftk_farm_workspace_bytes): 0 while the [6N][6N+1] system fits in
-    shared memory, else one slab per resident CTA of the global-memory kernel.  Answers for an H100 without a device."""
-    d, c, f = RaftkDesigns(), RaftkCases(), RaftkFarm()
-    d.n_designs, d.nw, c.n_cases, f.n_fowt = int(n_fowt), int(nw), int(n_cases), int(n_fowt)
-    return int(lib.raftk_farm_workspace_bytes(C.byref(d), C.byref(c), C.byref(f)))
+    """Device workspace the farm system response needs: 0 while the [6N][6N+1] system fits in shared memory, else one slab
+    per resident CTA of the global-memory kernel.  Answers for an H100 without a device."""
+    return farm_batch_workspace_bytes(1, n_fowt, n_cases, nw)
 
 
 def farm_batch_workspace_bytes(n_farms, n_fowt, n_cases, nw):
@@ -2358,6 +2356,8 @@ class DeviceSession:
         """``tables=True`` sizes the workspace for ``excitation()`` / ``linearization()`` (global wave tables);
         the default covers ``solve()`` only (the fused solver keeps its tables on chip).  ``out_tensors``: outputs the
         caller already owns (name -> tensor of the documented shape), e.g. this rank's block of a peer-shared array."""
+        want = tuple(dict.fromkeys(tuple(want) + ("Xi", "status") + (("F_2nd", "F_2nd_mean") if batch.n_qtf_w else ())))
+        _check_outputs(want, _SESSION_OUTPUTS)
         import torch
         self.torch = torch
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
@@ -2388,18 +2388,14 @@ class DeviceSession:
             need = (lib.raftk_workspace_bytes if tables else lib.raftk_solve_workspace_bytes)(C.byref(self.d_struct), cases.n_cases)
             self.workspace_bytes = int(need if workspace_bytes is None else workspace_bytes)
             self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=self.device)
-            nD, nC, nw = batch.n_designs, cases.n_cases, batch.nw
-            want = tuple(dict.fromkeys(tuple(want) + ("Xi", "status") + (("F_2nd", "F_2nd_mean") if batch.n_qtf_w else ())))
-            shapes = dict(Xi=([nD, nC, 6, nw], torch.complex128), status=([nD, nC, 4], torch.int32),
-                          F_2nd=([nD, nC, 6, nw], torch.float64), F_2nd_mean=([nD, nC, 6], torch.float64),
-                          B_drag=([nD, nC, 6, 6], torch.float64), F_drag=([nD, nC, 6, nw], torch.complex128),
-                          F_iner=([nD, nC, 6, nw], torch.complex128), F_BEM=([nD, nC, 6, nw], torch.complex128),
-                          zeta=([nC, nw], torch.float64))
+            shapes = _output_table(batch.n_designs, cases.n_cases, batch.nw)
             given = dict(out_tensors or {})
             for k, t in given.items():
-                if tuple(t.shape) != tuple(shapes[k][0]) or t.dtype != shapes[k][1] or not t.is_contiguous():
-                    raise ValueError("out_tensors[%r] must be a contiguous %s tensor of shape %s" % (k, shapes[k][1], shapes[k][0]))
-            self.out = {k: (given[k] if k in given else torch.zeros(shapes[k][0], dtype=shapes[k][1], device=self.device)) for k in want}
+                shape, dt = shapes[k][0], _torch_dtype(shapes[k][1])
+                if tuple(t.shape) != tuple(shape) or t.dtype != dt or not t.is_contiguous():
+                    raise ValueError("out_tensors[%r] must be a contiguous %s tensor of shape %s" % (k, dt, shape))
+            zeros = _torch_zeros(self.device)
+            self.out = {k: (given[k] if k in given else zeros(*shapes[k])) for k in want}
             self.o_struct = _out_struct(self.out, lambda t: t.data_ptr())
 
     def _stream(self):
@@ -2409,7 +2405,7 @@ class DeviceSession:
         """Solve options; from the second call with the same cluster size on, the per-design plan blobs that the first call
         left in the session's workspace are reused (the session owns tables and workspace, so they cannot have changed)."""
         key = int(cluster_size)
-        o = RaftkSolveOpts(int(n_iter), key, float(tol), float(xi_start), 1 if getattr(self, "_plan_key", None) == key else 0, 0)
+        o = _opts(n_iter, tol, xi_start, key, 1 if getattr(self, "_plan_key", None) == key else 0)
         self._plan_key = key
         return o
 
@@ -2441,36 +2437,23 @@ class DeviceSession:
         of farm f), array matrices [6N,6N] for every farm or [F,6N,6N] -> (Xi_sys [F,nC,6N,nw], info [F,nC,nw]).  The
         matrices, outputs and workspace of either form are set up on its first call and kept with the session."""
         torch = self.torch
-        nC, nw = self.cases.n_cases, self.batch.nw
         N = self.batch.n_designs if n_fowt is None else int(n_fowt)
         if N < 1 or self.batch.n_designs % N:
             raise ValueError("n_fowt must divide the session's %d designs" % self.batch.n_designs)
-        F, n = self.batch.n_designs // N, 6 * N
-        key = "_farm" if n_fowt is None else "_farm_batch"
+        # one farm is kept as the single-farm struct (raftk_farm), which callers hand to the single-farm entries, and launches
+        # through them; its matrices and outputs are set up as a batch of one
+        key, query, launch = (("_farm", lib.raftk_farm_workspace_bytes, lib.raftk_farm_response_ws_dev) if n_fowt is None else
+                              ("_farm_batch", lib.raftk_farm_batch_workspace_bytes, lib.raftk_farm_batch_response_ws_dev))
         if not hasattr(self, key) or getattr(self, key)[0].n_fowt != N:
-            host, shared = _farm_batch_matrices(F, n, M_arr, B_arr, C_arr)
-            lead = [] if n_fowt is None else [F]
             with torch.cuda.device(self.device):
-                mats = {nm: (torch.from_numpy(host[nm]).to(self.device) if nm in host else None) for nm in ("M_arr", "B_arr", "C_arr")}
-                xi = torch.zeros(lead + [nC, n, nw], dtype=torch.complex128, device=self.device)
-                info = torch.zeros(lead + [nC, nw], dtype=torch.int32, device=self.device)
-            if n_fowt is None:
-                f = RaftkFarm()
-                query = lib.raftk_farm_workspace_bytes
-            else:
-                f = RaftkFarmBatch()
-                f.n_farms, f.arr_shared = F, shared
-                query = lib.raftk_farm_batch_workspace_bytes
-            f.n_fowt = N
-            for nm, t in mats.items():
-                setattr(f, nm, t.data_ptr() if t is not None else None)
-            f.Xi_sys, f.info = xi.data_ptr(), info.data_ptr()
-            wsb = int(query(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(f)))
-            with torch.cuda.device(self.device):
+                f, mats, xi, info = _farm_setup(N, None if n_fowt is None else self.batch.n_designs // N, self.cases.n_cases,
+                                                self.batch.nw, M_arr, B_arr, C_arr, device=self.device)
+                if n_fowt is None:
+                    f = RaftkFarm(n_fowt=N, M_arr=f.M_arr, B_arr=f.B_arr, C_arr=f.C_arr, Xi_sys=f.Xi_sys, info=f.info)
+                wsb = int(query(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(f)))
                 ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=self.device)
             setattr(self, key, (f, mats, xi, info, ws, wsb))
         f, _, xi, info, ws, wsb = getattr(self, key)
-        launch = lib.raftk_farm_response_ws_dev if n_fowt is None else lib.raftk_farm_batch_response_ws_dev
         with torch.cuda.device(self.device):
             check(launch(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f), ws.data_ptr(), wsb, self._stream()))
         return xi, info

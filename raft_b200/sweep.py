@@ -137,12 +137,7 @@ def solve_sweep(packed_designs, cases, n_iter=10, tol=0.01, xi_start=0.0, device
     """Solve this rank's designs on its GPU and all-gather the RAOs: -> (Xi [n_total,nC,6,nw], status [n_total,nC,4])."""
     from . import solver
     batch, ct = solver.DesignBatch(packed_designs), solver.CaseTable(cases)
-    out = solver.DeviceSession(batch, ct, device=device).solve(n_iter=n_iter, tol=tol, xi_start=xi_start)
-    if bool(((out["status"][..., 2] & solver.FLAG_PLAN) != 0).any()):
-        # units whose step classes overflowed the hints ran no pass and hold zeros: solve again with worst-case tables
-        out = solver.DeviceSession(solver.worst_case_hints(batch), ct, device=device).solve(n_iter=n_iter, tol=tol, xi_start=xi_start)
-        if bool(((out["status"][..., 2] & solver.FLAG_PLAN) != 0).any()):
-            raise solver._lib.RaftkError("step-class tables overflowed even with worst-case sizes")
+    out = solver._retry_on_plan(batch, lambda b: solver.DeviceSession(b, ct, device=device).solve(n_iter=n_iter, tol=tol, xi_start=xi_start))
     n_total = len(packed_designs) if n_total is None else n_total
     return all_gather_blocks(out["Xi"], n_total, group), all_gather_blocks(out["status"], n_total, group)
 
@@ -154,7 +149,7 @@ def solve_sweep_slender(packed_designs, cases, n_iter=10, tol=0.01, xi_start=0.0
     from . import solver
     out = solver.SlenderSession(packed_designs, solver.CaseTable(cases), device=device, qtf_chunk=qtf_chunk).solve(n_iter=n_iter, tol=tol,
                                                                                                                   xi_start=xi_start)
-    if bool(((out["status"][..., 2] & solver.FLAG_PLAN) != 0).any()):
+    if solver._plan_overflowed(out["status"]):
         raise solver._lib.RaftkError("step-class tables overflowed the hints of the design batch")
     n_total = len(packed_designs) if n_total is None else n_total
     return all_gather_blocks(out["Xi"], n_total, group), all_gather_blocks(out["status"], n_total, group)

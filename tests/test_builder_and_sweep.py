@@ -317,6 +317,25 @@ def test_host_struct_cache_follows_table_edits():
     assert solver._host_struct(c) is not t1
 
 
+def test_unknown_outputs_are_refused_before_any_device_use():
+    """An output name an entry does not offer is the same ValueError on the host solves, the potSecOrder 1 flows and
+    DeviceSession (which has no Xi_last), raised before a launch or any use of a device."""
+    from raft_b200 import solver
+    _, P = load_golden("cfg2_VolturnUS-S_nw64")
+    _, Ps = load_golden("slender_VolturnUS-S")
+    cs = dict(Hs=[6.0], Tp=[12.0], gamma=[0.0], beta_deg=[0.0], spec=np.zeros(1, dtype=np.int32))
+    b, c = solver.DesignBatch([P]), solver.CaseTable(cs)
+    before = solver.launch_count()
+    for call in (lambda: solver.solve_dynamics(b, c, want=("Xi", "F_nope")),
+                 lambda: solver.slender_flow_host([Ps], c, want=("F_nope",)),
+                 lambda: solver.SlenderSession([Ps], c, want=("F_nope",)),
+                 lambda: solver.DeviceSession(b, c, want=("F_nope",)),
+                 lambda: solver.DeviceSession(b, c, want=("Xi_last",))):
+        with pytest.raises(ValueError, match="unknown outputs"):
+            call()
+    assert solver.launch_count() == before
+
+
 def _general_family():
     from raft_b200 import batch_builder, grid
     members = [

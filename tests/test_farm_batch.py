@@ -143,6 +143,17 @@ def test_python_entry_checks_shapes():
         solver.solve_dynamics_farm_batch(batch, cases, 2, C_arr=np.zeros([2, 12, 12]))
     with pytest.raises(ValueError, match="Xi_sys"):
         solver.solve_dynamics_farm_batch(batch, cases, 2, out=dict(Xi_sys=np.zeros([1, 12, 48], dtype=complex)))
+    one = solver.DesignBatch(packs)                                           # the single-farm form: a batch of one farm
+    for bad in (np.eye(6), np.zeros([2, 12, 12]), np.zeros([1, 12, 13])):
+        with pytest.raises(ValueError, match=r"must all be \[12, 12\] or all be \[1, 12, 12\]"):
+            solver.solve_dynamics_farm(one, cases, C_arr=bad)
+    with pytest.raises(ValueError, match="must all be"):
+        solver.solve_dynamics_farm(one, cases, C_arr=np.eye(12), M_arr=np.zeros([1, 12, 12]))
+    for bad in (np.zeros([1, 1, 12, 48], dtype=complex), np.zeros([1, 12, 48]), np.zeros([1, 12, 96], dtype=complex)[..., ::2]):
+        with pytest.raises(ValueError, match=re.escape("out['Xi_sys'] must be a C-contiguous complex128 array [1, 12, 48]")):
+            solver.solve_dynamics_farm(one, cases, out=dict(Xi_sys=bad))
+    with pytest.raises(ValueError, match=re.escape("out['info'] must be a C-contiguous int32 array [1, 48]")):
+        solver.solve_dynamics_farm(one, cases, out=dict(info=np.zeros([1, 1, 48], dtype=np.int32)))
 
 
 # ---- farm batches from the fixtures -------------------------------------------------------------------------------------
@@ -271,6 +282,32 @@ def test_every_farm_equals_the_single_farm_entry(N, kernel, nw):
     _assert_farms_equal_single(packs, lambda f: ct, C_arr, out, N, kernel)
     for f in range(1, F):
         assert not np.array_equal(out["Xi_sys"][f], out["Xi_sys"][0])
+    # the single-farm C entry, which solve_dynamics_farm no longer calls (it is the farm-batch entry's batch of one), gives
+    # the same bits, launches and dispatch record; a [1, 6N, 6N] array matrix is that batch's own (arr_shared = 0)
+    row = solver.DesignBatch(packs[1])
+    l0 = solver.launch_count()
+    one = solver.solve_dynamics_farm(row, ct, C_arr=C_arr[1], want=PER_FOWT)
+    l1, rec = solver.launch_count(), solver.last_dispatch()
+    raw = _single_farm_entry(row, ct, C_arr[1], PER_FOWT)
+    assert solver.launch_count() - l1 == l1 - l0 and solver.last_dispatch() == rec and rec["kernel"] == kernel
+    lead = solver.solve_dynamics_farm(row, ct, C_arr=C_arr[1][None], want=PER_FOWT)
+    assert solver.last_dispatch() == rec
+    for k in ("Xi_sys", "info") + PER_FOWT:
+        assert np.array_equal(raw[k], one[k]) and np.array_equal(lead[k], one[k]), k
+
+
+def _single_farm_entry(batch, ct, C_arr, want):
+    """raftk_solve_dynamics_farm_host called directly on one farm: the per-FOWT outputs plus Xi_sys and info."""
+    from raft_b200 import _lib, solver
+    N, nC, nw = batch.n_designs, ct.n_cases, batch.nw
+    outs = solver._alloc_outputs(N, nC, nw, want)
+    xi, info = np.zeros([nC, 6 * N, nw], dtype=complex), np.zeros([nC, nw], dtype=np.int32)
+    Cm = np.ascontiguousarray(C_arr, dtype=float)
+    f = _lib.RaftkFarm(n_fowt=N, C_arr=Cm.ctypes.data, Xi_sys=xi.ctypes.data, info=info.ctypes.data)
+    o = _lib.RaftkSolveOpts(10, 0, 0.01, 0.0, 0, 0)
+    _lib.check(_lib.lib.raftk_solve_dynamics_farm_host(C.byref(solver._host_struct(batch)), C.byref(solver._host_struct(ct)), C.byref(o),
+                                                       C.byref(solver._out_struct(outs, lambda a: a.ctypes.data)), C.byref(f)))
+    return dict(outs, Xi_sys=xi, info=info)
 
 
 @gpu
