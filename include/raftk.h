@@ -723,6 +723,30 @@ int raftk_solve_dynamics_farm_batch_host(const raftk_designs *d, const raftk_cas
                                          const raftk_outputs *out, const raftk_farm_batch *f);
 
 /*
+ * Farm batches sharded over GPUs (raft_b200.sweep.ShardedFarmSolve): rank r solves a contiguous run of whole farms and stores
+ * their results into EVERY rank's gathered copy (raftk_peers above); a farm is never split across ranks.  F_max is the largest
+ * shard: smaller shards leave their last farm slots unwritten.  Rank p's copy holds
+ *     gathered[p]: complex Xi_sys [n_ranks * F_max, nC, 6N, nw]    (peers.block_elems = F_max * nC * 6N * nw)
+ *     status[p]:   int32 info [n_ranks * F_max, nC, nw], followed by the per-FOWT status [n_ranks * F_max * N, nC, 4]
+ *     flags[p]:    the arrival flags of raftk_peer_barrier_dev.
+ * raftk_farm_batch_response_gather_dev is raftk_farm_batch_response_ws_dev for this rank's f->n_farms farms, which are farms
+ * [farm_row0, farm_row0 + n_farms) of the gathered copies (farm_row0 = rank * F_max); f->Xi_sys and f->info must be those rows of
+ * this rank's own copy, and `solved` must carry the per-FOWT status of raftk_solve_dynamics_dev.  With the system in shared
+ * memory or registers (N <= 20 on an H100) the solve kernel itself stores each finished (farm, case, bin) solution and info word
+ * into the other ranks' copies; larger farms (k_farm_response_global, whose LU leaves Xi_sys final only at its end) are copied
+ * by a second kernel, k_farm_publish, that this entry enqueues after the solve.  Either way the per-FOWT status rows of the
+ * rank's farms go to every copy, and the results are identical to raftk_farm_batch_response_ws_dev's, bit for bit.  Follow with
+ * raftk_peer_barrier_dev; a rank without farms (more ranks than farms) calls only the barrier.
+ * RAFTK_EINVAL before any launch, besides every refusal of raftk_farm_batch_response_ws_dev: NULL peers, n_ranks outside
+ * [1, RAFTK_MAX_PEERS] or rank outside [0, n_ranks), a rank's gathered / flags / status pointer missing, no info or per-FOWT
+ * status, block_elems not a positive multiple of nC * 6N * nw, n_farms > F_max, farm_row0 other than rank * F_max, and
+ * Xi_sys / info that are not this rank's rows of its own copy.
+ */
+int raftk_farm_batch_response_gather_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
+                                         const raftk_farm_batch *f, const raftk_peers *peers, int32_t farm_row0, void *workspace,
+                                         size_t workspace_bytes, void *stream);
+
+/*
  * Output channels of farm batches: mooring line tensions (the array level of Model.analyzeCases, raft_model.py:371-433, and
  * a FOWT's own lines, raft_fowt.py:2355-2399, moorMod 0) and any other real linear functional of the coupled response,
  *   Y[f,r,ch,w] = w^wpow[ch] sum_b R_f[ch,b] Xi_sys[f,r,b,w]

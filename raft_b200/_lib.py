@@ -215,6 +215,7 @@ SYMBOLS = [
     "raftk_solve_dynamics_gather_dev", "raftk_peer_barrier_dev", "raftk_general_publish_dev",
     "raftk_farm_response_dev", "raftk_solve_dynamics_farm_host", "raftk_farm_workspace_bytes", "raftk_farm_response_ws_dev",
     "raftk_farm_batch_workspace_bytes", "raftk_farm_batch_response_ws_dev", "raftk_solve_dynamics_farm_batch_host",
+    "raftk_farm_batch_response_gather_dev",
     "raftk_family_sizes", "raftk_build_family_host",
     "raftk_eigen_workspace_bytes", "raftk_eigen_dev", "raftk_eigen_host",
     "raftk_farm_channel_stats_workspace_bytes", "raftk_farm_channel_stats_dev", "raftk_farm_channel_stats_host",
@@ -360,6 +361,9 @@ def _load():
     lib.raftk_farm_batch_response_ws_dev.restype = C.c_int
     lib.raftk_solve_dynamics_farm_batch_host.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkSolveOpts), P(RaftkOutputs), P(RaftkFarmBatch)]
     lib.raftk_solve_dynamics_farm_batch_host.restype = C.c_int
+    lib.raftk_farm_batch_response_gather_dev.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkOutputs), P(RaftkFarmBatch), P(RaftkPeers),
+                                                         C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.raftk_farm_batch_response_gather_dev.restype = C.c_int
     lib.raftk_eigen_workspace_bytes.argtypes = [P(RaftkEigen)]
     lib.raftk_eigen_workspace_bytes.restype = C.c_size_t
     lib.raftk_eigen_dev.argtypes = [P(RaftkEigen), C.c_void_p, C.c_size_t, C.c_void_p]

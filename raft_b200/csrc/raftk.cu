@@ -1007,8 +1007,10 @@ static int farm_batch_shape(const raftk_designs *d, const raftk_farm_batch *f)
     return RAFTK_OK;
 }
 
+// The farm response of a batch; with `px` (raftk_farm_batch_response_gather_dev) its peer fields are set and the results also go
+// to the other ranks: the shared-memory kernels through their PEER instantiations, k_farm_response_global through k_farm_publish.
 static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm_batch *f, void *ws,
-                       size_t ws_bytes, cudaStream_t st)
+                       size_t ws_bytes, cudaStream_t st, const FarmPeerParams *px = nullptr)
 {
     if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "farm response: null argument");
     if (int rc = farm_batch_shape(d, f)) return rc;
@@ -1016,7 +1018,8 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
         return set_err(RAFTK_EINVAL, "farm response needs B_drag, F_drag, F_iner of the per-FOWT solve");
     if (d->n_bem_head > 0 && !solved->F_BEM) return set_err(RAFTK_EINVAL, "farm response: the designs carry BEM excitation, F_BEM is required");
     const int n = 6 * f->n_fowt;
-    FarmParams P;
+    FarmPeerParams Q = px ? *px : FarmPeerParams{};
+    FarmParams &P = Q;
     P.N = f->n_fowt; P.nC = c->n_cases; P.nw = d->nw; P.nF = f->n_farms;
     P.arr_stride = f->arr_shared ? 0 : (size_t)n * n;
     P.B_drag = solved->B_drag;
@@ -1048,6 +1051,12 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
         }
         g_launches++;
         CUDA_TRY(cudaGetLastError());
+        if (px) {
+            const size_t nx = (size_t)f->n_farms * c->n_cases * n * d->nw;
+            k_farm_publish<<<dim3((unsigned)std::min<size_t>((nx + 255) / 256, 1024), (unsigned)px->n_peers), 256, 0, st>>>(Q);
+            g_launches++;
+            CUDA_TRY(cudaGetLastError());
+        }
         return RAFTK_OK;
     }
     const bool warp = n <= 24;                          // one warp per (frequency, case), wpc systems per CTA; blocked LU above
@@ -1057,30 +1066,38 @@ static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk
     // grid = (frequency groups, case, farm): the y and z extents of a grid end at 65535
     if (c->n_cases > 65535) return set_err(RAFTK_EINVAL, "farm response: more than 65535 cases per call");
     if (f->n_farms > 65535) return set_err(RAFTK_EINVAL, "farm response: more than 65535 farms per call with the system in shared memory (6N <= 120)");
-    static SmemOptIn opt_w(48 * 1024), opt_b(48 * 1024), opt_wo(48 * 1024), opt_bo(48 * 1024);
-    const bool op = c->op != nullptr;                       // the instantiations with operating points
-    if (warp) CUDA_TRY(op ? opt_wo.ensure(k_farm_response<true, true>, smem) : opt_w.ensure(k_farm_response<true>, smem));
-    else CUDA_TRY(op ? opt_bo.ensure(k_farm_response<false, true>, smem) : opt_b.ensure(k_farm_response<false>, smem));
-    DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
-    CasesDev C = to_dev(c);
-    {
-        ProfScope ps(st, 1);
-        // 6N = 12 (the shipped two-FOWT farm): rows in registers, one lane per row, two systems per warp (k_farm_rows);
-        // RAFTK_FARM_SMEM=1 keeps the shared-memory warp kernel (A/B).  At 6N = 18 / 24 the register rows need 188 / 238
-        // registers, so those stay on the warp kernel.
-        const bool rows = n == 12 && !getenv("RAFTK_FARM_SMEM");
-        const unsigned gy = c->n_cases, gz = f->n_farms;
-        const dim3 gr((d->nw + 7) / 8, gy, gz), gw((d->nw + wpc - 1) / wpc, gy, gz), gb(d->nw, gy, gz);
-        if (rows) { if (op) k_farm_rows<12, true><<<gr, 128, 0, st>>>(D, C, P); else k_farm_rows<12><<<gr, 128, 0, st>>>(D, C, P); }
-        else if (warp) { if (op) k_farm_response<true, true><<<gw, 32 * wpc, smem, st>>>(D, C, P); else k_farm_response<true><<<gw, 32 * wpc, smem, st>>>(D, C, P); }
-        else { if (op) k_farm_response<false, true><<<gb, 256, smem, st>>>(D, C, P); else k_farm_response<false><<<gb, 256, smem, st>>>(D, C, P); }
-        if (rows) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_ROWS12, 128);
-        else if (warp) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_WARP, 32 * wpc);
-        else disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_BLOCK, 256);
-    }
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
-    return RAFTK_OK;
+    // 6N = 12 (the shipped two-FOWT farm): rows in registers, one lane per row, two systems per warp (k_farm_rows);
+    // RAFTK_FARM_SMEM=1 keeps the shared-memory warp kernel (A/B).  At 6N = 18 / 24 the register rows need 188 / 238
+    // registers, so those stay on the warp kernel.
+    const bool rows = n == 12 && !getenv("RAFTK_FARM_SMEM");
+    const unsigned gy = c->n_cases, gz = f->n_farms;
+    const dim3 gr((d->nw + 7) / 8, gy, gz), gw((d->nw + wpc - 1) / wpc, gy, gz), gb(d->nw, gy, gz);
+    // one instantiation per (operating points, peer stores); the shared-memory opt-in is per instantiation
+    auto go = [&](auto op_c, auto peer_c) -> int {
+        constexpr bool OP = decltype(op_c)::value, PEER = decltype(peer_c)::value;
+        static SmemOptIn opt_w(48 * 1024), opt_b(48 * 1024);
+        if (warp) CUDA_TRY(opt_w.ensure(k_farm_response<true, OP, PEER>, smem));
+        else CUDA_TRY(opt_b.ensure(k_farm_response<false, OP, PEER>, smem));
+        DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
+        CasesDev C = to_dev(c);
+        const FarmArg<PEER> &A = Q;
+        {
+            ProfScope ps(st, 1);
+            if (rows) k_farm_rows<12, OP, PEER><<<gr, 128, 0, st>>>(D, C, A);
+            else if (warp) k_farm_response<true, OP, PEER><<<gw, 32 * wpc, smem, st>>>(D, C, A);
+            else k_farm_response<false, OP, PEER><<<gb, 256, smem, st>>>(D, C, A);
+            if (rows) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_ROWS12, 128);
+            else if (warp) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_WARP, 32 * wpc);
+            else disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_BLOCK, 256);
+        }
+        g_launches++;
+        CUDA_TRY(cudaGetLastError());
+        return RAFTK_OK;
+    };
+    using T = std::true_type;
+    using F = std::false_type;
+    if (c->op) return px ? go(T{}, T{}) : go(T{}, F{});
+    return px ? go(F{}, T{}) : go(F{}, F{});
 }
 
 // the single-farm entries: farm.n_fowt names the whole batch of designs
@@ -1116,6 +1133,42 @@ extern "C" int raftk_farm_batch_response_ws_dev(const raftk_designs *d, const ra
     disp_reset();
     if (int rc = validate_op_dev(c)) return rc;
     return farm_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int raftk_farm_batch_response_gather_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
+                                                    const raftk_farm_batch *f, const raftk_peers *peers, int32_t farm_row0,
+                                                    void *workspace, size_t workspace_bytes, void *stream)
+{
+    disp_reset();
+    if (int rc = validate_peers(peers)) return rc;
+    if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "farm gather: null argument");
+    if (int rc = farm_batch_shape(d, f)) return rc;
+    if (!f->info || !solved->status) return set_err(RAFTK_EINVAL, "farm gather: farm_batch.info and the per-FOWT status are required");
+    for (int r = 0; r < peers->n_ranks; r++)
+        if (!peers->status[r]) return set_err(RAFTK_EINVAL, "farm gather: a rank's gathered info and status (peers.status) is missing");
+    const size_t per_farm = (size_t)c->n_cases * 6 * f->n_fowt * d->nw;          // complex elements of one farm's Xi_sys
+    if (c->n_cases < 1 || d->nw < 1 || peers->block_elems == 0 || peers->block_elems % per_farm)
+        return set_err(RAFTK_EINVAL, "farm gather: peers.block_elems must be F_max * nC * 6N * nw with F_max >= 1");
+    const long long F_max = (long long)(peers->block_elems / per_farm);
+    if (f->n_farms > F_max) return set_err(RAFTK_EINVAL, "farm gather: farm_batch.n_farms exceeds F_max, the farms of a rank block");
+    if (farm_row0 != (long long)peers->rank * F_max)                              // a rank writes its own block, no other rank's
+        return set_err(RAFTK_EINVAL, "farm gather: farm_row0 must be rank * F_max, the first farm slot of this rank's block");
+    const size_t info_farm = (size_t)c->n_cases * d->nw, st_farm = (size_t)f->n_fowt * c->n_cases * 4;
+    const size_t info_all = (size_t)peers->n_ranks * F_max * info_farm;
+    if (f->Xi_sys != peers->gathered[peers->rank] + 2 * (size_t)farm_row0 * per_farm ||
+        f->info != peers->status[peers->rank] + (size_t)farm_row0 * info_farm)
+        return set_err(RAFTK_EINVAL, "farm gather: farm_batch.Xi_sys and info must be this rank's farms in its own gathered copy");
+    if (int rc = validate_op_dev(c)) return rc;
+    FarmPeerParams px{};
+    px.n_peers = peers->n_ranks;
+    px.status = solved->status;
+    for (int r = 0; r < peers->n_ranks; r++) {
+        const bool other = r != peers->rank;
+        px.X[r] = other ? reinterpret_cast<double2 *>(peers->gathered[r]) + (size_t)farm_row0 * per_farm : nullptr;
+        px.I[r] = other ? peers->status[r] + (size_t)farm_row0 * info_farm : nullptr;
+        px.S[r] = peers->status[r] + info_all + (size_t)farm_row0 * st_farm;
+    }
+    return farm_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream, &px);
 }
 
 

@@ -221,6 +221,47 @@ struct FarmParams {
 };
 #define FARM_WPC 4
 
+// The farm batch sharded over ranks (raftk_farm_batch_response_gather_dev): the PEER instantiations also store every result
+// into the other ranks' gathered copies.  Pointers are rank p's copy as mapped in this process, already at this rank's first
+// farm, so a slot has the index of the local write.  X[p] / I[p] (Xi_sys, info) are NULL for this rank, whose local write
+// lands in its own copy; S[p] (the per-FOWT status rows of the drag solve, copied from `status`) is set for every rank.
+struct FarmPeerParams : FarmParams {
+    int n_peers;
+    const int *status;                          // [nF * N][nC][4]
+    double2 *X[RAFTK_MAX_PEERS];                // [nF][nC][6N][nw]
+    int *I[RAFTK_MAX_PEERS];                    // [nF][nC][nw]
+    int *S[RAFTK_MAX_PEERS];                    // [nF * N][nC][4]
+};
+template <bool PEER> using FarmArg = typename std::conditional<PEER, FarmPeerParams, FarmParams>::type;
+
+// farm f's N status rows of case c to every rank's copy, spread over the gsize threads of a group
+__device__ __forceinline__ void farm_peer_status(const FarmPeerParams &P, int f, int c, int gtid, int gsize)
+{
+    for (int t = gtid; t < 4 * P.N; t += gsize) {
+        const size_t o = (((size_t)f * P.N + t / 4) * P.nC + c) * 4 + (t & 3);
+        const int v = P.status[o];
+#pragma unroll 1
+        for (int p = 0; p < P.n_peers; p++) if (P.S[p]) P.S[p][o] = v;
+    }
+}
+
+// PEER epilogue of k_farm_response: system (u, iw)'s solution (column n of A [n][nc]) and info word to the other ranks, fire
+// and forget as k_rao_fused2's; the group that solved bin 0 of (farm f, case c) also publishes that farm's status rows
+__device__ __forceinline__ void farm_peer_store(const FarmPeerParams &P, const double2 *A, int nc, size_t u, int iw, int bad, int f, int c,
+                                                int gtid, int gsize)
+{
+    const int n = 6 * P.N, nw = P.nw;
+    for (int a = gtid; a < n; a += gsize) {
+        const double2 v = A[a * nc + n];
+#pragma unroll 1
+        for (int p = 0; p < P.n_peers; p++) if (P.X[p]) P.X[p][(u * n + a) * nw + iw] = v;
+    }
+    if (gtid == 0)
+#pragma unroll 1
+        for (int p = 0; p < P.n_peers; p++) if (P.I[p]) P.I[p][u * nw + iw] = bad;
+    if (iw == 0) farm_peer_status(P, f, c, gtid, gsize);
+}
+
 // The frequency-dependent terms of design i's block entry e at bin iw for a case c with an operating point: the design's
 // A_w / B_w plus the operating point's (tab_term), added to M and B.  (A secondary train's operating point is its primary's:
 // raftk_cases.op.)
@@ -273,8 +314,8 @@ __device__ __forceinline__ void farm_assemble(const DesignsDev &D, const CasesDe
     }
 }
 
-template <bool WARP, bool OP = false>
-__global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(DesignsDev D, CasesDev Cs, FarmParams P)
+template <bool WARP, bool OP = false, bool PEER = false>
+__global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(DesignsDev D, CasesDev Cs, FarmArg<PEER> P)
 {
     extern __shared__ __align__(16) double smem_raw[];
     __shared__ int piv_s[FARM_WPC], bad_s[FARM_WPC];
@@ -293,6 +334,7 @@ __global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(De
     else lu_blocked(A, n, nc, 1, &piv_s[g], &rinv_s[g], &bad_s[g]);
     for (int a = gtid; a < n; a += gsize) P.Xi[(u * n + a) * nw + iw] = A[a * nc + n];
     if (gtid == 0 && P.info) P.info[u * nw + iw] = bad_s[g];
+    if constexpr (PEER) farm_peer_store(P, A, nc, u, iw, bad_s[g], f, c, gtid, gsize);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -477,8 +519,8 @@ __global__ void __launch_bounds__(GLU_T, 2) k_system_solve_global(int n, int nw,
 // entry moves the pivot row to everybody and old row k to the pivot's lane, every row below k eliminates itself.  No shared
 // memory, no barriers; back substitution broadcasts one unknown per step.  Same assembly arithmetic as k_farm_response.
 // ------------------------------------------------------------------------------------------------
-template <int N6, bool OP = false>
-__global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, FarmParams P)
+template <int N6, bool OP = false, bool PEER = false>
+__global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, FarmArg<PEER> P)
 {
     constexpr int LPS = N6 <= 16 ? 16 : 32, SPW = 32 / LPS, NC = N6 + 1;
     const int nw = P.nw, lane = threadIdx.x & 31, r = lane & (LPS - 1);
@@ -577,6 +619,28 @@ __global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, Fa
     });
     if (live && row_ok) P.Xi[(u * N6 + r) * nw + iw] = x;
     if (live && r == 0 && P.info) P.info[u * nw + iw] = bad;
+    if constexpr (PEER) {                              // as farm_peer_store, from the lanes' registers
+        if (live) {
+#pragma unroll 1
+            for (int p = 0; p < P.n_peers; p++) {
+                if (row_ok && P.X[p]) P.X[p][(u * N6 + r) * nw + iw] = x;
+                if (r == 0 && P.I[p]) P.I[p][u * nw + iw] = bad;
+            }
+            if (iw == 0) farm_peer_status(P, f, c, r, LPS);
+        }
+    }
+}
+
+// K3e: a rank's farms solved by k_farm_response_global, to the other ranks' copies after the kernel (the global LU leaves Xi_sys
+// final only at its end): blockIdx.y = p; Xi_sys and info where X[p] / I[p] are set, the per-FOWT status rows to every S[p]
+__global__ void __launch_bounds__(256) k_farm_publish(FarmPeerParams P)
+{
+    const int p = blockIdx.y;
+    const size_t stride = (size_t)gridDim.x * 256, t0 = (size_t)blockIdx.x * 256 + threadIdx.x;
+    const size_t sys = (size_t)P.nF * P.nC, nx = sys * 6 * P.N * P.nw, ni = sys * P.nw, ns = sys * P.N * 4;
+    if (double2 *x = P.X[p]) for (size_t t = t0; t < nx; t += stride) x[t] = P.Xi[t];
+    if (int *d = P.I[p]) for (size_t t = t0; t < ni; t += stride) d[t] = P.info[t];
+    if (int *d = P.S[p]) for (size_t t = t0; t < ns; t += stride) d[t] = P.status[t];
 }
 
 // std = sqrt(1/2 sum_w |Y|^2) of one 128-thread CTA from each thread's partial sum s: warp shuffles, then the four warps

@@ -192,6 +192,36 @@ class DesignBatch:
         self.walk_exact = fused_walk_exact(a, self.k, self.depth)
         return self
 
+    PER_DESIGN = ("M0", "B0", "C0", "A_w", "B_w", "X_BEM", "bem_xyh")
+    PER_MEMBER = ("mem_frame", "mem_rA", "mem_arm", "mem_circ")
+
+    def take(self, lo, hi):
+        """Designs [lo, hi) as a batch of their own (a shard of ``sweep.ShardedFarmSolve``).  The size and step-class hints and the
+        choice of node walk stay this batch's, so every design is planned, and solved, as it is here."""
+        lo, hi = int(lo), int(hi)
+        if not 0 <= lo < hi <= self.n_designs:
+            raise ValueError("take(%d, %d): a non-empty range of the batch's %d designs" % (lo, hi, self.n_designs))
+        a = self.arrays
+        mo, ns = np.asarray(a["member_offset"]), np.asarray(a["mem_node_start"])
+        m0, m1 = int(mo[lo]), int(mo[hi])
+        n0, n1 = int(ns[m0]), int(ns[m1])
+        b = copy.copy(self)
+        b.__dict__.pop("_host_struct_cache", None)
+        b.arrays = t = _Tables()
+        for k, v in a.items():
+            if k in self.PER_DESIGN or (k == "qtf" and not self.qtf_shared):
+                t[k] = np.ascontiguousarray(v[lo:hi])
+            elif k in self.PER_MEMBER:
+                t[k] = np.ascontiguousarray(v[m0:m1])
+            elif k.startswith("node_"):
+                t[k] = np.ascontiguousarray(v[n0:n1])
+            else:
+                t[k] = v
+        t["member_offset"] = np.ascontiguousarray(mo[lo:hi + 1] - m0, dtype=_I4)
+        t["mem_node_start"] = np.ascontiguousarray(ns[m0:m1 + 1] - n0, dtype=_I4)
+        b.n_designs, b.n_members_total, b.n_nodes_total = hi - lo, m1 - m0, n1 - n0
+        return b
+
     @staticmethod
     def _step_classes(packed):
         """Step-class hints of the fused solvers: the largest number of classes of any design, counted by the kernels' rule
@@ -450,10 +480,11 @@ def _farm_batch_matrices(n_farms, n, M_arr, B_arr, C_arr):
     return mats, 0 if shapes == {(n_farms, n, n)} else 1
 
 
-def _farm_setup(N, F, nC, nw, M_arr, B_arr, C_arr, out=None, device=None):
+def _farm_setup(N, F, nC, nw, M_arr, B_arr, C_arr, out=None, device=None, outputs=True):
     """``F`` farms of ``N`` FOWTs as the farm-batch entries take them; ``F`` None is one farm, a batch of one whose outputs
     have no farm axis.  -> (RaftkFarmBatch, matrices, Xi_sys [F,nC,6N,nw], info [F,nC,nw]).  Host arrays, or with ``device``
-    torch tensors there; ``out``: host Xi_sys / info the caller owns, checked and used in place."""
+    torch tensors there; ``out``: host Xi_sys / info the caller owns, checked and used in place; ``outputs=False``: none are
+    allocated (Xi_sys, info None), the caller sets them on the struct."""
     n = 6 * N
     mats, shared = _farm_batch_matrices(F or 1, n, M_arr, B_arr, C_arr)
     lead = [] if F is None else [F]
@@ -469,12 +500,12 @@ def _farm_setup(N, F, nC, nw, M_arr, B_arr, C_arr, out=None, device=None):
         import torch
         ptr = lambda t: t.data_ptr()    # noqa: E731
         mats = {nm: torch.from_numpy(a).to(device) for nm, a in mats.items()}
-        res = {k: _torch_zeros(device)(*v) for k, v in res.items()}
+        res = {k: _torch_zeros(device)(*v) if outputs else None for k, v in res.items()}
     f = RaftkFarmBatch()
     f.n_farms, f.n_fowt, f.arr_shared = F or 1, N, shared
     for nm in ("M_arr", "B_arr", "C_arr"):
         setattr(f, nm, ptr(mats[nm]) if nm in mats else None)
-    f.Xi_sys, f.info = ptr(res["Xi_sys"]), ptr(res["info"])
+    f.Xi_sys, f.info = (ptr(res["Xi_sys"]), ptr(res["info"])) if outputs else (None, None)
     return f, mats, res["Xi_sys"], res["info"]
 
 
@@ -1154,6 +1185,17 @@ class _Device:
             check(getattr(lib, "raftk_%s_dev" % name)(*args, torch.cuda.current_stream(self.device).cuda_stream))
 
 
+def _buffers_for(Xi):
+    """The buffers a module-level reduction runs on: ``_Device`` on Xi's device when Xi is a torch CUDA tensor (a resident
+    response, e.g. the gathered ``Xi_sys`` of ``sweep.ShardedFarmSolve.step``), else host buffers.  The device form enqueues on
+    torch's current stream and returns torch tensors; tensors it made from host inputs are freed in stream order."""
+    import sys
+    torch = sys.modules.get("torch")
+    if torch is not None and isinstance(Xi, torch.Tensor) and Xi.is_cuda:
+        return _Device(Xi.device)
+    return _HOST
+
+
 def _session_buffers(session):
     """Device buffers for one reduction of ``session``, held as its ``_reads`` until its next reduction."""
     session._reads = _Device(session.device)
@@ -1266,8 +1308,10 @@ def farm_channel_stats(R, Xi_sys, dw, w=None, wpow=None, psd=True, amp=False, ti
     for one farm); ``dw`` the PSD divisor (the reference's Tmoor_PSD uses w[0]); ``w`` [nw], needed when a ``wpow`` is 1 or 2.
     -> (std [F,nR,nch], PSD [F,nR,nch,nw] or None, amplitudes complex [F,nR,nch,nw] or None), without the farm axis when
     ``Xi_sys`` had none.  Bit-identical to ``general_channel_stats`` on the same R and Xi.  Several wave trains of a case:
-    ``combine_trains``.  ``tile_w``: bins per CTA (0 automatic; -1 reads Xi_sys from L2), the results do not depend on it."""
-    return _farm_channel_stats(_HOST, R, Xi_sys, dw, w, wpow, psd, amp, tile_w)
+    ``combine_trains``.  ``tile_w``: bins per CTA (0 automatic; -1 reads Xi_sys from L2), the results do not depend on it.
+    With ``Xi_sys`` a torch CUDA tensor (a resident response, e.g. ``sweep.ShardedFarmSolve.step``'s gathered ``Xi_sys``) it runs
+    raftk_farm_channel_stats_dev on torch's current stream instead and returns torch tensors."""
+    return _farm_channel_stats(_buffers_for(Xi_sys), R, Xi_sys, dw, w, wpow, psd, amp, tile_w)
 
 
 def _farm_channel_stats(be, R, Xi_sys, dw, w, wpow, psd, amp, tile_w):
@@ -1334,8 +1378,10 @@ def rotor_stats(R, C_, V_w, gains, w, Xi, dw, case_row0=None, col0=None, psd=Tru
     ``V_w``, ``gains`` as ``packer.pack_rotor_outputs`` gives them for every unit, or with a leading unit axis;
     ``case_row0`` [nC + 1] the first row of every case (None: one row per case); ``col0`` [nrot] the first column of every
     rotor's hub row (None: 0).  -> (std [n_units, nC, nrot, 3] (omega rpm, torque N m, bPitch deg), PSD [n_units, nC, nrot,
-    3, nw] or None), without the unit axis when ``Xi`` had none."""
-    return _rotor_stats(_HOST, R, C_, V_w, gains, w, Xi, dw, case_row0, col0, psd)
+    3, nw] or None), without the unit axis when ``Xi`` had none.
+    With ``Xi`` a torch CUDA tensor (a resident response, e.g. ``sweep.ShardedFarmSolve.step``'s gathered ``Xi_sys``) it runs
+    raftk_rotor_stats_dev on torch's current stream instead and returns torch tensors."""
+    return _rotor_stats(_buffers_for(Xi), R, C_, V_w, gains, w, Xi, dw, case_row0, col0, psd)
 
 
 def _rotor_stats(be, R, C_, V_w, gains, w, Xi, dw, case_row0, col0, psd):
@@ -1435,8 +1481,10 @@ def fatigue(Xi, w, m, R=None, wpow=None, coef=None, case_row0=None, f_eq=1.0, me
     every case (None: one row per case); ``weights`` [nC] case probabilities; ``life`` (default: weights given) adds DEL_life
     = (sum_c p_c d_c / (f_eq sum_c p_c))^(1/m).  -> dict(DEL [n_units, nC, nch], info int32 (FATIGUE_ZERO, FATIGUE_NARROWBAND
     bits), moments [n_units, nC, nch, 4] (l0, l1, l2, l4) or absent, DEL_life [n_units, nch] or absent), without the unit
-    axis when ``Xi`` had none.  ``tile_w``: bins per CTA (0 automatic, -1 reads Xi from L2); the results do not depend on it."""
-    return _fatigue(_HOST, Xi, w, m, R, wpow, coef, case_row0, f_eq, method, weights, life, moments, tile_w)
+    axis when ``Xi`` had none.  ``tile_w``: bins per CTA (0 automatic, -1 reads Xi from L2); the results do not depend on it.
+    With ``Xi`` a torch CUDA tensor (a resident response, e.g. ``sweep.ShardedFarmSolve.step``'s gathered ``Xi_sys``) it runs
+    raftk_fatigue_dev on torch's current stream instead and returns torch tensors."""
+    return _fatigue(_buffers_for(Xi), Xi, w, m, R, wpow, coef, case_row0, f_eq, method, weights, life, moments, tile_w)
 
 
 def _fatigue(be, Xi, w, m, R, wpow, coef, case_row0, f_eq, method, weights, life, moments, tile_w):
@@ -1521,8 +1569,11 @@ def stress_ring(Xi, w, fa, ss, angles=None, d=10.0, t=0.083, m=None, f_eq=1.0, m
     -> dict(std, avg, max, min [n_units, nC, n_rings, nA] (max / min = avg +- 3 std), hot [n_units, nC, n_rings, 6] (
     ``STRESS_HOT``: sampled argmax angle and std, argmax angle and DEL, exact largest std and its angle in [0, pi)), DEL and
     info (with m), DEL_life [n_units, n_rings, nA] and hot_life [n_units, n_rings, 2] (angle, DEL) with weights and m, psd [n_units,
-    nC, n_rings, nA, nw] with psd), without the unit axis when ``Xi`` had none.  ``tile_w`` as ``fatigue``."""
-    return _stress_ring(_HOST, Xi, w, fa, ss, angles, d, t, m, f_eq, method, weights, case_row0, col0, psd, mean, wpow, dw, tile_w)
+    nC, n_rings, nA, nw] with psd), without the unit axis when ``Xi`` had none.  ``tile_w`` as ``fatigue``.
+    With ``Xi`` a torch CUDA tensor (a resident response, e.g. ``sweep.ShardedFarmSolve.step``'s gathered ``Xi_sys``) it runs
+    raftk_stress_ring_dev on torch's current stream instead and returns torch tensors."""
+    return _stress_ring(_buffers_for(Xi), Xi, w, fa, ss, angles, d, t, m, f_eq, method, weights, case_row0, col0, psd, mean, wpow, dw,
+                        tile_w)
 
 
 def _stress_ring(be, Xi, w, fa, ss, angles, d, t, m, f_eq, method, weights, case_row0, col0, psd, mean, wpow, dw, tile_w):
@@ -2440,23 +2491,46 @@ class DeviceSession:
         N = self.batch.n_designs if n_fowt is None else int(n_fowt)
         if N < 1 or self.batch.n_designs % N:
             raise ValueError("n_fowt must divide the session's %d designs" % self.batch.n_designs)
+        f, _, xi, info, ws, wsb = self._farm_setup(N, n_fowt, M_arr, B_arr, C_arr)
+        launch = lib.raftk_farm_response_ws_dev if n_fowt is None else lib.raftk_farm_batch_response_ws_dev
+        with torch.cuda.device(self.device):
+            check(launch(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f), ws.data_ptr(), wsb, self._stream()))
+        return xi, info
+
+    def _farm_setup(self, N, n_fowt, M_arr, B_arr, C_arr, gather=False):
+        """The farm struct, matrices, outputs and workspace of ``farm_response``'s form ``n_fowt``, set up on first use;
+        ``gather``: those of ``farm_response_gather``, kept apart and without outputs (they live in the gathered copies)."""
+        torch = self.torch
         # one farm is kept as the single-farm struct (raftk_farm), which callers hand to the single-farm entries, and launches
         # through them; its matrices and outputs are set up as a batch of one
-        key, query, launch = (("_farm", lib.raftk_farm_workspace_bytes, lib.raftk_farm_response_ws_dev) if n_fowt is None else
-                              ("_farm_batch", lib.raftk_farm_batch_workspace_bytes, lib.raftk_farm_batch_response_ws_dev))
+        key, query = ("_farm", lib.raftk_farm_workspace_bytes) if n_fowt is None else ("_farm_batch", lib.raftk_farm_batch_workspace_bytes)
+        if gather:
+            key = "_farm_gather"
         if not hasattr(self, key) or getattr(self, key)[0].n_fowt != N:
             with torch.cuda.device(self.device):
                 f, mats, xi, info = _farm_setup(N, None if n_fowt is None else self.batch.n_designs // N, self.cases.n_cases,
-                                                self.batch.nw, M_arr, B_arr, C_arr, device=self.device)
+                                                self.batch.nw, M_arr, B_arr, C_arr, device=self.device, outputs=not gather)
                 if n_fowt is None:
                     f = RaftkFarm(n_fowt=N, M_arr=f.M_arr, B_arr=f.B_arr, C_arr=f.C_arr, Xi_sys=f.Xi_sys, info=f.info)
                 wsb = int(query(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(f)))
                 ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=self.device)
             setattr(self, key, (f, mats, xi, info, ws, wsb))
-        f, _, xi, info, ws, wsb = getattr(self, key)
-        with torch.cuda.device(self.device):
-            check(launch(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f), ws.data_ptr(), wsb, self._stream()))
-        return xi, info
+        return getattr(self, key)
+
+    def farm_response_gather(self, peers, farm_row0, Xi_sys, info, n_fowt, C_arr=None, M_arr=None, B_arr=None):
+        """``farm_response(n_fowt=...)`` of this rank's farms with the results stored into every rank's gathered copy
+        (raftk_farm_batch_response_gather_dev; ``sweep.ShardedFarmSolve``): ``Xi_sys`` [F,nC,6N,nw] and ``info`` [F,nC,nw] are
+        farms [farm_row0, farm_row0 + F) of this rank's own copy, and the per-FOWT status of the last ``solve`` goes to every
+        copy too.  Matrices and workspace as ``farm_response``; follow with raftk_peer_barrier_dev."""
+        N = int(n_fowt)
+        if N < 1 or self.batch.n_designs % N:
+            raise ValueError("n_fowt must divide the session's %d designs" % self.batch.n_designs)
+        f, _, _, _, ws, wsb = self._farm_setup(N, N, M_arr, B_arr, C_arr, gather=True)
+        g = RaftkFarmBatch.from_buffer_copy(f)
+        g.Xi_sys, g.info = Xi_sys.data_ptr(), info.data_ptr()
+        with self.torch.cuda.device(self.device):
+            check(lib.raftk_farm_batch_response_gather_dev(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct),
+                                                           C.byref(g), C.byref(peers), int(farm_row0), ws.data_ptr(), wsb, self._stream()))
 
     def _response(self, what, farm, n_fowt):
         """The resident response reduction ``what`` runs on: the last ``solve``'s Xi [nD,nC,6,nw], or with ``farm`` the Xi_sys of

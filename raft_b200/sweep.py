@@ -166,6 +166,10 @@ def _align(n, a=256):
     return (int(n) + a - 1) // a * a
 
 
+class PeerSetupError(RuntimeError):
+    """The peer-mapped copies of a ``PeerExchange`` could not be set up on some rank (e.g. no CUDA IPC); raised on every rank."""
+
+
 class PeerExchange:
     """Peer-shared gathered arrays for the exchange fused into the solve kernel (include/raftk.h ``raftk_peers``).
 
@@ -174,9 +178,10 @@ class PeerExchange:
     allocated by the library (cudaMalloc + CUDA IPC handle).  Handles are exchanged once with ``all_gather_object``
     and opened, so rank r's kernel can store its finished units straight into every rank's copy over NVLink -- the
     step has no separate collective.  Two copies alternate between steps because a rank may start the next step
-    (and overwrite its block in a peer's copy) while that peer still reads the previous one."""
+    (and overwrite its block in a peer's copy) while that peer still reads the previous one.  ``status_elems``: int32 elements
+    per rank of the status region, viewed flat ([world * status_elems]); default 4 per unit, viewed [world, units, 4]."""
 
-    def __init__(self, units_per_rank, nw, device, group=None, n_buffers=2, dof=6):
+    def __init__(self, units_per_rank, nw, device, group=None, n_buffers=2, dof=6, status_elems=None):
         import ctypes as C
         import torch
         import torch.distributed as dist
@@ -193,30 +198,42 @@ class PeerExchange:
         self.xi_bytes = self.world * self.block_elems * 16
         self.off_flags = _align(self.xi_bytes)
         self.off_status = self.off_flags + 256
-        self.total = _align(self.off_status + self.world * self.units * 16)
+        self.status_elems = self.units * 4 if status_elems is None else int(status_elems)
+        self.total = _align(self.off_status + self.world * self.status_elems * 4)
         self.local, self.remote, self.peers, self.gathered, self.status = [], [], [], [], []
+        self.dist, self.group = dist, group
         with torch.cuda.device(self.device):
-            handles = []
-            for _ in range(n_buffers):
-                ptr, h = C.c_void_p(), C.create_string_buffer(64)
-                check(lib.raftk_peer_alloc(self.total, C.byref(ptr), h))
-                self.local.append(ptr.value)
-                handles.append(h.raw)
+            handles, err = [], None
+            try:
+                for _ in range(n_buffers):
+                    ptr, h = C.c_void_p(), C.create_string_buffer(64)
+                    check(lib.raftk_peer_alloc(self.total, C.byref(ptr), h))
+                    self.local.append(ptr.value)
+                    handles.append(h.raw)
+            except Exception as e:                    # noqa: BLE001  (agreed on below, then raised on every rank)
+                err = "%s: %s" % (type(e).__name__, e)
+            self._agree(err, "allocation")
             allh = [None] * self.world
             if self.world > 1:
                 dist.all_gather_object(allh, handles, group=group)
             else:
                 allh = [handles]
+            bases = [[None] * self.world for _ in range(n_buffers)]
+            try:
+                for b in range(n_buffers):
+                    for r in range(self.world):
+                        if r == self.rank:
+                            bases[b][r] = self.local[b]
+                        else:
+                            ptr = C.c_void_p()
+                            check(lib.raftk_peer_open(allh[r][b], C.byref(ptr)))
+                            self.remote.append(ptr.value)
+                            bases[b][r] = ptr.value
+            except Exception as e:                    # noqa: BLE001
+                err = "%s: %s" % (type(e).__name__, e)
+            self._agree(err, "peer mapping")
             for b in range(n_buffers):
-                base = []
-                for r in range(self.world):
-                    if r == self.rank:
-                        base.append(self.local[b])
-                    else:
-                        ptr = C.c_void_p()
-                        check(lib.raftk_peer_open(allh[r][b], C.byref(ptr)))
-                        self.remote.append(ptr.value)
-                        base.append(ptr.value)
+                base = bases[b]
                 pr = RaftkPeers()
                 pr.n_ranks, pr.rank, pr.epoch, pr.block_elems = self.world, self.rank, 0, self.block_elems
                 for r in range(self.world):
@@ -227,12 +244,24 @@ class PeerExchange:
                 raw = torch.as_tensor(_DevMem(self.local[b], self.total), device=self.device)
                 self.gathered.append(torch.view_as_complex(raw[:self.xi_bytes].view(torch.float64).view(-1, 2))
                                      .view(self.world, self.units, self.dof, self.nw))
-                self.status.append(raw[self.off_status:self.off_status + self.world * self.units * 16].view(torch.int32)
-                                   .view(self.world, self.units, 4))
+                st = raw[self.off_status:self.off_status + self.world * self.status_elems * 4].view(torch.int32)
+                self.status.append(st.view(self.world, self.units, 4) if status_elems is None else st)
             self.timeout = torch.zeros(1, dtype=torch.int32, device=self.device)
         if self.world > 1:
             dist.barrier(group=group)          # every rank has opened every handle before anyone stores into a peer
         self.n_steps = 0
+
+    def _agree(self, err, stage):
+        """Every rank learns every rank's outcome of a setup stage (one all_gather_object); if any failed, all free what they
+        hold and raise PeerSetupError together, so no rank enters the next collective alone."""
+        errs = [err]
+        if self.world > 1:
+            errs = [None] * self.world
+            self.dist.all_gather_object(errs, err, group=self.group)
+        bad = [(r, e) for r, e in enumerate(errs) if e is not None]
+        if bad:
+            self.close()
+            raise PeerSetupError("peer exchange %s failed on rank %d: %s" % ((stage,) + bad[0]))
 
     def next(self):
         """-> (buffer index, peers struct) for the next exchange; epochs count steps across both buffers."""
@@ -453,6 +482,155 @@ class ShardedGeneralSolve:
     def close(self):
         if self.px is not None:
             self.px.close()
+
+
+def farm_shards(n_farms, world):
+    """[lo, hi) farms of every rank: contiguous runs of whole farms whose sizes differ by at most one (``shard_bounds``); with
+    more ranks than farms the last ranks get none."""
+    return [shard_bounds(n_farms, r, world) for r in range(int(world))]
+
+
+def shard_design_cases(cases, lo, hi):
+    """A ``solver.CaseTable`` for designs [lo, hi) of its batch: every case, with those designs' rows of F_2nd, Xi_init and
+    per-design operating-point tables (a shared operating-point set stays whole)."""
+    from . import solver
+    a = cases.arrays
+    sub = {k: a[k] for k in ("Hs", "Tp", "gamma", "beta_deg", "spec", "primary") if k in a}
+    ops = cases.ops
+    if ops is not None and not cases.op_shared:
+        ops = dict(ops, A_w=ops["A_w"][lo:hi], B_w=ops["B_w"][lo:hi])
+    rows = {k: a[k][lo:hi] for k in ("F_2nd", "Xi_init") if k in a}
+    return solver.CaseTable(sub, zeta=a.get("zeta"), ops=ops, **rows)
+
+
+def farm_rows(bounds, per=1):
+    """Rows of a gathered array [world * F_max * per, ...] (rank r's block at r * F_max * per, ``per`` rows per farm) that hold
+    farms 0..F-1 in order, F_max the largest shard of ``bounds`` (``farm_shards``): the index that drops the padding."""
+    import torch
+    rows = max(1, max(h - l for l, h in bounds))
+    return torch.cat([torch.arange((h - l) * per) + r * rows * per for r, (l, h) in enumerate(bounds)])
+
+
+def gather_farm_shards(blocks, bounds, n_fowt, group=None):
+    """The ``exchange="nccl"`` path of ``ShardedFarmSolve``: this rank's (Xi_sys [F_r,nC,6N,nw], info [F_r,nC,nw], status
+    [F_r*N,nC,4]) padded to the largest shard, one ``all_gather_into_tensor`` each, and the padding dropped
+    -> the whole batch's three tensors in farm order.  Backend-agnostic (NCCL on GPUs, gloo on CPU tensors)."""
+    import torch
+    import torch.distributed as dist
+    world = len(bounds)
+    rows = max(1, max(h - l for l, h in bounds))
+    out = []
+    for t, per in zip(blocks, (1, 1, int(n_fowt))):
+        pad = t.new_zeros((rows * per,) + tuple(t.shape[1:]))
+        pad[:t.shape[0]].copy_(t)
+        if world > 1:
+            full = t.new_empty((world * rows * per,) + tuple(t.shape[1:]))
+            dist.all_gather_into_tensor(full, pad, group=group)
+        else:
+            full = pad
+        out.append(full.index_select(0, farm_rows(bounds, per).to(full.device)))
+    return tuple(out)
+
+
+class ShardedFarmSolve:
+    """A farm batch (``solver.solve_dynamics_farm_batch``) sharded over GPUs: rank r takes the whole farms
+    ``farm_shards(F, world)[r]`` (a farm's coupled system stays on one GPU), runs its FOWTs' drag linearisation and its farms'
+    coupled 6N-DOF solves in a ``solver.DeviceSession`` of its own, and ``step()`` returns (Xi_sys [F,nC,6N,nw], info [F,nC,nw],
+    status [F*N,nC,4]) of the WHOLE batch as device tensors, valid in stream order on every rank: bit for bit what one
+    ``solve_dynamics_farm_batch`` call over all F farms returns.
+
+    ``designs``: ``solver.DesignBatch`` of F * n_fowt FOWTs in the farm batch's order (design f * N + i is FOWT i of farm f), or
+    the packed designs; ``cases``: ``solver.CaseTable`` as for the single-GPU entry (operating points, wave trains, F_2nd);
+    array matrices [6N,6N] for every farm or [F,6N,6N], sliced to each rank's farms.
+    ``exchange="peer"``: the farm kernel stores each rank's results into every rank's gathered copy through CUDA IPC peer
+    pointers (raftk_farm_batch_response_gather_dev; farms too large for shared memory are copied by k_farm_publish after their
+    solve), then raftk_peer_barrier_dev; the copies hold F_max = the largest shard's farm count per rank.  ``exchange="nccl"``:
+    ``gather_farm_shards`` instead; a peer exchange that cannot be set up (CUDA IPC unavailable) falls back to it on every
+    rank.  With one rank it is ``DeviceSession.farm_response(n_fowt=N)`` with the exchange's copies as outputs."""
+
+    WANT = ("Xi", "status", "B_drag", "F_drag", "F_iner")
+
+    def __init__(self, designs, cases, n_fowt, C_arr=None, M_arr=None, B_arr=None, device=None, group=None, exchange="peer"):
+        import torch
+        import torch.distributed as dist
+        from . import solver
+        if exchange not in ("peer", "nccl"):
+            raise ValueError("exchange must be 'peer' or 'nccl'")
+        self.torch, self.dist, self.group = torch, dist, group
+        batch = designs if isinstance(designs, solver.DesignBatch) else solver.DesignBatch(designs)
+        ct = cases if isinstance(cases, solver.CaseTable) else solver.CaseTable(cases)
+        N = self.N = int(n_fowt)
+        if N < 1 or batch.n_designs % N:
+            raise ValueError("n_fowt must divide the batch's %d designs" % batch.n_designs)
+        ct.check_ops(batch)
+        on = dist.is_available() and dist.is_initialized()
+        self.world = dist.get_world_size(group) if on else 1
+        self.rank = dist.get_rank(group) if on else 0
+        self.F, self.nC, self.nw, n = batch.n_designs // N, ct.n_cases, batch.nw, 6 * N
+        mats, shared = solver._farm_batch_matrices(self.F, n, M_arr, B_arr, C_arr)
+        self.bounds = farm_shards(self.F, self.world)
+        self.lo, self.hi = self.bounds[self.rank]
+        self.rows = max(1, max(h - l for l, h in self.bounds))
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.sess, self.mats = None, {}
+        if self.hi > self.lo:
+            want = self.WANT + (("F_BEM",) if batch.n_bem_head else ())
+            self.sess = solver.DeviceSession(batch.take(self.lo * N, self.hi * N), shard_design_cases(ct, self.lo * N, self.hi * N),
+                                             device=self.device, want=want)
+            self.mats = {k: v if shared else v[self.lo:self.hi] for k, v in mats.items()}
+        self.px, self.exchange, self.fallback = None, exchange, None
+        if exchange == "peer":
+            # PeerExchange raises on every rank together when the IPC allocation or mapping fails on any (PeerSetupError), so
+            # all ranks fall back to NCCL and none is left alone in a collective of the setup
+            try:
+                self.px = PeerExchange(self.rows * self.nC, self.nw, self.device, group=group, dof=n,
+                                       status_elems=self.rows * self.nC * (self.nw + 4 * N))
+            except PeerSetupError as e:
+                self.fallback, self.exchange = str(e), "nccl"
+        if self.px is not None:
+            R = self.world * self.rows
+            self.views = []
+            for b in range(len(self.px.peers)):
+                ints = self.px.status[b]
+                self.views.append((self.px.gathered[b].view(R, self.nC, n, self.nw), ints[:R * self.nC * self.nw].view(R, self.nC, self.nw),
+                                   ints[R * self.nC * self.nw:].view(R * N, self.nC, 4)))
+            self.keep = [farm_rows(self.bounds).to(self.device), farm_rows(self.bounds, N).to(self.device)]
+
+    def step(self, n_iter=10, tol=0.01, xi_start=0.0):
+        """Enqueue the per-FOWT solve, the coupled solve and the exchange of this rank's farms on the current stream
+        -> (Xi_sys [F,nC,6N,nw], info [F,nC,nw], status [F*N,nC,4]) of the whole batch (device tensors, stream order)."""
+        import ctypes as C
+        from ._lib import check, lib
+        torch, N, m = self.torch, self.N, self.hi - self.lo
+        with torch.cuda.device(self.device):
+            if self.sess is not None:
+                self.sess.solve(n_iter=n_iter, tol=tol, xi_start=xi_start)
+            if self.px is not None:
+                b, peers = self.px.next()
+                X, I, S = self.views[b]
+                if m:
+                    r0 = self.rank * self.rows
+                    self.sess.farm_response_gather(peers, r0, X[r0:r0 + m], I[r0:r0 + m], N, **self.mats)
+                check(lib.raftk_peer_barrier_dev(C.byref(peers), self.px.timeout.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream))
+                fk, sk = self.keep
+                return X.index_select(0, fk), I.index_select(0, fk), S.index_select(0, sk)
+            if m:
+                xi, info = self.sess.farm_response(n_fowt=N, **self.mats)
+                blocks = (xi, info, self.sess.out["status"])
+            else:
+                n = 6 * N
+                blocks = (torch.zeros([0, self.nC, n, self.nw], dtype=torch.complex128, device=self.device),
+                          torch.zeros([0, self.nC, self.nw], dtype=torch.int32, device=self.device),
+                          torch.zeros([0, self.nC, 4], dtype=torch.int32, device=self.device))
+            return gather_farm_shards(blocks, self.bounds, N, self.group)
+
+    def timed_out(self):
+        return bool(self.px.timeout.item()) if self.px is not None else False
+
+    def close(self):
+        if self.px is not None:
+            self.px.close()
+            self.px = None
 
 
 class PipelinedSolve:

@@ -1,0 +1,81 @@
+#!/usr/bin/env python
+"""Compare the SASS of two builds of the library, kernel by kernel (profiles/sm90a_farm_peer_sass.txt).
+
+The two inputs are `cuobjdump -sass` listings of raft_b200/csrc/raftk.cu compiled for sm_90a, one before and one after the
+farm kernels' PEER instantiations.  Kernels are matched by demangled name and template arguments, not by parameter types
+(the non-PEER instantiations now spell FarmParams through the FarmArg alias); a kernel that gained PEER as its last template
+argument is matched through its PEER = false instantiation.  Instruction text is compared with addresses and encodings
+dropped.  Each matched farm kernel, and any kernel that differs, prints SAME or DIFF with its instruction counts; kernels
+found on one side only are listed at the end.
+
+Usage:  python tools/farm_sass_diff.py BEFORE.sass AFTER.sass
+"""
+import argparse
+import re
+import subprocess
+
+PEER_KERNELS = ("k_farm_response", "k_farm_rows")
+
+
+def functions(path):
+    """mangled name -> list of instruction strings of every function in a cuobjdump -sass listing."""
+    out, cur = {}, None
+    with open(path) as fh:
+        for line in fh:
+            m = re.match(r"\s*Function : (\S+)", line)
+            if m:
+                cur = m.group(1)
+                out[cur] = []
+                continue
+            m = re.search(r"/\*[0-9a-f]{4,6}\*/\s+(.*?)\s*;", line)
+            if cur and m:
+                out[cur].append(m.group(1))
+    return out
+
+
+def demangle(names):
+    res = subprocess.run(["c++filt"], input="\n".join(names), capture_output=True, text=True, check=True)
+    return dict(zip(names, res.stdout.splitlines()))
+
+
+def key(demangled, after):
+    """Kernel name and template arguments; on the after side a trailing PEER argument: (key, is_peer)."""
+    m = re.match(r"(?:void )?(\w+)(?:<(.*?)>)?\(", demangled)
+    if not m:
+        return demangled, False
+    name, targs = m.group(1), [a.strip() for a in (m.group(2) or "").split(",") if a.strip()]
+    peer = False
+    if after and name in PEER_KERNELS:
+        peer = targs.pop() == "true"
+    return "%s<%s>" % (name, ", ".join(targs)), peer
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("before")
+    ap.add_argument("after")
+    args = ap.parse_args()
+    before, after = functions(args.before), functions(args.after)
+    dm = demangle(sorted(set(before) | set(after)))
+    b_by_key = {key(dm[n], False)[0]: n for n in before}
+    a_by_key, peer_only = {}, []
+    for n in after:
+        k, peer = key(dm[n], True)
+        if peer:
+            peer_only.append(k + " PEER")
+        else:
+            a_by_key[k] = n
+    same = diff = 0
+    for k in sorted(set(b_by_key) & set(a_by_key)):
+        b, a = before[b_by_key[k]], after[a_by_key[k]]
+        ok = b == a
+        same, diff = same + ok, diff + (not ok)
+        if any(k.startswith(p + "<") for p in PEER_KERNELS + ("k_farm_response_global",)) or not ok:
+            print("%-4s %6d %6d  %s" % ("SAME" if ok else "DIFF", len(b), len(a), k))
+    print("matched kernels: %d identical, %d different" % (same, diff))
+    print("only before: %s" % sorted(set(b_by_key) - set(a_by_key)))
+    print("only after: %s" % sorted((set(a_by_key) - set(b_by_key)) | set(peer_only)))
+
+
+if __name__ == "__main__":
+    main()
