@@ -389,6 +389,8 @@ int raftk_solve_dynamics_slender_host(const raftk_designs *d, const raftk_slende
  * Xi complex [n_cases,n_dof,nw]; status [n_cases,4] = passes, converged, flags, 0.  The n_dof x n_dof impedance of every (case,
  * frequency, pass) is solved by a blocked LU with partial pivoting (LAPACK's pivot rule and elimination order); validated on
  * the GPU against the reference's 150-DOF VolturnUS-S-flexible run (tests/test_general_dofs.py, 1e-10).  n_dof <= 256.
+ * Status flags: RAFTK_FLAG_NAN for NaN in a response, RAFTK_FLAG_SINGULAR for an exactly zero pivot at some bin (its
+ * response is NaN as well); either stops the case.  A secondary train solved with its primary's singular factors carries both.
  * Wave trains (cases.primary, raft_model.py:1200-1236): a secondary train runs no pass of its own; its response is solved with
  * the LU factors of its primary's last impedance and the drag excitation of its own wave kinematics with the primary's last
  * node drag coefficients.  Primaries keep the loop's final Xi.  Status rows of secondaries: 0, 1, flags, primary + 1.

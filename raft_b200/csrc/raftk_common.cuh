@@ -127,6 +127,38 @@ __device__ __forceinline__ void static_for(F &&f)
     }
 }
 
+// Pivot reciprocals and back-substitution quotients of the dense LUs in global and shared memory (the farm and system solves,
+// the generalised-DOF solves) are formed at the pivot's own scale: p is multiplied by sc = 2^-e, e the binary exponent of
+// max(|re|, |im|), before |p|^2 is taken, and the result by sc again.  |p|^2 alone overflows above |p| ~ 1.3e154 (a zero
+// reciprocal: nothing eliminated) and underflows below 1.5e-154 (a false zero pivot).  Power-of-two scaling is exact, so
+// wherever the unscaled formula stayed in the normal range the bits are the same.  sc is built from the exponent field,
+// clamped to [1, 2045] so that it stays a normal double (a subnormal or zero pivot takes 2^1022, one at or above 2^1022
+// takes 2^-1022); a zero pivot still gives |q|^2 = 0, and inf / NaN go through as before.
+__device__ __forceinline__ double piv_scale(const double2 p)
+{
+    const int eb = min(max((__double2hiint(fmax(fabs(p.x), fabs(p.y))) >> 20) & 0x7ff, 1), 2045);
+    return __hiloint2double((2046 - eb) << 20, 0);
+}
+
+// 1 / p, and 0 for a zero pivot (zero set)
+__device__ __forceinline__ double2 piv_recip(const double2 p, bool &zero)
+{
+    const double sc = piv_scale(p);
+    const double2 q = make_double2(p.x * sc, p.y * sc);
+    const double den = q.x * q.x + q.y * q.y;
+    zero = !(den > 0.0);
+    return zero ? make_double2(0.0, 0.0) : make_double2(q.x / den * sc, -q.y / den * sc);
+}
+
+// s / p
+__device__ __forceinline__ double2 piv_div(const double2 s, const double2 p)
+{
+    const double sc = piv_scale(p);
+    const double2 q = make_double2(p.x * sc, p.y * sc);
+    const double den = q.x * q.x + q.y * q.y;
+    return make_double2((s.x * q.x + s.y * q.y) / den * sc, (s.y * q.x - s.x * q.y) / den * sc);
+}
+
 // 6x6 complex solve in registers: LU with partial pivoting (|re|+|im| metric, as LAPACK izamax),
 // forward elimination applied to b on the fly, back substitution.  Returns false on a zero pivot.
 __device__ __forceinline__ bool solve6(double (&ar)[6][6], double (&ai)[6][6], double (&br)[6], double (&bi)[6])

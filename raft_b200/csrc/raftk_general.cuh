@@ -91,7 +91,7 @@ struct GenWork {                 // per-call workspace views
     double *B_drag;              // [nC][n][n]
     double2 *Z;                  // [nC][nw][n][n+1]  augmented systems; after a case's last pass its LU factors (LAPACK layout)
     int *piv;                    // [nC][nw][n]       pivot row of every elimination step of that factorisation
-    int *flags;                  // [nC][4]: done, pass_not_converged, passes, nan
+    int *flags;                  // [nC][4]: done, pass_not_converged, passes, RAFTK_FLAG_NAN | RAFTK_FLAG_SINGULAR (a zero pivot)
 };
 
 // k_gen_wave: grid (ceil(nw/128), Ns, nC), block 128
@@ -427,14 +427,13 @@ __global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 
             for (int t = 1; t < 8; t++) if (pv[t] > b0 || (pv[t] == b0 && pi_[t] < r0)) { b0 = pv[t]; r0 = pi_[t]; }
             prow = r0;
             W.piv[((size_t)c * nw + i) * n + k] = r0;
-            if (!(b0 > 0.0)) bad = 1;
         }
         __syncthreads();
         const int p = prow;
         // whole rows, so that L ends in LAPACK's layout (k_gen_train_solve reuses these factors)
         if (p != k) for (int b = tid; b < nc; b += 256) { const double2 t1 = A[(size_t)k * nc + b]; A[(size_t)k * nc + b] = A[(size_t)p * nc + b]; A[(size_t)p * nc + b] = t1; }
         __syncthreads();
-        if (tid == 0) { const double2 a = A[(size_t)k * nc + k]; const double dd = a.x * a.x + a.y * a.y; piv = make_double2(a.x / dd, -a.y / dd); }
+        if (tid == 0) { bool zero; piv = piv_recip(A[(size_t)k * nc + k], zero); if (zero) bad = 1; }
         __syncthreads();
         const double2 ip = piv;
         // multipliers l_r = a_rk / a_kk, then trailing update a_rb -= l_r a_kb (b = k+1 .. n incl. the right-hand side)
@@ -453,9 +452,7 @@ __global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 
     // back substitution on the last column
     for (int k = n - 1; k >= 0; k--) {
         if (tid == 0) {
-            const double2 a = A[(size_t)k * nc + k], b = A[(size_t)k * nc + n];
-            const double dd = a.x * a.x + a.y * a.y;
-            A[(size_t)k * nc + n] = make_double2((b.x * a.x + b.y * a.y) / dd, (b.y * a.x - b.x * a.y) / dd);
+            A[(size_t)k * nc + n] = piv_div(A[(size_t)k * nc + n], A[(size_t)k * nc + k]);
         }
         __syncthreads();
         const double2 x = A[(size_t)k * nc + n];
@@ -476,7 +473,7 @@ __global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 
         if (!(sqrt(dx * dx + dy * dy) / (sqrt(x.x * x.x + x.y * x.y) + tol) < tol)) notconv = 1;     // raft_model.py:1101-1102
     }
     if (notconv) atomicOr(&W.flags[4 * c + 1], 1);
-    if (nan || bad) atomicOr(&W.flags[4 * c + 3], 1);
+    if (nan || bad) atomicOr(&W.flags[4 * c + 3], (nan ? RAFTK_FLAG_NAN : 0) | (bad ? RAFTK_FLAG_SINGULAR : 0));
 }
 
 // k_gen_solve_blocked: grid (nw, units), block 256.  Same system, same pivot rule and the same elimination order as
@@ -541,10 +538,9 @@ __global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W
             double b0 = pv[0]; int p = pi_[0];
 #pragma unroll
             for (int t = 1; t < GT / 32; t++) if (pv[t] > b0 || (pv[t] == b0 && pi_[t] < p)) { b0 = pv[t]; p = pi_[t]; }
-            const double2 a = P[p * GB + j];
-            const double dd = a.x * a.x + a.y * a.y;
-            const double2 ip = make_double2(a.x / dd, -a.y / dd);
-            if (tid == 0) { pivrow[j] = p; W.piv[((size_t)c * nw + i) * n + kb + j] = kb + p; if (!(b0 > 0.0)) bad = 1; }
+            bool zero;
+            const double2 ip = piv_recip(P[p * GB + j], zero);
+            if (tid == 0) { pivrow[j] = p; W.piv[((size_t)c * nw + i) * n + kb + j] = kb + p; if (zero) bad = 1; }
             __syncthreads();
             if (p != j && tid < nb) { const double2 t1 = P[j * GB + tid]; P[j * GB + tid] = P[p * GB + tid]; P[p * GB + tid] = t1; }
             __syncthreads();
@@ -626,9 +622,7 @@ __global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W
     // back substitution on the last column
     for (int k = n - 1; k >= 0; k--) {
         if (tid == 0) {
-            const double2 a = A[(size_t)k * nc + k], b = A[(size_t)k * nc + n];
-            const double dd = a.x * a.x + a.y * a.y;
-            A[(size_t)k * nc + n] = make_double2((b.x * a.x + b.y * a.y) / dd, (b.y * a.x - b.x * a.y) / dd);
+            A[(size_t)k * nc + n] = piv_div(A[(size_t)k * nc + n], A[(size_t)k * nc + k]);
         }
         __syncthreads();
         const double2 x = A[(size_t)k * nc + n];
@@ -649,7 +643,7 @@ __global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W
         if (!(sqrt(dx * dx + dy * dy) / (sqrt(x.x * x.x + x.y * x.y) + tol) < tol)) notconv = 1;     // raft_model.py:1101-1102
     }
     if (notconv) atomicOr(&W.flags[4 * c + 1], 1);
-    if (nan || bad) atomicOr(&W.flags[4 * c + 3], 1);
+    if (nan || bad) atomicOr(&W.flags[4 * c + 3], (nan ? RAFTK_FLAG_NAN : 0) | (bad ? RAFTK_FLAG_SINGULAR : 0));
 }
 
 // k_gen_init: grid (nC), block 256: XiLast = XiStart (raft_model.py:999), flags = 0; secondary trains start done
@@ -663,7 +657,8 @@ __global__ void __launch_bounds__(256) k_gen_init(GenDev D, GenWork W, double xi
 }
 
 // k_gen_train_solve: grid (nw, nC), block 128, secondary trains only: Xi = Z_p^-1 (F_iner + F_drag) with the LU factors of the
-// primary's last pass (L unit lower, U upper, row interchanges piv applied in elimination order; raft_model.py:1200-1236)
+// primary's last pass (L unit lower, U upper, row interchanges piv applied in elimination order; raft_model.py:1200-1236).
+// A zero diagonal of U (the primary's singular bin) sets RAFTK_FLAG_SINGULAR in the secondary's flag word 3 as well.
 __global__ void __launch_bounds__(128) k_gen_train_solve(GenDev D, GenWork W, const int *primary, double2 *Xi)
 {
     __shared__ double2 b[256];
@@ -690,11 +685,12 @@ __global__ void __launch_bounds__(128) k_gen_train_solve(GenDev D, GenWork W, co
         }
         __syncthreads();
     }
+    int zero = 0;                                               // a zero diagonal of U (thread 0)
     for (int k = n - 1; k >= 0; k--) {                          // U x = y, as the back substitution of k_gen_solve*
         if (tid == 0) {
-            const double2 a = A[(size_t)k * nc + k], v = b[k];
-            const double dd = a.x * a.x + a.y * a.y;
-            b[k] = make_double2((v.x * a.x + v.y * a.y) / dd, (v.y * a.x - v.x * a.y) / dd);
+            const double2 a = A[(size_t)k * nc + k];
+            if (a.x == 0.0 && a.y == 0.0) zero = 1;
+            b[k] = piv_div(b[k], a);
         }
         __syncthreads();
         const double2 x = b[k];
@@ -712,7 +708,7 @@ __global__ void __launch_bounds__(128) k_gen_train_solve(GenDev D, GenWork W, co
         Xi[((size_t)c * n + a) * nw + i] = x;
         if (isnan(x.x) || isnan(x.y)) nan = 1;
     }
-    if (nan) atomicOr(&W.flags[4 * c + 3], 1);
+    if (nan || zero) atomicOr(&W.flags[4 * c + 3], (nan ? RAFTK_FLAG_NAN : 0) | (zero ? RAFTK_FLAG_SINGULAR : 0));
 }
 
 // k_gen_relax: grid (nC), block 256: close the pass (raft_model.py:1098-1133)
@@ -723,7 +719,7 @@ __global__ void __launch_bounds__(256) k_gen_relax(GenDev D, GenWork W, const do
     if (W.flags[4 * c]) return;
     if (tid == 0) { st[0] = W.flags[4 * c + 1]; st[1] = W.flags[4 * c + 3]; }
     __syncthreads();
-    const int notconv = st[0], nan = st[1];
+    const int notconv = st[0], nan = st[1];                   // NaN or a zero pivot: the unit stops
     if (!nan && notconv) {
         const size_t tot = (size_t)D.n * D.nw;
         double2 *L = W.XiLast + (size_t)c * tot;
@@ -733,7 +729,7 @@ __global__ void __launch_bounds__(256) k_gen_relax(GenDev D, GenWork W, const do
     __syncthreads();
     if (tid == 0) {
         W.flags[4 * c + 2] += 1;                              // passes
-        if (nan || !notconv) W.flags[4 * c] = nan ? 2 : 1;   // done: 1 converged, 2 NaN
+        if (nan || !notconv) W.flags[4 * c] = nan ? 2 : 1;   // done: 1 converged, 2 NaN or a zero pivot
         W.flags[4 * c + 1] = 0;
     }
 }
@@ -766,7 +762,8 @@ struct GenPublish {
     int *S[RAFTK_MAX_PEERS];
 };
 
-// status rows for the caller: passes, converged, flags (RAFTK_FLAG_NAN), 0; a secondary train: 0, 1, flags, primary + 1
+// status rows for the caller: passes, converged, flags (flag word 3: RAFTK_FLAG_NAN, RAFTK_FLAG_SINGULAR), 0; a secondary
+// train: 0, 1, flags, primary + 1
 __global__ void __launch_bounds__(128) k_gen_status(int nC, const int *flags, const int *primary, int *status)
 {
     const int c = blockIdx.x * 128 + threadIdx.x;
@@ -774,6 +771,6 @@ __global__ void __launch_bounds__(128) k_gen_status(int nC, const int *flags, co
     const int p = primary ? primary[c] : c;
     status[4 * c + 0] = flags[4 * c + 2];
     status[4 * c + 1] = flags[4 * c] == 1 ? 1 : 0;
-    status[4 * c + 2] = (flags[4 * c] == 2 || flags[4 * c + 3]) ? RAFTK_FLAG_NAN : 0;
+    status[4 * c + 2] = flags[4 * c + 3] & (RAFTK_FLAG_NAN | RAFTK_FLAG_SINGULAR);
     status[4 * c + 3] = p != c ? p + 1 : 0;
 }
