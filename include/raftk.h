@@ -218,7 +218,7 @@ enum {
     RAFTK_KERNEL_QTF_DIAG = 7,        /* k_qtf_force<false> (one QTF heading)                                             */
     RAFTK_KERNEL_QTF_DIAG_MIX = 8,    /* k_qtf_force<true> (heading interpolation)                                        */
     RAFTK_KERNEL_GEN_BLOCKED = 9,     /* k_gen_solve_blocked                                                              */
-    RAFTK_KERNEL_GEN_UNBLOCKED = 10,  /* k_gen_solve                                                                      */
+    RAFTK_KERNEL_GEN_UNBLOCKED = 10,  /* retired (the column-at-a-time k_gen_solve): never reported, kept for the numbering  */
     RAFTK_KERNEL_FARM_ROWS12 = 11,    /* k_farm_rows<12>                                                                  */
     RAFTK_KERNEL_FARM_WARP = 12,      /* k_farm_response<true>                                                            */
     RAFTK_KERNEL_FARM_BLOCK = 13,     /* k_farm_response<false>                                                           */

@@ -149,6 +149,7 @@ extern "C" int raftk_last_dispatch(raftk_dispatch *out)
 #include "raftk_fused2.cuh"
 #include "raftk_qtf.cuh"
 #include "raftk_slender.cuh"
+#include "raftk_lu.cuh"
 #include "raftk_general.cuh"
 #include "raftk_misc.cuh"
 #include "raftk_rotor.cuh"
@@ -889,7 +890,7 @@ extern "C" int raftk_peer_barrier_dev(const raftk_peers *peers, int32_t *timeout
 // ---- farm system solve ----------------------------------------------------------------------------
 // Which dense solver takes a system.  The shared-memory kernels (k_system_solve, k_farm_response) keep every system whose
 // augmented matrix fits in the device's opt-in shared memory next to the kernel's static shared memory; everything larger
-// goes to the global-memory LU (lu_global).  Without a device the rule uses an H100's limits and the static sizes of the
+// goes to the global-memory kernels (lu_blocked with a staged panel).  Without a device the rule uses an H100's limits and the static sizes of the
 // sm_90a build, so that the workspace query answers the same on a machine without a GPU.
 static size_t dev_attr(cudaDeviceAttr a, size_t fallback)
 {
@@ -1673,15 +1674,14 @@ static int gen_launch(const raftk_general *g, const GenBatch &Bt, const raftk_ge
     CasesDev C = to_dev(c);
     double2 *X = reinterpret_cast<double2 *>(Xi);
     const unsigned fb = (unsigned)((g->nw + 127) / 128);
-    // blocked LU (panel + row block in shared memory); RAFTK_GEN_UNBLOCKED=1 keeps the first, column-at-a-time kernel for A/B runs
+    // the blocked LU's panel and row block in shared memory (n_dof <= 256: at most 65.7 KB)
     const size_t lu_smem = ((size_t)g->n_dof * GB + (size_t)GB * (g->n_dof + 1)) * sizeof(double2);
-    const bool blocked = !getenv("RAFTK_GEN_UNBLOCKED") && lu_smem <= 110 * 1024;
     const bool fdz = Fx.n_fd > 0;                      // impedance with the frequency-dependent terms on their support
     const bool op = c->op != nullptr;                  // plus every case's operating point there (validate_gen_op: n_fd >= 1)
     GenFdOpDev Fo;
     static_cast<GenFdDev &>(Fo) = Fx;
     Fo.op = c->op; Fo.n_op = c->n_op; Fo.op_shared = c->op_shared; Fo.op_A_w = c->op_A_w; Fo.op_B_w = c->op_B_w;
-    if (blocked) {
+    {
         static SmemOptIn opt(48 * 1024), opt_fd(48 * 1024), opt_op(48 * 1024);
         CUDA_TRY(op ? opt_op.ensure(k_gen_solve_blocked<true, true>, lu_smem)
                     : fdz ? opt_fd.ensure(k_gen_solve_blocked<true>, lu_smem) : opt.ensure(k_gen_solve_blocked<false>, lu_smem));
@@ -1727,16 +1727,11 @@ static int gen_launch(const raftk_general *g, const GenBatch &Bt, const raftk_ge
         if (Ns_grid > 0) k_gen_node_pass<false><<<dim3(Ns_grid, (unsigned)nC), 128, 0, st>>>(D, W, nullptr);
         k_gen_bdrag<<<dim3(g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W);
         k_gen_project<false, false><<<dim3(fb, g->n_dof, (unsigned)nC), 128, 0, st>>>(D, W, W.F_drag, 1, nullptr, Fx);
-        if (blocked) {
+        {
             ProfScope ps(st, 2);
             if (op) k_gen_solve_blocked<true, true><<<dim3(g->nw, (unsigned)nC), GT, lu_smem, st>>>(D, W, X, o->tol, Fo);
             else if (fdz) k_gen_solve_blocked<true><<<dim3(g->nw, (unsigned)nC), GT, lu_smem, st>>>(D, W, X, o->tol, Fx);
             else k_gen_solve_blocked<false><<<dim3(g->nw, (unsigned)nC), GT, lu_smem, st>>>(D, W, X, o->tol, Fx);
-        } else {
-            ProfScope ps(st, 2);
-            if (op) k_gen_solve<true, true><<<dim3(g->nw, (unsigned)nC), 256, 0, st>>>(D, W, X, o->tol, Fo);
-            else if (fdz) k_gen_solve<true><<<dim3(g->nw, (unsigned)nC), 256, 0, st>>>(D, W, X, o->tol, Fx);
-            else k_gen_solve<false><<<dim3(g->nw, (unsigned)nC), 256, 0, st>>>(D, W, X, o->tol, Fx);
         }
         k_gen_relax<<<(unsigned)nC, 256, 0, st>>>(D, W, X);
         g_launches += 5;
@@ -1747,7 +1742,7 @@ static int gen_launch(const raftk_general *g, const GenBatch &Bt, const raftk_ge
         k_gen_train_solve<<<dim3(g->nw, (unsigned)nC), 128, 0, st>>>(D, W, prim, X);
         g_launches += 3;
     }
-    disp_launch(RAFTK_FAMILY_GENERAL, blocked ? RAFTK_KERNEL_GEN_BLOCKED : RAFTK_KERNEL_GEN_UNBLOCKED, blocked ? GT : 256);
+    disp_launch(RAFTK_FAMILY_GENERAL, RAFTK_KERNEL_GEN_BLOCKED, GT);
     g_disp.trains = prim != nullptr;
     k_gen_status<<<(unsigned)((nC + 127) / 128), 128, 0, st>>>((int)nC, W.flags, prim, status);
     g_launches++;

@@ -14,7 +14,7 @@
 //   k_gen_node_pass (case, node)      node velocity from Tn_j XiLast, RMS over w, linearised Bmat_j, drag load f6
 //   k_gen_bdrag     (case, row)       B_drag = sum_j Tn_j^T B6_j Tn_j
 //   k_gen_project                     F_drag
-//   k_gen_solve     (case, w)         Z = -w^2 M + i w (B + B_drag) + C, dense complex LU with partial pivoting, Xi;
+//   k_gen_solve_blocked (case, w)     Z = -w^2 M + i w (B + B_drag) + C, dense complex LU with partial pivoting, Xi;
 //                                     on the support of the frequency-dependent terms M + A_w(w) and B + B_w(w) (gen_impedance),
 //                                     plus the case's operating point there when the case table carries them (OP)
 //   k_gen_relax     (case)            convergence bookkeeping, XiLast = 0.2 XiLast + 0.8 Xi
@@ -73,7 +73,7 @@ struct GenFdDev {
 };
 
 // per-case operating points (raftk_cases.op) on the support of fd_idx: GenFdDev plus the case table's op column and the tables
-// [nD or 1][n_op][n_fd][n_fd][nw].  Only the OP instantiations of k_gen_solve* take it, so that every other kernel keeps its
+// [nD or 1][n_op][n_fd][n_fd][nw].  Only the OP instantiations of k_gen_solve_blocked take it, so that every other kernel keeps its
 // parameter layout.
 struct GenFdOpDev : GenFdDev {
     const int *op;               // [nC of the whole table] operating point of every case
@@ -89,8 +89,9 @@ struct GenWork {                 // per-call workspace views
     double2 *XiLast;             // [nC][n][nw]
     double *Bmat;                // [nC][Ns][9]
     double *B_drag;              // [nC][n][n]
-    double2 *Z;                  // [nC][nw][n][n+1]  augmented systems; after a case's last pass its LU factors (LAPACK layout)
-    int *piv;                    // [nC][nw][n]       pivot row of every elimination step of that factorisation
+    double2 *Z;                  // [nC][nw][n][n+1]  augmented systems; after a case's last pass its LU factors (lu_blocked's
+                                 //                   layout: the columns of each panel of GB keep the rows they had then)
+    int *piv;                    // [nC][nw][n]       pivot row (of the whole system) of every elimination step of that factorisation
     int *flags;                  // [nC][4]: done, pass_not_converged, passes, RAFTK_FLAG_NAN | RAFTK_FLAG_SINGULAR (a zero pivot)
 };
 
@@ -378,112 +379,12 @@ __global__ void __launch_bounds__(128) k_gen_bdrag(GenDev D, GenWork W)
     for (int e = 0; e < 2; e++) { const int cc = tid + 128 * e; if (cc < n) W.B_drag[((size_t)c * n + r) * n + cc] = acc[e]; }
 }
 
-// k_gen_solve: grid (nw, units), block 256.  Augmented system [Z | F] (n x (n+1)) in global memory (L2-resident), right-looking
-// LU with partial pivoting on |re| + |im| (LAPACK izamax), back substitution; writes Xi and the convergence verdict.
-// OP (with FD): the case table carries operating points (GenFdOpDev); an instantiation of its own, so that the solves without
-// them compile as before.
-template <bool FD, bool OP = false>
-__global__ void __launch_bounds__(256) k_gen_solve(GenDev D, GenWork W, double2 *Xi, double tol, GenFdArg<OP> X)
-{
-    static_assert(FD || !OP, "operating points live on the support of the frequency-dependent terms");
-    __shared__ double pv[8];
-    __shared__ int pi_[8];
-    __shared__ double2 piv;
-    __shared__ int prow, bad;
-    __shared__ int fdpos[FD ? 256 : 1];
-    const int i = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, n = D.n, nw = D.nw, nc = n + 1;
-    if (W.flags[4 * c]) return;
-    const GenUnit U = gen_unit(D, c);
-    const int d = U.d;
-    const GenMats G = gen_mats(D, X, d);
-    const double *Ao = nullptr, *Bo = nullptr;
-    if constexpr (OP) gen_op_tables(D, X, U, Ao, Bo);
-    double2 *A = W.Z + ((size_t)c * nw + i) * (size_t)n * nc;
-    const double w = D.w[i], w2 = w * w;
-    const double *Bd = W.B_drag + (size_t)c * n * n;
-    if constexpr (FD) gen_fd_map(D, X, d, fdpos, tid, 256);
-    for (int t = tid; t < n * n; t += 256) {
-        const int a = t / n, b = t % n;
-        A[(size_t)a * nc + b] = gen_impedance<FD, OP>(D, X, G, fdpos, Bd, t, i, w, w2, Ao, Bo);
-    }
-    for (int a = tid; a < n; a += 256) {
-        const double2 f1 = W.F_iner[((size_t)c * n + a) * nw + i], f2 = W.F_drag[((size_t)c * n + a) * nw + i];
-        A[(size_t)a * nc + n] = make_double2(f1.x + f2.x, f1.y + f2.y);
-    }
-    if (tid == 0) bad = 0;
-    __syncthreads();
-    for (int k = 0; k < n; k++) {
-        // pivot search in column k, rows k..n-1 (first maximum wins, like izamax)
-        double best = -1.0; int bi = k;
-        for (int r = k + tid; r < n; r += 256) { const double2 v = A[(size_t)r * nc + k]; const double m = fabs(v.x) + fabs(v.y); if (m > best) { best = m; bi = r; } }
-        for (int o = 16; o >= 1; o >>= 1) {
-            const double ob = __shfl_xor_sync(0xffffffffu, best, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
-        }
-        if ((tid & 31) == 0) { pv[tid >> 5] = best; pi_[tid >> 5] = bi; }
-        __syncthreads();
-        if (tid == 0) {
-            double b0 = pv[0]; int r0 = pi_[0];
-            for (int t = 1; t < 8; t++) if (pv[t] > b0 || (pv[t] == b0 && pi_[t] < r0)) { b0 = pv[t]; r0 = pi_[t]; }
-            prow = r0;
-            W.piv[((size_t)c * nw + i) * n + k] = r0;
-        }
-        __syncthreads();
-        const int p = prow;
-        // whole rows, so that L ends in LAPACK's layout (k_gen_train_solve reuses these factors)
-        if (p != k) for (int b = tid; b < nc; b += 256) { const double2 t1 = A[(size_t)k * nc + b]; A[(size_t)k * nc + b] = A[(size_t)p * nc + b]; A[(size_t)p * nc + b] = t1; }
-        __syncthreads();
-        if (tid == 0) { bool zero; piv = piv_recip(A[(size_t)k * nc + k], zero); if (zero) bad = 1; }
-        __syncthreads();
-        const double2 ip = piv;
-        // multipliers l_r = a_rk / a_kk, then trailing update a_rb -= l_r a_kb (b = k+1 .. n incl. the right-hand side)
-        for (int r = k + 1 + tid; r < n; r += 256) { const double2 a = A[(size_t)r * nc + k]; A[(size_t)r * nc + k] = make_double2(a.x * ip.x - a.y * ip.y, a.x * ip.y + a.y * ip.x); }
-        __syncthreads();
-        const int rows = n - k - 1, cols = nc - k - 1;
-        for (int t = tid; t < rows * cols; t += 256) {
-            const int r = k + 1 + t / cols, b = k + 1 + t % cols;
-            const double2 l = A[(size_t)r * nc + k], ak = A[(size_t)k * nc + b];
-            double2 v = A[(size_t)r * nc + b];
-            v.x -= l.x * ak.x - l.y * ak.y; v.y -= l.x * ak.y + l.y * ak.x;
-            A[(size_t)r * nc + b] = v;
-        }
-        __syncthreads();
-    }
-    // back substitution on the last column
-    for (int k = n - 1; k >= 0; k--) {
-        if (tid == 0) {
-            A[(size_t)k * nc + n] = piv_div(A[(size_t)k * nc + n], A[(size_t)k * nc + k]);
-        }
-        __syncthreads();
-        const double2 x = A[(size_t)k * nc + n];
-        for (int r = tid; r < k; r += 256) {
-            const double2 a = A[(size_t)r * nc + k];
-            double2 b = A[(size_t)r * nc + n];
-            b.x -= a.x * x.x - a.y * x.y; b.y -= a.x * x.y + a.y * x.x;
-            A[(size_t)r * nc + n] = b;
-        }
-        __syncthreads();
-    }
-    int notconv = 0, nan = 0;
-    for (int a = tid; a < n; a += 256) {
-        const double2 x = A[(size_t)a * nc + n], l = W.XiLast[((size_t)c * n + a) * nw + i];
-        Xi[((size_t)c * n + a) * nw + i] = x;
-        if (isnan(x.x) || isnan(x.y)) nan = 1;
-        const double dx = x.x - l.x, dy = x.y - l.y;
-        if (!(sqrt(dx * dx + dy * dy) / (sqrt(x.x * x.x + x.y * x.y) + tol) < tol)) notconv = 1;     // raft_model.py:1101-1102
-    }
-    if (notconv) atomicOr(&W.flags[4 * c + 1], 1);
-    if (nan || bad) atomicOr(&W.flags[4 * c + 3], (nan ? RAFTK_FLAG_NAN : 0) | (bad ? RAFTK_FLAG_SINGULAR : 0));
-}
-
-// k_gen_solve_blocked: grid (nw, units), block 256.  Same system, same pivot rule and the same elimination order as
-// k_gen_solve, organised as a blocked right-looking LU (LAPACK zgetrf's structure) so that the work is done on chip:
-//   per block of GB columns:  panel (rows kb.., GB columns) factored in SHARED memory with partial pivoting; its row swaps
-//   applied to the rest of the rows; the GB x (rest) row block solved against the unit-lower panel head in shared memory;
-//   trailing update A22 -= L21 U12 with a 4 x 2 register tile per thread -- every A22 element is loaded once, receives its
-//   GB rank-1 contributions IN ELIMINATION ORDER (k ascending, the rounding sequence of the unblocked algorithm) and is
-//   stored once.  Traffic to the L2-resident matrix drops by GB (16) against the unblocked kernel's one pass per column;
-//   9 Mflop per 150 x 150 system then run from registers and shared memory.
+// k_gen_solve_blocked: grid (nw, units), block GT.  Augmented system [Z | F] (n x (n+1)) assembled in global memory
+// (L2-resident), factored by lu_blocked in panels of GB columns with the panel and the row block staged in shared memory
+// (raftk_lu.cuh): every element loaded once per panel, 9 Mflop per 150 x 150 system run from registers and shared memory.
+// Back substitution, then Xi and the convergence verdict.  The factors and pivot rows stay in W.Z / W.piv for the secondary
+// trains (k_gen_train_solve).  OP (with FD): the case table carries operating points (GenFdOpDev); an instantiation of its
+// own, so that the solves without them compile as before.
 #define GB 8
 #define GT 128
 template <bool FD, bool OP = false>
@@ -491,10 +392,7 @@ __global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W
 {
     static_assert(FD || !OP, "operating points live on the support of the frequency-dependent terms");
     extern __shared__ __align__(16) double smem_raw[];
-    __shared__ double pv[GT / 32];
-    __shared__ int pi_[GT / 32];
-    __shared__ int bad;
-    __shared__ int pivrow[GB];
+    __shared__ LuStaged<GT, GB> S;
     __shared__ int fdpos[FD ? 256 : 1];
     const int i = blockIdx.x, c = blockIdx.y, tid = threadIdx.x, n = D.n, nw = D.nw, nc = n + 1;
     if (W.flags[4 * c]) return;
@@ -517,123 +415,9 @@ __global__ void __launch_bounds__(GT, 4) k_gen_solve_blocked(GenDev D, GenWork W
         const double2 f1 = W.F_iner[((size_t)c * n + a) * nw + i], f2 = W.F_drag[((size_t)c * n + a) * nw + i];
         A[(size_t)a * nc + n] = make_double2(f1.x + f2.x, f1.y + f2.y);
     }
-    if (tid == 0) bad = 0;
     __syncthreads();
-    for (int kb = 0; kb < n; kb += GB) {
-        const int nb = min(GB, n - kb), m = n - kb;
-        // ---- 1. panel into shared memory ------------------------------------------------------------------------
-        for (int t = tid; t < m * nb; t += GT) { const int r = t / nb, j = t % nb; P[r * GB + j] = A[(size_t)(kb + r) * nc + kb + j]; }
-        __syncthreads();
-        // ---- 2. unblocked LU of the panel (pivot on |re| + |im|, first maximum wins, like izamax) ---------------------
-        for (int j = 0; j < nb; j++) {
-            double best = -1.0; int bi = j;
-            for (int r = j + tid; r < m; r += GT) { const double2 v = P[r * GB + j]; const double mg = fabs(v.x) + fabs(v.y); if (mg > best) { best = mg; bi = r; } }
-            for (int o = 16; o >= 1; o >>= 1) {
-                const double ob = __shfl_xor_sync(0xffffffffu, best, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-                if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
-            }
-            if ((tid & 31) == 0) { pv[tid >> 5] = best; pi_[tid >> 5] = bi; }
-            __syncthreads();
-            // every thread finishes the reduction itself (same winner everywhere) and reads the pivot before rows move
-            double b0 = pv[0]; int p = pi_[0];
-#pragma unroll
-            for (int t = 1; t < GT / 32; t++) if (pv[t] > b0 || (pv[t] == b0 && pi_[t] < p)) { b0 = pv[t]; p = pi_[t]; }
-            bool zero;
-            const double2 ip = piv_recip(P[p * GB + j], zero);
-            if (tid == 0) { pivrow[j] = p; W.piv[((size_t)c * nw + i) * n + kb + j] = kb + p; if (zero) bad = 1; }
-            __syncthreads();
-            if (p != j && tid < nb) { const double2 t1 = P[j * GB + tid]; P[j * GB + tid] = P[p * GB + tid]; P[p * GB + tid] = t1; }
-            __syncthreads();
-            // multipliers and the update of the panel's remaining columns in one sweep: thread per row
-            const int cols = nb - j - 1;
-            for (int r = j + 1 + tid; r < m; r += GT) {
-                const double2 v = P[r * GB + j];
-                const double2 l = make_double2(v.x * ip.x - v.y * ip.y, v.x * ip.y + v.y * ip.x);
-                P[r * GB + j] = l;
-                for (int b = 0; b < cols; b++) {
-                    const double2 ak = P[j * GB + j + 1 + b];
-                    double2 x = P[r * GB + j + 1 + b];
-                    x.x -= l.x * ak.x - l.y * ak.y; x.y -= l.x * ak.y + l.y * ak.x;
-                    P[r * GB + j + 1 + b] = x;
-                }
-            }
-            __syncthreads();
-        }
-        // ---- 3. panel back to the matrix; its row swaps applied, in order, to the columns outside the panel -------
-        for (int t = tid; t < m * nb; t += GT) { const int r = t / nb, j = t % nb; A[(size_t)(kb + r) * nc + kb + j] = P[r * GB + j]; }
-        for (int col = tid; col < nc; col += GT) {
-            if (col >= kb && col < kb + nb) continue;
-            for (int j = 0; j < nb; j++) {
-                const int p = pivrow[j];
-                if (p != j) { const double2 t1 = A[(size_t)(kb + j) * nc + col]; A[(size_t)(kb + j) * nc + col] = A[(size_t)(kb + p) * nc + col]; A[(size_t)(kb + p) * nc + col] = t1; }
-            }
-        }
-        __syncthreads();
-        // ---- 4. row block U12 = L11^-1 A12 (unit lower triangular solve per column, elimination order) -----------------
-        const int c0 = kb + nb, ncol = nc - c0;
-        for (int t = tid; t < nb * ncol; t += GT) { const int j = t / ncol, b = t % ncol; U[j * nc + b] = A[(size_t)(kb + j) * nc + c0 + b]; }
-        __syncthreads();
-        for (int b = tid; b < ncol; b += GT) {
-            for (int j = 0; j < nb; j++) {
-                const double2 uj = U[j * nc + b];
-                for (int r = j + 1; r < nb; r++) {
-                    const double2 l = P[r * GB + j];
-                    double2 v = U[r * nc + b];
-                    v.x -= l.x * uj.x - l.y * uj.y; v.y -= l.x * uj.y + l.y * uj.x;
-                    U[r * nc + b] = v;
-                }
-            }
-        }
-        __syncthreads();
-        for (int t = tid; t < nb * ncol; t += GT) { const int j = t / ncol, b = t % ncol; A[(size_t)(kb + j) * nc + c0 + b] = U[j * nc + b]; }
-        // ---- 5. trailing update A22 -= L21 U12: 4 x 2 register tile per thread, contributions in elimination order --
-        const int m2 = m - nb;
-        const int tr = (m2 + 3) / 4, tc = (ncol + 1) / 2;
-        for (int t = tid; t < tr * tc; t += GT) {
-            const int r0 = 4 * (t / tc), b0 = 2 * (t % tc);
-            double2 acc[4][2];
-#pragma unroll
-            for (int x = 0; x < 4; x++)
-#pragma unroll
-                for (int y = 0; y < 2; y++)
-                    acc[x][y] = (r0 + x < m2 && b0 + y < ncol) ? A[(size_t)(c0 + r0 + x) * nc + c0 + b0 + y] : make_double2(0.0, 0.0);
-            for (int j = 0; j < nb; j++) {
-                double2 l[4], u[2];
-#pragma unroll
-                for (int x = 0; x < 4; x++) l[x] = P[min(nb + r0 + x, m - 1) * GB + j];
-#pragma unroll
-                for (int y = 0; y < 2; y++) u[y] = U[j * nc + min(b0 + y, ncol - 1)];
-#pragma unroll
-                for (int x = 0; x < 4; x++)
-#pragma unroll
-                    for (int y = 0; y < 2; y++) {
-                        acc[x][y].x -= l[x].x * u[y].x - l[x].y * u[y].y;
-                        acc[x][y].y -= l[x].x * u[y].y + l[x].y * u[y].x;
-                    }
-            }
-#pragma unroll
-            for (int x = 0; x < 4; x++)
-#pragma unroll
-                for (int y = 0; y < 2; y++)
-                    if (r0 + x < m2 && b0 + y < ncol) A[(size_t)(c0 + r0 + x) * nc + c0 + b0 + y] = acc[x][y];
-        }
-        __syncthreads();
-    }
-    // back substitution on the last column
-    for (int k = n - 1; k >= 0; k--) {
-        if (tid == 0) {
-            A[(size_t)k * nc + n] = piv_div(A[(size_t)k * nc + n], A[(size_t)k * nc + k]);
-        }
-        __syncthreads();
-        const double2 x = A[(size_t)k * nc + n];
-        for (int r = tid; r < k; r += GT) {
-            const double2 a = A[(size_t)r * nc + k];
-            double2 b = A[(size_t)r * nc + n];
-            b.x -= a.x * x.x - a.y * x.y; b.y -= a.x * x.y + a.y * x.x;
-            A[(size_t)r * nc + n] = b;
-        }
-        __syncthreads();
-    }
+    const int bad = lu_blocked<GT, true, true>(A, nc, A + n, nc, n, 1, GB, S, P, U, W.piv + ((size_t)c * nw + i) * n);
+    lu_back_subst<GT>(A, (size_t)nc, A + n, (size_t)nc, n, 1, tid);
     int notconv = 0, nan = 0;
     for (int a = tid; a < n; a += GT) {
         const double2 x = A[(size_t)a * nc + n], l = W.XiLast[((size_t)c * n + a) * nw + i];
@@ -657,8 +441,10 @@ __global__ void __launch_bounds__(256) k_gen_init(GenDev D, GenWork W, double xi
 }
 
 // k_gen_train_solve: grid (nw, nC), block 128, secondary trains only: Xi = Z_p^-1 (F_iner + F_drag) with the LU factors of the
-// primary's last pass (L unit lower, U upper, row interchanges piv applied in elimination order; raft_model.py:1200-1236).
-// A zero diagonal of U (the primary's singular bin) sets RAFTK_FLAG_SINGULAR in the secondary's flag word 3 as well.
+// primary's last pass (raft_model.py:1200-1236): the unit-lower solve applies each panel's interchanges (W.piv) as it reaches
+// the panel's first column, which is where k_gen_solve_blocked applied them to the right-hand side, so that every element
+// receives the same updates in the same order; then the upper solve.  A zero diagonal of U (the primary's singular bin)
+// sets RAFTK_FLAG_SINGULAR in the secondary's flag word 3 as well.
 __global__ void __launch_bounds__(128) k_gen_train_solve(GenDev D, GenWork W, const int *primary, double2 *Xi)
 {
     __shared__ double2 b[256];
@@ -672,36 +458,19 @@ __global__ void __launch_bounds__(128) k_gen_train_solve(GenDev D, GenWork W, co
         b[a] = make_double2(f1.x + f2.x, f1.y + f2.y);
     }
     __syncthreads();
-    if (tid == 0)
-        for (int k = 0; k < n; k++) { const int q = pv[k]; if (q != k) { const double2 t = b[k]; b[k] = b[q]; b[q] = t; } }
-    __syncthreads();
     for (int k = 0; k < n - 1; k++) {                           // L y = P b
-        const double2 x = b[k];
-        for (int r = k + 1 + tid; r < n; r += 128) {
-            const double2 l = A[(size_t)r * nc + k];
-            double2 v = b[r];
-            v.x -= l.x * x.x - l.y * x.y; v.y -= l.x * x.y + l.y * x.x;
-            b[r] = v;
+        if (k % GB == 0) {
+            if (tid == 0)
+                for (int j = k; j < min(k + GB, n); j++) { const int q = pv[j]; if (q != j) { const double2 t = b[j]; b[j] = b[q]; b[q] = t; } }
+            __syncthreads();
         }
+        const double2 x = b[k];
+        for (int r = k + 1 + tid; r < n; r += 128) { double2 v = b[r]; cmsub(v, A[(size_t)r * nc + k], x); b[r] = v; }
         __syncthreads();
     }
-    int zero = 0;                                               // a zero diagonal of U (thread 0)
-    for (int k = n - 1; k >= 0; k--) {                          // U x = y, as the back substitution of k_gen_solve*
-        if (tid == 0) {
-            const double2 a = A[(size_t)k * nc + k];
-            if (a.x == 0.0 && a.y == 0.0) zero = 1;
-            b[k] = piv_div(b[k], a);
-        }
-        __syncthreads();
-        const double2 x = b[k];
-        for (int r = tid; r < k; r += 128) {
-            const double2 a = A[(size_t)r * nc + k];
-            double2 v = b[r];
-            v.x -= a.x * x.x - a.y * x.y; v.y -= a.x * x.y + a.y * x.x;
-            b[r] = v;
-        }
-        __syncthreads();
-    }
+    int zero = 0;                                               // a zero diagonal of U
+    for (int k = tid; k < n; k += 128) { const double2 a = A[(size_t)k * nc + k]; if (a.x == 0.0 && a.y == 0.0) zero = 1; }
+    lu_back_subst<128>(A, (size_t)nc, b, (size_t)1, n, 1, tid);                 // U x = y
     int nan = 0;
     for (int a = tid; a < n; a += 128) {
         const double2 x = b[a];

@@ -3,171 +3,25 @@
 
 // ------------------------------------------------------------------------------------------------
 // K3: dense complex solve per frequency (farm system response).  One CTA per frequency, matrix in
-// shared memory, LU with partial pivoting, nrhs right-hand sides.
+// shared memory, LU with partial pivoting (raftk_lu.cuh: column at a time up to n = 24, else in panels of 8 columns), nrhs
+// right-hand sides.
 // ------------------------------------------------------------------------------------------------
-// Dense complex LU in shared memory, shared by the system-solve kernels.  A [n][nc] is the augmented system (nc = n + nrhs),
-// partial pivoting on |re| + |im| with the first maximum winning (LAPACK izamax), right-hand sides eliminated along.
-// A "group" of gsize threads (a warp when WARP, else the whole CTA) works on one system; gtid is the thread's index in it.
-template <bool WARP> __device__ __forceinline__ void gsync() { if (WARP) __syncwarp(); else __syncthreads(); }
-
-// Pivot reciprocals and back-substitution quotients at the pivot's own scale: piv_recip / piv_div (raftk_common.cuh).
-
-// one elimination step on column col: pivot search over rows col..n-1, swap of the full rows, multipliers.  Returns via *bad.
-template <bool WARP>
-__device__ __forceinline__ void lu_pivot_step(double2 *A, int n, int nc, int col, int gtid, int gsize, int *piv_s, double2 *rinv_s, int *bad_s)
-{
-    if (gtid < 32) {
-        double best = -1.0; int p = col;
-        for (int r = col + gtid; r < n; r += 32) {
-            const double t = fabs(A[r * nc + col].x) + fabs(A[r * nc + col].y);
-            if (t > best) { best = t; p = r; }
-        }
-        for (int o = 16; o >= 1; o >>= 1) {
-            const double ob = __shfl_xor_sync(0xffffffffu, best, o);
-            const int op = __shfl_xor_sync(0xffffffffu, p, o);
-            if (ob > best || (ob == best && op < p)) { best = ob; p = op; }
-        }
-        if (gtid == 0) {
-            *piv_s = p;
-            bool zero;
-            *rinv_s = piv_recip(A[p * nc + col], zero);
-            if (zero && *bad_s == 0) *bad_s = col + 1;
-        }
-    }
-    gsync<WARP>();
-    const int p = *piv_s;
-    if (p != col) for (int t = gtid; t < nc; t += gsize) { const double2 tmp = A[col * nc + t]; A[col * nc + t] = A[p * nc + t]; A[p * nc + t] = tmp; }
-    gsync<WARP>();
-    const double2 ri = *rinv_s;
-    for (int r = col + 1 + gtid; r < n; r += gsize) {
-        const double2 v = A[r * nc + col];
-        A[r * nc + col] = make_double2(v.x * ri.x - v.y * ri.y, v.x * ri.y + v.y * ri.x);
-    }
-    gsync<WARP>();
-}
-
-// back substitution of every right-hand side, row by row from the bottom, the column updates spread over the group
-template <bool WARP>
-__device__ __forceinline__ void lu_back_subst(double2 *A, int n, int nc, int nrhs, int gtid, int gsize)
-{
-    for (int r = n - 1; r >= 0; r--) {
-        const double2 pv = A[r * nc + r];
-        for (int rh = gtid; rh < nrhs; rh += gsize) A[r * nc + n + rh] = piv_div(A[r * nc + n + rh], pv);
-        gsync<WARP>();
-        for (int t = gtid; t < r * nrhs; t += gsize) {
-            const int rr = t / nrhs, rh = t - rr * nrhs;
-            const double2 a = A[rr * nc + r], x = A[r * nc + n + rh];
-            double2 b = A[rr * nc + n + rh];
-            b.x -= a.x * x.x - a.y * x.y; b.y -= a.x * x.y + a.y * x.x;
-            A[rr * nc + n + rh] = b;
-        }
-        gsync<WARP>();
-    }
-}
-
-// column-at-a-time LU (small systems: one warp per system, or any size with one CTA per system)
-template <bool WARP>
-__device__ __forceinline__ void lu_unblocked(double2 *A, int n, int nc, int nrhs, int gtid, int gsize, int *piv_s, double2 *rinv_s, int *bad_s)
-{
-    for (int k = 0; k < n; k++) {
-        lu_pivot_step<WARP>(A, n, nc, k, gtid, gsize, piv_s, rinv_s, bad_s);
-        const int rows = n - k - 1, cols = nc - k - 1;
-        for (int t = gtid; t < rows * cols; t += gsize) {
-            const int r = k + 1 + t / cols, cidx = k + 1 + t % cols;
-            const double2 l = A[r * nc + k], u = A[k * nc + cidx];
-            double2 v = A[r * nc + cidx];
-            v.x -= l.x * u.x - l.y * u.y; v.y -= l.x * u.y + l.y * u.x;
-            A[r * nc + cidx] = v;
-        }
-        gsync<WARP>();
-    }
-    lu_back_subst<WARP>(A, n, nc, nrhs, gtid, gsize);
-}
-
-// blocked right-looking LU (one CTA per system): panels of LB columns factored column by column, then the row block and the
-// trailing matrix receive the panel's LB rank-1 contributions from registers (4 x 2 tile per thread), in elimination order --
-// the rounding sequence of the column-at-a-time algorithm with a quarter of its shared-memory traffic.
-#define LB 8
-__device__ __forceinline__ void lu_blocked(double2 *A, int n, int nc, int nrhs, int *piv_s, double2 *rinv_s, int *bad_s)
-{
-    const int tid = threadIdx.x, T = blockDim.x;
-    for (int kb = 0; kb < n; kb += LB) {
-        const int nb = min(LB, n - kb), c0 = kb + nb;
-        for (int j = 0; j < nb; j++) {                                 // panel: pivot, swap, multipliers, update of the panel's own columns
-            const int col = kb + j;
-            lu_pivot_step<false>(A, n, nc, col, tid, T, piv_s, rinv_s, bad_s);
-            const int rows = n - col - 1, cols = c0 - col - 1;
-            for (int t = tid; t < rows * cols; t += T) {
-                const int r = col + 1 + t / cols, cidx = col + 1 + t % cols;
-                const double2 l = A[r * nc + col], u = A[col * nc + cidx];
-                double2 v = A[r * nc + cidx];
-                v.x -= l.x * u.x - l.y * u.y; v.y -= l.x * u.y + l.y * u.x;
-                A[r * nc + cidx] = v;
-            }
-            __syncthreads();
-        }
-        const int ncol = nc - c0;
-        for (int b = tid; b < ncol; b += T) {                          // row block: unit-lower triangular solve per column
-            for (int j = 0; j < nb; j++) {
-                const double2 uj = A[(kb + j) * nc + c0 + b];
-                for (int r = j + 1; r < nb; r++) {
-                    const double2 l = A[(kb + r) * nc + kb + j];
-                    double2 v = A[(kb + r) * nc + c0 + b];
-                    v.x -= l.x * uj.x - l.y * uj.y; v.y -= l.x * uj.y + l.y * uj.x;
-                    A[(kb + r) * nc + c0 + b] = v;
-                }
-            }
-        }
-        __syncthreads();
-        const int m2 = n - c0, tr = (m2 + 3) / 4, tc = (ncol + 1) / 2;
-        for (int t = tid; t < tr * tc; t += T) {                       // trailing update, 4 x 2 register tile
-            const int r0 = c0 + 4 * (t / tc), b0 = c0 + 2 * (t % tc);
-            double2 acc[4][2];
-#pragma unroll
-            for (int x = 0; x < 4; x++)
-#pragma unroll
-                for (int y = 0; y < 2; y++) acc[x][y] = A[min(r0 + x, n - 1) * nc + min(b0 + y, nc - 1)];
-            for (int j = 0; j < nb; j++) {
-                double2 l[4], u[2];
-#pragma unroll
-                for (int x = 0; x < 4; x++) l[x] = A[min(r0 + x, n - 1) * nc + kb + j];
-#pragma unroll
-                for (int y = 0; y < 2; y++) u[y] = A[(kb + j) * nc + min(b0 + y, nc - 1)];
-#pragma unroll
-                for (int x = 0; x < 4; x++)
-#pragma unroll
-                    for (int y = 0; y < 2; y++) {
-                        acc[x][y].x -= l[x].x * u[y].x - l[x].y * u[y].y;
-                        acc[x][y].y -= l[x].x * u[y].y + l[x].y * u[y].x;
-                    }
-            }
-#pragma unroll
-            for (int x = 0; x < 4; x++)
-#pragma unroll
-                for (int y = 0; y < 2; y++)
-                    if (r0 + x < n && b0 + y < nc) A[(r0 + x) * nc + b0 + y] = acc[x][y];
-        }
-        __syncthreads();
-    }
-    lu_back_subst<false>(A, n, nc, nrhs, tid, T);
-}
-
 __global__ void __launch_bounds__(128) k_system_solve(int n, int nrhs, double2 *Z, double2 *F, int *info)
 {
     extern __shared__ __align__(16) double smem_raw[];
     double2 *A = reinterpret_cast<double2 *>(smem_raw);              // [n][n+nrhs] augmented
     __shared__ int piv_s, bad_s;
     __shared__ double2 rinv_s;
+    LuSlots S{&piv_s, &rinv_s, &bad_s};
     const int iw = blockIdx.x, tid = threadIdx.x, nc = n + nrhs;
     double2 *Zg = Z + (size_t)iw * n * n, *Fg = F + (size_t)iw * n * nrhs;
     for (int t = tid; t < n * n; t += blockDim.x) A[(t / n) * nc + (t % n)] = Zg[t];
     for (int t = tid; t < n * nrhs; t += blockDim.x) A[(t / nrhs) * nc + n + (t % nrhs)] = Fg[t];
-    if (tid == 0) bad_s = 0;
     __syncthreads();
-    if (n > 24) lu_blocked(A, n, nc, nrhs, &piv_s, &rinv_s, &bad_s);
-    else lu_unblocked<false>(A, n, nc, nrhs, tid, blockDim.x, &piv_s, &rinv_s, &bad_s);
+    const int bad = n > 24 ? lu_blocked<128, false, false>(A, nc, A + n, nc, n, nrhs, 8, S) : lu_unblocked<128>(A, n, nc, tid, S);
+    lu_back_subst<128>(A, nc, A + n, nc, n, nrhs, tid);
     for (int t = tid; t < n * nrhs; t += blockDim.x) Fg[t] = A[(t / nrhs) * nc + n + (t % nrhs)];
-    if (tid == 0 && info) info[iw] = bad_s;
+    if (tid == 0 && info) info[iw] = bad;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -176,7 +30,7 @@ __global__ void __launch_bounds__(128) k_system_solve(int n, int nrhs, double2 *
 // F = F_BEM_i + F_iner_i + F_drag_i (+ F_2nd_i) stacked, Xi_sys = Z_sys^-1 F.  Everything is read from device-resident
 // outputs of the drag-linearisation solve: no host assembly of Z, no per-case transfer of nw n^2 complex numbers.
 // WARP = true : small systems (6N <= 24), one WARP per (frequency, case), up to FARM_WPC systems per CTA, no CTA-wide barriers;
-// WARP = false: one CTA per (frequency, case), blocked LU.
+// WARP = false: one CTA per (frequency, case) of 256 threads, blocked LU in panels of 8 columns.
 // A call solves nF farms of N FOWTs each (one farm: nF = 1): design f * N + i is FOWT i of farm f.  The shared-memory and
 // register kernels take the farm from blockIdx.z, so the systems a CTA packs along the frequency axis belong to one farm and
 // a ragged last group ends at nw; k_farm_response_global walks (farm, case, frequency) systems.
@@ -298,152 +152,28 @@ __global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(De
     if (iw >= nw) return;                                            // (warp-uniform; no CTA-wide barrier follows in the WARP variant)
     double2 *A = reinterpret_cast<double2 *>(smem_raw) + (size_t)g * n * nc;
     const size_t u = (size_t)f * P.nC + c;                           // row of Xi and info
+    LuSlots S{&piv_s[g], &rinv_s[g], &bad_s[g]};
     farm_assemble<OP>(D, Cs, P, f, c, iw, A, gtid, gsize);
-    if (gtid == 0) bad_s[g] = 0;
-    gsync<WARP>();
-    if (WARP) lu_unblocked<true>(A, n, nc, 1, gtid, gsize, &piv_s[g], &rinv_s[g], &bad_s[g]);
-    else lu_blocked(A, n, nc, 1, &piv_s[g], &rinv_s[g], &bad_s[g]);
+    constexpr int T = WARP ? 32 : 256;
+    gsync<T>();
+    int bad;
+    if constexpr (WARP) bad = lu_unblocked<T>(A, n, nc, gtid, S);
+    else bad = lu_blocked<T, false, false>(A, nc, A + n, nc, n, 1, 8, S);
+    lu_back_subst<T>(A, nc, A + n, nc, n, 1, gtid);
     for (int a = gtid; a < n; a += gsize) P.Xi[(u * n + a) * nw + iw] = A[a * nc + n];
-    if (gtid == 0 && P.info) P.info[u * nw + iw] = bad_s[g];
-    if constexpr (PEER) farm_peer_store(P, A, nc, u, iw, bad_s[g], f, c, gtid, gsize);
+    if (gtid == 0 && P.info) P.info[u * nw + iw] = bad;
+    if constexpr (PEER) farm_peer_store(P, A, nc, u, iw, bad, f, c, gtid, gsize);
 }
 
 // ------------------------------------------------------------------------------------------------
 // K3d: dense solves whose augmented system does not fit in one CTA's shared memory (farms of 20 and more FOWTs, any n for
-// raftk_system_solve).  The system stays in global memory (L2-resident while the CTA works on it); lu_global factors it with
-// the numerical contract of lu_blocked: partial pivoting on |re| + |im| with the first maximum winning (LAPACK izamax), row
-// swaps over every column the solve still reads, and each trailing element receiving its rank-1 contributions in elimination
-// order, so the rounding sequence is the column-at-a-time algorithm's.  Per panel of pw columns:
-//   1. the panel (rows kb..n-1) is copied to shared memory and factored there column by column;
-//   2. it goes back, and one thread per remaining column applies the panel's row swaps in order and the unit-lower solve
-//      of the row block;
-//   3. the trailing matrix takes the panel's pw rank-1 contributions from a 4 x 2 register tile per thread: every element is
-//      loaded and stored once per panel, so the panel width divides the traffic to the matrix.
-// Back substitution of the nrhs right-hand sides follows row by row.  Every thread of the CTA takes part; each kernel
-// loops over its systems with persistent CTAs, so a result depends on nothing but the system itself.
+// raftk_system_solve).  The system stays in global memory (L2-resident while the CTA works on it) and lu_blocked factors it
+// with its panel staged in shared memory (raftk_lu.cuh), pw columns wide (glu_plan); back substitution of the nrhs
+// right-hand sides follows.  Every thread of the CTA takes part; each kernel loops over its systems with persistent CTAs, so
+// a result depends on nothing but the system itself.
 // ------------------------------------------------------------------------------------------------
 #define GLU_T 256
 #define GLU_PWMAX 16
-struct GluShared {
-    double best[GLU_T / 32];
-    int idx[GLU_T / 32];
-    int piv[GLU_PWMAX];
-    int bad;
-};
-
-__device__ __forceinline__ void cmsub(double2 &v, const double2 l, const double2 u)
-{
-    v.x -= l.x * u.x - l.y * u.y; v.y -= l.x * u.y + l.y * u.x;
-}
-
-// The augmented system [A | B]: A [n][lda] (columns 0..n-1), B [n][ldb] (the nrhs right-hand sides, columns n..n+nrhs-1).
-// Ps: dynamic shared memory of n * pw double2.  On return B holds the solutions and S.bad the info word (k+1 of the first
-// zero pivot, else 0; read it after a __syncthreads()).  The factored A's columns left of each panel keep their pre-swap rows.
-__device__ __forceinline__ void lu_global(double2 *A, int lda, double2 *B, int ldb, int n, int nrhs, int pw, double2 *Ps, GluShared &S)
-{
-    const int tid = threadIdx.x, nc = n + nrhs;
-    auto el = [&](int r, int col) -> double2 * { return col < n ? A + (size_t)r * lda + col : B + (size_t)r * ldb + (col - n); };
-    if (tid == 0) S.bad = 0;
-    for (int kb = 0; kb < n; kb += pw) {
-        const int nb = min(pw, n - kb), m = n - kb, c0 = kb + nb;
-        // ---- 1. panel LU in shared memory -----------------------------------------------------------------------
-        for (int t = tid; t < m * nb; t += GLU_T) { const int r = t / nb, j = t - r * nb; Ps[r * pw + j] = A[(size_t)(kb + r) * lda + kb + j]; }
-        __syncthreads();
-        for (int j = 0; j < nb; j++) {
-            double best = -1.0; int p = j;
-            for (int r = j + tid; r < m; r += GLU_T) {
-                const double2 v = Ps[r * pw + j];
-                const double t = fabs(v.x) + fabs(v.y);
-                if (t > best) { best = t; p = r; }
-            }
-            for (int o = 16; o >= 1; o >>= 1) {
-                const double ob = __shfl_xor_sync(0xffffffffu, best, o);
-                const int op = __shfl_xor_sync(0xffffffffu, p, o);
-                if (ob > best || (ob == best && op < p)) { best = ob; p = op; }
-            }
-            if ((tid & 31) == 0) { S.best[tid >> 5] = best; S.idx[tid >> 5] = p; }
-            __syncthreads();
-            best = S.best[0]; p = S.idx[0];                            // every thread finishes the reduction: same winner everywhere
-#pragma unroll
-            for (int q = 1; q < GLU_T / 32; q++) if (S.best[q] > best || (S.best[q] == best && S.idx[q] < p)) { best = S.best[q]; p = S.idx[q]; }
-            bool zero;
-            const double2 ri = piv_recip(Ps[p * pw + j], zero);
-            __syncthreads();                                           // pivot and reduction slots read by all before they change
-            if (tid == 0) { S.piv[j] = p; if (zero && S.bad == 0) S.bad = kb + j + 1; }
-            if (p != j && tid < nb) { const double2 t1 = Ps[j * pw + tid]; Ps[j * pw + tid] = Ps[p * pw + tid]; Ps[p * pw + tid] = t1; }
-            __syncthreads();
-            for (int r = j + 1 + tid; r < m; r += GLU_T) {             // multiplier, then the panel's columns right of j
-                const double2 v = Ps[r * pw + j];
-                const double2 l = make_double2(v.x * ri.x - v.y * ri.y, v.x * ri.y + v.y * ri.x);
-                Ps[r * pw + j] = l;
-                for (int b = j + 1; b < nb; b++) { double2 x = Ps[r * pw + b]; cmsub(x, l, Ps[j * pw + b]); Ps[r * pw + b] = x; }
-            }
-            __syncthreads();
-        }
-        // ---- 2. panel back; row swaps and the row block's unit-lower solve, one thread per column ---------------------
-        for (int t = tid; t < m * nb; t += GLU_T) { const int r = t / nb, j = t - r * nb; A[(size_t)(kb + r) * lda + kb + j] = Ps[r * pw + j]; }
-        for (int col = c0 + tid; col < nc; col += GLU_T) {
-            for (int j = 0; j < nb; j++) {
-                const int p = S.piv[j];
-                if (p != j) { double2 *x = el(kb + j, col), *y = el(kb + p, col); const double2 t1 = *x; *x = *y; *y = t1; }
-            }
-            for (int j = 0; j < nb; j++) {
-                const double2 uj = *el(kb + j, col);
-                for (int r = j + 1; r < nb; r++) { double2 *q = el(kb + r, col); double2 v = *q; cmsub(v, Ps[r * pw + j], uj); *q = v; }
-            }
-        }
-        __syncthreads();
-        // ---- 3. trailing update, 4 x 2 register tile, contributions in elimination order --------------------------------
-        const int m2 = n - c0, ncol = nc - c0, tr = (m2 + 3) / 4, tc = (ncol + 1) / 2;
-        for (int t = tid; t < tr * tc; t += GLU_T) {
-            const int r0 = 4 * (t / tc), b0 = 2 * (t - (t / tc) * tc);
-            double2 *cp[2];
-            size_t ld[2];
-#pragma unroll
-            for (int y = 0; y < 2; y++) {
-                const int col = min(c0 + b0 + y, nc - 1);
-                cp[y] = col < n ? A + col : B + (col - n);
-                ld[y] = col < n ? (size_t)lda : (size_t)ldb;
-            }
-            double2 acc[4][2];
-#pragma unroll
-            for (int x = 0; x < 4; x++)
-#pragma unroll
-                for (int y = 0; y < 2; y++)
-                    acc[x][y] = (r0 + x < m2 && b0 + y < ncol) ? cp[y][(size_t)(c0 + r0 + x) * ld[y]] : make_double2(0.0, 0.0);
-            for (int j = 0; j < nb; j++) {
-                double2 l[4], u[2];
-#pragma unroll
-                for (int x = 0; x < 4; x++) l[x] = Ps[min(nb + r0 + x, m - 1) * pw + j];
-#pragma unroll
-                for (int y = 0; y < 2; y++) u[y] = cp[y][(size_t)(kb + j) * ld[y]];
-#pragma unroll
-                for (int x = 0; x < 4; x++)
-#pragma unroll
-                    for (int y = 0; y < 2; y++) cmsub(acc[x][y], l[x], u[y]);
-            }
-#pragma unroll
-            for (int x = 0; x < 4; x++)
-#pragma unroll
-                for (int y = 0; y < 2; y++)
-                    if (r0 + x < m2 && b0 + y < ncol) cp[y][(size_t)(c0 + r0 + x) * ld[y]] = acc[x][y];
-        }
-        __syncthreads();
-    }
-    // ---- back substitution, every right-hand side ------------------------------------------------------------------
-    for (int r = n - 1; r >= 0; r--) {
-        const double2 pv = A[(size_t)r * lda + r];
-        for (int rh = tid; rh < nrhs; rh += GLU_T) B[(size_t)r * ldb + rh] = piv_div(B[(size_t)r * ldb + rh], pv);
-        __syncthreads();
-        for (int t = tid; t < r * nrhs; t += GLU_T) {
-            const int rr = t / nrhs, rh = t - rr * nrhs;
-            double2 b = B[(size_t)rr * ldb + rh];
-            cmsub(b, A[(size_t)rr * lda + r], B[(size_t)r * ldb + rh]);
-            B[(size_t)rr * ldb + rh] = b;
-        }
-        __syncthreads();
-    }
-}
 
 // farm system response of k_farm_response (same assembly) for any N: persistent CTAs, CTA b owns slab b of the workspace
 // ([6N][6N+1] double2) and solves the (farm, case, frequency) systems b, b + gridDim.x, ... of the nF * nC * nw in all
@@ -451,7 +181,7 @@ template <bool OP = false>
 __global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D, CasesDev Cs, FarmParams P, double2 *ws, int pw)
 {
     extern __shared__ __align__(16) double smem_raw[];
-    __shared__ GluShared S;
+    __shared__ LuStaged<GLU_T, GLU_PWMAX> S;
     double2 *Ps = reinterpret_cast<double2 *>(smem_raw);
     const int n = 6 * P.N, nc = n + 1, nw = P.nw;
     double2 *A = ws + (size_t)blockIdx.x * n * nc;
@@ -461,9 +191,10 @@ __global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D,
         const int iw = (int)(s - u * nw), f = (int)(u / P.nC), c = (int)(u - (long long)f * P.nC);
         farm_assemble<OP>(D, Cs, P, f, c, iw, A, threadIdx.x, GLU_T);
         __syncthreads();
-        lu_global(A, nc, A + n, nc, n, 1, pw, Ps, S);
+        const int bad = lu_blocked<GLU_T, true, false>(A, nc, A + n, nc, n, 1, pw, S, Ps);
+        lu_back_subst<GLU_T>(A, (size_t)nc, A + n, (size_t)nc, n, 1, threadIdx.x);
         for (int a = threadIdx.x; a < n; a += GLU_T) P.Xi[((size_t)u * n + a) * nw + iw] = A[(size_t)a * nc + n];
-        if (threadIdx.x == 0 && P.info) P.info[(size_t)u * nw + iw] = S.bad;
+        if (threadIdx.x == 0 && P.info) P.info[(size_t)u * nw + iw] = bad;
         __syncthreads();                                               // the slab is rewritten by the next system
     }
 }
@@ -472,11 +203,13 @@ __global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D,
 __global__ void __launch_bounds__(GLU_T, 2) k_system_solve_global(int n, int nw, int nrhs, int pw, double2 *Z, double2 *F, int *info)
 {
     extern __shared__ __align__(16) double smem_raw[];
-    __shared__ GluShared S;
+    __shared__ LuStaged<GLU_T, GLU_PWMAX> S;
     double2 *Ps = reinterpret_cast<double2 *>(smem_raw);
     for (int iw = blockIdx.x; iw < nw; iw += gridDim.x) {
-        lu_global(Z + (size_t)iw * n * n, n, F + (size_t)iw * n * nrhs, nrhs, n, nrhs, pw, Ps, S);
-        if (threadIdx.x == 0 && info) info[iw] = S.bad;
+        double2 *A = Z + (size_t)iw * n * n, *B = F + (size_t)iw * n * nrhs;
+        const int bad = lu_blocked<GLU_T, true, false>(A, n, B, nrhs, n, nrhs, pw, S, Ps);
+        lu_back_subst<GLU_T>(A, (size_t)n, B, (size_t)nrhs, n, nrhs, threadIdx.x);
+        if (threadIdx.x == 0 && info) info[iw] = bad;
         __syncthreads();
     }
 }

@@ -1,13 +1,11 @@
-"""Generalised degrees of freedom: both LU kernels of raftk_general_solve_dynamics -- k_gen_solve_blocked (default) and the
-column-at-a-time k_gen_solve (RAFTK_GEN_UNBLOCKED=1) -- at sizes around the blocked kernel's panel width (8) and up to the
-limit of 256 DOFs, against oracle.general_solve_dynamics, asserted through solver.last_dispatch().
+"""Generalised degrees of freedom: the LU kernel of raftk_general_solve_dynamics, k_gen_solve_blocked, at sizes around its
+panel width (8) and up to the limit of 256 DOFs, against oracle.general_solve_dynamics, asserted through solver.last_dispatch().
 
 The designs are synthetic: the rigid OC3spar on a small grid, with n - 6 seeded smooth mode shapes added to the node
 transformation (gen_Tn = [I6 | modes], gen_rr = node offset from the reference point) and modal blocks in M, B, C.  The
 modal stiffness couples each mode to the next (a cyclic shift of weight 3), so partial pivoting swaps rows.  At n = 6 the
 construction is the rigid design itself: the CPU test below checks that the oracle's generalised solve reproduces its rigid
 solve there."""
-import os
 
 import numpy as np
 import pytest
@@ -85,34 +83,26 @@ def test_construction_pivots_and_couples(oracle):
     assert np.abs(F[6:]).max() > 1e-3 * np.abs(F[:6]).max()
 
 
-def _gpu_solve(monkeypatch, unblocked, P, M, B, C, cs, n_iter):
+def _gpu_solve(P, M, B, C, cs, n_iter):
     from raft_b200 import solver
-    if unblocked:
-        monkeypatch.setenv("RAFTK_GEN_UNBLOCKED", "1")
-    else:
-        monkeypatch.delenv("RAFTK_GEN_UNBLOCKED", raising=False)
     Xi, st = solver.general_solve_dynamics(P, M, B, C, solver.CaseTable(cs), n_iter=n_iter)
     return Xi, st, solver.last_dispatch()
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("n", [6, 7, 8, 9, 16, 17, 64, 256])
-def test_lu_kernels_vs_oracle(n, monkeypatch, oracle):
+def test_lu_kernels_vs_oracle(n, oracle):
     nw = 12 if n > 64 else 32
     n_iter = 4 if n > 64 else 10
     P, M, B, C = general_design(n, nw)
     cs = _sea()
     gd = oracle.GeneralDesign(P)
     ref = [oracle.general_solve_dynamics(gd, M, B, C, 0, cs["Hs"][c], cs["Tp"][c], 0.0, cs["beta_deg"][c], nIter=n_iter) for c in range(2)]
-    runs = {}
-    for unblocked in (False, True):
-        Xi, st, rec = _gpu_solve(monkeypatch, unblocked, P, M, B, C, cs, n_iter)
-        assert rec["family"] == "general" and rec["kernel"] == ("gen-unblocked" if unblocked else "gen-blocked"), rec
-        for c, (Xo, so) in enumerate(ref):
-            assert st[c, 0] == so[0] and st[c, 1] == so[1] and st[c, 2] == 0, (c, st[c], so)
-            assert relerr(Xi[c], Xo) < RTOL, (unblocked, c, relerr(Xi[c], Xo))
-        runs[unblocked] = Xi
-    assert relerr(runs[True], runs[False]) < 1e-12
+    Xi, st, rec = _gpu_solve(P, M, B, C, cs, n_iter)
+    assert rec["family"] == "general" and rec["kernel"] == "gen-blocked", rec
+    for c, (Xo, so) in enumerate(ref):
+        assert st[c, 0] == so[0] and st[c, 1] == so[1] and st[c, 2] == 0, (c, st[c], so)
+        assert relerr(Xi[c], Xo) < RTOL, (c, relerr(Xi[c], Xo))
 
 
 @pytest.mark.gpu
@@ -122,41 +112,3 @@ def test_more_than_256_dofs_is_rejected():
     with pytest.raises(_lib.RaftkError, match="n_dof <= 256"):
         solver.general_solve_dynamics(P, M, B, C, solver.CaseTable(_sea(1)), n_iter=2)
     assert solver.last_dispatch()["kernel"] == "none"
-
-
-def _flexout():
-    z = np.load(os.path.join(GOLDEN, "flexout_VolturnUS-S-flexible.npz"))
-    G = {k: z[k] for k in z.files}
-    cases = []
-    for ic in range(3):
-        tr = G["ref_run_case%d_trains" % ic]
-        cases.append(dict(wave_spectrum=["JONSWAP"] * len(tr), wave_height=list(tr[:, 0]), wave_period=list(tr[:, 1]),
-                          wave_heading=list(tr[:, 2]), wave_gamma=[0.0] * len(tr)))
-    return G, {k[2:]: v for k, v in G.items() if k.startswith("P_")}, cases
-
-
-@pytest.mark.gpu
-def test_unblocked_kernel_trains_vs_reference_run(monkeypatch):
-    """k_gen_solve (whole-row swaps, whose factors k_gen_train_solve reuses) on the 150-DOF flexible design with wave trains:
-    every train within 1e-10 of the reference run, and the independent cases of a mixed table bit-identical to a call without
-    trains."""
-    from raft_b200 import packer, solver
-    monkeypatch.setenv("RAFTK_GEN_UNBLOCKED", "1")
-    G, P, cases = _flexout()
-    n_iter, xs = int(G["n_iter"]), float(G["xi_start"])
-    table, owner, first = packer.pack_case_trains(cases)
-    Xi, st = solver.general_solve_dynamics(P, G["gen_M"], G["gen_B"], G["gen_C"], solver.CaseTable(table), n_iter=n_iter, xi_start=xs)
-    rec = solver.last_dispatch()
-    assert rec["kernel"] == "gen-unblocked" and rec["trains"], rec
-    for ic in range(3):
-        ref = G["ref_run_case%d_Xi" % ic]
-        assert st[first[ic], 0] == int(G["ref_run_case%d_passes" % ic])
-        for ih, t in enumerate(np.nonzero(owner == ic)[0]):
-            assert relerr(Xi[t], ref[ih]) < RTOL, (ic, ih, relerr(Xi[t], ref[ih]))
-    assert st[:3, 3].tolist() == [0, 0, 0] and st[3].tolist() == [0, 1, 0, 3]
-    mixed, _, _ = packer.pack_case_trains([cases[0], cases[2], cases[1]])
-    Xm, sm = solver.general_solve_dynamics(P, G["gen_M"], G["gen_B"], G["gen_C"], solver.CaseTable(mixed), n_iter=n_iter, xi_start=xs)
-    solo, ss = solver.general_solve_dynamics(P, G["gen_M"], G["gen_B"], G["gen_C"], solver.CaseTable(packer.pack_cases([cases[0], cases[1]])),
-                                             n_iter=n_iter, xi_start=xs)
-    assert not solver.last_dispatch()["trains"]
-    assert np.array_equal(Xm[0], solo[0]) and np.array_equal(Xm[3], solo[1]) and np.array_equal(sm[[0, 3]], ss)

@@ -11,7 +11,7 @@ checkers (tests/general_fd_checker.py, tests/general_qtf_checker.py) on syntheti
 * BEM heading tables of one and of four headings with heading_adjust and x_ref / y_ref;
 * output-channel statistics (every wpow, 0, 1 and 2) and the response / channel statistics at 1, 127, 128, 129 and more bins.
 
-Every solve goes through solver.general_solve_dynamics with both LU kernels (default and RAFTK_GEN_UNBLOCKED=1; both force
+Every solve goes through solver.general_solve_dynamics (both force
 kernels with a QTF: tiles and RAFTK_QTF_DIAG=1) and asserts the kernel it ran.  Pass counts and the converged flag equal
 the checker's; Xi is held per train to RTOL over the whole array and, per DOF row with a peak >= 1e-6 of the train's, to
 ROW_RTOL of that row's own peak (an array-level bound alone would hide a wrong modal row at 1 % of the peak); measured
@@ -35,12 +35,11 @@ _WORST = {"array": 0.0, "row": 0.0}
 _CHECKER = {}
 
 
-def _env(monkeypatch, unblocked, diag=False):
-    for name, on in (("RAFTK_GEN_UNBLOCKED", unblocked), ("RAFTK_QTF_DIAG", diag)):
-        if on:
-            monkeypatch.setenv(name, "1")
-        else:
-            monkeypatch.delenv(name, raising=False)
+def _env(monkeypatch, diag=False):
+    if diag:
+        monkeypatch.setenv("RAFTK_QTF_DIAG", "1")
+    else:
+        monkeypatch.delenv("RAFTK_QTF_DIAG", raising=False)
 
 
 def _checker(key, oracle, P, M, B, Cm, fd, qtf, trains, n_iter):
@@ -50,17 +49,17 @@ def _checker(key, oracle, P, M, B, Cm, fd, qtf, trains, n_iter):
     return _CHECKER[key]
 
 
-def _solve_and_check(monkeypatch, oracle, unblocked, name, arg=None, diag=False):
+def _solve_and_check(monkeypatch, oracle, name, arg=None, diag=False):
     from raft_b200 import solver
     r = gs.row(name, arg)
     P, M, B, Cm, fd, qtf, n_iter = r["P"], r["M"], r["B"], r["Cm"], r["fd"], r["qtf"], r["n_iter"]
     table, owner, first, trains = r["ct"]
-    _env(monkeypatch, unblocked, diag)
+    _env(monkeypatch, diag)
     bem = fd.get("X_BEM") is not None
     out = solver.general_solve_dynamics(P, M, B, Cm, solver.CaseTable(table), n_iter=n_iter, fd=fd, F_BEM=True, qtf=qtf, F_2nd=qtf is not None)
     Xi, st, Fb = out[:3]
     rec = solver.last_dispatch()
-    assert rec["family"] == "general" and rec["kernel"] == ("gen-unblocked" if unblocked else "gen-blocked"), rec
+    assert rec["family"] == "general" and rec["kernel"] == "gen-blocked", rec
     assert rec["trains"] == (len(owner) > len(first)), rec
     ref = _checker((name, arg), oracle, P, M, B, Cm, fd, qtf, trains, n_iter)
     for ic, (Xo, so, Fo, F2o, F2mo) in enumerate(ref):
@@ -82,55 +81,49 @@ def _solve_and_check(monkeypatch, oracle, unblocked, name, arg=None, diag=False)
     print("%s %s: largest Xi error so far %.2e (array), %.2e (per row)" % (name, arg, _WORST["array"], _WORST["row"]))
 
 
-@pytest.mark.parametrize("unblocked", [False, True])
 @pytest.mark.parametrize("n", [7, 9, 17])
-def test_a_panel_crossing_support_with_trains(n, unblocked, monkeypatch, oracle):
+def test_a_panel_crossing_support_with_trains(n, monkeypatch, oracle):
     """fd support {0, 3, 7, 8, 15, 16} & [0, n) | {n - 1}, rotor and BEM tables, dense T0, 129 bins, trains."""
-    _solve_and_check(monkeypatch, oracle, unblocked, "a", n)
+    _solve_and_check(monkeypatch, oracle, "a", n)
 
 
-@pytest.mark.parametrize("unblocked", [False, True])
-def test_b_modal_support_rotor_only(unblocked, monkeypatch, oracle):
+def test_b_modal_support_rotor_only(monkeypatch, oracle):
     """n = 64, 257 bins, support {6, 31, 32, 63} (no platform DOF), rotor tables without BEM, trains."""
-    _solve_and_check(monkeypatch, oracle, unblocked, "b")
+    _solve_and_check(monkeypatch, oracle, "b")
 
 
-@pytest.mark.parametrize("unblocked", [False, True])
 @pytest.mark.parametrize("nw", [128, 129])
-def test_c_bem_only(nw, unblocked, monkeypatch, oracle):
+def test_c_bem_only(nw, monkeypatch, oracle):
     """BEM table with n_fd = 0 (the constant-matrix LU with the BEM projection), dense T0, 128 and 129 bins."""
-    _solve_and_check(monkeypatch, oracle, unblocked, "c", nw)
+    _solve_and_check(monkeypatch, oracle, "c", nw)
 
 
-@pytest.mark.parametrize("unblocked", [False, True])
 @pytest.mark.parametrize("which", ["full", "last"])
-def test_d_full_and_single_dof_support(which, unblocked, monkeypatch, oracle):
+def test_d_full_and_single_dof_support(which, monkeypatch, oracle):
     """n = 17, 33 bins: every DOF on the support (with BEM), or only the last one."""
-    _solve_and_check(monkeypatch, oracle, unblocked, "d", which)
+    _solve_and_check(monkeypatch, oracle, "d", which)
 
 
-@pytest.mark.parametrize("unblocked", [False, True])
 @pytest.mark.parametrize("which", ["stride", "full"])
-def test_e_256_dofs(which, unblocked, monkeypatch, oracle):
+def test_e_256_dofs(which, monkeypatch, oracle):
     """n = 256 (k_gen_train_solve's b[256] full), support {0..5, 127, 128, 255} across the 128-thread stride of gen_fd_map,
     or all 256 DOFs; trains; n_iter 4 as in test_dispatch_general."""
-    _solve_and_check(monkeypatch, oracle, unblocked, "e", which)
+    _solve_and_check(monkeypatch, oracle, "e", which)
 
 
-QTF_ROWS = [(6, 33, False, False), (6, 33, True, True), (9, 129, False, True), (9, 129, True, False), (17, 129, False, False),
-            (17, 129, True, True), (64, 257, False, False), (64, 257, False, True), (64, 257, True, False)]
+QTF_ROWS = [(6, 33, False), (9, 129, True), (17, 129, False), (64, 257, False), (64, 257, True)]
 
 
-@pytest.mark.parametrize("n,nw,unblocked,diag", QTF_ROWS)
-def test_f_second_order_loads(n, nw, unblocked, diag, monkeypatch, oracle):
-    """Second-order loads with a 3-heading QTF that covers bins nw/6 .. 2 nw/3; both force kernels, both LU kernels; trains."""
-    _solve_and_check(monkeypatch, oracle, unblocked, "f", (n, nw), diag=diag)
+@pytest.mark.parametrize("n,nw,diag", QTF_ROWS)
+def test_f_second_order_loads(n, nw, diag, monkeypatch, oracle):
+    """Second-order loads with a 3-heading QTF that covers bins nw/6 .. 2 nw/3; both force kernels; trains."""
+    _solve_and_check(monkeypatch, oracle, "f", (n, nw), diag=diag)
 
 
 def test_f_session_is_bit_identical_to_host_entry(monkeypatch):
     """With the reproducible force kernel (RAFTK_QTF_DIAG=1) at 129 bins: GeneralSession gives the host entry's bits."""
     from raft_b200 import solver
-    _env(monkeypatch, False, True)
+    _env(monkeypatch, True)
     r = gs.row("f", (17, 129))
     P, M, B, Cm, fd, qtf = r["P"], r["M"], r["B"], r["Cm"], r["fd"], r["qtf"]
     table = solver.CaseTable(r["ct"][0])
@@ -142,12 +135,11 @@ def test_f_session_is_bit_identical_to_host_entry(monkeypatch):
     assert np.array_equal(S.F_2nd.cpu().numpy(), F2h) and np.array_equal(S.F_2nd_mean.cpu().numpy(), F2mh)
 
 
-@pytest.mark.parametrize("unblocked", [False, True])
 @pytest.mark.parametrize("heads", [(40.0,), (20.0, 95.0, 200.0, 290.0)])
-def test_g_bem_headings(heads, unblocked, monkeypatch, oracle):
+def test_g_bem_headings(heads, monkeypatch, oracle):
     """One BEM heading, or four; case headings 0, 20, 300, 355 (between the last table heading and the first) and -45 deg;
     heading_adjust 12.5 deg, x_ref 3 m, y_ref -2 m."""
-    _solve_and_check(monkeypatch, oracle, unblocked, "g", heads)
+    _solve_and_check(monkeypatch, oracle, "g", heads)
 
 
 # ---- statistics kernels at the bin-count edges, against long-double references ------------------------------------------

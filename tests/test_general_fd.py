@@ -28,19 +28,14 @@ def _cases(z):
     return cases, table, owner, first
 
 
-@pytest.mark.parametrize("unblocked", [False, True])
-def test_fd_vs_reference_run_and_oracle(unblocked, monkeypatch, oracle):
+def test_fd_vs_reference_run_and_oracle(oracle):
     from raft_b200 import solver
-    if unblocked:
-        monkeypatch.setenv("RAFTK_GEN_UNBLOCKED", "1")
-    else:
-        monkeypatch.delenv("RAFTK_GEN_UNBLOCKED", raising=False)
     P, M, B, Cm, fd, z = load_flexfd()
     _, table, owner, first = _cases(z)
     Xi, st, Fb = solver.general_solve_dynamics(P, M, B, Cm, solver.CaseTable(table), n_iter=int(z["n_iter"]), xi_start=float(z["xi_start"]),
                                                fd=fd, F_BEM=True)
     rec = solver.last_dispatch()
-    assert rec["family"] == "general" and rec["kernel"] == ("gen-unblocked" if unblocked else "gen-blocked") and rec["trains"]
+    assert rec["family"] == "general" and rec["kernel"] == "gen-blocked" and rec["trains"]
     for ic in range(int(z["n_cases"])):
         idx = np.nonzero(owner == ic)[0]
         assert st[first[ic], 0] == int(z["ref_run_case%d_passes" % ic]) and st[first[ic], 2] == 0
@@ -112,15 +107,10 @@ def _rigid_as_general():
     return P, G, M, B, C, fd, z
 
 
-@pytest.mark.parametrize("unblocked", [False, True])
-def test_n6_reproduces_rigid_solver_on_bem_design(unblocked, monkeypatch):
+def test_n6_reproduces_rigid_solver_on_bem_design():
     """The new impedance and BEM code against the validated rigid path: same design, headings 0, 30, 175, 180, 355 (between
     the last BEM heading, 350, and the first) and -60 deg."""
     from raft_b200 import solver
-    if unblocked:
-        monkeypatch.setenv("RAFTK_GEN_UNBLOCKED", "1")
-    else:
-        monkeypatch.delenv("RAFTK_GEN_UNBLOCKED", raising=False)
     P, G, M, B, C, fd, z = _rigid_as_general()
     beta = np.array([0.0, 30.0, 175.0, 180.0, 355.0, -60.0])
     n = len(beta)
@@ -128,7 +118,7 @@ def test_n6_reproduces_rigid_solver_on_bem_design(unblocked, monkeypatch):
     ni = int(z["n_iter"])
     rig = solver.solve_dynamics(solver.DesignBatch(P), solver.CaseTable(cs), n_iter=ni, want=("Xi", "status", "F_BEM"))
     Xg, sg, Fg = solver.general_solve_dynamics(G, M, B, C, solver.CaseTable(cs), n_iter=ni, fd=fd, F_BEM=True)
-    assert solver.last_dispatch()["kernel"] == ("gen-unblocked" if unblocked else "gen-blocked")
+    assert solver.last_dispatch()["kernel"] == "gen-blocked"
     assert np.array_equal(sg[:, 0], rig["status"][0, :, 0])
     for c in range(n):
         assert relerr(Xg[c], rig["Xi"][0, c]) < RTOL, (beta[c], relerr(Xg[c], rig["Xi"][0, c]))

@@ -360,8 +360,7 @@ def test_checker_with_each_point_folded_vs_reference(name, oracle):
 
 # ---- on the GPU -----------------------------------------------------------------------------------------------------
 def _env(monkeypatch, **env):
-    for k in ("RAFTK_GEN_UNBLOCKED", "RAFTK_QTF_DIAG"):
-        monkeypatch.delenv(k, raising=False)
+    monkeypatch.delenv("RAFTK_QTF_DIAG", raising=False)
     for k, v in env.items():
         monkeypatch.setenv(k, v)
 
@@ -432,10 +431,10 @@ def _same(got, ref, rows):
 
 
 @gpu
-@pytest.mark.parametrize("kernel", ["gen-blocked", "gen-unblocked"])
+@pytest.mark.parametrize("kernel", ["gen-blocked"])
 def test_equals_one_call_per_point(kernel, monkeypatch):
     from raft_b200 import solver
-    _env(monkeypatch, **({"RAFTK_GEN_UNBLOCKED": "1"} if kernel == "gen-unblocked" else {}))
+    _env(monkeypatch)
     P, M, B, Cm, fd, ops, z = load_flexops("bem")
     table, owner, first = _train_table(z)
     assert "primary" in table                                                  # wave trains

@@ -33,25 +33,23 @@ def _cases(z):
     return cases, table, owner, first
 
 
-def _env(monkeypatch, unblocked, diag):
-    for name, on in (("RAFTK_GEN_UNBLOCKED", unblocked), ("RAFTK_QTF_DIAG", diag)):
-        if on:
-            monkeypatch.setenv(name, "1")
-        else:
-            monkeypatch.delenv(name, raising=False)
+def _env(monkeypatch, diag):
+    if diag:
+        monkeypatch.setenv("RAFTK_QTF_DIAG", "1")
+    else:
+        monkeypatch.delenv("RAFTK_QTF_DIAG", raising=False)
 
 
 @pytest.mark.parametrize("diag", [False, True])
-@pytest.mark.parametrize("unblocked", [False, True])
-def test_qtf_vs_reference_run_and_oracle(unblocked, diag, monkeypatch, oracle, tmp_path):
+def test_qtf_vs_reference_run_and_oracle(diag, monkeypatch, oracle, tmp_path):
     from raft_b200 import solver
-    _env(monkeypatch, unblocked, diag)
+    _env(monkeypatch, diag)
     P, M, B, Cm, fd, qtf, z = load_flexqtf(tmp_path)
     _, table, owner, first = _cases(z)
     Xi, st, F2, F2m = solver.general_solve_dynamics(P, M, B, Cm, solver.CaseTable(table), n_iter=int(z["n_iter"]), xi_start=float(z["xi_start"]),
                                                     fd=fd, qtf=qtf, F_2nd=True)
     rec = solver.last_dispatch()
-    assert rec["family"] == "general" and rec["kernel"] == ("gen-unblocked" if unblocked else "gen-blocked") and rec["trains"]
+    assert rec["family"] == "general" and rec["kernel"] == "gen-blocked" and rec["trains"]
     worst = [0.0, 0.0]
     for ic in range(int(z["n_cases"])):
         idx = np.nonzero(owner == ic)[0]
@@ -81,7 +79,7 @@ def test_four_heading_table_vs_checker(diag, monkeypatch, oracle, tmp_path):
     """Headings inside the table's range (20, 100 deg), on its headings (0, 45 deg) and outside it (-120, 200, 355 deg: the
     nearest table, scipy interp1d's fill values); RAFTK_QTF_DIAG=1 runs k_qtf_force<true> (MIX)."""
     from raft_b200 import solver
-    _env(monkeypatch, False, diag)
+    _env(monkeypatch, diag)
     P, M, B, Cm, fd, qtf, z = load_flexqtf(tmp_path)
     q4 = _four_headings(qtf)
     beta = np.array([20.0, 100.0, 0.0, 45.0, -120.0, 200.0, 355.0])
@@ -134,7 +132,7 @@ def test_host_session_and_analyze_cases_agree(monkeypatch, tmp_path):
     device) and general_analyze_cases (per case Fhydro_2nd [nTrains,nDOF,nw], Fhydro_2nd_mean [nTrains,nDOF], zero from row
     6) give the same bits."""
     from raft_b200 import solver
-    _env(monkeypatch, False, True)
+    _env(monkeypatch, True)
     P, M, B, Cm, fd, qtf, z = load_flexqtf(tmp_path)
     cases, table, owner, first = _cases(z)
     kw = dict(n_iter=int(z["n_iter"]), xi_start=float(z["xi_start"]))

@@ -1,6 +1,6 @@
-"""The generalised-DOF solves (raftk_general.cuh: k_gen_solve, k_gen_solve_blocked and k_gen_train_solve, each LU kernel with
-its FD and OP instantiations) against a high-precision reference of the same system, on inputs that reach every pivot
-pattern of both kernels' thread layouts, exact ties, ill-conditioned and graded bins, wave trains, a design axis, an exactly
+"""The generalised-DOF solves (raftk_general.cuh: k_gen_solve_blocked with its FD and OP instantiations, and
+k_gen_train_solve) against a high-precision reference of the same system, on inputs that reach every pivot pattern of the
+LU's thread layout, exact ties, ill-conditioned and graded bins, wave trains, a design axis, an exactly
 singular bin and the ends of the exponent range, at n = 9, 40, 150 and 256.
 
 The reference is the one of test_farm_edges and does not share the kernels' algorithm: the residual of the kernel's x is
@@ -25,7 +25,7 @@ returns is the kernels' right-hand side.  Drag-free, every pass solves the same 
 nw = 24 bins (16 at n = 256).  A physical case: general_synth's design with rotor and BEM tables on a support that crosses
 the panels, drag-free, B_w zeroed within two bins of a resonance; its Z restated with an exact fma.
 
-On the GPU, for each n and each LU kernel (asserted through solver.last_dispatch()):
+On the GPU, for each n (the LU kernel asserted through solver.last_dispatch()):
   * a train table (case 0 with two trains of different headings, case 1 with one): every primary and every secondary train
     (k_gen_train_solve: the primary's L, U and pivot rows with the secondary's own F_BEM) within the bounds;
   * the planted tables carried by op_A_w / op_B_w with A_w = B_w = 0 (the OP instantiations): Xi and status bit for bit;
@@ -37,7 +37,7 @@ On the GPU, for each n and each LU kernel (asserted through solver.last_dispatch
     (below 1.5e-154);
   * one case of a three-case call with a zero column at one bin: RAFTK_FLAG_SINGULAR in its status word 2, the other cases
     bit-identical to the call without it, and solver.raise_on_flags raises.
-Without a GPU the suite proves with the restated pivot rule that every pattern occurs at each n in both kernels' layouts,
+Without a GPU the suite proves with the restated pivot rule that every pattern occurs at each n in the kernel's layout,
 that a wrong pivot on a dominant bin leaves a backward error far above the bound, that the refinement agrees with a 50-digit
 mpmath LU solve, and that every scaled input stays in the normal range.
 
@@ -63,8 +63,8 @@ FWD_CEIL = 2e-14             # forward error on bins with kappa_inf(Z) <= 1e4
 RAFTK_FLAG_SINGULAR = 2
 S = 2.0 ** 27                # planted impedance scale, as test_rigid_solve_edges
 SIZES = (9, 40, 150, 256)
-KERNELS = [("gen-blocked", 128), ("gen-unblocked", 256)]       # (kernel, threads per CTA)
-KID = ["blocked", "unblocked"]
+KERNELS = [("gen-blocked", 128)]                               # (kernel, threads per CTA)
+KID = ["blocked"]
 FAMILIES = ("piv", "piv", "piv", "dom", "dom", "tie", "ill", "graded")
 LMAX = {"piv": 0.5, "dom": 1e-6}                               # largest other candidate / pivot, in |re| + |im|
 SCALES = (-560, -300, 300, 560)
@@ -277,7 +277,7 @@ _REF = {}
 
 
 def _errors_cached(z, f, x):
-    """test_farm_edges._errors, the refined solution and kappa of each (Z, F) computed once: both LU kernels solve the
+    """test_farm_edges._errors, the refined solution and kappa of each (Z, F) computed once: every call solves the
     same systems.  -> (eta, forward error, kappa_inf)."""
     key = hashlib.sha1(z.tobytes() + f.tobytes()).hexdigest()
     if key not in _REF:
@@ -484,13 +484,6 @@ def test_scaled_inputs_stay_in_range(n):
 
 
 # ---- on the GPU ---------------------------------------------------------------------------------------------------------
-def _env(monkeypatch, kernel):
-    if kernel == "gen-unblocked":
-        monkeypatch.setenv("RAFTK_GEN_UNBLOCKED", "1")
-    else:
-        monkeypatch.delenv("RAFTK_GEN_UNBLOCKED", raising=False)
-
-
 def _solve(D, ct, kernel, fd=None):
     from raft_b200 import solver
     out = solver.general_solve_dynamics(D["P"], D["M"], D["B"], D["Cm"], ct, n_iter=10, fd=D["fd"] if fd is None else fd, F_BEM=True)
@@ -517,7 +510,6 @@ def test_planted_trains_and_operating_points_vs_reference(n, kernel, T, monkeypa
     """The planted design with wave trains: every train within the bounds; the same tables as one operating point shared by
     every case, the design's own A_w / B_w zero: Xi and status bit for bit."""
     from raft_b200 import solver
-    _env(monkeypatch, kernel)
     D, _, _ = _design(n)
     nw = _nw(n)
     table = _trains()
@@ -540,7 +532,6 @@ def test_physical_case_vs_reference(n, kernel, T, monkeypatch):
     """general_synth's design with rotor and BEM tables, drag-free, B_w zero around a resonance: two cases within the bounds
     of its Z restated with an exact fma."""
     from raft_b200 import solver
-    _env(monkeypatch, kernel)
     D, _ = _physical(n)
     Xi, st, Fb = _solve(D, solver.CaseTable(_sea(2), zeta=_zeta(2, _nw(n))), kernel)
     assert not np.any(st[:, 2]), st
@@ -555,7 +546,6 @@ def test_physical_case_vs_reference(n, kernel, T, monkeypatch):
 def test_design_axis_vs_reference(n, kernel, T, monkeypatch):
     """general_solve_dynamics_batch on two designs with different planted tables: each design against its own reference."""
     from raft_b200 import solver
-    _env(monkeypatch, kernel)
     designs = [_design(n, seed=s)[0] for s in (1, 2)]
     nw = _nw(n)
     Xi, st, Fb = solver.general_solve_dynamics_batch(designs, solver.CaseTable(_sea(2), zeta=_zeta(2, nw)), n_iter=10, F_BEM=True)
@@ -577,7 +567,6 @@ def test_power_of_two_scaling_is_exact(n, kernel, T, s, monkeypatch):
     """A_w and B_w times 2^s (and zeta times 2^s for s < 0), with trains: Xi times 2^-s (the unscaled Xi for s < 0) bit for
     bit, flags 0."""
     from raft_b200 import solver
-    _env(monkeypatch, kernel)
     D, _, _ = _design(n)
     nw = _nw(n)
     table = _trains()
@@ -602,7 +591,6 @@ def test_a_singular_bin_is_flagged_singular(n, kernel, T, monkeypatch):
     carries RAFTK_FLAG_SINGULAR in status word 2, cases 0 and 2 keep the bits of the call where every case runs point 0,
     and solver.raise_on_flags raises."""
     from raft_b200 import solver
-    _env(monkeypatch, kernel)
     D, _, _ = _design(n)
     nw = _nw(n)
     fd = D["fd"]
