@@ -160,11 +160,15 @@ typedef struct raftk_cases {
     const double *op_B_w;    /* sum_r B_aero + sum_r B_gyro   -- added to B0 + B_w                                         */
 } raftk_cases;
 
-/* Fixed-point loop controls (raft_model.py:966 tol, :977 nIter, :978 XiStart, :1133 relaxation) */
+/* Fixed-point loop controls (raft_model.py:966 tol, :977 nIter, :978 XiStart, :1133 relaxation).  The kernels test
+ * |Xi - XiLast| / (|Xi| + tol) < tol in forms that square or take sqrt(d.d); with tol >= RAFTK_TOL_MIN those squares
+ * stay in the normal range wherever they decide (|Xi| below ~1e150), so every kernel decides as the reference does.  tol = 0 (never
+ * converge, run n_iter + 1 passes) is accepted too; a tol in (0, RAFTK_TOL_MIN), negative or NaN is refused. */
+#define RAFTK_TOL_MIN 1e-70
 typedef struct raftk_solve_opts {
     int32_t n_iter;          /* settings.nIter; the loop runs at most n_iter+1 passes           */
     int32_t cluster_size;    /* CTAs per (design,case): 0 = auto, else 1,2,4,8                  */
-    double tol;              /* 0.01                                                            */
+    double tol;              /* 0.01; 0 or >= RAFTK_TOL_MIN, else RAFTK_EINVAL                  */
     double xi_start;         /* settings.XiStart                                                */
     int32_t flags;           /* RAFTK_SOLVE_* bits, 0 = none                                    */
     int32_t _pad0;

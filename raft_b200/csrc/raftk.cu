@@ -239,6 +239,20 @@ extern "C" size_t raftk_workspace_bytes(const raftk_designs *d, int32_t n_cases)
     return full <= cap ? full : std::max(cap, one);
 }
 
+// The solve options every fixed-point loop takes.  tol is 0 or at least RAFTK_TOL_MIN (include/raftk.h): below that the
+// kernels' forms of the convergence test |d| / (|x| + tol) < tol (squared in the fused solvers, sqrt(d.d) in v1 and the
+// generalised-DOF solve) underflow and no longer decide as the reference does.
+static int validate_opts(const raftk_solve_opts *o)
+{
+    if (!o) return set_err(RAFTK_EINVAL, "null solve options");
+    if (!(o->tol == 0.0 || o->tol >= RAFTK_TOL_MIN)) {
+        char got[32];
+        snprintf(got, sizeof got, "%g", o->tol);
+        return set_err(RAFTK_EINVAL, "solve options: tol must be 0 or at least 1e-70 (RAFTK_TOL_MIN), got %s", got);
+    }
+    return 0;
+}
+
 static int validate(const raftk_designs *d, const raftk_cases *c)
 {
     if (!d || !c) return set_err(RAFTK_EINVAL, "null designs/cases");
@@ -766,6 +780,7 @@ static int solve(const raftk_designs *d, const raftk_cases *c, const raftk_solve
                  void *workspace, size_t wbytes, cudaStream_t st, const raftk_peers *peers = nullptr)
 {
     if (int rc = validate(d, c)) return rc;
+    if (int rc = validate_opts(o)) return rc;
     const SolvePlan pl = plan_solve(d, c->n_cases, o->cluster_size, workspace ? wbytes : 0);
     return launch_solve(d, c, o, out, pl, workspace, wbytes, st, peers);
 }
@@ -1376,6 +1391,7 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
     disp_reset();
     int rc = validate(d, c);
     if (rc) return rc;
+    if (mode == 0 && (rc = validate_opts(o))) return rc;
     if (!out) return set_err(RAFTK_EINVAL, "null outputs");
     raftk_cases cin = *c;
     if (mode != 0) cin.op = nullptr;                      // excitation and linearisation assemble no impedance
@@ -1897,6 +1913,7 @@ static int gen_check_counts(const GenCall &k, GenMode mode, const raftk_solve_op
     const bool one = mode == GEN_ONE_SHOT, batch = mode == GEN_BATCH;
     if (!g || !c || !o || !Xi || !status || (batch && (!k.b || !k.b->node_offset)))
         return set_err(RAFTK_EINVAL, batch ? "general batch: null argument" : "general solve: null argument");
+    if (int rc = validate_opts(o)) return rc;
     if (batch && (k.nD <= 0 || k.b->max_nodes < 0)) return set_err(RAFTK_EINVAL, "general batch: n_designs > 0 and max_nodes >= 0");
     if (g->n_dof <= 0 || g->n_dof > 256 || g->nw <= 0 || g->n_nodes < 0 || c->n_cases <= 0 || (one && c->n_cases > 65535))
         return set_err(RAFTK_EINVAL, one ? "general solve: 0 < n_dof <= 256, nw > 0, 0 < n_cases <= 65535"
