@@ -144,6 +144,7 @@ extern "C" int raftk_last_dispatch(raftk_dispatch *out)
 }
 
 #include "raftk_common.cuh"
+#include "raftk_rigid.cuh"
 #include "raftk_tables.cuh"
 #include "raftk_fused.cuh"
 #include "raftk_fused2.cuh"

@@ -74,6 +74,32 @@ __device__ __forceinline__ void op_impedance(double (&ar)[6][6], double (&ai)[6]
         }
 }
 
+// The fused solvers' impedance at bin i without operating points: with the design's frequency-dependent added mass and
+// damping tables Aw, Bw (BEM, aero) when Aw is non-NULL, else from the constant matrices alone.
+__device__ __forceinline__ void impedance(double (&ar)[6][6], double (&ai)[6][6], const double *Ms, const double *Bs, const double *Cm,
+                                          const double *Aw, const double *Bw, int i, int nw, double w, double w2)
+{
+    if (Aw) {
+#pragma unroll
+        for (int a = 0; a < 6; a++)
+#pragma unroll
+            for (int b = 0; b < 6; b++) {
+                const double M = Ms[6 * a + b] + Aw[(size_t)(6 * a + b) * nw + i];
+                const double B = Bs[6 * a + b] + Bw[(size_t)(6 * a + b) * nw + i];
+                ar[a][b] = fma(-w2, M, Cm[6 * a + b]);
+                ai[a][b] = w * B;
+            }
+    } else {
+#pragma unroll
+        for (int a = 0; a < 6; a++)
+#pragma unroll
+            for (int b = 0; b < 6; b++) {
+                ar[a][b] = fma(-w2, Ms[6 * a + b], Cm[6 * a + b]);
+                ai[a][b] = w * Bs[6 * a + b];
+            }
+    }
+}
+
 struct Work {          // workspace views for one chunk of designs [d0, d0+nDc)
     int d0, nDc;
     double2 *depth_tab;   // [nDc][max_nodes][nw]           (C, S)

@@ -39,9 +39,6 @@ struct FusedParams {
     int *peer_status[RAFTK_MAX_PEERS];    // [p]: likewise for status, or NULL
 };
 
-#define IMEM_STRIDE 6      // ints per member: node start, node end, circular, (spare), z-class, (spare)
-#define NCOEF 5            // per-node linearised coefficients: bq, b1, ls*b1, b2, ls*b2
-
 struct FSmem {
     double *mem, *node, *coef, *msum, *mat, *warp_part, *sums, *tot, *xi, *f0, *ckpt, *wkey, *hkey, *zkey, *scr, *trans;
     double2 *ebase, *abase, *wtab, *htab;
@@ -188,14 +185,7 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
         const double *fr = D.mem_frame + 9 * (m0 + m);
         const double *arm = D.mem_arm + 3 * (m0 + m);
         double *o = S.mem + m * MEM_STRIDE;
-        for (int t = 0; t < 9; t++) o[t] = fr[t];
-        for (int v = 0; v < 3; v++) {
-            const double d0_ = fr[3 * v], d1_ = fr[3 * v + 1], d2_ = fr[3 * v + 2];
-            o[9 + 3 * v + 0] = arm[1] * d2_ - arm[2] * d1_;
-            o[9 + 3 * v + 1] = arm[2] * d0_ - arm[0] * d2_;
-            o[9 + 3 * v + 2] = arm[0] * d1_ - arm[1] * d0_;
-            o[18 + v] = d0_ * cb + d1_ * sb;
-        }
+        member_row<true>(o, fr, arm, cb, sb);
         const int js = D.mem_node_start[m0 + m] - nbase;
         S.imem[IMEM_STRIDE * m + 0] = js;
         S.imem[IMEM_STRIDE * m + 1] = D.mem_node_start[m0 + m + 1] - nbase;
@@ -310,31 +300,9 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
                     L1r += ls * f1r; L1i += ls * f1i; L2r += ls * f2r; L2i += ls * f2i;
                 }
             }
-#pragma unroll
-            for (int a = 0; a < 3; a++) {
-                Fr[a] += o[a] * Aqr + o[3 + a] * A1r + o[6 + a] * A2r;
-                Fi[a] += o[a] * Aqi + o[3 + a] * A1i + o[6 + a] * A2i;
-                Fr[3 + a] += o[9 + a] * Aqr + o[12 + a] * A1r + o[15 + a] * A2r + o[6 + a] * L1r - o[3 + a] * L2r;
-                Fi[3 + a] += o[9 + a] * Aqi + o[12 + a] * A1i + o[15 + a] * A2i + o[6 + a] * L1i - o[3 + a] * L2i;
-            }
+            member_force6(o, Aqr, Aqi, A1r, A1i, A2r, A2i, L1r, L1i, L2r, L2i, Fr, Fi);
         }
-        if (P.Finer_out)
-            for (int a = 0; a < 6; a++) P.Finer_out[ogl + (size_t)a * nw + i] = make_double2(Fr[a], Fi[a]);
-        if (D.n_bem_head > 0) {
-            double Br[6], Bi[6];
-            bem_excitation(D, d, i, k, beta, sb, cb, zeta, Br, Bi);
-#pragma unroll
-            for (int a = 0; a < 6; a++) {
-                if (P.Fbem_out) P.Fbem_out[ogl + (size_t)a * nw + i] = make_double2(Br[a], Bi[a]);
-                Fr[a] += Br[a]; Fi[a] += Bi[a];
-            }
-        } else if (P.Fbem_out) {
-            for (int a = 0; a < 6; a++) P.Fbem_out[ogl + (size_t)a * nw + i] = make_double2(0.0, 0.0);
-        }
-        if (Cs.F_2nd) {                                  // difference-frequency force amplitudes (raft_model.py:1048, :1212)
-#pragma unroll
-            for (int a = 0; a < 6; a++) Fr[a] += Cs.F_2nd[ogl + (size_t)a * nw + i];
-        }
+        excitation_sum(D, Cs, P, d, ogl, nw, i, k, beta, sb, cb, [&] { return zeta; }, Fr, Fi);
 #pragma unroll
         for (int a = 0; a < 6; a++) {
             if (P.F0g) P.F0g[ogl + (size_t)a * nw + i] = make_double2(Fr[a], Fi[a]);
@@ -343,12 +311,7 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
             else { S.xi[(2 * a) * nwl + t] = P.xi_start; S.xi[(2 * a + 1) * nwl + t] = 0.0; }
         }
     }
-    if (plan_overflow) {          // no pass will run: never hand back whatever the output buffers held before
-        for (int t = tid; t < nloc; t += T)
-            for (int a = 0; a < 6; a++) P.Xi_out[ogl + (size_t)a * nw + f_begin + t] = make_double2(0.0, 0.0);
-        if (P.Xilast_out)
-            for (int t = tid; t < 6 * nloc; t += T) P.Xilast_out[ogl + (size_t)(t / nloc) * nw + f_begin + t % nloc] = make_double2(0.0, 0.0);
-    }
+    if (plan_overflow) zero_unit_outputs<T>(P.Xi_out, P.Xilast_out, ogl, nw, f_begin, nloc);
     __syncthreads();
 
     const double *Aw = D.A_w ? D.A_w + (size_t)d * 36 * nw : nullptr;
@@ -387,22 +350,8 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
                         do { mcur++; } while (jfirst >= S.imem[IMEM_STRIDE * mcur + 1]);
                         const int mstart = S.imem[IMEM_STRIDE * mcur], jlast = S.imem[IMEM_STRIDE * mcur + 1] - jc0;
                         const double *o = S.mem + mcur * MEM_STRIDE;
-                        double sr, si;
-                        sr = o[0] * xr[0] + o[1] * xr[1] + o[2] * xr[2] + o[9] * xr[3] + o[10] * xr[4] + o[11] * xr[5];
-                        si = o[0] * xi[0] + o[1] * xi[1] + o[2] * xi[2] + o[9] * xi[3] + o[10] * xi[4] + o[11] * xi[5];
-                        const double mqr = w * si, mqi = -w * sr;
-                        sr = o[3] * xr[0] + o[4] * xr[1] + o[5] * xr[2] + o[12] * xr[3] + o[13] * xr[4] + o[14] * xr[5];
-                        si = o[3] * xi[0] + o[4] * xi[1] + o[5] * xi[2] + o[12] * xi[3] + o[13] * xi[4] + o[14] * xi[5];
-                        const double m1r = w * si, m1i = -w * sr;
-                        sr = o[6] * xr[0] + o[7] * xr[1] + o[8] * xr[2] + o[15] * xr[3] + o[16] * xr[4] + o[17] * xr[5];
-                        si = o[6] * xi[0] + o[7] * xi[1] + o[8] * xi[2] + o[15] * xi[3] + o[16] * xi[4] + o[17] * xi[5];
-                        const double m2r = w * si, m2i = -w * sr;
-                        sr = o[3] * xr[3] + o[4] * xr[4] + o[5] * xr[5];
-                        si = o[3] * xi[3] + o[4] * xi[4] + o[5] * xi[5];
-                        const double t1r = w * si, t1i = -w * sr;
-                        sr = o[6] * xr[3] + o[7] * xr[4] + o[8] * xr[5];
-                        si = o[6] * xi[3] + o[7] * xi[4] + o[8] * xi[5];
-                        const double t2r = w * si, t2i = -w * sr;
+                        double mqr, mqi, m1r, m1i, m2r, m2i, t1r, t1i, t2r, t2i;
+                        member_velocity(o, xr, xi, w, mqr, mqi, m1r, m1i, m2r, m2i, t1r, t1i, t2r, t2i);
                         const double hq = o[18], h1 = o[19], h2 = o[20], dzq = o[2], dz1 = o[5], dz2 = o[8];
                         if (jfirst == mstart) {
                             const double2 e0 = S.ebase[mcur * nwl + t], a0 = S.abase[S.imem[IMEM_STRIDE * mcur + 4] * nwl + t];
@@ -467,27 +416,7 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
             }
         }
         __syncthreads();
-        for (int t = tid; t < nchunk * 32; t += T) {
-            const int ch = t >> 5, l = t & 31;
-            double s = 0.0;
-            for (int wv = 0; wv < nwarps; wv++) s += S.warp_part[(ch * nwarps + wv) * 32 + l];
-            S.sums[par * sums_stride + t] = s;
-        }
-        if (CS > 1) {
-            cluster.sync();
-            for (int t = tid; t < nchunk * 32; t += T) {
-                double s = 0.0;
-                for (int r = 0; r < CS; r++) {
-                    const double *rem = cluster.map_shared_rank(S.sums, r);
-                    s += rem[par * sums_stride + t];
-                }
-                S.tot[t] = s;
-            }
-        } else {
-            __syncthreads();
-            for (int t = tid; t < nchunk * 32; t += T) S.tot[t] = S.sums[par * sums_stride + t];
-        }
-        __syncthreads();
+        rms_exchange<T>(cluster, CS, nchunk, par, sums_stride, S.warp_part, S.sums, S.tot);
 
         // ================= linearised coefficients per node, member sums, B_drag ===================
         for (int j = tid; j < Ns; j += T) {
@@ -495,40 +424,18 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
             const double sq = S.tot[ch * 32 + 3 * jj], s1 = S.tot[ch * 32 + 3 * jj + 1], s2 = S.tot[ch * 32 + 3 * jj + 2];
             int m = 0;
             while (j >= S.imem[IMEM_STRIDE * m + 1]) m++;
-            const bool circ = S.imem[IMEM_STRIDE * m + 2] != 0;
-            const double vq = sqrt(0.5 * sq);
-            const double v1 = circ ? sqrt(0.5 * (s1 + s2)) : sqrt(0.5 * s1);
-            const double v2 = circ ? v1 : sqrt(0.5 * s2);
+            double vq, v1, v2;
+            drag_rms(sq, s1, s2, S.imem[IMEM_STRIDE * m + 2] != 0, vq, v1, v2);
             const double ls = S.node[j], b1 = S.node[2 * NsP + j] * v1, b2 = S.node[3 * NsP + j] * v2;
             S.coef[0 * NsP + j] = S.node[1 * NsP + j] * vq;
             S.coef[1 * NsP + j] = b1; S.coef[2 * NsP + j] = ls * b1;
             S.coef[3 * NsP + j] = b2; S.coef[4 * NsP + j] = ls * b2;
         }
         __syncthreads();
-        for (int m = tid; m < Nm; m += T) {
-            double bq = 0, b1 = 0, b1l = 0, b1ll = 0, b2 = 0, b2l = 0, b2ll = 0;
-            for (int j = S.imem[IMEM_STRIDE * m]; j < S.imem[IMEM_STRIDE * m + 1]; j++) {
-                const double ls = S.node[j], q_ = S.coef[j], p1_ = S.coef[NsP + j], p2_ = S.coef[3 * NsP + j];
-                bq += q_; b1 += p1_; b1l += p1_ * ls; b1ll += p1_ * ls * ls; b2 += p2_; b2l += p2_ * ls; b2ll += p2_ * ls * ls;
-            }
-            double *o = S.msum + m * 8;
-            o[0] = bq; o[1] = b1; o[2] = b1l; o[3] = b1ll; o[4] = b2; o[5] = b2l; o[6] = b2ll;
-        }
+        drag_member_sums<T, IMEM_STRIDE>(Nm, S.imem, S.node, S.coef, 0, NsP, 3 * NsP, S.msum);
         __syncthreads();
         if (tid < 36) {
-            const int a = tid / 6, b = tid % 6;
-            double s = 0.0;
-            for (int m = 0; m < Nm; m++) {
-                const double *o = S.mem + m * MEM_STRIDE, *ms = S.msum + m * 8;
-                const double vqa = a < 3 ? o[a] : o[9 + a - 3], vqb = b < 3 ? o[b] : o[9 + b - 3];
-                const double v1a = a < 3 ? o[3 + a] : o[12 + a - 3], v1b = b < 3 ? o[3 + b] : o[12 + b - 3];
-                const double v2a = a < 3 ? o[6 + a] : o[15 + a - 3], v2b = b < 3 ? o[6 + b] : o[15 + b - 3];
-                const double u1a = a < 3 ? 0.0 : o[6 + a - 3], u1b = b < 3 ? 0.0 : o[6 + b - 3];
-                const double u2a = a < 3 ? 0.0 : -o[3 + a - 3], u2b = b < 3 ? 0.0 : -o[3 + b - 3];
-                s += ms[0] * vqa * vqb;
-                s += ms[1] * v1a * v1b + ms[2] * (v1a * u1b + u1a * v1b) + ms[3] * u1a * u1b;
-                s += ms[4] * v2a * v2b + ms[5] * (v2a * u2b + u2a * v2b) + ms[6] * u2a * u2b;
-            }
+            const double s = drag_bmat_entry(tid, Nm, S.mem, S.msum);
             S.mat[36 + tid] = D.B0[(size_t)d * 36 + tid] + s;
             if (P.Bdrag_out && rank == 0) P.Bdrag_out[((size_t)d * Cs.nC + c) * 36 + tid] = s;
         }
@@ -574,13 +481,7 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
                     proj(er, ei, Cc, Sc, h2, dz2, cr, ci);
                     A2r = fma(b2, cr, A2r); A2i = fma(b2, ci, A2i); L2r = fma(lb2, cr, L2r); L2i = fma(lb2, ci, L2i);
                 }
-#pragma unroll
-                for (int a = 0; a < 3; a++) {
-                    br[a] += o[a] * Aqr + o[3 + a] * A1r + o[6 + a] * A2r;
-                    bi[a] += o[a] * Aqi + o[3 + a] * A1i + o[6 + a] * A2i;
-                    br[3 + a] += o[9 + a] * Aqr + o[12 + a] * A1r + o[15 + a] * A2r + o[6 + a] * L1r - o[3 + a] * L2r;
-                    bi[3 + a] += o[9 + a] * Aqi + o[12 + a] * A1i + o[15 + a] * A2i + o[6 + a] * L1i - o[3 + a] * L2i;
-                }
+                member_force6(o, Aqr, Aqi, A1r, A1i, A2r, A2i, L1r, L1i, L2r, L2i, br, bi);
             }
             if (P.Fdrag_out) {
 #pragma unroll
@@ -599,24 +500,8 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
                 const double *Ao = op_table(Cs, Cs.op_A_w, d, c, nw), *Bo = op_table(Cs, Cs.op_B_w, d, c, nw);
                 if (Aw) op_impedance<true>(ar, ai, S.mat, S.mat + 36, S.mat + 72, Aw, Bw, Ao, Bo, i, nw, w, w2);
                 else op_impedance<false>(ar, ai, S.mat, S.mat + 36, S.mat + 72, nullptr, nullptr, Ao, Bo, i, nw, w, w2);
-            } else if (Aw) {               // frequency-dependent added mass / damping tables (BEM, aero)
-#pragma unroll
-                for (int a = 0; a < 6; a++)
-#pragma unroll
-                    for (int b = 0; b < 6; b++) {
-                        const double M = S.mat[6 * a + b] + Aw[(size_t)(6 * a + b) * nw + i];
-                        const double B = S.mat[36 + 6 * a + b] + Bw[(size_t)(6 * a + b) * nw + i];
-                        ar[a][b] = fma(-w2, M, S.mat[72 + 6 * a + b]);
-                        ai[a][b] = w * B;
-                    }
             } else {
-#pragma unroll
-                for (int a = 0; a < 6; a++)
-#pragma unroll
-                    for (int b = 0; b < 6; b++) {
-                        ar[a][b] = fma(-w2, S.mat[6 * a + b], S.mat[72 + 6 * a + b]);
-                        ai[a][b] = w * S.mat[36 + 6 * a + b];
-                    }
+                impedance(ar, ai, S.mat, S.mat + 36, S.mat + 72, Aw, Bw, i, nw, w, w2);
             }
             const bool ok = solve6(ar, ai, br, bi);
             if (!ok) nan_local |= RAFTK_FLAG_SINGULAR;
@@ -635,51 +520,13 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
             }
         }
         passes++;
-        int conv_all = __syncthreads_and(conv_local);
-        // __syncthreads_or returns a boolean, so reduce the two flag bits separately
-        int nan_all = (__syncthreads_or(nan_local & RAFTK_FLAG_NAN) ? RAFTK_FLAG_NAN : 0)
-                      | (__syncthreads_or(nan_local & RAFTK_FLAG_SINGULAR) ? RAFTK_FLAG_SINGULAR : 0);
-        if (CS > 1) {
-            if (tid == 0) { S.sums[par * sums_stride + nchunk * 32] = (double)conv_all; S.sums[par * sums_stride + nchunk * 32 + 1] = (double)nan_all; }
-            cluster.sync();
-            int ca = 1, na = 0;
-            for (int r = 0; r < CS; r++) {
-                const double *rem = cluster.map_shared_rank(S.sums, r);
-                ca &= (int)rem[par * sums_stride + nchunk * 32];
-                na |= (int)rem[par * sums_stride + nchunk * 32 + 1];
-            }
-            conv_all = ca; nan_all = na;
-        }
+        int conv_all, nan_all;
+        flags_exchange(cluster, CS, nchunk, par, sums_stride, conv_local, nan_local, S.sums, conv_all, nan_all);
         par ^= 1;
         flags |= nan_all;
         if (nan_all & RAFTK_FLAG_NAN) break;
         if (conv_all) { converged = 1; break; }
     }
-    if (P.status && rank == 0 && tid == 0) {
-        int *st = P.status + ((size_t)d * Cs.nC + c) * 4;
-        st[0] = secondary ? 0 : passes; st[1] = secondary ? 1 : converged; st[2] = flags; st[3] = secondary ? prim + 1 : 0;
-    }
-    if (P.n_peers > 1) {
-        // the unit is final: push this CTA's slice of Xi to every peer.  Each thread re-reads the values it stored itself
-        // in the last pass (L2 hits); the peer stores are fire-and-forget and overlap the units still iterating.
-        for (int t = tid; t < nloc; t += T) {
-            const int i = f_begin + t;
-#pragma unroll
-            for (int a = 0; a < 6; a++) {
-                const size_t o_ = ogl + (size_t)a * nw + i;
-                const double2 v = P.Xi_out[o_];
-                for (int p = 0; p < P.n_peers; p++)
-                    if (p != P.peer_rank) P.peer_Xi[p][o_] = v;
-            }
-        }
-        if (rank == 0 && tid == 0) {
-            const size_t so = ((size_t)d * Cs.nC + c) * 4;
-            for (int p = 0; p < P.n_peers; p++)
-                if (p != P.peer_rank && P.peer_status[p]) {
-                    int *st = P.peer_status[p] + so;
-                    st[0] = secondary ? 0 : passes; st[1] = secondary ? 1 : converged; st[2] = flags; st[3] = secondary ? prim + 1 : 0;
-                }
-        }
-    }
+    unit_epilogue<T, 4>(P, d, c, Cs.nC, rank, ogl, nw, f_begin, nloc, passes, converged, flags, secondary, prim);
     if (CS > 1) cluster.sync();
 }

@@ -77,16 +77,9 @@ __global__ void __launch_bounds__(128) k_fused_plan(DesignsDev D, double *plan, 
     __syncthreads();
     for (int m = tid; m < Nm; m += T) {
         const double *fr = D.mem_frame + 9 * (m0 + m);
-        const double *arm = D.mem_arm + 3 * (m0 + m);
         const double *rA = D.mem_rA + 3 * (m0 + m);
         double *o = mem + m * MEM_STRIDE;
-        for (int t = 0; t < 9; t++) o[t] = fr[t];
-        for (int v = 0; v < 3; v++) {
-            const double d0_ = fr[3 * v], d1_ = fr[3 * v + 1], d2_ = fr[3 * v + 2];
-            o[9 + 3 * v + 0] = arm[1] * d2_ - arm[2] * d1_;
-            o[9 + 3 * v + 1] = arm[2] * d0_ - arm[0] * d2_;
-            o[9 + 3 * v + 2] = arm[0] * d1_ - arm[1] * d0_;
-        }
+        member_row<false>(o, fr, D.mem_arm + 3 * (m0 + m));
         const int js = D.mem_node_start[m0 + m] - nbase, je = D.mem_node_start[m0 + m + 1] - nbase;
         imem[IMEM_STRIDE * m + 0] = js;
         imem[IMEM_STRIDE * m + 1] = je;
@@ -370,7 +363,7 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
     const int Ns = D.mem_node_start[m0 + Nm] - nbase;
     for (int m = tid; m < Nm; m += T) {                       // heading projections of the member frame: per case
         double *o = s_mem + m * MEM_STRIDE;
-        for (int v = 0; v < 3; v++) o[18 + v] = o[3 * v] * cb + o[3 * v + 1] * sb;
+        for (int v = 0; v < 3; v++) o[18 + v] = heading_proj(o[3 * v], o[3 * v + 1], cb, sb);
     }
     __syncthreads();
     const int nW = s_cnt[0], nH = s_cnt[1], nZ = s_cnt[3];
@@ -498,17 +491,8 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
                 F2_F0_NODE(erB, eiB, apB, amB, w1, kB, i1, thB, deepB, AqrB, AqiB, A1rB, A1iB, A2rB, A2iB, L1rB, L1iB, L2rB, L2iB)
 #undef F2_F0_NODE
             }
-#pragma unroll
-            for (int a = 0; a < 3; a++) {
-                FrA[a] += o[a] * AqrA + o[3 + a] * A1rA + o[6 + a] * A2rA;
-                FiA[a] += o[a] * AqiA + o[3 + a] * A1iA + o[6 + a] * A2iA;
-                FrA[3 + a] += o[9 + a] * AqrA + o[12 + a] * A1rA + o[15 + a] * A2rA + o[6 + a] * L1rA - o[3 + a] * L2rA;
-                FiA[3 + a] += o[9 + a] * AqiA + o[12 + a] * A1iA + o[15 + a] * A2iA + o[6 + a] * L1iA - o[3 + a] * L2iA;
-                FrB[a] += o[a] * AqrB + o[3 + a] * A1rB + o[6 + a] * A2rB;
-                FiB[a] += o[a] * AqiB + o[3 + a] * A1iB + o[6 + a] * A2iB;
-                FrB[3 + a] += o[9 + a] * AqrB + o[12 + a] * A1rB + o[15 + a] * A2rB + o[6 + a] * L1rB - o[3 + a] * L2rB;
-                FiB[3 + a] += o[9 + a] * AqiB + o[12 + a] * A1iB + o[15 + a] * A2iB + o[6 + a] * L1iB - o[3 + a] * L2iB;
-            }
+            member_force6(o, AqrA, AqiA, A1rA, A1iA, A2rA, A2iA, L1rA, L1iA, L2rA, L2iA, FrA, FiA);
+            member_force6(o, AqrB, AqiB, A1rB, A1iB, A2rB, A2iB, L1rB, L1iB, L2rB, L2iB, FrB, FiB);
         }
         // per bin: optional outputs, BEM excitation, second-order forces; the sum is parked in the workspace
 #pragma unroll 1
@@ -518,35 +502,12 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
             double Fr[6], Fi[6];
 #pragma unroll
             for (int a = 0; a < 6; a++) { Fr[a] = bsel == 0 ? FrA[a] : FrB[a]; Fi[a] = bsel == 0 ? FiA[a] : FiB[a]; }
-            if (P.Finer_out)
-                for (int a = 0; a < 6; a++) P.Finer_out[ogl + (size_t)a * nw + i] = make_double2(Fr[a], Fi[a]);
-            if (D.n_bem_head > 0) {
-                const double k = D.k[i], w = D.w[i];
-                const double zeta = zeta_f2(Cs, c, i, nw, w, D.dw);
-                double Br[6], Bi[6];
-                bem_excitation(D, d, i, k, beta, sb, cb, zeta, Br, Bi);
-#pragma unroll
-                for (int a = 0; a < 6; a++) {
-                    if (P.Fbem_out) P.Fbem_out[ogl + (size_t)a * nw + i] = make_double2(Br[a], Bi[a]);
-                    Fr[a] += Br[a]; Fi[a] += Bi[a];
-                }
-            } else if (P.Fbem_out) {
-                for (int a = 0; a < 6; a++) P.Fbem_out[ogl + (size_t)a * nw + i] = make_double2(0.0, 0.0);
-            }
-            if (Cs.F_2nd) {
-#pragma unroll
-                for (int a = 0; a < 6; a++) Fr[a] += Cs.F_2nd[ogl + (size_t)a * nw + i];
-            }
+            excitation_sum(D, Cs, P, d, ogl, nw, i, D.k[i], beta, sb, cb, [&] { return zeta_f2(Cs, c, i, nw, D.w[i], D.dw); }, Fr, Fi);
 #pragma unroll
             for (int a = 0; a < 6; a++) P.F0g[ogl + (size_t)a * nw + i] = make_double2(Fr[a], Fi[a]);
         }
     }
-    if (plan_overflow) {          // no pass will run: never hand back whatever the output buffers held before
-        for (int t = tid; t < nloc; t += T)
-            for (int a = 0; a < 6; a++) P.Xi_out[ogl + (size_t)a * nw + f_begin + t] = make_double2(0.0, 0.0);
-        if (P.Xilast_out)
-            for (int t = tid; t < 6 * nloc; t += T) P.Xilast_out[ogl + (size_t)(t / nloc) * nw + f_begin + t % nloc] = make_double2(0.0, 0.0);
-    }
+    if (plan_overflow) zero_unit_outputs<T>(P.Xi_out, P.Xilast_out, ogl, nw, f_begin, nloc);
     __syncthreads();
 
     const double *Aw = D.A_w ? D.A_w + (size_t)d * 36 * nw : nullptr;
@@ -589,34 +550,15 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
                     const int mcur = s_nodem[jfirst];
                     const int mstart = s_imem[IMEM_STRIDE * mcur], jlast = s_imem[IMEM_STRIDE * mcur + 1] - jc0;
                     const double *o = s_mem + mcur * MEM_STRIDE;
-#define F2_MEMBER_PROJ(TT, WW, OKK, MQR, MQI, M1R, M1I, M2R, M2I, U1R, U1I, U2R, U2I)                                          \
-    {                                                                                                                             \
-        double xr[6], xi[6];                                                                                                      \
-        _Pragma("unroll") for (int a = 0; a < 6; a++) {                                                                           \
-            xr[a] = OKK ? s_xi[(2 * a) * nwl + TT] : 0.0; xi[a] = OKK ? s_xi[(2 * a + 1) * nwl + TT] : 0.0;                      \
-        }                                                                                                                         \
-        double sr, si;                                                                                                            \
-        sr = o[0] * xr[0] + o[1] * xr[1] + o[2] * xr[2] + o[9] * xr[3] + o[10] * xr[4] + o[11] * xr[5];                           \
-        si = o[0] * xi[0] + o[1] * xi[1] + o[2] * xi[2] + o[9] * xi[3] + o[10] * xi[4] + o[11] * xi[5];                           \
-        MQR = WW * si; MQI = -WW * sr;                                                                                            \
-        sr = o[3] * xr[0] + o[4] * xr[1] + o[5] * xr[2] + o[12] * xr[3] + o[13] * xr[4] + o[14] * xr[5];                          \
-        si = o[3] * xi[0] + o[4] * xi[1] + o[5] * xi[2] + o[12] * xi[3] + o[13] * xi[4] + o[14] * xi[5];                          \
-        M1R = WW * si; M1I = -WW * sr;                                                                                            \
-        sr = o[6] * xr[0] + o[7] * xr[1] + o[8] * xr[2] + o[15] * xr[3] + o[16] * xr[4] + o[17] * xr[5];                          \
-        si = o[6] * xi[0] + o[7] * xi[1] + o[8] * xi[2] + o[15] * xi[3] + o[16] * xi[4] + o[17] * xi[5];                          \
-        M2R = WW * si; M2I = -WW * sr;                                                                                            \
-        sr = o[3] * xr[3] + o[4] * xr[4] + o[5] * xr[5];                                                                          \
-        si = o[3] * xi[3] + o[4] * xi[4] + o[5] * xi[5];                                                                          \
-        U1R = WW * si; U1I = -WW * sr;                                                                                            \
-        sr = o[6] * xr[3] + o[7] * xr[4] + o[8] * xr[5];                                                                          \
-        si = o[6] * xi[3] + o[7] * xi[4] + o[8] * xi[5];                                                                          \
-        U2R = WW * si; U2I = -WW * sr;                                                                                            \
-    }
                     if (jfirst == mstart) {
-                        F2_MEMBER_PROJ(t0, w0, ok0, mqrA, mqiA, m1rA, m1iA, m2rA, m2iA, u1rA, u1iA, u2rA, u2iA)
-                        F2_MEMBER_PROJ(t1, w1, ok1, mqrB, mqiB, m1rB, m1iB, m2rB, m2iB, u1rB, u1iB, u2rB, u2iB)
+                        double xr[6], xi[6];
+#pragma unroll
+                        for (int a = 0; a < 6; a++) { xr[a] = ok0 ? s_xi[(2 * a) * nwl + t0] : 0.0; xi[a] = ok0 ? s_xi[(2 * a + 1) * nwl + t0] : 0.0; }
+                        member_velocity(o, xr, xi, w0, mqrA, mqiA, m1rA, m1iA, m2rA, m2iA, u1rA, u1iA, u2rA, u2iA);
+#pragma unroll
+                        for (int a = 0; a < 6; a++) { xr[a] = ok1 ? s_xi[(2 * a) * nwl + t1] : 0.0; xi[a] = ok1 ? s_xi[(2 * a + 1) * nwl + t1] : 0.0; }
+                        member_velocity(o, xr, xi, w1, mqrB, mqiB, m1rB, m1iB, m2rB, m2iB, u1rB, u1iB, u2rB, u2iB);
                     }
-#undef F2_MEMBER_PROJ
                     const double hq = o[18], h1 = o[19], h2 = o[20], dzq = o[2], dz1 = o[5], dz2 = o[8];
                     if (jfirst == mstart) {
                         const int zc = s_imem[IMEM_STRIDE * mcur + 4];
@@ -755,40 +697,18 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
             // slot layout of the chunk (k_fused_plan): transverse-1 | transverse-2 | axial-when-both; axial alone sits in slot 0
             const double sA = s_tot[ch * 32 + jj], sB = s_tot[ch * 32 + 10 + jj], sC = s_tot[ch * 32 + 20 + jj];
             const double sq = (mk & 1u) ? ((mk & 2u) ? sC : sA) : 0.0, s1 = (mk & 2u) ? sA : 0.0, s2 = (mk & 2u) ? sB : 0.0;
-            const bool circ = s_imem[IMEM_STRIDE * s_nodem[j] + 2] != 0;
-            const double vq = sqrt(0.5 * sq);
-            const double v1 = circ ? sqrt(0.5 * (s1 + s2)) : sqrt(0.5 * s1);
-            const double v2 = circ ? v1 : sqrt(0.5 * s2);
+            double vq, v1, v2;
+            drag_rms(sq, s1, s2, s_imem[IMEM_STRIDE * s_nodem[j] + 2] != 0, vq, v1, v2);
             const double ls = n_ls[j], b1 = n_cd1[j] * v1, b2 = n_cd2[j] * v2;
             s_coef[0 * NsP + j] = n_cdq[j] * vq;
             s_coef[1 * NsP + j] = b1; s_coef[2 * NsP + j] = ls * b1;
             s_coef[3 * NsP + j] = b2; s_coef[4 * NsP + j] = ls * b2;
         }
         __syncthreads();
-        for (int m = tid; m < Nm; m += T) {
-            double bq = 0, b1 = 0, b1l = 0, b1ll = 0, b2 = 0, b2l = 0, b2ll = 0;
-            for (int j = s_imem[IMEM_STRIDE * m]; j < s_imem[IMEM_STRIDE * m + 1]; j++) {
-                const double ls = n_ls[j], q_ = s_coef[j], p1_ = s_coef[NsP + j], p2_ = s_coef[3 * NsP + j];
-                bq += q_; b1 += p1_; b1l += p1_ * ls; b1ll += p1_ * ls * ls; b2 += p2_; b2l += p2_ * ls; b2ll += p2_ * ls * ls;
-            }
-            double *o = s_msum + m * 8;
-            o[0] = bq; o[1] = b1; o[2] = b1l; o[3] = b1ll; o[4] = b2; o[5] = b2l; o[6] = b2ll;
-        }
+        drag_member_sums<T, IMEM_STRIDE>(Nm, s_imem, n_ls, s_coef, 0, NsP, 3 * NsP, s_msum);
         __syncthreads();
         if (tid < 36) {
-            const int a = tid / 6, b = tid % 6;
-            double s = 0.0;
-            for (int m = 0; m < Nm; m++) {
-                const double *o = s_mem + m * MEM_STRIDE, *ms = s_msum + m * 8;
-                const double vqa = a < 3 ? o[a] : o[9 + a - 3], vqb = b < 3 ? o[b] : o[9 + b - 3];
-                const double v1a = a < 3 ? o[3 + a] : o[12 + a - 3], v1b = b < 3 ? o[3 + b] : o[12 + b - 3];
-                const double v2a = a < 3 ? o[6 + a] : o[15 + a - 3], v2b = b < 3 ? o[6 + b] : o[15 + b - 3];
-                const double u1a = a < 3 ? 0.0 : o[6 + a - 3], u1b = b < 3 ? 0.0 : o[6 + b - 3];
-                const double u2a = a < 3 ? 0.0 : -o[3 + a - 3], u2b = b < 3 ? 0.0 : -o[3 + b - 3];
-                s += ms[0] * vqa * vqb;
-                s += ms[1] * v1a * v1b + ms[2] * (v1a * u1b + u1a * v1b) + ms[3] * u1a * u1b;
-                s += ms[4] * v2a * v2b + ms[5] * (v2a * u2b + u2a * v2b) + ms[6] * u2a * u2b;
-            }
+            const double s = drag_bmat_entry(tid, Nm, s_mem, s_msum);
             s_bmat[tid] = s_mat[36 + tid] + s;
             if (P.Bdrag_out && rank == 0) P.Bdrag_out[((size_t)d * Cs.nC + c) * 36 + tid] = s;
         }
@@ -848,17 +768,8 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
                         A2rB = fma(b2, crB, A2rB); A2iB = fma(b2, ciB, A2iB); L2rB = fma(lb2, crB, L2rB); L2iB = fma(lb2, ciB, L2iB);
                     }
                 }
-#pragma unroll
-                for (int a = 0; a < 3; a++) {
-                    brA[a] += o[a] * AqrA + o[3 + a] * A1rA + o[6 + a] * A2rA;
-                    biA[a] += o[a] * AqiA + o[3 + a] * A1iA + o[6 + a] * A2iA;
-                    brA[3 + a] += o[9 + a] * AqrA + o[12 + a] * A1rA + o[15 + a] * A2rA + o[6 + a] * L1rA - o[3 + a] * L2rA;
-                    biA[3 + a] += o[9 + a] * AqiA + o[12 + a] * A1iA + o[15 + a] * A2iA + o[6 + a] * L1iA - o[3 + a] * L2iA;
-                    brB[a] += o[a] * AqrB + o[3 + a] * A1rB + o[6 + a] * A2rB;
-                    biB[a] += o[a] * AqiB + o[3 + a] * A1iB + o[6 + a] * A2iB;
-                    brB[3 + a] += o[9 + a] * AqrB + o[12 + a] * A1rB + o[15 + a] * A2rB + o[6 + a] * L1rB - o[3 + a] * L2rB;
-                    biB[3 + a] += o[9 + a] * AqiB + o[12 + a] * A1iB + o[15 + a] * A2iB + o[6 + a] * L1iB - o[3 + a] * L2iB;
-                }
+                member_force6(o, AqrA, AqiA, A1rA, A1iA, A2rA, A2iA, L1rA, L1iA, L2rA, L2iA, brA, biA);
+                member_force6(o, AqrB, AqiB, A1rB, A1iB, A2rB, A2iB, L1rB, L1iB, L2rB, L2iB, brB, biB);
             }
         }
         // bin B's drag excitation waits in its own output slot (global, L2) while bin A is solved: the 6x6 system needs
@@ -896,24 +807,8 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
                 const double *Ao = op_table(Cs, Cs.op_A_w, d, c, nw), *Bo = op_table(Cs, Cs.op_B_w, d, c, nw);
                 if (Aw) op_impedance<true>(ar, ai, s_mat, s_bmat, s_mat + 72, Aw, Bw, Ao, Bo, i, nw, w, w2);
                 else op_impedance<false>(ar, ai, s_mat, s_bmat, s_mat + 72, nullptr, nullptr, Ao, Bo, i, nw, w, w2);
-            } else if (Aw) {
-#pragma unroll
-                for (int a = 0; a < 6; a++)
-#pragma unroll
-                    for (int b = 0; b < 6; b++) {
-                        const double M = s_mat[6 * a + b] + Aw[(size_t)(6 * a + b) * nw + i];
-                        const double B = s_bmat[6 * a + b] + Bw[(size_t)(6 * a + b) * nw + i];
-                        ar[a][b] = fma(-w2, M, s_mat[72 + 6 * a + b]);
-                        ai[a][b] = w * B;
-                    }
             } else {
-#pragma unroll
-                for (int a = 0; a < 6; a++)
-#pragma unroll
-                    for (int b = 0; b < 6; b++) {
-                        ar[a][b] = fma(-w2, s_mat[6 * a + b], s_mat[72 + 6 * a + b]);
-                        ai[a][b] = w * s_bmat[6 * a + b];
-                    }
+                impedance(ar, ai, s_mat, s_bmat, s_mat + 72, Aw, Bw, i, nw, w, w2);
             }
             const bool ok = solve6(ar, ai, br, bi);
             if (!ok) nan_local |= RAFTK_FLAG_SINGULAR;
@@ -980,32 +875,7 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
         if (nan_all & (GRID ? RAFTK_FLAG_NAN | RAFTK_FLAG_XCHG : RAFTK_FLAG_NAN)) break;
         if (conv_all) { converged = 1; break; }
     }
-    if (P.status && rank == 0 && tid == 0) {
-        int *st = P.status + ((size_t)d * Cs.nC + c) * 4;
-        st[0] = secondary ? 0 : passes; st[1] = secondary ? 1 : converged; st[2] = flags; st[3] = secondary ? prim + 1 : 0;
-    }
-    if (P.n_peers > 1) {
-        for (int t = tid; t < nloc; t += T) {
-            const int i = f_begin + t;
-#pragma unroll
-            for (int a = 0; a < 6; a++) {
-                const size_t o_ = ogl + (size_t)a * nw + i;
-                const double2 v = P.Xi_out[o_];
-#pragma unroll 1
-                for (int pr = 0; pr < P.n_peers; pr++)
-                    if (pr != P.peer_rank) P.peer_Xi[pr][o_] = v;
-            }
-        }
-        if (rank == 0 && tid == 0) {
-            const size_t so = ((size_t)d * Cs.nC + c) * 4;
-#pragma unroll 1
-            for (int pr = 0; pr < P.n_peers; pr++)
-                if (pr != P.peer_rank && P.peer_status[pr]) {
-                    int *st = P.peer_status[pr] + so;
-                    st[0] = secondary ? 0 : passes; st[1] = secondary ? 1 : converged; st[2] = flags; st[3] = secondary ? prim + 1 : 0;
-                }
-        }
-    }
+    unit_epilogue<T, 1>(P, d, c, Cs.nC, rank, ogl, nw, f_begin, nloc, passes, converged, flags, secondary, prim);
     if (!GRID && CS > 1) cluster.sync();          // no CTA may leave while a peer still reads its shared memory
     F2_TRACE(2);
 }

@@ -288,14 +288,7 @@ k_drag_solve(DesignsDev D, CasesDev Cs, Work W, SolveParams P)
         const double *fr = D.mem_frame + 9 * (m0 + m);
         const double *arm = D.mem_arm + 3 * (m0 + m);
         double *o = S.mem + m * MEM_STRIDE;
-        for (int t = 0; t < 9; t++) o[t] = fr[t];
-        for (int v = 0; v < 3; v++) {                    // a x d for d = q, p1, p2
-            const double d0_ = fr[3 * v], d1_ = fr[3 * v + 1], d2_ = fr[3 * v + 2];
-            o[9 + 3 * v + 0] = arm[1] * d2_ - arm[2] * d1_;
-            o[9 + 3 * v + 1] = arm[2] * d0_ - arm[0] * d2_;
-            o[9 + 3 * v + 2] = arm[0] * d1_ - arm[1] * d0_;
-            o[18 + v] = d0_ * cb + d1_ * sb;             // h_d
-        }
+        member_row<true>(o, fr, arm, cb, sb);
         S.imem[3 * m + 0] = D.mem_node_start[m0 + m] - nbase;
         S.imem[3 * m + 1] = D.mem_node_start[m0 + m + 1] - nbase;
         S.imem[3 * m + 2] = D.mem_circ[m0 + m];
@@ -356,23 +349,7 @@ k_drag_solve(DesignsDev D, CasesDev Cs, Work W, SolveParams P)
                             if (j >= mend) {        // (uniform) entered a new member: member-level projections of the body velocity
                                 do { mcur++; mend = S.imem[3 * mcur + 1]; } while (j >= mend);
                                 const double *o = S.mem + mcur * MEM_STRIDE;
-                                double sr, si;
-                                // -i w (d . Xi_t + (a x d) . Xi_r)
-                                sr = o[0] * xr[0] + o[1] * xr[1] + o[2] * xr[2] + o[9] * xr[3] + o[10] * xr[4] + o[11] * xr[5];
-                                si = o[0] * xi[0] + o[1] * xi[1] + o[2] * xi[2] + o[9] * xi[3] + o[10] * xi[4] + o[11] * xi[5];
-                                mqr = w * si; mqi = -w * sr;
-                                sr = o[3] * xr[0] + o[4] * xr[1] + o[5] * xr[2] + o[12] * xr[3] + o[13] * xr[4] + o[14] * xr[5];
-                                si = o[3] * xi[0] + o[4] * xi[1] + o[5] * xi[2] + o[12] * xi[3] + o[13] * xi[4] + o[14] * xi[5];
-                                m1r = w * si; m1i = -w * sr;
-                                sr = o[6] * xr[0] + o[7] * xr[1] + o[8] * xr[2] + o[15] * xr[3] + o[16] * xr[4] + o[17] * xr[5];
-                                si = o[6] * xi[0] + o[7] * xi[1] + o[8] * xi[2] + o[15] * xi[3] + o[16] * xi[4] + o[17] * xi[5];
-                                m2r = w * si; m2i = -w * sr;
-                                sr = o[3] * xr[3] + o[4] * xr[4] + o[5] * xr[5];     // p1 . Xi_r
-                                si = o[3] * xi[3] + o[4] * xi[4] + o[5] * xi[5];
-                                t1r = w * si; t1i = -w * sr;
-                                sr = o[6] * xr[3] + o[7] * xr[4] + o[8] * xr[5];     // p2 . Xi_r
-                                si = o[6] * xi[3] + o[7] * xi[4] + o[8] * xi[5];
-                                t2r = w * si; t2i = -w * sr;
+                                member_velocity(o, xr, xi, w, mqr, mqi, m1r, m1i, m2r, m2i, t1r, t1i, t2r, t2i);
                                 hq = o[18]; h1 = o[19]; h2 = o[20]; dzq = o[2]; dz1 = o[5]; dz2 = o[8];
                             }
                             const double ls = S.node[j];
@@ -396,27 +373,7 @@ k_drag_solve(DesignsDev D, CasesDev Cs, Work W, SolveParams P)
             S.warp_part[((size_t)ch * nwarps + warp) * 32 + lane] = r;
         }
         __syncthreads();
-        for (int t = tid; t < nchunk * 32; t += SOLVE_THREADS) {
-            const int ch = t >> 5, l = t & 31;
-            double s = 0.0;
-            for (int wv = 0; wv < nwarps; wv++) s += S.warp_part[((size_t)ch * nwarps + wv) * 32 + l];
-            S.sums[par * sums_stride + t] = s;
-        }
-        if (CS > 1) {
-            cluster.sync();
-            for (int t = tid; t < nchunk * 32; t += SOLVE_THREADS) {
-                double s = 0.0;
-                for (int r = 0; r < CS; r++) {
-                    const double *rem = cluster.map_shared_rank(S.sums, r);
-                    s += rem[par * sums_stride + t];
-                }
-                S.tot[t] = s;
-            }
-        } else {
-            __syncthreads();
-            for (int t = tid; t < nchunk * 32; t += SOLVE_THREADS) S.tot[t] = S.sums[par * sums_stride + t];
-        }
-        __syncthreads();
+        rms_exchange<SOLVE_THREADS>(cluster, CS, nchunk, par, sums_stride, S.warp_part, S.sums, S.tot);
 
         // ================= linearised coefficients per node, member sums, B_drag ===================
         for (int j = tid; j < Ns; j += SOLVE_THREADS) {
@@ -424,41 +381,17 @@ k_drag_solve(DesignsDev D, CasesDev Cs, Work W, SolveParams P)
             const double sq = S.tot[ch * 32 + 3 * jj], s1 = S.tot[ch * 32 + 3 * jj + 1], s2 = S.tot[ch * 32 + 3 * jj + 2];
             int m = 0;
             while (j >= S.imem[3 * m + 1]) m++;
-            const bool circ = S.imem[3 * m + 2] != 0;
-            // getRMS (helpers.py:684): sqrt(0.5*sum |.|^2); circular members use the total transverse RMS
-            const double vq = sqrt(0.5 * sq);
-            const double v1 = circ ? sqrt(0.5 * (s1 + s2)) : sqrt(0.5 * s1);
-            const double v2 = circ ? v1 : sqrt(0.5 * s2);
+            double vq, v1, v2;
+            drag_rms(sq, s1, s2, S.imem[3 * m + 2] != 0, vq, v1, v2);
             S.node[4 * NsP + j] = S.node[1 * NsP + j] * vq;
             S.node[5 * NsP + j] = S.node[2 * NsP + j] * v1;
             S.node[6 * NsP + j] = S.node[3 * NsP + j] * v2;
         }
         __syncthreads();
-        for (int m = tid; m < Nm; m += SOLVE_THREADS) {
-            double bq = 0, b1 = 0, b1l = 0, b1ll = 0, b2 = 0, b2l = 0, b2ll = 0;
-            for (int j = S.imem[3 * m]; j < S.imem[3 * m + 1]; j++) {
-                const double ls = S.node[j], q_ = S.node[4 * NsP + j], p1_ = S.node[5 * NsP + j], p2_ = S.node[6 * NsP + j];
-                bq += q_; b1 += p1_; b1l += p1_ * ls; b1ll += p1_ * ls * ls; b2 += p2_; b2l += p2_ * ls; b2ll += p2_ * ls * ls;
-            }
-            double *o = S.msum + m * 8;
-            o[0] = bq; o[1] = b1; o[2] = b1l; o[3] = b1ll; o[4] = b2; o[5] = b2l; o[6] = b2ll;
-        }
+        drag_member_sums<SOLVE_THREADS, 3>(Nm, S.imem, S.node, S.node, 4 * NsP, 5 * NsP, 6 * NsP, S.msum);
         __syncthreads();
         if (tid < 36) {
-            const int a = tid / 6, b = tid % 6;
-            double s = 0.0;
-            for (int m = 0; m < Nm; m++) {
-                const double *o = S.mem + m * MEM_STRIDE, *ms = S.msum + m * 8;
-                // V_q = [q ; a x q]; V_1 = [p1 ; a x p1] + ls [0 ; p2]; V_2 = [p2 ; a x p2] - ls [0 ; p1]
-                const double vqa = a < 3 ? o[a] : o[9 + a - 3], vqb = b < 3 ? o[b] : o[9 + b - 3];
-                const double v1a = a < 3 ? o[3 + a] : o[12 + a - 3], v1b = b < 3 ? o[3 + b] : o[12 + b - 3];
-                const double v2a = a < 3 ? o[6 + a] : o[15 + a - 3], v2b = b < 3 ? o[6 + b] : o[15 + b - 3];
-                const double u1a = a < 3 ? 0.0 : o[6 + a - 3], u1b = b < 3 ? 0.0 : o[6 + b - 3];       // +p2
-                const double u2a = a < 3 ? 0.0 : -o[3 + a - 3], u2b = b < 3 ? 0.0 : -o[3 + b - 3];     // -p1
-                s += ms[0] * vqa * vqb;
-                s += ms[1] * v1a * v1b + ms[2] * (v1a * u1b + u1a * v1b) + ms[3] * u1a * u1b;
-                s += ms[4] * v2a * v2b + ms[5] * (v2a * u2b + u2a * v2b) + ms[6] * u2a * u2b;
-            }
+            const double s = drag_bmat_entry(tid, Nm, S.mem, S.msum);
             S.mat[36 + tid] = D.B0[(size_t)d * 36 + tid] + s;
             if (P.Bdrag_out && rank == 0) P.Bdrag_out[((size_t)d * Cs.nC + c) * 36 + tid] = s;
         }
@@ -490,13 +423,7 @@ k_drag_solve(DesignsDev D, CasesDev Cs, Work W, SolveParams P)
                     gr = cs.x * h2; gi = cs.y * dz2; cr = e.x * gr - e.y * gi; ci = e.x * gi + e.y * gr;
                     cr *= b2; ci *= b2; A2r += cr; A2i += ci; L2r += ls * cr; L2i += ls * ci;
                 }
-#pragma unroll
-                for (int a = 0; a < 3; a++) {
-                    br[a] += o[a] * Aqr + o[3 + a] * A1r + o[6 + a] * A2r;
-                    bi[a] += o[a] * Aqi + o[3 + a] * A1i + o[6 + a] * A2i;
-                    br[3 + a] += o[9 + a] * Aqr + o[12 + a] * A1r + o[15 + a] * A2r + o[6 + a] * L1r - o[3 + a] * L2r;
-                    bi[3 + a] += o[9 + a] * Aqi + o[12 + a] * A1i + o[15 + a] * A2i + o[6 + a] * L1i - o[3 + a] * L2i;
-                }
+                member_force6(o, Aqr, Aqi, A1r, A1i, A2r, A2i, L1r, L1i, L2r, L2i, br, bi);
             }
             if (P.Fdrag_out)
                 for (int a = 0; a < 6; a++) P.Fdrag_out[ogl + (size_t)a * nw + i] = make_double2(br[a], bi[a]);
@@ -552,29 +479,13 @@ k_drag_solve(DesignsDev D, CasesDev Cs, Work W, SolveParams P)
         if (P.mode == 1) break;
 
         // ---- all-reduce of (converged, flags) over the CTA and the cluster ----
-        int conv_all = __syncthreads_and(conv_local);
-        // __syncthreads_or returns a boolean, so reduce the two flag bits separately
-        int nan_all = (__syncthreads_or(nan_local & RAFTK_FLAG_NAN) ? RAFTK_FLAG_NAN : 0)
-                      | (__syncthreads_or(nan_local & RAFTK_FLAG_SINGULAR) ? RAFTK_FLAG_SINGULAR : 0);
-        if (CS > 1) {
-            if (tid == 0) { S.sums[par * sums_stride + nchunk * 32] = (double)conv_all; S.sums[par * sums_stride + nchunk * 32 + 1] = (double)nan_all; }
-            cluster.sync();
-            int ca = 1, na = 0;
-            for (int r = 0; r < CS; r++) {
-                const double *rem = cluster.map_shared_rank(S.sums, r);
-                ca &= (int)rem[par * sums_stride + nchunk * 32];
-                na |= (int)rem[par * sums_stride + nchunk * 32 + 1];
-            }
-            conv_all = ca; nan_all = na;
-        }
+        int conv_all, nan_all;
+        flags_exchange(cluster, CS, nchunk, par, sums_stride, conv_local, nan_local, S.sums, conv_all, nan_all);
         par ^= 1;
         flags |= nan_all;
         if (nan_all & RAFTK_FLAG_NAN) break;              // raft_model.py:1098-1099 raises here
         if (conv_all) { converged = 1; break; }
     }
-    if (P.status && rank == 0 && tid == 0) {
-        int *st = P.status + ((size_t)d * Cs.nC + c) * 4;
-        st[0] = passes; st[1] = converged; st[2] = flags; st[3] = 0;
-    }
+    if (P.status && rank == 0 && tid == 0) store_status(P.status + ((size_t)d * Cs.nC + c) * 4, passes, converged, flags, false, 0);
     if (CS > 1) cluster.sync();      // keep shared memory alive until every peer finished reading it
 }
