@@ -246,6 +246,9 @@ typedef struct raftk_dispatch {
                                  solve its secondary-train step                                                          */
     int32_t chunks;           /* v1 solver: launches over design chunks (1 = the whole batch at once)                    */
     int32_t inexact_walk;     /* the v1 solver ran because designs.walk_exact is 0                                       */
+    int32_t farm_classes;     /* farm family: bit (1 << RAFTK_KERNEL_FARM_*) of every farm kernel the call launched (the
+                                 kernel's bit for a uniform farm or batch; one per kernel class its farms occupy for a
+                                 ragged batch)                                                                           */
 } raftk_dispatch;
 int raftk_last_dispatch(raftk_dispatch *out);
 
@@ -729,6 +732,65 @@ int raftk_solve_dynamics_farm_batch_host(const raftk_designs *d, const raftk_cas
                                          const raftk_outputs *out, const raftk_farm_batch *f);
 
 /*
+ * Ragged farm batches (array-size studies: 4-, 6- and 9-turbine clusters, or how many turbines a lease area takes, in one
+ * call): n_farms farms of N_f FOWTs each, N_f = farm_fowt0[f + 1] - farm_fowt0[f].  The designs of the batch are every farm's
+ * FOWTs in order, farm after farm; all farms share the case table, frequency grid, depth and rho.  Each farm is assembled and
+ * solved exactly as raftk_farm or a uniform batch of its N solves it alone: its Xi_sys and info are bit-identical.
+ * Farms go to the kernel a uniform batch picks for their N (k_farm_rows<12> for N = 2, k_farm_response's warp form for
+ * 6N <= 24, its CTA form while the [6N][6N+1] system fits in shared memory, k_farm_response_global above); each class that
+ * occurs gets one launch over its own farms, which read their first design, N and output / matrix offsets from a descriptor
+ * table the entry writes at the head of the workspace.
+ * farm_fowt0 [n_farms + 1], HOST: farm_fowt0[0] = 0, strictly increasing, farm_fowt0[n_farms] = designs.n_designs.
+ * M_arr / B_arr / C_arr, any may be NULL: arr_shared = 1: one [6N,6N] set for every farm (only when every N_f is equal);
+ *   arr_shared = 0: farm f's [6N_f,6N_f] matrix starts at arr_offset[f] doubles, arr_offset [n_farms + 1] HOST with
+ *   arr_offset[0] = 0 and arr_offset[f + 1] - arr_offset[f] = 36 N_f^2 (NULL allowed when every matrix is NULL).
+ * Xi_sys complex, flat: farm f's [nC, 6N_f, nw] block starts at 6 nC nw farm_fowt0[f] complex values (n_designs nC 6 nw in
+ *   all); info [n_farms, nC, nw] or NULL: a zero pivot is flagged in its own farm's rows only.
+ * raftk_farm_ragged_workspace_bytes: the descriptor table plus, when a farm needs k_farm_response_global, its slabs (one
+ *   [6N_max][6N_max+1] per resident CTA, N_max the largest such farm, no more than that class's systems); 0 for a bad shape.
+ *   A smaller workspace that holds the table and one slab gives the same results with fewer CTAs.
+ * raftk_farm_ragged_response_ws_dev: `solved` holds the device outputs of raftk_solve_dynamics_dev on the same (d, c);
+ *   farm_fowt0 / arr_offset stay on the host, everything else is device memory.  _host: host pointers everywhere.
+ * RAFTK_EINVAL before any launch, with a named reason: n_farms < 1, no farm_fowt0, a CSR that does not start at 0, is not
+ * increasing (an empty farm) or does not end at n_designs, arr_shared not 0 or 1, arr_shared = 1 with unequal N_f, matrix
+ * offsets that do not match the farm sizes, no Xi_sys, a missing per-FOWT output (B_drag, F_drag, F_iner; F_BEM with BEM
+ * excitation), more than 65535 cases or 65535 farms of one on-chip class, or a workspace without the table and one slab.
+ */
+typedef struct raftk_farm_ragged {
+    int32_t n_farms;
+    int32_t arr_shared;             /* 1: one M_arr/B_arr/C_arr for every farm (equal N_f only); 0: CSR by arr_offset */
+    const int32_t *farm_fowt0;      /* HOST [n_farms + 1] */
+    const int64_t *arr_offset;      /* HOST [n_farms + 1] doubles, or NULL (arr_shared = 1, or no matrices) */
+    const double *M_arr, *B_arr, *C_arr;
+    double *Xi_sys;
+    int32_t *info;
+} raftk_farm_ragged;
+
+size_t raftk_farm_ragged_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm_ragged *f);
+int raftk_farm_ragged_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
+                                      const raftk_farm_ragged *f, void *workspace, size_t workspace_bytes, void *stream);
+int raftk_solve_dynamics_farm_ragged_host(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o,
+                                          const raftk_outputs *out, const raftk_farm_ragged *f);
+
+/*
+ * Ragged farm batches sharded over GPUs (raft_b200.sweep.ShardedFarmSolve(farm_sizes=...)): rank r solves a contiguous run of
+ * whole farms, farms [farm_row0, farm_row0 + f->n_farms) of the n_farms_total, whose FOWTs are designs [fowt_row0,
+ * fowt_row0 + d->n_designs) of the whole batch, and stores their results at their global offsets of EVERY rank's copy (no
+ * padding).  Rank p's copy holds
+ *     gathered[p]: complex Xi_sys, flat as raftk_farm_ragged's (n_ranks * peers.block_elems >= 6 nC nw n_designs_total)
+ *     status[p]:   int32 info [n_farms_total, nC, nw], followed by the per-FOWT status [n_designs_total, nC, 4]
+ * f describes this rank's farms (farm_fowt0 from 0, arr_offset from 0); f->Xi_sys and f->info must be their rows of this
+ * rank's own copy.  The farms are solved as raftk_farm_ragged_response_ws_dev solves them (same bits), then k_farm_publish_flat
+ * copies the rank's three contiguous runs (Xi_sys, info, status) to the other copies; follow with raftk_peer_barrier_dev.
+ * RAFTK_EINVAL before any launch, besides every refusal of raftk_farm_ragged_response_ws_dev: a bad raftk_peers, no info or
+ * per-FOWT status, a rank's status pointer missing, farm rows outside [0, n_farms_total), copies too small for this rank's
+ * FOWTs, and Xi_sys / info that are not this rank's rows of its own copy.
+ */
+int raftk_farm_ragged_response_gather_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
+                                          const raftk_farm_ragged *f, const raftk_peers *peers, int32_t farm_row0, int32_t fowt_row0,
+                                          int32_t n_farms_total, void *workspace, size_t workspace_bytes, void *stream);
+
+/*
  * Farm batches sharded over GPUs (raft_b200.sweep.ShardedFarmSolve): rank r solves a contiguous run of whole farms and stores
  * their results into EVERY rank's gathered copy (raftk_peers above); a farm is never split across ranks.  F_max is the largest
  * shard: smaller shards leave their last farm slots unwritten.  Rank p's copy holds
@@ -790,6 +852,23 @@ int raftk_farm_channel_stats_dev(int32_t n_farms, int32_t n_rows, int32_t n_dof,
                                  const raftk_farm_channels *ch, void *workspace, size_t workspace_bytes, void *stream);
 int raftk_farm_channel_stats_host(int32_t n_farms, int32_t n_rows, int32_t n_dof, int32_t nw, const double *w, const double *Xi_sys,
                                   const raftk_farm_channels *ch);
+
+/*
+ * Channels of a ragged farm batch (raftk_farm_ragged's flat Xi_sys): farm f has n_dof_f = 6 N_f, N_f = farm_fowt0[f + 1] -
+ * farm_fowt0[f], and channels [ch0[f], ch0[f + 1]) of the n_ch = ch0[n_farms] in all.  farm_fowt0 and ch0 are HOST arrays
+ * starting at 0 and strictly increasing.  ch->R packs every R_f [n_ch_f, n_dof_f] farm after farm (R_shared must be 0); wpow
+ * [n_ch] as the uniform entry's.  Outputs farm after farm: std [n_rows, n_ch_f] at n_rows ch0[f], psd / amp [n_rows, n_ch_f, nw]
+ * at n_rows ch0[f] nw.  Each farm's values are bit-identical to raftk_farm_channel_stats_* on that farm alone.  The workspace
+ * holds the farm descriptors (the query's 256-aligned head) and, without psd, |Y|^2.  Refusals: those of the uniform entry
+ * plus a bad CSR, n_ch != ch0[n_farms] and R_shared != 0.
+ */
+size_t raftk_farm_ragged_channel_stats_workspace_bytes(int32_t n_farms, int32_t n_rows, int32_t nw, const int32_t *farm_fowt0,
+                                                       const int32_t *ch0, const raftk_farm_channels *ch);
+int raftk_farm_ragged_channel_stats_dev(int32_t n_farms, int32_t n_rows, int32_t nw, const int32_t *farm_fowt0, const int32_t *ch0,
+                                        const double *w, const double *Xi_sys, const raftk_farm_channels *ch, void *workspace,
+                                        size_t workspace_bytes, void *stream);
+int raftk_farm_ragged_channel_stats_host(int32_t n_farms, int32_t n_rows, int32_t nw, const int32_t *farm_fowt0, const int32_t *ch0,
+                                         const double *w, const double *Xi_sys, const raftk_farm_channels *ch);
 
 /*
  * Rotor speed, generator torque and blade pitch statistics (FOWT.saveTurbineOutputs raft_fowt.py:2610-2679) for

@@ -76,6 +76,12 @@ class RaftkFarmBatch(C.Structure):
                 ("M_arr", C.c_void_p), ("B_arr", C.c_void_p), ("C_arr", C.c_void_p), ("Xi_sys", C.c_void_p), ("info", C.c_void_p)]
 
 
+class RaftkFarmRagged(C.Structure):
+    """include/raftk.h raftk_farm_ragged: n_farms farms of their own N_f FOWTs each (farm_fowt0, arr_offset: host CSR arrays)."""
+    _fields_ = [("n_farms", C.c_int32), ("arr_shared", C.c_int32), ("farm_fowt0", C.c_void_p), ("arr_offset", C.c_void_p),
+                ("M_arr", C.c_void_p), ("B_arr", C.c_void_p), ("C_arr", C.c_void_p), ("Xi_sys", C.c_void_p), ("info", C.c_void_p)]
+
+
 SLENDER_ARRAYS = ("w", "k", "mem_q", "mem_p1", "mem_p2", "mem_mcf", "mem_wl", "mem_r_int", "mem_a_wl", "mem_rwl", "mem_R_wl", "mem_node_start",
                   "node_r", "node_v_side", "node_Ca_p1", "node_Ca_p2", "node_Ca_End", "node_v_end", "node_a_i",
                   "seg_mem", "seg_z1", "seg_z2", "seg_R", "seg_rmid", "M_struc")
@@ -165,7 +171,7 @@ class RaftkSlenderOutputs(C.Structure):
 class RaftkDispatch(C.Structure):
     """include/raftk.h raftk_dispatch: the kernel variant the last call on this thread launched."""
     _fields_ = [(n, C.c_int32) for n in ("family", "kernel", "cluster_size", "bins_per_cta", "threads_per_cta", "f0_global", "direct_d2h",
-                                         "trains", "chunks", "inexact_walk")]
+                                         "trains", "chunks", "inexact_walk", "farm_classes")]
 
 
 # every symbol include/raftk.h declares (tests/test_abi.py checks the header against this list)
@@ -216,6 +222,9 @@ SYMBOLS = [
     "raftk_farm_response_dev", "raftk_solve_dynamics_farm_host", "raftk_farm_workspace_bytes", "raftk_farm_response_ws_dev",
     "raftk_farm_batch_workspace_bytes", "raftk_farm_batch_response_ws_dev", "raftk_solve_dynamics_farm_batch_host",
     "raftk_farm_batch_response_gather_dev",
+    "raftk_farm_ragged_workspace_bytes", "raftk_farm_ragged_response_ws_dev", "raftk_solve_dynamics_farm_ragged_host",
+    "raftk_farm_ragged_response_gather_dev", "raftk_farm_ragged_channel_stats_workspace_bytes", "raftk_farm_ragged_channel_stats_dev",
+    "raftk_farm_ragged_channel_stats_host",
     "raftk_family_sizes", "raftk_build_family_host",
     "raftk_eigen_workspace_bytes", "raftk_eigen_dev", "raftk_eigen_host",
     "raftk_farm_channel_stats_workspace_bytes", "raftk_farm_channel_stats_dev", "raftk_farm_channel_stats_host",
@@ -364,6 +373,24 @@ def _load():
     lib.raftk_farm_batch_response_gather_dev.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkOutputs), P(RaftkFarmBatch), P(RaftkPeers),
                                                          C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
     lib.raftk_farm_batch_response_gather_dev.restype = C.c_int
+    lib.raftk_farm_ragged_workspace_bytes.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkFarmRagged)]
+    lib.raftk_farm_ragged_workspace_bytes.restype = C.c_size_t
+    lib.raftk_farm_ragged_response_ws_dev.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkOutputs), P(RaftkFarmRagged), C.c_void_p,
+                                                      C.c_size_t, C.c_void_p]
+    lib.raftk_farm_ragged_response_ws_dev.restype = C.c_int
+    lib.raftk_solve_dynamics_farm_ragged_host.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkSolveOpts), P(RaftkOutputs),
+                                                          P(RaftkFarmRagged)]
+    lib.raftk_solve_dynamics_farm_ragged_host.restype = C.c_int
+    lib.raftk_farm_ragged_response_gather_dev.argtypes = [P(RaftkDesigns), P(RaftkCases), P(RaftkOutputs), P(RaftkFarmRagged), P(RaftkPeers),
+                                                          C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.raftk_farm_ragged_response_gather_dev.restype = C.c_int
+    lib.raftk_farm_ragged_channel_stats_workspace_bytes.argtypes = [C.c_int32] * 3 + [C.c_void_p, C.c_void_p, P(RaftkFarmChannels)]
+    lib.raftk_farm_ragged_channel_stats_workspace_bytes.restype = C.c_size_t
+    lib.raftk_farm_ragged_channel_stats_dev.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 4 + [P(RaftkFarmChannels), C.c_void_p, C.c_size_t,
+                                                                                          C.c_void_p]
+    lib.raftk_farm_ragged_channel_stats_dev.restype = C.c_int
+    lib.raftk_farm_ragged_channel_stats_host.argtypes = [C.c_int32] * 3 + [C.c_void_p] * 4 + [P(RaftkFarmChannels)]
+    lib.raftk_farm_ragged_channel_stats_host.restype = C.c_int
     lib.raftk_eigen_workspace_bytes.argtypes = [P(RaftkEigen)]
     lib.raftk_eigen_workspace_bytes.restype = C.c_size_t
     lib.raftk_eigen_dev.argtypes = [P(RaftkEigen), C.c_void_p, C.c_size_t, C.c_void_p]

@@ -135,6 +135,7 @@ static void disp_launch(int family, int kernel, int threads, int cluster_size = 
     disp_reset();
     g_disp.family = family; g_disp.kernel = kernel; g_disp.threads_per_cta = threads;
     g_disp.cluster_size = cluster_size; g_disp.bins_per_cta = bins_per_cta;
+    if (family == RAFTK_FAMILY_FARM) g_disp.farm_classes = 1 << kernel;
 }
 extern "C" int raftk_last_dispatch(raftk_dispatch *out)
 {
@@ -1188,6 +1189,224 @@ extern "C" int raftk_farm_batch_response_gather_dev(const raftk_designs *d, cons
     return farm_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream, &px);
 }
 
+// ---- ragged farm batches (raftk_farm_ragged) ---------------------------------------------------------------------------
+// Every farm goes to the kernel class farm_launch picks for a uniform batch of its N; a class is launched once over its own
+// farms, in this order.  The descriptors are grouped by class (farms of a class in batch order) and copied to the head of
+// the workspace, where the class's launch finds its run.
+enum { FC_ROWS, FC_WARP, FC_BLOCK, FC_GLOBAL, FC_N };
+static const int fc_kernel[FC_N] = {RAFTK_KERNEL_FARM_ROWS12, RAFTK_KERNEL_FARM_WARP, RAFTK_KERNEL_FARM_BLOCK, RAFTK_KERNEL_FARM_GLOBAL};
+static int farm_class(int N)
+{
+    if (!farm_on_chip(N)) return FC_GLOBAL;
+    if (6 * N == 12 && !getenv("RAFTK_FARM_SMEM")) return FC_ROWS;
+    return 6 * N <= 24 ? FC_WARP : FC_BLOCK;
+}
+
+struct RagPlan {
+    std::vector<FarmDesc> fd;           // grouped by class: class k is fd[first[k], first[k + 1])
+    int first[FC_N + 1] = {};
+    int nmax[FC_N] = {};                // largest N of each class
+    size_t table = 0;                   // bytes of the descriptor table at the head of the workspace (256-aligned)
+    size_t slab = 0;                    // double2 elements of one k_farm_response_global slab (the class's largest N)
+    size_t pan_smem = 0;                // k_farm_response_global's panel: the largest n * pw of its farms
+    int per_sm = 0;                     // its CTAs per SM: the fewest any of its farms' glu_plan allows
+    long long gsys = 0;                 // (farm, case, bin) systems of that class
+    size_t bytes = 0;                   // the full workspace: table + min(gsys, resident CTAs) slabs
+};
+
+static int rag_plan(const raftk_designs *d, const raftk_cases *c, const raftk_farm_ragged *f, RagPlan &R)
+{
+    if (!d || !c || !f) return set_err(RAFTK_EINVAL, "ragged farm batch: null argument");
+    auto bad_farm = [](const char *fmt, int k) { char b[16]; snprintf(b, sizeof(b), "%d", k); return set_err(RAFTK_EINVAL, fmt, b); };
+    const int F = f->n_farms;
+    if (F < 1) return set_err(RAFTK_EINVAL, "ragged farm batch: n_farms must be >= 1");
+    if (!f->farm_fowt0) return set_err(RAFTK_EINVAL, "ragged farm batch: farm_fowt0 is required");
+    if (f->farm_fowt0[0] != 0) return set_err(RAFTK_EINVAL, "ragged farm batch: farm_fowt0[0] must be 0");
+    for (int k = 0; k < F; k++)
+        if (f->farm_fowt0[k + 1] <= f->farm_fowt0[k])
+            return bad_farm("ragged farm batch: farm_fowt0 must be strictly increasing (farm %s is empty)", k);
+    if (f->farm_fowt0[F] != d->n_designs) return set_err(RAFTK_EINVAL, "ragged farm batch: farm_fowt0[n_farms] must equal designs.n_designs");
+    if (f->arr_shared != 0 && f->arr_shared != 1) return set_err(RAFTK_EINVAL, "ragged farm batch: arr_shared must be 0 or 1");
+    const bool mats = f->M_arr || f->B_arr || f->C_arr;
+    for (int k = 0; k < F; k++) {
+        const long long N = f->farm_fowt0[k + 1] - f->farm_fowt0[k];
+        if (f->arr_shared && N != f->farm_fowt0[1])
+            return bad_farm("ragged farm batch: arr_shared = 1 needs every farm to have the same N (farm %s differs)", k);
+        if (!f->arr_shared && mats) {
+            if (!f->arr_offset) return set_err(RAFTK_EINVAL, "ragged farm batch: arr_offset is required with per-farm array matrices");
+            if (f->arr_offset[0] != 0 || f->arr_offset[k + 1] - f->arr_offset[k] != 36 * N * N)
+                return bad_farm("ragged farm batch: arr_offset must start at 0 and step by 36 N^2 (farm %s does not)", k);
+        }
+    }
+    if (c->n_cases < 1 || d->nw < 1) return set_err(RAFTK_EINVAL, "ragged farm batch: no cases or no frequency bins");
+    std::vector<int> cls(F);
+    int count[FC_N] = {};
+    for (int k = 0; k < F; k++) {
+        const int N = f->farm_fowt0[k + 1] - f->farm_fowt0[k];
+        cls[k] = farm_class(N);
+        count[cls[k]]++;
+        R.nmax[cls[k]] = std::max(R.nmax[cls[k]], N);
+    }
+    for (int k = 0; k < FC_N; k++) R.first[k + 1] = R.first[k] + count[k];
+    if (R.first[FC_GLOBAL] > 0) {      // the grids of the on-chip classes are (frequency groups, case, farm of the class)
+        if (c->n_cases > 65535) return set_err(RAFTK_EINVAL, "ragged farm batch: more than 65535 cases per call with farms solved on chip (6N <= 120)");
+        for (int k = 0; k < FC_GLOBAL; k++)
+            if (count[k] > 65535) return set_err(RAFTK_EINVAL, "ragged farm batch: more than 65535 farms of one on-chip kernel class per call");
+    }
+    R.fd.resize(F);
+    int next[FC_N];
+    for (int k = 0; k < FC_N; k++) next[k] = R.first[k];
+    R.per_sm = 2;
+    for (int k = 0; k < F; k++) {
+        FarmDesc &e = R.fd[next[cls[k]]++];
+        e.d0 = f->farm_fowt0[k]; e.N = f->farm_fowt0[k + 1] - f->farm_fowt0[k]; e.pw = 0; e._pad = 0;
+        e.xo = (size_t)6 * c->n_cases * d->nw * e.d0;
+        e.io = (size_t)k * c->n_cases * d->nw;
+        e.ao = (!f->arr_shared && mats) ? (size_t)f->arr_offset[k] : 0;
+        if (cls[k] == FC_GLOBAL) {
+            const GluPlan g = glu_plan(6 * e.N);
+            if (!g.pw) return bad_farm("ragged farm batch: farm %s: 6N too large for one panel column in shared memory", k);
+            e.pw = g.pw;
+            R.pan_smem = std::max(R.pan_smem, g.smem);
+            R.per_sm = std::min(R.per_sm, g.per_sm);
+        }
+    }
+    // the global class walks its systems in descriptor order, dealt round-robin over the resident CTAs: largest farms first,
+    // so that no CTA is left with two of the largest systems while others finish small ones (a farm's bits do not depend on it)
+    std::stable_sort(R.fd.begin() + R.first[FC_GLOBAL], R.fd.begin() + R.first[FC_GLOBAL + 1],
+                     [](const FarmDesc &a, const FarmDesc &b) { return a.N > b.N; });
+    R.table = align_up((size_t)F * sizeof(FarmDesc), 256);
+    R.bytes = R.table;
+    if (count[FC_GLOBAL]) {
+        R.slab = (size_t)6 * R.nmax[FC_GLOBAL] * (6 * R.nmax[FC_GLOBAL] + 1);
+        R.gsys = (long long)count[FC_GLOBAL] * c->n_cases * d->nw;
+        R.bytes += (size_t)std::min<long long>(R.gsys, (long long)R.per_sm * sm_count()) * R.slab * sizeof(double2);
+    }
+    return RAFTK_OK;
+}
+
+extern "C" size_t raftk_farm_ragged_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm_ragged *f)
+{
+    RagPlan R;
+    return rag_plan(d, c, f, R) ? 0 : R.bytes;
+}
+
+static int farm_ragged_launch(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm_ragged *f,
+                              void *ws, size_t ws_bytes, cudaStream_t st)
+{
+    if (!solved) return set_err(RAFTK_EINVAL, "ragged farm batch: null argument");
+    RagPlan R;
+    if (int rc = rag_plan(d, c, f, R)) return rc;
+    if (!f->Xi_sys) return set_err(RAFTK_EINVAL, "ragged farm batch: Xi_sys is required");
+    if (!solved->B_drag || !solved->F_drag || !solved->F_iner)
+        return set_err(RAFTK_EINVAL, "ragged farm batch needs B_drag, F_drag, F_iner of the per-FOWT solve");
+    if (d->n_bem_head > 0 && !solved->F_BEM) return set_err(RAFTK_EINVAL, "ragged farm batch: the designs carry BEM excitation, F_BEM is required");
+    const size_t slab_bytes = R.slab * sizeof(double2);
+    if (!ws || ws_bytes < R.table + slab_bytes)
+        return set_err(RAFTK_EINVAL, "ragged farm batch: the workspace must hold the farm descriptor table%s (raftk_farm_ragged_workspace_bytes)",
+                       R.slab ? " and one [6N][6N+1] slab of the largest farm solved in global memory" : "");
+    FarmDesc *dfd = static_cast<FarmDesc *>(ws);
+    CUDA_TRY(cudaMemcpyAsync(dfd, R.fd.data(), R.fd.size() * sizeof(FarmDesc), cudaMemcpyHostToDevice, st));
+    FarmRagParams P{};
+    P.nC = c->n_cases; P.nw = d->nw;
+    P.B_drag = solved->B_drag;
+    P.F_drag = reinterpret_cast<const double2 *>(solved->F_drag);
+    P.F_iner = reinterpret_cast<const double2 *>(solved->F_iner);
+    P.F_BEM = d->n_bem_head > 0 ? reinterpret_cast<const double2 *>(solved->F_BEM) : nullptr;
+    P.M_arr = f->M_arr; P.B_arr = f->B_arr; P.C_arr = f->C_arr;
+    P.Xi = reinterpret_cast<double2 *>(f->Xi_sys); P.info = f->info;
+    P.slab = R.slab;
+    DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
+    CasesDev C = to_dev(c);
+    const unsigned gy = c->n_cases;
+    int mask = 0, last = FC_N;
+    auto go = [&](auto op_c) -> int {
+        constexpr bool OP = decltype(op_c)::value;
+        static SmemOptIn opt_w(48 * 1024), opt_b(48 * 1024), opt_g(0);
+        for (int k = 0; k < FC_N; k++) {
+            const int nk = R.first[k + 1] - R.first[k];
+            if (!nk) continue;
+            P.fd = dfd + R.first[k]; P.nF = nk;
+            const int n = 6 * R.nmax[k];
+            const size_t sys_bytes = (size_t)n * (n + 1) * sizeof(double2);
+            ProfScope ps(st, 1);
+            if (k == FC_ROWS) {
+                k_farm_rows<12, OP, false, true><<<dim3((d->nw + 7) / 8, gy, nk), 128, 0, st>>>(D, C, P);
+            } else if (k == FC_WARP) {   // shared memory for wpc systems of the class's largest N (farm_launch's rule)
+                const int wpc = (int)std::max<size_t>(1, std::min<size_t>(FARM_WPC, (100 * 1024) / sys_bytes));
+                CUDA_TRY(opt_w.ensure(k_farm_response<true, OP, false, true>, wpc * sys_bytes));
+                k_farm_response<true, OP, false, true><<<dim3((d->nw + wpc - 1) / wpc, gy, nk), 32 * wpc, wpc * sys_bytes, st>>>(D, C, P);
+            } else if (k == FC_BLOCK) {
+                CUDA_TRY(opt_b.ensure(k_farm_response<false, OP, false, true>, sys_bytes));
+                k_farm_response<false, OP, false, true><<<dim3(d->nw, gy, nk), 256, sys_bytes, st>>>(D, C, P);
+            } else {
+                CUDA_TRY(opt_g.ensure(k_farm_response_global<OP, true>, R.pan_smem));
+                double2 *slabs = reinterpret_cast<double2 *>(static_cast<char *>(ws) + R.table);
+                const long long fit = (long long)((ws_bytes - R.table) / slab_bytes);
+                const int grid = (int)std::min<long long>(std::min<long long>(R.gsys, fit), (long long)R.per_sm * sm_count());
+                k_farm_response_global<OP, true><<<grid, GLU_T, R.pan_smem, st>>>(D, C, P, slabs, 0);
+            }
+            g_launches++;
+            CUDA_TRY(cudaGetLastError());
+            mask |= 1 << fc_kernel[k];
+            last = k;
+        }
+        return RAFTK_OK;
+    };
+    const int rc = c->op ? go(std::true_type{}) : go(std::false_type{});
+    if (rc) return rc;
+    disp_launch(RAFTK_FAMILY_FARM, fc_kernel[last], last == FC_ROWS ? 128 : last == FC_WARP ? 32 * FARM_WPC : GLU_T);
+    g_disp.farm_classes = mask;
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_farm_ragged_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
+                                                 const raftk_farm_ragged *f, void *workspace, size_t workspace_bytes, void *stream)
+{
+    disp_reset();
+    if (int rc = validate_op_dev(c)) return rc;
+    return farm_ragged_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int raftk_farm_ragged_response_gather_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
+                                                     const raftk_farm_ragged *f, const raftk_peers *peers, int32_t farm_row0,
+                                                     int32_t fowt_row0, int32_t n_farms_total, void *workspace, size_t workspace_bytes,
+                                                     void *stream)
+{
+    disp_reset();
+    if (int rc = validate_peers(peers)) return rc;
+    if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "ragged farm gather: null argument");
+    if (!f->info || !solved->status) return set_err(RAFTK_EINVAL, "ragged farm gather: farm.info and the per-FOWT status are required");
+    for (int r = 0; r < peers->n_ranks; r++)
+        if (!peers->status[r]) return set_err(RAFTK_EINVAL, "ragged farm gather: a rank's gathered info and status (peers.status) is missing");
+    if (farm_row0 < 0 || fowt_row0 < 0 || (long long)farm_row0 + f->n_farms > n_farms_total)
+        return set_err(RAFTK_EINVAL, "ragged farm gather: farms [farm_row0, farm_row0 + n_farms) must lie in [0, n_farms_total)");
+    const size_t per = (size_t)6 * c->n_cases * d->nw;                        // complex elements of one FOWT's rows of Xi_sys
+    if (c->n_cases < 1 || d->nw < 1 || per * ((size_t)fowt_row0 + d->n_designs) > (size_t)peers->n_ranks * peers->block_elems)
+        return set_err(RAFTK_EINVAL, "ragged farm gather: the gathered copies (n_ranks * peers.block_elems) do not hold this rank's farms");
+    const size_t info_farm = (size_t)c->n_cases * d->nw, info_all = (size_t)n_farms_total * info_farm;
+    if (f->Xi_sys != peers->gathered[peers->rank] + 2 * per * fowt_row0 || f->info != peers->status[peers->rank] + (size_t)farm_row0 * info_farm)
+        return set_err(RAFTK_EINVAL, "ragged farm gather: farm.Xi_sys and info must be this rank's farms in its own gathered copy");
+    if (int rc = validate_op_dev(c)) return rc;
+    if (int rc = farm_ragged_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream)) return rc;
+    const raftk_dispatch rec = g_disp;
+    FarmFlatPeer P{};
+    P.n_peers = peers->n_ranks;
+    P.nx = per * d->n_designs; P.ni = (size_t)f->n_farms * info_farm; P.ns = (size_t)d->n_designs * c->n_cases * 4;
+    P.Xi = reinterpret_cast<const double2 *>(f->Xi_sys); P.info = f->info; P.status = solved->status;
+    for (int r = 0; r < peers->n_ranks; r++) {
+        const bool other = r != peers->rank;
+        P.X[r] = other ? reinterpret_cast<double2 *>(peers->gathered[r]) + per * fowt_row0 : nullptr;
+        P.I[r] = other ? peers->status[r] + (size_t)farm_row0 * info_farm : nullptr;
+        P.S[r] = peers->status[r] + info_all + (size_t)fowt_row0 * c->n_cases * 4;
+    }
+    k_farm_publish_flat<<<dim3((unsigned)std::min<size_t>((P.nx + 255) / 256, 1024), (unsigned)P.n_peers), 256, 0, (cudaStream_t)stream>>>(P);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    g_disp = rec;                                                              // the record names the solve's classes
+    return RAFTK_OK;
+}
+
 
 // ---- native node-table builder for design families (pure host code, raftk_builder.h) ---------------------------------
 static int set_err_i(int code, const char *fmt, int a = 0, int b = 0)
@@ -1387,7 +1606,7 @@ static void stage_designs_cases(Staging &S, const raftk_designs *d, const raftk_
 }
 
 static int host_run(const char *who, const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
-                    const double *Xi_in, int mode, const raftk_farm_batch *farm = nullptr)
+                    const double *Xi_in, int mode, const raftk_farm_batch *farm = nullptr, const raftk_farm_ragged *rag = nullptr)
 {
     disp_reset();
     int rc = validate(d, c);
@@ -1413,6 +1632,15 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
         const size_t nA = (farm->arr_shared ? 1 : (size_t)farm->n_farms) * 36 * farm->n_fowt * farm->n_fowt;
         S.in(fd.M_arr, farm->M_arr, nA); S.in(fd.B_arr, farm->B_arr, nA); S.in(fd.C_arr, farm->C_arr, nA);
     }
+    raftk_farm_ragged rd;
+    memset(&rd, 0, sizeof(rd));
+    if (rag) {                                            // (rag_plan has accepted its shape)
+        rd = *rag;
+        const size_t N0 = (size_t)rag->farm_fowt0[1];
+        const size_t nA = rag->arr_shared ? 36 * N0 * N0 : (rag->arr_offset ? (size_t)rag->arr_offset[rag->n_farms] : 0);
+        S.in(rd.M_arr, rag->M_arr, nA); S.in(rd.B_arr, rag->B_arr, nA); S.in(rd.C_arr, rag->C_arr, nA);
+    }
+    const bool farms = farm || rag;
     // the solve is planned once, at the caller's cluster size, and launched with the workspace that plan needs; excitation
     // and linearisation need the whole batch's tables in one chunk
     const SolvePlan pl = mode == 0 ? plan_solve(d, (int)nC, o->cluster_size, WS_UNBOUNDED) : SolvePlan{};
@@ -1440,18 +1668,19 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
     S.out(od.Xi, out->Xi ? nR : 0, xi_direct ? nullptr : out->Xi);
     S.out(od.status, out->status ? nD * nC * 4 : 0, st_direct ? nullptr : out->status);
     // the system response reads the per-FOWT loads on the device: those buffers exist even when the caller does not want them back
-    S.out(od.B_drag, out->B_drag || farm ? nD * nC * 36 : 0, out->B_drag);
-    S.out(od.F_drag, out->F_drag || farm ? nR : 0, out->F_drag);
-    S.out(od.F_iner, out->F_iner || farm ? nR : 0, out->F_iner);
-    S.out(od.F_BEM, out->F_BEM || (farm && d->n_bem_head > 0) ? nR : 0, out->F_BEM);
+    S.out(od.B_drag, out->B_drag || farms ? nD * nC * 36 : 0, out->B_drag);
+    S.out(od.F_drag, out->F_drag || farms ? nR : 0, out->F_drag);
+    S.out(od.F_iner, out->F_iner || farms ? nR : 0, out->F_iner);
+    S.out(od.F_BEM, out->F_BEM || (farms && d->n_bem_head > 0) ? nR : 0, out->F_BEM);
     S.out(od.zeta, out->zeta ? nC * nw : 0, out->zeta);
     const bool qtf_solve = (mode == 0 && d->n_qtf_w > 0 && !c->F_2nd);   // potSecOrder 2: compute the force on the device first
     if (qtf_solve) { S.out(od.F_2nd, nR / 2, out->F_2nd); S.out(od.F_2nd_mean, nD * nC * 6, out->F_2nd_mean); }
     S.out(od.Xi_last, out->Xi_last ? nR : 0, out->Xi_last);
     char *ws, *fws = nullptr;
     S.buf(ws, wb);
-    const size_t fwb = farm ? farm_ws_bytes(d, c, farm) : 0;                  // slabs of the global-memory system kernel (0 on chip)
+    const size_t fwb = farm ? farm_ws_bytes(d, c, farm) : rag ? raftk_farm_ragged_workspace_bytes(d, c, rag) : 0;
     if (farm) { S.out(fd.Xi_sys, nR, farm->Xi_sys); S.out(fd.info, farm->info ? farm->n_farms * nC * nw : 0, farm->info); S.buf(fws, fwb); }
+    if (rag) { S.out(rd.Xi_sys, nR, rag->Xi_sys); S.out(rd.info, rag->info ? rag->n_farms * nC * nw : 0, rag->info); S.buf(fws, fwb); }
     if ((rc = S.commit())) return rc;
     if (qtf_solve) {
         if ((rc = run_qtf(&dd, &cc, od.F_2nd, od.F_2nd_mean, 0))) return rc;
@@ -1470,6 +1699,7 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
     }
     if (rc) return rc;
     if (farm && (rc = farm_launch(&dd, &cc, &od, &fd, fws, fwb, 0))) return rc;
+    if (rag && (rc = farm_ragged_launch(&dd, &cc, &od, &rd, fws, fwb, 0))) return rc;
     g_disp.direct_d2h = xi_direct != nullptr;
     return S.finish();
 }
@@ -1506,6 +1736,17 @@ extern "C" int raftk_solve_dynamics_farm_batch_host(const raftk_designs *d, cons
     if (!d || !f) return set_err(RAFTK_EINVAL, "farm batch: null argument");
     if (int rc = farm_batch_shape(d, f)) return rc;
     return host_run("raftk_solve_dynamics_farm_batch_host", d, c, o, out, nullptr, 0, f);
+}
+
+extern "C" int raftk_solve_dynamics_farm_ragged_host(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o,
+                                                     const raftk_outputs *out, const raftk_farm_ragged *f)
+{
+    disp_reset();
+    if (!out || !out->Xi || !out->status || !o) return set_err(RAFTK_EINVAL, "Xi, status and opts are required");
+    RagPlan R;
+    if (int rc = rag_plan(d, c, f, R)) return rc;
+    if (!f->Xi_sys) return set_err(RAFTK_EINVAL, "ragged farm batch: Xi_sys is required");
+    return host_run("raftk_solve_dynamics_farm_ragged_host", d, c, o, out, nullptr, 0, nullptr, f);
 }
 
 extern "C" int raftk_second_order_force_host(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *out)
@@ -2754,6 +2995,112 @@ extern "C" int raftk_farm_channel_stats_host(int32_t n_farms, int32_t n_rows, in
     S.buf(ws, wb);
     int rc;
     if ((rc = S.commit()) || (rc = raftk_farm_channel_stats_dev(n_farms, n_rows, n_dof, nw, dW, dXi, &d, ws, wb, nullptr))) return rc;
+    return S.finish();
+}
+
+// ---- channels of ragged farm batches (raftk_farm_ragged_channel_stats_*) ---------------------------------------------------
+struct RagChPlan {
+    std::vector<FarmChDesc> fd;
+    int n_max = 0, n_ch = 0;
+    size_t table = 0, n_r = 0, n_xi = 0;   // descriptor bytes (256-aligned); doubles of the packed R; complex elements of Xi_sys
+};
+static int ragch_plan(int32_t n_farms, int32_t n_rows, int32_t nw, const int32_t *farm_fowt0, const int32_t *ch0, const double *w,
+                      const double *Xi_sys, const raftk_farm_channels *ch, RagChPlan &R)
+{
+    if (!ch || !farm_fowt0 || !ch0) return set_err(RAFTK_EINVAL, "ragged farm channel-stats: null argument");
+    if (n_farms < 1 || n_rows < 1 || nw < 1) return set_err(RAFTK_EINVAL, "ragged farm channel-stats: n_farms, n_rows and nw must be >= 1");
+    if (farm_fowt0[0] != 0 || ch0[0] != 0) return set_err(RAFTK_EINVAL, "ragged farm channel-stats: farm_fowt0[0] and ch0[0] must be 0");
+    for (int k = 0; k < n_farms; k++)
+        if (farm_fowt0[k + 1] <= farm_fowt0[k] || ch0[k + 1] <= ch0[k])
+            return set_err(RAFTK_EINVAL, "ragged farm channel-stats: farm_fowt0 and ch0 must be strictly increasing (a farm without FOWTs or channels)");
+    if (ch->n_ch != ch0[n_farms]) return set_err(RAFTK_EINVAL, "ragged farm channel-stats: channels.n_ch must equal ch0[n_farms]");
+    if (ch->R_shared != 0) return set_err(RAFTK_EINVAL, "ragged farm channel-stats: R_shared must be 0 (R_f is per farm)");
+    int nmax = 0;
+    for (int k = 0; k < n_farms; k++) nmax = std::max(nmax, 6 * (farm_fowt0[k + 1] - farm_fowt0[k]));
+    if (int rc = farm_ch_check(n_farms, n_rows, nmax, nw, w, Xi_sys, ch)) return rc;
+    R.fd.resize(n_farms);
+    size_t ro = 0;
+    for (int k = 0; k < n_farms; k++) {
+        FarmChDesc &e = R.fd[k];
+        e.n = 6 * (farm_fowt0[k + 1] - farm_fowt0[k]); e.nch = ch0[k + 1] - ch0[k]; e.ch0 = ch0[k]; e._pad = 0;
+        e.xo = (size_t)6 * n_rows * nw * farm_fowt0[k]; e.ro = ro;
+        ro += (size_t)e.nch * e.n;
+    }
+    R.n_max = nmax; R.n_ch = ch->n_ch; R.n_r = ro; R.n_xi = (size_t)6 * n_rows * nw * farm_fowt0[n_farms];
+    R.table = align_up((size_t)n_farms * sizeof(FarmChDesc), 256);
+    return RAFTK_OK;
+}
+
+extern "C" size_t raftk_farm_ragged_channel_stats_workspace_bytes(int32_t n_farms, int32_t n_rows, int32_t nw, const int32_t *farm_fowt0,
+                                                                  const int32_t *ch0, const raftk_farm_channels *ch)
+{
+    RagChPlan R;
+    static const double one = 1.0;                                             // (w and Xi_sys are not read by the query)
+    if (ragch_plan(n_farms, n_rows, nw, farm_fowt0, ch0, &one, &one, ch, R)) return 0;
+    return R.table + (ch->psd ? 0 : (size_t)n_rows * ch->n_ch * nw * sizeof(double));
+}
+
+extern "C" int raftk_farm_ragged_channel_stats_dev(int32_t n_farms, int32_t n_rows, int32_t nw, const int32_t *farm_fowt0,
+                                                   const int32_t *ch0, const double *w, const double *Xi_sys,
+                                                   const raftk_farm_channels *ch, void *workspace, size_t workspace_bytes, void *stream)
+{
+    RagChPlan R;
+    if (int rc = ragch_plan(n_farms, n_rows, nw, farm_fowt0, ch0, w, Xi_sys, ch, R)) return rc;
+    const size_t scratch = ch->psd ? 0 : (size_t)n_rows * ch->n_ch * nw * sizeof(double);
+    if (!workspace || workspace_bytes < R.table + scratch)
+        return set_err(RAFTK_EINVAL, "ragged farm channel-stats: the workspace must hold the farm descriptors and, without psd, |Y|^2 "
+                                     "(raftk_farm_ragged_channel_stats_workspace_bytes)");
+    const cudaStream_t st = (cudaStream_t)stream;
+    FarmChDesc *dfd = static_cast<FarmChDesc *>(workspace);
+    CUDA_TRY(cudaMemcpyAsync(dfd, R.fd.data(), R.fd.size() * sizeof(FarmChDesc), cudaMemcpyHostToDevice, st));
+    const int32_t units = n_farms * n_rows;
+    FarmChRagParams P = {};
+    P.n = R.n_max; P.nch = ch->n_ch; P.nw = nw; P.n_rows = n_rows;
+    P.w = w; P.R = ch->R; P.Xi = reinterpret_cast<const double2 *>(Xi_sys);
+    P.a2 = ch->psd ? ch->psd : reinterpret_cast<double *>(static_cast<char *>(workspace) + R.table);
+    P.amp = reinterpret_cast<double2 *>(ch->amp);
+    P.fd = dfd;
+    for (int32_t t = 0; ch->wpow && t < ch->n_ch; t++) P.wbits[t >> 4] |= (unsigned)ch->wpow[t] << ((t & 15) * 2);
+    const int tile = farm_ch_tile(units, R.n_max, nw, ch->tile_w);            // one tile width for every farm: the largest n's
+    P.tile = tile ? tile : std::min<int32_t>(nw, 64);
+    P.n_tiles = (nw + P.tile - 1) / P.tile;
+    const long long grid = (long long)units * P.n_tiles;
+    if (grid > 2147483647LL) return set_err(RAFTK_EINVAL, "ragged farm channel-stats: too many (farm, row, bin tile) blocks");
+    if (tile) {
+        const size_t smem = (size_t)R.n_max * tile * sizeof(double2);
+        static SmemOptIn opt(48 * 1024);
+        CUDA_TRY(opt.ensure(k_farm_channels_ragged<true>, smem));
+        k_farm_channels_ragged<true><<<(unsigned)grid, FARM_CH_T, smem, st>>>(P);
+    } else {
+        k_farm_channels_ragged<false><<<(unsigned)grid, FARM_CH_T, 0, st>>>(P);
+    }
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    // the output rows are farm after farm, [n_rows, n_ch_f] each: n_rows * n_ch rows in all, reduced as the uniform batch's
+    k_farm_channel_reduce<<<(unsigned)((size_t)n_rows * ch->n_ch), 128, 0, st>>>(nw, ch->dw, P.a2, ch->std, ch->psd);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_farm_ragged_channel_stats_host(int32_t n_farms, int32_t n_rows, int32_t nw, const int32_t *farm_fowt0,
+                                                    const int32_t *ch0, const double *w, const double *Xi_sys,
+                                                    const raftk_farm_channels *ch)
+{
+    RagChPlan R;
+    if (int rc = ragch_plan(n_farms, n_rows, nw, farm_fowt0, ch0, w, Xi_sys, ch, R)) return rc;
+    const size_t rows = (size_t)n_rows * ch->n_ch;
+    const size_t wb = raftk_farm_ragged_channel_stats_workspace_bytes(n_farms, n_rows, nw, farm_fowt0, ch0, ch);
+    raftk_farm_channels d = *ch;
+    const double *dW, *dXi;
+    char *ws;
+    Staging S("raftk_farm_ragged_channel_stats_host");
+    S.in(dW, w, nw); S.in(d.R, ch->R, R.n_r); S.in(dXi, Xi_sys, R.n_xi * 2);
+    S.out(d.std, rows, ch->std); S.out(d.psd, ch->psd ? rows * nw : 0, ch->psd); S.out(d.amp, ch->amp ? rows * nw * 2 : 0, ch->amp);
+    S.buf(ws, wb);
+    int rc;
+    if ((rc = S.commit()) || (rc = raftk_farm_ragged_channel_stats_dev(n_farms, n_rows, nw, farm_fowt0, ch0, dW, dXi, &d, ws, wb, nullptr)))
+        return rc;
     return S.finish();
 }
 

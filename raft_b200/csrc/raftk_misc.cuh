@@ -57,7 +57,47 @@ struct FarmPeerParams : FarmParams {
     int *I[RAFTK_MAX_PEERS];                    // [nF][nC][nw]
     int *S[RAFTK_MAX_PEERS];                    // [nF * N][nC][4]
 };
-template <bool PEER> using FarmArg = typename std::conditional<PEER, FarmPeerParams, FarmParams>::type;
+// A ragged batch (raftk_farm_ragged): one launch per kernel class over that class's farms, blockIdx.z (or the system walk)
+// indexing the class's run of descriptors.  A descriptor holds what a uniform batch derives from the farm index: the first
+// design, N, the offsets of the farm's Xi_sys / info rows and array matrices, and (k_farm_response_global) the panel width
+// glu_plan gives its 6N, so that every farm is factored exactly as a uniform batch of its N would factor it.
+struct FarmDesc {
+    int d0, N, pw, _pad;
+    size_t xo, io, ao;                          // complex elements of Xi, words of info, doubles of M_arr / B_arr / C_arr
+};
+struct FarmRagParams : FarmParams {
+    const FarmDesc *fd;                         // [nF]: this class's farms
+    size_t slab;                                // double2 elements between two CTAs' slabs (k_farm_response_global)
+};
+template <bool PEER, bool RAG = false>
+using FarmArg = typename std::conditional<RAG, FarmRagParams, typename std::conditional<PEER, FarmPeerParams, FarmParams>::type>::type;
+
+// Farm f of a launch: N, first design, array-matrix offset, the base of its Xi / info and its row there for case c.  A
+// uniform batch derives them from f (the expressions its kernels always used), a ragged one reads f's descriptor.
+template <bool RAG, class Prm> __device__ __forceinline__ int farm_n(const Prm &P, int f)
+{
+    if constexpr (RAG) return P.fd[f].N; else return P.N;
+}
+template <bool RAG, class Prm> __device__ __forceinline__ size_t farm_d0(const Prm &P, int f)
+{
+    if constexpr (RAG) return (size_t)P.fd[f].d0; else return (size_t)f * P.N;
+}
+template <bool RAG, class Prm> __device__ __forceinline__ size_t farm_ao(const Prm &P, int f)
+{
+    if constexpr (RAG) return P.fd[f].ao; else return (size_t)f * P.arr_stride;
+}
+template <bool RAG, class Prm> __device__ __forceinline__ double2 *farm_xi(const Prm &P, int f)
+{
+    if constexpr (RAG) return P.Xi + P.fd[f].xo; else return P.Xi;
+}
+template <bool RAG, class Prm> __device__ __forceinline__ int *farm_info(const Prm &P, int f)
+{
+    if constexpr (RAG) return P.info ? P.info + P.fd[f].io : nullptr; else return P.info;
+}
+template <bool RAG, class Prm> __device__ __forceinline__ size_t farm_row(const Prm &P, int f, int c)
+{
+    if constexpr (RAG) return (size_t)c; else return (size_t)f * P.nC + c;
+}
 
 // farm f's N status rows of case c to every rank's copy, spread over the gsize threads of a group
 __device__ __forceinline__ void farm_peer_status(const FarmPeerParams &P, int f, int c, int gtid, int gsize)
@@ -102,14 +142,14 @@ __device__ __forceinline__ void farm_op_terms(const DesignsDev &D, const CasesDe
 // A [n][nc] (nc = n + 1) and the right-hand side into its column n, spread over the gsize threads of a group.
 // OP: the case table carries operating points (cases.op) -- the farm kernels take it in instantiations of their own, so that
 // the calls without them compile as before.
-template <bool OP>
-__device__ __forceinline__ void farm_assemble(const DesignsDev &D, const CasesDev &Cs, const FarmParams &P, int farm, int c, int iw, double2 *A,
+template <bool OP, bool RAG = false, class Prm = FarmParams>
+__device__ __forceinline__ void farm_assemble(const DesignsDev &D, const CasesDev &Cs, const Prm &P, int farm, int c, int iw, double2 *A,
                                               int gtid, int gsize)
 {
-    const int n = 6 * P.N, nc = n + 1, nw = P.nw;
+    const int n = 6 * farm_n<RAG>(P, farm), nc = n + 1, nw = P.nw;
     const double w = D.w[iw], w2 = w * w;
     const int cp = Cs.primary ? Cs.primary[c] : c;                   // secondary wave trains use their primary's damping
-    const size_t d0 = (size_t)farm * P.N, ao = (size_t)farm * P.arr_stride;
+    const size_t d0 = farm_d0<RAG>(P, farm), ao = farm_ao<RAG>(P, farm);
     for (int t = gtid; t < n * n; t += gsize) {
         const int a = t / n, b = t % n, j = b / 6;
         const size_t i = d0 + a / 6;                                 // design of block row a
@@ -139,29 +179,33 @@ __device__ __forceinline__ void farm_assemble(const DesignsDev &D, const CasesDe
     }
 }
 
-template <bool WARP, bool OP = false, bool PEER = false>
-__global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(DesignsDev D, CasesDev Cs, FarmArg<PEER> P)
+// RAG: one class of a ragged batch, blockIdx.z indexing its descriptors; shared memory sized for the class's largest N
+template <bool WARP, bool OP = false, bool PEER = false, bool RAG = false>
+__global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(DesignsDev D, CasesDev Cs, FarmArg<PEER, RAG> P)
 {
+    static_assert(!(PEER && RAG), "ragged batches have no peer stores");
     extern __shared__ __align__(16) double smem_raw[];
     __shared__ int piv_s[FARM_WPC], bad_s[FARM_WPC];
     __shared__ double2 rinv_s[FARM_WPC];
-    const int n = 6 * P.N, nc = n + 1, nw = P.nw;
+    const int n = 6 * farm_n<RAG>(P, blockIdx.z), nc = n + 1, nw = P.nw;
     const int g = WARP ? (int)(threadIdx.x >> 5) : 0, gtid = WARP ? (int)(threadIdx.x & 31) : (int)threadIdx.x;
     const int gsize = WARP ? 32 : (int)blockDim.x;
     const int iw = WARP ? (int)(blockIdx.x * (blockDim.x >> 5)) + g : (int)blockIdx.x, c = blockIdx.y, f = blockIdx.z;
     if (iw >= nw) return;                                            // (warp-uniform; no CTA-wide barrier follows in the WARP variant)
     double2 *A = reinterpret_cast<double2 *>(smem_raw) + (size_t)g * n * nc;
-    const size_t u = (size_t)f * P.nC + c;                           // row of Xi and info
+    const size_t u = farm_row<RAG>(P, f, c);                         // row of Xi and info
     LuSlots S{&piv_s[g], &rinv_s[g], &bad_s[g]};
-    farm_assemble<OP>(D, Cs, P, f, c, iw, A, gtid, gsize);
+    farm_assemble<OP, RAG>(D, Cs, P, f, c, iw, A, gtid, gsize);
     constexpr int T = WARP ? 32 : 256;
     gsync<T>();
     int bad;
     if constexpr (WARP) bad = lu_unblocked<T>(A, n, nc, gtid, S);
     else bad = lu_blocked<T, false, false>(A, nc, A + n, nc, n, 1, 8, S);
     lu_back_subst<T>(A, nc, A + n, nc, n, 1, gtid);
-    for (int a = gtid; a < n; a += gsize) P.Xi[(u * n + a) * nw + iw] = A[a * nc + n];
-    if (gtid == 0 && P.info) P.info[u * nw + iw] = bad;
+    double2 *Xi = farm_xi<RAG>(P, f);
+    int *info = farm_info<RAG>(P, f);
+    for (int a = gtid; a < n; a += gsize) Xi[(u * n + a) * nw + iw] = A[a * nc + n];
+    if (gtid == 0 && info) info[u * nw + iw] = bad;
     if constexpr (PEER) farm_peer_store(P, A, nc, u, iw, bad, f, c, gtid, gsize);
 }
 
@@ -176,26 +220,48 @@ __global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(De
 #define GLU_PWMAX 16
 
 // farm system response of k_farm_response (same assembly) for any N: persistent CTAs, CTA b owns slab b of the workspace
-// ([6N][6N+1] double2) and solves the (farm, case, frequency) systems b, b + gridDim.x, ... of the nF * nC * nw in all
-template <bool OP = false>
-__global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D, CasesDev Cs, FarmParams P, double2 *ws, int pw)
+// ([6N][6N+1] double2) and solves the (farm, case, frequency) systems b, b + gridDim.x, ... of the nF * nC * nw in all.
+// RAG: the farms of one class of a ragged batch, each with its own N and panel width (its descriptor); slabs P.slab elements
+// apart (the class's largest N) and the panel sized for the largest n * pw by the launch
+template <bool OP = false, bool RAG = false>
+__global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D, CasesDev Cs, FarmArg<false, RAG> P, double2 *ws, int pw)
 {
     extern __shared__ __align__(16) double smem_raw[];
     __shared__ LuStaged<GLU_T, GLU_PWMAX> S;
     double2 *Ps = reinterpret_cast<double2 *>(smem_raw);
-    const int n = 6 * P.N, nc = n + 1, nw = P.nw;
-    double2 *A = ws + (size_t)blockIdx.x * n * nc;
-    const long long nsys = (long long)P.nF * P.nC * nw;
-    for (long long s = blockIdx.x; s < nsys; s += gridDim.x) {
-        const long long u = s / nw;                                    // f * nC + c: row of Xi and info
-        const int iw = (int)(s - u * nw), f = (int)(u / P.nC), c = (int)(u - (long long)f * P.nC);
-        farm_assemble<OP>(D, Cs, P, f, c, iw, A, threadIdx.x, GLU_T);
-        __syncthreads();
-        const int bad = lu_blocked<GLU_T, true, false>(A, nc, A + n, nc, n, 1, pw, S, Ps);
-        lu_back_subst<GLU_T>(A, (size_t)nc, A + n, (size_t)nc, n, 1, threadIdx.x);
-        for (int a = threadIdx.x; a < n; a += GLU_T) P.Xi[((size_t)u * n + a) * nw + iw] = A[(size_t)a * nc + n];
-        if (threadIdx.x == 0 && P.info) P.info[(size_t)u * nw + iw] = bad;
-        __syncthreads();                                               // the slab is rewritten by the next system
+    if constexpr (RAG) {
+        const int nw = P.nw;
+        double2 *A = ws + (size_t)blockIdx.x * P.slab;
+        const long long nsys = (long long)P.nF * P.nC * nw;
+        for (long long s = blockIdx.x; s < nsys; s += gridDim.x) {
+            const long long fc = s / nw;                               // f * nC + c of the class
+            const int iw = (int)(s - fc * nw), f = (int)(fc / P.nC), c = (int)(fc - (long long)f * P.nC);
+            const int n = 6 * P.fd[f].N, nc = n + 1;
+            double2 *Xi = farm_xi<true>(P, f);
+            int *info = farm_info<true>(P, f);
+            farm_assemble<OP, true>(D, Cs, P, f, c, iw, A, threadIdx.x, GLU_T);
+            __syncthreads();
+            const int bad = lu_blocked<GLU_T, true, false>(A, nc, A + n, nc, n, 1, P.fd[f].pw, S, Ps);
+            lu_back_subst<GLU_T>(A, (size_t)nc, A + n, (size_t)nc, n, 1, threadIdx.x);
+            for (int a = threadIdx.x; a < n; a += GLU_T) Xi[((size_t)c * n + a) * nw + iw] = A[(size_t)a * nc + n];
+            if (threadIdx.x == 0 && info) info[(size_t)c * nw + iw] = bad;
+            __syncthreads();                                           // the slab is rewritten by the next system
+        }
+    } else {
+        const int n = 6 * P.N, nc = n + 1, nw = P.nw;
+        double2 *A = ws + (size_t)blockIdx.x * n * nc;
+        const long long nsys = (long long)P.nF * P.nC * nw;
+        for (long long s = blockIdx.x; s < nsys; s += gridDim.x) {
+            const long long u = s / nw;                                    // f * nC + c: row of Xi and info
+            const int iw = (int)(s - u * nw), f = (int)(u / P.nC), c = (int)(u - (long long)f * P.nC);
+            farm_assemble<OP>(D, Cs, P, f, c, iw, A, threadIdx.x, GLU_T);
+            __syncthreads();
+            const int bad = lu_blocked<GLU_T, true, false>(A, nc, A + n, nc, n, 1, pw, S, Ps);
+            lu_back_subst<GLU_T>(A, (size_t)nc, A + n, (size_t)nc, n, 1, threadIdx.x);
+            for (int a = threadIdx.x; a < n; a += GLU_T) P.Xi[((size_t)u * n + a) * nw + iw] = A[(size_t)a * nc + n];
+            if (threadIdx.x == 0 && P.info) P.info[(size_t)u * nw + iw] = bad;
+            __syncthreads();                                               // the slab is rewritten by the next system
+        }
     }
 }
 
@@ -223,9 +289,10 @@ __global__ void __launch_bounds__(GLU_T, 2) k_system_solve_global(int n, int nw,
 // entry moves the pivot row to everybody and old row k to the pivot's lane, every row below k eliminates itself.  No shared
 // memory, no barriers; back substitution broadcasts one unknown per step.  Same assembly arithmetic as k_farm_response.
 // ------------------------------------------------------------------------------------------------
-template <int N6, bool OP = false, bool PEER = false>
-__global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, FarmArg<PEER> P)
+template <int N6, bool OP = false, bool PEER = false, bool RAG = false>
+__global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, FarmArg<PEER, RAG> P)
 {
+    static_assert(!(PEER && RAG), "ragged batches have no peer stores");
     constexpr int LPS = N6 <= 16 ? 16 : 32, SPW = 32 / LPS, NC = N6 + 1;
     const int nw = P.nw, lane = threadIdx.x & 31, r = lane & (LPS - 1);
     const int sys = ((int)blockIdx.x * ((int)blockDim.x >> 5) + ((int)threadIdx.x >> 5)) * SPW + lane / LPS;
@@ -237,7 +304,8 @@ __global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, Fa
     const double w = D.w[iw], w2 = w * w;
     const int cp = Cs.primary ? Cs.primary[c] : c;
     const int ib = a / 6, ea = a - 6 * ib;             // block row of the system; its design is FOWT ib of farm f
-    const size_t i = (size_t)f * P.N + ib, ao = (size_t)f * P.arr_stride, u = (size_t)f * P.nC + c;
+    // (a ragged class of this kernel holds farms with 6N = N6 only)
+    const size_t i = farm_d0<RAG>(P, f) + ib, ao = farm_ao<RAG>(P, f), u = farm_row<RAG>(P, f, c);
     double2 row[NC];
 #pragma unroll
     for (int b = 0; b < N6; b++) {
@@ -321,8 +389,10 @@ __global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, Fa
             row[N6].y -= pv.x * xk.y + pv.y * xk.x;
         }
     });
-    if (live && row_ok) P.Xi[(u * N6 + r) * nw + iw] = x;
-    if (live && r == 0 && P.info) P.info[u * nw + iw] = bad;
+    double2 *Xi = farm_xi<RAG>(P, f);
+    int *info = farm_info<RAG>(P, f);
+    if (live && row_ok) Xi[(u * N6 + r) * nw + iw] = x;
+    if (live && r == 0 && info) info[u * nw + iw] = bad;
     if constexpr (PEER) {                              // as farm_peer_store, from the lanes' registers
         if (live) {
 #pragma unroll 1
@@ -345,6 +415,27 @@ __global__ void __launch_bounds__(256) k_farm_publish(FarmPeerParams P)
     if (double2 *x = P.X[p]) for (size_t t = t0; t < nx; t += stride) x[t] = P.Xi[t];
     if (int *d = P.I[p]) for (size_t t = t0; t < ni; t += stride) d[t] = P.info[t];
     if (int *d = P.S[p]) for (size_t t = t0; t < ns; t += stride) d[t] = P.status[t];
+}
+
+// K3f: a rank's farms of a ragged batch (raftk_farm_ragged_response_gather_dev) to the other ranks' copies after their solve.
+// The rank's farms are contiguous, so their Xi_sys, info and per-FOWT status are three contiguous runs, stored at the same
+// offsets of every copy: blockIdx.y = p; Xi_sys and info where X[p] / I[p] are set, the status rows to every S[p]
+struct FarmFlatPeer {
+    int n_peers;
+    size_t nx, ni, ns;                          // complex elements of Xi_sys, info words, status words of this rank's farms
+    const double2 *Xi;
+    const int *info, *status;
+    double2 *X[RAFTK_MAX_PEERS];
+    int *I[RAFTK_MAX_PEERS];
+    int *S[RAFTK_MAX_PEERS];
+};
+__global__ void __launch_bounds__(256) k_farm_publish_flat(FarmFlatPeer P)
+{
+    const int p = blockIdx.y;
+    const size_t stride = (size_t)gridDim.x * 256, t0 = (size_t)blockIdx.x * 256 + threadIdx.x;
+    if (double2 *x = P.X[p]) for (size_t t = t0; t < P.nx; t += stride) x[t] = P.Xi[t];
+    if (int *d = P.I[p]) for (size_t t = t0; t < P.ni; t += stride) d[t] = P.info[t];
+    if (int *d = P.S[p]) for (size_t t = t0; t < P.ns; t += stride) d[t] = P.status[t];
 }
 
 // std = sqrt(1/2 sum_w |Y|^2) of one 128-thread CTA from each thread's partial sum s: warp shuffles, then the four warps
@@ -471,6 +562,46 @@ struct FarmChParams {
     unsigned wbits[RAFTK_FARM_CH_MAX / 16];
 };
 
+// A ragged batch's farm (raftk_farm_ragged_channel_stats_*): its n = 6N_f, channel count and first channel, and where its
+// Xi_sys block (complex elements) and R_f (doubles) start.  Its output rows start at n_rows * ch0.
+struct FarmChDesc {
+    int n, nch, ch0, _pad;
+    size_t xo, ro;
+};
+struct FarmChRagParams : FarmChParams {
+    const FarmChDesc *fd;                               // [F]
+};
+template <bool RAG> using FarmChArg = typename std::conditional<RAG, FarmChRagParams, FarmChParams>::type;
+// Farm f's n, channel count, Xi tile base, R_f and first output row for row fr = f * n_rows + r; a uniform batch derives them
+// from P (the expressions its kernel always used), a ragged one from f's descriptor
+template <bool RAG, class Prm> __device__ __forceinline__ int farmch_n(const Prm &P, int f)
+{
+    if constexpr (RAG) return P.fd[f].n; else return P.n;
+}
+template <bool RAG, class Prm> __device__ __forceinline__ int farmch_nch(const Prm &P, int f)
+{
+    if constexpr (RAG) return P.fd[f].nch; else return P.nch;
+}
+template <bool RAG, class Prm> __device__ __forceinline__ const double2 *farmch_xi(const Prm &P, size_t fr, int f, int i0)
+{
+    if constexpr (RAG) return P.Xi + P.fd[f].xo + (fr - (size_t)f * P.n_rows) * P.fd[f].n * P.nw + i0;
+    else return P.Xi + fr * (size_t)P.n * P.nw + i0;
+}
+template <bool RAG, class Prm> __device__ __forceinline__ const double *farmch_r(const Prm &P, int f)
+{
+    if constexpr (RAG) return P.R + P.fd[f].ro; else return P.R + (size_t)f * P.r_stride;
+}
+template <bool RAG, class Prm> __device__ __forceinline__ size_t farmch_row0(const Prm &P, size_t fr, int f)
+{
+    if constexpr (RAG) return (size_t)P.n_rows * P.fd[f].ch0 + (fr - (size_t)f * P.n_rows) * P.fd[f].nch;
+    else return fr * P.nch;
+}
+template <bool RAG, class Prm> __device__ __forceinline__ int farmch_ch0(const Prm &P, int f)
+{
+    if constexpr (RAG) return P.fd[f].ch0; else return 0;
+}
+struct XiTileShape { int n, nw; };
+
 template <bool SMEM>
 __global__ void __launch_bounds__(FARM_CH_T) k_farm_channels(const __grid_constant__ FarmChParams P)
 {
@@ -510,6 +641,55 @@ __global__ void __launch_bounds__(FARM_CH_T) k_farm_channels(const __grid_consta
             if (p == 2) { const double w2 = P.w[iw] * P.w[iw]; re *= w2; im *= w2; }
             else if (p == 1) { const double w1 = P.w[iw]; re *= w1; im *= w1; }
             const size_t o = (fr * P.nch + ch) * P.nw + iw;
+            P.a2[o] = re * re + im * im;
+            if (P.amp) P.amp[o] = make_double2(re, im);
+        }
+    }
+}
+
+// k_farm_channels for a ragged batch (raftk_farm_ragged_channel_stats_*): one tile width for every farm (the largest n's),
+// each farm's n, channels and offsets from its descriptor, the same per-channel arithmetic.  Kept apart from k_farm_channels
+// so that the uniform kernel compiles as before.
+template <bool SMEM, bool RAG = true>
+__global__ void __launch_bounds__(FARM_CH_T) k_farm_channels_ragged(const __grid_constant__ FarmChRagParams P)
+{
+    extern __shared__ double2 xs[];                     // [n][tw] when SMEM
+    const int tid = threadIdx.x;
+    const int t = (int)(blockIdx.x % (unsigned)P.n_tiles);
+    const size_t fr = blockIdx.x / (unsigned)P.n_tiles;    // farm * n_rows + row
+    const int f = (int)(fr / (size_t)P.n_rows);
+    const int i0 = t * P.tile, tw = min(P.tile, P.nw - i0);
+    const double2 *x = farmch_xi<RAG>(P, fr, f, i0);
+    const int n = farmch_n<RAG>(P, f), nch = farmch_nch<RAG>(P, f);
+    stage_xi_tile<SMEM, FARM_CH_T>(XiTileShape{n, P.nw}, xs, x, tw, tid);
+    // a thread computes FARM_CH_B channels of one bin: each Xi value read feeds FARM_CH_B independent chains (every chain
+    // still runs over b = 0..n-1 in order); a warp's threads share their channels, so the R loads are broadcasts
+    const double *Rf = farmch_r<RAG>(P, f);
+    const int nchb = (nch + FARM_CH_B - 1) / FARM_CH_B;
+    for (int k = tid; k < nchb * tw; k += FARM_CH_T) {
+        const int c0 = (k / tw) * FARM_CH_B, i = k - (k / tw) * tw;
+        const double *r[FARM_CH_B];
+        double yr[FARM_CH_B], yi[FARM_CH_B];
+#pragma unroll
+        for (int j = 0; j < FARM_CH_B; j++) { r[j] = Rf + (size_t)min(c0 + j, nch - 1) * n; yr[j] = 0.0; yi[j] = 0.0; }
+        for (int b = 0; b < n; b++) {
+            const double2 v = SMEM ? xs[b * tw + i] : x[(size_t)b * P.nw + i];
+#pragma unroll
+            for (int j = 0; j < FARM_CH_B; j++) {
+                const double c = r[j][b];
+                yr[j] = fma(c, v.x, yr[j]); yi[j] = fma(c, v.y, yi[j]);
+            }
+        }
+        const int iw = i0 + i;
+#pragma unroll
+        for (int j = 0; j < FARM_CH_B; j++) {
+            const int ch = c0 + j, cw = farmch_ch0<RAG>(P, f) + ch;
+            if (ch >= nch) break;
+            double re = yr[j], im = yi[j];
+            const int p = (P.wbits[cw >> 4] >> ((cw & 15) * 2)) & 3;
+            if (p == 2) { const double w2 = P.w[iw] * P.w[iw]; re *= w2; im *= w2; }
+            else if (p == 1) { const double w1 = P.w[iw]; re *= w1; im *= w1; }
+            const size_t o = (farmch_row0<RAG>(P, fr, f) + ch) * P.nw + iw;
             P.a2[o] = re * re + im * im;
             if (P.amp) P.amp[o] = make_double2(re, im);
         }

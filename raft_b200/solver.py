@@ -15,7 +15,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from ._lib import (RaftkCases, RaftkDesigns, RaftkFarm, RaftkFarmBatch, RaftkGeneral, RaftkGeneralBatch, RaftkGeneralFd, RaftkGeneralQtf, RaftkOutputs, RaftkSlender, RaftkSlenderBatch,
+from ._lib import (RaftkCases, RaftkDesigns, RaftkFarm, RaftkFarmBatch, RaftkFarmRagged, RaftkGeneral, RaftkGeneralBatch, RaftkGeneralFd, RaftkGeneralQtf, RaftkOutputs, RaftkSlender, RaftkSlenderBatch,
                    RaftkSlenderOutputs, RaftkSolveOpts, check, lib)
 
 _F8 = np.float64
@@ -537,6 +537,112 @@ def solve_dynamics_farm_batch(batch, cases, n_fowt, C_arr=None, M_arr=None, B_ar
         raise ValueError("n_fowt must divide the batch's %d designs" % batch.n_designs)
     return _solve_farms(batch, cases, N, batch.n_designs // N, M_arr, B_arr, C_arr, _opts(n_iter, tol, xi_start, cluster_size), want,
                         out)
+
+
+def ragged_offsets(farm_sizes):
+    """The CSR arrays of a ragged farm batch: -> (farm_fowt0 int32 [F+1], the first design of each farm and n_designs last;
+    arr_offset int64 [F+1], the first double of each farm's [6N_f,6N_f] array matrix in the packed M_arr / B_arr / C_arr)."""
+    N = np.asarray(farm_sizes, dtype=np.int64).reshape(-1)
+    fowt0 = np.zeros(len(N) + 1, dtype=np.int32)
+    fowt0[1:] = np.cumsum(N)
+    arr = np.zeros(len(N) + 1, dtype=np.int64)
+    arr[1:] = np.cumsum(36 * N * N)
+    return fowt0, arr
+
+
+def ragged_views(Xi_flat, farm_sizes, n_cases, nw):
+    """Farm f's [nC, 6N_f, nw] block of a ragged batch's flat Xi_sys (numpy or torch), as views of ``Xi_flat``: farm f starts at
+    6 nC nw farm_fowt0[f] complex values."""
+    fowt0, _ = ragged_offsets(farm_sizes)
+    per = 6 * n_cases * nw
+    return [Xi_flat[per * int(a):per * int(b)].reshape(n_cases, 6 * (int(b) - int(a)), nw) for a, b in zip(fowt0[:-1], fowt0[1:])]
+
+
+def _ragged_matrices(farm_sizes, M_arr, B_arr, C_arr):
+    """The array matrices of a ragged batch -> (dict name -> C-contiguous float64 array, arr_shared): each given matrix is a
+    list of F matrices [6N_f,6N_f], packed farm after farm; when every N_f is the same N it may also be one [6N,6N] set for
+    every farm or a stacked [F,6N,6N] (one per farm), as the uniform batch takes them."""
+    sizes = [int(n) for n in farm_sizes]
+    mats, shared = {}, set()
+    for nm, v in (("M_arr", M_arr), ("B_arr", B_arr), ("C_arr", C_arr)):
+        if v is None:
+            continue
+        if not isinstance(v, (list, tuple)):
+            a, n = np.asarray(v), 6 * sizes[0]
+            equal = len(set(sizes)) == 1
+            if equal and a.shape == (len(sizes), n, n):
+                v = list(a)
+            elif not (equal and a.shape == (n, n)):
+                raise ValueError("%s: a list of %d matrices [6N_f, 6N_f] in farm order, or with every N_f = N one [6N, 6N] set "
+                                 "or a stacked [F, 6N, 6N]; got shape %s for sizes %s" % (nm, len(sizes), a.shape, sizes))
+        if isinstance(v, (list, tuple)):
+            if len(v) != len(sizes) or any(np.shape(m) != (6 * n, 6 * n) for m, n in zip(v, sizes)):
+                raise ValueError("%s: a list of %d matrices [6N_f, 6N_f] in farm order" % (nm, len(sizes)))
+            mats[nm] = np.concatenate([np.ascontiguousarray(m, dtype=_F8).reshape(-1) for m in v])
+            shared.add(0)
+        else:
+            mats[nm] = np.ascontiguousarray(v, dtype=_F8)
+            shared.add(1)
+    if len(shared) > 1:
+        raise ValueError("M_arr, B_arr and C_arr must all be shared [6N,6N] sets or all be per-farm lists")
+    return mats, (1 if shared == {1} else 0)
+
+
+def _ragged_setup(farm_sizes, nC, nw, M_arr, B_arr, C_arr, out=None, device=None):
+    """A ragged batch as raftk_farm_ragged takes it -> (RaftkFarmRagged, arrays to keep alive, Xi_sys flat, info [F,nC,nw]).
+    Host arrays, or with ``device`` torch tensors there (the CSR arrays stay on the host either way)."""
+    fowt0, arr = ragged_offsets(farm_sizes)
+    mats, shared = _ragged_matrices(farm_sizes, M_arr, B_arr, C_arr)
+    F, nD = len(fowt0) - 1, int(fowt0[-1])
+    res = dict(Xi_sys=([6 * nD * nC * nw], _C16), info=([F, nC, nw], _I4))
+    if device is None:
+        ptr = lambda a: a.ctypes.data   # noqa: E731
+        for k, (shape, dt) in res.items():
+            a = (out or {}).get(k)
+            if a is not None and (a.shape != tuple(shape) or a.dtype != dt or not a.flags.c_contiguous):
+                raise ValueError("out[%r] must be a C-contiguous %s array %s" % (k, np.dtype(dt).name, shape))
+            res[k] = np.zeros(shape, dt) if a is None else a
+    else:
+        import torch
+        ptr = lambda t: t.data_ptr()    # noqa: E731
+        mats = {nm: torch.from_numpy(a).to(device) for nm, a in mats.items()}
+        res = {k: _torch_zeros(device)(*v) for k, v in res.items()}
+    f = RaftkFarmRagged()
+    f.n_farms, f.arr_shared = F, shared
+    f.farm_fowt0, f.arr_offset = fowt0.ctypes.data, arr.ctypes.data
+    for nm in ("M_arr", "B_arr", "C_arr"):
+        setattr(f, nm, ptr(mats[nm]) if nm in mats else None)
+    f.Xi_sys, f.info = ptr(res["Xi_sys"]), ptr(res["info"])
+    return f, (fowt0, arr, mats), res["Xi_sys"], res["info"]
+
+
+def solve_dynamics_farm_ragged(batch, cases, farm_sizes, C_arr=None, M_arr=None, B_arr=None, n_iter=10, tol=0.01, xi_start=0.0,
+                               cluster_size=0, want=("Xi", "status", "B_drag"), out=None):
+    """``solve_dynamics_farm`` for farms of different sizes in ONE call (array-size and layout studies): farm f has
+    ``farm_sizes[f]`` FOWTs, the designs of ``batch`` are every farm's FOWTs in order, farm after farm, all farms over the same
+    case table.  Array matrices: one [6N,6N] set for every farm (only when all sizes are equal), or lists of F matrices
+    [6N_f,6N_f].  -> the per-FOWT output dict plus ``Xi_sys``, a list of per-farm complex [nC, 6N_f, nw] views of the flat
+    buffer ``Xi_sys_flat``, and ``info`` [F, nC, nw]; farm f's arrays are what ``solve_dynamics_farm`` returns for that farm
+    alone, bit for bit.  ``out``: caller-owned per-FOWT arrays, ``Xi_sys`` (flat) and ``info``."""
+    cases.check_ops(batch)
+    nC, nw = cases.n_cases, batch.nw
+    f, keep, xi, info = _ragged_setup(farm_sizes, nC, nw, M_arr, B_arr, C_arr, out)
+    want = tuple(dict.fromkeys(tuple(want) + ("Xi", "status")))
+    outs = dict(out) if out is not None else {}
+    outs.update(_alloc_outputs(batch.n_designs, nC, nw, tuple(k for k in want if k not in outs and k not in ("Xi_sys", "info"))))
+    outs.pop("Xi_sys", None)
+    c = _host_struct(cases)
+    o = _opts(n_iter, tol, xi_start, cluster_size)
+    os_ = _out_struct(outs, lambda a: a.ctypes.data)
+
+    def run(b):
+        check(lib.raftk_solve_dynamics_farm_ragged_host(C.byref(_host_struct(b)), C.byref(c), C.byref(o), C.byref(os_), C.byref(f)))
+        return outs
+    res = _retry_on_plan(batch, run)
+    del keep
+    res["Xi_sys_flat"], res["info"] = xi, info
+    res["Xi_sys"] = ragged_views(xi, farm_sizes, nC, nw)
+    return res
 
 
 FLAG_NAN, FLAG_SINGULAR, FLAG_PLAN, FLAG_XCHG = 1, 2, 4, 8        # include/raftk.h RAFTK_FLAG_*
@@ -1310,8 +1416,78 @@ def farm_channel_stats(R, Xi_sys, dw, w=None, wpow=None, psd=True, amp=False, ti
     ``Xi_sys`` had none.  Bit-identical to ``general_channel_stats`` on the same R and Xi.  Several wave trains of a case:
     ``combine_trains``.  ``tile_w``: bins per CTA (0 automatic; -1 reads Xi_sys from L2), the results do not depend on it.
     With ``Xi_sys`` a torch CUDA tensor (a resident response, e.g. ``sweep.ShardedFarmSolve.step``'s gathered ``Xi_sys``) it runs
-    raftk_farm_channel_stats_dev on torch's current stream instead and returns torch tensors."""
+    raftk_farm_channel_stats_dev on torch's current stream instead and returns torch tensors.
+    A ragged batch (``solve_dynamics_farm_ragged``): ``Xi_sys`` the list of per-farm [nR,6N_f,nw] views and ``R`` a list of
+    [nch_f,6N_f] -> lists of per-farm results, each farm's as this function returns for that farm alone."""
+    if isinstance(Xi_sys, (list, tuple)):
+        return _farm_ragged_channel_stats(_buffers_for(Xi_sys[0]), R, Xi_sys, dw, w, wpow, psd, amp, tile_w)
     return _farm_channel_stats(_buffers_for(Xi_sys), R, Xi_sys, dw, w, wpow, psd, amp, tile_w)
+
+
+def _ptr_of(a):
+    return a.data_ptr() if hasattr(a, "data_ptr") else a.__array_interface__["data"][0]
+
+
+def _contiguous_run(views):
+    """Whether complex128 ``views`` (numpy or torch) lie back to back, in order, in one buffer."""
+    for k, v in enumerate(views):
+        if hasattr(v, "data_ptr"):
+            ok, nb = v.is_contiguous() and str(v.dtype) == "torch.complex128", v.numel() * 16
+        else:
+            ok, nb = v.flags.c_contiguous and v.dtype == _C16, v.nbytes
+        if not ok or (k + 1 < len(views) and _ptr_of(views[k + 1]) != _ptr_of(v) + nb):
+            return False
+    return True
+
+
+def _farm_ragged_channel_stats(be, R, views, dw, w, wpow, psd, amp, tile_w):
+    """``farm_channel_stats`` of a ragged batch (raftk_farm_ragged_channel_stats_*): ``views`` the per-farm [nR,6N_f,nw] arrays
+    (one flat buffer, as ``solve_dynamics_farm_ragged`` returns them, is read in place; otherwise they are packed), ``R`` a
+    list of [nch_f,6N_f], ``wpow`` None or a list of [nch_f] -> lists of per-farm (std [nR,nch_f], PSD, amplitudes)."""
+    F = len(views)
+    if not isinstance(R, (list, tuple)) or len(R) != F:
+        raise ValueError("a ragged Xi_sys (a list of per-farm views) takes a list of one R per farm")
+    if any(v.ndim != 3 or v.shape[0] != views[0].shape[0] or v.shape[2] != views[0].shape[2] or v.shape[1] % 6 for v in views):
+        raise ValueError("ragged Xi_sys: per-farm [nR, 6N_f, nw] arrays with one nR and nw")
+    nR, nw = int(views[0].shape[0]), int(views[0].shape[2])
+    sizes = [int(v.shape[1]) // 6 for v in views]
+    Rs = [np.ascontiguousarray(r, dtype=_F8) for r in R]
+    if any(r.ndim != 2 or r.shape[1] != 6 * n or r.shape[0] < 1 for r, n in zip(Rs, sizes)):
+        raise ValueError("R: a list of [nch_f, 6N_f] matrices, one per farm")
+    nch = [r.shape[0] for r in Rs]
+    ch0 = np.zeros(F + 1, dtype=_I4)
+    ch0[1:] = np.cumsum(nch)
+    wp = np.zeros(int(ch0[-1]), dtype=_I4) if wpow is None else np.concatenate([np.asarray(p, dtype=_I4).reshape(-1) for p in wpow])
+    if wp.shape != (int(ch0[-1]),):
+        raise ValueError("wpow: a list of [nch_f], one per farm")
+    _check_wpow(wp)
+    if not dw > 0:
+        raise ValueError("dw must be > 0")
+    ch = _lib.RaftkFarmChannels()
+    ch.n_ch, ch.R_shared, ch.wpow, ch.dw, ch.tile_w = int(ch0[-1]), 0, wp.ctypes.data, float(dw), int(tile_w)
+    fowt0, _ = ragged_offsets(sizes)
+    if _contiguous_run(views):
+        xi = views[0]
+    elif hasattr(views[0], "data_ptr"):
+        import torch
+        xi = torch.cat([v.reshape(-1).to(torch.complex128) for v in views])
+        be.reads.append(xi)                     # read by the enqueued launch
+    else:
+        xi = np.concatenate([np.asarray(v, dtype=_C16).reshape(-1) for v in views])
+    w = None if w is None else be.array(w, _F8)
+    if w is not None and tuple(w.shape) != (nw,):
+        raise ValueError("w must be [nw]")
+    Rd = be.array(np.concatenate([r.reshape(-1) for r in Rs]), _F8)
+    n_all = int(ch0[-1]) * nR
+    sd = be.empty([n_all])
+    P = be.empty([n_all * nw]) if psd else None
+    A = be.empty([n_all * nw], _C16) if amp else None
+    ch.R, ch.std, ch.psd, ch.amp = be.ptr(Rd), be.ptr(sd), be.ptr(P), be.ptr(A)
+    be.call("farm_ragged_channel_stats", F, nR, nw, fowt0.ctypes.data, ch0.ctypes.data, be.ptr(w), _ptr_of(xi), C.byref(ch),
+            ws=(F, nR, nw, fowt0.ctypes.data, ch0.ctypes.data, C.byref(ch)))
+    cut = lambda a, per: [a[nR * int(ch0[k]) * per:nR * int(ch0[k + 1]) * per].reshape(  # noqa: E731
+        (nR, nch[k]) + ((nw,) if per > 1 else ())) for k in range(F)]
+    return cut(sd, 1), (cut(P, nw) if psd else None), (cut(A, nw) if amp else None)
 
 
 def _farm_channel_stats(be, R, Xi_sys, dw, w, wpow, psd, amp, tile_w):
@@ -2479,15 +2655,22 @@ class DeviceSession:
                                                       C.byref(peers), self.workspace.data_ptr(), self.workspace_bytes, self._stream()))
             check(lib.raftk_peer_barrier_dev(C.byref(peers), timeout_flag, self._stream()))
 
-    def farm_response(self, C_arr=None, M_arr=None, B_arr=None, n_fowt=None):
+    def farm_response(self, C_arr=None, M_arr=None, B_arr=None, n_fowt=None, farm_sizes=None):
         """Enqueue the coupled 6N-DOF system response of the LAST ``solve`` (the session's designs are the FOWTs of the
         array; it must have been created with want including B_drag, F_drag, F_iner [+ F_BEM]).  -> (Xi_sys [nC,6N,nw], info).
         Any N: farms whose system does not fit in shared memory are solved in a device workspace sized once
         (raftk_farm_workspace_bytes) and kept with the session.
         ``n_fowt``: the session's designs are n_designs / n_fowt farms of n_fowt FOWTs each (design f * n_fowt + i is FOWT i
         of farm f), array matrices [6N,6N] for every farm or [F,6N,6N] -> (Xi_sys [F,nC,6N,nw], info [F,nC,nw]).  The
-        matrices, outputs and workspace of either form are set up on its first call and kept with the session."""
+        matrices, outputs and workspace of either form are set up on its first call and kept with the session.
+        ``farm_sizes``: the session's designs are farms of farm_sizes[f] FOWTs each, farm after farm (a ragged batch,
+        raftk_farm_ragged_response_ws_dev), array matrices as ``solve_dynamics_farm_ragged`` -> (Xi_sys, a list of per-farm
+        [nC,6N_f,nw] views of one flat tensor, info [F,nC,nw]); set up again when the sizes change."""
         torch = self.torch
+        if farm_sizes is not None:
+            if n_fowt is not None:
+                raise ValueError("farm_response: give n_fowt or farm_sizes, not both")
+            return self._farm_ragged(farm_sizes, M_arr, B_arr, C_arr)
         N = self.batch.n_designs if n_fowt is None else int(n_fowt)
         if N < 1 or self.batch.n_designs % N:
             raise ValueError("n_fowt must divide the session's %d designs" % self.batch.n_designs)
@@ -2496,6 +2679,45 @@ class DeviceSession:
         with torch.cuda.device(self.device):
             check(launch(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f), ws.data_ptr(), wsb, self._stream()))
         return xi, info
+
+    def _farm_ragged(self, farm_sizes, M_arr, B_arr, C_arr):
+        sizes = tuple(int(n) for n in farm_sizes)
+        if getattr(self, "_farm_rag", (None,))[0] != sizes:
+            with self.torch.cuda.device(self.device):
+                f, keep, xi, info = _ragged_setup(sizes, self.cases.n_cases, self.batch.nw, M_arr, B_arr, C_arr, device=self.device)
+                wsb = int(lib.raftk_farm_ragged_workspace_bytes(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(f)))
+                if wsb == 0:                # a shape raftk_farm_ragged refuses: its reason
+                    raise _lib.RaftkError("raftk error: %s" % lib.raftk_last_error().decode("utf-8", "replace"))
+                ws = self.torch.empty(wsb, dtype=self.torch.uint8, device=self.device)
+            self._farm_rag = (sizes, f, keep, xi, info, ws, wsb, ragged_views(xi, sizes, self.cases.n_cases, self.batch.nw))
+        _, f, _, _, info, ws, wsb, views = self._farm_rag
+        with self.torch.cuda.device(self.device):
+            check(lib.raftk_farm_ragged_response_ws_dev(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct), C.byref(f),
+                                                        ws.data_ptr(), wsb, self._stream()))
+        return views, info
+
+    def farm_response_ragged_gather(self, peers, farm_row0, fowt_row0, n_farms_total, Xi_sys, info, farm_sizes, C_arr=None, M_arr=None,
+                                    B_arr=None):
+        """``farm_response(farm_sizes=...)`` of this rank's farms stored at their global offsets of every rank's copy
+        (raftk_farm_ragged_response_gather_dev; ``sweep.ShardedFarmSolve(farm_sizes=...)``): the session's designs are
+        designs [fowt_row0, ...) of the whole batch, farms [farm_row0, farm_row0 + len(farm_sizes)) of ``n_farms_total``;
+        ``Xi_sys`` (flat) and ``info`` [F_r,nC,nw] are their rows of this rank's own copy.  Follow with raftk_peer_barrier_dev."""
+        sizes = tuple(int(n) for n in farm_sizes)
+        if getattr(self, "_farm_rag_gather", (None,))[0] != sizes:
+            with self.torch.cuda.device(self.device):
+                f, keep, _, _ = _ragged_setup(sizes, self.cases.n_cases, self.batch.nw, M_arr, B_arr, C_arr, device=self.device)
+                wsb = int(lib.raftk_farm_ragged_workspace_bytes(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(f)))
+                if wsb == 0:
+                    raise _lib.RaftkError("raftk error: %s" % lib.raftk_last_error().decode("utf-8", "replace"))
+                ws = self.torch.empty(wsb, dtype=self.torch.uint8, device=self.device)
+            self._farm_rag_gather = (sizes, f, keep, ws, wsb)
+        _, f, _, ws, wsb = self._farm_rag_gather
+        g = RaftkFarmRagged.from_buffer_copy(f)
+        g.Xi_sys, g.info = Xi_sys.data_ptr(), info.data_ptr()
+        with self.torch.cuda.device(self.device):
+            check(lib.raftk_farm_ragged_response_gather_dev(C.byref(self.d_struct), C.byref(self.c_struct), C.byref(self.o_struct),
+                                                            C.byref(g), C.byref(peers), int(farm_row0), int(fowt_row0),
+                                                            int(n_farms_total), ws.data_ptr(), wsb, self._stream()))
 
     def _farm_setup(self, N, n_fowt, M_arr, B_arr, C_arr, gather=False):
         """The farm struct, matrices, outputs and workspace of ``farm_response``'s form ``n_fowt``, set up on first use;
@@ -2632,6 +2854,7 @@ def last_dispatch():
     check(lib.raftk_last_dispatch(C.byref(r)))
     d = {n: int(getattr(r, n)) for n, _ in r._fields_ if not n.startswith("_")}
     d["family"], d["kernel"] = DISPATCH_FAMILIES[d["family"]], DISPATCH_KERNELS[d["kernel"]]
+    d["farm_classes"] = tuple(DISPATCH_KERNELS[k] for k in range(len(DISPATCH_KERNELS)) if d["farm_classes"] >> k & 1)
     for n in ("f0_global", "direct_d2h", "trains"):
         d[n] = bool(d[n])
     return d

@@ -532,6 +532,71 @@ def gather_farm_shards(blocks, bounds, n_fowt, group=None):
     return tuple(out)
 
 
+def ragged_farm_cost(N):
+    """Estimated work of one farm of N FOWTs, per (case, bin): N per-FOWT solves plus one dense (6N)^3 factorisation."""
+    N = int(N)
+    return N + (6 * N) ** 3
+
+
+def ragged_farm_shards(sizes, world):
+    """Contiguous runs of whole farms of a ragged batch (farm f: ``sizes[f]`` FOWTs), one [lo, hi) per rank, that minimise the
+    largest rank's estimated work (``ragged_farm_cost``; every farm shares the case table and grid, so nC * nw drops out).
+    The bottleneck is found exactly: bisection over integer loads with a greedy fill, which is optimal for contiguous runs.
+    Ranks past the last farm get empty runs."""
+    cost = [ragged_farm_cost(n) for n in sizes]
+    world = int(world)
+    if world < 1:
+        raise ValueError("world must be >= 1")
+
+    def fill(cap):
+        bounds, lo, load = [], 0, 0
+        for f, c in enumerate(cost):
+            if load + c > cap and f > lo:
+                bounds.append((lo, f))
+                lo, load = f, 0
+            load += c
+        bounds.append((lo, len(cost)))
+        return bounds
+
+    lo, hi = max(cost, default=0), sum(cost)
+    while lo < hi:
+        mid = (lo + hi) // 2
+        if len(fill(mid)) <= world:
+            hi = mid
+        else:
+            lo = mid + 1
+    bounds = fill(lo) if cost else []
+    return bounds + [(len(cost), len(cost))] * (world - len(bounds))
+
+
+def _gather_rows(t, spans, group=None):
+    """Rows [a_r, b_r) of a tensor sharded by rank (``t``: this rank's rows) -> every rank's rows in order: padded to the
+    largest span, one ``all_gather_into_tensor``, padding dropped."""
+    import torch
+    import torch.distributed as dist
+    world, rmax = len(spans), max(1, max(b - a for a, b in spans))
+    pad = t.new_zeros((rmax,) + tuple(t.shape[1:]))
+    pad[:t.shape[0]].copy_(t)
+    if world > 1:
+        full = t.new_empty((world * rmax,) + tuple(t.shape[1:]))
+        dist.all_gather_into_tensor(full, pad, group=group)
+    else:
+        full = pad
+    idx = torch.cat([torch.arange(b - a) + r * rmax for r, (a, b) in enumerate(spans)])
+    return full.index_select(0, idx.to(full.device))
+
+
+def gather_ragged_farm_shards(blocks, bounds, farm_fowt0, group=None):
+    """The ``exchange="nccl"`` path of ``ShardedFarmSolve(farm_sizes=...)``: this rank's (Xi_sys [D_r, 6 nC nw] -- its farms'
+    flat Xi_sys in rows of one FOWT's length --, info [F_r,nC,nw], status [D_r,nC,4]) -> the whole batch's ([nD, 6 nC nw],
+    [F,nC,nw], [nD,nC,4]), every rank's rows at their global offsets.  ``bounds``: [lo, hi) farms of every rank
+    (``ragged_farm_shards``); ``farm_fowt0``: the batch's CSR of designs.  Backend-agnostic (NCCL on GPUs, gloo on CPU)."""
+    fowt0 = [int(v) for v in farm_fowt0]
+    dspans = [(fowt0[lo], fowt0[hi]) for lo, hi in bounds]
+    xi, info, st = blocks
+    return _gather_rows(xi, dspans, group), _gather_rows(info, list(bounds), group), _gather_rows(st, dspans, group)
+
+
 class ShardedFarmSolve:
     """A farm batch (``solver.solve_dynamics_farm_batch``) sharded over GPUs: rank r takes the whole farms
     ``farm_shards(F, world)[r]`` (a farm's coupled system stays on one GPU), runs its FOWTs' drag linearisation and its farms'
@@ -546,11 +611,19 @@ class ShardedFarmSolve:
     pointers (raftk_farm_batch_response_gather_dev; farms too large for shared memory are copied by k_farm_publish after their
     solve), then raftk_peer_barrier_dev; the copies hold F_max = the largest shard's farm count per rank.  ``exchange="nccl"``:
     ``gather_farm_shards`` instead; a peer exchange that cannot be set up (CUDA IPC unavailable) falls back to it on every
-    rank.  With one rank it is ``DeviceSession.farm_response(n_fowt=N)`` with the exchange's copies as outputs."""
+    rank.  With one rank it is ``DeviceSession.farm_response(n_fowt=N)`` with the exchange's copies as outputs.
+
+    ``farm_sizes`` instead of ``n_fowt``: a ragged batch (``solver.solve_dynamics_farm_ragged``), farm f of farm_sizes[f]
+    FOWTs, array matrices as that function takes them.  Rank r takes the whole farms ``ragged_farm_shards(farm_sizes,
+    world)[r]`` (balanced by estimated work), and every farm is stored at its global offset of every rank's copy, no padding:
+    ``exchange="peer"`` through raftk_farm_ragged_response_gather_dev (solve, then k_farm_publish_flat), ``"nccl"`` through
+    ``gather_ragged_farm_shards``.  ``step()`` -> (Xi_sys: per-farm [nC,6N_f,nw] views of one flat tensor, info [F,nC,nw],
+    status [nD,nC,4]), bit for bit what one ``solve_dynamics_farm_ragged`` call returns."""
 
     WANT = ("Xi", "status", "B_drag", "F_drag", "F_iner")
 
-    def __init__(self, designs, cases, n_fowt, C_arr=None, M_arr=None, B_arr=None, device=None, group=None, exchange="peer"):
+    def __init__(self, designs, cases, n_fowt=None, C_arr=None, M_arr=None, B_arr=None, device=None, group=None, exchange="peer",
+                 farm_sizes=None):
         import torch
         import torch.distributed as dist
         from . import solver
@@ -559,6 +632,11 @@ class ShardedFarmSolve:
         self.torch, self.dist, self.group = torch, dist, group
         batch = designs if isinstance(designs, solver.DesignBatch) else solver.DesignBatch(designs)
         ct = cases if isinstance(cases, solver.CaseTable) else solver.CaseTable(cases)
+        self.sizes = None
+        if farm_sizes is not None:
+            if n_fowt is not None:
+                raise ValueError("give n_fowt or farm_sizes, not both")
+            return self._init_ragged(batch, ct, farm_sizes, M_arr, B_arr, C_arr, device, group, exchange)
         N = self.N = int(n_fowt)
         if N < 1 or batch.n_designs % N:
             raise ValueError("n_fowt must divide the batch's %d designs" % batch.n_designs)
@@ -596,9 +674,79 @@ class ShardedFarmSolve:
                                    ints[R * self.nC * self.nw:].view(R * N, self.nC, 4)))
             self.keep = [farm_rows(self.bounds).to(self.device), farm_rows(self.bounds, N).to(self.device)]
 
+    def _init_ragged(self, batch, ct, farm_sizes, M_arr, B_arr, C_arr, device, group, exchange):
+        torch, dist = self.torch, self.dist
+        from . import solver
+        sizes = self.sizes = tuple(int(n) for n in farm_sizes)
+        fowt0 = self.fowt0 = [int(v) for v in solver.ragged_offsets(sizes)[0]]
+        if min(sizes, default=0) < 1 or fowt0[-1] != batch.n_designs:
+            raise ValueError("farm_sizes must be >= 1 and add up to the batch's %d designs" % batch.n_designs)
+        solver._ragged_matrices(sizes, M_arr, B_arr, C_arr)                  # the whole batch's matrices, checked once
+        ct.check_ops(batch)
+        on = dist.is_available() and dist.is_initialized()
+        self.world = dist.get_world_size(group) if on else 1
+        self.rank = dist.get_rank(group) if on else 0
+        self.F, self.nC, self.nw = len(sizes), ct.n_cases, batch.nw
+        self.bounds = ragged_farm_shards(sizes, self.world)
+        self.lo, self.hi = self.bounds[self.rank]
+        self.d_lo, self.d_hi = fowt0[self.lo], fowt0[self.hi]
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.sess, self.mats = None, {}
+        if self.hi > self.lo:
+            want = self.WANT + (("F_BEM",) if batch.n_bem_head else ())
+            self.sess = solver.DeviceSession(batch.take(self.d_lo, self.d_hi), shard_design_cases(ct, self.d_lo, self.d_hi),
+                                             device=self.device, want=want)
+            for k, v in (("M_arr", M_arr), ("B_arr", B_arr), ("C_arr", C_arr)):
+                if v is not None:                                              # a shared [6N,6N] set stays whole
+                    self.mats[k] = v if (not isinstance(v, (list, tuple)) and np.ndim(v) == 2) else list(v)[self.lo:self.hi]
+        self.px, self.exchange, self.fallback = None, exchange, None
+        nD, U = batch.n_designs, 6 * self.nC * self.nw
+        if exchange == "peer":
+            try:
+                self.px = PeerExchange(-(-nD // self.world), self.nw, self.device, group=group, dof=6 * self.nC,
+                                       status_elems=-(-(self.F * self.nC * self.nw + nD * self.nC * 4) // self.world))
+            except PeerSetupError as e:
+                self.fallback, self.exchange = str(e), "nccl"
+        if self.px is not None:
+            ni = self.F * self.nC * self.nw
+            self.views = [(self.px.gathered[b].reshape(-1)[:nD * U], self.px.status[b].reshape(-1)[:ni].view(self.F, self.nC, self.nw),
+                           self.px.status[b].reshape(-1)[ni:ni + nD * self.nC * 4].view(nD, self.nC, 4)) for b in range(len(self.px.peers))]
+
+    def _step_ragged(self, n_iter, tol, xi_start):
+        import ctypes as C
+        from . import solver
+        from ._lib import check, lib
+        torch, U = self.torch, 6 * self.nC * self.nw
+        m = self.hi - self.lo
+        with torch.cuda.device(self.device):
+            if self.sess is not None:
+                self.sess.solve(n_iter=n_iter, tol=tol, xi_start=xi_start)
+            if self.px is not None:
+                b, peers = self.px.next()
+                X, I, S = self.views[b]
+                if m:
+                    self.sess.farm_response_ragged_gather(peers, self.lo, self.d_lo, self.F, X[self.d_lo * U:self.d_hi * U], I[self.lo:self.hi],
+                                                          self.sizes[self.lo:self.hi], **self.mats)
+                check(lib.raftk_peer_barrier_dev(C.byref(peers), self.px.timeout.data_ptr(), torch.cuda.current_stream(self.device).cuda_stream))
+                X, I, S = X.clone(), I.clone(), S.clone()                  # the copy is rewritten two steps on
+            else:
+                if m:
+                    _, info = self.sess.farm_response(farm_sizes=self.sizes[self.lo:self.hi], **self.mats)
+                    blocks = (self.sess._farm_rag[3].view(-1, U), info, self.sess.out["status"])
+                else:
+                    blocks = (torch.zeros([0, U], dtype=torch.complex128, device=self.device),
+                              torch.zeros([0, self.nC, self.nw], dtype=torch.int32, device=self.device),
+                              torch.zeros([0, self.nC, 4], dtype=torch.int32, device=self.device))
+                X, I, S = gather_ragged_farm_shards(blocks, self.bounds, self.fowt0, self.group)
+                X = X.reshape(-1)
+            return solver.ragged_views(X, self.sizes, self.nC, self.nw), I, S
+
     def step(self, n_iter=10, tol=0.01, xi_start=0.0):
         """Enqueue the per-FOWT solve, the coupled solve and the exchange of this rank's farms on the current stream
-        -> (Xi_sys [F,nC,6N,nw], info [F,nC,nw], status [F*N,nC,4]) of the whole batch (device tensors, stream order)."""
+        -> (Xi_sys [F,nC,6N,nw], info [F,nC,nw], status [F*N,nC,4]) of the whole batch (device tensors, stream order); a
+        ragged batch (``farm_sizes``): (Xi_sys per-farm views, info, status) as the class documents."""
+        if self.sizes is not None:
+            return self._step_ragged(n_iter, tol, xi_start)
         import ctypes as C
         from ._lib import check, lib
         torch, N, m = self.torch, self.N, self.hi - self.lo

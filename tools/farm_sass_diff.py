@@ -1,20 +1,23 @@
 #!/usr/bin/env python
-"""Compare the SASS of two builds of the library, kernel by kernel (profiles/sm90a_farm_peer_sass.txt).
+"""Compare the SASS of two builds of the library, kernel by kernel (profiles/sm90a_farm_peer_sass.txt,
+profiles/sm90a_farm_ragged_sass.txt).
 
 The two inputs are `cuobjdump -sass` listings of raft_b200/csrc/raftk.cu compiled for sm_90a, one before and one after the
-farm kernels' PEER instantiations.  Kernels are matched by demangled name and template arguments, not by parameter types
-(the non-PEER instantiations now spell FarmParams through the FarmArg alias); a kernel that gained PEER as its last template
-argument is matched through its PEER = false instantiation.  Instruction text is compared with addresses and encodings
+farm kernels gained a template flag (--flag PEER: the peer-store instantiations; --flag RAG: the ragged-batch ones).
+Kernels are matched by demangled name and template arguments, not by parameter types (instantiations without the flag
+spell their parameter struct through the FarmArg alias); a kernel that gained the flag as its last template argument is
+matched through its flag = false instantiation.  Instruction text is compared with addresses and encodings
 dropped.  Each matched farm kernel, and any kernel that differs, prints SAME or DIFF with its instruction counts; kernels
 found on one side only are listed at the end.
 
-Usage:  python tools/farm_sass_diff.py BEFORE.sass AFTER.sass
+Usage:  python tools/farm_sass_diff.py [--flag PEER|RAG] BEFORE.sass AFTER.sass
 """
 import argparse
 import re
 import subprocess
 
-PEER_KERNELS = ("k_farm_response", "k_farm_rows")
+FLAG_KERNELS = {"PEER": ("k_farm_response", "k_farm_rows"), "RAG": ("k_farm_response", "k_farm_rows", "k_farm_response_global")}
+PEER_KERNELS = FLAG_KERNELS["PEER"]
 
 
 def functions(path):
@@ -38,20 +41,21 @@ def demangle(names):
     return dict(zip(names, res.stdout.splitlines()))
 
 
-def key(demangled, after):
-    """Kernel name and template arguments; on the after side a trailing PEER argument: (key, is_peer)."""
+def key(demangled, after, flagged=PEER_KERNELS):
+    """Kernel name and template arguments; on the after side a trailing flag argument: (key, flag is true)."""
     m = re.match(r"(?:void )?(\w+)(?:<(.*?)>)?\(", demangled)
     if not m:
         return demangled, False
     name, targs = m.group(1), [a.strip() for a in (m.group(2) or "").split(",") if a.strip()]
     peer = False
-    if after and name in PEER_KERNELS:
+    if after and name in flagged:
         peer = targs.pop() == "true"
     return "%s<%s>" % (name, ", ".join(targs)), peer
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--flag", choices=sorted(FLAG_KERNELS), default="PEER")
     ap.add_argument("before")
     ap.add_argument("after")
     args = ap.parse_args()
@@ -60,9 +64,9 @@ def main():
     b_by_key = {key(dm[n], False)[0]: n for n in before}
     a_by_key, peer_only = {}, []
     for n in after:
-        k, peer = key(dm[n], True)
+        k, peer = key(dm[n], True, FLAG_KERNELS[args.flag])
         if peer:
-            peer_only.append(k + " PEER")
+            peer_only.append(k + " " + args.flag)
         else:
             a_by_key[k] = n
     same = diff = 0
