@@ -780,7 +780,7 @@ int raftk_solve_dynamics_farm_ragged_host(const raftk_designs *d, const raftk_ca
  *     gathered[p]: complex Xi_sys, flat as raftk_farm_ragged's (n_ranks * peers.block_elems >= 6 nC nw n_designs_total)
  *     status[p]:   int32 info [n_farms_total, nC, nw], followed by the per-FOWT status [n_designs_total, nC, 4]
  * f describes this rank's farms (farm_fowt0 from 0, arr_offset from 0); f->Xi_sys and f->info must be their rows of this
- * rank's own copy.  The farms are solved as raftk_farm_ragged_response_ws_dev solves them (same bits), then k_farm_publish_flat
+ * rank's own copy.  The farms are solved as raftk_farm_ragged_response_ws_dev solves them (same bits), then k_farm_publish
  * copies the rank's three contiguous runs (Xi_sys, info, status) to the other copies; follow with raftk_peer_barrier_dev.
  * RAFTK_EINVAL before any launch, besides every refusal of raftk_farm_ragged_response_ws_dev: a bad raftk_peers, no info or
  * per-FOWT status, a rank's status pointer missing, farm rows outside [0, n_farms_total), copies too small for this rank's
@@ -799,11 +799,10 @@ int raftk_farm_ragged_response_gather_dev(const raftk_designs *d, const raftk_ca
  *     flags[p]:    the arrival flags of raftk_peer_barrier_dev.
  * raftk_farm_batch_response_gather_dev is raftk_farm_batch_response_ws_dev for this rank's f->n_farms farms, which are farms
  * [farm_row0, farm_row0 + n_farms) of the gathered copies (farm_row0 = rank * F_max); f->Xi_sys and f->info must be those rows of
- * this rank's own copy, and `solved` must carry the per-FOWT status of raftk_solve_dynamics_dev.  With the system in shared
- * memory or registers (N <= 20 on an H100) the solve kernel itself stores each finished (farm, case, bin) solution and info word
- * into the other ranks' copies; larger farms (k_farm_response_global, whose LU leaves Xi_sys final only at its end) are copied
- * by a second kernel, k_farm_publish, that this entry enqueues after the solve.  Either way the per-FOWT status rows of the
- * rank's farms go to every copy, and the results are identical to raftk_farm_batch_response_ws_dev's, bit for bit.  Follow with
+ * this rank's own copy, and `solved` must carry the per-FOWT status of raftk_solve_dynamics_dev.  The farms are solved as
+ * raftk_farm_batch_response_ws_dev solves them, then a second kernel, k_farm_publish, copies the rank's Xi_sys, info and
+ * per-FOWT status rows to the other ranks' copies (and the status rows to its own), so a call makes two launches whatever the
+ * farm size; the results are identical to raftk_farm_batch_response_ws_dev's, bit for bit.  Follow with
  * raftk_peer_barrier_dev; a rank without farms (more ranks than farms) calls only the barrier.
  * RAFTK_EINVAL before any launch, besides every refusal of raftk_farm_batch_response_ws_dev: NULL peers, n_ranks outside
  * [1, RAFTK_MAX_PEERS] or rank outside [0, n_ranks), a rank's gathered / flags / status pointer missing, no info or per-FOWT

@@ -973,248 +973,81 @@ extern "C" int raftk_system_solve_dev(int32_t n, int32_t nw, int32_t nrhs, doubl
     return RAFTK_OK;
 }
 
-// true when the shared-memory farm kernels take a farm of N FOWTs (6N <= 24: warp per system; else one CTA per system with
-// the [6N][6N+1] system in shared memory); false sends it to k_farm_response_global
-static bool farm_on_chip(int N)
-{
-    const int n = 6 * N;
-    return n <= 24 || smem_fits((size_t)n * (n + 1) * sizeof(double2), static_smem(k_farm_response<false>, SMEM_STATIC_FARM_BLOCK));
-}
-
-// workspace of k_farm_response_global: one [6N][6N+1] slab per resident CTA, no more slabs than (farm, case, frequency) systems
-static size_t farm_slab_bytes(int N) { return (size_t)6 * N * (6 * N + 1) * sizeof(double2); }
-static size_t farm_ws_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm_batch *f)
-{
-    if (!d || !c || !f || f->n_farms < 1 || f->n_fowt < 1 || d->nw < 1 || c->n_cases < 1 || farm_on_chip(f->n_fowt)) return 0;
-    const GluPlan g = glu_plan(6 * f->n_fowt);
-    const long long slabs = std::min<long long>((long long)f->n_farms * c->n_cases * d->nw, (long long)std::max(g.per_sm, 1) * sm_count());
-    return (size_t)slabs * farm_slab_bytes(f->n_fowt);
-}
-
-// one farm is a batch of one: its matrices are the shared set
-static raftk_farm_batch farm_as_batch(const raftk_farm *f)
-{
-    raftk_farm_batch b;
-    memset(&b, 0, sizeof(b));
-    b.n_farms = 1; b.n_fowt = f->n_fowt; b.arr_shared = 1;
-    b.M_arr = f->M_arr; b.B_arr = f->B_arr; b.C_arr = f->C_arr;
-    b.Xi_sys = f->Xi_sys; b.info = f->info;
-    return b;
-}
-
-extern "C" size_t raftk_farm_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm *f)
-{
-    if (!f) return 0;
-    const raftk_farm_batch b = farm_as_batch(f);
-    return farm_ws_bytes(d, c, &b);
-}
-
-extern "C" size_t raftk_farm_batch_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm_batch *f)
-{
-    return farm_ws_bytes(d, c, f);
-}
-
-// the shape of a farm batch against its designs (everything the host entry can refuse before it stages anything)
-static int farm_batch_shape(const raftk_designs *d, const raftk_farm_batch *f)
-{
-    if (f->n_farms < 1 || f->n_fowt < 1) return set_err(RAFTK_EINVAL, "farm batch: n_farms and n_fowt must be >= 1");
-    if ((long long)f->n_farms * f->n_fowt != d->n_designs)
-        return set_err(RAFTK_EINVAL, "farm batch: n_farms * n_fowt must equal designs.n_designs");
-    if (f->arr_shared != 0 && f->arr_shared != 1) return set_err(RAFTK_EINVAL, "farm batch: arr_shared must be 0 or 1");
-    if (!f->Xi_sys) return set_err(RAFTK_EINVAL, "farm batch: Xi_sys is required");
-    return RAFTK_OK;
-}
-
-// The farm response of a batch; with `px` (raftk_farm_batch_response_gather_dev) its peer fields are set and the results also go
-// to the other ranks: the shared-memory kernels through their PEER instantiations, k_farm_response_global through k_farm_publish.
-static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm_batch *f, void *ws,
-                       size_t ws_bytes, cudaStream_t st, const FarmPeerParams *px = nullptr)
-{
-    if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "farm response: null argument");
-    if (int rc = farm_batch_shape(d, f)) return rc;
-    if (!solved->B_drag || !solved->F_drag || !solved->F_iner)
-        return set_err(RAFTK_EINVAL, "farm response needs B_drag, F_drag, F_iner of the per-FOWT solve");
-    if (d->n_bem_head > 0 && !solved->F_BEM) return set_err(RAFTK_EINVAL, "farm response: the designs carry BEM excitation, F_BEM is required");
-    const int n = 6 * f->n_fowt;
-    FarmPeerParams Q = px ? *px : FarmPeerParams{};
-    FarmParams &P = Q;
-    P.N = f->n_fowt; P.nC = c->n_cases; P.nw = d->nw; P.nF = f->n_farms;
-    P.arr_stride = f->arr_shared ? 0 : (size_t)n * n;
-    P.B_drag = solved->B_drag;
-    P.F_drag = reinterpret_cast<const double2 *>(solved->F_drag);
-    P.F_iner = reinterpret_cast<const double2 *>(solved->F_iner);
-    P.F_BEM = d->n_bem_head > 0 ? reinterpret_cast<const double2 *>(solved->F_BEM) : nullptr;
-    P.M_arr = f->M_arr; P.B_arr = f->B_arr; P.C_arr = f->C_arr;
-    P.Xi = reinterpret_cast<double2 *>(f->Xi_sys); P.info = f->info;
-    if (!farm_on_chip(f->n_fowt)) {
-        // persistent CTAs over the (farm, case, frequency) systems, each CTA on its own slab of the caller's workspace
-        const GluPlan g = glu_plan(n);
-        if (!g.pw) return set_err(RAFTK_EINVAL, "farm response: 6N too large for one panel column in shared memory");
-        const size_t slab = farm_slab_bytes(f->n_fowt);
-        if (!ws || ws_bytes < slab)
-            return set_err(RAFTK_EINVAL, "farm response: a farm this size needs a workspace of at least one [6N][6N+1] slab "
-                                         "(raftk_farm_workspace_bytes, raftk_farm_response_ws_dev)");
-        const long long nsys = (long long)f->n_farms * c->n_cases * d->nw;
-        const int grid = (int)std::min<long long>(std::min<long long>(nsys, (long long)(ws_bytes / slab)), (long long)g.per_sm * sm_count());
-        static SmemOptIn opt_g(0), opt_go(0);
-        const bool op = c->op != nullptr;                   // the instantiations with operating points
-        CUDA_TRY(op ? opt_go.ensure(k_farm_response_global<true>, g.smem) : opt_g.ensure(k_farm_response_global<false>, g.smem));
-        DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
-        CasesDev C = to_dev(c);
-        {
-            ProfScope ps(st, 1);
-            if (op) k_farm_response_global<true><<<grid, GLU_T, g.smem, st>>>(D, C, P, static_cast<double2 *>(ws), g.pw);
-            else k_farm_response_global<false><<<grid, GLU_T, g.smem, st>>>(D, C, P, static_cast<double2 *>(ws), g.pw);
-            disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_GLOBAL, GLU_T);
-        }
-        g_launches++;
-        CUDA_TRY(cudaGetLastError());
-        if (px) {
-            const size_t nx = (size_t)f->n_farms * c->n_cases * n * d->nw;
-            k_farm_publish<<<dim3((unsigned)std::min<size_t>((nx + 255) / 256, 1024), (unsigned)px->n_peers), 256, 0, st>>>(Q);
-            g_launches++;
-            CUDA_TRY(cudaGetLastError());
-        }
-        return RAFTK_OK;
-    }
-    const bool warp = n <= 24;                          // one warp per (frequency, case), wpc systems per CTA; blocked LU above
-    const size_t sys_bytes = (size_t)n * (n + 1) * sizeof(double2);
-    const int wpc = warp ? (int)std::max<size_t>(1, std::min<size_t>(FARM_WPC, (100 * 1024) / sys_bytes)) : 1;
-    const size_t smem = (size_t)wpc * sys_bytes;
-    // grid = (frequency groups, case, farm): the y and z extents of a grid end at 65535
-    if (c->n_cases > 65535) return set_err(RAFTK_EINVAL, "farm response: more than 65535 cases per call");
-    if (f->n_farms > 65535) return set_err(RAFTK_EINVAL, "farm response: more than 65535 farms per call with the system in shared memory (6N <= 120)");
-    // 6N = 12 (the shipped two-FOWT farm): rows in registers, one lane per row, two systems per warp (k_farm_rows);
-    // RAFTK_FARM_SMEM=1 keeps the shared-memory warp kernel (A/B).  At 6N = 18 / 24 the register rows need 188 / 238
-    // registers, so those stay on the warp kernel.
-    const bool rows = n == 12 && !getenv("RAFTK_FARM_SMEM");
-    const unsigned gy = c->n_cases, gz = f->n_farms;
-    const dim3 gr((d->nw + 7) / 8, gy, gz), gw((d->nw + wpc - 1) / wpc, gy, gz), gb(d->nw, gy, gz);
-    // one instantiation per (operating points, peer stores); the shared-memory opt-in is per instantiation
-    auto go = [&](auto op_c, auto peer_c) -> int {
-        constexpr bool OP = decltype(op_c)::value, PEER = decltype(peer_c)::value;
-        static SmemOptIn opt_w(48 * 1024), opt_b(48 * 1024);
-        if (warp) CUDA_TRY(opt_w.ensure(k_farm_response<true, OP, PEER>, smem));
-        else CUDA_TRY(opt_b.ensure(k_farm_response<false, OP, PEER>, smem));
-        DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
-        CasesDev C = to_dev(c);
-        const FarmArg<PEER> &A = Q;
-        {
-            ProfScope ps(st, 1);
-            if (rows) k_farm_rows<12, OP, PEER><<<gr, 128, 0, st>>>(D, C, A);
-            else if (warp) k_farm_response<true, OP, PEER><<<gw, 32 * wpc, smem, st>>>(D, C, A);
-            else k_farm_response<false, OP, PEER><<<gb, 256, smem, st>>>(D, C, A);
-            if (rows) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_ROWS12, 128);
-            else if (warp) disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_WARP, 32 * wpc);
-            else disp_launch(RAFTK_FAMILY_FARM, RAFTK_KERNEL_FARM_BLOCK, 256);
-        }
-        g_launches++;
-        CUDA_TRY(cudaGetLastError());
-        return RAFTK_OK;
-    };
-    using T = std::true_type;
-    using F = std::false_type;
-    if (c->op) return px ? go(T{}, T{}) : go(T{}, F{});
-    return px ? go(F{}, T{}) : go(F{}, F{});
-}
-
-// the single-farm entries: farm.n_fowt names the whole batch of designs
-static int farm_launch_one(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f, void *ws,
-                           size_t ws_bytes, cudaStream_t st)
-{
-    if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "farm response: null argument");
-    if (f->n_fowt != d->n_designs || f->n_fowt < 1) return set_err(RAFTK_EINVAL, "farm response: farm.n_fowt must equal designs.n_designs");
-    if (!f->Xi_sys) return set_err(RAFTK_EINVAL, "farm response needs farm.Xi_sys");
-    const raftk_farm_batch b = farm_as_batch(f);
-    return farm_launch(d, c, solved, &b, ws, ws_bytes, st);
-}
-
-extern "C" int raftk_farm_response_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f,
-                                       void *stream)
-{
-    disp_reset();
-    if (int rc = validate_op_dev(c)) return rc;
-    return farm_launch_one(d, c, solved, f, nullptr, 0, (cudaStream_t)stream);
-}
-
-extern "C" int raftk_farm_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f,
-                                          void *workspace, size_t workspace_bytes, void *stream)
-{
-    disp_reset();
-    if (int rc = validate_op_dev(c)) return rc;
-    return farm_launch_one(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
-}
-
-extern "C" int raftk_farm_batch_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
-                                                const raftk_farm_batch *f, void *workspace, size_t workspace_bytes, void *stream)
-{
-    disp_reset();
-    if (int rc = validate_op_dev(c)) return rc;
-    return farm_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
-}
-
-extern "C" int raftk_farm_batch_response_gather_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
-                                                    const raftk_farm_batch *f, const raftk_peers *peers, int32_t farm_row0,
-                                                    void *workspace, size_t workspace_bytes, void *stream)
-{
-    disp_reset();
-    if (int rc = validate_peers(peers)) return rc;
-    if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "farm gather: null argument");
-    if (int rc = farm_batch_shape(d, f)) return rc;
-    if (!f->info || !solved->status) return set_err(RAFTK_EINVAL, "farm gather: farm_batch.info and the per-FOWT status are required");
-    for (int r = 0; r < peers->n_ranks; r++)
-        if (!peers->status[r]) return set_err(RAFTK_EINVAL, "farm gather: a rank's gathered info and status (peers.status) is missing");
-    const size_t per_farm = (size_t)c->n_cases * 6 * f->n_fowt * d->nw;          // complex elements of one farm's Xi_sys
-    if (c->n_cases < 1 || d->nw < 1 || peers->block_elems == 0 || peers->block_elems % per_farm)
-        return set_err(RAFTK_EINVAL, "farm gather: peers.block_elems must be F_max * nC * 6N * nw with F_max >= 1");
-    const long long F_max = (long long)(peers->block_elems / per_farm);
-    if (f->n_farms > F_max) return set_err(RAFTK_EINVAL, "farm gather: farm_batch.n_farms exceeds F_max, the farms of a rank block");
-    if (farm_row0 != (long long)peers->rank * F_max)                              // a rank writes its own block, no other rank's
-        return set_err(RAFTK_EINVAL, "farm gather: farm_row0 must be rank * F_max, the first farm slot of this rank's block");
-    const size_t info_farm = (size_t)c->n_cases * d->nw, st_farm = (size_t)f->n_fowt * c->n_cases * 4;
-    const size_t info_all = (size_t)peers->n_ranks * F_max * info_farm;
-    if (f->Xi_sys != peers->gathered[peers->rank] + 2 * (size_t)farm_row0 * per_farm ||
-        f->info != peers->status[peers->rank] + (size_t)farm_row0 * info_farm)
-        return set_err(RAFTK_EINVAL, "farm gather: farm_batch.Xi_sys and info must be this rank's farms in its own gathered copy");
-    if (int rc = validate_op_dev(c)) return rc;
-    FarmPeerParams px{};
-    px.n_peers = peers->n_ranks;
-    px.status = solved->status;
-    for (int r = 0; r < peers->n_ranks; r++) {
-        const bool other = r != peers->rank;
-        px.X[r] = other ? reinterpret_cast<double2 *>(peers->gathered[r]) + (size_t)farm_row0 * per_farm : nullptr;
-        px.I[r] = other ? peers->status[r] + (size_t)farm_row0 * info_farm : nullptr;
-        px.S[r] = peers->status[r] + info_all + (size_t)farm_row0 * st_farm;
-    }
-    return farm_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream, &px);
-}
-
-// ---- ragged farm batches (raftk_farm_ragged) ---------------------------------------------------------------------------
-// Every farm goes to the kernel class farm_launch picks for a uniform batch of its N; a class is launched once over its own
-// farms, in this order.  The descriptors are grouped by class (farms of a class in batch order) and copied to the head of
-// the workspace, where the class's launch finds its run.
+// ---- farm system response: single farms, uniform and ragged batches --------------------------------------------------------
+// Every farm goes to one of four kernel classes by its N alone, and a call launches each class it needs once, over that class's
+// farms, in this order.  A uniform batch (a single farm is a batch of one) is one run of F farms of one N, whose kernels derive
+// every offset from the farm index.  A ragged batch (raftk_farm_ragged) groups its farms by class (farms of a class in batch
+// order); each farm's first design, N, offsets and panel width are in a descriptor copied to the head of the workspace, where
+// the class's launch finds its run.
 enum { FC_ROWS, FC_WARP, FC_BLOCK, FC_GLOBAL, FC_N };
 static const int fc_kernel[FC_N] = {RAFTK_KERNEL_FARM_ROWS12, RAFTK_KERNEL_FARM_WARP, RAFTK_KERNEL_FARM_BLOCK, RAFTK_KERNEL_FARM_GLOBAL};
+
+// The class of a farm of N FOWTs.  6N <= 24: one warp per (frequency, case), except 6N = 12 (the shipped two-FOWT farm), whose
+// rows live in registers, one lane per row, two systems per warp (k_farm_rows; RAFTK_FARM_SMEM=1 keeps the shared-memory warp
+// kernel, for A/B).  At 6N = 18 / 24 the register rows would need 188 / 238 registers, so those stay on the warp kernel.
+// Above 24, one CTA per system while its [6N][6N+1] fits in shared memory, else k_farm_response_global.
 static int farm_class(int N)
 {
-    if (!farm_on_chip(N)) return FC_GLOBAL;
-    if (6 * N == 12 && !getenv("RAFTK_FARM_SMEM")) return FC_ROWS;
-    return 6 * N <= 24 ? FC_WARP : FC_BLOCK;
+    const int n = 6 * N;
+    if (n > 24 && !smem_fits((size_t)n * (n + 1) * sizeof(double2), static_smem(k_farm_response<false>, SMEM_STATIC_FARM_BLOCK)))
+        return FC_GLOBAL;
+    if (n == 12 && !getenv("RAFTK_FARM_SMEM")) return FC_ROWS;
+    return n <= 24 ? FC_WARP : FC_BLOCK;
 }
 
-struct RagPlan {
-    std::vector<FarmDesc> fd;           // grouped by class: class k is fd[first[k], first[k + 1])
-    int first[FC_N + 1] = {};
+// What a call launches and the workspace it needs, from a raftk_farm_batch or a raftk_farm_ragged (farm_plan)
+struct FarmPlan {
+    bool rag = false;                   // a ragged batch: the descriptor table heads the workspace
+    const char *who = "farm response";  // the refusals' prefix
+    int N = 0, F = 0;                   // uniform: farms of N FOWTs; F farms in all
+    std::vector<FarmDesc> fd;           // ragged: grouped by class
+    int first[FC_N + 1] = {};           // class k is farms [first[k], first[k + 1]) of the launch order
     int nmax[FC_N] = {};                // largest N of each class
     size_t table = 0;                   // bytes of the descriptor table at the head of the workspace (256-aligned)
     size_t slab = 0;                    // double2 elements of one k_farm_response_global slab (the class's largest N)
     size_t pan_smem = 0;                // k_farm_response_global's panel: the largest n * pw of its farms
+    int pw = 0;                         // uniform: that panel's width (ragged farms carry their own)
     int per_sm = 0;                     // its CTAs per SM: the fewest any of its farms' glu_plan allows
     long long gsys = 0;                 // (farm, case, bin) systems of that class
     size_t bytes = 0;                   // the full workspace: table + min(gsys, resident CTAs) slabs
+    const double *M_arr = nullptr, *B_arr = nullptr, *C_arr = nullptr;
+    size_t n_arr = 0, arr_stride = 0;   // doubles of each array-matrix set; uniform: between two farms' sets (0: shared)
+    double *Xi_sys = nullptr;
+    int32_t *info = nullptr;
 };
 
-static int rag_plan(const raftk_designs *d, const raftk_cases *c, const raftk_farm_ragged *f, RagPlan &R)
+// the global class's slabs after the table: one [6N][6N+1] of its largest N per resident CTA, no more than its systems
+static void farm_plan_slabs(const raftk_designs *d, const raftk_cases *c, FarmPlan &R)
+{
+    const int nk = R.first[FC_GLOBAL + 1] - R.first[FC_GLOBAL], N = R.nmax[FC_GLOBAL];
+    R.bytes = R.table;
+    if (!nk) return;
+    R.slab = (size_t)6 * N * (6 * N + 1);
+    R.gsys = (long long)nk * c->n_cases * d->nw;
+    R.bytes += (size_t)std::max<long long>(0, std::min<long long>(R.gsys, (long long)R.per_sm * sm_count())) * R.slab * sizeof(double2);
+}
+
+// A uniform batch: one class run of F farms of N, no descriptor table, its slab and panel from glu_plan(6N).  It refuses
+// nothing (its grid limits are farm_run's), so the workspace queries never touch the last-error string.
+static void farm_plan(const raftk_designs *d, const raftk_cases *c, const raftk_farm_batch *f, FarmPlan &R)
+{
+    const int k = farm_class(f->n_fowt);
+    R.N = f->n_fowt; R.F = std::max(f->n_farms, 0);
+    for (int j = k + 1; j <= FC_N; j++) R.first[j] = R.F;
+    R.nmax[k] = R.N;
+    if (k == FC_GLOBAL) {
+        const GluPlan g = glu_plan(6 * R.N);
+        R.pw = g.pw; R.pan_smem = g.smem; R.per_sm = std::max(g.per_sm, 1);
+    }
+    farm_plan_slabs(d, c, R);
+    R.n_arr = (f->arr_shared ? 1 : (size_t)R.F) * 36 * R.N * R.N;
+    R.arr_stride = f->arr_shared ? 0 : (size_t)36 * R.N * R.N;
+    R.M_arr = f->M_arr; R.B_arr = f->B_arr; R.C_arr = f->C_arr;
+    R.Xi_sys = f->Xi_sys; R.info = f->info;
+}
+
+// A ragged batch: its CSR arrays checked, each farm's descriptor in its class's run
+static int farm_plan(const raftk_designs *d, const raftk_cases *c, const raftk_farm_ragged *f, FarmPlan &R)
 {
     if (!d || !c || !f) return set_err(RAFTK_EINVAL, "ragged farm batch: null argument");
     auto bad_farm = [](const char *fmt, int k) { char b[16]; snprintf(b, sizeof(b), "%d", k); return set_err(RAFTK_EINVAL, fmt, b); };
@@ -1239,6 +1072,7 @@ static int rag_plan(const raftk_designs *d, const raftk_cases *c, const raftk_fa
         }
     }
     if (c->n_cases < 1 || d->nw < 1) return set_err(RAFTK_EINVAL, "ragged farm batch: no cases or no frequency bins");
+    R.rag = true; R.who = "ragged farm batch"; R.F = F;
     std::vector<int> cls(F);
     int count[FC_N] = {};
     for (int k = 0; k < F; k++) {
@@ -1276,88 +1110,200 @@ static int rag_plan(const raftk_designs *d, const raftk_cases *c, const raftk_fa
     std::stable_sort(R.fd.begin() + R.first[FC_GLOBAL], R.fd.begin() + R.first[FC_GLOBAL + 1],
                      [](const FarmDesc &a, const FarmDesc &b) { return a.N > b.N; });
     R.table = align_up((size_t)F * sizeof(FarmDesc), 256);
-    R.bytes = R.table;
-    if (count[FC_GLOBAL]) {
-        R.slab = (size_t)6 * R.nmax[FC_GLOBAL] * (6 * R.nmax[FC_GLOBAL] + 1);
-        R.gsys = (long long)count[FC_GLOBAL] * c->n_cases * d->nw;
-        R.bytes += (size_t)std::min<long long>(R.gsys, (long long)R.per_sm * sm_count()) * R.slab * sizeof(double2);
-    }
+    farm_plan_slabs(d, c, R);
+    const size_t N0 = (size_t)f->farm_fowt0[1];
+    R.n_arr = f->arr_shared ? 36 * N0 * N0 : (f->arr_offset ? (size_t)f->arr_offset[F] : 0);
+    R.M_arr = f->M_arr; R.B_arr = f->B_arr; R.C_arr = f->C_arr;
+    R.Xi_sys = f->Xi_sys; R.info = f->info;
     return RAFTK_OK;
+}
+
+// one farm is a batch of one: its matrices are the shared set
+static raftk_farm_batch farm_as_batch(const raftk_farm *f)
+{
+    raftk_farm_batch b;
+    memset(&b, 0, sizeof(b));
+    b.n_farms = 1; b.n_fowt = f->n_fowt; b.arr_shared = 1;
+    b.M_arr = f->M_arr; b.B_arr = f->B_arr; b.C_arr = f->C_arr;
+    b.Xi_sys = f->Xi_sys; b.info = f->info;
+    return b;
+}
+
+extern "C" size_t raftk_farm_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm *f)
+{
+    if (!f) return 0;
+    const raftk_farm_batch b = farm_as_batch(f);
+    return raftk_farm_batch_workspace_bytes(d, c, &b);
+}
+
+extern "C" size_t raftk_farm_batch_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm_batch *f)
+{
+    if (!d || !c || !f) return 0;
+    FarmPlan R;
+    farm_plan(d, c, f, R);
+    return R.bytes;
 }
 
 extern "C" size_t raftk_farm_ragged_workspace_bytes(const raftk_designs *d, const raftk_cases *c, const raftk_farm_ragged *f)
 {
-    RagPlan R;
-    return rag_plan(d, c, f, R) ? 0 : R.bytes;
+    FarmPlan R;
+    return farm_plan(d, c, f, R) ? 0 : R.bytes;
+}
+
+// the launch of class k's run of farms: grid, shared memory and its opt-in (per instantiation), and the dispatch record
+template <bool OP, bool RAG>
+static int farm_launch_class(int k, const FarmPlan &R, const FarmArg<RAG> &P, const DesignsDev &D, const CasesDev &C, void *ws,
+                             size_t ws_bytes, cudaStream_t st)
+{
+    static SmemOptIn opt_w(48 * 1024), opt_b(48 * 1024), opt_g(0);
+    const int n = 6 * R.nmax[k], nw = P.nw;              // shared memory for the class's largest N
+    const size_t sys_bytes = (size_t)n * (n + 1) * sizeof(double2);
+    const unsigned gy = P.nC, gz = P.nF;
+    int threads = GLU_T;
+    {
+        ProfScope ps(st, 1);
+        if (k == FC_ROWS) {
+            threads = 128;
+            k_farm_rows<12, OP, RAG><<<dim3((nw + 7) / 8, gy, gz), threads, 0, st>>>(D, C, P);
+        } else if (k == FC_WARP) {                        // one warp per (frequency, case), wpc systems per CTA
+            const int wpc = (int)std::max<size_t>(1, std::min<size_t>(FARM_WPC, (100 * 1024) / sys_bytes));
+            threads = 32 * wpc;
+            CUDA_TRY(opt_w.ensure(k_farm_response<true, OP, RAG>, wpc * sys_bytes));
+            k_farm_response<true, OP, RAG><<<dim3((nw + wpc - 1) / wpc, gy, gz), threads, wpc * sys_bytes, st>>>(D, C, P);
+        } else if (k == FC_BLOCK) {
+            threads = 256;
+            CUDA_TRY(opt_b.ensure(k_farm_response<false, OP, RAG>, sys_bytes));
+            k_farm_response<false, OP, RAG><<<dim3(nw, gy, gz), threads, sys_bytes, st>>>(D, C, P);
+        } else {                                          // persistent CTAs, each on its own slab of the workspace after the table
+            CUDA_TRY(opt_g.ensure(k_farm_response_global<OP, RAG>, R.pan_smem));
+            double2 *slabs = reinterpret_cast<double2 *>(static_cast<char *>(ws) + R.table);
+            const long long fit = (long long)((ws_bytes - R.table) / (R.slab * sizeof(double2)));
+            const int grid = (int)std::min<long long>(std::min<long long>(R.gsys, fit), (long long)R.per_sm * sm_count());
+            k_farm_response_global<OP, RAG><<<grid, GLU_T, R.pan_smem, st>>>(D, C, P, slabs, R.pw);
+        }
+        disp_launch(RAFTK_FAMILY_FARM, fc_kernel[k], threads);
+    }
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
+// The farm response of a plan: each non-empty class run launched in class order.  The dispatch record names the last launch,
+// and farm_classes every class that ran.
+static int farm_run(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const FarmPlan &R, void *ws,
+                    size_t ws_bytes, cudaStream_t st)
+{
+    if (!solved->B_drag || !solved->F_drag || !solved->F_iner)
+        return set_err(RAFTK_EINVAL, "%s needs B_drag, F_drag, F_iner of the per-FOWT solve", R.who);
+    if (d->n_bem_head > 0 && !solved->F_BEM) return set_err(RAFTK_EINVAL, "%s: the designs carry BEM excitation, F_BEM is required", R.who);
+    if (R.rag) {
+        if (!ws || ws_bytes < R.table + R.slab * sizeof(double2))
+            return set_err(RAFTK_EINVAL, "ragged farm batch: the workspace must hold the farm descriptor table%s (raftk_farm_ragged_workspace_bytes)",
+                           R.slab ? " and one [6N][6N+1] slab of the largest farm solved in global memory" : "");
+    } else if (!R.slab) {               // the grid is (frequency groups, case, farm): its y and z extents end at 65535
+        if (c->n_cases > 65535) return set_err(RAFTK_EINVAL, "farm response: more than 65535 cases per call");
+        if (R.F > 65535) return set_err(RAFTK_EINVAL, "farm response: more than 65535 farms per call with the system in shared memory (6N <= 120)");
+    } else {
+        if (!R.pw) return set_err(RAFTK_EINVAL, "farm response: 6N too large for one panel column in shared memory");
+        if (!ws || ws_bytes < R.slab * sizeof(double2))
+            return set_err(RAFTK_EINVAL, "farm response: a farm this size needs a workspace of at least one [6N][6N+1] slab "
+                                         "(raftk_farm_workspace_bytes, raftk_farm_response_ws_dev)");
+    }
+    FarmRagParams P{};
+    P.N = R.N; P.nC = c->n_cases; P.nw = d->nw;
+    P.arr_stride = R.arr_stride;
+    P.B_drag = solved->B_drag;
+    P.F_drag = reinterpret_cast<const double2 *>(solved->F_drag);
+    P.F_iner = reinterpret_cast<const double2 *>(solved->F_iner);
+    P.F_BEM = d->n_bem_head > 0 ? reinterpret_cast<const double2 *>(solved->F_BEM) : nullptr;
+    P.M_arr = R.M_arr; P.B_arr = R.B_arr; P.C_arr = R.C_arr;
+    P.Xi = reinterpret_cast<double2 *>(R.Xi_sys); P.info = R.info;
+    P.slab = R.slab;
+    FarmDesc *dfd = static_cast<FarmDesc *>(ws);
+    if (R.rag) CUDA_TRY(cudaMemcpyAsync(dfd, R.fd.data(), R.fd.size() * sizeof(FarmDesc), cudaMemcpyHostToDevice, st));
+    DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
+    CasesDev C = to_dev(c);
+    int mask = 0;
+    for (int k = 0; k < FC_N; k++) {
+        if (R.first[k + 1] == R.first[k]) continue;
+        P.nF = R.first[k + 1] - R.first[k];
+        if (R.rag) P.fd = dfd + R.first[k];
+        const FarmParams &U = P;
+        const int rc = R.rag ? (c->op ? farm_launch_class<true, true>(k, R, P, D, C, ws, ws_bytes, st)
+                                      : farm_launch_class<false, true>(k, R, P, D, C, ws, ws_bytes, st))
+                             : (c->op ? farm_launch_class<true, false>(k, R, U, D, C, ws, ws_bytes, st)
+                                      : farm_launch_class<false, false>(k, R, U, D, C, ws, ws_bytes, st));
+        if (rc) return rc;
+        mask |= 1 << fc_kernel[k];
+    }
+    g_disp.farm_classes = mask;
+    return RAFTK_OK;
+}
+
+// the shape of a farm batch against its designs (everything the host entry can refuse before it stages anything)
+static int farm_batch_shape(const raftk_designs *d, const raftk_farm_batch *f)
+{
+    if (f->n_farms < 1 || f->n_fowt < 1) return set_err(RAFTK_EINVAL, "farm batch: n_farms and n_fowt must be >= 1");
+    if ((long long)f->n_farms * f->n_fowt != d->n_designs)
+        return set_err(RAFTK_EINVAL, "farm batch: n_farms * n_fowt must equal designs.n_designs");
+    if (f->arr_shared != 0 && f->arr_shared != 1) return set_err(RAFTK_EINVAL, "farm batch: arr_shared must be 0 or 1");
+    if (!f->Xi_sys) return set_err(RAFTK_EINVAL, "farm batch: Xi_sys is required");
+    return RAFTK_OK;
+}
+
+static int farm_launch(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm_batch *f, void *ws,
+                       size_t ws_bytes, cudaStream_t st)
+{
+    if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "farm response: null argument");
+    if (int rc = farm_batch_shape(d, f)) return rc;
+    FarmPlan R;
+    farm_plan(d, c, f, R);
+    return farm_run(d, c, solved, R, ws, ws_bytes, st);
 }
 
 static int farm_ragged_launch(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm_ragged *f,
                               void *ws, size_t ws_bytes, cudaStream_t st)
 {
     if (!solved) return set_err(RAFTK_EINVAL, "ragged farm batch: null argument");
-    RagPlan R;
-    if (int rc = rag_plan(d, c, f, R)) return rc;
+    FarmPlan R;
+    if (int rc = farm_plan(d, c, f, R)) return rc;
     if (!f->Xi_sys) return set_err(RAFTK_EINVAL, "ragged farm batch: Xi_sys is required");
-    if (!solved->B_drag || !solved->F_drag || !solved->F_iner)
-        return set_err(RAFTK_EINVAL, "ragged farm batch needs B_drag, F_drag, F_iner of the per-FOWT solve");
-    if (d->n_bem_head > 0 && !solved->F_BEM) return set_err(RAFTK_EINVAL, "ragged farm batch: the designs carry BEM excitation, F_BEM is required");
-    const size_t slab_bytes = R.slab * sizeof(double2);
-    if (!ws || ws_bytes < R.table + slab_bytes)
-        return set_err(RAFTK_EINVAL, "ragged farm batch: the workspace must hold the farm descriptor table%s (raftk_farm_ragged_workspace_bytes)",
-                       R.slab ? " and one [6N][6N+1] slab of the largest farm solved in global memory" : "");
-    FarmDesc *dfd = static_cast<FarmDesc *>(ws);
-    CUDA_TRY(cudaMemcpyAsync(dfd, R.fd.data(), R.fd.size() * sizeof(FarmDesc), cudaMemcpyHostToDevice, st));
-    FarmRagParams P{};
-    P.nC = c->n_cases; P.nw = d->nw;
-    P.B_drag = solved->B_drag;
-    P.F_drag = reinterpret_cast<const double2 *>(solved->F_drag);
-    P.F_iner = reinterpret_cast<const double2 *>(solved->F_iner);
-    P.F_BEM = d->n_bem_head > 0 ? reinterpret_cast<const double2 *>(solved->F_BEM) : nullptr;
-    P.M_arr = f->M_arr; P.B_arr = f->B_arr; P.C_arr = f->C_arr;
-    P.Xi = reinterpret_cast<double2 *>(f->Xi_sys); P.info = f->info;
-    P.slab = R.slab;
-    DesignsDev D = to_dev(d, d->max_nodes, d->max_members);
-    CasesDev C = to_dev(c);
-    const unsigned gy = c->n_cases;
-    int mask = 0, last = FC_N;
-    auto go = [&](auto op_c) -> int {
-        constexpr bool OP = decltype(op_c)::value;
-        static SmemOptIn opt_w(48 * 1024), opt_b(48 * 1024), opt_g(0);
-        for (int k = 0; k < FC_N; k++) {
-            const int nk = R.first[k + 1] - R.first[k];
-            if (!nk) continue;
-            P.fd = dfd + R.first[k]; P.nF = nk;
-            const int n = 6 * R.nmax[k];
-            const size_t sys_bytes = (size_t)n * (n + 1) * sizeof(double2);
-            ProfScope ps(st, 1);
-            if (k == FC_ROWS) {
-                k_farm_rows<12, OP, false, true><<<dim3((d->nw + 7) / 8, gy, nk), 128, 0, st>>>(D, C, P);
-            } else if (k == FC_WARP) {   // shared memory for wpc systems of the class's largest N (farm_launch's rule)
-                const int wpc = (int)std::max<size_t>(1, std::min<size_t>(FARM_WPC, (100 * 1024) / sys_bytes));
-                CUDA_TRY(opt_w.ensure(k_farm_response<true, OP, false, true>, wpc * sys_bytes));
-                k_farm_response<true, OP, false, true><<<dim3((d->nw + wpc - 1) / wpc, gy, nk), 32 * wpc, wpc * sys_bytes, st>>>(D, C, P);
-            } else if (k == FC_BLOCK) {
-                CUDA_TRY(opt_b.ensure(k_farm_response<false, OP, false, true>, sys_bytes));
-                k_farm_response<false, OP, false, true><<<dim3(d->nw, gy, nk), 256, sys_bytes, st>>>(D, C, P);
-            } else {
-                CUDA_TRY(opt_g.ensure(k_farm_response_global<OP, true>, R.pan_smem));
-                double2 *slabs = reinterpret_cast<double2 *>(static_cast<char *>(ws) + R.table);
-                const long long fit = (long long)((ws_bytes - R.table) / slab_bytes);
-                const int grid = (int)std::min<long long>(std::min<long long>(R.gsys, fit), (long long)R.per_sm * sm_count());
-                k_farm_response_global<OP, true><<<grid, GLU_T, R.pan_smem, st>>>(D, C, P, slabs, 0);
-            }
-            g_launches++;
-            CUDA_TRY(cudaGetLastError());
-            mask |= 1 << fc_kernel[k];
-            last = k;
-        }
-        return RAFTK_OK;
-    };
-    const int rc = c->op ? go(std::true_type{}) : go(std::false_type{});
-    if (rc) return rc;
-    disp_launch(RAFTK_FAMILY_FARM, fc_kernel[last], last == FC_ROWS ? 128 : last == FC_WARP ? 32 * FARM_WPC : GLU_T);
-    g_disp.farm_classes = mask;
-    return RAFTK_OK;
+    return farm_run(d, c, solved, R, ws, ws_bytes, st);
+}
+
+// the single-farm entries: farm.n_fowt names the whole batch of designs
+static int farm_launch_one(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f, void *ws,
+                           size_t ws_bytes, cudaStream_t st)
+{
+    if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "farm response: null argument");
+    if (f->n_fowt != d->n_designs || f->n_fowt < 1) return set_err(RAFTK_EINVAL, "farm response: farm.n_fowt must equal designs.n_designs");
+    if (!f->Xi_sys) return set_err(RAFTK_EINVAL, "farm response needs farm.Xi_sys");
+    const raftk_farm_batch b = farm_as_batch(f);
+    return farm_launch(d, c, solved, &b, ws, ws_bytes, st);
+}
+
+extern "C" int raftk_farm_response_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f,
+                                       void *stream)
+{
+    disp_reset();
+    if (int rc = validate_op_dev(c)) return rc;
+    return farm_launch_one(d, c, solved, f, nullptr, 0, (cudaStream_t)stream);
+}
+
+extern "C" int raftk_farm_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const raftk_farm *f,
+                                          void *workspace, size_t workspace_bytes, void *stream)
+{
+    disp_reset();
+    if (int rc = validate_op_dev(c)) return rc;
+    return farm_launch_one(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int raftk_farm_batch_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
+                                                const raftk_farm_batch *f, void *workspace, size_t workspace_bytes, void *stream)
+{
+    disp_reset();
+    if (int rc = validate_op_dev(c)) return rc;
+    return farm_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int raftk_farm_ragged_response_ws_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
@@ -1366,6 +1312,58 @@ extern "C" int raftk_farm_ragged_response_ws_dev(const raftk_designs *d, const r
     disp_reset();
     if (int rc = validate_op_dev(c)) return rc;
     return farm_ragged_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+// After a rank's solve: k_farm_publish copies its farms' Xi_sys, info and per-FOWT status rows (three contiguous runs, its
+// n_farms farms from farm_row0 and its d->n_designs FOWTs from fowt_row0, of the n_farms_total) to the same offsets of the other
+// ranks' copies, and the status rows to its own.
+static int farm_publish(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved, const double *Xi_sys,
+                        const int32_t *info, int n_farms, const raftk_peers *peers, long long farm_row0, long long fowt_row0,
+                        long long n_farms_total, cudaStream_t st)
+{
+    const size_t per = (size_t)6 * c->n_cases * d->nw, info_farm = (size_t)c->n_cases * d->nw;   // one FOWT's Xi_sys, one farm's info
+    FarmFlatPeer P{};
+    P.n_peers = peers->n_ranks;
+    P.nx = per * d->n_designs; P.ni = (size_t)n_farms * info_farm; P.ns = (size_t)d->n_designs * c->n_cases * 4;
+    P.Xi = reinterpret_cast<const double2 *>(Xi_sys); P.info = info; P.status = solved->status;
+    for (int r = 0; r < peers->n_ranks; r++) {
+        const bool other = r != peers->rank;
+        P.X[r] = other ? reinterpret_cast<double2 *>(peers->gathered[r]) + per * fowt_row0 : nullptr;
+        P.I[r] = other ? peers->status[r] + farm_row0 * info_farm : nullptr;
+        P.S[r] = peers->status[r] + n_farms_total * info_farm + fowt_row0 * c->n_cases * 4;
+    }
+    k_farm_publish<<<dim3((unsigned)std::min<size_t>((P.nx + 255) / 256, 1024), (unsigned)P.n_peers), 256, 0, st>>>(P);
+    g_launches++;
+    CUDA_TRY(cudaGetLastError());
+    return RAFTK_OK;
+}
+
+extern "C" int raftk_farm_batch_response_gather_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
+                                                    const raftk_farm_batch *f, const raftk_peers *peers, int32_t farm_row0,
+                                                    void *workspace, size_t workspace_bytes, void *stream)
+{
+    disp_reset();
+    if (int rc = validate_peers(peers)) return rc;
+    if (!d || !c || !solved || !f) return set_err(RAFTK_EINVAL, "farm gather: null argument");
+    if (int rc = farm_batch_shape(d, f)) return rc;
+    if (!f->info || !solved->status) return set_err(RAFTK_EINVAL, "farm gather: farm_batch.info and the per-FOWT status are required");
+    for (int r = 0; r < peers->n_ranks; r++)
+        if (!peers->status[r]) return set_err(RAFTK_EINVAL, "farm gather: a rank's gathered info and status (peers.status) is missing");
+    const size_t per_farm = (size_t)c->n_cases * 6 * f->n_fowt * d->nw;          // complex elements of one farm's Xi_sys
+    if (c->n_cases < 1 || d->nw < 1 || peers->block_elems == 0 || peers->block_elems % per_farm)
+        return set_err(RAFTK_EINVAL, "farm gather: peers.block_elems must be F_max * nC * 6N * nw with F_max >= 1");
+    const long long F_max = (long long)(peers->block_elems / per_farm);
+    if (f->n_farms > F_max) return set_err(RAFTK_EINVAL, "farm gather: farm_batch.n_farms exceeds F_max, the farms of a rank block");
+    if (farm_row0 != (long long)peers->rank * F_max)                              // a rank writes its own block, no other rank's
+        return set_err(RAFTK_EINVAL, "farm gather: farm_row0 must be rank * F_max, the first farm slot of this rank's block");
+    const size_t info_farm = (size_t)c->n_cases * d->nw;
+    if (f->Xi_sys != peers->gathered[peers->rank] + 2 * (size_t)farm_row0 * per_farm ||
+        f->info != peers->status[peers->rank] + (size_t)farm_row0 * info_farm)
+        return set_err(RAFTK_EINVAL, "farm gather: farm_batch.Xi_sys and info must be this rank's farms in its own gathered copy");
+    if (int rc = validate_op_dev(c)) return rc;
+    if (int rc = farm_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream)) return rc;
+    return farm_publish(d, c, solved, f->Xi_sys, f->info, f->n_farms, peers, farm_row0, (long long)farm_row0 * f->n_fowt,
+                        peers->n_ranks * F_max, (cudaStream_t)stream);
 }
 
 extern "C" int raftk_farm_ragged_response_gather_dev(const raftk_designs *d, const raftk_cases *c, const raftk_outputs *solved,
@@ -1384,27 +1382,12 @@ extern "C" int raftk_farm_ragged_response_gather_dev(const raftk_designs *d, con
     const size_t per = (size_t)6 * c->n_cases * d->nw;                        // complex elements of one FOWT's rows of Xi_sys
     if (c->n_cases < 1 || d->nw < 1 || per * ((size_t)fowt_row0 + d->n_designs) > (size_t)peers->n_ranks * peers->block_elems)
         return set_err(RAFTK_EINVAL, "ragged farm gather: the gathered copies (n_ranks * peers.block_elems) do not hold this rank's farms");
-    const size_t info_farm = (size_t)c->n_cases * d->nw, info_all = (size_t)n_farms_total * info_farm;
+    const size_t info_farm = (size_t)c->n_cases * d->nw;
     if (f->Xi_sys != peers->gathered[peers->rank] + 2 * per * fowt_row0 || f->info != peers->status[peers->rank] + (size_t)farm_row0 * info_farm)
         return set_err(RAFTK_EINVAL, "ragged farm gather: farm.Xi_sys and info must be this rank's farms in its own gathered copy");
     if (int rc = validate_op_dev(c)) return rc;
     if (int rc = farm_ragged_launch(d, c, solved, f, workspace, workspace_bytes, (cudaStream_t)stream)) return rc;
-    const raftk_dispatch rec = g_disp;
-    FarmFlatPeer P{};
-    P.n_peers = peers->n_ranks;
-    P.nx = per * d->n_designs; P.ni = (size_t)f->n_farms * info_farm; P.ns = (size_t)d->n_designs * c->n_cases * 4;
-    P.Xi = reinterpret_cast<const double2 *>(f->Xi_sys); P.info = f->info; P.status = solved->status;
-    for (int r = 0; r < peers->n_ranks; r++) {
-        const bool other = r != peers->rank;
-        P.X[r] = other ? reinterpret_cast<double2 *>(peers->gathered[r]) + per * fowt_row0 : nullptr;
-        P.I[r] = other ? peers->status[r] + (size_t)farm_row0 * info_farm : nullptr;
-        P.S[r] = peers->status[r] + info_all + (size_t)fowt_row0 * c->n_cases * 4;
-    }
-    k_farm_publish_flat<<<dim3((unsigned)std::min<size_t>((P.nx + 255) / 256, 1024), (unsigned)P.n_peers), 256, 0, (cudaStream_t)stream>>>(P);
-    g_launches++;
-    CUDA_TRY(cudaGetLastError());
-    g_disp = rec;                                                              // the record names the solve's classes
-    return RAFTK_OK;
+    return farm_publish(d, c, solved, f->Xi_sys, f->info, f->n_farms, peers, farm_row0, fowt_row0, n_farms_total, (cudaStream_t)stream);
 }
 
 
@@ -1617,6 +1600,10 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
     if (mode != 0) cin.op = nullptr;                      // excitation and linearisation assemble no impedance
     else if ((rc = validate_op(c, c->op, c->primary))) return rc;
     c = &cin;
+    FarmPlan fp;
+    const bool farms = farm || rag;
+    if (farm) farm_plan(d, c, farm, fp);
+    if (rag && (rc = farm_plan(d, c, rag, fp))) return rc;
     Staging S(who);
     const size_t nD = d->n_designs, nw = d->nw, nC = c->n_cases;
     const size_t nR = nD * nC * 6 * nw * 2;             // doubles of one complex [nD,nC,6,nw] array
@@ -1625,22 +1612,9 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
     stage_designs_cases(S, d, c, dd, cc);
     const double *Xi_in_d = nullptr;
     S.in(Xi_in_d, Xi_in, nR);
-    raftk_farm_batch fd;
-    memset(&fd, 0, sizeof(fd));
-    if (farm) {                                           // array-level matrices (one set, or one per farm): staged with the other small inputs
-        fd = *farm;
-        const size_t nA = (farm->arr_shared ? 1 : (size_t)farm->n_farms) * 36 * farm->n_fowt * farm->n_fowt;
-        S.in(fd.M_arr, farm->M_arr, nA); S.in(fd.B_arr, farm->B_arr, nA); S.in(fd.C_arr, farm->C_arr, nA);
+    if (farms) {                                          // array-level matrices (one set, or one per farm): staged with the other small inputs
+        S.in(fp.M_arr, fp.M_arr, fp.n_arr); S.in(fp.B_arr, fp.B_arr, fp.n_arr); S.in(fp.C_arr, fp.C_arr, fp.n_arr);
     }
-    raftk_farm_ragged rd;
-    memset(&rd, 0, sizeof(rd));
-    if (rag) {                                            // (rag_plan has accepted its shape)
-        rd = *rag;
-        const size_t N0 = (size_t)rag->farm_fowt0[1];
-        const size_t nA = rag->arr_shared ? 36 * N0 * N0 : (rag->arr_offset ? (size_t)rag->arr_offset[rag->n_farms] : 0);
-        S.in(rd.M_arr, rag->M_arr, nA); S.in(rd.B_arr, rag->B_arr, nA); S.in(rd.C_arr, rag->C_arr, nA);
-    }
-    const bool farms = farm || rag;
     // the solve is planned once, at the caller's cluster size, and launched with the workspace that plan needs; excitation
     // and linearisation need the whole batch's tables in one chunk
     const SolvePlan pl = mode == 0 ? plan_solve(d, (int)nC, o->cluster_size, WS_UNBOUNDED) : SolvePlan{};
@@ -1678,9 +1652,7 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
     S.out(od.Xi_last, out->Xi_last ? nR : 0, out->Xi_last);
     char *ws, *fws = nullptr;
     S.buf(ws, wb);
-    const size_t fwb = farm ? farm_ws_bytes(d, c, farm) : rag ? raftk_farm_ragged_workspace_bytes(d, c, rag) : 0;
-    if (farm) { S.out(fd.Xi_sys, nR, farm->Xi_sys); S.out(fd.info, farm->info ? farm->n_farms * nC * nw : 0, farm->info); S.buf(fws, fwb); }
-    if (rag) { S.out(rd.Xi_sys, nR, rag->Xi_sys); S.out(rd.info, rag->info ? rag->n_farms * nC * nw : 0, rag->info); S.buf(fws, fwb); }
+    if (farms) { S.out(fp.Xi_sys, nR, fp.Xi_sys); S.out(fp.info, fp.info ? fp.F * nC * nw : 0, fp.info); S.buf(fws, fp.bytes); }
     if ((rc = S.commit())) return rc;
     if (qtf_solve) {
         if ((rc = run_qtf(&dd, &cc, od.F_2nd, od.F_2nd_mean, 0))) return rc;
@@ -1698,8 +1670,7 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
         if (!rc && mode == 1) rc = tables(&dd, &cc, Xi_in_d, &od, 1, ws, wb, 0);
     }
     if (rc) return rc;
-    if (farm && (rc = farm_launch(&dd, &cc, &od, &fd, fws, fwb, 0))) return rc;
-    if (rag && (rc = farm_ragged_launch(&dd, &cc, &od, &rd, fws, fwb, 0))) return rc;
+    if (farms && (rc = farm_run(&dd, &cc, &od, fp, fws, fp.bytes, 0))) return rc;
     g_disp.direct_d2h = xi_direct != nullptr;
     return S.finish();
 }
@@ -1743,8 +1714,8 @@ extern "C" int raftk_solve_dynamics_farm_ragged_host(const raftk_designs *d, con
 {
     disp_reset();
     if (!out || !out->Xi || !out->status || !o) return set_err(RAFTK_EINVAL, "Xi, status and opts are required");
-    RagPlan R;
-    if (int rc = rag_plan(d, c, f, R)) return rc;
+    FarmPlan R;
+    if (int rc = farm_plan(d, c, f, R)) return rc;
     if (!f->Xi_sys) return set_err(RAFTK_EINVAL, "ragged farm batch: Xi_sys is required");
     return host_run("raftk_solve_dynamics_farm_ragged_host", d, c, o, out, nullptr, 0, nullptr, f);
 }

@@ -46,17 +46,6 @@ struct FarmParams {
 };
 #define FARM_WPC 4
 
-// The farm batch sharded over ranks (raftk_farm_batch_response_gather_dev): the PEER instantiations also store every result
-// into the other ranks' gathered copies.  Pointers are rank p's copy as mapped in this process, already at this rank's first
-// farm, so a slot has the index of the local write.  X[p] / I[p] (Xi_sys, info) are NULL for this rank, whose local write
-// lands in its own copy; S[p] (the per-FOWT status rows of the drag solve, copied from `status`) is set for every rank.
-struct FarmPeerParams : FarmParams {
-    int n_peers;
-    const int *status;                          // [nF * N][nC][4]
-    double2 *X[RAFTK_MAX_PEERS];                // [nF][nC][6N][nw]
-    int *I[RAFTK_MAX_PEERS];                    // [nF][nC][nw]
-    int *S[RAFTK_MAX_PEERS];                    // [nF * N][nC][4]
-};
 // A ragged batch (raftk_farm_ragged): one launch per kernel class over that class's farms, blockIdx.z (or the system walk)
 // indexing the class's run of descriptors.  A descriptor holds what a uniform batch derives from the farm index: the first
 // design, N, the offsets of the farm's Xi_sys / info rows and array matrices, and (k_farm_response_global) the panel width
@@ -69,8 +58,7 @@ struct FarmRagParams : FarmParams {
     const FarmDesc *fd;                         // [nF]: this class's farms
     size_t slab;                                // double2 elements between two CTAs' slabs (k_farm_response_global)
 };
-template <bool PEER, bool RAG = false>
-using FarmArg = typename std::conditional<RAG, FarmRagParams, typename std::conditional<PEER, FarmPeerParams, FarmParams>::type>::type;
+template <bool RAG> using FarmArg = typename std::conditional<RAG, FarmRagParams, FarmParams>::type;
 
 // Farm f of a launch: N, first design, array-matrix offset, the base of its Xi / info and its row there for case c.  A
 // uniform batch derives them from f (the expressions its kernels always used), a ragged one reads f's descriptor.
@@ -98,33 +86,14 @@ template <bool RAG, class Prm> __device__ __forceinline__ size_t farm_row(const 
 {
     if constexpr (RAG) return (size_t)c; else return (size_t)f * P.nC + c;
 }
-
-// farm f's N status rows of case c to every rank's copy, spread over the gsize threads of a group
-__device__ __forceinline__ void farm_peer_status(const FarmPeerParams &P, int f, int c, int gtid, int gsize)
+// k_farm_response_global: double2 elements between two CTAs' slabs, and farm f's panel width (a uniform launch's `pw`)
+template <bool RAG, class Prm> __device__ __forceinline__ size_t farm_slab(const Prm &P)
 {
-    for (int t = gtid; t < 4 * P.N; t += gsize) {
-        const size_t o = (((size_t)f * P.N + t / 4) * P.nC + c) * 4 + (t & 3);
-        const int v = P.status[o];
-#pragma unroll 1
-        for (int p = 0; p < P.n_peers; p++) if (P.S[p]) P.S[p][o] = v;
-    }
+    if constexpr (RAG) return P.slab; else return (size_t)6 * P.N * (6 * P.N + 1);
 }
-
-// PEER epilogue of k_farm_response: system (u, iw)'s solution (column n of A [n][nc]) and info word to the other ranks, fire
-// and forget as k_rao_fused2's; the group that solved bin 0 of (farm f, case c) also publishes that farm's status rows
-__device__ __forceinline__ void farm_peer_store(const FarmPeerParams &P, const double2 *A, int nc, size_t u, int iw, int bad, int f, int c,
-                                                int gtid, int gsize)
+template <bool RAG, class Prm> __device__ __forceinline__ int farm_pw(const Prm &P, int f, int pw)
 {
-    const int n = 6 * P.N, nw = P.nw;
-    for (int a = gtid; a < n; a += gsize) {
-        const double2 v = A[a * nc + n];
-#pragma unroll 1
-        for (int p = 0; p < P.n_peers; p++) if (P.X[p]) P.X[p][(u * n + a) * nw + iw] = v;
-    }
-    if (gtid == 0)
-#pragma unroll 1
-        for (int p = 0; p < P.n_peers; p++) if (P.I[p]) P.I[p][u * nw + iw] = bad;
-    if (iw == 0) farm_peer_status(P, f, c, gtid, gsize);
+    if constexpr (RAG) return P.fd[f].pw; else return pw;
 }
 
 // The frequency-dependent terms of design i's block entry e at bin iw for a case c with an operating point: the design's
@@ -180,10 +149,9 @@ __device__ __forceinline__ void farm_assemble(const DesignsDev &D, const CasesDe
 }
 
 // RAG: one class of a ragged batch, blockIdx.z indexing its descriptors; shared memory sized for the class's largest N
-template <bool WARP, bool OP = false, bool PEER = false, bool RAG = false>
-__global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(DesignsDev D, CasesDev Cs, FarmArg<PEER, RAG> P)
+template <bool WARP, bool OP = false, bool RAG = false>
+__global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(DesignsDev D, CasesDev Cs, FarmArg<RAG> P)
 {
-    static_assert(!(PEER && RAG), "ragged batches have no peer stores");
     extern __shared__ __align__(16) double smem_raw[];
     __shared__ int piv_s[FARM_WPC], bad_s[FARM_WPC];
     __shared__ double2 rinv_s[FARM_WPC];
@@ -206,7 +174,6 @@ __global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(De
     int *info = farm_info<RAG>(P, f);
     for (int a = gtid; a < n; a += gsize) Xi[(u * n + a) * nw + iw] = A[a * nc + n];
     if (gtid == 0 && info) info[u * nw + iw] = bad;
-    if constexpr (PEER) farm_peer_store(P, A, nc, u, iw, bad, f, c, gtid, gsize);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -224,44 +191,28 @@ __global__ void __launch_bounds__(WARP ? 32 * FARM_WPC : 256) k_farm_response(De
 // RAG: the farms of one class of a ragged batch, each with its own N and panel width (its descriptor); slabs P.slab elements
 // apart (the class's largest N) and the panel sized for the largest n * pw by the launch
 template <bool OP = false, bool RAG = false>
-__global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D, CasesDev Cs, FarmArg<false, RAG> P, double2 *ws, int pw)
+__global__ void __launch_bounds__(GLU_T, 2) k_farm_response_global(DesignsDev D, CasesDev Cs, FarmArg<RAG> P, double2 *ws, int pw)
 {
     extern __shared__ __align__(16) double smem_raw[];
     __shared__ LuStaged<GLU_T, GLU_PWMAX> S;
     double2 *Ps = reinterpret_cast<double2 *>(smem_raw);
-    if constexpr (RAG) {
-        const int nw = P.nw;
-        double2 *A = ws + (size_t)blockIdx.x * P.slab;
-        const long long nsys = (long long)P.nF * P.nC * nw;
-        for (long long s = blockIdx.x; s < nsys; s += gridDim.x) {
-            const long long fc = s / nw;                               // f * nC + c of the class
-            const int iw = (int)(s - fc * nw), f = (int)(fc / P.nC), c = (int)(fc - (long long)f * P.nC);
-            const int n = 6 * P.fd[f].N, nc = n + 1;
-            double2 *Xi = farm_xi<true>(P, f);
-            int *info = farm_info<true>(P, f);
-            farm_assemble<OP, true>(D, Cs, P, f, c, iw, A, threadIdx.x, GLU_T);
-            __syncthreads();
-            const int bad = lu_blocked<GLU_T, true, false>(A, nc, A + n, nc, n, 1, P.fd[f].pw, S, Ps);
-            lu_back_subst<GLU_T>(A, (size_t)nc, A + n, (size_t)nc, n, 1, threadIdx.x);
-            for (int a = threadIdx.x; a < n; a += GLU_T) Xi[((size_t)c * n + a) * nw + iw] = A[(size_t)a * nc + n];
-            if (threadIdx.x == 0 && info) info[(size_t)c * nw + iw] = bad;
-            __syncthreads();                                           // the slab is rewritten by the next system
-        }
-    } else {
-        const int n = 6 * P.N, nc = n + 1, nw = P.nw;
-        double2 *A = ws + (size_t)blockIdx.x * n * nc;
-        const long long nsys = (long long)P.nF * P.nC * nw;
-        for (long long s = blockIdx.x; s < nsys; s += gridDim.x) {
-            const long long u = s / nw;                                    // f * nC + c: row of Xi and info
-            const int iw = (int)(s - u * nw), f = (int)(u / P.nC), c = (int)(u - (long long)f * P.nC);
-            farm_assemble<OP>(D, Cs, P, f, c, iw, A, threadIdx.x, GLU_T);
-            __syncthreads();
-            const int bad = lu_blocked<GLU_T, true, false>(A, nc, A + n, nc, n, 1, pw, S, Ps);
-            lu_back_subst<GLU_T>(A, (size_t)nc, A + n, (size_t)nc, n, 1, threadIdx.x);
-            for (int a = threadIdx.x; a < n; a += GLU_T) P.Xi[((size_t)u * n + a) * nw + iw] = A[(size_t)a * nc + n];
-            if (threadIdx.x == 0 && P.info) P.info[(size_t)u * nw + iw] = bad;
-            __syncthreads();                                               // the slab is rewritten by the next system
-        }
+    const int nw = P.nw;
+    double2 *A = ws + (size_t)blockIdx.x * farm_slab<RAG>(P);
+    const long long nsys = (long long)P.nF * P.nC * nw;
+    for (long long s = blockIdx.x; s < nsys; s += gridDim.x) {
+        const long long fc = s / nw;                                   // f * nC + c
+        const int iw = (int)(s - fc * nw), f = (int)(fc / P.nC), c = (int)(fc - (long long)f * P.nC);
+        const int n = 6 * farm_n<RAG>(P, f), nc = n + 1;
+        const size_t u = farm_row<RAG>(P, f, c);                       // row of Xi and info
+        double2 *Xi = farm_xi<RAG>(P, f);
+        int *info = farm_info<RAG>(P, f);
+        farm_assemble<OP, RAG>(D, Cs, P, f, c, iw, A, threadIdx.x, GLU_T);
+        __syncthreads();
+        const int bad = lu_blocked<GLU_T, true, false>(A, nc, A + n, nc, n, 1, farm_pw<RAG>(P, f, pw), S, Ps);
+        lu_back_subst<GLU_T>(A, (size_t)nc, A + n, (size_t)nc, n, 1, threadIdx.x);
+        for (int a = threadIdx.x; a < n; a += GLU_T) Xi[(u * n + a) * nw + iw] = A[(size_t)a * nc + n];
+        if (threadIdx.x == 0 && info) info[u * nw + iw] = bad;
+        __syncthreads();                                               // the slab is rewritten by the next system
     }
 }
 
@@ -289,10 +240,9 @@ __global__ void __launch_bounds__(GLU_T, 2) k_system_solve_global(int n, int nw,
 // entry moves the pivot row to everybody and old row k to the pivot's lane, every row below k eliminates itself.  No shared
 // memory, no barriers; back substitution broadcasts one unknown per step.  Same assembly arithmetic as k_farm_response.
 // ------------------------------------------------------------------------------------------------
-template <int N6, bool OP = false, bool PEER = false, bool RAG = false>
-__global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, FarmArg<PEER, RAG> P)
+template <int N6, bool OP = false, bool RAG = false>
+__global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, FarmArg<RAG> P)
 {
-    static_assert(!(PEER && RAG), "ragged batches have no peer stores");
     constexpr int LPS = N6 <= 16 ? 16 : 32, SPW = 32 / LPS, NC = N6 + 1;
     const int nw = P.nw, lane = threadIdx.x & 31, r = lane & (LPS - 1);
     const int sys = ((int)blockIdx.x * ((int)blockDim.x >> 5) + ((int)threadIdx.x >> 5)) * SPW + lane / LPS;
@@ -393,33 +343,12 @@ __global__ void __launch_bounds__(128) k_farm_rows(DesignsDev D, CasesDev Cs, Fa
     int *info = farm_info<RAG>(P, f);
     if (live && row_ok) Xi[(u * N6 + r) * nw + iw] = x;
     if (live && r == 0 && info) info[u * nw + iw] = bad;
-    if constexpr (PEER) {                              // as farm_peer_store, from the lanes' registers
-        if (live) {
-#pragma unroll 1
-            for (int p = 0; p < P.n_peers; p++) {
-                if (row_ok && P.X[p]) P.X[p][(u * N6 + r) * nw + iw] = x;
-                if (r == 0 && P.I[p]) P.I[p][u * nw + iw] = bad;
-            }
-            if (iw == 0) farm_peer_status(P, f, c, r, LPS);
-        }
-    }
 }
 
-// K3e: a rank's farms solved by k_farm_response_global, to the other ranks' copies after the kernel (the global LU leaves Xi_sys
-// final only at its end): blockIdx.y = p; Xi_sys and info where X[p] / I[p] are set, the per-FOWT status rows to every S[p]
-__global__ void __launch_bounds__(256) k_farm_publish(FarmPeerParams P)
-{
-    const int p = blockIdx.y;
-    const size_t stride = (size_t)gridDim.x * 256, t0 = (size_t)blockIdx.x * 256 + threadIdx.x;
-    const size_t sys = (size_t)P.nF * P.nC, nx = sys * 6 * P.N * P.nw, ni = sys * P.nw, ns = sys * P.N * 4;
-    if (double2 *x = P.X[p]) for (size_t t = t0; t < nx; t += stride) x[t] = P.Xi[t];
-    if (int *d = P.I[p]) for (size_t t = t0; t < ni; t += stride) d[t] = P.info[t];
-    if (int *d = P.S[p]) for (size_t t = t0; t < ns; t += stride) d[t] = P.status[t];
-}
-
-// K3f: a rank's farms of a ragged batch (raftk_farm_ragged_response_gather_dev) to the other ranks' copies after their solve.
-// The rank's farms are contiguous, so their Xi_sys, info and per-FOWT status are three contiguous runs, stored at the same
-// offsets of every copy: blockIdx.y = p; Xi_sys and info where X[p] / I[p] are set, the status rows to every S[p]
+// K3e: a rank's farms of a sharded batch (raftk_farm_batch_response_gather_dev, raftk_farm_ragged_response_gather_dev) to the
+// other ranks' copies after their solve.  The rank's farms are contiguous, so their
+// Xi_sys, info and per-FOWT status are three contiguous runs, stored at the same offsets of every copy: blockIdx.y = p; Xi_sys
+// and info where X[p] / I[p] are set, the status rows to every S[p]
 struct FarmFlatPeer {
     int n_peers;
     size_t nx, ni, ns;                          // complex elements of Xi_sys, info words, status words of this rank's farms
@@ -429,7 +358,7 @@ struct FarmFlatPeer {
     int *I[RAFTK_MAX_PEERS];
     int *S[RAFTK_MAX_PEERS];
 };
-__global__ void __launch_bounds__(256) k_farm_publish_flat(FarmFlatPeer P)
+__global__ void __launch_bounds__(256) k_farm_publish(FarmFlatPeer P)
 {
     const int p = blockIdx.y;
     const size_t stride = (size_t)gridDim.x * 256, t0 = (size_t)blockIdx.x * 256 + threadIdx.x;

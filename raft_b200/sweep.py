@@ -513,23 +513,11 @@ def farm_rows(bounds, per=1):
 
 def gather_farm_shards(blocks, bounds, n_fowt, group=None):
     """The ``exchange="nccl"`` path of ``ShardedFarmSolve``: this rank's (Xi_sys [F_r,nC,6N,nw], info [F_r,nC,nw], status
-    [F_r*N,nC,4]) padded to the largest shard, one ``all_gather_into_tensor`` each, and the padding dropped
-    -> the whole batch's three tensors in farm order.  Backend-agnostic (NCCL on GPUs, gloo on CPU tensors)."""
-    import torch
-    import torch.distributed as dist
-    world = len(bounds)
-    rows = max(1, max(h - l for l, h in bounds))
-    out = []
-    for t, per in zip(blocks, (1, 1, int(n_fowt))):
-        pad = t.new_zeros((rows * per,) + tuple(t.shape[1:]))
-        pad[:t.shape[0]].copy_(t)
-        if world > 1:
-            full = t.new_empty((world * rows * per,) + tuple(t.shape[1:]))
-            dist.all_gather_into_tensor(full, pad, group=group)
-        else:
-            full = pad
-        out.append(full.index_select(0, farm_rows(bounds, per).to(full.device)))
-    return tuple(out)
+    [F_r*N,nC,4]) -> the whole batch's three tensors in farm order (``_gather_rows``: padded to the largest shard, one
+    ``all_gather_into_tensor`` each, padding dropped).  Backend-agnostic (NCCL on GPUs, gloo on CPU tensors)."""
+    N = int(n_fowt)
+    spans = (list(bounds), list(bounds), [(lo * N, hi * N) for lo, hi in bounds])
+    return tuple(_gather_rows(t, sp, group) for t, sp in zip(blocks, spans))
 
 
 def ragged_farm_cost(N):
@@ -607,16 +595,15 @@ class ShardedFarmSolve:
     ``designs``: ``solver.DesignBatch`` of F * n_fowt FOWTs in the farm batch's order (design f * N + i is FOWT i of farm f), or
     the packed designs; ``cases``: ``solver.CaseTable`` as for the single-GPU entry (operating points, wave trains, F_2nd);
     array matrices [6N,6N] for every farm or [F,6N,6N], sliced to each rank's farms.
-    ``exchange="peer"``: the farm kernel stores each rank's results into every rank's gathered copy through CUDA IPC peer
-    pointers (raftk_farm_batch_response_gather_dev; farms too large for shared memory are copied by k_farm_publish after their
-    solve), then raftk_peer_barrier_dev; the copies hold F_max = the largest shard's farm count per rank.  ``exchange="nccl"``:
+    ``exchange="peer"``: each rank solves its farms, then k_farm_publish copies its results into every rank's gathered copy
+    through CUDA IPC peer pointers (raftk_farm_batch_response_gather_dev), then raftk_peer_barrier_dev; the copies hold F_max = the largest shard's farm count per rank.  ``exchange="nccl"``:
     ``gather_farm_shards`` instead; a peer exchange that cannot be set up (CUDA IPC unavailable) falls back to it on every
     rank.  With one rank it is ``DeviceSession.farm_response(n_fowt=N)`` with the exchange's copies as outputs.
 
     ``farm_sizes`` instead of ``n_fowt``: a ragged batch (``solver.solve_dynamics_farm_ragged``), farm f of farm_sizes[f]
     FOWTs, array matrices as that function takes them.  Rank r takes the whole farms ``ragged_farm_shards(farm_sizes,
     world)[r]`` (balanced by estimated work), and every farm is stored at its global offset of every rank's copy, no padding:
-    ``exchange="peer"`` through raftk_farm_ragged_response_gather_dev (solve, then k_farm_publish_flat), ``"nccl"`` through
+    ``exchange="peer"`` through raftk_farm_ragged_response_gather_dev (solve, then k_farm_publish), ``"nccl"`` through
     ``gather_ragged_farm_shards``.  ``step()`` -> (Xi_sys: per-farm [nC,6N_f,nw] views of one flat tensor, info [F,nC,nw],
     status [nD,nC,4]), bit for bit what one ``solve_dynamics_farm_ragged`` call returns."""
 

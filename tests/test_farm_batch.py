@@ -277,7 +277,7 @@ def test_every_farm_equals_the_single_farm_entry(N, kernel, nw):
     ct = solver.CaseTable(_cases(rows))
     out = solver.solve_dynamics_farm_batch(solver.DesignBatch(_flat(packs)), ct, N, C_arr=C_arr, want=PER_FOWT)
     rec = solver.last_dispatch()
-    assert rec["family"] == "farm" and rec["kernel"] == kernel, rec
+    assert rec["family"] == "farm" and rec["kernel"] == kernel and rec["farm_classes"] == (kernel,), rec
     assert not np.any(out["info"])
     _assert_farms_equal_single(packs, lambda f: ct, C_arr, out, N, kernel)
     for f in range(1, F):

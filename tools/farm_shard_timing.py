@@ -1,10 +1,10 @@
-"""Cost of the sharded farm batch's exchange on one GPU (profiles/h100_farm_shard.txt).
+"""Cost of the sharded farm batch's exchange on one GPU (profiles/h100_farm_shard.txt, profiles/h100_farm_one_path.txt).
 
-* The fused peer stores: the coupled farm solve of a DeviceSession through raftk_farm_batch_response_gather_dev with one
-  emulated peer (a second gathered copy on the same device, so every result is stored twice) against the plain
-  instantiation (raftk_farm_batch_response_ws_dev), alternated, CUDA events around `--calls` launches per sample.
-* k_farm_publish, the copy that follows k_farm_response_global for farms too large for shared memory: its kernel time and the
-  solve's from torch.profiler, in a run of its own after the timed one.
+* The gather: the coupled farm solve of a DeviceSession through raftk_farm_batch_response_gather_dev with one emulated peer
+  (a second gathered copy on the same device, so every result is stored twice: the solve, then k_farm_publish's copy)
+  against the plain solve (raftk_farm_batch_response_ws_dev), alternated, CUDA events around a run of calls per sample.
+  One shape per kernel class: 16 farms of 2 (rows12), 4 (warp) and 8 (block) FOWTs, 4 farms of 64 (global).
+* k_farm_publish: its kernel time and the solve's from torch.profiler, in a run of its own after the timed one.
 The multi-GPU speed-up needs several GPUs and is not measured here.  Usage: python tools/farm_shard_timing.py [--out FILE]"""
 import argparse
 import ctypes as C
@@ -79,10 +79,10 @@ class Shape:
         self.gi = raw[off_status:off_status + 2 * F * nC * nw * 4].view(torch.int32).view(2 * F, nC, nw)
 
     def plain(self):
-        self.sess.farm_response(n_fowt=self.N)
+        self.sess.farm_response(C_arr=self.C_arr, n_fowt=self.N)
 
     def peer(self):
-        self.sess.farm_response_gather(self.peers, 0, self.gx[:self.F], self.gi[:self.F], self.N)
+        self.sess.farm_response_gather(self.peers, 0, self.gx[:self.F], self.gi[:self.F], self.N, C_arr=self.C_arr)
 
     def same_bits(self):
         """The peer call's local rows and the emulated peer's copy against the plain call's output."""
@@ -128,7 +128,7 @@ def main():
              "shape: %d cases x %d bins; per sample: CUDA events around a run of calls on one stream, after 3 warm-up calls of each;"
              " plain and peer alternated, %d samples each, median and spread (min..max) reported" % (args.nC, args.nw, args.reps)]
     rec = dict(gpu=info, nC=args.nC, nw=args.nw, shapes=[])
-    for F, N, calls in ((16, 8, 40), (4, 64, 3)):
+    for F, N, calls in ((16, 2, 100), (16, 4, 100), (16, 8, 40), (4, 64, 3)):
         s = Shape(F, N, args.nC, args.nw)
         for _ in range(3):
             s.plain()
@@ -146,24 +146,23 @@ def main():
         lines.append("%2d farms x %2d FOWTs (%s): plain %.3f ms [%.3f..%.3f], peer (one emulated peer) %.3f ms [%.3f..%.3f], "
                      "ratio %.3f; peer results == plain results: %s"
                      % (F, N, s.kernel, med["plain"], *r["plain_range"], med["peer"], *r["peer_range"], r["peer_over_plain"], same))
-        if N > 20:
-            from torch.profiler import ProfilerActivity, profile
+        from torch.profiler import ProfilerActivity, profile
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(calls):
+                s.peer()
             torch.cuda.synchronize()
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                for _ in range(calls):
-                    s.peer()
-                torch.cuda.synchronize()
-            ker = {}
-            for e in prof.key_averages():
-                for nm in ("k_farm_publish", "k_farm_response_global"):
-                    if nm in e.key:
-                        ker[nm] = ker.get(nm, 0.0) + e.device_time_total / 1e3 / calls
-            r["profiler_ms"] = ker
-            pub_bytes = F * args.nC * (6 * N * args.nw * 16 + args.nw * 4 + N * 4 * 4)
-            lines.append("   torch.profiler, %d peer calls: k_farm_response_global %.3f ms/call, k_farm_publish %.4f ms/call "
-                         "(%.1f MB to the one peer copy + status rows: %.0f GB/s device-to-device on one GPU)"
-                         % (calls, ker.get("k_farm_response_global", float("nan")), ker.get("k_farm_publish", float("nan")),
-                            pub_bytes / 1e6, pub_bytes / (ker.get("k_farm_publish", float("nan")) * 1e-3) / 1e9))
+        ker = {}
+        for e in prof.key_averages():
+            nm = "k_farm_publish" if "k_farm_publish" in e.key else "solve" if ("k_farm_r" in e.key) else None
+            if nm:
+                ker[nm] = ker.get(nm, 0.0) + e.device_time_total / 1e3 / calls
+        r["profiler_ms"] = ker
+        pub_bytes = F * args.nC * (6 * N * args.nw * 16 + args.nw * 4 + N * 4 * 4)
+        pub = ker.get("k_farm_publish", float("nan"))
+        lines.append("   torch.profiler, %d peer calls: solve kernel %.3f ms/call, k_farm_publish %.4f ms/call "
+                     "(%.1f MB to the one peer copy + status rows: %.0f GB/s device-to-device on one GPU)"
+                     % (calls, ker.get("solve", float("nan")), pub, pub_bytes / 1e6, pub_bytes / (pub * 1e-3) / 1e9))
         rec["shapes"].append(r)
         s.close()
     lines.append("multi-GPU speed-up of ShardedFarmSolve: not measured (one GPU)")
