@@ -116,6 +116,18 @@ typedef struct raftk_designs {
     const double *qtf_heads;    /* [n_qtf_head] rad, ascending                                  */
     const double *qtf;          /* complex [nD or 1 or nD*nC, n_qtf_w, n_qtf_w, n_qtf_head, 6]: fowt.qtf, dimensional,
                                    Hermitian-filled (raft_fowt.py:2112-2128)                     */
+    /* inertial wave excitation of submerged rotors (MHK turbines, hub below the waterline; raft_fowt.py:1859-1888), or
+       max_rotors = 0.  Rotor r of design d adds G ud(r3) to F_iner, ud = i w u the wave acceleration of getWaveKin at its hub
+       (helpers.py:188-236), G = T_node^T ([I3; H(r3 - r6)] I[:3,:3] + [0; I[3:,:3]]) with I = rotateMatrix6(I_hydro, R_q) and
+       T_node the hub node's 6 rows of fowt.T (raft_b200.packer.pack_rotor_excitation).  As in the reference, only the last
+       wave train of a case gets the term: a row of the case table when it ends its group of cases.primary (every row without
+       primary), so the groups must be contiguous with their primary first (*_host entries refuse other maps).  The rotor's added mass is the caller's, in M0 (the reference has it in A_hydro_morison).  *_host entries
+       check rot_count in [0, max_rotors], r3[2] < 0 and a finite G; *_dev entries the counts and pointers only. */
+    int32_t max_rotors;         /* table stride: the most rotors of any design                  */
+    int32_t _pad3;
+    const int32_t *rot_count;   /* [nD] submerged rotors of each design                         */
+    const double *rot_r3;       /* [nD, max_rotors, 3] global hub positions (x_ref, y_ref included) */
+    const double *rot_G;        /* [nD, max_rotors, 6, 3] row-major                              */
 } raftk_designs;
 
 /* Load cases, shared by all designs: units of work are (design, case) pairs.

@@ -31,6 +31,7 @@ class RaftkDesigns(C.Structure):
         ("bem_headings", C.c_void_p), ("X_BEM", C.c_void_p), ("bem_xyh", C.c_void_p),
         ("n_qtf_w", C.c_int32), ("n_qtf_head", C.c_int32), ("qtf_shared", C.c_int32), ("_pad2", C.c_int32),
         ("qtf_w", C.c_void_p), ("qtf_heads", C.c_void_p), ("qtf", C.c_void_p),
+        ("max_rotors", C.c_int32), ("_pad3", C.c_int32), ("rot_count", C.c_void_p), ("rot_r3", C.c_void_p), ("rot_G", C.c_void_p),
     ]
 
 

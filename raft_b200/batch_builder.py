@@ -238,6 +238,20 @@ def _count_classes(keys, valid, tol):
     return n
 
 
+def _base_rotors(matrices, A_mor, arrays, nD):
+    """The base design's submerged rotors (``matrices['rotor_excitation']``, ``['A_hydro_rotor']``, as ``fowt.FOWT`` takes
+    them) for every design of a family: the hubs do not move with the platform members a family varies, so every design
+    gets the base table, and the rotor's added mass joins A_hydro_morison (in place) as in FOWT.calcHydroConstants."""
+    if "A_hydro_rotor" in matrices:
+        A_mor += np.asarray(matrices["A_hydro_rotor"], dtype=float)[None]
+    rot = matrices.get("rotor_excitation")
+    if rot is not None and len(rot["r3"]):
+        r3, G = np.asarray(rot["r3"], dtype=float).reshape(-1, 3), np.asarray(rot["G"], dtype=float).reshape(-1, 6, 3)
+        arrays["rot_count"] = np.full(nD, len(r3), dtype=np.int32)
+        arrays["rot_r3"] = np.ascontiguousarray(np.broadcast_to(r3, (nD,) + r3.shape))
+        arrays["rot_G"] = np.ascontiguousarray(np.broadcast_to(G, (nD,) + G.shape))
+
+
 def build_family(family, w, k, depth, matrices, r6=None):
     """-> ``solver.DesignBatch`` of every design of ``family`` on the grid (w, k): the CSR node / member tables and the
     system matrices M0 = M_struc + A_hydro_morison, B0, C0 (statics stay at ``matrices``, as in sweep.build_variants)."""
@@ -286,6 +300,7 @@ def build_family(family, w, k, depth, matrices, r6=None):
     arrays["mem_circ"] = np.ascontiguousarray(np.broadcast_to(np.array([1 if T["circ"] else 0 for T in tabs], dtype=np.int32), (nD, Nm))[has])
     arrays["member_offset"] = np.concatenate([[0], np.cumsum(has.sum(axis=1))]).astype(np.int32)
     arrays["mem_node_start"] = np.concatenate([[0], np.cumsum(cnt[has])]).astype(np.int32)
+    _base_rotors(matrices, A_mor, arrays, nD)
     M_struc = np.asarray(matrices.get("M_struc", np.zeros([6, 6])), dtype=float)
     arrays["M0"] = np.ascontiguousarray((M_struc[None] + A_mor).reshape(nD, 36))
     B0 = np.asarray(matrices.get("B_struc", np.zeros([6, 6])), dtype=float)
@@ -411,6 +426,7 @@ def build_family_native(family, w, k, depth, matrices, r6=None):
         setattr(t, name, a.ctypes.data)
     t.A_morison = A_mor.ctypes.data
     check(lib.raftk_build_family_host(C.byref(fam), C.byref(t)))
+    _base_rotors(matrices, A_mor, arrays, nD)
     M_struc = np.asarray(matrices.get("M_struc", np.zeros([6, 6])), dtype=float)
     arrays["M0"] = np.ascontiguousarray((M_struc[None] + A_mor).reshape(nD, 36))
     B0 = np.asarray(matrices.get("B_struc", np.zeros([6, 6])), dtype=float)

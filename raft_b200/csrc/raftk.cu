@@ -22,6 +22,7 @@
 #include <cuda_runtime.h>
 #include <cooperative_groups.h>
 #include <math_constants.h>
+#include <cmath>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -177,6 +178,7 @@ static DesignsDev to_dev(const raftk_designs *d, int max_nodes, int max_members)
     D.node_in_p2_w = reinterpret_cast<const double2 *>(d->node_in_p2_w);
     D.M0 = d->M0; D.B0 = d->B0; D.C0 = d->C0; D.A_w = d->A_w; D.B_w = d->B_w;
     D.bem_headings = d->bem_headings; D.X_BEM = d->X_BEM; D.bem_xyh = d->bem_xyh;
+    D.max_rotors = d->max_rotors; D.rot_count = d->rot_count; D.rot_r3 = d->rot_r3; D.rot_G = d->rot_G;
     return D;
 }
 
@@ -262,6 +264,46 @@ static int validate(const raftk_designs *d, const raftk_cases *c)
     if (d->max_nodes <= 0 || d->max_members <= 0) return set_err(RAFTK_EINVAL, "max_nodes/max_members must be > 0");
     if (d->max_members > 512 || d->max_nodes > 4096) return set_err(RAFTK_EINVAL, "design too large for the shared-memory tables");
     if ((d->node_in_p1_w == nullptr) != (d->node_in_p2_w == nullptr)) return set_err(RAFTK_EINVAL, "node_in_p1_w / node_in_p2_w must both be given or both NULL");
+    if (d->max_rotors < 0) return set_err(RAFTK_EINVAL, "designs.max_rotors must be >= 0");
+    if (d->max_rotors > 0 && (!d->rot_count || !d->rot_r3 || !d->rot_G))
+        return set_err(RAFTK_EINVAL, "designs.max_rotors > 0 needs rot_count, rot_r3 and rot_G");
+    return 0;
+}
+
+// The submerged-rotor table of a host call: every design's count in [0, max_rotors], every hub below the waterline (the
+// reference adds the term only there, raft_fowt.py:1861) and every G finite; with a cases.primary map, every train group
+// contiguous with its primary first, which is how the kernels find a group's last train (rotor_excitation).
+static int validate_rotors_host(const raftk_designs *d, const raftk_cases *c)
+{
+    char m[160];
+    if (d->max_rotors > 0 && c->primary)
+        for (int i = 0; i < c->n_cases; i++) {
+            const int p = c->primary[i];
+            if (!(p == i || (i > 0 && p < i && c->primary[i - 1] == p))) {
+                snprintf(m, sizeof(m), "cases.primary: with submerged rotors every train group must be contiguous with its primary "
+                         "first (case %d names primary %d)", i, p);
+                return set_err(RAFTK_EINVAL, "%s", m);
+            }
+        }
+    for (int i = 0; i < d->n_designs && d->max_rotors > 0; i++) {
+        const int n = d->rot_count[i];
+        if (n < 0 || n > d->max_rotors) {
+            snprintf(m, sizeof(m), "designs.rot_count[%d] = %d is outside [0, max_rotors = %d]", i, n, d->max_rotors);
+            return set_err(RAFTK_EINVAL, "%s", m);
+        }
+        for (int r = 0; r < n; r++) {
+            const size_t e = (size_t)i * d->max_rotors + r;
+            if (!(d->rot_r3[3 * e + 2] < 0.0)) {
+                snprintf(m, sizeof(m), "designs.rot_r3: rotor %d of design %d is not submerged (z = %g)", r, i, d->rot_r3[3 * e + 2]);
+                return set_err(RAFTK_EINVAL, "%s", m);
+            }
+            for (int t = 0; t < 18; t++)
+                if (!std::isfinite(d->rot_G[18 * e + t])) {
+                    snprintf(m, sizeof(m), "designs.rot_G: rotor %d of design %d has a non-finite entry", r, i);
+                    return set_err(RAFTK_EINVAL, "%s", m);
+                }
+        }
+    }
     return 0;
 }
 
@@ -506,17 +548,17 @@ static FusedParams fused_params(const raftk_designs *d, const raftk_cases *c, co
     return P;
 }
 
-template <int T>
+template <int T, bool ROT>
 static int fused_launch(const DesignsDev &D, const CasesDev &C, const FusedParams &P, const SolvePlan &pl, int units, cudaStream_t st)
 {
     static SmemOptIn opt;
-    CUDA_TRY(opt.ensure(k_rao_fused<T>, pl.smem));
+    CUDA_TRY(opt.ensure(k_rao_fused<T, ROT>, pl.smem));
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute at;
     cluster_config(cfg, at, (size_t)units * pl.CS, T, pl.smem, pl.CS, st);
     {
         ProfScope ps(st, 2);
-        CUDA_TRY(cudaLaunchKernelEx(&cfg, k_rao_fused<T>, D, C, P));
+        CUDA_TRY(cudaLaunchKernelEx(&cfg, k_rao_fused<T, ROT>, D, C, P));
     }
     g_launches++;
     disp_launch(RAFTK_FAMILY_SOLVE, T == 128 ? RAFTK_KERNEL_FUSED128 : RAFTK_KERNEL_FUSED256, T, pl.CS, pl.nwl);
@@ -524,6 +566,14 @@ static int fused_launch(const DesignsDev &D, const CasesDev &C, const FusedParam
     g_disp.trains = P.phase >= 0;
     CUDA_TRY(cudaGetLastError());
     return RAFTK_OK;
+}
+
+// k_rao_fused at the plan's CTA size, in the instantiation with the submerged-rotor term when the designs carry rotors
+static int fused_launch(const DesignsDev &D, const CasesDev &C, const FusedParams &P, const SolvePlan &pl, int units, cudaStream_t st)
+{
+    const bool rot = D.max_rotors > 0;
+    if (pl.T == 128) return rot ? fused_launch<128, true>(D, C, P, pl, units, st) : fused_launch<128, false>(D, C, P, pl, units, st);
+    return rot ? fused_launch<256, true>(D, C, P, pl, units, st) : fused_launch<256, false>(D, C, P, pl, units, st);
 }
 
 static int run_fused(const raftk_designs *d, const raftk_cases *c, const raftk_solve_opts *o, const raftk_outputs *out,
@@ -540,20 +590,29 @@ static int run_fused(const raftk_designs *d, const raftk_cases *c, const raftk_s
         P.lin_g = reinterpret_cast<double *>(static_cast<char *>(workspace) + pl.o_lin);
         for (int phase = 0; phase < 2; phase++) {
             P.phase = phase;
-            const int rc = (pl.T == 128) ? fused_launch<128>(D, C, P, pl, units, st) : fused_launch<256>(D, C, P, pl, units, st);
-            if (rc) return rc;
+            if (int rc = fused_launch(D, C, P, pl, units, st)) return rc;
         }
         return RAFTK_OK;
     }
-    if (pl.T == 128) return fused_launch<128>(D, C, P, pl, units, st);
-    return fused_launch<256>(D, C, P, pl, units, st);
+    return fused_launch(D, C, P, pl, units, st);
 }
 
 // Grid or cluster exchange for k_rao_fused2 (RAFTK_FUSED2_XCHG=cluster|grid overrides, read per call, for A/B runs and
 // tests).  The grid variant runs when a unit spans several CTAs, every CTA of the launch can be resident at once, and the
 // hardware cannot place every unit's cluster at once (cudaOccupancyMaxActiveClusters < units): then the clusters that do not
 // fit would start only when the first units finish.  The occupancy queries are cached per device and launch shape.
-static SmemOptIn g_f2_opt_cluster, g_f2_opt_grid, g_f2_opt_cluster_op, g_f2_opt_grid_op;
+static SmemOptIn g_f2_opt_var[8];
+
+// k_rao_fused2's instantiation number var: bit 0 GRID, bit 1 OP, bit 2 ROT
+using F2Kernel = void (*)(DesignsDev, CasesDev, FusedParams);
+static F2Kernel f2_kernel(int var)
+{
+    static const F2Kernel k[8] = {k_rao_fused2<false>, k_rao_fused2<true>, k_rao_fused2<false, true>, k_rao_fused2<true, true>,
+                                  k_rao_fused2<false, false, true>, k_rao_fused2<true, false, true>, k_rao_fused2<false, true, true>,
+                                  k_rao_fused2<true, true, true>};
+    return k[var];
+}
+static cudaError_t f2_opt_in(int var, size_t smem) { return g_f2_opt_var[var].ensure(f2_kernel(var), smem); }
 struct F2Occ { int dev, units, CS; size_t smem; int clusters, resident; };
 static std::mutex g_f2_occ_mu;
 static std::vector<F2Occ> g_f2_occ;
@@ -566,8 +625,8 @@ static int f2_occupancy(const SolvePlan &pl, int units, int &clusters, int &resi
         for (const F2Occ &e : g_f2_occ)
             if (e.dev == dev && e.units == units && e.CS == pl.CS && e.smem == pl.smem) { clusters = e.clusters; resident = e.resident; return RAFTK_OK; }
     }
-    CUDA_TRY(g_f2_opt_cluster.ensure(k_rao_fused2<false>, pl.smem));
-    CUDA_TRY(g_f2_opt_grid.ensure(k_rao_fused2<true>, pl.smem));
+    CUDA_TRY(f2_opt_in(0, pl.smem));
+    CUDA_TRY(f2_opt_in(1, pl.smem));
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute at;
     cluster_config(cfg, at, (size_t)units * pl.CS, F2_T, pl.smem, pl.CS, 0);
@@ -617,9 +676,9 @@ static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_
     const int units = d->n_designs * c->n_cases;
     bool grid = false;
     if (int rc = f2_pick_grid(pl, units, grid)) return rc;
-    const bool op = c->op != nullptr;        // the instantiation with operating points (same registers and occupancy)
-    if (op) CUDA_TRY(grid ? g_f2_opt_grid_op.ensure(k_rao_fused2<true, true>, pl.smem) : g_f2_opt_cluster_op.ensure(k_rao_fused2<false, true>, pl.smem));
-    else CUDA_TRY(grid ? g_f2_opt_grid.ensure(k_rao_fused2<true>, pl.smem) : g_f2_opt_cluster.ensure(k_rao_fused2<false>, pl.smem));
+    // the instantiations with operating points and with submerged rotors (same registers and occupancy)
+    const int var = (grid ? 1 : 0) | (c->op ? 2 : 0) | (d->max_rotors > 0 ? 4 : 0);
+    CUDA_TRY(f2_opt_in(var, pl.smem));
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute at;
     cluster_config(cfg, at, (size_t)units * pl.CS, F2_T, pl.smem, pl.CS, st);
@@ -635,12 +694,8 @@ static int run_fused2(const raftk_designs *d, const raftk_cases *c, const raftk_
         P.phase = c->primary ? phase : -1;
         {
             ProfScope ps(st, 2);
-            if (grid) {
-                CUDA_TRY(cudaMemsetAsync(P.xcnt, 0, (size_t)units * sizeof(unsigned), st));      // counters count up from 0 per launch
-                CUDA_TRY(op ? cudaLaunchKernelEx(&cfg, k_rao_fused2<true, true>, D, C, P) : cudaLaunchKernelEx(&cfg, k_rao_fused2<true>, D, C, P));
-            } else {
-                CUDA_TRY(op ? cudaLaunchKernelEx(&cfg, k_rao_fused2<false, true>, D, C, P) : cudaLaunchKernelEx(&cfg, k_rao_fused2<false>, D, C, P));
-            }
+            if (grid) CUDA_TRY(cudaMemsetAsync(P.xcnt, 0, (size_t)units * sizeof(unsigned), st));      // counters count up from 0 per launch
+            CUDA_TRY(cudaLaunchKernelEx(&cfg, f2_kernel(var), D, C, P));
         }
         g_launches++;
     }
@@ -1570,6 +1625,11 @@ static void stage_designs_cases(Staging &S, const raftk_designs *d, const raftk_
         S.in(dd.X_BEM, d->X_BEM, nD * d->n_bem_head * 6 * nw * 2);
         S.in(dd.bem_xyh, d->bem_xyh, nD * 3);
     }
+    if (d->max_rotors > 0) {
+        S.in(dd.rot_count, d->rot_count, nD);
+        S.in(dd.rot_r3, d->rot_r3, nD * d->max_rotors * 3);
+        S.in(dd.rot_G, d->rot_G, nD * d->max_rotors * 18);
+    }
     S.in(cc.Hs, c->Hs, nC); S.in(cc.Tp, c->Tp, nC); S.in(cc.gamma, c->gamma, nC);
     S.in(cc.beta_deg, c->beta_deg, nC); S.in(cc.spec, c->spec, nC);
     S.in(cc.zeta, c->zeta, nC * nw);
@@ -1593,7 +1653,7 @@ static int host_run(const char *who, const raftk_designs *d, const raftk_cases *
 {
     disp_reset();
     int rc = validate(d, c);
-    if (rc) return rc;
+    if (rc || (rc = validate_rotors_host(d, c))) return rc;
     if (mode == 0 && (rc = validate_opts(o))) return rc;
     if (!out) return set_err(RAFTK_EINVAL, "null outputs");
     raftk_cases cin = *c;
@@ -2682,6 +2742,7 @@ extern "C" int raftk_solve_dynamics_slender_host(const raftk_designs *d, const r
     if (o->n_iter < 1) return set_err(RAFTK_EINVAL, "slender flow: potSecOrder 1 needs n_iter >= 1");
     const int qtf_chunk = so ? so->qtf_chunk : 0;
     if (int rc = validate_slender_flow(d, s, c, qtf_chunk)) return rc;
+    if (int rc = validate_rotors_host(d, c)) return rc;
     if (int rc = validate_op(c, c->op, nullptr)) return rc;
     Staging S("raftk_solve_dynamics_slender_host");
     raftk_designs dd = *d;

@@ -26,6 +26,9 @@ struct DesignsDev {
     const double2 *node_in_p1_w, *node_in_p2_w;
     const double *M0, *B0, *C0, *A_w, *B_w;
     const double *bem_headings, *X_BEM, *bem_xyh;
+    int max_rotors;                                  // submerged rotors (raftk_designs.rot_*), 0: none
+    const int *rot_count;
+    const double *rot_r3, *rot_G;
 };
 
 struct CasesDev {

@@ -120,7 +120,7 @@ __device__ __forceinline__ void proj(double er, double ei, double Cc, double Sc,
     ci = fma(er, gi, ei * gr);
 }
 
-template <int T>
+template <int T, bool ROT = false>
 __global__ void __launch_bounds__(T, 256 / T)
 k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
 {
@@ -302,7 +302,7 @@ k_rao_fused(DesignsDev D, CasesDev Cs, FusedParams P)
             }
             member_force6(o, Aqr, Aqi, A1r, A1i, A2r, A2i, L1r, L1i, L2r, L2i, Fr, Fi);
         }
-        excitation_sum(D, Cs, P, d, ogl, nw, i, k, beta, sb, cb, [&] { return zeta; }, Fr, Fi);
+        excitation_sum<ROT>(D, Cs, P, d, c, ogl, nw, i, k, beta, sb, cb, [&] { return zeta; }, Fr, Fi);
 #pragma unroll
         for (int a = 0; a < 6; a++) {
             if (P.F0g) P.F0g[ogl + (size_t)a * nw + i] = make_double2(Fr[a], Fi[a]);

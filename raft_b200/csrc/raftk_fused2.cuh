@@ -295,8 +295,9 @@ __device__ __forceinline__ void f2_xchg_arrive_wait(unsigned *cnt, unsigned targ
 // bit-identical.  The grid variant lets the hardware place the CTAs freely: on an H100, 64 4-CTA clusters of this kernel
 // do not all fit at once (cudaOccupancyMaxActiveClusters = 62) while its 256 CTAs do.
 // OP: the case table carries operating points (cases.op); a separate instantiation, so that the solves without them compile
-// exactly as before (this kernel is at the register cap: any term in its per-bin assembly costs spill).
-template <bool GRID, bool OP = false>
+// exactly as before (this kernel is at the register cap: any term in its per-bin assembly costs spill).  ROT: the designs
+// carry submerged rotors (raftk_designs.rot_*), likewise an instantiation of its own.
+template <bool GRID, bool OP = false, bool ROT = false>
 __global__ void __launch_bounds__(F2_T, 2)
 k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
 {
@@ -502,7 +503,7 @@ k_rao_fused2(DesignsDev D, CasesDev Cs, FusedParams P)
             double Fr[6], Fi[6];
 #pragma unroll
             for (int a = 0; a < 6; a++) { Fr[a] = bsel == 0 ? FrA[a] : FrB[a]; Fi[a] = bsel == 0 ? FiA[a] : FiB[a]; }
-            excitation_sum(D, Cs, P, d, ogl, nw, i, D.k[i], beta, sb, cb, [&] { return zeta_f2(Cs, c, i, nw, D.w[i], D.dw); }, Fr, Fi);
+            excitation_sum<ROT>(D, Cs, P, d, c, ogl, nw, i, D.k[i], beta, sb, cb, [&] { return zeta_f2(Cs, c, i, nw, D.w[i], D.dw); }, Fr, Fi);
 #pragma unroll
             for (int a = 0; a < 6; a++) P.F0g[ogl + (size_t)a * nw + i] = make_double2(Fr[a], Fi[a]);
         }

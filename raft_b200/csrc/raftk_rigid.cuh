@@ -115,11 +115,14 @@ __device__ __forceinline__ double drag_bmat_entry(int e, int Nm, const double *m
 // The fused solvers' linear excitation of a unit at bin i, in place (P: FusedParams): Fr + i Fi comes in as the strip
 // inertial and dynamic-pressure force, which goes to P.Finer_out; the BEM excitation (bem_excitation, raftk_tables.cuh) goes
 // to P.Fbem_out (zeros without BEM tables) and is added, and so is the second-order force (raft_model.py:1048, :1212).
-// zeta() gives the bin's wave amplitude; only the BEM term evaluates it.
-template <class Params, class Zeta>
-__device__ __forceinline__ void excitation_sum(const DesignsDev &D, const CasesDev &Cs, const Params &P, int d, size_t ogl, int nw, int i,
-                                               double k, double beta, double sb, double cb, Zeta zeta, double (&Fr)[6], double (&Fi)[6])
+// zeta() gives the bin's wave amplitude; only the BEM and rotor terms evaluate it.  ROT: the designs carry submerged rotors,
+// whose excitation (rotor_excitation, raftk_tables.cuh) joins the inertial force first; a template flag, so that the solves
+// without rotors compile as before.
+template <bool ROT, class Params, class Zeta>
+__device__ __forceinline__ void excitation_sum(const DesignsDev &D, const CasesDev &Cs, const Params &P, int d, int c, size_t ogl, int nw,
+                                               int i, double k, double beta, double sb, double cb, Zeta zeta, double (&Fr)[6], double (&Fi)[6])
 {
+    if constexpr (ROT) rotor_excitation(D, Cs, d, c, i, k, D.w[i], beta, sb, cb, zeta(), Fr, Fi);
     if (P.Finer_out)
         for (int a = 0; a < 6; a++) P.Finer_out[ogl + (size_t)a * nw + i] = make_double2(Fr[a], Fi[a]);
     if (D.n_bem_head > 0) {

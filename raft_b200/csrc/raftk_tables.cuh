@@ -116,6 +116,35 @@ __device__ __forceinline__ void bem_excitation(const DesignsDev &D, int d, int i
                          D.bem_xyh[3 * d], D.bem_xyh[3 * d + 1], D.bem_xyh[3 * d + 2], i, k, beta, sb, cb, zeta, Br, Bi);
 }
 
+// Inertial wave excitation of design d's submerged rotors at bin i (raft_fowt.py:1859-1888), added to Fr + i Fi: the wave
+// acceleration ud = i w u of getWaveKin at each hub r3 (helpers.py:188-236; phase from the hub's global x, y, depth terms at
+// z = r3[2]) through the packed G [6][3] (raftk_designs.rot_G).  The reference applies the term after its wave-train loop,
+// with the train index left at the last train, so only the last row of each group of Cs.primary gets it (groups are
+// contiguous, primary first; without primary every row is its own group).
+__device__ __forceinline__ void rotor_excitation(const DesignsDev &D, const CasesDev &Cs, int d, int c, int i, double k, double w,
+                                                 double beta, double sb, double cb, double zeta, double (&Fr)[6], double (&Fi)[6])
+{
+    if (Cs.primary && c + 1 < Cs.nC && Cs.primary[c + 1] != c + 1) return;
+    const int n = D.rot_count[d];
+    for (int r = 0; r < n; r++) {
+        const size_t e = (size_t)d * D.max_rotors + r;
+        const double *r3 = D.rot_r3 + 3 * e, *G = D.rot_G + 18 * e;
+        double S_, C_, P_;
+        depth_funcs(k, D.depth, r3[2], S_, C_, P_);
+        double se, ce;
+        sincos(-(k * (cb * r3[0] + sb * r3[1])), &se, &ce);     // local elevation zeta (ce + i se)
+        // u = w zeta_l (C cb, C sb, i S); ud = i w u
+        const double a = w * w * zeta;
+        const double hr = a * C_ * cb, vr = a * C_ * sb, zr = a * S_;
+        const double ur[3] = {-hr * se, -vr * se, -zr * ce}, ui[3] = {hr * ce, vr * ce, -zr * se};
+#pragma unroll
+        for (int t = 0; t < 6; t++) {
+            Fr[t] += G[3 * t] * ur[0] + G[3 * t + 1] * ur[1] + G[3 * t + 2] * ur[2];
+            Fi[t] += G[3 * t] * ui[0] + G[3 * t + 1] * ui[1] + G[3 * t + 2] * ui[2];
+        }
+    }
+}
+
 struct ExcOut { double2 *F_iner, *F_BEM; double *zeta; };
 
 __global__ void __launch_bounds__(128) k_excitation(DesignsDev D, CasesDev Cs, Work W, ExcOut O)
@@ -199,6 +228,7 @@ __global__ void __launch_bounds__(128) k_excitation(DesignsDev D, CasesDev Cs, W
         Fi[5] += aq2 * Aqi + b12 * A1i + b22 * A2i + p22 * L1i - p12 * L2i;
     }
     const size_t ogl = ((size_t)d * Cs.nC + c) * 6 * nw;     // global output index base
+    if (D.max_rotors > 0) rotor_excitation(D, Cs, d, c, i, k, w, beta, sb, cb, zeta, Fr, Fi);
     if (O.F_iner)
         for (int a = 0; a < 6; a++) O.F_iner[ogl + (size_t)a * nw + i] = make_double2(Fr[a], Fi[a]);
 

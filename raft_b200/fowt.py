@@ -90,6 +90,13 @@ class FOWT:
             self.X_BEM = np.array(mats["X_BEM"], dtype=complex)
             self.BEM_headings = np.array(mats["BEM_headings"], dtype=float)
         self.B_gyro = np.zeros([6, 6, 0])
+        # submerged rotors (MHK turbines), which this FOWT does not build: their inertial wave excitation as
+        # packer.pack_rotor_excitation would pack it for the FOWT at x_ref = y_ref = 0 (dict(r3 [nR,3] hub positions relative
+        # to the FOWT's reference point, G [nR,6,3]); pack_fowt adds (x_ref, y_ref)) and their reduced
+        # added mass A_hydro_rotor [6,6], which calcHydroConstants adds to A_hydro_morison as the reference does
+        # (raft_fowt.py:1616-1625)
+        self.rotor_excitation = mats.get("rotor_excitation")
+        self.A_hydro_rotor = np.array(mats.get("A_hydro_rotor", np.zeros([6, 6])), dtype=float)
         self.A_hydro_morison = np.zeros([6, 6])
         self.Xi = np.zeros([6, self.nw], dtype=complex)
         self.setPosition(np.array([self.x_ref, self.y_ref, 0, 0, 0, 0], dtype=float))
@@ -110,9 +117,9 @@ class FOWT:
         for mem in self.memberList:
             mem.calcHydroConstants(rho=self.rho_water, g=self.g, k_array=self.k if mem.MCF else None)
             A += mem.added_mass_6dof(self.r6[:3])
-        self.A_hydro_morison = A
+        self.A_hydro_morison = A + self.A_hydro_rotor
         self._batch = None
-        return A
+        return self.A_hydro_morison
 
     def pack(self):
         return packer.pack_fowt(self)
@@ -135,7 +142,8 @@ class FOWT:
     # raft_fowt.py:1732-1888 -------------------------------------------------------------------------------
     def calcHydroExcitation(self, case, memberList=None):
         """Wave kinematics + linear excitation for ``case`` on the GPU; leaves nWaves, beta, zeta, F_BEM,
-        F_hydro_iner like the reference (first wave train; multi-train cases loop over trains)."""
+        F_hydro_iner like the reference (first wave train; multi-train cases loop over trains).  A submerged rotor's
+        excitation goes to the last train only, as in the reference (raft_fowt.py:1861-1883): the trains form one group."""
         heads = np.atleast_1d(np.array(case.get("wave_heading", 0.0), dtype=float))
         self.nWaves = len(heads)
         trains = []
@@ -143,7 +151,10 @@ class FOWT:
             pick = lambda key, dflt: (case.get(key, dflt) if np.isscalar(case.get(key, dflt)) else case.get(key, dflt)[ih])
             trains.append(dict(wave_spectrum=pick("wave_spectrum", "JONSWAP"), wave_period=pick("wave_period", None),
                                wave_height=pick("wave_height", None), wave_heading=heads[ih], wave_gamma=pick("wave_gamma", 0.0)))
-        self._cases = solver.CaseTable(packer.pack_cases(trains))          # ValueError on an unknown spectrum (:1774)
+        table = packer.pack_cases(trains)                                  # ValueError on an unknown spectrum (:1774)
+        if self.nWaves > 1:
+            table["primary"] = np.zeros(self.nWaves, dtype=np.int32)
+        self._cases = solver.CaseTable(table)
         self.beta = np.deg2rad(heads)
         out = solver.hydro_excitation(self._get_batch(), self._cases)
         self.zeta = out["zeta"]
@@ -199,7 +210,7 @@ class FOWT:
         """Linearised drag damping for response ``Xi`` [6,nw] (first wave train); also stores F_hydro_drag."""
         if not hasattr(self, "_cases"):
             raise RuntimeError("calcHydroExcitation must be called first (the reference needs mem.u as well)")
-        one = solver.CaseTable({k: v[:1] for k, v in self._cases.arrays.items()})
+        one = solver.CaseTable({k: v[:1] for k, v in self._cases.arrays.items() if k != "primary"})
         out = solver.hydro_linearization(self._get_batch(), one, np.asarray(Xi, dtype=complex))
         self.B_hydro_drag = out["B_drag"][0, 0]
         self.F_hydro_drag = out["F_drag"][0, 0]

@@ -6,7 +6,8 @@ the same function packs (a) live reference objects, when ``raft_b200`` is droppe
 install (INTEGRATION.md), and (b) the objects built by ``raft_b200.member`` / ``raft_b200.fowt``.
 
 Scope: rigid 6-DOF FOWTs (every member has one structural node that is rigidly tied to the FOWT's
-reference node), no underwater rotors -- the BASELINE.json configs plus MacCamy-Fuchs members.
+reference node), with the inertial wave excitation of submerged rotors (``pack_rotor_excitation``) -- the BASELINE.json
+configs plus MacCamy-Fuchs members and MHK turbines.
 Anything else raises ``NotImplementedError`` (the caller falls back to the reference path; see
 SURVEY.md section 8f row 4).
 
@@ -240,8 +241,57 @@ def pack_bem_excitation(fowt):
                 heading_adjust=np.float64(fowt.heading_adjust))
 
 
+def _skew(r):
+    """H(r) with H(r) f = r x f (the moment rows of translateForce3to6DOF, helpers.py:468-483)."""
+    return np.array([[0.0, -r[2], r[1]], [r[2], 0.0, -r[0]], [-r[1], r[0], 0.0]])
+
+
+def _submerged_rotors(fowt):
+    return [rot for rot in (getattr(fowt, "rotorList", None) or []) if np.asarray(rot.r3, dtype=float)[2] < 0]
+
+
+def pack_rotor_excitation(fowt):
+    """Inertial wave excitation of the FOWT's submerged rotors (MHK turbines; raft_fowt.py:1859-1888), duck-typed on a live
+    FOWT: ``rotorList`` (``r3``, ``I_hydro``, ``R_q``, ``nodeList[0].id``), ``T`` and ``r6``.
+
+    Per rotor with r3[2] < 0 the reference adds f6 = [f3; (r3 - r6) x f3 + I[3:,:3] ud] with f3 = I[:3,:3] ud,
+    I = rotateMatrix6(I_hydro, R_q), to the hub node's rows of F_hydro_iner_fullDOF, and projects it through fowt.T.  So the
+    reduced force is G ud with the real G = T_node^T ([I3; H(r3 - r6)] I[:3,:3] + [0; I[3:,:3]]) [6,3], T_node the hub node's
+    6 rows of T; ud = i w u is the wave acceleration of getWaveKin at r3 (the kernels evaluate it per bin and wave train).
+    The force is taken about the PRP and then through T_node, which for a hub node tied rigidly to the PRP adds the lever arm
+    a second time -- the reference's arithmetic, kept.  The rotor's added mass is not packed here: the reference already
+    has it in A_hydro_morison (raft_fowt.py:1616-1625), which ``pack_matrices`` puts into M0.
+    -> dict(rot_r3 [nR,3], rot_G [nR,6,3]), empty without submerged rotors.  ValueError when a submerged rotor has no
+    I_hydro (calcHydroConstants has not run)."""
+    rotors = _submerged_rotors(fowt)
+    if not rotors:
+        return {}
+    T = np.asarray(fowt.T, dtype=float)
+    r6 = np.asarray(fowt.r6, dtype=float)
+    r3s, Gs = [], []
+    for rot in rotors:
+        if getattr(rot, "I_hydro", None) is None:
+            raise ValueError("submerged rotor at r3 = %s has no I_hydro: run calcHydroConstants first" % list(np.asarray(rot.r3)))
+        R = np.asarray(rot.R_q, dtype=float)
+        I6 = np.asarray(rot.I_hydro, dtype=float)
+        I = np.zeros([6, 6])                     # rotateMatrix6 (helpers.py:604-640): the lower-left block is the upper-right's transpose
+        I[:3, :3] = np.matmul(np.matmul(R, I6[:3, :3]), R.T)
+        I[:3, 3:] = np.matmul(np.matmul(R, I6[:3, 3:]), R.T)
+        I[3:, :3] = I[:3, 3:].T
+        r3 = np.asarray(rot.r3, dtype=float)
+        L = np.vstack([I[:3, :3], _skew(r3 - r6[:3]) @ I[:3, :3] + I[3:, :3]])
+        nid = int(rot.nodeList[0].id)
+        Gs.append(T[6 * nid:6 * nid + 6, :].T @ L)
+        r3s.append(r3)
+    if Gs[0].shape[0] != 6:
+        raise NotImplementedError("rotor excitation: only rigid 6-DOF FOWTs (fowt.T must be [nFullDOF, 6])")
+    return dict(rot_r3=np.array(r3s), rot_G=np.array(Gs))
+
+
 def pack_fowt(fowt, w=None, k=None):
-    """Everything the kernels need for one FOWT design: node/member tables, matrices, grid."""
+    """Everything the kernels need for one FOWT design: node/member tables, matrices, grid, and the excitation table of its
+    submerged rotors (``pack_rotor_excitation``, or the ``rotor_excitation`` dict(r3, G) injected into a FOWT that builds no
+    rotors: r3 relative to the FOWT's (x_ref, y_ref), G as pack_rotor_excitation gives it)."""
     w = np.array(fowt.w if w is None else w, dtype=float)
     k = np.array(fowt.k if k is None else k, dtype=float)
     out = pack_members(fowt)
@@ -252,6 +302,17 @@ def pack_fowt(fowt, w=None, k=None):
     out.update(w=w, k=k, depth=np.float64(fowt.depth), dw=np.float64(w[1] - w[0]),
                x_ref=np.float64(getattr(fowt, "x_ref", 0.0)), y_ref=np.float64(getattr(fowt, "y_ref", 0.0)))
     out.update(pack_qtf(fowt))
+    inj = getattr(fowt, "rotor_excitation", None)
+    if inj is None:
+        out.update(pack_rotor_excitation(fowt))
+    elif len(inj["r3"]):
+        # injected hubs are relative to the FOWT's reference point (x_ref, y_ref), so that one table serves every FOWT of an
+        # array; G is a global-frame matrix and does not turn with heading_adjust
+        if float(getattr(fowt, "heading_adjust", 0.0)) != 0.0:
+            raise NotImplementedError("an injected rotor_excitation table on a FOWT with heading_adjust != 0: G would have to "
+                                      "turn with the FOWT; pack the rotated rotor with pack_rotor_excitation instead")
+        off = np.array([float(getattr(fowt, "x_ref", 0.0)), float(getattr(fowt, "y_ref", 0.0)), 0.0])
+        out.update(rot_r3=np.asarray(inj["r3"], dtype=float).reshape(-1, 3) + off, rot_G=np.asarray(inj["G"], dtype=float).reshape(-1, 6, 3))
     return out
 
 
@@ -284,7 +345,10 @@ def pack_general_dofs(fowt):
     Adds ``gen_nDOF``, ``gen_Tn`` [Ns,6,nDOF] (T rows of each strip node's structural node) and ``gen_rr`` [Ns,3]
     (offset from that node; zero on flexible members, whose strip nodes are their structural nodes).
     The nodes of potential-flow members (potMod) carry no strip-theory inertial excitation (raft_member.py:1980): their
-    ``node_a_i`` is zero, like their Imat, and their wave force comes from the BEM table (``pack_general_matrices``)."""
+    ``node_a_i`` is zero, like their Imat, and their wave force comes from the BEM table (``pack_general_matrices``).
+    NotImplementedError for a FOWT with a submerged rotor: its inertial wave excitation (raft_fowt.py:1859-1888) is not part
+    of the generalised-DOF solve."""
+    _no_submerged_rotor(fowt)
     out = pack_members(fowt, allow_flexible=True)
     T = np.asarray(fowt.T, dtype=float)
     Tn, rr, pot = [], [], []
@@ -322,7 +386,9 @@ def pack_general_matrices(fowt, states=None):
     FOWT right after ``calcTurbineConstants(case)``, or a dict).  The FOWT's own A_aero, B_aero and B_gyro are then ignored:
     B = B_struc; ``fd_idx`` is the union of the BEM support and the support of every state; ``fd``'s A_w / B_w carry the BEM
     terms alone (zero on the DOFs only the operating points touch); and the result gains ``ops``, the
-    ``pack_general_operating_points`` dict on that support, for ``solver.CaseTable(ops=)``."""
+    ``pack_general_operating_points`` dict on that support, for ``solver.CaseTable(ops=)``.
+    NotImplementedError for a FOWT with a submerged rotor (``pack_general_dofs``)."""
+    _no_submerged_rotor(fowt)
     n, nw = int(fowt.nDOF), len(fowt.w)
     M = np.array(fowt.M_struc, dtype=float) + np.array(fowt.A_hydro_morison, dtype=float)
     B = np.array(fowt.B_struc, dtype=float)
@@ -355,6 +421,12 @@ def pack_general_matrices(fowt, states=None):
     if states is not None:
         out["ops"] = pack_general_operating_points([states], idx)
     return out
+
+
+def _no_submerged_rotor(fowt):
+    if _submerged_rotors(fowt):
+        raise NotImplementedError("generalised DOFs: the inertial wave excitation of submerged rotors (MHK, raft_fowt.py:1859-1888) "
+                                  "is on the rigid 6-DOF path only")
 
 
 def _general_state(s):

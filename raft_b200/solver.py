@@ -166,6 +166,17 @@ class DesignBatch:
                 a["qtf"] = np.ascontiguousarray(np.stack([np.asarray(P["qtf"], dtype=np.complex128) for P in packed]))
             if a["qtf"].shape[-4:] != (self.n_qtf_w, self.n_qtf_w, self.n_qtf_head, 6):
                 raise ValueError("qtf must be [nw1, nw2, nheads, 6] with nw1 == nw2 == len(qtf_w)")
+        # submerged rotors (packer.pack_rotor_excitation): padded per design, designs without rotors get rot_count = 0
+        self.max_rotors = max(len(P.get("rot_r3", ())) for P in packed)
+        if self.max_rotors:
+            R = self.max_rotors
+            a["rot_count"] = np.array([len(P.get("rot_r3", ())) for P in packed], dtype=_I4)
+            a["rot_r3"], a["rot_G"] = np.zeros([self.n_designs, R, 3]), np.zeros([self.n_designs, R, 6, 3])
+            for i, P in enumerate(packed):
+                n = int(a["rot_count"][i])
+                if n:
+                    a["rot_r3"][i, :n] = np.asarray(P["rot_r3"], dtype=_F8).reshape(n, 3)
+                    a["rot_G"][i, :n] = np.asarray(P["rot_G"], dtype=_F8).reshape(n, 6, 3)
         a["w"], a["k"] = self.w, self.k
         self.n_members_total = int(member_offset[-1])
         self.n_nodes_total = int(mem_node_start[-1])
@@ -185,6 +196,7 @@ class DesignBatch:
         self.nw = len(self.w)
         self.depth, self.rho, self.g, self.dw = float(depth), float(rho), float(g), float(dw)
         self.n_bem_head = self.n_qtf_w = self.n_qtf_head = self.qtf_shared = 0
+        self.max_rotors = int(a["rot_r3"].shape[1]) if "rot_r3" in a else 0
         self.n_members_total = int(a["member_offset"][-1])
         self.n_nodes_total = int(a["mem_node_start"][-1])
         self.max_nodes, self.max_members = int(max_nodes), int(max_members)
@@ -192,7 +204,7 @@ class DesignBatch:
         self.walk_exact = fused_walk_exact(a, self.k, self.depth)
         return self
 
-    PER_DESIGN = ("M0", "B0", "C0", "A_w", "B_w", "X_BEM", "bem_xyh")
+    PER_DESIGN = ("M0", "B0", "C0", "A_w", "B_w", "X_BEM", "bem_xyh", "rot_count", "rot_r3", "rot_G")
     PER_MEMBER = ("mem_frame", "mem_rA", "mem_arm", "mem_circ")
 
     def take(self, lo, hi):
@@ -266,9 +278,10 @@ class DesignBatch:
         for name in ("w", "k", "member_offset", "mem_frame", "mem_rA", "mem_arm", "mem_node_start", "mem_circ",
                      "node_ls", "node_cd_q", "node_cd_p1", "node_cd_p2", "node_in_q", "node_in_p1", "node_in_p2",
                      "node_pa", "node_in_p1_w", "node_in_p2_w", "M0", "B0", "C0", "A_w", "B_w",
-                     "bem_headings", "X_BEM", "bem_xyh", "qtf_w", "qtf_heads", "qtf"):
+                     "bem_headings", "X_BEM", "bem_xyh", "qtf_w", "qtf_heads", "qtf", "rot_count", "rot_r3", "rot_G"):
             setattr(s, name, ptr(name) if name in self.arrays else None)
         s.n_bem_head = self.n_bem_head
+        s.max_rotors = self.max_rotors
         s.n_qtf_w, s.n_qtf_head, s.qtf_shared = self.n_qtf_w, self.n_qtf_head, self.qtf_shared
         return s
 
